@@ -21,10 +21,15 @@ Workloads (`--scene`):
           qb200_register_batch), CUDA events on the launching stream, max over ranks.
   e2e   : the same call with pinned HOST buffers -- H2D of every scan and D2H of the result records are
           inside the timed region.
-  roofline      : the dominant kernel (tc_nn_kernel, the N_src x N_tgt x 33 contraction on tcgen05) from CUDA events
+  roofline      : the dominant kernel (tc_nn_kernel, the N_src x N_tgt x 33 contraction on wgmma) from CUDA events
                   recorded around it inside the timed steps.
-  cpu_baseline  : the CPU oracle (restatement of the reference path; the reference binary itself cannot be
-                  built here) timed on this box's host cores on a bounded sample of the same pairs.
+  cpu_baseline  : the CPU oracle (restatement of the reference path; the reference binary itself needs
+                  PCL/FLANN/pmc) timed on the host's cores on a bounded sample of the same pairs.
+
+  --dump-outputs DIR : after the timed steps, the result records of the last step (what qb200_register_batch hands
+                  its caller) as DIR/<field>.npy in float64, one array per record field, all finite (the +inf `cost` of a
+                  pair whose GNC stopped before evaluating one is split into cost.npy and cost_evaluated.npy).  The inputs are seeded, so two
+                  builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -103,14 +108,23 @@ def load_peaks():
         d = json.loads(f.read_text())
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d.get("bf16_tflops_sustained"),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (dense, 700 W card): denominators only, never reached figures
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": None, "source": "H100 SXM data sheet (not measured)"}
 
 
-def load_ncu_facts():
-    """Per-launch DRAM traffic of the roofline kernels, read from the committed summary of the round's ncu --set full capture
-    (profiles/r02_ncu_facts.json, written by tools/ncu_facts.py from the .ncu-rep); None when the file is absent."""
-    f = ROOT / "profiles" / "r02_ncu_facts.json"
-    return json.loads(f.read_text()) if f.exists() else None
+def dump_outputs(path, records):
+    """The result records of the last timed step, one float64 array per field (T: P x 16, column-major 4 x 4 poses).
+    `cost` is +inf where GNC stops before its first cost evaluation (every residual already inside the noise bound, as
+    Quatro::cost_ does); it is written as cost.npy (0 there) and cost_evaluated.npy (1 where a cost was evaluated)."""
+    d = Path(path)
+    d.mkdir(parents=True, exist_ok=True)
+    for name in records.dtype.names:
+        v = records[name].astype(np.float64)
+        if name == "cost":
+            ok = np.isfinite(v)
+            np.save(d / "cost_evaluated.npy", ok.astype(np.float64))
+            v = np.where(ok, v, 0.0)
+        np.save(d / f"{name}.npy", v)
 
 
 def gen_pairs(seeds, scene="street"):
@@ -219,7 +233,7 @@ def run_reference(args, rank, world):
                           "sample": f"{best_n} registrations, {cores} pairs in flight, one single-threaded oracle call per core"},
         "e2e": {"value": val, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "reference_sample_pairs_per_step": per_step,
-        "note": "CPU restatement of the reference path (oracle/); the PCL/FLANN/pmc binary cannot be built in this image",
+        "note": "CPU restatement of the reference path (oracle/); the reference binary itself needs PCL/FLANN/pmc",
     }))
 
 
@@ -234,8 +248,8 @@ def workload_config(args, world):
     return {"workload": what, "scene": args.scene,
             "pairs_per_gpu": args.pairs, "global_pairs": args.pairs * world, "scan": scan,
             "params": SCENES[args.scene]["what"],
-            "l2": "inputs larger than L2 (~0.9 GB of raw scans per GPU per step vs 126 MB)" if args.scene != "indoor" else
-                  f"inputs of {args.pairs} x 16 MB per step; L2 (126 MB) is flushed by the first pair's 0.8 GB of K6 operand traffic",
+            "l2": "inputs larger than L2 (~0.9 GB of raw scans per GPU per step vs 50 MB)" if args.scene != "indoor" else
+                  f"inputs of {args.pairs} x 16 MB per step; L2 (50 MB) is flushed by the first pair's 0.8 GB of K6 operand traffic",
             "parallelism": f"dp{world}: independent pairs sharded across ranks, one NCCL all_gather of result records per step"}
 
 
@@ -255,6 +269,7 @@ def main():
     ap.add_argument("--sync-steps", action="store_true", help="time the blocking qb200_register_batch per step (no batch k+1 under the tail of batch k)")
     ap.add_argument("--no-dense", action="store_true", help="skip the dense sub-measurement of the default (street) run")
     ap.add_argument("--cross-rank-pairs", type=int, default=8, help="pairs of the next rank every rank re-registers and compares (N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's result records to DIR/<field>.npy (float64)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -415,6 +430,8 @@ def main():
     host_ms = {"enqueue": 0.0, "collective_wait": 0.0}
     dev_ms, launches, kms, kcalls, sms, clocks = timed(handle, p, pa_dev, MEM_DEVICE, args.steps, ClockSampler(local_rank) if rank == 0 else None)
     res_dev = out.copy()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res_dev)
     out_all_dev = out_all.copy() if world > 1 else None
     host_dev = dict(host_ms)
     if world > 1:
@@ -531,7 +548,6 @@ def main():
 
     if rank == 0:
         peaks = load_peaks()
-        facts = load_ncu_facts()
         nA, nB, L = res_dev["n_src_vox"].astype(np.float64), res_dev["n_tgt_vox"].astype(np.float64), res_dev["n_corr"].astype(np.float64)
         # K6: 66 flop per (src,tgt) descriptor pair (the 2*33 of the ||a||^2+||b||^2-2ab contraction, SURVEY.md 8d)
         match_flops_step = float((66.0 * nA * nB).sum())
@@ -544,19 +560,13 @@ def main():
         graph_gbs = graph_bytes_step / (kcalls[1] / args.steps) / (graph_ms_launch * 1e-3) / 1e9 if graph_ms_launch > 0 else 0.0
         step_ms = dev_ms / args.steps
         flops_launch = match_flops_step / max(launches_per_step, 1)
-        tc_fact = (facts or {}).get("tc_nn_kernel")
-        traffic = None
-        if tc_fact:  # bytes per launch of the captured 64-pair launch, scaled by this run's work per launch
-            traffic = tc_fact["dram_bytes_per_launch"] * flops_launch / tc_fact["algorithmic_flops_per_launch"]
         tf32_peak = peaks["bf16_tflops"] / 2.0
-        roofline = {"kernel": "tc_nn_kernel (K6: tcgen05 3xTF32 filter of the N_src x N_tgt x 33 distance matrix + in-kernel exact fp32 evaluation)",
+        roofline = {"kernel": "tc_nn_kernel (K6: wgmma 3xTF32 filter of the N_src x N_tgt x 33 distance matrix + in-kernel exact fp32 evaluation)",
                     "bound": "tensor", "achieved": match_tflops, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
                     "frac": match_tflops / peaks["bf16_tflops"],
                     "frac_of_tf32_peak": match_tflops / tf32_peak,
-                    "tf32_peak": tf32_peak, "tf32_peak_source": "half of the measured bf16 peak (the kernel's MMAs are kind::tf32; nominal dense tf32 = bf16 / 2)",
-                    "traffic": traffic,
-                    "traffic_source": ("profiles/r02_ncu_facts.json: dram__bytes_read.sum + dram__bytes_write.sum of one ncu --set full launch, scaled "
-                                       "by this run's algorithmic flops per launch") if tc_fact else "no ncu capture committed for this round",
+                    "tf32_peak": tf32_peak, "tf32_peak_source": "half of the bf16 peak (the kernel's MMAs are TF32; nominal dense tf32 = bf16 / 2)",
+                    "traffic": None,
                     "algorithmic_bytes_per_launch": float(((nA + nB) * 132.0).sum()) / max(launches_per_step, 1),
                     "peak_source": peaks["source"] + ", burst bf16",
                     "launch_ms": match_ms_launch, "launches_per_step": launches_per_step, "share_of_step": float(kms[0] / args.steps / step_ms),
@@ -590,18 +600,19 @@ def main():
             g_bytes = 32 * (2 * Lg * 16 + Lg * np.ceil(Lg / 32) * 4 + 4 * Lg)
             g_ms = gms / max(gcalls, 1)
             g_pairs = 32 * Lg * (Lg - 1) / 2
-            # fp32 view: 14 fma-pipe operations (9 FFMA + 5 FADD) per pair test against 148 SMs x 128 lanes x clock (1 op/lane/clk)
-            fp32_ops_peak = 148 * 128 * 1.965e9
-            g_fact = (facts or {}).get("tim_graph_kernel")
+            # fp32 view: 14 fma-pipe operations (9 FFMA + 5 FADD) per pair test against SMs x 128 lanes x clock (1 op/lane/clk),
+            # at the largest SM clock sampled during the timed steps (H100 SXM boost clock when nvidia-smi is unavailable)
+            n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
+            sm_hz = ((clocks or {}).get("sm_max_mhz") or 1980.0) * 1e6
+            fp32_ops_peak = n_sm * 128 * sm_hz
             roofline_graph_3k = {"kernel": "tim_graph_kernel (K8)", "bound": "fp32 pipe (named bound); hbm fraction reported as BASELINE asks",
                                  "achieved": g_bytes / (g_ms * 1e-3) / 1e9, "peak": peaks["hbm_gbs"],
                                  "unit": "GB/s", "frac": g_bytes / (g_ms * 1e-3) / 1e9 / peaks["hbm_gbs"],
-                                 "traffic": g_fact["dram_bytes_per_launch"] if g_fact else None,
-                                 "traffic_source": "profiles/r02_ncu_facts.json (same 32 x L=3000 launch under ncu --set full)" if g_fact else None,
+                                 "traffic": None,
                                  "launch_ms": g_ms,
                                  "L": int(Lg), "sets_per_launch": 32, "bytes_per_launch": g_bytes, "pair_tests_per_s": g_pairs / (g_ms * 1e-3),
                                  "fp32_frac": 14.0 * g_pairs / (g_ms * 1e-3) / fp32_ops_peak,
-                                 "fp32_frac_note": "14 fma-pipe operations per pair test (9 FFMA + 5 FADD; 18.5 issued instructions) x pair tests/s / (148 SMs x 128 lanes x 1.965 GHz)",
+                                 "fp32_frac_note": f"14 fma-pipe operations per pair test (9 FFMA + 5 FADD) x pair tests/s / ({n_sm} SMs x 128 lanes x {sm_hz / 1e9:.3f} GHz)",
                                  "solve_batch_stage_ms": {"graph": float(gst[4] / 5), "clique": float(gst[5] / 5), "pose": float(gst[6] / 5)},
                                  "valid_sets": int(rg["valid"].sum()),
                                  "note": "algorithmic-minimum bytes (0.27 B per pair test) against ~18 fp32 instructions per pair test: the kernel is bound by the fp32 pipe, pair_tests_per_s is the meaningful rate"}

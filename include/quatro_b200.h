@@ -1,5 +1,5 @@
 /*
- * quatro_b200.h -- C-ABI of the B200-native global-registration hot path.
+ * quatro_b200.h -- C-ABI of the H100-native (sm_90a) global-registration hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  Every entry point replaces one stage
  * boundary of the reference (url-kaist/Quatro, paths relative to the reference root):
@@ -365,7 +365,7 @@ int qb200_get_stage_ms(qb200_handle* h, float* ms, int32_t n);
  * [1] = tim_graph_kernel (TIM consistency graph); n <= 2. */
 int qb200_get_kernel_ms(qb200_handle* h, float* ms, int32_t* launches, int32_t n);
 
-/* Diagnostics: the tensor-core (tcgen05, 3xTF32) approximate squared distances that pre-filter the 33-D
+/* Diagnostics: the tensor-core (wgmma, 3xTF32) approximate squared distances that pre-filter the 33-D
  * nearest-neighbour search, for up to 128 x 128 descriptors (out[128*128], row = a).  The matcher's results
  * never depend on these values (exact fp32 re-rank); tests use this to measure the filter's error margin. */
 int qb200_debug_tc_distances(qb200_handle* h, const float* a33, int32_t na, const float* b33, int32_t nb, float* out);

@@ -1,8 +1,8 @@
-"""quatro_b200 -- B200-native global-registration hot path (drop-in for url-kaist/Quatro's
+"""quatro_b200 -- H100-native global-registration hot path (drop-in for url-kaist/Quatro's
 voxel-FPFH -> match -> TIM graph -> max clique -> GNC-TLS yaw + COTE path).
 
 The product is the C-ABI shared library (include/quatro_b200.h, built from quatro_b200/csrc/*.cu
-for sm_100a).  This package only carries the ctypes binding used by tests/bench, the build helper
+for sm_90a).  This package only carries the ctypes binding used by tests/bench, the build helper
 and the synthetic-scan generator.  There is no CPU fallback anywhere in this package.
 """
 from .capi import (  # noqa: F401

@@ -1,8 +1,7 @@
-"""Build helpers: compile the in-tree native libraries (nvcc for sm_100a, g++ for host helpers).
+"""Build helpers: compile the in-tree native libraries (nvcc for sm_90a, g++ for host helpers).
 
-Everything is built IN-TREE under quatro_b200/lib/ so the .so files travel to the GPU box with
-the repo snapshot.  Nothing here falls back to a CPU implementation: if nvcc is missing the build
-raises.
+Everything is built in-tree under quatro_b200/lib/, so the package is importable from the source
+tree.  Nothing here falls back to a CPU implementation: if nvcc is missing the build raises.
 """
 from __future__ import annotations
 
@@ -20,7 +19,7 @@ SYNTH_LIB = LIB_DIR / "libqb200_synth.so"
 HOST_CXX = "/usr/bin/g++"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     # no implicit FMA contraction: float results must match the CPU oracle bit for bit; kernels
     # that want an FMA ask for it explicitly with fmaf()/__fmaf_rn().
@@ -42,6 +41,12 @@ def nvcc_path() -> str:
         if cand and Path(cand).exists():
             return cand
     raise RuntimeError("nvcc not found: the CUDA path cannot be built (there is no CPU fallback)")
+
+
+def cuda_tool(name: str) -> str:
+    """A program of the CUDA toolkit the build uses (cuobjdump, ...): next to its nvcc, else from PATH."""
+    cand = Path(nvcc_path()).parent / name
+    return str(cand) if cand.exists() else name
 
 
 def build_cuda(force: bool = False, verbose: bool = False) -> Path:

@@ -318,7 +318,8 @@ int qb200_create(const qb200_config* cfg_in, qb200_handle** out) {
   h->cfg = cfg; h->device = cfg.device;
   h->S = cfg.max_batch_slots; h->R = cfg.max_raw_points; h->V = cfg.max_voxel_points; h->Lc = cfg.max_corr;
   h->W = h->Lc / 32; h->NS = h->V / kMatchTile;
-  // K6 implementation switch: the tcgen05 filter + in-kernel exact evaluation is the default; QB200_MATCH_EXACT=1 forces
+  if (cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, cfg.device) != cudaSuccess || h->n_sm <= 0) { delete h; return QB200_ERR_NO_DEVICE; }
+  // K6 implementation switch: the tensor-core filter + in-kernel exact evaluation is the default; QB200_MATCH_EXACT=1 forces
   // the exact CUDA-core kernel everywhere (identical results; A/B and triage)
   const char* fe = getenv("QB200_MATCH_EXACT");
   h->force_exact_match = (fe && fe[0] == '1') ? 1 : 0;

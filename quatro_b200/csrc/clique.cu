@@ -1,4 +1,4 @@
-// clique.cu -- K9: k-core decomposition + PMC heuristic maximum clique on the bit adjacency.  sm_100a
+// clique.cu -- K9: k-core decomposition + PMC heuristic maximum clique on the bit adjacency.  sm_90a
 //
 // Replaces teaser::MaxCliqueSolver::findMaxClique (src/graph.cc:12-130) and the pmc routines it
 // calls ([EXT] pmc_graph::compute_cores, pmc_heu::search with heu_strat = "kcore").  pmc is

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host declarations of libquatro_b200 (sm_100a).
+// common.cuh -- shared device/host declarations of libquatro_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,4 +1,4 @@
-// frontend.cu -- K1..K5: voxel down-sampling, neighbour lattice, normals, SPFH, FPFH  (sm_100a)
+// frontend.cu -- K1..K5: voxel down-sampling, neighbour lattice, normals, SPFH, FPFH  (sm_90a)
 //
 // Replaces: voxelize<T>() (include/quatro.hpp:49-57 -> [EXT] pcl::VoxelGrid) and
 // FPFHEstimation::computeFPFHFeatures (src/teaser_utils/fpfh.cc:44-75 -> [EXT] pcl::NormalEstimation,

@@ -1,4 +1,4 @@
-// graph.cu -- K8: translation-invariant-measurement (TIM) consistency graph.   sm_100a
+// graph.cu -- K8: translation-invariant-measurement (TIM) consistency graph.   sm_90a
 //
 // Replaces Quatro::computeTIMs + solveForScale + the inlier_graph_.addEdge loop
 // (include/quatro.hpp:307-386, 784-789; include/teaser/graph.h:96-104).  The reference
@@ -13,15 +13,14 @@
 // The kernel evaluates this in fp32 with A, B in Gram form (|a_i|^2 + |a_j|^2 - 2 a_i.a_j: 4 instead of 6 operations per
 // distance) -- ~18 instructions per pair test -- together with a RIGOROUS bound of its own rounding error:
 //        |t_c - t| <= 36u M |D_c| + 1500 u^2 M^2 + 46 u beta^2 M =: q,   u = 2^-24,  M >= |a_i|^2+|b_i|^2+|a_j|^2+|b_j|^2 + 2 beta^2
-// (derivation in DESIGN.md 5.2).  The arithmetic runs on packed pairs (fma.rn.f32x2 -> FFMA2 / FADD2: the fp32 pipe issues one
-// 3-register FMA per two cycles per scheduler, so two columns per instruction double the rate; results are bit-identical to the
-// scalar forms).  Only pairs with |t_c| <= q -- a band of ~1e-4 relative width around the threshold --
+// (derivation in DESIGN.md 5.2).  Each lane evaluates its columns in pairs of scalar IEEE-rn operations (explicit
+// __fmaf_rn / __fadd_rn: no contraction decides the rounding).  Only pairs with |t_c| <= q -- a band of ~1e-4 relative width around the threshold --
 // or with both distances ~0 (the literal expression is NaN -> false for coincident duplicates) evaluate the literal fp64
 // expression, so the adjacency is bit-identical to the fp64 reference.
 //
 // Work decomposition.  A WARP work item is 64 rows x 128 columns of the upper triangle (any pair of the launch: one global item
 // list); the warp stages its 64 row points in shared memory as (-2a, |a|^2 - beta^2/4 | -2b, |b|^2 - beta^2/4) -- read back as
-// broadcast operands of the packed FMAs -- and each lane keeps FOUR columns in registers as two packed pairs.  No CTA barrier in
+// broadcast operands of the FMAs -- and each lane keeps FOUR columns in registers as two pairs.  No CTA barrier in
 // the item loop.  Result bits are shifted in from the SIGN BITS of t, s' and |t| - q with funnel shifts (no compare / select per
 // test); a warp shuffle transpose turns the per-column words into the row-major half, so both halves of the symmetric matrix come
 // out of one evaluation of the M pair tests.  (Timing experiment, round 2: without the two 4-byte row-strided stores and the
@@ -63,30 +62,13 @@ __device__ __forceinline__ uint32_t warp_transpose32(uint32_t x) {
   return x;
 }
 
-// packed fp32 pairs (sm_100 FFMA2 / FADD2: one instruction, two IEEE-rn results -- bit-identical to the scalar forms)
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) {
-  f32x2 d;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2 abs2(f32x2 a) { return a & 0x7fffffff7fffffffull; }
+// fp32 column pairs: two IEEE-rn scalar operations per helper (sm_90 has no packed fp32 FMA)
+struct f32x2 { float x, y; };
+__device__ __forceinline__ f32x2 pk2(float lo, float hi) { return {lo, hi}; }
+__device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) { lo = v.x; hi = v.y; }
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return {__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return {__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
+__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) { return {__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)}; }
 
 struct GraphConst {
   float b2, hb2q, twob2, b4;   // beta^2, beta^2/4, 2 beta^2, beta^4 (fp32)
@@ -232,7 +214,7 @@ __global__ void __launch_bounds__(kGW * 32, kGC == 2 ? 8 : 4) tim_graph_kernel(c
           const f32x2 t = fma2(D, D, ng);
           float t0, t1, s0, s1, D0, D1;
           upk2(t, t0, t1); upk2(sp, s0, s1); upk2(D, D0, D1);
-          // |t| - q, q = |D| c1 M + K: scalar forms, where |.| is an operand modifier (the packed forms need two LOPs per |.|)
+          // |t| - q, q = |D| c1 M + K (|.| is an operand modifier)
           const float w0 = fabsf(t0) - fmaf(fabsf(D0), qa[2 * p], qk[2 * p]);
           const float w1 = fabsf(t1) - fmaf(fabsf(D1), qa[2 * p + 1], qk[2 * p + 1]);
           wt[2 * p] = __funnelshift_l(__float_as_uint(t0), wt[2 * p], 1);          // sign(t):  t < 0
@@ -340,8 +322,8 @@ int launch_graph(qb200_handle* h, int n_pairs, double noise_bound, double cbar2)
   // (64 registers, 8 CTAs per SM) for A/B runs; results are identical
   static const int cols = (getenv("QB200_GRAPH_COLS") && getenv("QB200_GRAPH_COLS")[0] == '2') ? 2 : 4;
   cudaEventRecord(h->kev[2], h->stream);
-  if (cols == 2) tim_graph_kernel<2><<<dim3(148 * 8), kGW * 32, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, n_pairs, h->Lc, h->W, gc, h->adj);
-  else tim_graph_kernel<4><<<dim3(148 * 4), kGW * 32, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, n_pairs, h->Lc, h->W, gc, h->adj);
+  if (cols == 2) tim_graph_kernel<2><<<dim3(h->n_sm * 8), kGW * 32, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, n_pairs, h->Lc, h->W, gc, h->adj);
+  else tim_graph_kernel<4><<<dim3(h->n_sm * 4), kGW * 32, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, n_pairs, h->Lc, h->W, gc, h->adj);
   cudaEventRecord(h->kev[3], h->stream);
   h->kev_armed[1] = 1;
   const dim3 gd((h->Lc + 7) / 8, n_pairs);

@@ -11,6 +11,7 @@ struct qb200_handle {
   int S, R, V, Lc, W;        // slots, raw cap / cloud, voxel cap / cloud, corr cap / pair, words per adjacency row
   int NS;                    // match stripes per pair = V / kMatchTile
   int device;
+  int n_sm;                  // multiprocessors of the device (grid size of the persistent kernels)
   cudaStream_t own_stream, stream;
   char err[512];
   int64_t launches;
@@ -49,12 +50,12 @@ struct qb200_handle {
   unsigned short* nbr_list;   // [2S][kNbrGlobalCap][V] neighbour indices found by K4 (lattice order), reused by K5
   int* nbr_cnt;               // [2S*V] neighbour count (self included); > kNbrGlobalCap: K5 walks the lattice itself
   float* desc_t;              // [2S*40*V] FPFH, dimension-major per cloud (row d = bin d over all points; rows 33..39 zero)
-  float* desc_tiles;          // [2S*(V/128)*3*5120] per 128-point block: centred TF32 hi | lo | exact fp32 images in the UMMA
+  float* desc_tiles;          // [2S*(V/128)*3*5120] per 128-point block: centred TF32 hi | lo | exact fp32 images in the wgmma
                               // shared-memory operand layout (one bulk copy per tile)
   float* desc_norm;           // [2S*V] squared norms (fp32 fma chain)
   int* tc_fallback;           // [S] 1 = too many exact ties for the filter to pay off: pair re-done by the exact fp32 kernel
   unsigned long long* tc_stats; // [32] diagnostics, cumulative: [0..3] exact evaluations, tiles drained, warm-up passes, aborted stripes; [4..5] QB200_TC_VERIFY; [8..31] QB200_TC_PROF
-  int force_exact_match;      // 0 (default): tcgen05 filter + exact evaluation; 1 (QB200_MATCH_EXACT=1): exact CUDA-core K6 only
+  int force_exact_match;      // 0 (default): tensor-core filter + exact evaluation; 1 (QB200_MATCH_EXACT=1): exact CUDA-core K6 only
   // ---- matching ----
   unsigned long long* rowbest;// [S*V] packed (dist bits << 32 | tgt idx) per source point
   unsigned long long* colpart;// [S*NS*V] per-stripe partial column minima

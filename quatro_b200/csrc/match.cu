@@ -1,5 +1,5 @@
 // match.cu -- K6 (33-D all-pairs nearest neighbour, both directions) + K7 (mutual check, tuple
-// test, dedupe/sort, packing of the matched point pairs).   sm_100a
+// test, dedupe/sort, packing of the matched point pairs).   sm_90a
 //
 // Replaces Matcher::calculateCorrespondences / normalizePoints / advancedMatching
 // (include/teaser_utils/feature_matcher.h:42-74, src/teaser_utils/feature_matcher.cc:18-265, which

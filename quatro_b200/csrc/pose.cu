@@ -1,4 +1,4 @@
-// pose.cu -- K10 (GNC-TLS yaw) + K11 (component-wise translation estimate, COTE).   sm_100a
+// pose.cu -- K10 (GNC-TLS yaw) + K11 (component-wise translation estimate, COTE).   sm_90a
 //
 // Replaces the tail of Quatro::computeTransformation (include/quatro.hpp:806-936):
 // chain TIMs over the sorted clique (:817-844), solveForRotation2D (:430-572, with

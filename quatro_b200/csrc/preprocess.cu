@@ -1,4 +1,4 @@
-// preprocess.cu -- ground removal BEFORE the registration path (SURVEY.md 8f-1), sm_100a.
+// preprocess.cu -- ground removal BEFORE the registration path (SURVEY.md 8f-1), sm_90a.
 //
 // Replaces PatchWork<PointT>::estimate_ground (include/patchwork.hpp:329-455): concentric-zone binning (pc2czm, :512-543),
 // per-patch z order (the global z sort of :348 only matters inside a patch), region-wise ground plane fitting

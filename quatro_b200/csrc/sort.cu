@@ -1,4 +1,4 @@
-// sort.cu -- per-cloud stable radix sort in shared memory (sm_100a): the lattice-cell sort of K2 and the descriptor-norm sort of K6.
+// sort.cu -- per-cloud stable radix sort in shared memory (sm_90a): the lattice-cell sort of K2 and the descriptor-norm sort of K6.
 //
 // Both sorts order at most max_voxel_points (key, point index) pairs PER CLOUD, and only the first n_vox of them carry live keys.  A
 // device-wide radix sort (round 1: cub::DeviceRadixSort over n_clouds * V items, 6-9 launches of 25-30 us per wave each) moves every

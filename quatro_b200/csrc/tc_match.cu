@@ -1,4 +1,4 @@
-// tc_match.cu -- K6 on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a.   (QB200_MATCH_EXACT=1 bypasses it.)
+// tc_match.cu -- K6 on the Hopper tensor cores (wgmma, TF32), sm_90a.   (QB200_MATCH_EXACT=1 bypasses it.)
 //
 // The N_src x N_tgt x 33 descriptor-distance matrix is the one genuinely dense contraction of the path
 // (north_star): d(i,j) = |a_i|^2 + |b_j|^2 - 2 a_i.b_j.  The reference does two exact 1-NN searches (FLANN kd-trees,
@@ -15,7 +15,7 @@
 //   tc_nn_kernel      : per 128-row stripe, column tiles in nearest-norm-first order; a tile whose lower bound
 //                       (gap of the norm ranges)^2 exceeds every current best of the stripe's rows and of its columns is
 //                       skipped unloaded; otherwise
-//                         d~ = |a'|^2 + |b'|^2 - 2 (hi.hi + hi.lo + lo.hi)      3 x 5 tcgen05.mma.kind::tf32, fp32 in TMEM
+//                         d~ = |a'|^2 + |b'|^2 - 2 (hi.hi + hi.lo + lo.hi)      3 x 5 wgmma m64n64k8 TF32 per warpgroup, fp32 in registers
 //                         |d~ - d| <= e_ij = c/2 (|a'_i|^2 + |b'_j|^2),  c = 6e-5   (split + accumulation + chain rounding)
 //                         (i,j) is evaluated EXACTLY (fp32 chain from the exact images) iff its lower bound d~ - e_ij
 //                         does not exceed the best exact distance known so far for row i or for column j;
@@ -25,9 +25,9 @@
 //                       exact CUDA-core kernel, so results never depend on the filter.
 //   broadcast_best_kernel : class results -> every member, in point order for the mutual-NN stage
 //
-// tc_nn_kernel, one CTA per SM, 19 warps, mbarrier hand-offs only: warp 18 chooses tiles and issues the exact-image copies
-// (4 stages), warp 17 the operand copies (2 stages), warp 16 issues the 15 MMAs per tile into one of 4 TMEM accumulator stages,
-// warps 0..15 drain them with tcgen05.ld.32x32b.x32 (lane = row) and run the filter / exact evaluation (DESIGN.md 5.1).
+// tc_nn_kernel, one CTA per SM, 18 warps, mbarrier hand-offs only: warp 17 chooses tiles and issues the exact-image copies
+// (4 stages), warp 16 the operand copies (2 stages); warps 0..15 are 4 warpgroups, each issues the 15 wgmma of its 64 x 64
+// quadrant of the tile and runs the filter / exact evaluation on the accumulator fragment it holds (DESIGN.md 5.1).
 #include "handle.cuh"
 #include <cstdlib>
 
@@ -38,46 +38,54 @@ constexpr int kTcKB = kDescK / 8;                 // K blocks of 8 (TF32 MMA K)
 constexpr int kTcTileBytes = kDescK * 128 * 4;    // one operand image (128 points x 40 dims) = 20480 B
 constexpr int kTileFloats = kDescK * 128;         // 5120
 constexpr int kTcImages = 3;                      // hi | lo | exact
-constexpr int kTcEpiWarps = 16;                   // filter / evaluation warps: TMEM lane quadrant = warp & 3, column quarter = warp >> 2
-constexpr int kTcThreads = (kTcEpiWarps + 3) * 32;  // + MMA warp + operand-copy warp + scheduler warp
-constexpr int kTcAcc = 4;                          // TMEM accumulator stages (4 x 128 columns = all of TMEM)
+constexpr int kTcEpiWarps = 16;                   // MMA + filter / evaluation warps: warpgroup g = rows 64 (g & 1), columns 64 (g >> 1)
+constexpr int kTcThreads = (kTcEpiWarps + 2) * 32;  // + operand-copy warp + scheduler warp
+constexpr int kTcDone = 4;                         // ring of "MMAs of position k done by every warp" barriers
 constexpr int kTcStages = 4;                      // ring of exact B images (prefetch distance 3); operand images: 2 stages
 constexpr float kTcC = 1.2e-4f;                   // |d~ - d| <= kTcC/2 * (|a'|^2 + |b'|^2): 3x the worst error measured (test_tc_filter_error_bound)
 constexpr int kSpinLimit = 400000;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// Operand images use the canonical K-major / no-swizzle UMMA layout (validated by tools/tc_probe.cu on B200; MN-major
-// TF32 without swizzle yields zeros): core matrix = 8 points x 16 B (4 consecutive K values), byte offset
-// kc*2048 + p*16 for K chunk kc (4 dims) and point p of the 128-point block.
+// Operand images use the canonical K-major / no-swizzle (interleave) wgmma layout: core matrix = 8 points x 16 B
+// (4 consecutive K values), byte offset kc*2048 + p*16 for K chunk kc (4 dims) and point p of the 128-point block.
 __device__ __forceinline__ uint64_t tc_smem_desc(uint32_t addr) {
-  // start address >> 4 | LBO = 2048 B (next 4-wide K chunk) | SBO = 128 B (next 8-point group) | version 1 (sm_100) | SWIZZLE_NONE
-  return (uint64_t)((addr & 0x3FFFF) >> 4) | ((uint64_t)(2048 >> 4) << 16) | ((uint64_t)(128 >> 4) << 32) | (1ull << 46);
+  // start address >> 4 | LBO = 2048 B (next 4-wide K chunk) | SBO = 128 B (next 8-point group) | no swizzle (bits 62-63 = 0)
+  return (uint64_t)((addr & 0x3FFFF) >> 4) | ((uint64_t)(2048 >> 4) << 16) | ((uint64_t)(128 >> 4) << 32);
 }
 
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D (64 x 64, fp32, registers of the warpgroup) (+)= A (64 x 8) * B (64 x 8)^T, both TF32 and K-major in shared memory.
+// Fragment: thread (warp w of the warpgroup, lane l) holds d[i] = D[16 w + l / 4 + 8 ((i >> 1) & 1)][8 (i >> 2) + 2 (l & 3) + (i & 1)].
+__device__ __forceinline__ void wgmma_tf32_64x64x8(float (&d)[32], uint64_t adesc, uint64_t bdesc, int accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
 }
 
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+// AND of v over the 128 threads of warpgroup g (named barrier 1 + g): every exit from the tile loop is decided by this vote,
+// so no warp of a warpgroup can leave while the others enter a wgmma
+__device__ __forceinline__ bool wg_all(bool v, int g) {
+  uint32_t r;
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-        "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
+      "{\n\t.reg .pred p, q;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "bar.red.and.pred q, %2, 128, p;\n\t"
+      "selp.u32 %0, 1, 0, q;\n\t}\n"
+      : "=r"(r)
+      : "r"((uint32_t)v), "r"(1 + g)
       : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+  return r != 0;
 }
 
 __device__ __forceinline__ float tc_mu(int d) { return (d == 5 || d == 16 || d == 27) ? 100.0f : 0.0f; }
@@ -260,13 +268,14 @@ __device__ __forceinline__ float tc_fkey_inv(unsigned key) { return __uint_as_fl
 // dump d~ of the first tile of stripe 0 (validation hook).
 //
 // Warp roles (no CTA-wide barrier inside the tile loop, everything is handed over through mbarriers):
-//   warp 17      : copy + schedule warp.  Picks the stripe's next column tile, nearest norm range first, and SKIPS a tile when
+//   warp 17      : schedule warp.  Picks the stripe's next column tile, nearest norm range first, and SKIPS a tile when
 //                  its lower bound (gap between the norm ranges)^2 exceeds every current best of the stripe's rows and of
-//                  the tile's columns; issues the bulk copies (2 operand stages, 4 exact-image stages)
-//   warp 16      : one elected lane issues the 15 MMAs per tile into one of 4 TMEM accumulator stages
-//   warps 0..15  : warp w owns TMEM lanes 32 (w & 3) .. +31 (rows) and columns 32 (w >> 2) .. +31 of every tile:
-//                  tcgen05.ld -> release the TMEM stage -> branch-free filter -> the warp's survivors are compacted
-//                  into batches of 32 and evaluated exactly, ONE CANDIDATE PER LANE -> release the exact-image stage.
+//                  the tile's columns; issues the exact-image copies (4 stages)
+//   warp 16      : operand-copy warp (A images once, hi | lo images of every decided tile, 2 stages)
+//   warps 0..15  : warpgroup g = warps 4g .. 4g+3 owns rows 64 (g & 1) .. +63 and columns 64 (g >> 1) .. +63 of every tile;
+//                  warp w of it holds the accumulators of 16 of those rows (wgmma fragment).  15 wgmma -> release the operand
+//                  stage -> branch-free filter -> the warp's survivors are compacted into batches of 32 and evaluated exactly,
+//                  ONE CANDIDATE PER LANE -> release the exact-image stage.
 // kProf: clock64 accounting of every role's waits into stats[8..31] (tools/tc_profile.py; QB200_TC_PROF=1)
 template <bool kDbg, bool kProf = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
@@ -275,12 +284,10 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
              unsigned* __restrict__ tile_cmax, int* __restrict__ fallback, unsigned long long* __restrict__ stats,
              float* __restrict__ dbg_tile, int no_prune) {
   extern __shared__ __align__(128) unsigned char smem[];  // 220 KB of operand images; static + dynamic must stay <= 227 KB
-  __shared__ uint64_t s_fullx[kTcStages], s_sfree[kTcStages], s_fullhl[2], s_mma[kTcAcc], s_tfree[kTcAcc], s_afull;
-  __shared__ uint32_t s_tmem;
+  __shared__ uint64_t s_fullx[kTcStages], s_sfree[kTcStages], s_fullhl[2], s_mma[kTcDone], s_afull;
   __shared__ unsigned long long s_rbest[kTcM];                 // best exact (distance | target index) per row of the stripe
-  __shared__ __align__(16) float s_wnbm[kTcEpiWarps][32];      // per warp: kLow |b'_j|^2 of its 32 columns
-  __shared__ __align__(16) float s_wcj[kTcEpiWarps][32];       //           kLow |b'_j|^2 - (best exact distance of column j)
-  __shared__ unsigned short s_queue[kTcEpiWarps][32];          //           one batch of candidates (row lane << 5 | column)
+  __shared__ __align__(16) float s_wcj[kTcEpiWarps][64];       // per warp: threshold of each of its 64 columns (best exact distance)
+  __shared__ unsigned short s_queue[kTcEpiWarps][32];          //           one batch of candidates (lane << 5 | fragment index)
   __shared__ int s_seq[8];                                     // column tile of sequence position n (ring), -1 = end of the stripe
   __shared__ float s_tlb[128];                                 // lower bound of every distance between the stripe and column tile t
   __shared__ int s_dead, s_abort, s_evals, s_warm, s_npos;
@@ -311,26 +318,19 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
   const uint32_t* __restrict__ permB = perm + (size_t)cloudB * V;
   unsigned long long* __restrict__ cbg = colbest_r + (size_t)pair * V;
   const uint32_t bar_fullx0 = smem_u32(&s_fullx[0]), bar_sfree0 = smem_u32(&s_sfree[0]), bar_fullhl0 = smem_u32(&s_fullhl[0]),
-                 bar_mma0 = smem_u32(&s_mma[0]), bar_tfree0 = smem_u32(&s_tfree[0]), bar_a = smem_u32(&s_afull);
+                 bar_mma0 = smem_u32(&s_mma[0]), bar_a = smem_u32(&s_afull);
   const int n_tiles = (nB + kTcN - 1) / kTcN;
 
-  if (warp == 0) {  // TMEM: 4 accumulator stages x 128 fp32 columns
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(&s_tmem)), "r"(kTcAcc * kTcN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-  }
   if (threadIdx.x == 0) {
     for (int i = 0; i < kTcStages; ++i) { mbar_init(bar_fullx0 + 8 * i, 1); mbar_init(bar_sfree0 + 8 * i, kTcEpiWarps); }
     for (int i = 0; i < 2; ++i) mbar_init(bar_fullhl0 + 8 * i, 1);
-    for (int i = 0; i < kTcAcc; ++i) { mbar_init(bar_mma0 + 8 * i, 1); mbar_init(bar_tfree0 + 8 * i, kTcEpiWarps); }
+    for (int i = 0; i < kTcDone; ++i) mbar_init(bar_mma0 + 8 * i, kTcEpiWarps);
     mbar_init(bar_a, 1);
     s_dead = 0; s_abort = 0; s_evals = 0; s_warm = 0; s_npos = 0; s_ndec = 0;
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   if (threadIdx.x < kTcM) s_rbest[threadIdx.x] = ~0ull;
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  const uint32_t tmem = s_tmem;
   const long long t_setup = tick();
   if (kProf && threadIdx.x == 0) { atomicAdd(stats + 8, 1ull); atomicAdd(stats + 10, (unsigned long long)(t_setup - t_begin)); }
   volatile int* v_dead = &s_dead;
@@ -348,43 +348,6 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
   volatile unsigned long long* v_rbest = s_rbest;
 
   if (warp == kTcEpiWarps) {
-    // ================= MMA warp =================
-    // instruction descriptor: D=F32 (bits 4-5), A=B=TF32 (bits 7-9, 10-12), both K-major (bits 15,16 = 0), N>>3 (17-22), M>>4 (24-28)
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kTcN >> 3) << 17) | ((uint32_t)(kTcM >> 4) << 24);
-    bool ok = mbar_wait(bar_a, 0);
-    long long p_hl = 0, p_tf = 0, p_is = 0;
-    prof(15, tick() - t_setup);
-    for (int k = 0; ok; ++k) {
-      const int ts = k & (kTcAcc - 1), hs = k & 1;
-      const long long t0 = tick();
-      ok = mbar_wait(bar_fullhl0 + 8 * hs, (uint32_t)((k >> 1) & 1));
-      const long long t1 = tick();
-      p_hl += t1 - t0;
-      if (!ok || v_seq[k & 7] < 0) break;
-      if (k >= kTcAcc) ok = mbar_wait(bar_tfree0 + 8 * ts, (uint32_t)(((k >> 2) - 1) & 1));  // accumulator stage drained (position k-4)
-      const long long t2 = tick();
-      p_tf += t2 - t1;
-      if (!ok) break;
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-      if (lane == 0) {
-        const uint32_t aH = sA, aL = sA + kTcTileBytes, bH = sHL0 + hs * kHLBytes, bL = bH + kTcTileBytes, d = tmem + (uint32_t)(ts * kTcN);
-        uint32_t acc = 0;
-#pragma unroll
-        for (int kb = 0; kb < kTcKB; ++kb) {  // small cross terms first, then hi.hi
-          tc_mma_tf32(d, tc_smem_desc(aH + kb * 4096), tc_smem_desc(bL + kb * 4096), idesc, acc);
-          acc = 1;
-          tc_mma_tf32(d, tc_smem_desc(aL + kb * 4096), tc_smem_desc(bH + kb * 4096), idesc, 1);
-        }
-#pragma unroll
-        for (int kb = 0; kb < kTcKB; ++kb) tc_mma_tf32(d, tc_smem_desc(aH + kb * 4096), tc_smem_desc(bH + kb * 4096), idesc, 1);
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar_mma0 + 8 * ts) : "memory");
-      }
-      __syncwarp();
-      p_is += tick() - t2;
-    }
-    prof(16, p_hl); prof(17, p_tf); prof(18, p_is);
-    if (!ok) *v_dead = 1;
-  } else if (warp == kTcEpiWarps + 1) {
     // ================= operand-copy warp: A images once, then the hi | lo images of every decided position =================
     auto issue_hl = [&](int n) {  // operand images (hi | lo, 40 KB) of position n -> stage n & 1; end marker: plain arrive
       const int t = v_seq[n & 7];
@@ -404,9 +367,9 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     long long p_wm = 0, p_wd = 0;
     bool ended = !ok || v_seq[0] < 0 || v_seq[1] < 0;  // (an end marker has gone out already)
     for (int k = 0; ok && !ended; ++k) {
-      // operand stage k & 1 is free once the MMAs of position k completed
+      // operand stage k & 1 is free once every warp completed its MMAs of position k
       const long long t0 = tick();
-      ok = mbar_wait(bar_mma0 + 8 * (k & (kTcAcc - 1)), (uint32_t)((k >> 2) & 1));
+      ok = mbar_wait(bar_mma0 + 8 * (k & (kTcDone - 1)), (uint32_t)((k >> 2) & 1));
       const long long t1 = tick();
       p_wm += t1 - t0;
       if (ok) ok = wait_decided(k + 2);
@@ -417,7 +380,7 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     }
     prof(12, p_wm); prof(28, p_wd);
     if (!ok) *v_dead = 1;
-  } else if (warp == kTcEpiWarps + 2) {
+  } else if (warp == kTcEpiWarps + 1) {
     // ================= scheduler warp: chooses the tiles and issues the exact-image copies =================
     // norm range of the stripe's rows and of a column tile (ranks are sorted by norm: first / last valid entry)
     const float amin = sqrtf(nrmA[r0]), amax = sqrtf(nrmA[(r0 + kTcM < nA ? r0 + kTcM : nA) - 1]);
@@ -556,7 +519,7 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     long long t_idle = 0;
     while (ok && !(end_decided && nx == nd)) {
       const uint32_t bar_s = bar_sfree0 + 8 * (nx & (kTcStages - 1)), par_s = (uint32_t)(((nx - 4) >> 2) & 1);
-      const uint32_t bar_m = bar_mma0 + 8 * ((nd - 3) & (kTcAcc - 1)), par_m = (uint32_t)(((nd - 3) >> 2) & 1);
+      const uint32_t bar_m = bar_mma0 + 8 * ((nd - 3) & (kTcDone - 1)), par_m = (uint32_t)(((nd - 3) >> 2) & 1);
       const bool can_x = nx < nd, can_d = !end_decided && nd < nx + 4;
       if (can_x && (nx < 4 || mbar_test(bar_s, par_s))) {
         if (kProf && idle) { (can_d ? p_wm : p_sf) += tick() - t_idle; }
@@ -583,19 +546,30 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     if (!ok) *v_dead = 1;
     if (lane == 0) s_npos = n_issued;
   } else {
-    // ================= filter / evaluation warps =================
-    const int quad = warp & 3, cq = warp >> 2, cb = cq * 32;
-    const int row = quad * 32 + lane, gi = r0 + row;
-    const bool row_ok = gi < nA;
-    const float4* __restrict__ aex = reinterpret_cast<const float4*>(smem + 2 * kTcTileBytes) + quad * 32;  // exact image of the A block
-    // TMEM holds LB_ij = d~_ij - e_ij = kLow (na' + nb') - 2 dot (split_desc_kernel); an entry is a candidate iff LB_ij <= the best
-    // exact distance known for row i or for column j
+    // ================= MMA + filter / evaluation warps =================
+    const int wg = warp >> 2;                                // warpgroup
+    const int rbase = (wg & 1) * 64 + 16 * (warp & 3);      // this warp's 16 rows of the stripe
+    const int cb = (wg >> 1) * 64;                           // this warpgroup's 64 columns of the tile
+    const int cl = 2 * (lane & 3);                           // fragment d[i]: row rbase + lane / 4 + 8 ((i >> 1) & 1),
+                                                             //                column cb + 8 (i >> 2) + cl + (i & 1)
+    // the accumulators hold LB_ij = d~_ij - e_ij = kLow (na' + nb') - 2 dot (split_desc_kernel); an entry is a candidate iff
+    // LB_ij <= the best exact distance known for row i or for column j
     const float kLow = 1.0f - 0.5f * kTcC;
     const float kW = kTcC / kLow;                            // d~ + e = LB + kW (kLow na' + kLow nb')
-    const float nam = row_ok ? kLow * nrmA[gi] : INFINITY;   // +inf: a padded row yields no upper bounds
-    const unsigned oa = row_ok ? permA[gi] : 0u;             // point index of this lane's row
-    float Ri_ub = row_ok ? INFINITY : -INFINITY;             // row threshold from the tile-local upper bounds (padded rows: never)
-    float* wnbm = s_wnbm[warp];
+    bool row_ok[2];
+    float nam[2], Ri_ub[2];
+    unsigned oa[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int gi = r0 + rbase + (lane >> 2) + 8 * h;
+      row_ok[h] = gi < nA;
+      nam[h] = row_ok[h] ? kLow * nrmA[gi] : INFINITY;      // +inf: a padded row yields no upper bounds
+      oa[h] = row_ok[h] ? permA[gi] : 0u;                    // point index of the row
+      Ri_ub[h] = row_ok[h] ? INFINITY : -INFINITY;           // row threshold from the tile-local upper bounds (padded rows: never)
+    }
+    const uint32_t row_bits = (row_ok[0] ? 0x33333333u : 0u) | (row_ok[1] ? 0xCCCCCCCCu : 0u);  // fragment entries of valid rows
+    const float4* __restrict__ aex = reinterpret_cast<const float4*>(smem + 2 * kTcTileBytes);  // exact image of the A block
+    const uint32_t aH = sA + (uint32_t)((wg & 1) * 64 * 16), aL = aH + kTcTileBytes;           // operand rows of this warpgroup
     float* wcj = s_wcj[warp];
     unsigned short* wq = s_queue[warp];
     int evals_w = 0;
@@ -605,138 +579,182 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     long long p_wx = 0, p_wmm = 0, p_ld = 0, p_prep = 0, p_fil = 0, p_ev = 0;
     int p_tiles = 0;
     // column snapshot (best | point index) of the NEXT tile, fetched while the current one is processed when the scheduler
-    // has already published it (pf_tile = tile the prefetch belongs to, -1 = none)
+    // has already published it (pf_tile = tile the prefetch belongs to, -1 = none).  Lane l snapshots columns cb + l, cb + 32 + l.
     int pf_tile = -1;
-    unsigned long long pf_cb = ~0ull;
-    unsigned pf_ob = 0;
-    // shared per-tile column maxima (scheduler warp): after a tile is evaluated its 32 column bests are read again, and one tile
-    // later (the load has landed) their max refreshes tcm4[tile][cq]
-    unsigned* __restrict__ tcmw = tile_cmax + ((size_t)pair * (V >> 7)) * 4 + cq;
+    unsigned long long pf_cb[2] = {~0ull, ~0ull};
+    unsigned pf_ob[2] = {0u, 0u};
+    // shared per-tile column maxima (scheduler warp): after a tile is evaluated its 64 column bests are read again, and one tile
+    // later (the load has landed) their max refreshes tcm4[tile][g] of both 32-column groups g of the warp
+    unsigned* __restrict__ tcmw = tile_cmax + ((size_t)pair * (V >> 7)) * 4 + (cb >> 5);
     int rr_tile = -1;
-    unsigned rr_val = 0;
+    unsigned rr_val[2] = {0u, 0u};
     auto rr_flush = [&]() {
       if (rr_tile < 0) return;
-      const unsigned m = __reduce_max_sync(0xffffffffu, rr_val);
-      if (lane == 0) atomicMin(tcmw + (size_t)rr_tile * 4, m);
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        const unsigned m = __reduce_max_sync(0xffffffffu, rr_val[s]);
+        if (lane == 0) atomicMin(tcmw + (size_t)rr_tile * 4 + s, m);
+      }
       rr_tile = -1;
     };
     for (int k = 0;; ++k) {
-      const int ts = k & (kTcAcc - 1), st = k & (kTcStages - 1);
+      const int ts = k & (kTcDone - 1), st = k & (kTcStages - 1), hs = k & 1;
       const long long q0 = tick();
       if (alive) alive = mbar_wait(bar_fullx0 + 8 * st, (uint32_t)((k >> 2) & 1));  // the exact image is read below
       const long long q1 = tick();
       p_wx += q1 - q0;
       alive = __all_sync(0xffffffffu, alive);
-      if (!alive) { *v_dead = 1; break; }
-      const int jt = v_seq[k & 7];
-      if (jt < 0) break;
+      const int jt = alive ? v_seq[k & 7] : -1;
       const int c0 = jt * kTcN;
-      // snapshot of the column's best and its point index (lane = column); the load overlaps the wait for the MMAs
-      unsigned long long cb_cur = ~0ull;
-      unsigned ob = 0;
-      if (pf_tile == jt) {
-        cb_cur = pf_cb; ob = pf_ob;
-      } else if (c0 + cb + lane < nB) {
-        cb_cur = __ldcg(cbg + c0 + cb + lane);
-        ob = permB[c0 + cb + lane];
-      }
-      pf_tile = -1;
-      {  // the next position is normally decided already (the scheduler runs 3 ahead): start its snapshot loads now
+      // snapshot of the columns' bests and their point indices; the loads overlap the wait for the operands and the MMAs
+      unsigned long long cb_cur[2] = {~0ull, ~0ull};
+      unsigned ob[2] = {0u, 0u};
+      if (jt >= 0) {
+        if (pf_tile == jt) {
+#pragma unroll
+          for (int s = 0; s < 2; ++s) { cb_cur[s] = pf_cb[s]; ob[s] = pf_ob[s]; }
+        } else {
+#pragma unroll
+          for (int s = 0; s < 2; ++s)
+            if (c0 + cb + 32 * s + lane < nB) {
+              cb_cur[s] = __ldcg(cbg + c0 + cb + 32 * s + lane);
+              ob[s] = permB[c0 + cb + 32 * s + lane];
+            }
+        }
+        pf_tile = -1;
+        // the next position is normally decided already (the scheduler runs 3 ahead): start its snapshot loads now
         if (__all_sync(0xffffffffu, *v_ndec > k + 1)) {  // (volatile shared loads of one warp are performed in order: no fence,
           const int jn = v_seq[(k + 1) & 7];               //  which would wait for this warp's global loads in flight)
           if (jn >= 0) {
-            pf_tile = jn; pf_cb = ~0ull; pf_ob = 0;
-            if (jn * kTcN + cb + lane < nB) {
-              pf_cb = __ldcg(cbg + jn * kTcN + cb + lane);
-              pf_ob = permB[jn * kTcN + cb + lane];
+            pf_tile = jn;
+#pragma unroll
+            for (int s = 0; s < 2; ++s) {
+              pf_cb[s] = ~0ull; pf_ob[s] = 0u;
+              if (jn * kTcN + cb + 32 * s + lane < nB) {
+                pf_cb[s] = __ldcg(cbg + jn * kTcN + cb + 32 * s + lane);
+                pf_ob[s] = permB[jn * kTcN + cb + 32 * s + lane];
+              }
             }
           }
         }
       }
       const long long q2 = tick();
-      alive = mbar_wait(bar_mma0 + 8 * ts, (uint32_t)((k >> 2) & 1));
+      if (alive && jt >= 0) alive = mbar_wait(bar_fullhl0 + 8 * hs, (uint32_t)((k >> 1) & 1));  // operand images of the tile
+      alive = __all_sync(0xffffffffu, alive);
+      if (!wg_all(alive && jt >= 0, wg)) {  // end of the stripe, or a barrier that never completed: the warpgroup leaves together
+        if (!alive) *v_dead = 1;
+        break;
+      }
+      // ---- 15 wgmma: small cross terms first, then hi.hi
+      float d[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) d[i] = 0.0f;
+      {
+        const uint32_t bH = sHL0 + hs * kHLBytes + (uint32_t)(cb * 16), bL = bH + kTcTileBytes;
+        asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory");
+#pragma unroll
+        for (int kb = 0; kb < kTcKB; ++kb) {
+          wgmma_tf32_64x64x8(d, tc_smem_desc(aH + kb * 4096), tc_smem_desc(bL + kb * 4096), kb > 0);
+          wgmma_tf32_64x64x8(d, tc_smem_desc(aL + kb * 4096), tc_smem_desc(bH + kb * 4096), 1);
+        }
+#pragma unroll
+        for (int kb = 0; kb < kTcKB; ++kb) wgmma_tf32_64x64x8(d, tc_smem_desc(aH + kb * 4096), tc_smem_desc(bH + kb * 4096), 1);
+        asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
+        asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
+#pragma unroll
+        for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_mma0 + 8 * ts);  // this warp no longer reads the operand stage
       const long long q3 = tick();
       p_wmm += q3 - q2;
       p_prep += q2 - q1;
       ++p_tiles;
-      alive = __all_sync(0xffffffffu, alive);
-      if (!alive) { *v_dead = 1; break; }
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
       const bool skip = __any_sync(0xffffffffu, (*v_abort | *v_dead) != 0);
-      uint32_t v[32];
-      if (!skip) tc_ld32(tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(ts * kTcN + cb), v);
-      asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tfree0 + 8 * ts);  // accumulators are in registers: the stage may be overwritten
       const long long q4 = tick();
       p_ld += q4 - q3;
       if (!skip) {
         const float4* __restrict__ bex = reinterpret_cast<const float4*>(smem + kABytes + 2 * kHLBytes + st * kXBytes);  // exact image
-        // ---- per-column filter data of this warp's 32 columns (lane = column)
-        const float nbm = bex[9 * 128 + cb + lane].x;  // kLow |b'_j|^2, +inf for padded columns (split_desc_kernel)
-        const float dbest = cb_cur == ~0ull ? INFINITY : __uint_as_float((unsigned)(cb_cur >> 32));
-        float cj = nbm == INFINITY ? -INFINITY : dbest;  // column threshold: +inf while the column has no exact distance yet
-        const unsigned long long rb = v_rbest[row];
-        float Ri = fminf(Ri_ub, rb == ~0ull ? INFINITY : __uint_as_float((unsigned)(rb >> 32)));
-        wnbm[lane] = nbm;
+        // ---- per-column filter data of the lane's two snapshot columns
+        float dbest[2];
+        bool col_warm = false;
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          const float nbm = bex[9 * 128 + cb + 32 * s + lane].x;  // kLow |b'_j|^2, +inf for padded columns (split_desc_kernel)
+          dbest[s] = cb_cur[s] == ~0ull ? INFINITY : __uint_as_float((unsigned)(cb_cur[s] >> 32));
+          wcj[32 * s + lane] = nbm == INFINITY ? -INFINITY : dbest[s];  // column threshold: +inf while the column has no exact distance yet
+          col_warm |= cb_cur[s] == ~0ull && nbm != INFINITY;
+        }
+        float Ri[2];
+        bool row_warm = false;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const unsigned long long rb = v_rbest[rbase + (lane >> 2) + 8 * h];
+          Ri[h] = fminf(Ri_ub[h], rb == ~0ull ? INFINITY : __uint_as_float((unsigned)(rb >> 32)));
+          row_warm |= row_ok[h] && Ri[h] == INFINITY;
+        }
         __syncwarp();
-        const float4* __restrict__ wn4 = reinterpret_cast<const float4*>(wnbm);
-        const float4* __restrict__ wc4 = reinterpret_cast<const float4*>(wcj);
         // ---- warm-up: a row / column without any exact distance would let every entry through.  Upper bounds of the
         // exact minima come from the tile itself: UB_ij = d~_ij + e_ij = (1+c/2)(na'+nb') - 2 dot >= d_ij.
-        if (__any_sync(0xffffffffu, (row_ok && Ri == INFINITY) || (cb_cur == ~0ull && nbm != INFINITY))) {
+        if (__any_sync(0xffffffffu, row_warm || col_warm)) {
           if (lane == 0) atomicAdd(&s_warm, 1);
-          float rowub = INFINITY;
-          unsigned mine = 0xFFFFFFFFu;
+          float rowub[2] = {INFINITY, INFINITY};
 #pragma unroll
-          for (int c4 = 0; c4 < 8; ++c4) {
-            const float4 w = wn4[c4];
-            const float wv[4] = {w.x, w.y, w.z, w.w};
+          for (int i = 0; i < 32; i += 4) {
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int c = 4 * c4 + e;
-              const float ub = fmaf(kW, nam + wv[e], __uint_as_float(v[c]));
-              rowub = fminf(rowub, ub);
-              // min over the warp's 32 rows; an upper bound of a distance is >= 0 (bit patterns order them), anything else is dropped
-              const unsigned mn = __reduce_min_sync(0xffffffffu, ub >= 0.0f ? __float_as_uint(ub) : 0xFFFFFFFFu);
-              if (lane == c) mine = mn;
+            for (int e = 0; e < 2; ++e) {
+              const int c = 2 * i + cl + e;  // = 8 (i >> 2) + cl + e: this entry pair's column of the warp's 64
+              const float nbc = bex[9 * 128 + cb + c].x;
+              const float ub0 = fmaf(kW, nam[0] + nbc, d[i + e]), ub1 = fmaf(kW, nam[1] + nbc, d[i + 2 + e]);
+              rowub[0] = fminf(rowub[0], ub0);
+              rowub[1] = fminf(rowub[1], ub1);
+              // min over the warp's 16 rows (lanes of equal lane & 3); an upper bound of a distance is >= 0 (bit patterns order
+              // them), anything else is dropped
+              unsigned mn = min(ub0 >= 0.0f ? __float_as_uint(ub0) : 0xFFFFFFFFu, ub1 >= 0.0f ? __float_as_uint(ub1) : 0xFFFFFFFFu);
+              mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, 4));
+              mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, 8));
+              mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, 16));
+              if (lane < 4 && mn != 0xFFFFFFFFu && nbc != INFINITY) wcj[c] = fminf(wcj[c], __uint_as_float(mn));
             }
           }
-          if (mine != 0xFFFFFFFFu && nbm != INFINITY) cj = fminf(cj, __uint_as_float(mine));
-          if (row_ok) { Ri_ub = fminf(Ri_ub, rowub); Ri = fminf(Ri, Ri_ub); }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {  // min over the row's 64 columns (the 4 lanes of a row)
+            rowub[h] = fminf(rowub[h], __shfl_xor_sync(0xffffffffu, rowub[h], 1));
+            rowub[h] = fminf(rowub[h], __shfl_xor_sync(0xffffffffu, rowub[h], 2));
+            if (row_ok[h]) { Ri_ub[h] = fminf(Ri_ub[h], rowub[h]); Ri[h] = fminf(Ri[h], Ri_ub[h]); }
+          }
         }
-        wcj[lane] = cj;
         __syncwarp();
         const long long q5 = tick();
         p_prep += q5 - q4;
-        // ---- branch-free filter of this lane's row over the 32 columns: two compares and a predicated OR per entry
-        uint32_t mask = 0;
+        // ---- branch-free filter of the lane's 32 entries: two compares and a predicated OR per entry
+        const int ncol = nB - c0 - cb;  // valid columns of the warp's 64 (padding never competes, see below)
+        uint32_t mask = 0, col_bits = 0;
 #pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4) {
-          const float4 x = wc4[c4];
-          const float xv[4] = {x.x, x.y, x.z, x.w};
+        for (int i = 0; i < 32; i += 4) {
+          const float2 x = *reinterpret_cast<const float2*>(wcj + 2 * i + cl);
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
-            const int c = 4 * c4 + e;
-            const float lbv = __uint_as_float(v[c]);
+            const float lbv = d[i + e];
+            const float xc = (e & 1) ? x.y : x.x;
             asm("{\n\t.reg .pred p, q;\n\t"
                 "setp.le.f32 p, %1, %2;\n\t"
                 "setp.le.or.f32 q, %1, %3, p;\n\t"
                 "@q or.b32 %0, %0, %4;\n\t}\n"
                 : "+r"(mask)
-                : "f"(lbv), "f"(xv[e]), "f"(Ri), "r"(1u << c));
+                : "f"(lbv), "f"(xc), "f"(Ri[e >> 1]), "r"(1u << (i + e)));
+            if (2 * i + cl + (e & 1) < ncol) col_bits |= 1u << (i + e);
             if (kDbg) {
-              const unsigned oc = __shfl_sync(0xffffffffu, ob, c);
-              const float nbc = wnbm[c];
-              if (stripe == 0 && k == 0 && row_ok && c0 + cb + c < nB) dbg_tile[(size_t)oa * kTcN + oc] = fmaf(0.5f * kW, nam + nbc, lbv);
+              const int h = e >> 1, c = 2 * i + cl + (e & 1);
+              if (stripe == 0 && k == 0 && row_ok[h] && c < ncol)
+                dbg_tile[(size_t)oa[h] * kTcN + permB[c0 + cb + c]] = fmaf(0.5f * kW, nam[h] + bex[9 * 128 + cb + c].x, lbv);
             }
           }
         }
         // padding never competes: a padded row (-inf thresholds) would pass the column test of a column without a best
         // (-inf <= -inf), a padded column (+inf terms) the row test of a row without one -- and their zero images look
         // like the all-zero descriptor of an isolated point
-        mask &= __ballot_sync(0xffffffffu, c0 + cb + lane < nB);
-        if (!row_ok) mask = 0;
+        mask &= col_bits & row_bits;
         // ---- exact evaluation, one candidate per lane, 32 per round
         int remaining = __reduce_add_sync(0xffffffffu, __popc(mask));
         const long long q6 = tick();
@@ -746,30 +764,35 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
           int tot;
           int p = warp_excl_scan(__popc(mask), &tot);
           while (mask && p < 32) {
-            const int c = __ffs(mask) - 1;
+            const int i = __ffs(mask) - 1;
             mask &= mask - 1;
-            wq[p++] = (unsigned short)((lane << 5) | c);
+            wq[p++] = (unsigned short)((lane << 5) | i);
           }
           __syncwarp();
           const int nb = tot < 32 ? tot : 32;
           const int q = lane < nb ? wq[lane] : 0;
-          const int rl = q >> 5, c = q & 31;
+          const int sl = q >> 5, i = q & 31, h = (i >> 1) & 1;
+          const int rr = rbase + (sl >> 2) + 8 * h;            // row of the stripe
+          const int c = 8 * (i >> 2) + 2 * (sl & 3) + (i & 1);  // column of the warp's 64
           const int pcol = cb + c;
           float acc = 0.0f;
 #pragma unroll
           for (int kc = 0; kc < (kDescDim + 3) / 4; ++kc) {
-            const float4 a = aex[kc * 128 + rl], b = bex[kc * 128 + pcol];
+            const float4 a = aex[kc * 128 + rr], b = bex[kc * 128 + pcol];
             float diff = a.x - b.x;
             acc = __fmaf_rn(diff, diff, acc);
             if (4 * kc + 1 < kDescDim) { diff = a.y - b.y; acc = __fmaf_rn(diff, diff, acc); }
             if (4 * kc + 2 < kDescDim) { diff = a.z - b.z; acc = __fmaf_rn(diff, diff, acc); }
             if (4 * kc + 3 < kDescDim) { diff = a.w - b.w; acc = __fmaf_rn(diff, diff, acc); }
           }
-          const float dbc = __shfl_sync(0xffffffffu, dbest, c);
-          const unsigned oc = __shfl_sync(0xffffffffu, ob, c);   // point index of the candidate's column
-          const unsigned orow = __shfl_sync(0xffffffffu, oa, rl);  // ... and of its row
+          // column data live in lane c & 31 (snapshot s = c >> 5), row point indices in lane sl & ~3 (h)
+          const float db0 = __shfl_sync(0xffffffffu, dbest[0], c & 31), db1 = __shfl_sync(0xffffffffu, dbest[1], c & 31);
+          const unsigned ob0 = __shfl_sync(0xffffffffu, ob[0], c & 31), ob1 = __shfl_sync(0xffffffffu, ob[1], c & 31);
+          const unsigned oa0 = __shfl_sync(0xffffffffu, oa[0], sl & ~3), oa1 = __shfl_sync(0xffffffffu, oa[1], sl & ~3);
+          const float dbc = c < 32 ? db0 : db1;
+          const unsigned oc = c < 32 ? ob0 : ob1;  // point index of the candidate's column
+          const unsigned orow = h ? oa1 : oa0;      // ... and of its row
           if (lane < nb && acc == acc) {  // NaN never wins
-            const int rr = quad * 32 + rl;
             const unsigned long long pr = tc_pack(acc, (int)oc);
             if (pr < v_rbest[rr]) atomicMin(&s_rbest[rr], pr);
             if (acc <= dbc) atomicMin(cbg + c0 + pcol, tc_pack(acc, (int)orow));
@@ -790,10 +813,13 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
       rr_flush();
       if (!skip) {
         rr_tile = jt;
-        rr_val = 0;  // padding columns do not count
-        if (c0 + cb + lane < nB) {
-          const unsigned long long cbn = __ldcg(cbg + c0 + cb + lane);
-          rr_val = cbn == ~0ull ? 0x7F800000u : (unsigned)(cbn >> 32);
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          rr_val[s] = 0;  // padding columns do not count
+          if (c0 + cb + 32 * s + lane < nB) {
+            const unsigned long long cbn = __ldcg(cbg + c0 + cb + 32 * s + lane);
+            rr_val[s] = cbn == ~0ull ? 0x7F800000u : (unsigned)(cbn >> 32);
+          }
         }
       }
     }
@@ -801,7 +827,6 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     prof(20, p_wx); prof(21, p_wmm); prof(22, p_ld); prof(23, p_prep); prof(24, p_fil); prof(25, p_ev);
     prof(26, tick() - t_loop); prof(27, p_tiles);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   __syncthreads();
   const bool aborted = (s_abort | s_dead) != 0;
   if (kProf && threadIdx.x == 0) atomicAdd(stats + 9, (unsigned long long)(tick() - t_begin));
@@ -815,8 +840,6 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     }
   }
   if (!aborted && threadIdx.x < kTcM && r0 + (int)threadIdx.x < nA) rowbest[(size_t)pair * V + r0 + threadIdx.x] = s_rbest[threadIdx.x];
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem), "r"(kTcAcc * kTcN) : "memory");
 }
 
 static size_t tc_smem_bytes() { return (size_t)kTcImages * kTcTileBytes + 2 * 2 * (size_t)kTcTileBytes + (size_t)kTcStages * kTcTileBytes; }  // 220 KB

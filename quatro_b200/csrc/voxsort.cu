@@ -1,4 +1,4 @@
-// voxsort.cu -- K1: the voxel sort of a wave as a per-cloud, multi-CTA radix sort over the KEPT points only (sm_100a).
+// voxsort.cu -- K1: the voxel sort of a wave as a per-cloud, multi-CTA radix sort over the KEPT points only (sm_90a).
 //
 // Round 1 sorted (cloud | voxel | index) keys of EVERY raw point of the wave with cub::DeviceRadixSort (onesweep: 5 passes over
 // 38 key bits, 13 % of a street wave) although (a) the points the voxel filter drops (non-finite, flagged ground: 3 of 4

@@ -178,7 +178,7 @@ def _tc_rel_error(handle, a, b):
 
 
 def test_tc_filter_error_bound(handle):
-    """The tensor-core (tcgen05, 3xTF32) approximate distances must stay inside the margin the candidate filter assumes:
+    """The tensor-core (wgmma, 3xTF32) approximate distances must stay inside the margin the candidate filter assumes:
     |d~ - d| <= kTcC/2 * (|a'|^2 + |b'|^2) with kTcC = 1.2e-4, a' = a - mu (csrc/tc_match.cu).  Analytic budget: the dropped lo.lo
     term and the TF32 rounding of lo contribute <= 2^-21 (|a'|^2 + |b'|^2); the undocumented part is the fp32 accumulation inside
     the MMA (120 products per entry), measured here on random and adversarial descriptors.  The margin asserted is 3x."""
@@ -206,7 +206,7 @@ def test_tc_filter_error_bound(handle):
 
 
 def test_match_exact_kernel_and_tie_fallback(oracle, scan_pair):
-    """Default K6 = tcgen05 filter + in-kernel exact evaluation; thousands of identical descriptors make its stripes abort
+    """Default K6 = tensor-core filter + in-kernel exact evaluation; thousands of identical descriptors make its stripes abort
     to the exact CUDA-core kernel.  QB200_MATCH_EXACT=1 forces the exact kernel everywhere.  All must equal the oracle."""
     import os
     from quatro_b200.capi import Handle

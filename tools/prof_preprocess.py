@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Two scans through qb200_patchwork + qb200_segment_cloud (the workload of the ncu capture of the pre-processing kernels); prints one
-JSON line shaped like a bench line so that tools/ncu_facts.py can label the capture."""
+"""Two scans through qb200_patchwork + qb200_segment_cloud (a small workload for profiling the pre-processing kernels); prints one
+JSON line shaped like a bench line that labels the run."""
 import json
 import sys
 from pathlib import Path

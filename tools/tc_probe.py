@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Probe of the tcgen05 distance tile (qb200_debug_tc_distances): structured inputs that reveal row/column/K mapping."""
+"""Probe of the tensor-core distance tile (qb200_debug_tc_distances): structured inputs that reveal row/column/K mapping."""
 import sys
 from pathlib import Path
 import numpy as np

@@ -11,8 +11,8 @@ import numpy as np
 import torch
 from quatro_b200 import capi, synth
 
-NAMES = ["n_cta", "cta_total", "setup", "copy_prologue", "copy_wait_mma", "copy_decide", "copy_wait_sfree", "mma_wait_a", "mma_wait_hl",
-         "mma_wait_tfree", "mma_issue", "epi_wait_a", "epi_wait_x", "epi_wait_mma", "epi_ld", "epi_prep", "epi_filter", "epi_eval",
+NAMES = ["n_cta", "cta_total", "setup", "copy_prologue", "copy_wait_mma", "copy_decide", "copy_wait_sfree", "unused_15", "unused_16",
+         "unused_17", "unused_18", "epi_wait_a", "epi_wait_x", "epi_wait_hl_and_mma", "epi_vote", "epi_prep", "epi_filter", "epi_eval",
          "epi_loop_total", "epi_tiles"]
 
 def main():
