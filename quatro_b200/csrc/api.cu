@@ -95,15 +95,18 @@ int alloc_all(qb200_handle* h) {
   QB_CUDA_TRY(h, cudaEventCreate(&h->ev_fork));  // (timing enabled: QB200_TIMELINE measures the waves against it)
   QB_CUDA_TRY(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
   QB_CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_copied, cudaEventDisableTiming));
-  // the sort workspace serves the voxel sort (C*R items), the lattice / norm sorts (C*V items) and, afterwards, the duplicate-class
-  // tables of K6 (2S*V + 2S words in key_a): size it for the largest user
+  // the sort workspace serves the voxel sort (C*R items, digit histograms in val_a, chunk counts C*kVsChunks <= n_sort in val_b),
+  // the lattice / norm sorts (C*V items) and, afterwards, the duplicate-class tables of K6 (2S*V + 2S words in key_a): size it for
+  // the largest user
   const size_t n_sort = C * (R > V ? R : V) + 64;
+  const size_t n_hist = C * 256 * ((R + kVsTile - 1) / kVsTile);
   QB_ALLOC(h, h->key_a, n_sort);
   QB_ALLOC(h, h->key_b, n_sort);
-  QB_ALLOC(h, h->val_a, n_sort);
+  QB_ALLOC(h, h->val_a, n_sort > n_hist ? n_sort : n_hist);
   QB_ALLOC(h, h->val_b, n_sort);
   QB_ALLOC(h, h->aos_scratch, 2 * V * kDescDim);
-  h->cub_bytes = sort_temp_bytes((int)n_sort);
+  // the library radix sort only sorts lattice / norm keys of clouds too large for cloud_sort_kernel: at most C*V items
+  h->cub_bytes = sort_temp_bytes((int)(C * V));
   QB_CUDA_TRY(h, cudaMalloc(&h->cub_temp, h->cub_bytes));
   QB_ALLOC(h, h->vox_start, C * (V + 1));
   QB_ALLOC(h, h->vox_pts, C * V);
@@ -400,7 +403,7 @@ int qb200_voxelize(qb200_handle* h, const float* pts4, int32_t n, float leaf, in
   QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_cloud_ptr, h->h_cloud_ptr, sizeof(float4*), cudaMemcpyHostToDevice, h->stream));
   QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_cloud_n, h->h_cloud_n, sizeof(int), cudaMemcpyHostToDevice, h->stream));
   QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_raw_off, h->h_raw_off, 2 * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  if ((rc = launch_voxel(h, 1, n, leaf, skip_flagged))) return rc;
+  if ((rc = launch_voxel(h, 1, leaf, skip_flagged))) return rc;
   int nv = 0, st = 0;
   if ((rc = get_counter(h, h->ctr.n_vox, &nv))) return rc;
   if ((rc = get_counter(h, h->ctr.cloud_status, &st))) return rc;
@@ -766,7 +769,7 @@ static int wave_submit(qb200_handle* L, const qb200_pair* pairs, int w0, int np,
     QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, L->ev_copied, 0));
   }
   cudaEventRecord(L->ev[1], L->stream);
-  if ((rc = launch_voxel(L, ncl, total, p->voxel_size, p->skip_flagged))) return rc;
+  if ((rc = launch_voxel(L, ncl, p->voxel_size, p->skip_flagged))) return rc;
   cudaEventRecord(L->ev[2], L->stream);
   if ((rc = launch_fpfh(L, ncl, p->normal_radius, p->fpfh_radius, cell))) return rc;
   cudaEventRecord(L->ev[3], L->stream);
@@ -914,19 +917,6 @@ int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32
       left -= wave_n[n_waves++];
     }
     if (left > 0) n_waves = 0;  // more than ~60 waves: no special opening, walk uniformly below
-    // experiments: QB200_WAVE_PLAN="16,48,64,..." replaces the plan when it covers exactly n_pairs with waves of at most S pairs
-    if (const char* wp = getenv("QB200_WAVE_PLAN")) {
-      int plan[64], k = 0, sum = 0;
-      bool good = true;
-      for (const char* c = wp; *c && k < 63;) {
-        const int v = atoi(c);
-        if (v <= 0 || v > h->S) { good = false; break; }
-        plan[k++] = v; sum += v;
-        while (*c && *c != ',') ++c;
-        if (*c == ',') ++c;
-      }
-      if (good && sum == n_pairs) { n_waves = k; for (int i = 0; i < k; ++i) wave_n[i] = plan[i]; }
-    }
   }
   const bool planned = n_waves > 0;
   if (!planned) n_waves = (n_pairs + h->S - 1) / h->S;
@@ -1208,7 +1198,7 @@ int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t
     QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_cloud_n, h->h_cloud_n, (size_t)nc * sizeof(int), cudaMemcpyHostToDevice, h->stream));
     QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_raw_off, h->h_raw_off, (size_t)(nc + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
     if ((rc = wave_reset(h, nc))) return rc;
-    if ((rc = launch_voxel(h, nc, total, p->voxel_size, p->skip_flagged))) return rc;
+    if ((rc = launch_voxel(h, nc, p->voxel_size, p->skip_flagged))) return rc;
     if ((rc = launch_fpfh(h, nc, p->normal_radius, p->fpfh_radius, cell))) return rc;
     if ((rc = cache_copy(h, 1, nc))) return rc;
     QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // the pinned tables are reused by the next wave

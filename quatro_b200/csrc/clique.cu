@@ -720,19 +720,20 @@ __global__ void __launch_bounds__(32) clique_exact_kernel(const uint32_t* __rest
   if (lane == 0 && truncated) flags[pair] |= QB200_FLAG_CLIQUE_TRUNCATED;
 }
 
+// shared memory of the k-core peel: whole graphs up to L ~ 680 at max_corr 4096; the rest of the SM stays free for the dense
+// kernels of the other lanes
+constexpr size_t kKcoreSmemBudget = 144 * 1024;
+
 template <int WPL>
-static int launch_kcore(qb200_handle* h, int n_pairs, bool set_attr) {
+static int launch_kcore(qb200_handle* h, int n_pairs) {
   const int Lc = h->Lc, W = h->W;
   const size_t fixed = (size_t)(Lc + 2) * sizeof(int) + (size_t)3 * kKcWarps * 32 * WPL * sizeof(uint32_t) +
                        (size_t)(4 + kKcWarps) * Lc * sizeof(unsigned short);
-  // rows: what is left of a 144 KB budget (whole graphs up to L ~ 680 at max_corr 4096; the rest of the SM stays free for the
-  // dense kernels of the other lanes), at least the prefetch ring
-  static const size_t budget_kb = [] { const char* e = getenv("QB200_KCORE_SMEM_KB"); const int v = e ? atoi(e) : 0; return (size_t)(v >= 64 && v <= 220 ? v : 144); }();
-  size_t row_words = fixed + 8 * 1024 < budget_kb * 1024 ? (budget_kb * 1024 - fixed) / 4 : 0;
+  // rows: what is left of the budget, at least the prefetch ring
+  size_t row_words = fixed + 8 * 1024 < kKcoreSmemBudget ? (kKcoreSmemBudget - fixed) / 4 : 0;
   if (row_words < (size_t)kRing * W) row_words = (size_t)kRing * W;
   if (row_words > (size_t)Lc * W) row_words = (size_t)Lc * W;
   const size_t smem = fixed + row_words * 4;
-  (void)set_attr;
   if (int rc = ensure_dyn_smem(h, (const void*)kcore_kernel<WPL>, smem)) return rc;
   kcore_kernel<WPL><<<n_pairs, kKcWarps * 32, smem, h->stream>>>(h->adj, h->deg, h->ctr.n_corr, Lc, W, (int)row_words, h->kcore, h->korder,
                                                                  h->rank_of, h->by_rank, h->kbin, h->ctr.max_core);
@@ -770,14 +771,13 @@ int launch_clique(qb200_handle* h, int n_pairs, int mode, double kcore_thr, long
   // shared-memory adjacency cache of the descent: 14336 words (56 KB) hold graphs up to L ~ 660
   const int cache_words = 14336;
   const size_t sm_clique = (size_t)kCliqueWarps * Lc * sizeof(unsigned short) + (size_t)W * sizeof(uint32_t) + (size_t)cache_words * 4;
-  const bool set_attr = true;
   int rc;
   if ((rc = ensure_dyn_smem(h, (const void*)clique_cta_kernel, sm_clique))) return rc;
   if (mode == QB200_PMC_EXACT && (rc = ensure_exact_scratch(h))) return rc;
-  if (W <= 32) rc = launch_kcore<1>(h, n_pairs, set_attr);
-  else if (W <= 64) rc = launch_kcore<2>(h, n_pairs, set_attr);
-  else if (W <= 128) rc = launch_kcore<4>(h, n_pairs, set_attr);
-  else rc = launch_kcore<8>(h, n_pairs, set_attr);
+  if (W <= 32) rc = launch_kcore<1>(h, n_pairs);
+  else if (W <= 64) rc = launch_kcore<2>(h, n_pairs);
+  else if (W <= 128) rc = launch_kcore<4>(h, n_pairs);
+  else rc = launch_kcore<8>(h, n_pairs);
   if (rc) return rc;
   const dim3 gp((Lc + 7) / 8, n_pairs);
   permute_adj_kernel<<<gp, 256, 8 * W * sizeof(uint32_t), h->stream>>>(h->adj, h->ctr.n_corr, Lc, W, h->rank_of, h->adjp);

@@ -34,6 +34,7 @@ constexpr int kVoxShift = 31;
 constexpr uint64_t kVoxMask = (1ull << kVoxShift) - 1;
 constexpr uint64_t kVoxInvalid = kVoxMask;  // dx dy dz <= INT_MAX: a valid index is at most 2^31 - 2
 constexpr int kVsChunks = 64;               // contiguous chunks of a raw scan whose kept points the bbox pass counts
+constexpr int kVsTile = 2048;               // items per tile of the voxel sort (voxsort.cu): 8 warps x 8 rounds x 32 lanes
 
 __device__ __forceinline__ bool raw_point_kept(const float4 p, int skip_flagged) {
   return isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && !(skip_flagged && p.w < 0.0f);
@@ -91,7 +92,7 @@ __host__ __device__ __forceinline__ float ordered_float(int i) {
 }
 
 // number of 8-bit digits the voxel keys of a cloud occupy: the keys are below dx dy dz of pcl::VoxelGrid's own linear index
-// (voxel_keys / voxel_pack use the same min_b / div_b expressions)
+// (voxel_pack uses the same min_b / div_b expressions)
 __device__ __forceinline__ int vox_digits(const int* __restrict__ bbox, int n_valid, float inv_leaf) {
   if (n_valid <= 0) return 0;
   const long long m0 = (long long)floorf(ordered_float(bbox[0]) * inv_leaf), m1 = (long long)floorf(ordered_float(bbox[1]) * inv_leaf),

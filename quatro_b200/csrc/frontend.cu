@@ -6,15 +6,11 @@
 //
 // Design: every cloud of a batch wave is processed by the same launches (grid.y = cloud); sizes
 // stay on the device.  Voxelisation is a stable per-cloud radix sort of the (voxel | point index) items of the KEPT
-// points (voxsort.cu; the device-wide library sort below is the fallback for handles too small for its scratch and the
-// QB200_VOXEL_SORT=cub A/B switch) followed by a segmented, in-order centroid sum (bit-identical to the sequential CPU sum).  The kd-tree is
+// points (voxsort.cu) followed by a segmented, in-order centroid sum (bit-identical to the sequential CPU sum).  The kd-tree is
 // replaced by a sorted-cell lattice: a point's neighbours are found by (2m+1)^2 binary searches for
 // x-runs of cells, visited in ascending (cell, index) order -- the accumulation order the CPU oracle
 // uses, so the single-pass float covariance matches bit for bit.
 #include <cub/device/device_radix_sort.cuh>
-
-#include <cstdlib>
-#include <cstring>
 
 #include "fpfh_math.cuh"
 #include "handle.cuh"
@@ -40,15 +36,6 @@ int sort_pairs(qb200_handle* h, int n_items, int end_bit) {
   return QB200_OK;
 }
 
-// keys only (the payload rides in the low key bits below begin_bit: 8 instead of 12 bytes per item and pass)
-int sort_keys(qb200_handle* h, int n_items, int begin_bit, int end_bit) {
-  if (n_items <= 0) return QB200_OK;
-  size_t bytes = h->cub_bytes;
-  QB_CUDA_TRY(h, cub::DeviceRadixSort::SortKeys(h->cub_temp, bytes, h->key_a, h->key_b, n_items, begin_bit, end_bit, h->stream));
-  h->launches += 1 + (end_bit - begin_bit + 7) / 8;
-  return QB200_OK;
-}
-
 static int clog2(int n) {
   int b = 0;
   while ((1 << b) < n) ++b;
@@ -56,10 +43,10 @@ static int clog2(int n) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// K1a: bounding box of the kept raw points (one pass, 128-bit loads), then raw point -> (cloud | voxel) key.
-// The voxel key is PCL's own linear index  (i - min_i) + (j - min_j) dx + (k - min_k) dx dy  ([EXT] pcl::VoxelGrid,
+// K1a: bounding box and per-chunk counts of the kept raw points (one pass, 128-bit loads).  The voxel key that the pack pass
+// (voxsort.cu) then builds is PCL's own linear index  (i - min_i) + (j - min_j) dx + (k - min_k) dx dy  ([EXT] pcl::VoxelGrid,
 // called from include/quatro.hpp:49-57), which the library requires to fit an int: at most 31 key bits, and for a given cloud
-// only the bits of dx dy dz (vox_digits()); the library-sort fallback adds the cloud id above them (5 passes over 38 bits).
+// only the bits of dx dy dz (vox_digits()).
 // ------------------------------------------------------------------------------------------------
 
 __global__ void __launch_bounds__(256) voxel_bbox_kernel(const float4* const* __restrict__ cloud_ptr, const int* __restrict__ cloud_n,
@@ -139,45 +126,15 @@ __global__ void __launch_bounds__(256) voxel_bbox_kernel(const float4* const* __
   }
 }
 
-__global__ void __launch_bounds__(256) voxel_keys_kernel(const float4* const* __restrict__ cloud_ptr, const int* __restrict__ cloud_n,
-                                                         const int* __restrict__ raw_off, float inv_leaf, int skip_flagged,
-                                                         const int* __restrict__ bbox, const int* __restrict__ n_valid, int idx_bits,
-                                                         uint64_t* __restrict__ keys) {
-  const int cloud = blockIdx.y;
-  const int n = cloud_n[cloud], off = raw_off[cloud];
-  const float4* __restrict__ pts = cloud_ptr[cloud];
-  // min_b / div_b of pcl::VoxelGrid::applyFilter
-  long long m0 = 0, m1 = 0, m2 = 0, d0 = 1, d1 = 1, d2 = 1;
-  if (n_valid[cloud] > 0) {
-    const int* b = bbox + cloud * 6;
-    m0 = (long long)floorf(ordered_float(b[0]) * inv_leaf); m1 = (long long)floorf(ordered_float(b[1]) * inv_leaf);
-    m2 = (long long)floorf(ordered_float(b[2]) * inv_leaf);
-    d0 = (long long)floorf(ordered_float(b[3]) * inv_leaf) - m0 + 1; d1 = (long long)floorf(ordered_float(b[4]) * inv_leaf) - m1 + 1;
-    d2 = (long long)floorf(ordered_float(b[5]) * inv_leaf) - m2 + 1;
-  }
-  (void)d2;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float4 p = __ldg(pts + i);
-    uint64_t cell = kVoxInvalid;
-    if (raw_point_kept(p, skip_flagged)) {
-      const int ci = (int)floorf(p.x * inv_leaf), cj = (int)floorf(p.y * inv_leaf), ck = (int)floorf(p.z * inv_leaf);
-      if (cell_ok(ci, cj, ck)) {
-        const long long lin = ((long long)ci - m0) + ((long long)cj - m1) * d0 + ((long long)ck - m2) * d0 * d1;
-        if (lin >= 0 && lin < (long long)kVoxInvalid) cell = (uint64_t)lin;  // otherwise the cloud is refused (overflow) anyway
-      }
-    }
-    keys[off + i] = ((((uint64_t)cloud << kVoxShift) | cell) << idx_bits) | (uint64_t)i;  // stable sort on the bits above idx_bits
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
 // K1b / K2b: run heads of the sorted keys of one cloud -> start position of every voxel / cell.
 // One CTA per cloud walks its segment with a carried block scan (sizes never leave the device).
-//   mode 0 (voxels): segment = [raw_off, raw_off + n_raw), writes starts[], n_out = #voxels
-//   mode 1 (cells):  segment = [cloud*V, cloud*V + V),     writes starts[] and cell keys
+//   mode 0 (voxels): segment = [raw_off, raw_off + n_valid) of the voxel sort's A (keys) or B (keys_b) array, by the parity of
+//                    the cloud's digit count (voxsort.cu); writes starts[], n_out = #voxels
+//   mode 1 (cells):  segment = [cloud*V, cloud*V + V) of keys, writes starts[] and cell keys
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) run_heads_kernel(int mode, const uint64_t* keys, const uint64_t* keys_alt, const int* __restrict__ seg_off,
-                                                         const int* __restrict__ seg_n, int V, int key_shift, float inv_leaf, const int* __restrict__ bbox,
+__global__ void __launch_bounds__(1024) run_heads_kernel(int mode, const uint64_t* keys, const uint64_t* keys_b, const int* __restrict__ seg_off,
+                                                         int V, int key_shift, float inv_leaf, const int* __restrict__ bbox,
                                                          const int* __restrict__ n_valid_in, int* __restrict__ starts,
                                                          uint64_t* __restrict__ cell_keys, int* __restrict__ n_out, int* __restrict__ n_valid_out,
                                                          int* __restrict__ cloud_status) {
@@ -185,11 +142,8 @@ __global__ void __launch_bounds__(1024) run_heads_kernel(int mode, const uint64_
   __shared__ int s_overflow;
   const int cloud = blockIdx.x;
   const int off = mode == 0 ? seg_off[cloud] : cloud * V;
-  int n = mode == 0 ? seg_n[cloud] : V;
-  if (mode == 0 && keys_alt) {  // own voxel sort: the kept points only, in A or B by the parity of the cloud's digit count
-    n = n_valid_in[cloud];
-    if (vox_digits(bbox + cloud * 6, n, inv_leaf) & 1) keys = keys_alt;
-  }
+  const int n = mode == 0 ? n_valid_in[cloud] : V;
+  if (mode == 0 && (vox_digits(bbox + cloud * 6, n, inv_leaf) & 1)) keys = keys_b;
   if (threadIdx.x == 0) {
     int ov = 0;
     if (mode == 0 && n_valid_in[cloud] > 0) {
@@ -267,14 +221,14 @@ __global__ void __launch_bounds__(1024) run_heads_kernel(int mode, const uint64_
 // K1c: centroid of each voxel, summed in original point order (stable sort) -> identical to the
 // sequential CPU sum.  One thread per voxel; points are gathered through the sorted index.
 __global__ void __launch_bounds__(128) voxel_centroid_kernel(const float4* const* __restrict__ cloud_ptr, const int* __restrict__ raw_off,
-                                                             const uint64_t* sorted_keys, const uint64_t* keys_alt, const int* __restrict__ bbox,
+                                                             const uint64_t* sorted_keys, const uint64_t* keys_b, const int* __restrict__ bbox,
                                                              const int* __restrict__ n_valid, float inv_leaf, uint64_t idx_mask,
                                                              const int* __restrict__ starts, const int* __restrict__ n_vox, int V,
                                                              float4* __restrict__ vox_pts) {
   const int cloud = blockIdx.y;
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n_vox[cloud]) return;
-  if (keys_alt && (vox_digits(bbox + cloud * 6, n_valid[cloud], inv_leaf) & 1)) sorted_keys = keys_alt;
+  if (vox_digits(bbox + cloud * 6, n_valid[cloud], inv_leaf) & 1) sorted_keys = keys_b;
   const float4* __restrict__ pts = cloud_ptr[cloud];
   const int off = raw_off[cloud];
   const int a = starts[(size_t)cloud * (V + 1) + r], b = starts[(size_t)cloud * (V + 1) + r + 1];
@@ -685,35 +639,20 @@ __global__ void desc_from_aos_kernel(const float* __restrict__ in, int V, int n,
 // ------------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------------
-int launch_voxel(qb200_handle* h, int n_clouds, int total_raw, float leaf, int skip_flagged) {
+int launch_voxel(qb200_handle* h, int n_clouds, float leaf, int skip_flagged) {
   if (n_clouds <= 0) return QB200_OK;
   const float inv = 1.0f / leaf;
-  const dim3 gk(64, n_clouds);
   const dim3 gb(n_clouds >= 16 ? 16 : 64, n_clouds);  // ~30 points per thread when the batch fills the device on its own
   int* chunk_cnt = reinterpret_cast<int*>(h->val_b);   // [clouds][kVsChunks]
   voxel_bbox_kernel<<<gb, 256, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, inv, skip_flagged, h->ctr.bbox, h->ctr.n_valid, h->ctr.cloud_status,
                                                chunk_cnt);
+  h->launches += 1;
   const int idx_bits = clog2(h->R > 2 ? h->R : 2);  // point index inside its scan
-  // QB200_VOXEL_SORT=cub: round 1's device-wide library sort of every raw point (kept for A/B runs; results are identical)
-  static const bool use_cub = getenv("QB200_VOXEL_SORT") && !strcmp(getenv("QB200_VOXEL_SORT"), "cub");
-  const bool own = !use_cub && h->R >= 16384;   // the histogram scratch (val_a) holds 256 x R / 2048 words per cloud
-  const uint64_t* keys_alt = nullptr;
-  if (own) {
-    h->launches += 1;
-    if (int rc = launch_voxel_sort(h, n_clouds, inv, skip_flagged, idx_bits)) return rc;
-    keys_alt = h->key_b;
-  } else {
-    voxel_keys_kernel<<<gk, 256, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, h->d_raw_off, inv, skip_flagged, h->ctr.bbox, h->ctr.n_valid,
-                                                 idx_bits, h->key_a);
-    h->launches += 2;
-    const int rc = sort_keys(h, total_raw, idx_bits, idx_bits + kVoxShift + clog2(n_clouds > 1 ? n_clouds : 2));
-    if (rc) return rc;
-  }
-  const uint64_t* sorted = own ? h->key_a : h->key_b;
-  run_heads_kernel<<<n_clouds, 1024, 0, h->stream>>>(0, sorted, keys_alt, h->d_raw_off, h->d_cloud_n, h->V, idx_bits, inv, h->ctr.bbox, h->ctr.n_valid,
+  if (int rc = launch_voxel_sort(h, n_clouds, inv, skip_flagged, idx_bits)) return rc;
+  run_heads_kernel<<<n_clouds, 1024, 0, h->stream>>>(0, h->key_a, h->key_b, h->d_raw_off, h->V, idx_bits, inv, h->ctr.bbox, h->ctr.n_valid,
                                                      h->vox_start, nullptr, h->ctr.n_vox, nullptr, h->ctr.cloud_status);
   const dim3 gc((h->V + 127) / 128, n_clouds);
-  voxel_centroid_kernel<<<gc, 128, 0, h->stream>>>(h->d_cloud_ptr, h->d_raw_off, sorted, keys_alt, h->ctr.bbox, h->ctr.n_valid, inv,
+  voxel_centroid_kernel<<<gc, 128, 0, h->stream>>>(h->d_cloud_ptr, h->d_raw_off, h->key_a, h->key_b, h->ctr.bbox, h->ctr.n_valid, inv,
                                                    (1ull << idx_bits) - 1, h->vox_start, h->ctr.n_vox, h->V, h->vox_pts);
   h->launches += 2;
   QB_CUDA_TRY(h, cudaGetLastError());
@@ -733,7 +672,7 @@ int launch_fpfh(qb200_handle* h, int n_clouds, float normal_radius, float fpfh_r
   int rc = launch_cloud_sort(h, n_clouds, h->ctr.n_vox, 18, 36);  // fields of cell_key(): i | j | k
   if (rc == QB200_ERR_UNSUPPORTED) rc = sort_pairs(h, n_clouds * V, kCloudShift + clog2(n_clouds > 1 ? n_clouds : 2));
   if (rc) return rc;
-  run_heads_kernel<<<n_clouds, 1024, 0, h->stream>>>(1, h->key_b, nullptr, nullptr, nullptr, V, 0, inv, nullptr, nullptr, h->cell_start, h->cell_key,
+  run_heads_kernel<<<n_clouds, 1024, 0, h->stream>>>(1, h->key_b, nullptr, nullptr, V, 0, inv, nullptr, nullptr, h->cell_start, h->cell_key,
                                                      h->ctr.n_cells, h->ctr.n_lat, h->ctr.cloud_status);
   const dim3 gp((V + 127) / 128, n_clouds);
   nbr_list_kernel<<<gp, kNbrThreads, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->cell_key, h->cell_start, h->val_b, h->ctr.n_cells, inv, mf,

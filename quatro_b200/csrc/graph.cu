@@ -13,27 +13,25 @@
 // The kernel evaluates this in fp32 with A, B in Gram form (|a_i|^2 + |a_j|^2 - 2 a_i.a_j: 4 instead of 6 operations per
 // distance) -- ~18 instructions per pair test -- together with a RIGOROUS bound of its own rounding error:
 //        |t_c - t| <= 36u M |D_c| + 1500 u^2 M^2 + 46 u beta^2 M =: q,   u = 2^-24,  M >= |a_i|^2+|b_i|^2+|a_j|^2+|b_j|^2 + 2 beta^2
-// (derivation in DESIGN.md 5.2).  Each lane evaluates its columns in pairs of scalar IEEE-rn operations (explicit
+// (derivation in DESIGN.md 5.2).  Each lane evaluates its columns with scalar IEEE-rn operations (explicit
 // __fmaf_rn / __fadd_rn: no contraction decides the rounding).  Only pairs with |t_c| <= q -- a band of ~1e-4 relative width around the threshold --
 // or with both distances ~0 (the literal expression is NaN -> false for coincident duplicates) evaluate the literal fp64
 // expression, so the adjacency is bit-identical to the fp64 reference.
 //
 // Work decomposition.  A WARP work item is 64 rows x 128 columns of the upper triangle (any pair of the launch: one global item
 // list); the warp stages its 64 row points in shared memory as (-2a, |a|^2 - beta^2/4 | -2b, |b|^2 - beta^2/4) -- read back as
-// broadcast operands of the FMAs -- and each lane keeps FOUR columns in registers as two pairs.  No CTA barrier in
+// broadcast operands of the FMAs -- and each lane keeps FOUR columns in registers.  No CTA barrier in
 // the item loop.  Result bits are shifted in from the SIGN BITS of t, s' and |t| - q with funnel shifts (no compare / select per
 // test); a warp shuffle transpose turns the per-column words into the row-major half, so both halves of the symmetric matrix come
 // out of one evaluation of the M pair tests.  (Timing experiment, round 2: without the two 4-byte row-strided stores and the
 // transpose per 32 x 32 block the kernel runs 0.144 instead of 0.174 ms at 32 x L = 3000.)
-#include <stdlib.h>
-
 #include "handle.cuh"
 
 namespace qb {
 
 constexpr int kGW = 4;    // warps per CTA
-// columns per lane = template parameter GC (2 or 4: one or two packed pairs; a warp covers GC x 32 columns)
-constexpr int kGRB = 2;   // 32-row blocks per work item (a WARP's work item: 64 rows x GC x 32 columns)
+constexpr int kGC = 4;    // columns per lane (a warp covers kGC x 32 columns)
+constexpr int kGRB = 2;   // 32-row blocks per work item (a WARP's work item: 64 rows x kGC x 32 columns)
 
 // the literal reference expression (fp64, no FMA contraction: library is built with -fmad=false)
 __device__ __noinline__ bool tim_consistent_fp64(const float4 ai, const float4 aj, const float4 bi, const float4 bj, double beta) {
@@ -62,14 +60,6 @@ __device__ __forceinline__ uint32_t warp_transpose32(uint32_t x) {
   return x;
 }
 
-// fp32 column pairs: two IEEE-rn scalar operations per helper (sm_90 has no packed fp32 FMA)
-struct f32x2 { float x, y; };
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) { return {lo, hi}; }
-__device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) { lo = v.x; hi = v.y; }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return {__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return {__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
-__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) { return {__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)}; }
-
 struct GraphConst {
   float b2, hb2q, twob2, b4;   // beta^2, beta^2/4, 2 beta^2, beta^4 (fp32)
   float c1, c2, c3;            // q = c1 M |D| + (c2 M + c3) M
@@ -82,7 +72,6 @@ struct GraphConst {
 // rows staged once per CTA -- 29 % of the items of an L = 3000 pair touch the diagonal, where one of the four warps has half the work,
 // and the barrier around the staging was the top stall reason (1.5 warps per issue).  Every warp now stages its own 64 rows
 // (~1 % of the item's instructions) and no barrier is left in the item loop.
-template <int kGC>
 __device__ __forceinline__ int graph_items(int L) {
   if (L <= 0) return 0;
   const int nb = (L + 31) >> 5, ncq = (nb + kGC - 1) / kGC, nrg = (nb + kGRB - 1) / kGRB;
@@ -93,11 +82,9 @@ __device__ __forceinline__ int graph_items(int L) {
 
 constexpr int kGraphMaxPairs = 2048;  // = the largest max_batch_slots qb200_create accepts
 
-template <int kGC>
-__global__ void __launch_bounds__(kGW * 32, kGC == 2 ? 8 : 4) tim_graph_kernel(const float4* __restrict__ ma, const float4* __restrict__ mb,
-                                                             const int* __restrict__ n_corr, int n_pairs, int Lc, int W, GraphConst gc,
-                                                             uint32_t* __restrict__ adj) {
-  constexpr int kGP = kGC / 2;
+__global__ void __launch_bounds__(kGW * 32, 4) tim_graph_kernel(const float4* __restrict__ ma, const float4* __restrict__ mb,
+                                                                const int* __restrict__ n_corr, int n_pairs, int Lc, int W, GraphConst gc,
+                                                                uint32_t* __restrict__ adj) {
   __shared__ float4 s_row[kGW][kGRB * 32][2];  // per warp and row: (-2a, |a|^2 - beta^2/4) | (-2b, |b|^2 - beta^2/4)
   __shared__ int s_pref[kGraphMaxPairs + 1];   // exclusive prefix of the pairs' item counts: the warps stride over ALL pairs' items,
   __shared__ int s_scan[33];                   // so a pair with many correspondences is spread over the whole grid
@@ -107,7 +94,7 @@ __global__ void __launch_bounds__(kGW * 32, kGC == 2 ? 8 : 4) tim_graph_kernel(c
     int carry = 0;
     for (int base = 0; base < n_pairs; base += kGW * 32) {
       const int p = base + tid;
-      const int c = p < n_pairs ? graph_items<kGC>(n_corr[p]) : 0;
+      const int c = p < n_pairs ? graph_items(n_corr[p]) : 0;
       int tot;
       const int ex = block_excl_scan(c, s_scan, &tot);
       if (p < n_pairs) s_pref[p] = carry + ex;
@@ -172,16 +159,7 @@ __global__ void __launch_bounds__(kGW * 32, kGC == 2 ? 8 : 4) tim_graph_kernel(c
       cb[c] = make_float4(pb.x, pb.y, pb.z, nbn - gc.hb2q);
       cm[c] = na + nbn;
     }
-    // the columns as packed pairs
-    f32x2 cax[kGP], cay[kGP], caz[kGP], can[kGP], cbx[kGP], cby[kGP], cbz[kGP], cbn[kGP];
-#pragma unroll
-    for (int p = 0; p < kGP; ++p) {
-      cax[p] = pk2(ca[2 * p].x, ca[2 * p + 1].x); cay[p] = pk2(ca[2 * p].y, ca[2 * p + 1].y);
-      caz[p] = pk2(ca[2 * p].z, ca[2 * p + 1].z); can[p] = pk2(ca[2 * p].w, ca[2 * p + 1].w);
-      cbx[p] = pk2(cb[2 * p].x, cb[2 * p + 1].x); cby[p] = pk2(cb[2 * p].y, cb[2 * p + 1].y);
-      cbz[p] = pk2(cb[2 * p].z, cb[2 * p + 1].z); cbn[p] = pk2(cb[2 * p].w, cb[2 * p + 1].w);
-    }
-    const f32x2 ntwob2 = pk2(-gc.twob2, -gc.twob2), nb4 = pk2(-gc.b4, -gc.b4);
+    const float ntwob2 = -gc.twob2, nb4 = -gc.b4;
 #pragma unroll
     for (int rbl = 0; rbl < kGRB; ++rbl) {
       const int bi = rg * kGRB + rbl;
@@ -203,28 +181,19 @@ __global__ void __launch_bounds__(kGW * 32, kGC == 2 ? 8 : 4) tim_graph_kernel(c
 #pragma unroll 8
       for (int r = 0; r < 32; ++r) {
         const float4 r0 = row_p[r][0], r1 = row_p[r][1];
-        const f32x2 rax = pk2(r0.x, r0.x), ray = pk2(r0.y, r0.y), raz = pk2(r0.z, r0.z), ran = pk2(r0.w, r0.w);
-        const f32x2 rbx = pk2(r1.x, r1.x), rby = pk2(r1.y, r1.y), rbz = pk2(r1.z, r1.z), rbn = pk2(r1.w, r1.w);
 #pragma unroll
-        for (int p = 0; p < kGP; ++p) {
-          const f32x2 Ap = fma2(rax, cax[p], fma2(ray, cay[p], fma2(raz, caz[p], add2(ran, can[p]))));
-          const f32x2 Bp = fma2(rbx, cbx[p], fma2(rby, cby[p], fma2(rbz, cbz[p], add2(rbn, cbn[p]))));
-          const f32x2 D = sub2(Ap, Bp), sp = add2(Ap, Bp);
-          const f32x2 ng = fma2(ntwob2, sp, nb4);               // -g = -(2 beta^2 s' + beta^4)
-          const f32x2 t = fma2(D, D, ng);
-          float t0, t1, s0, s1, D0, D1;
-          upk2(t, t0, t1); upk2(sp, s0, s1); upk2(D, D0, D1);
+        for (int c = 0; c < kGC; ++c) {
+          const float Ap = __fmaf_rn(r0.x, ca[c].x, __fmaf_rn(r0.y, ca[c].y, __fmaf_rn(r0.z, ca[c].z, __fadd_rn(r0.w, ca[c].w))));
+          const float Bp = __fmaf_rn(r1.x, cb[c].x, __fmaf_rn(r1.y, cb[c].y, __fmaf_rn(r1.z, cb[c].z, __fadd_rn(r1.w, cb[c].w))));
+          const float D = __fsub_rn(Ap, Bp), sp = __fadd_rn(Ap, Bp);
+          const float ng = __fmaf_rn(ntwob2, sp, nb4);           // -g = -(2 beta^2 s' + beta^4)
+          const float t = __fmaf_rn(D, D, ng);
           // |t| - q, q = |D| c1 M + K (|.| is an operand modifier)
-          const float w0 = fabsf(t0) - fmaf(fabsf(D0), qa[2 * p], qk[2 * p]);
-          const float w1 = fabsf(t1) - fmaf(fabsf(D1), qa[2 * p + 1], qk[2 * p + 1]);
-          wt[2 * p] = __funnelshift_l(__float_as_uint(t0), wt[2 * p], 1);          // sign(t):  t < 0
-          wt[2 * p + 1] = __funnelshift_l(__float_as_uint(t1), wt[2 * p + 1], 1);
-          ws[2 * p] = __funnelshift_l(__float_as_uint(s0), ws[2 * p], 1);          // sign(s'): s' < 0
-          ws[2 * p + 1] = __funnelshift_l(__float_as_uint(s1), ws[2 * p + 1], 1);
-          wa[2 * p] = __funnelshift_l(__float_as_uint(w0), wa[2 * p], 1);          // |t| inside the error band
-          wa[2 * p + 1] = __funnelshift_l(__float_as_uint(w1), wa[2 * p + 1], 1);
-          smin[2 * p] = fminf(smin[2 * p], s0);
-          smin[2 * p + 1] = fminf(smin[2 * p + 1], s1);
+          const float w = fabsf(t) - fmaf(fabsf(D), qa[c], qk[c]);
+          wt[c] = __funnelshift_l(__float_as_uint(t), wt[c], 1);    // sign(t):  t < 0
+          ws[c] = __funnelshift_l(__float_as_uint(sp), ws[c], 1);   // sign(s'): s' < 0
+          wa[c] = __funnelshift_l(__float_as_uint(w), wa[c], 1);    // |t| inside the error band
+          smin[c] = fminf(smin[c], sp);
         }
       }
       const int nvalid = L - bi * 32;
@@ -318,12 +287,9 @@ int launch_graph(qb200_handle* h, int n_pairs, double noise_bound, double cbar2)
   gc.c2 = (float)(1500.0 * u * u * 1.02);
   gc.c3 = (float)(46.0 * u * beta * beta * 1.02);
   gc.two_b2_slack = (float)(2.0 * beta * beta * 1.00001);
-  // one wave of resident CTAs whose warps stride over every pair's work items (64 rows x 128 columns each).  QB200_GRAPH_COLS=2 selects the 2-columns-per-lane variant
-  // (64 registers, 8 CTAs per SM) for A/B runs; results are identical
-  static const int cols = (getenv("QB200_GRAPH_COLS") && getenv("QB200_GRAPH_COLS")[0] == '2') ? 2 : 4;
+  // one wave of resident CTAs whose warps stride over every pair's work items (64 rows x 128 columns each)
   cudaEventRecord(h->kev[2], h->stream);
-  if (cols == 2) tim_graph_kernel<2><<<dim3(h->n_sm * 8), kGW * 32, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, n_pairs, h->Lc, h->W, gc, h->adj);
-  else tim_graph_kernel<4><<<dim3(h->n_sm * 4), kGW * 32, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, n_pairs, h->Lc, h->W, gc, h->adj);
+  tim_graph_kernel<<<dim3(h->n_sm * 4), kGW * 32, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, n_pairs, h->Lc, h->W, gc, h->adj);
   cudaEventRecord(h->kev[3], h->stream);
   h->kev_armed[1] = 1;
   const dim3 gd((h->Lc + 7) / 8, n_pairs);

@@ -35,9 +35,9 @@ struct qb200_handle {
   cudaEvent_t ev_copied;      // this lane's scans have arrived (recorded on the copy stream)
 
   // ---- sort workspace (voxel sort, then lattice sort) ----
-  uint64_t *key_a, *key_b;    // [2S*R]
-  uint32_t *val_a, *val_b;    // [2S*R]
-  void* cub_temp; size_t cub_bytes;
+  uint64_t *key_a, *key_b;    // [2S*max(R,V)]
+  uint32_t *val_a, *val_b;    // [2S*max(R,V)]; val_a also holds the voxel sort's digit histograms
+  void* cub_temp; size_t cub_bytes;  // library radix sort of up to 2S*V items (lattice / norm sorts of clouds too large for sort.cu)
   float* aos_scratch;         // [2*V*33] AoS descriptors of the stage entry points (qb200_compute_fpfh / qb200_match)
 
   // ---- front end ----
@@ -124,7 +124,7 @@ struct qb200_handle {
 namespace qb {
 
 // Stage launchers (each enqueues kernels on h->stream for clouds/pairs [0, n) of the current wave).
-int launch_voxel(qb200_handle* h, int n_clouds, int total_raw, float leaf, int skip_flagged);
+int launch_voxel(qb200_handle* h, int n_clouds, float leaf, int skip_flagged);
 int launch_fpfh(qb200_handle* h, int n_clouds, float normal_radius, float fpfh_radius, float cell);
 int launch_match(qb200_handle* h, int n_pairs, const qb200_params& p);
 int launch_graph(qb200_handle* h, int n_pairs, double noise_bound, double cbar2);
@@ -149,7 +149,6 @@ int collect_batch(qb200_handle* h, const qb200_result* dst);  // api.cu: wait fo
 // (function, device), not of a handle: handles of different capacities share it, so it is only ever raised (process-wide maximum).
 int ensure_dyn_smem(qb200_handle* h, const void* kernel, size_t bytes);
 int sort_pairs(qb200_handle* h, int n_items, int end_bit);
-int sort_keys(qb200_handle* h, int n_items, int begin_bit, int end_bit);
 int launch_voxel_sort(qb200_handle* h, int n_clouds, float inv_leaf, int skip_flagged, int idx_bits);
 int launch_cloud_sort(qb200_handle* h, int n_clouds, const int* n_items, int f1, int f2);
 

@@ -282,7 +282,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, const int* __restrict__ n_vox, int V,
              const uint32_t* __restrict__ perm, unsigned long long* __restrict__ rowbest, unsigned long long* __restrict__ colbest_r,
              unsigned* __restrict__ tile_cmax, int* __restrict__ fallback, unsigned long long* __restrict__ stats,
-             float* __restrict__ dbg_tile, int no_prune) {
+             float* __restrict__ dbg_tile) {
   extern __shared__ __align__(128) unsigned char smem[];  // 220 KB of operand images; static + dynamic must stay <= 227 KB
   __shared__ uint64_t s_fullx[kTcStages], s_sfree[kTcStages], s_fullhl[2], s_mma[kTcDone], s_afull;
   __shared__ unsigned long long s_rbest[kTcM];                 // best exact (distance | target index) per row of the stripe
@@ -397,12 +397,10 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     uint4 pq0, pq1, pq2, pq3;
     auto fetch_tcm = [&]() {
       pq0 = pq1 = pq2 = pq3 = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu);
-      if (!no_prune) {
-        if (lane < n_tiles) pq0 = __ldcg(tcm4 + lane);
-        if (lane + 32 < n_tiles) pq1 = __ldcg(tcm4 + lane + 32);
-        if (lane + 64 < n_tiles) pq2 = __ldcg(tcm4 + lane + 64);
-        if (lane + 96 < n_tiles) pq3 = __ldcg(tcm4 + lane + 96);
-      }
+      if (lane < n_tiles) pq0 = __ldcg(tcm4 + lane);
+      if (lane + 32 < n_tiles) pq1 = __ldcg(tcm4 + lane + 32);
+      if (lane + 64 < n_tiles) pq2 = __ldcg(tcm4 + lane + 64);
+      if (lane + 96 < n_tiles) pq3 = __ldcg(tcm4 + lane + 96);
     };
     auto max4 = [](const uint4& q) -> unsigned { return max(max(q.x, q.y), max(q.z, q.w)); };
     fetch_tcm();
@@ -456,9 +454,9 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
           const unsigned a0 = __shfl_sync(0xffffffffu, tc0, src), a1 = __shfl_sync(0xffffffffu, tc1, src);
           const unsigned a2 = __shfl_sync(0xffffffffu, tc2, src), a3 = __shfl_sync(0xffffffffu, tc3, src);
           if (valid && t < 128) cm = sl == 0 ? a0 : sl == 1 ? a1 : sl == 2 ? a2 : a3;
-          else if (valid && !no_prune) cm = max4(__ldcg(tcm4 + t));
+          else if (valid) cm = max4(__ldcg(tcm4 + t));
         }
-        const bool visit = valid && (no_prune || lb <= 0.0f || !(lb > rmaxf) || !(lb > __uint_as_float(cm)));
+        const bool visit = valid && (lb <= 0.0f || !(lb > rmaxf) || !(lb > __uint_as_float(cm)));
         const unsigned vb = __ballot_sync(0xffffffffu, visit);
         const int fl = (vb & 0xFFFFu) ? __ffs(vb & 0xFFFFu) - 1 : 16;   // first tile to visit on either side (16 = none in this window)
         const int fr = (vb >> 16) ? __ffs(vb >> 16) - 1 : 16;
@@ -868,11 +866,7 @@ int launch_match_nn(qb200_handle* h, int n_pairs) {
   const int V = h->V;
   const size_t smem = tc_smem_bytes();
   if (int rc = ensure_dyn_smem(h, (const void*)tc_nn_kernel<false>, smem)) return rc;
-  // triage switches (results are identical either way): QB200_TC_NODEDUP=1 keeps duplicate descriptors, QB200_TC_NOPRUNE=1
-  // visits every column tile
-  static const int no_dedup = (getenv("QB200_TC_NODEDUP") && getenv("QB200_TC_NODEDUP")[0] == '1') ? 1 : 0;
-  static const int no_prune = (getenv("QB200_TC_NOPRUNE") && getenv("QB200_TC_NOPRUNE")[0] == '1') ? 1 : 0;
-  int rc = sort_and_dedup(h, 2 * n_pairs, no_dedup ? 0 : 1);
+  int rc = sort_and_dedup(h, 2 * n_pairs, 1);
   if (rc) return rc;
   const uint32_t* uperm = h->val_a;
   const uint32_t* class_of = reinterpret_cast<const uint32_t*>(h->key_a);
@@ -893,10 +887,10 @@ int launch_match_nn(qb200_handle* h, int n_pairs) {
   if (tc_prof) {
     if (int rc2 = ensure_dyn_smem(h, (const void*)tc_nn_kernel<false, true>, smem)) return rc2;
     tc_nn_kernel<false, true><<<g, kTcThreads, smem, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, V, uperm, rowbest_u, colbest_u,
-                                                                  tile_cmax, h->tc_fallback, h->tc_stats, nullptr, no_prune);
+                                                                  tile_cmax, h->tc_fallback, h->tc_stats, nullptr);
   } else {
     tc_nn_kernel<false><<<g, kTcThreads, smem, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, V, uperm, rowbest_u, colbest_u,
-                                                            tile_cmax, h->tc_fallback, h->tc_stats, nullptr, no_prune);
+                                                            tile_cmax, h->tc_fallback, h->tc_stats, nullptr);
   }
   cudaEventRecord(h->kev[1], h->stream);
   h->kev_armed[0] = 1;
@@ -921,7 +915,7 @@ int launch_tc_debug_tile(qb200_handle* h, float* d_out) {
   split_desc_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_t, n_unique, h->V, uperm, h->desc_tiles, h->desc_norm);
   const dim3 g(1, 1);
   tc_nn_kernel<true><<<g, kTcThreads, smem, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, h->V, uperm, h->colpart + (size_t)h->S * h->V,
-                                                         h->colpart, reinterpret_cast<unsigned*>(h->colpart + (size_t)2 * h->S * h->V), h->tc_fallback, h->tc_stats, d_out, 0);
+                                                         h->colpart, reinterpret_cast<unsigned*>(h->colpart + (size_t)2 * h->S * h->V), h->tc_fallback, h->tc_stats, d_out);
   h->launches += 2;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;

@@ -455,14 +455,26 @@ def test_graph_error_band_adversarial(handle, oracle):
 
 
 def test_small_capacity_handles(oracle, small_pair):
-    """Configurations the default tests never touch (ADVICE r1): one slot, V = 128 / 256, max_raw_points < max_voxel_points."""
+    """Configurations the default tests never touch (ADVICE r1): one slot, V = 128 / 256, max_raw_points < max_voxel_points,
+    max_raw_points = 200 (the voxel sort's 256 histogram words per tile exceed R)."""
     src, tgt, _ = small_pair
     p = default_params()
     sv, _ = oracle.voxelize(src, 0.3, 1); tv, _ = oracle.voxelize(tgt, 0.3, 1)
-    for kw in (dict(max_batch_slots=1, max_voxel_points=16384, max_raw_points=4096), dict(max_batch_slots=1, max_voxel_points=128),
+    for kw in (dict(max_batch_slots=1, max_voxel_points=16384, max_raw_points=4096),
+               dict(max_batch_slots=1, max_voxel_points=128, max_raw_points=200), dict(max_batch_slots=1, max_voxel_points=128),
                dict(max_batch_slots=1, max_voxel_points=256), dict(max_batch_slots=1)):
         with Handle(**kw) as h:
             V = h.cfg.max_voxel_points
+            raw = src[:min(len(src), h.cfg.max_raw_points)]
+            for skip in (0, 1):
+                ref, st_r = oracle.voxelize(raw, 0.3, skip)
+                got, st_g = h.voxelize(raw, 0.3, skip)
+                if len(ref) > V:   # QB200_CAPACITY_EXCEEDED, the first V voxels still computed
+                    assert st_g == 3 and len(got) == V, (kw, skip)
+                    ref = ref[:V]
+                else:
+                    assert st_g == st_r == 0, (kw, skip)
+                assert np.array_equal(got.view(np.uint32), ref.view(np.uint32)), (kw, skip)
             a, b = sv[:min(len(sv), V, h.cfg.max_raw_points)], tv[:min(len(tv), V, h.cfg.max_raw_points)]
             n_g, d_g = h.compute_fpfh(a, 0.5, 0.75, DEFAULT_CELL)
             n_r, d_r = oracle.compute_fpfh(a, 0.5, 0.75, DEFAULT_CELL)
