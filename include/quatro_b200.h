@@ -102,12 +102,17 @@ typedef struct qb200_params {
   double RyRx[9];                   /* row-major 3x3, setPreEstaimatedRyRx, quatro.hpp:276-279 */
 } qb200_params;
 
+/* Largest max_voxel_points qb200_create accepts (2^18): dense indoor scans at a 0.05 m voxel reach 100-150 k points per cloud.
+ * The handle's device memory grows linearly with it, about 1.2 KB per voxel point and cloud: a one-slot handle with 262144 voxel and
+ * 524288 raw points per cloud allocates 0.74 GB. */
+#define QB200_MAX_VOXEL_POINTS 262144
+
 /* Handle configuration: device and per-pair capacities (device workspaces are sized once). */
 typedef struct qb200_config {
   int32_t device;            /* CUDA ordinal */
   int32_t max_batch_slots;   /* pairs resident in one wave of the batch pipeline (default 64) */
   int32_t max_raw_points;    /* per cloud (default 131072) */
-  int32_t max_voxel_points;  /* per cloud (default 16384; multiple of 128) */
+  int32_t max_voxel_points;  /* per cloud (default 16384; multiple of 128, <= QB200_MAX_VOXEL_POINTS) */
   int32_t max_corr;          /* per pair  (default 4096; multiple of 32, <= 8192; the pose solver holds cliques of <= 4096) */
   int32_t reserved[3];
 } qb200_config;
@@ -303,7 +308,8 @@ int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pai
  * scan instead of once per pair.  Slots are indexed 0 .. n_slots-1; results never depend on whether a scan came from the cache
  * (tests/test_gpu_parity.py::test_scan_cache_*). */
 typedef struct qb200_slot_pair { int32_t src_slot, tgt_slot; } qb200_slot_pair;
-int qb200_cache_reserve(qb200_handle* h, int32_t n_slots);   /* (re)allocates; 0 frees.  ~3.1 MB per slot at max_voxel_points = 16384 */
+int qb200_cache_reserve(qb200_handle* h, int32_t n_slots);   /* (re)allocates; 0 frees.  192 B per voxel point and slot: ~3.1 MB at
+                                                                 max_voxel_points = 16384, ~50 MB at 262144 */
 /* voxelize + normals + FPFH of n_scans raw scans (scans4[i]: n_points[i] x {x,y,z,w}) into slots slot_ids[i] */
 int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
                       const qb200_params* p, qb200_mem_kind kind);

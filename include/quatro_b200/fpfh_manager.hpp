@@ -76,7 +76,8 @@ class FPFHManager {
     qb200_handle* h = qb200::shared_handle();
     int st = qb200_match_and_pack(h, qb200::as_float4(src_cloud_), ns, qb200::as_float4(tgt_cloud_), nt, &p, c.data(),
                                   reinterpret_cast<float*>(sm.data()), reinterpret_cast<float*>(tm.data()), cap, &n);
-    if (st == QB200_ERR_BAD_ARG && (ns > 16384 || nt > 16384)) {  // a cloud beyond the default voxel capacity: grow once, never truncate
+    // a cloud beyond the default voxel capacity, or more correspondences than the default max_corr: grow once, never truncate
+    if (!qb200::shared_handle_grown() && ((st == QB200_ERR_BAD_ARG && (ns > 16384 || nt > 16384)) || st == QB200_CAPACITY_EXCEEDED)) {
       h = qb200::grow_shared_handle();
       st = qb200_match_and_pack(h, qb200::as_float4(src_cloud_), ns, qb200::as_float4(tgt_cloud_), nt, &p, c.data(),
                                 reinterpret_cast<float*>(sm.data()), reinterpret_cast<float*>(tm.data()), cap, &n);

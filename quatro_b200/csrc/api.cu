@@ -125,10 +125,7 @@ int alloc_all(qb200_handle* h) {
   QB_ALLOC(h, h->tc_stats, 32);
   QB_CUDA_TRY(h, cudaMemset(h->tc_stats, 0, 32 * sizeof(unsigned long long)));
   QB_ALLOC(h, h->rowbest, S * V);
-  {  // two layouts share colpart: [S][NS][V] stripe partials (exact kernel) and [2][S][V] class results + tile cache (tc_match.cu)
-    const size_t a = S * h->NS * V, b = 2 * S * V + S * (V >> 7) * 2 + 2;
-    QB_ALLOC(h, h->colpart, a > b ? a : b);
-  }
+  QB_ALLOC(h, h->colpart, 2 * S * V + S * (V >> 7) * 2 + 2);  // tensor-core K6: [2][S][V] class results + tile cache (tc_match.cu)
   QB_ALLOC(h, h->colbest, S * V);
   QB_ALLOC(h, h->mut_i, S * V);
   QB_ALLOC(h, h->mut_j, S * V);
@@ -308,7 +305,7 @@ int qb200_create(const qb200_config* cfg_in, qb200_handle** out) {
   qb200_config cfg;
   if (cfg_in) cfg = *cfg_in; else qb200_default_config(&cfg);
   if (cfg.max_batch_slots < 1 || cfg.max_batch_slots > 2048 || cfg.max_raw_points < 1 || cfg.max_voxel_points < kMatchTile ||
-      cfg.max_voxel_points % kMatchTile != 0 || cfg.max_voxel_points > 65536 || cfg.max_corr < 32 || cfg.max_corr % 32 != 0 ||
+      cfg.max_voxel_points % kMatchTile != 0 || cfg.max_voxel_points > QB200_MAX_VOXEL_POINTS || cfg.max_corr < 32 || cfg.max_corr % 32 != 0 ||
       cfg.max_corr > 8192 || (long long)cfg.max_batch_slots * 2 * cfg.max_raw_points > 2000000000LL ||
       (long long)cfg.max_batch_slots * 2 * cfg.max_voxel_points > 2000000000LL)
     return QB200_ERR_BAD_ARG;

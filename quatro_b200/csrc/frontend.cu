@@ -381,18 +381,20 @@ __device__ __forceinline__ LatticeView make_view(int cloud, int V, const float4*
 // K4 / K5 walk the same neighbourhoods.  A thread first COLLECTS its neighbour indices (cheap distance tests, divergent)
 // into a shared-memory list and then processes the list in a dense loop, so the expensive per-neighbour work (pair
 // features, 33-bin gathers) runs with most lanes of the warp active instead of whenever any lane found a neighbour.
-// Neighbourhoods larger than the list are handled window by window (ordinals [base, base + cap)), order preserved.
+// Neighbourhoods larger than the list are handled window by window (ordinals [base, base + cap)), order preserved, so the
+// results do not depend on the window size.  64 32-bit indices per thread are 32 KB of static shared memory: spfh_kernel<true>
+// adds its 8.4 KB of bin counts and stays within the 48 KB static limit.
 constexpr int kNbrThreads = 128;
-constexpr int kNbrCap = 96;
+constexpr int kNbrCap = 64;
 
 template <class Process>
 __device__ __forceinline__ int for_each_neighbor_listed(const LatticeView& L, const float4 pq, int m, float r2,
-                                                        unsigned short (*nbr)[kNbrThreads], Process&& process) {
+                                                        uint32_t (*nbr)[kNbrThreads], Process&& process) {
   int k_total = 0;
   for (int base = 0;; base += kNbrCap) {
     int k = 0;
     for_each_neighbor(L, pq, m, r2, [&](int p, float, const float4) {
-      if (k >= base && k < base + kNbrCap) nbr[k - base][threadIdx.x] = (unsigned short)p;
+      if (k >= base && k < base + kNbrCap) nbr[k - base][threadIdx.x] = (uint32_t)p;
       ++k;
     });
     k_total = k;
@@ -409,16 +411,16 @@ __device__ __forceinline__ int for_each_neighbor_listed(const LatticeView& L, co
 __global__ void __launch_bounds__(kNbrThreads) nbr_list_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V,
                                                                const uint64_t* __restrict__ cell_key, const int* __restrict__ cell_start,
                                                                const uint32_t* __restrict__ order, const int* __restrict__ n_cells, float inv,
-                                                               int m, float r2, unsigned short* __restrict__ nbr_list,
+                                                               int m, float r2, uint32_t* __restrict__ nbr_list,
                                                                int* __restrict__ nbr_cnt) {
   const int cloud = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_pts[cloud]) return;
   const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, inv);
-  unsigned short* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
+  uint32_t* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
   int k = 0;
   for_each_neighbor(L, L.pts[q], m, r2, [&](int p, float, const float4) {
-    if (k < kNbrGlobalCap) gl[(size_t)k * V] = (unsigned short)p;
+    if (k < kNbrGlobalCap) gl[(size_t)k * V] = (uint32_t)p;
     ++k;
   });
   nbr_cnt[(size_t)cloud * V + q] = k;
@@ -429,7 +431,7 @@ __global__ void __launch_bounds__(kNbrThreads) nbr_list_kernel(const float4* __r
 __global__ void __launch_bounds__(128) normals_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V,
                                                       const uint64_t* __restrict__ cell_key, const int* __restrict__ cell_start,
                                                       const uint32_t* __restrict__ order, const int* __restrict__ n_cells, float inv, int m,
-                                                      float r2, const unsigned short* __restrict__ nbr_list, const int* __restrict__ nbr_cnt,
+                                                      float r2, const uint32_t* __restrict__ nbr_list, const int* __restrict__ nbr_cnt,
                                                       int list_usable, float4* __restrict__ normals) {
   const int cloud = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -446,7 +448,7 @@ __global__ void __launch_bounds__(128) normals_kernel(const float4* __restrict__
   };
   const int kq = nbr_cnt[(size_t)cloud * V + q];
   if (list_usable && kq <= kNbrGlobalCap) {
-    const unsigned short* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
+    const uint32_t* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
     for (int t = 0; t < kq; ++t) {
       const float4 pp = L.pts[gl[(size_t)t * V]];
       const float dx = pq.x - pp.x, dy = pq.y - pp.y, dz = pq.z - pp.z;
@@ -473,10 +475,10 @@ __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __rest
                                                             const int* __restrict__ n_pts, int V, const uint64_t* __restrict__ cell_key,
                                                             const int* __restrict__ cell_start, const uint32_t* __restrict__ order,
                                                             const int* __restrict__ n_cells, float inv, int m, float r2,
-                                                            float* __restrict__ spfh, const unsigned short* __restrict__ nbr_list,
+                                                            float* __restrict__ spfh, const uint32_t* __restrict__ nbr_list,
                                                             const int* __restrict__ nbr_cnt) {
   __shared__ unsigned short cnts[kDescDim][kSpfhThreads];
-  __shared__ unsigned short nbr[kRare ? kNbrCap : 1][kNbrThreads];
+  __shared__ uint32_t nbr[kRare ? kNbrCap : 1][kNbrThreads];
   const int cloud = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_pts[cloud]) return;
@@ -501,7 +503,7 @@ __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __rest
     cnts[22 + b3][threadIdx.x]++;
   };
   if (!kRare) {
-    const unsigned short* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
+    const uint32_t* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
     for (int t = 0; t < k; ++t) feature((int)gl[(size_t)t * V]);
   } else {
     k = for_each_neighbor_listed(L, pq, m, r2, nbr, feature);
@@ -525,7 +527,7 @@ __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __rest
 // and three 16-byte gathers per neighbour each instead of 33 and nine: 3x the warps at well under half the registers.
 // Per-bin accumulation order (lattice order of the neighbours) is unchanged.
 __global__ void __launch_bounds__(3 * kNbrThreads, 3) fpfh_list_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V,
-                                                                    const float* __restrict__ spfh, const unsigned short* __restrict__ nbr_list,
+                                                                    const float* __restrict__ spfh, const uint32_t* __restrict__ nbr_list,
                                                                     const int* __restrict__ nbr_cnt, float* __restrict__ desc_t) {
   const int cloud = blockIdx.y;
   const int third = threadIdx.x / kNbrThreads;  // warp-uniform
@@ -540,7 +542,7 @@ __global__ void __launch_bounds__(3 * kNbrThreads, 3) fpfh_list_kernel(const flo
 #pragma unroll
   for (int b = 0; b < 11; ++b) o[b] = 0.0f;
   double sum = 0.0;
-  const unsigned short* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
+  const uint32_t* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
   // Two-deep software pipeline: the index of neighbour t + 2 and the point / SPFH third of neighbour t + 1 are in flight while
   // neighbour t is accumulated (the chain index -> rows -> 11 dependent adds was one full L1/L2 latency per step: 66 % of the
   // scheduler cycles had no eligible warp).  The accumulation order is unchanged.
@@ -577,7 +579,7 @@ __global__ void __launch_bounds__(kNbrThreads) fpfh_rare_kernel(const float4* __
                                                                 const uint32_t* __restrict__ order, const int* __restrict__ n_cells, float inv,
                                                                 int m, float r2, const float* __restrict__ spfh,
                                                                 const int* __restrict__ nbr_cnt, float* __restrict__ desc_t) {
-  __shared__ unsigned short nbr[kNbrCap][kNbrThreads];
+  __shared__ uint32_t nbr[kNbrCap][kNbrThreads];
   const int cloud = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_pts[cloud]) return;

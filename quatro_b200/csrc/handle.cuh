@@ -47,7 +47,7 @@ struct qb200_handle {
   int* cell_start;            // [2S*(V+1)]
   float4* normals;            // [2S*V]
   float* spfh;                // [2S*V*36] rows padded to 36 floats
-  unsigned short* nbr_list;   // [2S][kNbrGlobalCap][V] neighbour indices found by K4 (lattice order), reused by K5
+  uint32_t* nbr_list;         // [2S][kNbrGlobalCap][V] fpfh_radius neighbour indices found by K2c (lattice order), read by K3..K5
   int* nbr_cnt;               // [2S*V] neighbour count (self included); > kNbrGlobalCap: K5 walks the lattice itself
   float* desc_t;              // [2S*40*V] FPFH, dimension-major per cloud (row d = bin d over all points; rows 33..39 zero)
   float* desc_tiles;          // [2S*(V/128)*3*5120] per 128-point block: centred TF32 hi | lo | exact fp32 images in the wgmma
@@ -58,8 +58,8 @@ struct qb200_handle {
   int force_exact_match;      // 0 (default): tensor-core filter + exact evaluation; 1 (QB200_MATCH_EXACT=1): exact CUDA-core K6 only
   // ---- matching ----
   unsigned long long* rowbest;// [S*V] packed (dist bits << 32 | tgt idx) per source point
-  unsigned long long* colpart;// [S*NS*V] per-stripe partial column minima
-  unsigned long long* colbest;// [S*V]
+  unsigned long long* colpart;// [2SV + S*(V/128)*2 + 2] tensor-core K6 scratch: class results [2][S][V] and the tile-max cache
+  unsigned long long* colbest;// [S*V] packed (dist bits << 32 | src idx) per target point (the exact K6 atomicMins into it)
   int *mut_i, *mut_j;         // [S*V] mutual NN list (larger-cloud idx, smaller-cloud idx)
   unsigned char* mark;        // [S*V] tuple-test survivors
   int* partner;               // [S*V] tgt partner per source index (-1)

@@ -9,10 +9,11 @@
 // The two exact 1-NN searches are the row- and column-argmin of one N_src x N_tgt distance matrix
 // that is never materialised: a CTA owns a 128-row stripe of source descriptors (staged once in
 // shared memory, dimension-major), streams 128-column target tiles through a cp.async double
-// buffer, keeps row minima in registers and emits per-stripe column minima that a second kernel
-// folds.  Distances are the fused-multiply-add chain over d = 0..32 of (a_d - b_d)^2 and minima
-// carry the candidate index in the low word, so ties resolve to the lowest index -- exactly the
-// CPU oracle's arithmetic, hence bit-identical argmins.
+// buffer, keeps row minima in registers and folds each tile's column minima into colbest with
+// one 64-bit atomicMin per column.  Distances are the fused-multiply-add chain over d = 0..32 of
+// (a_d - b_d)^2 and minima carry the candidate index in the low word, so ties resolve to the
+// lowest index whatever order the stripes arrive in -- exactly the CPU oracle's arithmetic, hence
+// bit-identical argmins.  The scratch is colbest itself: linear in max_voxel_points.
 #include <stdlib.h>
 
 #include "handle.cuh"
@@ -48,8 +49,8 @@ __device__ __forceinline__ void load_tile_async(float (*dst)[kMT], const float* 
 }
 
 __global__ void __launch_bounds__(kMatchThreads, 2)
-match_stripe_kernel(const float* __restrict__ desc_t, const int* __restrict__ n_vox, int V, int NS, const int* __restrict__ only,
-                    unsigned long long* __restrict__ rowbest, unsigned long long* __restrict__ colpart) {
+match_stripe_kernel(const float* __restrict__ desc_t, const int* __restrict__ n_vox, int V, const int* __restrict__ only,
+                    unsigned long long* __restrict__ rowbest, unsigned long long* __restrict__ colbest) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float(*As)[kMT] = reinterpret_cast<float(*)[kMT]>(smem_raw);                                    // [33][128]
   float(*Bs0)[kMT] = reinterpret_cast<float(*)[kMT]>(smem_raw + sizeof(float) * kDescDim * kMT);  // [33][128]
@@ -136,7 +137,7 @@ match_stripe_kernel(const float* __restrict__ desc_t, const int* __restrict__ n_
 #pragma unroll
       for (int w = 1; w < 8; ++w) m = umin64(m, colred[w][threadIdx.x]);
       const int col = jt * kMT + threadIdx.x;
-      if (col < nB) colpart[((size_t)pair * NS + stripe) * V + col] = m;
+      if (col < nB && m != ~0ull) atomicMin(colbest + (size_t)pair * V + col, m);  // the minimum does not depend on stripe order
     }
     // the next iteration's first __syncthreads orders the colred reads above before its writes,
     // and the B buffer being overwritten next was last read two barriers ago.
@@ -153,18 +154,14 @@ match_stripe_kernel(const float* __restrict__ desc_t, const int* __restrict__ n_
   }
 }
 
-// fold per-stripe column minima
-__global__ void __launch_bounds__(256) match_colfold_kernel(const unsigned long long* __restrict__ colpart, const int* __restrict__ n_vox, int V,
-                                                            int NS, const int* __restrict__ only, unsigned long long* __restrict__ colbest) {
+// column minima of the pairs being (re)done start at "none" (~0); match_stripe_kernel then atomicMins every stripe's minima into them
+__global__ void __launch_bounds__(256) match_colreset_kernel(const int* __restrict__ n_vox, int V, const int* __restrict__ only,
+                                                             unsigned long long* __restrict__ colbest) {
   const int pair = blockIdx.y;
   if (only != nullptr && only[pair] == 0) return;
   const int col = blockIdx.x * blockDim.x + threadIdx.x;
-  const int nA = n_vox[2 * pair], nB = n_vox[2 * pair + 1];
-  if (col >= nB) return;
-  const int ns = (nA + kMT - 1) / kMT;
-  unsigned long long m = ~0ull;
-  for (int s = 0; s < ns; ++s) m = umin64(m, colpart[((size_t)pair * NS + s) * V + col]);
-  colbest[(size_t)pair * V + col] = m;
+  if (col >= n_vox[2 * pair + 1]) return;
+  colbest[(size_t)pair * V + col] = ~0ull;
 }
 
 // mutual nearest neighbours, listed by ascending index in the LARGER cloud (feature_matcher.cc:84-89,146-177).
@@ -381,15 +378,15 @@ int launch_match_exact(qb200_handle* h, int n_pairs, const int* only) {
   const int V = h->V;
   const size_t smem = match_smem_bytes();
   if (int rc = ensure_dyn_smem(h, (const void*)match_stripe_kernel, smem)) return rc;
+  const dim3 gf((V + 255) / 256, n_pairs);
+  match_colreset_kernel<<<gf, 256, 0, h->stream>>>(h->ctr.n_vox, V, only, h->colbest);
   const dim3 gs(h->NS, n_pairs);
   if (only == nullptr) cudaEventRecord(h->kev[0], h->stream);
-  match_stripe_kernel<<<gs, kMatchThreads, smem, h->stream>>>(h->desc_t, h->ctr.n_vox, V, h->NS, only, h->rowbest, h->colpart);
+  match_stripe_kernel<<<gs, kMatchThreads, smem, h->stream>>>(h->desc_t, h->ctr.n_vox, V, only, h->rowbest, h->colbest);
   if (only == nullptr) {
     cudaEventRecord(h->kev[1], h->stream);
     h->kev_armed[0] = 1;
   }
-  const dim3 gf((V + 255) / 256, n_pairs);
-  match_colfold_kernel<<<gf, 256, 0, h->stream>>>(h->colpart, h->ctr.n_vox, V, h->NS, only, h->colbest);
   h->launches += 2;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;

@@ -404,8 +404,9 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     };
     auto max4 = [](const uint4& q) -> unsigned { return max(max(q.x, q.y), max(q.z, q.w)); };
     fetch_tcm();
-    // lower bounds of all column tiles (at most 128: V <= 16384 ... 65536 / 128 = 512 tiles are covered by the loop stride),
-    // kept in shared memory; start at the tile whose norm range is closest to the stripe's, then walk outwards on both sides
+    // lower bounds of all column tiles: tiles 0..127 (V <= 16384) are kept in shared memory, later ones (up to 2048 at
+    // max_voxel_points = 262144) are recomputed from the norms by tlb() and their column maxima read from tcm4 in global memory;
+    // the loop stride covers any count.  Start at the tile whose norm range is closest to the stripe's, then walk outwards.
     int t0 = 0;
     {
       float best = INFINITY;
@@ -871,7 +872,7 @@ int launch_match_nn(qb200_handle* h, int n_pairs) {
   const uint32_t* uperm = h->val_a;
   const uint32_t* class_of = reinterpret_cast<const uint32_t*>(h->key_a);
   const int* n_unique = reinterpret_cast<const int*>(class_of + (size_t)2 * h->S * V);
-  // class results, indexed by unique rank (colpart is scratch of the exact kernel, which runs later)
+  // class results, indexed by unique rank (colpart is this kernel's scratch; the exact fallback works in rowbest / colbest)
   unsigned long long* colbest_u = h->colpart;
   unsigned long long* rowbest_u = h->colpart + (size_t)h->S * V;
   unsigned* tile_cmax = reinterpret_cast<unsigned*>(h->colpart + (size_t)2 * h->S * V);  // [S][V/128][4] float bits, start above "+inf"

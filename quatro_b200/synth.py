@@ -58,7 +58,7 @@ def outdoor_pair(seed: int, rings: int = 64, azimuths: int = 1800, scene=STREET)
 def indoor_pair(seed: int, n_rays: int = 500000, extent: float = 3.0, n_furniture: int = 40):
     """Dense indoor pair (BASELINE configs[4]): a furnished room of 2*extent x 2*extent x 3 m scanned with n_rays uniformly distributed
     rays from two poses, 5 mm range noise, nothing flagged (the floor stays in).  The default 6 x 6 m room gives 34-53 k voxel points
-    per cloud at a 0.05 m voxel (within max_voxel_points <= 65536); a 18 x 18 m hall (extent 9) gives 43-152 k.  Returns (src (n,4), tgt (m,4), T_gt 4x4) with p_tgt = T_gt @ p_src."""
+    per cloud at a 0.05 m voxel; a 18 x 18 m hall (extent 9) gives 43-152 k (max_voxel_points up to 262144 holds either).  Returns (src (n,4), tgt (m,4), T_gt 4x4) with p_tgt = T_gt @ p_src."""
     src = np.zeros((n_rays, 4), np.float32)
     tgt = np.zeros((n_rays, 4), np.float32)
     ns, nt = C.c_int(0), C.c_int(0)
