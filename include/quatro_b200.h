@@ -378,11 +378,14 @@ int qb200_debug_tc_distances(qb200_handle* h, const float* a33, int32_t na, cons
 
 
 /* Diagnostics: cumulative counters of the tensor-core matcher since creation / the last reset:
- * out4[0] = descriptor pairs that went through the exact fp32 chain, [1] = 128 x 128 tiles drained,
+ * out4[0] = descriptor pairs that went through the exact fp32 chain, [1] = 128 x 64 tiles drained,
  * [2] = warm-up passes, [3] = stripes handed to the exact kernel.  Synchronises the handle's stream. */
 int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset);
 /* QB200_TC_PROF=1 only: per-role clock64 accounting of tc_nn_kernel (24 counters, see tools/tc_profile.py) */
 int qb200_debug_tc_profile(qb200_handle* h, uint64_t* out24, int32_t reset);
+/* Diagnostics: footprint of the tensor-core nearest-neighbour kernel as launched: out5[0] = threads per CTA,
+ * [1] = dynamic shared bytes, [2] = static shared bytes, [3] = registers per thread, [4] = resident CTAs per SM. */
+int qb200_debug_tc_footprint(qb200_handle* h, int32_t* out5);
 
 /* Diagnostics: with QB200_TC_VERIFY=1 in the environment every batch is matched by the tensor-core path AND by the exact CUDA-core
  * kernel; out2[0] = nearest-neighbour table entries compared so far, out2[1] = entries whose packed (distance, index) differ

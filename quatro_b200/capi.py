@@ -158,6 +158,7 @@ def load_library(build: bool = True) -> C.CDLL:
         "qb200_register_batch_enqueue": (i32, [vp, vp, i32, vp, i32, vp]),
         "qb200_register_batch_flush": (i32, [vp]),
         "qb200_debug_tc_profile": (i32, [vp, vp, i32]),
+        "qb200_debug_tc_footprint": (i32, [vp, vp]),
         "qb200_solve_batch": (i32, [vp, vp, i32, vp, i32, vp]),
         "qb200_comm_init_all": (i32, [P(vp), i32]),
         "qb200_register_batch_sharded": (i32, [P(vp), i32, P(Pair), i32, P(Params), i32, vp]),
@@ -193,6 +194,7 @@ EXPORTED_SYMBOLS = [
     "qb200_register_batch_enqueue",
     "qb200_register_batch_flush",
     "qb200_debug_tc_profile",
+    "qb200_debug_tc_footprint",
     "qb200_solve_batch",
     "qb200_comm_init_all", "qb200_register_batch_sharded", "qb200_comm_unique_id", "qb200_comm_init_rank",
     "qb200_register_batch_rank", "qb200_comm_wait", "qb200_bind_numa",
@@ -564,6 +566,13 @@ class Handle:
         out = np.zeros(24, np.uint64)
         self._check(self.lib.qb200_debug_tc_profile(self.h, _ptr(out), int(reset)), "qb200_debug_tc_profile")
         return out
+
+    def debug_tc_footprint(self) -> dict:
+        """Threads, shared memory, registers and resident CTAs per SM of the tensor-core nearest-neighbour kernel."""
+        out = np.zeros(5, np.int32)
+        self._check(self.lib.qb200_debug_tc_footprint(self.h, _ptr(out)), "qb200_debug_tc_footprint")
+        return {"threads": int(out[0]), "dyn_smem": int(out[1]), "static_smem": int(out[2]), "regs": int(out[3]),
+                "ctas_per_sm": int(out[4])}
 
     def debug_match_verify(self, reset: bool = True) -> dict:
         out = np.zeros(2, np.uint64)

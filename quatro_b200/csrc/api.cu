@@ -1085,6 +1085,14 @@ int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset) {
   return QB200_OK;
 }
 
+// Footprint of the tensor-core nearest-neighbour kernel as it is launched: out5 = threads per CTA, dynamic and static shared
+// bytes, registers per thread, resident CTAs per SM (occupancy calculator at that shared-memory size)
+int qb200_debug_tc_footprint(qb200_handle* h, int32_t* out5) {
+  if (!h || !out5) return QB200_ERR_BAD_ARG;
+  cudaSetDevice(h->device);
+  return tc_footprint(h, out5);
+}
+
 // Validation hook: tensor-core (3xTF32) approximate squared distances between up to 128 source and 128 target
 // descriptors -> out[128*128] (row = source).  Lets tests measure the filter's error against the exact chain.
 int qb200_debug_tc_distances(qb200_handle* h, const float* a33, int32_t na, const float* b33, int32_t nb, float* out) {

@@ -50,8 +50,8 @@ struct qb200_handle {
   uint32_t* nbr_list;         // [2S][kNbrGlobalCap][V] fpfh_radius neighbour indices found by K2c (lattice order), read by K3..K5
   int* nbr_cnt;               // [2S*V] neighbour count (self included); > kNbrGlobalCap: K5 walks the lattice itself
   float* desc_t;              // [2S*40*V] FPFH, dimension-major per cloud (row d = bin d over all points; rows 33..39 zero)
-  float* desc_tiles;          // [2S*(V/128)*3*5120] per 128-point block: centred TF32 hi | lo | exact fp32 images in the wgmma
-                              // shared-memory operand layout (one bulk copy per tile)
+  float* desc_tiles;          // [2S*(V/64)*3*2560] per 64-point block: centred TF32 hi | lo | exact fp32 images in the wgmma
+                              // shared-memory operand layout (one bulk copy per column tile, one per 128-row stripe)
   float* desc_norm;           // [2S*V] squared norms (fp32 fma chain)
   int* tc_fallback;           // [S] 1 = too many exact ties for the filter to pay off: pair re-done by the exact fp32 kernel
   unsigned long long* tc_stats; // [32] diagnostics, cumulative: [0..3] exact evaluations, tiles drained, warm-up passes, aborted stripes; [4..5] QB200_TC_VERIFY; [8..31] QB200_TC_PROF
@@ -59,6 +59,7 @@ struct qb200_handle {
   // ---- matching ----
   unsigned long long* rowbest;// [S*V] packed (dist bits << 32 | tgt idx) per source point
   unsigned long long* colpart;// [2SV + S*(V/128)*2 + 2] tensor-core K6 scratch: class results [2][S][V] and the tile-max cache
+                              // ([S][V/64][2] 32-bit maxima of 32-column groups)
   unsigned long long* colbest;// [S*V] packed (dist bits << 32 | src idx) per target point (the exact K6 atomicMins into it)
   int *mut_i, *mut_j;         // [S*V] mutual NN list (larger-cloud idx, smaller-cloud idx)
   unsigned char* mark;        // [S*V] tuple-test survivors
@@ -139,6 +140,7 @@ int launch_patchwork(qb200_handle* h, const float4* pts, int n, const qb200_patc
 int launch_match_nn(qb200_handle* h, int n_pairs);
 int launch_match_exact(qb200_handle* h, int n_pairs, const int* only);
 int launch_tc_debug_tile(qb200_handle* h, float* d_out);
+int tc_footprint(qb200_handle* h, int* out5);
 int launch_desc_to_aos(qb200_handle* h, int cloud, int n, float* d_out33);
 int launch_desc_from_aos(qb200_handle* h, int cloud, int n, const float* d_in33);
 int desc_to_aos_rows(qb200_handle* h, const float* desc_rows, int n, float* d_out33);

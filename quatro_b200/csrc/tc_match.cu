@@ -10,9 +10,9 @@
 //                       are dominated by planar points, centring makes THEIR dot products tiny and therefore the filter's
 //                       absolute error tiny exactly where near-ties are dense) -> one radix sort orders every cloud by norm
 //   dedup_kernel      : runs of bit-identical descriptors (adjacent after the sort) collapse to their first rank = lowest index
-//   split_desc_kernel : hi = TF32(x'), lo = TF32(x' - hi), exact x, per block of 128 unique descriptors as ready-made
+//   split_desc_kernel : hi = TF32(x'), lo = TF32(x' - hi), exact x, per block of 64 unique descriptors as ready-made
 //                       shared-memory operand images (hi | lo | exact), so an image is ONE cp.async.bulk
-//   tc_nn_kernel      : per 128-row stripe, column tiles in nearest-norm-first order; a tile whose lower bound
+//   tc_nn_kernel      : per 128-row stripe, 64-column tiles in nearest-norm-first order; a tile whose lower bound
 //                       (gap of the norm ranges)^2 exceeds every current best of the stripe's rows and of its columns is
 //                       skipped unloaded; otherwise
 //                         d~ = |a'|^2 + |b'|^2 - 2 (hi.hi + hi.lo + lo.hi)      3 x 5 wgmma m64n64k8 TF32 per warpgroup, fp32 in registers
@@ -25,33 +25,36 @@
 //                       exact CUDA-core kernel, so results never depend on the filter.
 //   broadcast_best_kernel : class results -> every member, in point order for the mutual-NN stage
 //
-// tc_nn_kernel, one CTA per SM, 18 warps, mbarrier hand-offs only: warp 17 chooses tiles and issues the exact-image copies
-// (4 stages), warp 16 the operand copies (2 stages); warps 0..15 are 4 warpgroups, each issues the 15 wgmma of its 64 x 64
-// quadrant of the tile and runs the filter / exact evaluation on the accumulator fragment it holds (DESIGN.md 5.1).
+// tc_nn_kernel, two CTAs per SM (320 threads, <= 96 registers, 100 KB dynamic shared memory each), mbarrier hand-offs only:
+// warp 9 chooses tiles and issues the exact-image copies (2 stages), warp 8 the operand copies (1 stage); warps 0..7 are
+// 2 warpgroups, each issues the 15 wgmma of its 64 rows x the tile's 64 columns and runs the filter / exact evaluation on the
+// accumulator fragment it holds.  One CTA's wgmma runs while the other CTA of the SM filters and evaluates (DESIGN.md 5.1).
 #include "handle.cuh"
 #include <cstdlib>
 
 namespace qb {
 
-constexpr int kTcM = 128, kTcN = 128;
+constexpr int kTcM = 128, kTcN = 64;              // stripe rows x column-tile width
+constexpr int kTcBlk = 64;                        // points per operand-image block: a stripe is 2 blocks, a column tile 1
 constexpr int kTcKB = kDescK / 8;                 // K blocks of 8 (TF32 MMA K)
-constexpr int kTcTileBytes = kDescK * 128 * 4;    // one operand image (128 points x 40 dims) = 20480 B
-constexpr int kTileFloats = kDescK * 128;         // 5120
+constexpr int kTcTileBytes = kDescK * kTcBlk * 4; // one operand image (64 points x 40 dims) = 10240 B
+constexpr int kTileFloats = kDescK * kTcBlk;      // 2560
 constexpr int kTcImages = 3;                      // hi | lo | exact
-constexpr int kTcEpiWarps = 16;                   // MMA + filter / evaluation warps: warpgroup g = rows 64 (g & 1), columns 64 (g >> 1)
+constexpr int kTcEpiWarps = 8;                    // MMA + filter / evaluation warps: warpgroup g = rows 64 g .. 64 g + 63
 constexpr int kTcThreads = (kTcEpiWarps + 2) * 32;  // + operand-copy warp + scheduler warp
 constexpr int kTcDone = 4;                         // ring of "MMAs of position k done by every warp" barriers
-constexpr int kTcStages = 4;                      // ring of exact B images (prefetch distance 3); operand images: 2 stages
+constexpr int kTcStages = 2;                      // ring of exact B images (prefetch distance 1); operand images: 1 stage
+constexpr int kTcSmemTiles = 256;                 // column tiles whose lower bounds live in shared memory (V <= 16384)
 constexpr float kTcC = 1.2e-4f;                   // |d~ - d| <= kTcC/2 * (|a'|^2 + |b'|^2): 3x the worst error measured (test_tc_filter_error_bound)
 constexpr int kSpinLimit = 400000;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // Operand images use the canonical K-major / no-swizzle (interleave) wgmma layout: core matrix = 8 points x 16 B
-// (4 consecutive K values), byte offset kc*2048 + p*16 for K chunk kc (4 dims) and point p of the 128-point block.
+// (4 consecutive K values), byte offset kc*1024 + p*16 for K chunk kc (4 dims) and point p of the 64-point block.
 __device__ __forceinline__ uint64_t tc_smem_desc(uint32_t addr) {
-  // start address >> 4 | LBO = 2048 B (next 4-wide K chunk) | SBO = 128 B (next 8-point group) | no swizzle (bits 62-63 = 0)
-  return (uint64_t)((addr & 0x3FFFF) >> 4) | ((uint64_t)(2048 >> 4) << 16) | ((uint64_t)(128 >> 4) << 32);
+  // start address >> 4 | LBO = 1024 B (next 4-wide K chunk) | SBO = 128 B (next 8-point group) | no swizzle (bits 62-63 = 0)
+  return (uint64_t)((addr & 0x3FFFF) >> 4) | ((uint64_t)((kTcBlk * 16) >> 4) << 16) | ((uint64_t)(128 >> 4) << 32);
 }
 
 // D (64 x 64, fp32, registers of the warpgroup) (+)= A (64 x 8) * B (64 x 8)^T, both TF32 and K-major in shared memory.
@@ -92,7 +95,7 @@ __device__ __forceinline__ float tc_mu(int d) { return (d == 5 || d == 16 || d =
 
 // centred squared norm of every descriptor (the fp32 chain split_desc_kernel repeats) as the sort key cloud | norm bits:
 // K6 processes the points of a cloud in ascending-norm order, which turns the reverse triangle inequality
-// d(a,b) >= (|a'| - |b'|)^2 into a tile-level lower bound (whole 128 x 128 blocks are skipped without being loaded).
+// d(a,b) >= (|a'| - |b'|)^2 into a tile-level lower bound (whole 128 x 64 blocks are skipped without being loaded).
 __global__ void __launch_bounds__(256) norm_key_kernel(const float* __restrict__ desc_t, const int* __restrict__ n_vox, int V,
                                                        uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
   const int cloud = blockIdx.y;
@@ -121,10 +124,11 @@ __global__ void __launch_bounds__(256) split_desc_kernel(const float* __restrict
   const int cloud = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   const int n = n_vox[cloud];
-  const int NB = V >> 7;
-  if (q >= ((n + 127) & ~127)) return;  // the last block is padded with zeros so stale data never reaches the tensor core
+  const int NB = V / kTcBlk;
+  // the last stripe (both of its blocks) is padded with zeros so stale data never reaches the tensor core
+  if (q >= ((n + kTcM - 1) & ~(kTcM - 1))) return;
   const size_t base = (size_t)cloud * kDescK * V + (q < n ? perm[(size_t)cloud * V + q] : 0u);
-  const int blk = q >> 7, p = q & 127;
+  const int blk = q / kTcBlk, p = q % kTcBlk;
   float4* __restrict__ img = reinterpret_cast<float4*>(tiles + (size_t)(cloud * NB + blk) * kTcImages * kTileFloats) + p;
   // The tensor core delivers the filter's LOWER BOUND itself: rows (source clouds, even) carry x' in dims 0..32, kLow |x'|^2 in
   // dim 33 and 1 in dim 34; columns (target clouds, odd) carry -2 x', 1 and kLow |x'|^2 -- the contraction over the 35 dims is
@@ -149,12 +153,12 @@ __global__ void __launch_bounds__(256) split_desc_kernel(const float* __restrict
       hv[e] = __uint_as_float(__float_as_uint(xs) & 0xFFFFE000u);
       lv[e] = __uint_as_float(__float_as_uint(xs - hv[e]) & 0xFFFFE000u);
     }
-    img[0 * (kTileFloats / 4) + kc * 128] = make_float4(hv[0], hv[1], hv[2], hv[3]);
-    img[1 * (kTileFloats / 4) + kc * 128] = make_float4(lv[0], lv[1], lv[2], lv[3]);
-    if (kc < kDescK / 4 - 1) img[2 * (kTileFloats / 4) + kc * 128] = make_float4(xv[0], xv[1], xv[2], xv[3]);
+    img[0 * (kTileFloats / 4) + kc * kTcBlk] = make_float4(hv[0], hv[1], hv[2], hv[3]);
+    img[1 * (kTileFloats / 4) + kc * kTcBlk] = make_float4(lv[0], lv[1], lv[2], lv[3]);
+    if (kc < kDescK / 4 - 1) img[2 * (kTileFloats / 4) + kc * kTcBlk] = make_float4(xv[0], xv[1], xv[2], xv[3]);
   }
   // the exact image has no data in dims 36..39: slot 36 carries the column's filter term kLow |x'|^2 (+inf = padding)
-  img[2 * (kTileFloats / 4) + (kDescK / 4 - 1) * 128] = make_float4(q < n ? kLow * acc : INFINITY, 0.0f, 0.0f, 0.0f);
+  img[2 * (kTileFloats / 4) + (kDescK / 4 - 1) * kTcBlk] = make_float4(q < n ? kLow * acc : INFINITY, 0.0f, 0.0f, 0.0f);
   if (q < n) norm[(size_t)cloud * V + q] = acc;  // rank order
 }
 
@@ -265,31 +269,33 @@ __device__ __forceinline__ float tc_fkey_inv(unsigned key) { return __uint_as_fl
 // rows = source cloud (2*pair), columns = target cloud (2*pair+1): their UNIQUE descriptors in ascending-norm (rank) order;
 // n_vox / perm are the per-cloud unique counts and the point index of every unique rank.  rowbest / colbest_r are indexed by
 // unique rank (broadcast_best_kernel maps them back).  kDbg: additionally
-// dump d~ of the first tile of stripe 0 (validation hook).
+// dump d~ of every tile of stripe 0 (validation hook, at most 128 x 128 descriptors).
 //
 // Warp roles (no CTA-wide barrier inside the tile loop, everything is handed over through mbarriers):
-//   warp 17      : schedule warp.  Picks the stripe's next column tile, nearest norm range first, and SKIPS a tile when
+//   warp 9       : schedule warp.  Picks the stripe's next column tile, nearest norm range first, and SKIPS a tile when
 //                  its lower bound (gap between the norm ranges)^2 exceeds every current best of the stripe's rows and of
-//                  the tile's columns; issues the exact-image copies (4 stages)
-//   warp 16      : operand-copy warp (A images once, hi | lo images of every decided tile, 2 stages)
-//   warps 0..15  : warpgroup g = warps 4g .. 4g+3 owns rows 64 (g & 1) .. +63 and columns 64 (g >> 1) .. +63 of every tile;
-//                  warp w of it holds the accumulators of 16 of those rows (wgmma fragment).  15 wgmma -> release the operand
-//                  stage -> branch-free filter -> the warp's survivors are compacted into batches of 32 and evaluated exactly,
+//                  the tile's columns; issues the exact-image copies (2 stages)
+//   warp 8       : operand-copy warp (A images once, hi | lo images of every decided tile, 1 stage)
+//   warps 0..7   : warpgroup g = warps 4g .. 4g+3 owns rows 64 g .. +63 and the 64 columns of every tile; warp w of it
+//                  holds the accumulators of 16 of those rows (wgmma fragment).  15 wgmma -> release the operand stage ->
+//                  branch-free filter -> the warp's survivors are compacted into batches of 32 and evaluated exactly,
 //                  ONE CANDIDATE PER LANE -> release the exact-image stage.
+// Two CTAs share an SM: the tensor core works for one while the other filters and evaluates, so one operand stage is enough
+// (the next tile's operands load during this tile's filter and evaluation).
 // kProf: clock64 accounting of every role's waits into stats[8..31] (tools/tc_profile.py; QB200_TC_PROF=1)
 template <bool kDbg, bool kProf = false>
-__global__ void __launch_bounds__(kTcThreads, 1)
+__global__ void __launch_bounds__(kTcThreads, 2)
 tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, const int* __restrict__ n_vox, int V,
              const uint32_t* __restrict__ perm, unsigned long long* __restrict__ rowbest, unsigned long long* __restrict__ colbest_r,
              unsigned* __restrict__ tile_cmax, int* __restrict__ fallback, unsigned long long* __restrict__ stats,
              float* __restrict__ dbg_tile) {
-  extern __shared__ __align__(128) unsigned char smem[];  // 220 KB of operand images; static + dynamic must stay <= 227 KB
-  __shared__ uint64_t s_fullx[kTcStages], s_sfree[kTcStages], s_fullhl[2], s_mma[kTcDone], s_afull;
+  extern __shared__ __align__(128) unsigned char smem[];  // 100 KB of operand images; two CTAs (static + dynamic + 1 KB each) fit in 228 KB
+  __shared__ uint64_t s_fullx[kTcStages], s_sfree[kTcStages], s_fullhl, s_mma[kTcDone], s_afull;
   __shared__ unsigned long long s_rbest[kTcM];                 // best exact (distance | target index) per row of the stripe
-  __shared__ __align__(16) float s_wcj[kTcEpiWarps][64];       // per warp: threshold of each of its 64 columns (best exact distance)
+  __shared__ __align__(16) float s_wcj[kTcEpiWarps][kTcN];     // per warp: threshold of each of the tile's 64 columns (best exact distance)
   __shared__ unsigned short s_queue[kTcEpiWarps][32];          //           one batch of candidates (lane << 5 | fragment index)
   __shared__ int s_seq[8];                                     // column tile of sequence position n (ring), -1 = end of the stripe
-  __shared__ float s_tlb[128];                                 // lower bound of every distance between the stripe and column tile t
+  __shared__ float s_tlb[kTcSmemTiles];                        // lower bound of every distance between the stripe and column tile t
   __shared__ int s_dead, s_abort, s_evals, s_warm, s_npos;
   __shared__ int s_ndec;                                       // sequence positions 0 .. s_ndec-1 have been decided (s_seq ring)
 
@@ -300,16 +306,17 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
   if (r0 >= nA || nB <= 0) return;  // uniform for the CTA, before any barrier / allocation
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int NB = V >> 7;
+  const int NB = V / kTcBlk;
   auto tick = [&]() -> long long { return kProf ? clock64() : 0ll; };
   auto prof = [&](int slot, long long cyc) { if (kProf && lane == 0) atomicAdd(stats + slot, (unsigned long long)cyc); };
   const long long t_begin = tick();
-  // shared-memory map: A block (hi | lo | exact) | 2 stages of B (hi | lo) | 4 stages of B exact images.  The operand images
-  // are dead as soon as the MMAs of their tile completed, the exact image only when every warp evaluated the tile.
-  constexpr uint32_t kABytes = kTcImages * kTcTileBytes;
+  // shared-memory map: A (2 blocks of hi | lo | exact, 60 KB) | 1 stage of B (hi | lo, 20 KB) | 2 stages of B exact images
+  // (10 KB each).  The operand images are dead as soon as the MMAs of their tile completed, the exact image only when every
+  // warp evaluated the tile.
+  constexpr uint32_t kABytes = (kTcM / kTcBlk) * kTcImages * kTcTileBytes;
   constexpr uint32_t kHLBytes = 2 * kTcTileBytes;
   constexpr uint32_t kXBytes = kTcTileBytes;
-  const uint32_t sA = smem_u32(smem), sHL0 = sA + kABytes, sX0 = sHL0 + 2 * kHLBytes;
+  const uint32_t sA = smem_u32(smem), sHL = sA + kABytes, sX0 = sHL + kHLBytes;
   const float* __restrict__ tA = tiles + (size_t)cloudA * NB * kTcImages * kTileFloats;
   const float* __restrict__ tB = tiles + (size_t)cloudB * NB * kTcImages * kTileFloats;
   const float* __restrict__ nrmA = norm + (size_t)cloudA * V;   // rank order, ascending
@@ -317,13 +324,13 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
   const uint32_t* __restrict__ permA = perm + (size_t)cloudA * V;
   const uint32_t* __restrict__ permB = perm + (size_t)cloudB * V;
   unsigned long long* __restrict__ cbg = colbest_r + (size_t)pair * V;
-  const uint32_t bar_fullx0 = smem_u32(&s_fullx[0]), bar_sfree0 = smem_u32(&s_sfree[0]), bar_fullhl0 = smem_u32(&s_fullhl[0]),
+  const uint32_t bar_fullx0 = smem_u32(&s_fullx[0]), bar_sfree0 = smem_u32(&s_sfree[0]), bar_fullhl = smem_u32(&s_fullhl),
                  bar_mma0 = smem_u32(&s_mma[0]), bar_a = smem_u32(&s_afull);
   const int n_tiles = (nB + kTcN - 1) / kTcN;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kTcStages; ++i) { mbar_init(bar_fullx0 + 8 * i, 1); mbar_init(bar_sfree0 + 8 * i, kTcEpiWarps); }
-    for (int i = 0; i < 2; ++i) mbar_init(bar_fullhl0 + 8 * i, 1);
+    mbar_init(bar_fullhl, 1);
     for (int i = 0; i < kTcDone; ++i) mbar_init(bar_mma0 + 8 * i, kTcEpiWarps);
     mbar_init(bar_a, 1);
     s_dead = 0; s_abort = 0; s_evals = 0; s_warm = 0; s_npos = 0; s_ndec = 0;
@@ -349,34 +356,32 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
 
   if (warp == kTcEpiWarps) {
     // ================= operand-copy warp: A images once, then the hi | lo images of every decided position =================
-    auto issue_hl = [&](int n) {  // operand images (hi | lo, 40 KB) of position n -> stage n & 1; end marker: plain arrive
+    auto issue_hl = [&](int n) {  // operand images (hi | lo, 20 KB) of position n -> the operand stage; end marker: plain arrive
       const int t = v_seq[n & 7];
       if (lane != 0) return;
-      const uint32_t bar = bar_fullhl0 + 8 * (n & 1);
-      if (t < 0) { mbar_arrive(bar); return; }
-      mbar_expect_tx(bar, kHLBytes);
-      bulk_g2s(sHL0 + (n & 1) * kHLBytes, tB + (size_t)t * kTcImages * kTileFloats, kHLBytes, bar);
+      if (t < 0) { mbar_arrive(bar_fullhl); return; }
+      mbar_expect_tx(bar_fullhl, kHLBytes);
+      bulk_g2s(sHL, tB + (size_t)t * kTcImages * kTileFloats, kHLBytes, bar_fullhl);
     };
     if (lane == 0) {
       mbar_expect_tx(bar_a, kABytes);
-      bulk_g2s(sA, tA + (size_t)stripe * kTcImages * kTileFloats, kABytes, bar_a);
+      bulk_g2s(sA, tA + (size_t)stripe * (kTcM / kTcBlk) * kTcImages * kTileFloats, kABytes, bar_a);
     }
     bool ok = wait_decided(0);
-    if (ok) { issue_hl(0); ok = wait_decided(1); }
-    if (ok) issue_hl(1);
+    if (ok) issue_hl(0);
     long long p_wm = 0, p_wd = 0;
-    bool ended = !ok || v_seq[0] < 0 || v_seq[1] < 0;  // (an end marker has gone out already)
+    bool ended = !ok || v_seq[0] < 0;  // (an end marker has gone out already)
     for (int k = 0; ok && !ended; ++k) {
-      // operand stage k & 1 is free once every warp completed its MMAs of position k
+      // the operand stage is free once every warp completed its MMAs of position k
       const long long t0 = tick();
       ok = mbar_wait(bar_mma0 + 8 * (k & (kTcDone - 1)), (uint32_t)((k >> 2) & 1));
       const long long t1 = tick();
       p_wm += t1 - t0;
-      if (ok) ok = wait_decided(k + 2);
+      if (ok) ok = wait_decided(k + 1);
       p_wd += tick() - t1;
       if (!ok) break;
-      issue_hl(k + 2);
-      ended = v_seq[(k + 2) & 7] < 0;  // that was the end marker
+      issue_hl(k + 1);
+      ended = v_seq[(k + 1) & 7] < 0;  // that was the end marker
     }
     prof(12, p_wm); prof(28, p_wd);
     if (!ok) *v_dead = 1;
@@ -390,29 +395,27 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
       if (!(amin <= amax && bmin <= bmax)) return 0.0f;               // NaN norms: never skip
       return gap > 0.0f ? gap * gap * 0.9999f : 0.0f;
     };
-    // Shared per-tile column maxima: tcm4[t][g] = an upper bound of the best exact distances of columns 32 g .. 32 g + 31 of tile t
-    // (float bits; every filter warp refreshes its group after evaluating the tile, bests only shrink).  The values of the first
-    // 128 tiles (4 tiles per lane) are fetched at the END of a choice for the NEXT one, so no choice waits for L2.
-    const uint4* __restrict__ tcm4 = reinterpret_cast<const uint4*>(tile_cmax) + (size_t)pair * (V >> 7);
-    uint4 pq0, pq1, pq2, pq3;
+    // Shared per-tile column maxima: tcm2[t][g] = an upper bound of the best exact distances of columns 32 g .. 32 g + 31 of tile t
+    // (float bits; every filter warp refreshes both groups after evaluating the tile, bests only shrink).  The values of the first
+    // 256 tiles (8 tiles per lane: tile 32 i + lane in pq[i]) are fetched at the END of a choice for the NEXT one, so no choice
+    // waits for L2.
+    constexpr int kPq = kTcSmemTiles / 32;
+    const uint2* __restrict__ tcm2 = reinterpret_cast<const uint2*>(tile_cmax) + (size_t)pair * (V / kTcN);
+    uint2 pq[kPq];
     auto fetch_tcm = [&]() {
-      pq0 = pq1 = pq2 = pq3 = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu);
-      if (lane < n_tiles) pq0 = __ldcg(tcm4 + lane);
-      if (lane + 32 < n_tiles) pq1 = __ldcg(tcm4 + lane + 32);
-      if (lane + 64 < n_tiles) pq2 = __ldcg(tcm4 + lane + 64);
-      if (lane + 96 < n_tiles) pq3 = __ldcg(tcm4 + lane + 96);
+#pragma unroll
+      for (int i = 0; i < kPq; ++i) pq[i] = lane + 32 * i < n_tiles ? __ldcg(tcm2 + lane + 32 * i) : make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu);
     };
-    auto max4 = [](const uint4& q) -> unsigned { return max(max(q.x, q.y), max(q.z, q.w)); };
     fetch_tcm();
-    // lower bounds of all column tiles: tiles 0..127 (V <= 16384) are kept in shared memory, later ones (up to 2048 at
-    // max_voxel_points = 262144) are recomputed from the norms by tlb() and their column maxima read from tcm4 in global memory;
+    // lower bounds of all column tiles: tiles 0..255 (V <= 16384) are kept in shared memory, later ones (up to 4096 at
+    // max_voxel_points = 262144) are recomputed from the norms by tlb() and their column maxima read from tcm2 in global memory;
     // the loop stride covers any count.  Start at the tile whose norm range is closest to the stripe's, then walk outwards.
     int t0 = 0;
     {
       float best = INFINITY;
       for (int t = lane; t < n_tiles; t += 32) {
         const float g = tile_lb(t);
-        if (t < 128) s_tlb[t] = g;
+        if (t < kTcSmemTiles) s_tlb[t] = g;
         if (g < best) { best = g; t0 = t; }
       }
       const unsigned key = __reduce_min_sync(0xffffffffu, tc_fkey(best));
@@ -420,7 +423,7 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
       t0 = __shfl_sync(0xffffffffu, t0, __ffs(who) - 1);
       __syncwarp();
     }
-    auto tlb = [&](int t) -> float { return t < 128 ? s_tlb[t] : tile_lb(t); };
+    auto tlb = [&](int t) -> float { return t < kTcSmemTiles ? s_tlb[t] : tile_lb(t); };
     int lo = t0 - 1, hi = t0 + 1;
     bool first = true, done = false;
     auto next_tile = [&]() -> int {  // warp-uniform
@@ -437,7 +440,9 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
         }
       }
       const float rmaxf = __uint_as_float(__reduce_max_sync(0xffffffffu, rmax));  // distances are >= 0: the bit patterns order them
-      const unsigned tc0 = max4(pq0), tc1 = max4(pq1), tc2 = max4(pq2), tc3 = max4(pq3);
+      unsigned tcm[kPq];
+#pragma unroll
+      for (int i = 0; i < kPq; ++i) tcm[i] = max(pq[i].x, pq[i].y);
       if (*v_abort || *v_dead) return -1;
       // The walk, 32 candidates per round: lanes 0..15 look at the next 16 tiles on the left (lo, lo-1, ...), lanes 16..31 at the
       // next 16 on the right.  Lower bounds grow outwards on either side, so the next tile in nearest-first order is the first
@@ -451,11 +456,14 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
         const float lb = valid ? tlb(t) : INFINITY;
         unsigned cm = 0xFFFFFFFFu;
         {
-          const int src = t & 31, sl = (t >> 5) & 3;
-          const unsigned a0 = __shfl_sync(0xffffffffu, tc0, src), a1 = __shfl_sync(0xffffffffu, tc1, src);
-          const unsigned a2 = __shfl_sync(0xffffffffu, tc2, src), a3 = __shfl_sync(0xffffffffu, tc3, src);
-          if (valid && t < 128) cm = sl == 0 ? a0 : sl == 1 ? a1 : sl == 2 ? a2 : a3;
-          else if (valid) cm = max4(__ldcg(tcm4 + t));
+          const int src = t & 31, sl = (t >> 5) & (kPq - 1);
+#pragma unroll
+          for (int i = 0; i < kPq; ++i) {
+            const unsigned a = __shfl_sync(0xffffffffu, tcm[i], src);
+            if (sl == i) cm = a;
+          }
+          if (!valid) cm = 0xFFFFFFFFu;
+          else if (t >= kTcSmemTiles) { const uint2 q = __ldcg(tcm2 + t); cm = max(q.x, q.y); }
         }
         const bool visit = valid && (lb <= 0.0f || !(lb > rmaxf) || !(lb > __uint_as_float(cm)));
         const unsigned vb = __ballot_sync(0xffffffffu, visit);
@@ -486,15 +494,18 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
       if (!done) fetch_tcm();  // for the next choice: lands while this warp waits for the MMAs / the free exact-image stage
       return t;
     };
-    auto issue_x = [&](int n) {  // exact image (20 KB) of position n -> stage n & 3
+    auto issue_x = [&](int n) {  // exact image (10 KB) of position n -> stage n % kTcStages
       const int t = v_seq[n & 7];
       if (lane != 0) return;
-      const uint32_t bar = bar_fullx0 + 8 * (n & (kTcStages - 1));
+      const uint32_t bar = bar_fullx0 + 8 * (n % kTcStages);
       if (t < 0) { mbar_arrive(bar); return; }
       mbar_expect_tx(bar, kXBytes);
-      bulk_g2s(sX0 + (n & (kTcStages - 1)) * kXBytes, tB + ((size_t)t * kTcImages + 2) * kTileFloats, kXBytes, bar);
+      bulk_g2s(sX0 + (n % kTcStages) * kXBytes, tB + ((size_t)t * kTcImages + 2) * kTileFloats, kXBytes, bar);
     };
-    for (int n = 0; n < 3; ++n) { decide(n); issue_x(n); }
+    for (int n = 0; n < 3; ++n) {
+      decide(n);
+      if (n < kTcStages) issue_x(n);
+    }
     prof(11, tick() - t_setup);
     long long p_wm = 0, p_dec = 0, p_sf = 0;
     auto mbar_test = [&](uint32_t bar, uint32_t parity) -> bool {
@@ -508,19 +519,18 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
           : "memory");
       return __all_sync(0xffffffffu, ready != 0);
     };
-    // Two duties, neither blocks the other: the exact image of position nx goes out as soon as every warp evaluated position nx-4
-    // (its stage), and positions are chosen ahead (at most 3 beyond nx: the s_seq ring, and not before the MMAs of position nd-3
-    // completed, so that a choice sees the bests of the tiles before it) while that stage is still busy.
-    int nd = 3, nx = 3;
+    // Two duties, neither blocks the other: the exact image of position nx goes out as soon as every warp evaluated position
+    // nx - kTcStages (its stage), and positions are chosen ahead (at most 3 beyond nx: the s_seq ring, and not before the MMAs of
+    // position nd-3 completed, so that a choice sees the bests of the tiles before it) while that stage is still busy.
+    int nd = 3, nx = kTcStages;
     bool ok = true, end_decided = v_seq[0] < 0 || v_seq[1] < 0 || v_seq[2] < 0;
-    if (end_decided) nx = nd;  // (all three end-marker arrivals were issued above; nothing else to do)
     int idle = 0;
     long long t_idle = 0;
     while (ok && !(end_decided && nx == nd)) {
-      const uint32_t bar_s = bar_sfree0 + 8 * (nx & (kTcStages - 1)), par_s = (uint32_t)(((nx - 4) >> 2) & 1);
+      const uint32_t bar_s = bar_sfree0 + 8 * (nx % kTcStages), par_s = (uint32_t)((nx / kTcStages - 1) & 1);
       const uint32_t bar_m = bar_mma0 + 8 * ((nd - 3) & (kTcDone - 1)), par_m = (uint32_t)(((nd - 3) >> 2) & 1);
       const bool can_x = nx < nd, can_d = !end_decided && nd < nx + 4;
-      if (can_x && (nx < 4 || mbar_test(bar_s, par_s))) {
+      if (can_x && mbar_test(bar_s, par_s)) {
         if (kProf && idle) { (can_d ? p_wm : p_sf) += tick() - t_idle; }
         idle = 0;
         issue_x(nx);
@@ -546,11 +556,10 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     if (lane == 0) s_npos = n_issued;
   } else {
     // ================= MMA + filter / evaluation warps =================
-    const int wg = warp >> 2;                                // warpgroup
-    const int rbase = (wg & 1) * 64 + 16 * (warp & 3);      // this warp's 16 rows of the stripe
-    const int cb = (wg >> 1) * 64;                           // this warpgroup's 64 columns of the tile
+    const int wg = warp >> 2;                                // warpgroup = 64-row block of the stripe
+    const int rbase = wg * 64 + 16 * (warp & 3);            // this warp's 16 rows of the stripe
     const int cl = 2 * (lane & 3);                           // fragment d[i]: row rbase + lane / 4 + 8 ((i >> 1) & 1),
-                                                             //                column cb + 8 (i >> 2) + cl + (i & 1)
+                                                             //                column 8 (i >> 2) + cl + (i & 1) of the tile
     // the accumulators hold LB_ij = d~_ij - e_ij = kLow (na' + nb') - 2 dot (split_desc_kernel); an entry is a candidate iff
     // LB_ij <= the best exact distance known for row i or for column j
     const float kLow = 1.0f - 0.5f * kTcC;
@@ -567,8 +576,9 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
       Ri_ub[h] = row_ok[h] ? INFINITY : -INFINITY;           // row threshold from the tile-local upper bounds (padded rows: never)
     }
     const uint32_t row_bits = (row_ok[0] ? 0x33333333u : 0u) | (row_ok[1] ? 0xCCCCCCCCu : 0u);  // fragment entries of valid rows
-    const float4* __restrict__ aex = reinterpret_cast<const float4*>(smem + 2 * kTcTileBytes);  // exact image of the A block
-    const uint32_t aH = sA + (uint32_t)((wg & 1) * 64 * 16), aL = aH + kTcTileBytes;           // operand rows of this warpgroup
+    // the warpgroup's A block (hi | lo | exact): operand rows of the MMAs, exact image of rows 64 wg + p (index p)
+    const float4* __restrict__ aex = reinterpret_cast<const float4*>(smem + (wg * kTcImages + 2) * kTcTileBytes);
+    const uint32_t aH = sA + (uint32_t)(wg * kTcImages * kTcTileBytes), aL = aH + kTcTileBytes;
     float* wcj = s_wcj[warp];
     unsigned short* wq = s_queue[warp];
     int evals_w = 0;
@@ -578,13 +588,13 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     long long p_wx = 0, p_wmm = 0, p_ld = 0, p_prep = 0, p_fil = 0, p_ev = 0;
     int p_tiles = 0;
     // column snapshot (best | point index) of the NEXT tile, fetched while the current one is processed when the scheduler
-    // has already published it (pf_tile = tile the prefetch belongs to, -1 = none).  Lane l snapshots columns cb + l, cb + 32 + l.
+    // has already published it (pf_tile = tile the prefetch belongs to, -1 = none).  Lane l snapshots columns l, 32 + l.
     int pf_tile = -1;
     unsigned long long pf_cb[2] = {~0ull, ~0ull};
     unsigned pf_ob[2] = {0u, 0u};
     // shared per-tile column maxima (scheduler warp): after a tile is evaluated its 64 column bests are read again, and one tile
-    // later (the load has landed) their max refreshes tcm4[tile][g] of both 32-column groups g of the warp
-    unsigned* __restrict__ tcmw = tile_cmax + ((size_t)pair * (V >> 7)) * 4 + (cb >> 5);
+    // later (the load has landed) their max refreshes tcm2[tile][g] of both 32-column groups g
+    unsigned* __restrict__ tcmw = tile_cmax + ((size_t)pair * (V / kTcN)) * 2;
     int rr_tile = -1;
     unsigned rr_val[2] = {0u, 0u};
     auto rr_flush = [&]() {
@@ -592,14 +602,14 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
 #pragma unroll
       for (int s = 0; s < 2; ++s) {
         const unsigned m = __reduce_max_sync(0xffffffffu, rr_val[s]);
-        if (lane == 0) atomicMin(tcmw + (size_t)rr_tile * 4 + s, m);
+        if (lane == 0) atomicMin(tcmw + (size_t)rr_tile * 2 + s, m);
       }
       rr_tile = -1;
     };
     for (int k = 0;; ++k) {
-      const int ts = k & (kTcDone - 1), st = k & (kTcStages - 1), hs = k & 1;
+      const int ts = k & (kTcDone - 1), st = k % kTcStages;
       const long long q0 = tick();
-      if (alive) alive = mbar_wait(bar_fullx0 + 8 * st, (uint32_t)((k >> 2) & 1));  // the exact image is read below
+      if (alive) alive = mbar_wait(bar_fullx0 + 8 * st, (uint32_t)((k / kTcStages) & 1));  // the exact image is read below
       const long long q1 = tick();
       p_wx += q1 - q0;
       alive = __all_sync(0xffffffffu, alive);
@@ -615,9 +625,9 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
         } else {
 #pragma unroll
           for (int s = 0; s < 2; ++s)
-            if (c0 + cb + 32 * s + lane < nB) {
-              cb_cur[s] = __ldcg(cbg + c0 + cb + 32 * s + lane);
-              ob[s] = permB[c0 + cb + 32 * s + lane];
+            if (c0 + 32 * s + lane < nB) {
+              cb_cur[s] = __ldcg(cbg + c0 + 32 * s + lane);
+              ob[s] = permB[c0 + 32 * s + lane];
             }
         }
         pf_tile = -1;
@@ -629,16 +639,16 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
 #pragma unroll
             for (int s = 0; s < 2; ++s) {
               pf_cb[s] = ~0ull; pf_ob[s] = 0u;
-              if (jn * kTcN + cb + 32 * s + lane < nB) {
-                pf_cb[s] = __ldcg(cbg + jn * kTcN + cb + 32 * s + lane);
-                pf_ob[s] = permB[jn * kTcN + cb + 32 * s + lane];
+              if (jn * kTcN + 32 * s + lane < nB) {
+                pf_cb[s] = __ldcg(cbg + jn * kTcN + 32 * s + lane);
+                pf_ob[s] = permB[jn * kTcN + 32 * s + lane];
               }
             }
           }
         }
       }
       const long long q2 = tick();
-      if (alive && jt >= 0) alive = mbar_wait(bar_fullhl0 + 8 * hs, (uint32_t)((k >> 1) & 1));  // operand images of the tile
+      if (alive && jt >= 0) alive = mbar_wait(bar_fullhl, (uint32_t)(k & 1));  // operand images of the tile
       alive = __all_sync(0xffffffffu, alive);
       if (!wg_all(alive && jt >= 0, wg)) {  // end of the stripe, or a barrier that never completed: the warpgroup leaves together
         if (!alive) *v_dead = 1;
@@ -649,15 +659,16 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
 #pragma unroll
       for (int i = 0; i < 32; ++i) d[i] = 0.0f;
       {
-        const uint32_t bH = sHL0 + hs * kHLBytes + (uint32_t)(cb * 16), bL = bH + kTcTileBytes;
+        constexpr uint32_t kKB = 2 * kTcBlk * 16;  // bytes per K block of 8 (two 4-wide K chunks)
+        const uint32_t bH = sHL, bL = bH + kTcTileBytes;
         asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory");
 #pragma unroll
         for (int kb = 0; kb < kTcKB; ++kb) {
-          wgmma_tf32_64x64x8(d, tc_smem_desc(aH + kb * 4096), tc_smem_desc(bL + kb * 4096), kb > 0);
-          wgmma_tf32_64x64x8(d, tc_smem_desc(aL + kb * 4096), tc_smem_desc(bH + kb * 4096), 1);
+          wgmma_tf32_64x64x8(d, tc_smem_desc(aH + kb * kKB), tc_smem_desc(bL + kb * kKB), kb > 0);
+          wgmma_tf32_64x64x8(d, tc_smem_desc(aL + kb * kKB), tc_smem_desc(bH + kb * kKB), 1);
         }
 #pragma unroll
-        for (int kb = 0; kb < kTcKB; ++kb) wgmma_tf32_64x64x8(d, tc_smem_desc(aH + kb * 4096), tc_smem_desc(bH + kb * 4096), 1);
+        for (int kb = 0; kb < kTcKB; ++kb) wgmma_tf32_64x64x8(d, tc_smem_desc(aH + kb * kKB), tc_smem_desc(bH + kb * kKB), 1);
         asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
         asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
 #pragma unroll
@@ -673,13 +684,13 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
       const long long q4 = tick();
       p_ld += q4 - q3;
       if (!skip) {
-        const float4* __restrict__ bex = reinterpret_cast<const float4*>(smem + kABytes + 2 * kHLBytes + st * kXBytes);  // exact image
+        const float4* __restrict__ bex = reinterpret_cast<const float4*>(smem + kABytes + kHLBytes + st * kXBytes);  // exact image
         // ---- per-column filter data of the lane's two snapshot columns
         float dbest[2];
         bool col_warm = false;
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
-          const float nbm = bex[9 * 128 + cb + 32 * s + lane].x;  // kLow |b'_j|^2, +inf for padded columns (split_desc_kernel)
+          const float nbm = bex[9 * kTcBlk + 32 * s + lane].x;  // kLow |b'_j|^2, +inf for padded columns (split_desc_kernel)
           dbest[s] = cb_cur[s] == ~0ull ? INFINITY : __uint_as_float((unsigned)(cb_cur[s] >> 32));
           wcj[32 * s + lane] = nbm == INFINITY ? -INFINITY : dbest[s];  // column threshold: +inf while the column has no exact distance yet
           col_warm |= cb_cur[s] == ~0ull && nbm != INFINITY;
@@ -702,8 +713,8 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
           for (int i = 0; i < 32; i += 4) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              const int c = 2 * i + cl + e;  // = 8 (i >> 2) + cl + e: this entry pair's column of the warp's 64
-              const float nbc = bex[9 * 128 + cb + c].x;
+              const int c = 2 * i + cl + e;  // = 8 (i >> 2) + cl + e: this entry pair's column of the tile
+              const float nbc = bex[9 * kTcBlk + c].x;
               const float ub0 = fmaf(kW, nam[0] + nbc, d[i + e]), ub1 = fmaf(kW, nam[1] + nbc, d[i + 2 + e]);
               rowub[0] = fminf(rowub[0], ub0);
               rowub[1] = fminf(rowub[1], ub1);
@@ -727,7 +738,7 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
         const long long q5 = tick();
         p_prep += q5 - q4;
         // ---- branch-free filter of the lane's 32 entries: two compares and a predicated OR per entry
-        const int ncol = nB - c0 - cb;  // valid columns of the warp's 64 (padding never competes, see below)
+        const int ncol = nB - c0;  // valid columns of the tile (padding never competes, see below)
         uint32_t mask = 0, col_bits = 0;
 #pragma unroll
         for (int i = 0; i < 32; i += 4) {
@@ -745,8 +756,8 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
             if (2 * i + cl + (e & 1) < ncol) col_bits |= 1u << (i + e);
             if (kDbg) {
               const int h = e >> 1, c = 2 * i + cl + (e & 1);
-              if (stripe == 0 && k == 0 && row_ok[h] && c < ncol)
-                dbg_tile[(size_t)oa[h] * kTcN + permB[c0 + cb + c]] = fmaf(0.5f * kW, nam[h] + bex[9 * 128 + cb + c].x, lbv);
+              if (stripe == 0 && row_ok[h] && c < ncol)  // 128 x 128 dump, row = source point
+                dbg_tile[(size_t)oa[h] * 128 + permB[c0 + c]] = fmaf(0.5f * kW, nam[h] + bex[9 * kTcBlk + c].x, lbv);
             }
           }
         }
@@ -772,12 +783,11 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
           const int q = lane < nb ? wq[lane] : 0;
           const int sl = q >> 5, i = q & 31, h = (i >> 1) & 1;
           const int rr = rbase + (sl >> 2) + 8 * h;            // row of the stripe
-          const int c = 8 * (i >> 2) + 2 * (sl & 3) + (i & 1);  // column of the warp's 64
-          const int pcol = cb + c;
+          const int c = 8 * (i >> 2) + 2 * (sl & 3) + (i & 1);  // column of the tile
           float acc = 0.0f;
 #pragma unroll
           for (int kc = 0; kc < (kDescDim + 3) / 4; ++kc) {
-            const float4 a = aex[kc * 128 + rr], b = bex[kc * 128 + pcol];
+            const float4 a = aex[kc * kTcBlk + (rr & (kTcBlk - 1))], b = bex[kc * kTcBlk + c];
             float diff = a.x - b.x;
             acc = __fmaf_rn(diff, diff, acc);
             if (4 * kc + 1 < kDescDim) { diff = a.y - b.y; acc = __fmaf_rn(diff, diff, acc); }
@@ -794,15 +804,16 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
           if (lane < nb && acc == acc) {  // NaN never wins
             const unsigned long long pr = tc_pack(acc, (int)oc);
             if (pr < v_rbest[rr]) atomicMin(&s_rbest[rr], pr);
-            if (acc <= dbc) atomicMin(cbg + c0 + pcol, tc_pack(acc, (int)orow));
+            if (acc <= dbc) atomicMin(cbg + c0 + c, tc_pack(acc, (int)orow));
           }
           __syncwarp();
           remaining = tot - nb;
         }
-        // massive ties: once more than half of the entries seen needed the exact chain, hand the pair to the exact kernel
+        // massive ties: once more than half of the entries seen needed the exact chain (after at least 8 x 128 x 128 entries),
+        // hand the pair to the exact kernel
         if (lane == 0 && evals_w) {
           const int seen = atomicAdd(&s_evals, evals_w) + evals_w;
-          if (k >= 7 && seen > (k + 1) * (kTcM * kTcN / 2)) *v_abort = 1;
+          if ((k + 1) * (kTcM * kTcN) >= 8 * 128 * 128 && seen > (k + 1) * (kTcM * kTcN / 2)) *v_abort = 1;
         }
         evals_w = 0;
         p_ev += tick() - q6;
@@ -815,8 +826,8 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
           rr_val[s] = 0;  // padding columns do not count
-          if (c0 + cb + 32 * s + lane < nB) {
-            const unsigned long long cbn = __ldcg(cbg + c0 + cb + 32 * s + lane);
+          if (c0 + 32 * s + lane < nB) {
+            const unsigned long long cbn = __ldcg(cbg + c0 + 32 * s + lane);
             rr_val[s] = cbn == ~0ull ? 0x7F800000u : (unsigned)(cbn >> 32);
           }
         }
@@ -841,7 +852,33 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
   if (!aborted && threadIdx.x < kTcM && r0 + (int)threadIdx.x < nA) rowbest[(size_t)pair * V + r0 + threadIdx.x] = s_rbest[threadIdx.x];
 }
 
-static size_t tc_smem_bytes() { return (size_t)kTcImages * kTcTileBytes + 2 * 2 * (size_t)kTcTileBytes + (size_t)kTcStages * kTcTileBytes; }  // 220 KB
+// A (2 blocks x 3 images) + operand stage (hi | lo) + exact-image stages = 100 KB
+static size_t tc_smem_bytes() {
+  return ((size_t)(kTcM / kTcBlk) * kTcImages + 2 + kTcStages) * kTcTileBytes;
+}
+
+// dynamic shared memory of tc_nn_kernel and a shared-memory-first carveout, so that two CTAs fit on every SM
+static int tc_prepare(qb200_handle* h, const void* kernel) {
+  if (int rc = ensure_dyn_smem(h, kernel, tc_smem_bytes())) return rc;
+  QB_CUDA_TRY(h, cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  return QB200_OK;
+}
+
+// threads, dynamic and static shared bytes, registers per thread and resident CTAs per SM of tc_nn_kernel as launched
+int tc_footprint(qb200_handle* h, int* out5) {
+  const void* kernel = (const void*)tc_nn_kernel<false>;
+  if (int rc = tc_prepare(h, kernel)) return rc;
+  cudaFuncAttributes fa;
+  QB_CUDA_TRY(h, cudaFuncGetAttributes(&fa, kernel));
+  int ctas = 0;
+  QB_CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, kernel, kTcThreads, tc_smem_bytes()));
+  out5[0] = kTcThreads;
+  out5[1] = (int)tc_smem_bytes();
+  out5[2] = (int)fa.sharedSizeBytes;
+  out5[3] = fa.numRegs;
+  out5[4] = ctas;
+  return QB200_OK;
+}
 
 // norm keys -> one radix sort for all clouds (h->val_b = rank -> point) -> duplicate classes.
 // Scratch (free once the sort consumed its inputs): val_a = unique rank -> point, key_a = [class of rank | unique counts].
@@ -866,7 +903,7 @@ static int sort_and_dedup(qb200_handle* h, int n_clouds, int dedup) {
 int launch_match_nn(qb200_handle* h, int n_pairs) {
   const int V = h->V;
   const size_t smem = tc_smem_bytes();
-  if (int rc = ensure_dyn_smem(h, (const void*)tc_nn_kernel<false>, smem)) return rc;
+  if (int rc = tc_prepare(h, (const void*)tc_nn_kernel<false>)) return rc;
   int rc = sort_and_dedup(h, 2 * n_pairs, 1);
   if (rc) return rc;
   const uint32_t* uperm = h->val_a;
@@ -875,7 +912,7 @@ int launch_match_nn(qb200_handle* h, int n_pairs) {
   // class results, indexed by unique rank (colpart is this kernel's scratch; the exact fallback works in rowbest / colbest)
   unsigned long long* colbest_u = h->colpart;
   unsigned long long* rowbest_u = h->colpart + (size_t)h->S * V;
-  unsigned* tile_cmax = reinterpret_cast<unsigned*>(h->colpart + (size_t)2 * h->S * V);  // [S][V/128][4] float bits, start above "+inf"
+  unsigned* tile_cmax = reinterpret_cast<unsigned*>(h->colpart + (size_t)2 * h->S * V);  // [S][V/64][2] float bits, start above "+inf"
   QB_CUDA_TRY(h, cudaMemsetAsync(h->rowbest, 0xFF, (size_t)n_pairs * V * 8, h->stream));
   QB_CUDA_TRY(h, cudaMemsetAsync(h->colbest, 0xFF, (size_t)n_pairs * V * 8, h->stream));
   QB_CUDA_TRY(h, cudaMemsetAsync(h->colpart, 0xFF, ((size_t)2 * h->S * V + (size_t)h->S * (V >> 7) * 2 + 2) * 8, h->stream));  // 0xFFFFFFFF > +inf bits
@@ -886,7 +923,7 @@ int launch_match_nn(qb200_handle* h, int n_pairs) {
   cudaEventRecord(h->kev[0], h->stream);
   static const int tc_prof = (getenv("QB200_TC_PROF") && getenv("QB200_TC_PROF")[0] == '1') ? 1 : 0;
   if (tc_prof) {
-    if (int rc2 = ensure_dyn_smem(h, (const void*)tc_nn_kernel<false, true>, smem)) return rc2;
+    if (int rc2 = tc_prepare(h, (const void*)tc_nn_kernel<false, true>)) return rc2;
     tc_nn_kernel<false, true><<<g, kTcThreads, smem, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, V, uperm, rowbest_u, colbest_u,
                                                                   tile_cmax, h->tc_fallback, h->tc_stats, nullptr);
   } else {
@@ -901,11 +938,11 @@ int launch_match_nn(qb200_handle* h, int n_pairs) {
   return launch_match_exact(h, n_pairs, h->tc_fallback);
 }
 
-// debug/validation hook: approximate distances d~ of the first 128 x 128 tile of pair 0 (descriptors already in desc_t;
-// duplicates are kept so that every (row, column) of the dump is filled)
+// debug/validation hook: approximate distances d~ of stripe 0 of pair 0, both 64-column tiles of up to 128 x 128 descriptors
+// (descriptors already in desc_t; duplicates are kept so that every (row, column) of the dump is filled)
 int launch_tc_debug_tile(qb200_handle* h, float* d_out) {
   const size_t smem = tc_smem_bytes();
-  if (int rc0 = ensure_dyn_smem(h, (const void*)tc_nn_kernel<true>, smem)) return rc0;
+  if (int rc0 = tc_prepare(h, (const void*)tc_nn_kernel<true>)) return rc0;
   int rc = sort_and_dedup(h, 2, 0);
   if (rc) return rc;
   const uint32_t* uperm = h->val_a;

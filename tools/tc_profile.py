@@ -1,7 +1,8 @@
 """Where tc_nn_kernel's time goes: per-role clock64 accounting (QB200_TC_PROF=1 build path), one 64-pair wave of street scans.
 
   QB200_TC_PROF=1 QB200_LANES=1 python tools/tc_profile.py [--pairs 64] [--scene street|dense]
-Prints per-CTA averages in microseconds at the measured SM clock.
+Prints per-CTA averages in microseconds at the measured SM clock.  Roles: "sched" = the scheduler warp (chooses the tiles,
+issues the exact-image copies), "copy" = the operand-copy warp, "epi" = the MMA + filter / evaluation warps (averaged over them).
 """
 import argparse, json, os, sys
 os.environ.setdefault("QB200_TC_PROF", "1")
@@ -11,9 +12,10 @@ import numpy as np
 import torch
 from quatro_b200 import capi, synth
 
-NAMES = ["n_cta", "cta_total", "setup", "copy_prologue", "copy_wait_mma", "copy_decide", "copy_wait_sfree", "unused_15", "unused_16",
-         "unused_17", "unused_18", "epi_wait_a", "epi_wait_x", "epi_wait_hl_and_mma", "epi_vote", "epi_prep", "epi_filter", "epi_eval",
-         "epi_loop_total", "epi_tiles"]
+# stats[8 + i] of the kernel (its prof() slots 8..31)
+NAMES = {0: "n_cta", 1: "cta_total", 2: "setup", 3: "sched_prologue", 4: "copy_wait_mma", 5: "sched_decide",
+         6: "sched_wait_sfree", 11: "epi_wait_a", 12: "epi_wait_x", 13: "epi_wait_hl_and_mma", 14: "epi_vote", 15: "epi_prep",
+         16: "epi_filter", 17: "epi_eval", 18: "epi_loop_total", 19: "epi_tiles", 20: "copy_wait_decided", 21: "sched_wait_mma"}
 
 def main():
     ap = argparse.ArgumentParser()
@@ -25,19 +27,23 @@ def main():
     p = bench.scene_params(a.scene)
     pairs = [synth.outdoor_pair(1000 + i)[:2] for i in range(a.pairs)]
     h = capi.Handle(device=0, max_batch_slots=a.pairs, **bench.SCENES[a.scene]["cfg"])
+    fp = h.debug_tc_footprint()
+    epi_warps = fp["threads"] // 32 - 2   # all warps but the copy and scheduler warps
     for rep in range(3):
         res = h.register_batch(pairs, p)
         prof = h.debug_tc_profile(reset=True)
         st = h.debug_match_stats(reset=True)
     n = float(prof[0])
-    out = {"stats": st, "n_cta": int(n)}
+    out = {"stats": st, "footprint": fp, "n_cta": int(n)}
     cyc_us = 1.0 / a.mhz
-    for i, name in enumerate(NAMES[1:], start=1):
+    for i, name in sorted(NAMES.items()):
+        if i == 0:
+            continue
         v = float(prof[i])
-        if name.startswith("epi_") and name != "epi_tiles":
-            v /= 16.0  # summed over the 16 filter warps
+        if name.startswith("epi_"):
+            v /= epi_warps  # summed over the filter warps
         if name == "epi_tiles":
-            out[name + "_per_cta"] = round(v / 16.0 / n, 2)
+            out[name + "_per_cta"] = round(v / n, 2)
         else:
             out[name + "_us_per_cta"] = round(v / n * cyc_us, 2)
     print(json.dumps(out, indent=1))
