@@ -381,6 +381,11 @@ int qb200_debug_tc_distances(qb200_handle* h, const float* a33, int32_t na, cons
  * out4[0] = descriptor pairs that went through the exact fp32 chain, [1] = 128 x 64 tiles drained,
  * [2] = warm-up passes, [3] = stripes handed to the exact kernel.  Synchronises the handle's stream. */
 int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset);
+/* Diagnostics: both nearest-neighbour tables of the most recent qb200_match, in point order: rowbest[i] = packed
+ * (distance bits << 32 | target index) of the best target of source point i, colbest[j] = the same for the best source of target
+ * point j, ~0 = none.  min(cap_rows, n_src) and min(cap_cols, n_tgt) entries are written (either pointer may be NULL); the
+ * tables are those the mutual check read, after any stripe was redone by the exact kernel.  Synchronises the handle's stream. */
+int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, uint64_t* colbest, int32_t cap_cols);
 /* QB200_TC_PROF=1 only: per-role clock64 accounting of tc_nn_kernel (24 counters, see tools/tc_profile.py) */
 int qb200_debug_tc_profile(qb200_handle* h, uint64_t* out24, int32_t reset);
 /* Diagnostics: footprint of the tensor-core nearest-neighbour kernel as launched: out5[0] = threads per CTA,

@@ -36,6 +36,7 @@ class Oracle:
         L.qo_neighbors.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_int]
         L.qo_match.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.POINTER(Params), C.c_void_p, C.c_int,
                                C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]
+        L.qo_nn_tables.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         L.qo_build_graph.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p, C.c_int, C.c_void_p,
                                      C.POINTER(C.c_int64)]
         L.qo_max_clique.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double, C.c_void_p, C.POINTER(C.c_int), C.c_void_p,
@@ -154,6 +155,15 @@ class Oracle:
         if want_mutual:
             return corr[: min(n.value, cap)].copy(), nm.value, st, mutual[: nm.value].copy()
         return corr[: min(n.value, cap)].copy(), nm.value, st
+
+    def nn_tables(self, adesc, bdesc):
+        """Both nearest-neighbour tables of match() for adesc (rows) against bdesc (columns), without the larger-cloud swap:
+        (best B of every A row, best A of every B column) as packed uint64 (distance bits << 32 | index), ~0 = none."""
+        adesc, bdesc = _f32(adesc, 33), _f32(bdesc, 33)
+        ba, bb = np.zeros(len(adesc), np.uint64), np.zeros(len(bdesc), np.uint64)
+        st = self.lib.qo_nn_tables(_ptr(adesc), len(adesc), _ptr(bdesc), len(bdesc), _ptr(ba), _ptr(bb))
+        assert st == 0, st
+        return ba, bb
 
     def build_graph(self, a4, b4, noise_bound: float, cbar2: float, words_per_row: Optional[int] = None):
         a4, b4 = _f32(a4, 4), _f32(b4, 4)

@@ -458,8 +458,9 @@ inline uint64_t pack_dist(float d, int idx) {
   return ((uint64_t)u << 32) | (uint32_t)idx;
 }
 
+// packA / packB (optional): the packed (distance bits << 32 | index) minima themselves, ~0 = no candidate
 void nn_both_ways(const float* A, int nA, const float* B, int nB, std::vector<int>& nnA /* per A row: argmin B */,
-                  std::vector<int>& nnB /* per B row: argmin A */) {
+                  std::vector<int>& nnB /* per B row: argmin A */, uint64_t* packA = nullptr, uint64_t* packB = nullptr) {
   // B transposed so the inner loop runs over candidates
   std::vector<float> Bt((size_t)33 * nB);
   for (int j = 0; j < nB; ++j)
@@ -492,6 +493,7 @@ void nn_both_ways(const float* A, int nA, const float* B, int nB, std::vector<in
         if (ki < myB[j]) myB[j] = ki;
       }
       nnA[i] = best == ~0ull ? -1 : (int)(uint32_t)best;
+      if (packA) packA[i] = best;
     }
 #pragma omp critical
     for (int j = 0; j < nB; ++j)
@@ -499,6 +501,7 @@ void nn_both_ways(const float* A, int nA, const float* B, int nB, std::vector<in
   }
   nnB.assign(nB, -1);
   for (int j = 0; j < nB; ++j) nnB[j] = bestB[j] == ~0ull ? -1 : (int)(uint32_t)bestB[j];
+  if (packB) std::copy(bestB.begin(), bestB.end(), packB);
 }
 
 void center_points(const P4* pts, int n, std::vector<float>& out /* n x 3 */) {
@@ -1207,6 +1210,15 @@ int qo_match(const float* src4, int n_src, const float* sdesc, const float* tgt4
   const int m = std::min((int)mo.corr.size(), cap);
   for (int i = 0; i < m; ++i) { corr[2 * i] = mo.corr[i].first; corr[2 * i + 1] = mo.corr[i].second; }
   return (int)mo.corr.size() > cap ? QB200_CAPACITY_EXCEEDED : QB200_OK;
+}
+
+// both nearest-neighbour tables of match() for A (nA x 33) against B (nB x 33), in the given order (no larger-cloud swap):
+// bestA[i] = packed (distance bits << 32 | j) of row i's nearest B, bestB[j] = the same for column j's nearest A, ~0 = none
+int qo_nn_tables(const float* A, int nA, const float* B, int nB, uint64_t* bestA, uint64_t* bestB) {
+  if (nA < 0 || nB < 0) return QB200_ERR_BAD_ARG;
+  std::vector<int> nnA, nnB;
+  nn_both_ways(A, nA, B, nB, nnA, nnB, bestA, bestB);
+  return QB200_OK;
 }
 
 int qo_build_graph(const float* a4, const float* b4, int L, double noise_bound, double cbar2, uint32_t* adj, int wpr,

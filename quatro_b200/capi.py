@@ -155,6 +155,7 @@ def load_library(build: bool = True) -> C.CDLL:
         "qb200_get_kernel_ms": (i32, [vp, vp, vp, i32]),
         "qb200_debug_tc_distances": (i32, [vp, vp, i32, vp, i32, vp]),
         "qb200_debug_match_stats": (i32, [vp, vp, i32]),
+        "qb200_debug_nn_tables": (i32, [vp, vp, i32, vp, i32]),
         "qb200_register_batch_enqueue": (i32, [vp, vp, i32, vp, i32, vp]),
         "qb200_register_batch_flush": (i32, [vp]),
         "qb200_debug_tc_profile": (i32, [vp, vp, i32]),
@@ -191,6 +192,7 @@ EXPORTED_SYMBOLS = [
     "qb200_get_last_final_inliers", "qb200_get_last_correspondences", "qb200_get_stage_ms", "qb200_get_kernel_ms",
     "qb200_debug_tc_distances",
     "qb200_debug_match_stats",
+    "qb200_debug_nn_tables",
     "qb200_register_batch_enqueue",
     "qb200_register_batch_flush",
     "qb200_debug_tc_profile",
@@ -561,6 +563,13 @@ class Handle:
         out = np.zeros(4, np.uint64)
         self._check(self.lib.qb200_debug_match_stats(self.h, _ptr(out), int(reset)), "qb200_debug_match_stats")
         return {"exact_evals": int(out[0]), "tiles": int(out[1]), "warmups": int(out[2]), "aborted_stripes": int(out[3])}
+
+    def debug_nn_tables(self, n_src: int, n_tgt: int):
+        """(best target of every source point, best source of every target point) of the last match, packed uint64
+        (distance bits << 32 | index), ~0 = none."""
+        rb, cb = np.full(n_src, ~np.uint64(0)), np.full(n_tgt, ~np.uint64(0))
+        self._check(self.lib.qb200_debug_nn_tables(self.h, _ptr(rb), n_src, _ptr(cb), n_tgt), "qb200_debug_nn_tables")
+        return rb, cb
 
     def debug_tc_profile(self, reset: bool = True) -> np.ndarray:
         out = np.zeros(24, np.uint64)

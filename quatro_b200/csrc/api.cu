@@ -524,11 +524,14 @@ int qb200_match(qb200_handle* h, const float* src4, int32_t n_src, const float* 
   if (n_mutual) *n_mutual = 0;
   if (n_src > h->V || n_tgt > h->V) { h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points"); return QB200_ERR_BAD_ARG; }
   cudaSetDevice(h->device);
+  h->last_match_n[0] = h->last_match_n[1] = 0;
   if (n_src == 0 || n_tgt == 0) return QB200_OK;
   int rc = wave_reset(h, 2);
   if (rc) return rc;
   if ((rc = upload_cloud_as_voxels(h, 0, src4, n_src))) return rc;
   if ((rc = upload_cloud_as_voxels(h, 1, tgt4, n_tgt))) return rc;
+  h->last_match_n[0] = n_src;
+  h->last_match_n[1] = n_tgt;
   float* scratch = h->aos_scratch;
   QB_CUDA_TRY(h, cudaMemcpyAsync(scratch, src_desc33, (size_t)n_src * kDescDim * sizeof(float), cudaMemcpyHostToDevice, h->stream));
   if ((rc = launch_desc_from_aos(h, 0, n_src, scratch))) return rc;
@@ -1082,6 +1085,18 @@ int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset) {
     if (rc) return rc;
     for (int i = 0; i < 4; ++i) out4[i] += o2[i];
   }
+  return QB200_OK;
+}
+
+// Nearest-neighbour tables of the most recent qb200_match (pair 0 of the handle, point order): what match_mutual_kernel read
+int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, uint64_t* colbest, int32_t cap_cols) {
+  if (!h || cap_rows < 0 || cap_cols < 0) return QB200_ERR_BAD_ARG;
+  cudaSetDevice(h->device);
+  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  const int nr = cap_rows < h->last_match_n[0] ? cap_rows : h->last_match_n[0];
+  const int nc = cap_cols < h->last_match_n[1] ? cap_cols : h->last_match_n[1];
+  if (rowbest && nr > 0) QB_CUDA_TRY(h, cudaMemcpy(rowbest, h->rowbest, (size_t)nr * 8, cudaMemcpyDeviceToHost));
+  if (colbest && nc > 0) QB_CUDA_TRY(h, cudaMemcpy(colbest, h->colbest, (size_t)nc * 8, cudaMemcpyDeviceToHost));
   return QB200_OK;
 }
 

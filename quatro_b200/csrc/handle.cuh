@@ -109,6 +109,7 @@ struct qb200_handle {
   // ---- state mirrored from the reference's statics ----
   double rot_noise_bound_latched;  // quatro.hpp:469-470 (0 = not latched yet)
   int last_n_corr, last_n_clique, last_n_final;  // slot 0 of the most recent single-pair call
+  int last_match_n[2];        // source / target points of the most recent qb200_match (qb200_debug_nn_tables)
 
   cudaEvent_t ev[9];
   float stage_ms[8];

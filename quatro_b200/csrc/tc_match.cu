@@ -46,6 +46,14 @@ constexpr int kTcDone = 4;                         // ring of "MMAs of position 
 constexpr int kTcStages = 2;                      // ring of exact B images (prefetch distance 1); operand images: 1 stage
 constexpr int kTcSmemTiles = 256;                 // column tiles whose lower bounds live in shared memory (V <= 16384)
 constexpr float kTcC = 1.2e-4f;                   // |d~ - d| <= kTcC/2 * (|a'|^2 + |b'|^2): 3x the worst error measured (test_tc_filter_error_bound)
+// Largest centred squared norm the tensor-core path takes: below it every term of kLow (|a'|^2 + |b'|^2) - 2 a'.b' and every exact
+// distance stays below 2^127 < FLT_MAX.  A pair with a larger, infinite or NaN norm goes to the exact kernel (split_desc_kernel).
+constexpr float kTcNormMax = 0x1p124f;
+// Relative part of the tile-skip slack, per unit of square-rooted norm (tile_lb in tc_nn_kernel).  The norm chain rounds
+// x' = x - mu (1 ulp), 33 fma (33 ulp of |x'|^2) and the square root (1 ulp): |x'| computed = |x'| (1 + e), |e| <= 18.5 * 2^-24
+// = 1.1e-6, so the gap of two norm ranges is off by at most 1.1e-6 (amax + bmax).  4e-6 leaves a factor of 3.6 for the float
+// arithmetic of the bound itself.  The 0.9999 factor covers the exact chain's own rounding (d computed >= d (1 - 36 * 2^-24)).
+constexpr float kTcNormRel = 4.0e-6f;
 constexpr int kSpinLimit = 400000;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -117,10 +125,12 @@ __global__ void __launch_bounds__(256) norm_key_kernel(const float* __restrict__
 }
 
 // centred TF32 split + exact image + centred squared norm, written block-wise in the shared-memory operand layout;
-// rank r of the cloud (ascending norm, ties by index) is point perm[r]
+// rank r of the cloud (ascending norm, ties by index) is point perm[r].  A norm above kTcNormMax, +inf or NaN (a non-finite bin,
+// or finite values whose squares overflow) would turn the filter's lower bounds into NaN or inf, which no threshold passes:
+// such a pair is flagged for the exact kernel, whose NaN / inf handling is the oracle's.
 __global__ void __launch_bounds__(256) split_desc_kernel(const float* __restrict__ desc_t, const int* __restrict__ n_vox, int V,
                                                          const uint32_t* __restrict__ perm, float* __restrict__ tiles,
-                                                         float* __restrict__ norm) {
+                                                         float* __restrict__ norm, int* __restrict__ fallback) {
   const int cloud = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   const int n = n_vox[cloud];
@@ -160,6 +170,7 @@ __global__ void __launch_bounds__(256) split_desc_kernel(const float* __restrict
   // the exact image has no data in dims 36..39: slot 36 carries the column's filter term kLow |x'|^2 (+inf = padding)
   img[2 * (kTileFloats / 4) + (kDescK / 4 - 1) * kTcBlk] = make_float4(q < n ? kLow * acc : INFINITY, 0.0f, 0.0f, 0.0f);
   if (q < n) norm[(size_t)cloud * V + q] = acc;  // rank order
+  if (q < n && !(acc <= kTcNormMax)) fallback[cloud >> 1] = 1;
 }
 
 // Exact duplicates.  Street scenes contain hundreds of points with bit-identical descriptors (the histogram of a perfect
@@ -391,7 +402,8 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     const float amin = sqrtf(nrmA[r0]), amax = sqrtf(nrmA[(r0 + kTcM < nA ? r0 + kTcM : nA) - 1]);
     auto tile_lb = [&](int t) -> float {  // lower bound of every exact distance between the stripe and column tile t
       const float bmin = sqrtf(nrmB[t * kTcN]), bmax = sqrtf(nrmB[(t * kTcN + kTcN < nB ? t * kTcN + kTcN : nB) - 1]);
-      const float gap = fmaxf(amin - bmax, bmin - amax) - 2.0e-3f;  // slack: rounding of the norm chains and square roots
+      // slack: rounding of the norm chains and square roots (kTcNormRel), absolute 2e-3 for norms near 0
+      const float gap = fmaxf(amin - bmax, bmin - amax) - (2.0e-3f + kTcNormRel * (amax + bmax));
       if (!(amin <= amax && bmin <= bmax)) return 0.0f;               // NaN norms: never skip
       return gap > 0.0f ? gap * gap * 0.9999f : 0.0f;
     };
@@ -918,7 +930,7 @@ int launch_match_nn(qb200_handle* h, int n_pairs) {
   QB_CUDA_TRY(h, cudaMemsetAsync(h->colpart, 0xFF, ((size_t)2 * h->S * V + (size_t)h->S * (V >> 7) * 2 + 2) * 8, h->stream));  // 0xFFFFFFFF > +inf bits
   QB_CUDA_TRY(h, cudaMemsetAsync(h->tc_fallback, 0, (size_t)n_pairs * sizeof(int), h->stream));
   const dim3 gsplit((V + 255) / 256, 2 * n_pairs);
-  split_desc_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_t, n_unique, V, uperm, h->desc_tiles, h->desc_norm);
+  split_desc_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_t, n_unique, V, uperm, h->desc_tiles, h->desc_norm, h->tc_fallback);
   const dim3 g(h->NS, n_pairs);
   cudaEventRecord(h->kev[0], h->stream);
   static const int tc_prof = (getenv("QB200_TC_PROF") && getenv("QB200_TC_PROF")[0] == '1') ? 1 : 0;
@@ -950,7 +962,7 @@ int launch_tc_debug_tile(qb200_handle* h, float* d_out) {
   QB_CUDA_TRY(h, cudaMemsetAsync(h->colpart, 0xFF, ((size_t)2 * h->S * h->V + (size_t)h->S * (h->V >> 7) * 2 + 2) * 8, h->stream));
   QB_CUDA_TRY(h, cudaMemsetAsync(h->tc_fallback, 0, sizeof(int), h->stream));
   const dim3 gsplit((h->V + 255) / 256, 2);
-  split_desc_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_t, n_unique, h->V, uperm, h->desc_tiles, h->desc_norm);
+  split_desc_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_t, n_unique, h->V, uperm, h->desc_tiles, h->desc_norm, h->tc_fallback);
   const dim3 g(1, 1);
   tc_nn_kernel<true><<<g, kTcThreads, smem, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, h->V, uperm, h->colpart + (size_t)h->S * h->V,
                                                          h->colpart, reinterpret_cast<unsigned*>(h->colpart + (size_t)2 * h->S * h->V), h->tc_fallback, h->tc_stats, d_out);
