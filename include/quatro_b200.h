@@ -295,8 +295,8 @@ int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const
 /* Batch of independent pairs.  kind says where pairs[i].src/tgt live; results is a host array.
  * The batch is processed in waves of max_batch_slots pairs.  Batches larger than one wave rotate over up to
  * 4 lanes (each further lane -- same buffers again, own stream -- is allocated on first use) so that one wave's
- * host->device copies and solver tail overlap the other waves' dense kernels; QB200_LANES=n (1..4) in the
- * environment caps the lane count (1 = strictly one wave at a time).  Results never depend on the wave size
+ * host->device copies and solver tail overlap the other waves' dense kernels; QB200_LANES=n (1..8, default 4) in
+ * the environment sets the lane count (1 = strictly one wave at a time).  Results never depend on the wave size
  * or the lane. */
 int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs,
                          const qb200_params* p, qb200_mem_kind kind, qb200_result* results);

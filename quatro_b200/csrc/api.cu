@@ -18,18 +18,19 @@
 using namespace qb;
 
 namespace qb {
-int launch_degree(qb200_handle* h, int n_pairs);
+int launch_degree(Lane* h, int n_pairs);
 
-int ensure_dyn_smem(qb200_handle* h, const void* kernel, size_t bytes) {
+cudaError_t ensure_dyn_smem(int device, const void* kernel, size_t bytes) {
   static std::mutex mu;
   static std::map<std::pair<const void*, int>, size_t> current;
   std::lock_guard<std::mutex> lock(mu);
-  size_t& cur = current[std::make_pair(kernel, h->device)];
+  size_t& cur = current[std::make_pair(kernel, device)];
   if (bytes > cur) {
-    QB_CUDA_TRY(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return e;
     cur = bytes;
   }
-  return QB200_OK;
+  return cudaSuccess;
 }
 }
 
@@ -83,115 +84,143 @@ cudaError_t dalloc(T** p, size_t count) {
     }                                                                              \
   } while (0)
 
-int alloc_all(qb200_handle* h) {
-  const size_t S = h->S, R = h->R, V = h->V, Lc = h->Lc, W = h->W, C = 2 * S;
-  QB_CUDA_TRY(h, cudaMalloc((void**)&h->d_cloud_ptr, C * sizeof(float4*)));
-  QB_ALLOC(h, h->d_cloud_n, C);
-  QB_ALLOC(h, h->d_raw_off, C + 1);
-  QB_CUDA_TRY(h, cudaMallocHost((void**)&h->h_cloud_ptr, C * sizeof(float4*)));
-  QB_CUDA_TRY(h, cudaMallocHost((void**)&h->h_cloud_n, C * sizeof(int)));
-  QB_CUDA_TRY(h, cudaMallocHost((void**)&h->h_raw_off, (C + 1) * sizeof(int)));
-  QB_ALLOC(h, h->raw_stage, C * R);
-  QB_CUDA_TRY(h, cudaEventCreate(&h->ev_fork));  // (timing enabled: QB200_TIMELINE measures the waves against it)
-  QB_CUDA_TRY(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
-  QB_CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_copied, cudaEventDisableTiming));
+// A new lane with the settings of `like` (dims, device, n_sm, matcher switch, error sink), its own stream and every buffer of
+// DESIGN §4.  *out is set first, so lane_free releases whatever a failed allocation left behind.
+int lane_alloc(const Lane& like, Lane** out) {
+  Lane* L = *out = new (std::nothrow) Lane();
+  if (!L) return QB200_ERR_CUDA;
+  L->S = like.S; L->R = like.R; L->V = like.V; L->Lc = like.Lc; L->W = like.W; L->NS = like.NS;
+  L->device = like.device; L->n_sm = like.n_sm; L->force_exact_match = like.force_exact_match; L->err = like.err;
+  QB_CUDA_TRY(L, cudaStreamCreateWithFlags(&L->own_stream, cudaStreamNonBlocking));
+  L->stream = L->own_stream;
+  const size_t S = L->S, R = L->R, V = L->V, Lc = L->Lc, W = L->W, C = 2 * S;
+  QB_CUDA_TRY(L, cudaMalloc((void**)&L->d_cloud_ptr, C * sizeof(float4*)));
+  QB_ALLOC(L, L->d_cloud_n, C);
+  QB_ALLOC(L, L->d_raw_off, C + 1);
+  QB_CUDA_TRY(L, cudaMallocHost((void**)&L->h_cloud_ptr, C * sizeof(float4*)));
+  QB_CUDA_TRY(L, cudaMallocHost((void**)&L->h_cloud_n, C * sizeof(int)));
+  QB_CUDA_TRY(L, cudaMallocHost((void**)&L->h_raw_off, (C + 1) * sizeof(int)));
+  QB_ALLOC(L, L->raw_stage, C * R);
   // the sort workspace serves the voxel sort (C*R items, digit histograms in val_a, chunk counts C*kVsChunks <= n_sort in val_b),
   // the lattice / norm sorts (C*V items) and, afterwards, the duplicate-class tables of K6 (2S*V + 2S words in key_a): size it for
   // the largest user
   const size_t n_sort = C * (R > V ? R : V) + 64;
   const size_t n_hist = C * 256 * ((R + kVsTile - 1) / kVsTile);
-  QB_ALLOC(h, h->key_a, n_sort);
-  QB_ALLOC(h, h->key_b, n_sort);
-  QB_ALLOC(h, h->val_a, n_sort > n_hist ? n_sort : n_hist);
-  QB_ALLOC(h, h->val_b, n_sort);
-  QB_ALLOC(h, h->aos_scratch, 2 * V * kDescDim);
+  QB_ALLOC(L, L->key_a, n_sort);
+  QB_ALLOC(L, L->key_b, n_sort);
+  QB_ALLOC(L, L->val_a, n_sort > n_hist ? n_sort : n_hist);
+  QB_ALLOC(L, L->val_b, n_sort);
+  QB_ALLOC(L, L->aos_scratch, 2 * V * kDescDim);
   // the library radix sort only sorts lattice / norm keys of clouds too large for cloud_sort_kernel: at most C*V items
-  h->cub_bytes = sort_temp_bytes((int)(C * V));
-  QB_CUDA_TRY(h, cudaMalloc(&h->cub_temp, h->cub_bytes));
-  QB_ALLOC(h, h->vox_start, C * (V + 1));
-  QB_ALLOC(h, h->vox_pts, C * V);
-  QB_ALLOC(h, h->cell_key, C * V);
-  QB_ALLOC(h, h->cell_start, C * (V + 1));
-  QB_ALLOC(h, h->normals, C * V);
-  QB_ALLOC(h, h->spfh, C * V * kDescPad);
-  QB_ALLOC(h, h->nbr_list, C * kNbrGlobalCap * V);
-  QB_ALLOC(h, h->nbr_cnt, C * V);
-  QB_ALLOC(h, h->desc_t, C * kDescK * V);
-  QB_CUDA_TRY(h, cudaMemset(h->desc_t, 0, C * kDescK * V * sizeof(float)));
-  QB_ALLOC(h, h->desc_tiles, C * kDescK * V * 3);
-  QB_CUDA_TRY(h, cudaMemset(h->desc_tiles, 0, C * kDescK * V * 3 * sizeof(float)));
-  QB_ALLOC(h, h->desc_norm, C * V);
-  QB_ALLOC(h, h->tc_fallback, S);
-  QB_ALLOC(h, h->tc_stats, 32);
-  QB_CUDA_TRY(h, cudaMemset(h->tc_stats, 0, 32 * sizeof(unsigned long long)));
-  QB_ALLOC(h, h->rowbest, S * V);
-  QB_ALLOC(h, h->colpart, 2 * S * V + S * (V >> 7) * 2 + 2);  // tensor-core K6: [2][S][V] class results + tile cache (tc_match.cu)
-  QB_ALLOC(h, h->colbest, S * V);
-  QB_ALLOC(h, h->mut_i, S * V);
-  QB_ALLOC(h, h->mut_j, S * V);
-  QB_ALLOC(h, h->mark, S * V);
-  QB_ALLOC(h, h->partner, S * V);
-  QB_ALLOC(h, h->mean, C * 4);
-  QB_ALLOC(h, h->corr_src, S * Lc);
-  QB_ALLOC(h, h->corr_tgt, S * Lc);
-  QB_ALLOC(h, h->ma, S * Lc);
-  QB_ALLOC(h, h->mb, S * Lc);
-  QB_ALLOC(h, h->adj, S * Lc * W);
-  QB_ALLOC(h, h->adjp, S * Lc * W);
-  QB_ALLOC(h, h->deg, S * Lc);
-  QB_ALLOC(h, h->kcore, S * (Lc + 2));
-  QB_ALLOC(h, h->korder, S * (Lc + 2));
-  QB_ALLOC(h, h->rank_of, S * (Lc + 2));
-  QB_ALLOC(h, h->by_rank, S * (Lc + 2));
-  QB_ALLOC(h, h->kbin, S * (Lc + 2));
-  QB_ALLOC(h, h->clique, S * Lc);
-  QB_ALLOC(h, h->final_inl, S * Lc);
-  QB_ALLOC(h, h->rot_mask, S * Lc);
-  QB_ALLOC(h, h->trans_mask, S * Lc);
-  QB_ALLOC(h, h->d_results, S);
-  QB_CUDA_TRY(h, cudaMemset(h->d_results, 0, S * sizeof(qb200_result)));
-  QB_CUDA_TRY(h, cudaMallocHost((void**)&h->h_results, S * sizeof(qb200_result)));
+  L->cub_bytes = sort_temp_bytes((int)(C * V));
+  QB_CUDA_TRY(L, cudaMalloc(&L->cub_temp, L->cub_bytes));
+  QB_ALLOC(L, L->vox_start, C * (V + 1));
+  QB_ALLOC(L, L->vox_pts, C * V);
+  QB_ALLOC(L, L->cell_key, C * V);
+  QB_ALLOC(L, L->cell_start, C * (V + 1));
+  QB_ALLOC(L, L->normals, C * V);
+  QB_ALLOC(L, L->spfh, C * V * kDescPad);
+  QB_ALLOC(L, L->nbr_list, C * kNbrGlobalCap * V);
+  QB_ALLOC(L, L->nbr_cnt, C * V);
+  QB_ALLOC(L, L->desc_t, C * kDescK * V);
+  QB_CUDA_TRY(L, cudaMemset(L->desc_t, 0, C * kDescK * V * sizeof(float)));
+  QB_ALLOC(L, L->desc_tiles, C * kDescK * V * 3);
+  QB_CUDA_TRY(L, cudaMemset(L->desc_tiles, 0, C * kDescK * V * 3 * sizeof(float)));
+  QB_ALLOC(L, L->desc_norm, C * V);
+  QB_ALLOC(L, L->tc_fallback, S);
+  QB_ALLOC(L, L->tc_stats, 32);
+  QB_CUDA_TRY(L, cudaMemset(L->tc_stats, 0, 32 * sizeof(unsigned long long)));
+  QB_ALLOC(L, L->rowbest, S * V);
+  QB_ALLOC(L, L->colpart, 2 * S * V + S * (V >> 7) * 2 + 2);  // tensor-core K6: [2][S][V] class results + tile cache (tc_match.cu)
+  QB_ALLOC(L, L->colbest, S * V);
+  QB_ALLOC(L, L->mut_i, S * V);
+  QB_ALLOC(L, L->mut_j, S * V);
+  QB_ALLOC(L, L->mark, S * V);
+  QB_ALLOC(L, L->partner, S * V);
+  QB_ALLOC(L, L->mean, C * 4);
+  QB_ALLOC(L, L->corr_src, S * Lc);
+  QB_ALLOC(L, L->corr_tgt, S * Lc);
+  QB_ALLOC(L, L->ma, S * Lc);
+  QB_ALLOC(L, L->mb, S * Lc);
+  QB_ALLOC(L, L->adj, S * Lc * W);
+  QB_ALLOC(L, L->adjp, S * Lc * W);
+  QB_ALLOC(L, L->deg, S * Lc);
+  QB_ALLOC(L, L->kcore, S * (Lc + 2));
+  QB_ALLOC(L, L->korder, S * (Lc + 2));
+  QB_ALLOC(L, L->rank_of, S * (Lc + 2));
+  QB_ALLOC(L, L->by_rank, S * (Lc + 2));
+  QB_ALLOC(L, L->kbin, S * (Lc + 2));
+  QB_ALLOC(L, L->clique, S * Lc);
+  QB_ALLOC(L, L->final_inl, S * Lc);
+  QB_ALLOC(L, L->rot_mask, S * Lc);
+  QB_ALLOC(L, L->trans_mask, S * Lc);
+  QB_ALLOC(L, L->d_results, S);
+  QB_CUDA_TRY(L, cudaMemset(L->d_results, 0, S * sizeof(qb200_result)));
+  QB_CUDA_TRY(L, cudaMallocHost((void**)&L->h_results, S * sizeof(qb200_result)));
   // counters: one int block so a wave reset is a single launch.  n_edges (long long) lives at an 8-byte offset.
   const size_t n_ints = C * 5 + C * 6 + S * 7 + 2 * S + 2;
-  QB_ALLOC(h, h->ctr_block, n_ints);
-  h->ctr_ints = n_ints;
-  int* p = h->ctr_block;
-  h->ctr.n_edges = reinterpret_cast<long long*>(p); p += 2 * S;
-  h->ctr.n_valid = p; p += C;
-  h->ctr.n_vox = p; p += C;
-  h->ctr.n_lat = p; p += C;
-  h->ctr.n_cells = p; p += C;
-  h->ctr.cloud_status = p; p += C;
-  h->ctr.bbox = p; p += C * 6;
-  h->ctr.n_mutual = p; p += S;
-  h->ctr.n_corr = p; p += S;
-  h->ctr.swapped = p; p += S;
-  h->ctr.n_clique = p; p += S;
-  h->ctr.max_core = p; p += S;
-  h->ctr.n_final = p; p += S;
-  h->ctr.flags = p; p += S;
-  for (int i = 0; i < 9; ++i) QB_CUDA_TRY(h, cudaEventCreate(&h->ev[i]));
-  for (int i = 0; i < 4; ++i) QB_CUDA_TRY(h, cudaEventCreate(&h->kev[i]));
+  QB_ALLOC(L, L->ctr_block, n_ints);
+  L->ctr_ints = n_ints;
+  int* p = L->ctr_block;
+  L->ctr.n_edges = reinterpret_cast<long long*>(p); p += 2 * S;
+  L->ctr.n_valid = p; p += C;
+  L->ctr.n_vox = p; p += C;
+  L->ctr.n_lat = p; p += C;
+  L->ctr.n_cells = p; p += C;
+  L->ctr.cloud_status = p; p += C;
+  L->ctr.bbox = p; p += C * 6;
+  L->ctr.n_mutual = p; p += S;
+  L->ctr.n_corr = p; p += S;
+  L->ctr.swapped = p; p += S;
+  L->ctr.n_clique = p; p += S;
+  L->ctr.max_core = p; p += S;
+  L->ctr.n_final = p; p += S;
+  L->ctr.flags = p; p += S;
+  for (int i = 0; i < 9; ++i) QB_CUDA_TRY(L, cudaEventCreate(&L->ev[i]));
+  for (int i = 0; i < 4; ++i) QB_CUDA_TRY(L, cudaEventCreate(&L->kev[i]));
+  QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
   return QB200_OK;
 }
 
-int wave_reset(qb200_handle* h, int n_clouds) {
-  const int n = (int)h->ctr_ints;
-  wave_init_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(h->ctr_block, n, h->ctr.bbox, n_clouds);
-  h->launches++;
-  QB_CUDA_TRY(h, cudaGetLastError());
+void lane_free(Lane* L) {
+  if (!L) return;
+  void* dev_ptrs[] = {(void*)L->d_cloud_ptr, L->d_cloud_n, L->d_raw_off, L->raw_stage, L->key_a, L->key_b, L->val_a, L->val_b, L->cub_temp,
+                      L->vox_start, L->vox_pts, L->cell_key, L->cell_start, L->normals, L->spfh, L->nbr_list, L->nbr_cnt, L->desc_t, L->rowbest, L->colpart, L->colbest,
+                      L->desc_tiles, L->desc_norm, L->tc_fallback, L->tc_stats, L->aos_scratch,
+                      L->mut_i, L->mut_j, L->mark, L->partner, L->mean, L->corr_src, L->corr_tgt, L->ma, L->mb, L->adj, L->adjp, L->deg,
+                      L->kcore, L->korder, L->rank_of, L->by_rank, L->kbin, L->clique, L->ex_stack, L->ex_pool, L->ex_lvl, L->ex_cur, L->pw_ints, L->pw_out, L->ip_buf, L->final_inl, L->rot_mask, L->trans_mask, L->d_results,
+                      L->ctr_block};
+  for (void* p : dev_ptrs)
+    if (p) cudaFree(p);
+  if (L->h_cloud_ptr) cudaFreeHost((void*)L->h_cloud_ptr);
+  if (L->h_cloud_n) cudaFreeHost(L->h_cloud_n);
+  if (L->h_raw_off) cudaFreeHost(L->h_raw_off);
+  if (L->h_results) cudaFreeHost(L->h_results);
+  for (int i = 0; i < 9; ++i)
+    if (L->ev[i]) cudaEventDestroy(L->ev[i]);
+  for (int i = 0; i < 4; ++i)
+    if (L->kev[i]) cudaEventDestroy(L->kev[i]);
+  if (L->own_stream) cudaStreamDestroy(L->own_stream);
+  delete L;
+}
+
+int wave_reset(Lane* L, int n_clouds) {
+  const int n = (int)L->ctr_ints;
+  wave_init_kernel<<<(n + 255) / 256, 256, 0, L->stream>>>(L->ctr_block, n, L->ctr.bbox, n_clouds);
+  L->launches++;
+  QB_CUDA_TRY(L, cudaGetLastError());
   return QB200_OK;
 }
 
-int set_counter(qb200_handle* h, int* dptr, int value) {
-  QB_CUDA_TRY(h, cudaMemcpyAsync(dptr, &value, sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // 'value' is a stack variable
+int set_counter(Lane* L, int* dptr, int value) {
+  QB_CUDA_TRY(L, cudaMemcpyAsync(dptr, &value, sizeof(int), cudaMemcpyHostToDevice, L->stream));
+  QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));  // 'value' is a stack variable
   return QB200_OK;
 }
 
-int get_counter(qb200_handle* h, const int* dptr, int* value) {
-  QB_CUDA_TRY(h, cudaMemcpyAsync(value, dptr, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+int get_counter(Lane* L, const int* dptr, int* value) {
+  QB_CUDA_TRY(L, cudaMemcpyAsync(value, dptr, sizeof(int), cudaMemcpyDeviceToHost, L->stream));
+  QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
   return QB200_OK;
 }
 
@@ -210,73 +239,347 @@ bool params_ok(const qb200_params* p) {
 // neighbour within +-1 even after the float rounding of x / cell, so the walk covers 27 cells instead of 125
 float lattice_cell(const qb200_params& p) { return p.grid_cell > 0 ? p.grid_cell : p.fpfh_radius * 1.001953125f; }
 
+// p with its rotation noise bound resolved.  The reference latches 2*noise_bound of the FIRST registration into a function-local
+// static (quatro.hpp:469-470 after :851); here the latch is a per-handle field, overridable via params.  Every lane gets the
+// resolved value, so a pair's GNC bound never depends on the wave / lane it lands on.
+qb200_params resolve_params(qb200_handle* h, const qb200_params& p) {
+  qb200_params r = p;
+  if (!(r.rot_noise_bound > 0)) {
+    if (h->rot_noise_bound_latched <= 0) h->rot_noise_bound_latched = 2.0 * p.noise_bound;
+    r.rot_noise_bound = h->rot_noise_bound_latched;
+  }
+  return r;
+}
+
+// what qb200_get_last_* read back after a single-pair registration or solve
+void set_last(qb200_handle* h, const qb200_result& r) {
+  h->last_n_corr = r.n_corr;
+  h->last_n_clique = r.clique_size;
+  h->last_n_final = r.n_final_inliers;
+}
+
+// stage and kernel times of a batch call start from zero
+void reset_timers(qb200_handle* h) {
+  memset(h->stage_ms, 0, sizeof(h->stage_ms));
+  memset(h->kernel_ms, 0, sizeof(h->kernel_ms));
+  memset(h->kernel_calls, 0, sizeof(h->kernel_calls));
+}
+
 // graph -> clique -> pose for pairs [0, n) whose matched points / n_corr are already on the device
-int run_solver(qb200_handle* h, int n_pairs, const qb200_params& p, int have_frontend) {
+int run_solver(Lane* L, int n_pairs, const qb200_params& p, int have_frontend) {
   int rc;
   if (p.inlier_selection_mode == QB200_INLIER_NONE) {
     // the reference leaves max_clique_ empty in this mode (quatro.hpp:782); TEASER++ semantics: all measurements
-    if ((rc = launch_iota_clique(h, n_pairs))) return rc;
+    if ((rc = launch_iota_clique(L, n_pairs))) return rc;
   } else {
-    if ((rc = launch_graph(h, n_pairs, p.noise_bound, p.cbar2))) return rc;
-    if (h->ev[5]) cudaEventRecord(h->ev[5], h->stream);
-    if ((rc = launch_clique(h, n_pairs, p.inlier_selection_mode, p.kcore_heuristic_threshold, p.max_clique_node_limit))) return rc;
+    if ((rc = launch_graph(L, n_pairs, p.noise_bound, p.cbar2))) return rc;
+    if (L->ev[5]) cudaEventRecord(L->ev[5], L->stream);
+    if ((rc = launch_clique(L, n_pairs, p.inlier_selection_mode, p.kcore_heuristic_threshold, p.max_clique_node_limit))) return rc;
   }
-  if (h->ev[6]) cudaEventRecord(h->ev[6], h->stream);
-  if ((rc = launch_fill_counters(h, n_pairs, have_frontend))) return rc;
-  if ((rc = launch_pose(h, n_pairs, p))) return rc;
-  if ((rc = launch_finalize_status(h, n_pairs))) return rc;
+  if (L->ev[6]) cudaEventRecord(L->ev[6], L->stream);
+  if ((rc = launch_fill_counters(L, n_pairs, have_frontend))) return rc;
+  if ((rc = launch_pose(L, n_pairs, p))) return rc;
+  if ((rc = launch_finalize_status(L, n_pairs))) return rc;
   return QB200_OK;
 }
 
-int upload_matched(qb200_handle* h, const float* a4, const float* b4, int L) {
-  if (L > h->Lc) {
-    h->fail(__FILE__, __LINE__, "L exceeds max_corr");
+int upload_matched(Lane* L, const float* a4, const float* b4, int n) {
+  if (n > L->Lc) {
+    L->fail(__FILE__, __LINE__, "L exceeds max_corr");
     return QB200_ERR_BAD_ARG;
   }
-  int rc = wave_reset(h, 2);
+  int rc = wave_reset(L, 2);
   if (rc) return rc;
-  if (L > 0) {
-    QB_CUDA_TRY(h, cudaMemcpyAsync(h->ma, a4, (size_t)L * sizeof(float4), cudaMemcpyHostToDevice, h->stream));
-    QB_CUDA_TRY(h, cudaMemcpyAsync(h->mb, b4, (size_t)L * sizeof(float4), cudaMemcpyHostToDevice, h->stream));
+  if (n > 0) {
+    QB_CUDA_TRY(L, cudaMemcpyAsync(L->ma, a4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
+    QB_CUDA_TRY(L, cudaMemcpyAsync(L->mb, b4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
   }
-  return set_counter(h, h->ctr.n_corr, L);
+  return set_counter(L, L->ctr.n_corr, n);
 }
 
-int upload_cloud_as_voxels(qb200_handle* h, int cloud, const float* pts4, int n) {
-  if (n > h->V) {
-    h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points");
+int upload_cloud_as_voxels(Lane* L, int cloud, const float* pts4, int n) {
+  if (n > L->V) {
+    L->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points");
     return QB200_ERR_BAD_ARG;
   }
-  if (n > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(h->vox_pts + (size_t)cloud * h->V, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, h->stream));
-  return set_counter(h, h->ctr.n_vox + cloud, n);
+  if (n > 0) QB_CUDA_TRY(L, cudaMemcpyAsync(L->vox_pts + (size_t)cloud * L->V, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
+  return set_counter(L, L->ctr.n_vox + cloud, n);
 }
 
+// the record of a single-pair solve on lane 0
 int fetch_result(qb200_handle* h, qb200_result* res) {
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->h_results, h->d_results, sizeof(qb200_result), cudaMemcpyDeviceToHost, h->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  *res = h->h_results[0];
-  h->last_n_corr = res->n_corr;
-  h->last_n_clique = res->clique_size;
-  h->last_n_final = res->n_final_inliers;
+  Lane* L = h->lane[0];
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
+  QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
+  *res = L->h_results[0];
+  set_last(h, *res);
   return res->status;
 }
 
-}  // namespace
-
-// entry points that use the handle's wave buffers first collect whatever qb200_register_batch_enqueue left in flight
-#define QB_IDLE(h)                                        \
-  do {                                                    \
-    if ((h) && (h)->lanes_active) {                       \
-      const int rc_idle_ = batch_flush(h);                \
-      if (rc_idle_) return rc_idle_;                      \
-    }                                                     \
-  } while (0)
-
-extern "C" {
-static int batch_flush(qb200_handle* h);
-static void cache_free(qb200_handle* h);
+// the first min(n, cap) correspondences of pair 0: index pairs (src, tgt) and matched points, any of them may be NULL
+int download_corr(Lane* L, int n, int32_t* corr, float* sm4, float* tm4, int cap) {
+  const int m = n < cap ? n : cap;
+  if (m > 0) {
+    std::vector<int> s(m), t(m);
+    QB_CUDA_TRY(L, cudaMemcpyAsync(s.data(), L->corr_src, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
+    QB_CUDA_TRY(L, cudaMemcpyAsync(t.data(), L->corr_tgt, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
+    if (sm4) QB_CUDA_TRY(L, cudaMemcpyAsync(sm4, L->ma, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
+    if (tm4) QB_CUDA_TRY(L, cudaMemcpyAsync(tm4, L->mb, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
+    QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
+    if (corr)
+      for (int i = 0; i < m; ++i) { corr[2 * i] = s[i]; corr[2 * i + 1] = t[i]; }
+  }
+  return n > cap ? QB200_CAPACITY_EXCEEDED : QB200_OK;
 }
-static void cache_free_public(qb200_handle* h) { cache_free(h); }
+
+// Stage the raw clouds [0, ncl) of a wave whose caller pointers and point counts are in L->h_cloud_ptr / h_cloud_n, then copy the
+// cloud tables; every copy goes on stream cs.  Device clouds are read in place.  Host clouds go to raw_stage; clouds that lie back
+// to back in the caller's memory (one big pinned buffer is the usual case) cross PCIe as one copy: far fewer DMA descriptors than
+// one per cloud.
+int stage_raw(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs) {
+  int total = 0, run_dst = 0, run_n = 0, rc;
+  const float4* run_src = nullptr;
+  auto flush_run = [&]() -> int {
+    if (run_n > 0)
+      QB_CUDA_TRY(L, cudaMemcpyAsync(L->raw_stage + run_dst, run_src, (size_t)run_n * sizeof(float4), cudaMemcpyHostToDevice, cs));
+    run_n = 0;
+    return QB200_OK;
+  };
+  for (int c = 0; c < ncl; ++c) {
+    const float4* src = L->h_cloud_ptr[c];
+    const int n = L->h_cloud_n[c];
+    L->h_raw_off[c] = total;
+    if (kind == QB200_MEM_HOST) {
+      L->h_cloud_ptr[c] = L->raw_stage + total;
+      if (n > 0) {
+        if (run_n > 0 && src == run_src + run_n && run_n < (1 << 26)) {
+          run_n += n;
+        } else {
+          if ((rc = flush_run())) return rc;
+          run_src = src; run_dst = total; run_n = n;
+        }
+      }
+    }
+    total += n;
+  }
+  if ((rc = flush_run())) return rc;
+  L->h_raw_off[ncl] = total;
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_cloud_ptr, L->h_cloud_ptr, (size_t)ncl * sizeof(float4*), cudaMemcpyHostToDevice, cs));
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_cloud_n, L->h_cloud_n, (size_t)ncl * sizeof(int), cudaMemcpyHostToDevice, cs));
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_raw_off, L->h_raw_off, (size_t)(ncl + 1) * sizeof(int), cudaMemcpyHostToDevice, cs));
+  return QB200_OK;
+}
+
+// ---- scan cache ---------------------------------------------------------------------------------------------------------
+// FPFHManager keeps the last target's descriptors and reuses them as the next source (odometry mode, fpfh_manager.hpp:74-77,
+// 111-118); a loop-closure sweep matches one scan against many.  The cache keeps voxel points, normals and FPFH-33 of a scan
+// resident on the device so that the front end (voxel + normals + FPFH, ~45 % of a wave) runs once per SCAN, not once per pair.
+void cache_free(qb200_handle* h) {
+  if (h->c_vox) cudaFree(h->c_vox);
+  if (h->c_nrm) cudaFree(h->c_nrm);
+  if (h->c_desc) cudaFree(h->c_desc);
+  if (h->c_n) cudaFree(h->c_n);
+  if (h->c_status) cudaFree(h->c_status);
+  if (h->d_slot_of_cloud) cudaFree(h->d_slot_of_cloud);
+  if (h->h_slot_of_cloud) cudaFreeHost(h->h_slot_of_cloud);
+  delete[] h->c_sig;
+  h->c_vox = h->c_nrm = nullptr; h->c_desc = nullptr; h->c_n = h->c_status = h->d_slot_of_cloud = h->h_slot_of_cloud = nullptr;
+  h->c_sig = nullptr;
+  h->c_slots = 0;
+}
+
+// clouds [0, n_clouds) of lane L's wave to (to_cache = 1) or from their cache slots h->h_slot_of_cloud[]
+int cache_copy(qb200_handle* h, Lane* L, int to_cache, int n_clouds) {
+  QB_CUDA_TRY(L, cudaMemcpyAsync(h->d_slot_of_cloud, h->h_slot_of_cloud, (size_t)n_clouds * sizeof(int), cudaMemcpyHostToDevice, L->stream));
+  const dim3 g((L->V + 255) / 256, 43, n_clouds);
+  cache_copy_kernel<<<g, 256, 0, L->stream>>>(to_cache, h->d_slot_of_cloud, L->V, L->vox_pts, L->normals, L->desc_t, L->ctr.n_vox, L->ctr.cloud_status,
+                                              h->c_vox, h->c_nrm, h->c_desc, h->c_n, h->c_status);
+  L->launches++;
+  QB_CUDA_TRY(L, cudaGetLastError());
+  return QB200_OK;
+}
+
+// ---- waves ----------------------------------------------------------------------------------------------------------------
+// What a wave starts from: pairs of raw scans (in `kind` memory), pairs of cached scans, or correspondence sets (in `kind`
+// memory).  Exactly one of the three is set.
+struct WaveInput {
+  const qb200_pair* pairs = nullptr;
+  const qb200_slot_pair* slots = nullptr;
+  const qb200_corr_set* sets = nullptr;
+  qb200_mem_kind kind = QB200_MEM_HOST;
+  // raw host scans of a multi-wave batch: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies queued on
+  // several streams share the PCIe link, so every wave's scans would arrive late; on one stream they arrive wave after wave and
+  // the first waves compute while the later ones are still crossing.
+  cudaStream_t copy_stream = nullptr;
+};
+
+// Enqueue one wave (pairs [w0, w0 + np), np <= S) on lane L: the front of the wave its input needs (raw scans: H2D, K1..K6;
+// cached scans: the copy out of the cache, K6; correspondence sets: their H2D), then K8..K11 and the D2H of the result records.
+// No sync: wave_collect hands the records out to dst[w0...].  The lane's previous wave must have been collected.
+int wave_submit(qb200_handle* h, Lane* L, const WaveInput& in, int w0, int np, const qb200_params& p, qb200_result* dst) {
+  const int ncl = 2 * np;
+  int rc;
+  L->kev_armed[0] = L->kev_armed[1] = 0;
+  if (in.pairs) {
+    cudaEventRecord(L->ev[0], L->stream);
+    for (int s = 0; s < np; ++s) {
+      const qb200_pair& pr = in.pairs[w0 + s];
+      L->h_cloud_ptr[2 * s] = reinterpret_cast<const float4*>(pr.src);
+      L->h_cloud_ptr[2 * s + 1] = reinterpret_cast<const float4*>(pr.tgt);
+      L->h_cloud_n[2 * s] = pr.n_src;
+      L->h_cloud_n[2 * s + 1] = pr.n_tgt;
+    }
+    if ((rc = stage_raw(L, ncl, in.kind, in.copy_stream ? in.copy_stream : L->stream))) return rc;
+    if ((rc = wave_reset(L, ncl))) return rc;
+    if (in.copy_stream) {
+      QB_CUDA_TRY(L, cudaEventRecord(h->ev_copied, in.copy_stream));
+      QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, h->ev_copied, 0));
+    }
+    cudaEventRecord(L->ev[1], L->stream);
+    if ((rc = launch_voxel(L, ncl, p.voxel_size, p.skip_flagged))) return rc;
+    cudaEventRecord(L->ev[2], L->stream);
+    if ((rc = launch_fpfh(L, ncl, p.normal_radius, p.fpfh_radius, lattice_cell(p)))) return rc;
+    cudaEventRecord(L->ev[3], L->stream);
+  } else if (in.slots) {
+    for (int s = 0; s < np; ++s) {
+      h->h_slot_of_cloud[2 * s] = in.slots[w0 + s].src_slot;
+      h->h_slot_of_cloud[2 * s + 1] = in.slots[w0 + s].tgt_slot;
+    }
+    if ((rc = wave_reset(L, ncl))) return rc;
+    cudaEventRecord(L->ev[2], L->stream);
+    if ((rc = cache_copy(h, L, 0, ncl))) return rc;
+    cudaEventRecord(L->ev[3], L->stream);
+  } else {
+    if ((rc = wave_reset(L, ncl))) return rc;
+    const cudaMemcpyKind ck = in.kind == QB200_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+    for (int s = 0; s < np; ++s) {
+      const qb200_corr_set& cs = in.sets[w0 + s];
+      L->h_cloud_n[s] = cs.L;
+      if (cs.L > 0) {
+        QB_CUDA_TRY(L, cudaMemcpyAsync(L->ma + (size_t)s * L->Lc, cs.a, (size_t)cs.L * sizeof(float4), ck, L->stream));
+        QB_CUDA_TRY(L, cudaMemcpyAsync(L->mb + (size_t)s * L->Lc, cs.b, (size_t)cs.L * sizeof(float4), ck, L->stream));
+      }
+    }
+    QB_CUDA_TRY(L, cudaMemcpyAsync(L->ctr.n_corr, L->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, L->stream));
+  }
+  if (!in.sets && (rc = launch_match(L, np, p))) return rc;
+  cudaEventRecord(L->ev[4], L->stream);
+  cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
+  if ((rc = run_solver(L, np, p, in.sets ? 0 : 1))) return rc;
+  cudaEventRecord(L->ev[7], L->stream);
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
+  cudaEventRecord(L->ev[8], L->stream);
+  L->pend_w0 = w0;
+  L->pend_np = np;
+  L->pend_dst = dst;
+  // stage-time slots of qb200_get_stage_ms this wave reports: raw scans all eight, the other inputs their first stage to pose
+  L->pend_t0 = in.pairs ? 0 : in.slots ? 2 : 4;
+  L->pend_t1 = in.pairs ? 8 : 7;
+  return QB200_OK;
+}
+
+// wait for the wave in flight on lane L, hand out its records and add its stage / kernel times to the handle
+int wave_collect(qb200_handle* h, Lane* L) {
+  if (L->pend_np == 0) return QB200_OK;
+  const int np = L->pend_np;
+  L->pend_np = 0;
+  if (cudaStreamSynchronize(L->stream) != cudaSuccess) {
+    h->fail(__FILE__, __LINE__, cudaGetErrorString(cudaGetLastError()));
+    return QB200_ERR_CUDA;
+  }
+  memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
+  static const int timeline = (getenv("QB200_TIMELINE") && getenv("QB200_TIMELINE")[0] == '1') ? 1 : 0;
+  if (timeline && L->pend_t0 == 0) {  // stage boundaries of a raw-scan wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
+    fprintf(stderr, "[qb200 timeline] wave w0=%d np=%d:", L->pend_w0, np);
+    for (int i = 0; i < 9; ++i) {
+      float ms = -1.f;
+      cudaEventElapsedTime(&ms, h->ev_fork, L->ev[i]);
+      fprintf(stderr, " %.2f", ms);
+    }
+    fprintf(stderr, "\n");
+  }
+  for (int i = L->pend_t0; i < L->pend_t1; ++i) {
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, L->ev[i], L->ev[i + 1]) == cudaSuccess) h->stage_ms[i] += ms;
+  }
+  for (int k = 0; k < 2; ++k) {
+    float ms = 0.f;
+    if (L->kev_armed[k] && cudaEventElapsedTime(&ms, L->kev[2 * k], L->kev[2 * k + 1]) == cudaSuccess) {
+      h->kernel_ms[k] += ms;
+      h->kernel_calls[k] += 1;
+    }
+    L->kev_armed[k] = 0;
+  }
+  return QB200_OK;
+}
+
+// wait for the waves in flight (oldest first) whose records go to dst, or for all of them (dst == nullptr), and hand out their records
+int collect_waves(qb200_handle* h, const qb200_result* dst) {
+  int rc = QB200_OK;
+  const int n = h->lanes_active > 0 ? h->lanes_active : 1;
+  for (int i = 0; i < n; ++i) {
+    Lane* L = h->lane[(h->lane_cursor + i) % n];
+    if (!L || (dst && L->pend_dst != dst)) continue;
+    const int rc2 = wave_collect(h, L);
+    if (rc == QB200_OK) rc = rc2;
+  }
+  return rc;
+}
+
+int batch_flush(qb200_handle* h) {
+  const int rc = collect_waves(h, nullptr);
+  h->lanes_active = 0;
+  h->lane_cursor = 0;
+  return rc;
+}
+
+// one wave at a time on lane 0, each collected before the next is submitted
+int run_waves(qb200_handle* h, const WaveInput& in, int n, const qb200_params& p, qb200_result* results) {
+  reset_timers(h);
+  const int S = h->cfg.max_batch_slots;
+  for (int w0 = 0; w0 < n; w0 += S) {
+    int rc = wave_submit(h, h->lane[0], in, w0, n - w0 < S ? n - w0 : S, p, results);
+    if (rc == QB200_OK) rc = wave_collect(h, h->lane[0]);
+    if (rc) return rc;
+  }
+  if (n == 1) set_last(h, results[0]);
+  return QB200_OK;
+}
+
+// Prologue of every entry point that uses lane 0's buffers or stream: a handle, its device current, and no wave of
+// qb200_register_batch_enqueue in flight any more (their records are completed first).
+int enter(qb200_handle* h) {
+  if (!h) return QB200_ERR_BAD_ARG;
+  cudaSetDevice(h->cfg.device);
+  return h->lanes_active ? batch_flush(h) : QB200_OK;
+}
+
+// tc_stats[first, first + n) summed over the lanes (then zeroed on every lane if reset)
+int read_tc_stats(qb200_handle* h, int first, int n, uint64_t* out, int reset) {
+  for (int i = 0; i < n; ++i) out[i] = 0;
+  for (Lane* L : h->lane) {
+    if (!L) continue;
+    uint64_t o[32];
+    QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
+    QB_CUDA_TRY(L, cudaMemcpy(o, L->tc_stats + first, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    if (reset) QB_CUDA_TRY(L, cudaMemset(L->tc_stats + first, 0, n * sizeof(unsigned long long)));
+    for (int i = 0; i < n; ++i) out[i] += o[i];
+  }
+  return QB200_OK;
+}
+
+int copy_ints(Lane* L, const int* dsrc, int n_have, int32_t* dst, int32_t cap, int32_t* n) {
+  if (!n || cap < 0) return QB200_ERR_BAD_ARG;
+  *n = n_have;
+  const int m = n_have < cap ? n_have : cap;
+  if (m > 0 && dst) {
+    QB_CUDA_TRY(L, cudaMemcpyAsync(dst, dsrc, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
+    QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
+  }
+  return n_have > cap ? QB200_CAPACITY_EXCEEDED : QB200_OK;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -312,98 +615,84 @@ int qb200_create(const qb200_config* cfg_in, qb200_handle** out) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || cfg.device < 0 || cfg.device >= ndev) return QB200_ERR_NO_DEVICE;
   if (cudaSetDevice(cfg.device) != cudaSuccess) return QB200_ERR_NO_DEVICE;
-  qb200_handle* h = new (std::nothrow) qb200_handle();
-  if (!h) return QB200_ERR_CUDA;
-  memset(h, 0, sizeof(*h));
-  h->cfg = cfg; h->device = cfg.device;
-  h->S = cfg.max_batch_slots; h->R = cfg.max_raw_points; h->V = cfg.max_voxel_points; h->Lc = cfg.max_corr;
-  h->W = h->Lc / 32; h->NS = h->V / kMatchTile;
-  if (cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, cfg.device) != cudaSuccess || h->n_sm <= 0) { delete h; return QB200_ERR_NO_DEVICE; }
+  Lane like{};  // the settings every lane of the handle shares
+  like.S = cfg.max_batch_slots; like.R = cfg.max_raw_points; like.V = cfg.max_voxel_points; like.Lc = cfg.max_corr;
+  like.W = like.Lc / 32; like.NS = like.V / kMatchTile;
+  like.device = cfg.device;
+  if (cudaDeviceGetAttribute(&like.n_sm, cudaDevAttrMultiProcessorCount, cfg.device) != cudaSuccess || like.n_sm <= 0) return QB200_ERR_NO_DEVICE;
   // K6 implementation switch: the tensor-core filter + in-kernel exact evaluation is the default; QB200_MATCH_EXACT=1 forces
   // the exact CUDA-core kernel everywhere (identical results; A/B and triage)
   const char* fe = getenv("QB200_MATCH_EXACT");
-  h->force_exact_match = (fe && fe[0] == '1') ? 1 : 0;
+  like.force_exact_match = (fe && fe[0] == '1') ? 1 : 0;
+  qb200_handle* h = new (std::nothrow) qb200_handle();
+  if (!h) return QB200_ERR_CUDA;
+  h->cfg = cfg;
   const char* ln = getenv("QB200_LANES");
   h->max_lanes = (ln && ln[0] >= '1' && ln[0] <= '8') ? ln[0] - '0' : 4;
-  if (cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess) { delete h; return QB200_ERR_CUDA; }
-  h->stream = h->own_stream;
-  const int rc = alloc_all(h);
+  like.err = h->err;
+  auto alloc = [&]() -> int {
+    QB_CUDA_TRY(h, cudaEventCreate(&h->ev_fork));  // (timing enabled: QB200_TIMELINE measures the waves against it)
+    QB_CUDA_TRY(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
+    QB_CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_copied, cudaEventDisableTiming));
+    return lane_alloc(like, &h->lane[0]);
+  };
+  const int rc = alloc();
   if (rc != QB200_OK) {
     fprintf(stderr, "qb200_create: %s\n", h->err);
     qb200_destroy(h);
     return rc;
   }
-  cudaStreamSynchronize(h->stream);
   *out = h;
   return QB200_OK;
 }
 
 void qb200_destroy(qb200_handle* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
+  cudaSetDevice(h->cfg.device);
   cudaDeviceSynchronize();
   comm_release(h);
-  cache_free_public(h);
-  void* dev_ptrs[] = {(void*)h->d_cloud_ptr, h->d_cloud_n, h->d_raw_off, h->raw_stage, h->key_a, h->key_b, h->val_a, h->val_b, h->cub_temp,
-                      h->vox_start, h->vox_pts, h->cell_key, h->cell_start, h->normals, h->spfh, h->nbr_list, h->nbr_cnt, h->desc_t, h->rowbest, h->colpart, h->colbest,
-                      h->desc_tiles, h->desc_norm, h->tc_fallback, h->tc_stats, h->aos_scratch,
-                      h->mut_i, h->mut_j, h->mark, h->partner, h->mean, h->corr_src, h->corr_tgt, h->ma, h->mb, h->adj, h->adjp, h->deg,
-                      h->kcore, h->korder, h->rank_of, h->by_rank, h->kbin, h->clique, h->ex_stack, h->ex_pool, h->ex_lvl, h->ex_cur, h->pw_ints, h->pw_out, h->ip_buf, h->final_inl, h->rot_mask, h->trans_mask, h->d_results,
-                      h->ctr_block};
-  for (void* p : dev_ptrs)
-    if (p) cudaFree(p);
-  if (h->h_cloud_ptr) cudaFreeHost((void*)h->h_cloud_ptr);
-  if (h->h_cloud_n) cudaFreeHost(h->h_cloud_n);
-  if (h->h_raw_off) cudaFreeHost(h->h_raw_off);
-  if (h->h_results) cudaFreeHost(h->h_results);
-  for (int i = 0; i < 9; ++i)
-    if (h->ev[i]) cudaEventDestroy(h->ev[i]);
-  for (int i = 0; i < 4; ++i)
-    if (h->kev[i]) cudaEventDestroy(h->kev[i]);
+  cache_free(h);
+  for (Lane* L : h->lane) lane_free(L);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   if (h->ev_copied) cudaEventDestroy(h->ev_copied);
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-  for (int i = 0; i < 7; ++i)
-    if (h->lane[i]) qb200_destroy(h->lane[i]);
-  if (h->own_stream) cudaStreamDestroy(h->own_stream);
   delete h;
 }
 
 int qb200_set_stream(qb200_handle* h, void* cuda_stream) {
-  if (!h) return QB200_ERR_BAD_ARG;
-  h->stream = cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream;
+  if (int rc = enter(h)) return rc;
+  Lane* L = h->lane[0];
+  L->stream = cuda_stream ? (cudaStream_t)cuda_stream : L->own_stream;
   return QB200_OK;
 }
 
 const char* qb200_last_error(const qb200_handle* h) { return h ? h->err : "null handle"; }
 int64_t qb200_launch_count(const qb200_handle* h) {
   if (!h) return 0;
-  int64_t n = h->launches;
-  for (int i = 0; i < 7; ++i)
-    if (h->lane[i]) n += h->lane[i]->launches;
+  int64_t n = 0;
+  for (const Lane* L : h->lane)
+    if (L) n += L->launches;
   return n;
 }
 
 // ---- stage: voxelize ----------------------------------------------------------------------------
 int qb200_voxelize(qb200_handle* h, const float* pts4, int32_t n, float leaf, int32_t skip_flagged, float* out4, int32_t cap,
                    int32_t* n_out) {
-  QB_IDLE(h);
-  if (!h || !n_out || n < 0 || (n > 0 && !pts4) || !(leaf > 0) || cap < 0 || (cap > 0 && !out4)) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (!n_out || n < 0 || (n > 0 && !pts4) || !(leaf > 0) || cap < 0 || (cap > 0 && !out4)) return QB200_ERR_BAD_ARG;
   *n_out = 0;
-  if (n > h->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
-  cudaSetDevice(h->device);
+  Lane* L = h->lane[0];
+  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
   if (n == 0) return QB200_OK;
-  int rc = wave_reset(h, 1);
+  int rc = wave_reset(L, 1);
   if (rc) return rc;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->raw_stage, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, h->stream));
-  h->h_cloud_ptr[0] = h->raw_stage; h->h_cloud_n[0] = n; h->h_raw_off[0] = 0; h->h_raw_off[1] = n;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_cloud_ptr, h->h_cloud_ptr, sizeof(float4*), cudaMemcpyHostToDevice, h->stream));
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_cloud_n, h->h_cloud_n, sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_raw_off, h->h_raw_off, 2 * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  if ((rc = launch_voxel(h, 1, leaf, skip_flagged))) return rc;
+  L->h_cloud_ptr[0] = reinterpret_cast<const float4*>(pts4);
+  L->h_cloud_n[0] = n;
+  if ((rc = stage_raw(L, 1, QB200_MEM_HOST, L->stream))) return rc;
+  if ((rc = launch_voxel(L, 1, leaf, skip_flagged))) return rc;
   int nv = 0, st = 0;
-  if ((rc = get_counter(h, h->ctr.n_vox, &nv))) return rc;
-  if ((rc = get_counter(h, h->ctr.cloud_status, &st))) return rc;
+  if ((rc = get_counter(L, L->ctr.n_vox, &nv))) return rc;
+  if ((rc = get_counter(L, L->ctr.cloud_status, &st))) return rc;
   if (st == QB200_ERR_VOXEL_OVERFLOW) {
     // [EXT] pcl::VoxelGrid: "leaf size is too small ... integer indices would overflow" -> output = input
     int m = 0;
@@ -419,8 +708,8 @@ int qb200_voxelize(qb200_handle* h, const float* pts4, int32_t n, float leaf, in
   *n_out = nv;
   const int m = nv < cap ? nv : cap;
   if (m > 0) {
-    QB_CUDA_TRY(h, cudaMemcpyAsync(out4, h->vox_pts, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    QB_CUDA_TRY(h, cudaMemcpyAsync(out4, L->vox_pts, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
+    QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   }
   if (st == QB200_CAPACITY_EXCEEDED || nv > cap) return QB200_CAPACITY_EXCEEDED;
   return QB200_OK;
@@ -429,156 +718,147 @@ int qb200_voxelize(qb200_handle* h, const float* pts4, int32_t n, float leaf, in
 // ---- pre-processing: ground removal (patchwork.hpp:329-455) ---------------------------------------------
 int qb200_patchwork(qb200_handle* h, const float* pts4, int32_t n, const qb200_patchwork_params* p, float* ground4, int32_t* n_ground,
                     float* nonground4, int32_t* n_nonground) {
-  QB_IDLE(h);
-  if (!h || !p || !n_ground || !n_nonground || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (!p || !n_ground || !n_nonground || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
   *n_ground = *n_nonground = 0;
-  if (n > h->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
-  cudaSetDevice(h->device);
-  if (n > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(h->raw_stage, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, h->stream));
+  Lane* L = h->lane[0];
+  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
+  if (n > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(L->raw_stage, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
   int ng = 0, nn = 0, st = 0;
-  const int rc = launch_patchwork(h, h->raw_stage, n, *p, &ng, &nn, &st);
+  const int rc = launch_patchwork(L, L->raw_stage, n, *p, &ng, &nn, &st);
   if (rc) return rc;
   *n_ground = ng;
   *n_nonground = nn;
-  if (ground4 && ng > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ground4, h->pw_out, (size_t)ng * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
+  if (ground4 && ng > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ground4, L->pw_out, (size_t)ng * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
   if (nonground4 && nn > 0)
-    QB_CUDA_TRY(h, cudaMemcpyAsync(nonground4, h->pw_out + h->R, (size_t)nn * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    QB_CUDA_TRY(h, cudaMemcpyAsync(nonground4, L->pw_out + L->R, (size_t)nn * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
+  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   return st;
 }
 
 // ---- pre-processing: range-image sub-cluster removal (imageProjection.hpp:273-294) ------------------------
 int qb200_segment_cloud(qb200_handle* h, const float* pts4, int32_t n, const qb200_segment_params* p, float* valid4, int32_t* n_valid,
                         float* outlier4, int32_t* n_outlier) {
-  QB_IDLE(h);
-  if (!h || !p || !n_valid || !n_outlier || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (!p || !n_valid || !n_outlier || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
   *n_valid = *n_outlier = 0;
-  if (n > h->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
-  cudaSetDevice(h->device);
-  if (n > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(h->raw_stage, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, h->stream));
+  Lane* L = h->lane[0];
+  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
+  if (n > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(L->raw_stage, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
   int nv = 0, no = 0;
   const float4 *dv = nullptr, *dout = nullptr;
-  const int rc = launch_segment_cloud(h, h->raw_stage, n, *p, &nv, &no, &dv, &dout);
+  const int rc = launch_segment_cloud(L, L->raw_stage, n, *p, &nv, &no, &dv, &dout);
   if (rc) return rc;
   *n_valid = nv;
   *n_outlier = no;
-  if (valid4 && nv > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(valid4, dv, (size_t)nv * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-  if (outlier4 && no > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(outlier4, dout, (size_t)no * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (valid4 && nv > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(valid4, dv, (size_t)nv * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
+  if (outlier4 && no > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(outlier4, dout, (size_t)no * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
+  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   return QB200_OK;
 }
 
 // ---- stage: normals + FPFH ------------------------------------------------------------------------
 int qb200_compute_fpfh(qb200_handle* h, const float* pts4, int32_t n, float normal_radius, float fpfh_radius, float grid_cell,
                        float* normals4, float* desc33) {
-  QB_IDLE(h);
-  if (!h || n < 0 || (n > 0 && !pts4) || !(normal_radius > 0) || !(fpfh_radius > 0) || !(grid_cell > 0)) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (n < 0 || (n > 0 && !pts4) || !(normal_radius > 0) || !(fpfh_radius > 0) || !(grid_cell > 0)) return QB200_ERR_BAD_ARG;
   if (normal_radius > fpfh_radius) return QB200_ERR_BAD_ARG;  // fpfh_manager.hpp:99-102
-  cudaSetDevice(h->device);
   if (n == 0) return QB200_OK;
-  int rc = wave_reset(h, 1);
+  Lane* L = h->lane[0];
+  int rc = wave_reset(L, 1);
   if (rc) return rc;
-  if ((rc = upload_cloud_as_voxels(h, 0, pts4, n))) return rc;
-  if ((rc = launch_fpfh(h, 1, normal_radius, fpfh_radius, grid_cell))) return rc;
-  if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, h->normals, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
+  if ((rc = upload_cloud_as_voxels(L, 0, pts4, n))) return rc;
+  if ((rc = launch_fpfh(L, 1, normal_radius, fpfh_radius, grid_cell))) return rc;
+  if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, L->normals, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
   if (desc33) {
-    float* scratch = h->aos_scratch;
-    if ((rc = launch_desc_to_aos(h, 0, n, scratch))) return rc;
-    QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, scratch, (size_t)n * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    float* scratch = L->aos_scratch;
+    if ((rc = launch_desc_to_aos(L, 0, n, scratch))) return rc;
+    QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, scratch, (size_t)n * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
   }
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   return QB200_OK;
 }
 
 // ---- stage: matching ------------------------------------------------------------------------------
-static int download_corr(qb200_handle* h, int32_t* corr, float* sm4, float* tm4, int cap, int32_t* n_corr, int32_t* n_mutual) {
+// the correspondences launch_match left for pair 0: counts, then the first cap of them
+static int match_result(qb200_handle* h, int32_t* corr, float* sm4, float* tm4, int cap, int32_t* n_corr, int32_t* n_mutual) {
+  Lane* L = h->lane[0];
   int nc = 0, nm = 0, st = 0, rc;
-  if ((rc = get_counter(h, h->ctr.n_corr, &nc))) return rc;
-  if ((rc = get_counter(h, h->ctr.n_mutual, &nm))) return rc;
-  if ((rc = get_counter(h, h->ctr.cloud_status, &st))) return rc;
+  if ((rc = get_counter(L, L->ctr.n_corr, &nc))) return rc;
+  if ((rc = get_counter(L, L->ctr.n_mutual, &nm))) return rc;
+  if ((rc = get_counter(L, L->ctr.cloud_status, &st))) return rc;
   *n_corr = nc;
   if (n_mutual) *n_mutual = nm;
   h->last_n_corr = nc;
-  const int m = nc < cap ? nc : cap;
-  if (m > 0) {
-    std::vector<int> s(m), t(m);
-    QB_CUDA_TRY(h, cudaMemcpyAsync(s.data(), h->corr_src, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    QB_CUDA_TRY(h, cudaMemcpyAsync(t.data(), h->corr_tgt, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    if (sm4) QB_CUDA_TRY(h, cudaMemcpyAsync(sm4, h->ma, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    if (tm4) QB_CUDA_TRY(h, cudaMemcpyAsync(tm4, h->mb, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    if (corr)
-      for (int i = 0; i < m; ++i) { corr[2 * i] = s[i]; corr[2 * i + 1] = t[i]; }
-  }
-  if (st == QB200_CAPACITY_EXCEEDED || nc > cap) return QB200_CAPACITY_EXCEEDED;
-  return QB200_OK;
+  if ((rc = download_corr(L, nc, corr, sm4, tm4, cap))) return rc;
+  return st == QB200_CAPACITY_EXCEEDED ? QB200_CAPACITY_EXCEEDED : QB200_OK;
 }
 
 int qb200_match(qb200_handle* h, const float* src4, int32_t n_src, const float* src_desc33, const float* tgt4, int32_t n_tgt,
                 const float* tgt_desc33, const qb200_params* p, int32_t* corr, int32_t cap, int32_t* n_corr, int32_t* n_mutual) {
-  QB_IDLE(h);
-  if (!h || !p || !n_corr || n_src < 0 || n_tgt < 0 || cap < 0) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (!p || !n_corr || n_src < 0 || n_tgt < 0 || cap < 0) return QB200_ERR_BAD_ARG;
   if ((n_src > 0 && (!src4 || !src_desc33)) || (n_tgt > 0 && (!tgt4 || !tgt_desc33))) return QB200_ERR_BAD_ARG;
   if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
   *n_corr = 0;
   if (n_mutual) *n_mutual = 0;
-  if (n_src > h->V || n_tgt > h->V) { h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points"); return QB200_ERR_BAD_ARG; }
-  cudaSetDevice(h->device);
+  Lane* L = h->lane[0];
+  if (n_src > L->V || n_tgt > L->V) { h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points"); return QB200_ERR_BAD_ARG; }
   h->last_match_n[0] = h->last_match_n[1] = 0;
   if (n_src == 0 || n_tgt == 0) return QB200_OK;
-  int rc = wave_reset(h, 2);
+  int rc = wave_reset(L, 2);
   if (rc) return rc;
-  if ((rc = upload_cloud_as_voxels(h, 0, src4, n_src))) return rc;
-  if ((rc = upload_cloud_as_voxels(h, 1, tgt4, n_tgt))) return rc;
+  if ((rc = upload_cloud_as_voxels(L, 0, src4, n_src))) return rc;
+  if ((rc = upload_cloud_as_voxels(L, 1, tgt4, n_tgt))) return rc;
   h->last_match_n[0] = n_src;
   h->last_match_n[1] = n_tgt;
-  float* scratch = h->aos_scratch;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch, src_desc33, (size_t)n_src * kDescDim * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  if ((rc = launch_desc_from_aos(h, 0, n_src, scratch))) return rc;
-  float* scratch2 = scratch + (size_t)h->V * kDescDim;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch2, tgt_desc33, (size_t)n_tgt * kDescDim * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  if ((rc = launch_desc_from_aos(h, 1, n_tgt, scratch2))) return rc;
-  if ((rc = launch_match(h, 1, *p))) return rc;
-  return download_corr(h, corr, nullptr, nullptr, cap, n_corr, n_mutual);
+  float* scratch = L->aos_scratch;
+  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch, src_desc33, (size_t)n_src * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
+  if ((rc = launch_desc_from_aos(L, 0, n_src, scratch))) return rc;
+  float* scratch2 = scratch + (size_t)L->V * kDescDim;
+  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch2, tgt_desc33, (size_t)n_tgt * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
+  if ((rc = launch_desc_from_aos(L, 1, n_tgt, scratch2))) return rc;
+  if ((rc = launch_match(L, 1, *p))) return rc;
+  return match_result(h, corr, nullptr, nullptr, cap, n_corr, n_mutual);
 }
 
 int qb200_match_and_pack(qb200_handle* h, const float* src4, int32_t n_src, const float* tgt4, int32_t n_tgt, const qb200_params* p,
                          int32_t* corr, float* src_matched4, float* tgt_matched4, int32_t cap, int32_t* n_corr) {
-  QB_IDLE(h);
-  if (!h || !n_corr || !params_ok(p) || n_src < 0 || n_tgt < 0 || cap < 0) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (!n_corr || !params_ok(p) || n_src < 0 || n_tgt < 0 || cap < 0) return QB200_ERR_BAD_ARG;
   if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
   *n_corr = 0;
-  if (n_src > h->V || n_tgt > h->V) { h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points"); return QB200_ERR_BAD_ARG; }
-  cudaSetDevice(h->device);
+  Lane* L = h->lane[0];
+  if (n_src > L->V || n_tgt > L->V) { h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points"); return QB200_ERR_BAD_ARG; }
   if (n_src == 0 || n_tgt == 0) return QB200_OK;
-  int rc = wave_reset(h, 2);
+  int rc = wave_reset(L, 2);
   if (rc) return rc;
-  if ((rc = upload_cloud_as_voxels(h, 0, src4, n_src))) return rc;
-  if ((rc = upload_cloud_as_voxels(h, 1, tgt4, n_tgt))) return rc;
-  if ((rc = launch_fpfh(h, 2, p->normal_radius, p->fpfh_radius, lattice_cell(*p)))) return rc;
-  if ((rc = launch_match(h, 1, *p))) return rc;
-  return download_corr(h, corr, src_matched4, tgt_matched4, cap, n_corr, nullptr);
+  if ((rc = upload_cloud_as_voxels(L, 0, src4, n_src))) return rc;
+  if ((rc = upload_cloud_as_voxels(L, 1, tgt4, n_tgt))) return rc;
+  if ((rc = launch_fpfh(L, 2, p->normal_radius, p->fpfh_radius, lattice_cell(*p)))) return rc;
+  if ((rc = launch_match(L, 1, *p))) return rc;
+  return match_result(h, corr, src_matched4, tgt_matched4, cap, n_corr, nullptr);
 }
 
 // ---- stage: graph ---------------------------------------------------------------------------------
 int qb200_build_graph(qb200_handle* h, const float* a4, const float* b4, int32_t L, double noise_bound, double cbar2, uint32_t* adj,
                       int32_t words_per_row, int32_t* degree, int64_t* n_edges) {
-  QB_IDLE(h);
-  if (!h || L < 0 || (L > 0 && (!a4 || !b4 || !adj)) || words_per_row < (L + 31) / 32 || !(noise_bound > 0) || !(cbar2 > 0))
+  if (int rc = enter(h)) return rc;
+  if (L < 0 || (L > 0 && (!a4 || !b4 || !adj)) || words_per_row < (L + 31) / 32 || !(noise_bound > 0) || !(cbar2 > 0))
     return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
   if (n_edges) *n_edges = 0;
   if (L == 0) return QB200_OK;
-  int rc = upload_matched(h, a4, b4, L);
+  Lane* ln = h->lane[0];
+  int rc = upload_matched(ln, a4, b4, L);
   if (rc) return rc;
-  if ((rc = launch_graph(h, 1, noise_bound, cbar2))) return rc;
+  if ((rc = launch_graph(ln, 1, noise_bound, cbar2))) return rc;
   const int nb = (L + 31) / 32;
   memset(adj, 0, (size_t)L * words_per_row * sizeof(uint32_t));
-  QB_CUDA_TRY(h, cudaMemcpy2DAsync(adj, (size_t)words_per_row * 4, h->adj, (size_t)h->W * 4, (size_t)nb * 4, L, cudaMemcpyDeviceToHost, h->stream));
-  if (degree) QB_CUDA_TRY(h, cudaMemcpyAsync(degree, h->deg, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  QB_CUDA_TRY(h, cudaMemcpy2DAsync(adj, (size_t)words_per_row * 4, ln->adj, (size_t)ln->W * 4, (size_t)nb * 4, L, cudaMemcpyDeviceToHost, ln->stream));
+  if (degree) QB_CUDA_TRY(h, cudaMemcpyAsync(degree, ln->deg, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, ln->stream));
   long long e2 = 0;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(&e2, h->ctr.n_edges, sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  QB_CUDA_TRY(h, cudaMemcpyAsync(&e2, ln->ctr.n_edges, sizeof(long long), cudaMemcpyDeviceToHost, ln->stream));
+  QB_CUDA_TRY(h, cudaStreamSynchronize(ln->stream));
   if (n_edges) *n_edges = e2 / 2;
   return QB200_OK;
 }
@@ -587,35 +867,35 @@ int qb200_build_graph(qb200_handle* h, const float* a4, const float* b4, int32_t
 int qb200_max_clique_ex(qb200_handle* h, const uint32_t* adj, int32_t L, int32_t words_per_row, int32_t mode, double kcore_thr,
                         int64_t node_limit, int32_t* clique, int32_t* n_clique, int32_t* kcore, int32_t* kcore_order, int32_t* max_core,
                         int32_t* flags) {
-  QB_IDLE(h);
-  if (!h || !n_clique || L < 0 || (L > 0 && (!adj || !clique)) || words_per_row < (L + 31) / 32) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (!n_clique || L < 0 || (L > 0 && (!adj || !clique)) || words_per_row < (L + 31) / 32) return QB200_ERR_BAD_ARG;
   if (mode != QB200_PMC_EXACT && mode != QB200_PMC_HEU && mode != QB200_KCORE_HEU) return QB200_ERR_BAD_ARG;
   if (node_limit < 0) return QB200_ERR_BAD_ARG;
   if (flags) *flags = 0;
   *n_clique = 0;
   if (max_core) *max_core = 0;
-  if (L > h->Lc) { h->fail(__FILE__, __LINE__, "L exceeds max_corr"); return QB200_ERR_BAD_ARG; }
-  cudaSetDevice(h->device);
+  Lane* ln = h->lane[0];
+  if (L > ln->Lc) { h->fail(__FILE__, __LINE__, "L exceeds max_corr"); return QB200_ERR_BAD_ARG; }
   if (L == 0) return QB200_OK;
-  int rc = wave_reset(h, 2);
+  int rc = wave_reset(ln, 2);
   if (rc) return rc;
   const int nb = (L + 31) / 32;
-  QB_CUDA_TRY(h, cudaMemsetAsync(h->adj, 0, (size_t)L * h->W * 4, h->stream));
-  QB_CUDA_TRY(h, cudaMemcpy2DAsync(h->adj, (size_t)h->W * 4, adj, (size_t)words_per_row * 4, (size_t)nb * 4, L, cudaMemcpyHostToDevice, h->stream));
-  if ((rc = set_counter(h, h->ctr.n_corr, L))) return rc;
-  if ((rc = launch_degree(h, 1))) return rc;
-  if ((rc = launch_clique(h, 1, mode, kcore_thr, node_limit))) return rc;
+  QB_CUDA_TRY(h, cudaMemsetAsync(ln->adj, 0, (size_t)L * ln->W * 4, ln->stream));
+  QB_CUDA_TRY(h, cudaMemcpy2DAsync(ln->adj, (size_t)ln->W * 4, adj, (size_t)words_per_row * 4, (size_t)nb * 4, L, cudaMemcpyHostToDevice, ln->stream));
+  if ((rc = set_counter(ln, ln->ctr.n_corr, L))) return rc;
+  if ((rc = launch_degree(ln, 1))) return rc;
+  if ((rc = launch_clique(ln, 1, mode, kcore_thr, node_limit))) return rc;
   int nc = 0, mc = 0, fl = 0;
-  if ((rc = get_counter(h, h->ctr.n_clique, &nc))) return rc;
-  if ((rc = get_counter(h, h->ctr.max_core, &mc))) return rc;
-  if ((rc = get_counter(h, h->ctr.flags, &fl))) return rc;
+  if ((rc = get_counter(ln, ln->ctr.n_clique, &nc))) return rc;
+  if ((rc = get_counter(ln, ln->ctr.max_core, &mc))) return rc;
+  if ((rc = get_counter(ln, ln->ctr.flags, &fl))) return rc;
   if (flags) *flags = fl;
   *n_clique = nc;
   if (max_core) *max_core = mc;
-  if (nc > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(clique, h->clique, (size_t)nc * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  if (kcore) QB_CUDA_TRY(h, cudaMemcpyAsync(kcore, h->kcore, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  if (kcore_order) QB_CUDA_TRY(h, cudaMemcpyAsync(kcore_order, h->korder, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (nc > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(clique, ln->clique, (size_t)nc * sizeof(int), cudaMemcpyDeviceToHost, ln->stream));
+  if (kcore) QB_CUDA_TRY(h, cudaMemcpyAsync(kcore, ln->kcore, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, ln->stream));
+  if (kcore_order) QB_CUDA_TRY(h, cudaMemcpyAsync(kcore_order, ln->korder, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, ln->stream));
+  QB_CUDA_TRY(h, cudaStreamSynchronize(ln->stream));
   h->last_n_clique = nc;
   return QB200_OK;
 }
@@ -628,233 +908,56 @@ int qb200_max_clique(qb200_handle* h, const uint32_t* adj, int32_t L, int32_t wo
 // ---- stage: pose given the clique -------------------------------------------------------------------
 int qb200_solve_pose(qb200_handle* h, const float* a4, const float* b4, int32_t L, const int32_t* clique, int32_t n_clique,
                      const qb200_params* p, qb200_result* res, uint8_t* rot_inlier_mask, uint8_t* trans_inlier_mask) {
-  QB_IDLE(h);
-  if (!h || !res || !params_ok(p) || L < 0 || (L > 0 && (!a4 || !b4)) || n_clique < 0 || n_clique > L || (n_clique > 0 && !clique))
+  if (int rc = enter(h)) return rc;
+  if (!res || !params_ok(p) || L < 0 || (L > 0 && (!a4 || !b4)) || n_clique < 0 || n_clique > L || (n_clique > 0 && !clique))
     return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  int rc = upload_matched(h, a4, b4, L);
+  Lane* ln = h->lane[0];
+  int rc = upload_matched(ln, a4, b4, L);
   if (rc) return rc;
-  if (n_clique > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(h->clique, clique, (size_t)n_clique * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  if ((rc = set_counter(h, h->ctr.n_clique, n_clique))) return rc;
-  if ((rc = launch_fill_counters(h, 1, 0))) return rc;
-  if ((rc = launch_pose(h, 1, *p))) return rc;
+  if (n_clique > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ln->clique, clique, (size_t)n_clique * sizeof(int), cudaMemcpyHostToDevice, ln->stream));
+  if ((rc = set_counter(ln, ln->ctr.n_clique, n_clique))) return rc;
+  if ((rc = launch_fill_counters(ln, 1, 0))) return rc;
+  if ((rc = launch_pose(ln, 1, resolve_params(h, *p)))) return rc;
   rc = fetch_result(h, res);
   if (rc < 0) return rc;
   if (res->valid) {
     const int nc = res->clique_size;
-    if (rot_inlier_mask) QB_CUDA_TRY(h, cudaMemcpyAsync(rot_inlier_mask, h->rot_mask, (size_t)nc, cudaMemcpyDeviceToHost, h->stream));
-    if (trans_inlier_mask) QB_CUDA_TRY(h, cudaMemcpyAsync(trans_inlier_mask, h->trans_mask, (size_t)nc, cudaMemcpyDeviceToHost, h->stream));
-    QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    if (rot_inlier_mask) QB_CUDA_TRY(h, cudaMemcpyAsync(rot_inlier_mask, ln->rot_mask, (size_t)nc, cudaMemcpyDeviceToHost, ln->stream));
+    if (trans_inlier_mask) QB_CUDA_TRY(h, cudaMemcpyAsync(trans_inlier_mask, ln->trans_mask, (size_t)nc, cudaMemcpyDeviceToHost, ln->stream));
+    QB_CUDA_TRY(h, cudaStreamSynchronize(ln->stream));
   }
   return rc;
 }
 
 // ---- Quatro::computeTransformation ------------------------------------------------------------------
 int qb200_solve_correspondences(qb200_handle* h, const float* a4, const float* b4, int32_t L, const qb200_params* p, qb200_result* res) {
-  if (!h || !res || !params_ok(p) || L < 0 || (L > 0 && (!a4 || !b4))) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  int rc = upload_matched(h, a4, b4, L);
+  if (int rc = enter(h)) return rc;
+  if (!res || !params_ok(p) || L < 0 || (L > 0 && (!a4 || !b4))) return QB200_ERR_BAD_ARG;
+  Lane* ln = h->lane[0];
+  int rc = upload_matched(ln, a4, b4, L);
   if (rc) return rc;
-  if ((rc = run_solver(h, 1, *p, 0))) return rc;
+  if ((rc = run_solver(ln, 1, resolve_params(h, *p), 0))) return rc;
   return fetch_result(h, res);
 }
 
 // ---- batches of precomputed correspondences -> poses ------------------------------------------------------
 int qb200_solve_batch(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p, qb200_mem_kind kind,
                       qb200_result* results) {
-  QB_IDLE(h);
-  if (!h || n_sets < 0 || (n_sets > 0 && (!sets || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (n_sets < 0 || (n_sets > 0 && (!sets || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
   for (int i = 0; i < n_sets; ++i)
-    if (sets[i].L < 0 || sets[i].L > h->Lc || (sets[i].L > 0 && (!sets[i].a || !sets[i].b))) {
+    if (sets[i].L < 0 || sets[i].L > h->cfg.max_corr || (sets[i].L > 0 && (!sets[i].a || !sets[i].b))) {
       h->fail(__FILE__, __LINE__, "correspondence set is null or exceeds max_corr");
       return QB200_ERR_BAD_ARG;
     }
-  cudaSetDevice(h->device);
-  for (int i = 0; i < 8; ++i) h->stage_ms[i] = 0.f;
-  for (int i = 0; i < 2; ++i) { h->kernel_ms[i] = 0.f; h->kernel_calls[i] = 0; h->kev_armed[i] = 0; }
-  const cudaMemcpyKind ck = kind == QB200_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
-  for (int w0 = 0; w0 < n_sets; w0 += h->S) {
-    const int np = n_sets - w0 < h->S ? n_sets - w0 : h->S;
-    int rc = wave_reset(h, 2 * np);
-    if (rc) return rc;
-    for (int s = 0; s < np; ++s) {
-      const qb200_corr_set& cs = sets[w0 + s];
-      h->h_cloud_n[s] = cs.L;
-      if (cs.L > 0) {
-        QB_CUDA_TRY(h, cudaMemcpyAsync(h->ma + (size_t)s * h->Lc, cs.a, (size_t)cs.L * sizeof(float4), ck, h->stream));
-        QB_CUDA_TRY(h, cudaMemcpyAsync(h->mb + (size_t)s * h->Lc, cs.b, (size_t)cs.L * sizeof(float4), ck, h->stream));
-      }
-    }
-    QB_CUDA_TRY(h, cudaMemcpyAsync(h->ctr.n_corr, h->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    cudaEventRecord(h->ev[4], h->stream);
-    cudaEventRecord(h->ev[5], h->stream);
-    if ((rc = run_solver(h, np, *p, 0))) return rc;
-    cudaEventRecord(h->ev[7], h->stream);
-    QB_CUDA_TRY(h, cudaMemcpyAsync(h->h_results, h->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, h->stream));
-    QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    memcpy(results + w0, h->h_results, (size_t)np * sizeof(qb200_result));
-    for (int i = 4; i < 7; ++i) {
-      float ms = 0.f;
-      if (cudaEventElapsedTime(&ms, h->ev[i], h->ev[i + 1]) == cudaSuccess) h->stage_ms[i] += ms;
-    }
-    if (h->kev_armed[1]) {
-      float ms = 0.f;
-      if (cudaEventElapsedTime(&ms, h->kev[2], h->kev[3]) == cudaSuccess) { h->kernel_ms[1] += ms; h->kernel_calls[1] += 1; }
-      h->kev_armed[1] = 0;
-    }
-  }
-  if (n_sets == 1) {
-    h->last_n_corr = results[0].n_corr;
-    h->last_n_clique = results[0].clique_size;
-    h->last_n_final = results[0].n_final_inliers;
-  }
-  return QB200_OK;
+  WaveInput in;
+  in.sets = sets;
+  in.kind = kind;
+  return run_waves(h, in, n_sets, n_sets > 0 ? resolve_params(h, *p) : *p, results);
 }
 
 // ---- raw scans -> pose ------------------------------------------------------------------------------
-// enqueue one wave (np <= S pairs) on lane L: H2D of the scans (host kind), K1..K11, D2H of the result records.  No sync.
-// cs: the batch's copy stream (host scans of a multi-wave batch), or nullptr = copy on the lane's own stream.  Copies queued on
-// several streams share the PCIe link, so every wave's scans would arrive late; on one stream they arrive wave after wave and the
-// first waves compute while the later ones are still crossing.
-static int wave_submit(qb200_handle* L, const qb200_pair* pairs, int w0, int np, qb200_mem_kind kind, const qb200_params* p, float cell,
-                       cudaStream_t cs) {
-  const int ncl = 2 * np;
-  int rc;
-  cudaEventRecord(L->ev[0], L->stream);
-  const cudaStream_t cps = cs ? cs : L->stream;
-  // (the lane's previous wave has been collected: raw_stage and the pinned tables are free)
-  int total = 0;
-  // host scans that lie back to back in the caller's memory (one big pinned buffer is the usual case) go over PCIe as one
-  // copy: far fewer DMA descriptors than one per scan
-  const float* run_src = nullptr;
-  int run_dst = 0, run_n = 0;
-  auto flush_run = [&]() -> int {
-    if (run_n > 0)
-      QB_CUDA_TRY(L, cudaMemcpyAsync(L->raw_stage + run_dst, run_src, (size_t)run_n * sizeof(float4), cudaMemcpyHostToDevice, cps));
-    run_n = 0;
-    return QB200_OK;
-  };
-  for (int s = 0; s < np; ++s) {
-    const qb200_pair& pr = pairs[w0 + s];
-    const float* ptr[2] = {pr.src, pr.tgt};
-    const int cnt[2] = {pr.n_src, pr.n_tgt};
-    for (int k = 0; k < 2; ++k) {
-      const int cloud = 2 * s + k;
-      L->h_raw_off[cloud] = total;
-      L->h_cloud_n[cloud] = cnt[k];
-      if (kind == QB200_MEM_HOST) {
-        L->h_cloud_ptr[cloud] = L->raw_stage + total;
-        if (cnt[k] > 0) {
-          if (run_n > 0 && ptr[k] == run_src + (size_t)run_n * 4 && run_n < (1 << 26)) {
-            run_n += cnt[k];
-          } else {
-            if ((rc = flush_run())) return rc;
-            run_src = ptr[k]; run_dst = total; run_n = cnt[k];
-          }
-        }
-      } else {
-        L->h_cloud_ptr[cloud] = reinterpret_cast<const float4*>(ptr[k]);
-      }
-      total += cnt[k];
-    }
-  }
-  if ((rc = flush_run())) return rc;
-  L->h_raw_off[ncl] = total;
-  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_cloud_ptr, L->h_cloud_ptr, (size_t)ncl * sizeof(float4*), cudaMemcpyHostToDevice, cps));
-  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_cloud_n, L->h_cloud_n, (size_t)ncl * sizeof(int), cudaMemcpyHostToDevice, cps));
-  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_raw_off, L->h_raw_off, (size_t)(ncl + 1) * sizeof(int), cudaMemcpyHostToDevice, cps));
-  if ((rc = wave_reset(L, ncl))) return rc;
-  if (cs) {
-    QB_CUDA_TRY(L, cudaEventRecord(L->ev_copied, cs));
-    QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, L->ev_copied, 0));
-  }
-  cudaEventRecord(L->ev[1], L->stream);
-  if ((rc = launch_voxel(L, ncl, p->voxel_size, p->skip_flagged))) return rc;
-  cudaEventRecord(L->ev[2], L->stream);
-  if ((rc = launch_fpfh(L, ncl, p->normal_radius, p->fpfh_radius, cell))) return rc;
-  cudaEventRecord(L->ev[3], L->stream);
-  if ((rc = launch_match(L, np, *p))) return rc;
-  cudaEventRecord(L->ev[4], L->stream);
-  cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
-  if ((rc = run_solver(L, np, *p, 1))) return rc;
-  cudaEventRecord(L->ev[7], L->stream);
-  QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
-  cudaEventRecord(L->ev[8], L->stream);
-  L->pend_w0 = w0;
-  L->pend_np = np;
-  return QB200_OK;
-}
-
-// wait for the wave in flight on lane L, hand out its records and add its stage / kernel times to the public handle h
-static int wave_collect(qb200_handle* h, qb200_handle* L) {
-  if (L->pend_np == 0) return QB200_OK;
-  const int np = L->pend_np;
-  L->pend_np = 0;
-  if (cudaStreamSynchronize(L->stream) != cudaSuccess) {
-    h->fail(__FILE__, __LINE__, cudaGetErrorString(cudaGetLastError()));
-    return QB200_ERR_CUDA;
-  }
-  memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
-  static const int timeline = (getenv("QB200_TIMELINE") && getenv("QB200_TIMELINE")[0] == '1') ? 1 : 0;
-  if (timeline) {  // stage boundaries of this wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
-    fprintf(stderr, "[qb200 timeline] wave w0=%d np=%d:", L->pend_w0, np);
-    for (int i = 0; i < 9; ++i) {
-      float ms = -1.f;
-      cudaEventElapsedTime(&ms, h->ev_fork, L->ev[i]);
-      fprintf(stderr, " %.2f", ms);
-    }
-    fprintf(stderr, "\n");
-  }
-  for (int i = 0; i < 8; ++i) {
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, L->ev[i], L->ev[i + 1]) == cudaSuccess) h->stage_ms[i] += ms;
-  }
-  for (int k = 0; k < 2; ++k) {
-    float ms = 0.f;
-    if (L->kev_armed[k] && cudaEventElapsedTime(&ms, L->kev[2 * k], L->kev[2 * k + 1]) == cudaSuccess) {
-      h->kernel_ms[k] += ms;
-      h->kernel_calls[k] += 1;
-    }
-    L->kev_armed[k] = 0;
-  }
-  return QB200_OK;
-}
-
-// wait for every wave in flight (oldest first) and hand out its records
-static int batch_flush(qb200_handle* h) {
-  int rc = QB200_OK;
-  const int n = h->lanes_active > 0 ? h->lanes_active : 1;
-  for (int i = 0; i < n; ++i) {
-    const int l = (h->lane_cursor + i) % n;
-    qb200_handle* L = l == 0 ? h : h->lane[l - 1];
-    if (!L) continue;
-    const int rc2 = wave_collect(h, L);
-    if (rc == QB200_OK) rc = rc2;
-  }
-  h->lanes_active = 0;
-  h->lane_cursor = 0;
-  return rc;
-}
-
-// wait for the waves in flight whose records go to dst (a batch queued by qb200_register_batch_enqueue), oldest first
-static int collect_batch_impl(qb200_handle* h, const qb200_result* dst) {
-  int rc = QB200_OK;
-  const int n = h->lanes_active > 0 ? h->lanes_active : 1;
-  for (int i = 0; i < n; ++i) {
-    const int l = (h->lane_cursor + i) % n;
-    qb200_handle* L = l == 0 ? h : h->lane[l - 1];
-    if (!L || L->pend_np == 0 || L->pend_dst != dst) continue;
-    const int rc2 = wave_collect(h, L);
-    if (rc == QB200_OK) rc = rc2;
-  }
-  return rc;
-}
-
-int qb200_register_batch_flush(qb200_handle* h) {
-  if (!h) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  return batch_flush(h);
-}
+int qb200_register_batch_flush(qb200_handle* h) { return enter(h); }
 
 int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                          qb200_result* results) {
@@ -862,11 +965,7 @@ int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pai
   const int rc2 = h ? batch_flush(h) : QB200_OK;  // on an error still wait for everything in flight (the copies read caller memory)
   if (rc == QB200_OK) rc = rc2;
   if (rc != QB200_OK) return rc;
-  if (n_pairs == 1) {
-    h->last_n_corr = results[0].n_corr;
-    h->last_n_clique = results[0].clique_size;
-    h->last_n_final = results[0].n_final_inliers;
-  }
+  if (n_pairs == 1) set_last(h, results[0]);
   return QB200_OK;
 }
 
@@ -877,28 +976,18 @@ int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32
                                  qb200_result* results) {
   if (!h || n_pairs < 0 || (n_pairs > 0 && (!pairs || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
   if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
+  const int S = h->cfg.max_batch_slots, R = h->cfg.max_raw_points;
   for (int i = 0; i < n_pairs; ++i) {
-    if (pairs[i].n_src < 0 || pairs[i].n_tgt < 0 || pairs[i].n_src > h->R || pairs[i].n_tgt > h->R ||
+    if (pairs[i].n_src < 0 || pairs[i].n_tgt < 0 || pairs[i].n_src > R || pairs[i].n_tgt > R ||
         (pairs[i].n_src > 0 && !pairs[i].src) || (pairs[i].n_tgt > 0 && !pairs[i].tgt)) {
       h->fail(__FILE__, __LINE__, "pair has a null cloud or exceeds max_raw_points");
       return QB200_ERR_BAD_ARG;
     }
   }
-  cudaSetDevice(h->device);
+  cudaSetDevice(h->cfg.device);
   const bool pipelined = h->lanes_active > 0;  // waves of an earlier enqueue are still in flight
-  if (!pipelined) {
-    for (int i = 0; i < 8; ++i) h->stage_ms[i] = 0.f;
-    for (int i = 0; i < 2; ++i) { h->kernel_ms[i] = 0.f; h->kernel_calls[i] = 0; h->kev_armed[i] = 0; }
-  }
-  // the rotation noise bound latches on the PUBLIC handle (quatro.hpp:469-470) and every lane gets the resolved value, so a pair's
-  // GNC bound never depends on the wave / lane it lands on
-  qb200_params p_resolved = *p;
-  if (!(p_resolved.rot_noise_bound > 0)) {
-    if (h->rot_noise_bound_latched <= 0) h->rot_noise_bound_latched = 2.0 * p->noise_bound;
-    p_resolved.rot_noise_bound = h->rot_noise_bound_latched;
-  }
-  p = &p_resolved;
-  const float cell = lattice_cell(*p);
+  if (!pipelined) reset_timers(h);
+  const qb200_params pr = resolve_params(h, *p);
   // More than one wave: rotate over the lanes so that one wave's PCIe copies and single-warp solver tail run under the
   // other waves' dense kernels.  Results do not depend on the lane (no state is shared between waves).
   // Wave plan.  Host inputs: nothing can run before the first wave's scans crossed PCIe, so the batch opens with a quarter
@@ -907,59 +996,58 @@ int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32
   int wave_n[64], n_waves = 0;
   {
     int left = n_pairs;
-    if (kind == QB200_MEM_HOST && n_pairs > h->S && h->S >= 8 && h->max_lanes > 1) {
-      wave_n[n_waves++] = h->S / 4;
-      wave_n[n_waves++] = h->S - h->S / 4;
-      left -= h->S;
+    if (kind == QB200_MEM_HOST && n_pairs > S && S >= 8 && h->max_lanes > 1) {
+      wave_n[n_waves++] = S / 4;
+      wave_n[n_waves++] = S - S / 4;
+      left -= S;
     }
     while (left > 0 && n_waves < 63) {
-      wave_n[n_waves] = left < h->S ? left : h->S;
+      wave_n[n_waves] = left < S ? left : S;
       left -= wave_n[n_waves++];
     }
     if (left > 0) n_waves = 0;  // more than ~60 waves: no special opening, walk uniformly below
   }
   const bool planned = n_waves > 0;
-  if (!planned) n_waves = (n_pairs + h->S - 1) / h->S;
+  if (!planned) n_waves = (n_pairs + S - 1) / S;
   int n_lanes = n_waves < h->max_lanes ? (n_waves < 1 ? 1 : n_waves) : h->max_lanes;
   if (pipelined && h->lanes_active != n_lanes) {  // a different lane count: start a fresh rotation
     const int rc0 = batch_flush(h);
     if (rc0) return rc0;
   }
   const bool fresh = h->lanes_active == 0;
-  qb200_handle* lanes[8] = {h, h, h, h, h, h, h, h};
   for (int l = 1; l < n_lanes; ++l) {
-    if (!h->lane[l - 1]) {
-      const int rc = qb200_create(&h->cfg, &h->lane[l - 1]);
+    if (!h->lane[l]) {
+      const int rc = lane_alloc(*h->lane[0], &h->lane[l]);
       if (rc != QB200_OK) {
+        lane_free(h->lane[l]);
+        h->lane[l] = nullptr;
         h->fail(__FILE__, __LINE__, "cannot allocate another lane");
         return rc;
       }
-      h->lane[l - 1]->max_lanes = 1;
     }
-    lanes[l] = h->lane[l - 1];
-    // the lanes start after whatever the caller queued on this handle's stream (first batch of a pipelined sequence only: later
-    // on this handle's stream carries a wave of its own)
+    // the lanes start after whatever the caller queued on lane 0's stream (first batch of a pipelined sequence only: later
+    // on lane 0's stream carries a wave of its own)
     if (fresh) {
-      if (l == 1) QB_CUDA_TRY(h, cudaEventRecord(h->ev_fork, h->stream));
-      QB_CUDA_TRY(h, cudaStreamWaitEvent(lanes[l]->stream, h->ev_fork, 0));
+      if (l == 1) QB_CUDA_TRY(h, cudaEventRecord(h->ev_fork, h->lane[0]->stream));
+      QB_CUDA_TRY(h, cudaStreamWaitEvent(h->lane[l]->stream, h->ev_fork, 0));
     }
   }
-  // host scans of a multi-wave batch: one copy stream, ordered after whatever the caller queued on this handle's stream
-  cudaStream_t copy_stream = nullptr;
+  WaveInput in;
+  in.pairs = pairs;
+  in.kind = kind;
+  // host scans of a multi-wave batch: one copy stream, ordered after whatever the caller queued on lane 0's stream
   if (kind == QB200_MEM_HOST && n_lanes > 1) {
-    copy_stream = h->copy_stream;
-    if (fresh) QB_CUDA_TRY(h, cudaStreamWaitEvent(copy_stream, h->ev_fork, 0));
+    in.copy_stream = h->copy_stream;
+    if (fresh) QB_CUDA_TRY(h, cudaStreamWaitEvent(in.copy_stream, h->ev_fork, 0));
   }
   h->lanes_active = n_lanes;
   int rc = QB200_OK, wave = 0;
   for (int w0 = 0; w0 < n_pairs && rc == QB200_OK; ++wave) {
-    qb200_handle* L = lanes[h->lane_cursor];
-    int np = planned ? wave_n[wave] : h->S;
+    Lane* L = h->lane[h->lane_cursor];
+    int np = planned ? wave_n[wave] : S;
     if (np > n_pairs - w0) np = n_pairs - w0;
     if ((rc = wave_collect(h, L))) break;  // the lane's previous wave (its pinned tables are reused)
-    L->pend_dst = results;
-    rc = wave_submit(L, pairs, w0, np, kind, p, cell, copy_stream);
-    if (rc != QB200_OK && L != h) h->fail(__FILE__, __LINE__, L->err);
+    rc = wave_submit(h, L, in, w0, np, pr, results);
     h->lane_cursor = (h->lane_cursor + 1) % n_lanes;  // always the lane that has been busy longest
     w0 += np;
   }
@@ -977,56 +1065,36 @@ int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const
 }
 
 // ---- introspection ----------------------------------------------------------------------------------
-static int copy_ints(qb200_handle* h, const int* dsrc, int n_have, int32_t* dst, int32_t cap, int32_t* n) {
-  if (!h || !n || cap < 0) return QB200_ERR_BAD_ARG;
-  *n = n_have;
-  const int m = n_have < cap ? n_have : cap;
-  cudaSetDevice(h->device);
-  if (m > 0 && dst) {
-    QB_CUDA_TRY(h, cudaMemcpyAsync(dst, dsrc, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  }
-  return n_have > cap ? QB200_CAPACITY_EXCEEDED : QB200_OK;
-}
 int qb200_get_last_clique(qb200_handle* h, int32_t* idx, int32_t cap, int32_t* n) {
-  return h ? copy_ints(h, h->clique, h->last_n_clique, idx, cap, n) : QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  return copy_ints(h->lane[0], h->lane[0]->clique, h->last_n_clique, idx, cap, n);
 }
 int qb200_get_last_final_inliers(qb200_handle* h, int32_t* idx, int32_t cap, int32_t* n) {
-  return h ? copy_ints(h, h->final_inl, h->last_n_final, idx, cap, n) : QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  return copy_ints(h->lane[0], h->lane[0]->final_inl, h->last_n_final, idx, cap, n);
 }
 int qb200_get_last_correspondences(qb200_handle* h, int32_t* corr, float* src_matched4, float* tgt_matched4, int32_t cap, int32_t* n) {
-  if (!h || !n || cap < 0) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  const int nc = h->last_n_corr;
-  *n = nc;
-  const int m = nc < cap ? nc : cap;
-  if (m > 0) {
-    std::vector<int> s(m), t(m);
-    QB_CUDA_TRY(h, cudaMemcpyAsync(s.data(), h->corr_src, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    QB_CUDA_TRY(h, cudaMemcpyAsync(t.data(), h->corr_tgt, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    if (src_matched4) QB_CUDA_TRY(h, cudaMemcpyAsync(src_matched4, h->ma, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    if (tgt_matched4) QB_CUDA_TRY(h, cudaMemcpyAsync(tgt_matched4, h->mb, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    if (corr)
-      for (int i = 0; i < m; ++i) { corr[2 * i] = s[i]; corr[2 * i + 1] = t[i]; }
-  }
-  return nc > cap ? QB200_CAPACITY_EXCEEDED : QB200_OK;
+  if (int rc = enter(h)) return rc;
+  if (!n || cap < 0) return QB200_ERR_BAD_ARG;
+  *n = h->last_n_corr;
+  return download_corr(h->lane[0], h->last_n_corr, corr, src_matched4, tgt_matched4, cap);
 }
 
 int qb200_get_last_features(qb200_handle* h, int32_t which, float* normals4, float* desc33, int32_t cap, int32_t* n_out) {
-  if (!h || !n_out || which < 0 || which > 1 || cap < 0) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
+  if (int rc = enter(h)) return rc;
+  if (!n_out || which < 0 || which > 1 || cap < 0) return QB200_ERR_BAD_ARG;
+  Lane* L = h->lane[0];
   int n = 0, rc;
-  if ((rc = get_counter(h, h->ctr.n_vox + which, &n))) return rc;
+  if ((rc = get_counter(L, L->ctr.n_vox + which, &n))) return rc;
   *n_out = n;
   const int m = n < cap ? n : cap;
   if (m > 0) {
-    if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, h->normals + (size_t)which * h->V, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
+    if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, L->normals + (size_t)which * L->V, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
     if (desc33) {
-      if ((rc = launch_desc_to_aos(h, which, m, h->aos_scratch))) return rc;
-      QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, h->aos_scratch, (size_t)m * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+      if ((rc = launch_desc_to_aos(L, which, m, L->aos_scratch))) return rc;
+      QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, L->aos_scratch, (size_t)m * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
     }
-    QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   }
   return n > cap ? QB200_CAPACITY_EXCEEDED : QB200_OK;
 }
@@ -1040,63 +1108,31 @@ int qb200_get_stage_ms(qb200_handle* h, float* ms, int32_t n) {
 // QB200_TC_VERIFY=1: every batch is matched by BOTH K6 implementations and the packed (distance, index) results are compared;
 // out2[0] = nearest-neighbour entries compared, out2[1] = entries that differ (must stay 0: the tensor-core filter is exact).
 int qb200_debug_match_verify(qb200_handle* h, uint64_t* out2, int32_t reset) {
-  if (!h || !out2) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  QB_CUDA_TRY(h, cudaMemcpy(out2, h->tc_stats + 4, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  if (reset) QB_CUDA_TRY(h, cudaMemset(h->tc_stats + 4, 0, 2 * sizeof(unsigned long long)));
-  for (int l = 0; l < 7; ++l) {
-    if (!h->lane[l]) continue;
-    uint64_t o2[2];
-    const int rc = qb200_debug_match_verify(h->lane[l], o2, reset);
-    if (rc) return rc;
-    out2[0] += o2[0]; out2[1] += o2[1];
-  }
-  return QB200_OK;
+  if (int rc = enter(h)) return rc;
+  return out2 ? read_tc_stats(h, 4, 2, out2, reset) : QB200_ERR_BAD_ARG;
 }
 
 // QB200_TC_PROF=1: clock64 accounting of tc_nn_kernel's roles (cycles summed over CTAs / warps), stats[8..31] -> out24
 int qb200_debug_tc_profile(qb200_handle* h, uint64_t* out24, int32_t reset) {
-  if (!h || !out24) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  QB_CUDA_TRY(h, cudaMemcpy(out24, h->tc_stats + 8, 24 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  if (reset) QB_CUDA_TRY(h, cudaMemset(h->tc_stats + 8, 0, 24 * sizeof(unsigned long long)));
-  for (int l = 0; l < 7; ++l) {
-    if (!h->lane[l]) continue;
-    uint64_t o[24];
-    const int rc = qb200_debug_tc_profile(h->lane[l], o, reset);
-    if (rc) return rc;
-    for (int i = 0; i < 24; ++i) out24[i] += o[i];
-  }
-  return QB200_OK;
+  if (int rc = enter(h)) return rc;
+  return out24 ? read_tc_stats(h, 8, 24, out24, reset) : QB200_ERR_BAD_ARG;
 }
 
 int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset) {
-  if (!h || !out4) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  QB_CUDA_TRY(h, cudaMemcpy(out4, h->tc_stats, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  if (reset) QB_CUDA_TRY(h, cudaMemset(h->tc_stats, 0, 4 * sizeof(unsigned long long)));
-  for (int l = 0; l < 7; ++l) {
-    if (!h->lane[l]) continue;
-    uint64_t o2[4];
-    const int rc = qb200_debug_match_stats(h->lane[l], o2, reset);
-    if (rc) return rc;
-    for (int i = 0; i < 4; ++i) out4[i] += o2[i];
-  }
-  return QB200_OK;
+  if (int rc = enter(h)) return rc;
+  return out4 ? read_tc_stats(h, 0, 4, out4, reset) : QB200_ERR_BAD_ARG;
 }
 
 // Nearest-neighbour tables of the most recent qb200_match (pair 0 of the handle, point order): what match_mutual_kernel read
 int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, uint64_t* colbest, int32_t cap_cols) {
-  if (!h || cap_rows < 0 || cap_cols < 0) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (int rc = enter(h)) return rc;
+  if (cap_rows < 0 || cap_cols < 0) return QB200_ERR_BAD_ARG;
+  Lane* L = h->lane[0];
+  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   const int nr = cap_rows < h->last_match_n[0] ? cap_rows : h->last_match_n[0];
   const int nc = cap_cols < h->last_match_n[1] ? cap_cols : h->last_match_n[1];
-  if (rowbest && nr > 0) QB_CUDA_TRY(h, cudaMemcpy(rowbest, h->rowbest, (size_t)nr * 8, cudaMemcpyDeviceToHost));
-  if (colbest && nc > 0) QB_CUDA_TRY(h, cudaMemcpy(colbest, h->colbest, (size_t)nc * 8, cudaMemcpyDeviceToHost));
+  if (rowbest && nr > 0) QB_CUDA_TRY(h, cudaMemcpy(rowbest, L->rowbest, (size_t)nr * 8, cudaMemcpyDeviceToHost));
+  if (colbest && nc > 0) QB_CUDA_TRY(h, cudaMemcpy(colbest, L->colbest, (size_t)nc * 8, cudaMemcpyDeviceToHost));
   return QB200_OK;
 }
 
@@ -1104,66 +1140,49 @@ int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, 
 // bytes, registers per thread, resident CTAs per SM (occupancy calculator at that shared-memory size)
 int qb200_debug_tc_footprint(qb200_handle* h, int32_t* out5) {
   if (!h || !out5) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  return tc_footprint(h, out5);
+  cudaSetDevice(h->cfg.device);
+  return tc_footprint(h->lane[0], out5);
 }
 
 // Validation hook: tensor-core (3xTF32) approximate squared distances between up to 128 source and 128 target
 // descriptors -> out[128*128] (row = source).  Lets tests measure the filter's error against the exact chain.
 int qb200_debug_tc_distances(qb200_handle* h, const float* a33, int32_t na, const float* b33, int32_t nb, float* out) {
-  QB_IDLE(h);
-  if (!h || !a33 || !b33 || !out || na < 1 || nb < 1 || na > 128 || nb > 128) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  int rc = wave_reset(h, 2);
+  if (int rc = enter(h)) return rc;
+  if (!a33 || !b33 || !out || na < 1 || nb < 1 || na > 128 || nb > 128) return QB200_ERR_BAD_ARG;
+  Lane* L = h->lane[0];
+  int rc = wave_reset(L, 2);
   if (rc) return rc;
-  if ((rc = set_counter(h, h->ctr.n_vox + 0, na))) return rc;
-  if ((rc = set_counter(h, h->ctr.n_vox + 1, nb))) return rc;
-  float* scratch = h->aos_scratch;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch, a33, (size_t)na * kDescDim * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  if ((rc = launch_desc_from_aos(h, 0, na, scratch))) return rc;
+  if ((rc = set_counter(L, L->ctr.n_vox + 0, na))) return rc;
+  if ((rc = set_counter(L, L->ctr.n_vox + 1, nb))) return rc;
+  float* scratch = L->aos_scratch;
+  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch, a33, (size_t)na * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
+  if ((rc = launch_desc_from_aos(L, 0, na, scratch))) return rc;
   float* scratch2 = scratch + (size_t)128 * kDescDim;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch2, b33, (size_t)nb * kDescDim * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  if ((rc = launch_desc_from_aos(h, 1, nb, scratch2))) return rc;
-  float* d_out = h->spfh;  // not the sort scratch: K6 sorts the descriptors by norm first
-  QB_CUDA_TRY(h, cudaMemsetAsync(d_out, 0, 128 * 128 * sizeof(float), h->stream));
-  if ((rc = launch_tc_debug_tile(h, d_out))) return rc;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(out, d_out, 128 * 128 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch2, b33, (size_t)nb * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
+  if ((rc = launch_desc_from_aos(L, 1, nb, scratch2))) return rc;
+  float* d_out = L->spfh;  // not the sort scratch: K6 sorts the descriptors by norm first
+  QB_CUDA_TRY(h, cudaMemsetAsync(d_out, 0, 128 * 128 * sizeof(float), L->stream));
+  if ((rc = launch_tc_debug_tile(L, d_out))) return rc;
+  QB_CUDA_TRY(h, cudaMemcpyAsync(out, d_out, 128 * 128 * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
+  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   return QB200_OK;
 }
 
 // ---- scan cache ---------------------------------------------------------------------------------------------------------
-// FPFHManager keeps the last target's descriptors and reuses them as the next source (odometry mode, fpfh_manager.hpp:74-77,
-// 111-118); a loop-closure sweep matches one scan against many.  The cache keeps voxel points, normals and FPFH-33 of a scan
-// resident on the device so that the front end (voxel + normals + FPFH, ~45 % of a wave) runs once per SCAN, not once per pair.
-static void cache_free(qb200_handle* h) {
-  if (h->c_vox) cudaFree(h->c_vox);
-  if (h->c_nrm) cudaFree(h->c_nrm);
-  if (h->c_desc) cudaFree(h->c_desc);
-  if (h->c_n) cudaFree(h->c_n);
-  if (h->c_status) cudaFree(h->c_status);
-  if (h->d_slot_of_cloud) cudaFree(h->d_slot_of_cloud);
-  if (h->h_slot_of_cloud) cudaFreeHost(h->h_slot_of_cloud);
-  delete[] h->c_sig;
-  h->c_vox = h->c_nrm = nullptr; h->c_desc = nullptr; h->c_n = h->c_status = h->d_slot_of_cloud = h->h_slot_of_cloud = nullptr;
-  h->c_sig = nullptr;
-  h->c_slots = 0;
-}
-
 int qb200_cache_reserve(qb200_handle* h, int32_t n_slots) {
-  if (!h || n_slots < 0 || n_slots > (1 << 20)) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (int rc = enter(h)) return rc;
+  if (n_slots < 0 || n_slots > (1 << 20)) return QB200_ERR_BAD_ARG;
+  QB_CUDA_TRY(h, cudaStreamSynchronize(h->lane[0]->stream));
   cache_free(h);
   if (n_slots == 0) return QB200_OK;
-  const size_t V = h->V, N = (size_t)n_slots;
+  const size_t V = h->cfg.max_voxel_points, N = (size_t)n_slots;
   QB_ALLOC(h, h->c_vox, N * V);
   QB_ALLOC(h, h->c_nrm, N * V);
   QB_ALLOC(h, h->c_desc, N * kDescK * V);
   QB_ALLOC(h, h->c_n, N);
   QB_ALLOC(h, h->c_status, N);
-  QB_ALLOC(h, h->d_slot_of_cloud, 2 * (size_t)h->S);
-  QB_CUDA_TRY(h, cudaMallocHost((void**)&h->h_slot_of_cloud, 2 * (size_t)h->S * sizeof(int)));
+  QB_ALLOC(h, h->d_slot_of_cloud, 2 * (size_t)h->cfg.max_batch_slots);
+  QB_CUDA_TRY(h, cudaMallocHost((void**)&h->h_slot_of_cloud, 2 * (size_t)h->cfg.max_batch_slots * sizeof(int)));
   QB_CUDA_TRY(h, cudaMemset(h->c_n, 0, N * sizeof(int)));
   QB_CUDA_TRY(h, cudaMemset(h->c_status, 0, N * sizeof(int)));
   QB_CUDA_TRY(h, cudaMemset(h->c_desc, 0, N * kDescK * V * sizeof(float)));
@@ -1173,62 +1192,41 @@ int qb200_cache_reserve(qb200_handle* h, int32_t n_slots) {
   return QB200_OK;
 }
 
-static int cache_copy(qb200_handle* h, int to_cache, int n_clouds) {
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_slot_of_cloud, h->h_slot_of_cloud, (size_t)n_clouds * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  const dim3 g((h->V + 255) / 256, 43, n_clouds);
-  cache_copy_kernel<<<g, 256, 0, h->stream>>>(to_cache, h->d_slot_of_cloud, h->V, h->vox_pts, h->normals, h->desc_t, h->ctr.n_vox, h->ctr.cloud_status,
-                                              h->c_vox, h->c_nrm, h->c_desc, h->c_n, h->c_status);
-  h->launches++;
-  QB_CUDA_TRY(h, cudaGetLastError());
-  return QB200_OK;
-}
-
 int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
                       const qb200_params* p, qb200_mem_kind kind) {
-  QB_IDLE(h);
-  if (!h || n_scans < 0 || (n_scans > 0 && (!scans4 || !n_points || !slot_ids)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (n_scans < 0 || (n_scans > 0 && (!scans4 || !n_points || !slot_ids)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
+  Lane* L = h->lane[0];
   for (int i = 0; i < n_scans; ++i)
-    if (slot_ids[i] < 0 || slot_ids[i] >= h->c_slots || n_points[i] < 0 || n_points[i] > h->R || (n_points[i] > 0 && !scans4[i])) {
+    if (slot_ids[i] < 0 || slot_ids[i] >= h->c_slots || n_points[i] < 0 || n_points[i] > L->R || (n_points[i] > 0 && !scans4[i])) {
       h->fail(__FILE__, __LINE__, "scan is null, exceeds max_raw_points or names a slot outside qb200_cache_reserve()");
       return QB200_ERR_BAD_ARG;
     }
-  cudaSetDevice(h->device);
   const float cell = lattice_cell(*p);
-  const int C = 2 * h->S;
+  const int C = 2 * L->S;
   for (int c0 = 0; c0 < n_scans; c0 += C) {
     const int nc = n_scans - c0 < C ? n_scans - c0 : C;
-    int total = 0, rc;
+    int rc;
     for (int c = 0; c < nc; ++c) {
-      const int n = n_points[c0 + c];
-      h->h_raw_off[c] = total;
-      h->h_cloud_n[c] = n;
+      L->h_cloud_ptr[c] = reinterpret_cast<const float4*>(scans4[c0 + c]);
+      L->h_cloud_n[c] = n_points[c0 + c];
       h->h_slot_of_cloud[c] = slot_ids[c0 + c];
-      if (kind == QB200_MEM_HOST) {
-        h->h_cloud_ptr[c] = h->raw_stage + total;
-        if (n > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(h->raw_stage + total, scans4[c0 + c], (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, h->stream));
-      } else {
-        h->h_cloud_ptr[c] = reinterpret_cast<const float4*>(scans4[c0 + c]);
-      }
-      total += n;
       float* sig = h->c_sig + 4 * (size_t)slot_ids[c0 + c];
       sig[0] = p->voxel_size; sig[1] = p->normal_radius; sig[2] = p->fpfh_radius; sig[3] = cell;
     }
-    h->h_raw_off[nc] = total;
-    QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_cloud_ptr, h->h_cloud_ptr, (size_t)nc * sizeof(float4*), cudaMemcpyHostToDevice, h->stream));
-    QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_cloud_n, h->h_cloud_n, (size_t)nc * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    QB_CUDA_TRY(h, cudaMemcpyAsync(h->d_raw_off, h->h_raw_off, (size_t)(nc + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    if ((rc = wave_reset(h, nc))) return rc;
-    if ((rc = launch_voxel(h, nc, p->voxel_size, p->skip_flagged))) return rc;
-    if ((rc = launch_fpfh(h, nc, p->normal_radius, p->fpfh_radius, cell))) return rc;
-    if ((rc = cache_copy(h, 1, nc))) return rc;
-    QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // the pinned tables are reused by the next wave
+    if ((rc = stage_raw(L, nc, kind, L->stream))) return rc;
+    if ((rc = wave_reset(L, nc))) return rc;
+    if ((rc = launch_voxel(L, nc, p->voxel_size, p->skip_flagged))) return rc;
+    if ((rc = launch_fpfh(L, nc, p->normal_radius, p->fpfh_radius, cell))) return rc;
+    if ((rc = cache_copy(h, L, 1, nc))) return rc;
+    QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));  // the pinned tables are reused by the next wave
   }
   return QB200_OK;
 }
 
 int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_result* results) {
-  QB_IDLE(h);
-  if (!h || n_pairs < 0 || (n_pairs > 0 && (!pairs || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (n_pairs < 0 || (n_pairs > 0 && (!pairs || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
   if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
   const float cell = lattice_cell(*p);
   for (int i = 0; i < n_pairs; ++i) {
@@ -1242,76 +1240,44 @@ int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t
       }
     }
   }
-  cudaSetDevice(h->device);
-  qb200_params pr = *p;
-  if (!(pr.rot_noise_bound > 0)) {
-    if (h->rot_noise_bound_latched <= 0) h->rot_noise_bound_latched = 2.0 * p->noise_bound;
-    pr.rot_noise_bound = h->rot_noise_bound_latched;
-  }
-  for (int i = 0; i < 8; ++i) h->stage_ms[i] = 0.f;
-  for (int w0 = 0; w0 < n_pairs; w0 += h->S) {
-    const int np = n_pairs - w0 < h->S ? n_pairs - w0 : h->S;
-    int rc;
-    for (int s = 0; s < np; ++s) {
-      h->h_slot_of_cloud[2 * s] = pairs[w0 + s].src_slot;
-      h->h_slot_of_cloud[2 * s + 1] = pairs[w0 + s].tgt_slot;
-    }
-    if ((rc = wave_reset(h, 2 * np))) return rc;
-    cudaEventRecord(h->ev[2], h->stream);
-    if ((rc = cache_copy(h, 0, 2 * np))) return rc;
-    cudaEventRecord(h->ev[3], h->stream);
-    if ((rc = launch_match(h, np, pr))) return rc;
-    cudaEventRecord(h->ev[4], h->stream);
-    cudaEventRecord(h->ev[5], h->stream);
-    if ((rc = run_solver(h, np, pr, 1))) return rc;
-    cudaEventRecord(h->ev[7], h->stream);
-    QB_CUDA_TRY(h, cudaMemcpyAsync(h->h_results, h->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, h->stream));
-    QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    memcpy(results + w0, h->h_results, (size_t)np * sizeof(qb200_result));
-    for (int i = 2; i < 7; ++i) {
-      float ms = 0.f;
-      if (cudaEventElapsedTime(&ms, h->ev[i], h->ev[i + 1]) == cudaSuccess) h->stage_ms[i] += ms;
-    }
-  }
-  if (n_pairs == 1) {
-    h->last_n_corr = results[0].n_corr;
-    h->last_n_clique = results[0].clique_size;
-    h->last_n_final = results[0].n_final_inliers;
-  }
-  return QB200_OK;
+  WaveInput in;
+  in.slots = pairs;
+  return run_waves(h, in, n_pairs, resolve_params(h, *p), results);
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {
-  if (!h || from_slot < 0 || to_slot < 0 || from_slot >= h->c_slots || to_slot >= h->c_slots) return QB200_ERR_BAD_ARG;
+  if (int rc = enter(h)) return rc;
+  if (from_slot < 0 || to_slot < 0 || from_slot >= h->c_slots || to_slot >= h->c_slots) return QB200_ERR_BAD_ARG;
   if (from_slot == to_slot) return QB200_OK;
-  cudaSetDevice(h->device);
-  const size_t V = h->V;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_vox + to_slot * V, h->c_vox + from_slot * V, V * sizeof(float4), cudaMemcpyDeviceToDevice, h->stream));
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_nrm + to_slot * V, h->c_nrm + from_slot * V, V * sizeof(float4), cudaMemcpyDeviceToDevice, h->stream));
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_desc + to_slot * kDescK * V, h->c_desc + from_slot * kDescK * V, kDescK * V * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_n + to_slot, h->c_n + from_slot, sizeof(int), cudaMemcpyDeviceToDevice, h->stream));
-  QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_status + to_slot, h->c_status + from_slot, sizeof(int), cudaMemcpyDeviceToDevice, h->stream));
+  const cudaStream_t st = h->lane[0]->stream;
+  const size_t V = h->cfg.max_voxel_points;
+  QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_vox + to_slot * V, h->c_vox + from_slot * V, V * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+  QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_nrm + to_slot * V, h->c_nrm + from_slot * V, V * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+  QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_desc + to_slot * kDescK * V, h->c_desc + from_slot * kDescK * V, kDescK * V * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_n + to_slot, h->c_n + from_slot, sizeof(int), cudaMemcpyDeviceToDevice, st));
+  QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_status + to_slot, h->c_status + from_slot, sizeof(int), cudaMemcpyDeviceToDevice, st));
   memcpy(h->c_sig + 4 * (size_t)to_slot, h->c_sig + 4 * (size_t)from_slot, 4 * sizeof(float));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  QB_CUDA_TRY(h, cudaStreamSynchronize(st));
   return QB200_OK;
 }
 
 int qb200_cache_read(qb200_handle* h, int32_t slot, float* vox4, float* normals4, float* desc33, int32_t cap, int32_t* n_out) {
-  if (!h || !n_out || slot < 0 || slot >= h->c_slots || cap < 0) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->device);
+  if (int rc = enter(h)) return rc;
+  if (!n_out || slot < 0 || slot >= h->c_slots || cap < 0) return QB200_ERR_BAD_ARG;
+  Lane* L = h->lane[0];
   int n = 0, rc;
-  if ((rc = get_counter(h, h->c_n + slot, &n))) return rc;
+  if ((rc = get_counter(L, h->c_n + slot, &n))) return rc;
   *n_out = n;
   const int m = n < cap ? n : cap;
-  const size_t V = h->V;
+  const size_t V = L->V;
   if (m > 0) {
-    if (vox4) QB_CUDA_TRY(h, cudaMemcpyAsync(vox4, h->c_vox + slot * V, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
-    if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, h->c_nrm + slot * V, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
+    if (vox4) QB_CUDA_TRY(h, cudaMemcpyAsync(vox4, h->c_vox + slot * V, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
+    if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, h->c_nrm + slot * V, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
     if (desc33) {
-      desc_to_aos_rows(h, h->c_desc + slot * kDescK * V, m, h->aos_scratch);
-      QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, h->aos_scratch, (size_t)m * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+      desc_to_aos_rows(L, h->c_desc + slot * kDescK * V, m, L->aos_scratch);
+      QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, L->aos_scratch, (size_t)m * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
     }
-    QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   }
   return n > cap ? QB200_CAPACITY_EXCEEDED : QB200_OK;
 }
@@ -1329,7 +1295,7 @@ int qb200_get_kernel_ms(qb200_handle* h, float* ms, int32_t* launches, int32_t n
 
 namespace qb {
 int collect_batch(qb200_handle* h, const qb200_result* dst) {
-  cudaSetDevice(h->device);
-  return collect_batch_impl(h, dst);
+  cudaSetDevice(h->cfg.device);
+  return collect_waves(h, dst);
 }
 }  // namespace qb

@@ -725,7 +725,7 @@ __global__ void __launch_bounds__(32) clique_exact_kernel(const uint32_t* __rest
 constexpr size_t kKcoreSmemBudget = 144 * 1024;
 
 template <int WPL>
-static int launch_kcore(qb200_handle* h, int n_pairs) {
+static int launch_kcore(Lane* h, int n_pairs) {
   const int Lc = h->Lc, W = h->W;
   const size_t fixed = (size_t)(Lc + 2) * sizeof(int) + (size_t)3 * kKcWarps * 32 * WPL * sizeof(uint32_t) +
                        (size_t)(4 + kKcWarps) * Lc * sizeof(unsigned short);
@@ -734,14 +734,14 @@ static int launch_kcore(qb200_handle* h, int n_pairs) {
   if (row_words < (size_t)kRing * W) row_words = (size_t)kRing * W;
   if (row_words > (size_t)Lc * W) row_words = (size_t)Lc * W;
   const size_t smem = fixed + row_words * 4;
-  if (int rc = ensure_dyn_smem(h, (const void*)kcore_kernel<WPL>, smem)) return rc;
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)kcore_kernel<WPL>, smem));
   kcore_kernel<WPL><<<n_pairs, kKcWarps * 32, smem, h->stream>>>(h->adj, h->deg, h->ctr.n_corr, Lc, W, (int)row_words, h->kcore, h->korder,
                                                                  h->rank_of, h->by_rank, h->kbin, h->ctr.max_core);
   return QB200_OK;
 }
 
 // PMC_EXACT scratch (level stack, list pool), allocated on the first exact call of a handle
-static int ensure_exact_scratch(qb200_handle* h) {
+static int ensure_exact_scratch(Lane* h) {
   if (h->ex_stack) return QB200_OK;
   const size_t S = h->S < kExactChunk ? h->S : kExactChunk;
   QB_CUDA_TRY(h, cudaMalloc((void**)&h->ex_stack, S * kExactDepth * (size_t)h->W * sizeof(uint32_t)));
@@ -752,8 +752,8 @@ static int ensure_exact_scratch(qb200_handle* h) {
 }
 
 template <int WPL>
-static int launch_exact(qb200_handle* h, int n_pairs, long long node_limit, int cache_words) {
-  if (int rc = ensure_dyn_smem(h, (const void*)clique_exact_kernel<WPL>, (size_t)cache_words * 4)) return rc;
+static int launch_exact(Lane* h, int n_pairs, long long node_limit, int cache_words) {
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)clique_exact_kernel<WPL>, (size_t)cache_words * 4));
   const int chunk = h->S < kExactChunk ? h->S : kExactChunk;
   for (int base = 0; base < n_pairs; base += chunk) {   // chunks run one after the other on the stream and share the scratch
     const int np = n_pairs - base < chunk ? n_pairs - base : chunk;
@@ -765,14 +765,14 @@ static int launch_exact(qb200_handle* h, int n_pairs, long long node_limit, int 
   return QB200_OK;
 }
 
-int launch_clique(qb200_handle* h, int n_pairs, int mode, double kcore_thr, long long node_limit) {
+int launch_clique(Lane* h, int n_pairs, int mode, double kcore_thr, long long node_limit) {
   if (n_pairs <= 0) return QB200_OK;
   const int Lc = h->Lc, W = h->W;
   // shared-memory adjacency cache of the descent: 14336 words (56 KB) hold graphs up to L ~ 660
   const int cache_words = 14336;
   const size_t sm_clique = (size_t)kCliqueWarps * Lc * sizeof(unsigned short) + (size_t)W * sizeof(uint32_t) + (size_t)cache_words * 4;
   int rc;
-  if ((rc = ensure_dyn_smem(h, (const void*)clique_cta_kernel, sm_clique))) return rc;
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)clique_cta_kernel, sm_clique));
   if (mode == QB200_PMC_EXACT && (rc = ensure_exact_scratch(h))) return rc;
   if (W <= 32) rc = launch_kcore<1>(h, n_pairs);
   else if (W <= 64) rc = launch_kcore<2>(h, n_pairs);

@@ -70,7 +70,7 @@ NcclApi& nccl() {
 // staging for n_local records per rank
 int ensure_staging(qb200_handle* h, int n_local) {
   if (n_local <= h->comm_cap) return QB200_OK;
-  cudaSetDevice(h->device);
+  cudaSetDevice(h->cfg.device);
   if (h->d_send) cudaFree(h->d_send);
   if (h->d_recv) cudaFree(h->d_recv);
   if (h->h_send) cudaFreeHost(h->h_send);
@@ -89,7 +89,7 @@ int ensure_staging(qb200_handle* h, int n_local) {
 int comm_common_init(qb200_handle* h, int world, int rank) {
   h->comm_world = world;
   h->comm_rank = rank;
-  cudaSetDevice(h->device);
+  cudaSetDevice(h->cfg.device);
   if (!h->comm_stream) QB_CUDA_TRY(h, cudaStreamCreateWithFlags(&h->comm_stream, cudaStreamNonBlocking));
   if (!h->comm_done) QB_CUDA_TRY(h, cudaEventCreateWithFlags(&h->comm_done, cudaEventDisableTiming));
   return QB200_OK;
@@ -176,7 +176,7 @@ int qb200_comm_init_all(qb200_handle** hs, int32_t n_dev) {
   std::vector<ncclComm_t> comms(n_dev, nullptr);
   for (int i = 0; i < n_dev; ++i) {
     if (hs[i]->comm) qb::comm_release(hs[i]);
-    devs[i] = hs[i]->device;
+    devs[i] = hs[i]->cfg.device;
     const int rc = comm_common_init(hs[i], n_dev, i);
     if (rc) return rc;
   }
@@ -190,7 +190,7 @@ int qb200_comm_init_all(qb200_handle** hs, int32_t n_dev) {
 int qb200_bind_numa(qb200_handle* h) {
   if (!h) return QB200_ERR_BAD_ARG;
   char bus[32] = {0};
-  if (cudaDeviceGetPCIBusId(bus, sizeof(bus), h->device) != cudaSuccess) return 0;
+  if (cudaDeviceGetPCIBusId(bus, sizeof(bus), h->cfg.device) != cudaSuccess) return 0;
   for (char* c = bus; *c; ++c)
     if (*c >= 'A' && *c <= 'Z') *c = (char)(*c - 'A' + 'a');
   char path[128];
@@ -227,10 +227,10 @@ int qb200_bind_numa(qb200_handle* h) {
 // wait for the gather in flight and hand out its records
 static int gather_wait(qb200_handle* h) {
   if (h->pend_gather_n <= 0) return QB200_OK;
-  cudaSetDevice(h->device);
+  cudaSetDevice(h->cfg.device);
   QB_CUDA_TRY(h, cudaEventSynchronize(h->comm_done));
   // whatever the caller records on the handle's stream next is ordered after the gather
-  QB_CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->comm_done, 0));
+  QB_CUDA_TRY(h, cudaStreamWaitEvent(h->lane[0]->stream, h->comm_done, 0));
   scatter_round_robin(h->h_recv, h->comm_world, h->pend_gather_n, h->pend_gather_dst, h->comm_world * h->pend_gather_n);
   h->pend_gather_n = 0;
   h->pend_gather_dst = nullptr;
@@ -319,7 +319,7 @@ int qb200_register_batch_sharded(qb200_handle** hs, int32_t n_dev, const qb200_p
     if (rcs[d]) { if (d) hs[0]->fail(__FILE__, __LINE__, hs[d]->err); return rcs[d]; }
   // one grouped all-gather over every device of this process
   for (int d = 0; d < n_dev; ++d) {
-    cudaSetDevice(hs[d]->device);
+    cudaSetDevice(hs[d]->cfg.device);
     QB_CUDA_TRY(hs[d], cudaMemcpyAsync(hs[d]->d_send, hs[d]->h_send, (size_t)n_local * sizeof(qb200_result), cudaMemcpyHostToDevice, hs[d]->comm_stream));
   }
   QB_NCCL_TRY(hs[0], nccl().GroupStart());
@@ -330,7 +330,7 @@ int qb200_register_batch_sharded(qb200_handle** hs, int32_t n_dev, const qb200_p
   int rc = enqueue_readback(hs[0], n_local);
   if (rc) return rc;
   for (int d = 0; d < n_dev; ++d) {
-    cudaSetDevice(hs[d]->device);
+    cudaSetDevice(hs[d]->cfg.device);
     QB_CUDA_TRY(hs[d], cudaStreamSynchronize(hs[d]->comm_stream));
   }
   scatter_round_robin(hs[0]->h_recv, n_dev, n_local, results, n_pairs);

@@ -27,7 +27,7 @@ size_t sort_temp_bytes(int max_items) {
   return bytes;
 }
 
-int sort_pairs(qb200_handle* h, int n_items, int end_bit) {
+int sort_pairs(Lane* h, int n_items, int end_bit) {
   if (n_items <= 0) return QB200_OK;
   size_t bytes = h->cub_bytes;
   QB_CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->cub_temp, bytes, h->key_a, h->key_b, h->val_a, h->val_b, n_items, 0, end_bit,
@@ -641,7 +641,7 @@ __global__ void desc_from_aos_kernel(const float* __restrict__ in, int V, int n,
 // ------------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------------
-int launch_voxel(qb200_handle* h, int n_clouds, float leaf, int skip_flagged) {
+int launch_voxel(Lane* h, int n_clouds, float leaf, int skip_flagged) {
   if (n_clouds <= 0) return QB200_OK;
   const float inv = 1.0f / leaf;
   const dim3 gb(n_clouds >= 16 ? 16 : 64, n_clouds);  // ~30 points per thread when the batch fills the device on its own
@@ -661,7 +661,7 @@ int launch_voxel(qb200_handle* h, int n_clouds, float leaf, int skip_flagged) {
   return QB200_OK;
 }
 
-int launch_fpfh(qb200_handle* h, int n_clouds, float normal_radius, float fpfh_radius, float cell) {
+int launch_fpfh(Lane* h, int n_clouds, float normal_radius, float fpfh_radius, float cell) {
   if (n_clouds <= 0) return QB200_OK;
   const int V = h->V;
   const float inv = 1.0f / cell;
@@ -699,7 +699,7 @@ int launch_fpfh(qb200_handle* h, int n_clouds, float normal_radius, float fpfh_r
   return QB200_OK;
 }
 
-int launch_desc_to_aos(qb200_handle* h, int cloud, int n, float* d_out33) {
+int launch_desc_to_aos(Lane* h, int cloud, int n, float* d_out33) {
   if (n <= 0) return QB200_OK;
   desc_to_aos_kernel<<<(n * kDescDim + 255) / 256, 256, 0, h->stream>>>(h->desc_t + (size_t)cloud * kDescK * h->V, h->V, n, d_out33);
   h->launches++;
@@ -707,14 +707,14 @@ int launch_desc_to_aos(qb200_handle* h, int cloud, int n, float* d_out33) {
   return QB200_OK;
 }
 // any dimension-major descriptor block [40][V] (e.g. a cache slot) -> AoS n x 33
-int desc_to_aos_rows(qb200_handle* h, const float* desc_rows, int n, float* d_out33) {
+int desc_to_aos_rows(Lane* h, const float* desc_rows, int n, float* d_out33) {
   if (n <= 0) return QB200_OK;
   desc_to_aos_kernel<<<(n * kDescDim + 255) / 256, 256, 0, h->stream>>>(desc_rows, h->V, n, d_out33);
   h->launches++;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;
 }
-int launch_desc_from_aos(qb200_handle* h, int cloud, int n, const float* d_in33) {
+int launch_desc_from_aos(Lane* h, int cloud, int n, const float* d_in33) {
   if (n <= 0) return QB200_OK;
   desc_from_aos_kernel<<<(n * kDescDim + 255) / 256, 256, 0, h->stream>>>(d_in33, h->V, n, h->desc_t + (size_t)cloud * kDescK * h->V);
   h->launches++;

@@ -264,7 +264,7 @@ __global__ void __launch_bounds__(256) degree_kernel(uint32_t* __restrict__ adj,
   }
 }
 
-int launch_degree(qb200_handle* h, int n_pairs) {
+int launch_degree(Lane* h, int n_pairs) {
   if (n_pairs <= 0) return QB200_OK;
   const dim3 gd((h->Lc + 7) / 8, n_pairs);
   degree_kernel<<<gd, 256, 0, h->stream>>>(h->adj, h->ctr.n_corr, h->Lc, h->W, h->deg, h->ctr.n_edges);
@@ -273,7 +273,7 @@ int launch_degree(qb200_handle* h, int n_pairs) {
   return QB200_OK;
 }
 
-int launch_graph(qb200_handle* h, int n_pairs, double noise_bound, double cbar2) {
+int launch_graph(Lane* h, int n_pairs, double noise_bound, double cbar2) {
   if (n_pairs <= 0) return QB200_OK;
   const double beta = 2 * noise_bound * sqrt(cbar2);  // quatro.hpp:367
   const double u = 5.9604644775390625e-8;             // 2^-24

@@ -1,4 +1,4 @@
-// handle.cuh -- the opaque qb200_handle: one device, one stream, device workspaces for one wave of
+// handle.cuh -- the opaque qb200_handle and its lanes: one device, per lane one stream and the device workspaces for one wave of
 // max_batch_slots pairs.  Replaces the reference's process-global state (function-local statics at
 // include/quatro.hpp:53,64,469-470,660 and include/fpfh_manager.hpp:110) with per-handle state.
 #pragma once
@@ -6,14 +6,19 @@
 
 #include "common.cuh"
 
-struct qb200_handle {
-  qb200_config cfg;
+namespace qb {
+
+// One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
+// of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
+// kernels of the others.
+struct Lane {
   int S, R, V, Lc, W;        // slots, raw cap / cloud, voxel cap / cloud, corr cap / pair, words per adjacency row
   int NS;                    // match stripes per pair = V / kMatchTile
   int device;
   int n_sm;                  // multiprocessors of the device (grid size of the persistent kernels)
+  int force_exact_match;     // 0 (default): tensor-core filter + exact evaluation; 1 (QB200_MATCH_EXACT=1): exact CUDA-core K6 only
   cudaStream_t own_stream, stream;
-  char err[512];
+  char* err;                 // the handle's message buffer (qb200_last_error)
   int64_t launches;
 
   // ---- wave description (host-known inputs) ----
@@ -22,17 +27,9 @@ struct qb200_handle {
   int* d_raw_off;             // [2S+1] offsets into the concatenated sort arrays
   const float4** h_cloud_ptr; int* h_cloud_n; int* h_raw_off;  // pinned mirrors
   float4* raw_stage;          // [2S*R] staging for host inputs
-  // Multi-wave batches rotate over this handle and up to 7 more lanes (own stream and buffers, created on first use):
-  // the H2D copies and the latency-bound solver tail of one wave overlap the dense kernels of the others.
-  qb200_handle* lane[7];
-  int max_lanes;              // 1..8 (QB200_LANES, default 4)
-  unsigned func_attr_set;     // which kernels already got their dynamic shared-memory opt-in on this handle's device
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
+  int pend_t0, pend_t1;       // ... the stage-time slots [t0, t1) it records
   qb200_result* pend_dst;     // ... and the caller's record array of its batch
-  int lanes_active, lane_cursor;  // public handle: lanes of the rotation in use (0 = nothing in flight), next lane = busy longest
-  cudaEvent_t ev_fork;
-  cudaStream_t copy_stream;   // host scans of a multi-wave batch cross PCIe on ONE stream, wave after wave (api.cu: wave_submit)
-  cudaEvent_t ev_copied;      // this lane's scans have arrived (recorded on the copy stream)
 
   // ---- sort workspace (voxel sort, then lattice sort) ----
   uint64_t *key_a, *key_b;    // [2S*max(R,V)]
@@ -55,7 +52,6 @@ struct qb200_handle {
   float* desc_norm;           // [2S*V] squared norms (fp32 fma chain)
   int* tc_fallback;           // [S] 1 = too many exact ties for the filter to pay off: pair re-done by the exact fp32 kernel
   unsigned long long* tc_stats; // [32] diagnostics, cumulative: [0..3] exact evaluations, tiles drained, warm-up passes, aborted stripes; [4..5] QB200_TC_VERIFY; [8..31] QB200_TC_PROF
-  int force_exact_match;      // 0 (default): tensor-core filter + exact evaluation; 1 (QB200_MATCH_EXACT=1): exact CUDA-core K6 only
   // ---- matching ----
   unsigned long long* rowbest;// [S*V] packed (dist bits << 32 | tgt idx) per source point
   unsigned long long* colpart;// [2SV + S*(V/128)*2 + 2] tensor-core K6 scratch: class results [2][S][V] and the tile-max cache
@@ -84,8 +80,28 @@ struct qb200_handle {
   // ---- results ----
   qb200_result* d_results;    // [S]
   qb200_result* h_results;    // pinned [S]
-  qb::WaveCounters ctr;
+  WaveCounters ctr;
   int* ctr_block; size_t ctr_ints;
+
+  cudaEvent_t ev[9];          // stage boundaries of the last wave: start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
+  cudaEvent_t kev[4];         // [0,1] around match_stripe_kernel, [2,3] around tim_graph_kernel (last wave)
+  int kev_armed[2];
+
+  void fail(const char* file, int line, const char* msg) { snprintf(err, kErrLen, "%s:%d: %s", file, line, msg); }
+  static constexpr int kErrLen = 512;
+};
+
+}  // namespace qb
+
+struct qb200_handle {
+  qb200_config cfg;
+  char err[qb::Lane::kErrLen];
+  qb::Lane* lane[8];          // lane[0] is created with the handle, the others on first use
+  int max_lanes;              // 1..8 (QB200_LANES, default 4)
+  int lanes_active, lane_cursor;  // lanes of the rotation in use (0 = nothing in flight), next lane = busy longest
+  cudaEvent_t ev_fork;
+  cudaStream_t copy_stream;   // host scans of a multi-wave batch cross PCIe on ONE stream, wave after wave (api.cu: wave_submit)
+  cudaEvent_t ev_copied;      // a wave's scans have arrived (recorded on the copy stream)
 
   // ---- scan cache (qb200_cache_*): front-end results of whole scans, resident on the device ----
   int c_slots;
@@ -111,48 +127,43 @@ struct qb200_handle {
   int last_n_corr, last_n_clique, last_n_final;  // slot 0 of the most recent single-pair call
   int last_match_n[2];        // source / target points of the most recent qb200_match (qb200_debug_nn_tables)
 
-  cudaEvent_t ev[9];
   float stage_ms[8];
-  cudaEvent_t kev[4];        // [0,1] around match_stripe_kernel, [2,3] around tim_graph_kernel (last wave)
   float kernel_ms[2];
   int kernel_calls[2];
-  int kev_armed[2];
 
-  void fail(const char* file, int line, const char* msg) {
-    snprintf(err, sizeof(err), "%s:%d: %s", file, line, msg);
-  }
+  void fail(const char* file, int line, const char* msg) { snprintf(err, sizeof(err), "%s:%d: %s", file, line, msg); }
 };
 
 namespace qb {
 
-// Stage launchers (each enqueues kernels on h->stream for clouds/pairs [0, n) of the current wave).
-int launch_voxel(qb200_handle* h, int n_clouds, float leaf, int skip_flagged);
-int launch_fpfh(qb200_handle* h, int n_clouds, float normal_radius, float fpfh_radius, float cell);
-int launch_match(qb200_handle* h, int n_pairs, const qb200_params& p);
-int launch_graph(qb200_handle* h, int n_pairs, double noise_bound, double cbar2);
-int launch_clique(qb200_handle* h, int n_pairs, int mode, double kcore_thr, long long node_limit);
-int launch_pose(qb200_handle* h, int n_pairs, const qb200_params& p);
-int launch_fill_counters(qb200_handle* h, int n_pairs, int have_frontend);
-int launch_finalize_status(qb200_handle* h, int n_pairs);
-int launch_iota_clique(qb200_handle* h, int n_pairs);
-int launch_segment_cloud(qb200_handle* h, const float4* pts, int n, const qb200_segment_params& sp, int* n_valid, int* n_outlier,
+// Stage launchers (each enqueues kernels on the lane's stream for clouds/pairs [0, n) of its current wave).
+int launch_voxel(Lane* h, int n_clouds, float leaf, int skip_flagged);
+int launch_fpfh(Lane* h, int n_clouds, float normal_radius, float fpfh_radius, float cell);
+int launch_match(Lane* h, int n_pairs, const qb200_params& p);
+int launch_graph(Lane* h, int n_pairs, double noise_bound, double cbar2);
+int launch_clique(Lane* h, int n_pairs, int mode, double kcore_thr, long long node_limit);
+int launch_pose(Lane* h, int n_pairs, const qb200_params& p);
+int launch_fill_counters(Lane* h, int n_pairs, int have_frontend);
+int launch_finalize_status(Lane* h, int n_pairs);
+int launch_iota_clique(Lane* h, int n_pairs);
+int launch_segment_cloud(Lane* h, const float4* pts, int n, const qb200_segment_params& sp, int* n_valid, int* n_outlier,
                          const float4** valid_dev, const float4** outlier_dev);
-int launch_patchwork(qb200_handle* h, const float4* pts, int n, const qb200_patchwork_params& pp, int* n_ground, int* n_nonground, int* status);
-int launch_match_nn(qb200_handle* h, int n_pairs);
-int launch_match_exact(qb200_handle* h, int n_pairs, const int* only);
-int launch_tc_debug_tile(qb200_handle* h, float* d_out);
-int tc_footprint(qb200_handle* h, int* out5);
-int launch_desc_to_aos(qb200_handle* h, int cloud, int n, float* d_out33);
-int launch_desc_from_aos(qb200_handle* h, int cloud, int n, const float* d_in33);
-int desc_to_aos_rows(qb200_handle* h, const float* desc_rows, int n, float* d_out33);
+int launch_patchwork(Lane* h, const float4* pts, int n, const qb200_patchwork_params& pp, int* n_ground, int* n_nonground, int* status);
+int launch_match_nn(Lane* h, int n_pairs);
+int launch_match_exact(Lane* h, int n_pairs, const int* only);
+int launch_tc_debug_tile(Lane* h, float* d_out);
+int tc_footprint(Lane* h, int* out5);
+int launch_desc_to_aos(Lane* h, int cloud, int n, float* d_out33);
+int launch_desc_from_aos(Lane* h, int cloud, int n, const float* d_in33);
+int desc_to_aos_rows(Lane* h, const float* desc_rows, int n, float* d_out33);
 size_t sort_temp_bytes(int max_items);
 void comm_release(qb200_handle* h);
 int collect_batch(qb200_handle* h, const qb200_result* dst);  // api.cu: wait for every wave in flight that writes into dst[...]
-// Raise a kernel's dynamic shared-memory opt-in to at least `bytes` on the handle's device.  The attribute is a property of the
+// Raise a kernel's dynamic shared-memory opt-in to at least `bytes` on `device`.  The attribute is a property of the
 // (function, device), not of a handle: handles of different capacities share it, so it is only ever raised (process-wide maximum).
-int ensure_dyn_smem(qb200_handle* h, const void* kernel, size_t bytes);
-int sort_pairs(qb200_handle* h, int n_items, int end_bit);
-int launch_voxel_sort(qb200_handle* h, int n_clouds, float inv_leaf, int skip_flagged, int idx_bits);
-int launch_cloud_sort(qb200_handle* h, int n_clouds, const int* n_items, int f1, int f2);
+cudaError_t ensure_dyn_smem(int device, const void* kernel, size_t bytes);
+int sort_pairs(Lane* h, int n_items, int end_bit);
+int launch_voxel_sort(Lane* h, int n_clouds, float inv_leaf, int skip_flagged, int idx_bits);
+int launch_cloud_sort(Lane* h, int n_clouds, const int* n_items, int f1, int f2);
 
 }  // namespace qb

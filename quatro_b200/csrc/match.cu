@@ -374,10 +374,10 @@ size_t match_smem_bytes() { return 3 * sizeof(float) * kDescDim * kMT + 8 * kMT 
 
 // exact fp32 CUDA-core nearest neighbours (both directions).  only == nullptr: every pair; otherwise just the
 // pairs flagged in only[] (the tensor-core filter's overflow fallback).
-int launch_match_exact(qb200_handle* h, int n_pairs, const int* only) {
+int launch_match_exact(Lane* h, int n_pairs, const int* only) {
   const int V = h->V;
   const size_t smem = match_smem_bytes();
-  if (int rc = ensure_dyn_smem(h, (const void*)match_stripe_kernel, smem)) return rc;
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)match_stripe_kernel, smem));
   const dim3 gf((V + 255) / 256, n_pairs);
   match_colreset_kernel<<<gf, 256, 0, h->stream>>>(h->ctr.n_vox, V, only, h->colbest);
   const dim3 gs(h->NS, n_pairs);
@@ -411,7 +411,7 @@ __global__ void match_verify_kernel(const unsigned long long* __restrict__ rb_tc
   }
 }
 
-int launch_match(qb200_handle* h, int n_pairs, const qb200_params& p) {
+int launch_match(Lane* h, int n_pairs, const qb200_params& p) {
   if (n_pairs <= 0) return QB200_OK;
   const int V = h->V;
   int rc = h->force_exact_match ? launch_match_exact(h, n_pairs, nullptr) : launch_match_nn(h, n_pairs);

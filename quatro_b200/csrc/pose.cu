@@ -359,16 +359,10 @@ static int next_pow2(int n) {
 }
 size_t pose_smem_bytes(int Lp) { return (size_t)4 * Lp * sizeof(double) + (size_t)4 * Lp * sizeof(unsigned short) + (size_t)2 * Lp; }
 
-int launch_pose(qb200_handle* h, int n_pairs, const qb200_params& p) {
+int launch_pose(Lane* h, int n_pairs, const qb200_params& p) {
   if (n_pairs <= 0) return QB200_OK;
   PoseParams pp;
-  // The reference latches 2*noise_bound of the FIRST registration into a function-local static
-  // (quatro.hpp:469-470 after :851); here the latch is a per-handle field, overridable via params.
-  if (p.rot_noise_bound > 0) pp.rot_noise_bound = p.rot_noise_bound;
-  else {
-    if (h->rot_noise_bound_latched <= 0) h->rot_noise_bound_latched = 2.0 * p.noise_bound;
-    pp.rot_noise_bound = h->rot_noise_bound_latched;
-  }
+  pp.rot_noise_bound = p.rot_noise_bound;  // resolved by the entry point (api.cu: resolve_params, the handle's latch)
   pp.cote_range = p.cote_noise_bound * sqrt(p.cbar2);
   pp.gnc_factor = p.rotation_gnc_factor;
   pp.cost_threshold = p.rotation_cost_threshold;
@@ -379,7 +373,7 @@ int launch_pose(qb200_handle* h, int n_pairs, const qb200_params& p) {
   for (int i = 0; i < 9; ++i) pp.RyRx[i] = p.RyRx[i];
   const int Lp = next_pow2(h->Lc < 4096 ? h->Lc : 4096);
   const size_t smem = pose_smem_bytes(Lp);
-  if (int rc = ensure_dyn_smem(h, (const void*)pose_kernel, smem)) return rc;
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)pose_kernel, smem));
   pose_kernel<<<n_pairs, kPoseThreads, smem, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, h->Lc, Lp, h->clique, h->ctr.n_clique, pp, h->d_results,
                                                           h->rot_mask, h->trans_mask, h->final_inl, h->ctr.n_final);
   h->launches++;
@@ -387,17 +381,17 @@ int launch_pose(qb200_handle* h, int n_pairs, const qb200_params& p) {
   return QB200_OK;
 }
 
-int launch_fill_counters(qb200_handle* h, int n_pairs, int have_frontend) {
+int launch_fill_counters(Lane* h, int n_pairs, int have_frontend) {
   fill_counters_kernel<<<(n_pairs + 127) / 128, 128, 0, h->stream>>>(h->d_results, n_pairs, h->ctr, have_frontend);
   h->launches++;
   return QB200_OK;
 }
-int launch_finalize_status(qb200_handle* h, int n_pairs) {
+int launch_finalize_status(Lane* h, int n_pairs) {
   finalize_status_kernel<<<(n_pairs + 127) / 128, 128, 0, h->stream>>>(h->d_results, n_pairs, h->ctr);
   h->launches++;
   return QB200_OK;
 }
-int launch_iota_clique(qb200_handle* h, int n_pairs) {
+int launch_iota_clique(Lane* h, int n_pairs) {
   const dim3 g((h->Lc + 255) / 256, n_pairs);
   iota_clique_kernel<<<g, 256, 0, h->stream>>>(h->ctr.n_corr, h->Lc, h->clique, h->ctr.n_clique, h->ctr.max_core);
   h->launches++;

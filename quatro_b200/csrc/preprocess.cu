@@ -333,7 +333,7 @@ __global__ void __launch_bounds__(256) pw_gather_kernel(const float4* __restrict
   }
 }
 
-static int ensure_pw_scratch(qb200_handle* h) {
+static int ensure_pw_scratch(Lane* h) {
   if (h->pw_ints) return QB200_OK;
   const size_t R = h->R;
   // ints: patch_of [R] | rank [R] | count, start(+1), cursor, n_ground, n_nonground, goff, ngoff [each 4096+1] | out_n [2] | status [1]
@@ -343,7 +343,7 @@ static int ensure_pw_scratch(qb200_handle* h) {
 }
 
 // pts: n points on the device.  Leaves the two outputs in h->pw_out ([0, R) ground, [R, 2R) non-ground) and returns their sizes.
-int launch_patchwork(qb200_handle* h, const float4* pts, int n, const qb200_patchwork_params& pp, int* n_ground, int* n_nonground, int* status) {
+int launch_patchwork(Lane* h, const float4* pts, int n, const qb200_patchwork_params& pp, int* n_ground, int* n_nonground, int* status) {
   *n_ground = *n_nonground = 0;
   *status = QB200_OK;
   if (!pw_params_valid(pp)) return QB200_ERR_BAD_ARG;
@@ -374,7 +374,7 @@ int launch_patchwork(qb200_handle* h, const float4* pts, int n, const qb200_patc
   pw_scan_kernel<<<1, 1024, 0, h->stream>>>(count, NP, start, cursor);
   pw_scatter_kernel<<<nb, 256, 0, h->stream>>>(pts, n, patch_of, cursor, items);
   const size_t smem = (size_t)kPwMaxPatchPts * 9;
-  if (int rc = ensure_dyn_smem(h, (const void*)pw_patch_kernel, smem)) return rc;
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)pw_patch_kernel, smem));
   pw_patch_kernel<<<NP, kPwThreads, smem, h->stream>>>(pts, c, start, items, kPwMaxPatchPts, ng_ground, ng_non, rank, out_n + 2);
   pw_offsets_kernel<<<1, 1024, 0, h->stream>>>(ng_ground, ng_non, NP, goff, ngoff, out_n);
   pw_gather_kernel<<<NP, 256, 0, h->stream>>>(pts, start, ng_ground, ng_non, items, rank, goff, ngoff, h->pw_out, h->pw_out + R);
@@ -560,7 +560,7 @@ __global__ void __launch_bounds__(1024) ip_extract_kernel(const float4* __restri
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) { out_n[0] = s_base[0] + (both & 0xFFFF); out_n[1] = s_base[1] + (both >> 16); }
 }
 
-static int ensure_ip_scratch(qb200_handle* h, int npix) {
+static int ensure_ip_scratch(Lane* h, int npix) {
   if (h->ip_buf && h->ip_npix >= npix) return QB200_OK;
   if (h->ip_buf) { cudaFree(h->ip_buf); h->ip_buf = nullptr; }
   // per pixel: rows u64 | valid float4 | outlier float4 | winner, parent, size int | range float | kind u8 ; + out_n [2] + block counts
@@ -576,7 +576,7 @@ static bool ip_params_valid(const qb200_segment_params& sp) {
 }
 
 // pts: n device points.  Leaves the outputs in the handle's scratch; *valid_dev / *outlier_dev point at them.
-int launch_segment_cloud(qb200_handle* h, const float4* pts, int n, const qb200_segment_params& sp, int* n_valid, int* n_outlier,
+int launch_segment_cloud(Lane* h, const float4* pts, int n, const qb200_segment_params& sp, int* n_valid, int* n_outlier,
                          const float4** valid_dev, const float4** outlier_dev) {
   *n_valid = *n_outlier = 0;
   if (!ip_params_valid(sp)) return QB200_ERR_BAD_ARG;

@@ -125,11 +125,11 @@ __global__ void __launch_bounds__(kSortThreads) cloud_sort_kernel(const uint64_t
 
 // Sort the first n_items[c] keys of every cloud c (key_a -> key_b, val_b = source index).  Returns QB200_ERR_UNSUPPORTED when
 // max_voxel_points is too large for the shared-memory layout (the caller then uses the device-wide sort).
-int launch_cloud_sort(qb200_handle* h, int n_clouds, const int* n_items, int f1, int f2) {
+int launch_cloud_sort(Lane* h, int n_clouds, const int* n_items, int f1, int f2) {
   if (n_clouds <= 0) return QB200_OK;
   const size_t smem = cloud_sort_smem_bytes(h->V);
   if (smem > 227 * 1024 || h->V > 65535) return QB200_ERR_UNSUPPORTED;
-  if (int rc = ensure_dyn_smem(h, (const void*)cloud_sort_kernel, smem)) return rc;
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)cloud_sort_kernel, smem));
   cloud_sort_kernel<<<n_clouds, kSortThreads, smem, h->stream>>>(h->key_a, n_items, h->V, f1, f2, h->key_b, h->val_b);
   h->launches += 1;
   QB_CUDA_TRY(h, cudaGetLastError());

@@ -870,14 +870,14 @@ static size_t tc_smem_bytes() {
 }
 
 // dynamic shared memory of tc_nn_kernel and a shared-memory-first carveout, so that two CTAs fit on every SM
-static int tc_prepare(qb200_handle* h, const void* kernel) {
-  if (int rc = ensure_dyn_smem(h, kernel, tc_smem_bytes())) return rc;
+static int tc_prepare(Lane* h, const void* kernel) {
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, kernel, tc_smem_bytes()));
   QB_CUDA_TRY(h, cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   return QB200_OK;
 }
 
 // threads, dynamic and static shared bytes, registers per thread and resident CTAs per SM of tc_nn_kernel as launched
-int tc_footprint(qb200_handle* h, int* out5) {
+int tc_footprint(Lane* h, int* out5) {
   const void* kernel = (const void*)tc_nn_kernel<false>;
   if (int rc = tc_prepare(h, kernel)) return rc;
   cudaFuncAttributes fa;
@@ -894,7 +894,7 @@ int tc_footprint(qb200_handle* h, int* out5) {
 
 // norm keys -> one radix sort for all clouds (h->val_b = rank -> point) -> duplicate classes.
 // Scratch (free once the sort consumed its inputs): val_a = unique rank -> point, key_a = [class of rank | unique counts].
-static int sort_and_dedup(qb200_handle* h, int n_clouds, int dedup) {
+static int sort_and_dedup(Lane* h, int n_clouds, int dedup) {
   const int V = h->V;
   const dim3 g((V + 255) / 256, n_clouds);
   norm_key_kernel<<<g, 256, 0, h->stream>>>(h->desc_t, h->ctr.n_vox, V, h->key_a, h->val_a);
@@ -912,7 +912,7 @@ static int sort_and_dedup(qb200_handle* h, int n_clouds, int dedup) {
   return QB200_OK;
 }
 
-int launch_match_nn(qb200_handle* h, int n_pairs) {
+int launch_match_nn(Lane* h, int n_pairs) {
   const int V = h->V;
   const size_t smem = tc_smem_bytes();
   if (int rc = tc_prepare(h, (const void*)tc_nn_kernel<false>)) return rc;
@@ -952,7 +952,7 @@ int launch_match_nn(qb200_handle* h, int n_pairs) {
 
 // debug/validation hook: approximate distances d~ of stripe 0 of pair 0, both 64-column tiles of up to 128 x 128 descriptors
 // (descriptors already in desc_t; duplicates are kept so that every (row, column) of the dump is filled)
-int launch_tc_debug_tile(qb200_handle* h, float* d_out) {
+int launch_tc_debug_tile(Lane* h, float* d_out) {
   const size_t smem = tc_smem_bytes();
   if (int rc0 = tc_prepare(h, (const void*)tc_nn_kernel<true>)) return rc0;
   int rc = sort_and_dedup(h, 2, 0);

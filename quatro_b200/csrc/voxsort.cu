@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(kVsThreads) vsort_scatter_kernel(int pass, con
 
 // Sort the packed items of every cloud (A = key_a, B = key_b).  Afterwards cloud c's sorted segment starts at
 // (vox_digits(c) odd ? B : A) + raw_off[c] and holds n_valid[c] items.
-int launch_voxel_sort(qb200_handle* h, int n_clouds, float inv_leaf, int skip_flagged, int idx_bits) {
+int launch_voxel_sort(Lane* h, int n_clouds, float inv_leaf, int skip_flagged, int idx_bits) {
   const int tiles_cap = (h->R + kVsTile - 1) / kVsTile;
   unsigned* hist = reinterpret_cast<unsigned*>(h->val_a);        // [clouds][256][tiles_cap]  (alloc_all sizes val_a for it)
   const int* chunk_cnt = reinterpret_cast<const int*>(h->val_b); // [clouds][64]

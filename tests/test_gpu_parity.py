@@ -646,6 +646,24 @@ def test_register_batch_enqueue_flush_pipelined(oracle):
         again = h.register_batch(batches[1], p)
         assert outs[0].tobytes() == ref[0].tobytes() and again.tobytes() == ref[1].tobytes()
         h.register_batch_flush()   # nothing in flight: a no-op
+        # solve_correspondences and set_stream flush as well: the queued record is the blocking call's, the solve's its own
+        import torch
+        one = h.register_batch(batches[0][:1], p)
+        a4, b4 = synth.matched_pairs(250, 500, inlier_ratio=0.3, noise=0.04)[:2]
+        solo, _ = h.solve_correspondences(a4, b4, p)
+        out1 = np.zeros(1, RESULT_DTYPE)
+        h.register_batch_enqueue_raw(arrs[0], 1, p, MEM_HOST, out1)
+        got, _ = h.solve_correspondences(a4, b4, p)
+        h.register_batch_flush()
+        assert out1.tobytes() == one.tobytes() and bytes(got) == bytes(solo)
+        side = torch.cuda.Stream()
+        out1[:] = 0
+        h.solve_correspondences(a4, b4, p)   # leaves the solve's record where the batch's will be copied from
+        h.register_batch_enqueue_raw(arrs[0], 1, p, MEM_HOST, out1)
+        h.set_stream(side.cuda_stream)
+        h.register_batch_flush()
+        h.set_stream(0)
+        assert out1.tobytes() == one.tobytes()
     r_ref, _ = oracle.register_pair(batches[0][0][0], batches[0][0][1], p)
     _same_record(ref[0][0], r_ref)
 
