@@ -107,13 +107,19 @@ typedef struct qb200_params {
  * 524288 raw points per cloud allocates 0.74 GB. */
 #define QB200_MAX_VOXEL_POINTS 262144
 
+/* Largest max_corr qb200_create accepts (2^15): correspondence ids, ranks and degrees fit 16 bits and the 2 x 32768 COTE events
+ * of a pair are tagged 0..65535.  A slot's two adjacency copies take max_corr^2 / 4 bytes (256 MB at 32768), so a handle of
+ * this capacity wants few slots.  Graphs and cliques above 8192 vertices keep their per-vertex k-core / clique arrays in a
+ * global-memory scratch of about 1.2 MB per slot, cliques above 4096 members the pose workspace (42 bytes per member). */
+#define QB200_MAX_CORR 32768
+
 /* Handle configuration: device and per-pair capacities (device workspaces are sized once). */
 typedef struct qb200_config {
   int32_t device;            /* CUDA ordinal */
   int32_t max_batch_slots;   /* pairs resident in one wave of the batch pipeline (default 64) */
   int32_t max_raw_points;    /* per cloud (default 131072) */
   int32_t max_voxel_points;  /* per cloud (default 16384; multiple of 128, <= QB200_MAX_VOXEL_POINTS) */
-  int32_t max_corr;          /* per pair  (default 4096; multiple of 32, <= 8192; the pose solver holds cliques of <= 4096) */
+  int32_t max_corr;          /* per pair  (default 4096; multiple of 32, <= QB200_MAX_CORR; cliques of any size up to max_corr) */
   int32_t reserved[3];
 } qb200_config;
 

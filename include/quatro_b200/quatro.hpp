@@ -25,7 +25,7 @@ struct HandleDeleter {
 using HandlePtr = std::unique_ptr<qb200_handle, HandleDeleter>;
 
 constexpr int kDefaultRawPoints = 262144;  // the example's loader reads at most 250 k points (run_global_registration.cpp:384-388)
-constexpr int kMaxCorr = 8192;              // qb200_config::max_corr limit
+constexpr int kMaxCorr = QB200_MAX_CORR;    // qb200_config::max_corr limit
 
 inline HandlePtr make_handle(int device = 0, int slots = 1, int max_voxel_points = 16384, int max_raw_points = kDefaultRawPoints,
                              int max_corr = 4096) {
@@ -56,7 +56,7 @@ inline SharedHandle& shared_state() {
 inline qb200_handle* shared_handle() { return shared_state().h.get(); }
 inline bool shared_handle_grown() { return shared_state().grown; }
 // pcl::VoxelGrid / FLANN have no capacity: when a scan or a match overflows the handle's capacities, the shared handle is rebuilt
-// with the largest ones (QB200_MAX_VOXEL_POINTS per cloud, 8192 correspondences) instead of handing truncated data to the next
+// with the largest ones (QB200_MAX_VOXEL_POINTS per cloud, QB200_MAX_CORR correspondences) instead of handing truncated data to the next
 // stage.  max_raw_points grows to n_raw (rounded up to a multiple of 65536) when a scan holds more points than the handle takes.
 inline qb200_handle* grow_shared_handle(size_t n_raw = 0) {
   SharedHandle& s = shared_state();

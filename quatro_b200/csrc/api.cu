@@ -154,6 +154,12 @@ int lane_alloc(const Lane& like, Lane** out) {
   QB_ALLOC(L, L->final_inl, S * Lc);
   QB_ALLOC(L, L->rot_mask, S * Lc);
   QB_ALLOC(L, L->trans_mask, S * Lc);
+  // workspaces of the pairs whose graph or clique outgrows the shared-memory layouts (clique.cu, pose.cu); only wide handles have them
+  if (Lc > (size_t)kKcoreSmemVerts) {
+    QB_ALLOC(L, L->kcore_ws, S * kcore_ws_bytes((int)Lc));
+    QB_ALLOC(L, L->chain_ws, S * kCliqueWarps * Lc);
+  }
+  if (Lc > (size_t)kPoseSmemClique) QB_ALLOC(L, L->pose_ws, S * pose_ws_bytes((int)Lc));
   QB_ALLOC(L, L->d_results, S);
   QB_CUDA_TRY(L, cudaMemset(L->d_results, 0, S * sizeof(qb200_result)));
   QB_CUDA_TRY(L, cudaMallocHost((void**)&L->h_results, S * sizeof(qb200_result)));
@@ -188,7 +194,7 @@ void lane_free(Lane* L) {
                       L->vox_start, L->vox_pts, L->cell_key, L->cell_start, L->normals, L->spfh, L->nbr_list, L->nbr_cnt, L->desc_t, L->rowbest, L->colpart, L->colbest,
                       L->desc_tiles, L->desc_norm, L->tc_fallback, L->tc_stats, L->aos_scratch,
                       L->mut_i, L->mut_j, L->mark, L->partner, L->mean, L->corr_src, L->corr_tgt, L->ma, L->mb, L->adj, L->adjp, L->deg,
-                      L->kcore, L->korder, L->rank_of, L->by_rank, L->kbin, L->clique, L->ex_stack, L->ex_pool, L->ex_lvl, L->ex_cur, L->pw_ints, L->pw_out, L->ip_buf, L->final_inl, L->rot_mask, L->trans_mask, L->d_results,
+                      L->kcore, L->korder, L->rank_of, L->by_rank, L->kbin, L->clique, L->ex_stack, L->ex_pool, L->ex_lvl, L->ex_cur, L->kcore_ws, L->chain_ws, L->pose_ws, L->pw_ints, L->pw_out, L->ip_buf, L->final_inl, L->rot_mask, L->trans_mask, L->d_results,
                       L->ctr_block};
   for (void* p : dev_ptrs)
     if (p) cudaFree(p);
@@ -609,7 +615,7 @@ int qb200_create(const qb200_config* cfg_in, qb200_handle** out) {
   if (cfg_in) cfg = *cfg_in; else qb200_default_config(&cfg);
   if (cfg.max_batch_slots < 1 || cfg.max_batch_slots > 2048 || cfg.max_raw_points < 1 || cfg.max_voxel_points < kMatchTile ||
       cfg.max_voxel_points % kMatchTile != 0 || cfg.max_voxel_points > QB200_MAX_VOXEL_POINTS || cfg.max_corr < 32 || cfg.max_corr % 32 != 0 ||
-      cfg.max_corr > 8192 || (long long)cfg.max_batch_slots * 2 * cfg.max_raw_points > 2000000000LL ||
+      cfg.max_corr > QB200_MAX_CORR || (long long)cfg.max_batch_slots * 2 * cfg.max_raw_points > 2000000000LL ||
       (long long)cfg.max_batch_slots * 2 * cfg.max_voxel_points > 2000000000LL)
     return QB200_ERR_BAD_ARG;
   int ndev = 0;

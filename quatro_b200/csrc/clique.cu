@@ -180,27 +180,36 @@ __device__ __forceinline__ int kcore_expand(const uint32_t (&w)[WPL], int w0, un
 //     different buckets commute, so the four warps apply their classes' events concurrently from their own `above` bitsets; a
 //     neighbour whose degree drops moves to the next lower class through a double-buffered `add` bitset that the receiving warp
 //     merges at the start of the next step -- ONE block barrier per step.  Rows arrive through a cp.async ring of kRing rows (warp 0 prefetches kRing - 1 steps ahead).
-// smem: bin (int x (Lc + 2)) | above [4][32 WPL] | add [2][4][32 WPL] | rows [row_words] | deg, pos, vert, mrk (u16 x Lc) | nbl [4][Lc] u16
-template <int WPL>
-__global__ void __launch_bounds__(kKcWarps * 32) kcore_kernel(const uint32_t* __restrict__ adj, const int* __restrict__ deg_in,
-                                                              const int* __restrict__ n_corr, int Lc, int W, int row_words, int* __restrict__ kcore,
+// smem: bin (int x (Ls + 2)) | above [4][32 WPL] | add [2][4][32 WPL] | rows [row_words] | deg, pos, vert, mrk (u16 x Ls) | nbl [4][Ls] u16,
+// Ls = min(Lc, kKcoreSmemVerts).  A pair with L > Ls keeps bin .. nbl in its slot of `ws` (kcore_ws_bytes(Lc) each, L2-resident) and
+// uses the whole shared area behind the bitsets as its prefetch ring: the same code runs on either set of arrays.  The two cases are
+// two instances (kWs = false: pairs with L <= Ls, true: the others), so every array access keeps its address space (LDS / LDG).
+template <int WPL, bool kWs>
+__global__ void __maxnreg__(168) kcore_kernel(const uint32_t* __restrict__ adj, const int* __restrict__ deg_in,
+                                                              const int* __restrict__ n_corr, int Lc, int W, int Ls, int row_words,
+                                                              unsigned char* __restrict__ ws, int* __restrict__ kcore,
                                                               int* __restrict__ korder, int* __restrict__ rank_of, int* __restrict__ by_rank,
                                                               int* __restrict__ kbin, int* __restrict__ max_core_out) {
   constexpr int NW = kKcWarps, AW = 32 * WPL;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  int* bin = reinterpret_cast<int*>(smem_raw);                       // [Lc + 2] start of every degree bucket
-  uint32_t* above = reinterpret_cast<uint32_t*>(bin + Lc + 2);       // [NW][AW] vertices with current degree > current level (per class)
-  uint32_t* add = above + NW * AW;                                   // [2][NW][AW] arrivals of the next step, by parity
-  uint32_t* rows = add + 2 * NW * AW;                                // [row_words] adjacency cache or prefetch ring
-  unsigned short* deg = reinterpret_cast<unsigned short*>(rows + row_words);
-  unsigned short* pos = deg + Lc;
-  unsigned short* vert = pos + Lc;
-  unsigned short* mrk = vert + Lc;                                   // mrk[u] = 1 + rank of u inside its group during a pass, else 0
-  unsigned short* nbl_all = mrk + Lc;                                // [NW][Lc] ascending list of a warp's live neighbours of the step
   __shared__ int ring_tag[kRing];
 
   const int pair = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int L = n_corr[pair];
+  if ((L > Ls) != kWs) return;                                       // the other instance runs this pair
+  constexpr bool in_smem = !kWs;
+  const int Lv = in_smem ? Ls : Lc;                                  // capacity of the per-vertex arrays
+  int* bin = in_smem ? reinterpret_cast<int*>(smem_raw)              // [Lv + 2] start of every degree bucket
+                     : reinterpret_cast<int*>(ws + (size_t)pair * kcore_ws_bytes(Lc));
+  uint32_t* above = in_smem ? reinterpret_cast<uint32_t*>(bin + Ls + 2)  // [NW][AW] vertices with current degree > current level (per class)
+                            : reinterpret_cast<uint32_t*>(smem_raw);
+  uint32_t* add = above + NW * AW;                                   // [2][NW][AW] arrivals of the next step, by parity
+  uint32_t* rows = add + 2 * NW * AW;                                // [row_words] adjacency cache or prefetch ring
+  unsigned short* deg = in_smem ? reinterpret_cast<unsigned short*>(rows + row_words) : reinterpret_cast<unsigned short*>(bin + Lc + 2);
+  unsigned short* pos = deg + Lv;
+  unsigned short* vert = pos + Lv;
+  unsigned short* mrk = vert + Lv;                                   // mrk[u] = 1 + rank of u inside its group during a pass, else 0
+  unsigned short* nbl_all = mrk + Lv;                                // [NW][Lv] ascending list of a warp's live neighbours of the step
   int* __restrict__ kc = kcore + (size_t)pair * (Lc + 2);
   int* __restrict__ ko = korder + (size_t)pair * (Lc + 2);
   int* __restrict__ ro = rank_of + (size_t)pair * (Lc + 2);
@@ -213,9 +222,10 @@ __global__ void __launch_bounds__(kKcWarps * 32) kcore_kernel(const uint32_t* __
   const uint32_t* __restrict__ G = adj + (size_t)pair * Lc * W;
   const int nbw = (L + 31) >> 5;   // adjacency words per row in use
   const int nwl = (nbw + 31) >> 5; // words per lane in use (<= WPL)
-  const bool cached = (long long)L * nbw <= (long long)row_words;
+  const bool cached = in_smem && (long long)L * nbw <= (long long)row_words;
+  const int rs = in_smem ? Ls / 32 : W;  // row stride of the prefetch ring (>= nbw)
   const int w0 = lane * nwl;       // first adjacency word of this lane
-  unsigned short* nbl = nbl_all + (size_t)warp * Lc;
+  unsigned short* nbl = nbl_all + (size_t)warp * Lv;
 
   // ---- set-up: degrees, row cache, bucket sort by degree (warp 0 sorts; everybody helps loading) ----
   int md = 0;
@@ -276,7 +286,7 @@ __global__ void __launch_bounds__(kKcWarps * 32) kcore_kernel(const uint32_t* __
         if (lane == 0) ring_tag[sl] = x;
 #pragma unroll
         for (int k = 0; k < WPL; ++k)
-          if (k < nwl && w0 + k < nbw) cp_async4(rows + sl * W + w0 + k, G + (size_t)x * W + w0 + k);
+          if (k < nwl && w0 + k < nbw) cp_async4(rows + sl * rs + w0 + k, G + (size_t)x * W + w0 + k);
       }
       cp_async_commit();
     };
@@ -301,7 +311,7 @@ __global__ void __launch_bounds__(kKcWarps * 32) kcore_kernel(const uint32_t* __
         if (k < nwl && w0 + k < nbw) {
           const uint32_t a = add_in[w0 + k];
           if (a) { above_w[w0 + k] |= a; add_in[w0 + k] = 0u; }
-          w[k] = hit ? rows[sl * W + w0 + k] : G[(size_t)v * W + w0 + k];
+          w[k] = hit ? rows[sl * rs + w0 + k] : G[(size_t)v * W + w0 + k];
         }
       }
       __syncwarp();
@@ -376,8 +386,6 @@ __global__ void __launch_bounds__(256) permute_adj_kernel(const uint32_t* __rest
   for (int w = lane; w < nb; w += 32) dst[w] = row[w];  // the descent never reads beyond ceil(L/32) words
 }
 
-constexpr int kCliqueWarps = 8;
-
 // One greedy descent by one warp in rank space.  P = candidates of start vertex rv with rank >= thr; returns the chain
 // length + 1 (the start vertex), or 0 when |P| <= mc.  WPL = adjacency words per lane.
 template <int WPL>
@@ -418,8 +426,10 @@ __device__ __forceinline__ int clique_descent(const uint32_t* __restrict__ rows,
 }
 
 // One CTA (8 warps) per pair: PMC heuristic in rank space, start vertices tried speculatively by the warps and committed
-// in sequential order.  smem: chains [8][Lc] u16, ids bitset [W], adjacency cache [cache_words].
+// in sequential order.  smem: chains [8][Ls] u16 (Ls = min(Lc, kKcoreSmemVerts)), ids bitset [W], adjacency cache [cache_words].
+// A pair with L > Ls keeps its chains in its slot of chain_ws ([8][Lc] u16 per pair).
 __global__ void __launch_bounds__(kCliqueWarps * 32) clique_cta_kernel(const uint32_t* __restrict__ adjp, const int* __restrict__ n_corr, int Lc, int W,
+                                                                       int Ls, unsigned short* __restrict__ chain_ws,
                                                                        const int* __restrict__ kcore, const int* __restrict__ korder,
                                                                        const int* __restrict__ rank_of, const int* __restrict__ by_rank,
                                                                        const int* __restrict__ kbin, const int* __restrict__ max_core_in, int mode,
@@ -427,13 +437,15 @@ __global__ void __launch_bounds__(kCliqueWarps * 32) clique_cta_kernel(const uin
                                                                        int* __restrict__ n_clique) {
   constexpr int NT = kCliqueWarps * 32;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  unsigned short* chains = reinterpret_cast<unsigned short*>(smem_raw);       // [8][Lc]
-  uint32_t* idbits = reinterpret_cast<uint32_t*>(chains + (size_t)kCliqueWarps * Lc);  // [W]
+  uint32_t* idbits = reinterpret_cast<uint32_t*>(smem_raw + (size_t)kCliqueWarps * Ls * sizeof(unsigned short));  // [W]
   uint32_t* cache = idbits + W;                                                // [cache_words]
   __shared__ int s_sz[kCliqueWarps];
   __shared__ int s_scan[33];
   const int pair = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int L = n_corr[pair];
+  const bool in_smem = L <= Ls;
+  unsigned short* chains = in_smem ? reinterpret_cast<unsigned short*>(smem_raw) : chain_ws + (size_t)pair * kCliqueWarps * Lc;
+  const int Lv = in_smem ? Ls : Lc;  // chain capacity
   int* __restrict__ out = clique + (size_t)pair * Lc;
   if (L <= 0) {
     if (tid == 0) n_clique[pair] = 0;
@@ -462,7 +474,7 @@ __global__ void __launch_bounds__(kCliqueWarps * 32) clique_cta_kernel(const uin
       for (int idx = tid; idx < L * nbw; idx += NT) cache[idx] = G[(size_t)(idx / nbw) * W + (idx % nbw)];
     const uint32_t* rows = cached ? cache : G;
     const int stride = cached ? nbw : W;
-    unsigned short* chain = chains + (size_t)warp * Lc;
+    unsigned short* chain = chains + (size_t)warp * Lv;
     const int ub = max_core + 1;  // src/graph.cc:84-86
     int mc = 0, i = L - 1;
     __syncthreads();
@@ -479,7 +491,9 @@ __global__ void __launch_bounds__(kCliqueWarps * 32) clique_cta_kernel(const uin
           const int rv = ro[v];
           if (nwl == 1) sz = clique_descent<1>(rows, stride, nbw, rv, thr, mc, chain);
           else if (nwl <= 4) sz = clique_descent<4>(rows, stride, nbw, rv, thr, mc, chain);
-          else sz = clique_descent<8>(rows, stride, nbw, rv, thr, mc, chain);
+          else if (nwl <= 8) sz = clique_descent<8>(rows, stride, nbw, rv, thr, mc, chain);
+          else if (nwl <= 16) sz = clique_descent<16>(rows, stride, nbw, rv, thr, mc, chain);
+          else sz = clique_descent<32>(rows, stride, nbw, rv, thr, mc, chain);
         }
       }
       if (lane == 0) s_sz[warp] = sz;
@@ -546,10 +560,14 @@ __global__ void __launch_bounds__(kCliqueWarps * 32) clique_cta_kernel(const uin
 // node_limit expanded nodes (QB200_FLAG_CLIQUE_TRUNCATED).  The warp keeps a candidate set as WPL words per lane (word index
 // lane + 32 k, like clique_descent); the level stack -- one candidate bitset and one (rank | colour << 16) list segment per
 // depth -- lives in global scratch (L1/L2-resident: the live part is a few KB), rows come from the shared-memory adjacency cache
-// when the graph fits.  Stack or list-pool exhaustion ends the search like the node limit does.
+// when the graph fits.  Stack or list-pool exhaustion ends the search like the node limit does.  Both limits exist on the device
+// only (the CPU search grows its stack): a search that would go deeper than kExactDepth levels, or whose lists on the current path
+// hold more than kExactPool entries, stops with QB200_FLAG_CLIQUE_TRUNCATED and the best clique found so far.  The root list (at
+// most L entries) always fits.
 // ------------------------------------------------------------------------------------------------
 constexpr int kExactDepth = 1024;      // levels of the stack (a clique larger than this ends the search with the truncation flag)
 constexpr int kExactPool = 1 << 17;    // list entries per pair
+static_assert(kExactPool >= QB200_MAX_CORR, "the root colour list of a pair must fit into the list pool");
 constexpr int kExactChunk = 64;        // pairs searched by one launch (the scratch is sized for these, not for max_batch_slots)
 
 template <int WPL>
@@ -727,16 +745,27 @@ constexpr size_t kKcoreSmemBudget = 144 * 1024;
 template <int WPL>
 static int launch_kcore(Lane* h, int n_pairs) {
   const int Lc = h->Lc, W = h->W;
-  const size_t fixed = (size_t)(Lc + 2) * sizeof(int) + (size_t)3 * kKcWarps * 32 * WPL * sizeof(uint32_t) +
-                       (size_t)(4 + kKcWarps) * Lc * sizeof(unsigned short);
+  const int Ls = Lc < kKcoreSmemVerts ? Lc : kKcoreSmemVerts, Ws = Ls / 32;  // vertices / row words of the shared-memory layout
+  const size_t bits = (size_t)3 * kKcWarps * 32 * WPL * sizeof(uint32_t);
+  const size_t fixed = (size_t)(Ls + 2) * sizeof(int) + bits + (size_t)(4 + kKcWarps) * Ls * sizeof(unsigned short);
   // rows: what is left of the budget, at least the prefetch ring
   size_t row_words = fixed + 8 * 1024 < kKcoreSmemBudget ? (kKcoreSmemBudget - fixed) / 4 : 0;
-  if (row_words < (size_t)kRing * W) row_words = (size_t)kRing * W;
-  if (row_words > (size_t)Lc * W) row_words = (size_t)Lc * W;
+  if (row_words < (size_t)kRing * Ws) row_words = (size_t)kRing * Ws;
+  if (row_words > (size_t)Ls * Ws) row_words = (size_t)Ls * Ws;
   const size_t smem = fixed + row_words * 4;
-  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)kcore_kernel<WPL>, smem));
-  kcore_kernel<WPL><<<n_pairs, kKcWarps * 32, smem, h->stream>>>(h->adj, h->deg, h->ctr.n_corr, Lc, W, (int)row_words, h->kcore, h->korder,
-                                                                 h->rank_of, h->by_rank, h->kbin, h->ctr.max_core);
+  if (Ls < Lc && smem - bits < (size_t)kRing * W * 4) {  // a pair above Ls streams full-width rows through the area behind the bitsets
+    h->fail(__FILE__, __LINE__, "k-core prefetch ring does not fit");
+    return QB200_ERR_CUDA;
+  }
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)kcore_kernel<WPL, false>, smem));
+  kcore_kernel<WPL, false><<<n_pairs, kKcWarps * 32, smem, h->stream>>>(h->adj, h->deg, h->ctr.n_corr, Lc, W, Ls, (int)row_words, h->kcore_ws,
+                                                                        h->kcore, h->korder, h->rank_of, h->by_rank, h->kbin, h->ctr.max_core);
+  if (Ls < Lc) {  // pairs above the shared-memory layout: same shared-memory size, per-vertex arrays in kcore_ws
+    QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)kcore_kernel<WPL, true>, smem));
+    kcore_kernel<WPL, true><<<n_pairs, kKcWarps * 32, smem, h->stream>>>(h->adj, h->deg, h->ctr.n_corr, Lc, W, Ls, (int)row_words, h->kcore_ws,
+                                                                         h->kcore, h->korder, h->rank_of, h->by_rank, h->kbin, h->ctr.max_core);
+    h->launches++;
+  }
   return QB200_OK;
 }
 
@@ -768,30 +797,36 @@ static int launch_exact(Lane* h, int n_pairs, long long node_limit, int cache_wo
 int launch_clique(Lane* h, int n_pairs, int mode, double kcore_thr, long long node_limit) {
   if (n_pairs <= 0) return QB200_OK;
   const int Lc = h->Lc, W = h->W;
+  const int Ls = Lc < kKcoreSmemVerts ? Lc : kKcoreSmemVerts;
   // shared-memory adjacency cache of the descent: 14336 words (56 KB) hold graphs up to L ~ 660
   const int cache_words = 14336;
-  const size_t sm_clique = (size_t)kCliqueWarps * Lc * sizeof(unsigned short) + (size_t)W * sizeof(uint32_t) + (size_t)cache_words * 4;
+  const size_t sm_clique = (size_t)kCliqueWarps * Ls * sizeof(unsigned short) + (size_t)W * sizeof(uint32_t) + (size_t)cache_words * 4;
   int rc;
   QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)clique_cta_kernel, sm_clique));
   if (mode == QB200_PMC_EXACT && (rc = ensure_exact_scratch(h))) return rc;
   if (W <= 32) rc = launch_kcore<1>(h, n_pairs);
   else if (W <= 64) rc = launch_kcore<2>(h, n_pairs);
   else if (W <= 128) rc = launch_kcore<4>(h, n_pairs);
-  else rc = launch_kcore<8>(h, n_pairs);
+  else if (W <= 256) rc = launch_kcore<8>(h, n_pairs);
+  else if (W <= 512) rc = launch_kcore<16>(h, n_pairs);
+  else rc = launch_kcore<32>(h, n_pairs);
   if (rc) return rc;
   const dim3 gp((Lc + 7) / 8, n_pairs);
   permute_adj_kernel<<<gp, 256, 8 * W * sizeof(uint32_t), h->stream>>>(h->adj, h->ctr.n_corr, Lc, W, h->rank_of, h->adjp);
   // PMC_EXACT starts from the heuristic clique (graph.cc:88-104: in.lb = pmc_heu.search, returned as is when lb == ub)
-  clique_cta_kernel<<<n_pairs, kCliqueWarps * 32, sm_clique, h->stream>>>(h->adjp, h->ctr.n_corr, Lc, W, h->kcore, h->korder, h->rank_of, h->by_rank,
-                                                                          h->kbin, h->ctr.max_core, mode == QB200_PMC_EXACT ? QB200_PMC_HEU : mode,
-                                                                          kcore_thr, cache_words, h->clique, h->ctr.n_clique);
+  clique_cta_kernel<<<n_pairs, kCliqueWarps * 32, sm_clique, h->stream>>>(h->adjp, h->ctr.n_corr, Lc, W, Ls, h->chain_ws, h->kcore, h->korder,
+                                                                          h->rank_of, h->by_rank, h->kbin, h->ctr.max_core,
+                                                                          mode == QB200_PMC_EXACT ? QB200_PMC_HEU : mode, kcore_thr, cache_words,
+                                                                          h->clique, h->ctr.n_clique);
   h->launches += 3;
   if (mode == QB200_PMC_EXACT) {
     const long long lim = node_limit > 0 ? node_limit : (long long)QB200_DEFAULT_CLIQUE_NODE_LIMIT;
     if (W <= 32) rc = launch_exact<1>(h, n_pairs, lim, cache_words);
     else if (W <= 64) rc = launch_exact<2>(h, n_pairs, lim, cache_words);
     else if (W <= 128) rc = launch_exact<4>(h, n_pairs, lim, cache_words);
-    else rc = launch_exact<8>(h, n_pairs, lim, cache_words);
+    else if (W <= 256) rc = launch_exact<8>(h, n_pairs, lim, cache_words);
+    else if (W <= 512) rc = launch_exact<16>(h, n_pairs, lim, cache_words);
+    else rc = launch_exact<32>(h, n_pairs, lim, cache_words);
     if (rc) return rc;
   }
   QB_CUDA_TRY(h, cudaGetLastError());

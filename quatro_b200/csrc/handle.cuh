@@ -71,6 +71,9 @@ struct Lane {
   uint32_t *ex_stack, *ex_pool;  // PMC_EXACT scratch, allocated on first use: [min(S,64)*1024*W] candidate sets per level, [min(S,64)*2^17] list entries
   int* ex_lvl;                // [2*min(S,64)*1024] list segment (begin | remaining) per level
   unsigned short* ex_cur;     // [min(S,64)*1024] clique under construction (ranks)
+  unsigned char* kcore_ws;    // [S * kcore_ws_bytes(Lc)] k-core arrays of graphs above kKcoreSmemVerts vertices (Lc > kKcoreSmemVerts only)
+  unsigned short* chain_ws;   // [S*8*Lc] descent chains of those graphs (Lc > kKcoreSmemVerts only)
+  unsigned char* pose_ws;     // [S * pose_ws_bytes(Lc)] pose workspace of cliques above kPoseSmemClique members (Lc > kPoseSmemClique only)
   int* final_inl;             // [S*Lc]
   unsigned char *rot_mask, *trans_mask;  // [S*Lc]
   // ---- pre-processing (preprocess.cu), allocated on first use ----
@@ -135,6 +138,17 @@ struct qb200_handle {
 };
 
 namespace qb {
+
+// Per-pair choice between shared memory and global scratch (clique.cu, pose.cu): a graph of up to kKcoreSmemVerts vertices keeps its
+// k-core and clique arrays in shared memory, a clique of up to kPoseSmemClique members its pose workspace.  The layouts are sized
+// for min(Lc, limit), so a wide handle launches with about the shared memory of an 8192 handle and its small pairs keep their arrays
+// in shared memory.
+constexpr int kKcoreSmemVerts = 8192;
+constexpr int kPoseSmemClique = 4096;
+constexpr int kCliqueWarps = 8;
+// bin (int x (Lc + 2)) | deg, pos, vert, mrk (u16 x Lc) | nbl [4][Lc] u16, 16-byte aligned
+__host__ __device__ inline size_t kcore_ws_bytes(int Lc) { return ((size_t)(Lc + 2) * 4 + (size_t)8 * Lc * 2 + 15) & ~(size_t)15; }
+size_t pose_ws_bytes(int Lc);
 
 // Stage launchers (each enqueues kernels on the lane's stream for clouds/pairs [0, n) of its current wave).
 int launch_voxel(Lane* h, int n_clouds, float leaf, int skip_flagged);

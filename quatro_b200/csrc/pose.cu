@@ -8,8 +8,9 @@
 //
 //  * svdRot2d: for a 2x2 correlation H = sum w x y^T the rotation V U^T (with the det fix) is the
 //    maximiser of trace(R H), i.e. yaw = atan2(H01 - H10, H00 + H11): no SVD is needed.
-//  * COTE: the 2c interval end points are sorted with an in-shared-memory bitonic network on the key
-//    (value, insertion index) -- the total order a stable sort by value produces -- and the running
+//  * COTE: the 2c interval end points are sorted with a bitonic network on the key (value, insertion index) -- the total
+//    order a stable sort by value produces -- in shared memory, or for cliques of more than kPoseSmemClique members in a
+//    global-memory workspace of the pair (same code, L2-resident) -- and the running
 //    sums of the sweep are then accumulated sequentially by one thread in exactly the reference's
 //    order, so the argmin and the "median" candidate set follow the CPU path.
 #include "handle.cuh"
@@ -45,6 +46,15 @@ __device__ __forceinline__ double block_max(double v, double* scratch) {
   return t;
 }
 
+static int next_pow2(int n) {
+  int p = 32;
+  while (p < n) p <<= 1;
+  return p;
+}
+__host__ __device__ inline size_t pose_smem_bytes(int Lp) {
+  return (size_t)4 * Lp * sizeof(double) + (size_t)4 * Lp * sizeof(unsigned short) + (size_t)2 * Lp;
+}
+
 // ascending bitonic sort of n2 (power of two) keys (val, tag); every thread of the block calls it
 __device__ void bitonic_sort(double* val, unsigned short* tag, int n2) {
   for (int k = 2; k <= n2; k <<= 1) {
@@ -67,22 +77,14 @@ __device__ void bitonic_sort(double* val, unsigned short* tag, int n2) {
   }
 }
 
+template <bool kWs>
 __global__ void __launch_bounds__(kPoseThreads) pose_kernel(const float4* __restrict__ ma, const float4* __restrict__ mb, const int* __restrict__ n_corr,
-                                                            int Lc, int Lp, const int* __restrict__ clique_all, const int* __restrict__ n_clique, PoseParams pp,
+                                                            int Lc, int Lp, int Lg, unsigned char* __restrict__ ws, const int* __restrict__ clique_all,
+                                                            const int* __restrict__ n_clique, PoseParams pp,
                                                             qb200_result* __restrict__ results, unsigned char* __restrict__ rot_mask_out,
                                                             unsigned char* __restrict__ trans_mask_out, int* __restrict__ final_inl,
                                                             int* __restrict__ n_final) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  // layout (Lp = capacity rounded up to a power of two so the bitonic networks fit):
-  //   ev[2Lp] f64 | wX[Lp] f64 | aux[Lp] f64 | tag[2Lp] u16 | ctag[Lp] u16 | list[Lp] u16 | rm[Lp] u8 | tm[Lp] u8
-  double* ev = reinterpret_cast<double*>(smem_raw);
-  double* wX = ev + 2 * Lp;
-  double* aux = wX + Lp;
-  unsigned short* tag = reinterpret_cast<unsigned short*>(aux + Lp);
-  unsigned short* ctag = tag + 2 * Lp;
-  unsigned short* list = ctag + Lp;
-  unsigned char* rm = reinterpret_cast<unsigned char*>(list + Lp);
-  unsigned char* tm = rm + Lp;
   __shared__ double scratch[kPoseThreads / 32];
   __shared__ double s_bcast[4];
   __shared__ int s_ibcast[4];
@@ -91,6 +93,20 @@ __global__ void __launch_bounds__(kPoseThreads) pose_kernel(const float4* __rest
   const int pair = blockIdx.x, tid = threadIdx.x;
   const int L = n_corr[pair];
   const int c = n_clique[pair];
+  if ((c > Lp) != kWs) return;  // the other instance solves this pair
+  // workspace of Lq = power-of-two capacity (so the bitonic networks fit): shared memory (Lp) for cliques of up to Lp members, else
+  // the pair's slot of ws (Lg = next_pow2(Lc)).  At Lq = 32768 the 65536 COTE events fill the u16 tags 0..65535 without padding.
+  //   ev[2Lq] f64 | wX[Lq] f64 | aux[Lq] f64 | tag[2Lq] u16 | ctag[Lq] u16 | list[Lq] u16 | rm[Lq] u8 | tm[Lq] u8
+  constexpr bool in_smem = !kWs;
+  const int Lq = in_smem ? Lp : Lg;
+  double* ev = reinterpret_cast<double*>(in_smem ? smem_raw : ws + (size_t)pair * pose_smem_bytes(Lg));
+  double* wX = ev + 2 * Lq;
+  double* aux = wX + Lq;
+  unsigned short* tag = reinterpret_cast<unsigned short*>(aux + Lq);
+  unsigned short* ctag = tag + 2 * Lq;
+  unsigned short* list = ctag + Lq;
+  unsigned char* rm = reinterpret_cast<unsigned char*>(list + Lq);
+  unsigned char* tm = rm + Lq;
   const float4* __restrict__ A = ma + (size_t)pair * Lc;
   const float4* __restrict__ B = mb + (size_t)pair * Lc;
   const int* __restrict__ cl = clique_all + (size_t)pair * Lc;
@@ -100,17 +116,6 @@ __global__ void __launch_bounds__(kPoseThreads) pose_kernel(const float4* __rest
     if (tid == 0) {
       res->valid = 0;
       res->status = (L < 2) ? QB200_DEGENERATE_INPUT : QB200_DEGENERATE_CLIQUE;
-      res->clique_size = c; res->gnc_iters = 0; res->n_rot_inliers = 0; res->n_final_inliers = 0; res->cost = 0.0;
-      for (int i = 0; i < 16; ++i) res->T[i] = (i % 5 == 0) ? 1.0 : 0.0;
-      n_final[pair] = 0;
-    }
-    return;
-  }
-
-  if (c > Lp) {  // the solver workspace holds 4096 clique members (max_corr may be 8192): report, do not truncate
-    if (tid == 0) {
-      res->valid = 0;
-      res->status = QB200_CAPACITY_EXCEEDED;
       res->clique_size = c; res->gnc_iters = 0; res->n_rot_inliers = 0; res->n_final_inliers = 0; res->cost = 0.0;
       for (int i = 0; i < 16; ++i) res->T[i] = (i % 5 == 0) ? 1.0 : 0.0;
       n_final[pair] = 0;
@@ -352,12 +357,7 @@ __global__ void iota_clique_kernel(const int* __restrict__ n_corr, int Lc, int* 
   if (i == 0) { n_clique[pair] = L; max_core[pair] = 0; }
 }
 
-static int next_pow2(int n) {
-  int p = 32;
-  while (p < n) p <<= 1;
-  return p;
-}
-size_t pose_smem_bytes(int Lp) { return (size_t)4 * Lp * sizeof(double) + (size_t)4 * Lp * sizeof(unsigned short) + (size_t)2 * Lp; }
+size_t pose_ws_bytes(int Lc) { return pose_smem_bytes(next_pow2(Lc)); }
 
 int launch_pose(Lane* h, int n_pairs, const qb200_params& p) {
   if (n_pairs <= 0) return QB200_OK;
@@ -371,12 +371,19 @@ int launch_pose(Lane* h, int n_pairs, const qb200_params& p) {
   pp.use_rot_inliers = p.using_rot_inliers_when_estimating_cote;
   pp.use_RyRx = p.use_pre_estimated_RyRx;
   for (int i = 0; i < 9; ++i) pp.RyRx[i] = p.RyRx[i];
-  const int Lp = next_pow2(h->Lc < 4096 ? h->Lc : 4096);
+  const int Lp = next_pow2(h->Lc < kPoseSmemClique ? h->Lc : kPoseSmemClique);
   const size_t smem = pose_smem_bytes(Lp);
-  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)pose_kernel, smem));
-  pose_kernel<<<n_pairs, kPoseThreads, smem, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, h->Lc, Lp, h->clique, h->ctr.n_clique, pp, h->d_results,
-                                                          h->rot_mask, h->trans_mask, h->final_inl, h->ctr.n_final);
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)pose_kernel<false>, smem));
+  pose_kernel<false><<<n_pairs, kPoseThreads, smem, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, h->Lc, Lp, next_pow2(h->Lc), h->pose_ws, h->clique,
+                                                                 h->ctr.n_clique, pp, h->d_results, h->rot_mask, h->trans_mask, h->final_inl,
+                                                                 h->ctr.n_final);
   h->launches++;
+  if (h->Lc > kPoseSmemClique) {  // cliques above Lp members: the same code on the pair's slot of pose_ws
+    pose_kernel<true><<<n_pairs, kPoseThreads, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, h->Lc, Lp, next_pow2(h->Lc), h->pose_ws, h->clique,
+                                                               h->ctr.n_clique, pp, h->d_results, h->rot_mask, h->trans_mask, h->final_inl,
+                                                               h->ctr.n_final);
+    h->launches++;
+  }
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;
 }
