@@ -70,144 +70,120 @@ __global__ void cache_copy_kernel(int to_cache, const int* __restrict__ slot_of_
   }
 }
 
-template <class T>
-cudaError_t dalloc(T** p, size_t count) {
-  return cudaMalloc(reinterpret_cast<void**>(p), count * sizeof(T));
+// Carve the counter block at `base` into *c and return its size in ints; base == nullptr only counts.  One int block, so a wave
+// reset is a single launch.  n_edges (long long) comes first, at an 8-byte offset; two spare ints close the block.
+size_t carve_counters(int* base, size_t S, WaveCounters* c) {
+  const size_t C = 2 * S;
+  size_t n = 0;
+  auto take = [&](size_t k) {
+    int* p = base ? base + n : nullptr;
+    n += k;
+    return p;
+  };
+  c->n_edges = reinterpret_cast<long long*>(take(2 * S));
+  c->n_valid = take(C);
+  c->n_vox = take(C);
+  c->n_lat = take(C);
+  c->n_cells = take(C);
+  c->cloud_status = take(C);
+  c->bbox = take(C * 6);
+  c->n_mutual = take(S);
+  c->n_corr = take(S);
+  c->swapped = take(S);
+  c->n_clique = take(S);
+  c->max_core = take(S);
+  c->n_final = take(S);
+  c->flags = take(S);
+  return n + 2;
 }
 
-#define QB_ALLOC(h, ptr, count)                                                    \
-  do {                                                                             \
-    cudaError_t _e = dalloc(&(ptr), (size_t)(count));                              \
-    if (_e != cudaSuccess) {                                                       \
-      (h)->fail(__FILE__, __LINE__, cudaGetErrorString(_e));                       \
-      return QB200_ERR_CUDA;                                                       \
-    }                                                                              \
-  } while (0)
-
-// A new lane with the settings of `like` (dims, device, n_sm, matcher switch, error sink), its own stream and every buffer of
-// DESIGN §4.  *out is set first, so lane_free releases whatever a failed allocation left behind.
-int lane_alloc(const Lane& like, Lane** out) {
-  Lane* L = *out = new (std::nothrow) Lane();
+// A new lane in *out with the settings of `like` (dims, device, n_sm, matcher switch, error sink), its own stream and every
+// buffer of DESIGN §4.  On failure *out is left as it was.
+int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
+  std::unique_ptr<Lane> L(new (std::nothrow) Lane());
   if (!L) return QB200_ERR_CUDA;
   L->S = like.S; L->R = like.R; L->V = like.V; L->Lc = like.Lc; L->W = like.W; L->NS = like.NS;
   L->device = like.device; L->n_sm = like.n_sm; L->force_exact_match = like.force_exact_match; L->err = like.err;
-  QB_CUDA_TRY(L, cudaStreamCreateWithFlags(&L->own_stream, cudaStreamNonBlocking));
+  QB_CUDA_TRY(L, L->own_stream.create(cudaStreamNonBlocking));
   L->stream = L->own_stream;
   const size_t S = L->S, R = L->R, V = L->V, Lc = L->Lc, W = L->W, C = 2 * S;
-  QB_CUDA_TRY(L, cudaMalloc((void**)&L->d_cloud_ptr, C * sizeof(float4*)));
-  QB_ALLOC(L, L->d_cloud_n, C);
-  QB_ALLOC(L, L->d_raw_off, C + 1);
-  QB_CUDA_TRY(L, cudaMallocHost((void**)&L->h_cloud_ptr, C * sizeof(float4*)));
-  QB_CUDA_TRY(L, cudaMallocHost((void**)&L->h_cloud_n, C * sizeof(int)));
-  QB_CUDA_TRY(L, cudaMallocHost((void**)&L->h_raw_off, (C + 1) * sizeof(int)));
-  QB_ALLOC(L, L->raw_stage, C * R);
+  QB_CUDA_TRY(L, L->d_cloud_ptr.alloc(C));
+  QB_CUDA_TRY(L, L->d_cloud_n.alloc(C));
+  QB_CUDA_TRY(L, L->d_raw_off.alloc(C + 1));
+  QB_CUDA_TRY(L, L->h_cloud_ptr.alloc(C));
+  QB_CUDA_TRY(L, L->h_cloud_n.alloc(C));
+  QB_CUDA_TRY(L, L->h_raw_off.alloc(C + 1));
+  QB_CUDA_TRY(L, L->raw_stage.alloc(C * R));
   // the sort workspace serves the voxel sort (C*R items, digit histograms in val_a, chunk counts C*kVsChunks <= n_sort in val_b),
   // the lattice / norm sorts (C*V items) and, afterwards, the duplicate-class tables of K6 (2S*V + 2S words in key_a): size it for
   // the largest user
   const size_t n_sort = C * (R > V ? R : V) + 64;
   const size_t n_hist = C * 256 * ((R + kVsTile - 1) / kVsTile);
-  QB_ALLOC(L, L->key_a, n_sort);
-  QB_ALLOC(L, L->key_b, n_sort);
-  QB_ALLOC(L, L->val_a, n_sort > n_hist ? n_sort : n_hist);
-  QB_ALLOC(L, L->val_b, n_sort);
-  QB_ALLOC(L, L->aos_scratch, 2 * V * kDescDim);
+  QB_CUDA_TRY(L, L->key_a.alloc(n_sort));
+  QB_CUDA_TRY(L, L->key_b.alloc(n_sort));
+  QB_CUDA_TRY(L, L->val_a.alloc(n_sort > n_hist ? n_sort : n_hist));
+  QB_CUDA_TRY(L, L->val_b.alloc(n_sort));
+  QB_CUDA_TRY(L, L->aos_scratch.alloc(2 * V * kDescDim));
   // the library radix sort only sorts lattice / norm keys of clouds too large for cloud_sort_kernel: at most C*V items
   L->cub_bytes = sort_temp_bytes((int)(C * V));
-  QB_CUDA_TRY(L, cudaMalloc(&L->cub_temp, L->cub_bytes));
-  QB_ALLOC(L, L->vox_start, C * (V + 1));
-  QB_ALLOC(L, L->vox_pts, C * V);
-  QB_ALLOC(L, L->cell_key, C * V);
-  QB_ALLOC(L, L->cell_start, C * (V + 1));
-  QB_ALLOC(L, L->normals, C * V);
-  QB_ALLOC(L, L->spfh, C * V * kDescPad);
-  QB_ALLOC(L, L->nbr_list, C * kNbrGlobalCap * V);
-  QB_ALLOC(L, L->nbr_cnt, C * V);
-  QB_ALLOC(L, L->desc_t, C * kDescK * V);
+  QB_CUDA_TRY(L, L->cub_temp.alloc_bytes(L->cub_bytes));
+  QB_CUDA_TRY(L, L->vox_start.alloc(C * (V + 1)));
+  QB_CUDA_TRY(L, L->vox_pts.alloc(C * V));
+  QB_CUDA_TRY(L, L->cell_key.alloc(C * V));
+  QB_CUDA_TRY(L, L->cell_start.alloc(C * (V + 1)));
+  QB_CUDA_TRY(L, L->normals.alloc(C * V));
+  QB_CUDA_TRY(L, L->spfh.alloc(C * V * kDescPad));
+  QB_CUDA_TRY(L, L->nbr_list.alloc(C * kNbrGlobalCap * V));
+  QB_CUDA_TRY(L, L->nbr_cnt.alloc(C * V));
+  QB_CUDA_TRY(L, L->desc_t.alloc(C * kDescK * V));
   QB_CUDA_TRY(L, cudaMemset(L->desc_t, 0, C * kDescK * V * sizeof(float)));
-  QB_ALLOC(L, L->desc_tiles, C * kDescK * V * 3);
+  QB_CUDA_TRY(L, L->desc_tiles.alloc(C * kDescK * V * 3));
   QB_CUDA_TRY(L, cudaMemset(L->desc_tiles, 0, C * kDescK * V * 3 * sizeof(float)));
-  QB_ALLOC(L, L->desc_norm, C * V);
-  QB_ALLOC(L, L->tc_fallback, S);
-  QB_ALLOC(L, L->tc_stats, 32);
+  QB_CUDA_TRY(L, L->desc_norm.alloc(C * V));
+  QB_CUDA_TRY(L, L->tc_fallback.alloc(S));
+  QB_CUDA_TRY(L, L->tc_stats.alloc(32));
   QB_CUDA_TRY(L, cudaMemset(L->tc_stats, 0, 32 * sizeof(unsigned long long)));
-  QB_ALLOC(L, L->rowbest, S * V);
-  QB_ALLOC(L, L->colpart, 2 * S * V + S * (V >> 7) * 2 + 2);  // tensor-core K6: [2][S][V] class results + tile cache (tc_match.cu)
-  QB_ALLOC(L, L->colbest, S * V);
-  QB_ALLOC(L, L->mut_i, S * V);
-  QB_ALLOC(L, L->mut_j, S * V);
-  QB_ALLOC(L, L->mark, S * V);
-  QB_ALLOC(L, L->partner, S * V);
-  QB_ALLOC(L, L->mean, C * 4);
-  QB_ALLOC(L, L->corr_src, S * Lc);
-  QB_ALLOC(L, L->corr_tgt, S * Lc);
-  QB_ALLOC(L, L->ma, S * Lc);
-  QB_ALLOC(L, L->mb, S * Lc);
-  QB_ALLOC(L, L->adj, S * Lc * W);
-  QB_ALLOC(L, L->adjp, S * Lc * W);
-  QB_ALLOC(L, L->deg, S * Lc);
-  QB_ALLOC(L, L->kcore, S * (Lc + 2));
-  QB_ALLOC(L, L->korder, S * (Lc + 2));
-  QB_ALLOC(L, L->rank_of, S * (Lc + 2));
-  QB_ALLOC(L, L->by_rank, S * (Lc + 2));
-  QB_ALLOC(L, L->kbin, S * (Lc + 2));
-  QB_ALLOC(L, L->clique, S * Lc);
-  QB_ALLOC(L, L->final_inl, S * Lc);
-  QB_ALLOC(L, L->rot_mask, S * Lc);
-  QB_ALLOC(L, L->trans_mask, S * Lc);
+  QB_CUDA_TRY(L, L->rowbest.alloc(S * V));
+  QB_CUDA_TRY(L, L->colpart.alloc(L->colpart_count()));
+  QB_CUDA_TRY(L, L->colbest.alloc(S * V));
+  QB_CUDA_TRY(L, L->mut_i.alloc(S * V));
+  QB_CUDA_TRY(L, L->mut_j.alloc(S * V));
+  QB_CUDA_TRY(L, L->mark.alloc(S * V));
+  QB_CUDA_TRY(L, L->partner.alloc(S * V));
+  QB_CUDA_TRY(L, L->mean.alloc(C * 4));
+  QB_CUDA_TRY(L, L->corr_src.alloc(S * Lc));
+  QB_CUDA_TRY(L, L->corr_tgt.alloc(S * Lc));
+  QB_CUDA_TRY(L, L->ma.alloc(S * Lc));
+  QB_CUDA_TRY(L, L->mb.alloc(S * Lc));
+  QB_CUDA_TRY(L, L->adj.alloc(S * Lc * W));
+  QB_CUDA_TRY(L, L->adjp.alloc(S * Lc * W));
+  QB_CUDA_TRY(L, L->deg.alloc(S * Lc));
+  QB_CUDA_TRY(L, L->kcore.alloc(S * (Lc + 2)));
+  QB_CUDA_TRY(L, L->korder.alloc(S * (Lc + 2)));
+  QB_CUDA_TRY(L, L->rank_of.alloc(S * (Lc + 2)));
+  QB_CUDA_TRY(L, L->by_rank.alloc(S * (Lc + 2)));
+  QB_CUDA_TRY(L, L->kbin.alloc(S * (Lc + 2)));
+  QB_CUDA_TRY(L, L->clique.alloc(S * Lc));
+  QB_CUDA_TRY(L, L->final_inl.alloc(S * Lc));
+  QB_CUDA_TRY(L, L->rot_mask.alloc(S * Lc));
+  QB_CUDA_TRY(L, L->trans_mask.alloc(S * Lc));
   // workspaces of the pairs whose graph or clique outgrows the shared-memory layouts (clique.cu, pose.cu); only wide handles have them
   if (Lc > (size_t)kKcoreSmemVerts) {
-    QB_ALLOC(L, L->kcore_ws, S * kcore_ws_bytes((int)Lc));
-    QB_ALLOC(L, L->chain_ws, S * kCliqueWarps * Lc);
+    QB_CUDA_TRY(L, L->kcore_ws.alloc(S * kcore_ws_bytes((int)Lc)));
+    QB_CUDA_TRY(L, L->chain_ws.alloc(S * kCliqueWarps * Lc));
   }
-  if (Lc > (size_t)kPoseSmemClique) QB_ALLOC(L, L->pose_ws, S * pose_ws_bytes((int)Lc));
-  QB_ALLOC(L, L->d_results, S);
+  if (Lc > (size_t)kPoseSmemClique) QB_CUDA_TRY(L, L->pose_ws.alloc(S * pose_ws_bytes((int)Lc)));
+  QB_CUDA_TRY(L, L->d_results.alloc(S));
   QB_CUDA_TRY(L, cudaMemset(L->d_results, 0, S * sizeof(qb200_result)));
-  QB_CUDA_TRY(L, cudaMallocHost((void**)&L->h_results, S * sizeof(qb200_result)));
-  // counters: one int block so a wave reset is a single launch.  n_edges (long long) lives at an 8-byte offset.
-  const size_t n_ints = C * 5 + C * 6 + S * 7 + 2 * S + 2;
-  QB_ALLOC(L, L->ctr_block, n_ints);
-  L->ctr_ints = n_ints;
-  int* p = L->ctr_block;
-  L->ctr.n_edges = reinterpret_cast<long long*>(p); p += 2 * S;
-  L->ctr.n_valid = p; p += C;
-  L->ctr.n_vox = p; p += C;
-  L->ctr.n_lat = p; p += C;
-  L->ctr.n_cells = p; p += C;
-  L->ctr.cloud_status = p; p += C;
-  L->ctr.bbox = p; p += C * 6;
-  L->ctr.n_mutual = p; p += S;
-  L->ctr.n_corr = p; p += S;
-  L->ctr.swapped = p; p += S;
-  L->ctr.n_clique = p; p += S;
-  L->ctr.max_core = p; p += S;
-  L->ctr.n_final = p; p += S;
-  L->ctr.flags = p; p += S;
-  for (int i = 0; i < 9; ++i) QB_CUDA_TRY(L, cudaEventCreate(&L->ev[i]));
-  for (int i = 0; i < 4; ++i) QB_CUDA_TRY(L, cudaEventCreate(&L->kev[i]));
+  QB_CUDA_TRY(L, L->h_results.alloc(S));
+  L->ctr_ints = carve_counters(nullptr, S, &L->ctr);
+  QB_CUDA_TRY(L, L->ctr_block.alloc(L->ctr_ints));
+  carve_counters(L->ctr_block, S, &L->ctr);
+  for (Event& e : L->ev) QB_CUDA_TRY(L, e.create());
+  for (Event& e : L->kev) QB_CUDA_TRY(L, e.create());
   QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
+  *out = std::move(L);
   return QB200_OK;
-}
-
-void lane_free(Lane* L) {
-  if (!L) return;
-  void* dev_ptrs[] = {(void*)L->d_cloud_ptr, L->d_cloud_n, L->d_raw_off, L->raw_stage, L->key_a, L->key_b, L->val_a, L->val_b, L->cub_temp,
-                      L->vox_start, L->vox_pts, L->cell_key, L->cell_start, L->normals, L->spfh, L->nbr_list, L->nbr_cnt, L->desc_t, L->rowbest, L->colpart, L->colbest,
-                      L->desc_tiles, L->desc_norm, L->tc_fallback, L->tc_stats, L->aos_scratch,
-                      L->mut_i, L->mut_j, L->mark, L->partner, L->mean, L->corr_src, L->corr_tgt, L->ma, L->mb, L->adj, L->adjp, L->deg,
-                      L->kcore, L->korder, L->rank_of, L->by_rank, L->kbin, L->clique, L->ex_stack, L->ex_pool, L->ex_lvl, L->ex_cur, L->kcore_ws, L->chain_ws, L->pose_ws, L->pw_ints, L->pw_out, L->ip_buf, L->final_inl, L->rot_mask, L->trans_mask, L->d_results,
-                      L->ctr_block};
-  for (void* p : dev_ptrs)
-    if (p) cudaFree(p);
-  if (L->h_cloud_ptr) cudaFreeHost((void*)L->h_cloud_ptr);
-  if (L->h_cloud_n) cudaFreeHost(L->h_cloud_n);
-  if (L->h_raw_off) cudaFreeHost(L->h_raw_off);
-  if (L->h_results) cudaFreeHost(L->h_results);
-  for (int i = 0; i < 9; ++i)
-    if (L->ev[i]) cudaEventDestroy(L->ev[i]);
-  for (int i = 0; i < 4; ++i)
-    if (L->kev[i]) cudaEventDestroy(L->kev[i]);
-  if (L->own_stream) cudaStreamDestroy(L->own_stream);
-  delete L;
 }
 
 int wave_reset(Lane* L, int n_clouds) {
@@ -314,7 +290,7 @@ int upload_cloud_as_voxels(Lane* L, int cloud, const float* pts4, int n) {
 
 // the record of a single-pair solve on lane 0
 int fetch_result(qb200_handle* h, qb200_result* res) {
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
   QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
   *res = L->h_results[0];
@@ -380,19 +356,6 @@ int stage_raw(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs) {
 // FPFHManager keeps the last target's descriptors and reuses them as the next source (odometry mode, fpfh_manager.hpp:74-77,
 // 111-118); a loop-closure sweep matches one scan against many.  The cache keeps voxel points, normals and FPFH-33 of a scan
 // resident on the device so that the front end (voxel + normals + FPFH, ~45 % of a wave) runs once per SCAN, not once per pair.
-void cache_free(qb200_handle* h) {
-  if (h->c_vox) cudaFree(h->c_vox);
-  if (h->c_nrm) cudaFree(h->c_nrm);
-  if (h->c_desc) cudaFree(h->c_desc);
-  if (h->c_n) cudaFree(h->c_n);
-  if (h->c_status) cudaFree(h->c_status);
-  if (h->d_slot_of_cloud) cudaFree(h->d_slot_of_cloud);
-  if (h->h_slot_of_cloud) cudaFreeHost(h->h_slot_of_cloud);
-  delete[] h->c_sig;
-  h->c_vox = h->c_nrm = nullptr; h->c_desc = nullptr; h->c_n = h->c_status = h->d_slot_of_cloud = h->h_slot_of_cloud = nullptr;
-  h->c_sig = nullptr;
-  h->c_slots = 0;
-}
 
 // clouds [0, n_clouds) of lane L's wave to (to_cache = 1) or from their cache slots h->h_slot_of_cloud[]
 int cache_copy(qb200_handle* h, Lane* L, int to_cache, int n_clouds) {
@@ -524,7 +487,7 @@ int collect_waves(qb200_handle* h, const qb200_result* dst) {
   int rc = QB200_OK;
   const int n = h->lanes_active > 0 ? h->lanes_active : 1;
   for (int i = 0; i < n; ++i) {
-    Lane* L = h->lane[(h->lane_cursor + i) % n];
+    Lane* L = h->lane[(h->lane_cursor + i) % n].get();
     if (!L || (dst && L->pend_dst != dst)) continue;
     const int rc2 = wave_collect(h, L);
     if (rc == QB200_OK) rc = rc2;
@@ -544,8 +507,8 @@ int run_waves(qb200_handle* h, const WaveInput& in, int n, const qb200_params& p
   reset_timers(h);
   const int S = h->cfg.max_batch_slots;
   for (int w0 = 0; w0 < n; w0 += S) {
-    int rc = wave_submit(h, h->lane[0], in, w0, n - w0 < S ? n - w0 : S, p, results);
-    if (rc == QB200_OK) rc = wave_collect(h, h->lane[0]);
+    int rc = wave_submit(h, h->lane[0].get(), in, w0, n - w0 < S ? n - w0 : S, p, results);
+    if (rc == QB200_OK) rc = wave_collect(h, h->lane[0].get());
     if (rc) return rc;
   }
   if (n == 1) set_last(h, results[0]);
@@ -563,7 +526,7 @@ int enter(qb200_handle* h) {
 // tc_stats[first, first + n) summed over the lanes (then zeroed on every lane if reset)
 int read_tc_stats(qb200_handle* h, int first, int n, uint64_t* out, int reset) {
   for (int i = 0; i < n; ++i) out[i] = 0;
-  for (Lane* L : h->lane) {
+  for (const auto& L : h->lane) {
     if (!L) continue;
     uint64_t o[32];
     QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
@@ -637,9 +600,9 @@ int qb200_create(const qb200_config* cfg_in, qb200_handle** out) {
   h->max_lanes = (ln && ln[0] >= '1' && ln[0] <= '8') ? ln[0] - '0' : 4;
   like.err = h->err;
   auto alloc = [&]() -> int {
-    QB_CUDA_TRY(h, cudaEventCreate(&h->ev_fork));  // (timing enabled: QB200_TIMELINE measures the waves against it)
-    QB_CUDA_TRY(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
-    QB_CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_copied, cudaEventDisableTiming));
+    QB_CUDA_TRY(h, h->ev_fork.create());  // (timing enabled: QB200_TIMELINE measures the waves against it)
+    QB_CUDA_TRY(h, h->copy_stream.create(cudaStreamNonBlocking));
+    QB_CUDA_TRY(h, h->ev_copied.create(cudaEventDisableTiming));
     return lane_alloc(like, &h->lane[0]);
   };
   const int rc = alloc();
@@ -657,17 +620,12 @@ void qb200_destroy(qb200_handle* h) {
   cudaSetDevice(h->cfg.device);
   cudaDeviceSynchronize();
   comm_release(h);
-  cache_free(h);
-  for (Lane* L : h->lane) lane_free(L);
-  if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-  if (h->ev_copied) cudaEventDestroy(h->ev_copied);
-  if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
   delete h;
 }
 
 int qb200_set_stream(qb200_handle* h, void* cuda_stream) {
   if (int rc = enter(h)) return rc;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   L->stream = cuda_stream ? (cudaStream_t)cuda_stream : L->own_stream;
   return QB200_OK;
 }
@@ -676,7 +634,7 @@ const char* qb200_last_error(const qb200_handle* h) { return h ? h->err : "null 
 int64_t qb200_launch_count(const qb200_handle* h) {
   if (!h) return 0;
   int64_t n = 0;
-  for (const Lane* L : h->lane)
+  for (const auto& L : h->lane)
     if (L) n += L->launches;
   return n;
 }
@@ -687,7 +645,7 @@ int qb200_voxelize(qb200_handle* h, const float* pts4, int32_t n, float leaf, in
   if (int rc = enter(h)) return rc;
   if (!n_out || n < 0 || (n > 0 && !pts4) || !(leaf > 0) || cap < 0 || (cap > 0 && !out4)) return QB200_ERR_BAD_ARG;
   *n_out = 0;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
   if (n == 0) return QB200_OK;
   int rc = wave_reset(L, 1);
@@ -727,7 +685,7 @@ int qb200_patchwork(qb200_handle* h, const float* pts4, int32_t n, const qb200_p
   if (int rc = enter(h)) return rc;
   if (!p || !n_ground || !n_nonground || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
   *n_ground = *n_nonground = 0;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
   if (n > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(L->raw_stage, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
   int ng = 0, nn = 0, st = 0;
@@ -748,7 +706,7 @@ int qb200_segment_cloud(qb200_handle* h, const float* pts4, int32_t n, const qb2
   if (int rc = enter(h)) return rc;
   if (!p || !n_valid || !n_outlier || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
   *n_valid = *n_outlier = 0;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
   if (n > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(L->raw_stage, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
   int nv = 0, no = 0;
@@ -770,7 +728,7 @@ int qb200_compute_fpfh(qb200_handle* h, const float* pts4, int32_t n, float norm
   if (n < 0 || (n > 0 && !pts4) || !(normal_radius > 0) || !(fpfh_radius > 0) || !(grid_cell > 0)) return QB200_ERR_BAD_ARG;
   if (normal_radius > fpfh_radius) return QB200_ERR_BAD_ARG;  // fpfh_manager.hpp:99-102
   if (n == 0) return QB200_OK;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   int rc = wave_reset(L, 1);
   if (rc) return rc;
   if ((rc = upload_cloud_as_voxels(L, 0, pts4, n))) return rc;
@@ -788,7 +746,7 @@ int qb200_compute_fpfh(qb200_handle* h, const float* pts4, int32_t n, float norm
 // ---- stage: matching ------------------------------------------------------------------------------
 // the correspondences launch_match left for pair 0: counts, then the first cap of them
 static int match_result(qb200_handle* h, int32_t* corr, float* sm4, float* tm4, int cap, int32_t* n_corr, int32_t* n_mutual) {
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   int nc = 0, nm = 0, st = 0, rc;
   if ((rc = get_counter(L, L->ctr.n_corr, &nc))) return rc;
   if ((rc = get_counter(L, L->ctr.n_mutual, &nm))) return rc;
@@ -808,7 +766,7 @@ int qb200_match(qb200_handle* h, const float* src4, int32_t n_src, const float* 
   if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
   *n_corr = 0;
   if (n_mutual) *n_mutual = 0;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   if (n_src > L->V || n_tgt > L->V) { h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points"); return QB200_ERR_BAD_ARG; }
   h->last_match_n[0] = h->last_match_n[1] = 0;
   if (n_src == 0 || n_tgt == 0) return QB200_OK;
@@ -834,7 +792,7 @@ int qb200_match_and_pack(qb200_handle* h, const float* src4, int32_t n_src, cons
   if (!n_corr || !params_ok(p) || n_src < 0 || n_tgt < 0 || cap < 0) return QB200_ERR_BAD_ARG;
   if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
   *n_corr = 0;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   if (n_src > L->V || n_tgt > L->V) { h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points"); return QB200_ERR_BAD_ARG; }
   if (n_src == 0 || n_tgt == 0) return QB200_OK;
   int rc = wave_reset(L, 2);
@@ -854,7 +812,7 @@ int qb200_build_graph(qb200_handle* h, const float* a4, const float* b4, int32_t
     return QB200_ERR_BAD_ARG;
   if (n_edges) *n_edges = 0;
   if (L == 0) return QB200_OK;
-  Lane* ln = h->lane[0];
+  Lane* ln = h->lane[0].get();
   int rc = upload_matched(ln, a4, b4, L);
   if (rc) return rc;
   if ((rc = launch_graph(ln, 1, noise_bound, cbar2))) return rc;
@@ -880,7 +838,7 @@ int qb200_max_clique_ex(qb200_handle* h, const uint32_t* adj, int32_t L, int32_t
   if (flags) *flags = 0;
   *n_clique = 0;
   if (max_core) *max_core = 0;
-  Lane* ln = h->lane[0];
+  Lane* ln = h->lane[0].get();
   if (L > ln->Lc) { h->fail(__FILE__, __LINE__, "L exceeds max_corr"); return QB200_ERR_BAD_ARG; }
   if (L == 0) return QB200_OK;
   int rc = wave_reset(ln, 2);
@@ -917,7 +875,7 @@ int qb200_solve_pose(qb200_handle* h, const float* a4, const float* b4, int32_t 
   if (int rc = enter(h)) return rc;
   if (!res || !params_ok(p) || L < 0 || (L > 0 && (!a4 || !b4)) || n_clique < 0 || n_clique > L || (n_clique > 0 && !clique))
     return QB200_ERR_BAD_ARG;
-  Lane* ln = h->lane[0];
+  Lane* ln = h->lane[0].get();
   int rc = upload_matched(ln, a4, b4, L);
   if (rc) return rc;
   if (n_clique > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ln->clique, clique, (size_t)n_clique * sizeof(int), cudaMemcpyHostToDevice, ln->stream));
@@ -939,7 +897,7 @@ int qb200_solve_pose(qb200_handle* h, const float* a4, const float* b4, int32_t 
 int qb200_solve_correspondences(qb200_handle* h, const float* a4, const float* b4, int32_t L, const qb200_params* p, qb200_result* res) {
   if (int rc = enter(h)) return rc;
   if (!res || !params_ok(p) || L < 0 || (L > 0 && (!a4 || !b4))) return QB200_ERR_BAD_ARG;
-  Lane* ln = h->lane[0];
+  Lane* ln = h->lane[0].get();
   int rc = upload_matched(ln, a4, b4, L);
   if (rc) return rc;
   if ((rc = run_solver(ln, 1, resolve_params(h, *p), 0))) return rc;
@@ -1025,8 +983,6 @@ int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32
     if (!h->lane[l]) {
       const int rc = lane_alloc(*h->lane[0], &h->lane[l]);
       if (rc != QB200_OK) {
-        lane_free(h->lane[l]);
-        h->lane[l] = nullptr;
         h->fail(__FILE__, __LINE__, "cannot allocate another lane");
         return rc;
       }
@@ -1049,7 +1005,7 @@ int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32
   h->lanes_active = n_lanes;
   int rc = QB200_OK, wave = 0;
   for (int w0 = 0; w0 < n_pairs && rc == QB200_OK; ++wave) {
-    Lane* L = h->lane[h->lane_cursor];
+    Lane* L = h->lane[h->lane_cursor].get();
     int np = planned ? wave_n[wave] : S;
     if (np > n_pairs - w0) np = n_pairs - w0;
     if ((rc = wave_collect(h, L))) break;  // the lane's previous wave (its pinned tables are reused)
@@ -1073,23 +1029,23 @@ int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const
 // ---- introspection ----------------------------------------------------------------------------------
 int qb200_get_last_clique(qb200_handle* h, int32_t* idx, int32_t cap, int32_t* n) {
   if (int rc = enter(h)) return rc;
-  return copy_ints(h->lane[0], h->lane[0]->clique, h->last_n_clique, idx, cap, n);
+  return copy_ints(h->lane[0].get(), h->lane[0]->clique, h->last_n_clique, idx, cap, n);
 }
 int qb200_get_last_final_inliers(qb200_handle* h, int32_t* idx, int32_t cap, int32_t* n) {
   if (int rc = enter(h)) return rc;
-  return copy_ints(h->lane[0], h->lane[0]->final_inl, h->last_n_final, idx, cap, n);
+  return copy_ints(h->lane[0].get(), h->lane[0]->final_inl, h->last_n_final, idx, cap, n);
 }
 int qb200_get_last_correspondences(qb200_handle* h, int32_t* corr, float* src_matched4, float* tgt_matched4, int32_t cap, int32_t* n) {
   if (int rc = enter(h)) return rc;
   if (!n || cap < 0) return QB200_ERR_BAD_ARG;
   *n = h->last_n_corr;
-  return download_corr(h->lane[0], h->last_n_corr, corr, src_matched4, tgt_matched4, cap);
+  return download_corr(h->lane[0].get(), h->last_n_corr, corr, src_matched4, tgt_matched4, cap);
 }
 
 int qb200_get_last_features(qb200_handle* h, int32_t which, float* normals4, float* desc33, int32_t cap, int32_t* n_out) {
   if (int rc = enter(h)) return rc;
   if (!n_out || which < 0 || which > 1 || cap < 0) return QB200_ERR_BAD_ARG;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   int n = 0, rc;
   if ((rc = get_counter(L, L->ctr.n_vox + which, &n))) return rc;
   *n_out = n;
@@ -1133,7 +1089,7 @@ int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset) {
 int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, uint64_t* colbest, int32_t cap_cols) {
   if (int rc = enter(h)) return rc;
   if (cap_rows < 0 || cap_cols < 0) return QB200_ERR_BAD_ARG;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   const int nr = cap_rows < h->last_match_n[0] ? cap_rows : h->last_match_n[0];
   const int nc = cap_cols < h->last_match_n[1] ? cap_cols : h->last_match_n[1];
@@ -1147,7 +1103,7 @@ int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, 
 int qb200_debug_tc_footprint(qb200_handle* h, int32_t* out5) {
   if (!h || !out5) return QB200_ERR_BAD_ARG;
   cudaSetDevice(h->cfg.device);
-  return tc_footprint(h->lane[0], out5);
+  return tc_footprint(h->lane[0].get(), out5);
 }
 
 // Validation hook: tensor-core (3xTF32) approximate squared distances between up to 128 source and 128 target
@@ -1155,7 +1111,7 @@ int qb200_debug_tc_footprint(qb200_handle* h, int32_t* out5) {
 int qb200_debug_tc_distances(qb200_handle* h, const float* a33, int32_t na, const float* b33, int32_t nb, float* out) {
   if (int rc = enter(h)) return rc;
   if (!a33 || !b33 || !out || na < 1 || nb < 1 || na > 128 || nb > 128) return QB200_ERR_BAD_ARG;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   int rc = wave_reset(L, 2);
   if (rc) return rc;
   if ((rc = set_counter(L, L->ctr.n_vox + 0, na))) return rc;
@@ -1179,20 +1135,23 @@ int qb200_cache_reserve(qb200_handle* h, int32_t n_slots) {
   if (int rc = enter(h)) return rc;
   if (n_slots < 0 || n_slots > (1 << 20)) return QB200_ERR_BAD_ARG;
   QB_CUDA_TRY(h, cudaStreamSynchronize(h->lane[0]->stream));
-  cache_free(h);
+  // the old cache goes first, so the device never holds two
+  h->c_slots = 0;
+  h->c_vox.reset(); h->c_nrm.reset(); h->c_desc.reset(); h->c_n.reset(); h->c_status.reset();
+  h->d_slot_of_cloud.reset(); h->h_slot_of_cloud.reset(); h->c_sig.reset();
   if (n_slots == 0) return QB200_OK;
   const size_t V = h->cfg.max_voxel_points, N = (size_t)n_slots;
-  QB_ALLOC(h, h->c_vox, N * V);
-  QB_ALLOC(h, h->c_nrm, N * V);
-  QB_ALLOC(h, h->c_desc, N * kDescK * V);
-  QB_ALLOC(h, h->c_n, N);
-  QB_ALLOC(h, h->c_status, N);
-  QB_ALLOC(h, h->d_slot_of_cloud, 2 * (size_t)h->cfg.max_batch_slots);
-  QB_CUDA_TRY(h, cudaMallocHost((void**)&h->h_slot_of_cloud, 2 * (size_t)h->cfg.max_batch_slots * sizeof(int)));
+  QB_CUDA_TRY(h, h->c_vox.alloc(N * V));
+  QB_CUDA_TRY(h, h->c_nrm.alloc(N * V));
+  QB_CUDA_TRY(h, h->c_desc.alloc(N * kDescK * V));
+  QB_CUDA_TRY(h, h->c_n.alloc(N));
+  QB_CUDA_TRY(h, h->c_status.alloc(N));
+  QB_CUDA_TRY(h, h->d_slot_of_cloud.alloc(2 * (size_t)h->cfg.max_batch_slots));
+  QB_CUDA_TRY(h, h->h_slot_of_cloud.alloc(2 * (size_t)h->cfg.max_batch_slots));
   QB_CUDA_TRY(h, cudaMemset(h->c_n, 0, N * sizeof(int)));
   QB_CUDA_TRY(h, cudaMemset(h->c_status, 0, N * sizeof(int)));
   QB_CUDA_TRY(h, cudaMemset(h->c_desc, 0, N * kDescK * V * sizeof(float)));
-  h->c_sig = new (std::nothrow) float[4 * N]();
+  h->c_sig.reset(new (std::nothrow) float[4 * N]());
   if (!h->c_sig) return QB200_ERR_CUDA;
   h->c_slots = n_slots;
   return QB200_OK;
@@ -1202,7 +1161,7 @@ int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t
                       const qb200_params* p, qb200_mem_kind kind) {
   if (int rc = enter(h)) return rc;
   if (n_scans < 0 || (n_scans > 0 && (!scans4 || !n_points || !slot_ids)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   for (int i = 0; i < n_scans; ++i)
     if (slot_ids[i] < 0 || slot_ids[i] >= h->c_slots || n_points[i] < 0 || n_points[i] > L->R || (n_points[i] > 0 && !scans4[i])) {
       h->fail(__FILE__, __LINE__, "scan is null, exceeds max_raw_points or names a slot outside qb200_cache_reserve()");
@@ -1217,7 +1176,7 @@ int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t
       L->h_cloud_ptr[c] = reinterpret_cast<const float4*>(scans4[c0 + c]);
       L->h_cloud_n[c] = n_points[c0 + c];
       h->h_slot_of_cloud[c] = slot_ids[c0 + c];
-      float* sig = h->c_sig + 4 * (size_t)slot_ids[c0 + c];
+      float* sig = h->c_sig.get() + 4 * (size_t)slot_ids[c0 + c];
       sig[0] = p->voxel_size; sig[1] = p->normal_radius; sig[2] = p->fpfh_radius; sig[3] = cell;
     }
     if ((rc = stage_raw(L, nc, kind, L->stream))) return rc;
@@ -1239,7 +1198,7 @@ int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t
     const int sl[2] = {pairs[i].src_slot, pairs[i].tgt_slot};
     for (int k = 0; k < 2; ++k) {
       if (sl[k] < 0 || sl[k] >= h->c_slots) { h->fail(__FILE__, __LINE__, "slot outside qb200_cache_reserve()"); return QB200_ERR_BAD_ARG; }
-      const float* sig = h->c_sig + 4 * (size_t)sl[k];
+      const float* sig = h->c_sig.get() + 4 * (size_t)sl[k];
       if (sig[0] != p->voxel_size || sig[1] != p->normal_radius || sig[2] != p->fpfh_radius || sig[3] != cell) {
         h->fail(__FILE__, __LINE__, "cached scan was computed with other front-end parameters (or the slot is empty)");
         return QB200_ERR_BAD_ARG;
@@ -1262,7 +1221,7 @@ int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {
   QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_desc + to_slot * kDescK * V, h->c_desc + from_slot * kDescK * V, kDescK * V * sizeof(float), cudaMemcpyDeviceToDevice, st));
   QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_n + to_slot, h->c_n + from_slot, sizeof(int), cudaMemcpyDeviceToDevice, st));
   QB_CUDA_TRY(h, cudaMemcpyAsync(h->c_status + to_slot, h->c_status + from_slot, sizeof(int), cudaMemcpyDeviceToDevice, st));
-  memcpy(h->c_sig + 4 * (size_t)to_slot, h->c_sig + 4 * (size_t)from_slot, 4 * sizeof(float));
+  memcpy(h->c_sig.get() + 4 * (size_t)to_slot, h->c_sig.get() + 4 * (size_t)from_slot, 4 * sizeof(float));
   QB_CUDA_TRY(h, cudaStreamSynchronize(st));
   return QB200_OK;
 }
@@ -1270,7 +1229,7 @@ int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {
 int qb200_cache_read(qb200_handle* h, int32_t slot, float* vox4, float* normals4, float* desc33, int32_t cap, int32_t* n_out) {
   if (int rc = enter(h)) return rc;
   if (!n_out || slot < 0 || slot >= h->c_slots || cap < 0) return QB200_ERR_BAD_ARG;
-  Lane* L = h->lane[0];
+  Lane* L = h->lane[0].get();
   int n = 0, rc;
   if ((rc = get_counter(L, h->c_n + slot, &n))) return rc;
   *n_out = n;

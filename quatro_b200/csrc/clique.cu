@@ -769,14 +769,21 @@ static int launch_kcore(Lane* h, int n_pairs) {
   return QB200_OK;
 }
 
-// PMC_EXACT scratch (level stack, list pool), allocated on the first exact call of a handle
+// PMC_EXACT scratch (level stack, list pool), allocated on the first exact call of a handle: all of it or none
 static int ensure_exact_scratch(Lane* h) {
   if (h->ex_stack) return QB200_OK;
   const size_t S = h->S < kExactChunk ? h->S : kExactChunk;
-  QB_CUDA_TRY(h, cudaMalloc((void**)&h->ex_stack, S * kExactDepth * (size_t)h->W * sizeof(uint32_t)));
-  QB_CUDA_TRY(h, cudaMalloc((void**)&h->ex_pool, S * (size_t)kExactPool * sizeof(uint32_t)));
-  QB_CUDA_TRY(h, cudaMalloc((void**)&h->ex_lvl, S * 2 * (size_t)kExactDepth * sizeof(int)));
-  QB_CUDA_TRY(h, cudaMalloc((void**)&h->ex_cur, S * (size_t)kExactDepth * sizeof(unsigned short)));
+  DeviceMem<uint32_t> stack, pool;
+  DeviceMem<int> lvl;
+  DeviceMem<unsigned short> cur;
+  QB_CUDA_TRY(h, stack.alloc(S * kExactDepth * (size_t)h->W));
+  QB_CUDA_TRY(h, pool.alloc(S * (size_t)kExactPool));
+  QB_CUDA_TRY(h, lvl.alloc(S * 2 * (size_t)kExactDepth));
+  QB_CUDA_TRY(h, cur.alloc(S * (size_t)kExactDepth));
+  h->ex_stack = std::move(stack);
+  h->ex_pool = std::move(pool);
+  h->ex_lvl = std::move(lvl);
+  h->ex_cur = std::move(cur);
   return QB200_OK;
 }
 

@@ -71,17 +71,14 @@ NcclApi& nccl() {
 int ensure_staging(qb200_handle* h, int n_local) {
   if (n_local <= h->comm_cap) return QB200_OK;
   cudaSetDevice(h->cfg.device);
-  if (h->d_send) cudaFree(h->d_send);
-  if (h->d_recv) cudaFree(h->d_recv);
-  if (h->h_send) cudaFreeHost(h->h_send);
-  if (h->h_recv) cudaFreeHost(h->h_recv);
-  h->d_send = h->d_recv = h->h_send = h->h_recv = nullptr;
+  // the old buffers go first, so the device never holds two sets
   h->comm_cap = 0;
-  const size_t one = (size_t)n_local * sizeof(qb200_result), all = one * (size_t)h->comm_world;
-  QB_CUDA_TRY(h, cudaMalloc((void**)&h->d_send, one));
-  QB_CUDA_TRY(h, cudaMalloc((void**)&h->d_recv, all));
-  QB_CUDA_TRY(h, cudaMallocHost((void**)&h->h_send, 2 * one));  // two halves: the pipelined mode fills one while the other is gathered
-  QB_CUDA_TRY(h, cudaMallocHost((void**)&h->h_recv, all));
+  h->d_send.reset(); h->d_recv.reset(); h->h_send.reset(); h->h_recv.reset();
+  const size_t one = (size_t)n_local, all = one * (size_t)h->comm_world;
+  QB_CUDA_TRY(h, h->d_send.alloc(one));
+  QB_CUDA_TRY(h, h->d_recv.alloc(all));
+  QB_CUDA_TRY(h, h->h_send.alloc(2 * one));  // two halves: the pipelined mode fills one while the other is gathered
+  QB_CUDA_TRY(h, h->h_recv.alloc(all));
   h->comm_cap = n_local;
   return QB200_OK;
 }
@@ -90,8 +87,8 @@ int comm_common_init(qb200_handle* h, int world, int rank) {
   h->comm_world = world;
   h->comm_rank = rank;
   cudaSetDevice(h->cfg.device);
-  if (!h->comm_stream) QB_CUDA_TRY(h, cudaStreamCreateWithFlags(&h->comm_stream, cudaStreamNonBlocking));
-  if (!h->comm_done) QB_CUDA_TRY(h, cudaEventCreateWithFlags(&h->comm_done, cudaEventDisableTiming));
+  if (!h->comm_stream) QB_CUDA_TRY(h, h->comm_stream.create(cudaStreamNonBlocking));
+  if (!h->comm_done) QB_CUDA_TRY(h, h->comm_done.create(cudaEventDisableTiming));
   return QB200_OK;
 }
 
@@ -127,15 +124,6 @@ void comm_release(qb200_handle* h) {
   if (!h) return;
   if (h->comm && nccl().ok) nccl().CommDestroy((ncclComm_t)h->comm);
   h->comm = nullptr;
-  if (h->d_send) cudaFree(h->d_send);
-  if (h->d_recv) cudaFree(h->d_recv);
-  if (h->h_send) cudaFreeHost(h->h_send);
-  if (h->h_recv) cudaFreeHost(h->h_recv);
-  h->d_send = h->d_recv = h->h_send = h->h_recv = nullptr;
-  if (h->comm_done) cudaEventDestroy(h->comm_done);
-  if (h->comm_stream) cudaStreamDestroy(h->comm_stream);
-  h->comm_done = nullptr;
-  h->comm_stream = nullptr;
   h->comm_cap = 0;
   h->comm_world = 0;
 }

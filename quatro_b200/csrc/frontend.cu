@@ -30,7 +30,7 @@ size_t sort_temp_bytes(int max_items) {
 int sort_pairs(Lane* h, int n_items, int end_bit) {
   if (n_items <= 0) return QB200_OK;
   size_t bytes = h->cub_bytes;
-  QB_CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->cub_temp, bytes, h->key_a, h->key_b, h->val_a, h->val_b, n_items, 0, end_bit,
+  QB_CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->cub_temp.get(), bytes, h->key_a.get(), h->key_b.get(), h->val_a.get(), h->val_b.get(), n_items, 0, end_bit,
                                                  h->stream));
   h->launches += 1 + (end_bit + 7) / 8;  // onesweep: histogram + one pass per 8 key bits
   return QB200_OK;
@@ -645,7 +645,7 @@ int launch_voxel(Lane* h, int n_clouds, float leaf, int skip_flagged) {
   if (n_clouds <= 0) return QB200_OK;
   const float inv = 1.0f / leaf;
   const dim3 gb(n_clouds >= 16 ? 16 : 64, n_clouds);  // ~30 points per thread when the batch fills the device on its own
-  int* chunk_cnt = reinterpret_cast<int*>(h->val_b);   // [clouds][kVsChunks]
+  int* chunk_cnt = reinterpret_cast<int*>(h->val_b.get());   // [clouds][kVsChunks]
   voxel_bbox_kernel<<<gb, 256, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, inv, skip_flagged, h->ctr.bbox, h->ctr.n_valid, h->ctr.cloud_status,
                                                chunk_cnt);
   h->launches += 1;

@@ -4,94 +4,108 @@
 #pragma once
 #include <string.h>
 
+#include <memory>
+
 #include "common.cuh"
+#include "owners.cuh"
 
 namespace qb {
 
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
-// kernels of the others.
+// kernels of the others.  The lane owns its stream, buffers and events: deleting it releases them.
 struct Lane {
   int S, R, V, Lc, W;        // slots, raw cap / cloud, voxel cap / cloud, corr cap / pair, words per adjacency row
   int NS;                    // match stripes per pair = V / kMatchTile
   int device;
   int n_sm;                  // multiprocessors of the device (grid size of the persistent kernels)
   int force_exact_match;     // 0 (default): tensor-core filter + exact evaluation; 1 (QB200_MATCH_EXACT=1): exact CUDA-core K6 only
-  cudaStream_t own_stream, stream;
+  Stream own_stream;
+  cudaStream_t stream;       // own_stream, or the caller's stream of qb200_set_stream (lane 0)
   char* err;                 // the handle's message buffer (qb200_last_error)
   int64_t launches;
 
   // ---- wave description (host-known inputs) ----
-  const float4** d_cloud_ptr; // [2S]
-  int* d_cloud_n;             // [2S]
-  int* d_raw_off;             // [2S+1] offsets into the concatenated sort arrays
-  const float4** h_cloud_ptr; int* h_cloud_n; int* h_raw_off;  // pinned mirrors
-  float4* raw_stage;          // [2S*R] staging for host inputs
+  DeviceMem<const float4*> d_cloud_ptr; // [2S]
+  DeviceMem<int> d_cloud_n;   // [2S]
+  DeviceMem<int> d_raw_off;   // [2S+1] offsets into the concatenated sort arrays
+  PinnedMem<const float4*> h_cloud_ptr; PinnedMem<int> h_cloud_n, h_raw_off;  // pinned mirrors
+  DeviceMem<float4> raw_stage; // [2S*R] staging for host inputs
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
   int pend_t0, pend_t1;       // ... the stage-time slots [t0, t1) it records
   qb200_result* pend_dst;     // ... and the caller's record array of its batch
 
   // ---- sort workspace (voxel sort, then lattice sort) ----
-  uint64_t *key_a, *key_b;    // [2S*max(R,V)]
-  uint32_t *val_a, *val_b;    // [2S*max(R,V)]; val_a also holds the voxel sort's digit histograms
-  void* cub_temp; size_t cub_bytes;  // library radix sort of up to 2S*V items (lattice / norm sorts of clouds too large for sort.cu)
-  float* aos_scratch;         // [2*V*33] AoS descriptors of the stage entry points (qb200_compute_fpfh / qb200_match)
+  DeviceMem<uint64_t> key_a, key_b;  // [2S*max(R,V)]
+  DeviceMem<uint32_t> val_a, val_b;  // [2S*max(R,V)]; val_a also holds the voxel sort's digit histograms
+  DeviceMem<void> cub_temp; size_t cub_bytes;  // library radix sort of up to 2S*V items (lattice / norm sorts of clouds too large for sort.cu)
+  DeviceMem<float> aos_scratch;  // [2*V*33] AoS descriptors of the stage entry points (qb200_compute_fpfh / qb200_match)
 
   // ---- front end ----
-  int* vox_start;             // [2S*(V+1)] position (in the sorted raw array) of each voxel's first point
-  float4* vox_pts;            // [2S*V] centroids, ascending (k,j,i)
-  uint64_t* cell_key;         // [2S*V] occupied lattice cells, ascending
-  int* cell_start;            // [2S*(V+1)]
-  float4* normals;            // [2S*V]
-  float* spfh;                // [2S*V*36] rows padded to 36 floats
-  uint32_t* nbr_list;         // [2S][kNbrGlobalCap][V] fpfh_radius neighbour indices found by K2c (lattice order), read by K3..K5
-  int* nbr_cnt;               // [2S*V] neighbour count (self included); > kNbrGlobalCap: K5 walks the lattice itself
-  float* desc_t;              // [2S*40*V] FPFH, dimension-major per cloud (row d = bin d over all points; rows 33..39 zero)
-  float* desc_tiles;          // [2S*(V/64)*3*2560] per 64-point block: centred TF32 hi | lo | exact fp32 images in the wgmma
+  DeviceMem<int> vox_start;   // [2S*(V+1)] position (in the sorted raw array) of each voxel's first point
+  DeviceMem<float4> vox_pts;  // [2S*V] centroids, ascending (k,j,i)
+  DeviceMem<uint64_t> cell_key; // [2S*V] occupied lattice cells, ascending
+  DeviceMem<int> cell_start;  // [2S*(V+1)]
+  DeviceMem<float4> normals;  // [2S*V]
+  DeviceMem<float> spfh;      // [2S*V*36] rows padded to 36 floats
+  DeviceMem<uint32_t> nbr_list; // [2S][kNbrGlobalCap][V] fpfh_radius neighbour indices found by K2c (lattice order), read by K3..K5
+  DeviceMem<int> nbr_cnt;     // [2S*V] neighbour count (self included); > kNbrGlobalCap: K5 walks the lattice itself
+  DeviceMem<float> desc_t;    // [2S*40*V] FPFH, dimension-major per cloud (row d = bin d over all points; rows 33..39 zero)
+  DeviceMem<float> desc_tiles; // [2S*(V/64)*3*2560] per 64-point block: centred TF32 hi | lo | exact fp32 images in the wgmma
                               // shared-memory operand layout (one bulk copy per column tile, one per 128-row stripe)
-  float* desc_norm;           // [2S*V] squared norms (fp32 fma chain)
-  int* tc_fallback;           // [S] 1 = too many exact ties for the filter to pay off: pair re-done by the exact fp32 kernel
-  unsigned long long* tc_stats; // [32] diagnostics, cumulative: [0..3] exact evaluations, tiles drained, warm-up passes, aborted stripes; [4..5] QB200_TC_VERIFY; [8..31] QB200_TC_PROF
+  DeviceMem<float> desc_norm; // [2S*V] squared norms (fp32 fma chain)
+  DeviceMem<int> tc_fallback; // [S] 1 = too many exact ties for the filter to pay off: pair re-done by the exact fp32 kernel
+  DeviceMem<unsigned long long> tc_stats; // [32] diagnostics, cumulative: [0..3] exact evaluations, tiles drained, warm-up passes, aborted stripes; [4..5] QB200_TC_VERIFY; [8..31] QB200_TC_PROF
   // ---- matching ----
-  unsigned long long* rowbest;// [S*V] packed (dist bits << 32 | tgt idx) per source point
-  unsigned long long* colpart;// [2SV + S*(V/128)*2 + 2] tensor-core K6 scratch: class results [2][S][V] and the tile-max cache
-                              // ([S][V/64][2] 32-bit maxima of 32-column groups)
-  unsigned long long* colbest;// [S*V] packed (dist bits << 32 | src idx) per target point (the exact K6 atomicMins into it)
-  int *mut_i, *mut_j;         // [S*V] mutual NN list (larger-cloud idx, smaller-cloud idx)
-  unsigned char* mark;        // [S*V] tuple-test survivors
-  int* partner;               // [S*V] tgt partner per source index (-1)
-  float* mean;                // [2S*4]
-  int *corr_src, *corr_tgt;   // [S*Lc]
-  float4 *ma, *mb;            // [S*Lc] matched points (src, tgt)
+  DeviceMem<unsigned long long> rowbest; // [S*V] packed (dist bits << 32 | tgt idx) per source point
+  DeviceMem<unsigned long long> colpart; // [colpart_count()] tensor-core K6 scratch: class results [2][S][V] and the tile-max cache
+                                         // ([S][V/64][2] 32-bit maxima of 32-column groups)
+  DeviceMem<unsigned long long> colbest; // [S*V] packed (dist bits << 32 | src idx) per target point (the exact K6 atomicMins into it)
+  DeviceMem<int> mut_i, mut_j; // [S*V] mutual NN list (larger-cloud idx, smaller-cloud idx)
+  DeviceMem<unsigned char> mark; // [S*V] tuple-test survivors
+  DeviceMem<int> partner;     // [S*V] tgt partner per source index (-1)
+  DeviceMem<float> mean;      // [2S*4]
+  DeviceMem<int> corr_src, corr_tgt; // [S*Lc]
+  DeviceMem<float4> ma, mb;   // [S*Lc] matched points (src, tgt)
   // ---- graph / clique ----
-  uint32_t *adj, *adjp;       // [S*Lc*W] adjacency bits, and the same in (core, id)-rank space
-  int* deg;                   // [S*Lc]
-  int *kcore, *korder, *rank_of, *by_rank, *kbin;  // [S*(Lc+2)]
-  int* clique;                // [S*Lc] ascending ids
-  uint32_t *ex_stack, *ex_pool;  // PMC_EXACT scratch, allocated on first use: [min(S,64)*1024*W] candidate sets per level, [min(S,64)*2^17] list entries
-  int* ex_lvl;                // [2*min(S,64)*1024] list segment (begin | remaining) per level
-  unsigned short* ex_cur;     // [min(S,64)*1024] clique under construction (ranks)
-  unsigned char* kcore_ws;    // [S * kcore_ws_bytes(Lc)] k-core arrays of graphs above kKcoreSmemVerts vertices (Lc > kKcoreSmemVerts only)
-  unsigned short* chain_ws;   // [S*8*Lc] descent chains of those graphs (Lc > kKcoreSmemVerts only)
-  unsigned char* pose_ws;     // [S * pose_ws_bytes(Lc)] pose workspace of cliques above kPoseSmemClique members (Lc > kPoseSmemClique only)
-  int* final_inl;             // [S*Lc]
-  unsigned char *rot_mask, *trans_mask;  // [S*Lc]
+  DeviceMem<uint32_t> adj, adjp; // [S*Lc*W] adjacency bits, and the same in (core, id)-rank space
+  DeviceMem<int> deg;         // [S*Lc]
+  DeviceMem<int> kcore, korder, rank_of, by_rank, kbin; // [S*(Lc+2)]
+  DeviceMem<int> clique;      // [S*Lc] ascending ids
+  DeviceMem<uint32_t> ex_stack, ex_pool; // PMC_EXACT scratch, allocated on first use: [min(S,64)*1024*W] candidate sets per level, [min(S,64)*2^17] list entries
+  DeviceMem<int> ex_lvl;      // [2*min(S,64)*1024] list segment (begin | remaining) per level
+  DeviceMem<unsigned short> ex_cur; // [min(S,64)*1024] clique under construction (ranks)
+  DeviceMem<unsigned char> kcore_ws; // [S * kcore_ws_bytes(Lc)] k-core arrays of graphs above kKcoreSmemVerts vertices (Lc > kKcoreSmemVerts only)
+  DeviceMem<unsigned short> chain_ws; // [S*8*Lc] descent chains of those graphs (Lc > kKcoreSmemVerts only)
+  DeviceMem<unsigned char> pose_ws; // [S * pose_ws_bytes(Lc)] pose workspace of cliques above kPoseSmemClique members (Lc > kPoseSmemClique only)
+  DeviceMem<int> final_inl;   // [S*Lc]
+  DeviceMem<unsigned char> rot_mask, trans_mask; // [S*Lc]
   // ---- pre-processing (preprocess.cu), allocated on first use ----
-  int* pw_ints;               // patch id / rank per point, per-patch counters and offsets
-  float4* pw_out;             // [2*R] ground | non-ground
-  void* ip_buf; int ip_npix;  // range-image scratch (per pixel: winner, parent, size, range, row set, two outputs)
+  DeviceMem<int> pw_ints;     // patch id / rank per point, per-patch counters and offsets
+  DeviceMem<float4> pw_out;   // [2*R] ground | non-ground
+  DeviceMem<void> ip_buf; int ip_npix;  // range-image scratch (per pixel: winner, parent, size, range, row set, two outputs)
   // ---- results ----
-  qb200_result* d_results;    // [S]
-  qb200_result* h_results;    // pinned [S]
+  DeviceMem<qb200_result> d_results; // [S]
+  PinnedMem<qb200_result> h_results; // [S]
   WaveCounters ctr;
-  int* ctr_block; size_t ctr_ints;
+  DeviceMem<int> ctr_block; size_t ctr_ints;
 
-  cudaEvent_t ev[9];          // stage boundaries of the last wave: start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
-  cudaEvent_t kev[4];         // [0,1] around match_stripe_kernel, [2,3] around tim_graph_kernel (last wave)
+  Event ev[9];                // stage boundaries of the last wave: start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
+  Event kev[4];               // [0,1] around match_stripe_kernel, [2,3] around tim_graph_kernel (last wave)
   int kev_armed[2];
 
   void fail(const char* file, int line, const char* msg) { snprintf(err, kErrLen, "%s:%d: %s", file, line, msg); }
   static constexpr int kErrLen = 512;
+
+  // colpart: class-indexed column results [S][V], row results [S][V], then the tile-max cache ([S][V/64][2] u32) and two spare words
+  size_t colpart_count() const { return (size_t)2 * S * V + (size_t)S * (V >> 7) * 2 + 2; }
+  unsigned long long* colpart_col() const { return colpart; }
+  unsigned long long* colpart_row() const { return colpart + (size_t)S * V; }
+  unsigned* colpart_tile_cmax() const { return reinterpret_cast<unsigned*>(colpart + (size_t)2 * S * V); }
+  // the duplicate-class tables K6 keeps in key_a once the norm sort is done with it: class of every rank [2S][V], then the unique
+  // count of every cloud [2S]
+  uint32_t* class_of() const { return reinterpret_cast<uint32_t*>(key_a.get()); }
+  int* n_unique() const { return reinterpret_cast<int*>(class_of() + (size_t)2 * S * V); }
 };
 
 }  // namespace qb
@@ -99,27 +113,29 @@ struct Lane {
 struct qb200_handle {
   qb200_config cfg;
   char err[qb::Lane::kErrLen];
-  qb::Lane* lane[8];          // lane[0] is created with the handle, the others on first use
+  std::unique_ptr<qb::Lane> lane[8];  // lane[0] is created with the handle, the others on first use
   int max_lanes;              // 1..8 (QB200_LANES, default 4)
   int lanes_active, lane_cursor;  // lanes of the rotation in use (0 = nothing in flight), next lane = busy longest
-  cudaEvent_t ev_fork;
-  cudaStream_t copy_stream;   // host scans of a multi-wave batch cross PCIe on ONE stream, wave after wave (api.cu: wave_submit)
-  cudaEvent_t ev_copied;      // a wave's scans have arrived (recorded on the copy stream)
+  qb::Event ev_fork;
+  qb::Stream copy_stream;     // host scans of a multi-wave batch cross PCIe on ONE stream, wave after wave (api.cu: wave_submit)
+  qb::Event ev_copied;        // a wave's scans have arrived (recorded on the copy stream)
 
   // ---- scan cache (qb200_cache_*): front-end results of whole scans, resident on the device ----
   int c_slots;
-  float4 *c_vox, *c_nrm;      // [slots*V]
-  float* c_desc;              // [slots*40*V] dimension-major like desc_t
-  int *c_n, *c_status;        // [slots]
-  int *d_slot_of_cloud, *h_slot_of_cloud;   // [2S] cache slot of every cloud of the current wave (device / pinned)
-  float* c_sig;               // host [slots*4]: (voxel, normal_r, fpfh_r, cell) a slot was computed with
+  qb::DeviceMem<float4> c_vox, c_nrm;  // [slots*V]
+  qb::DeviceMem<float> c_desc;         // [slots*40*V] dimension-major like desc_t
+  qb::DeviceMem<int> c_n, c_status;    // [slots]
+  qb::DeviceMem<int> d_slot_of_cloud;  // [2S] cache slot of every cloud of the current wave
+  qb::PinnedMem<int> h_slot_of_cloud;  // [2S] its pinned mirror
+  std::unique_ptr<float[]> c_sig;      // host [slots*4]: (voxel, normal_r, fpfh_r, cell) a slot was computed with
 
   // ---- multi-GPU gather of the result records (comm.cu) ----
   void* comm;                 // ncclComm_t
   int comm_world, comm_rank, comm_cap;   // cap: records per rank the staging buffers hold
-  cudaStream_t comm_stream;
-  cudaEvent_t comm_done;
-  qb200_result *d_send, *d_recv, *h_send, *h_recv;   // device staging; pinned host staging (h_recv is rank-major)
+  qb::Stream comm_stream;
+  qb::Event comm_done;
+  qb::DeviceMem<qb200_result> d_send, d_recv;  // device staging
+  qb::PinnedMem<qb200_result> h_send, h_recv;  // pinned host staging (h_recv is rank-major)
   int pend_gather_n;          // > 0: a deferred gather is in flight (records per rank)
   qb200_result* pend_gather_dst;
   int pipe_n, pipe_buf;       // pipelined rank mode: local batch queued, gather not started yet (records per rank, half of h_send)

@@ -419,7 +419,7 @@ int launch_match(Lane* h, int n_pairs, const qb200_params& p) {
   static const int verify = (getenv("QB200_TC_VERIFY") && getenv("QB200_TC_VERIFY")[0] == '1') ? 1 : 0;
   if (verify && !h->force_exact_match) {
     // whole-batch self-check: keep the tensor-core results, redo every pair with the exact CUDA-core kernel, compare
-    unsigned long long* rb_tc = reinterpret_cast<unsigned long long*>(h->key_b);                   // the sort workspace is idle here
+    unsigned long long* rb_tc = reinterpret_cast<unsigned long long*>(h->key_b.get());                   // the sort workspace is idle here
     unsigned long long* cb_tc = rb_tc + (size_t)h->S * V;
     QB_CUDA_TRY(h, cudaMemcpyAsync(rb_tc, h->rowbest, (size_t)n_pairs * V * 8, cudaMemcpyDeviceToDevice, h->stream));
     QB_CUDA_TRY(h, cudaMemcpyAsync(cb_tc, h->colbest, (size_t)n_pairs * V * 8, cudaMemcpyDeviceToDevice, h->stream));

@@ -333,12 +333,17 @@ __global__ void __launch_bounds__(256) pw_gather_kernel(const float4* __restrict
   }
 }
 
+// allocated on the first call of a lane: both buffers or neither
 static int ensure_pw_scratch(Lane* h) {
   if (h->pw_ints) return QB200_OK;
   const size_t R = h->R;
+  DeviceMem<int> ints;
+  DeviceMem<float4> out;
   // ints: patch_of [R] | rank [R] | count, start(+1), cursor, n_ground, n_nonground, goff, ngoff [each 4096+1] | out_n [2] | status [1]
-  QB_CUDA_TRY(h, cudaMalloc((void**)&h->pw_ints, (2 * R + 7 * (kPwMaxPatches + 1) + 4) * sizeof(int)));
-  QB_CUDA_TRY(h, cudaMalloc((void**)&h->pw_out, 2 * R * sizeof(float4)));
+  QB_CUDA_TRY(h, ints.alloc(2 * R + 7 * (kPwMaxPatches + 1) + 4));
+  QB_CUDA_TRY(h, out.alloc(2 * R));
+  h->pw_ints = std::move(ints);
+  h->pw_out = std::move(out);
   return QB200_OK;
 }
 
@@ -366,7 +371,7 @@ int launch_patchwork(Lane* h, const float4* pts, int n, const qb200_patchwork_pa
   int* goff = ng_non + (kPwMaxPatches + 1);
   int* ngoff = goff + (kPwMaxPatches + 1);
   int* out_n = ngoff + (kPwMaxPatches + 1);   // [0] ground, [1] non-ground, [2] status
-  unsigned long long* items = reinterpret_cast<unsigned long long*>(h->key_a);   // [>= R]
+  unsigned long long* items = reinterpret_cast<unsigned long long*>(h->key_a.get());   // [>= R]
   QB_CUDA_TRY(h, cudaMemsetAsync(count, 0, (kPwMaxPatches + 1) * sizeof(int), h->stream));
   QB_CUDA_TRY(h, cudaMemsetAsync(out_n, 0, 4 * sizeof(int), h->stream));
   const int nb = (n + 255) / 256;
@@ -560,11 +565,13 @@ __global__ void __launch_bounds__(1024) ip_extract_kernel(const float4* __restri
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) { out_n[0] = s_base[0] + (both & 0xFFFF); out_n[1] = s_base[1] + (both >> 16); }
 }
 
+// grown to the largest image of the lane so far; a failed call keeps the old buffer
 static int ensure_ip_scratch(Lane* h, int npix) {
   if (h->ip_buf && h->ip_npix >= npix) return QB200_OK;
-  if (h->ip_buf) { cudaFree(h->ip_buf); h->ip_buf = nullptr; }
+  DeviceMem<void> buf;
   // per pixel: rows u64 | valid float4 | outlier float4 | winner, parent, size int | range float | kind u8 ; + out_n [2] + block counts
-  QB_CUDA_TRY(h, cudaMalloc((void**)&h->ip_buf, (size_t)npix * (8 + 16 + 16 + 4 * 4 + 1) + 16 + 8 * (size_t)((npix + 1023) / 1024) + 64));
+  QB_CUDA_TRY(h, buf.alloc_bytes((size_t)npix * (8 + 16 + 16 + 4 * 4 + 1) + 16 + 8 * (size_t)((npix + 1023) / 1024) + 64));
+  h->ip_buf = std::move(buf);
   h->ip_npix = npix;
   return QB200_OK;
 }
@@ -582,7 +589,7 @@ int launch_segment_cloud(Lane* h, const float4* pts, int n, const qb200_segment_
   if (!ip_params_valid(sp)) return QB200_ERR_BAD_ARG;
   const int npix = sp.n_scan * sp.horizon_scan;
   if (int rc = ensure_ip_scratch(h, npix)) return rc;
-  unsigned char* b = reinterpret_cast<unsigned char*>(h->ip_buf);
+  unsigned char* b = reinterpret_cast<unsigned char*>(h->ip_buf.get());
   float4* valid = reinterpret_cast<float4*>(b); b += (size_t)npix * 16;      // 16-byte records first: aligned for any image size
   float4* outlier = reinterpret_cast<float4*>(b); b += (size_t)npix * 16;
   unsigned long long* rows = reinterpret_cast<unsigned long long*>(b); b += (size_t)npix * 8;

@@ -904,9 +904,7 @@ static int sort_and_dedup(Lane* h, int n_clouds, int dedup) {
   int rc = launch_cloud_sort(h, n_clouds, h->ctr.n_vox, 32, 32);  // per-cloud shared-memory sort; device-wide radix sort for very large clouds
   if (rc == QB200_ERR_UNSUPPORTED) rc = sort_pairs(h, n_clouds * V, 32 + bits);
   if (rc) return rc;
-  uint32_t* class_of = reinterpret_cast<uint32_t*>(h->key_a);
-  int* n_unique = reinterpret_cast<int*>(class_of + (size_t)2 * h->S * V);
-  dedup_kernel<<<n_clouds, 1024, 0, h->stream>>>(h->desc_t, h->ctr.n_vox, V, h->key_b, h->val_b, dedup, h->val_a, class_of, n_unique);
+  dedup_kernel<<<n_clouds, 1024, 0, h->stream>>>(h->desc_t, h->ctr.n_vox, V, h->key_b, h->val_b, dedup, h->val_a, h->class_of(), h->n_unique());
   h->launches += 1;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;
@@ -919,15 +917,15 @@ int launch_match_nn(Lane* h, int n_pairs) {
   int rc = sort_and_dedup(h, 2 * n_pairs, 1);
   if (rc) return rc;
   const uint32_t* uperm = h->val_a;
-  const uint32_t* class_of = reinterpret_cast<const uint32_t*>(h->key_a);
-  const int* n_unique = reinterpret_cast<const int*>(class_of + (size_t)2 * h->S * V);
+  const uint32_t* class_of = h->class_of();
+  const int* n_unique = h->n_unique();
   // class results, indexed by unique rank (colpart is this kernel's scratch; the exact fallback works in rowbest / colbest)
-  unsigned long long* colbest_u = h->colpart;
-  unsigned long long* rowbest_u = h->colpart + (size_t)h->S * V;
-  unsigned* tile_cmax = reinterpret_cast<unsigned*>(h->colpart + (size_t)2 * h->S * V);  // [S][V/64][2] float bits, start above "+inf"
+  unsigned long long* colbest_u = h->colpart_col();
+  unsigned long long* rowbest_u = h->colpart_row();
+  unsigned* tile_cmax = h->colpart_tile_cmax();  // [S][V/64][2] float bits, start above "+inf"
   QB_CUDA_TRY(h, cudaMemsetAsync(h->rowbest, 0xFF, (size_t)n_pairs * V * 8, h->stream));
   QB_CUDA_TRY(h, cudaMemsetAsync(h->colbest, 0xFF, (size_t)n_pairs * V * 8, h->stream));
-  QB_CUDA_TRY(h, cudaMemsetAsync(h->colpart, 0xFF, ((size_t)2 * h->S * V + (size_t)h->S * (V >> 7) * 2 + 2) * 8, h->stream));  // 0xFFFFFFFF > +inf bits
+  QB_CUDA_TRY(h, cudaMemsetAsync(h->colpart, 0xFF, h->colpart_count() * 8, h->stream));  // 0xFFFFFFFF > +inf bits
   QB_CUDA_TRY(h, cudaMemsetAsync(h->tc_fallback, 0, (size_t)n_pairs * sizeof(int), h->stream));
   const dim3 gsplit((V + 255) / 256, 2 * n_pairs);
   split_desc_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_t, n_unique, V, uperm, h->desc_tiles, h->desc_norm, h->tc_fallback);
@@ -958,14 +956,14 @@ int launch_tc_debug_tile(Lane* h, float* d_out) {
   int rc = sort_and_dedup(h, 2, 0);
   if (rc) return rc;
   const uint32_t* uperm = h->val_a;
-  const int* n_unique = reinterpret_cast<const int*>(reinterpret_cast<const uint32_t*>(h->key_a) + (size_t)2 * h->S * h->V);
-  QB_CUDA_TRY(h, cudaMemsetAsync(h->colpart, 0xFF, ((size_t)2 * h->S * h->V + (size_t)h->S * (h->V >> 7) * 2 + 2) * 8, h->stream));
+  const int* n_unique = h->n_unique();
+  QB_CUDA_TRY(h, cudaMemsetAsync(h->colpart, 0xFF, h->colpart_count() * 8, h->stream));
   QB_CUDA_TRY(h, cudaMemsetAsync(h->tc_fallback, 0, sizeof(int), h->stream));
   const dim3 gsplit((h->V + 255) / 256, 2);
   split_desc_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_t, n_unique, h->V, uperm, h->desc_tiles, h->desc_norm, h->tc_fallback);
   const dim3 g(1, 1);
-  tc_nn_kernel<true><<<g, kTcThreads, smem, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, h->V, uperm, h->colpart + (size_t)h->S * h->V,
-                                                         h->colpart, reinterpret_cast<unsigned*>(h->colpart + (size_t)2 * h->S * h->V), h->tc_fallback, h->tc_stats, d_out);
+  tc_nn_kernel<true><<<g, kTcThreads, smem, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, h->V, uperm, h->colpart_row(), h->colpart_col(),
+                                                         h->colpart_tile_cmax(), h->tc_fallback, h->tc_stats, d_out);
   h->launches += 2;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;

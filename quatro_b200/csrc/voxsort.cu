@@ -193,8 +193,8 @@ __global__ void __launch_bounds__(kVsThreads) vsort_scatter_kernel(int pass, con
 // (vox_digits(c) odd ? B : A) + raw_off[c] and holds n_valid[c] items.
 int launch_voxel_sort(Lane* h, int n_clouds, float inv_leaf, int skip_flagged, int idx_bits) {
   const int tiles_cap = (h->R + kVsTile - 1) / kVsTile;
-  unsigned* hist = reinterpret_cast<unsigned*>(h->val_a);        // [clouds][256][tiles_cap]  (alloc_all sizes val_a for it)
-  const int* chunk_cnt = reinterpret_cast<const int*>(h->val_b); // [clouds][64]
+  unsigned* hist = reinterpret_cast<unsigned*>(h->val_a.get());        // [clouds][256][tiles_cap]  (alloc_all sizes val_a for it)
+  const int* chunk_cnt = reinterpret_cast<const int*>(h->val_b.get()); // [clouds][64]
   const dim3 gp(kVsChunks, n_clouds), gt(tiles_cap, n_clouds);
   voxel_pack_kernel<<<gp, kVsThreads, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, h->d_raw_off, inv_leaf, skip_flagged, h->ctr.bbox, h->ctr.n_valid,
                                                      chunk_cnt, idx_bits, h->key_a);
