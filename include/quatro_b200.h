@@ -18,6 +18,8 @@
  *   qb200_match_and_pack        <- FPFHManager::setFeaturePair          include/fpfh_manager.hpp:98-153
  *   qb200_register_pair/_batch  <- examples/run_global_registration.cpp:206-246 (voxelize .. computeTransformation)
  *   qb200_register_batch_sharded / _rank  <- the same loop over a list of pairs, sharded over the GPUs of one box
+ *   qb200_pair_lists (_ex forms) <- FPFHManager::getCorrespondences, Quatro::getMaxCliques / getFinalInliersIndices for every
+ *                                  pair of a batch (examples/run_global_registration.cpp:268, 292)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -285,6 +287,36 @@ typedef struct qb200_corr_set {
 int qb200_solve_batch(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p,
                       qb200_mem_kind kind, qb200_result* results);
 
+/* --- per-pair lists of the batch entry points: correspondences, max clique, final inliers, inlier masks -------------------------
+ * The single-pair getters (qb200_get_last_*) read slot 0 after a single-pair call; the _ex forms of the batch entry points hand out
+ * the same lists for every pair of a batch.  The caller owns every array; pair i's entries start at i * cap_per_pair whatever wave or
+ * lane ran it.  Pair i gets min(count, cap_per_pair) entries of each list, count taken from its record: n_corr for corr and the
+ * matched points, clique_size for the clique and both masks, n_final_inliers for the final inliers.  Entries past that count are
+ * left untouched, and a pair whose status is QB200_CAPACITY_EXCEEDED gets no entries.  A pair whose clique has at most one member
+ * is not solved: its mask entries are 0.  When a list that was asked for (a non-NULL array) held more than cap_per_pair entries,
+ * the pair's record carries QB200_FLAG_LISTS_TRUNCATED; records of calls without lists never do.  The lists never depend on the
+ * wave size, the lane count, the destination kind, or whether the pair came through the scan cache.
+ * QB200_MEM_HOST arrays are complete when the call returns (enqueue: when the flush returns).  QB200_MEM_DEVICE arrays (memory of
+ * the handle's device; corr 8-byte, matched points 16-byte aligned) are written by the call's stream work and are complete when it
+ * is done, under the same rule.  The descriptor itself is copied by the call. */
+typedef struct qb200_pair_lists {
+  int32_t cap_per_pair;       /* 1 .. max_corr: entries reserved per pair in every array below */
+  int32_t kind;               /* qb200_mem_kind of every array below (QB200_MEM_DEVICE: memory of the handle's device) */
+  int32_t* corr;              /* [n][cap][2] (source voxel idx, target voxel idx), same order as qb200_get_last_correspondences */
+  float* src_matched4;        /* [n][cap][4] matched points (getSrcKps), aligned with corr */
+  float* tgt_matched4;        /* [n][cap][4] */
+  int32_t* clique;            /* [n][cap] ascending correspondence ids = qb200_get_last_clique (getMaxCliques) */
+  int32_t* final_inliers;     /* [n][cap] = qb200_get_last_final_inliers (getFinalInliersIndices) */
+  uint8_t* rot_inlier_mask;   /* [n][cap] per clique member, as qb200_solve_pose writes it */
+  uint8_t* trans_inlier_mask; /* [n][cap] */
+} qb200_pair_lists;           /* any array may be NULL: nothing is written to it */
+enum { QB200_FLAG_LISTS_TRUNCATED = 2 /* a list of this pair had more than cap_per_pair entries */ };
+
+/* qb200_solve_batch + the lists (Quatro::getMaxCliques / getFinalInliersIndices, include/quatro.hpp:949-972).  The caller supplied
+ * the correspondences, so corr, src_matched4 and tgt_matched4 must be NULL (else QB200_ERR_BAD_ARG). */
+int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p, qb200_mem_kind kind,
+                         qb200_result* results, const qb200_pair_lists* lists);
+
 /* Pipelined form of qb200_register_batch for a stream of batches: _enqueue queues the batch and returns (it collects a lane's
  * earlier wave only when it needs that lane again), so the single-warp tail of one batch runs under the PCIe copies and front-end
  * kernels of the next; _flush waits for everything queued and completes the record arrays.  The scans (host kind) and `results` of
@@ -293,6 +325,9 @@ int qb200_solve_batch(qb200_handle* h, const qb200_corr_set* sets, int32_t n_set
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                                  qb200_result* results);
 int qb200_register_batch_flush(qb200_handle* h);
+/* qb200_register_batch_enqueue + the lists of qb200_register_batch_ex; the arrays must stay valid until the flush, as results must */
+int qb200_register_batch_enqueue_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p,
+                                    qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
 
 /* raw scans in -> pose out. */
 int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const float* tgt4,
@@ -306,6 +341,11 @@ int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const
  * or the lane. */
 int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs,
                          const qb200_params* p, qb200_mem_kind kind, qb200_result* results);
+/* qb200_register_batch + every pair's lists: FPFHManager::getCorrespondences / getSrcKps / getTgtKps (include/fpfh_manager.hpp:
+ * 234-236), Quatro::getMaxCliques / getFinalInliersIndices (include/quatro.hpp:949-972).  lists == NULL: = qb200_register_batch.
+ * With one pair it also sets what qb200_get_last_* read. */
+int qb200_register_batch_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
+                            qb200_result* results, const qb200_pair_lists* lists);
 
 /* --- scan cache: one scan against many (loop-closure sweeps) and odometry chains -------------------------------------------------
  * FPFHManager keeps the previous target's cloud and descriptors and reuses them as the next source (swapTgt2Src / is_odometry_test_,
@@ -322,6 +362,10 @@ int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t
 /* match + graph + clique + pose for pairs of cached scans (= qb200_register_batch without its front end); p's front-end parameters
  * must be the ones the slots were cached with */
 int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_result* results);
+/* qb200_register_cached + the lists of qb200_register_batch_ex (getCorrespondences, getMaxCliques, getFinalInliersIndices); corr
+ * indexes the voxel order qb200_cache_read returns */
+int qb200_register_cached_ex(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p,
+                             qb200_result* results, const qb200_pair_lists* lists);
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot);   /* swapTgt2Src */
 /* read a cached scan back: voxel points (n x 4), normals (n x {nx,ny,nz,curvature}), descriptors (n x 33); any may be NULL */
 int qb200_cache_read(qb200_handle* h, int32_t slot, float* vox4, float* normals4, float* desc33, int32_t cap, int32_t* n);

@@ -14,6 +14,7 @@ from . import _build
 
 PMC_EXACT, PMC_HEU, KCORE_HEU, INLIER_NONE = 0, 1, 2, 3
 FLAG_CLIQUE_TRUNCATED = 1
+FLAG_LISTS_TRUNCATED = 2
 COTE_MEDIAN, COTE_WEIGHTED_MEAN = 0, 1
 MEM_HOST, MEM_DEVICE = 0, 1
 
@@ -85,6 +86,65 @@ class Pair(C.Structure):
 
 class CorrSet(C.Structure):
     _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("L", C.c_int32), ("reserved", C.c_int32)]
+
+
+class PairLists(C.Structure):
+    """qb200_pair_lists: caller-owned per-pair lists of the batch entry points, cap_per_pair entries reserved per pair."""
+    _fields_ = [("cap_per_pair", C.c_int32), ("kind", C.c_int32), ("corr", C.c_void_p), ("src_matched4", C.c_void_p),
+                ("tgt_matched4", C.c_void_p), ("clique", C.c_void_p), ("final_inliers", C.c_void_p),
+                ("rot_inlier_mask", C.c_void_p), ("trans_inlier_mask", C.c_void_p)]
+
+
+# list name -> (element dtype, trailing shape, count field of the record)
+LIST_LAYOUT = {
+    "corr": (np.int32, (2,), "n_corr"),
+    "src_matched4": (np.float32, (4,), "n_corr"),
+    "tgt_matched4": (np.float32, (4,), "n_corr"),
+    "clique": (np.int32, (), "clique_size"),
+    "final_inliers": (np.int32, (), "n_final_inliers"),
+    "rot_inlier_mask": (np.uint8, (), "clique_size"),
+    "trans_inlier_mask": (np.uint8, (), "clique_size"),
+}
+SET_LISTS = ("clique", "final_inliers", "rot_inlier_mask", "trans_inlier_mask")   # what qb200_solve_batch_ex can return
+
+
+class ListBuffers:
+    """The arrays of one qb200_pair_lists: zeroed numpy arrays (MEM_HOST) or CUDA tensors of `device` (MEM_DEVICE), each of shape
+    (n, cap, *trailing)."""
+
+    def __init__(self, n: int, cap: int, kind: int = MEM_HOST, lists: Sequence[str] = tuple(LIST_LAYOUT), device: int = 0):
+        self.n, self.cap, self.kind = n, cap, kind
+        self.arrays = {}
+        for name in lists:
+            dt, tail, _ = LIST_LAYOUT[name]
+            shape = (max(n, 1), cap, *tail)
+            if kind == MEM_HOST:
+                self.arrays[name] = np.zeros(shape, dt)
+            else:
+                import torch
+                self.arrays[name] = torch.zeros(shape, dtype=getattr(torch, np.dtype(dt).name), device=f"cuda:{device}")
+
+    def descriptor(self) -> PairLists:
+        d = PairLists(self.cap, self.kind)
+        for name, a in self.arrays.items():
+            setattr(d, name, a.ctypes.data if self.kind == MEM_HOST else a.data_ptr())
+        return d
+
+    def host(self, name: str) -> np.ndarray:
+        a = self.arrays[name]
+        return a if self.kind == MEM_HOST else a.cpu().numpy()
+
+    def trimmed(self, records: np.ndarray) -> list:
+        """Per pair a dict of its lists cut to min(count, cap) entries (numpy copies, or tensor views on the device); a pair whose status
+        is CAPACITY_EXCEEDED gets empty lists."""
+        out = []
+        for i, r in enumerate(records):
+            d = {}
+            for name, a in self.arrays.items():
+                m = 0 if r["status"] == 3 else min(int(r[LIST_LAYOUT[name][2]]), self.cap)
+                d[name] = a[i, :m].copy() if self.kind == MEM_HOST else a[i, :m]
+            out.append(d)
+        return out
 
 
 RESULT_DTYPE = np.dtype([
@@ -175,6 +235,10 @@ def load_library(build: bool = True) -> C.CDLL:
         "qb200_register_cached": (i32, [vp, vp, i32, P(Params), vp]),
         "qb200_cache_copy": (i32, [vp, i32, i32]),
         "qb200_cache_read": (i32, [vp, i32, vp, vp, vp, i32, P(i32)]),
+        "qb200_register_batch_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+        "qb200_register_batch_enqueue_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+        "qb200_register_cached_ex": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
+        "qb200_solve_batch_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError = header/library mismatch: fail loudly
@@ -201,6 +265,7 @@ EXPORTED_SYMBOLS = [
     "qb200_comm_init_all", "qb200_register_batch_sharded", "qb200_comm_unique_id", "qb200_comm_init_rank",
     "qb200_register_batch_rank", "qb200_comm_wait", "qb200_bind_numa",
     "qb200_debug_match_verify", "qb200_get_last_features", "qb200_cache_reserve", "qb200_cache_scans", "qb200_register_cached", "qb200_cache_copy", "qb200_cache_read",
+    "qb200_register_batch_ex", "qb200_register_batch_enqueue_ex", "qb200_register_cached_ex", "qb200_solve_batch_ex",
 ]
 
 
@@ -427,11 +492,10 @@ class Handle:
                          "qb200_register_pair")
         return res, st
 
-    def register_batch(self, pairs: Sequence, params: Params, kind: int = MEM_HOST) -> np.ndarray:
-        """pairs: sequence of (src, tgt).  MEM_HOST: numpy (n,4) float32 arrays; MEM_DEVICE:
-        (src_ptr, n_src, tgt_ptr, n_tgt) tuples of raw device addresses.  Returns a RESULT_DTYPE array."""
-        n = len(pairs)
-        arr = (Pair * n)()
+    @staticmethod
+    def pair_array(pairs: Sequence, kind: int = MEM_HOST):
+        """(Pair * n) array of `pairs` and the contiguous scans it points to (keep them alive while the array is in use)."""
+        arr = (Pair * len(pairs))()
         keep = []
         for i, pr in enumerate(pairs):
             if kind == MEM_HOST:
@@ -440,15 +504,11 @@ class Handle:
                 arr[i].src, arr[i].n_src, arr[i].tgt, arr[i].n_tgt = s.ctypes.data, len(s), t.ctypes.data, len(t)
             else:
                 arr[i].src, arr[i].n_src, arr[i].tgt, arr[i].n_tgt = pr[0], pr[1], pr[2], pr[3]
-        out = np.zeros(n, RESULT_DTYPE)
-        self._check(self.lib.qb200_register_batch(self.h, arr, n, C.byref(params), kind, _ptr(out)), "qb200_register_batch")
-        return out
+        return arr, keep
 
-    def solve_batch(self, sets: Sequence, params: Params, kind: int = MEM_HOST) -> np.ndarray:
-        """sets: sequence of (a4, b4) matched point arrays (MEM_HOST: numpy (L,4) float32; MEM_DEVICE: (a_ptr, b_ptr, L)).
-        Graph -> clique -> pose for every set; returns a RESULT_DTYPE array."""
-        n = len(sets)
-        arr = (CorrSet * n)()
+    @staticmethod
+    def _set_array(sets: Sequence, kind: int):
+        arr = (CorrSet * len(sets))()
         keep = []
         for i, st in enumerate(sets):
             if kind == MEM_HOST:
@@ -458,9 +518,69 @@ class Handle:
                 arr[i].a, arr[i].b, arr[i].L = a.ctypes.data, b.ctypes.data, len(a)
             else:
                 arr[i].a, arr[i].b, arr[i].L = st[0], st[1], st[2]
-        out = np.zeros(n, RESULT_DTYPE)
-        self._check(self.lib.qb200_solve_batch(self.h, arr, n, C.byref(params), kind, _ptr(out)), "qb200_solve_batch")
+        return arr, keep
+
+    def register_batch(self, pairs: Sequence, params: Params, kind: int = MEM_HOST) -> np.ndarray:
+        """pairs: sequence of (src, tgt).  MEM_HOST: numpy (n,4) float32 arrays; MEM_DEVICE:
+        (src_ptr, n_src, tgt_ptr, n_tgt) tuples of raw device addresses.  Returns a RESULT_DTYPE array."""
+        arr, keep = self.pair_array(pairs, kind)
+        out = np.zeros(len(pairs), RESULT_DTYPE)
+        self._check(self.lib.qb200_register_batch(self.h, arr, len(pairs), C.byref(params), kind, _ptr(out)), "qb200_register_batch")
         return out
+
+    def solve_batch(self, sets: Sequence, params: Params, kind: int = MEM_HOST) -> np.ndarray:
+        """sets: sequence of (a4, b4) matched point arrays (MEM_HOST: numpy (L,4) float32; MEM_DEVICE: (a_ptr, b_ptr, L)).
+        Graph -> clique -> pose for every set; returns a RESULT_DTYPE array."""
+        arr, keep = self._set_array(sets, kind)
+        out = np.zeros(len(sets), RESULT_DTYPE)
+        self._check(self.lib.qb200_solve_batch(self.h, arr, len(sets), C.byref(params), kind, _ptr(out)), "qb200_solve_batch")
+        return out
+
+    # ---- per-pair lists of the batch entry points (qb200_pair_lists) ----
+    # Each returns (records, lists): lists[i] is a dict of pair i's lists cut to their counts (ListBuffers.trimmed).  dest picks
+    # where the call writes them (MEM_HOST: numpy, MEM_DEVICE: CUDA tensors of the handle's device); `buffers` hands in
+    # caller-made ListBuffers instead (cap_per_pair / dest are then theirs).
+    def _lists_for(self, n: int, cap_per_pair: Optional[int], dest: int, buffers: Optional[ListBuffers], names) -> ListBuffers:
+        return buffers or ListBuffers(n, cap_per_pair or self.cfg.max_corr, dest, names, self.cfg.device)
+
+    def register_batch_lists(self, pairs: Sequence, params: Params, kind: int = MEM_HOST, cap_per_pair: Optional[int] = None,
+                             dest: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
+        """qb200_register_batch_ex: register_batch + every pair's correspondences, matched points, clique, final inliers and masks."""
+        arr, keep = self.pair_array(pairs, kind)
+        out = np.zeros(len(pairs), RESULT_DTYPE)
+        lb = self._lists_for(len(pairs), cap_per_pair, dest, buffers, tuple(LIST_LAYOUT))
+        d = lb.descriptor()
+        self._check(self.lib.qb200_register_batch_ex(self.h, arr, len(pairs), C.byref(params), kind, _ptr(out), C.byref(d)),
+                    "qb200_register_batch_ex")
+        return out, lb.trimmed(out)
+
+    def register_batch_enqueue_lists_raw(self, pair_array, n: int, params: Params, kind: int, out: np.ndarray, buffers: ListBuffers):
+        """qb200_register_batch_enqueue_ex: pair_array, its scans, `out` and the buffers must stay alive until register_batch_flush."""
+        d = buffers.descriptor()
+        return self._check(self.lib.qb200_register_batch_enqueue_ex(self.h, pair_array, n, C.byref(params), kind, _ptr(out), C.byref(d)),
+                           "qb200_register_batch_enqueue_ex")
+
+    def register_cached_lists(self, slot_pairs, params: Params, cap_per_pair: Optional[int] = None, dest: int = MEM_HOST,
+                              buffers: Optional[ListBuffers] = None):
+        """qb200_register_cached_ex: corr indexes the voxel points cache_read returns."""
+        sp = np.ascontiguousarray(np.asarray(slot_pairs, np.int32).reshape(-1, 2))
+        out = np.zeros(len(sp), RESULT_DTYPE)
+        lb = self._lists_for(len(sp), cap_per_pair, dest, buffers, tuple(LIST_LAYOUT))
+        d = lb.descriptor()
+        self._check(self.lib.qb200_register_cached_ex(self.h, _ptr(sp), len(sp), C.byref(params), _ptr(out), C.byref(d)),
+                    "qb200_register_cached_ex")
+        return out, lb.trimmed(out)
+
+    def solve_batch_lists(self, sets: Sequence, params: Params, kind: int = MEM_HOST, cap_per_pair: Optional[int] = None,
+                          dest: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
+        """qb200_solve_batch_ex: solve_batch + every set's clique, final inliers and masks (the caller has the correspondences)."""
+        arr, keep = self._set_array(sets, kind)
+        out = np.zeros(len(sets), RESULT_DTYPE)
+        lb = self._lists_for(len(sets), cap_per_pair, dest, buffers, SET_LISTS)
+        d = lb.descriptor()
+        self._check(self.lib.qb200_solve_batch_ex(self.h, arr, len(sets), C.byref(params), kind, _ptr(out), C.byref(d)),
+                    "qb200_solve_batch_ex")
+        return out, lb.trimmed(out)
 
     def last_features(self, which: int, cap: Optional[int] = None):
         """(normals (n,4), descriptors (n,33)) of the source (0) / target (1) cloud of the last match_and_pack."""

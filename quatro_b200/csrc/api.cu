@@ -380,7 +380,81 @@ struct WaveInput {
   // several streams share the PCIe link, so every wave's scans would arrive late; on one stream they arrive wave after wave and
   // the first waves compute while the later ones are still crossing.
   cudaStream_t copy_stream = nullptr;
+  // the batch's per-pair lists (qb200_pair_lists), nullptr = records only
+  const qb200_pair_lists* lists = nullptr;
 };
+
+// Host-kind lists: the lane's pinned staging block holds cap entries of every list for each slot.  It only grows, and a failed
+// allocation leaves the lane as it was.  The lane's previous wave has been collected, so the old block is not in use.
+int ensure_list_stage(Lane* L, const qb200_pair_lists& l) {
+  if (L->lst_cap >= l.cap_per_pair) return QB200_OK;
+  ListDst d;
+  PinnedMem<unsigned char> m;
+  QB_CUDA_TRY(L, m.alloc(ListDst::carve(nullptr, L->S, l.cap_per_pair, l, &d)));
+  L->lst_stage = std::move(m);
+  L->lst_cap = l.cap_per_pair;
+  return QB200_OK;
+}
+
+// Enqueue the list pack of the wave on lane L (pairs [w0, w0 + np)): straight into the caller's device arrays, or into the lane's
+// staging block that wave_collect hands on to the caller's host arrays.  It marks clipped records, so it precedes their D2H.
+int submit_lists(Lane* L, const qb200_pair_lists& l, int w0, int np) {
+  int rc;
+  ListDst d = ListDst::caller(l, w0);
+  if (l.kind == QB200_MEM_HOST) {
+    if ((rc = ensure_list_stage(L, l))) return rc;
+    ListDst::carve(L->lst_stage, L->S, L->lst_cap, l, &d);
+  }
+  return launch_pack_lists(L, np, d);
+}
+
+// the live prefix of every pair's lists from the lane's staging block to the caller's host arrays (h_results holds the records)
+void deliver_lists(Lane* L, const qb200_pair_lists& l, int w0, int np) {
+  ListDst st, to = ListDst::caller(l, w0);
+  ListDst::carve(L->lst_stage, L->S, L->lst_cap, l, &st);
+  auto put = [](auto* dst, const auto* src, size_t d0, size_t s0, int m) {
+    if (dst && m > 0) memcpy(dst + d0, src + s0, (size_t)m * sizeof(*dst));
+  };
+  for (int s = 0; s < np; ++s) {
+    const qb200_result& r = L->h_results[s];
+    if (r.status == QB200_CAPACITY_EXCEEDED) continue;
+    const int mc = list_entries(r.n_corr, L->Lc, to.cap), mq = list_entries(r.clique_size, L->Lc, to.cap);
+    const size_t d0 = (size_t)s * to.stride, s0 = (size_t)s * st.stride;
+    put(to.corr, st.corr, d0, s0, mc);
+    put(to.sm, st.sm, d0, s0, mc);
+    put(to.tm, st.tm, d0, s0, mc);
+    put(to.clique, st.clique, d0, s0, mq);
+    put(to.rm, st.rm, d0, s0, mq);
+    put(to.tmask, st.tmask, d0, s0, mq);
+    put(to.fin, st.fin, d0, s0, list_entries(r.n_final_inliers, L->Lc, to.cap));
+  }
+}
+
+// A list descriptor from the caller: capacity and kind in range, device arrays on the handle's device and aligned for the pack's
+// vector stores; for_sets: the caller supplied the correspondences, so there are none to hand back.
+int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
+  if (!l) return QB200_OK;
+  const char* why = nullptr;
+  if (l->cap_per_pair < 1 || l->cap_per_pair > h->cfg.max_corr) why = "cap_per_pair outside 1 .. max_corr";
+  else if (l->kind != QB200_MEM_HOST && l->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the lists";
+  else if (for_sets && (l->corr || l->src_matched4 || l->tgt_matched4)) why = "a correspondence-set batch has no corr / matched points to return";
+  else if (l->kind == QB200_MEM_DEVICE) {
+    if (((uintptr_t)l->corr & 7) || ((uintptr_t)l->src_matched4 & 15) || ((uintptr_t)l->tgt_matched4 & 15)) why = "device corr / matched points misaligned";
+    const void* arrays[] = {l->corr, l->src_matched4, l->tgt_matched4, l->clique, l->final_inliers, l->rot_inlier_mask, l->trans_inlier_mask};
+    for (const void* a : arrays) {
+      cudaPointerAttributes at;
+      if (!a || why) continue;
+      if (cudaPointerGetAttributes(&at, a) != cudaSuccess || at.device != h->cfg.device ||
+          (at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged)) {
+        cudaGetLastError();
+        why = "device list array is not memory of the handle's device";
+      }
+    }
+  }
+  if (!why) return QB200_OK;
+  h->fail(__FILE__, __LINE__, why);
+  return QB200_ERR_BAD_ARG;
+}
 
 // Enqueue one wave (pairs [w0, w0 + np), np <= S) on lane L: the front of the wave its input needs (raw scans: H2D, K1..K6;
 // cached scans: the copy out of the cache, K6; correspondence sets: their H2D), then K8..K11 and the D2H of the result records.
@@ -436,11 +510,14 @@ int wave_submit(qb200_handle* h, Lane* L, const WaveInput& in, int w0, int np, c
   cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
   if ((rc = run_solver(L, np, p, in.sets ? 0 : 1))) return rc;
   cudaEventRecord(L->ev[7], L->stream);
+  if (in.lists && (rc = submit_lists(L, *in.lists, w0, np))) return rc;
   QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
   cudaEventRecord(L->ev[8], L->stream);
   L->pend_w0 = w0;
   L->pend_np = np;
   L->pend_dst = dst;
+  if (in.lists) L->pend_lists = *in.lists;
+  else L->pend_lists.cap_per_pair = 0;
   // stage-time slots of qb200_get_stage_ms this wave reports: raw scans all eight, the other inputs their first stage to pose
   L->pend_t0 = in.pairs ? 0 : in.slots ? 2 : 4;
   L->pend_t1 = in.pairs ? 8 : 7;
@@ -457,6 +534,7 @@ int wave_collect(qb200_handle* h, Lane* L) {
     return QB200_ERR_CUDA;
   }
   memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
+  if (L->pend_lists.cap_per_pair > 0 && L->pend_lists.kind == QB200_MEM_HOST) deliver_lists(L, L->pend_lists, L->pend_w0, np);
   static const int timeline = (getenv("QB200_TIMELINE") && getenv("QB200_TIMELINE")[0] == '1') ? 1 : 0;
   if (timeline && L->pend_t0 == 0) {  // stage boundaries of a raw-scan wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
     fprintf(stderr, "[qb200 timeline] wave w0=%d np=%d:", L->pend_w0, np);
@@ -907,8 +985,14 @@ int qb200_solve_correspondences(qb200_handle* h, const float* a4, const float* b
 // ---- batches of precomputed correspondences -> poses ------------------------------------------------------
 int qb200_solve_batch(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p, qb200_mem_kind kind,
                       qb200_result* results) {
+  return qb200_solve_batch_ex(h, sets, n_sets, p, kind, results, nullptr);
+}
+
+int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p, qb200_mem_kind kind,
+                         qb200_result* results, const qb200_pair_lists* lists) {
   if (int rc = enter(h)) return rc;
   if (n_sets < 0 || (n_sets > 0 && (!sets || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
+  if (int rc = check_lists(h, lists, true)) return rc;
   for (int i = 0; i < n_sets; ++i)
     if (sets[i].L < 0 || sets[i].L > h->cfg.max_corr || (sets[i].L > 0 && (!sets[i].a || !sets[i].b))) {
       h->fail(__FILE__, __LINE__, "correspondence set is null or exceeds max_corr");
@@ -917,6 +1001,7 @@ int qb200_solve_batch(qb200_handle* h, const qb200_corr_set* sets, int32_t n_set
   WaveInput in;
   in.sets = sets;
   in.kind = kind;
+  in.lists = lists;
   return run_waves(h, in, n_sets, n_sets > 0 ? resolve_params(h, *p) : *p, results);
 }
 
@@ -925,7 +1010,12 @@ int qb200_register_batch_flush(qb200_handle* h) { return enter(h); }
 
 int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                          qb200_result* results) {
-  int rc = qb200_register_batch_enqueue(h, pairs, n_pairs, p, kind, results);
+  return qb200_register_batch_ex(h, pairs, n_pairs, p, kind, results, nullptr);
+}
+
+int qb200_register_batch_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
+                            qb200_result* results, const qb200_pair_lists* lists) {
+  int rc = qb200_register_batch_enqueue_ex(h, pairs, n_pairs, p, kind, results, lists);
   const int rc2 = h ? batch_flush(h) : QB200_OK;  // on an error still wait for everything in flight (the copies read caller memory)
   if (rc == QB200_OK) rc = rc2;
   if (rc != QB200_OK) return rc;
@@ -938,8 +1028,14 @@ int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pai
 // `results` must stay valid until qb200_register_batch_flush (or a later enqueue / qb200_register_batch) has returned them.
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                                  qb200_result* results) {
+  return qb200_register_batch_enqueue_ex(h, pairs, n_pairs, p, kind, results, nullptr);
+}
+
+int qb200_register_batch_enqueue_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
+                                    qb200_result* results, const qb200_pair_lists* lists) {
   if (!h || n_pairs < 0 || (n_pairs > 0 && (!pairs || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
   if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
+  if (int rc = check_lists(h, lists, false)) return rc;
   const int S = h->cfg.max_batch_slots, R = h->cfg.max_raw_points;
   for (int i = 0; i < n_pairs; ++i) {
     if (pairs[i].n_src < 0 || pairs[i].n_tgt < 0 || pairs[i].n_src > R || pairs[i].n_tgt > R ||
@@ -997,6 +1093,7 @@ int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32
   WaveInput in;
   in.pairs = pairs;
   in.kind = kind;
+  in.lists = lists;
   // host scans of a multi-wave batch: one copy stream, ordered after whatever the caller queued on lane 0's stream
   if (kind == QB200_MEM_HOST && n_lanes > 1) {
     in.copy_stream = h->copy_stream;
@@ -1190,9 +1287,15 @@ int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t
 }
 
 int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_result* results) {
+  return qb200_register_cached_ex(h, pairs, n_pairs, p, results, nullptr);
+}
+
+int qb200_register_cached_ex(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_result* results,
+                             const qb200_pair_lists* lists) {
   if (int rc = enter(h)) return rc;
   if (n_pairs < 0 || (n_pairs > 0 && (!pairs || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
   if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
+  if (int rc = check_lists(h, lists, false)) return rc;
   const float cell = lattice_cell(*p);
   for (int i = 0; i < n_pairs; ++i) {
     const int sl[2] = {pairs[i].src_slot, pairs[i].tgt_slot};
@@ -1207,6 +1310,7 @@ int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t
   }
   WaveInput in;
   in.slots = pairs;
+  in.lists = lists;
   return run_waves(h, in, n_pairs, resolve_params(h, *p), results);
 }
 

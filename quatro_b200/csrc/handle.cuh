@@ -34,6 +34,7 @@ struct Lane {
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
   int pend_t0, pend_t1;       // ... the stage-time slots [t0, t1) it records
   qb200_result* pend_dst;     // ... and the caller's record array of its batch
+  qb200_pair_lists pend_lists; // ... and a copy of its batch's list descriptor (cap_per_pair == 0: no lists)
 
   // ---- sort workspace (voxel sort, then lattice sort) ----
   DeviceMem<uint64_t> key_a, key_b;  // [2S*max(R,V)]
@@ -87,6 +88,8 @@ struct Lane {
   // ---- results ----
   DeviceMem<qb200_result> d_results; // [S]
   PinnedMem<qb200_result> h_results; // [S]
+  PinnedMem<unsigned char> lst_stage; int lst_cap;  // host-kind pair lists, grown on first use: [S][lst_cap] entries of every list
+                                                    // (ListDst::carve), written by pack_lists_kernel through the mapped address
   WaveCounters ctr;
   DeviceMem<int> ctr_block; size_t ctr_ints;
 
@@ -176,6 +179,23 @@ int launch_pose(Lane* h, int n_pairs, const qb200_params& p);
 int launch_fill_counters(Lane* h, int n_pairs, int have_frontend);
 int launch_finalize_status(Lane* h, int n_pairs);
 int launch_iota_clique(Lane* h, int n_pairs);
+// Where pack_lists_kernel writes pair s's lists: each array (nullptr = not asked for) + s * stride entries, at most cap of them.
+struct ListDst {
+  int2* corr; float4* sm; float4* tm; int* clique; int* fin; unsigned char* rm; unsigned char* tmask;
+  long long stride;
+  int cap;
+  // the caller's arrays from pair `first` on (stride = cap_per_pair)
+  static ListDst caller(const qb200_pair_lists& d, long long first);
+  // lists' arrays, placed in a staging block of S pairs of `cap` entries each (base == nullptr: only the size); only requested lists
+  // get a non-null pointer
+  static size_t carve(unsigned char* base, int S, int cap, const qb200_pair_lists& d, ListDst* out);
+};
+int launch_pack_lists(Lane* h, int n_pairs, const ListDst& dst);
+// entries of a list of `count` entries that a pair's stride of `cap` receives (counts never exceed the lane's Lc)
+__host__ __device__ inline int list_entries(int count, int Lc, int cap) {
+  const int n = count < 0 ? 0 : count > Lc ? Lc : count;
+  return n < cap ? n : cap;
+}
 int launch_segment_cloud(Lane* h, const float4* pts, int n, const qb200_segment_params& sp, int* n_valid, int* n_outlier,
                          const float4** valid_dev, const float4** outlier_dev);
 int launch_patchwork(Lane* h, const float4* pts, int n, const qb200_patchwork_params& pp, int* n_ground, int* n_nonground, int* status);
