@@ -31,6 +31,9 @@
 //      (1 + 2^-9) * fpfh_radius (params.grid_cell overrides it): the neighbour SETS never depend on the cell,
 //      the accumulation order does, so the CUDA library uses the same default.
 //   D9 2x2 rotation: own two-sided Jacobi SVD (Eigen::JacobiSVD unavailable); fp64 sums in index order
+//   D10 VoxelGrid refuses a cloud (QB200_ERR_VOXEL_OVERFLOW, input returned unfiltered) not only on PCL's own check
+//      (truncated spans dx*dy*dz > INT_MAX) but wherever PCL's int arithmetic would overflow (UB, wraps in practice): a kept
+//      point's floor(p * inv) outside int32, or a product of the floor-based div_b above INT_MAX
 // =====================================================================================
 #include <algorithm>
 #include <cfloat>
@@ -105,21 +108,28 @@ int voxelize(const P4* pts, int n, float leaf, int skip_flagged, std::vector<P4>
     mx[0] = std::max(mx[0], p.x); mx[1] = std::max(mx[1], p.y); mx[2] = std::max(mx[2], p.z);
   }
   if (kept.empty()) return QB200_OK;
-  // overflow check: PCL warns and copies the input through
-  const int64_t dx = (int64_t)((mx[0] - mn[0]) * inv) + 1;
-  const int64_t dy = (int64_t)((mx[1] - mn[1]) * inv) + 1;
-  const int64_t dz = (int64_t)((mx[2] - mn[2]) * inv) + 1;
-  if (dx * dy * dz > (int64_t)std::numeric_limits<int32_t>::max()) {
+  // overflow check: PCL warns and copies the input through.  D10: also refused wherever PCL's own int arithmetic would overflow
+  // (a floor(p * inv) outside int32 -- the bbox corners decide, floor(p * inv) is monotone in p -- or a product of the floor-based
+  // div_b above INT_MAX), and PCL's int64 span product is evaluated without overflowing.
+  const auto product_exceeds = [](int64_t a, int64_t b, int64_t c) {  // factors >= 1
+    const int64_t lim = std::numeric_limits<int32_t>::max();
+    return a > lim || b > lim || c > lim || a * b > lim || a * b * c > lim;
+  };
+  bool refuse = false;
+  int64_t span[3], min_b[3], div_b[3];
+  for (int a = 0; a < 3; ++a) {
+    const float lo = std::floor(mn[a] * inv), hi = std::floor(mx[a] * inv);
+    const float s = (mx[a] - mn[a]) * inv;
+    if (!(lo >= -2147483648.0f && hi < 2147483648.0f && s < 2147483648.0f)) { refuse = true; break; }
+    span[a] = (int64_t)s + 1;
+    min_b[a] = (int64_t)lo;
+    div_b[a] = (int64_t)hi - min_b[a] + 1;
+  }
+  if (refuse || product_exceeds(span[0], span[1], span[2]) || product_exceeds(div_b[0], div_b[1], div_b[2])) {
     for (int i : kept) out.push_back(pts[i]);
     return QB200_ERR_VOXEL_OVERFLOW;
   }
-  int min_b[3], max_b[3], div_b[3];
-  for (int a = 0; a < 3; ++a) {
-    min_b[a] = (int)std::floor(mn[a] * inv);
-    max_b[a] = (int)std::floor(mx[a] * inv);
-    div_b[a] = max_b[a] - min_b[a] + 1;
-  }
-  const int mul[3] = {1, div_b[0], div_b[0] * div_b[1]};
+  const int mul[3] = {1, (int)div_b[0], (int)(div_b[0] * div_b[1])};
   std::vector<std::pair<int, int>> iv;  // (voxel idx, point idx)
   iv.reserve(kept.size());
   for (int i : kept) {

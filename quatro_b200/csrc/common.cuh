@@ -91,17 +91,47 @@ __host__ __device__ __forceinline__ float ordered_float(int i) {
 #endif
 }
 
-// number of 8-bit digits the voxel keys of a cloud occupy: the keys are below dx dy dz of pcl::VoxelGrid's own linear index
-// (voxel_pack uses the same min_b / div_b expressions)
+// a * b * c > INT_MAX for factors >= 1, without overflowing 64 bits
+__host__ __device__ __forceinline__ bool vox_product_exceeds(long long a, long long b, long long c) {
+  const long long lim = 2147483647LL;
+  if (a > lim || b > lim || c > lim) return true;
+  const long long ab = a * b;  // < 2^62
+  return ab > lim || ab * c > lim;
+}
+// pcl::VoxelGrid's grid of a cloud from the ordered-int bbox of its kept points: min_b and div_b.  False when the cloud is refused
+// with QB200_ERR_VOXEL_OVERFLOW, i.e. wherever PCL's own int arithmetic would overflow:
+//   - PCL's check: the truncated spans (int64)((max - min) * inv) + 1 multiply to more than INT_MAX;
+//   - a kept point's floor(p * inv) lies outside int32 (floor(p * inv) is monotone in p: the bbox corners decide);
+//   - the floor-based div_b = max_b - min_b + 1, which can be one larger per axis than the truncated span, multiply to more than
+//     INT_MAX (the linear index would not fit an int).
+// The index is relative to min_b, so a cloud far from the origin is voxelised like the same cloud moved to the origin.
+__device__ __forceinline__ bool vox_axis(int omin, int omax, float inv_leaf, long long* span, long long* min_b, long long* div_b) {
+  const float mn = ordered_float(omin), mx = ordered_float(omax);
+  const float lo = floorf(mn * inv_leaf), hi = floorf(mx * inv_leaf);
+  if (!(lo >= -2147483648.0f && hi < 2147483648.0f)) return false;
+  const float s = (mx - mn) * inv_leaf;
+  if (!(s < 2147483648.0f)) return false;  // a truncated span above INT_MAX (or +inf) fails PCL's check on its own
+  *span = (long long)s + 1;
+  *min_b = (long long)lo;
+  *div_b = (long long)hi - *min_b + 1;
+  return true;
+}
+__device__ __forceinline__ bool vox_grid(const int* __restrict__ bbox, float inv_leaf, long long* min_b, long long* div_b) {
+  long long t0, t1, t2;
+  if (!vox_axis(bbox[0], bbox[3], inv_leaf, &t0, &min_b[0], &div_b[0]) || !vox_axis(bbox[1], bbox[4], inv_leaf, &t1, &min_b[1], &div_b[1]) ||
+      !vox_axis(bbox[2], bbox[5], inv_leaf, &t2, &min_b[2], &div_b[2]))
+    return false;
+  return !vox_product_exceeds(t0, t1, t2) && !vox_product_exceeds(div_b[0], div_b[1], div_b[2]);
+}
+
+// number of 8-bit digits the voxel keys of a cloud occupy: the keys are below div_b[0] div_b[1] div_b[2] of pcl::VoxelGrid's own
+// linear index (voxel_pack uses the same min_b / div_b).  -1: the cloud is refused (vox_grid()), nothing is sorted and run_heads
+// drops it.
 __device__ __forceinline__ int vox_digits(const int* __restrict__ bbox, int n_valid, float inv_leaf) {
   if (n_valid <= 0) return 0;
-  const long long m0 = (long long)floorf(ordered_float(bbox[0]) * inv_leaf), m1 = (long long)floorf(ordered_float(bbox[1]) * inv_leaf),
-                  m2 = (long long)floorf(ordered_float(bbox[2]) * inv_leaf);
-  const long long d0 = (long long)floorf(ordered_float(bbox[3]) * inv_leaf) - m0 + 1, d1 = (long long)floorf(ordered_float(bbox[4]) * inv_leaf) - m1 + 1,
-                  d2 = (long long)floorf(ordered_float(bbox[5]) * inv_leaf) - m2 + 1;
-  unsigned long long span = (unsigned long long)d0 * (unsigned long long)d1;   // each factor < 2^18 (cell_ok)
-  if (span > (1ull << 31) || span * (unsigned long long)d2 > (1ull << 31)) return 4;  // refused by run_heads (overflow); any order will do
-  span *= (unsigned long long)d2;
+  long long m[3], d[3];
+  if (!vox_grid(bbox, inv_leaf, m, d)) return -1;
+  const unsigned long long span = (unsigned long long)(d[0] * d[1] * d[2]);  // <= INT_MAX
   int bits = 0;
   while (bits < 31 && (1ull << bits) < span) ++bits;
   return (bits + 7) >> 3;

@@ -11,6 +11,7 @@
 // x-runs of cells, visited in ascending (cell, index) order -- the accumulation order the CPU oracle
 // uses, so the single-pass float covariance matches bit for bit.
 #include <cub/device/device_radix_sort.cuh>
+#include <type_traits>
 
 #include "fpfh_math.cuh"
 #include "handle.cuh"
@@ -46,16 +47,17 @@ static int clog2(int n) {
 // K1a: bounding box and per-chunk counts of the kept raw points (one pass, 128-bit loads).  The voxel key that the pack pass
 // (voxsort.cu) then builds is PCL's own linear index  (i - min_i) + (j - min_j) dx + (k - min_k) dx dy  ([EXT] pcl::VoxelGrid,
 // called from include/quatro.hpp:49-57), which the library requires to fit an int: at most 31 key bits, and for a given cloud
-// only the bits of dx dy dz (vox_digits()).
+// only the bits of dx dy dz (vox_digits()).  The bbox alone decides whether a cloud is refused (vox_grid()), so this pass keeps
+// no per-point range test.
 // ------------------------------------------------------------------------------------------------
 
 __global__ void __launch_bounds__(256) voxel_bbox_kernel(const float4* const* __restrict__ cloud_ptr, const int* __restrict__ cloud_n,
-                                                         float inv_leaf, int skip_flagged, int* __restrict__ bbox,
-                                                         int* __restrict__ n_valid, int* __restrict__ cloud_status, int* __restrict__ chunk_cnt) {
+                                                         int skip_flagged, int* __restrict__ bbox, int* __restrict__ n_valid,
+                                                         int* __restrict__ chunk_cnt) {
   const int cloud = blockIdx.y;
   const int n = cloud_n[cloud];
   const float4* __restrict__ pts = cloud_ptr[cloud];
-  int mn0 = INT_MAX, mn1 = INT_MAX, mn2 = INT_MAX, mx0 = INT_MIN, mx1 = INT_MIN, mx2 = INT_MIN, cnt = 0, bad = 0;
+  int mn0 = INT_MAX, mn1 = INT_MAX, mn2 = INT_MAX, mx0 = INT_MIN, mx1 = INT_MIN, mx2 = INT_MIN, cnt = 0;
   // eight independent 16-byte loads in flight per thread and ~30 points per thread: this pass streams the raw scans (230 MB per
   // 64-pair wave) from HBM, and the reduction tail (shuffles, atomics) is paid once per 30 points instead of once per 7.
   // A CTA walks kVsChunks / gridDim.x CONTIGUOUS chunks of the scan and also reports how many points of each chunk are kept:
@@ -78,15 +80,10 @@ __global__ void __launch_bounds__(256) voxel_bbox_kernel(const float4* const* __
       for (int j = 0; j < kInFlight; ++j) {
         const float4 p = pp[j];
         if (i0 + j * 256 >= c1 || !raw_point_kept(p, skip_flagged)) continue;
-        const int ci = (int)floorf(p.x * inv_leaf), cj = (int)floorf(p.y * inv_leaf), ck = (int)floorf(p.z * inv_leaf);
-        if (cell_ok(ci, cj, ck)) {
-          const int ox = float_ordered(p.x), oy = float_ordered(p.y), oz = float_ordered(p.z);
-          mn0 = min(mn0, ox); mn1 = min(mn1, oy); mn2 = min(mn2, oz);
-          mx0 = max(mx0, ox); mx1 = max(mx1, oy); mx2 = max(mx2, oz);
-          ++ccnt;
-        } else {
-          bad = 1;  // outside the representable lattice: PCL's index would overflow as well
-        }
+        const int ox = float_ordered(p.x), oy = float_ordered(p.y), oz = float_ordered(p.z);
+        mn0 = min(mn0, ox); mn1 = min(mn1, oy); mn2 = min(mn2, oz);
+        mx0 = max(mx0, ox); mx1 = max(mx1, oy); mx2 = max(mx2, oz);
+        ++ccnt;
       }
     }
     cnt += ccnt;
@@ -100,29 +97,23 @@ __global__ void __launch_bounds__(256) voxel_bbox_kernel(const float4* const* __
     mn0 = min(mn0, __shfl_xor_sync(0xffffffffu, mn0, o)); mn1 = min(mn1, __shfl_xor_sync(0xffffffffu, mn1, o));
     mn2 = min(mn2, __shfl_xor_sync(0xffffffffu, mn2, o)); mx0 = max(mx0, __shfl_xor_sync(0xffffffffu, mx0, o));
     mx1 = max(mx1, __shfl_xor_sync(0xffffffffu, mx1, o)); mx2 = max(mx2, __shfl_xor_sync(0xffffffffu, mx2, o));
-    cnt += __shfl_xor_sync(0xffffffffu, cnt, o); bad |= __shfl_xor_sync(0xffffffffu, bad, o);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
   }
   // one set of global atomics per CTA
-  __shared__ int s_red[8];
-  if (threadIdx.x == 0) { s_red[0] = s_red[1] = s_red[2] = INT_MAX; s_red[3] = s_red[4] = s_red[5] = INT_MIN; s_red[6] = 0; s_red[7] = 0; }
+  __shared__ int s_red[7];
+  if (threadIdx.x == 0) { s_red[0] = s_red[1] = s_red[2] = INT_MAX; s_red[3] = s_red[4] = s_red[5] = INT_MIN; s_red[6] = 0; }
   __syncthreads();
-  if (lane_id() == 0) {
-    if (cnt) {
-      atomicMin(&s_red[0], mn0); atomicMin(&s_red[1], mn1); atomicMin(&s_red[2], mn2);
-      atomicMax(&s_red[3], mx0); atomicMax(&s_red[4], mx1); atomicMax(&s_red[5], mx2);
-      atomicAdd(&s_red[6], cnt);
-    }
-    if (bad) s_red[7] = 1;
+  if (lane_id() == 0 && cnt) {
+    atomicMin(&s_red[0], mn0); atomicMin(&s_red[1], mn1); atomicMin(&s_red[2], mn2);
+    atomicMax(&s_red[3], mx0); atomicMax(&s_red[4], mx1); atomicMax(&s_red[5], mx2);
+    atomicAdd(&s_red[6], cnt);
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    if (s_red[6]) {
-      int* b = bbox + cloud * 6;
-      atomicMin(b + 0, s_red[0]); atomicMin(b + 1, s_red[1]); atomicMin(b + 2, s_red[2]);
-      atomicMax(b + 3, s_red[3]); atomicMax(b + 4, s_red[4]); atomicMax(b + 5, s_red[5]);
-      atomicAdd(n_valid + cloud, s_red[6]);
-    }
-    if (s_red[7]) cloud_status[cloud] = QB200_ERR_VOXEL_OVERFLOW;
+  if (threadIdx.x == 0 && s_red[6]) {
+    int* b = bbox + cloud * 6;
+    atomicMin(b + 0, s_red[0]); atomicMin(b + 1, s_red[1]); atomicMin(b + 2, s_red[2]);
+    atomicMax(b + 3, s_red[3]); atomicMax(b + 4, s_red[4]); atomicMax(b + 5, s_red[5]);
+    atomicAdd(n_valid + cloud, s_red[6]);
   }
 }
 
@@ -143,20 +134,11 @@ __global__ void __launch_bounds__(1024) run_heads_kernel(int mode, const uint64_
   const int cloud = blockIdx.x;
   const int off = mode == 0 ? seg_off[cloud] : cloud * V;
   const int n = mode == 0 ? n_valid_in[cloud] : V;
-  if (mode == 0 && (vox_digits(bbox + cloud * 6, n, inv_leaf) & 1)) keys = keys_b;
-  if (threadIdx.x == 0) {
-    int ov = 0;
-    if (mode == 0 && n_valid_in[cloud] > 0) {
-      // [EXT] pcl::VoxelGrid: dx*dy*dz > INT_MAX -> "leaf size too small", input returned unfiltered
-      const int* b = bbox + cloud * 6;
-      const long long dx = (long long)((ordered_float(b[3]) - ordered_float(b[0])) * inv_leaf) + 1;
-      const long long dy = (long long)((ordered_float(b[4]) - ordered_float(b[1])) * inv_leaf) + 1;
-      const long long dz = (long long)((ordered_float(b[5]) - ordered_float(b[2])) * inv_leaf) + 1;
-      if (dx * dy * dz > (long long)INT_MAX) ov = 1;
-    }
-    if (mode == 0 && cloud_status[cloud] == QB200_ERR_VOXEL_OVERFLOW) ov = 1;
-    s_overflow = ov;
-  }
+  const int digits = mode == 0 ? vox_digits(bbox + cloud * 6, n, inv_leaf) : 0;
+  if (digits & 1) keys = keys_b;
+  // [EXT] pcl::VoxelGrid: dx*dy*dz > INT_MAX -> "leaf size too small", input returned unfiltered; also every other case in which
+  // PCL's int index would overflow (vox_grid())
+  if (threadIdx.x == 0) s_overflow = digits < 0 ? 1 : 0;
   __syncthreads();
   if (s_overflow) {
     if (threadIdx.x == 0) {
@@ -304,13 +286,14 @@ __device__ __forceinline__ void walk_cells(const LatticeView& L, const float4 pq
   }
 }
 
-template <class F>
+// kLockstep = false: rows one after the other, in the same order; for callbacks too heavy to be repeated for nine unrolled rows
+template <bool kLockstep = true, class F>
 __device__ __forceinline__ void for_each_neighbor(const LatticeView& L, const float4 pq, int m, float r2, F&& f) {
   if (!(isfinite(pq.x) && isfinite(pq.y) && isfinite(pq.z))) return;
   const int ci = (int)floorf(pq.x * L.inv), cj = (int)floorf(pq.y * L.inv), ck = (int)floorf(pq.z * L.inv);
   if (!cell_ok(ci, cj, ck)) return;
   const int ilo = max(ci - m, -kOffIJ), ihi = min(ci + m, kOffIJ - 2);
-  if (m == 1) {
+  if (kLockstep && m == 1) {
     // the usual case (cell >= radius): the 9 (k, j) rows are located by 9 binary searches that advance in lockstep, so
     // their loads are independent (one round trip per step instead of nine), and each row is one contiguous cell range
     uint64_t lo[9], hi[9];
@@ -378,31 +361,54 @@ __device__ __forceinline__ LatticeView make_view(int cloud, int V, const float4*
   return L;
 }
 
-// K4 / K5 walk the same neighbourhoods.  A thread first COLLECTS its neighbour indices (cheap distance tests, divergent)
-// into a shared-memory list and then processes the list in a dense loop, so the expensive per-neighbour work (pair
-// features, 33-bin gathers) runs with most lanes of the warp active instead of whenever any lane found a neighbour.
-// Neighbourhoods larger than the list are handled window by window (ordinals [base, base + cap)), order preserved, so the
-// results do not depend on the window size.  64 32-bit indices per thread are 32 KB of static shared memory: spfh_kernel<true>
-// adds its 8.4 KB of bin counts and stays within the 48 KB static limit.
+// K4 / K5 of a point with more than kNbrGlobalCap neighbours (the rare kernels) walk the lattice ONCE, in lattice order.  These
+// points are rare in LiDAR scans, but a dense or degenerate cloud can give every point tens of thousands of neighbours, and a walk
+// per window of neighbours would then cost O(k^2) per point.  fpfh_rare_kernel accumulates inside the walk.  spfh_kernel<true>
+// collects up to kNbrCap neighbour indices at a time in shared memory (walk_chunk: the walk stops when the list is full and
+// resumes where it stopped), then computes their pair features in a dense loop with no walk state live across the feature's
+// division slow paths.
 constexpr int kNbrThreads = 128;
-constexpr int kNbrCap = 64;
+constexpr int kNbrCap = 32;
 
-template <class Process>
-__device__ __forceinline__ int for_each_neighbor_listed(const LatticeView& L, const float4 pq, int m, float r2,
-                                                        uint32_t (*nbr)[kNbrThreads], Process&& process) {
-  int k_total = 0;
-  for (int base = 0;; base += kNbrCap) {
-    int k = 0;
-    for_each_neighbor(L, pq, m, r2, [&](int p, float, const float4) {
-      if (k >= base && k < base + kNbrCap) nbr[k - base][threadIdx.x] = (uint32_t)p;
-      ++k;
-    });
-    k_total = k;
-    const int kl = k_total - base < kNbrCap ? k_total - base : kNbrCap;
-    for (int t = 0; t < kl; ++t) process((int)nbr[t][threadIdx.x]);
-    if (base + kNbrCap >= k_total) break;
+struct WalkPos {
+  int row = 0;   // (k, j) row of the walk, (dk + m) (2m + 1) + (dj + m)
+  int t = -1;    // next candidate (position in the sorted index) of that row; -1: the row is not started
+};
+
+// the rows of for_each_neighbor<false> from `pos` on, in the same order: writes up to kNbrCap neighbours to nbr[][threadIdx.x],
+// returns how many; pos.row == (2m + 1)^2 once the walk is complete
+__device__ __forceinline__ int walk_chunk(const LatticeView& L, const float4 pq, int m, float r2, WalkPos& pos,
+                                          uint32_t (*nbr)[kNbrThreads]) {
+  const int w = 2 * m + 1;
+  if (!(isfinite(pq.x) && isfinite(pq.y) && isfinite(pq.z))) { pos.row = w * w; return 0; }
+  const int ci = (int)floorf(pq.x * L.inv), cj = (int)floorf(pq.y * L.inv), ck = (int)floorf(pq.z * L.inv);
+  if (!cell_ok(ci, cj, ck)) { pos.row = w * w; return 0; }
+  const int ilo = max(ci - m, -kOffIJ), ihi = min(ci + m, kOffIJ - 2);
+  int n = 0;
+  for (; pos.row < w * w; ++pos.row, pos.t = -1) {
+    const int k = ck + pos.row / w - m, j = cj + pos.row % w - m;
+    if (k < -kOffK || k >= kOffK - 1 || j < -kOffIJ || j >= kOffIJ - 1) continue;
+    const uint64_t lo = cell_key(ilo, j, k), hi = cell_key(ihi, j, k);
+    int a = 0, b = L.n_cells;
+    while (a < b) {
+      const int mid = (a + b) >> 1;
+      if (L.ckeys[mid] < lo) a = mid + 1; else b = mid;
+    }
+    int c = a;
+    while (c < L.n_cells && L.ckeys[c] <= hi) ++c;
+    if (a >= c) continue;
+    const int t1 = L.cstart[c];
+    for (int t = pos.t >= 0 ? pos.t : L.cstart[a]; t < t1; ++t) {
+      const int p = (int)L.order[t];
+      const float4 pp = L.pts[p];
+      const float dx = pq.x - pp.x, dy = pq.y - pp.y, dz = pq.z - pp.z;
+      const float d2 = (dx * dx + dy * dy) + dz * dz;
+      if (!(d2 < r2)) continue;
+      if (n == kNbrCap) { pos.t = t; return n; }
+      nbr[n++][threadIdx.x] = (uint32_t)p;
+    }
   }
-  return k_total;
+  return n;
 }
 
 // K2c: the fpfh_radius neighbourhood of every point, found ONCE: indices in lattice (cell, index) order, written
@@ -465,10 +471,13 @@ __global__ void __launch_bounds__(128) normals_kernel(const float4* __restrict__
 
 // K4: SPFH.  Bin COUNTS are order-free; the float histogram value is rebuilt by repeated addition
 // of the same increment, which is what the sequential reference loop produces.
-// kRare = false: the points whose neighbourhood is in the K2c list (all but a handful): no lattice walk compiled in, no list
-// buffer in shared memory.  kRare = true: only the points with more than kNbrGlobalCap neighbours, which walk the lattice.
+// kRare = false: the points whose neighbourhood is in the K2c list (all but a handful): no lattice walk compiled in, and at most
+// kNbrGlobalCap pairs, so 16-bit bin counts.  kRare = true: only the points with more than kNbrGlobalCap neighbours, which walk
+// the lattice; a bin can then collect every neighbour of the point (all pairs of a planar neighbourhood share their f2 and f3
+// bins), so its counts are 32-bit: 16.5 KB of static shared memory, plus 16 KB of neighbour list (walk_chunk).
 // SPFH rows are stored as three padded thirds [11 bins, 0][11 bins, 0][11 bins, 0] (36 floats): a third is three 16-byte loads.
 constexpr int kSpfhThreads = kNbrThreads;
+static_assert(kNbrGlobalCap < 65536, "spfh_kernel<false> counts in 16 bits");
 __device__ __forceinline__ int spfh_slot(int b) { return b + b / 11; }
 template <bool kRare>
 __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __restrict__ pts, const float4* __restrict__ normals,
@@ -477,7 +486,8 @@ __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __rest
                                                             const int* __restrict__ n_cells, float inv, int m, float r2,
                                                             float* __restrict__ spfh, const uint32_t* __restrict__ nbr_list,
                                                             const int* __restrict__ nbr_cnt) {
-  __shared__ unsigned short cnts[kDescDim][kSpfhThreads];
+  using Count = typename std::conditional<kRare, unsigned, unsigned short>::type;
+  __shared__ Count cnts[kDescDim][kSpfhThreads];
   __shared__ uint32_t nbr[kRare ? kNbrCap : 1][kNbrThreads];
   const int cloud = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -506,12 +516,19 @@ __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __rest
     const uint32_t* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
     for (int t = 0; t < k; ++t) feature((int)gl[(size_t)t * V]);
   } else {
-    k = for_each_neighbor_listed(L, pq, m, r2, nbr, feature);
+    k = 0;
+    WalkPos pos;
+    const int rows = (2 * m + 1) * (2 * m + 1);
+    while (pos.row < rows) {
+      const int n = walk_chunk(L, pq, m, r2, pos, nbr);
+      for (int t = 0; t < n; ++t) feature((int)nbr[t][threadIdx.x]);
+      k += n;
+    }
   }
   float* __restrict__ out = spfh + ((size_t)cloud * V + q) * kDescPad;  // three padded thirds: 16-byte gathers in K5
   const float incr = k >= 2 ? 100.0f / (float)(k - 1) : 0.0f;
   for (int b = 0; b < kDescDim; ++b) {
-    const int c = cnts[b][threadIdx.x];
+    const int c = (int)cnts[b][threadIdx.x];  // at most the neighbour count, which fits an int
     float v = 0.0f;
     for (int t = 0; t < c; ++t) v += incr;
     out[spfh_slot(b)] = v;
@@ -573,13 +590,12 @@ __global__ void __launch_bounds__(3 * kNbrThreads, 3) fpfh_list_kernel(const flo
   for (int b = 0; b < 11; ++b) out[(size_t)b * V] = o[b] * g;
 }
 
-// the rare point with more than kNbrGlobalCap neighbours walks the lattice itself (one thread, all 33 bins)
+// the rare point with more than kNbrGlobalCap neighbours walks the lattice itself (one thread, all 33 bins, one walk)
 __global__ void __launch_bounds__(kNbrThreads) fpfh_rare_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V,
                                                                 const uint64_t* __restrict__ cell_key, const int* __restrict__ cell_start,
                                                                 const uint32_t* __restrict__ order, const int* __restrict__ n_cells, float inv,
                                                                 int m, float r2, const float* __restrict__ spfh,
                                                                 const int* __restrict__ nbr_cnt, float* __restrict__ desc_t) {
-  __shared__ uint32_t nbr[kNbrCap][kNbrThreads];
   const int cloud = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_pts[cloud]) return;
@@ -591,10 +607,8 @@ __global__ void __launch_bounds__(kNbrThreads) fpfh_rare_kernel(const float4* __
 #pragma unroll
   for (int b = 0; b < kDescDim; ++b) o[b] = 0.0f;
   double s0 = 0.0, s1 = 0.0, s2 = 0.0;
-  auto accumulate = [&](int p) {
-    const float4 pp = L.pts[p];
-    const float dx = pq.x - pp.x, dy = pq.y - pp.y, dz = pq.z - pp.z;
-    const float d2 = (dx * dx + dy * dy) + dz * dz;  // the same expression as the neighbour test: bit-identical
+  // the walk's own d2: the expression the list kernel recomputes, bit-identical
+  for_each_neighbor<false>(L, pq, m, r2, [&](int p, float d2, const float4) {
     if (d2 == 0.0f) return;
     const float weight = 1.0f / d2;
     float s[kDescPad];
@@ -609,8 +623,7 @@ __global__ void __launch_bounds__(kNbrThreads) fpfh_rare_kernel(const float4* __
     for (int b = 0; b < 11; ++b) { const float v = s[12 + b] * weight; s1 += v; o[11 + b] += v; }
 #pragma unroll
     for (int b = 0; b < 11; ++b) { const float v = s[24 + b] * weight; s2 += v; o[22 + b] += v; }
-  };
-  for_each_neighbor_listed(L, pq, m, r2, nbr, accumulate);
+  });
   if (s0 != 0.0) s0 = 100.0 / s0;
   if (s1 != 0.0) s1 = 100.0 / s1;
   if (s2 != 0.0) s2 = 100.0 / s2;
@@ -646,8 +659,7 @@ int launch_voxel(Lane* h, int n_clouds, float leaf, int skip_flagged) {
   const float inv = 1.0f / leaf;
   const dim3 gb(n_clouds >= 16 ? 16 : 64, n_clouds);  // ~30 points per thread when the batch fills the device on its own
   int* chunk_cnt = reinterpret_cast<int*>(h->val_b.get());   // [clouds][kVsChunks]
-  voxel_bbox_kernel<<<gb, 256, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, inv, skip_flagged, h->ctr.bbox, h->ctr.n_valid, h->ctr.cloud_status,
-                                               chunk_cnt);
+  voxel_bbox_kernel<<<gb, 256, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, skip_flagged, h->ctr.bbox, h->ctr.n_valid, chunk_cnt);
   h->launches += 1;
   const int idx_bits = clog2(h->R > 2 ? h->R : 2);  // point index inside its scan
   if (int rc = launch_voxel_sort(h, n_clouds, inv, skip_flagged, idx_bits)) return rc;

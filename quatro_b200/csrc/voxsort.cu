@@ -36,13 +36,8 @@ __global__ void __launch_bounds__(kVsThreads) voxel_pack_kernel(const float4* co
   const int c0 = chunk * cs, c1 = min(n, c0 + cs);
   if (c0 >= n) return;
   const float4* __restrict__ pts = cloud_ptr[cloud];
-  long long m0 = 0, m1 = 0, m2 = 0, d0 = 1, d1 = 1;
-  if (n_valid[cloud] > 0) {  // min_b / div_b of pcl::VoxelGrid::applyFilter
-    const int* b = bbox + cloud * 6;
-    m0 = (long long)floorf(ordered_float(b[0]) * inv_leaf); m1 = (long long)floorf(ordered_float(b[1]) * inv_leaf);
-    m2 = (long long)floorf(ordered_float(b[2]) * inv_leaf);
-    d0 = (long long)floorf(ordered_float(b[3]) * inv_leaf) - m0 + 1; d1 = (long long)floorf(ordered_float(b[4]) * inv_leaf) - m1 + 1;
-  }
+  long long m[3] = {0, 0, 0}, d[3] = {1, 1, 1};  // min_b / div_b of pcl::VoxelGrid::applyFilter
+  const bool grid_ok = n_valid[cloud] > 0 && vox_grid(bbox + cloud * 6, inv_leaf, m, d);
   int base = 0;  // kept points of the preceding chunks
   {
     int v = 0;
@@ -62,14 +57,14 @@ __global__ void __launch_bounds__(kVsThreads) voxel_pack_kernel(const float4* co
       keep[j] = 0; it[j] = 0;
       if (i < c1) {
         const float4 p = __ldg(pts + i);
-        if (raw_point_kept(p, skip_flagged)) {
-          const int ci = (int)floorf(p.x * inv_leaf), cj = (int)floorf(p.y * inv_leaf), ck = (int)floorf(p.z * inv_leaf);
-          if (cell_ok(ci, cj, ck)) {   // exactly the points the bbox pass counted
-            const long long lin = ((long long)ci - m0) + ((long long)cj - m1) * d0 + ((long long)ck - m2) * d0 * d1;
-            const uint64_t cell = (lin >= 0 && lin < (long long)kVoxInvalid) ? (uint64_t)lin : kVoxInvalid;  // else: refused cloud
-            it[j] = (cell << idx_bits) | (uint64_t)i;
-            keep[j] = 1;
+        if (raw_point_kept(p, skip_flagged)) {  // exactly the points the bbox pass counted
+          uint64_t cell = kVoxInvalid;         // refused cloud: run_heads drops it, any key will do
+          if (grid_ok) {                       // every floor(p * inv) fits an int and the index is below INT_MAX
+            const int ci = (int)floorf(p.x * inv_leaf), cj = (int)floorf(p.y * inv_leaf), ck = (int)floorf(p.z * inv_leaf);
+            cell = (uint64_t)(((long long)ci - m[0]) + ((long long)cj - m[1]) * d[0] + ((long long)ck - m[2]) * d[0] * d[1]);
           }
+          it[j] = (cell << idx_bits) | (uint64_t)i;
+          keep[j] = 1;
         }
       }
       nk += keep[j];
