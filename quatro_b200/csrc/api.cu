@@ -1,9 +1,5 @@
-// api.cu -- the C-ABI of include/quatro_b200.h: handle lifetime, stage entry points, batch pipeline.
-//
-// Every entry point enqueues the SAME kernels the batch pipeline uses (a stage call is a wave of
-// one), so the per-stage parity tests exercise the production kernels.  There is no CPU
-// implementation of any stage in this library.
-#include <math.h>
+// api.cu -- the C-ABI of include/quatro_b200.h: handle lifetime, lanes, waves, pair lists, the scan cache and the batch entry
+// points.  The single-pair stage entry points, the qb200_get_last_* getters and the debug hooks are in stages.cu.
 #include <new>
 #include <stdio.h>
 #include <stdlib.h>
@@ -11,28 +7,10 @@
 #include <map>
 #include <mutex>
 #include <utility>
-#include <vector>
 
 #include "handle.cuh"
 
 using namespace qb;
-
-namespace qb {
-int launch_degree(Lane* h, int n_pairs);
-
-cudaError_t ensure_dyn_smem(int device, const void* kernel, size_t bytes) {
-  static std::mutex mu;
-  static std::map<std::pair<const void*, int>, size_t> current;
-  std::lock_guard<std::mutex> lock(mu);
-  size_t& cur = current[std::make_pair(kernel, device)];
-  if (bytes > cur) {
-    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) return e;
-    cur = bytes;
-  }
-  return cudaSuccess;
-}
-}
 
 namespace {
 
@@ -178,7 +156,9 @@ int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   QB_CUDA_TRY(L, L->h_results.alloc(S));
   L->ctr_ints = carve_counters(nullptr, S, &L->ctr);
   QB_CUDA_TRY(L, L->ctr_block.alloc(L->ctr_ints));
+  QB_CUDA_TRY(L, L->hctr_block.alloc(L->ctr_ints));
   carve_counters(L->ctr_block, S, &L->ctr);
+  carve_counters(L->hctr_block, S, &L->hctr);
   for (Event& e : L->ev) QB_CUDA_TRY(L, e.create());
   for (Event& e : L->kev) QB_CUDA_TRY(L, e.create());
   QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
@@ -186,23 +166,34 @@ int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   return QB200_OK;
 }
 
+// stage and kernel times of a batch call start from zero
+void reset_timers(qb200_handle* h) {
+  memset(h->stage_ms, 0, sizeof(h->stage_ms));
+  memset(h->kernel_ms, 0, sizeof(h->kernel_ms));
+  memset(h->kernel_calls, 0, sizeof(h->kernel_calls));
+}
+
+}  // namespace
+
+namespace qb {
+cudaError_t ensure_dyn_smem(int device, const void* kernel, size_t bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> current;
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& cur = current[std::make_pair(kernel, device)];
+  if (bytes > cur) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return e;
+    cur = bytes;
+  }
+  return cudaSuccess;
+}
+
 int wave_reset(Lane* L, int n_clouds) {
   const int n = (int)L->ctr_ints;
   wave_init_kernel<<<(n + 255) / 256, 256, 0, L->stream>>>(L->ctr_block, n, L->ctr.bbox, n_clouds);
   L->launches++;
   QB_CUDA_TRY(L, cudaGetLastError());
-  return QB200_OK;
-}
-
-int set_counter(Lane* L, int* dptr, int value) {
-  QB_CUDA_TRY(L, cudaMemcpyAsync(dptr, &value, sizeof(int), cudaMemcpyHostToDevice, L->stream));
-  QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));  // 'value' is a stack variable
-  return QB200_OK;
-}
-
-int get_counter(Lane* L, const int* dptr, int* value) {
-  QB_CUDA_TRY(L, cudaMemcpyAsync(value, dptr, sizeof(int), cudaMemcpyDeviceToHost, L->stream));
-  QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
   return QB200_OK;
 }
 
@@ -240,13 +231,6 @@ void set_last(qb200_handle* h, const qb200_result& r) {
   h->last_n_final = r.n_final_inliers;
 }
 
-// stage and kernel times of a batch call start from zero
-void reset_timers(qb200_handle* h) {
-  memset(h->stage_ms, 0, sizeof(h->stage_ms));
-  memset(h->kernel_ms, 0, sizeof(h->kernel_ms));
-  memset(h->kernel_calls, 0, sizeof(h->kernel_calls));
-}
-
 // graph -> clique -> pose for pairs [0, n) whose matched points / n_corr are already on the device
 int run_solver(Lane* L, int n_pairs, const qb200_params& p, int have_frontend) {
   int rc;
@@ -263,55 +247,6 @@ int run_solver(Lane* L, int n_pairs, const qb200_params& p, int have_frontend) {
   if ((rc = launch_pose(L, n_pairs, p))) return rc;
   if ((rc = launch_finalize_status(L, n_pairs))) return rc;
   return QB200_OK;
-}
-
-int upload_matched(Lane* L, const float* a4, const float* b4, int n) {
-  if (n > L->Lc) {
-    L->fail(__FILE__, __LINE__, "L exceeds max_corr");
-    return QB200_ERR_BAD_ARG;
-  }
-  int rc = wave_reset(L, 2);
-  if (rc) return rc;
-  if (n > 0) {
-    QB_CUDA_TRY(L, cudaMemcpyAsync(L->ma, a4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
-    QB_CUDA_TRY(L, cudaMemcpyAsync(L->mb, b4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
-  }
-  return set_counter(L, L->ctr.n_corr, n);
-}
-
-int upload_cloud_as_voxels(Lane* L, int cloud, const float* pts4, int n) {
-  if (n > L->V) {
-    L->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points");
-    return QB200_ERR_BAD_ARG;
-  }
-  if (n > 0) QB_CUDA_TRY(L, cudaMemcpyAsync(L->vox_pts + (size_t)cloud * L->V, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
-  return set_counter(L, L->ctr.n_vox + cloud, n);
-}
-
-// the record of a single-pair solve on lane 0
-int fetch_result(qb200_handle* h, qb200_result* res) {
-  Lane* L = h->lane[0].get();
-  QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
-  QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
-  *res = L->h_results[0];
-  set_last(h, *res);
-  return res->status;
-}
-
-// the first min(n, cap) correspondences of pair 0: index pairs (src, tgt) and matched points, any of them may be NULL
-int download_corr(Lane* L, int n, int32_t* corr, float* sm4, float* tm4, int cap) {
-  const int m = n < cap ? n : cap;
-  if (m > 0) {
-    std::vector<int> s(m), t(m);
-    QB_CUDA_TRY(L, cudaMemcpyAsync(s.data(), L->corr_src, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
-    QB_CUDA_TRY(L, cudaMemcpyAsync(t.data(), L->corr_tgt, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
-    if (sm4) QB_CUDA_TRY(L, cudaMemcpyAsync(sm4, L->ma, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
-    if (tm4) QB_CUDA_TRY(L, cudaMemcpyAsync(tm4, L->mb, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
-    QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
-    if (corr)
-      for (int i = 0; i < m; ++i) { corr[2 * i] = s[i]; corr[2 * i + 1] = t[i]; }
-  }
-  return n > cap ? QB200_CAPACITY_EXCEEDED : QB200_OK;
 }
 
 // Stage the raw clouds [0, ncl) of a wave whose caller pointers and point counts are in L->h_cloud_ptr / h_cloud_n, then copy the
@@ -351,6 +286,10 @@ int stage_raw(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs) {
   QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_raw_off, L->h_raw_off, (size_t)(ncl + 1) * sizeof(int), cudaMemcpyHostToDevice, cs));
   return QB200_OK;
 }
+
+}  // namespace qb
+
+namespace {
 
 // ---- scan cache ---------------------------------------------------------------------------------------------------------
 // FPFHManager keeps the last target's descriptors and reuses them as the next source (odometry mode, fpfh_manager.hpp:74-77,
@@ -593,39 +532,6 @@ int run_waves(qb200_handle* h, const WaveInput& in, int n, const qb200_params& p
   return QB200_OK;
 }
 
-// Prologue of every entry point that uses lane 0's buffers or stream: a handle, its device current, and no wave of
-// qb200_register_batch_enqueue in flight any more (their records are completed first).
-int enter(qb200_handle* h) {
-  if (!h) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->cfg.device);
-  return h->lanes_active ? batch_flush(h) : QB200_OK;
-}
-
-// tc_stats[first, first + n) summed over the lanes (then zeroed on every lane if reset)
-int read_tc_stats(qb200_handle* h, int first, int n, uint64_t* out, int reset) {
-  for (int i = 0; i < n; ++i) out[i] = 0;
-  for (const auto& L : h->lane) {
-    if (!L) continue;
-    uint64_t o[32];
-    QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
-    QB_CUDA_TRY(L, cudaMemcpy(o, L->tc_stats + first, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    if (reset) QB_CUDA_TRY(L, cudaMemset(L->tc_stats + first, 0, n * sizeof(unsigned long long)));
-    for (int i = 0; i < n; ++i) out[i] += o[i];
-  }
-  return QB200_OK;
-}
-
-int copy_ints(Lane* L, const int* dsrc, int n_have, int32_t* dst, int32_t cap, int32_t* n) {
-  if (!n || cap < 0) return QB200_ERR_BAD_ARG;
-  *n = n_have;
-  const int m = n_have < cap ? n_have : cap;
-  if (m > 0 && dst) {
-    QB_CUDA_TRY(L, cudaMemcpyAsync(dst, dsrc, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
-    QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
-  }
-  return n_have > cap ? QB200_CAPACITY_EXCEEDED : QB200_OK;
-}
-
 }  // namespace
 
 extern "C" {
@@ -717,46 +623,6 @@ int64_t qb200_launch_count(const qb200_handle* h) {
   return n;
 }
 
-// ---- stage: voxelize ----------------------------------------------------------------------------
-int qb200_voxelize(qb200_handle* h, const float* pts4, int32_t n, float leaf, int32_t skip_flagged, float* out4, int32_t cap,
-                   int32_t* n_out) {
-  if (int rc = enter(h)) return rc;
-  if (!n_out || n < 0 || (n > 0 && !pts4) || !(leaf > 0) || cap < 0 || (cap > 0 && !out4)) return QB200_ERR_BAD_ARG;
-  *n_out = 0;
-  Lane* L = h->lane[0].get();
-  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
-  if (n == 0) return QB200_OK;
-  int rc = wave_reset(L, 1);
-  if (rc) return rc;
-  L->h_cloud_ptr[0] = reinterpret_cast<const float4*>(pts4);
-  L->h_cloud_n[0] = n;
-  if ((rc = stage_raw(L, 1, QB200_MEM_HOST, L->stream))) return rc;
-  if ((rc = launch_voxel(L, 1, leaf, skip_flagged))) return rc;
-  int nv = 0, st = 0;
-  if ((rc = get_counter(L, L->ctr.n_vox, &nv))) return rc;
-  if ((rc = get_counter(L, L->ctr.cloud_status, &st))) return rc;
-  if (st == QB200_ERR_VOXEL_OVERFLOW) {
-    // [EXT] pcl::VoxelGrid: "leaf size is too small ... integer indices would overflow" -> output = input
-    int m = 0;
-    for (int i = 0; i < n; ++i) {
-      const float* p = pts4 + 4 * (size_t)i;
-      if (!(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2])) || (skip_flagged && p[3] < 0.0f)) continue;
-      if (m < cap) memcpy(out4 + 4 * (size_t)m, p, 4 * sizeof(float));
-      ++m;
-    }
-    *n_out = m;
-    return m > cap ? QB200_CAPACITY_EXCEEDED : QB200_ERR_VOXEL_OVERFLOW;
-  }
-  *n_out = nv;
-  const int m = nv < cap ? nv : cap;
-  if (m > 0) {
-    QB_CUDA_TRY(h, cudaMemcpyAsync(out4, L->vox_pts, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
-    QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
-  }
-  if (st == QB200_CAPACITY_EXCEEDED || nv > cap) return QB200_CAPACITY_EXCEEDED;
-  return QB200_OK;
-}
-
 // ---- pre-processing: ground removal (patchwork.hpp:329-455) ---------------------------------------------
 int qb200_patchwork(qb200_handle* h, const float* pts4, int32_t n, const qb200_patchwork_params* p, float* ground4, int32_t* n_ground,
                     float* nonground4, int32_t* n_nonground) {
@@ -797,189 +663,6 @@ int qb200_segment_cloud(qb200_handle* h, const float* pts4, int32_t n, const qb2
   if (outlier4 && no > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(outlier4, dout, (size_t)no * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
   QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   return QB200_OK;
-}
-
-// ---- stage: normals + FPFH ------------------------------------------------------------------------
-int qb200_compute_fpfh(qb200_handle* h, const float* pts4, int32_t n, float normal_radius, float fpfh_radius, float grid_cell,
-                       float* normals4, float* desc33) {
-  if (int rc = enter(h)) return rc;
-  if (n < 0 || (n > 0 && !pts4) || !(normal_radius > 0) || !(fpfh_radius > 0) || !(grid_cell > 0)) return QB200_ERR_BAD_ARG;
-  if (normal_radius > fpfh_radius) return QB200_ERR_BAD_ARG;  // fpfh_manager.hpp:99-102
-  if (n == 0) return QB200_OK;
-  Lane* L = h->lane[0].get();
-  int rc = wave_reset(L, 1);
-  if (rc) return rc;
-  if ((rc = upload_cloud_as_voxels(L, 0, pts4, n))) return rc;
-  if ((rc = launch_fpfh(L, 1, normal_radius, fpfh_radius, grid_cell))) return rc;
-  if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, L->normals, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
-  if (desc33) {
-    float* scratch = L->aos_scratch;
-    if ((rc = launch_desc_to_aos(L, 0, n, scratch))) return rc;
-    QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, scratch, (size_t)n * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
-  }
-  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
-  return QB200_OK;
-}
-
-// ---- stage: matching ------------------------------------------------------------------------------
-// the correspondences launch_match left for pair 0: counts, then the first cap of them
-static int match_result(qb200_handle* h, int32_t* corr, float* sm4, float* tm4, int cap, int32_t* n_corr, int32_t* n_mutual) {
-  Lane* L = h->lane[0].get();
-  int nc = 0, nm = 0, st = 0, rc;
-  if ((rc = get_counter(L, L->ctr.n_corr, &nc))) return rc;
-  if ((rc = get_counter(L, L->ctr.n_mutual, &nm))) return rc;
-  if ((rc = get_counter(L, L->ctr.cloud_status, &st))) return rc;
-  *n_corr = nc;
-  if (n_mutual) *n_mutual = nm;
-  h->last_n_corr = nc;
-  if ((rc = download_corr(L, nc, corr, sm4, tm4, cap))) return rc;
-  return st == QB200_CAPACITY_EXCEEDED ? QB200_CAPACITY_EXCEEDED : QB200_OK;
-}
-
-int qb200_match(qb200_handle* h, const float* src4, int32_t n_src, const float* src_desc33, const float* tgt4, int32_t n_tgt,
-                const float* tgt_desc33, const qb200_params* p, int32_t* corr, int32_t cap, int32_t* n_corr, int32_t* n_mutual) {
-  if (int rc = enter(h)) return rc;
-  if (!p || !n_corr || n_src < 0 || n_tgt < 0 || cap < 0) return QB200_ERR_BAD_ARG;
-  if ((n_src > 0 && (!src4 || !src_desc33)) || (n_tgt > 0 && (!tgt4 || !tgt_desc33))) return QB200_ERR_BAD_ARG;
-  if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
-  *n_corr = 0;
-  if (n_mutual) *n_mutual = 0;
-  Lane* L = h->lane[0].get();
-  if (n_src > L->V || n_tgt > L->V) { h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points"); return QB200_ERR_BAD_ARG; }
-  h->last_match_n[0] = h->last_match_n[1] = 0;
-  if (n_src == 0 || n_tgt == 0) return QB200_OK;
-  int rc = wave_reset(L, 2);
-  if (rc) return rc;
-  if ((rc = upload_cloud_as_voxels(L, 0, src4, n_src))) return rc;
-  if ((rc = upload_cloud_as_voxels(L, 1, tgt4, n_tgt))) return rc;
-  h->last_match_n[0] = n_src;
-  h->last_match_n[1] = n_tgt;
-  float* scratch = L->aos_scratch;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch, src_desc33, (size_t)n_src * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
-  if ((rc = launch_desc_from_aos(L, 0, n_src, scratch))) return rc;
-  float* scratch2 = scratch + (size_t)L->V * kDescDim;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch2, tgt_desc33, (size_t)n_tgt * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
-  if ((rc = launch_desc_from_aos(L, 1, n_tgt, scratch2))) return rc;
-  if ((rc = launch_match(L, 1, *p))) return rc;
-  return match_result(h, corr, nullptr, nullptr, cap, n_corr, n_mutual);
-}
-
-int qb200_match_and_pack(qb200_handle* h, const float* src4, int32_t n_src, const float* tgt4, int32_t n_tgt, const qb200_params* p,
-                         int32_t* corr, float* src_matched4, float* tgt_matched4, int32_t cap, int32_t* n_corr) {
-  if (int rc = enter(h)) return rc;
-  if (!n_corr || !params_ok(p) || n_src < 0 || n_tgt < 0 || cap < 0) return QB200_ERR_BAD_ARG;
-  if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
-  *n_corr = 0;
-  Lane* L = h->lane[0].get();
-  if (n_src > L->V || n_tgt > L->V) { h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points"); return QB200_ERR_BAD_ARG; }
-  if (n_src == 0 || n_tgt == 0) return QB200_OK;
-  int rc = wave_reset(L, 2);
-  if (rc) return rc;
-  if ((rc = upload_cloud_as_voxels(L, 0, src4, n_src))) return rc;
-  if ((rc = upload_cloud_as_voxels(L, 1, tgt4, n_tgt))) return rc;
-  if ((rc = launch_fpfh(L, 2, p->normal_radius, p->fpfh_radius, lattice_cell(*p)))) return rc;
-  if ((rc = launch_match(L, 1, *p))) return rc;
-  return match_result(h, corr, src_matched4, tgt_matched4, cap, n_corr, nullptr);
-}
-
-// ---- stage: graph ---------------------------------------------------------------------------------
-int qb200_build_graph(qb200_handle* h, const float* a4, const float* b4, int32_t L, double noise_bound, double cbar2, uint32_t* adj,
-                      int32_t words_per_row, int32_t* degree, int64_t* n_edges) {
-  if (int rc = enter(h)) return rc;
-  if (L < 0 || (L > 0 && (!a4 || !b4 || !adj)) || words_per_row < (L + 31) / 32 || !(noise_bound > 0) || !(cbar2 > 0))
-    return QB200_ERR_BAD_ARG;
-  if (n_edges) *n_edges = 0;
-  if (L == 0) return QB200_OK;
-  Lane* ln = h->lane[0].get();
-  int rc = upload_matched(ln, a4, b4, L);
-  if (rc) return rc;
-  if ((rc = launch_graph(ln, 1, noise_bound, cbar2))) return rc;
-  const int nb = (L + 31) / 32;
-  memset(adj, 0, (size_t)L * words_per_row * sizeof(uint32_t));
-  QB_CUDA_TRY(h, cudaMemcpy2DAsync(adj, (size_t)words_per_row * 4, ln->adj, (size_t)ln->W * 4, (size_t)nb * 4, L, cudaMemcpyDeviceToHost, ln->stream));
-  if (degree) QB_CUDA_TRY(h, cudaMemcpyAsync(degree, ln->deg, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, ln->stream));
-  long long e2 = 0;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(&e2, ln->ctr.n_edges, sizeof(long long), cudaMemcpyDeviceToHost, ln->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(ln->stream));
-  if (n_edges) *n_edges = e2 / 2;
-  return QB200_OK;
-}
-
-// ---- stage: max clique ------------------------------------------------------------------------------
-int qb200_max_clique_ex(qb200_handle* h, const uint32_t* adj, int32_t L, int32_t words_per_row, int32_t mode, double kcore_thr,
-                        int64_t node_limit, int32_t* clique, int32_t* n_clique, int32_t* kcore, int32_t* kcore_order, int32_t* max_core,
-                        int32_t* flags) {
-  if (int rc = enter(h)) return rc;
-  if (!n_clique || L < 0 || (L > 0 && (!adj || !clique)) || words_per_row < (L + 31) / 32) return QB200_ERR_BAD_ARG;
-  if (mode != QB200_PMC_EXACT && mode != QB200_PMC_HEU && mode != QB200_KCORE_HEU) return QB200_ERR_BAD_ARG;
-  if (node_limit < 0) return QB200_ERR_BAD_ARG;
-  if (flags) *flags = 0;
-  *n_clique = 0;
-  if (max_core) *max_core = 0;
-  Lane* ln = h->lane[0].get();
-  if (L > ln->Lc) { h->fail(__FILE__, __LINE__, "L exceeds max_corr"); return QB200_ERR_BAD_ARG; }
-  if (L == 0) return QB200_OK;
-  int rc = wave_reset(ln, 2);
-  if (rc) return rc;
-  const int nb = (L + 31) / 32;
-  QB_CUDA_TRY(h, cudaMemsetAsync(ln->adj, 0, (size_t)L * ln->W * 4, ln->stream));
-  QB_CUDA_TRY(h, cudaMemcpy2DAsync(ln->adj, (size_t)ln->W * 4, adj, (size_t)words_per_row * 4, (size_t)nb * 4, L, cudaMemcpyHostToDevice, ln->stream));
-  if ((rc = set_counter(ln, ln->ctr.n_corr, L))) return rc;
-  if ((rc = launch_degree(ln, 1))) return rc;
-  if ((rc = launch_clique(ln, 1, mode, kcore_thr, node_limit))) return rc;
-  int nc = 0, mc = 0, fl = 0;
-  if ((rc = get_counter(ln, ln->ctr.n_clique, &nc))) return rc;
-  if ((rc = get_counter(ln, ln->ctr.max_core, &mc))) return rc;
-  if ((rc = get_counter(ln, ln->ctr.flags, &fl))) return rc;
-  if (flags) *flags = fl;
-  *n_clique = nc;
-  if (max_core) *max_core = mc;
-  if (nc > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(clique, ln->clique, (size_t)nc * sizeof(int), cudaMemcpyDeviceToHost, ln->stream));
-  if (kcore) QB_CUDA_TRY(h, cudaMemcpyAsync(kcore, ln->kcore, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, ln->stream));
-  if (kcore_order) QB_CUDA_TRY(h, cudaMemcpyAsync(kcore_order, ln->korder, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, ln->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(ln->stream));
-  h->last_n_clique = nc;
-  return QB200_OK;
-}
-
-int qb200_max_clique(qb200_handle* h, const uint32_t* adj, int32_t L, int32_t words_per_row, int32_t mode, double kcore_thr,
-                     int32_t* clique, int32_t* n_clique, int32_t* kcore, int32_t* kcore_order, int32_t* max_core) {
-  return qb200_max_clique_ex(h, adj, L, words_per_row, mode, kcore_thr, 0, clique, n_clique, kcore, kcore_order, max_core, nullptr);
-}
-
-// ---- stage: pose given the clique -------------------------------------------------------------------
-int qb200_solve_pose(qb200_handle* h, const float* a4, const float* b4, int32_t L, const int32_t* clique, int32_t n_clique,
-                     const qb200_params* p, qb200_result* res, uint8_t* rot_inlier_mask, uint8_t* trans_inlier_mask) {
-  if (int rc = enter(h)) return rc;
-  if (!res || !params_ok(p) || L < 0 || (L > 0 && (!a4 || !b4)) || n_clique < 0 || n_clique > L || (n_clique > 0 && !clique))
-    return QB200_ERR_BAD_ARG;
-  Lane* ln = h->lane[0].get();
-  int rc = upload_matched(ln, a4, b4, L);
-  if (rc) return rc;
-  if (n_clique > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ln->clique, clique, (size_t)n_clique * sizeof(int), cudaMemcpyHostToDevice, ln->stream));
-  if ((rc = set_counter(ln, ln->ctr.n_clique, n_clique))) return rc;
-  if ((rc = launch_fill_counters(ln, 1, 0))) return rc;
-  if ((rc = launch_pose(ln, 1, resolve_params(h, *p)))) return rc;
-  rc = fetch_result(h, res);
-  if (rc < 0) return rc;
-  if (res->valid) {
-    const int nc = res->clique_size;
-    if (rot_inlier_mask) QB_CUDA_TRY(h, cudaMemcpyAsync(rot_inlier_mask, ln->rot_mask, (size_t)nc, cudaMemcpyDeviceToHost, ln->stream));
-    if (trans_inlier_mask) QB_CUDA_TRY(h, cudaMemcpyAsync(trans_inlier_mask, ln->trans_mask, (size_t)nc, cudaMemcpyDeviceToHost, ln->stream));
-    QB_CUDA_TRY(h, cudaStreamSynchronize(ln->stream));
-  }
-  return rc;
-}
-
-// ---- Quatro::computeTransformation ------------------------------------------------------------------
-int qb200_solve_correspondences(qb200_handle* h, const float* a4, const float* b4, int32_t L, const qb200_params* p, qb200_result* res) {
-  if (int rc = enter(h)) return rc;
-  if (!res || !params_ok(p) || L < 0 || (L > 0 && (!a4 || !b4))) return QB200_ERR_BAD_ARG;
-  Lane* ln = h->lane[0].get();
-  int rc = upload_matched(ln, a4, b4, L);
-  if (rc) return rc;
-  if ((rc = run_solver(ln, 1, resolve_params(h, *p), 0))) return rc;
-  return fetch_result(h, res);
 }
 
 // ---- batches of precomputed correspondences -> poses ------------------------------------------------------
@@ -1123,107 +806,9 @@ int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const
   return res->status;
 }
 
-// ---- introspection ----------------------------------------------------------------------------------
-int qb200_get_last_clique(qb200_handle* h, int32_t* idx, int32_t cap, int32_t* n) {
-  if (int rc = enter(h)) return rc;
-  return copy_ints(h->lane[0].get(), h->lane[0]->clique, h->last_n_clique, idx, cap, n);
-}
-int qb200_get_last_final_inliers(qb200_handle* h, int32_t* idx, int32_t cap, int32_t* n) {
-  if (int rc = enter(h)) return rc;
-  return copy_ints(h->lane[0].get(), h->lane[0]->final_inl, h->last_n_final, idx, cap, n);
-}
-int qb200_get_last_correspondences(qb200_handle* h, int32_t* corr, float* src_matched4, float* tgt_matched4, int32_t cap, int32_t* n) {
-  if (int rc = enter(h)) return rc;
-  if (!n || cap < 0) return QB200_ERR_BAD_ARG;
-  *n = h->last_n_corr;
-  return download_corr(h->lane[0].get(), h->last_n_corr, corr, src_matched4, tgt_matched4, cap);
-}
-
-int qb200_get_last_features(qb200_handle* h, int32_t which, float* normals4, float* desc33, int32_t cap, int32_t* n_out) {
-  if (int rc = enter(h)) return rc;
-  if (!n_out || which < 0 || which > 1 || cap < 0) return QB200_ERR_BAD_ARG;
-  Lane* L = h->lane[0].get();
-  int n = 0, rc;
-  if ((rc = get_counter(L, L->ctr.n_vox + which, &n))) return rc;
-  *n_out = n;
-  const int m = n < cap ? n : cap;
-  if (m > 0) {
-    if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, L->normals + (size_t)which * L->V, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
-    if (desc33) {
-      if ((rc = launch_desc_to_aos(L, which, m, L->aos_scratch))) return rc;
-      QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, L->aos_scratch, (size_t)m * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
-    }
-    QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
-  }
-  return n > cap ? QB200_CAPACITY_EXCEEDED : QB200_OK;
-}
-
 int qb200_get_stage_ms(qb200_handle* h, float* ms, int32_t n) {
   if (!h || !ms || n < 0) return QB200_ERR_BAD_ARG;
   for (int i = 0; i < n && i < 8; ++i) ms[i] = h->stage_ms[i];
-  return QB200_OK;
-}
-
-// QB200_TC_VERIFY=1: every batch is matched by BOTH K6 implementations and the packed (distance, index) results are compared;
-// out2[0] = nearest-neighbour entries compared, out2[1] = entries that differ (must stay 0: the tensor-core filter is exact).
-int qb200_debug_match_verify(qb200_handle* h, uint64_t* out2, int32_t reset) {
-  if (int rc = enter(h)) return rc;
-  return out2 ? read_tc_stats(h, 4, 2, out2, reset) : QB200_ERR_BAD_ARG;
-}
-
-// QB200_TC_PROF=1: clock64 accounting of tc_nn_kernel's roles (cycles summed over CTAs / warps), stats[8..31] -> out24
-int qb200_debug_tc_profile(qb200_handle* h, uint64_t* out24, int32_t reset) {
-  if (int rc = enter(h)) return rc;
-  return out24 ? read_tc_stats(h, 8, 24, out24, reset) : QB200_ERR_BAD_ARG;
-}
-
-int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset) {
-  if (int rc = enter(h)) return rc;
-  return out4 ? read_tc_stats(h, 0, 4, out4, reset) : QB200_ERR_BAD_ARG;
-}
-
-// Nearest-neighbour tables of the most recent qb200_match (pair 0 of the handle, point order): what match_mutual_kernel read
-int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, uint64_t* colbest, int32_t cap_cols) {
-  if (int rc = enter(h)) return rc;
-  if (cap_rows < 0 || cap_cols < 0) return QB200_ERR_BAD_ARG;
-  Lane* L = h->lane[0].get();
-  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
-  const int nr = cap_rows < h->last_match_n[0] ? cap_rows : h->last_match_n[0];
-  const int nc = cap_cols < h->last_match_n[1] ? cap_cols : h->last_match_n[1];
-  if (rowbest && nr > 0) QB_CUDA_TRY(h, cudaMemcpy(rowbest, L->rowbest, (size_t)nr * 8, cudaMemcpyDeviceToHost));
-  if (colbest && nc > 0) QB_CUDA_TRY(h, cudaMemcpy(colbest, L->colbest, (size_t)nc * 8, cudaMemcpyDeviceToHost));
-  return QB200_OK;
-}
-
-// Footprint of the tensor-core nearest-neighbour kernel as it is launched: out5 = threads per CTA, dynamic and static shared
-// bytes, registers per thread, resident CTAs per SM (occupancy calculator at that shared-memory size)
-int qb200_debug_tc_footprint(qb200_handle* h, int32_t* out5) {
-  if (!h || !out5) return QB200_ERR_BAD_ARG;
-  cudaSetDevice(h->cfg.device);
-  return tc_footprint(h->lane[0].get(), out5);
-}
-
-// Validation hook: tensor-core (3xTF32) approximate squared distances between up to 128 source and 128 target
-// descriptors -> out[128*128] (row = source).  Lets tests measure the filter's error against the exact chain.
-int qb200_debug_tc_distances(qb200_handle* h, const float* a33, int32_t na, const float* b33, int32_t nb, float* out) {
-  if (int rc = enter(h)) return rc;
-  if (!a33 || !b33 || !out || na < 1 || nb < 1 || na > 128 || nb > 128) return QB200_ERR_BAD_ARG;
-  Lane* L = h->lane[0].get();
-  int rc = wave_reset(L, 2);
-  if (rc) return rc;
-  if ((rc = set_counter(L, L->ctr.n_vox + 0, na))) return rc;
-  if ((rc = set_counter(L, L->ctr.n_vox + 1, nb))) return rc;
-  float* scratch = L->aos_scratch;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch, a33, (size_t)na * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
-  if ((rc = launch_desc_from_aos(L, 0, na, scratch))) return rc;
-  float* scratch2 = scratch + (size_t)128 * kDescDim;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch2, b33, (size_t)nb * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
-  if ((rc = launch_desc_from_aos(L, 1, nb, scratch2))) return rc;
-  float* d_out = L->spfh;  // not the sort scratch: K6 sorts the descriptors by norm first
-  QB_CUDA_TRY(h, cudaMemsetAsync(d_out, 0, 128 * 128 * sizeof(float), L->stream));
-  if ((rc = launch_tc_debug_tile(L, d_out))) return rc;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(out, d_out, 128 * 128 * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   return QB200_OK;
 }
 
@@ -1334,8 +919,9 @@ int qb200_cache_read(qb200_handle* h, int32_t slot, float* vox4, float* normals4
   if (int rc = enter(h)) return rc;
   if (!n_out || slot < 0 || slot >= h->c_slots || cap < 0) return QB200_ERR_BAD_ARG;
   Lane* L = h->lane[0].get();
-  int n = 0, rc;
-  if ((rc = get_counter(L, h->c_n + slot, &n))) return rc;
+  int n = 0;
+  QB_CUDA_TRY(h, cudaMemcpyAsync(&n, h->c_n + slot, sizeof(int), cudaMemcpyDeviceToHost, L->stream));
+  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   *n_out = n;
   const int m = n < cap ? n : cap;
   const size_t V = L->V;
@@ -1363,6 +949,14 @@ int qb200_get_kernel_ms(qb200_handle* h, float* ms, int32_t* launches, int32_t n
 }  // extern "C"
 
 namespace qb {
+// Prologue of every entry point that uses lane 0's buffers or stream: a handle, its device current, and no wave of
+// qb200_register_batch_enqueue in flight any more (their records are completed first).
+int enter(qb200_handle* h) {
+  if (!h) return QB200_ERR_BAD_ARG;
+  cudaSetDevice(h->cfg.device);
+  return h->lanes_active ? batch_flush(h) : QB200_OK;
+}
+
 int collect_batch(qb200_handle* h, const qb200_result* dst) {
   cudaSetDevice(h->cfg.device);
   return collect_waves(h, dst);

@@ -90,8 +90,8 @@ struct Lane {
   PinnedMem<qb200_result> h_results; // [S]
   PinnedMem<unsigned char> lst_stage; int lst_cap;  // host-kind pair lists, grown on first use: [S][lst_cap] entries of every list
                                                     // (ListDst::carve), written by pack_lists_kernel through the mapped address
-  WaveCounters ctr;
-  DeviceMem<int> ctr_block; size_t ctr_ints;
+  WaveCounters ctr, hctr;     // the counter block, and the same layout over its pinned mirror (stage calls read it back whole)
+  DeviceMem<int> ctr_block; PinnedMem<int> hctr_block; size_t ctr_ints;
 
   Event ev[9];                // stage boundaries of the last wave: start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
   Event kev[4];               // [0,1] around match_stripe_kernel, [2,3] around tim_graph_kernel (last wave)
@@ -209,6 +209,16 @@ int desc_to_aos_rows(Lane* h, const float* desc_rows, int n, float* d_out33);
 size_t sort_temp_bytes(int max_items);
 void comm_release(qb200_handle* h);
 int collect_batch(qb200_handle* h, const qb200_result* dst);  // api.cu: wait for every wave in flight that writes into dst[...]
+// api.cu, shared with the single-pair entry points of stages.cu
+int enter(qb200_handle* h);  // entry prologue: a handle, its device current, no enqueued batch in flight
+int wave_reset(Lane* L, int n_clouds);
+int stage_raw(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs);
+int run_solver(Lane* L, int n_pairs, const qb200_params& p, int have_frontend);
+int launch_degree(Lane* h, int n_pairs);
+bool params_ok(const qb200_params* p);
+float lattice_cell(const qb200_params& p);
+qb200_params resolve_params(qb200_handle* h, const qb200_params& p);
+void set_last(qb200_handle* h, const qb200_result& r);
 // Raise a kernel's dynamic shared-memory opt-in to at least `bytes` on `device`.  The attribute is a property of the
 // (function, device), not of a handle: handles of different capacities share it, so it is only ever raised (process-wide maximum).
 cudaError_t ensure_dyn_smem(int device, const void* kernel, size_t bytes);
