@@ -235,6 +235,28 @@ void qb200_default_segment_params(qb200_segment_params* p);
 int qb200_segment_cloud(qb200_handle* h, const float* pts4, int32_t n, const qb200_segment_params* p,
                         float* valid4, int32_t* n_valid, float* outlier4, int32_t* n_outlier);
 
+/* qb200_preprocess_batch: the example's pre-processing (examples/run_global_registration.cpp:136-162) for many scans in one call.
+ * For every scan i each output array and each count is byte-identical to qb200_patchwork(scan i) followed by
+ * qb200_segment_cloud on that scan's non-ground output, on the same handle; nothing depends on the batch size or the scan's
+ * position in it.  Scans are processed in waves of 2 * max_batch_slots; the non-ground clouds stay on the device between the two
+ * steps.  scans4[i]: n_points[i] x {x,y,z,w} in `kind` memory (n_points[i] <= max_raw_points).  sp == NULL: ground removal only
+ * (valid and outlier counts are 0 and their arrays are not touched).
+ * Bad arguments fail the whole call with QB200_ERR_BAD_ARG before any work starts. */
+typedef struct qb200_preprocess_out {
+  int32_t cap_per_scan;  /* >= 1: points reserved per scan in every point array below */
+  int32_t kind;          /* qb200_mem_kind of the four point arrays (QB200_MEM_DEVICE: memory of the handle's device, 16-byte aligned) */
+  float* ground4;        /* [n][cap][4] or NULL */
+  float* nonground4;     /* [n][cap][4] or NULL */
+  float* valid4;         /* [n][cap][4] valid segments of the non-ground cloud, or NULL */
+  float* outlier4;       /* [n][cap][4] or NULL */
+  int32_t* counts;       /* host [n][4] ground, non-ground, valid, outlier: full counts, never clipped */
+  int32_t* status;       /* host [n] what qb200_patchwork returns for that scan (QB200_OK / QB200_CAPACITY_EXCEEDED) */
+} qb200_preprocess_out;  /* scan i's entries start at i * cap_per_scan; it gets min(count, cap_per_scan) of them, and nothing past
+                            that is written: a count above cap_per_scan shows the clipping */
+int qb200_preprocess_batch(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
+                           qb200_mem_kind kind, const qb200_patchwork_params* pp,
+                           const qb200_segment_params* sp /* NULL: ground removal only */, const qb200_preprocess_out* out);
+
 /* normals4: n x {nx,ny,nz,curvature}; desc33: n x 33 floats (pcl::FPFHSignature33). Either may be NULL. */
 int qb200_compute_fpfh(qb200_handle* h, const float* pts4, int32_t n, float normal_radius,
                        float fpfh_radius, float grid_cell, float* normals4, float* desc33);

@@ -95,6 +95,15 @@ class PairLists(C.Structure):
                 ("rot_inlier_mask", C.c_void_p), ("trans_inlier_mask", C.c_void_p)]
 
 
+class PreprocessOut(C.Structure):
+    """qb200_preprocess_out: caller-owned outputs of qb200_preprocess_batch, cap_per_scan points reserved per scan."""
+    _fields_ = [("cap_per_scan", C.c_int32), ("kind", C.c_int32), ("ground4", C.c_void_p), ("nonground4", C.c_void_p),
+                ("valid4", C.c_void_p), ("outlier4", C.c_void_p), ("counts", C.c_void_p), ("status", C.c_void_p)]
+
+
+PREPROCESS_ARRAYS = ("ground4", "nonground4", "valid4", "outlier4")   # in the order of the four counts
+
+
 # list name -> (element dtype, trailing shape, count field of the record)
 LIST_LAYOUT = {
     "corr": (np.int32, (2,), "n_corr"),
@@ -239,6 +248,7 @@ def load_library(build: bool = True) -> C.CDLL:
         "qb200_register_batch_enqueue_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
         "qb200_register_cached_ex": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
         "qb200_solve_batch_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+        "qb200_preprocess_batch": (i32, [vp, vp, vp, i32, i32, P(PatchworkParams), P(SegmentParams), P(PreprocessOut)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError = header/library mismatch: fail loudly
@@ -266,6 +276,7 @@ EXPORTED_SYMBOLS = [
     "qb200_register_batch_rank", "qb200_comm_wait", "qb200_bind_numa",
     "qb200_debug_match_verify", "qb200_get_last_features", "qb200_cache_reserve", "qb200_cache_scans", "qb200_register_cached", "qb200_cache_copy", "qb200_cache_read",
     "qb200_register_batch_ex", "qb200_register_batch_enqueue_ex", "qb200_register_cached_ex", "qb200_solve_batch_ex",
+    "qb200_preprocess_batch",
 ]
 
 
@@ -434,6 +445,45 @@ class Handle:
         self._check(self.lib.qb200_segment_cloud(self.h, _ptr(pts), len(pts), C.byref(sp), _ptr(v), C.byref(a), _ptr(o), C.byref(b)),
                     "qb200_segment_cloud")
         return v[: a.value].copy(), o[: b.value].copy()
+
+    def preprocess_batch(self, scans: Sequence, pp: "PatchworkParams", sp: Optional["SegmentParams"] = None, cap: Optional[int] = None,
+                         kind: int = MEM_HOST, dest: int = MEM_HOST, arrays: Optional[dict] = None):
+        """qb200_preprocess_batch.  scans: (n,4) float32 arrays (MEM_HOST) or (device_ptr, n) tuples (MEM_DEVICE).  cap: points per
+        scan and array (default: room for the largest output).  arrays: the caller's own output arrays by name (PREPROCESS_ARRAYS),
+        numpy (dest MEM_HOST) or CUDA tensors (dest MEM_DEVICE) of shape (n_scans, cap, 4); a name left out is passed as NULL.
+        Returns (per scan a tuple (ground, nonground, valid, outlier) trimmed to min(count, cap), None for a NULL array;
+        counts (n,4) int32; status (n,) int32)."""
+        n = len(scans)
+        keep = [_f32(sc, 4) for sc in scans] if kind == MEM_HOST else None
+        sizes = [len(a) for a in keep] if kind == MEM_HOST else [int(sc[1]) for sc in scans]
+        ptrs = (C.c_void_p * max(n, 1))(*([a.ctypes.data for a in keep] if kind == MEM_HOST else [sc[0] for sc in scans]))
+        cnts = (C.c_int32 * max(n, 1))(*sizes)
+        if cap is None:
+            cap = max([1, *sizes] + ([sp.n_scan * sp.horizon_scan] if sp is not None else []))
+        if arrays is None:
+            names = PREPROCESS_ARRAYS if sp is not None else PREPROCESS_ARRAYS[:2]
+            if dest == MEM_HOST:
+                arrays = {k: np.zeros((max(n, 1), cap, 4), np.float32) for k in names}
+            else:
+                import torch
+                arrays = {k: torch.zeros((max(n, 1), cap, 4), dtype=torch.float32, device=f"cuda:{self.cfg.device}") for k in names}
+        counts = np.zeros((max(n, 1), 4), np.int32)
+        status = np.zeros(max(n, 1), np.int32)
+        out = PreprocessOut(cap, dest)
+        for k, a in arrays.items():
+            setattr(out, k, a.ctypes.data if dest == MEM_HOST else a.data_ptr())
+        out.counts, out.status = counts.ctypes.data, status.ctypes.data
+        self._check(self.lib.qb200_preprocess_batch(self.h, ptrs, cnts, n, kind, C.byref(pp), C.byref(sp) if sp is not None else None,
+                                                    C.byref(out)), "qb200_preprocess_batch")
+        per_scan = []
+        for i in range(n):
+            row = []
+            for j, k in enumerate(PREPROCESS_ARRAYS):
+                a = arrays.get(k)
+                m = min(int(counts[i, j]), cap)
+                row.append(None if a is None else (a[i, :m].copy() if dest == MEM_HOST else a[i, :m].cpu().numpy()))
+            per_scan.append(tuple(row))
+        return per_scan, counts[:n], status[:n]
 
     def max_clique(self, adj, mode: int = PMC_HEU, kcore_thr: float = 0.5):
         adj = np.ascontiguousarray(adj, np.uint32)

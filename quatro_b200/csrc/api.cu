@@ -623,48 +623,6 @@ int64_t qb200_launch_count(const qb200_handle* h) {
   return n;
 }
 
-// ---- pre-processing: ground removal (patchwork.hpp:329-455) ---------------------------------------------
-int qb200_patchwork(qb200_handle* h, const float* pts4, int32_t n, const qb200_patchwork_params* p, float* ground4, int32_t* n_ground,
-                    float* nonground4, int32_t* n_nonground) {
-  if (int rc = enter(h)) return rc;
-  if (!p || !n_ground || !n_nonground || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
-  *n_ground = *n_nonground = 0;
-  Lane* L = h->lane[0].get();
-  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
-  if (n > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(L->raw_stage, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
-  int ng = 0, nn = 0, st = 0;
-  const int rc = launch_patchwork(L, L->raw_stage, n, *p, &ng, &nn, &st);
-  if (rc) return rc;
-  *n_ground = ng;
-  *n_nonground = nn;
-  if (ground4 && ng > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ground4, L->pw_out, (size_t)ng * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
-  if (nonground4 && nn > 0)
-    QB_CUDA_TRY(h, cudaMemcpyAsync(nonground4, L->pw_out + L->R, (size_t)nn * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
-  return st;
-}
-
-// ---- pre-processing: range-image sub-cluster removal (imageProjection.hpp:273-294) ------------------------
-int qb200_segment_cloud(qb200_handle* h, const float* pts4, int32_t n, const qb200_segment_params* p, float* valid4, int32_t* n_valid,
-                        float* outlier4, int32_t* n_outlier) {
-  if (int rc = enter(h)) return rc;
-  if (!p || !n_valid || !n_outlier || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
-  *n_valid = *n_outlier = 0;
-  Lane* L = h->lane[0].get();
-  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
-  if (n > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(L->raw_stage, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
-  int nv = 0, no = 0;
-  const float4 *dv = nullptr, *dout = nullptr;
-  const int rc = launch_segment_cloud(L, L->raw_stage, n, *p, &nv, &no, &dv, &dout);
-  if (rc) return rc;
-  *n_valid = nv;
-  *n_outlier = no;
-  if (valid4 && nv > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(valid4, dv, (size_t)nv * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
-  if (outlier4 && no > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(outlier4, dout, (size_t)no * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
-  return QB200_OK;
-}
-
 // ---- batches of precomputed correspondences -> poses ------------------------------------------------------
 int qb200_solve_batch(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p, qb200_mem_kind kind,
                       qb200_result* results) {

@@ -81,10 +81,12 @@ struct Lane {
   DeviceMem<unsigned char> pose_ws; // [S * pose_ws_bytes(Lc)] pose workspace of cliques above kPoseSmemClique members (Lc > kPoseSmemClique only)
   DeviceMem<int> final_inl;   // [S*Lc]
   DeviceMem<unsigned char> rot_mask, trans_mask; // [S*Lc]
-  // ---- pre-processing (preprocess.cu), allocated on first use ----
-  DeviceMem<int> pw_ints;     // patch id / rank per point, per-patch counters and offsets
-  DeviceMem<float4> pw_out;   // [2*R] ground | non-ground
-  DeviceMem<void> ip_buf; int ip_npix;  // range-image scratch (per pixel: winner, parent, size, range, row set, two outputs)
+  // ---- pre-processing (preprocess.cu), allocated on first use for the largest wave so far (pw_scans / ip_cap) ----
+  DeviceMem<int> pp_cnt; PinnedMem<int> pp_hcnt;  // [2S][8] per-scan counts and status of a wave, and its pinned mirror
+  DeviceMem<int> pw_ints;     // [pw_scans] x (patch id / rank per point, per-patch counters and offsets)
+  DeviceMem<float4> pw_out;   // [pw_scans][R] ground | non-ground
+  int pw_scans;
+  DeviceMem<void> ip_buf; size_t ip_cap;  // range-image scratch (per scan and pixel: winner, parent, size, range, row set, output)
   // ---- results ----
   DeviceMem<qb200_result> d_results; // [S]
   PinnedMem<qb200_result> h_results; // [S]
@@ -196,9 +198,6 @@ __host__ __device__ inline int list_entries(int count, int Lc, int cap) {
   const int n = count < 0 ? 0 : count > Lc ? Lc : count;
   return n < cap ? n : cap;
 }
-int launch_segment_cloud(Lane* h, const float4* pts, int n, const qb200_segment_params& sp, int* n_valid, int* n_outlier,
-                         const float4** valid_dev, const float4** outlier_dev);
-int launch_patchwork(Lane* h, const float4* pts, int n, const qb200_patchwork_params& pp, int* n_ground, int* n_nonground, int* status);
 int launch_match_nn(Lane* h, int n_pairs);
 int launch_match_exact(Lane* h, int n_pairs, const int* only);
 int launch_tc_debug_tile(Lane* h, float* d_out);

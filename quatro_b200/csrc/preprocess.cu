@@ -25,6 +25,9 @@ namespace qb {
 constexpr int kPwThreads = 256;
 constexpr int kPwMaxPatchPts = 16384;   // keys of one patch in shared memory (128 KB)
 constexpr int kPwMaxPatches = 4096;
+constexpr int kPwStride = kPwMaxPatches + 1;   // per-scan entries of every per-patch array
+// per-scan count block of a wave, [scan][kPpCnt]: ground, non-ground, patchwork status, valid, outlier (+ 3 spare)
+constexpr int kPpCnt = 8;
 
 struct PwDev {   // device copy of the parameters + derived table
   qb200_patchwork_params p;
@@ -66,21 +69,26 @@ __device__ __forceinline__ int pw_patch_of(const float4 pt, const PwDev& c) {
   return c.patch_base[k] + ring * pp.num_sectors_each_zone[k] + sector;
 }
 
-__global__ void __launch_bounds__(256) pw_bin_kernel(const float4* __restrict__ pts, int n, PwDev c, int* __restrict__ patch_of,
-                                                     int* __restrict__ count) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float4 p = pts[i];
+// Every kernel serves a wave of scans: blockIdx.y (or the one CTA of the per-scan scans) is the scan s, and scan s's scratch sits at
+// fixed strides -- R points (patch_of, rank, items, the two outputs) and kPwStride patches (counts, starts, offsets) -- so that a
+// scan's results never depend on the wave it rides in.
+__global__ void __launch_bounds__(256) pw_bin_kernel(const float4* const* __restrict__ pts_of, const int* __restrict__ n_of, PwDev c, int R,
+                                                     int* __restrict__ patch_of, int* __restrict__ count) {
+  const int s = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_of[s]) return;
+  const float4 p = pts_of[s][i];
   int pid = -1;
   // non-finite points never enter (D11); :356-368 drops everything below -1.8 sensor_height
   if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z) && !((double)p.z < -1.8 * c.p.sensor_height)) pid = pw_patch_of(p, c);
-  patch_of[i] = pid;
-  if (pid >= 0) atomicAdd(&count[pid], 1);
+  patch_of[(size_t)s * R + i] = pid;
+  if (pid >= 0) atomicAdd(&count[(size_t)s * kPwStride + pid], 1);
 }
 
-// start[] = exclusive scan of count[0..np), start[np] = total; cursor = copy of start
+// one CTA per scan: start[] = exclusive scan of count[0..np), start[np] = total; cursor = copy of start
 __global__ void __launch_bounds__(1024) pw_scan_kernel(const int* __restrict__ count, int np, int* __restrict__ start, int* __restrict__ cursor) {
   __shared__ int sm[33];
+  const size_t o = (size_t)blockIdx.x * kPwStride;
+  count += o; start += o; cursor += o;
   int carry = 0;
   for (int base = 0; base < np; base += 1024) {
     const int q = base + threadIdx.x;
@@ -93,17 +101,18 @@ __global__ void __launch_bounds__(1024) pw_scan_kernel(const int* __restrict__ c
   if (threadIdx.x == 0) start[np] = carry;
 }
 
-__global__ void __launch_bounds__(256) pw_scatter_kernel(const float4* __restrict__ pts, int n, const int* __restrict__ patch_of,
-                                                         int* __restrict__ cursor, unsigned long long* __restrict__ items) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int pid = patch_of[i];
+__global__ void __launch_bounds__(256) pw_scatter_kernel(const float4* const* __restrict__ pts_of, const int* __restrict__ n_of, int R,
+                                                         const int* __restrict__ patch_of, int* __restrict__ cursor,
+                                                         unsigned long long* __restrict__ items) {
+  const int s = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_of[s]) return;
+  const int pid = patch_of[(size_t)s * R + i];
   if (pid < 0) return;
-  const float z = pts[i].z + 0.0f;  // -0 -> +0: the comparator z_a < z_b does not tell them apart
+  const float z = pts_of[s][i].z + 0.0f;  // -0 -> +0: the comparator z_a < z_b does not tell them apart
   unsigned zb = __float_as_uint(z);
   zb = (zb & 0x80000000u) ? ~zb : (zb | 0x80000000u);  // order-preserving
-  const int pos = atomicAdd(&cursor[pid], 1);
-  items[pos] = ((unsigned long long)zb << 32) | (unsigned)i;
+  const int pos = atomicAdd(&cursor[(size_t)s * kPwStride + pid], 1);
+  items[(size_t)s * R + pos] = ((unsigned long long)zb << 32) | (unsigned)i;
 }
 
 __device__ __forceinline__ void pw_plane_from_accu(float accu[9], int cnt, float n[3], float mean[3], float* surf) {
@@ -126,11 +135,11 @@ __device__ __forceinline__ void pw_plane_from_accu(float accu[9], int cnt, float
   mean[0] = accu[6]; mean[1] = accu[7]; mean[2] = accu[8];
 }
 
-// One CTA per patch.  keys: sorted (z | index); flag[p] = sorted position p belongs to the current ground set.
-__global__ void __launch_bounds__(kPwThreads) pw_patch_kernel(const float4* __restrict__ pts, PwDev c, const int* __restrict__ start,
-                                                              unsigned long long* __restrict__ items, int cap_pow2,
-                                                              int* __restrict__ n_ground, int* __restrict__ n_nonground,
-                                                              int* __restrict__ rank_out, int* __restrict__ status) {
+// One CTA per (patch, scan).  keys: sorted (z | index); flag[p] = sorted position p belongs to the current ground set.
+__global__ void __launch_bounds__(kPwThreads) pw_patch_kernel(const float4* const* __restrict__ pts_of, PwDev c, int R,
+                                                              const int* __restrict__ start, unsigned long long* __restrict__ items,
+                                                              int cap_pow2, int* __restrict__ n_ground, int* __restrict__ n_nonground,
+                                                              int* __restrict__ rank_out, int* __restrict__ cnt) {
   extern __shared__ __align__(16) unsigned char pw_smem[];
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(pw_smem);   // [cap_pow2]
   unsigned char* flag = reinterpret_cast<unsigned char*>(keys + cap_pow2);     // [cap_pow2]
@@ -140,12 +149,15 @@ __global__ void __launch_bounds__(kPwThreads) pw_patch_kernel(const float4* __re
   __shared__ double s_lpr;
   __shared__ int s_init, s_keep, s_scan[33];
   const qb200_patchwork_params& pp = c.p;
-  const int pid = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int pid = blockIdx.x, scan = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const float4* __restrict__ pts = pts_of[scan];
+  start += (size_t)scan * kPwStride; n_ground += (size_t)scan * kPwStride; n_nonground += (size_t)scan * kPwStride;
+  items += (size_t)scan * R; rank_out += (size_t)scan * R;
   const int s0 = start[pid], m = start[pid + 1] - s0;
   if (!(m > pp.num_min_pts) || m > kPwMaxPatchPts) {   // :382 -- small patches are dropped altogether
     if (tid == 0) {
       n_ground[pid] = 0; n_nonground[pid] = 0;
-      if (m > kPwMaxPatchPts) *status = QB200_CAPACITY_EXCEEDED;
+      if (m > kPwMaxPatchPts) cnt[(size_t)scan * kPpCnt + 2] = QB200_CAPACITY_EXCEEDED;
     }
     return;
   }
@@ -300,10 +312,12 @@ __global__ void __launch_bounds__(kPwThreads) pw_patch_kernel(const float4* __re
   }
 }
 
-// exclusive scans of the per-patch output counts; totals -> out_n[0] (ground), out_n[1] (non-ground)
+// one CTA per scan: exclusive scans of the per-patch output counts; totals -> cnt[0] (ground), cnt[1] (non-ground)
 __global__ void __launch_bounds__(1024) pw_offsets_kernel(const int* __restrict__ n_ground, const int* __restrict__ n_nonground, int np,
-                                                          int* __restrict__ goff, int* __restrict__ ngoff, int* __restrict__ out_n) {
+                                                          int* __restrict__ goff, int* __restrict__ ngoff, int* __restrict__ cnt) {
   __shared__ int sm[33];
+  const size_t o = (size_t)blockIdx.x * kPwStride;
+  n_ground += o; n_nonground += o; goff += o; ngoff += o;
   int cg = 0, cn = 0;
   for (int base = 0; base < np; base += 1024) {
     const int q = base + threadIdx.x;
@@ -315,85 +329,43 @@ __global__ void __launch_bounds__(1024) pw_offsets_kernel(const int* __restrict_
     if (q < np) ngoff[q] = cn + ex;
     cn += tot;
   }
-  if (threadIdx.x == 0) { out_n[0] = cg; out_n[1] = cn; }
+  if (threadIdx.x == 0) { cnt[(size_t)blockIdx.x * kPpCnt] = cg; cnt[(size_t)blockIdx.x * kPpCnt + 1] = cn; }
 }
 
-__global__ void __launch_bounds__(256) pw_gather_kernel(const float4* __restrict__ pts, const int* __restrict__ start, const int* __restrict__ n_ground,
-                                                        const int* __restrict__ n_nonground, const unsigned long long* __restrict__ items,
-                                                        const int* __restrict__ rank, const int* __restrict__ goff, const int* __restrict__ ngoff,
-                                                        float4* __restrict__ ground, float4* __restrict__ nonground) {
-  const int pid = blockIdx.x;
-  if (n_ground[pid] + n_nonground[pid] == 0) return;
-  const int s0 = start[pid], m = start[pid + 1] - s0;
+// The caller's device arrays of a wave (ground, non-ground, valid, outlier): scan s's entries start at s * cap, entries at or past cap
+// are not written; nullptr = not asked for.  The kernels write them next to the lane's scratch copy.
+struct PpDev {
+  float4* arr[4];
+  long long cap;
+};
+
+// one CTA per (patch, scan): scan s's outputs go to out[s * R ...]: ground at [0, n_ground), non-ground at [n_ground, n_ground + n_nonground)
+__global__ void __launch_bounds__(256) pw_gather_kernel(const float4* const* __restrict__ pts_of, int R, const int* __restrict__ start,
+                                                        const int* __restrict__ n_ground, const int* __restrict__ n_nonground,
+                                                        const unsigned long long* __restrict__ items, const int* __restrict__ rank,
+                                                        const int* __restrict__ goff, const int* __restrict__ ngoff, const int* __restrict__ cnt,
+                                                        float4* __restrict__ out, PpDev dst) {
+  const int pid = blockIdx.x, scan = blockIdx.y;
+  const size_t po = (size_t)scan * kPwStride + pid, ro = (size_t)scan * R;
+  if (n_ground[po] + n_nonground[po] == 0) return;
+  const float4* __restrict__ pts = pts_of[scan];
+  const int s0 = start[po], m = start[po + 1] - s0;
+  const int g0 = goff[po], n0 = cnt[(size_t)scan * kPpCnt] + ngoff[po];   // non-ground part of out follows the ground part
+  const int nn0 = ngoff[po];
   for (int p = threadIdx.x; p < m; p += blockDim.x) {
-    const int code = rank[s0 + p];
-    const float4 q = pts[(unsigned)items[s0 + p]];
-    if (code & (1 << 30)) ground[goff[pid] + (code & ~(1 << 30))] = q;
-    else nonground[ngoff[pid] + code] = q;
+    const int code = rank[ro + s0 + p];
+    const float4 q = pts[(unsigned)items[ro + s0 + p]];
+    if (code & (1 << 30)) {
+      const int pos = g0 + (code & ~(1 << 30));
+      out[ro + pos] = q;
+      if (dst.arr[0] && pos < dst.cap) dst.arr[0][scan * dst.cap + pos] = q;
+    } else {
+      out[ro + n0 + code] = q;
+      const int pos = nn0 + code;
+      if (dst.arr[1] && pos < dst.cap) dst.arr[1][scan * dst.cap + pos] = q;
+    }
   }
 }
-
-// allocated on the first call of a lane: both buffers or neither
-static int ensure_pw_scratch(Lane* h) {
-  if (h->pw_ints) return QB200_OK;
-  const size_t R = h->R;
-  DeviceMem<int> ints;
-  DeviceMem<float4> out;
-  // ints: patch_of [R] | rank [R] | count, start(+1), cursor, n_ground, n_nonground, goff, ngoff [each 4096+1] | out_n [2] | status [1]
-  QB_CUDA_TRY(h, ints.alloc(2 * R + 7 * (kPwMaxPatches + 1) + 4));
-  QB_CUDA_TRY(h, out.alloc(2 * R));
-  h->pw_ints = std::move(ints);
-  h->pw_out = std::move(out);
-  return QB200_OK;
-}
-
-// pts: n points on the device.  Leaves the two outputs in h->pw_out ([0, R) ground, [R, 2R) non-ground) and returns their sizes.
-int launch_patchwork(Lane* h, const float4* pts, int n, const qb200_patchwork_params& pp, int* n_ground, int* n_nonground, int* status) {
-  *n_ground = *n_nonground = 0;
-  *status = QB200_OK;
-  if (!pw_params_valid(pp)) return QB200_ERR_BAD_ARG;
-  if (n <= 0) return QB200_OK;
-  if (int rc = ensure_pw_scratch(h)) return rc;
-  PwDev c;
-  c.p = pp;
-  c.patch_base[0] = 0;
-  for (int k = 0; k < 4; ++k) c.patch_base[k + 1] = c.patch_base[k] + pp.num_sectors_each_zone[k] * pp.num_rings_each_zone[k];
-  c.n_patches = c.patch_base[4];
-  const int NP = c.n_patches;
-  const size_t R = h->R;
-  int* patch_of = h->pw_ints;
-  int* rank = patch_of + R;
-  int* count = rank + R;
-  int* start = count + (kPwMaxPatches + 1);
-  int* cursor = start + (kPwMaxPatches + 1);
-  int* ng_ground = cursor + (kPwMaxPatches + 1);
-  int* ng_non = ng_ground + (kPwMaxPatches + 1);
-  int* goff = ng_non + (kPwMaxPatches + 1);
-  int* ngoff = goff + (kPwMaxPatches + 1);
-  int* out_n = ngoff + (kPwMaxPatches + 1);   // [0] ground, [1] non-ground, [2] status
-  unsigned long long* items = reinterpret_cast<unsigned long long*>(h->key_a.get());   // [>= R]
-  QB_CUDA_TRY(h, cudaMemsetAsync(count, 0, (kPwMaxPatches + 1) * sizeof(int), h->stream));
-  QB_CUDA_TRY(h, cudaMemsetAsync(out_n, 0, 4 * sizeof(int), h->stream));
-  const int nb = (n + 255) / 256;
-  pw_bin_kernel<<<nb, 256, 0, h->stream>>>(pts, n, c, patch_of, count);
-  pw_scan_kernel<<<1, 1024, 0, h->stream>>>(count, NP, start, cursor);
-  pw_scatter_kernel<<<nb, 256, 0, h->stream>>>(pts, n, patch_of, cursor, items);
-  const size_t smem = (size_t)kPwMaxPatchPts * 9;
-  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)pw_patch_kernel, smem));
-  pw_patch_kernel<<<NP, kPwThreads, smem, h->stream>>>(pts, c, start, items, kPwMaxPatchPts, ng_ground, ng_non, rank, out_n + 2);
-  pw_offsets_kernel<<<1, 1024, 0, h->stream>>>(ng_ground, ng_non, NP, goff, ngoff, out_n);
-  pw_gather_kernel<<<NP, 256, 0, h->stream>>>(pts, start, ng_ground, ng_non, items, rank, goff, ngoff, h->pw_out, h->pw_out + R);
-  h->launches += 6;
-  QB_CUDA_TRY(h, cudaGetLastError());
-  int host_n[3];
-  QB_CUDA_TRY(h, cudaMemcpyAsync(host_n, out_n, 3 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  *n_ground = host_n[0];
-  *n_nonground = host_n[1];
-  *status = host_n[2];
-  return QB200_OK;
-}
-
 
 // ------------------------------------------------------------------------------------------------
 // Range-image sub-cluster removal: ImageProjection::segmentCloud in "Patchwork" mode (include/imageProjection.hpp:273-294).
@@ -433,31 +405,54 @@ __device__ __forceinline__ bool ip_project(const float4 pt, const qb200_segment_
   return true;
 }
 
-__global__ void __launch_bounds__(256) ip_project_kernel(const float4* __restrict__ pts, int n, IpDev c, int* __restrict__ winner) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+// Scan s of a wave: the cloud tables of stage_raw (ptr[s], n[s]), or the non-ground part of the patchwork output (base != nullptr:
+// base + s * R from cnt[s][0] on, cnt[s][1] points).
+struct IpIn {
+  const float4* const* ptr;
+  const int* n;
+  const float4* base;
+  const int* cnt;
+  int R;
+};
+
+__device__ __forceinline__ const float4* ip_input(const IpIn& in, int s, int* n) {
+  if (in.base) {
+    *n = in.cnt[(size_t)s * kPpCnt + 1];
+    return in.base + (size_t)s * in.R + in.cnt[(size_t)s * kPpCnt];
+  }
+  *n = in.n[s];
+  return in.ptr[s];
+}
+
+// blockIdx.y = scan; every per-pixel array holds npix entries per scan
+__global__ void __launch_bounds__(256) ip_project_kernel(IpIn in, IpDev c, int* __restrict__ winner) {
+  const int s = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  int n;
+  const float4* pts = ip_input(in, s, &n);
   if (i >= n) return;
   const float4 p = pts[i];
   if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z))) return;   // copyPointCloud, :260-266
   int r, col; float rg;
   if (!ip_project(p, c.p, &r, &col, &rg)) return;
-  atomicMax(&winner[r * c.p.horizon_scan + col], i);
+  atomicMax(&winner[(size_t)s * c.p.n_scan * c.p.horizon_scan + r * c.p.horizon_scan + col], i);
 }
 
-__global__ void __launch_bounds__(256) ip_range_kernel(const float4* __restrict__ pts, int npix, const int* __restrict__ winner,
-                                                       float* __restrict__ range, int* __restrict__ parent, int* __restrict__ size,
-                                                       unsigned long long* __restrict__ rows) {
-  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void __launch_bounds__(256) ip_range_kernel(IpIn in, int npix, const int* __restrict__ winner, float* __restrict__ range,
+                                                       int* __restrict__ parent, int* __restrict__ size, unsigned long long* __restrict__ rows) {
+  const int s = blockIdx.y, q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= npix) return;
-  const int w = winner[q];
+  const size_t o = (size_t)s * npix + q;
+  const int w = winner[o];
   float rg = FLT_MAX;
   if (w >= 0) {
-    const float4 p = pts[w];
+    int n;
+    const float4 p = ip_input(in, s, &n)[w];
     rg = sqrtf(p.x * p.x + p.y * p.y + p.z * p.z);
   }
-  range[q] = rg;
-  parent[q] = w >= 0 ? q : -1;
-  size[q] = 0;
-  rows[q] = 0ull;
+  range[o] = rg;
+  parent[o] = w >= 0 ? q : -1;
+  size[o] = 0;
+  rows[o] = 0ull;
 }
 
 __device__ __forceinline__ int ip_find(const int* parent, int a) {
@@ -471,6 +466,8 @@ __device__ __forceinline__ int ip_find(const int* parent, int a) {
 __global__ void __launch_bounds__(256) ip_union_kernel(int npix, IpDev c, const float* __restrict__ range, int* parent) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= npix) return;
+  range += (size_t)blockIdx.y * npix;
+  parent += (size_t)blockIdx.y * npix;
   const float ra = range[q];
   if (ra == FLT_MAX) return;
   const int H = c.p.n_scan, Wd = c.p.horizon_scan;
@@ -505,6 +502,8 @@ __global__ void __launch_bounds__(256) ip_union_kernel(int npix, IpDev c, const 
 __global__ void __launch_bounds__(256) ip_stats_kernel(int npix, int Wd, int* parent, int* __restrict__ size, unsigned long long* __restrict__ rows) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= npix) return;
+  const size_t o = (size_t)blockIdx.y * npix;
+  parent += o; size += o; rows += o;
   if (((volatile int*)parent)[q] < 0) return;
   const int root = ip_find(parent, q);
   atomicAdd(&size[root], 1);
@@ -512,13 +511,16 @@ __global__ void __launch_bounds__(256) ip_stats_kernel(int npix, int Wd, int* pa
 }
 
 // feasibility of every occupied pixel's segment (:559-571) -> kind[] (0 empty, 1 valid segment, 2 outlier) and the two counts of
-// every block of 1024 pixels
+// every block of 1024 pixels (blk_cnt: 2 * gridDim.x entries per scan)
 __global__ void __launch_bounds__(1024) ip_kind_kernel(int npix, IpDev c, const int* __restrict__ winner, const int* parent, const int* __restrict__ size,
                                                        const unsigned long long* __restrict__ rows, unsigned char* __restrict__ kind_out,
                                                        int* __restrict__ blk_cnt) {
   __shared__ int s_v, s_o;
   if (threadIdx.x == 0) { s_v = 0; s_o = 0; }
   __syncthreads();
+  const size_t o = (size_t)blockIdx.y * npix;
+  winner += o; parent += o; size += o; rows += o; kind_out += o;
+  blk_cnt += (size_t)blockIdx.y * 2 * gridDim.x;
   const int q = blockIdx.x * 1024 + threadIdx.x;
   int kind = 0;
   if (q < npix && winner[q] >= 0) {
@@ -538,42 +540,47 @@ __global__ void __launch_bounds__(1024) ip_kind_kernel(int npix, IpDev c, const 
   if (threadIdx.x == 0) { blk_cnt[2 * blockIdx.x] = s_v; blk_cnt[2 * blockIdx.x + 1] = s_o; }
 }
 
-// ordered extraction (row-major, :424-481): block base = counts of the preceding blocks, one block scan inside
-__global__ void __launch_bounds__(1024) ip_extract_kernel(const float4* __restrict__ pts, int npix, const int* __restrict__ winner,
+// ordered extraction (row-major, :424-481): block base = counts of the preceding blocks, one block scan inside.  Scan s's outputs go
+// to out[s * npix ...]: valid segments at [0, n_valid), outliers at [n_valid, n_valid + n_outlier); counts -> cnt[s][3], cnt[s][4].
+__global__ void __launch_bounds__(1024) ip_extract_kernel(IpIn in, int npix, const int* __restrict__ winner,
                                                           const unsigned char* __restrict__ kind_in, const int* __restrict__ blk_cnt,
-                                                          float4* __restrict__ valid, float4* __restrict__ outlier, int* __restrict__ out_n) {
+                                                          float4* __restrict__ out, int* __restrict__ cnt, PpDev dst) {
   __shared__ int sm[33];
-  __shared__ int s_base[2];
-  int bv = 0, bo = 0;
-  for (int b = threadIdx.x; b < (int)blockIdx.x; b += 1024) { bv += blk_cnt[2 * b]; bo += blk_cnt[2 * b + 1]; }
+  __shared__ int s_base[3];
+  const int scan = blockIdx.y;
+  const size_t o = (size_t)scan * npix;
+  winner += o; kind_in += o; out += o;
+  blk_cnt += (size_t)scan * 2 * gridDim.x;
+  int bv = 0, bo = 0, tv = 0;
+  for (int b = threadIdx.x; b < (int)gridDim.x; b += 1024) {
+    if (b < (int)blockIdx.x) { bv += blk_cnt[2 * b]; bo += blk_cnt[2 * b + 1]; }
+    tv += blk_cnt[2 * b];
+  }
   int tot;
   block_excl_scan(bv, sm, &tot);
   if (threadIdx.x == 0) s_base[0] = tot;
   block_excl_scan(bo, sm, &tot);
   if (threadIdx.x == 0) s_base[1] = tot;
+  block_excl_scan(tv, sm, &tot);
+  if (threadIdx.x == 0) s_base[2] = tot;
   __syncthreads();
   const int q = blockIdx.x * 1024 + threadIdx.x;
   const int kind = q < npix ? (int)kind_in[q] : 0;
   int both;
   const int ex = block_excl_scan((kind == 1 ? 1 : 0) | ((kind == 2 ? 1 : 0) << 16), sm, &both);
   if (kind) {
-    float4 p = pts[winner[q]];
+    int n;
+    float4 p = ip_input(in, scan, &n)[winner[q]];
     p.w = 1.0f;
-    if (kind == 1) valid[s_base[0] + (ex & 0xFFFF)] = p;
-    else outlier[s_base[1] + (ex >> 16)] = p;
+    const int pos = kind == 1 ? s_base[0] + (ex & 0xFFFF) : s_base[1] + (ex >> 16);
+    out[kind == 1 ? pos : s_base[2] + pos] = p;
+    float4* d = kind == 1 ? dst.arr[2] : dst.arr[3];
+    if (d && pos < dst.cap) d[scan * dst.cap + pos] = p;
   }
-  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) { out_n[0] = s_base[0] + (both & 0xFFFF); out_n[1] = s_base[1] + (both >> 16); }
-}
-
-// grown to the largest image of the lane so far; a failed call keeps the old buffer
-static int ensure_ip_scratch(Lane* h, int npix) {
-  if (h->ip_buf && h->ip_npix >= npix) return QB200_OK;
-  DeviceMem<void> buf;
-  // per pixel: rows u64 | valid float4 | outlier float4 | winner, parent, size int | range float | kind u8 ; + out_n [2] + block counts
-  QB_CUDA_TRY(h, buf.alloc_bytes((size_t)npix * (8 + 16 + 16 + 4 * 4 + 1) + 16 + 8 * (size_t)((npix + 1023) / 1024) + 64));
-  h->ip_buf = std::move(buf);
-  h->ip_npix = npix;
-  return QB200_OK;
+  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
+    cnt[(size_t)scan * kPpCnt + 3] = s_base[0] + (both & 0xFFFF);
+    cnt[(size_t)scan * kPpCnt + 4] = s_base[1] + (both >> 16);
+  }
 }
 
 static bool ip_params_valid(const qb200_segment_params& sp) {
@@ -582,25 +589,99 @@ static bool ip_params_valid(const qb200_segment_params& sp) {
          sp.segment_valid_line_num >= 0;
 }
 
-// pts: n device points.  Leaves the outputs in the handle's scratch; *valid_dev / *outlier_dev point at them.
-int launch_segment_cloud(Lane* h, const float4* pts, int n, const qb200_segment_params& sp, int* n_valid, int* n_outlier,
-                         const float4** valid_dev, const float4** outlier_dev) {
-  *n_valid = *n_outlier = 0;
-  if (!ip_params_valid(sp)) return QB200_ERR_BAD_ARG;
-  const int npix = sp.n_scan * sp.horizon_scan;
-  if (int rc = ensure_ip_scratch(h, npix)) return rc;
-  unsigned char* b = reinterpret_cast<unsigned char*>(h->ip_buf.get());
-  float4* valid = reinterpret_cast<float4*>(b); b += (size_t)npix * 16;      // 16-byte records first: aligned for any image size
-  float4* outlier = reinterpret_cast<float4*>(b); b += (size_t)npix * 16;
-  unsigned long long* rows = reinterpret_cast<unsigned long long*>(b); b += (size_t)npix * 8;
-  int* winner = reinterpret_cast<int*>(b); b += (size_t)npix * 4;
-  int* parent = reinterpret_cast<int*>(b); b += (size_t)npix * 4;
-  int* size = reinterpret_cast<int*>(b); b += (size_t)npix * 4;
-  float* range = reinterpret_cast<float*>(b); b += (size_t)npix * 4;
-  int* out_n = reinterpret_cast<int*>(b); b += 16;
-  int* blk_cnt = reinterpret_cast<int*>(b); b += 8 * (size_t)((npix + 1023) / 1024);
+// ------------------------------------------------------------------------------------------------
+// Waves.  One launch sequence serves up to 2S scans; the three entry points below run their scans through it on lane 0.
+// ------------------------------------------------------------------------------------------------
+// range-image scratch of ns scans of npix pixels: per pixel the output (float4), the row set (u64), winner, parent, size (int), range
+// (float), kind (u8); per scan the counts of every block of 1024 pixels
+static size_t ip_bytes(int npix, int ns) {
+  return (size_t)ns * ((size_t)npix * (16 + 8 + 4 * 4 + 1) + 8 * (size_t)((npix + 1023) / 1024)) + 64;
+}
+
+// Scratch of a wave of ns scans, grown on demand (a lane that never pre-processes holds none).  Each group -- the count block and
+// its pinned mirror, the patchwork buffers, the range-image buffer -- is allocated whole or not at all: a failed call leaves a group
+// either as it was or empty, and the next call allocates it again.
+static int ensure_pp_scratch(Lane* L, int ns, bool pw, int npix) {
+  const int C = 2 * L->S;
+  const bool grow_pw = pw && ns > L->pw_scans, grow_ip = npix > 0 && ip_bytes(npix, ns) > L->ip_cap;
+  DeviceMem<int> cnt, ints;
+  PinnedMem<int> hcnt;
+  DeviceMem<float4> out;
+  DeviceMem<void> ip;
+  if (!L->pp_cnt) {
+    QB_CUDA_TRY(L, cnt.alloc((size_t)C * kPpCnt));
+    QB_CUDA_TRY(L, hcnt.alloc((size_t)C * kPpCnt));
+  }
+  if (grow_pw) {
+    // the old buffers are idle (every wave ends in a sync): they go first, so the device never holds both
+    L->pw_ints.reset(); L->pw_out.reset();
+    L->pw_scans = 0;
+    // patch_of [ns*R] | rank [ns*R] | count, start(+1), cursor, n_ground, n_nonground, goff, ngoff [ns*kPwStride each]
+    QB_CUDA_TRY(L, ints.alloc((size_t)ns * (2 * (size_t)L->R + 7 * (size_t)kPwStride)));
+    QB_CUDA_TRY(L, out.alloc((size_t)ns * L->R));
+  }
+  if (grow_ip) {
+    L->ip_buf.reset();
+    L->ip_cap = 0;
+    QB_CUDA_TRY(L, ip.alloc_bytes(ip_bytes(npix, ns)));
+  }
+  if (!L->pp_cnt) { L->pp_cnt = std::move(cnt); L->pp_hcnt = std::move(hcnt); }
+  if (grow_pw) { L->pw_ints = std::move(ints); L->pw_out = std::move(out); L->pw_scans = ns; }
+  if (grow_ip) { L->ip_buf = std::move(ip); L->ip_cap = ip_bytes(npix, ns); }
+  return QB200_OK;
+}
+
+// Enqueue ground removal of the wave's scans [0, ns) (cloud tables of stage_raw); scan s's outputs -> pw_out + s * R, its counts and
+// status -> pp_cnt[s].  Launches do not depend on ns or on the scans' sizes.
+static int launch_patchwork_wave(Lane* L, int ns, int max_n, const qb200_patchwork_params& pp, const PpDev& dst) {
+  PwDev c;
+  c.p = pp;
+  c.patch_base[0] = 0;
+  for (int k = 0; k < 4; ++k) c.patch_base[k + 1] = c.patch_base[k] + pp.num_sectors_each_zone[k] * pp.num_rings_each_zone[k];
+  c.n_patches = c.patch_base[4];
+  const int NP = c.n_patches, R = L->R;
+  const size_t P = (size_t)L->pw_scans * kPwStride;
+  int* patch_of = L->pw_ints;
+  int* rank = patch_of + (size_t)L->pw_scans * R;
+  int* count = rank + (size_t)L->pw_scans * R;
+  int* start = count + P;
+  int* cursor = start + P;
+  int* ng_ground = cursor + P;
+  int* ng_non = ng_ground + P;
+  int* goff = ng_non + P;
+  int* ngoff = goff + P;
+  unsigned long long* items = reinterpret_cast<unsigned long long*>(L->key_a.get());   // [2S * R] >= [ns * R]
+  QB_CUDA_TRY(L, cudaMemsetAsync(count, 0, (size_t)ns * kPwStride * sizeof(int), L->stream));
+  const dim3 gp((max_n + 255) / 256 > 0 ? (max_n + 255) / 256 : 1, ns);
+  pw_bin_kernel<<<gp, 256, 0, L->stream>>>(L->d_cloud_ptr, L->d_cloud_n, c, R, patch_of, count);
+  pw_scan_kernel<<<ns, 1024, 0, L->stream>>>(count, NP, start, cursor);
+  pw_scatter_kernel<<<gp, 256, 0, L->stream>>>(L->d_cloud_ptr, L->d_cloud_n, R, patch_of, cursor, items);
+  const size_t smem = (size_t)kPwMaxPatchPts * 9;
+  QB_CUDA_TRY(L, ensure_dyn_smem(L->device, (const void*)pw_patch_kernel, smem));
+  pw_patch_kernel<<<dim3(NP, ns), kPwThreads, smem, L->stream>>>(L->d_cloud_ptr, c, R, start, items, kPwMaxPatchPts, ng_ground, ng_non, rank,
+                                                                 L->pp_cnt);
+  pw_offsets_kernel<<<ns, 1024, 0, L->stream>>>(ng_ground, ng_non, NP, goff, ngoff, L->pp_cnt);
+  pw_gather_kernel<<<dim3(NP, ns), 256, 0, L->stream>>>(L->d_cloud_ptr, R, start, ng_ground, ng_non, items, rank, goff, ngoff, L->pp_cnt,
+                                                        L->pw_out, dst);
+  L->launches += 6;
+  QB_CUDA_TRY(L, cudaGetLastError());
+  return QB200_OK;
+}
+
+// Enqueue sub-cluster removal of the wave's scans [0, ns) read through `in`; scan s's outputs -> the range-image scratch + s * npix,
+// its counts -> pp_cnt[s].  max_n bounds every scan's point count.
+static int launch_segment_wave(Lane* L, int ns, int max_n, const IpIn& in, const qb200_segment_params& sp, const PpDev& dst) {
+  const int npix = sp.n_scan * sp.horizon_scan, nblk = (npix + 1023) / 1024;
+  const size_t NPX = (size_t)ns * npix;
+  unsigned char* b = reinterpret_cast<unsigned char*>(L->ip_buf.get());
+  float4* out = reinterpret_cast<float4*>(b); b += NPX * 16;      // 16-byte records first: aligned for any image size
+  unsigned long long* rows = reinterpret_cast<unsigned long long*>(b); b += NPX * 8;
+  int* winner = reinterpret_cast<int*>(b); b += NPX * 4;
+  int* parent = reinterpret_cast<int*>(b); b += NPX * 4;
+  int* size = reinterpret_cast<int*>(b); b += NPX * 4;
+  float* range = reinterpret_cast<float*>(b); b += NPX * 4;
+  int* blk_cnt = reinterpret_cast<int*>(b); b += 8 * (size_t)ns * nblk;
   unsigned char* kind = b;
-  *valid_dev = valid; *outlier_dev = outlier;
   IpDev c;
   c.p = sp;
   // segmentAlphaX / segmentAlphaY and their sine / cosine (:132-133, :535-541): constants of the call, evaluated on the host
@@ -615,26 +696,163 @@ int launch_segment_cloud(Lane* h, const float4* pts, int n, const qb200_segment_
     const int(*src)[2] = sp.neighbor_mode == QB200_NEIGHBORS_4 ? n4 : (sp.neighbor_mode == QB200_NEIGHBORS_8 ? n8 : nx);
     c.nb[i][0] = src[i][0]; c.nb[i][1] = src[i][1];
   }
-  QB_CUDA_TRY(h, cudaMemsetAsync(winner, 0xFF, (size_t)npix * sizeof(int), h->stream));   // -1
-  const int gp = (npix + 255) / 256;
-  if (n > 0) ip_project_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(pts, n, c, winner);
-  ip_range_kernel<<<gp, 256, 0, h->stream>>>(pts, npix, winner, range, parent, size, rows);
-  ip_union_kernel<<<gp, 256, 0, h->stream>>>(npix, c, range, parent);
-  ip_stats_kernel<<<gp, 256, 0, h->stream>>>(npix, sp.horizon_scan, parent, size, rows);
-  const int nblk = (npix + 1023) / 1024;
-  ip_kind_kernel<<<nblk, 1024, 0, h->stream>>>(npix, c, winner, parent, size, rows, kind, blk_cnt);
-  ip_extract_kernel<<<nblk, 1024, 0, h->stream>>>(pts, npix, winner, kind, blk_cnt, valid, outlier, out_n);
-  h->launches += 6;
-  QB_CUDA_TRY(h, cudaGetLastError());
-  int host_n[2];
-  QB_CUDA_TRY(h, cudaMemcpyAsync(host_n, out_n, 2 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  QB_CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  *n_valid = host_n[0];
-  *n_outlier = host_n[1];
+  QB_CUDA_TRY(L, cudaMemsetAsync(winner, 0xFF, NPX * sizeof(int), L->stream));   // -1
+  const dim3 gpt((max_n + 255) / 256 > 0 ? (max_n + 255) / 256 : 1, ns), gpx((npix + 255) / 256, ns), gbk(nblk, ns);
+  ip_project_kernel<<<gpt, 256, 0, L->stream>>>(in, c, winner);
+  ip_range_kernel<<<gpx, 256, 0, L->stream>>>(in, npix, winner, range, parent, size, rows);
+  ip_union_kernel<<<gpx, 256, 0, L->stream>>>(npix, c, range, parent);
+  ip_stats_kernel<<<gpx, 256, 0, L->stream>>>(npix, sp.horizon_scan, parent, size, rows);
+  ip_kind_kernel<<<gbk, 1024, 0, L->stream>>>(npix, c, winner, parent, size, rows, kind, blk_cnt);
+  ip_extract_kernel<<<gbk, 1024, 0, L->stream>>>(in, npix, winner, kind, blk_cnt, out, L->pp_cnt, dst);
+  L->launches += 6;
+  QB_CUDA_TRY(L, cudaGetLastError());
   return QB200_OK;
 }
 
+// The caller's arrays of a whole call.  Host arrays are filled from the scratch after the counts are back, device arrays by the kernels.
+struct PpOut {
+  float4* arr[4];   // ground, non-ground, valid, outlier (nullptr: not asked for)
+  long long cap;
+  int device;
+};
+
+// One wave on lane L: scans [0, ns) whose pointers and sizes are in L->h_cloud_ptr / h_cloud_n (`kind` memory) through ground
+// removal (pp) and then sub-cluster removal of its non-ground output (sp), or through sub-cluster removal alone (pp == nullptr).
+// Scan s of the wave is scan first + s of `out`; its counts go to counts[s * 4 ...] (ground, non-ground, valid, outlier), its
+// patchwork status to status[s].  The counts of the wave come back in one copy.
+static int preprocess_wave(Lane* L, int ns, qb200_mem_kind kind, const qb200_patchwork_params* pp, const qb200_segment_params* sp,
+                           const PpOut& out, long long first, int32_t* counts, int32_t* status) {
+  int rc, max_n = 0;
+  for (int s = 0; s < ns; ++s) max_n = L->h_cloud_n[s] > max_n ? L->h_cloud_n[s] : max_n;
+  const int npix = sp ? sp->n_scan * sp->horizon_scan : 0;
+  if ((rc = ensure_pp_scratch(L, ns, pp != nullptr, npix))) return rc;
+  if ((rc = stage_raw(L, ns, kind, L->stream))) return rc;
+  QB_CUDA_TRY(L, cudaMemsetAsync(L->pp_cnt, 0, (size_t)ns * kPpCnt * sizeof(int), L->stream));
+  PpDev dst = {{nullptr, nullptr, nullptr, nullptr}, out.cap};
+  if (out.device)
+    for (int k = 0; k < 4; ++k) dst.arr[k] = out.arr[k] ? out.arr[k] + first * out.cap : nullptr;
+  if (pp && (rc = launch_patchwork_wave(L, ns, max_n, *pp, dst))) return rc;
+  if (sp) {
+    IpIn in = {L->d_cloud_ptr, L->d_cloud_n, pp ? L->pw_out.get() : nullptr, L->pp_cnt, L->R};
+    if ((rc = launch_segment_wave(L, ns, max_n, in, *sp, dst))) return rc;
+  }
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->pp_hcnt, L->pp_cnt, (size_t)ns * kPpCnt * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
+  QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
+  bool copied = false;
+  for (int s = 0; s < ns; ++s) {
+    const int* hc = L->pp_hcnt + (size_t)s * kPpCnt;
+    const int c4[4] = {hc[0], hc[1], hc[3], hc[4]};
+    for (int k = 0; k < 4; ++k) counts[4 * s + k] = c4[k];
+    status[s] = hc[2];
+    if (out.device) continue;
+    for (int k = 0; k < 4; ++k) {
+      const long long m = c4[k] < out.cap ? c4[k] : out.cap;
+      if (!out.arr[k] || m <= 0) continue;
+      // scratch of scan s: ground | non-ground at pw_out + s * R, valid | outlier at the range-image outputs + s * npix
+      const float4* src = k < 2 ? L->pw_out + (size_t)s * L->R + (k == 1 ? hc[0] : 0)
+                                : reinterpret_cast<const float4*>(L->ip_buf.get()) + (size_t)s * npix + (k == 3 ? hc[3] : 0);
+      QB_CUDA_TRY(L, cudaMemcpyAsync(out.arr[k] + (first + s) * out.cap, src, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
+      copied = true;
+    }
+  }
+  if (copied) QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
+  return QB200_OK;
+}
+
+// a caller's device output array: memory of the handle's device, 16-byte aligned (nullptr passes)
+static bool device_array_ok(const qb200_handle* h, const void* a) {
+  if (!a) return true;
+  cudaPointerAttributes at;
+  if ((uintptr_t)a & 15) return false;
+  if (cudaPointerGetAttributes(&at, a) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return at.device == h->cfg.device && (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged);
+}
+
 }  // namespace qb
+
+using namespace qb;
+
+extern "C" {
+
+// ---- pre-processing: ground removal (patchwork.hpp:329-455), a wave of one ----------------------------
+int qb200_patchwork(qb200_handle* h, const float* pts4, int32_t n, const qb200_patchwork_params* p, float* ground4, int32_t* n_ground,
+                    float* nonground4, int32_t* n_nonground) {
+  if (int rc = enter(h)) return rc;
+  if (!p || !n_ground || !n_nonground || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
+  *n_ground = *n_nonground = 0;
+  Lane* L = h->lane[0].get();
+  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
+  if (!pw_params_valid(*p)) return QB200_ERR_BAD_ARG;
+  L->h_cloud_ptr[0] = reinterpret_cast<const float4*>(pts4);
+  L->h_cloud_n[0] = n;
+  const PpOut out = {{reinterpret_cast<float4*>(ground4), reinterpret_cast<float4*>(nonground4), nullptr, nullptr}, n, 0};
+  int32_t counts[4], status = QB200_OK;
+  if (int rc = preprocess_wave(L, 1, QB200_MEM_HOST, p, nullptr, out, 0, counts, &status)) return rc;
+  *n_ground = counts[0];
+  *n_nonground = counts[1];
+  return status;
+}
+
+// ---- pre-processing: range-image sub-cluster removal (imageProjection.hpp:273-294), a wave of one ------------
+int qb200_segment_cloud(qb200_handle* h, const float* pts4, int32_t n, const qb200_segment_params* p, float* valid4, int32_t* n_valid,
+                        float* outlier4, int32_t* n_outlier) {
+  if (int rc = enter(h)) return rc;
+  if (!p || !n_valid || !n_outlier || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
+  *n_valid = *n_outlier = 0;
+  Lane* L = h->lane[0].get();
+  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
+  if (!ip_params_valid(*p)) return QB200_ERR_BAD_ARG;
+  L->h_cloud_ptr[0] = reinterpret_cast<const float4*>(pts4);
+  L->h_cloud_n[0] = n;
+  const PpOut out = {{nullptr, nullptr, reinterpret_cast<float4*>(valid4), reinterpret_cast<float4*>(outlier4)}, (long long)p->n_scan * p->horizon_scan, 0};
+  int32_t counts[4], status = QB200_OK;
+  if (int rc = preprocess_wave(L, 1, QB200_MEM_HOST, nullptr, p, out, 0, counts, &status)) return rc;
+  *n_valid = counts[2];
+  *n_outlier = counts[3];
+  return QB200_OK;
+}
+
+// ---- pre-processing of many scans: ground removal, then sub-cluster removal, in waves of 2S scans ----------
+int qb200_preprocess_batch(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans, qb200_mem_kind kind,
+                           const qb200_patchwork_params* pp, const qb200_segment_params* sp, const qb200_preprocess_out* out) {
+  if (int rc = enter(h)) return rc;
+  const char* why = nullptr;
+  if (n_scans < 0 || (n_scans > 0 && (!scans4 || !n_points))) why = "n_scans < 0, or no scan / size table";
+  else if (kind != QB200_MEM_HOST && kind != QB200_MEM_DEVICE) why = "unknown memory kind of the scans";
+  else if (!pp || !pw_params_valid(*pp)) why = "invalid patchwork parameters";
+  else if (sp && !ip_params_valid(*sp)) why = "invalid segment parameters";
+  else if (!out || !out->counts || !out->status) why = "no output descriptor, counts or status";
+  else if (out->cap_per_scan < 1) why = "cap_per_scan < 1";
+  else if (out->kind != QB200_MEM_HOST && out->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the outputs";
+  else if (out->kind == QB200_MEM_DEVICE && !(device_array_ok(h, out->ground4) && device_array_ok(h, out->nonground4) &&
+                                              device_array_ok(h, out->valid4) && device_array_ok(h, out->outlier4)))
+    why = "device output array is misaligned or not memory of the handle's device";
+  Lane* L = h->lane[0].get();
+  for (int i = 0; i < n_scans && !why; ++i)
+    if (n_points[i] < 0 || n_points[i] > L->R || (n_points[i] > 0 && !scans4[i])) why = "scan is null or exceeds max_raw_points";
+  if (why) {
+    h->fail(__FILE__, __LINE__, why);
+    return QB200_ERR_BAD_ARG;
+  }
+  const PpOut o = {{reinterpret_cast<float4*>(out->ground4), reinterpret_cast<float4*>(out->nonground4), reinterpret_cast<float4*>(out->valid4),
+                    reinterpret_cast<float4*>(out->outlier4)},
+                   out->cap_per_scan, out->kind == QB200_MEM_DEVICE ? 1 : 0};
+  const int C = 2 * L->S;
+  for (int w0 = 0; w0 < n_scans; w0 += C) {
+    const int ns = n_scans - w0 < C ? n_scans - w0 : C;
+    for (int s = 0; s < ns; ++s) {
+      L->h_cloud_ptr[s] = reinterpret_cast<const float4*>(scans4[w0 + s]);
+      L->h_cloud_n[s] = n_points[w0 + s];
+    }
+    if (int rc = preprocess_wave(L, ns, kind, pp, sp, o, w0, out->counts + 4 * (size_t)w0, out->status + w0)) return rc;
+  }
+  return QB200_OK;
+}
+
+}  // extern "C"
 
 extern "C" void qb200_default_patchwork_params(qb200_patchwork_params* p) {  // config/patchwork_params.yaml:1-48
   if (!p) return;
