@@ -157,6 +157,9 @@ void qb200_default_params(qb200_params* p);
 void qb200_default_config(qb200_config* c);
 int qb200_version(void);
 
+/* Every QB200_* environment switch (QB200_LANES, QB200_MATCH_EXACT, QB200_TC_VERIFY, QB200_TC_PROF, QB200_TIMELINE) is read here,
+ * when the handle is created: a switch applies to the handles created while it is set, and changing the environment later does
+ * not affect an existing handle. */
 int qb200_create(const qb200_config* cfg, qb200_handle** out);
 void qb200_destroy(qb200_handle* h);
 /* Run on a caller-owned CUDA stream (cudaStream_t as void*); NULL restores the handle's own stream. */
@@ -460,13 +463,13 @@ int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset);
  * point j, ~0 = none.  min(cap_rows, n_src) and min(cap_cols, n_tgt) entries are written (either pointer may be NULL); the
  * tables are those the mutual check read, after any stripe was redone by the exact kernel.  Synchronises the handle's stream. */
 int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, uint64_t* colbest, int32_t cap_cols);
-/* QB200_TC_PROF=1 only: per-role clock64 accounting of tc_nn_kernel (24 counters, see tools/tc_profile.py) */
+/* Handles created with QB200_TC_PROF=1 only: per-role clock64 accounting of tc_nn_kernel (24 counters, see tools/tc_profile.py) */
 int qb200_debug_tc_profile(qb200_handle* h, uint64_t* out24, int32_t reset);
 /* Diagnostics: footprint of the tensor-core nearest-neighbour kernel as launched: out5[0] = threads per CTA,
  * [1] = dynamic shared bytes, [2] = static shared bytes, [3] = registers per thread, [4] = resident CTAs per SM. */
 int qb200_debug_tc_footprint(qb200_handle* h, int32_t* out5);
 
-/* Diagnostics: with QB200_TC_VERIFY=1 in the environment every batch is matched by the tensor-core path AND by the exact CUDA-core
+/* Diagnostics: on a handle created with QB200_TC_VERIFY=1 every batch is matched by the tensor-core path AND by the exact CUDA-core
  * kernel; out2[0] = nearest-neighbour table entries compared so far, out2[1] = entries whose packed (distance, index) differ
  * (0 unless the filter's error bound is violated).  Synchronises the handle's stream. */
 int qb200_debug_match_verify(qb200_handle* h, uint64_t* out2, int32_t reset);

@@ -75,13 +75,14 @@ size_t carve_counters(int* base, size_t S, WaveCounters* c) {
   return n + 2;
 }
 
-// A new lane in *out with the settings of `like` (dims, device, n_sm, matcher switch, error sink), its own stream and every
+// A new lane in *out with the settings of `like` (dims, device, n_sm, matcher switches, error sink), its own stream and every
 // buffer of DESIGN §4.  On failure *out is left as it was.
 int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   std::unique_ptr<Lane> L(new (std::nothrow) Lane());
   if (!L) return QB200_ERR_CUDA;
   L->S = like.S; L->R = like.R; L->V = like.V; L->Lc = like.Lc; L->W = like.W; L->NS = like.NS;
   L->device = like.device; L->n_sm = like.n_sm; L->force_exact_match = like.force_exact_match; L->err = like.err;
+  L->tc_verify = like.tc_verify; L->tc_prof = like.tc_prof;
   QB_CUDA_TRY(L, L->own_stream.create(cudaStreamNonBlocking));
   L->stream = L->own_stream;
   const size_t S = L->S, R = L->R, V = L->V, Lc = L->Lc, W = L->W, C = 2 * S;
@@ -474,8 +475,7 @@ int wave_collect(qb200_handle* h, Lane* L) {
   }
   memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
   if (L->pend_lists.cap_per_pair > 0 && L->pend_lists.kind == QB200_MEM_HOST) deliver_lists(L, L->pend_lists, L->pend_w0, np);
-  static const int timeline = (getenv("QB200_TIMELINE") && getenv("QB200_TIMELINE")[0] == '1') ? 1 : 0;
-  if (timeline && L->pend_t0 == 0) {  // stage boundaries of a raw-scan wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
+  if (h->timeline && L->pend_t0 == 0) {  // stage boundaries of a raw-scan wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
     fprintf(stderr, "[qb200 timeline] wave w0=%d np=%d:", L->pend_w0, np);
     for (int i = 0; i < 9; ++i) {
       float ms = -1.f;
@@ -573,15 +573,18 @@ int qb200_create(const qb200_config* cfg_in, qb200_handle** out) {
   like.W = like.Lc / 32; like.NS = like.V / kMatchTile;
   like.device = cfg.device;
   if (cudaDeviceGetAttribute(&like.n_sm, cudaDevAttrMultiProcessorCount, cfg.device) != cudaSuccess || like.n_sm <= 0) return QB200_ERR_NO_DEVICE;
-  // K6 implementation switch: the tensor-core filter + in-kernel exact evaluation is the default; QB200_MATCH_EXACT=1 forces
-  // the exact CUDA-core kernel everywhere (identical results; A/B and triage)
-  const char* fe = getenv("QB200_MATCH_EXACT");
-  like.force_exact_match = (fe && fe[0] == '1') ? 1 : 0;
+  // Every QB200_* switch is read here, once per handle.  K6 implementation switch: the tensor-core filter + in-kernel exact
+  // evaluation is the default; QB200_MATCH_EXACT=1 forces the exact CUDA-core kernel everywhere (identical results; A/B and triage)
+  auto env_on = [](const char* name) { const char* v = getenv(name); return (v && v[0] == '1') ? 1 : 0; };
+  like.force_exact_match = env_on("QB200_MATCH_EXACT");
+  like.tc_verify = env_on("QB200_TC_VERIFY");
+  like.tc_prof = env_on("QB200_TC_PROF");
   qb200_handle* h = new (std::nothrow) qb200_handle();
   if (!h) return QB200_ERR_CUDA;
   h->cfg = cfg;
   const char* ln = getenv("QB200_LANES");
   h->max_lanes = (ln && ln[0] >= '1' && ln[0] <= '8') ? ln[0] - '0' : 4;
+  h->timeline = env_on("QB200_TIMELINE");
   like.err = h->err;
   auto alloc = [&]() -> int {
     QB_CUDA_TRY(h, h->ev_fork.create());  // (timing enabled: QB200_TIMELINE measures the waves against it)

@@ -20,6 +20,8 @@ struct Lane {
   int device;
   int n_sm;                  // multiprocessors of the device (grid size of the persistent kernels)
   int force_exact_match;     // 0 (default): tensor-core filter + exact evaluation; 1 (QB200_MATCH_EXACT=1): exact CUDA-core K6 only
+  int tc_verify;             // 1 (QB200_TC_VERIFY=1): every batch is matched again by the exact K6 and compared (stats[4..5])
+  int tc_prof;               // 1 (QB200_TC_PROF=1): tc_nn_kernel with clock64 accounting of every role's waits (stats[8..31])
   Stream own_stream;
   cudaStream_t stream;       // own_stream, or the caller's stream of qb200_set_stream (lane 0)
   char* err;                 // the handle's message buffer (qb200_last_error)
@@ -120,6 +122,7 @@ struct qb200_handle {
   char err[qb::Lane::kErrLen];
   std::unique_ptr<qb::Lane> lane[8];  // lane[0] is created with the handle, the others on first use
   int max_lanes;              // 1..8 (QB200_LANES, default 4)
+  int timeline;               // 1 (QB200_TIMELINE=1): stage boundaries of every raw-scan wave on stderr
   int lanes_active, lane_cursor;  // lanes of the rotation in use (0 = nothing in flight), next lane = busy longest
   qb::Event ev_fork;
   qb::Stream copy_stream;     // host scans of a multi-wave batch cross PCIe on ONE stream, wave after wave (api.cu: wave_submit)

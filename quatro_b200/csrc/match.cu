@@ -416,8 +416,7 @@ int launch_match(Lane* h, int n_pairs, const qb200_params& p) {
   const int V = h->V;
   int rc = h->force_exact_match ? launch_match_exact(h, n_pairs, nullptr) : launch_match_nn(h, n_pairs);
   if (rc) return rc;
-  static const int verify = (getenv("QB200_TC_VERIFY") && getenv("QB200_TC_VERIFY")[0] == '1') ? 1 : 0;
-  if (verify && !h->force_exact_match) {
+  if (h->tc_verify && !h->force_exact_match) {
     // whole-batch self-check: keep the tensor-core results, redo every pair with the exact CUDA-core kernel, compare
     unsigned long long* rb_tc = reinterpret_cast<unsigned long long*>(h->key_b.get());                   // the sort workspace is idle here
     unsigned long long* cb_tc = rb_tc + (size_t)h->S * V;

@@ -931,8 +931,7 @@ int launch_match_nn(Lane* h, int n_pairs) {
   split_desc_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_t, n_unique, V, uperm, h->desc_tiles, h->desc_norm, h->tc_fallback);
   const dim3 g(h->NS, n_pairs);
   cudaEventRecord(h->kev[0], h->stream);
-  static const int tc_prof = (getenv("QB200_TC_PROF") && getenv("QB200_TC_PROF")[0] == '1') ? 1 : 0;
-  if (tc_prof) {
+  if (h->tc_prof) {
     if (int rc2 = tc_prepare(h, (const void*)tc_nn_kernel<false, true>)) return rc2;
     tc_nn_kernel<false, true><<<g, kTcThreads, smem, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, V, uperm, rowbest_u, colbest_u,
                                                                   tile_cmax, h->tc_fallback, h->tc_stats, nullptr);

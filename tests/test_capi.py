@@ -64,35 +64,45 @@ def test_product_does_not_reference_the_oracle():
         assert "quatro_oracle" not in txt and "from oracle" not in txt and "import oracle" not in txt and "qo_" not in txt.replace("qo_math", ""), f
 
 
-def test_pod_layouts_match_the_header(tmp_path):
-    """The ctypes mirrors of every POD of include/quatro_b200.h have the size and field offsets a C compiler gives them."""
+POD_MIRRORS = {"qb200_params": capi.Params, "qb200_config": capi.Config, "qb200_result": capi.Result, "qb200_pair": capi.Pair,
+               "qb200_patchwork_params": capi.PatchworkParams, "qb200_segment_params": capi.SegmentParams,
+               "qb200_preprocess_out": capi.PreprocessOut, "qb200_corr_set": capi.CorrSet, "qb200_pair_lists": capi.PairLists}
+
+
+def header_fields(struct):
+    """Member names of `typedef struct <struct> { ... } <struct>;` in include/quatro_b200.h, in declaration order."""
+    hdr = (ROOT / "include" / "quatro_b200.h").read_text()
+    body = hdr[hdr.index(f"typedef struct {struct} {{"):hdr.index(f"}} {struct};")].split("{", 1)[1]
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    return [n for decl in body.split(";") for n in re.findall(r"(\w+)\s*(?:\[\w*\])?\s*(?:,|$)", decl.strip())]
+
+
+@pytest.fixture(scope="module")
+def pod_probe(tmp_path_factory):
+    """sizeof and every member's offsetof of each mirrored POD, and QB200_FLAG_LISTS_TRUNCATED, from a C compiler."""
     import subprocess
-    from quatro_b200 import capi
-    src = tmp_path / "pod.c"
-    src.write_text('''
-#include <stddef.h>
-#include <stdio.h>
-#include "quatro_b200.h"
-#define S(t) printf("%s %zu\\n", #t, sizeof(t))
-#define O(t, f) printf("%s.%s %zu\\n", #t, #f, offsetof(t, f))
-int main(void) {
-  S(qb200_params); S(qb200_config); S(qb200_result); S(qb200_pair); S(qb200_patchwork_params); S(qb200_segment_params);
-  O(qb200_params, seed); O(qb200_params, noise_bound); O(qb200_params, max_clique_node_limit); O(qb200_params, RyRx);
-  O(qb200_result, flags); O(qb200_result, n_edges); O(qb200_result, T);
-  O(qb200_patchwork_params, min_ranges_each_zone); O(qb200_patchwork_params, num_iter); O(qb200_patchwork_params, num_rings_each_zone);
-  O(qb200_segment_params, segment_theta); O(qb200_segment_params, segment_valid_line_num);
-  return 0;
-}
-''')
-    exe = tmp_path / "pod"
-    r = subprocess.run(["/usr/bin/gcc", "-std=c11", "-Wall", "-Werror", f"-I{ROOT / 'include'}", str(src), "-o", str(exe)], capture_output=True, text=True)
+    tmp = tmp_path_factory.mktemp("pod")
+    lines = [f'  printf("{t} %zu\\n", sizeof({t}));\n' +
+             "".join(f'  printf("{t}.{f} %zu\\n", offsetof({t}, {f}));\n' for f, _ in m._fields_) for t, m in POD_MIRRORS.items()]
+    (tmp / "pod.c").write_text('#include <stddef.h>\n#include <stdio.h>\n#include "quatro_b200.h"\nint main(void) {\n' + "".join(lines) +
+                               '  printf("QB200_FLAG_LISTS_TRUNCATED %d\\n", (int)QB200_FLAG_LISTS_TRUNCATED);\n  return 0;\n}\n')
+    r = subprocess.run(["/usr/bin/gcc", "-std=c11", "-Wall", "-Werror", f"-I{ROOT / 'include'}", str(tmp / "pod.c"), "-o", str(tmp / "pod")],
+                       capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
-    got = dict(ln.split() for ln in subprocess.run([str(exe)], capture_output=True, text=True).stdout.splitlines())
-    mirror = {"qb200_params": capi.Params, "qb200_config": capi.Config, "qb200_result": capi.Result, "qb200_pair": capi.Pair,
-              "qb200_patchwork_params": capi.PatchworkParams, "qb200_segment_params": capi.SegmentParams}
-    for name, val in got.items():
-        if "." in name:
-            t, f = name.split(".")
-            assert getattr(mirror[t], f).offset == int(val), name
-        else:
-            assert C.sizeof(mirror[name]) == int(val), name
+    return {k: int(v) for k, v in (ln.split() for ln in subprocess.run([str(tmp / "pod")], capture_output=True, text=True,
+                                                                         check=True).stdout.splitlines())}
+
+
+@pytest.mark.parametrize("struct", list(POD_MIRRORS))
+def test_pod_layouts_match_the_header(pod_probe, struct):
+    """The ctypes mirror of a POD of include/quatro_b200.h has the header's members, in order, at the offsets a C compiler gives
+    them, and the same size."""
+    mirror = POD_MIRRORS[struct]
+    fields = [f for f, _ in mirror._fields_]
+    assert fields == header_fields(struct)
+    assert C.sizeof(mirror) == pod_probe[struct]
+    for f in fields:
+        assert getattr(mirror, f).offset == pod_probe[f"{struct}.{f}"], f
+    if struct == "qb200_pair_lists":
+        assert pod_probe["QB200_FLAG_LISTS_TRUNCATED"] == capi.FLAG_LISTS_TRUNCATED
+        assert set(capi.LIST_LAYOUT) == set(fields) - {"cap_per_pair", "kind"}

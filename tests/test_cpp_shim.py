@@ -2,27 +2,17 @@
 reference's example: compiles and links on the CPU box; on the GPU box it runs and must reproduce the oracle."""
 import re
 import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
-ROOT = Path(__file__).resolve().parent.parent
+from support import ROOT, build_against_lib
 
-
-def build_example(tmp_path):
-    from quatro_b200 import _build
-    lib = _build.build_cuda()
-    exe = tmp_path / "run_example"
-    cmd = ["/usr/bin/g++", "-std=c++17", "-Wall", "-Werror", f"-I{ROOT / 'include'}", str(ROOT / "examples" / "run_global_registration.cpp"),
-           f"-L{lib.parent}", "-lquatro_b200", f"-Wl,-rpath,{lib.parent}", "-o", str(exe)]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return exe
+EXAMPLE = "examples/run_global_registration.cpp"
 
 
 def test_example_compiles_against_the_shim(tmp_path):
-    exe = build_example(tmp_path)
+    exe = build_against_lib(tmp_path, EXAMPLE)
     r = subprocess.run([str(exe)], capture_output=True, text=True)
     assert r.returncode == 2 and "usage" in r.stderr
 
@@ -59,7 +49,7 @@ def test_example_with_preprocessing_reproduces_the_oracle(tmp_path, oracle):
     """--preprocess: PatchWork + ImageProjection through the C++ shim in front of the path, against the oracle's chain."""
     from quatro_b200 import synth
     from quatro_b200.capi import default_params, default_patchwork_params, default_segment_params
-    exe = build_example(tmp_path)
+    exe = build_against_lib(tmp_path, EXAMPLE)
     src, tgt, T = synth.outdoor_pair(2)
     src[:, 3] = 1.0; tgt[:, 3] = 1.0                  # the .bin loader drops the 4th channel anyway
     (tmp_path / "src.bin").write_bytes(src.astype(np.float32).tobytes())
@@ -85,7 +75,7 @@ def test_example_with_preprocessing_reproduces_the_oracle(tmp_path, oracle):
 def test_example_reproduces_the_oracle(tmp_path, oracle):
     from quatro_b200 import synth
     from quatro_b200.capi import default_params
-    exe = build_example(tmp_path)
+    exe = build_against_lib(tmp_path, EXAMPLE)
     src, tgt, T = synth.outdoor_pair(1)
     src, tgt = src[src[:, 3] > 0], tgt[tgt[:, 3] > 0]      # the example has no ground filter: hand it the non-ground returns
     (tmp_path / "src.bin").write_bytes(src.astype(np.float32).tobytes())
@@ -106,25 +96,14 @@ def test_example_reproduces_the_oracle(tmp_path, oracle):
     assert rot < 2.0 and tr < 0.5
 
 
-def build_fixture(tmp_path, name):
-    from quatro_b200 import _build
-    lib = _build.build_cuda()
-    exe = tmp_path / name
-    cmd = ["/usr/bin/g++", "-std=c++17", "-Wall", "-Werror", f"-I{ROOT / 'include'}", str(ROOT / "tests" / "fixtures" / f"{name}.cpp"),
-           f"-L{lib.parent}", "-lquatro_b200", f"-Wl,-rpath,{lib.parent}", "-o", str(exe)]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return exe
-
-
 def test_shim_extras_compile(tmp_path):
-    build_fixture(tmp_path, "shim_extras")
+    build_against_lib(tmp_path, "tests/fixtures/shim_extras.cpp")
 
 
 @pytest.mark.gpu
 def test_fpfh_manager_getters_odometry_and_pcd_cache(tmp_path):
     from quatro_b200 import synth
-    exe = build_fixture(tmp_path, "shim_extras")
+    exe = build_against_lib(tmp_path, "tests/fixtures/shim_extras.cpp")
     a, b, _ = synth.outdoor_pair(11, rings=32, azimuths=900)
     c, _, _ = synth.outdoor_pair(12, rings=32, azimuths=900)
     names = []

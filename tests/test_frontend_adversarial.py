@@ -12,25 +12,11 @@ import pytest
 from quatro_b200 import synth
 from quatro_b200.capi import Handle, default_params
 from independent_ref import voxel_grid
+from support import P4, same_bits
 
 DEFAULT_CELL = float(np.float32(0.75) * np.float32(1.001953125))
 OK, CAPACITY, OVERFLOW = 0, 3, -5
 INT_MAX = 2**31 - 1
-
-
-def P4(xyz, w=1.0):
-    xyz = np.asarray(xyz, np.float32).reshape(-1, 3)
-    out = np.full((len(xyz), 4), w, np.float32)
-    out[:, :3] = xyz
-    return out
-
-
-def same_bits(a, b):
-    return a.shape == b.shape and np.array_equal(np.asarray(a, np.float32).view(np.uint32), np.asarray(b, np.float32).view(np.uint32))
-
-
-def same_normals(a, b):
-    return a.shape == b.shape and bool(((a.view(np.uint32) == b.view(np.uint32)) | (np.isnan(a) & np.isnan(b))).all())
 
 
 def grid_of(pts4, leaf, skip):
@@ -281,7 +267,7 @@ def test_mixed_waves_through_the_scan_cache(clouds, oracle_vox, oracle, slots):
                     assert st_r == OK and same_bits(vox, ref), name
                     if len(ref) <= 6000:
                         n_ref, d_ref = oracle.compute_fpfh(ref, p.normal_radius, p.fpfh_radius, DEFAULT_CELL)
-                        if not (same_normals(nrm, n_ref) and same_bits(desc, d_ref)):
+                        if not (same_bits(nrm, n_ref, nan_equal=True) and same_bits(desc, d_ref)):
                             bad.append(f"{name}: normals / descriptors differ from the oracle")
         assert not bad, "\n".join(bad)
 
@@ -344,7 +330,7 @@ def test_fpfh_edges_in_mixed_waves(oracle):
                 assert st == OK
                 vox, nrm, desc = h.cache_read(i)
                 n_ref, d_ref = oracle.compute_fpfh(ref, p.normal_radius, p.fpfh_radius, DEFAULT_CELL)
-                if not (same_bits(vox, ref) and same_normals(nrm, n_ref) and same_bits(desc, d_ref)):
+                if not (same_bits(vox, ref) and same_bits(nrm, n_ref, nan_equal=True) and same_bits(desc, d_ref)):
                     bad.append(name)
                 if name == "beyond_lattice":
                     assert np.isnan(nrm).all() and len(vox) > 100
@@ -356,7 +342,7 @@ def test_fpfh_edges_in_mixed_waves(oracle):
         dup = np.concatenate([base, base[::3], base[:5]])
         n_ref, d_ref = oracle.compute_fpfh(dup, 0.5, 0.75, DEFAULT_CELL)
         n_got, d_got = h.compute_fpfh(dup, 0.5, 0.75, DEFAULT_CELL)
-        assert same_normals(n_got, n_ref) and same_bits(d_got, d_ref)
+        assert same_bits(n_got, n_ref, nan_equal=True) and same_bits(d_got, d_ref)
 
 
 def wrap_cloud():
@@ -388,7 +374,7 @@ def test_spfh_counts_beyond_16_bits(wrap_ref):
     n_ref, d_ref, _, _ = wrap_ref
     with Handle(max_batch_slots=1, max_voxel_points=131072) as h:
         n_got, d_got = h.compute_fpfh(wrap_cloud(), 0.5, 0.75, DEFAULT_CELL)
-    assert same_normals(n_got, n_ref)
+    assert same_bits(n_got, n_ref, nan_equal=True)
     diff = (d_got.view(np.uint32) != d_ref.view(np.uint32)).any(1)
     assert not diff.any(), f"{diff.sum()} descriptors differ (first {np.nonzero(diff)[0][:5]})"
 

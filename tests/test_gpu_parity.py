@@ -7,18 +7,12 @@ import pytest
 from conftest import adj_to_dense, dense_to_adj
 from quatro_b200 import synth
 from quatro_b200.capi import Handle, default_params, PMC_HEU, KCORE_HEU, INLIER_NONE, COTE_WEIGHTED_MEAN, RESULT_DTYPE
+from support import P4, assert_same_record, fpfh_like, same_bits
 
 pytestmark = pytest.mark.gpu
 
 # the production default of the neighbour lattice: (1 + 2^-9) * fpfh_radius (api.cu lattice_cell(), oracle default)
 DEFAULT_CELL = float(np.float32(0.75) * np.float32(1.001953125))
-
-
-def P4(xyz, w=1.0):
-    xyz = np.asarray(xyz, np.float32).reshape(-1, 3)
-    out = np.full((len(xyz), 4), w, np.float32)
-    out[:, :3] = xyz
-    return out
 
 
 @pytest.fixture(scope="module")
@@ -50,8 +44,7 @@ def test_voxelize_bit_exact(handle, oracle, scan_pair, small_pair):
                 assert st_g == 3  # QB200_CAPACITY_EXCEEDED is reported, not silently truncated
                 continue
             assert st_g == st_r == 0
-            assert got.shape == ref.shape
-            assert np.array_equal(got.view(np.uint32), ref.view(np.uint32))  # centroids bit for bit, same order
+            assert same_bits(got, ref)  # centroids bit for bit, same order
 
 
 def test_voxelize_edge_cases(handle, oracle):
@@ -60,7 +53,7 @@ def test_voxelize_edge_cases(handle, oracle):
     for skip in (0, 1):
         ref, _ = oracle.voxelize(pts, 0.3, skip)
         got, st = handle.voxelize(pts, 0.3, skip)
-        assert st == 0 and np.array_equal(got.view(np.uint32), ref.view(np.uint32))
+        assert st == 0 and same_bits(got, ref)
     got, st = handle.voxelize(P4(np.zeros((0, 3))), 0.3, 1)
     assert len(got) == 0 and st == 0
     got, st = handle.voxelize(P4([[np.nan, 0, 0]]), 0.3, 1)
@@ -95,8 +88,8 @@ def test_fpfh_other_lattice_and_unsorted_input(handle, oracle):
     for cell in (0.3, 0.5, 0.2, DEFAULT_CELL):
         n_ref, d_ref = oracle.compute_fpfh(P4(pts), 0.5, 0.75, cell)
         n_got, d_got = handle.compute_fpfh(P4(pts), 0.5, 0.75, cell)
-        assert np.array_equal(d_got.view(np.uint32), d_ref.view(np.uint32))
-        assert ((n_got.view(np.uint32) == n_ref.view(np.uint32)) | (np.isnan(n_got) & np.isnan(n_ref))).all()
+        assert same_bits(d_got, d_ref)
+        assert same_bits(n_got, n_ref, nan_equal=True)
     # isolated / too-few-neighbour points: NaN normals, finite descriptors
     iso = P4([[0, 0, 0], [0.1, 0, 0], [10, 10, 10]])
     n_got, d_got = handle.compute_fpfh(iso, 0.5, 0.75, 0.3)
@@ -141,20 +134,13 @@ def test_match_ties_and_small_inputs(handle, oracle):
             assert np.array_equal(got[0], ref[0]) and got[1] == ref[1]
 
 
-def _fpfh_like(rng, n):
-    d = rng.gamma(0.3, 1.0, (n, 33)).astype(np.float32)
-    for t in range(3):
-        d[:, 11 * t:11 * t + 11] *= 100.0 / np.maximum(d[:, 11 * t:11 * t + 11].sum(1, keepdims=True), 1e-6)
-    return d.astype(np.float32)
-
-
 def test_match_isolated_points_and_padding(handle, oracle):
     """All-zero descriptors (FPFH of a point without neighbours) are bit-identical to the zero padding of the last
     128-point block: padded rows / columns must never enter the exact evaluation (regression: they once won ties)."""
     rng = np.random.default_rng(21)
     for na, nb in ((300, 290), (129, 257), (640, 513)):
         a, b = P4(rng.uniform(-30, 30, (na, 3))), P4(rng.uniform(-30, 30, (nb, 3)))
-        ad, bd = _fpfh_like(rng, na), _fpfh_like(rng, nb)
+        ad, bd = fpfh_like(rng, na), fpfh_like(rng, nb)
         ad[[7, na // 2, na - 1]] = 0.0
         bd[[3, nb - 2]] = 0.0
         ad[na // 3] = ad[5]; bd[nb // 3] = ad[5]                 # a duplicate class that is not the zero vector
@@ -186,16 +172,16 @@ def test_tc_filter_error_bound(handle):
     worst = 0.0
     cases = []
     for trial in range(4):
-        a, b = _fpfh_like(rng, 128), _fpfh_like(rng, 100 + trial)
+        a, b = fpfh_like(rng, 128), fpfh_like(rng, 100 + trial)
         if trial == 3:
             b[:50] = a[:50]                                    # exact duplicates: d = 0 rows
         cases.append((a, b))
     # adversarial: large dynamic range inside one descriptor, near-cancelling cross terms, tiny and huge norms side by side
     spike = np.zeros((128, 33), np.float32); spike[np.arange(128), rng.integers(0, 33, 128)] = 100.0; spike += rng.uniform(0, 1e-3, spike.shape).astype(np.float32)
     cases.append((spike, spike[::-1].copy()))
-    near = _fpfh_like(rng, 128); cases.append((near, (near * np.float32(1 + 2e-4)).astype(np.float32)))       # d ~ 1e-8 |a|^2: full cancellation
+    near = fpfh_like(rng, 128); cases.append((near, (near * np.float32(1 + 2e-4)).astype(np.float32)))       # d ~ 1e-8 |a|^2: full cancellation
     mu = np.zeros(33, np.float32); mu[[5, 16, 27]] = 100.0
-    tiny = (mu + rng.normal(0, 1e-3, (128, 33))).astype(np.float32); cases.append((tiny, _fpfh_like(rng, 128)))  # |a'| ~ 1e-3 next to |b'| ~ 100
+    tiny = (mu + rng.normal(0, 1e-3, (128, 33))).astype(np.float32); cases.append((tiny, fpfh_like(rng, 128)))  # |a'| ~ 1e-3 next to |b'| ~ 100
     cases.append((np.tile(mu, (128, 1)), np.zeros((128, 33), np.float32)))                                     # planes vs isolated points
     alt = np.zeros((128, 33), np.float32); alt[:, ::2] = 18.75; alt[:, 1::2] = 0.0; cases.append((alt, (alt.max() - alt).astype(np.float32)))
     for a, b in cases:
@@ -205,32 +191,27 @@ def test_tc_filter_error_bound(handle):
     assert worst < 2.0e-5, worst     # kTcC / 2 = 6e-5: three times the worst case seen
 
 
-def test_match_exact_kernel_and_tie_fallback(oracle, scan_pair):
+def test_match_exact_kernel_and_tie_fallback(oracle, scan_pair, monkeypatch):
     """Default K6 = tensor-core filter + in-kernel exact evaluation; thousands of identical descriptors make its stripes abort
     to the exact CUDA-core kernel.  QB200_MATCH_EXACT=1 forces the exact kernel everywhere.  All must equal the oracle."""
-    import os
-    from quatro_b200.capi import Handle
     rng = np.random.default_rng(4)
     n = 2600
     a, b = P4(rng.uniform(-30, 30, (n, 3))), P4(rng.uniform(-30, 30, (n - 7, 3)))
-    ad, bd = _fpfh_like(rng, n), _fpfh_like(rng, n - 7)
+    ad, bd = fpfh_like(rng, n), fpfh_like(rng, n - 7)
     ad[:2200] = ad[0]; bd[:2100] = ad[0]                        # massive exact ties -> lowest-index tie-breaks everywhere
     p = default_params(); p.use_tuple_test = 0
     ref = oracle.match(a, ad, b, bd, p)
     with Handle(max_batch_slots=2) as h:
         got = h.match(a, ad, b, bd, p)
         assert np.array_equal(got[0], ref[0]) and got[1] == ref[1]
-    os.environ["QB200_MATCH_EXACT"] = "1"
-    try:
-        with Handle(max_batch_slots=2) as h:
-            got = h.match(a, ad, b, bd, p)
-            assert np.array_equal(got[0], ref[0])
-            src, tgt, _ = scan_pair
-            r_ref, _ = oracle.register_pair(src, tgt, default_params())
-            r_got, _ = h.register_pair(src, tgt, default_params())
-            assert (r_got.n_mutual, r_got.n_corr, r_got.clique_size) == (r_ref.n_mutual, r_ref.n_corr, r_ref.clique_size)
-    finally:
-        del os.environ["QB200_MATCH_EXACT"]
+    monkeypatch.setenv("QB200_MATCH_EXACT", "1")
+    with Handle(max_batch_slots=2) as h:
+        got = h.match(a, ad, b, bd, p)
+        assert np.array_equal(got[0], ref[0])
+        src, tgt, _ = scan_pair
+        r_ref, _ = oracle.register_pair(src, tgt, default_params())
+        r_got, _ = h.register_pair(src, tgt, default_params())
+        assert (r_got.n_mutual, r_got.n_corr, r_got.clique_size) == (r_ref.n_mutual, r_ref.n_corr, r_ref.clique_size)
 
 
 def test_match_and_pack(handle, oracle, small_pair):
@@ -474,11 +455,11 @@ def test_small_capacity_handles(oracle, small_pair):
                     ref = ref[:V]
                 else:
                     assert st_g == st_r == 0, (kw, skip)
-                assert np.array_equal(got.view(np.uint32), ref.view(np.uint32)), (kw, skip)
+                assert same_bits(got, ref), (kw, skip)
             a, b = sv[:min(len(sv), V, h.cfg.max_raw_points)], tv[:min(len(tv), V, h.cfg.max_raw_points)]
             n_g, d_g = h.compute_fpfh(a, 0.5, 0.75, DEFAULT_CELL)
             n_r, d_r = oracle.compute_fpfh(a, 0.5, 0.75, DEFAULT_CELL)
-            assert np.array_equal(d_g.view(np.uint32), d_r.view(np.uint32)), kw
+            assert same_bits(d_g, d_r), kw
             _, d_b = oracle.compute_fpfh(b, 0.5, 0.75, DEFAULT_CELL)
             c_g = h.match(a, d_r, b, d_b, p)[0]
             c_r = oracle.match(a, d_r, b, d_b, p)[0]
@@ -572,49 +553,37 @@ def test_solve_batch_matches_single_and_oracle(handle, oracle):
 
 
 # ---- end to end ----------------------------------------------------------------------------------------
-def _same_record(g, r):
-    for k in ("valid", "status", "n_src_vox", "n_tgt_vox", "n_mutual", "n_corr", "n_edges", "max_core", "clique_size", "gnc_iters",
-              "n_rot_inliers", "n_final_inliers"):
-        assert g[k] == getattr(r, k), (k, g[k], getattr(r, k))
-    assert np.allclose(np.asarray(g["T"]).reshape(4, 4).T, r.matrix(), atol=1e-9)
-
-
 def test_register_pair_end_to_end(handle, oracle, scan_pair):
     src, tgt, T = scan_pair
     p = default_params()
     r_ref, st_r = oracle.register_pair(src, tgt, p)
     r_got, st_g = handle.register_pair(src, tgt, p)
     assert st_g == st_r == 0
-    _same_record({k: getattr(r_got, k) for k, _ in r_got._fields_ if k != "T"} | {"T": np.array(r_got.T[:])}, r_ref)
+    assert_same_record(r_got, r_ref)
     rot, tr = synth.pose_error(r_got.matrix(), T)
     assert rot < 2.0 and tr < 0.5        # vs ground truth (the z offset of a yaw-only model stays in the budget)
     rot, tr = synth.pose_error(r_got.matrix(), r_ref.matrix())
     assert rot < 1e-6 and tr < 1e-6      # vs the CPU reference path: north_star asks for 2 deg / 0.3 m
 
 
-def test_register_batch_matches_single_and_oracle(handle, oracle):
+def test_register_batch_matches_single_and_oracle(handle, oracle, monkeypatch):
     p = default_params()
     pairs = [synth.outdoor_pair(s, rings=32, azimuths=900)[:2] for s in range(10, 21)]   # 11 pairs > 8 slots: two waves
     out = handle.register_batch(pairs, p)
     assert out.dtype == RESULT_DTYPE and len(out) == len(pairs)
     for (src, tgt), g in zip(pairs, out):
         r_ref, _ = oracle.register_pair(src, tgt, p)
-        _same_record(g, r_ref)
+        assert_same_record(g, r_ref)
     # order / batch composition must not change any pair's result
     out2 = handle.register_batch(pairs[::-1], p)
     assert out2[::-1].tobytes() == out.tobytes()
     # three waves alternating between the two lanes, and the single-lane path (QB200_LANES=1): same records
-    import os
-    from quatro_b200.capi import Handle
     with Handle(max_batch_slots=4) as h4:
         assert h4.register_batch(pairs, p).tobytes() == out.tobytes()
         assert h4.register_batch(pairs, p).tobytes() == out.tobytes()      # lanes are reusable
-    os.environ["QB200_LANES"] = "1"
-    try:
-        with Handle(max_batch_slots=4) as h1:
-            assert h1.register_batch(pairs, p).tobytes() == out.tobytes()
-    finally:
-        del os.environ["QB200_LANES"]
+    monkeypatch.setenv("QB200_LANES", "1")
+    with Handle(max_batch_slots=4) as h1:
+        assert h1.register_batch(pairs, p).tobytes() == out.tobytes()
 
 
 def test_register_batch_enqueue_flush_pipelined(oracle):
@@ -665,7 +634,7 @@ def test_register_batch_enqueue_flush_pipelined(oracle):
         h.set_stream(0)
         assert out1.tobytes() == one.tobytes()
     r_ref, _ = oracle.register_pair(batches[0][0][0], batches[0][0][1], p)
-    _same_record(ref[0][0], r_ref)
+    assert_same_record(ref[0][0], r_ref)
 
 
 def test_register_batch_device_resident_inputs(handle, oracle):
@@ -727,9 +696,9 @@ def test_scan_cache_matches_uncached_pipeline(oracle):
         vox, nrm, desc = h.cache_read(slots[2])
         v_ref, _ = oracle.voxelize(scans[2], p.voxel_size, 1)
         n_ref, d_ref = oracle.compute_fpfh(v_ref, p.normal_radius, p.fpfh_radius, DEFAULT_CELL)
-        assert np.array_equal(vox.view(np.uint32), v_ref.view(np.uint32))
-        assert np.array_equal(desc.view(np.uint32), d_ref.view(np.uint32))
-        assert ((nrm.view(np.uint32) == n_ref.view(np.uint32)) | (np.isnan(nrm) & np.isnan(n_ref))).all()
+        assert same_bits(vox, v_ref)
+        assert same_bits(desc, d_ref)
+        assert same_bits(nrm, n_ref, nan_equal=True)
         # parameters other than the cached ones are refused
         q = default_params(); q.voxel_size = 0.25
         from quatro_b200.capi import QuatroB200Error
@@ -740,29 +709,14 @@ def test_scan_cache_matches_uncached_pipeline(oracle):
 def test_tc_verify_whole_batch(monkeypatch):
     """QB200_TC_VERIFY=1: every nearest-neighbour table entry of a batch is recomputed by the exact CUDA-core kernel and compared
     with the tensor-core path's result: zero mismatches (the filter's error bound held for every entry)."""
-    import quatro_b200.capi as capi
     monkeypatch.setenv("QB200_TC_VERIFY", "1")
     p = default_params()
     pairs = [synth.outdoor_pair(80 + i)[:2] for i in range(4)]
-    import subprocess, sys, json, textwrap
-    # the switch is read once per process: run the check in a fresh interpreter
-    code = textwrap.dedent("""
-        import json, sys
-        sys.path.insert(0, %r)
-        from quatro_b200 import synth
-        from quatro_b200.capi import Handle, default_params
-        p = default_params()
-        pairs = [synth.outdoor_pair(80 + i)[:2] for i in range(4)]
-        with Handle(max_batch_slots=4) as h:
-            a = h.register_batch(pairs, p)
-            v = h.debug_match_verify()
-        print(json.dumps({"v": v, "valid": int(a["valid"].sum())}))
-    """) % str(__import__("pathlib").Path(__file__).resolve().parent.parent)
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout + r.stderr
-    out = json.loads(r.stdout.strip().splitlines()[-1])
-    assert out["v"]["compared"] > 4 * 10000 and out["v"]["mismatches"] == 0, out
-    assert out["valid"] == 4
+    with Handle(max_batch_slots=4) as h:
+        a = h.register_batch(pairs, p)
+        v = h.debug_match_verify()
+    assert v["compared"] > 4 * 10000 and v["mismatches"] == 0, v
+    assert int(a["valid"].sum()) == 4
 
 
 def test_dense_indoor_pair_50k_voxels(oracle):

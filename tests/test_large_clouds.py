@@ -3,20 +3,16 @@
 The dense indoor hall pair (synth.indoor_pair(0, extent=9.0): 500 k rays per scan, 134 k / 101 k voxel points at a 0.05 m voxel) runs
 through every stage and must match the CPU oracle bit for bit, like the smaller clouds of test_gpu_parity.py.  The oracle needs ~15 s
 per hall pair on 8 cores, so its results are computed once per module."""
-import json
-import os
 import re
 import subprocess
-import sys
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 from quatro_b200 import synth
 from quatro_b200.capi import RESULT_DTYPE, Handle, QuatroB200Error, default_params
+from support import ROOT, assert_same_record, build_against_lib, same_bits
 
-ROOT = Path(__file__).resolve().parent.parent
 MAX_V = 262144
 HALL = dict(extent=9.0)
 HANDLE_CFG = dict(max_batch_slots=1, max_raw_points=524288, max_voxel_points=MAX_V, max_corr=8192)
@@ -94,11 +90,6 @@ def test_voxelize_hall_scan_bit_exact(gpu, hall, hall_ref):
     assert len(hall_ref["tv"]) > 65536
 
 
-def _desc_equal(a, b):
-    """Bit-identical float arrays, NaN pattern included."""
-    return a.shape == b.shape and a.view(np.uint32).tobytes() == b.view(np.uint32).tobytes()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("radii", [(0.10, 0.15), (0.15, 0.30)], ids=["production", "wide"])
 def test_fpfh_hall_cloud_bit_exact(gpu, hall_ref, oracle, radii):
@@ -112,8 +103,8 @@ def test_fpfh_hall_cloud_bit_exact(gpu, hall_ref, oracle, radii):
         assert (cnt > 80).sum() > 20000, (cnt > 80).sum()
     n_got, d_got = gpu.compute_fpfh(pts, rn, rf, default_cell(rf))
     n_ref, d_ref = oracle.compute_fpfh(pts, rn, rf, default_cell(rf))
-    assert _desc_equal(n_got, n_ref)
-    assert _desc_equal(d_got, d_ref)
+    assert same_bits(n_got, n_ref)
+    assert same_bits(d_got, d_ref)
 
 
 @pytest.fixture(scope="module")
@@ -137,41 +128,16 @@ def test_match_hall_descriptors_tensor_core_path(gpu, hall_ref, hall_features):
     assert stats["tiles"] > 0
 
 
-_EXACT_SCRIPT = r"""
-import json, sys, numpy as np
-sys.path.insert(0, sys.argv[1])
-from quatro_b200.capi import Handle, default_params
-d = np.load(sys.argv[2])
-p = default_params()
-for k, v in json.loads(sys.argv[4]).items():
-    setattr(p, k, v)
-with Handle(**json.loads(sys.argv[5])) as h:
-    corr, nm, st = h.match(d["sv"], d["sd"], d["tv"], d["td"], p, cap=8192)
-    stats = h.debug_match_stats()
-np.save(sys.argv[3], corr)
-print(nm, st, stats["tiles"])
-"""
-
-
 @pytest.mark.gpu
-def test_match_hall_descriptors_exact_kernel(hall_ref, hall_features, tmp_path):
+def test_match_hall_descriptors_exact_kernel(hall_ref, hall_features, monkeypatch):
     """QB200_MATCH_EXACT=1: the CUDA-core kernel alone, its column minima folded with atomicMin into one [V] row per pair."""
     f = hall_features
-    inp, out = tmp_path / "in.npz", tmp_path / "corr.npy"
-    np.savez(inp, sv=hall_ref["sv"], tv=hall_ref["tv"], sd=f["sd"], td=f["td"])
-    env = dict(os.environ, QB200_MATCH_EXACT="1")
-    p = indoor_params()
-    pj = json.dumps({k: getattr(p, k) for k in ("voxel_size", "normal_radius", "fpfh_radius", "noise_bound", "cote_noise_bound", "skip_flagged")})
-    r = subprocess.run([sys.executable, "-c", _EXACT_SCRIPT, str(ROOT), str(inp), str(out), pj, json.dumps(HANDLE_CFG)], capture_output=True,
-                       text=True, env=env, timeout=600)
-    assert r.returncode == 0, r.stdout + r.stderr
-    nm, st, tiles = map(int, r.stdout.split()[-3:])
-    assert (nm, st) == (f["nm"], f["st"]) and tiles == 0  # no tensor-core tile ran
-    assert np.array_equal(np.load(out), f["corr"])
-
-
-def _key(rec):
-    return (rec.n_src_vox, rec.n_tgt_vox, rec.n_mutual, rec.n_corr, rec.n_edges, rec.max_core, rec.clique_size)
+    monkeypatch.setenv("QB200_MATCH_EXACT", "1")
+    with Handle(**HANDLE_CFG) as h:
+        corr, nm, st = h.match(hall_ref["sv"], f["sd"], hall_ref["tv"], f["td"], indoor_params(), cap=8192)
+        stats = h.debug_match_stats()
+    assert (nm, st) == (f["nm"], f["st"]) and stats["tiles"] == 0  # no tensor-core tile ran
+    assert np.array_equal(corr, f["corr"])
 
 
 @pytest.mark.gpu
@@ -180,9 +146,8 @@ def test_register_hall_pair_matches_the_oracle(gpu, hall, hall_ref):
     ref, st_ref = hall_ref["rec"], hall_ref["st"]
     got, st = gpu.register_pair(src, tgt, indoor_params())
     assert st == st_ref == 0 and got.valid == 1 == ref.valid
-    assert _key(got) == _key(ref)
+    assert_same_record(got, ref)
     assert got.n_src_vox > 65536 and got.n_tgt_vox > 65536 and got.n_corr > 4096
-    assert np.allclose(got.matrix(), ref.matrix(), atol=1e-9)
     rot, tr = synth.pose_error(got.matrix(), T)
     assert rot < 2.0 and tr < 0.3
 
@@ -203,25 +168,17 @@ def test_batch_and_cache_records_equal_single_calls(gpu, hall):
     assert cached.tobytes() == single.tobytes()
 
 
-def _build_fixture(tmp_path, name):
-    from quatro_b200 import _build
-    lib = _build.build_cuda()
-    exe = tmp_path / name
-    cmd = ["/usr/bin/g++", "-std=c++17", "-Wall", "-Werror", f"-I{ROOT / 'include'}", str(ROOT / "tests" / "fixtures" / f"{name}.cpp"),
-           f"-L{lib.parent}", "-lquatro_b200", f"-Wl,-rpath,{lib.parent}", "-o", str(exe)]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return exe
+FIXTURE = "tests/fixtures/large_cloud_shim.cpp"
 
 
 def test_large_cloud_shim_driver_compiles(tmp_path):
-    _build_fixture(tmp_path, "large_cloud_shim")
+    build_against_lib(tmp_path, FIXTURE)
 
 
 @pytest.mark.gpu
 def test_cpp_shim_registers_the_hall_pair(tmp_path, hall, hall_ref):
     """voxelize / FPFHManager / Quatro grow their handles (500 k raw points, > 65536 voxel points, > 4096 correspondences)."""
-    exe = _build_fixture(tmp_path, "large_cloud_shim")
+    exe = build_against_lib(tmp_path, FIXTURE)
     src, tgt, T = hall
     (tmp_path / "src.bin").write_bytes(np.ascontiguousarray(src, np.float32).tobytes())
     (tmp_path / "tgt.bin").write_bytes(np.ascontiguousarray(tgt, np.float32).tobytes())

@@ -8,12 +8,11 @@ correct: the filter margin, the tile skipping (norm-gap bound, the 256-tile wind
 the abort to the exact kernel, and non-finite or overflowing descriptors.
 
 The CPU tests pin the oracle itself: float64 argmins, mutual pairs, and exact power-of-two scale invariance."""
-import os
-
 import numpy as np
 import pytest
 
 from quatro_b200.capi import default_params
+from support import P4, fpfh_like
 
 NONE = np.uint64(0xFFFFFFFFFFFFFFFF)
 MU = np.zeros(33, np.float32)
@@ -21,13 +20,6 @@ MU[[5, 16, 27]] = 100.0     # the centring vector of tc_match.cu (FPFH of a plan
 
 
 # ---- descriptor families ----------------------------------------------------------------------------------------------
-def _fpfh_like(rng, n):
-    d = rng.gamma(0.3, 1.0, (n, 33)).astype(np.float32)
-    for t in range(3):
-        d[:, 11 * t:11 * t + 11] *= 100.0 / np.maximum(d[:, 11 * t:11 * t + 11].sum(1, keepdims=True), 1e-6)
-    return d.astype(np.float32)
-
-
 def _norm_chain(x):
     """|x - mu|^2 by the fp32 chain of norm_key_kernel / split_desc_kernel (fma emulated in float64, exact for a square)."""
     xc = (x.astype(np.float32) - MU).astype(np.float32)
@@ -45,7 +37,7 @@ def _unit(rng, n):
 def fam_scaled(rng, k, na=1500, nb=2100):
     """FPFH-like descriptors scaled by 2^k: small k collapses every centred norm onto |mu|, large k stresses the margins."""
     s = np.float32(2.0 ** k)
-    return (_fpfh_like(rng, na) * s).astype(np.float32), (_fpfh_like(rng, nb) * s).astype(np.float32)
+    return (fpfh_like(rng, na) * s).astype(np.float32), (fpfh_like(rng, nb) * s).astype(np.float32)
 
 
 def fam_clustered(rng, n=8192, k=16):
@@ -90,7 +82,7 @@ def fam_collinear(rng, scale, n_sel=1024, m=6144):
 
 def fam_wide(rng, nb, na=2048, n_low=512):
     """nb columns, the true neighbours of most rows among the highest norms (column tiles >= 256 once nb > 16384)."""
-    B = _fpfh_like(rng, nb)
+    B = fpfh_like(rng, nb)
     hi = (MU + rng.uniform(400, 900, (na - n_low, 1)) * _unit(rng, na - n_low)).astype(np.float32)
     B[nb - len(hi):] = (hi + rng.normal(0, 0.5, hi.shape)).astype(np.float32)
     # 64 isolated columns above every other norm (tile 256 alone at nb = 16448): their own column bound keeps them from
@@ -105,7 +97,7 @@ def fam_equal_keys(rng, n_base=48, per=6, n_rows=1500):
     interleaved with bit-identical copies in index order P, Q, P, R, P, ...: dedup_kernel may only merge bit-identical runs."""
     free = np.array([d for d in range(33) if MU[d] == 0])
     cols = []
-    for base in _fpfh_like(rng, n_base):
+    for base in fpfh_like(rng, n_base):
         key = _norm_chain(base[None])[0]
         perms = []
         for _ in range(400):
@@ -120,7 +112,7 @@ def fam_equal_keys(rng, n_base=48, per=6, n_rows=1500):
         cols.append(base)
     cols.append(MU)        # the plane signature on both sides: its lower bound is exactly 0 = its exact distance
     B = np.array(cols, np.float32)
-    A = np.concatenate([B[rng.integers(0, len(B), n_rows // 2)], _fpfh_like(rng, n_rows - n_rows // 2)])
+    A = np.concatenate([B[rng.integers(0, len(B), n_rows // 2)], fpfh_like(rng, n_rows - n_rows // 2)])
     A[::3] = (A[::3] + rng.normal(0, 0.05, A[::3].shape)).astype(np.float32)
     A[1] = MU
     return A.astype(np.float32), B
@@ -128,7 +120,7 @@ def fam_equal_keys(rng, n_base=48, per=6, n_rows=1500):
 
 def fam_ulp(rng, na=1100, nb=1300):
     """1-ulp perturbations of one descriptor in random bins (none bit-identical): every entry is a near-tie."""
-    base = _fpfh_like(rng, 1)[0] + np.float32(1.0)
+    base = fpfh_like(rng, 1)[0] + np.float32(1.0)
     def cloud(n):
         x = np.tile(base, (n, 1))
         up = rng.random((n, 33)) < 0.3
@@ -139,7 +131,7 @@ def fam_ulp(rng, na=1100, nb=1300):
 
 def fam_nonfinite(rng, na=300, nb=400):
     """NaN / +-inf in one bin of a few rows and columns, and finite descriptors whose centred squared norm overflows."""
-    A, B = _fpfh_like(rng, na), _fpfh_like(rng, nb)
+    A, B = fpfh_like(rng, na), fpfh_like(rng, nb)
     A[3, 4] = np.nan; A[10, 7] = np.inf; A[11, 7] = -np.inf; A[12, 20] = np.inf
     B[5, 7] = np.inf; B[6, 0] = np.nan; B[8, 20] = -np.inf
     A[20] = 0; A[20, :2] = 2e19; B[30] = A[20]; B[30, 10] = 1.0           # exact distance 1, |x'|^2 = 8e38 overflows
@@ -166,12 +158,6 @@ def _mutual_from_tables(rb, cb):
         if j >= 0 and _idx(second[j]) == i:
             out.append((i, j))
     return np.array(out, np.int32).reshape(-1, 2)
-
-
-def _p4(rng, n):
-    out = np.ones((n, 4), np.float32)
-    out[:, :3] = rng.uniform(-30, 30, (n, 3))
-    return out
 
 
 def _table_diff(name, got, ref):
@@ -230,7 +216,8 @@ def test_oracle_tables_against_float64(oracle):
         _check_against_float64(A, B, rb, name + " rows", rng)
         _check_against_float64(B, A, cb, name + " cols", rng)
         # the mutual pairs derived from the tables are the ones match() lists
-        _, nm, _, mutual = oracle.match(_p4(rng, len(A)), A, _p4(rng, len(B)), B, p, want_mutual=True)
+        _, nm, _, mutual = oracle.match(P4(rng.uniform(-30, 30, (len(A), 3))), A, P4(rng.uniform(-30, 30, (len(B), 3))), B, p,
+                                        want_mutual=True)
         got = _mutual_from_tables(rb, cb)
         assert nm == len(got) and np.array_equal(got, mutual), name
 
@@ -254,7 +241,7 @@ def test_oracle_tables_power_of_two_invariance(oracle):
     def quant(x):
         q = np.round(x.astype(np.float64) * 1024.0) / 1024.0
         return np.where(q < 2.0 ** -10, 0.0, q).astype(np.float32)
-    A, B = quant(_fpfh_like(rng, 300)), quant(_fpfh_like(rng, 340))
+    A, B = quant(fpfh_like(rng, 300)), quant(fpfh_like(rng, 340))
     B[:40] = A[:40]
     B[40:80] = quant(A[40:80] + rng.normal(0, 0.01, (40, 33)))
     rb0, cb0 = oracle.nn_tables(A, B)
@@ -272,11 +259,9 @@ def test_oracle_tables_power_of_two_invariance(oracle):
 def handles():
     from quatro_b200.capi import Handle
     tc = Handle(max_batch_slots=2)
-    os.environ["QB200_MATCH_EXACT"] = "1"
-    try:
+    with pytest.MonkeyPatch.context() as mp:       # a module fixture has no monkeypatch of its own
+        mp.setenv("QB200_MATCH_EXACT", "1")
         ex = Handle(max_batch_slots=2)
-    finally:
-        del os.environ["QB200_MATCH_EXACT"]
     yield tc, ex
     tc.close()
     ex.close()
@@ -296,7 +281,7 @@ def _run_case(h, A, B, a4, b4, p, ref, want, label):
 
 def _both_paths(handles, oracle, A, B, label):
     rng = np.random.default_rng(len(A) * 7919 + len(B))
-    a4, b4 = _p4(rng, len(A)), _p4(rng, len(B))
+    a4, b4 = P4(rng.uniform(-30, 30, (len(A), 3))), P4(rng.uniform(-30, 30, (len(B), 3)))
     p = default_params()
     p.use_tuple_test = 0
     ref, want = oracle.nn_tables(A, B), oracle.match(a4, A, b4, B, p)
@@ -348,17 +333,14 @@ def test_nn_tables_collinear_near_ties(handles, oracle, scale):
 
 
 @pytest.mark.gpu
-def test_nn_tables_wide_column_counts(oracle):
+def test_nn_tables_wide_column_counts(oracle, monkeypatch):
     """Column counts around the scheduler's 256-tile shared-memory window (16384 columns) and far beyond it."""
     from quatro_b200.capi import Handle
     hs = []
     try:
         hs.append(Handle(max_batch_slots=2, max_voxel_points=40064))
-        os.environ["QB200_MATCH_EXACT"] = "1"
-        try:
-            hs.append(Handle(max_batch_slots=2, max_voxel_points=40064))
-        finally:
-            del os.environ["QB200_MATCH_EXACT"]
+        monkeypatch.setenv("QB200_MATCH_EXACT", "1")
+        hs.append(Handle(max_batch_slots=2, max_voxel_points=40064))
         for nb in (16384 - 64, 16384, 16384 + 64, 20000, 40000):
             A, B = fam_wide(np.random.default_rng(500 + nb), nb)
             _both_paths(hs, oracle, A, B, f"{len(A)} x {nb}")

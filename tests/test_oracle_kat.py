@@ -6,13 +6,7 @@ import pytest
 from conftest import adj_to_dense, dense_to_adj
 from quatro_b200 import synth
 from quatro_b200.capi import default_params, PMC_HEU, KCORE_HEU, COTE_WEIGHTED_MEAN
-
-
-def P4(xyz, w=1.0):
-    xyz = np.asarray(xyz, np.float32).reshape(-1, 3)
-    out = np.full((len(xyz), 4), w, np.float32)
-    out[:, :3] = xyz
-    return out
+from support import P4
 
 
 # ---- KAT-1 voxel ------------------------------------------------------------------------------

@@ -2,7 +2,6 @@
 inlier masks of every pair of qb200_register_batch_ex / _enqueue_ex, qb200_register_cached_ex and qb200_solve_batch_ex."""
 import ctypes as C
 import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -10,52 +9,14 @@ import pytest
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (Handle, ListBuffers, LIST_LAYOUT, SET_LISTS, FLAG_LISTS_TRUNCATED, MEM_HOST, MEM_DEVICE, PMC_EXACT,
                               INLIER_NONE, RESULT_DTYPE, default_params)
+from support import build_against_lib
 
-ROOT = Path(__file__).resolve().parent.parent
-
-
-# ---- CPU: ABI ---------------------------------------------------------------------------------------------------------------------
-def test_pair_lists_layout_matches_the_header(tmp_path):
-    src = tmp_path / "lists.c"
-    src.write_text('''
-#include <stddef.h>
-#include <stdio.h>
-#include "quatro_b200.h"
-#define O(f) printf("%s %zu\\n", #f, offsetof(qb200_pair_lists, f))
-int main(void) {
-  printf("sizeof %zu\\n", sizeof(qb200_pair_lists));
-  printf("flag %d\\n", (int)QB200_FLAG_LISTS_TRUNCATED);
-  O(cap_per_pair); O(kind); O(corr); O(src_matched4); O(tgt_matched4); O(clique); O(final_inliers); O(rot_inlier_mask);
-  O(trans_inlier_mask);
-  return 0;
-}
-''')
-    exe = tmp_path / "lists"
-    r = subprocess.run(["/usr/bin/gcc", "-std=c11", "-Wall", "-Werror", f"-I{ROOT / 'include'}", str(src), "-o", str(exe)],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    got = dict(ln.split() for ln in subprocess.run([str(exe)], capture_output=True, text=True).stdout.splitlines())
-    assert int(got.pop("sizeof")) == C.sizeof(capi.PairLists)
-    assert int(got.pop("flag")) == FLAG_LISTS_TRUNCATED
-    assert set(got) == {f for f, _ in capi.PairLists._fields_}
-    for f, off in got.items():
-        assert getattr(capi.PairLists, f).offset == int(off), f
-    assert set(LIST_LAYOUT) == set(got) - {"cap_per_pair", "kind"}
+FIXTURE = "tests/fixtures/pair_lists_shim.cpp"
 
 
-def build_fixture(tmp_path):
-    from quatro_b200 import _build
-    lib = _build.build_cuda()
-    exe = tmp_path / "pair_lists_shim"
-    cmd = ["/usr/bin/g++", "-std=c++17", "-Wall", "-Werror", f"-I{ROOT / 'include'}", str(ROOT / "tests" / "fixtures" / "pair_lists_shim.cpp"),
-           f"-L{lib.parent}", "-lquatro_b200", f"-Wl,-rpath,{lib.parent}", "-o", str(exe)]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return exe
-
-
+# ---- CPU: the C++ fixture builds ----------------------------------------------------------------------------------------------------
 def test_pair_lists_fixture_compiles(tmp_path):
-    exe = build_fixture(tmp_path)
+    exe = build_against_lib(tmp_path, FIXTURE)
     r = subprocess.run([str(exe)], capture_output=True, text=True)
     assert r.returncode == 2 and "usage" in r.stderr
 
@@ -317,7 +278,7 @@ def test_lists_cost_one_launch_per_wave_and_nothing_without(street):
 
 @pytest.mark.gpu
 def test_fixture_reads_inliers_of_a_sweep(tmp_path, street):
-    exe = build_fixture(tmp_path)
+    exe = build_against_lib(tmp_path, FIXTURE)
     scans = [street[0][0], street[0][1], street[2][1]]
     files = []
     for i, s in enumerate(scans):

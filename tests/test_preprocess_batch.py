@@ -3,53 +3,20 @@ in one call.  Every scan's four outputs, counts and status must be byte-identica
 on the same handle, and to the CPU oracle's chain, whatever the batch size, the wave, the scan's position, the memory kinds or the
 capacity per scan."""
 import ctypes as C
-import re
 import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 from quatro_b200 import capi, synth
 from quatro_b200.capi import MEM_DEVICE, MEM_HOST, PREPROCESS_ARRAYS, default_patchwork_params, default_segment_params
+from support import build_against_lib, same_bits
 
-ROOT = Path(__file__).resolve().parent.parent
 CANARY = np.uint32(0x7FC0DEAD)   # a NaN no kernel writes
 
 
-def test_preprocess_out_layout_matches_the_header(tmp_path):
-    src = tmp_path / "pp.c"
-    fields = [f for f, _ in capi.PreprocessOut._fields_]
-    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "quatro_b200.h"\nint main(void) {\n'
-                   '  printf("sizeof %zu\\n", sizeof(qb200_preprocess_out));\n' +
-                   "".join(f'  printf("{f} %zu\\n", offsetof(qb200_preprocess_out, {f}));\n' for f in fields) + "  return 0;\n}\n")
-    exe = tmp_path / "pp"
-    r = subprocess.run(["/usr/bin/gcc", "-std=c11", "-Wall", "-Werror", f"-I{ROOT / 'include'}", str(src), "-o", str(exe)],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    got = dict(ln.split() for ln in subprocess.run([str(exe)], capture_output=True, text=True).stdout.splitlines())
-    assert int(got.pop("sizeof")) == C.sizeof(capi.PreprocessOut)
-    for f in fields:
-        assert getattr(capi.PreprocessOut, f).offset == int(got[f]), f
-    # the header declares every field the mirror has, and nothing else
-    hdr = (ROOT / "include" / "quatro_b200.h").read_text()
-    body = hdr[hdr.index("typedef struct qb200_preprocess_out"):hdr.index("} qb200_preprocess_out;")]
-    assert re.findall(r"\*?\s*(\w+);", body) == fields
-
-
-def build_fixture(tmp_path):
-    from quatro_b200 import _build
-    lib = _build.build_cuda()
-    exe = tmp_path / "preprocess_batch_shim"
-    cmd = ["/usr/bin/g++", "-std=c++17", "-Wall", "-Werror", f"-I{ROOT / 'include'}", str(ROOT / "tests" / "fixtures" / "preprocess_batch_shim.cpp"),
-           f"-L{lib.parent}", "-lquatro_b200", f"-Wl,-rpath,{lib.parent}", "-o", str(exe)]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return exe
-
-
 def test_preprocess_batch_fixture_compiles(tmp_path):
-    exe = build_fixture(tmp_path)
+    exe = build_against_lib(tmp_path, "tests/fixtures/preprocess_batch_shim.cpp")
     r = subprocess.run([str(exe)], capture_output=True, text=True)
     assert r.returncode == 2 and "usage" in r.stderr
 
@@ -82,14 +49,6 @@ def _scene(seed, n_obj=20):
     return out[rng.permutation(len(out))]
 
 
-def _bits(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
-
-
-def _same(a, b):
-    return a.shape == b.shape and np.array_equal(_bits(a), _bits(b))
-
-
 def _single(h, scan, pp, sp):
     """The two single-scan calls: (ground, nonground, valid, outlier), counts, status."""
     g, ng, st = h.patchwork(scan, pp)
@@ -118,7 +77,7 @@ def _check_batch(h, scans, pp, sp, oracle=None, **kw):
                 if b is None:
                     assert counts[i][k] == 0
                     continue
-                assert _same(a, b), f"scan {i}: {PREPROCESS_ARRAYS[k]} differs"
+                assert same_bits(a, b), f"scan {i}: {PREPROCESS_ARRAYS[k]} differs"
     return per, counts, status
 
 
@@ -196,11 +155,11 @@ def test_shuffled_batch_gives_every_scan_the_same_bytes():
         per2, counts2, status2 = h.preprocess_batch([scans[i] for i in perm], pp, sp)
         for j, i in enumerate(perm):
             assert np.array_equal(counts2[j], counts[i]) and status2[j] == status[i]
-            assert all(_same(a, b) for a, b in zip(per2[j], per[i])), (i, j)
+            assert all(same_bits(a, b) for a, b in zip(per2[j], per[i])), (i, j)
         # one scan alone, and the batch again: nothing is left over from an earlier call or wave
         for i in (0, 10):
             one, c1, s1 = h.preprocess_batch([scans[i]], pp, sp)
-            assert np.array_equal(c1[0], counts[i]) and s1[0] == status[i] and all(_same(a, b) for a, b in zip(one[0], per[i]))
+            assert np.array_equal(c1[0], counts[i]) and s1[0] == status[i] and all(same_bits(a, b) for a, b in zip(one[0], per[i]))
 
 
 @pytest.mark.gpu
@@ -217,7 +176,7 @@ def test_host_and_device_inputs_and_outputs_give_the_same_bytes():
                 per, counts, status = h.preprocess_batch(inp, pp, sp, kind=kind, dest=dest)
                 assert np.array_equal(counts, rc) and np.array_equal(status, rs)
                 for i in range(len(scans)):
-                    assert all(_same(a, b) for a, b in zip(per[i], ref[i])), (kind, dest, i)
+                    assert all(same_bits(a, b) for a, b in zip(per[i], ref[i])), (kind, dest, i)
 
 
 @pytest.mark.gpu
@@ -240,7 +199,7 @@ def test_clipped_cap_keeps_prefixes_and_writes_nothing_past_it(dest):
         for i in range(n):
             for k, j in (("ground4", 0), ("valid4", 2)):
                 m = min(int(counts[i, j]), cap)
-                assert _same(got[k][i, :m], full[i][j][:m]), (i, k)
+                assert same_bits(got[k][i, :m], full[i][j][:m]), (i, k)
                 assert (got[k][i, m:].view(np.uint32) == CANARY).all(), (i, k, "written past the count or the cap")
             assert per[i][1] is None and per[i][3] is None
 

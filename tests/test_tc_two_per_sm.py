@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from quatro_b200 import _build
+from support import P4, fpfh_like
 
 DYN_SMEM = 100 * 1024        # A block (60 KB) + one operand stage (20 KB) + two exact-image stages (2 x 10 KB)
 SM_SMEM = 228 * 1024         # shared memory of an H100 SM
@@ -35,19 +36,6 @@ def test_tc_nn_kernel_fits_two_ctas_per_sm():
     assert 2 * (DYN_SMEM + use["SHARED"] + CTA_RESERVED) <= SM_SMEM, use
 
 
-def _p4(xyz):
-    out = np.ones((len(xyz), 4), np.float32)
-    out[:, :3] = xyz
-    return out
-
-
-def _fpfh_like(rng, n):
-    d = rng.gamma(0.3, 1.0, (n, 33)).astype(np.float32)
-    for t in range(3):
-        d[:, 11 * t:11 * t + 11] *= 100.0 / np.maximum(d[:, 11 * t:11 * t + 11].sum(1, keepdims=True), 1e-6)
-    return d.astype(np.float32)
-
-
 @pytest.mark.gpu
 def test_tc_footprint_two_ctas_per_sm(handle):
     fp = handle.debug_tc_footprint()
@@ -66,8 +54,8 @@ def test_match_at_tile_boundaries(handle, oracle, na):
     p.use_tuple_test = 0
     rng = np.random.default_rng(1000 + na)
     for nb in (1, 63, 64, 65, 127, 128, 129, 191):
-        a, b = _p4(rng.uniform(-20, 20, (na, 3))), _p4(rng.uniform(-20, 20, (nb, 3)))
-        ad, bd = _fpfh_like(rng, na), _fpfh_like(rng, nb)
+        a, b = P4(rng.uniform(-20, 20, (na, 3))), P4(rng.uniform(-20, 20, (nb, 3)))
+        ad, bd = fpfh_like(rng, na), fpfh_like(rng, nb)
         k = min(na, nb) // 3
         bd[:k] = ad[:k]                                   # exact duplicates -> zero distances and lowest-index ties
         ad[na - 1] = 0.0                                  # an isolated point: looks like the zero padding

@@ -6,7 +6,6 @@ Graphs above 8192 vertices keep the k-core and clique arrays in a per-pair globa
 computed once per module (the graph alone is 5e8 literal fp64 tests at L = 32768)."""
 import re
 import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -14,8 +13,7 @@ import pytest
 from quatro_b200 import synth
 from quatro_b200.capi import (COTE_WEIGHTED_MEAN, FLAG_CLIQUE_TRUNCATED, INLIER_NONE, KCORE_HEU, PMC_EXACT, PMC_HEU, RESULT_DTYPE, Handle,
                               QuatroB200Error, default_params)
-
-ROOT = Path(__file__).resolve().parent.parent
+from support import ROOT, assert_same_record, build_against_lib
 MAX_CORR = 32768
 GRAPH_SIZES = (8193, 12000, 20000, 32768)
 
@@ -43,19 +41,11 @@ def test_header_defines_the_limit():
     assert re.search(r"#define\s+QB200_MAX_CORR\s+32768\b", txt)
 
 
-def _build_fixture(tmp_path, name):
-    from quatro_b200 import _build
-    lib = _build.build_cuda()
-    exe = tmp_path / name
-    cmd = ["/usr/bin/g++", "-std=c++17", "-Wall", "-Werror", f"-I{ROOT / 'include'}", str(ROOT / "tests" / "fixtures" / f"{name}.cpp"),
-           f"-L{lib.parent}", "-lquatro_b200", f"-Wl,-rpath,{lib.parent}", "-o", str(exe)]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return exe
+FIXTURE = "tests/fixtures/wide_corr_shim.cpp"
 
 
 def test_wide_corr_shim_compiles(tmp_path):
-    _build_fixture(tmp_path, "wide_corr_shim")
+    build_against_lib(tmp_path, FIXTURE)
 
 
 # ---- graph helpers ---------------------------------------------------------------------------------------------------------
@@ -270,10 +260,6 @@ def _trans_mask_len(res, rot_inl):
     return res.n_rot_inliers if rot_inl and res.n_rot_inliers > 0 else res.clique_size
 
 
-def _rec_key(r):
-    return (r.valid, r.n_corr, r.max_core, r.n_edges, r.clique_size, r.gnc_iters, r.n_rot_inliers, r.n_final_inliers, r.flags)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("L", [4095, 4096, 4097, 6000, MAX_CORR])
 def test_pose_of_every_correspondence(h1, oracle, L):
@@ -288,15 +274,14 @@ def test_pose_of_every_correspondence(h1, oracle, L):
         r_g, st_g = h1.solve_correspondences(a4, b4, p)
         r_o, st_o, c_o, f_o = oracle.solve_correspondences(a4, b4, p, want_sets=True)
         assert st_g == st_o == 0 and r_g.clique_size == L
-        assert _rec_key(r_g) == _rec_key(r_o)
-        assert np.allclose(r_g.matrix(), r_o.matrix(), atol=1e-9, rtol=0)
+        assert_same_record(r_g, r_o)
         assert np.array_equal(h1.last_final_inliers(), f_o)
         clique = np.arange(L, dtype=np.int32)
         res_g, rm_g, tm_g, _ = h1.solve_pose(a4, b4, clique, p)
         res_o, rm_o, tm_o, _ = oracle.solve_pose(a4, b4, clique, p)
         n = _trans_mask_len(res_o, rot_inl)
         assert np.array_equal(rm_g, rm_o) and np.array_equal(tm_g[:n], tm_o[:n])
-        assert _rec_key(res_g) == _rec_key(res_o) and np.allclose(res_g.matrix(), res_o.matrix(), atol=1e-9, rtol=0)
+        assert_same_record(res_g, res_o)
 
 
 @pytest.mark.gpu
@@ -308,8 +293,7 @@ def test_pose_of_a_clique_above_4096(h1, oracle):
         r_g, st_g = h1.solve_correspondences(a4, b4, p)
         r_o, st_o, c_o, f_o = oracle.solve_correspondences(a4, b4, p, want_sets=True)
         assert st_g == st_o == 0 and r_o.clique_size > 4096
-        assert _rec_key(r_g) == _rec_key(r_o)
-        assert np.allclose(r_g.matrix(), r_o.matrix(), atol=1e-9, rtol=0)
+        assert_same_record(r_g, r_o)
         assert np.array_equal(h1.last_clique(), c_o) and np.array_equal(h1.last_final_inliers(), f_o)
         res_g, rm_g, tm_g, _ = h1.solve_pose(a4, b4, c_o, p)
         res_o, rm_o, tm_o, _ = oracle.solve_pose(a4, b4, c_o, p)
@@ -351,17 +335,14 @@ def test_register_hall_pair_without_tuple_test(h1, oracle):
     assert st_ref == 0 and 8192 < ref.n_corr <= MAX_CORR
     got, st = h1.register_pair(src, tgt, hall_params())
     assert st == 0 and got.valid == 1
-    key = lambda r: (r.n_src_vox, r.n_tgt_vox, r.n_mutual, r.n_corr, r.n_edges, r.max_core, r.clique_size, r.gnc_iters, r.n_rot_inliers,
-                     r.n_final_inliers, r.flags)
-    assert key(got) == key(ref)
-    assert np.allclose(got.matrix(), ref.matrix(), atol=1e-9, rtol=0)
+    assert_same_record(got, ref)
 
 
 # ---- 7. the C++ layer --------------------------------------------------------------------------------------------------------
 
 @pytest.mark.gpu
 def test_cpp_shim_grows_to_wide_sets(tmp_path, oracle):
-    exe = _build_fixture(tmp_path, "wide_corr_shim")
+    exe = build_against_lib(tmp_path, FIXTURE)
     a4, b4 = reg_set(10000, 61, 0.3)
     (tmp_path / "a.bin").write_bytes(np.ascontiguousarray(a4, np.float32).tobytes())
     (tmp_path / "b.bin").write_bytes(np.ascontiguousarray(b4, np.float32).tobytes())
