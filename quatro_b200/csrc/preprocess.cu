@@ -115,6 +115,21 @@ __global__ void __launch_bounds__(256) pw_scatter_kernel(const float4* const* __
   items[(size_t)s * R + pos] = ((unsigned long long)zb << 32) | (unsigned)i;
 }
 
+// D17 (oracle/preprocess_oracle.inc): unit vector of the smallest eigenvalue's eigenspace when the closed form's eigenvector is
+// undefined -- all points identical or on one line, every row of cov - lambda I parallel to one direction u.  (0,0,1) when it lies
+// in that eigenspace, else (u_y, -u_x, 0) normalised, or (1,0,0) for a vertical u.
+__device__ __forceinline__ void pw_degenerate_normal(const float cov[9], float ev, float e[3]) {
+  float m[9];
+  for (int i = 0; i < 9; ++i) m[i] = cov[i];
+  m[0] -= ev; m[4] -= ev; m[8] -= ev;
+  if (m[2] == 0.0f && m[5] == 0.0f && m[8] == 0.0f) { e[0] = 0.0f; e[1] = 0.0f; e[2] = 1.0f; return; }
+  const float l0 = qb_dot3(&m[0], &m[0]), l1 = qb_dot3(&m[3], &m[3]), l2 = qb_dot3(&m[6], &m[6]);
+  const float* u = (l0 >= l1 && l0 >= l2) ? &m[0] : (l1 >= l2 ? &m[3] : &m[6]);
+  const float h = sqrtf(u[0] * u[0] + u[1] * u[1]);
+  if (h > 0.0f) { e[0] = u[1] / h; e[1] = -u[0] / h; e[2] = 0.0f; }
+  else { e[0] = 1.0f; e[1] = 0.0f; e[2] = 0.0f; }
+}
+
 __device__ __forceinline__ void pw_plane_from_accu(float accu[9], int cnt, float n[3], float mean[3], float* surf) {
   const float fc = (float)cnt;
   for (int i = 0; i < 9; ++i) accu[i] /= fc;
@@ -128,6 +143,7 @@ __device__ __forceinline__ void pw_plane_from_accu(float accu[9], int cnt, float
   cov[3] = cov[1]; cov[6] = cov[2]; cov[7] = cov[5];
   float ev, e[3];
   qb_eigen33_smallest(cov, &ev, e);   // [EXT] Eigen::JacobiSVD in the reference (:267-271): closed form, oriented n_z >= 0
+  if (!(isfinite(e[0]) && isfinite(e[1]) && isfinite(e[2]))) pw_degenerate_normal(cov, ev, e);   // D17
   if (e[2] < 0.0f) { e[0] = -e[0]; e[1] = -e[1]; e[2] = -e[2]; }
   const float tr = cov[0] + cov[4] + cov[8];
   *surf = (tr != 0.0f) ? fabsf(ev / tr) : 0.0f;
