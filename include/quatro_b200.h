@@ -20,6 +20,7 @@
  *   qb200_register_batch_sharded / _rank  <- the same loop over a list of pairs, sharded over the GPUs of one box
  *   qb200_pair_lists (_ex forms) <- FPFHManager::getCorrespondences, Quatro::getMaxCliques / getFinalInliersIndices for every
  *                                  pair of a batch (examples/run_global_registration.cpp:268, 292)
+ *   qb200_*_each                <- one Quatro object per pair: Quatro::reset(Params) + setPreEstaimatedRyRx for every pair of a batch
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -335,7 +336,7 @@ typedef struct qb200_pair_lists {
   int32_t* clique;            /* [n][cap] ascending correspondence ids = qb200_get_last_clique (getMaxCliques) */
   int32_t* final_inliers;     /* [n][cap] = qb200_get_last_final_inliers (getFinalInliersIndices) */
   uint8_t* rot_inlier_mask;   /* [n][cap] per clique member, as qb200_solve_pose writes it */
-  uint8_t* trans_inlier_mask; /* [n][cap] */
+  uint8_t* trans_inlier_mask; /* [n][cap]; a translation estimated from the rotation inliers only leaves 0 past n_rot_inliers */
 } qb200_pair_lists;           /* any array may be NULL: nothing is written to it */
 enum { QB200_FLAG_LISTS_TRUNCATED = 2 /* a list of this pair had more than cap_per_pair entries */ };
 
@@ -394,6 +395,36 @@ int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t
 int qb200_register_cached_ex(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p,
                              qb200_result* results, const qb200_pair_lists* lists);
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot);   /* swapTgt2Src */
+
+/* --- per-pair solver parameters: one batch, N independently configured Quatro objects ---------------------------------------------
+ * The reference configures each Quatro object on its own (reset(Params), include/quatro.hpp:202-268, 755-765) and gives it the IMU
+ * roll/pitch of its scan (setPreEstaimatedRyRx, :276-279, applied at :419-426 and :891-893).  The _each forms take the same arguments
+ * as their _ex siblings, except that `params` points to n entries, one per pair (or correspondence set) in the order of the input
+ * array.  The array is copied by the call; `lists` may be NULL.
+ *   Solver fields (noise_bound .. RyRx: noise_bound, cbar2, rot_noise_bound, cote_noise_bound, rotation_gnc_factor,
+ *     rotation_cost_threshold, kcore_heuristic_threshold, rotation_max_iterations, inlier_selection_mode, cote_mode,
+ *     using_rot_inliers_when_estimating_cote, use_pre_estimated_RyRx, max_clique_node_limit, RyRx) may differ from pair to pair.
+ *   Front-end fields (voxel_size .. seed: the FPFHManager / voxelize configuration) must be bit-identical in every entry of
+ *     qb200_register_batch_each, _enqueue_each and qb200_register_cached_each (cached slots are bound to one set of them);
+ *     qb200_solve_batch_each ignores them.
+ *   Every entry must pass the checks of the _ex call; a bad entry or a front-end mismatch fails the whole call with QB200_ERR_BAD_ARG
+ *     before any work starts, and no record or list is written.
+ *   Pair i's record and lists are byte-identical to pair i of the _ex call made with params[i] for the whole batch (results never
+ *     depend on the batch, the wave or the lane).
+ *   Entries with rot_noise_bound == 0 are resolved in pair order through the handle's latch, as if the single-pair calls had been made
+ *     in that order: on a handle that has not latched yet, the first such entry latches 2 * its noise_bound. */
+/* qb200_register_batch_ex with one params entry per pair */
+int qb200_register_batch_each(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
+                              qb200_result* results, const qb200_pair_lists* lists);
+/* qb200_register_batch_enqueue_ex with one params entry per pair; completed by qb200_register_batch_flush like every enqueue */
+int qb200_register_batch_enqueue_each(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                      qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+/* qb200_register_cached_ex with one params entry per slot pair (front-end fields: the ones the slots were cached with) */
+int qb200_register_cached_each(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                               qb200_result* results, const qb200_pair_lists* lists);
+/* qb200_solve_batch_ex with one params entry per correspondence set (front-end fields ignored) */
+int qb200_solve_batch_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params, qb200_mem_kind kind,
+                           qb200_result* results, const qb200_pair_lists* lists);
 /* read a cached scan back: voxel points (n x 4), normals (n x {nx,ny,nz,curvature}), descriptors (n x 33); any may be NULL */
 int qb200_cache_read(qb200_handle* h, int32_t slot, float* vox4, float* normals4, float* desc33, int32_t cap, int32_t* n);
 

@@ -249,6 +249,10 @@ def load_library(build: bool = True) -> C.CDLL:
         "qb200_register_cached_ex": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
         "qb200_solve_batch_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
         "qb200_preprocess_batch": (i32, [vp, vp, vp, i32, i32, P(PatchworkParams), P(SegmentParams), P(PreprocessOut)]),
+        "qb200_register_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+        "qb200_register_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+        "qb200_register_cached_each": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
+        "qb200_solve_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError = header/library mismatch: fail loudly
@@ -277,6 +281,7 @@ EXPORTED_SYMBOLS = [
     "qb200_debug_match_verify", "qb200_get_last_features", "qb200_cache_reserve", "qb200_cache_scans", "qb200_register_cached", "qb200_cache_copy", "qb200_cache_read",
     "qb200_register_batch_ex", "qb200_register_batch_enqueue_ex", "qb200_register_cached_ex", "qb200_solve_batch_ex",
     "qb200_preprocess_batch",
+    "qb200_register_batch_each", "qb200_register_batch_enqueue_each", "qb200_register_cached_each", "qb200_solve_batch_each",
 ]
 
 
@@ -631,6 +636,52 @@ class Handle:
         self._check(self.lib.qb200_solve_batch_ex(self.h, arr, len(sets), C.byref(params), kind, _ptr(out), C.byref(d)),
                     "qb200_solve_batch_ex")
         return out, lb.trimmed(out)
+
+    # ---- one Params per pair (the _each entry points) ----
+    # params: one Params per pair (or set), in the order of the inputs.  buffers: the ListBuffers to fill, or None for records only.
+    # Each returns (records, lists): lists as ListBuffers.trimmed, None without buffers.
+    @staticmethod
+    def params_array(params: Sequence[Params]):
+        """(Params * n) array of `params` (at least one element, so that n = 0 still passes a valid pointer)."""
+        return (Params * max(len(params), 1))(*params)
+
+    @staticmethod
+    def _lists_arg(buffers: Optional[ListBuffers]):
+        return None if buffers is None else C.byref(buffers.descriptor())
+
+    def register_batch_each(self, pairs: Sequence, params: Sequence[Params], kind: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
+        """qb200_register_batch_each: pair i is registered with params[i] (front-end fields equal in every entry)."""
+        assert len(params) == len(pairs)
+        arr, keep = self.pair_array(pairs, kind)
+        out = np.zeros(len(pairs), RESULT_DTYPE)
+        self._check(self.lib.qb200_register_batch_each(self.h, arr, len(pairs), self.params_array(params), kind, _ptr(out),
+                                                       self._lists_arg(buffers)), "qb200_register_batch_each")
+        return out, (None if buffers is None else buffers.trimmed(out))
+
+    def register_batch_enqueue_each_raw(self, pair_array, n: int, params_array, kind: int, out: np.ndarray,
+                                        buffers: Optional[ListBuffers] = None):
+        """qb200_register_batch_enqueue_each: params_array (params_array()) is copied by the call; pair_array, its scans, `out` and the
+        buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_register_batch_enqueue_each(self.h, pair_array, n, params_array, kind, _ptr(out),
+                                                                      self._lists_arg(buffers)), "qb200_register_batch_enqueue_each")
+
+    def register_cached_each(self, slot_pairs, params: Sequence[Params], buffers: Optional[ListBuffers] = None):
+        """qb200_register_cached_each: slot pair i is registered with params[i] (front-end fields: the ones the slots were cached with)."""
+        sp = np.ascontiguousarray(np.asarray(slot_pairs, np.int32).reshape(-1, 2))
+        assert len(params) == len(sp)
+        out = np.zeros(len(sp), RESULT_DTYPE)
+        self._check(self.lib.qb200_register_cached_each(self.h, _ptr(sp), len(sp), self.params_array(params), _ptr(out),
+                                                        self._lists_arg(buffers)), "qb200_register_cached_each")
+        return out, (None if buffers is None else buffers.trimmed(out))
+
+    def solve_batch_each(self, sets: Sequence, params: Sequence[Params], kind: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
+        """qb200_solve_batch_each: set i is solved with params[i] (front-end fields ignored)."""
+        assert len(params) == len(sets)
+        arr, keep = self._set_array(sets, kind)
+        out = np.zeros(len(sets), RESULT_DTYPE)
+        self._check(self.lib.qb200_solve_batch_each(self.h, arr, len(sets), self.params_array(params), kind, _ptr(out),
+                                                    self._lists_arg(buffers)), "qb200_solve_batch_each")
+        return out, (None if buffers is None else buffers.trimmed(out))
 
     def last_features(self, which: int, cap: Optional[int] = None):
         """(normals (n,4), descriptors (n,33)) of the source (0) / target (1) cloud of the last match_and_pack."""

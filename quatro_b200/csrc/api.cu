@@ -1,6 +1,7 @@
 // api.cu -- the C-ABI of include/quatro_b200.h: handle lifetime, lanes, waves, pair lists, the scan cache and the batch entry
 // points.  The single-pair stage entry points, the qb200_get_last_* getters and the debug hooks are in stages.cu.
 #include <new>
+#include <stddef.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -146,6 +147,8 @@ int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   QB_CUDA_TRY(L, L->final_inl.alloc(S * Lc));
   QB_CUDA_TRY(L, L->rot_mask.alloc(S * Lc));
   QB_CUDA_TRY(L, L->trans_mask.alloc(S * Lc));
+  QB_CUDA_TRY(L, L->d_solve.alloc(S));
+  QB_CUDA_TRY(L, L->h_solve.alloc(S));
   // workspaces of the pairs whose graph or clique outgrows the shared-memory layouts (clique.cu, pose.cu); only wide handles have them
   if (Lc > (size_t)kKcoreSmemVerts) {
     QB_CUDA_TRY(L, L->kcore_ws.alloc(S * kcore_ws_bytes((int)Lc)));
@@ -232,20 +235,44 @@ void set_last(qb200_handle* h, const qb200_result& r) {
   h->last_n_final = r.n_final_inliers;
 }
 
-// graph -> clique -> pose for pairs [0, n) whose matched points / n_corr are already on the device
-int run_solver(Lane* L, int n_pairs, const qb200_params& p, int have_frontend) {
-  int rc;
-  if (p.inlier_selection_mode == QB200_INLIER_NONE) {
-    // the reference leaves max_clique_ empty in this mode (quatro.hpp:782); TEASER++ semantics: all measurements
-    if ((rc = launch_iota_clique(L, n_pairs))) return rc;
-  } else {
-    if ((rc = launch_graph(L, n_pairs, p.noise_bound, p.cbar2))) return rc;
-    if (L->ev[5]) cudaEventRecord(L->ev[5], L->stream);
-    if ((rc = launch_clique(L, n_pairs, p.inlier_selection_mode, p.kcore_heuristic_threshold, p.max_clique_node_limit))) return rc;
+PairSolve solve_entry(const qb200_params& p) {
+  PairSolve e;
+  memset(&e, 0, sizeof(e));
+  e.gc = graph_const(p.noise_bound, p.cbar2);
+  e.pp = pose_params(p);
+  e.kcore_thr = p.kcore_heuristic_threshold;
+  e.node_limit = p.max_clique_node_limit > 0 ? p.max_clique_node_limit : (long long)QB200_DEFAULT_CLIQUE_NODE_LIMIT;
+  e.mode = p.inlier_selection_mode;
+  return e;
+}
+
+int upload_solve(Lane* L, int n) {
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_solve, L->h_solve, (size_t)n * sizeof(PairSolve), cudaMemcpyHostToDevice, L->stream));
+  return QB200_OK;
+}
+
+// graph -> clique -> pose for pairs [0, n) whose matched points / n_corr are already on the device and whose solver entries are in
+// L->h_solve and (upload_solve) L->d_solve.  The host reads the wave's modes from the table and launches only what they need: no K8 / K9
+// when every pair is in QB200_INLIER_NONE, no exact search without a PMC_EXACT pair, no iota clique without a QB200_INLIER_NONE pair.
+int run_solver(Lane* L, int n_pairs, int have_frontend) {
+  bool graph = false, none = false, exact = false;
+  for (int s = 0; s < n_pairs; ++s) {
+    const int m = L->h_solve[s].mode;
+    graph |= m != QB200_INLIER_NONE;
+    none |= m == QB200_INLIER_NONE;
+    exact |= m == QB200_PMC_EXACT;
   }
+  int rc;
+  if (graph) {
+    if ((rc = launch_graph(L, n_pairs))) return rc;
+    if (L->ev[5]) cudaEventRecord(L->ev[5], L->stream);
+    if ((rc = launch_clique(L, n_pairs, exact))) return rc;
+  }
+  // the reference leaves max_clique_ empty in INLIER_NONE (quatro.hpp:782); TEASER++ semantics: all measurements
+  if (none && (rc = launch_iota_clique(L, n_pairs))) return rc;
   if (L->ev[6]) cudaEventRecord(L->ev[6], L->stream);
   if ((rc = launch_fill_counters(L, n_pairs, have_frontend))) return rc;
-  if ((rc = launch_pose(L, n_pairs, p))) return rc;
+  if ((rc = launch_pose(L, n_pairs))) return rc;
   if ((rc = launch_finalize_status(L, n_pairs))) return rc;
   return QB200_OK;
 }
@@ -322,6 +349,10 @@ struct WaveInput {
   cudaStream_t copy_stream = nullptr;
   // the batch's per-pair lists (qb200_pair_lists), nullptr = records only
   const qb200_pair_lists* lists = nullptr;
+  // the params the pairs are solved with, rotation noise bounds resolved: one entry for the whole batch, or (each) one per pair.  The
+  // front end reads params[0]: the front-end fields of every entry are equal.
+  const qb200_params* params = nullptr;
+  bool each = false;
 };
 
 // Host-kind lists: the lane's pinned staging block holds cap entries of every list for each slot.  It only grows, and a failed
@@ -399,10 +430,21 @@ int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
 // Enqueue one wave (pairs [w0, w0 + np), np <= S) on lane L: the front of the wave its input needs (raw scans: H2D, K1..K6;
 // cached scans: the copy out of the cache, K6; correspondence sets: their H2D), then K8..K11 and the D2H of the result records.
 // No sync: wave_collect hands the records out to dst[w0...].  The lane's previous wave must have been collected.
-int wave_submit(qb200_handle* h, Lane* L, const WaveInput& in, int w0, int np, const qb200_params& p, qb200_result* dst) {
+int wave_submit(qb200_handle* h, Lane* L, const WaveInput& in, int w0, int np, qb200_result* dst) {
   const int ncl = 2 * np;
+  const qb200_params& p = in.params[0];
   int rc;
   L->kev_armed[0] = L->kev_armed[1] = 0;
+  // the wave's solver table (the lane's previous wave has been collected: its pinned mirror is free), copied before anything else of
+  // the wave: on a stream of host batches the copy engine carries the scans, and a copy queued ahead of this wave's scans only waits
+  // for the earlier waves' scans, which the lane waits for anyway
+  if (in.each) {
+    for (int s = 0; s < np; ++s) L->h_solve[s] = solve_entry(in.params[w0 + s]);
+  } else {
+    const PairSolve e = solve_entry(p);
+    for (int s = 0; s < np; ++s) L->h_solve[s] = e;
+  }
+  if ((rc = upload_solve(L, np))) return rc;
   if (in.pairs) {
     cudaEventRecord(L->ev[0], L->stream);
     for (int s = 0; s < np; ++s) {
@@ -448,7 +490,7 @@ int wave_submit(qb200_handle* h, Lane* L, const WaveInput& in, int w0, int np, c
   if (!in.sets && (rc = launch_match(L, np, p))) return rc;
   cudaEventRecord(L->ev[4], L->stream);
   cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
-  if ((rc = run_solver(L, np, p, in.sets ? 0 : 1))) return rc;
+  if ((rc = run_solver(L, np, in.sets ? 0 : 1))) return rc;
   cudaEventRecord(L->ev[7], L->stream);
   if (in.lists && (rc = submit_lists(L, *in.lists, w0, np))) return rc;
   QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
@@ -520,16 +562,197 @@ int batch_flush(qb200_handle* h) {
 }
 
 // one wave at a time on lane 0, each collected before the next is submitted
-int run_waves(qb200_handle* h, const WaveInput& in, int n, const qb200_params& p, qb200_result* results) {
+int run_waves(qb200_handle* h, const WaveInput& in, int n, qb200_result* results) {
   reset_timers(h);
   const int S = h->cfg.max_batch_slots;
   for (int w0 = 0; w0 < n; w0 += S) {
-    int rc = wave_submit(h, h->lane[0].get(), in, w0, n - w0 < S ? n - w0 : S, p, results);
+    int rc = wave_submit(h, h->lane[0].get(), in, w0, n - w0 < S ? n - w0 : S, results);
     if (rc == QB200_OK) rc = wave_collect(h, h->lane[0].get());
     if (rc) return rc;
   }
   if (n == 1) set_last(h, results[0]);
   return QB200_OK;
+}
+
+// The params of a call: one entry for the whole batch, or (each) one per pair (n entries; NULL is fine when n == 0).  Every entry passes
+// params_ok; same_frontend: the call runs a front end or matches cached scans, so every entry carries the first entry's front-end
+// fields (voxel_size .. seed, bit for bit).
+int check_params(qb200_handle* h, const qb200_params* p, int n, bool each, bool same_frontend) {
+  const int m = each ? n : 1;
+  for (int i = 0; i < m; ++i) {
+    if (!params_ok(p ? p + i : nullptr)) {
+      h->fail(__FILE__, __LINE__, each ? "a params entry is null or out of range" : "params are null or out of range");
+      return QB200_ERR_BAD_ARG;
+    }
+    if (same_frontend && i > 0 && memcmp(p + i, p, offsetof(qb200_params, noise_bound)) != 0) {
+      h->fail(__FILE__, __LINE__, "params entries differ in their front-end fields (voxel_size .. seed)");
+      return QB200_ERR_BAD_ARG;
+    }
+  }
+  return QB200_OK;
+}
+
+// The entries of a checked call with their rotation noise bounds resolved (resolve_params): the one entry, or every pair's in pair
+// order, as a sequence of single-pair calls in that order would latch them.  Empty on an allocation failure.
+std::unique_ptr<qb200_params[]> resolve_call(qb200_handle* h, const qb200_params* p, int n, bool each) {
+  const int m = each ? n : 1;
+  std::unique_ptr<qb200_params[]> r(new (std::nothrow) qb200_params[m > 0 ? m : 1]);
+  if (!r) {
+    h->fail(__FILE__, __LINE__, "out of host memory for the params");
+    return r;
+  }
+  for (int i = 0; i < m; ++i) r[i] = resolve_params(h, p[i]);
+  return r;
+}
+
+int solve_batch_impl(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p, bool each, qb200_mem_kind kind,
+                     qb200_result* results, const qb200_pair_lists* lists) {
+  if (int rc = enter(h)) return rc;
+  if (n_sets < 0 || (n_sets > 0 && (!sets || !results))) return QB200_ERR_BAD_ARG;
+  if (int rc = check_params(h, p, n_sets, each, false)) return rc;
+  if (int rc = check_lists(h, lists, true)) return rc;
+  for (int i = 0; i < n_sets; ++i)
+    if (sets[i].L < 0 || sets[i].L > h->cfg.max_corr || (sets[i].L > 0 && (!sets[i].a || !sets[i].b))) {
+      h->fail(__FILE__, __LINE__, "correspondence set is null or exceeds max_corr");
+      return QB200_ERR_BAD_ARG;
+    }
+  WaveInput in;
+  in.sets = sets;
+  in.kind = kind;
+  in.lists = lists;
+  in.each = each;
+  if (n_sets == 0) return run_waves(h, in, 0, results);
+  const std::unique_ptr<qb200_params[]> pr = resolve_call(h, p, n_sets, each);
+  if (!pr) return QB200_ERR_CUDA;
+  in.params = pr.get();
+  return run_waves(h, in, n_sets, results);
+}
+
+// Queue a batch and return: waves rotate over the lanes, a lane is collected (its records copied out) only when it is needed
+// again, so the tail of one batch runs under the copies and front-end kernels of the next.  pairs' scans (host kind) and
+// `results` must stay valid until qb200_register_batch_flush (or a later enqueue / qb200_register_batch) has returned them.
+int enqueue_impl(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, bool each, qb200_mem_kind kind,
+                 qb200_result* results, const qb200_pair_lists* lists) {
+  if (!h || n_pairs < 0 || (n_pairs > 0 && (!pairs || !results))) return QB200_ERR_BAD_ARG;
+  if (int rc = check_params(h, p, n_pairs, each, true)) return rc;
+  if ((!each || n_pairs > 0) && !p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
+  if (int rc = check_lists(h, lists, false)) return rc;
+  const int S = h->cfg.max_batch_slots, R = h->cfg.max_raw_points;
+  for (int i = 0; i < n_pairs; ++i) {
+    if (pairs[i].n_src < 0 || pairs[i].n_tgt < 0 || pairs[i].n_src > R || pairs[i].n_tgt > R ||
+        (pairs[i].n_src > 0 && !pairs[i].src) || (pairs[i].n_tgt > 0 && !pairs[i].tgt)) {
+      h->fail(__FILE__, __LINE__, "pair has a null cloud or exceeds max_raw_points");
+      return QB200_ERR_BAD_ARG;
+    }
+  }
+  cudaSetDevice(h->cfg.device);
+  const bool pipelined = h->lanes_active > 0;  // waves of an earlier enqueue are still in flight
+  if (!pipelined) reset_timers(h);
+  const std::unique_ptr<qb200_params[]> pr = resolve_call(h, p, n_pairs, each);
+  if (!pr) return QB200_ERR_CUDA;
+  // More than one wave: rotate over the lanes so that one wave's PCIe copies and single-warp solver tail run under the
+  // other waves' dense kernels.  Results do not depend on the lane (no state is shared between waves).
+  // Wave plan.  Host inputs: nothing can run before the first wave's scans crossed PCIe, so the batch opens with a quarter
+  // wave (its copy is the only one that is not hidden) followed by the remaining three quarters; all other waves are full.
+  // (Closing with small waves as well does not pay: every wave carries the same single-warp solver tail.)
+  int wave_n[64], n_waves = 0;
+  {
+    int left = n_pairs;
+    if (kind == QB200_MEM_HOST && n_pairs > S && S >= 8 && h->max_lanes > 1) {
+      wave_n[n_waves++] = S / 4;
+      wave_n[n_waves++] = S - S / 4;
+      left -= S;
+    }
+    while (left > 0 && n_waves < 63) {
+      wave_n[n_waves] = left < S ? left : S;
+      left -= wave_n[n_waves++];
+    }
+    if (left > 0) n_waves = 0;  // more than ~60 waves: no special opening, walk uniformly below
+  }
+  const bool planned = n_waves > 0;
+  if (!planned) n_waves = (n_pairs + S - 1) / S;
+  int n_lanes = n_waves < h->max_lanes ? (n_waves < 1 ? 1 : n_waves) : h->max_lanes;
+  if (pipelined && h->lanes_active != n_lanes) {  // a different lane count: start a fresh rotation
+    const int rc0 = batch_flush(h);
+    if (rc0) return rc0;
+  }
+  const bool fresh = h->lanes_active == 0;
+  for (int l = 1; l < n_lanes; ++l) {
+    if (!h->lane[l]) {
+      const int rc = lane_alloc(*h->lane[0], &h->lane[l]);
+      if (rc != QB200_OK) {
+        h->fail(__FILE__, __LINE__, "cannot allocate another lane");
+        return rc;
+      }
+    }
+    // the lanes start after whatever the caller queued on lane 0's stream (first batch of a pipelined sequence only: later
+    // on lane 0's stream carries a wave of its own)
+    if (fresh) {
+      if (l == 1) QB_CUDA_TRY(h, cudaEventRecord(h->ev_fork, h->lane[0]->stream));
+      QB_CUDA_TRY(h, cudaStreamWaitEvent(h->lane[l]->stream, h->ev_fork, 0));
+    }
+  }
+  WaveInput in;
+  in.pairs = pairs;
+  in.kind = kind;
+  in.lists = lists;
+  in.params = pr.get();
+  in.each = each;
+  // host scans of a multi-wave batch: one copy stream, ordered after whatever the caller queued on lane 0's stream
+  if (kind == QB200_MEM_HOST && n_lanes > 1) {
+    in.copy_stream = h->copy_stream;
+    if (fresh) QB_CUDA_TRY(h, cudaStreamWaitEvent(in.copy_stream, h->ev_fork, 0));
+  }
+  h->lanes_active = n_lanes;
+  int rc = QB200_OK, wave = 0;
+  for (int w0 = 0; w0 < n_pairs && rc == QB200_OK; ++wave) {
+    Lane* L = h->lane[h->lane_cursor].get();
+    int np = planned ? wave_n[wave] : S;
+    if (np > n_pairs - w0) np = n_pairs - w0;
+    if ((rc = wave_collect(h, L))) break;  // the lane's previous wave (its pinned tables are reused)
+    rc = wave_submit(h, L, in, w0, np, results);
+    h->lane_cursor = (h->lane_cursor + 1) % n_lanes;  // always the lane that has been busy longest
+    w0 += np;
+  }
+  return rc;
+}
+
+int register_batch_impl(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, bool each, qb200_mem_kind kind,
+                        qb200_result* results, const qb200_pair_lists* lists) {
+  int rc = enqueue_impl(h, pairs, n_pairs, p, each, kind, results, lists);
+  const int rc2 = h ? batch_flush(h) : QB200_OK;  // on an error still wait for everything in flight (the copies read caller memory)
+  if (rc == QB200_OK) rc = rc2;
+  if (rc != QB200_OK) return rc;
+  if (n_pairs == 1) set_last(h, results[0]);
+  return QB200_OK;
+}
+
+int register_cached_impl(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, bool each,
+                         qb200_result* results, const qb200_pair_lists* lists) {
+  if (int rc = enter(h)) return rc;
+  if (n_pairs < 0 || (n_pairs > 0 && (!pairs || !results))) return QB200_ERR_BAD_ARG;
+  if (int rc = check_params(h, p, n_pairs, each, true)) return rc;
+  if ((!each || n_pairs > 0) && !p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
+  if (int rc = check_lists(h, lists, false)) return rc;
+  for (int i = 0; i < n_pairs; ++i) {
+    const int sl[2] = {pairs[i].src_slot, pairs[i].tgt_slot};
+    for (int k = 0; k < 2; ++k) {
+      if (sl[k] < 0 || sl[k] >= h->c_slots) { h->fail(__FILE__, __LINE__, "slot outside qb200_cache_reserve()"); return QB200_ERR_BAD_ARG; }
+      const float* sig = h->c_sig.get() + 4 * (size_t)sl[k];
+      if (sig[0] != p->voxel_size || sig[1] != p->normal_radius || sig[2] != p->fpfh_radius || sig[3] != lattice_cell(*p)) {
+        h->fail(__FILE__, __LINE__, "cached scan was computed with other front-end parameters (or the slot is empty)");
+        return QB200_ERR_BAD_ARG;
+      }
+    }
+  }
+  const std::unique_ptr<qb200_params[]> pr = resolve_call(h, p, n_pairs, each);
+  if (!pr) return QB200_ERR_CUDA;
+  WaveInput in;
+  in.slots = pairs;
+  in.lists = lists;
+  in.params = pr.get();
+  in.each = each;
+  return run_waves(h, in, n_pairs, results);
 }
 
 }  // namespace
@@ -634,19 +857,12 @@ int qb200_solve_batch(qb200_handle* h, const qb200_corr_set* sets, int32_t n_set
 
 int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p, qb200_mem_kind kind,
                          qb200_result* results, const qb200_pair_lists* lists) {
-  if (int rc = enter(h)) return rc;
-  if (n_sets < 0 || (n_sets > 0 && (!sets || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
-  if (int rc = check_lists(h, lists, true)) return rc;
-  for (int i = 0; i < n_sets; ++i)
-    if (sets[i].L < 0 || sets[i].L > h->cfg.max_corr || (sets[i].L > 0 && (!sets[i].a || !sets[i].b))) {
-      h->fail(__FILE__, __LINE__, "correspondence set is null or exceeds max_corr");
-      return QB200_ERR_BAD_ARG;
-    }
-  WaveInput in;
-  in.sets = sets;
-  in.kind = kind;
-  in.lists = lists;
-  return run_waves(h, in, n_sets, n_sets > 0 ? resolve_params(h, *p) : *p, results);
+  return solve_batch_impl(h, sets, n_sets, p, false, kind, results, lists);
+}
+
+int qb200_solve_batch_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params, qb200_mem_kind kind,
+                           qb200_result* results, const qb200_pair_lists* lists) {
+  return solve_batch_impl(h, sets, n_sets, params, true, kind, results, lists);
 }
 
 // ---- raw scans -> pose ------------------------------------------------------------------------------
@@ -659,102 +875,27 @@ int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pai
 
 int qb200_register_batch_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                             qb200_result* results, const qb200_pair_lists* lists) {
-  int rc = qb200_register_batch_enqueue_ex(h, pairs, n_pairs, p, kind, results, lists);
-  const int rc2 = h ? batch_flush(h) : QB200_OK;  // on an error still wait for everything in flight (the copies read caller memory)
-  if (rc == QB200_OK) rc = rc2;
-  if (rc != QB200_OK) return rc;
-  if (n_pairs == 1) set_last(h, results[0]);
-  return QB200_OK;
+  return register_batch_impl(h, pairs, n_pairs, p, false, kind, results, lists);
 }
 
-// Queue a batch and return: waves rotate over the lanes, a lane is collected (its records copied out) only when it is needed
-// again, so the tail of one batch runs under the copies and front-end kernels of the next.  pairs' scans (host kind) and
-// `results` must stay valid until qb200_register_batch_flush (or a later enqueue / qb200_register_batch) has returned them.
+int qb200_register_batch_each(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
+                              qb200_result* results, const qb200_pair_lists* lists) {
+  return register_batch_impl(h, pairs, n_pairs, params, true, kind, results, lists);
+}
+
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                                  qb200_result* results) {
-  return qb200_register_batch_enqueue_ex(h, pairs, n_pairs, p, kind, results, nullptr);
+  return enqueue_impl(h, pairs, n_pairs, p, false, kind, results, nullptr);
 }
 
 int qb200_register_batch_enqueue_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                                     qb200_result* results, const qb200_pair_lists* lists) {
-  if (!h || n_pairs < 0 || (n_pairs > 0 && (!pairs || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
-  if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
-  if (int rc = check_lists(h, lists, false)) return rc;
-  const int S = h->cfg.max_batch_slots, R = h->cfg.max_raw_points;
-  for (int i = 0; i < n_pairs; ++i) {
-    if (pairs[i].n_src < 0 || pairs[i].n_tgt < 0 || pairs[i].n_src > R || pairs[i].n_tgt > R ||
-        (pairs[i].n_src > 0 && !pairs[i].src) || (pairs[i].n_tgt > 0 && !pairs[i].tgt)) {
-      h->fail(__FILE__, __LINE__, "pair has a null cloud or exceeds max_raw_points");
-      return QB200_ERR_BAD_ARG;
-    }
-  }
-  cudaSetDevice(h->cfg.device);
-  const bool pipelined = h->lanes_active > 0;  // waves of an earlier enqueue are still in flight
-  if (!pipelined) reset_timers(h);
-  const qb200_params pr = resolve_params(h, *p);
-  // More than one wave: rotate over the lanes so that one wave's PCIe copies and single-warp solver tail run under the
-  // other waves' dense kernels.  Results do not depend on the lane (no state is shared between waves).
-  // Wave plan.  Host inputs: nothing can run before the first wave's scans crossed PCIe, so the batch opens with a quarter
-  // wave (its copy is the only one that is not hidden) followed by the remaining three quarters; all other waves are full.
-  // (Closing with small waves as well does not pay: every wave carries the same single-warp solver tail.)
-  int wave_n[64], n_waves = 0;
-  {
-    int left = n_pairs;
-    if (kind == QB200_MEM_HOST && n_pairs > S && S >= 8 && h->max_lanes > 1) {
-      wave_n[n_waves++] = S / 4;
-      wave_n[n_waves++] = S - S / 4;
-      left -= S;
-    }
-    while (left > 0 && n_waves < 63) {
-      wave_n[n_waves] = left < S ? left : S;
-      left -= wave_n[n_waves++];
-    }
-    if (left > 0) n_waves = 0;  // more than ~60 waves: no special opening, walk uniformly below
-  }
-  const bool planned = n_waves > 0;
-  if (!planned) n_waves = (n_pairs + S - 1) / S;
-  int n_lanes = n_waves < h->max_lanes ? (n_waves < 1 ? 1 : n_waves) : h->max_lanes;
-  if (pipelined && h->lanes_active != n_lanes) {  // a different lane count: start a fresh rotation
-    const int rc0 = batch_flush(h);
-    if (rc0) return rc0;
-  }
-  const bool fresh = h->lanes_active == 0;
-  for (int l = 1; l < n_lanes; ++l) {
-    if (!h->lane[l]) {
-      const int rc = lane_alloc(*h->lane[0], &h->lane[l]);
-      if (rc != QB200_OK) {
-        h->fail(__FILE__, __LINE__, "cannot allocate another lane");
-        return rc;
-      }
-    }
-    // the lanes start after whatever the caller queued on lane 0's stream (first batch of a pipelined sequence only: later
-    // on lane 0's stream carries a wave of its own)
-    if (fresh) {
-      if (l == 1) QB_CUDA_TRY(h, cudaEventRecord(h->ev_fork, h->lane[0]->stream));
-      QB_CUDA_TRY(h, cudaStreamWaitEvent(h->lane[l]->stream, h->ev_fork, 0));
-    }
-  }
-  WaveInput in;
-  in.pairs = pairs;
-  in.kind = kind;
-  in.lists = lists;
-  // host scans of a multi-wave batch: one copy stream, ordered after whatever the caller queued on lane 0's stream
-  if (kind == QB200_MEM_HOST && n_lanes > 1) {
-    in.copy_stream = h->copy_stream;
-    if (fresh) QB_CUDA_TRY(h, cudaStreamWaitEvent(in.copy_stream, h->ev_fork, 0));
-  }
-  h->lanes_active = n_lanes;
-  int rc = QB200_OK, wave = 0;
-  for (int w0 = 0; w0 < n_pairs && rc == QB200_OK; ++wave) {
-    Lane* L = h->lane[h->lane_cursor].get();
-    int np = planned ? wave_n[wave] : S;
-    if (np > n_pairs - w0) np = n_pairs - w0;
-    if ((rc = wave_collect(h, L))) break;  // the lane's previous wave (its pinned tables are reused)
-    rc = wave_submit(h, L, in, w0, np, pr, results);
-    h->lane_cursor = (h->lane_cursor + 1) % n_lanes;  // always the lane that has been busy longest
-    w0 += np;
-  }
-  return rc;
+  return enqueue_impl(h, pairs, n_pairs, p, false, kind, results, lists);
+}
+
+int qb200_register_batch_enqueue_each(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                      qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_impl(h, pairs, n_pairs, params, true, kind, results, lists);
 }
 
 int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const float* tgt4, int32_t n_tgt, const qb200_params* p,
@@ -838,26 +979,12 @@ int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t
 
 int qb200_register_cached_ex(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_result* results,
                              const qb200_pair_lists* lists) {
-  if (int rc = enter(h)) return rc;
-  if (n_pairs < 0 || (n_pairs > 0 && (!pairs || !results)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
-  if (!p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
-  if (int rc = check_lists(h, lists, false)) return rc;
-  const float cell = lattice_cell(*p);
-  for (int i = 0; i < n_pairs; ++i) {
-    const int sl[2] = {pairs[i].src_slot, pairs[i].tgt_slot};
-    for (int k = 0; k < 2; ++k) {
-      if (sl[k] < 0 || sl[k] >= h->c_slots) { h->fail(__FILE__, __LINE__, "slot outside qb200_cache_reserve()"); return QB200_ERR_BAD_ARG; }
-      const float* sig = h->c_sig.get() + 4 * (size_t)sl[k];
-      if (sig[0] != p->voxel_size || sig[1] != p->normal_radius || sig[2] != p->fpfh_radius || sig[3] != cell) {
-        h->fail(__FILE__, __LINE__, "cached scan was computed with other front-end parameters (or the slot is empty)");
-        return QB200_ERR_BAD_ARG;
-      }
-    }
-  }
-  WaveInput in;
-  in.slots = pairs;
-  in.lists = lists;
-  return run_waves(h, in, n_pairs, resolve_params(h, *p), results);
+  return register_cached_impl(h, pairs, n_pairs, p, false, results, lists);
+}
+
+int qb200_register_cached_each(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_result* results,
+                               const qb200_pair_lists* lists) {
+  return register_cached_impl(h, pairs, n_pairs, params, true, results, lists);
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

@@ -60,13 +60,6 @@ __device__ __forceinline__ uint32_t warp_transpose32(uint32_t x) {
   return x;
 }
 
-struct GraphConst {
-  float b2, hb2q, twob2, b4;   // beta^2, beta^2/4, 2 beta^2, beta^4 (fp32)
-  float c1, c2, c3;            // q = c1 M |D| + (c2 M + c3) M
-  float two_b2_slack;          // 2 beta^2 (1 + 1e-5): part of M
-  double beta;
-};
-
 // WARP work items (64 rows x kGC*32 columns) of the upper triangle of one pair: row group rg meets the column groups q >= rg*kGRB/kGC
 // (the first group that is not entirely below the diagonal).  Round 2, first version: a CTA item of 256 rows x 512 columns with the
 // rows staged once per CTA -- 29 % of the items of an L = 3000 pair touch the diagonal, where one of the four warps has half the work,
@@ -83,18 +76,19 @@ __device__ __forceinline__ int graph_items(int L) {
 constexpr int kGraphMaxPairs = 2048;  // = the largest max_batch_slots qb200_create accepts
 
 __global__ void __launch_bounds__(kGW * 32, 4) tim_graph_kernel(const float4* __restrict__ ma, const float4* __restrict__ mb,
-                                                                const int* __restrict__ n_corr, int n_pairs, int Lc, int W, GraphConst gc,
-                                                                uint32_t* __restrict__ adj) {
+                                                                const int* __restrict__ n_corr, int n_pairs, int Lc, int W,
+                                                                const PairSolve* __restrict__ solve, uint32_t* __restrict__ adj) {
   __shared__ float4 s_row[kGW][kGRB * 32][2];  // per warp and row: (-2a, |a|^2 - beta^2/4) | (-2b, |b|^2 - beta^2/4)
   __shared__ int s_pref[kGraphMaxPairs + 1];   // exclusive prefix of the pairs' item counts: the warps stride over ALL pairs' items,
   __shared__ int s_scan[33];                   // so a pair with many correspondences is spread over the whole grid
+  __shared__ GraphConst s_gc[kGW];             // per warp: the constants of its item's pair (read at their uses, like launch constants)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
   {
     int carry = 0;
     for (int base = 0; base < n_pairs; base += kGW * 32) {
       const int p = base + tid;
-      const int c = p < n_pairs ? graph_items(n_corr[p]) : 0;
+      const int c = (p < n_pairs && solve[p].mode != QB200_INLIER_NONE) ? graph_items(n_corr[p]) : 0;  // INLIER_NONE: no graph
       int tot;
       const int ex = block_excl_scan(c, s_scan, &tot);
       if (p < n_pairs) s_pref[p] = carry + ex;
@@ -129,6 +123,9 @@ __global__ void __launch_bounds__(kGW * 32, 4) tim_graph_kernel(const float4* __
     // ---- this warp's rows
     float mmr[kGRB];
     __syncwarp();
+    if (lane == 0) s_gc[warp] = solve[pair].gc;  // the pair's own beta
+    __syncwarp();
+    const volatile GraphConst& gc = s_gc[warp];  // volatile: loaded at every use, no register held across the item
 #pragma unroll
     for (int rb = 0; rb < kGRB; ++rb) {
       const int i = (rg * kGRB + rb) * 32 + lane;
@@ -246,8 +243,9 @@ __global__ void __launch_bounds__(kGW * 32, 4) tim_graph_kernel(const float4* __
 
 // degrees + edge count (one warp per row)
 __global__ void __launch_bounds__(256) degree_kernel(uint32_t* __restrict__ adj, const int* __restrict__ n_corr, int Lc, int W,
-                                                     int* __restrict__ deg, long long* __restrict__ n_edges) {
+                                                     const PairSolve* __restrict__ solve, int* __restrict__ deg, long long* __restrict__ n_edges) {
   const int pair = blockIdx.y;
+  if (solve[pair].mode == QB200_INLIER_NONE) return;  // n_edges stays 0, as when the whole wave skips K8
   const int L = n_corr[pair];
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= L) return;
@@ -267,14 +265,13 @@ __global__ void __launch_bounds__(256) degree_kernel(uint32_t* __restrict__ adj,
 int launch_degree(Lane* h, int n_pairs) {
   if (n_pairs <= 0) return QB200_OK;
   const dim3 gd((h->Lc + 7) / 8, n_pairs);
-  degree_kernel<<<gd, 256, 0, h->stream>>>(h->adj, h->ctr.n_corr, h->Lc, h->W, h->deg, h->ctr.n_edges);
+  degree_kernel<<<gd, 256, 0, h->stream>>>(h->adj, h->ctr.n_corr, h->Lc, h->W, h->d_solve, h->deg, h->ctr.n_edges);
   h->launches++;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;
 }
 
-int launch_graph(Lane* h, int n_pairs, double noise_bound, double cbar2) {
-  if (n_pairs <= 0) return QB200_OK;
+GraphConst graph_const(double noise_bound, double cbar2) {
   const double beta = 2 * noise_bound * sqrt(cbar2);  // quatro.hpp:367
   const double u = 5.9604644775390625e-8;             // 2^-24
   GraphConst gc;
@@ -287,13 +284,18 @@ int launch_graph(Lane* h, int n_pairs, double noise_bound, double cbar2) {
   gc.c2 = (float)(1500.0 * u * u * 1.02);
   gc.c3 = (float)(46.0 * u * beta * beta * 1.02);
   gc.two_b2_slack = (float)(2.0 * beta * beta * 1.00001);
+  return gc;
+}
+
+int launch_graph(Lane* h, int n_pairs) {
+  if (n_pairs <= 0) return QB200_OK;
   // one wave of resident CTAs whose warps stride over every pair's work items (64 rows x 128 columns each)
   cudaEventRecord(h->kev[2], h->stream);
-  tim_graph_kernel<<<dim3(h->n_sm * 4), kGW * 32, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, n_pairs, h->Lc, h->W, gc, h->adj);
+  tim_graph_kernel<<<dim3(h->n_sm * 4), kGW * 32, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, n_pairs, h->Lc, h->W, h->d_solve, h->adj);
   cudaEventRecord(h->kev[3], h->stream);
   h->kev_armed[1] = 1;
   const dim3 gd((h->Lc + 7) / 8, n_pairs);
-  degree_kernel<<<gd, 256, 0, h->stream>>>(h->adj, h->ctr.n_corr, h->Lc, h->W, h->deg, h->ctr.n_edges);
+  degree_kernel<<<gd, 256, 0, h->stream>>>(h->adj, h->ctr.n_corr, h->Lc, h->W, h->d_solve, h->deg, h->ctr.n_edges);
   h->launches += 2;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;

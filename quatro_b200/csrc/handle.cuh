@@ -11,6 +11,32 @@
 
 namespace qb {
 
+// K8's constants of one β = 2 noise_bound sqrt(cbar2) (graph.cu: graph_const)
+struct GraphConst {
+  float b2, hb2q, twob2, b4;   // beta^2, beta^2/4, 2 beta^2, beta^4 (fp32)
+  float c1, c2, c3;            // q = c1 M |D| + (c2 M + c3) M
+  float two_b2_slack;          // 2 beta^2 (1 + 1e-5): part of M
+  double beta;
+};
+
+// K10/11's parameters of one pair (pose.cu)
+struct PoseParams {
+  double rot_noise_bound, cote_range, gnc_factor, cost_threshold;
+  int max_iterations, cote_median, use_rot_inliers, use_RyRx;
+  double RyRx[9];
+};
+
+// One pair's solver configuration, as K8..K11 read it from the lane's table (DESIGN §5.4): the solver fields of its qb200_params,
+// resolved on the host.  mode == QB200_INLIER_NONE: the pair skips K8 / K9 and gets the identity clique.
+struct PairSolve {
+  GraphConst gc;
+  PoseParams pp;
+  double kcore_thr;
+  long long node_limit;      // PMC_EXACT nodes (0 already resolved to QB200_DEFAULT_CLIQUE_NODE_LIMIT)
+  int mode;                  // QB200_PMC_EXACT .. QB200_INLIER_NONE
+  int reserved;
+};
+
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
 // kernels of the others.  The lane owns its stream, buffers and events: deleting it releases them.
@@ -83,6 +109,7 @@ struct Lane {
   DeviceMem<unsigned char> pose_ws; // [S * pose_ws_bytes(Lc)] pose workspace of cliques above kPoseSmemClique members (Lc > kPoseSmemClique only)
   DeviceMem<int> final_inl;   // [S*Lc]
   DeviceMem<unsigned char> rot_mask, trans_mask; // [S*Lc]
+  DeviceMem<PairSolve> d_solve; PinnedMem<PairSolve> h_solve;  // [S] solver table of the wave, and its pinned mirror (upload_solve copies it)
   // ---- pre-processing (preprocess.cu), allocated on first use for the largest wave so far (pw_scans / ip_cap) ----
   DeviceMem<int> pp_cnt; PinnedMem<int> pp_hcnt;  // [2S][8] per-scan counts and status of a wave, and its pinned mirror
   DeviceMem<int> pw_ints;     // [pw_scans] x (patch id / rank per point, per-patch counters and offsets)
@@ -178,12 +205,20 @@ size_t pose_ws_bytes(int Lc);
 int launch_voxel(Lane* h, int n_clouds, float leaf, int skip_flagged);
 int launch_fpfh(Lane* h, int n_clouds, float normal_radius, float fpfh_radius, float cell);
 int launch_match(Lane* h, int n_pairs, const qb200_params& p);
-int launch_graph(Lane* h, int n_pairs, double noise_bound, double cbar2);
-int launch_clique(Lane* h, int n_pairs, int mode, double kcore_thr, long long node_limit);
-int launch_pose(Lane* h, int n_pairs, const qb200_params& p);
+// The solver stages read every pair's configuration from the lane's table d_solve (upload_solve): K8 skips the pairs in
+// QB200_INLIER_NONE, K9 runs each pair in its own mode (the exact search only when the table has a PMC_EXACT pair: any_exact),
+// iota_clique_kernel fills only the QB200_INLIER_NONE pairs.
+int launch_graph(Lane* h, int n_pairs);
+int launch_clique(Lane* h, int n_pairs, bool any_exact);
+int launch_pose(Lane* h, int n_pairs);
 int launch_fill_counters(Lane* h, int n_pairs, int have_frontend);
 int launch_finalize_status(Lane* h, int n_pairs);
 int launch_iota_clique(Lane* h, int n_pairs);
+GraphConst graph_const(double noise_bound, double cbar2);
+PoseParams pose_params(const qb200_params& p);  // p's rotation noise bound already resolved
+PairSolve solve_entry(const qb200_params& p);   // the same, every solver field
+// the entries [0, n) of h_solve to d_solve on the lane's stream: one copy (h_solve must stay as it is until the stream passed it)
+int upload_solve(Lane* h, int n);
 // Where pack_lists_kernel writes pair s's lists: each array (nullptr = not asked for) + s * stride entries, at most cap of them.
 struct ListDst {
   int2* corr; float4* sm; float4* tm; int* clique; int* fin; unsigned char* rm; unsigned char* tmask;
@@ -215,7 +250,7 @@ int collect_batch(qb200_handle* h, const qb200_result* dst);  // api.cu: wait fo
 int enter(qb200_handle* h);  // entry prologue: a handle, its device current, no enqueued batch in flight
 int wave_reset(Lane* L, int n_clouds);
 int stage_raw(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs);
-int run_solver(Lane* L, int n_pairs, const qb200_params& p, int have_frontend);
+int run_solver(Lane* L, int n_pairs, int have_frontend);  // pairs [0, n_pairs) with their entries in L->h_solve, uploaded
 int launch_degree(Lane* h, int n_pairs);
 bool params_ok(const qb200_params* p);
 float lattice_cell(const qb200_params& p);

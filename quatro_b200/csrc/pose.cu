@@ -19,12 +19,6 @@ namespace qb {
 
 constexpr int kPoseThreads = 256;
 
-struct PoseParams {
-  double rot_noise_bound, cote_range, gnc_factor, cost_threshold;
-  int max_iterations, cote_median, use_rot_inliers, use_RyRx;
-  double RyRx[9];
-};
-
 __device__ __forceinline__ double block_sum(double v, double* scratch) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -80,7 +74,7 @@ __device__ void bitonic_sort(double* val, unsigned short* tag, int n2) {
 template <bool kWs>
 __global__ void __launch_bounds__(kPoseThreads) pose_kernel(const float4* __restrict__ ma, const float4* __restrict__ mb, const int* __restrict__ n_corr,
                                                             int Lc, int Lp, int Lg, unsigned char* __restrict__ ws, const int* __restrict__ clique_all,
-                                                            const int* __restrict__ n_clique, PoseParams pp,
+                                                            const int* __restrict__ n_clique, const PairSolve* __restrict__ solve,
                                                             qb200_result* __restrict__ results, unsigned char* __restrict__ rot_mask_out,
                                                             unsigned char* __restrict__ trans_mask_out, int* __restrict__ final_inl,
                                                             int* __restrict__ n_final) {
@@ -94,6 +88,7 @@ __global__ void __launch_bounds__(kPoseThreads) pose_kernel(const float4* __rest
   const int L = n_corr[pair];
   const int c = n_clique[pair];
   if ((c > Lp) != kWs) return;  // the other instance solves this pair
+  const PoseParams& pp = solve[pair].pp;
   // workspace of Lq = power-of-two capacity (so the bitonic networks fit): shared memory (Lp) for cliques of up to Lp members, else
   // the pair's slot of ws (Lg = next_pow2(Lc)).  At Lq = 32768 the 65536 COTE events fill the u16 tags 0..65535 without padding.
   //   ev[2Lq] f64 | wX[Lq] f64 | aux[Lq] f64 | tag[2Lq] u16 | ctag[Lq] u16 | list[Lq] u16 | rm[Lq] u8 | tm[Lq] u8
@@ -307,7 +302,8 @@ __global__ void __launch_bounds__(kPoseThreads) pose_kernel(const float4* __rest
     n_fin = carry;
   }
   for (int j = tid; j < c; j += kPoseThreads) rot_mask_out[(size_t)pair * Lc + j] = rm[j];
-  for (int i = tid; i < N; i += kPoseThreads) trans_mask_out[(size_t)pair * Lc + i] = tm[i];
+  // members past the N COTE inputs (rotation-inlier COTE) get 0, so the mask never shows what an earlier pair left in the slot
+  for (int i = tid; i < c; i += kPoseThreads) trans_mask_out[(size_t)pair * Lc + i] = i < N ? tm[i] : 0;
   if (tid == 0) {
     res->valid = 1;
     res->status = QB200_OK;
@@ -349,8 +345,10 @@ __global__ void finalize_status_kernel(qb200_result* __restrict__ results, int n
   }
 }
 
-__global__ void iota_clique_kernel(const int* __restrict__ n_corr, int Lc, int* __restrict__ clique, int* __restrict__ n_clique, int* __restrict__ max_core) {
+__global__ void iota_clique_kernel(const int* __restrict__ n_corr, const PairSolve* __restrict__ solve, int Lc, int* __restrict__ clique,
+                                   int* __restrict__ n_clique, int* __restrict__ max_core) {
   const int pair = blockIdx.y;
+  if (solve[pair].mode != QB200_INLIER_NONE) return;
   const int L = n_corr[pair];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < L) clique[(size_t)pair * Lc + i] = i;
@@ -359,8 +357,7 @@ __global__ void iota_clique_kernel(const int* __restrict__ n_corr, int Lc, int* 
 
 size_t pose_ws_bytes(int Lc) { return pose_smem_bytes(next_pow2(Lc)); }
 
-int launch_pose(Lane* h, int n_pairs, const qb200_params& p) {
-  if (n_pairs <= 0) return QB200_OK;
+PoseParams pose_params(const qb200_params& p) {
   PoseParams pp;
   pp.rot_noise_bound = p.rot_noise_bound;  // resolved by the entry point (api.cu: resolve_params, the handle's latch)
   pp.cote_range = p.cote_noise_bound * sqrt(p.cbar2);
@@ -371,16 +368,21 @@ int launch_pose(Lane* h, int n_pairs, const qb200_params& p) {
   pp.use_rot_inliers = p.using_rot_inliers_when_estimating_cote;
   pp.use_RyRx = p.use_pre_estimated_RyRx;
   for (int i = 0; i < 9; ++i) pp.RyRx[i] = p.RyRx[i];
+  return pp;
+}
+
+int launch_pose(Lane* h, int n_pairs) {
+  if (n_pairs <= 0) return QB200_OK;
   const int Lp = next_pow2(h->Lc < kPoseSmemClique ? h->Lc : kPoseSmemClique);
   const size_t smem = pose_smem_bytes(Lp);
   QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)pose_kernel<false>, smem));
   pose_kernel<false><<<n_pairs, kPoseThreads, smem, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, h->Lc, Lp, next_pow2(h->Lc), h->pose_ws, h->clique,
-                                                                 h->ctr.n_clique, pp, h->d_results, h->rot_mask, h->trans_mask, h->final_inl,
+                                                                 h->ctr.n_clique, h->d_solve, h->d_results, h->rot_mask, h->trans_mask, h->final_inl,
                                                                  h->ctr.n_final);
   h->launches++;
   if (h->Lc > kPoseSmemClique) {  // cliques above Lp members: the same code on the pair's slot of pose_ws
     pose_kernel<true><<<n_pairs, kPoseThreads, 0, h->stream>>>(h->ma, h->mb, h->ctr.n_corr, h->Lc, Lp, next_pow2(h->Lc), h->pose_ws, h->clique,
-                                                               h->ctr.n_clique, pp, h->d_results, h->rot_mask, h->trans_mask, h->final_inl,
+                                                               h->ctr.n_clique, h->d_solve, h->d_results, h->rot_mask, h->trans_mask, h->final_inl,
                                                                h->ctr.n_final);
     h->launches++;
   }
@@ -400,7 +402,7 @@ int launch_finalize_status(Lane* h, int n_pairs) {
 }
 int launch_iota_clique(Lane* h, int n_pairs) {
   const dim3 g((h->Lc + 255) / 256, n_pairs);
-  iota_clique_kernel<<<g, 256, 0, h->stream>>>(h->ctr.n_corr, h->Lc, h->clique, h->ctr.n_clique, h->ctr.max_core);
+  iota_clique_kernel<<<g, 256, 0, h->stream>>>(h->ctr.n_corr, h->d_solve, h->Lc, h->clique, h->ctr.n_clique, h->ctr.max_core);
   h->launches++;
   return QB200_OK;
 }

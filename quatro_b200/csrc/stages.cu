@@ -183,7 +183,11 @@ int qb200_build_graph(qb200_handle* h, const float* a4, const float* b4, int32_t
   QB_CUDA_TRY(h, cudaMemcpyAsync(ln->ma, a4, (size_t)L * sizeof(float4), cudaMemcpyHostToDevice, ln->stream));
   QB_CUDA_TRY(h, cudaMemcpyAsync(ln->mb, b4, (size_t)L * sizeof(float4), cudaMemcpyHostToDevice, ln->stream));
   MirrorHold hold{ln};
-  if ((rc = write_counter(ln, ln->hctr.n_corr, L)) || (rc = launch_graph(ln, 1, noise_bound, cbar2))) return rc;
+  // a one-entry solver table: this beta (the mode only has to be one that builds a graph)
+  memset(&ln->h_solve[0], 0, sizeof(PairSolve));
+  ln->h_solve[0].gc = graph_const(noise_bound, cbar2);
+  ln->h_solve[0].mode = QB200_PMC_HEU;
+  if ((rc = write_counter(ln, ln->hctr.n_corr, L)) || (rc = upload_solve(ln, 1)) || (rc = launch_graph(ln, 1))) return rc;
   const int nb = (L + 31) / 32;
   memset(adj, 0, (size_t)L * words_per_row * sizeof(uint32_t));
   QB_CUDA_TRY(h, cudaMemcpy2DAsync(adj, (size_t)words_per_row * 4, ln->adj, (size_t)ln->W * 4, (size_t)nb * 4, L, cudaMemcpyDeviceToHost, ln->stream));
@@ -214,8 +218,12 @@ int qb200_max_clique_ex(qb200_handle* h, const uint32_t* adj, int32_t L, int32_t
   QB_CUDA_TRY(h, cudaMemsetAsync(ln->adj, 0, (size_t)L * ln->W * 4, ln->stream));
   QB_CUDA_TRY(h, cudaMemcpy2DAsync(ln->adj, (size_t)ln->W * 4, adj, (size_t)words_per_row * 4, (size_t)nb * 4, L, cudaMemcpyHostToDevice, ln->stream));
   MirrorHold hold{ln};
-  if ((rc = write_counter(ln, ln->hctr.n_corr, L)) || (rc = launch_degree(ln, 1))) return rc;
-  if ((rc = launch_clique(ln, 1, mode, kcore_thr, node_limit)) || (rc = read_counters(ln))) return rc;
+  memset(&ln->h_solve[0], 0, sizeof(PairSolve));  // a one-entry solver table: this mode, threshold and node limit
+  ln->h_solve[0].mode = mode;
+  ln->h_solve[0].kcore_thr = kcore_thr;
+  ln->h_solve[0].node_limit = node_limit > 0 ? node_limit : (long long)QB200_DEFAULT_CLIQUE_NODE_LIMIT;
+  if ((rc = write_counter(ln, ln->hctr.n_corr, L)) || (rc = upload_solve(ln, 1)) || (rc = launch_degree(ln, 1))) return rc;
+  if ((rc = launch_clique(ln, 1, mode == QB200_PMC_EXACT)) || (rc = read_counters(ln))) return rc;
   QB_CUDA_TRY(h, hold.sync());
   const int nc = ln->hctr.n_clique[0];
   if (flags) *flags = ln->hctr.flags[0];
@@ -249,7 +257,8 @@ int qb200_solve_pose(qb200_handle* h, const float* a4, const float* b4, int32_t 
   if (n_clique > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ln->clique, clique, (size_t)n_clique * sizeof(int), cudaMemcpyHostToDevice, ln->stream));
   MirrorHold hold{ln};
   if ((rc = write_counter(ln, ln->hctr.n_corr, L)) || (rc = write_counter(ln, ln->hctr.n_clique, n_clique))) return rc;
-  if ((rc = launch_fill_counters(ln, 1, 0)) || (rc = launch_pose(ln, 1, resolve_params(h, *p)))) return rc;
+  ln->h_solve[0] = solve_entry(resolve_params(h, *p));
+  if ((rc = upload_solve(ln, 1)) || (rc = launch_fill_counters(ln, 1, 0)) || (rc = launch_pose(ln, 1))) return rc;
   QB_CUDA_TRY(h, cudaMemcpyAsync(ln->h_results, ln->d_results, sizeof(qb200_result), cudaMemcpyDeviceToHost, ln->stream));
   QB_CUDA_TRY(h, hold.sync());
   *res = ln->h_results[0];
@@ -275,7 +284,8 @@ int qb200_solve_correspondences(qb200_handle* h, const float* a4, const float* b
   if (L > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ln->ma, a4, (size_t)L * sizeof(float4), cudaMemcpyHostToDevice, ln->stream));
   if (L > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ln->mb, b4, (size_t)L * sizeof(float4), cudaMemcpyHostToDevice, ln->stream));
   MirrorHold hold{ln};
-  if ((rc = write_counter(ln, ln->hctr.n_corr, L)) || (rc = run_solver(ln, 1, resolve_params(h, *p), 0))) return rc;
+  ln->h_solve[0] = solve_entry(resolve_params(h, *p));
+  if ((rc = write_counter(ln, ln->hctr.n_corr, L)) || (rc = upload_solve(ln, 1)) || (rc = run_solver(ln, 1, 0))) return rc;
   QB_CUDA_TRY(h, cudaMemcpyAsync(ln->h_results, ln->d_results, sizeof(qb200_result), cudaMemcpyDeviceToHost, ln->stream));
   QB_CUDA_TRY(h, hold.sync());
   *res = ln->h_results[0];
