@@ -366,7 +366,9 @@ int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const
  * 4 lanes (each further lane -- same buffers again, own stream -- is allocated on first use) so that one wave's
  * host->device copies and solver tail overlap the other waves' dense kernels; QB200_LANES=n (1..8, default 4) in
  * the environment sets the lane count (1 = strictly one wave at a time).  Results never depend on the wave size
- * or the lane. */
+ * or the lane.  Every batch call (raw, cached or correspondence-set input, any form) goes through the same checks and the same
+ * wave driver; cached pairs and correspondence sets run their waves on one lane.  A call with n = 0 pairs does no work and
+ * latches no rotation noise bound.  A kind other than QB200_MEM_HOST / QB200_MEM_DEVICE is QB200_ERR_BAD_ARG. */
 int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs,
                          const qb200_params* p, qb200_mem_kind kind, qb200_result* results);
 /* qb200_register_batch + every pair's lists: FPFHManager::getCorrespondences / getSrcKps / getTgtKps (include/fpfh_manager.hpp:
@@ -470,12 +472,12 @@ int qb200_get_last_correspondences(qb200_handle* h, int32_t* corr, float* src_ma
  * getTgtNormals (include/fpfh_manager.hpp:161-177).  Either pointer may be NULL. */
 int qb200_get_last_features(qb200_handle* h, int32_t which, float* normals4, float* desc33, int32_t cap, int32_t* n);
 
-/* Per-stage device time of the last qb200_register_batch call in milliseconds (CUDA events):
- * [0]=h2d [1]=voxel [2]=fpfh [3]=match [4]=graph [5]=clique [6]=pose [7]=d2h; n<=8. */
+/* Per-stage device time of the last batch call in milliseconds (CUDA events); the single-pair registration and solve are batches
+ * of one: [0]=h2d [1]=voxel [2]=fpfh [3]=match [4]=graph [5]=clique [6]=pose [7]=d2h; n<=8. */
 int qb200_get_stage_ms(qb200_handle* h, float* ms, int32_t n);
 
 /* Device time (CUDA events on the handle's stream) and launch count of the two roofline kernels
- * during the last qb200_register_batch call: [0] = the tensor-core nearest-neighbour passes (tc_match_kernel x3),
+ * during the last batch call: [0] = the tensor-core nearest-neighbour passes (tc_match_kernel x3),
  * [1] = tim_graph_kernel (TIM consistency graph); n <= 2. */
 int qb200_get_kernel_ms(qb200_handle* h, float* ms, int32_t* launches, int32_t n);
 

@@ -170,6 +170,73 @@ class QuatroB200Error(RuntimeError):
         super().__init__(f"{where}: {STATUS_NAMES.get(code, code)} {detail}")
 
 
+# restype and argtypes of every function include/quatro_b200.h declares
+vp, i32, i64, f32, f64, P = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_double, C.POINTER
+_SIGNATURES = {
+    "qb200_default_params": (None, [P(Params)]),
+    "qb200_default_config": (None, [P(Config)]),
+    "qb200_version": (i32, []),
+    "qb200_create": (i32, [P(Config), P(vp)]),
+    "qb200_destroy": (None, [vp]),
+    "qb200_set_stream": (i32, [vp, vp]),
+    "qb200_last_error": (C.c_char_p, [vp]),
+    "qb200_launch_count": (i64, [vp]),
+    "qb200_voxelize": (i32, [vp, vp, i32, f32, i32, vp, i32, P(i32)]),
+    "qb200_default_patchwork_params": (None, [P(PatchworkParams)]),
+    "qb200_default_segment_params": (None, [P(SegmentParams)]),
+    "qb200_segment_cloud": (i32, [vp, vp, i32, P(SegmentParams), vp, P(i32), vp, P(i32)]),
+    "qb200_patchwork": (i32, [vp, vp, i32, P(PatchworkParams), vp, P(i32), vp, P(i32)]),
+    "qb200_compute_fpfh": (i32, [vp, vp, i32, f32, f32, f32, vp, vp]),
+    "qb200_match": (i32, [vp, vp, i32, vp, vp, i32, vp, P(Params), vp, i32, P(i32), P(i32)]),
+    "qb200_build_graph": (i32, [vp, vp, vp, i32, f64, f64, vp, i32, vp, P(i64)]),
+    "qb200_max_clique": (i32, [vp, vp, i32, i32, i32, f64, vp, P(i32), vp, vp, P(i32)]),
+    "qb200_max_clique_ex": (i32, [vp, vp, i32, i32, i32, f64, i64, vp, P(i32), vp, vp, P(i32), P(i32)]),
+    "qb200_solve_pose": (i32, [vp, vp, vp, i32, vp, i32, P(Params), P(Result), vp, vp]),
+    "qb200_solve_correspondences": (i32, [vp, vp, vp, i32, P(Params), P(Result)]),
+    "qb200_match_and_pack": (i32, [vp, vp, i32, vp, i32, P(Params), vp, vp, vp, i32, P(i32)]),
+    "qb200_register_pair": (i32, [vp, vp, i32, vp, i32, P(Params), P(Result)]),
+    "qb200_register_batch": (i32, [vp, P(Pair), i32, P(Params), i32, vp]),
+    "qb200_get_last_clique": (i32, [vp, vp, i32, P(i32)]),
+    "qb200_get_last_final_inliers": (i32, [vp, vp, i32, P(i32)]),
+    "qb200_get_last_correspondences": (i32, [vp, vp, vp, vp, i32, P(i32)]),
+    "qb200_get_stage_ms": (i32, [vp, vp, i32]),
+    "qb200_get_kernel_ms": (i32, [vp, vp, vp, i32]),
+    "qb200_debug_tc_distances": (i32, [vp, vp, i32, vp, i32, vp]),
+    "qb200_debug_match_stats": (i32, [vp, vp, i32]),
+    "qb200_debug_nn_tables": (i32, [vp, vp, i32, vp, i32]),
+    "qb200_register_batch_enqueue": (i32, [vp, vp, i32, vp, i32, vp]),
+    "qb200_register_batch_flush": (i32, [vp]),
+    "qb200_debug_tc_profile": (i32, [vp, vp, i32]),
+    "qb200_debug_tc_footprint": (i32, [vp, vp]),
+    "qb200_solve_batch": (i32, [vp, vp, i32, vp, i32, vp]),
+    "qb200_comm_init_all": (i32, [P(vp), i32]),
+    "qb200_register_batch_sharded": (i32, [P(vp), i32, P(Pair), i32, P(Params), i32, vp]),
+    "qb200_comm_unique_id": (i32, [vp]),
+    "qb200_comm_init_rank": (i32, [vp, i32, i32, vp]),
+    "qb200_register_batch_rank": (i32, [vp, P(Pair), i32, P(Params), i32, vp, i32]),
+    "qb200_comm_wait": (i32, [vp]),
+    "qb200_bind_numa": (i32, [vp]),
+    "qb200_debug_match_verify": (i32, [vp, vp, i32]),
+    "qb200_get_last_features": (i32, [vp, i32, vp, vp, i32, P(i32)]),
+    "qb200_cache_reserve": (i32, [vp, i32]),
+    "qb200_cache_scans": (i32, [vp, P(vp), P(i32), P(i32), i32, P(Params), i32]),
+    "qb200_register_cached": (i32, [vp, vp, i32, P(Params), vp]),
+    "qb200_cache_copy": (i32, [vp, i32, i32]),
+    "qb200_cache_read": (i32, [vp, i32, vp, vp, vp, i32, P(i32)]),
+    "qb200_register_batch_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_register_batch_enqueue_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_register_cached_ex": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
+    "qb200_solve_batch_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_preprocess_batch": (i32, [vp, vp, vp, i32, i32, P(PatchworkParams), P(SegmentParams), P(PreprocessOut)]),
+    "qb200_register_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_register_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_register_cached_each": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
+    "qb200_solve_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+}
+del vp, i32, i64, f32, f64, P
+EXPORTED_SYMBOLS = list(_SIGNATURES)
+
+
 _LIB: Optional[C.CDLL] = None
 
 
@@ -184,6 +251,53 @@ def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+# ---- the ctypes input arrays of the batch calls: each returns the array and what must stay alive while it is in use ----
+def _pair_array(pairs: Sequence, kind: int = MEM_HOST):
+    """(Pair * n) array of `pairs`: (src, tgt) numpy arrays (MEM_HOST) or (src_ptr, n_src, tgt_ptr, n_tgt) device tuples (MEM_DEVICE);
+    and the contiguous scans it points to."""
+    arr = (Pair * len(pairs))()
+    keep = []
+    for i, pr in enumerate(pairs):
+        if kind == MEM_HOST:
+            s, t = _f32(pr[0], 4), _f32(pr[1], 4)
+            keep.append((s, t))
+            arr[i].src, arr[i].n_src, arr[i].tgt, arr[i].n_tgt = s.ctypes.data, len(s), t.ctypes.data, len(t)
+        else:
+            arr[i].src, arr[i].n_src, arr[i].tgt, arr[i].n_tgt = pr[0], pr[1], pr[2], pr[3]
+    return arr, keep
+
+
+def _set_array(sets: Sequence, kind: int):
+    """(CorrSet * n) array of `sets`: (a4, b4) numpy arrays (MEM_HOST) or (a_ptr, b_ptr, L) device tuples (MEM_DEVICE); and the
+    contiguous points it points to."""
+    arr = (CorrSet * len(sets))()
+    keep = []
+    for i, st in enumerate(sets):
+        if kind == MEM_HOST:
+            a, b = _f32(st[0], 4), _f32(st[1], 4)
+            assert len(a) == len(b)
+            keep.append((a, b))
+            arr[i].a, arr[i].b, arr[i].L = a.ctypes.data, b.ctypes.data, len(a)
+        else:
+            arr[i].a, arr[i].b, arr[i].L = st[0], st[1], st[2]
+    return arr, keep
+
+
+def _slot_array(slot_pairs) -> np.ndarray:
+    """(n, 2) int32 array of (source slot, target slot) pairs, laid out as qb200_slot_pair[n]."""
+    return np.ascontiguousarray(np.asarray(slot_pairs, np.int32).reshape(-1, 2))
+
+
+def _scan_arrays(scans: Sequence, kind: int):
+    """(void* * n) scan pointers and (int32 * n) point counts of `scans`: (n,4) float32 arrays (MEM_HOST) or (device_ptr, n) tuples
+    (MEM_DEVICE); and the contiguous scans they point to."""
+    keep = [_f32(sc, 4) for sc in scans] if kind == MEM_HOST else []
+    ptrs = [a.ctypes.data for a in keep] if kind == MEM_HOST else [sc[0] for sc in scans]
+    sizes = [len(a) for a in keep] if kind == MEM_HOST else [int(sc[1]) for sc in scans]
+    n = max(len(scans), 1)
+    return (C.c_void_p * n)(*ptrs), (C.c_int32 * n)(*sizes), keep
+
+
 def load_library(build: bool = True) -> C.CDLL:
     """Load libquatro_b200.so (building it with nvcc if stale).  Raises if it cannot be built/loaded."""
     global _LIB
@@ -191,98 +305,12 @@ def load_library(build: bool = True) -> C.CDLL:
         return _LIB
     path = _build.build_cuda() if build else _build.CUDA_LIB
     lib = C.CDLL(str(path))
-    vp, i32, i64, f32, f64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_double
-    P = C.POINTER
-    sig = {
-        "qb200_default_params": (None, [P(Params)]),
-        "qb200_default_config": (None, [P(Config)]),
-        "qb200_version": (i32, []),
-        "qb200_create": (i32, [P(Config), P(vp)]),
-        "qb200_destroy": (None, [vp]),
-        "qb200_set_stream": (i32, [vp, vp]),
-        "qb200_last_error": (C.c_char_p, [vp]),
-        "qb200_launch_count": (i64, [vp]),
-        "qb200_voxelize": (i32, [vp, vp, i32, f32, i32, vp, i32, P(i32)]),
-        "qb200_default_patchwork_params": (None, [P(PatchworkParams)]),
-        "qb200_default_segment_params": (None, [P(SegmentParams)]),
-        "qb200_segment_cloud": (i32, [vp, vp, i32, P(SegmentParams), vp, P(i32), vp, P(i32)]),
-        "qb200_patchwork": (i32, [vp, vp, i32, P(PatchworkParams), vp, P(i32), vp, P(i32)]),
-        "qb200_compute_fpfh": (i32, [vp, vp, i32, f32, f32, f32, vp, vp]),
-        "qb200_match": (i32, [vp, vp, i32, vp, vp, i32, vp, P(Params), vp, i32, P(i32), P(i32)]),
-        "qb200_build_graph": (i32, [vp, vp, vp, i32, f64, f64, vp, i32, vp, P(i64)]),
-        "qb200_max_clique": (i32, [vp, vp, i32, i32, i32, f64, vp, P(i32), vp, vp, P(i32)]),
-        "qb200_max_clique_ex": (i32, [vp, vp, i32, i32, i32, f64, i64, vp, P(i32), vp, vp, P(i32), P(i32)]),
-        "qb200_solve_pose": (i32, [vp, vp, vp, i32, vp, i32, P(Params), P(Result), vp, vp]),
-        "qb200_solve_correspondences": (i32, [vp, vp, vp, i32, P(Params), P(Result)]),
-        "qb200_match_and_pack": (i32, [vp, vp, i32, vp, i32, P(Params), vp, vp, vp, i32, P(i32)]),
-        "qb200_register_pair": (i32, [vp, vp, i32, vp, i32, P(Params), P(Result)]),
-        "qb200_register_batch": (i32, [vp, P(Pair), i32, P(Params), i32, vp]),
-        "qb200_get_last_clique": (i32, [vp, vp, i32, P(i32)]),
-        "qb200_get_last_final_inliers": (i32, [vp, vp, i32, P(i32)]),
-        "qb200_get_last_correspondences": (i32, [vp, vp, vp, vp, i32, P(i32)]),
-        "qb200_get_stage_ms": (i32, [vp, vp, i32]),
-        "qb200_get_kernel_ms": (i32, [vp, vp, vp, i32]),
-        "qb200_debug_tc_distances": (i32, [vp, vp, i32, vp, i32, vp]),
-        "qb200_debug_match_stats": (i32, [vp, vp, i32]),
-        "qb200_debug_nn_tables": (i32, [vp, vp, i32, vp, i32]),
-        "qb200_register_batch_enqueue": (i32, [vp, vp, i32, vp, i32, vp]),
-        "qb200_register_batch_flush": (i32, [vp]),
-        "qb200_debug_tc_profile": (i32, [vp, vp, i32]),
-        "qb200_debug_tc_footprint": (i32, [vp, vp]),
-        "qb200_solve_batch": (i32, [vp, vp, i32, vp, i32, vp]),
-        "qb200_comm_init_all": (i32, [P(vp), i32]),
-        "qb200_register_batch_sharded": (i32, [P(vp), i32, P(Pair), i32, P(Params), i32, vp]),
-        "qb200_comm_unique_id": (i32, [vp]),
-        "qb200_comm_init_rank": (i32, [vp, i32, i32, vp]),
-        "qb200_register_batch_rank": (i32, [vp, P(Pair), i32, P(Params), i32, vp, i32]),
-        "qb200_comm_wait": (i32, [vp]),
-        "qb200_bind_numa": (i32, [vp]),
-        "qb200_debug_match_verify": (i32, [vp, vp, i32]),
-        "qb200_get_last_features": (i32, [vp, i32, vp, vp, i32, P(i32)]),
-        "qb200_cache_reserve": (i32, [vp, i32]),
-        "qb200_cache_scans": (i32, [vp, P(vp), P(i32), P(i32), i32, P(Params), i32]),
-        "qb200_register_cached": (i32, [vp, vp, i32, P(Params), vp]),
-        "qb200_cache_copy": (i32, [vp, i32, i32]),
-        "qb200_cache_read": (i32, [vp, i32, vp, vp, vp, i32, P(i32)]),
-        "qb200_register_batch_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
-        "qb200_register_batch_enqueue_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
-        "qb200_register_cached_ex": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
-        "qb200_solve_batch_ex": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
-        "qb200_preprocess_batch": (i32, [vp, vp, vp, i32, i32, P(PatchworkParams), P(SegmentParams), P(PreprocessOut)]),
-        "qb200_register_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
-        "qb200_register_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
-        "qb200_register_cached_each": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
-        "qb200_solve_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
-    }
-    for name, (res, args) in sig.items():
+    for name, (res, args) in _SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError = header/library mismatch: fail loudly
         fn.restype = res
         fn.argtypes = args
     _LIB = lib
     return lib
-
-
-EXPORTED_SYMBOLS = [
-    "qb200_default_params", "qb200_default_config", "qb200_version", "qb200_create", "qb200_destroy",
-    "qb200_set_stream", "qb200_last_error", "qb200_launch_count", "qb200_voxelize", "qb200_compute_fpfh",
-    "qb200_default_patchwork_params", "qb200_patchwork", "qb200_default_segment_params", "qb200_segment_cloud", "qb200_match", "qb200_build_graph", "qb200_max_clique", "qb200_max_clique_ex", "qb200_solve_pose", "qb200_solve_correspondences",
-    "qb200_match_and_pack", "qb200_register_pair", "qb200_register_batch", "qb200_get_last_clique",
-    "qb200_get_last_final_inliers", "qb200_get_last_correspondences", "qb200_get_stage_ms", "qb200_get_kernel_ms",
-    "qb200_debug_tc_distances",
-    "qb200_debug_match_stats",
-    "qb200_debug_nn_tables",
-    "qb200_register_batch_enqueue",
-    "qb200_register_batch_flush",
-    "qb200_debug_tc_profile",
-    "qb200_debug_tc_footprint",
-    "qb200_solve_batch",
-    "qb200_comm_init_all", "qb200_register_batch_sharded", "qb200_comm_unique_id", "qb200_comm_init_rank",
-    "qb200_register_batch_rank", "qb200_comm_wait", "qb200_bind_numa",
-    "qb200_debug_match_verify", "qb200_get_last_features", "qb200_cache_reserve", "qb200_cache_scans", "qb200_register_cached", "qb200_cache_copy", "qb200_cache_read",
-    "qb200_register_batch_ex", "qb200_register_batch_enqueue_ex", "qb200_register_cached_ex", "qb200_solve_batch_ex",
-    "qb200_preprocess_batch",
-    "qb200_register_batch_each", "qb200_register_batch_enqueue_each", "qb200_register_cached_each", "qb200_solve_batch_each",
-]
 
 
 def default_params() -> Params:
@@ -313,15 +341,7 @@ def register_batch_sharded(handles: Sequence["Handle"], pairs: Sequence, params:
     """pairs: (src, tgt) numpy arrays (MEM_HOST) or (src_ptr, n_src, tgt_ptr, n_tgt) device tuples whose pair g lives on the device
     of handles[g % len(handles)].  Returns the records in the order of `pairs`."""
     n = len(pairs)
-    arr = (Pair * n)()
-    keep = []
-    for i, pr in enumerate(pairs):
-        if kind == MEM_HOST:
-            s, t = _f32(pr[0], 4), _f32(pr[1], 4)
-            keep.append((s, t))
-            arr[i].src, arr[i].n_src, arr[i].tgt, arr[i].n_tgt = s.ctypes.data, len(s), t.ctypes.data, len(t)
-        else:
-            arr[i].src, arr[i].n_src, arr[i].tgt, arr[i].n_tgt = pr[0], pr[1], pr[2], pr[3]
+    arr, keep = _pair_array(pairs, kind)
     out = np.zeros(n, RESULT_DTYPE)
     hs = (C.c_void_p * len(handles))(*[h.h for h in handles])
     st = load_library().qb200_register_batch_sharded(hs, len(handles), arr, n, C.byref(params), kind, _ptr(out))
@@ -459,12 +479,9 @@ class Handle:
         Returns (per scan a tuple (ground, nonground, valid, outlier) trimmed to min(count, cap), None for a NULL array;
         counts (n,4) int32; status (n,) int32)."""
         n = len(scans)
-        keep = [_f32(sc, 4) for sc in scans] if kind == MEM_HOST else None
-        sizes = [len(a) for a in keep] if kind == MEM_HOST else [int(sc[1]) for sc in scans]
-        ptrs = (C.c_void_p * max(n, 1))(*([a.ctypes.data for a in keep] if kind == MEM_HOST else [sc[0] for sc in scans]))
-        cnts = (C.c_int32 * max(n, 1))(*sizes)
+        ptrs, cnts, keep = _scan_arrays(scans, kind)
         if cap is None:
-            cap = max([1, *sizes] + ([sp.n_scan * sp.horizon_scan] if sp is not None else []))
+            cap = max([1, *cnts[:n]] + ([sp.n_scan * sp.horizon_scan] if sp is not None else []))
         if arrays is None:
             names = PREPROCESS_ARRAYS if sp is not None else PREPROCESS_ARRAYS[:2]
             if dest == MEM_HOST:
@@ -547,33 +564,8 @@ class Handle:
                          "qb200_register_pair")
         return res, st
 
-    @staticmethod
-    def pair_array(pairs: Sequence, kind: int = MEM_HOST):
-        """(Pair * n) array of `pairs` and the contiguous scans it points to (keep them alive while the array is in use)."""
-        arr = (Pair * len(pairs))()
-        keep = []
-        for i, pr in enumerate(pairs):
-            if kind == MEM_HOST:
-                s, t = _f32(pr[0], 4), _f32(pr[1], 4)
-                keep.append((s, t))
-                arr[i].src, arr[i].n_src, arr[i].tgt, arr[i].n_tgt = s.ctypes.data, len(s), t.ctypes.data, len(t)
-            else:
-                arr[i].src, arr[i].n_src, arr[i].tgt, arr[i].n_tgt = pr[0], pr[1], pr[2], pr[3]
-        return arr, keep
-
-    @staticmethod
-    def _set_array(sets: Sequence, kind: int):
-        arr = (CorrSet * len(sets))()
-        keep = []
-        for i, st in enumerate(sets):
-            if kind == MEM_HOST:
-                a, b = _f32(st[0], 4), _f32(st[1], 4)
-                assert len(a) == len(b)
-                keep.append((a, b))
-                arr[i].a, arr[i].b, arr[i].L = a.ctypes.data, b.ctypes.data, len(a)
-            else:
-                arr[i].a, arr[i].b, arr[i].L = st[0], st[1], st[2]
-        return arr, keep
+    pair_array = staticmethod(_pair_array)
+    _set_array = staticmethod(_set_array)
 
     def register_batch(self, pairs: Sequence, params: Params, kind: int = MEM_HOST) -> np.ndarray:
         """pairs: sequence of (src, tgt).  MEM_HOST: numpy (n,4) float32 arrays; MEM_DEVICE:
@@ -598,44 +590,37 @@ class Handle:
     def _lists_for(self, n: int, cap_per_pair: Optional[int], dest: int, buffers: Optional[ListBuffers], names) -> ListBuffers:
         return buffers or ListBuffers(n, cap_per_pair or self.cfg.max_corr, dest, names, self.cfg.device)
 
+    def _batch_lists(self, name: str, n: int, args: tuple, buffers: Optional[ListBuffers]):
+        """name(h, *args, records, lists) for n pairs -> (records, lists as ListBuffers.trimmed, or None without buffers)."""
+        out = np.zeros(n, RESULT_DTYPE)
+        self._check(getattr(self.lib, name)(self.h, *args, _ptr(out), self._lists_arg(buffers)), name)
+        return out, (None if buffers is None else buffers.trimmed(out))
+
     def register_batch_lists(self, pairs: Sequence, params: Params, kind: int = MEM_HOST, cap_per_pair: Optional[int] = None,
                              dest: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
         """qb200_register_batch_ex: register_batch + every pair's correspondences, matched points, clique, final inliers and masks."""
         arr, keep = self.pair_array(pairs, kind)
-        out = np.zeros(len(pairs), RESULT_DTYPE)
         lb = self._lists_for(len(pairs), cap_per_pair, dest, buffers, tuple(LIST_LAYOUT))
-        d = lb.descriptor()
-        self._check(self.lib.qb200_register_batch_ex(self.h, arr, len(pairs), C.byref(params), kind, _ptr(out), C.byref(d)),
-                    "qb200_register_batch_ex")
-        return out, lb.trimmed(out)
+        return self._batch_lists("qb200_register_batch_ex", len(pairs), (arr, len(pairs), C.byref(params), kind), lb)
 
     def register_batch_enqueue_lists_raw(self, pair_array, n: int, params: Params, kind: int, out: np.ndarray, buffers: ListBuffers):
         """qb200_register_batch_enqueue_ex: pair_array, its scans, `out` and the buffers must stay alive until register_batch_flush."""
-        d = buffers.descriptor()
-        return self._check(self.lib.qb200_register_batch_enqueue_ex(self.h, pair_array, n, C.byref(params), kind, _ptr(out), C.byref(d)),
-                           "qb200_register_batch_enqueue_ex")
+        return self._check(self.lib.qb200_register_batch_enqueue_ex(self.h, pair_array, n, C.byref(params), kind, _ptr(out),
+                                                                    self._lists_arg(buffers)), "qb200_register_batch_enqueue_ex")
 
     def register_cached_lists(self, slot_pairs, params: Params, cap_per_pair: Optional[int] = None, dest: int = MEM_HOST,
                               buffers: Optional[ListBuffers] = None):
         """qb200_register_cached_ex: corr indexes the voxel points cache_read returns."""
-        sp = np.ascontiguousarray(np.asarray(slot_pairs, np.int32).reshape(-1, 2))
-        out = np.zeros(len(sp), RESULT_DTYPE)
+        sp = _slot_array(slot_pairs)
         lb = self._lists_for(len(sp), cap_per_pair, dest, buffers, tuple(LIST_LAYOUT))
-        d = lb.descriptor()
-        self._check(self.lib.qb200_register_cached_ex(self.h, _ptr(sp), len(sp), C.byref(params), _ptr(out), C.byref(d)),
-                    "qb200_register_cached_ex")
-        return out, lb.trimmed(out)
+        return self._batch_lists("qb200_register_cached_ex", len(sp), (_ptr(sp), len(sp), C.byref(params)), lb)
 
     def solve_batch_lists(self, sets: Sequence, params: Params, kind: int = MEM_HOST, cap_per_pair: Optional[int] = None,
                           dest: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
         """qb200_solve_batch_ex: solve_batch + every set's clique, final inliers and masks (the caller has the correspondences)."""
         arr, keep = self._set_array(sets, kind)
-        out = np.zeros(len(sets), RESULT_DTYPE)
         lb = self._lists_for(len(sets), cap_per_pair, dest, buffers, SET_LISTS)
-        d = lb.descriptor()
-        self._check(self.lib.qb200_solve_batch_ex(self.h, arr, len(sets), C.byref(params), kind, _ptr(out), C.byref(d)),
-                    "qb200_solve_batch_ex")
-        return out, lb.trimmed(out)
+        return self._batch_lists("qb200_solve_batch_ex", len(sets), (arr, len(sets), C.byref(params), kind), lb)
 
     # ---- one Params per pair (the _each entry points) ----
     # params: one Params per pair (or set), in the order of the inputs.  buffers: the ListBuffers to fill, or None for records only.
@@ -653,10 +638,7 @@ class Handle:
         """qb200_register_batch_each: pair i is registered with params[i] (front-end fields equal in every entry)."""
         assert len(params) == len(pairs)
         arr, keep = self.pair_array(pairs, kind)
-        out = np.zeros(len(pairs), RESULT_DTYPE)
-        self._check(self.lib.qb200_register_batch_each(self.h, arr, len(pairs), self.params_array(params), kind, _ptr(out),
-                                                       self._lists_arg(buffers)), "qb200_register_batch_each")
-        return out, (None if buffers is None else buffers.trimmed(out))
+        return self._batch_lists("qb200_register_batch_each", len(pairs), (arr, len(pairs), self.params_array(params), kind), buffers)
 
     def register_batch_enqueue_each_raw(self, pair_array, n: int, params_array, kind: int, out: np.ndarray,
                                         buffers: Optional[ListBuffers] = None):
@@ -667,21 +649,15 @@ class Handle:
 
     def register_cached_each(self, slot_pairs, params: Sequence[Params], buffers: Optional[ListBuffers] = None):
         """qb200_register_cached_each: slot pair i is registered with params[i] (front-end fields: the ones the slots were cached with)."""
-        sp = np.ascontiguousarray(np.asarray(slot_pairs, np.int32).reshape(-1, 2))
+        sp = _slot_array(slot_pairs)
         assert len(params) == len(sp)
-        out = np.zeros(len(sp), RESULT_DTYPE)
-        self._check(self.lib.qb200_register_cached_each(self.h, _ptr(sp), len(sp), self.params_array(params), _ptr(out),
-                                                        self._lists_arg(buffers)), "qb200_register_cached_each")
-        return out, (None if buffers is None else buffers.trimmed(out))
+        return self._batch_lists("qb200_register_cached_each", len(sp), (_ptr(sp), len(sp), self.params_array(params)), buffers)
 
     def solve_batch_each(self, sets: Sequence, params: Sequence[Params], kind: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
         """qb200_solve_batch_each: set i is solved with params[i] (front-end fields ignored)."""
         assert len(params) == len(sets)
         arr, keep = self._set_array(sets, kind)
-        out = np.zeros(len(sets), RESULT_DTYPE)
-        self._check(self.lib.qb200_solve_batch_each(self.h, arr, len(sets), self.params_array(params), kind, _ptr(out),
-                                                    self._lists_arg(buffers)), "qb200_solve_batch_each")
-        return out, (None if buffers is None else buffers.trimmed(out))
+        return self._batch_lists("qb200_solve_batch_each", len(sets), (arr, len(sets), self.params_array(params), kind), buffers)
 
     def last_features(self, which: int, cap: Optional[int] = None):
         """(normals (n,4), descriptors (n,33)) of the source (0) / target (1) cloud of the last match_and_pack."""
@@ -699,14 +675,12 @@ class Handle:
     def cache_scans(self, scans: Sequence, slot_ids: Sequence[int], params: Params, kind: int = MEM_HOST):
         """scans: (n,4) float32 arrays (MEM_HOST) or (device_ptr, n) tuples (MEM_DEVICE)."""
         n = len(scans)
-        keep = [_f32(sc, 4) for sc in scans] if kind == MEM_HOST else None
-        ptrs = (C.c_void_p * n)(*([a.ctypes.data for a in keep] if kind == MEM_HOST else [sc[0] for sc in scans]))
-        cnts = (C.c_int32 * n)(*([len(a) for a in keep] if kind == MEM_HOST else [sc[1] for sc in scans]))
-        ids = (C.c_int32 * n)(*[int(x) for x in slot_ids])
+        ptrs, cnts, keep = _scan_arrays(scans, kind)
+        ids = (C.c_int32 * max(n, 1))(*[int(x) for x in slot_ids])
         self._check(self.lib.qb200_cache_scans(self.h, ptrs, cnts, ids, n, C.byref(params), kind), "qb200_cache_scans")
 
     def register_cached(self, slot_pairs, params: Params) -> np.ndarray:
-        sp = np.ascontiguousarray(np.asarray(slot_pairs, np.int32).reshape(-1, 2))
+        sp = _slot_array(slot_pairs)
         out = np.zeros(len(sp), RESULT_DTYPE)
         self._check(self.lib.qb200_register_cached(self.h, _ptr(sp), len(sp), C.byref(params), _ptr(out)), "qb200_register_cached")
         return out

@@ -335,24 +335,28 @@ int cache_copy(qb200_handle* h, Lane* L, int to_cache, int n_clouds) {
   return QB200_OK;
 }
 
-// ---- waves ----------------------------------------------------------------------------------------------------------------
-// What a wave starts from: pairs of raw scans (in `kind` memory), pairs of cached scans, or correspondence sets (in `kind`
-// memory).  Exactly one of the three is set.
-struct WaveInput {
+// ---- batch calls ----------------------------------------------------------------------------------------------------------
+// One batch call as its entry point received it.  Its input is n pairs of raw scans (in `kind` memory), n pairs of cached scans, or
+// n correspondence sets (in `kind` memory): exactly one of the three is set.  The entry points fill the fields up to `lists` in order.
+struct BatchCall {
   const qb200_pair* pairs = nullptr;
   const qb200_slot_pair* slots = nullptr;
   const qb200_corr_set* sets = nullptr;
+  int n = 0;
   qb200_mem_kind kind = QB200_MEM_HOST;
+  // the caller's params: one entry for the whole batch, or (each) one per pair
+  const qb200_params* caller = nullptr;
+  bool each = false;
+  qb200_result* results = nullptr;
+  // the batch's per-pair lists (qb200_pair_lists), nullptr = records only
+  const qb200_pair_lists* lists = nullptr;
+  // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved, laid out like `caller`; the front end
+  // reads params[0]: the front-end fields of every entry are equal.
+  const qb200_params* params = nullptr;
   // raw host scans of a multi-wave batch: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies queued on
   // several streams share the PCIe link, so every wave's scans would arrive late; on one stream they arrive wave after wave and
   // the first waves compute while the later ones are still crossing.
   cudaStream_t copy_stream = nullptr;
-  // the batch's per-pair lists (qb200_pair_lists), nullptr = records only
-  const qb200_pair_lists* lists = nullptr;
-  // the params the pairs are solved with, rotation noise bounds resolved: one entry for the whole batch, or (each) one per pair.  The
-  // front end reads params[0]: the front-end fields of every entry are equal.
-  const qb200_params* params = nullptr;
-  bool each = false;
 };
 
 // Host-kind lists: the lane's pinned staging block holds cap entries of every list for each slot.  It only grows, and a failed
@@ -409,19 +413,11 @@ int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
   if (l->cap_per_pair < 1 || l->cap_per_pair > h->cfg.max_corr) why = "cap_per_pair outside 1 .. max_corr";
   else if (l->kind != QB200_MEM_HOST && l->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the lists";
   else if (for_sets && (l->corr || l->src_matched4 || l->tgt_matched4)) why = "a correspondence-set batch has no corr / matched points to return";
-  else if (l->kind == QB200_MEM_DEVICE) {
-    if (((uintptr_t)l->corr & 7) || ((uintptr_t)l->src_matched4 & 15) || ((uintptr_t)l->tgt_matched4 & 15)) why = "device corr / matched points misaligned";
-    const void* arrays[] = {l->corr, l->src_matched4, l->tgt_matched4, l->clique, l->final_inliers, l->rot_inlier_mask, l->trans_inlier_mask};
-    for (const void* a : arrays) {
-      cudaPointerAttributes at;
-      if (!a || why) continue;
-      if (cudaPointerGetAttributes(&at, a) != cudaSuccess || at.device != h->cfg.device ||
-          (at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged)) {
-        cudaGetLastError();
-        why = "device list array is not memory of the handle's device";
-      }
-    }
-  }
+  else if (l->kind == QB200_MEM_DEVICE &&
+           !(device_array_of(h, l->corr, 8) && device_array_of(h, l->src_matched4, 16) && device_array_of(h, l->tgt_matched4, 16) &&
+             device_array_of(h, l->clique, 1) && device_array_of(h, l->final_inliers, 1) && device_array_of(h, l->rot_inlier_mask, 1) &&
+             device_array_of(h, l->trans_inlier_mask, 1)))
+    why = "device list array is misaligned or not memory of the handle's device";
   if (!why) return QB200_OK;
   h->fail(__FILE__, __LINE__, why);
   return QB200_ERR_BAD_ARG;
@@ -429,8 +425,8 @@ int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
 
 // Enqueue one wave (pairs [w0, w0 + np), np <= S) on lane L: the front of the wave its input needs (raw scans: H2D, K1..K6;
 // cached scans: the copy out of the cache, K6; correspondence sets: their H2D), then K8..K11 and the D2H of the result records.
-// No sync: wave_collect hands the records out to dst[w0...].  The lane's previous wave must have been collected.
-int wave_submit(qb200_handle* h, Lane* L, const WaveInput& in, int w0, int np, qb200_result* dst) {
+// No sync: wave_collect hands the records out to in.results[w0...].  The lane's previous wave must have been collected.
+int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   const int ncl = 2 * np;
   const qb200_params& p = in.params[0];
   int rc;
@@ -497,7 +493,7 @@ int wave_submit(qb200_handle* h, Lane* L, const WaveInput& in, int w0, int np, q
   cudaEventRecord(L->ev[8], L->stream);
   L->pend_w0 = w0;
   L->pend_np = np;
-  L->pend_dst = dst;
+  L->pend_dst = in.results;
   if (in.lists) L->pend_lists = *in.lists;
   else L->pend_lists.cap_per_pair = 0;
   // stage-time slots of qb200_get_stage_ms this wave reports: raw scans all eight, the other inputs their first stage to pose
@@ -561,19 +557,6 @@ int batch_flush(qb200_handle* h) {
   return rc;
 }
 
-// one wave at a time on lane 0, each collected before the next is submitted
-int run_waves(qb200_handle* h, const WaveInput& in, int n, qb200_result* results) {
-  reset_timers(h);
-  const int S = h->cfg.max_batch_slots;
-  for (int w0 = 0; w0 < n; w0 += S) {
-    int rc = wave_submit(h, h->lane[0].get(), in, w0, n - w0 < S ? n - w0 : S, results);
-    if (rc == QB200_OK) rc = wave_collect(h, h->lane[0].get());
-    if (rc) return rc;
-  }
-  if (n == 1) set_last(h, results[0]);
-  return QB200_OK;
-}
-
 // The params of a call: one entry for the whole batch, or (each) one per pair (n entries; NULL is fine when n == 0).  Every entry passes
 // params_ok; same_frontend: the call runs a front end or matches cached scans, so every entry carries the first entry's front-end
 // fields (voxel_size .. seed, bit for bit).
@@ -592,11 +575,11 @@ int check_params(qb200_handle* h, const qb200_params* p, int n, bool each, bool 
   return QB200_OK;
 }
 
-// The entries of a checked call with their rotation noise bounds resolved (resolve_params): the one entry, or every pair's in pair
-// order, as a sequence of single-pair calls in that order would latch them.  Empty on an allocation failure.
+// The entries of a checked call of n > 0 pairs with their rotation noise bounds resolved (resolve_params): the one entry, or every
+// pair's in pair order, as a sequence of single-pair calls in that order would latch them.  Empty on an allocation failure.
 std::unique_ptr<qb200_params[]> resolve_call(qb200_handle* h, const qb200_params* p, int n, bool each) {
   const int m = each ? n : 1;
-  std::unique_ptr<qb200_params[]> r(new (std::nothrow) qb200_params[m > 0 ? m : 1]);
+  std::unique_ptr<qb200_params[]> r(new (std::nothrow) qb200_params[m]);
   if (!r) {
     h->fail(__FILE__, __LINE__, "out of host memory for the params");
     return r;
@@ -605,51 +588,63 @@ std::unique_ptr<qb200_params[]> resolve_call(qb200_handle* h, const qb200_params
   return r;
 }
 
-int solve_batch_impl(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p, bool each, qb200_mem_kind kind,
-                     qb200_result* results, const qb200_pair_lists* lists) {
-  if (int rc = enter(h)) return rc;
-  if (n_sets < 0 || (n_sets > 0 && (!sets || !results))) return QB200_ERR_BAD_ARG;
-  if (int rc = check_params(h, p, n_sets, each, false)) return rc;
-  if (int rc = check_lists(h, lists, true)) return rc;
-  for (int i = 0; i < n_sets; ++i)
-    if (sets[i].L < 0 || sets[i].L > h->cfg.max_corr || (sets[i].L > 0 && (!sets[i].a || !sets[i].b))) {
-      h->fail(__FILE__, __LINE__, "correspondence set is null or exceeds max_corr");
-      return QB200_ERR_BAD_ARG;
-    }
-  WaveInput in;
-  in.sets = sets;
-  in.kind = kind;
-  in.lists = lists;
-  in.each = each;
-  if (n_sets == 0) return run_waves(h, in, 0, results);
-  const std::unique_ptr<qb200_params[]> pr = resolve_call(h, p, n_sets, each);
-  if (!pr) return QB200_ERR_CUDA;
-  in.params = pr.get();
-  return run_waves(h, in, n_sets, results);
-}
-
-// Queue a batch and return: waves rotate over the lanes, a lane is collected (its records copied out) only when it is needed
-// again, so the tail of one batch runs under the copies and front-end kernels of the next.  pairs' scans (host kind) and
-// `results` must stay valid until qb200_register_batch_flush (or a later enqueue / qb200_register_batch) has returned them.
-int enqueue_impl(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, bool each, qb200_mem_kind kind,
-                 qb200_result* results, const qb200_pair_lists* lists) {
-  if (!h || n_pairs < 0 || (n_pairs > 0 && (!pairs || !results))) return QB200_ERR_BAD_ARG;
-  if (int rc = check_params(h, p, n_pairs, each, true)) return rc;
-  if ((!each || n_pairs > 0) && !p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
-  if (int rc = check_lists(h, lists, false)) return rc;
-  const int S = h->cfg.max_batch_slots, R = h->cfg.max_raw_points;
-  for (int i = 0; i < n_pairs; ++i) {
-    if (pairs[i].n_src < 0 || pairs[i].n_tgt < 0 || pairs[i].n_src > R || pairs[i].n_tgt > R ||
-        (pairs[i].n_src > 0 && !pairs[i].src) || (pairs[i].n_tgt > 0 && !pairs[i].tgt)) {
-      h->fail(__FILE__, __LINE__, "pair has a null cloud or exceeds max_raw_points");
-      return QB200_ERR_BAD_ARG;
+// Every argument check of a batch call, in one order whatever its input, so that a call with several faults returns the same code:
+// counts and arrays, the params entries, the cross-check, the lists, then every pair or set.  A rejection names its fault in
+// qb200_last_error.
+int check_call(qb200_handle* h, const BatchCall& c) {
+  auto reject = [h](const char* why) {
+    h->fail(__FILE__, __LINE__, why);
+    return QB200_ERR_BAD_ARG;
+  };
+  if (c.n < 0) return reject("n < 0");
+  if (c.n > 0 && !c.pairs && !c.slots && !c.sets) return reject("the input array is null");
+  if (c.n > 0 && !c.results) return reject("the results array is null");
+  if (c.kind != QB200_MEM_HOST && c.kind != QB200_MEM_DEVICE) return reject("unknown memory kind of the inputs");
+  const qb200_params* p = c.caller;
+  if (int rc = check_params(h, p, c.n, c.each, !c.sets)) return rc;
+  if (!c.sets && (!c.each || c.n > 0) && !p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
+  if (int rc = check_lists(h, c.lists, c.sets != nullptr)) return rc;
+  const int R = h->cfg.max_raw_points;
+  for (int i = 0; i < c.n; ++i) {
+    if (c.pairs) {
+      const qb200_pair& q = c.pairs[i];
+      if (q.n_src < 0 || q.n_tgt < 0 || q.n_src > R || q.n_tgt > R || (q.n_src > 0 && !q.src) || (q.n_tgt > 0 && !q.tgt))
+        return reject("pair has a null cloud or exceeds max_raw_points");
+    } else if (c.slots) {
+      for (const int sl : {c.slots[i].src_slot, c.slots[i].tgt_slot}) {
+        if (sl < 0 || sl >= h->c_slots) return reject("slot outside qb200_cache_reserve()");
+        const float* sig = h->c_sig.get() + 4 * (size_t)sl;
+        if (sig[0] != p->voxel_size || sig[1] != p->normal_radius || sig[2] != p->fpfh_radius || sig[3] != lattice_cell(*p))
+          return reject("cached scan was computed with other front-end parameters (or the slot is empty)");
+      }
+    } else {
+      const qb200_corr_set& s = c.sets[i];
+      if (s.L < 0 || s.L > h->cfg.max_corr || (s.L > 0 && (!s.a || !s.b))) return reject("correspondence set is null or exceeds max_corr");
     }
   }
+  return QB200_OK;
+}
+
+// Check a batch call and queue it: its waves rotate over lanes, and a lane is collected (its records copied out) only when it is
+// needed again, so the tail of one batch runs under the copies and front-end kernels of the next.  Raw scans rotate over up to
+// h->max_lanes lanes.  Cached pairs and sets run on lane 0 alone, after the raw batches still queued are flushed: the slot table
+// h_slot_of_cloud is the handle's, and one lane keeps their schedule.  The caller's scans (host kind) and `results` must stay valid
+// until batch_flush (in qb200_register_batch_flush or the next call that is not an enqueue) has returned them.
+int enqueue_call(qb200_handle* h, BatchCall c) {
+  if (!h) return QB200_ERR_BAD_ARG;
+  int rc;
+  if (!c.pairs && (rc = enter(h))) return rc;
+  if ((rc = check_call(h, c))) return rc;
   cudaSetDevice(h->cfg.device);
   const bool pipelined = h->lanes_active > 0;  // waves of an earlier enqueue are still in flight
   if (!pipelined) reset_timers(h);
-  const std::unique_ptr<qb200_params[]> pr = resolve_call(h, p, n_pairs, each);
+  // An empty call resolves no params: the reference latches the rotation noise bound inside computeTransformation, which an empty
+  // batch never calls.
+  if (c.n == 0) return QB200_OK;
+  const std::unique_ptr<qb200_params[]> pr = resolve_call(h, c.caller, c.n, c.each);
   if (!pr) return QB200_ERR_CUDA;
+  c.params = pr.get();
+  const int S = h->cfg.max_batch_slots, lanes = c.pairs ? h->max_lanes : 1;
   // More than one wave: rotate over the lanes so that one wave's PCIe copies and single-warp solver tail run under the
   // other waves' dense kernels.  Results do not depend on the lane (no state is shared between waves).
   // Wave plan.  Host inputs: nothing can run before the first wave's scans crossed PCIe, so the batch opens with a quarter
@@ -657,8 +652,8 @@ int enqueue_impl(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, cons
   // (Closing with small waves as well does not pay: every wave carries the same single-warp solver tail.)
   int wave_n[64], n_waves = 0;
   {
-    int left = n_pairs;
-    if (kind == QB200_MEM_HOST && n_pairs > S && S >= 8 && h->max_lanes > 1) {
+    int left = c.n;
+    if (c.kind == QB200_MEM_HOST && c.n > S && S >= 8 && lanes > 1) {
       wave_n[n_waves++] = S / 4;
       wave_n[n_waves++] = S - S / 4;
       left -= S;
@@ -670,17 +665,15 @@ int enqueue_impl(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, cons
     if (left > 0) n_waves = 0;  // more than ~60 waves: no special opening, walk uniformly below
   }
   const bool planned = n_waves > 0;
-  if (!planned) n_waves = (n_pairs + S - 1) / S;
-  int n_lanes = n_waves < h->max_lanes ? (n_waves < 1 ? 1 : n_waves) : h->max_lanes;
+  if (!planned) n_waves = (c.n + S - 1) / S;
+  const int n_lanes = n_waves < lanes ? n_waves : lanes;
   if (pipelined && h->lanes_active != n_lanes) {  // a different lane count: start a fresh rotation
-    const int rc0 = batch_flush(h);
-    if (rc0) return rc0;
+    if ((rc = batch_flush(h))) return rc;
   }
   const bool fresh = h->lanes_active == 0;
   for (int l = 1; l < n_lanes; ++l) {
     if (!h->lane[l]) {
-      const int rc = lane_alloc(*h->lane[0], &h->lane[l]);
-      if (rc != QB200_OK) {
+      if ((rc = lane_alloc(*h->lane[0], &h->lane[l]))) {
         h->fail(__FILE__, __LINE__, "cannot allocate another lane");
         return rc;
       }
@@ -692,67 +685,32 @@ int enqueue_impl(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, cons
       QB_CUDA_TRY(h, cudaStreamWaitEvent(h->lane[l]->stream, h->ev_fork, 0));
     }
   }
-  WaveInput in;
-  in.pairs = pairs;
-  in.kind = kind;
-  in.lists = lists;
-  in.params = pr.get();
-  in.each = each;
   // host scans of a multi-wave batch: one copy stream, ordered after whatever the caller queued on lane 0's stream
-  if (kind == QB200_MEM_HOST && n_lanes > 1) {
-    in.copy_stream = h->copy_stream;
-    if (fresh) QB_CUDA_TRY(h, cudaStreamWaitEvent(in.copy_stream, h->ev_fork, 0));
+  if (c.kind == QB200_MEM_HOST && n_lanes > 1) {
+    c.copy_stream = h->copy_stream;
+    if (fresh) QB_CUDA_TRY(h, cudaStreamWaitEvent(c.copy_stream, h->ev_fork, 0));
   }
   h->lanes_active = n_lanes;
-  int rc = QB200_OK, wave = 0;
-  for (int w0 = 0; w0 < n_pairs && rc == QB200_OK; ++wave) {
+  for (int w0 = 0, wave = 0; w0 < c.n && rc == QB200_OK; ++wave) {
     Lane* L = h->lane[h->lane_cursor].get();
     int np = planned ? wave_n[wave] : S;
-    if (np > n_pairs - w0) np = n_pairs - w0;
+    if (np > c.n - w0) np = c.n - w0;
     if ((rc = wave_collect(h, L))) break;  // the lane's previous wave (its pinned tables are reused)
-    rc = wave_submit(h, L, in, w0, np, results);
+    rc = wave_submit(h, L, c, w0, np);
     h->lane_cursor = (h->lane_cursor + 1) % n_lanes;  // always the lane that has been busy longest
     w0 += np;
   }
   return rc;
 }
 
-int register_batch_impl(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, bool each, qb200_mem_kind kind,
-                        qb200_result* results, const qb200_pair_lists* lists) {
-  int rc = enqueue_impl(h, pairs, n_pairs, p, each, kind, results, lists);
-  const int rc2 = h ? batch_flush(h) : QB200_OK;  // on an error still wait for everything in flight (the copies read caller memory)
+// A blocking batch call: enqueue_call + batch_flush, which waits for everything in flight also after an error (the copies read caller
+// memory).  With one pair it also sets what qb200_get_last_* read.
+int run_call(qb200_handle* h, const BatchCall& c) {
+  int rc = enqueue_call(h, c);
+  const int rc2 = h ? batch_flush(h) : QB200_OK;
   if (rc == QB200_OK) rc = rc2;
-  if (rc != QB200_OK) return rc;
-  if (n_pairs == 1) set_last(h, results[0]);
-  return QB200_OK;
-}
-
-int register_cached_impl(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, bool each,
-                         qb200_result* results, const qb200_pair_lists* lists) {
-  if (int rc = enter(h)) return rc;
-  if (n_pairs < 0 || (n_pairs > 0 && (!pairs || !results))) return QB200_ERR_BAD_ARG;
-  if (int rc = check_params(h, p, n_pairs, each, true)) return rc;
-  if ((!each || n_pairs > 0) && !p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
-  if (int rc = check_lists(h, lists, false)) return rc;
-  for (int i = 0; i < n_pairs; ++i) {
-    const int sl[2] = {pairs[i].src_slot, pairs[i].tgt_slot};
-    for (int k = 0; k < 2; ++k) {
-      if (sl[k] < 0 || sl[k] >= h->c_slots) { h->fail(__FILE__, __LINE__, "slot outside qb200_cache_reserve()"); return QB200_ERR_BAD_ARG; }
-      const float* sig = h->c_sig.get() + 4 * (size_t)sl[k];
-      if (sig[0] != p->voxel_size || sig[1] != p->normal_radius || sig[2] != p->fpfh_radius || sig[3] != lattice_cell(*p)) {
-        h->fail(__FILE__, __LINE__, "cached scan was computed with other front-end parameters (or the slot is empty)");
-        return QB200_ERR_BAD_ARG;
-      }
-    }
-  }
-  const std::unique_ptr<qb200_params[]> pr = resolve_call(h, p, n_pairs, each);
-  if (!pr) return QB200_ERR_CUDA;
-  WaveInput in;
-  in.slots = pairs;
-  in.lists = lists;
-  in.params = pr.get();
-  in.each = each;
-  return run_waves(h, in, n_pairs, results);
+  if (rc == QB200_OK && c.n == 1) set_last(h, c.results[0]);
+  return rc;
 }
 
 }  // namespace
@@ -857,12 +815,12 @@ int qb200_solve_batch(qb200_handle* h, const qb200_corr_set* sets, int32_t n_set
 
 int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p, qb200_mem_kind kind,
                          qb200_result* results, const qb200_pair_lists* lists) {
-  return solve_batch_impl(h, sets, n_sets, p, false, kind, results, lists);
+  return run_call(h, {nullptr, nullptr, sets, n_sets, kind, p, false, results, lists});
 }
 
 int qb200_solve_batch_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params, qb200_mem_kind kind,
                            qb200_result* results, const qb200_pair_lists* lists) {
-  return solve_batch_impl(h, sets, n_sets, params, true, kind, results, lists);
+  return run_call(h, {nullptr, nullptr, sets, n_sets, kind, params, true, results, lists});
 }
 
 // ---- raw scans -> pose ------------------------------------------------------------------------------
@@ -875,27 +833,27 @@ int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pai
 
 int qb200_register_batch_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                             qb200_result* results, const qb200_pair_lists* lists) {
-  return register_batch_impl(h, pairs, n_pairs, p, false, kind, results, lists);
+  return run_call(h, {pairs, nullptr, nullptr, n_pairs, kind, p, false, results, lists});
 }
 
 int qb200_register_batch_each(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
                               qb200_result* results, const qb200_pair_lists* lists) {
-  return register_batch_impl(h, pairs, n_pairs, params, true, kind, results, lists);
+  return run_call(h, {pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists});
 }
 
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                                  qb200_result* results) {
-  return enqueue_impl(h, pairs, n_pairs, p, false, kind, results, nullptr);
+  return enqueue_call(h, {pairs, nullptr, nullptr, n_pairs, kind, p, false, results, nullptr});
 }
 
 int qb200_register_batch_enqueue_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                                     qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_impl(h, pairs, n_pairs, p, false, kind, results, lists);
+  return enqueue_call(h, {pairs, nullptr, nullptr, n_pairs, kind, p, false, results, lists});
 }
 
 int qb200_register_batch_enqueue_each(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                       qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_impl(h, pairs, n_pairs, params, true, kind, results, lists);
+  return enqueue_call(h, {pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists});
 }
 
 int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const float* tgt4, int32_t n_tgt, const qb200_params* p,
@@ -979,12 +937,12 @@ int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t
 
 int qb200_register_cached_ex(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_result* results,
                              const qb200_pair_lists* lists) {
-  return register_cached_impl(h, pairs, n_pairs, p, false, results, lists);
+  return run_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, p, false, results, lists});
 }
 
 int qb200_register_cached_each(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_result* results,
                                const qb200_pair_lists* lists) {
-  return register_cached_impl(h, pairs, n_pairs, params, true, results, lists);
+  return run_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists});
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {
@@ -1048,5 +1006,16 @@ int enter(qb200_handle* h) {
 int collect_batch(qb200_handle* h, const qb200_result* dst) {
   cudaSetDevice(h->cfg.device);
   return collect_waves(h, dst);
+}
+
+bool device_array_of(const qb200_handle* h, const void* a, size_t align) {
+  if (!a) return true;
+  if ((uintptr_t)a % align) return false;
+  cudaPointerAttributes at;
+  if (cudaPointerGetAttributes(&at, a) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return at.device == h->cfg.device && (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged);
 }
 }  // namespace qb

@@ -248,9 +248,10 @@ void comm_release(qb200_handle* h);
 int collect_batch(qb200_handle* h, const qb200_result* dst);  // api.cu: wait for every wave in flight that writes into dst[...]
 // api.cu, shared with the single-pair entry points of stages.cu
 int enter(qb200_handle* h);  // entry prologue: a handle, its device current, no enqueued batch in flight
+// a caller's array of QB200_MEM_DEVICE kind: device or managed memory of the handle's device, `align`-byte aligned (nullptr passes)
+bool device_array_of(const qb200_handle* h, const void* a, size_t align);
 int wave_reset(Lane* L, int n_clouds);
 int stage_raw(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs);
-int run_solver(Lane* L, int n_pairs, int have_frontend);  // pairs [0, n_pairs) with their entries in L->h_solve, uploaded
 int launch_degree(Lane* h, int n_pairs);
 bool params_ok(const qb200_params* p);
 float lattice_cell(const qb200_params& p);

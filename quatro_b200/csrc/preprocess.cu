@@ -775,18 +775,6 @@ static int preprocess_wave(Lane* L, int ns, qb200_mem_kind kind, const qb200_pat
   return QB200_OK;
 }
 
-// a caller's device output array: memory of the handle's device, 16-byte aligned (nullptr passes)
-static bool device_array_ok(const qb200_handle* h, const void* a) {
-  if (!a) return true;
-  cudaPointerAttributes at;
-  if ((uintptr_t)a & 15) return false;
-  if (cudaPointerGetAttributes(&at, a) != cudaSuccess) {
-    cudaGetLastError();
-    return false;
-  }
-  return at.device == h->cfg.device && (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged);
-}
-
 }  // namespace qb
 
 using namespace qb;
@@ -843,8 +831,8 @@ int qb200_preprocess_batch(qb200_handle* h, const float* const* scans4, const in
   else if (!out || !out->counts || !out->status) why = "no output descriptor, counts or status";
   else if (out->cap_per_scan < 1) why = "cap_per_scan < 1";
   else if (out->kind != QB200_MEM_HOST && out->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the outputs";
-  else if (out->kind == QB200_MEM_DEVICE && !(device_array_ok(h, out->ground4) && device_array_ok(h, out->nonground4) &&
-                                              device_array_ok(h, out->valid4) && device_array_ok(h, out->outlier4)))
+  else if (out->kind == QB200_MEM_DEVICE && !(device_array_of(h, out->ground4, 16) && device_array_of(h, out->nonground4, 16) &&
+                                              device_array_of(h, out->valid4, 16) && device_array_of(h, out->outlier4, 16)))
     why = "device output array is misaligned or not memory of the handle's device";
   Lane* L = h->lane[0].get();
   for (int i = 0; i < n_scans && !why; ++i)

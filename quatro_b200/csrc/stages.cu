@@ -273,23 +273,12 @@ int qb200_solve_pose(qb200_handle* h, const float* a4, const float* b4, int32_t 
   return res->status;
 }
 
-// ---- Quatro::computeTransformation ------------------------------------------------------------------
+// ---- Quatro::computeTransformation: a qb200_solve_batch of one set ------------------------------------
 int qb200_solve_correspondences(qb200_handle* h, const float* a4, const float* b4, int32_t L, const qb200_params* p, qb200_result* res) {
-  if (int rc = enter(h)) return rc;
-  if (!res || !params_ok(p) || L < 0 || (L > 0 && (!a4 || !b4))) return QB200_ERR_BAD_ARG;
-  Lane* ln = h->lane[0].get();
-  if (L > ln->Lc) { h->fail(__FILE__, __LINE__, "L exceeds max_corr"); return QB200_ERR_BAD_ARG; }
-  int rc = wave_reset(ln, 2);
-  if (rc) return rc;
-  if (L > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ln->ma, a4, (size_t)L * sizeof(float4), cudaMemcpyHostToDevice, ln->stream));
-  if (L > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ln->mb, b4, (size_t)L * sizeof(float4), cudaMemcpyHostToDevice, ln->stream));
-  MirrorHold hold{ln};
-  ln->h_solve[0] = solve_entry(resolve_params(h, *p));
-  if ((rc = write_counter(ln, ln->hctr.n_corr, L)) || (rc = upload_solve(ln, 1)) || (rc = run_solver(ln, 1, 0))) return rc;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(ln->h_results, ln->d_results, sizeof(qb200_result), cudaMemcpyDeviceToHost, ln->stream));
-  QB_CUDA_TRY(h, hold.sync());
-  *res = ln->h_results[0];
-  set_last(h, *res);
+  if (!res) return QB200_ERR_BAD_ARG;
+  const qb200_corr_set set = {a4, b4, L, 0};
+  const int rc = qb200_solve_batch(h, &set, 1, p, QB200_MEM_HOST, res);
+  if (rc != QB200_OK) return rc;
   return res->status;
 }
 

@@ -53,6 +53,18 @@ def assert_same_record(got, ref):
     assert np.allclose(pose(got), pose(ref), atol=1e-9, rtol=0)
 
 
+def same_lists(got: dict, want: dict):
+    """One pair's lists (dicts of arrays by list name): every list of `want` has the same shape and bytes in `got`."""
+    for name in want:
+        g, w = np.asarray(got[name]), np.asarray(want[name])
+        assert g.shape == w.shape and g.tobytes() == w.tobytes(), (name, g.shape, w.shape)
+
+
+def host_lists(lists):
+    """Per-pair lists with every CUDA tensor copied to a numpy array."""
+    return [{k: (v if isinstance(v, np.ndarray) else v.cpu().numpy()) for k, v in d.items()} for d in lists]
+
+
 def build_against_lib(tmp_path, source):
     """Compile the C++ file `source` (relative to the repository root) against include/ and link it to libquatro_b200, warnings as
     errors; returns the executable."""

@@ -9,7 +9,7 @@ import pytest
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (Handle, ListBuffers, LIST_LAYOUT, SET_LISTS, FLAG_LISTS_TRUNCATED, MEM_HOST, MEM_DEVICE, PMC_EXACT,
                               INLIER_NONE, RESULT_DTYPE, default_params)
-from support import build_against_lib
+from support import build_against_lib, host_lists, same_lists
 
 FIXTURE = "tests/fixtures/pair_lists_shim.cpp"
 
@@ -46,16 +46,6 @@ def oracle_lists(street, oracle):
     return out
 
 
-def _same_lists(got: dict, want: dict, names=None):
-    for name in names or want:
-        g, w = np.asarray(got[name]), np.asarray(want[name])
-        assert g.shape == w.shape and g.tobytes() == w.tobytes(), (name, g.shape, w.shape)
-
-
-def _host(lists):
-    return [{k: (v if isinstance(v, np.ndarray) else v.cpu().numpy()) for k, v in d.items()} for d in lists]
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("lanes", ["1", None])
 def test_batch_lists_match_oracle_and_single_pair(street, oracle_lists, monkeypatch, lanes):
@@ -70,11 +60,11 @@ def test_batch_lists_match_oracle_and_single_pair(street, oracle_lists, monkeypa
         assert not (recs["flags"] & FLAG_LISTS_TRUNCATED).any()
         for (src, tgt), r, got, want in zip(street, recs, lists, oracle_lists):
             assert r["status"] == 0 and r["n_final_inliers"] > 0
-            _same_lists(got, want)
+            same_lists(got, want)
             one, _ = h.register_pair(src, tgt, p)
             assert bytes(one) == r.tobytes()
             corr, sm, tm = h.last_correspondences()
-            _same_lists(got, {"corr": corr, "src_matched4": sm, "tgt_matched4": tm, "clique": h.last_clique(),
+            same_lists(got, {"corr": corr, "src_matched4": sm, "tgt_matched4": tm, "clique": h.last_clique(),
                               "final_inliers": h.last_final_inliers()})
         # one pair through _ex also sets what the single-pair getters read
         h.register_pair(*street[1], p)
@@ -125,8 +115,8 @@ def test_enqueue_ex_batches_land_in_their_own_arrays(street):
         for (recs, lists), out, lb in zip(ref, outs, bufs):
             assert out.tobytes() == recs.tobytes()
             if lb is not None:
-                for got, want in zip(_host(lb.trimmed(out)), lists):
-                    _same_lists(got, want)
+                for got, want in zip(host_lists(lb.trimmed(out)), lists):
+                    same_lists(got, want)
 
 
 @pytest.mark.gpu
@@ -141,7 +131,7 @@ def test_cached_lists_equal_batch_lists(street):
         crecs, clists = h.register_cached_lists(idx, p)
         assert crecs.tobytes() == recs.tobytes()
         for (a, b), got, want in zip(idx, clists, lists):
-            _same_lists(got, want)
+            same_lists(got, want)
             va, vb = h.cache_read(a)[0], h.cache_read(b)[0]
             assert np.array_equal(va[got["corr"][:, 0], :3], got["src_matched4"][:, :3])
             assert np.array_equal(vb[got["corr"][:, 1], :3], got["tgt_matched4"][:, :3])
@@ -167,14 +157,14 @@ def test_solve_batch_lists(oracle):
                 assert set(got) == set(SET_LISTS)
                 one, _ = h.solve_correspondences(a4, b4, p)
                 assert bytes(one) == r.tobytes()
-                _same_lists(got, {"clique": h.last_clique(), "final_inliers": h.last_final_inliers()})
+                same_lists(got, {"clique": h.last_clique(), "final_inliers": h.last_final_inliers()})
                 if len(a4) < 2:
                     # the oracle returns before it fills its sets; a degenerate clique has no solved masks
                     assert not got["rot_inlier_mask"].any() and not got["trans_inlier_mask"].any()
                     continue
                 _, _, clique, fin = oracle.solve_correspondences(a4, b4, p, want_sets=True)
                 _, rm, tm, _ = oracle.solve_pose(a4, b4, clique, p)
-                _same_lists(got, {"clique": clique, "final_inliers": fin, "rot_inlier_mask": rm, "trans_inlier_mask": tm})
+                same_lists(got, {"clique": clique, "final_inliers": fin, "rot_inlier_mask": rm, "trans_inlier_mask": tm})
             if mode is None:
                 assert recs["clique_size"][sizes.index(5000)] > 4096
                 dev = [(torch.from_numpy(np.ascontiguousarray(a)).cuda(), torch.from_numpy(np.ascontiguousarray(b)).cuda()) for a, b in sub]
@@ -182,8 +172,8 @@ def test_solve_batch_lists(oracle):
                 drecs, dlists = h.solve_batch_lists([(a.data_ptr() if len(a) else 0, b.data_ptr() if len(b) else 0, len(a)) for a, b in dev], p,
                                                     kind=MEM_DEVICE, dest=MEM_DEVICE)
                 assert drecs.tobytes() == recs.tobytes()
-                for got, want in zip(_host(dlists), lists):
-                    _same_lists(got, want)
+                for got, want in zip(host_lists(dlists), lists):
+                    same_lists(got, want)
         # the caller supplied the correspondences: asking for them back is refused
         lb = ListBuffers(2, 64, MEM_HOST, ("corr", "clique"))
         with pytest.raises(capi.QuatroB200Error) as e:

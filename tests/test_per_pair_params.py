@@ -10,7 +10,7 @@ import pytest
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (COTE_WEIGHTED_MEAN, FLAG_CLIQUE_TRUNCATED, INLIER_NONE, KCORE_HEU, LIST_LAYOUT, MEM_DEVICE, MEM_HOST,
                               PMC_EXACT, PMC_HEU, RESULT_DTYPE, SET_LISTS, Handle, ListBuffers, default_params)
-from support import ROOT, assert_same_record
+from support import ROOT, assert_same_record, host_lists, same_lists
 
 EACH = {"qb200_register_batch_each": "qb200_register_batch_ex", "qb200_register_batch_enqueue_each": "qb200_register_batch_enqueue_ex",
         "qb200_register_cached_each": "qb200_register_cached_ex", "qb200_solve_batch_each": "qb200_solve_batch_ex"}
@@ -82,16 +82,6 @@ def cycled(n, offset=0):
     return [SETS[(i + offset) % len(SETS)] for i in range(n)]
 
 
-def _same_lists(got: dict, want: dict):
-    for name in want:
-        g, w = np.asarray(got[name]), np.asarray(want[name])
-        assert g.shape == w.shape and g.tobytes() == w.tobytes(), (name, g.shape, w.shape)
-
-
-def _host(lists):
-    return [{k: (v if isinstance(v, np.ndarray) else v.cpu().numpy()) for k, v in d.items()} for d in lists]
-
-
 def _fresh_handle(monkeypatch, **kw):
     monkeypatch.delenv("QB200_LANES", raising=False)   # read when the handle is created
     return Handle(max_batch_slots=SLOTS, **kw)
@@ -123,7 +113,7 @@ def _check_against_broadcast(recs, lists, broadcast, index, params_index):
     for j, (i, k) in enumerate(zip(index, params_index)):
         want_recs, want_lists = broadcast[k]
         assert recs[j].tobytes() == want_recs[i].tobytes(), (j, i, k)
-        _same_lists(lists[j], want_lists[i])
+        same_lists(lists[j], want_lists[i])
 
 
 # ---- GPU: every _each call equals its broadcast equivalent, pair by pair ------------------------------------------------------------
@@ -170,7 +160,7 @@ def test_two_enqueued_each_batches_and_one_flush(h, street, broadcast):
     import torch
     torch.cuda.synchronize()
     for out, lb, (index, ks) in zip(outs, bufs, plans):
-        _check_against_broadcast(out, _host(lb.trimmed(out)), broadcast, index, ks)
+        _check_against_broadcast(out, host_lists(lb.trimmed(out)), broadcast, index, ks)
 
 
 @pytest.mark.gpu
