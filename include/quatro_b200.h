@@ -261,6 +261,19 @@ int qb200_preprocess_batch(qb200_handle* h, const float* const* scans4, const in
                            qb200_mem_kind kind, const qb200_patchwork_params* pp,
                            const qb200_segment_params* sp /* NULL: ground removal only */, const qb200_preprocess_out* out);
 
+/* qb200_preprocess_batch with one parameter entry per scan: pp[i] (and sp[i]) pre-process scan i.  pp and sp point to n_scans
+ * entries (NULL is fine when n_scans == 0); sp == NULL: ground removal only for every scan.  A batch of mixed sensors (each scan's
+ * own range image, as the reference builds one ImageProjection per cloud) or of per-scan mounting heights runs in one call.
+ * For every scan i each output array, count and status is byte-identical to qb200_preprocess_batch called on scan i alone with
+ * pp[i] / sp[i], on the same handle; nothing depends on the batch, the wave, the scan's position or the memory kinds.
+ * Every entry must pass the checks of qb200_preprocess_batch: a bad entry fails the whole call with QB200_ERR_BAD_ARG before any
+ * work starts (no count, status or output entry is written) and qb200_last_error names the entry.  cap_per_scan, the output
+ * descriptor, the memory kinds and QB200_CAPACITY_EXCEEDED behave as in qb200_preprocess_batch.  The parameter arrays are
+ * copied by the call. */
+int qb200_preprocess_batch_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
+                                qb200_mem_kind kind, const qb200_patchwork_params* pp, const qb200_segment_params* sp,
+                                const qb200_preprocess_out* out);
+
 /* normals4: n x {nx,ny,nz,curvature}; desc33: n x 33 floats (pcl::FPFHSignature33). Either may be NULL. */
 int qb200_compute_fpfh(qb200_handle* h, const float* pts4, int32_t n, float normal_radius,
                        float fpfh_radius, float grid_cell, float* normals4, float* desc33);

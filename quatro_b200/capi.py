@@ -232,6 +232,7 @@ _SIGNATURES = {
     "qb200_register_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_register_cached_each": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
     "qb200_solve_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_preprocess_batch_each": (i32, [vp, vp, vp, i32, i32, P(PatchworkParams), P(SegmentParams), P(PreprocessOut)]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -362,6 +363,24 @@ def default_segment_params() -> SegmentParams:
     return p
 
 
+# The reference's lidar models, as ImageProjection's constructor sets them (include/imageProjection.hpp:85-124): n_scan, horizon_scan,
+# ang_res_x, ang_res_y, ang_bottom (computed in double like the reference, stored as float)
+LIDAR_MODELS = {
+    "Velodyne-64-HDE": (64, 1800, 360.0 / 1800, 26.9 / 63, 25.0),
+    "VLP-16": (16, 1800, 0.2, 2.0, 15.0 + 0.1),
+    "HDL-32E": (32, 1800, 360.0 / 1800, 41.33 / 31, 30.67),
+    "Ouster-OS1-16": (16, 1024, 360.0 / 1024, 33.2 / 15, 16.6 + 0.1),
+    "Ouster-OS1-64": (64, 1024, 360.0 / 1024, 33.2 / 63, 16.6 + 0.1),
+}
+
+
+def lidar_segment_params(model: str) -> SegmentParams:
+    """The default segment parameters with the image of one of LIDAR_MODELS."""
+    p = default_segment_params()
+    p.n_scan, p.horizon_scan, p.ang_res_x, p.ang_res_y, p.ang_bottom = LIDAR_MODELS[model]
+    return p
+
+
 def default_config() -> Config:
     c = Config()
     c.device, c.max_batch_slots, c.max_raw_points, c.max_voxel_points, c.max_corr = 0, 64, 131072, 16384, 4096
@@ -478,12 +497,26 @@ class Handle:
         numpy (dest MEM_HOST) or CUDA tensors (dest MEM_DEVICE) of shape (n_scans, cap, 4); a name left out is passed as NULL.
         Returns (per scan a tuple (ground, nonground, valid, outlier) trimmed to min(count, cap), None for a NULL array;
         counts (n,4) int32; status (n,) int32)."""
+        return self._preprocess("qb200_preprocess_batch", scans, C.byref(pp), None if sp is None else C.byref(sp),
+                                [] if sp is None else [sp], cap, kind, dest, arrays)
+
+    def preprocess_batch_each(self, scans: Sequence, pps: Sequence["PatchworkParams"], sps: Optional[Sequence["SegmentParams"]] = None,
+                              cap: Optional[int] = None, kind: int = MEM_HOST, dest: int = MEM_HOST, arrays: Optional[dict] = None):
+        """qb200_preprocess_batch_each: preprocess_batch with pps[i] (and sps[i]) for scan i; sps None: ground removal only.  Returns
+        what preprocess_batch returns."""
+        n = len(scans)
+        pa = (PatchworkParams * n)(*pps) if n else None
+        sa = None if sps is None else ((SegmentParams * n)(*sps) if n else None)
+        return self._preprocess("qb200_preprocess_batch_each", scans, pa, sa, [] if sps is None else list(sps), cap, kind, dest, arrays)
+
+    def _preprocess(self, fn: str, scans, pp_arg, sp_arg, sps, cap, kind, dest, arrays):
+        """The two batch pre-processing calls: sps = the segment parameters in use (the default cap makes room for every image)."""
         n = len(scans)
         ptrs, cnts, keep = _scan_arrays(scans, kind)
         if cap is None:
-            cap = max([1, *cnts[:n]] + ([sp.n_scan * sp.horizon_scan] if sp is not None else []))
+            cap = max([1, *cnts[:n]] + [s.n_scan * s.horizon_scan for s in sps])
         if arrays is None:
-            names = PREPROCESS_ARRAYS if sp is not None else PREPROCESS_ARRAYS[:2]
+            names = PREPROCESS_ARRAYS if sp_arg is not None else PREPROCESS_ARRAYS[:2]
             if dest == MEM_HOST:
                 arrays = {k: np.zeros((max(n, 1), cap, 4), np.float32) for k in names}
             else:
@@ -495,8 +528,7 @@ class Handle:
         for k, a in arrays.items():
             setattr(out, k, a.ctypes.data if dest == MEM_HOST else a.data_ptr())
         out.counts, out.status = counts.ctypes.data, status.ctypes.data
-        self._check(self.lib.qb200_preprocess_batch(self.h, ptrs, cnts, n, kind, C.byref(pp), C.byref(sp) if sp is not None else None,
-                                                    C.byref(out)), "qb200_preprocess_batch")
+        self._check(getattr(self.lib, fn)(self.h, ptrs, cnts, n, kind, pp_arg, sp_arg, C.byref(out)), fn)
         per_scan = []
         for i in range(n):
             row = []

@@ -37,6 +37,8 @@ struct PairSolve {
   int reserved;
 };
 
+struct PpScan;   // one scan's pre-processing entry (preprocess.cu)
+
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
 // kernels of the others.  The lane owns its stream, buffers and events: deleting it releases them.
@@ -112,6 +114,7 @@ struct Lane {
   DeviceMem<PairSolve> d_solve; PinnedMem<PairSolve> h_solve;  // [S] solver table of the wave, and its pinned mirror (upload_solve copies it)
   // ---- pre-processing (preprocess.cu), allocated on first use for the largest wave so far (pw_scans / ip_cap) ----
   DeviceMem<int> pp_cnt; PinnedMem<int> pp_hcnt;  // [2S][8] per-scan counts and status of a wave, and its pinned mirror
+  DeviceMem<PpScan> d_pp; PinnedMem<PpScan> h_pp; // [2S] per-scan parameter table of a wave, and its pinned mirror (one H2D per wave)
   DeviceMem<int> pw_ints;     // [pw_scans] x (patch id / rank per point, per-patch counters and offsets)
   DeviceMem<float4> pw_out;   // [pw_scans][R] ground | non-ground
   int pw_scans;

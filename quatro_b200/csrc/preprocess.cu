@@ -29,10 +29,27 @@ constexpr int kPwStride = kPwMaxPatches + 1;   // per-scan entries of every per-
 // per-scan count block of a wave, [scan][kPpCnt]: ground, non-ground, patchwork status, valid, outlier (+ 3 spare)
 constexpr int kPpCnt = 8;
 
-struct PwDev {   // device copy of the parameters + derived table
+struct PwDev {   // one scan's parameters + the derived patch table
   qb200_patchwork_params p;
   int patch_base[QB200_PW_MAX_ZONES + 1];
   int n_patches;
+};
+
+struct IpDev {   // one scan's range-image parameters + the constants the host derives from them
+  qb200_segment_params p;
+  float sin_x, cos_x, sin_y, cos_y;
+  int nnb;
+  int nb[8][2];
+};
+
+// One scan's entry of a lane's pre-processing table (h_pp / d_pp, [2S]): what every kernel of the wave reads for its scan.  The range
+// image of scan s sits at pixel pix0 of the wave's per-pixel arrays (a prefix sum of n_scan * horizon_scan over the wave) and its
+// counts per block of 1024 pixels at block blk0, so a wave of small images reserves only what they need.
+struct PpScan {
+  PwDev pw;         // unused by qb200_segment_cloud
+  IpDev ip;         // unused without sub-cluster removal
+  long long pix0;
+  int blk0, npix;   // npix = n_scan * horizon_scan (0 without sub-cluster removal)
 };
 
 __host__ __device__ inline bool pw_params_valid(const qb200_patchwork_params& pp) {  // check_input_parameters_are_correct, :592-616
@@ -69,13 +86,15 @@ __device__ __forceinline__ int pw_patch_of(const float4 pt, const PwDev& c) {
   return c.patch_base[k] + ring * pp.num_sectors_each_zone[k] + sector;
 }
 
-// Every kernel serves a wave of scans: blockIdx.y (or the one CTA of the per-scan scans) is the scan s, and scan s's scratch sits at
-// fixed strides -- R points (patch_of, rank, items, the two outputs) and kPwStride patches (counts, starts, offsets) -- so that a
-// scan's results never depend on the wave it rides in.
-__global__ void __launch_bounds__(256) pw_bin_kernel(const float4* const* __restrict__ pts_of, const int* __restrict__ n_of, PwDev c, int R,
-                                                     int* __restrict__ patch_of, int* __restrict__ count) {
+// Every kernel serves a wave of scans: blockIdx.y (or the one CTA of the per-scan scans) is the scan s, it reads scan s's entry of the
+// table, and scan s's scratch sits at fixed strides -- R points (patch_of, rank, items, the two outputs) and kPwStride patches
+// (counts, starts, offsets) -- so that a scan's results never depend on the wave it rides in.  The per-patch grids cover the wave's
+// largest patch count; CTAs past their scan's count exit.
+__global__ void __launch_bounds__(256) pw_bin_kernel(const float4* const* __restrict__ pts_of, const int* __restrict__ n_of,
+                                                     const PpScan* __restrict__ tab, int R, int* __restrict__ patch_of, int* __restrict__ count) {
   const int s = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_of[s]) return;
+  const PwDev& c = tab[s].pw;
   const float4 p = pts_of[s][i];
   int pid = -1;
   // non-finite points never enter (D11); :356-368 drops everything below -1.8 sensor_height
@@ -85,8 +104,10 @@ __global__ void __launch_bounds__(256) pw_bin_kernel(const float4* const* __rest
 }
 
 // one CTA per scan: start[] = exclusive scan of count[0..np), start[np] = total; cursor = copy of start
-__global__ void __launch_bounds__(1024) pw_scan_kernel(const int* __restrict__ count, int np, int* __restrict__ start, int* __restrict__ cursor) {
+__global__ void __launch_bounds__(1024) pw_scan_kernel(const int* __restrict__ count, const PpScan* __restrict__ tab, int* __restrict__ start,
+                                                       int* __restrict__ cursor) {
   __shared__ int sm[33];
+  const int np = tab[blockIdx.x].pw.n_patches;
   const size_t o = (size_t)blockIdx.x * kPwStride;
   count += o; start += o; cursor += o;
   int carry = 0;
@@ -152,10 +173,17 @@ __device__ __forceinline__ void pw_plane_from_accu(float accu[9], int cnt, float
 }
 
 // One CTA per (patch, scan).  keys: sorted (z | index); flag[p] = sorted position p belongs to the current ground set.
-__global__ void __launch_bounds__(kPwThreads) pw_patch_kernel(const float4* const* __restrict__ pts_of, PwDev c, int R,
+__global__ void __launch_bounds__(kPwThreads) pw_patch_kernel(const float4* const* __restrict__ pts_of, const PpScan* __restrict__ tab, int R,
                                                               const int* __restrict__ start, unsigned long long* __restrict__ items,
                                                               int cap_pow2, int* __restrict__ n_ground, int* __restrict__ n_nonground,
                                                               int* __restrict__ rank_out, int* __restrict__ cnt) {
+  if ((int)blockIdx.x >= tab[blockIdx.y].pw.n_patches) return;
+  // the scan's entry in shared memory: the serial sections below (one thread) read it where they use it, at shared-memory latency
+  __shared__ PwDev s_entry;
+  for (int w = threadIdx.x; w < (int)(sizeof(PwDev) / 4); w += blockDim.x)
+    reinterpret_cast<int*>(&s_entry)[w] = reinterpret_cast<const int*>(&tab[blockIdx.y].pw)[w];
+  __syncthreads();
+  const PwDev& c = s_entry;
   extern __shared__ __align__(16) unsigned char pw_smem[];
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(pw_smem);   // [cap_pow2]
   unsigned char* flag = reinterpret_cast<unsigned char*>(keys + cap_pow2);     // [cap_pow2]
@@ -329,9 +357,11 @@ __global__ void __launch_bounds__(kPwThreads) pw_patch_kernel(const float4* cons
 }
 
 // one CTA per scan: exclusive scans of the per-patch output counts; totals -> cnt[0] (ground), cnt[1] (non-ground)
-__global__ void __launch_bounds__(1024) pw_offsets_kernel(const int* __restrict__ n_ground, const int* __restrict__ n_nonground, int np,
-                                                          int* __restrict__ goff, int* __restrict__ ngoff, int* __restrict__ cnt) {
+__global__ void __launch_bounds__(1024) pw_offsets_kernel(const int* __restrict__ n_ground, const int* __restrict__ n_nonground,
+                                                          const PpScan* __restrict__ tab, int* __restrict__ goff, int* __restrict__ ngoff,
+                                                          int* __restrict__ cnt) {
   __shared__ int sm[33];
+  const int np = tab[blockIdx.x].pw.n_patches;
   const size_t o = (size_t)blockIdx.x * kPwStride;
   n_ground += o; n_nonground += o; goff += o; ngoff += o;
   int cg = 0, cn = 0;
@@ -356,12 +386,13 @@ struct PpDev {
 };
 
 // one CTA per (patch, scan): scan s's outputs go to out[s * R ...]: ground at [0, n_ground), non-ground at [n_ground, n_ground + n_nonground)
-__global__ void __launch_bounds__(256) pw_gather_kernel(const float4* const* __restrict__ pts_of, int R, const int* __restrict__ start,
-                                                        const int* __restrict__ n_ground, const int* __restrict__ n_nonground,
-                                                        const unsigned long long* __restrict__ items, const int* __restrict__ rank,
-                                                        const int* __restrict__ goff, const int* __restrict__ ngoff, const int* __restrict__ cnt,
-                                                        float4* __restrict__ out, PpDev dst) {
+__global__ void __launch_bounds__(256) pw_gather_kernel(const float4* const* __restrict__ pts_of, const PpScan* __restrict__ tab, int R,
+                                                        const int* __restrict__ start, const int* __restrict__ n_ground,
+                                                        const int* __restrict__ n_nonground, const unsigned long long* __restrict__ items,
+                                                        const int* __restrict__ rank, const int* __restrict__ goff, const int* __restrict__ ngoff,
+                                                        const int* __restrict__ cnt, float4* __restrict__ out, PpDev dst) {
   const int pid = blockIdx.x, scan = blockIdx.y;
+  if (pid >= tab[scan].pw.n_patches) return;
   const size_t po = (size_t)scan * kPwStride + pid, ro = (size_t)scan * R;
   if (n_ground[po] + n_nonground[po] == 0) return;
   const float4* __restrict__ pts = pts_of[scan];
@@ -396,13 +427,6 @@ __global__ void __launch_bounds__(256) pw_gather_kernel(const float4* const* __r
 //   ip_kind_kernel     feasibility of every pixel's segment (:559-571), counts per block of 1024 pixels
 //   ip_extract_kernel  the two outputs in row-major order (:424-481): block base from the counts, one block scan inside
 // ------------------------------------------------------------------------------------------------
-struct IpDev {
-  qb200_segment_params p;
-  float sin_x, cos_x, sin_y, cos_y;
-  int nnb;
-  int nb[8][2];
-};
-
 __device__ __forceinline__ bool ip_project(const float4 pt, const qb200_segment_params& sp, int* row, int* col, float* range) {
   const float vert = (float)((double)(qb_atan2f(pt.z, sqrtf(pt.x * pt.x + pt.y * pt.y)) * 180.0f) / 3.14159265358979323846);
   const float rf = (vert + sp.ang_bottom) / sp.ang_res_y;
@@ -440,24 +464,27 @@ __device__ __forceinline__ const float4* ip_input(const IpIn& in, int s, int* n)
   return in.ptr[s];
 }
 
-// blockIdx.y = scan; every per-pixel array holds npix entries per scan
-__global__ void __launch_bounds__(256) ip_project_kernel(IpIn in, IpDev c, int* __restrict__ winner) {
+// blockIdx.y = scan; scan s's per-pixel entries are [tab[s].pix0, tab[s].pix0 + tab[s].npix) of every per-pixel array.  The
+// per-pixel grids cover the wave's largest image; threads past their scan's image exit.
+__global__ void __launch_bounds__(256) ip_project_kernel(IpIn in, const PpScan* __restrict__ tab, int* __restrict__ winner) {
   const int s = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   int n;
   const float4* pts = ip_input(in, s, &n);
   if (i >= n) return;
   const float4 p = pts[i];
   if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z))) return;   // copyPointCloud, :260-266
+  const PpScan& e = tab[s];
   int r, col; float rg;
-  if (!ip_project(p, c.p, &r, &col, &rg)) return;
-  atomicMax(&winner[(size_t)s * c.p.n_scan * c.p.horizon_scan + r * c.p.horizon_scan + col], i);
+  if (!ip_project(p, e.ip.p, &r, &col, &rg)) return;
+  atomicMax(&winner[(size_t)e.pix0 + r * e.ip.p.horizon_scan + col], i);
 }
 
-__global__ void __launch_bounds__(256) ip_range_kernel(IpIn in, int npix, const int* __restrict__ winner, float* __restrict__ range,
-                                                       int* __restrict__ parent, int* __restrict__ size, unsigned long long* __restrict__ rows) {
+__global__ void __launch_bounds__(256) ip_range_kernel(IpIn in, const PpScan* __restrict__ tab, const int* __restrict__ winner,
+                                                       float* __restrict__ range, int* __restrict__ parent, int* __restrict__ size,
+                                                       unsigned long long* __restrict__ rows) {
   const int s = blockIdx.y, q = blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= npix) return;
-  const size_t o = (size_t)s * npix + q;
+  if (q >= tab[s].npix) return;
+  const size_t o = (size_t)tab[s].pix0 + q;
   const int w = winner[o];
   float rg = FLT_MAX;
   if (w >= 0) {
@@ -479,11 +506,12 @@ __device__ __forceinline__ int ip_find(const int* parent, int a) {
   }
 }
 
-__global__ void __launch_bounds__(256) ip_union_kernel(int npix, IpDev c, const float* __restrict__ range, int* parent) {
+__global__ void __launch_bounds__(256) ip_union_kernel(const PpScan* __restrict__ tab, const float* __restrict__ range, int* parent) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= npix) return;
-  range += (size_t)blockIdx.y * npix;
-  parent += (size_t)blockIdx.y * npix;
+  if (q >= tab[blockIdx.y].npix) return;
+  const IpDev& c = tab[blockIdx.y].ip;
+  range += (size_t)tab[blockIdx.y].pix0;
+  parent += (size_t)tab[blockIdx.y].pix0;
   const float ra = range[q];
   if (ra == FLT_MAX) return;
   const int H = c.p.n_scan, Wd = c.p.horizon_scan;
@@ -515,10 +543,12 @@ __global__ void __launch_bounds__(256) ip_union_kernel(int npix, IpDev c, const 
   }
 }
 
-__global__ void __launch_bounds__(256) ip_stats_kernel(int npix, int Wd, int* parent, int* __restrict__ size, unsigned long long* __restrict__ rows) {
+__global__ void __launch_bounds__(256) ip_stats_kernel(const PpScan* __restrict__ tab, int* parent, int* __restrict__ size,
+                                                       unsigned long long* __restrict__ rows) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= npix) return;
-  const size_t o = (size_t)blockIdx.y * npix;
+  if (q >= tab[blockIdx.y].npix) return;
+  const int Wd = tab[blockIdx.y].ip.p.horizon_scan;
+  const size_t o = (size_t)tab[blockIdx.y].pix0;
   parent += o; size += o; rows += o;
   if (((volatile int*)parent)[q] < 0) return;
   const int root = ip_find(parent, q);
@@ -527,23 +557,26 @@ __global__ void __launch_bounds__(256) ip_stats_kernel(int npix, int Wd, int* pa
 }
 
 // feasibility of every occupied pixel's segment (:559-571) -> kind[] (0 empty, 1 valid segment, 2 outlier) and the two counts of
-// every block of 1024 pixels (blk_cnt: 2 * gridDim.x entries per scan)
-__global__ void __launch_bounds__(1024) ip_kind_kernel(int npix, IpDev c, const int* __restrict__ winner, const int* parent, const int* __restrict__ size,
-                                                       const unsigned long long* __restrict__ rows, unsigned char* __restrict__ kind_out,
-                                                       int* __restrict__ blk_cnt) {
+// every block of 1024 pixels (blk_cnt: 2 entries per block, scan s's blocks from tab[s].blk0 on)
+__global__ void __launch_bounds__(1024) ip_kind_kernel(const PpScan* __restrict__ tab, const int* __restrict__ winner, const int* parent,
+                                                       const int* __restrict__ size, const unsigned long long* __restrict__ rows,
+                                                       unsigned char* __restrict__ kind_out, int* __restrict__ blk_cnt) {
+  const PpScan& e = tab[blockIdx.y];
+  const int npix = e.npix;
+  if ((int)blockIdx.x * 1024 >= npix) return;   // past the scan's image: the whole CTA
   __shared__ int s_v, s_o;
   if (threadIdx.x == 0) { s_v = 0; s_o = 0; }
   __syncthreads();
-  const size_t o = (size_t)blockIdx.y * npix;
+  const size_t o = (size_t)e.pix0;
   winner += o; parent += o; size += o; rows += o; kind_out += o;
-  blk_cnt += (size_t)blockIdx.y * 2 * gridDim.x;
+  blk_cnt += (size_t)2 * e.blk0;
   const int q = blockIdx.x * 1024 + threadIdx.x;
   int kind = 0;
   if (q < npix && winner[q] >= 0) {
     const int root = ip_find(parent, q);
     const int sz = size[root];
-    bool feasible = sz >= c.p.min_pts_for_subclustering;
-    if (!feasible && sz >= c.p.segment_valid_point_num) feasible = __popcll(rows[root]) >= c.p.segment_valid_line_num;
+    bool feasible = sz >= e.ip.p.min_pts_for_subclustering;
+    if (!feasible && sz >= e.ip.p.segment_valid_point_num) feasible = __popcll(rows[root]) >= e.ip.p.segment_valid_line_num;
     kind = feasible ? 1 : 2;
   }
   if (q < npix) kind_out[q] = (unsigned char)kind;
@@ -557,18 +590,20 @@ __global__ void __launch_bounds__(1024) ip_kind_kernel(int npix, IpDev c, const 
 }
 
 // ordered extraction (row-major, :424-481): block base = counts of the preceding blocks, one block scan inside.  Scan s's outputs go
-// to out[s * npix ...]: valid segments at [0, n_valid), outliers at [n_valid, n_valid + n_outlier); counts -> cnt[s][3], cnt[s][4].
-__global__ void __launch_bounds__(1024) ip_extract_kernel(IpIn in, int npix, const int* __restrict__ winner,
+// to out[pix0 ...]: valid segments at [0, n_valid), outliers at [n_valid, n_valid + n_outlier); counts -> cnt[s][3], cnt[s][4].
+__global__ void __launch_bounds__(1024) ip_extract_kernel(IpIn in, const PpScan* __restrict__ tab, const int* __restrict__ winner,
                                                           const unsigned char* __restrict__ kind_in, const int* __restrict__ blk_cnt,
                                                           float4* __restrict__ out, int* __restrict__ cnt, PpDev dst) {
   __shared__ int sm[33];
   __shared__ int s_base[3];
   const int scan = blockIdx.y;
-  const size_t o = (size_t)scan * npix;
+  const int npix = tab[scan].npix, nblk = (npix + 1023) / 1024;
+  if ((int)blockIdx.x >= nblk) return;   // past the scan's image: the whole CTA
+  const size_t o = (size_t)tab[scan].pix0;
   winner += o; kind_in += o; out += o;
-  blk_cnt += (size_t)scan * 2 * gridDim.x;
+  blk_cnt += (size_t)2 * tab[scan].blk0;
   int bv = 0, bo = 0, tv = 0;
-  for (int b = threadIdx.x; b < (int)gridDim.x; b += 1024) {
+  for (int b = threadIdx.x; b < nblk; b += 1024) {
     if (b < (int)blockIdx.x) { bv += blk_cnt[2 * b]; bo += blk_cnt[2 * b + 1]; }
     tv += blk_cnt[2 * b];
   }
@@ -593,7 +628,7 @@ __global__ void __launch_bounds__(1024) ip_extract_kernel(IpIn in, int npix, con
     float4* d = kind == 1 ? dst.arr[2] : dst.arr[3];
     if (d && pos < dst.cap) d[scan * dst.cap + pos] = p;
   }
-  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) {
+  if ((int)blockIdx.x == nblk - 1 && threadIdx.x == 0) {
     cnt[(size_t)scan * kPpCnt + 3] = s_base[0] + (both & 0xFFFF);
     cnt[(size_t)scan * kPpCnt + 4] = s_base[1] + (both >> 16);
   }
@@ -606,27 +641,29 @@ static bool ip_params_valid(const qb200_segment_params& sp) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Waves.  One launch sequence serves up to 2S scans; the three entry points below run their scans through it on lane 0.
+// Waves.  One launch sequence serves up to 2S scans; the four entry points below run their scans through it on lane 0.
 // ------------------------------------------------------------------------------------------------
-// range-image scratch of ns scans of npix pixels: per pixel the output (float4), the row set (u64), winner, parent, size (int), range
-// (float), kind (u8); per scan the counts of every block of 1024 pixels
-static size_t ip_bytes(int npix, int ns) {
-  return (size_t)ns * ((size_t)npix * (16 + 8 + 4 * 4 + 1) + 8 * (size_t)((npix + 1023) / 1024)) + 64;
-}
+// range-image scratch of a wave whose images have pix pixels and blk blocks of 1024 pixels in all: per pixel the output (float4), the
+// row set (u64), winner, parent, size (int), range (float), kind (u8); per block its two counts
+static size_t ip_bytes(long long pix, long long blk) { return (size_t)pix * (16 + 8 + 4 * 4 + 1) + 8 * (size_t)blk + 64; }
 
-// Scratch of a wave of ns scans, grown on demand (a lane that never pre-processes holds none).  Each group -- the count block and
-// its pinned mirror, the patchwork buffers, the range-image buffer -- is allocated whole or not at all: a failed call leaves a group
-// either as it was or empty, and the next call allocates it again.
-static int ensure_pp_scratch(Lane* L, int ns, bool pw, int npix) {
+// Scratch of a wave of ns scans, grown on demand (a lane that never pre-processes holds none).  Each group -- the count block, the
+// parameter table and their pinned mirrors, the patchwork buffers, the range-image buffer (ipb bytes, 0 = none) -- is allocated whole
+// or not at all: a failed call leaves a group either as it was or empty, and the next call allocates it again.
+static int ensure_pp_scratch(Lane* L, int ns, bool pw, size_t ipb) {
   const int C = 2 * L->S;
-  const bool grow_pw = pw && ns > L->pw_scans, grow_ip = npix > 0 && ip_bytes(npix, ns) > L->ip_cap;
+  const bool grow_pw = pw && ns > L->pw_scans, grow_ip = ipb > L->ip_cap;
   DeviceMem<int> cnt, ints;
   PinnedMem<int> hcnt;
+  DeviceMem<PpScan> tab;
+  PinnedMem<PpScan> htab;
   DeviceMem<float4> out;
   DeviceMem<void> ip;
   if (!L->pp_cnt) {
     QB_CUDA_TRY(L, cnt.alloc((size_t)C * kPpCnt));
     QB_CUDA_TRY(L, hcnt.alloc((size_t)C * kPpCnt));
+    QB_CUDA_TRY(L, tab.alloc(C));
+    QB_CUDA_TRY(L, htab.alloc(C));
   }
   if (grow_pw) {
     // the old buffers are idle (every wave ends in a sync): they go first, so the device never holds both
@@ -639,68 +676,29 @@ static int ensure_pp_scratch(Lane* L, int ns, bool pw, int npix) {
   if (grow_ip) {
     L->ip_buf.reset();
     L->ip_cap = 0;
-    QB_CUDA_TRY(L, ip.alloc_bytes(ip_bytes(npix, ns)));
+    QB_CUDA_TRY(L, ip.alloc_bytes(ipb));
   }
-  if (!L->pp_cnt) { L->pp_cnt = std::move(cnt); L->pp_hcnt = std::move(hcnt); }
+  if (!L->pp_cnt) { L->pp_cnt = std::move(cnt); L->pp_hcnt = std::move(hcnt); L->d_pp = std::move(tab); L->h_pp = std::move(htab); }
   if (grow_pw) { L->pw_ints = std::move(ints); L->pw_out = std::move(out); L->pw_scans = ns; }
-  if (grow_ip) { L->ip_buf = std::move(ip); L->ip_cap = ip_bytes(npix, ns); }
+  if (grow_ip) { L->ip_buf = std::move(ip); L->ip_cap = ipb; }
   return QB200_OK;
 }
 
-// Enqueue ground removal of the wave's scans [0, ns) (cloud tables of stage_raw); scan s's outputs -> pw_out + s * R, its counts and
-// status -> pp_cnt[s].  Launches do not depend on ns or on the scans' sizes.
-static int launch_patchwork_wave(Lane* L, int ns, int max_n, const qb200_patchwork_params& pp, const PpDev& dst) {
+// a scan's Patchwork entry: its parameters and the first patch of every zone
+static PwDev pw_entry(const qb200_patchwork_params& pp) {
   PwDev c;
   c.p = pp;
   c.patch_base[0] = 0;
   for (int k = 0; k < 4; ++k) c.patch_base[k + 1] = c.patch_base[k] + pp.num_sectors_each_zone[k] * pp.num_rings_each_zone[k];
   c.n_patches = c.patch_base[4];
-  const int NP = c.n_patches, R = L->R;
-  const size_t P = (size_t)L->pw_scans * kPwStride;
-  int* patch_of = L->pw_ints;
-  int* rank = patch_of + (size_t)L->pw_scans * R;
-  int* count = rank + (size_t)L->pw_scans * R;
-  int* start = count + P;
-  int* cursor = start + P;
-  int* ng_ground = cursor + P;
-  int* ng_non = ng_ground + P;
-  int* goff = ng_non + P;
-  int* ngoff = goff + P;
-  unsigned long long* items = reinterpret_cast<unsigned long long*>(L->key_a.get());   // [2S * R] >= [ns * R]
-  QB_CUDA_TRY(L, cudaMemsetAsync(count, 0, (size_t)ns * kPwStride * sizeof(int), L->stream));
-  const dim3 gp((max_n + 255) / 256 > 0 ? (max_n + 255) / 256 : 1, ns);
-  pw_bin_kernel<<<gp, 256, 0, L->stream>>>(L->d_cloud_ptr, L->d_cloud_n, c, R, patch_of, count);
-  pw_scan_kernel<<<ns, 1024, 0, L->stream>>>(count, NP, start, cursor);
-  pw_scatter_kernel<<<gp, 256, 0, L->stream>>>(L->d_cloud_ptr, L->d_cloud_n, R, patch_of, cursor, items);
-  const size_t smem = (size_t)kPwMaxPatchPts * 9;
-  QB_CUDA_TRY(L, ensure_dyn_smem(L->device, (const void*)pw_patch_kernel, smem));
-  pw_patch_kernel<<<dim3(NP, ns), kPwThreads, smem, L->stream>>>(L->d_cloud_ptr, c, R, start, items, kPwMaxPatchPts, ng_ground, ng_non, rank,
-                                                                 L->pp_cnt);
-  pw_offsets_kernel<<<ns, 1024, 0, L->stream>>>(ng_ground, ng_non, NP, goff, ngoff, L->pp_cnt);
-  pw_gather_kernel<<<dim3(NP, ns), 256, 0, L->stream>>>(L->d_cloud_ptr, R, start, ng_ground, ng_non, items, rank, goff, ngoff, L->pp_cnt,
-                                                        L->pw_out, dst);
-  L->launches += 6;
-  QB_CUDA_TRY(L, cudaGetLastError());
-  return QB200_OK;
+  return c;
 }
 
-// Enqueue sub-cluster removal of the wave's scans [0, ns) read through `in`; scan s's outputs -> the range-image scratch + s * npix,
-// its counts -> pp_cnt[s].  max_n bounds every scan's point count.
-static int launch_segment_wave(Lane* L, int ns, int max_n, const IpIn& in, const qb200_segment_params& sp, const PpDev& dst) {
-  const int npix = sp.n_scan * sp.horizon_scan, nblk = (npix + 1023) / 1024;
-  const size_t NPX = (size_t)ns * npix;
-  unsigned char* b = reinterpret_cast<unsigned char*>(L->ip_buf.get());
-  float4* out = reinterpret_cast<float4*>(b); b += NPX * 16;      // 16-byte records first: aligned for any image size
-  unsigned long long* rows = reinterpret_cast<unsigned long long*>(b); b += NPX * 8;
-  int* winner = reinterpret_cast<int*>(b); b += NPX * 4;
-  int* parent = reinterpret_cast<int*>(b); b += NPX * 4;
-  int* size = reinterpret_cast<int*>(b); b += NPX * 4;
-  float* range = reinterpret_cast<float*>(b); b += NPX * 4;
-  int* blk_cnt = reinterpret_cast<int*>(b); b += 8 * (size_t)ns * nblk;
-  unsigned char* kind = b;
+// a scan's range-image entry: its parameters, segmentAlphaX / segmentAlphaY's sine and cosine (:132-133, :535-541, evaluated on the
+// host) and the neighbour offsets of its mode
+static IpDev ip_entry(const qb200_segment_params& sp) {
   IpDev c;
   c.p = sp;
-  // segmentAlphaX / segmentAlphaY and their sine / cosine (:132-133, :535-541): constants of the call, evaluated on the host
   const float alpha_x = (float)((double)sp.ang_res_x / 180.0 * 3.14159265358979323846), alpha_y = (float)((double)sp.ang_res_y / 180.0 * 3.14159265358979323846);
   c.sin_x = sinf(alpha_x); c.cos_x = cosf(alpha_x); c.sin_y = sinf(alpha_y); c.cos_y = cosf(alpha_y);
   static const int n4[4][2] = {{-1, 0}, {0, 1}, {0, -1}, {1, 0}};
@@ -712,14 +710,65 @@ static int launch_segment_wave(Lane* L, int ns, int max_n, const IpIn& in, const
     const int(*src)[2] = sp.neighbor_mode == QB200_NEIGHBORS_4 ? n4 : (sp.neighbor_mode == QB200_NEIGHBORS_8 ? n8 : nx);
     c.nb[i][0] = src[i][0]; c.nb[i][1] = src[i][1];
   }
+  return c;
+}
+
+// Enqueue ground removal of the wave's scans [0, ns) (cloud tables of stage_raw, entries d_pp[s]); scan s's outputs -> pw_out + s * R,
+// its counts and status -> pp_cnt[s].  max_np = the wave's largest patch count.  Launches do not depend on ns or on the scans.
+static int launch_patchwork_wave(Lane* L, int ns, int max_n, int max_np, const PpDev& dst) {
+  const int R = L->R;
+  const size_t P = (size_t)L->pw_scans * kPwStride;
+  int* patch_of = L->pw_ints;
+  int* rank = patch_of + (size_t)L->pw_scans * R;
+  int* count = rank + (size_t)L->pw_scans * R;
+  int* start = count + P;
+  int* cursor = start + P;
+  int* ng_ground = cursor + P;
+  int* ng_non = ng_ground + P;
+  int* goff = ng_non + P;
+  int* ngoff = goff + P;
+  unsigned long long* items = reinterpret_cast<unsigned long long*>(L->key_a.get());   // [2S * R] >= [ns * R]
+  const PpScan* tab = L->d_pp;
+  QB_CUDA_TRY(L, cudaMemsetAsync(count, 0, (size_t)ns * kPwStride * sizeof(int), L->stream));
+  const dim3 gp((max_n + 255) / 256 > 0 ? (max_n + 255) / 256 : 1, ns);
+  pw_bin_kernel<<<gp, 256, 0, L->stream>>>(L->d_cloud_ptr, L->d_cloud_n, tab, R, patch_of, count);
+  pw_scan_kernel<<<ns, 1024, 0, L->stream>>>(count, tab, start, cursor);
+  pw_scatter_kernel<<<gp, 256, 0, L->stream>>>(L->d_cloud_ptr, L->d_cloud_n, R, patch_of, cursor, items);
+  const size_t smem = (size_t)kPwMaxPatchPts * 9;
+  QB_CUDA_TRY(L, ensure_dyn_smem(L->device, (const void*)pw_patch_kernel, smem));
+  pw_patch_kernel<<<dim3(max_np, ns), kPwThreads, smem, L->stream>>>(L->d_cloud_ptr, tab, R, start, items, kPwMaxPatchPts, ng_ground, ng_non,
+                                                                     rank, L->pp_cnt);
+  pw_offsets_kernel<<<ns, 1024, 0, L->stream>>>(ng_ground, ng_non, tab, goff, ngoff, L->pp_cnt);
+  pw_gather_kernel<<<dim3(max_np, ns), 256, 0, L->stream>>>(L->d_cloud_ptr, tab, R, start, ng_ground, ng_non, items, rank, goff, ngoff,
+                                                            L->pp_cnt, L->pw_out, dst);
+  L->launches += 6;
+  QB_CUDA_TRY(L, cudaGetLastError());
+  return QB200_OK;
+}
+
+// Enqueue sub-cluster removal of the wave's scans [0, ns) read through `in` (entries d_pp[s]); scan s's outputs -> the range-image
+// scratch + d_pp[s].pix0, its counts -> pp_cnt[s].  max_n bounds every scan's point count; the wave's images have pix pixels and blk
+// blocks in all, max_npix pixels at most.
+static int launch_segment_wave(Lane* L, int ns, int max_n, const IpIn& in, long long pix, long long blk, int max_npix, const PpDev& dst) {
+  const size_t NPX = (size_t)pix;
+  unsigned char* b = reinterpret_cast<unsigned char*>(L->ip_buf.get());
+  float4* out = reinterpret_cast<float4*>(b); b += NPX * 16;      // 16-byte records first: aligned for any image size
+  unsigned long long* rows = reinterpret_cast<unsigned long long*>(b); b += NPX * 8;
+  int* winner = reinterpret_cast<int*>(b); b += NPX * 4;
+  int* parent = reinterpret_cast<int*>(b); b += NPX * 4;
+  int* size = reinterpret_cast<int*>(b); b += NPX * 4;
+  float* range = reinterpret_cast<float*>(b); b += NPX * 4;
+  int* blk_cnt = reinterpret_cast<int*>(b); b += 8 * (size_t)blk;
+  unsigned char* kind = b;
+  const PpScan* tab = L->d_pp;
   QB_CUDA_TRY(L, cudaMemsetAsync(winner, 0xFF, NPX * sizeof(int), L->stream));   // -1
-  const dim3 gpt((max_n + 255) / 256 > 0 ? (max_n + 255) / 256 : 1, ns), gpx((npix + 255) / 256, ns), gbk(nblk, ns);
-  ip_project_kernel<<<gpt, 256, 0, L->stream>>>(in, c, winner);
-  ip_range_kernel<<<gpx, 256, 0, L->stream>>>(in, npix, winner, range, parent, size, rows);
-  ip_union_kernel<<<gpx, 256, 0, L->stream>>>(npix, c, range, parent);
-  ip_stats_kernel<<<gpx, 256, 0, L->stream>>>(npix, sp.horizon_scan, parent, size, rows);
-  ip_kind_kernel<<<gbk, 1024, 0, L->stream>>>(npix, c, winner, parent, size, rows, kind, blk_cnt);
-  ip_extract_kernel<<<gbk, 1024, 0, L->stream>>>(in, npix, winner, kind, blk_cnt, out, L->pp_cnt, dst);
+  const dim3 gpt((max_n + 255) / 256 > 0 ? (max_n + 255) / 256 : 1, ns), gpx((max_npix + 255) / 256, ns), gbk((max_npix + 1023) / 1024, ns);
+  ip_project_kernel<<<gpt, 256, 0, L->stream>>>(in, tab, winner);
+  ip_range_kernel<<<gpx, 256, 0, L->stream>>>(in, tab, winner, range, parent, size, rows);
+  ip_union_kernel<<<gpx, 256, 0, L->stream>>>(tab, range, parent);
+  ip_stats_kernel<<<gpx, 256, 0, L->stream>>>(tab, parent, size, rows);
+  ip_kind_kernel<<<gbk, 1024, 0, L->stream>>>(tab, winner, parent, size, rows, kind, blk_cnt);
+  ip_extract_kernel<<<gbk, 1024, 0, L->stream>>>(in, tab, winner, kind, blk_cnt, out, L->pp_cnt, dst);
   L->launches += 6;
   QB_CUDA_TRY(L, cudaGetLastError());
   return QB200_OK;
@@ -734,23 +783,49 @@ struct PpOut {
 
 // One wave on lane L: scans [0, ns) whose pointers and sizes are in L->h_cloud_ptr / h_cloud_n (`kind` memory) through ground
 // removal (pp) and then sub-cluster removal of its non-ground output (sp), or through sub-cluster removal alone (pp == nullptr).
-// Scan s of the wave is scan first + s of `out`; its counts go to counts[s * 4 ...] (ground, non-ground, valid, outlier), its
-// patchwork status to status[s].  The counts of the wave come back in one copy.
-static int preprocess_wave(Lane* L, int ns, qb200_mem_kind kind, const qb200_patchwork_params* pp, const qb200_segment_params* sp,
+// Scan s of the wave uses pp[s] / sp[s] when `each` is set, else pp[0] / sp[0]; it is scan first + s of `out`; its counts go to
+// counts[s * 4 ...] (ground, non-ground, valid, outlier), its patchwork status to status[s].  The wave's parameter table goes to the
+// device in one copy ahead of its scans, and its counts come back in one copy.
+static int preprocess_wave(Lane* L, int ns, qb200_mem_kind kind, const qb200_patchwork_params* pp, const qb200_segment_params* sp, bool each,
                            const PpOut& out, long long first, int32_t* counts, int32_t* status) {
-  int rc, max_n = 0;
-  for (int s = 0; s < ns; ++s) max_n = L->h_cloud_n[s] > max_n ? L->h_cloud_n[s] : max_n;
-  const int npix = sp ? sp->n_scan * sp->horizon_scan : 0;
-  if ((rc = ensure_pp_scratch(L, ns, pp != nullptr, npix))) return rc;
+  int rc, max_n = 0, max_np = 0, max_npix = 0;
+  long long pix = 0, blk = 0;
+  for (int s = 0; s < ns; ++s) {
+    max_n = L->h_cloud_n[s] > max_n ? L->h_cloud_n[s] : max_n;
+    if (!sp) continue;
+    const int npix = sp[each ? s : 0].n_scan * sp[each ? s : 0].horizon_scan;
+    pix += npix;
+    blk += (npix + 1023) / 1024;
+  }
+  if ((rc = ensure_pp_scratch(L, ns, pp != nullptr, sp ? ip_bytes(pix, blk) : 0))) return rc;
+  pix = blk = 0;
+  for (int s = 0; s < ns; ++s) {   // the previous wave ended in a sync: the pinned table is free
+    PpScan& e = L->h_pp[s];
+    e = PpScan{};
+    if (pp) {
+      e.pw = pw_entry(pp[each ? s : 0]);
+      max_np = e.pw.n_patches > max_np ? e.pw.n_patches : max_np;
+    }
+    if (sp) {
+      e.ip = ip_entry(sp[each ? s : 0]);
+      e.npix = e.ip.p.n_scan * e.ip.p.horizon_scan;
+      e.pix0 = pix;
+      e.blk0 = (int)blk;
+      pix += e.npix;
+      blk += (e.npix + 1023) / 1024;
+      max_npix = e.npix > max_npix ? e.npix : max_npix;
+    }
+  }
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_pp, L->h_pp, (size_t)ns * sizeof(PpScan), cudaMemcpyHostToDevice, L->stream));
   if ((rc = stage_raw(L, ns, kind, L->stream))) return rc;
   QB_CUDA_TRY(L, cudaMemsetAsync(L->pp_cnt, 0, (size_t)ns * kPpCnt * sizeof(int), L->stream));
   PpDev dst = {{nullptr, nullptr, nullptr, nullptr}, out.cap};
   if (out.device)
     for (int k = 0; k < 4; ++k) dst.arr[k] = out.arr[k] ? out.arr[k] + first * out.cap : nullptr;
-  if (pp && (rc = launch_patchwork_wave(L, ns, max_n, *pp, dst))) return rc;
+  if (pp && (rc = launch_patchwork_wave(L, ns, max_n, max_np, dst))) return rc;
   if (sp) {
     IpIn in = {L->d_cloud_ptr, L->d_cloud_n, pp ? L->pw_out.get() : nullptr, L->pp_cnt, L->R};
-    if ((rc = launch_segment_wave(L, ns, max_n, in, *sp, dst))) return rc;
+    if ((rc = launch_segment_wave(L, ns, max_n, in, pix, blk, max_npix, dst))) return rc;
   }
   QB_CUDA_TRY(L, cudaMemcpyAsync(L->pp_hcnt, L->pp_cnt, (size_t)ns * kPpCnt * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
   QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
@@ -764,9 +839,9 @@ static int preprocess_wave(Lane* L, int ns, qb200_mem_kind kind, const qb200_pat
     for (int k = 0; k < 4; ++k) {
       const long long m = c4[k] < out.cap ? c4[k] : out.cap;
       if (!out.arr[k] || m <= 0) continue;
-      // scratch of scan s: ground | non-ground at pw_out + s * R, valid | outlier at the range-image outputs + s * npix
+      // scratch of scan s: ground | non-ground at pw_out + s * R, valid | outlier at the range-image outputs + pix0
       const float4* src = k < 2 ? L->pw_out + (size_t)s * L->R + (k == 1 ? hc[0] : 0)
-                                : reinterpret_cast<const float4*>(L->ip_buf.get()) + (size_t)s * npix + (k == 3 ? hc[3] : 0);
+                                : reinterpret_cast<const float4*>(L->ip_buf.get()) + (size_t)L->h_pp[s].pix0 + (k == 3 ? hc[3] : 0);
       QB_CUDA_TRY(L, cudaMemcpyAsync(out.arr[k] + (first + s) * out.cap, src, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
       copied = true;
     }
@@ -775,59 +850,32 @@ static int preprocess_wave(Lane* L, int ns, qb200_mem_kind kind, const qb200_pat
   return QB200_OK;
 }
 
-}  // namespace qb
-
-using namespace qb;
-
-extern "C" {
-
-// ---- pre-processing: ground removal (patchwork.hpp:329-455), a wave of one ----------------------------
-int qb200_patchwork(qb200_handle* h, const float* pts4, int32_t n, const qb200_patchwork_params* p, float* ground4, int32_t* n_ground,
-                    float* nonground4, int32_t* n_nonground) {
-  if (int rc = enter(h)) return rc;
-  if (!p || !n_ground || !n_nonground || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
-  *n_ground = *n_nonground = 0;
-  Lane* L = h->lane[0].get();
-  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
-  if (!pw_params_valid(*p)) return QB200_ERR_BAD_ARG;
-  L->h_cloud_ptr[0] = reinterpret_cast<const float4*>(pts4);
-  L->h_cloud_n[0] = n;
-  const PpOut out = {{reinterpret_cast<float4*>(ground4), reinterpret_cast<float4*>(nonground4), nullptr, nullptr}, n, 0};
-  int32_t counts[4], status = QB200_OK;
-  if (int rc = preprocess_wave(L, 1, QB200_MEM_HOST, p, nullptr, out, 0, counts, &status)) return rc;
-  *n_ground = counts[0];
-  *n_nonground = counts[1];
-  return status;
+// true when an entry of the per-scan tables pp[0..n) / sp[0..n) (sp may be nullptr) fails the checks of a broadcast call; msg names
+// the first such entry
+static bool bad_entry(const qb200_patchwork_params* pp, const qb200_segment_params* sp, int n, char* msg, size_t len) {
+  for (int i = 0; i < n; ++i) {
+    const char* what = !pw_params_valid(pp[i]) ? "patchwork" : (sp && !ip_params_valid(sp[i])) ? "segment" : nullptr;
+    if (what) {
+      snprintf(msg, len, "invalid %s parameters of scan %d", what, i);
+      return true;
+    }
+  }
+  return false;
 }
 
-// ---- pre-processing: range-image sub-cluster removal (imageProjection.hpp:273-294), a wave of one ------------
-int qb200_segment_cloud(qb200_handle* h, const float* pts4, int32_t n, const qb200_segment_params* p, float* valid4, int32_t* n_valid,
-                        float* outlier4, int32_t* n_outlier) {
-  if (int rc = enter(h)) return rc;
-  if (!p || !n_valid || !n_outlier || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
-  *n_valid = *n_outlier = 0;
-  Lane* L = h->lane[0].get();
-  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
-  if (!ip_params_valid(*p)) return QB200_ERR_BAD_ARG;
-  L->h_cloud_ptr[0] = reinterpret_cast<const float4*>(pts4);
-  L->h_cloud_n[0] = n;
-  const PpOut out = {{nullptr, nullptr, reinterpret_cast<float4*>(valid4), reinterpret_cast<float4*>(outlier4)}, (long long)p->n_scan * p->horizon_scan, 0};
-  int32_t counts[4], status = QB200_OK;
-  if (int rc = preprocess_wave(L, 1, QB200_MEM_HOST, nullptr, p, out, 0, counts, &status)) return rc;
-  *n_valid = counts[2];
-  *n_outlier = counts[3];
-  return QB200_OK;
-}
-
-// ---- pre-processing of many scans: ground removal, then sub-cluster removal, in waves of 2S scans ----------
-int qb200_preprocess_batch(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans, qb200_mem_kind kind,
-                           const qb200_patchwork_params* pp, const qb200_segment_params* sp, const qb200_preprocess_out* out) {
+// qb200_preprocess_batch (each == false: pp[0] / sp[0] serve every scan) and qb200_preprocess_batch_each (one entry per scan): every
+// check before any work, then waves of 2S scans on lane 0.
+static int preprocess_call(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans, qb200_mem_kind kind,
+                           const qb200_patchwork_params* pp, const qb200_segment_params* sp, bool each, const qb200_preprocess_out* out) {
   if (int rc = enter(h)) return rc;
   const char* why = nullptr;
+  char msg[96];
   if (n_scans < 0 || (n_scans > 0 && (!scans4 || !n_points))) why = "n_scans < 0, or no scan / size table";
   else if (kind != QB200_MEM_HOST && kind != QB200_MEM_DEVICE) why = "unknown memory kind of the scans";
-  else if (!pp || !pw_params_valid(*pp)) why = "invalid patchwork parameters";
-  else if (sp && !ip_params_valid(*sp)) why = "invalid segment parameters";
+  else if (!each && (!pp || !pw_params_valid(*pp))) why = "invalid patchwork parameters";
+  else if (!each && sp && !ip_params_valid(*sp)) why = "invalid segment parameters";
+  else if (each && n_scans > 0 && !pp) why = "no patchwork parameter table";
+  else if (each && bad_entry(pp, sp, n_scans, msg, sizeof(msg))) why = msg;
   else if (!out || !out->counts || !out->status) why = "no output descriptor, counts or status";
   else if (out->cap_per_scan < 1) why = "cap_per_scan < 1";
   else if (out->kind != QB200_MEM_HOST && out->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the outputs";
@@ -851,9 +899,67 @@ int qb200_preprocess_batch(qb200_handle* h, const float* const* scans4, const in
       L->h_cloud_ptr[s] = reinterpret_cast<const float4*>(scans4[w0 + s]);
       L->h_cloud_n[s] = n_points[w0 + s];
     }
-    if (int rc = preprocess_wave(L, ns, kind, pp, sp, o, w0, out->counts + 4 * (size_t)w0, out->status + w0)) return rc;
+    const size_t e0 = each ? (size_t)w0 : 0;
+    if (int rc = preprocess_wave(L, ns, kind, pp + e0, sp ? sp + e0 : nullptr, each, o, w0, out->counts + 4 * (size_t)w0, out->status + w0))
+      return rc;
   }
   return QB200_OK;
+}
+
+}  // namespace qb
+
+using namespace qb;
+
+extern "C" {
+
+// ---- pre-processing: ground removal (patchwork.hpp:329-455), a wave of one ----------------------------
+int qb200_patchwork(qb200_handle* h, const float* pts4, int32_t n, const qb200_patchwork_params* p, float* ground4, int32_t* n_ground,
+                    float* nonground4, int32_t* n_nonground) {
+  if (int rc = enter(h)) return rc;
+  if (!p || !n_ground || !n_nonground || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
+  *n_ground = *n_nonground = 0;
+  Lane* L = h->lane[0].get();
+  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
+  if (!pw_params_valid(*p)) return QB200_ERR_BAD_ARG;
+  L->h_cloud_ptr[0] = reinterpret_cast<const float4*>(pts4);
+  L->h_cloud_n[0] = n;
+  const PpOut out = {{reinterpret_cast<float4*>(ground4), reinterpret_cast<float4*>(nonground4), nullptr, nullptr}, n, 0};
+  int32_t counts[4], status = QB200_OK;
+  if (int rc = preprocess_wave(L, 1, QB200_MEM_HOST, p, nullptr, false, out, 0, counts, &status)) return rc;
+  *n_ground = counts[0];
+  *n_nonground = counts[1];
+  return status;
+}
+
+// ---- pre-processing: range-image sub-cluster removal (imageProjection.hpp:273-294), a wave of one ------------
+int qb200_segment_cloud(qb200_handle* h, const float* pts4, int32_t n, const qb200_segment_params* p, float* valid4, int32_t* n_valid,
+                        float* outlier4, int32_t* n_outlier) {
+  if (int rc = enter(h)) return rc;
+  if (!p || !n_valid || !n_outlier || n < 0 || (n > 0 && !pts4)) return QB200_ERR_BAD_ARG;
+  *n_valid = *n_outlier = 0;
+  Lane* L = h->lane[0].get();
+  if (n > L->R) { h->fail(__FILE__, __LINE__, "n exceeds max_raw_points"); return QB200_ERR_BAD_ARG; }
+  if (!ip_params_valid(*p)) return QB200_ERR_BAD_ARG;
+  L->h_cloud_ptr[0] = reinterpret_cast<const float4*>(pts4);
+  L->h_cloud_n[0] = n;
+  const PpOut out = {{nullptr, nullptr, reinterpret_cast<float4*>(valid4), reinterpret_cast<float4*>(outlier4)}, (long long)p->n_scan * p->horizon_scan, 0};
+  int32_t counts[4], status = QB200_OK;
+  if (int rc = preprocess_wave(L, 1, QB200_MEM_HOST, nullptr, p, false, out, 0, counts, &status)) return rc;
+  *n_valid = counts[2];
+  *n_outlier = counts[3];
+  return QB200_OK;
+}
+
+// ---- pre-processing of many scans: ground removal, then sub-cluster removal, in waves of 2S scans ----------
+int qb200_preprocess_batch(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans, qb200_mem_kind kind,
+                           const qb200_patchwork_params* pp, const qb200_segment_params* sp, const qb200_preprocess_out* out) {
+  return preprocess_call(h, scans4, n_points, n_scans, kind, pp, sp, false, out);
+}
+
+// ---- the same with one parameter entry per scan ----------
+int qb200_preprocess_batch_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans, qb200_mem_kind kind,
+                                const qb200_patchwork_params* pp, const qb200_segment_params* sp, const qb200_preprocess_out* out) {
+  return preprocess_call(h, scans4, n_points, n_scans, kind, pp, sp, true, out);
 }
 
 }  // extern "C"
