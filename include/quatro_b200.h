@@ -301,7 +301,8 @@ int qb200_max_clique_ex(qb200_handle* h, const uint32_t* adj, int32_t L, int32_t
                         int32_t mode, double kcore_heuristic_threshold, int64_t node_limit, int32_t* clique, int32_t* n_clique,
                         int32_t* kcore, int32_t* kcore_order, int32_t* max_core, int32_t* flags);
 
-/* rotation + translation given the (sorted) clique. inlier_mask (n_clique bytes) may be NULL. */
+/* rotation + translation given the (sorted) clique. inlier_mask (n_clique bytes) may be NULL.
+ * A clique entry outside [0, L) is refused with QB200_ERR_BAD_ARG before anything reaches the device. */
 int qb200_solve_pose(qb200_handle* h, const float* a4, const float* b4, int32_t L,
                      const int32_t* clique, int32_t n_clique, const qb200_params* p,
                      qb200_result* res, uint8_t* rot_inlier_mask, uint8_t* trans_inlier_mask);

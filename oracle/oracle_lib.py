@@ -44,7 +44,7 @@ class Oracle:
         L.qo_max_clique_ex.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int64, C.c_void_p, C.POINTER(C.c_int),
                                        C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.qo_solve_pose.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(Params), C.POINTER(Result),
-                                    C.c_void_p, C.c_void_p]
+                                    C.c_void_p, C.c_void_p, C.c_void_p]
         L.qo_solve_correspondences.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Params), C.POINTER(Result), C.c_void_p,
                                                C.POINTER(C.c_int), C.c_void_p, C.POINTER(C.c_int)]
         L.qo_match_and_pack.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(Params), C.c_void_p, C.c_void_p, C.c_void_p,
@@ -213,13 +213,17 @@ class Oracle:
         assert st >= 0, st
         return clique[: n.value].copy(), kcore[:L].copy(), order[:L].copy(), mc.value, fl.value
 
-    def solve_pose(self, a4, b4, clique, params: Params):
+    def solve_pose(self, a4, b4, clique, params: Params, want_final: bool = False):
+        """want_final: also return the final inlier list (correspondence ids, getFinalInliersIndices) as a fifth element."""
         a4, b4 = _f32(a4, 4), _f32(b4, 4)
         clique = np.ascontiguousarray(clique, np.int32)
         res = Result()
         rm, tm = np.zeros(max(len(clique), 1), np.uint8), np.zeros(max(len(clique), 1), np.uint8)
-        st = self.lib.qo_solve_pose(_ptr(a4), _ptr(b4), len(a4), _ptr(clique), len(clique), C.byref(params), C.byref(res), _ptr(rm), _ptr(tm))
-        return res, rm[: len(clique)], tm[: len(clique)], st
+        fi = np.zeros(max(len(clique), 1), np.int32)
+        st = self.lib.qo_solve_pose(_ptr(a4), _ptr(b4), len(a4), _ptr(clique), len(clique), C.byref(params), C.byref(res), _ptr(rm), _ptr(tm),
+                                    _ptr(fi))
+        out = (res, rm[: len(clique)], tm[: len(clique)], st)
+        return out + (fi[: res.n_final_inliers].copy(),) if want_final else out
 
     def solve_correspondences(self, a4, b4, params: Params, want_sets: bool = False):
         a4, b4 = _f32(a4, 4), _f32(b4, 4)

@@ -1040,11 +1040,13 @@ inline void set_identity(double T[16]) {
 // a13-a19. include/quatro.hpp:806-936 given the sorted clique
 int solve_pose(const P4* a, const P4* b, int L, const int* clique, int nc, const qb200_params& prm, qb200_result& res,
                std::vector<uint8_t>& rot_mask, std::vector<uint8_t>& trans_mask, std::vector<int>& final_inliers) {
-  (void)L;
   set_identity(res.T);
   res.valid = 0; res.clique_size = nc; res.gnc_iters = 0; res.n_rot_inliers = 0; res.n_final_inliers = 0; res.cost = 0;
   rot_mask.clear(); trans_mask.clear(); final_inliers.clear();
-  if (nc <= 1) { res.status = QB200_DEGENERATE_CLIQUE; return QB200_DEGENERATE_CLIQUE; }
+  if (nc <= 1) {  // fewer than 2 correspondences is a degenerate input, as in solve_correspondences and the device
+    res.status = L < 2 ? QB200_DEGENERATE_INPUT : QB200_DEGENERATE_CLIQUE;
+    return res.status;
+  }
   // chain TIMs (:817-844), XY rows only feed the rotation (:396-402)
   std::vector<double> s2(2 * (size_t)nc), d2(2 * (size_t)nc);
   for (int i = 0; i < nc; ++i) {
@@ -1282,7 +1284,7 @@ int qo_max_clique(const uint32_t* adj, int L, int wpr, int mode, double kcore_th
 }
 
 int qo_solve_pose(const float* a4, const float* b4, int L, const int* clique, int n_clique, const qb200_params* prm,
-                  qb200_result* res, uint8_t* rot_mask, uint8_t* trans_mask) {
+                  qb200_result* res, uint8_t* rot_mask, uint8_t* trans_mask, int* final_inliers) {
   std::vector<uint8_t> rm, tm;
   std::vector<int> fi;
   qb200_result r;
@@ -1292,6 +1294,7 @@ int qo_solve_pose(const float* a4, const float* b4, int L, const int* clique, in
   *res = r;
   if (rot_mask) std::copy(rm.begin(), rm.end(), rot_mask);
   if (trans_mask) std::copy(tm.begin(), tm.end(), trans_mask);
+  if (final_inliers) std::copy(fi.begin(), fi.end(), final_inliers);
   return st;
 }
 

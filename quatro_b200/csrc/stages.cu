@@ -250,6 +250,9 @@ int qb200_solve_pose(qb200_handle* h, const float* a4, const float* b4, int32_t 
     return QB200_ERR_BAD_ARG;
   Lane* ln = h->lane[0].get();
   if (L > ln->Lc) { h->fail(__FILE__, __LINE__, "L exceeds max_corr"); return QB200_ERR_BAD_ARG; }
+  // pose_kernel reads a4[clique[j]] / b4[clique[j]] unchecked: an entry outside [0, L) would read past the pair's points
+  for (int j = 0; j < n_clique; ++j)
+    if (clique[j] < 0 || clique[j] >= L) { h->fail(__FILE__, __LINE__, "clique entry outside [0, L)"); return QB200_ERR_BAD_ARG; }
   int rc = wave_reset(ln, 2);
   if (rc) return rc;
   if (L > 0) QB_CUDA_TRY(h, cudaMemcpyAsync(ln->ma, a4, (size_t)L * sizeof(float4), cudaMemcpyHostToDevice, ln->stream));
