@@ -21,6 +21,8 @@
  *   qb200_pair_lists (_ex forms) <- FPFHManager::getCorrespondences, Quatro::getMaxCliques / getFinalInliersIndices for every
  *                                  pair of a batch (examples/run_global_registration.cpp:268, 292)
  *   qb200_*_each                <- one Quatro object per pair: Quatro::reset(Params) + setPreEstaimatedRyRx for every pair of a batch
+ *   qb200_*_mixed               <- the same, plus voxelize / FPFHManager / matcher flags and seed per pair
+ *                                  (examples/run_global_registration.cpp:206-209)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -441,6 +443,37 @@ int qb200_register_cached_each(qb200_handle* h, const qb200_slot_pair* pairs, in
 /* qb200_solve_batch_ex with one params entry per correspondence set (front-end fields ignored) */
 int qb200_solve_batch_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params, qb200_mem_kind kind,
                            qb200_result* results, const qb200_pair_lists* lists);
+
+/* --- per-pair front-end parameters: presets, retries and seed sweeps in one batch ---------------------------------------------------
+ * The reference voxelizes and describes every registration with its own configuration: voxelize(..., voxel_size)
+ * (examples/run_global_registration.cpp:206-207), a fresh FPFHManager(normal_radius, fpfh_radius) per pair (:209), the matcher's tuple
+ * flags (include/fpfh_manager.hpp:125-127) and an RNG seed per run (src/teaser_utils/feature_matcher.cc:189).  The _mixed forms take
+ * exactly the arguments of their _each siblings; every field of every entry may differ, the front-end fields (voxel_size .. seed)
+ * included.  A pair's source and target are both voxelized and described with its entry.
+ *   Pair i's record and lists are byte-identical to pair i of the _ex call made with params[i] for the whole batch; they never depend
+ *     on the batch, the wave, the lane, the memory kind or the configurations of the other pairs of the wave.  A pair's size refusals
+ *     (QB200_ERR_VOXEL_OVERFLOW, QB200_CAPACITY_EXCEEDED) stay its own.
+ *   Checks happen before any work starts: every entry must pass the checks of the _ex call (QB200_ERR_BAD_ARG), an entry with
+ *     use_crosscheck = 0 fails the call with QB200_ERR_UNSUPPORTED, and a cached pair whose entry does not match the front-end
+ *     signature of one of its two slots (voxel_size, normal_radius, fpfh_radius, lattice cell) fails it with QB200_ERR_BAD_ARG.  A
+ *     rejected call writes no record, list or slot, and qb200_last_error names the entry.
+ *   Entries with rot_noise_bound == 0 are resolved in pair order through the handle's latch, as in the _each forms. */
+/* qb200_register_batch_each whose entries may differ in their front-end fields */
+int qb200_register_batch_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
+                               qb200_result* results, const qb200_pair_lists* lists);
+/* qb200_register_batch_enqueue_each whose entries may differ in their front-end fields; completed by qb200_register_batch_flush */
+int qb200_register_batch_enqueue_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                       qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+/* qb200_register_cached_each whose entries may differ in their front-end fields: pair i's entry must match the signature of its own
+ * two slots (not that of entry 0) */
+int qb200_register_cached_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                qb200_result* results, const qb200_pair_lists* lists);
+/* qb200_cache_scans with one params entry per scan: scan i is voxelized and described with params[i] and slot_ids[i] records that
+ * entry's front-end signature (qb200_cache_copy carries it).  Slot s's voxels, normals and descriptors (qb200_cache_read) are
+ * byte-identical to qb200_cache_scans of that scan alone with its entry.  A bad entry fails the call with QB200_ERR_BAD_ARG before
+ * any slot is written, and qb200_last_error names it. */
+int qb200_cache_scans_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
+                           const qb200_params* params, qb200_mem_kind kind);
 /* read a cached scan back: voxel points (n x 4), normals (n x {nx,ny,nz,curvature}), descriptors (n x 33); any may be NULL */
 int qb200_cache_read(qb200_handle* h, int32_t slot, float* vox4, float* normals4, float* desc33, int32_t cap, int32_t* n);
 

@@ -233,6 +233,10 @@ _SIGNATURES = {
     "qb200_register_cached_each": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
     "qb200_solve_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_preprocess_batch_each": (i32, [vp, vp, vp, i32, i32, P(PatchworkParams), P(SegmentParams), P(PreprocessOut)]),
+    "qb200_register_batch_mixed": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_register_batch_enqueue_mixed": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_register_cached_mixed": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
+    "qb200_cache_scans_each": (i32, [vp, P(vp), P(i32), P(i32), i32, P(Params), i32]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -691,6 +695,27 @@ class Handle:
         arr, keep = self._set_array(sets, kind)
         return self._batch_lists("qb200_solve_batch_each", len(sets), (arr, len(sets), self.params_array(params), kind), buffers)
 
+    # ---- one Params per pair, front end included (the _mixed entry points) ----
+    def register_batch_mixed(self, pairs: Sequence, params: Sequence[Params], kind: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
+        """qb200_register_batch_mixed: pair i is voxelized, described, matched and solved with params[i] (every field may differ)."""
+        assert len(params) == len(pairs)
+        arr, keep = self.pair_array(pairs, kind)
+        return self._batch_lists("qb200_register_batch_mixed", len(pairs), (arr, len(pairs), self.params_array(params), kind), buffers)
+
+    def register_batch_enqueue_mixed_raw(self, pair_array, n: int, params_array, kind: int, out: np.ndarray,
+                                         buffers: Optional[ListBuffers] = None):
+        """qb200_register_batch_enqueue_mixed: params_array (params_array()) is copied by the call; pair_array, its scans, `out` and the
+        buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_register_batch_enqueue_mixed(self.h, pair_array, n, params_array, kind, _ptr(out),
+                                                                       self._lists_arg(buffers)), "qb200_register_batch_enqueue_mixed")
+
+    def register_cached_mixed(self, slot_pairs, params: Sequence[Params], buffers: Optional[ListBuffers] = None):
+        """qb200_register_cached_mixed: slot pair i is registered with params[i], whose front-end fields must be the ones both of its
+        slots were cached with."""
+        sp = _slot_array(slot_pairs)
+        assert len(params) == len(sp)
+        return self._batch_lists("qb200_register_cached_mixed", len(sp), (_ptr(sp), len(sp), self.params_array(params)), buffers)
+
     def last_features(self, which: int, cap: Optional[int] = None):
         """(normals (n,4), descriptors (n,33)) of the source (0) / target (1) cloud of the last match_and_pack."""
         cap = cap or self.cfg.max_voxel_points
@@ -710,6 +735,14 @@ class Handle:
         ptrs, cnts, keep = _scan_arrays(scans, kind)
         ids = (C.c_int32 * max(n, 1))(*[int(x) for x in slot_ids])
         self._check(self.lib.qb200_cache_scans(self.h, ptrs, cnts, ids, n, C.byref(params), kind), "qb200_cache_scans")
+
+    def cache_scans_each(self, scans: Sequence, slot_ids: Sequence[int], params: Sequence[Params], kind: int = MEM_HOST):
+        """qb200_cache_scans_each: scan i goes to slot_ids[i], voxelized and described with params[i]."""
+        n = len(scans)
+        assert len(params) == n
+        ptrs, cnts, keep = _scan_arrays(scans, kind)
+        ids = (C.c_int32 * max(n, 1))(*[int(x) for x in slot_ids])
+        self._check(self.lib.qb200_cache_scans_each(self.h, ptrs, cnts, ids, n, self.params_array(params), kind), "qb200_cache_scans_each")
 
     def register_cached(self, slot_pairs, params: Params) -> np.ndarray:
         sp = _slot_array(slot_pairs)

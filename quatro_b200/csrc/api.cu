@@ -66,6 +66,7 @@ size_t carve_counters(int* base, size_t S, WaveCounters* c) {
   c->n_cells = take(C);
   c->cloud_status = take(C);
   c->bbox = take(C * 6);
+  c->vox_digits = take(C);
   c->n_mutual = take(S);
   c->n_corr = take(S);
   c->swapped = take(S);
@@ -149,6 +150,8 @@ int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   QB_CUDA_TRY(L, L->trans_mask.alloc(S * Lc));
   QB_CUDA_TRY(L, L->d_solve.alloc(S));
   QB_CUDA_TRY(L, L->h_solve.alloc(S));
+  QB_CUDA_TRY(L, L->d_front.alloc(C));
+  QB_CUDA_TRY(L, L->h_front.alloc(C));
   // workspaces of the pairs whose graph or clique outgrows the shared-memory layouts (clique.cu, pose.cu); only wide handles have them
   if (Lc > (size_t)kKcoreSmemVerts) {
     QB_CUDA_TRY(L, L->kcore_ws.alloc(S * kcore_ws_bytes((int)Lc)));
@@ -216,6 +219,14 @@ bool params_ok(const qb200_params* p) {
 // neighbour within +-1 even after the float rounding of x / cell, so the walk covers 27 cells instead of 125
 float lattice_cell(const qb200_params& p) { return p.grid_cell > 0 ? p.grid_cell : p.fpfh_radius * 1.001953125f; }
 
+CloudFront front_entry(const qb200_params& p) {
+  CloudFront e;
+  memset(&e, 0, sizeof(e));
+  front_voxel(&e, p.voxel_size, p.skip_flagged);
+  front_lattice(&e, p.normal_radius, p.fpfh_radius, lattice_cell(p));
+  return e;
+}
+
 // p with its rotation noise bound resolved.  The reference latches 2*noise_bound of the FIRST registration into a function-local
 // static (quatro.hpp:469-470 after :851); here the latch is a per-handle field, overridable via params.  Every lane gets the
 // resolved value, so a pair's GNC bound never depends on the wave / lane it lands on.
@@ -243,6 +254,7 @@ PairSolve solve_entry(const qb200_params& p) {
   e.kcore_thr = p.kcore_heuristic_threshold;
   e.node_limit = p.max_clique_node_limit > 0 ? p.max_clique_node_limit : (long long)QB200_DEFAULT_CLIQUE_NODE_LIMIT;
   e.mode = p.inlier_selection_mode;
+  match_fields(&e, p);
   return e;
 }
 
@@ -350,8 +362,9 @@ struct BatchCall {
   qb200_result* results = nullptr;
   // the batch's per-pair lists (qb200_pair_lists), nullptr = records only
   const qb200_pair_lists* lists = nullptr;
-  // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved, laid out like `caller`; the front end
-  // reads params[0]: the front-end fields of every entry are equal.
+  // (each) the entries may differ in their front-end fields too (the _mixed forms); otherwise those are bit-identical in every entry
+  bool mixed = false;
+  // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved, laid out like `caller`.
   const qb200_params* params = nullptr;
   // raw host scans of a multi-wave batch: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies queued on
   // several streams share the PCIe link, so every wave's scans would arrive late; on one stream they arrive wave after wave and
@@ -428,19 +441,19 @@ int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
 // No sync: wave_collect hands the records out to in.results[w0...].  The lane's previous wave must have been collected.
 int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   const int ncl = 2 * np;
-  const qb200_params& p = in.params[0];
   int rc;
   L->kev_armed[0] = L->kev_armed[1] = 0;
-  // the wave's solver table (the lane's previous wave has been collected: its pinned mirror is free), copied before anything else of
-  // the wave: on a stream of host batches the copy engine carries the scans, and a copy queued ahead of this wave's scans only waits
-  // for the earlier waves' scans, which the lane waits for anyway
-  if (in.each) {
-    for (int s = 0; s < np; ++s) L->h_solve[s] = solve_entry(in.params[w0 + s]);
-  } else {
-    const PairSolve e = solve_entry(p);
-    for (int s = 0; s < np; ++s) L->h_solve[s] = e;
+  // the wave's tables (the lane's previous wave has been collected: their pinned mirrors are free), copied before anything else of the
+  // wave: on a stream of host batches the copy engine carries the scans, and a copy queued ahead of this wave's scans only waits for
+  // the earlier waves' scans, which the lane waits for anyway.  A pair's entry and both of its clouds' come from its own params.
+  for (int s = 0; s < np; ++s) {
+    const bool own = in.each || s == 0;
+    const qb200_params& p = in.params[in.each ? w0 + s : 0];
+    L->h_solve[s] = own ? solve_entry(p) : L->h_solve[0];
+    if (in.pairs) L->h_front[2 * s] = L->h_front[2 * s + 1] = own ? front_entry(p) : L->h_front[0];
   }
   if ((rc = upload_solve(L, np))) return rc;
+  if (in.pairs && (rc = upload_front(L, ncl))) return rc;
   if (in.pairs) {
     cudaEventRecord(L->ev[0], L->stream);
     for (int s = 0; s < np; ++s) {
@@ -457,9 +470,9 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, h->ev_copied, 0));
     }
     cudaEventRecord(L->ev[1], L->stream);
-    if ((rc = launch_voxel(L, ncl, p.voxel_size, p.skip_flagged))) return rc;
+    if ((rc = launch_voxel(L, ncl))) return rc;
     cudaEventRecord(L->ev[2], L->stream);
-    if ((rc = launch_fpfh(L, ncl, p.normal_radius, p.fpfh_radius, lattice_cell(p)))) return rc;
+    if ((rc = launch_fpfh(L, ncl))) return rc;
     cudaEventRecord(L->ev[3], L->stream);
   } else if (in.slots) {
     for (int s = 0; s < np; ++s) {
@@ -483,7 +496,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     }
     QB_CUDA_TRY(L, cudaMemcpyAsync(L->ctr.n_corr, L->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, L->stream));
   }
-  if (!in.sets && (rc = launch_match(L, np, p))) return rc;
+  if (!in.sets && (rc = launch_match(L, np))) return rc;
   cudaEventRecord(L->ev[4], L->stream);
   cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
   if ((rc = run_solver(L, np, in.sets ? 0 : 1))) return rc;
@@ -558,17 +571,20 @@ int batch_flush(qb200_handle* h) {
 }
 
 // The params of a call: one entry for the whole batch, or (each) one per pair (n entries; NULL is fine when n == 0).  Every entry passes
-// params_ok; same_frontend: the call runs a front end or matches cached scans, so every entry carries the first entry's front-end
-// fields (voxel_size .. seed, bit for bit).
+// params_ok; same_frontend: the call runs a front end or matches cached scans with one front-end configuration (the _each forms), so
+// every entry carries the first entry's front-end fields (voxel_size .. seed, bit for bit).  A rejection names the entry.
 int check_params(qb200_handle* h, const qb200_params* p, int n, bool each, bool same_frontend) {
   const int m = each ? n : 1;
+  char why[128];
   for (int i = 0; i < m; ++i) {
     if (!params_ok(p ? p + i : nullptr)) {
-      h->fail(__FILE__, __LINE__, each ? "a params entry is null or out of range" : "params are null or out of range");
+      if (each) snprintf(why, sizeof(why), "params entry %d is null or out of range", i);
+      h->fail(__FILE__, __LINE__, each ? why : "params are null or out of range");
       return QB200_ERR_BAD_ARG;
     }
     if (same_frontend && i > 0 && memcmp(p + i, p, offsetof(qb200_params, noise_bound)) != 0) {
-      h->fail(__FILE__, __LINE__, "params entries differ in their front-end fields (voxel_size .. seed)");
+      snprintf(why, sizeof(why), "params entry %d differs from entry 0 in its front-end fields (voxel_size .. seed)", i);
+      h->fail(__FILE__, __LINE__, why);
       return QB200_ERR_BAD_ARG;
     }
   }
@@ -601,8 +617,17 @@ int check_call(qb200_handle* h, const BatchCall& c) {
   if (c.n > 0 && !c.results) return reject("the results array is null");
   if (c.kind != QB200_MEM_HOST && c.kind != QB200_MEM_DEVICE) return reject("unknown memory kind of the inputs");
   const qb200_params* p = c.caller;
-  if (int rc = check_params(h, p, c.n, c.each, !c.sets)) return rc;
-  if (!c.sets && (!c.each || c.n > 0) && !p->use_crosscheck) return QB200_ERR_UNSUPPORTED;
+  char why[128];
+  if (int rc = check_params(h, p, c.n, c.each, !c.sets && !c.mixed)) return rc;
+  for (int i = 0; !c.sets && i < (c.each ? c.n : 1); ++i) {
+    if (!p[i].use_crosscheck) {
+      if (c.each) {
+        snprintf(why, sizeof(why), "params entry %d: use_crosscheck = 0 is not supported", i);
+        h->fail(__FILE__, __LINE__, why);
+      }
+      return QB200_ERR_UNSUPPORTED;
+    }
+  }
   if (int rc = check_lists(h, c.lists, c.sets != nullptr)) return rc;
   const int R = h->cfg.max_raw_points;
   for (int i = 0; i < c.n; ++i) {
@@ -611,11 +636,15 @@ int check_call(qb200_handle* h, const BatchCall& c) {
       if (q.n_src < 0 || q.n_tgt < 0 || q.n_src > R || q.n_tgt > R || (q.n_src > 0 && !q.src) || (q.n_tgt > 0 && !q.tgt))
         return reject("pair has a null cloud or exceeds max_raw_points");
     } else if (c.slots) {
+      const qb200_params& pe = p[c.each ? i : 0];  // the pair's own entry
       for (const int sl : {c.slots[i].src_slot, c.slots[i].tgt_slot}) {
         if (sl < 0 || sl >= h->c_slots) return reject("slot outside qb200_cache_reserve()");
         const float* sig = h->c_sig.get() + 4 * (size_t)sl;
-        if (sig[0] != p->voxel_size || sig[1] != p->normal_radius || sig[2] != p->fpfh_radius || sig[3] != lattice_cell(*p))
-          return reject("cached scan was computed with other front-end parameters (or the slot is empty)");
+        if (sig[0] != pe.voxel_size || sig[1] != pe.normal_radius || sig[2] != pe.fpfh_radius || sig[3] != lattice_cell(pe)) {
+          snprintf(why, sizeof(why), "pair %d: cached scan in slot %d was computed with other front-end parameters (or the slot is empty)",
+                   i, sl);
+          return reject(why);
+        }
       }
     } else {
       const qb200_corr_set& s = c.sets[i];
@@ -711,6 +740,44 @@ int run_call(qb200_handle* h, const BatchCall& c) {
   if (rc == QB200_OK) rc = rc2;
   if (rc == QB200_OK && c.n == 1) set_last(h, c.results[0]);
   return rc;
+}
+
+// qb200_cache_scans (each = false: p is one entry for every scan) and qb200_cache_scans_each (p[i] for scan i): waves of up to 2S
+// scans on lane 0, each scan voxelized and described with its entry, and its slot records that entry's front-end signature
+int cache_scans(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
+                const qb200_params* p, bool each, qb200_mem_kind kind) {
+  if (int rc = enter(h)) return rc;
+  if (n_scans < 0 || (n_scans > 0 && (!scans4 || !n_points || !slot_ids))) return QB200_ERR_BAD_ARG;
+  if (!each && !params_ok(p)) return QB200_ERR_BAD_ARG;
+  if (each && n_scans > 0 && check_params(h, p, n_scans, true, false)) return QB200_ERR_BAD_ARG;
+  Lane* L = h->lane[0].get();
+  for (int i = 0; i < n_scans; ++i)
+    if (slot_ids[i] < 0 || slot_ids[i] >= h->c_slots || n_points[i] < 0 || n_points[i] > L->R || (n_points[i] > 0 && !scans4[i])) {
+      h->fail(__FILE__, __LINE__, "scan is null, exceeds max_raw_points or names a slot outside qb200_cache_reserve()");
+      return QB200_ERR_BAD_ARG;
+    }
+  const int C = 2 * L->S;
+  for (int c0 = 0; c0 < n_scans; c0 += C) {
+    const int nc = n_scans - c0 < C ? n_scans - c0 : C;
+    int rc;
+    for (int c = 0; c < nc; ++c) {
+      const qb200_params& pc = p[each ? c0 + c : 0];
+      L->h_cloud_ptr[c] = reinterpret_cast<const float4*>(scans4[c0 + c]);
+      L->h_cloud_n[c] = n_points[c0 + c];
+      L->h_front[c] = front_entry(pc);
+      h->h_slot_of_cloud[c] = slot_ids[c0 + c];
+      float* sig = h->c_sig.get() + 4 * (size_t)slot_ids[c0 + c];
+      sig[0] = pc.voxel_size; sig[1] = pc.normal_radius; sig[2] = pc.fpfh_radius; sig[3] = lattice_cell(pc);
+    }
+    if ((rc = upload_front(L, nc))) return rc;
+    if ((rc = stage_raw(L, nc, kind, L->stream))) return rc;
+    if ((rc = wave_reset(L, nc))) return rc;
+    if ((rc = launch_voxel(L, nc))) return rc;
+    if ((rc = launch_fpfh(L, nc))) return rc;
+    if ((rc = cache_copy(h, L, 1, nc))) return rc;
+    QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));  // the pinned tables are reused by the next wave
+  }
+  return QB200_OK;
 }
 
 }  // namespace
@@ -856,6 +923,16 @@ int qb200_register_batch_enqueue_each(qb200_handle* h, const qb200_pair* pairs, 
   return enqueue_call(h, {pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists});
 }
 
+int qb200_register_batch_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
+                               qb200_result* results, const qb200_pair_lists* lists) {
+  return run_call(h, {pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists, true});
+}
+
+int qb200_register_batch_enqueue_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                       qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_call(h, {pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists, true});
+}
+
 int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const float* tgt4, int32_t n_tgt, const qb200_params* p,
                         qb200_result* res) {
   if (!res) return QB200_ERR_BAD_ARG;
@@ -901,34 +978,12 @@ int qb200_cache_reserve(qb200_handle* h, int32_t n_slots) {
 
 int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
                       const qb200_params* p, qb200_mem_kind kind) {
-  if (int rc = enter(h)) return rc;
-  if (n_scans < 0 || (n_scans > 0 && (!scans4 || !n_points || !slot_ids)) || !params_ok(p)) return QB200_ERR_BAD_ARG;
-  Lane* L = h->lane[0].get();
-  for (int i = 0; i < n_scans; ++i)
-    if (slot_ids[i] < 0 || slot_ids[i] >= h->c_slots || n_points[i] < 0 || n_points[i] > L->R || (n_points[i] > 0 && !scans4[i])) {
-      h->fail(__FILE__, __LINE__, "scan is null, exceeds max_raw_points or names a slot outside qb200_cache_reserve()");
-      return QB200_ERR_BAD_ARG;
-    }
-  const float cell = lattice_cell(*p);
-  const int C = 2 * L->S;
-  for (int c0 = 0; c0 < n_scans; c0 += C) {
-    const int nc = n_scans - c0 < C ? n_scans - c0 : C;
-    int rc;
-    for (int c = 0; c < nc; ++c) {
-      L->h_cloud_ptr[c] = reinterpret_cast<const float4*>(scans4[c0 + c]);
-      L->h_cloud_n[c] = n_points[c0 + c];
-      h->h_slot_of_cloud[c] = slot_ids[c0 + c];
-      float* sig = h->c_sig.get() + 4 * (size_t)slot_ids[c0 + c];
-      sig[0] = p->voxel_size; sig[1] = p->normal_radius; sig[2] = p->fpfh_radius; sig[3] = cell;
-    }
-    if ((rc = stage_raw(L, nc, kind, L->stream))) return rc;
-    if ((rc = wave_reset(L, nc))) return rc;
-    if ((rc = launch_voxel(L, nc, p->voxel_size, p->skip_flagged))) return rc;
-    if ((rc = launch_fpfh(L, nc, p->normal_radius, p->fpfh_radius, cell))) return rc;
-    if ((rc = cache_copy(h, L, 1, nc))) return rc;
-    QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));  // the pinned tables are reused by the next wave
-  }
-  return QB200_OK;
+  return cache_scans(h, scans4, n_points, slot_ids, n_scans, p, false, kind);
+}
+
+int qb200_cache_scans_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
+                           const qb200_params* params, qb200_mem_kind kind) {
+  return cache_scans(h, scans4, n_points, slot_ids, n_scans, params, true, kind);
 }
 
 int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_result* results) {
@@ -943,6 +998,11 @@ int qb200_register_cached_ex(qb200_handle* h, const qb200_slot_pair* pairs, int3
 int qb200_register_cached_each(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_result* results,
                                const qb200_pair_lists* lists) {
   return run_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists});
+}
+
+int qb200_register_cached_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                qb200_result* results, const qb200_pair_lists* lists) {
+  return run_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists, true});
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

@@ -57,6 +57,7 @@ struct WaveCounters {
   int* n_cells;      // [clouds]
   int* cloud_status; // [clouds] qb200_status (0 ok)
   int* bbox;         // [clouds*6] ordered-int encoded min xyz / max xyz of kept raw points
+  int* vox_digits;   // [clouds] 8-bit digits of the cloud's voxel keys (run_heads_kernel; -1: refused), read by voxel_centroid_kernel
   int* n_mutual;     // [slots]
   int* n_corr;       // [slots]
   int* swapped;      // [slots]  target cloud larger than source (feature_matcher.cc:84-89)

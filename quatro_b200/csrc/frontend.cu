@@ -52,10 +52,11 @@ static int clog2(int n) {
 // ------------------------------------------------------------------------------------------------
 
 __global__ void __launch_bounds__(256) voxel_bbox_kernel(const float4* const* __restrict__ cloud_ptr, const int* __restrict__ cloud_n,
-                                                         int skip_flagged, int* __restrict__ bbox, int* __restrict__ n_valid,
-                                                         int* __restrict__ chunk_cnt) {
+                                                         const CloudFront* __restrict__ front, int* __restrict__ bbox,
+                                                         int* __restrict__ n_valid, int* __restrict__ chunk_cnt) {
   const int cloud = blockIdx.y;
   const int n = cloud_n[cloud];
+  const int skip_flagged = front[cloud].skip_flagged;
   const float4* __restrict__ pts = cloud_ptr[cloud];
   int mn0 = INT_MAX, mn1 = INT_MAX, mn2 = INT_MAX, mx0 = INT_MIN, mx1 = INT_MIN, mx2 = INT_MIN, cnt = 0;
   // eight independent 16-byte loads in flight per thread and ~30 points per thread: this pass streams the raw scans (230 MB per
@@ -121,24 +122,28 @@ __global__ void __launch_bounds__(256) voxel_bbox_kernel(const float4* const* __
 // K1b / K2b: run heads of the sorted keys of one cloud -> start position of every voxel / cell.
 // One CTA per cloud walks its segment with a carried block scan (sizes never leave the device).
 //   mode 0 (voxels): segment = [raw_off, raw_off + n_valid) of the voxel sort's A (keys) or B (keys_b) array, by the parity of
-//                    the cloud's digit count (voxsort.cu); writes starts[], n_out = #voxels
-//   mode 1 (cells):  segment = [cloud*V, cloud*V + V) of keys, writes starts[] and cell keys
+//                    the cloud's digit count (voxsort.cu); writes starts[], n_out = #voxels and digits_out = that digit count
+//   mode 1 (cells):  segment = [cloud*V, cloud*V + V) of keys, writes starts[] and cell keys (front is not read)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) run_heads_kernel(int mode, const uint64_t* keys, const uint64_t* keys_b, const int* __restrict__ seg_off,
-                                                         int V, int key_shift, float inv_leaf, const int* __restrict__ bbox,
+                                                         int V, int key_shift, const CloudFront* __restrict__ front, const int* __restrict__ bbox,
                                                          const int* __restrict__ n_valid_in, int* __restrict__ starts,
                                                          uint64_t* __restrict__ cell_keys, int* __restrict__ n_out, int* __restrict__ n_valid_out,
-                                                         int* __restrict__ cloud_status) {
+                                                         int* __restrict__ cloud_status, int* __restrict__ digits_out) {
   __shared__ int sm[33];
-  __shared__ int s_overflow;
+  __shared__ int s_overflow, s_valid;  // s_valid: thread 0's running count of valid keys (no register carried across the loop)
   const int cloud = blockIdx.x;
   const int off = mode == 0 ? seg_off[cloud] : cloud * V;
   const int n = mode == 0 ? n_valid_in[cloud] : V;
-  const int digits = mode == 0 ? vox_digits(bbox + cloud * 6, n, inv_leaf) : 0;
+  const int digits = mode == 0 ? vox_digits(bbox + cloud * 6, n, front[cloud].inv_leaf) : 0;
   if (digits & 1) keys = keys_b;
   // [EXT] pcl::VoxelGrid: dx*dy*dz > INT_MAX -> "leaf size too small", input returned unfiltered; also every other case in which
   // PCL's int index would overflow (vox_grid())
-  if (threadIdx.x == 0) s_overflow = digits < 0 ? 1 : 0;
+  if (threadIdx.x == 0) {
+    s_overflow = digits < 0 ? 1 : 0;
+    s_valid = 0;
+    if (digits_out) digits_out[cloud] = digits;
+  }
   __syncthreads();
   if (s_overflow) {
     if (threadIdx.x == 0) {
@@ -148,7 +153,7 @@ __global__ void __launch_bounds__(1024) run_heads_kernel(int mode, const uint64_
     }
     return;
   }
-  int carry = 0, valid_total = 0;
+  int carry = 0;
   // four consecutive keys per thread and round: a quarter of the block scans (three barriers each) of a key-per-thread loop
   constexpr int kPer = 4;
   for (int base = 0; base < n; base += kPer * blockDim.x) {
@@ -185,9 +190,10 @@ __global__ void __launch_bounds__(1024) run_heads_kernel(int mode, const uint64_
       }
     }
     carry += tot;
-    valid_total += vtot;
+    if (threadIdx.x == 0) s_valid += vtot;
   }
   if (threadIdx.x == 0) {
+    const int valid_total = s_valid;
     int nv = carry;
     if (nv > V) {
       nv = V;
@@ -203,21 +209,21 @@ __global__ void __launch_bounds__(1024) run_heads_kernel(int mode, const uint64_
 // K1c: centroid of each voxel, summed in original point order (stable sort) -> identical to the
 // sequential CPU sum.  One thread per voxel; points are gathered through the sorted index.
 __global__ void __launch_bounds__(128) voxel_centroid_kernel(const float4* const* __restrict__ cloud_ptr, const int* __restrict__ raw_off,
-                                                             const uint64_t* sorted_keys, const uint64_t* keys_b, const int* __restrict__ bbox,
-                                                             const int* __restrict__ n_valid, float inv_leaf, uint64_t idx_mask,
+                                                             const uint64_t* sorted_keys, const uint64_t* keys_b, const int* __restrict__ vox_digits,
+                                                             uint64_t idx_mask,
                                                              const int* __restrict__ starts, const int* __restrict__ n_vox, int V,
                                                              float4* __restrict__ vox_pts) {
   const int cloud = blockIdx.y;
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n_vox[cloud]) return;
-  if (vox_digits(bbox + cloud * 6, n_valid[cloud], inv_leaf) & 1) sorted_keys = keys_b;
+  // the cloud's sorted segment: B when run_heads_kernel found an odd digit count, else A
+  const uint64_t* __restrict__ keys = ((vox_digits[cloud] & 1) ? keys_b : sorted_keys) + raw_off[cloud];
   const float4* __restrict__ pts = cloud_ptr[cloud];
-  const int off = raw_off[cloud];
   const int a = starts[(size_t)cloud * (V + 1) + r], b = starts[(size_t)cloud * (V + 1) + r + 1];
   float sx = 0.f, sy = 0.f, sz = 0.f;
   int t = a;
   for (; t + 4 <= b; t += 4) {  // four gathers in flight, summed in order
-    const uint64_t k0 = sorted_keys[off + t], k1 = sorted_keys[off + t + 1], k2 = sorted_keys[off + t + 2], k3 = sorted_keys[off + t + 3];
+    const uint64_t k0 = keys[t], k1 = keys[t + 1], k2 = keys[t + 2], k3 = keys[t + 3];
     const float4 p0 = __ldg(pts + (k0 & idx_mask)), p1 = __ldg(pts + (k1 & idx_mask)), p2 = __ldg(pts + (k2 & idx_mask)),
                  p3 = __ldg(pts + (k3 & idx_mask));
     sx += p0.x; sy += p0.y; sz += p0.z;
@@ -226,7 +232,7 @@ __global__ void __launch_bounds__(128) voxel_centroid_kernel(const float4* const
     sx += p3.x; sy += p3.y; sz += p3.z;
   }
   for (; t < b; ++t) {
-    const float4 p = __ldg(pts + (sorted_keys[off + t] & idx_mask));
+    const float4 p = __ldg(pts + (keys[t] & idx_mask));
     sx += p.x; sy += p.y; sz += p.z;
   }
   const float cnt = (float)(b - a);
@@ -234,13 +240,15 @@ __global__ void __launch_bounds__(128) voxel_centroid_kernel(const float4* const
 }
 
 // K2a: lattice keys of the (voxelised) clouds
-__global__ void __launch_bounds__(256) lattice_keys_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V, float inv_cell,
-                                                           uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+__global__ void __launch_bounds__(256) lattice_keys_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V,
+                                                           const CloudFront* __restrict__ front, uint64_t* __restrict__ keys,
+                                                           uint32_t* __restrict__ vals) {
   const int cloud = blockIdx.y;
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= V) return;
   uint64_t cell = kCellInvalid;
   if (r < n_pts[cloud]) {
+    const float inv_cell = front[cloud].inv_cell;
     const float4 p = pts[(size_t)cloud * V + r];
     if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) {
       const int ci = (int)floorf(p.x * inv_cell), cj = (int)floorf(p.y * inv_cell), ck = (int)floorf(p.z * inv_cell);
@@ -265,9 +273,10 @@ struct LatticeView {
 
 // candidates of the occupied cells [c0, c1): loads are issued four points at a time (index -> point are dependent loads;
 // independent candidates overlap their latency), tests and callbacks stay in (cell, index) order
-template <class F>
-__device__ __forceinline__ void walk_cells(const LatticeView& L, const float4 pq, float r2, int c0, int c1, F&& f) {
+template <class R2, class F>
+__device__ __forceinline__ void walk_cells(const LatticeView& L, const float4 pq, const R2& r2_src, int c0, int c1, F&& f) {
   if (c0 >= c1) return;
+  const float r2 = r2_src;  // once per cell range (see for_each_neighbor)
   const int t1 = L.cstart[c1];
   for (int t = L.cstart[c0]; t < t1; t += 4) {
     int p[4];
@@ -286,9 +295,11 @@ __device__ __forceinline__ void walk_cells(const LatticeView& L, const float4 pq
   }
 }
 
-// kLockstep = false: rows one after the other, in the same order; for callbacks too heavy to be repeated for nine unrolled rows
-template <bool kLockstep = true, class F>
-__device__ __forceinline__ void for_each_neighbor(const LatticeView& L, const float4 pq, int m, float r2, F&& f) {
+// kLockstep = false: rows one after the other, in the same order; for callbacks too heavy to be repeated for nine unrolled rows.
+// r2: the squared radius, a float or a volatile shared-memory copy that each cell range reads once, so that no register holds it
+// across the binary searches.
+template <bool kLockstep = true, class R2, class F>
+__device__ __forceinline__ void for_each_neighbor(const LatticeView& L, const float4 pq, int m, const R2& r2, F&& f) {
   if (!(isfinite(pq.x) && isfinite(pq.y) && isfinite(pq.z))) return;
   const int ci = (int)floorf(pq.x * L.inv), cj = (int)floorf(pq.y * L.inv), ck = (int)floorf(pq.z * L.inv);
   if (!cell_ok(ci, cj, ck)) return;
@@ -416,16 +427,20 @@ __device__ __forceinline__ int walk_chunk(const LatticeView& L, const float4 pq,
 // consume the list; a point with more than kNbrGlobalCap neighbours makes its consumers walk the lattice themselves.
 __global__ void __launch_bounds__(kNbrThreads) nbr_list_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V,
                                                                const uint64_t* __restrict__ cell_key, const int* __restrict__ cell_start,
-                                                               const uint32_t* __restrict__ order, const int* __restrict__ n_cells, float inv,
-                                                               int m, float r2, uint32_t* __restrict__ nbr_list,
+                                                               const uint32_t* __restrict__ order, const int* __restrict__ n_cells,
+                                                               const CloudFront* __restrict__ front, uint32_t* __restrict__ nbr_list,
                                                                int* __restrict__ nbr_cnt) {
+  volatile __shared__ float s_r2;
   const int cloud = blockIdx.y;
+  if (threadIdx.x == 0) s_r2 = front[cloud].rf2;
+  __syncthreads();
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_pts[cloud]) return;
-  const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, inv);
+  const int m = front[cloud].mf;
+  const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, front[cloud].inv_cell);
   uint32_t* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
   int k = 0;
-  for_each_neighbor(L, L.pts[q], m, r2, [&](int p, float, const float4) {
+  for_each_neighbor(L, L.pts[q], m, s_r2, [&](int p, float, const float4) {
     if (k < kNbrGlobalCap) gl[(size_t)k * V] = (uint32_t)p;
     ++k;
   });
@@ -436,14 +451,17 @@ __global__ void __launch_bounds__(kNbrThreads) nbr_list_kernel(const float4* __r
 // normal_radius: the subsequence of the K2c list that passes the (bit-identical) distance test.
 __global__ void __launch_bounds__(128) normals_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V,
                                                       const uint64_t* __restrict__ cell_key, const int* __restrict__ cell_start,
-                                                      const uint32_t* __restrict__ order, const int* __restrict__ n_cells, float inv, int m,
-                                                      float r2, const uint32_t* __restrict__ nbr_list, const int* __restrict__ nbr_cnt,
-                                                      int list_usable, float4* __restrict__ normals) {
+                                                      const uint32_t* __restrict__ order, const int* __restrict__ n_cells,
+                                                      const CloudFront* __restrict__ front, const uint32_t* __restrict__ nbr_list,
+                                                      const int* __restrict__ nbr_cnt, float4* __restrict__ normals) {
+  volatile __shared__ float s_r2;
   const int cloud = blockIdx.y;
+  if (threadIdx.x == 0) s_r2 = front[cloud].rn2;
+  __syncthreads();
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_pts[cloud]) return;
-  const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, inv);
-  const float4 pq = L.pts[q];
+  const float4* __restrict__ P = pts + (size_t)cloud * V;
+  const float4 pq = P[q];
   float accu[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   int cnt = 0;
   auto add = [&](const float4 pp) {
@@ -453,16 +471,18 @@ __global__ void __launch_bounds__(128) normals_kernel(const float4* __restrict__
     ++cnt;
   };
   const int kq = nbr_cnt[(size_t)cloud * V + q];
-  if (list_usable && kq <= kNbrGlobalCap) {
+  if (front[cloud].list_usable && kq <= kNbrGlobalCap) {
     const uint32_t* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
+    const float r2 = s_r2;
     for (int t = 0; t < kq; ++t) {
-      const float4 pp = L.pts[gl[(size_t)t * V]];
+      const float4 pp = P[gl[(size_t)t * V]];
       const float dx = pq.x - pp.x, dy = pq.y - pp.y, dz = pq.z - pp.z;
       const float d2 = (dx * dx + dy * dy) + dz * dz;  // same expression as the lattice walk
       if (d2 < r2) add(pp);
     }
   } else {
-    for_each_neighbor(L, pq, m, r2, [&](int, float, const float4 pp) { add(pp); });
+    const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, front[cloud].inv_cell);
+    for_each_neighbor(L, pq, front[cloud].mn, s_r2, [&](int, float, const float4 pp) { add(pp); });
   }
   float out[4];
   qb_normal_from_accu(accu, cnt, pq.x, pq.y, pq.z, out);
@@ -483,7 +503,7 @@ template <bool kRare>
 __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __restrict__ pts, const float4* __restrict__ normals,
                                                             const int* __restrict__ n_pts, int V, const uint64_t* __restrict__ cell_key,
                                                             const int* __restrict__ cell_start, const uint32_t* __restrict__ order,
-                                                            const int* __restrict__ n_cells, float inv, int m, float r2,
+                                                            const int* __restrict__ n_cells, const CloudFront* __restrict__ front,
                                                             float* __restrict__ spfh, const uint32_t* __restrict__ nbr_list,
                                                             const int* __restrict__ nbr_cnt) {
   using Count = typename std::conditional<kRare, unsigned, unsigned short>::type;
@@ -494,7 +514,7 @@ __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __rest
   if (q >= n_pts[cloud]) return;
   int k = nbr_cnt[(size_t)cloud * V + q];
   if ((k > kNbrGlobalCap) != kRare) return;
-  const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, inv);
+  const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, front[cloud].inv_cell);
   const float4* __restrict__ nrm = normals + (size_t)cloud * V;
   const float4 pq = L.pts[q];
   const float4 nq = nrm[q];
@@ -518,6 +538,8 @@ __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __rest
   } else {
     k = 0;
     WalkPos pos;
+    const int m = front[cloud].mf;
+    const float r2 = front[cloud].rf2;
     const int rows = (2 * m + 1) * (2 * m + 1);
     while (pos.row < rows) {
       const int n = walk_chunk(L, pq, m, r2, pos, nbr);
@@ -593,14 +615,16 @@ __global__ void __launch_bounds__(3 * kNbrThreads, 3) fpfh_list_kernel(const flo
 // the rare point with more than kNbrGlobalCap neighbours walks the lattice itself (one thread, all 33 bins, one walk)
 __global__ void __launch_bounds__(kNbrThreads) fpfh_rare_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V,
                                                                 const uint64_t* __restrict__ cell_key, const int* __restrict__ cell_start,
-                                                                const uint32_t* __restrict__ order, const int* __restrict__ n_cells, float inv,
-                                                                int m, float r2, const float* __restrict__ spfh,
+                                                                const uint32_t* __restrict__ order, const int* __restrict__ n_cells,
+                                                                const CloudFront* __restrict__ front, const float* __restrict__ spfh,
                                                                 const int* __restrict__ nbr_cnt, float* __restrict__ desc_t) {
   const int cloud = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_pts[cloud]) return;
   if (nbr_cnt[(size_t)cloud * V + q] <= kNbrGlobalCap) return;  // fpfh_list_kernel
-  const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, inv);
+  const int m = front[cloud].mf;
+  const float r2 = front[cloud].rf2;
+  const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, front[cloud].inv_cell);
   const float4* __restrict__ sp = reinterpret_cast<const float4*>(spfh + (size_t)cloud * V * kDescPad);
   const float4 pq = L.pts[q];
   float o[kDescDim];
@@ -654,57 +678,71 @@ __global__ void desc_from_aos_kernel(const float* __restrict__ in, int V, int n,
 // ------------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------------
-int launch_voxel(Lane* h, int n_clouds, float leaf, int skip_flagged) {
+void front_voxel(CloudFront* e, float leaf, int skip_flagged) {
+  e->inv_leaf = 1.0f / leaf;
+  e->skip_flagged = skip_flagged;
+}
+
+void front_lattice(CloudFront* e, float normal_radius, float fpfh_radius, float cell) {
+  e->inv_cell = 1.0f / cell;
+  e->mn = (int)ceilf(normal_radius * e->inv_cell + 1e-3f);
+  e->mf = (int)ceilf(fpfh_radius * e->inv_cell + 1e-3f);
+  e->rn2 = (float)((double)normal_radius * (double)normal_radius);
+  e->rf2 = (float)((double)fpfh_radius * (double)fpfh_radius);
+  // the list serves K3 when the normal neighbourhood is a subset visited in the same order: radius <= fpfh radius (checked
+  // by the callers) and the same lattice reach for both walks
+  e->list_usable = (e->mn <= e->mf && e->rn2 <= e->rf2) ? 1 : 0;
+}
+
+int upload_front(Lane* L, int n) {
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_front, L->h_front, (size_t)n * sizeof(CloudFront), cudaMemcpyHostToDevice, L->stream));
+  return QB200_OK;
+}
+
+int launch_voxel(Lane* h, int n_clouds) {
   if (n_clouds <= 0) return QB200_OK;
-  const float inv = 1.0f / leaf;
   const dim3 gb(n_clouds >= 16 ? 16 : 64, n_clouds);  // ~30 points per thread when the batch fills the device on its own
   int* chunk_cnt = reinterpret_cast<int*>(h->val_b.get());   // [clouds][kVsChunks]
-  voxel_bbox_kernel<<<gb, 256, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, skip_flagged, h->ctr.bbox, h->ctr.n_valid, chunk_cnt);
+  voxel_bbox_kernel<<<gb, 256, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, h->d_front, h->ctr.bbox, h->ctr.n_valid, chunk_cnt);
   h->launches += 1;
   const int idx_bits = clog2(h->R > 2 ? h->R : 2);  // point index inside its scan
-  if (int rc = launch_voxel_sort(h, n_clouds, inv, skip_flagged, idx_bits)) return rc;
-  run_heads_kernel<<<n_clouds, 1024, 0, h->stream>>>(0, h->key_a, h->key_b, h->d_raw_off, h->V, idx_bits, inv, h->ctr.bbox, h->ctr.n_valid,
-                                                     h->vox_start, nullptr, h->ctr.n_vox, nullptr, h->ctr.cloud_status);
+  if (int rc = launch_voxel_sort(h, n_clouds, idx_bits)) return rc;
+  run_heads_kernel<<<n_clouds, 1024, 0, h->stream>>>(0, h->key_a, h->key_b, h->d_raw_off, h->V, idx_bits, h->d_front, h->ctr.bbox, h->ctr.n_valid,
+                                                     h->vox_start, nullptr, h->ctr.n_vox, nullptr, h->ctr.cloud_status, h->ctr.vox_digits);
   const dim3 gc((h->V + 127) / 128, n_clouds);
-  voxel_centroid_kernel<<<gc, 128, 0, h->stream>>>(h->d_cloud_ptr, h->d_raw_off, h->key_a, h->key_b, h->ctr.bbox, h->ctr.n_valid, inv,
+  voxel_centroid_kernel<<<gc, 128, 0, h->stream>>>(h->d_cloud_ptr, h->d_raw_off, h->key_a, h->key_b, h->ctr.vox_digits,
                                                    (1ull << idx_bits) - 1, h->vox_start, h->ctr.n_vox, h->V, h->vox_pts);
   h->launches += 2;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;
 }
 
-int launch_fpfh(Lane* h, int n_clouds, float normal_radius, float fpfh_radius, float cell) {
+int launch_fpfh(Lane* h, int n_clouds) {
   if (n_clouds <= 0) return QB200_OK;
   const int V = h->V;
-  const float inv = 1.0f / cell;
-  const int mn = (int)ceilf(normal_radius * inv + 1e-3f), mf = (int)ceilf(fpfh_radius * inv + 1e-3f);
-  const float rn2 = (float)((double)normal_radius * (double)normal_radius), rf2 = (float)((double)fpfh_radius * (double)fpfh_radius);
   const dim3 gl((V + 255) / 256, n_clouds);
-  lattice_keys_kernel<<<gl, 256, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, inv, h->key_a, h->val_a);
+  lattice_keys_kernel<<<gl, 256, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->d_front, h->key_a, h->val_a);
   h->launches++;
   // per-cloud shared-memory sort (sort.cu); clouds too large for it go through the device-wide radix sort
   int rc = launch_cloud_sort(h, n_clouds, h->ctr.n_vox, 18, 36);  // fields of cell_key(): i | j | k
   if (rc == QB200_ERR_UNSUPPORTED) rc = sort_pairs(h, n_clouds * V, kCloudShift + clog2(n_clouds > 1 ? n_clouds : 2));
   if (rc) return rc;
-  run_heads_kernel<<<n_clouds, 1024, 0, h->stream>>>(1, h->key_b, nullptr, nullptr, V, 0, inv, nullptr, nullptr, h->cell_start, h->cell_key,
-                                                     h->ctr.n_cells, h->ctr.n_lat, h->ctr.cloud_status);
+  run_heads_kernel<<<n_clouds, 1024, 0, h->stream>>>(1, h->key_b, nullptr, nullptr, V, 0, nullptr, nullptr, nullptr, h->cell_start, h->cell_key,
+                                                     h->ctr.n_cells, h->ctr.n_lat, h->ctr.cloud_status, nullptr);
   const dim3 gp((V + 127) / 128, n_clouds);
-  nbr_list_kernel<<<gp, kNbrThreads, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->cell_key, h->cell_start, h->val_b, h->ctr.n_cells, inv, mf,
-                                                     rf2, h->nbr_list, h->nbr_cnt);
-  // the list serves K3 when the normal neighbourhood is a subset visited in the same order: radius <= fpfh radius (checked
-  // by the callers) and the same lattice reach for both walks
-  const int list_usable = (mn <= mf && rn2 <= rf2) ? 1 : 0;
-  normals_kernel<<<gp, 128, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->cell_key, h->cell_start, h->val_b, h->ctr.n_cells, inv, mn, rn2,
-                                            h->nbr_list, h->nbr_cnt, list_usable, h->normals);
+  nbr_list_kernel<<<gp, kNbrThreads, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->cell_key, h->cell_start, h->val_b, h->ctr.n_cells,
+                                                     h->d_front, h->nbr_list, h->nbr_cnt);
+  normals_kernel<<<gp, 128, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->cell_key, h->cell_start, h->val_b, h->ctr.n_cells, h->d_front,
+                                            h->nbr_list, h->nbr_cnt, h->normals);
   // listed neighbourhoods (all but a handful of points) and the lattice-walking rest are separate launches: the common kernels
   // carry neither the walk's registers nor its list buffer
   spfh_kernel<false><<<gp, kSpfhThreads, 0, h->stream>>>(h->vox_pts, h->normals, h->ctr.n_vox, V, h->cell_key, h->cell_start, h->val_b,
-                                                         h->ctr.n_cells, inv, mf, rf2, h->spfh, h->nbr_list, h->nbr_cnt);
+                                                         h->ctr.n_cells, h->d_front, h->spfh, h->nbr_list, h->nbr_cnt);
   spfh_kernel<true><<<gp, kSpfhThreads, 0, h->stream>>>(h->vox_pts, h->normals, h->ctr.n_vox, V, h->cell_key, h->cell_start, h->val_b,
-                                                        h->ctr.n_cells, inv, mf, rf2, h->spfh, h->nbr_list, h->nbr_cnt);
+                                                        h->ctr.n_cells, h->d_front, h->spfh, h->nbr_list, h->nbr_cnt);
   fpfh_list_kernel<<<gp, 3 * kNbrThreads, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->spfh, h->nbr_list, h->nbr_cnt, h->desc_t);
-  fpfh_rare_kernel<<<gp, kNbrThreads, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->cell_key, h->cell_start, h->val_b, h->ctr.n_cells, inv, mf,
-                                                      rf2, h->spfh, h->nbr_cnt, h->desc_t);
+  fpfh_rare_kernel<<<gp, kNbrThreads, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->cell_key, h->cell_start, h->val_b, h->ctr.n_cells,
+                                                      h->d_front, h->spfh, h->nbr_cnt, h->desc_t);
   h->launches += 3;
   h->launches += 4;
   QB_CUDA_TRY(h, cudaGetLastError());

@@ -26,15 +26,29 @@ struct PoseParams {
   double RyRx[9];
 };
 
-// One pair's solver configuration, as K8..K11 read it from the lane's table (DESIGN §5.4): the solver fields of its qb200_params,
-// resolved on the host.  mode == QB200_INLIER_NONE: the pair skips K8 / K9 and gets the identity clique.
+// One pair's solver configuration, as K7..K11 read it from the lane's table (DESIGN §5.4): the matcher and solver fields of its
+// qb200_params, resolved on the host.  mode == QB200_INLIER_NONE: the pair skips K8 / K9 and gets the identity clique.
 struct PairSolve {
   GraphConst gc;
   PoseParams pp;
   double kcore_thr;
   long long node_limit;      // PMC_EXACT nodes (0 already resolved to QB200_DEFAULT_CLIQUE_NODE_LIMIT)
   int mode;                  // QB200_PMC_EXACT .. QB200_INLIER_NONE
-  int reserved;
+  int use_tuple;             // K7's tuple test runs for this pair: use_tuple_test and tuple_scale != 0 (match_fields)
+  float tuple_scale;
+  int tuple_trials;          // trials per mutual correspondence
+  unsigned long long seed;
+};
+
+// One cloud's front-end configuration, as K1..K5 read it from the lane's table d_front (DESIGN §5.4): the voxel and lattice fields of
+// its qb200_params, resolved on the host by front_voxel / front_lattice.  A kernel loads its cloud's entry once, at its start.
+struct CloudFront {
+  float inv_leaf;            // 1 / voxel_size
+  int skip_flagged;
+  float inv_cell;            // 1 / lattice cell
+  int mn, mf;                // lattice reach of the normal / FPFH radius, in cells
+  float rn2, rf2;            // squared normal / FPFH radius
+  int list_usable;           // K3 may read K2c's neighbour list (the normal neighbourhood is a subsequence of it)
 };
 
 struct PpScan;   // one scan's pre-processing entry (preprocess.cu)
@@ -112,6 +126,7 @@ struct Lane {
   DeviceMem<int> final_inl;   // [S*Lc]
   DeviceMem<unsigned char> rot_mask, trans_mask; // [S*Lc]
   DeviceMem<PairSolve> d_solve; PinnedMem<PairSolve> h_solve;  // [S] solver table of the wave, and its pinned mirror (upload_solve copies it)
+  DeviceMem<CloudFront> d_front; PinnedMem<CloudFront> h_front;  // [2S] front-end table of the wave, and its pinned mirror (upload_front)
   // ---- pre-processing (preprocess.cu), allocated on first use for the largest wave so far (pw_scans / ip_cap) ----
   DeviceMem<int> pp_cnt; PinnedMem<int> pp_hcnt;  // [2S][8] per-scan counts and status of a wave, and its pinned mirror
   DeviceMem<PpScan> d_pp; PinnedMem<PpScan> h_pp; // [2S] per-scan parameter table of a wave, and its pinned mirror (one H2D per wave)
@@ -204,10 +219,20 @@ constexpr int kCliqueWarps = 8;
 __host__ __device__ inline size_t kcore_ws_bytes(int Lc) { return ((size_t)(Lc + 2) * 4 + (size_t)8 * Lc * 2 + 15) & ~(size_t)15; }
 size_t pose_ws_bytes(int Lc);
 
-// Stage launchers (each enqueues kernels on the lane's stream for clouds/pairs [0, n) of its current wave).
-int launch_voxel(Lane* h, int n_clouds, float leaf, int skip_flagged);
-int launch_fpfh(Lane* h, int n_clouds, float normal_radius, float fpfh_radius, float cell);
-int launch_match(Lane* h, int n_pairs, const qb200_params& p);
+// Stage launchers (each enqueues kernels on the lane's stream for clouds/pairs [0, n) of its current wave).  K1..K5 read every cloud's
+// configuration from the lane's table d_front (upload_front), K7 every pair's tuple test from d_solve (upload_solve); launch_match
+// launches the tuple test only when h_solve has a pair that runs it.
+int launch_voxel(Lane* h, int n_clouds);
+int launch_fpfh(Lane* h, int n_clouds);
+int launch_match(Lane* h, int n_pairs);
+// a cloud's front-end entry: its voxel fields (frontend.cu), its lattice fields for these radii and this lattice cell (frontend.cu),
+// or both from p (api.cu)
+void front_voxel(CloudFront* e, float leaf, int skip_flagged);
+void front_lattice(CloudFront* e, float normal_radius, float fpfh_radius, float cell);
+CloudFront front_entry(const qb200_params& p);
+// the entries [0, n) of h_front to d_front on the lane's stream: one copy (h_front must stay as it is until the stream passed it)
+int upload_front(Lane* h, int n);
+void match_fields(PairSolve* e, const qb200_params& p);  // K7's fields of a pair's entry (match.cu)
 // The solver stages read every pair's configuration from the lane's table d_solve (upload_solve): K8 skips the pairs in
 // QB200_INLIER_NONE, K9 runs each pair in its own mode (the exact search only when the table has a PMC_EXACT pair: any_exact),
 // iota_clique_kernel fills only the QB200_INLIER_NONE pairs.
@@ -219,7 +244,7 @@ int launch_finalize_status(Lane* h, int n_pairs);
 int launch_iota_clique(Lane* h, int n_pairs);
 GraphConst graph_const(double noise_bound, double cbar2);
 PoseParams pose_params(const qb200_params& p);  // p's rotation noise bound already resolved
-PairSolve solve_entry(const qb200_params& p);   // the same, every solver field
+PairSolve solve_entry(const qb200_params& p);   // the same, every matcher and solver field
 // the entries [0, n) of h_solve to d_solve on the lane's stream: one copy (h_solve must stay as it is until the stream passed it)
 int upload_solve(Lane* h, int n);
 // Where pack_lists_kernel writes pair s's lists: each array (nullptr = not asked for) + s * stride entries, at most cap of them.
@@ -264,7 +289,7 @@ void set_last(qb200_handle* h, const qb200_result& r);
 // (function, device), not of a handle: handles of different capacities share it, so it is only ever raised (process-wide maximum).
 cudaError_t ensure_dyn_smem(int device, const void* kernel, size_t bytes);
 int sort_pairs(Lane* h, int n_items, int end_bit);
-int launch_voxel_sort(Lane* h, int n_clouds, float inv_leaf, int skip_flagged, int idx_bits);
+int launch_voxel_sort(Lane* h, int n_clouds, int idx_bits);
 int launch_cloud_sort(Lane* h, int n_clouds, const int* n_items, int f1, int f2);
 
 }  // namespace qb

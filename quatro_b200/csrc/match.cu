@@ -209,11 +209,14 @@ __global__ void __launch_bounds__(1024) match_mutual_kernel(const unsigned long 
 
 // Matcher::normalizePoints: float mean accumulated in index order.  One warp per cloud: chunks of 32 points are staged in
 // shared memory with coalesced loads (two chunks ahead); lanes 0..2 each own one coordinate and run its serial addition
-// chain from shared memory (a 4-cycle dependent add per point instead of a shuffle round trip).
-__global__ void __launch_bounds__(32) cloud_mean_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V, float* __restrict__ mean) {
+// chain from shared memory (a 4-cycle dependent add per point instead of a shuffle round trip).  Only the clouds of pairs that run
+// the tuple test, its only reader.
+__global__ void __launch_bounds__(32) cloud_mean_kernel(const float4* __restrict__ pts, const int* __restrict__ n_pts, int V,
+                                                        const PairSolve* __restrict__ solve, float* __restrict__ mean) {
   constexpr int kChunk = 4;                 // 32-point rows per round: 4 loads per lane in flight cover the L2 / DRAM latency
   __shared__ float buf[2][3][32 * kChunk];
   const int cloud = blockIdx.x, lane = (int)lane_id();
+  if (!solve[cloud >> 1].use_tuple) return;
   const int n = n_pts[cloud];
   const float4* __restrict__ p = pts + (size_t)cloud * V;
   const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -268,19 +271,23 @@ __device__ __forceinline__ float tri_side(const float4 a, const float4 b, const 
 
 // tuple (triangle side-ratio) test, feature_matcher.cc:187-247: one thread per trial, counter-based RNG.  Every trial reads six
 // random matched points: a CTA first stages the pair's matched points (both clouds, xyz) in shared memory when they fit
-// (<= kTupleStage mutual pairs, the usual case), so the random reads stay on chip.
+// (<= kTupleStage mutual pairs, the usual case), so the random reads stay on chip.  Scale, trials and seed are the pair's own
+// (solve[pair]); the CTAs of a pair that does not run the test leave at once.
 constexpr int kTupleStage = 1536;
 constexpr int kTupleThreads = 1024;
 constexpr int kTupleCtasPerPair = 8;
 __global__ void __launch_bounds__(kTupleThreads) tuple_test_kernel(const float4* __restrict__ vox_pts, int V, const int* __restrict__ mut_i,
                                                                    const int* __restrict__ mut_j, const int* __restrict__ n_mutual,
-                                                                   const int* __restrict__ swapped, const float* __restrict__ mean, float scale,
-                                                                   int trials_per_corr, unsigned long long seed, unsigned char* __restrict__ mark) {
+                                                                   const int* __restrict__ swapped, const float* __restrict__ mean,
+                                                                   const PairSolve* __restrict__ solve, unsigned char* __restrict__ mark) {
   __shared__ float sp[2][kTupleStage][3];
   const int pair = blockIdx.y;
+  if (!solve[pair].use_tuple) return;
   const int ncorr = n_mutual[pair];
   if (ncorr <= 0) return;
-  const long long trials = (long long)ncorr * trials_per_corr;
+  const float scale = solve[pair].tuple_scale;
+  const unsigned long long seed = solve[pair].seed;
+  const long long trials = (long long)ncorr * solve[pair].tuple_trials;
   const bool sw = swapped[pair] != 0;
   // fi = larger cloud, fj = smaller
   const int ci = sw ? 2 * pair + 1 : 2 * pair, cj = sw ? 2 * pair : 2 * pair + 1;
@@ -322,12 +329,12 @@ __global__ void __launch_bounds__(kTupleThreads) tuple_test_kernel(const float4*
 // survivors -> partner[src] = tgt  (mutual NN is a bijection, so sorting by (src,tgt) = sorting by src)
 __global__ void __launch_bounds__(256) scatter_partner_kernel(const int* __restrict__ mut_i, const int* __restrict__ mut_j,
                                                               const int* __restrict__ n_mutual, const int* __restrict__ swapped,
-                                                              const unsigned char* __restrict__ mark, int use_tuple, int V,
-                                                              int* __restrict__ partner) {
+                                                              const unsigned char* __restrict__ mark, const PairSolve* __restrict__ solve,
+                                                              int V, int* __restrict__ partner) {
   const int pair = blockIdx.y;
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n_mutual[pair]) return;
-  if (use_tuple && !mark[(size_t)pair * V + e]) return;
+  if (solve[pair].use_tuple && !mark[(size_t)pair * V + e]) return;
   const int i = mut_i[(size_t)pair * V + e], j = mut_j[(size_t)pair * V + e];
   const bool sw = swapped[pair] != 0;
   const int s = sw ? j : i, t = sw ? i : j;
@@ -411,7 +418,14 @@ __global__ void match_verify_kernel(const unsigned long long* __restrict__ rb_tc
   }
 }
 
-int launch_match(Lane* h, int n_pairs, const qb200_params& p) {
+void match_fields(PairSolve* e, const qb200_params& p) {
+  e->use_tuple = (p.use_tuple_test && p.tuple_scale != 0.0f) ? 1 : 0;
+  e->tuple_scale = p.tuple_scale;
+  e->tuple_trials = p.tuple_trials_per_corr;
+  e->seed = p.seed;
+}
+
+int launch_match(Lane* h, int n_pairs) {
   if (n_pairs <= 0) return QB200_OK;
   const int V = h->V;
   int rc = h->force_exact_match ? launch_match_exact(h, n_pairs, nullptr) : launch_match_nn(h, n_pairs);
@@ -430,16 +444,17 @@ int launch_match(Lane* h, int n_pairs, const qb200_params& p) {
   match_mutual_kernel<<<n_pairs, 1024, 0, h->stream>>>(h->rowbest, h->colbest, h->ctr.n_vox, V, h->mut_i, h->mut_j, h->ctr.n_mutual,
                                                        h->ctr.swapped, h->mark, h->partner);
   h->launches += 1;
-  const int use_tuple = (p.use_tuple_test && p.tuple_scale != 0.0f) ? 1 : 0;
-  if (use_tuple) {
-    cloud_mean_kernel<<<2 * n_pairs, 32, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->mean);
+  bool any_tuple = false;  // the host's copy of the pairs' table (h_solve) decides whether the tuple test is launched at all
+  for (int s = 0; s < n_pairs; ++s) any_tuple |= h->h_solve[s].use_tuple != 0;
+  if (any_tuple) {
+    cloud_mean_kernel<<<2 * n_pairs, 32, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->d_solve, h->mean);
     const dim3 gt(kTupleCtasPerPair, n_pairs);
-    tuple_test_kernel<<<gt, kTupleThreads, 0, h->stream>>>(h->vox_pts, V, h->mut_i, h->mut_j, h->ctr.n_mutual, h->ctr.swapped, h->mean, p.tuple_scale,
-                                                 p.tuple_trials_per_corr, (unsigned long long)p.seed, h->mark);
+    tuple_test_kernel<<<gt, kTupleThreads, 0, h->stream>>>(h->vox_pts, V, h->mut_i, h->mut_j, h->ctr.n_mutual, h->ctr.swapped, h->mean, h->d_solve,
+                                                           h->mark);
     h->launches += 2;
   }
   const dim3 gsc((V + 255) / 256, n_pairs);
-  scatter_partner_kernel<<<gsc, 256, 0, h->stream>>>(h->mut_i, h->mut_j, h->ctr.n_mutual, h->ctr.swapped, h->mark, use_tuple, V, h->partner);
+  scatter_partner_kernel<<<gsc, 256, 0, h->stream>>>(h->mut_i, h->mut_j, h->ctr.n_mutual, h->ctr.swapped, h->mark, h->d_solve, V, h->partner);
   pack_corr_kernel<<<n_pairs, 1024, 0, h->stream>>>(h->partner, h->vox_pts, h->ctr.n_vox, V, h->Lc, h->corr_src, h->corr_tgt, h->ma, h->mb,
                                                     h->ctr.n_corr, h->ctr.cloud_status);
   h->launches += 2;

@@ -64,9 +64,11 @@ int qb200_voxelize(qb200_handle* h, const float* pts4, int32_t n, float leaf, in
   if (rc) return rc;
   L->h_cloud_ptr[0] = reinterpret_cast<const float4*>(pts4);
   L->h_cloud_n[0] = n;
-  if ((rc = stage_raw(L, 1, QB200_MEM_HOST, L->stream))) return rc;
-  if ((rc = launch_voxel(L, 1, leaf, skip_flagged)) || (rc = read_counters(L))) return rc;
-  QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
+  MirrorHold hold{L};
+  front_voxel(&L->h_front[0], leaf, skip_flagged);  // a one-entry front-end table
+  if ((rc = upload_front(L, 1)) || (rc = stage_raw(L, 1, QB200_MEM_HOST, L->stream))) return rc;
+  if ((rc = launch_voxel(L, 1)) || (rc = read_counters(L))) return rc;
+  QB_CUDA_TRY(h, hold.sync());
   const int nv = L->hctr.n_vox[0], st = L->hctr.cloud_status[0];
   if (st == QB200_ERR_VOXEL_OVERFLOW) {
     // [EXT] pcl::VoxelGrid: "leaf size is too small ... integer indices would overflow" -> output = input
@@ -102,7 +104,8 @@ int qb200_compute_fpfh(qb200_handle* h, const float* pts4, int32_t n, float norm
   if (rc) return rc;
   QB_CUDA_TRY(h, cudaMemcpyAsync(L->vox_pts, pts4, (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
   MirrorHold hold{L};
-  if ((rc = write_counter(L, L->hctr.n_vox, n)) || (rc = launch_fpfh(L, 1, normal_radius, fpfh_radius, grid_cell))) return rc;
+  front_lattice(&L->h_front[0], normal_radius, fpfh_radius, grid_cell);  // a one-entry front-end table
+  if ((rc = write_counter(L, L->hctr.n_vox, n)) || (rc = upload_front(L, 1)) || (rc = launch_fpfh(L, 1))) return rc;
   if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, L->normals, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
   if (desc33) {
     if ((rc = launch_desc_to_aos(L, 0, n, L->aos_scratch))) return rc;
@@ -137,7 +140,9 @@ int qb200_match(qb200_handle* h, const float* src4, int32_t n_src, const float* 
   MirrorHold hold{L};
   if ((rc = write_counter(L, L->hctr.n_vox, n_src)) || (rc = write_counter(L, L->hctr.n_vox + 1, n_tgt))) return rc;
   if ((rc = launch_desc_from_aos(L, 0, n_src, scratch)) || (rc = launch_desc_from_aos(L, 1, n_tgt, scratch2))) return rc;
-  if ((rc = launch_match(L, 1, *p)) || (rc = read_counters(L))) return rc;
+  memset(&L->h_solve[0], 0, sizeof(PairSolve));  // a one-entry pair table: p's tuple test
+  match_fields(&L->h_solve[0], *p);
+  if ((rc = upload_solve(L, 1)) || (rc = launch_match(L, 1)) || (rc = read_counters(L))) return rc;
   QB_CUDA_TRY(h, hold.sync());
   if (n_mutual) *n_mutual = L->hctr.n_mutual[0];
   h->last_n_corr = L->hctr.n_corr[0];
@@ -160,8 +165,11 @@ int qb200_match_and_pack(qb200_handle* h, const float* src4, int32_t n_src, cons
   QB_CUDA_TRY(h, cudaMemcpyAsync(L->vox_pts + L->V, tgt4, (size_t)n_tgt * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
   MirrorHold hold{L};
   if ((rc = write_counter(L, L->hctr.n_vox, n_src)) || (rc = write_counter(L, L->hctr.n_vox + 1, n_tgt))) return rc;
-  if ((rc = launch_fpfh(L, 2, p->normal_radius, p->fpfh_radius, lattice_cell(*p)))) return rc;
-  if ((rc = launch_match(L, 1, *p)) || (rc = read_counters(L))) return rc;
+  L->h_front[0] = L->h_front[1] = front_entry(*p);  // one-entry tables: p's front end and tuple test
+  memset(&L->h_solve[0], 0, sizeof(PairSolve));
+  match_fields(&L->h_solve[0], *p);
+  if ((rc = upload_front(L, 2)) || (rc = upload_solve(L, 1)) || (rc = launch_fpfh(L, 2))) return rc;
+  if ((rc = launch_match(L, 1)) || (rc = read_counters(L))) return rc;
   QB_CUDA_TRY(h, hold.sync());
   h->last_n_corr = L->hctr.n_corr[0];
   if ((rc = qb200_get_last_correspondences(h, corr, src_matched4, tgt_matched4, cap, n_corr))) return rc;

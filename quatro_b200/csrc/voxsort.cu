@@ -26,7 +26,7 @@ constexpr int kVsThreads = 256;
 
 // (voxel << idx_bits | index) of the kept points of one chunk, compacted in scan order.  grid = (kVsChunks, clouds).
 __global__ void __launch_bounds__(kVsThreads) voxel_pack_kernel(const float4* const* __restrict__ cloud_ptr, const int* __restrict__ cloud_n,
-                                                                const int* __restrict__ raw_off, float inv_leaf, int skip_flagged,
+                                                                const int* __restrict__ raw_off, const CloudFront* __restrict__ front,
                                                                 const int* __restrict__ bbox, const int* __restrict__ n_valid,
                                                                 const int* __restrict__ chunk_cnt, int idx_bits, uint64_t* __restrict__ items) {
   __shared__ int sm[33];
@@ -36,6 +36,8 @@ __global__ void __launch_bounds__(kVsThreads) voxel_pack_kernel(const float4* co
   const int c0 = chunk * cs, c1 = min(n, c0 + cs);
   if (c0 >= n) return;
   const float4* __restrict__ pts = cloud_ptr[cloud];
+  const float inv_leaf = front[cloud].inv_leaf;
+  const int skip_flagged = front[cloud].skip_flagged;
   long long m[3] = {0, 0, 0}, d[3] = {1, 1, 1};  // min_b / div_b of pcl::VoxelGrid::applyFilter
   const bool grid_ok = n_valid[cloud] > 0 && vox_grid(bbox + cloud * 6, inv_leaf, m, d);
   int base = 0;  // kept points of the preceding chunks
@@ -81,12 +83,12 @@ __global__ void __launch_bounds__(kVsThreads) voxel_pack_kernel(const float4* co
 // tile histograms of digit `pass`.  hist[cloud][digit][tile], tiles_cap tiles per cloud.  grid = (tiles_cap, clouds).
 __global__ void __launch_bounds__(kVsThreads) vsort_hist_kernel(int pass, const uint64_t* __restrict__ a, const uint64_t* __restrict__ b,
                                                                 const int* __restrict__ raw_off, const int* __restrict__ bbox,
-                                                                const int* __restrict__ n_valid, float inv_leaf, int idx_bits, int tiles_cap,
-                                                                unsigned* __restrict__ hist) {
+                                                                const int* __restrict__ n_valid, const CloudFront* __restrict__ front, int idx_bits,
+                                                                int tiles_cap, unsigned* __restrict__ hist) {
   __shared__ unsigned s_h[256];
   const int cloud = blockIdx.y, tile = blockIdx.x, tid = threadIdx.x;
   const int m = n_valid[cloud];
-  if (tile * kVsTile >= m || pass >= vox_digits(bbox + cloud * 6, m, inv_leaf)) return;
+  if (tile * kVsTile >= m || pass >= vox_digits(bbox + cloud * 6, m, front[cloud].inv_leaf)) return;
   const uint64_t* __restrict__ src = ((pass & 1) ? b : a) + raw_off[cloud];
   s_h[tid] = 0u;
   __syncthreads();
@@ -98,12 +100,12 @@ __global__ void __launch_bounds__(kVsThreads) vsort_hist_kernel(int pass, const 
 }
 
 // exclusive scan of hist[cloud] in (digit, tile) order, in place.  One CTA per cloud.
-__global__ void __launch_bounds__(1024) vsort_scan_kernel(int pass, const int* __restrict__ bbox, const int* __restrict__ n_valid, float inv_leaf,
-                                                          int tiles_cap, unsigned* __restrict__ hist) {
+__global__ void __launch_bounds__(1024) vsort_scan_kernel(int pass, const int* __restrict__ bbox, const int* __restrict__ n_valid,
+                                                          const CloudFront* __restrict__ front, int tiles_cap, unsigned* __restrict__ hist) {
   __shared__ int sm[33];
   const int cloud = blockIdx.x, tid = threadIdx.x;
   const int m = n_valid[cloud];
-  if (m <= 0 || pass >= vox_digits(bbox + cloud * 6, m, inv_leaf)) return;
+  if (m <= 0 || pass >= vox_digits(bbox + cloud * 6, m, front[cloud].inv_leaf)) return;
   const int nt = (m + kVsTile - 1) / kVsTile;     // live tiles: the entries of the others were never written
   unsigned* __restrict__ H = hist + (size_t)cloud * 256 * tiles_cap;
   const int total = 256 * nt;                     // flattened (digit, live tile)
@@ -134,12 +136,12 @@ __global__ void __launch_bounds__(1024) vsort_scan_kernel(int pass, const int* _
 __global__ void __launch_bounds__(kVsThreads) vsort_scatter_kernel(int pass, const uint64_t* __restrict__ a, const uint64_t* __restrict__ b,
                                                                    uint64_t* __restrict__ a_out, uint64_t* __restrict__ b_out,
                                                                    const int* __restrict__ raw_off, const int* __restrict__ bbox,
-                                                                   const int* __restrict__ n_valid, float inv_leaf, int idx_bits, int tiles_cap,
-                                                                   const unsigned* __restrict__ offs) {
+                                                                   const int* __restrict__ n_valid, const CloudFront* __restrict__ front,
+                                                                   int idx_bits, int tiles_cap, const unsigned* __restrict__ offs) {
   __shared__ unsigned s_w[kVsThreads / 32][256];   // per warp: digit counts, then running output positions
   const int cloud = blockIdx.y, tile = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int m = n_valid[cloud];
-  if (tile * kVsTile >= m || pass >= vox_digits(bbox + cloud * 6, m, inv_leaf)) return;
+  if (tile * kVsTile >= m || pass >= vox_digits(bbox + cloud * 6, m, front[cloud].inv_leaf)) return;
   const uint64_t* __restrict__ src = ((pass & 1) ? b : a) + raw_off[cloud];
   uint64_t* __restrict__ dst = ((pass & 1) ? a_out : b_out) + raw_off[cloud];
   const int shift = idx_bits + 8 * pass;
@@ -185,20 +187,21 @@ __global__ void __launch_bounds__(kVsThreads) vsort_scatter_kernel(int pass, con
 }
 
 // Sort the packed items of every cloud (A = key_a, B = key_b).  Afterwards cloud c's sorted segment starts at
-// (vox_digits(c) odd ? B : A) + raw_off[c] and holds n_valid[c] items.
-int launch_voxel_sort(Lane* h, int n_clouds, float inv_leaf, int skip_flagged, int idx_bits) {
+// (vox_digits(c) odd ? B : A) + raw_off[c] and holds n_valid[c] items.  Every kernel takes cloud c's leaf from d_front[c], so all of
+// them agree on its digit count.
+int launch_voxel_sort(Lane* h, int n_clouds, int idx_bits) {
   const int tiles_cap = (h->R + kVsTile - 1) / kVsTile;
   unsigned* hist = reinterpret_cast<unsigned*>(h->val_a.get());        // [clouds][256][tiles_cap]  (alloc_all sizes val_a for it)
   const int* chunk_cnt = reinterpret_cast<const int*>(h->val_b.get()); // [clouds][64]
   const dim3 gp(kVsChunks, n_clouds), gt(tiles_cap, n_clouds);
-  voxel_pack_kernel<<<gp, kVsThreads, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, h->d_raw_off, inv_leaf, skip_flagged, h->ctr.bbox, h->ctr.n_valid,
+  voxel_pack_kernel<<<gp, kVsThreads, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, h->d_raw_off, h->d_front, h->ctr.bbox, h->ctr.n_valid,
                                                      chunk_cnt, idx_bits, h->key_a);
   for (int pass = 0; pass < 4; ++pass) {
-    vsort_hist_kernel<<<gt, kVsThreads, 0, h->stream>>>(pass, h->key_a, h->key_b, h->d_raw_off, h->ctr.bbox, h->ctr.n_valid, inv_leaf, idx_bits,
+    vsort_hist_kernel<<<gt, kVsThreads, 0, h->stream>>>(pass, h->key_a, h->key_b, h->d_raw_off, h->ctr.bbox, h->ctr.n_valid, h->d_front, idx_bits,
                                                        tiles_cap, hist);
-    vsort_scan_kernel<<<n_clouds, 1024, 0, h->stream>>>(pass, h->ctr.bbox, h->ctr.n_valid, inv_leaf, tiles_cap, hist);
+    vsort_scan_kernel<<<n_clouds, 1024, 0, h->stream>>>(pass, h->ctr.bbox, h->ctr.n_valid, h->d_front, tiles_cap, hist);
     vsort_scatter_kernel<<<gt, kVsThreads, 0, h->stream>>>(pass, h->key_a, h->key_b, h->key_a, h->key_b, h->d_raw_off, h->ctr.bbox, h->ctr.n_valid,
-                                                          inv_leaf, idx_bits, tiles_cap, hist);
+                                                          h->d_front, idx_bits, tiles_cap, hist);
   }
   h->launches += 13;
   QB_CUDA_TRY(h, cudaGetLastError());
