@@ -17,6 +17,7 @@
 #include <stdlib.h>
 
 #include "handle.cuh"
+#include "qb_math.cuh"
 
 namespace qb {
 
@@ -271,16 +272,28 @@ __device__ __forceinline__ float tri_side(const float4 a, const float4 b, const 
 
 // tuple (triangle side-ratio) test, feature_matcher.cc:187-247: one thread per trial, counter-based RNG.  Every trial reads six
 // random matched points: a CTA first stages the pair's matched points (both clouds, xyz) in shared memory when they fit
-// (<= kTupleStage mutual pairs, the usual case), so the random reads stay on chip.  Scale, trials and seed are the pair's own
+// (<= kTupleStage mutual pairs: a street pair has 1.2-2.3 k), so the random reads stay on chip instead of chasing mut_i / mut_j and
+// then the point through L2 for each of the six points of a trial.  Scale, trials and seed are the pair's own
 // (solve[pair]); the CTAs of a pair that does not run the test leave at once.
-constexpr int kTupleStage = 1536;
-constexpr int kTupleThreads = 1024;
-constexpr int kTupleCtasPerPair = 8;
+//
+// The mark is a conjunction over the three sides, and most random triples already fail side 0 (r0, r1).  So a warp tests side 0
+// of 32 trials, queues the ones that pass in shared memory (r0, r1 and the raw third draw), and tests sides 1 and 2 once 32 are
+// queued: the square roots and divisions of the other two sides run in full warps and only for the triples that need them.
+// Which trials mark a point does not change, nor does a mark (a trial sets it to 1 or leaves it).  r % ncorr is qb_fastmod.
+constexpr int kTupleStage = 4096;          // 96 KB of staged points
+// 512 threads at 55 registers and 108 KB of shared memory: a tuple CTA fits on an SM beside a tc_nn_kernel CTA of another lane
+constexpr int kTupleThreads = 512;
+constexpr int kTupleWarps = kTupleThreads / 32;
+constexpr int kTupleQueue = 64;             // < 32 entries left over + one warp's 32 pushes
+constexpr int kTupleCtasPerPair = 16;
+constexpr size_t kTupleSmem = sizeof(float) * 2 * kTupleStage * 3 + sizeof(unsigned) * kTupleWarps * 3 * kTupleQueue;
 __global__ void __launch_bounds__(kTupleThreads) tuple_test_kernel(const float4* __restrict__ vox_pts, int V, const int* __restrict__ mut_i,
                                                                    const int* __restrict__ mut_j, const int* __restrict__ n_mutual,
                                                                    const int* __restrict__ swapped, const float* __restrict__ mean,
                                                                    const PairSolve* __restrict__ solve, unsigned char* __restrict__ mark) {
-  __shared__ float sp[2][kTupleStage][3];
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  float(*sp)[kTupleStage][3] = reinterpret_cast<float(*)[kTupleStage][3]>(smem_raw);                                // [2][kTupleStage][3]
+  unsigned(*sq)[3][kTupleQueue] = reinterpret_cast<unsigned(*)[3][kTupleQueue]>(smem_raw + sizeof(float) * 2 * kTupleStage * 3);
   const int pair = blockIdx.y;
   if (!solve[pair].use_tuple) return;
   const int ncorr = n_mutual[pair];
@@ -288,6 +301,8 @@ __global__ void __launch_bounds__(kTupleThreads) tuple_test_kernel(const float4*
   const float scale = solve[pair].tuple_scale;
   const unsigned long long seed = solve[pair].seed;
   const long long trials = (long long)ncorr * solve[pair].tuple_trials;
+  const unsigned nc = (unsigned)ncorr;
+  const uint64_t magic = qb_fastmod_magic(nc);
   const bool sw = swapped[pair] != 0;
   // fi = larger cloud, fj = smaller
   const int ci = sw ? 2 * pair + 1 : 2 * pair, cj = sw ? 2 * pair : 2 * pair + 1;
@@ -311,19 +326,47 @@ __global__ void __launch_bounds__(kTupleThreads) tuple_test_kernel(const float4*
     if (staged) return make_float4(sp[side][r][0], sp[side][r][1], sp[side][r][2], 0.f);
     return side == 0 ? pi[li[r]] : pj[lj[r]];
   };
-  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < trials; t += (long long)gridDim.x * blockDim.x) {
-    unsigned r[4];
-    philox4x32_10(seed, (unsigned long long)t, r);
-    const int r0 = (int)(r[0] % (unsigned)ncorr), r1 = (int)(r[1] % (unsigned)ncorr), r2 = (int)(r[2] % (unsigned)ncorr);
+  const int lane = (int)lane_id();
+  unsigned* __restrict__ q0 = sq[threadIdx.x >> 5][0];
+  unsigned* __restrict__ q1 = sq[threadIdx.x >> 5][1];
+  unsigned* __restrict__ q2 = sq[threadIdx.x >> 5][2];
+  auto finish = [&](int e) {  // sides 1 and 2 of a queued trial
+    const int r0 = (int)q0[e], r1 = (int)q1[e], r2 = (int)qb_fastmod(q2[e], magic, nc);
     const float4 a0 = point(0, r0), a1 = point(0, r1), a2 = point(0, r2);
     const float4 b0 = point(1, r0), b1 = point(1, r1), b2 = point(1, r2);
-    const float li0 = tri_side(a0, a1, mi), li1 = tri_side(a1, a2, mi), li2 = tri_side(a2, a0, mi);
-    const float lj0 = tri_side(b0, b1, mj), lj1 = tri_side(b1, b2, mj), lj2 = tri_side(b2, b0, mj);
-    if ((li0 * scale < lj0) && (lj0 < li0 / scale) && (li1 * scale < lj1) && (lj1 < li1 / scale) && (li2 * scale < lj2) &&
-        (lj2 < li2 / scale)) {
+    const float li1 = tri_side(a1, a2, mi), li2 = tri_side(a2, a0, mi);
+    const float lj1 = tri_side(b1, b2, mj), lj2 = tri_side(b2, b0, mj);
+    if ((li1 * scale < lj1) && (lj1 < li1 / scale) && (li2 * scale < lj2) && (lj2 < li2 / scale)) {
       mk[r0] = 1; mk[r1] = 1; mk[r2] = 1;
     }
+  };
+  int queued = 0;  // warp-uniform
+  for (long long t0 = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); t0 < trials; t0 += (long long)gridDim.x * blockDim.x) {
+    const long long t = t0 + lane;
+    bool pass = false;
+    unsigned r[4] = {0u, 0u, 0u, 0u};
+    if (t < trials) {
+      philox4x32_10(seed, (unsigned long long)t, r);
+      r[0] = qb_fastmod(r[0], magic, nc);
+      r[1] = qb_fastmod(r[1], magic, nc);
+      const float li0 = tri_side(point(0, (int)r[0]), point(0, (int)r[1]), mi);
+      const float lj0 = tri_side(point(1, (int)r[0]), point(1, (int)r[1]), mj);
+      pass = (li0 * scale < lj0) && (lj0 < li0 / scale);
+    }
+    const unsigned ballot = __ballot_sync(0xffffffffu, pass);
+    if (pass) {
+      const int e = queued + __popc(ballot & ((1u << lane) - 1u));
+      q0[e] = r[0]; q1[e] = r[1]; q2[e] = r[2];
+    }
+    queued += __popc(ballot);
+    __syncwarp();
+    if (queued >= 32) {
+      queued -= 32;
+      finish(queued + lane);
+      __syncwarp();  // the next pushes overwrite these entries
+    }
   }
+  if (lane < queued) finish(lane);
 }
 
 // survivors -> partner[src] = tgt  (mutual NN is a bijection, so sorting by (src,tgt) = sorting by src)
@@ -448,8 +491,9 @@ int launch_match(Lane* h, int n_pairs) {
   for (int s = 0; s < n_pairs; ++s) any_tuple |= h->h_solve[s].use_tuple != 0;
   if (any_tuple) {
     cloud_mean_kernel<<<2 * n_pairs, 32, 0, h->stream>>>(h->vox_pts, h->ctr.n_vox, V, h->d_solve, h->mean);
+    QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)tuple_test_kernel, kTupleSmem));
     const dim3 gt(kTupleCtasPerPair, n_pairs);
-    tuple_test_kernel<<<gt, kTupleThreads, 0, h->stream>>>(h->vox_pts, V, h->mut_i, h->mut_j, h->ctr.n_mutual, h->ctr.swapped, h->mean, h->d_solve,
+    tuple_test_kernel<<<gt, kTupleThreads, kTupleSmem, h->stream>>>(h->vox_pts, V, h->mut_i, h->mut_j, h->ctr.n_mutual, h->ctr.swapped, h->mean, h->d_solve,
                                                            h->mark);
     h->launches += 2;
   }

@@ -111,3 +111,16 @@ QB_HD_FN void qb_sincosf(float x, float* s, float* c) {
   pc = pc * z + 4.166657478e-02f;
   *c = (1.0f - 0.5f * z) + (z * z) * pc;
 }
+
+// r % d for every 32-bit r and 1 <= d < 2^32 without a division: m = ceil(2^64 / d) (qb_fastmod_magic; d = 1 wraps to 0, which
+// gives 0), then r % d = ((m * r mod 2^64) * d) >> 64 (Lemire, Kaser & Kurz, "Faster remainder by direct computation", 2019,
+// Theorem 1: exact for N-bit r and d whenever the fraction has 2N bits).  tests/test_tuple_lazy.py checks it against % on the host.
+QB_HD_FN uint64_t qb_fastmod_magic(uint32_t d) { return UINT64_MAX / d + 1u; }
+QB_HD_FN uint32_t qb_fastmod(uint32_t r, uint64_t m, uint32_t d) {
+  const uint64_t low = m * r;
+#ifdef __CUDA_ARCH__
+  return (uint32_t)__umul64hi(low, (uint64_t)d);
+#else
+  return (uint32_t)(((unsigned __int128)low * d) >> 64);
+#endif
+}
