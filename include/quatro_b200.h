@@ -365,7 +365,10 @@ int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_
  * earlier wave only when it needs that lane again), so the single-warp tail of one batch runs under the PCIe copies and front-end
  * kernels of the next; _flush waits for everything queued and completes the record arrays.  The scans (host kind) and `results` of
  * every queued batch must stay valid until a flush (or qb200_register_batch, = enqueue + flush) returns.  Other entry points flush
- * implicitly. */
+ * implicitly.  Raw, cached and correspondence-set batches (qb200_register_cached_enqueue_mixed, qb200_solve_batch_enqueue_each) may
+ * be queued in one stream and completed by a single flush.  The calls that write the scan cache (qb200_cache_reserve,
+ * qb200_cache_scans, _cache_scans_each, qb200_cache_copy) and qb200_cache_read flush first, so a queued cached batch registers the
+ * slot contents it was enqueued against, and the calls after it see the new ones. */
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                                  qb200_result* results);
 int qb200_register_batch_flush(qb200_handle* h);
@@ -383,7 +386,8 @@ int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const
  * host->device copies and solver tail overlap the other waves' dense kernels; QB200_LANES=n (1..8, default 4) in
  * the environment sets the lane count (1 = strictly one wave at a time).  Results never depend on the wave size
  * or the lane.  Every batch call (raw, cached or correspondence-set input, any form) goes through the same checks and the same
- * wave driver; cached pairs and correspondence sets run their waves on one lane.  A call with n = 0 pairs does no work and
+ * wave driver, and its waves rotate over the same lanes; only raw host scans cross PCIe on the shared copy stream and open a
+ * multi-wave batch with a quarter wave.  A call with n = 0 pairs does no work and
  * latches no rotation noise bound.  A kind other than QB200_MEM_HOST / QB200_MEM_DEVICE is QB200_ERR_BAD_ARG. */
 int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs,
                          const qb200_params* p, qb200_mem_kind kind, qb200_result* results);
@@ -468,6 +472,19 @@ int qb200_register_batch_enqueue_mixed(qb200_handle* h, const qb200_pair* pairs,
  * two slots (not that of entry 0) */
 int qb200_register_cached_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                 qb200_result* results, const qb200_pair_lists* lists);
+/* Pipelined forms of qb200_register_cached_mixed and qb200_solve_batch_each, completed by qb200_register_batch_flush like every
+ * enqueue (a loop-closure back end queues candidate batches as keyframes arrive).  A narrower form is one of these with the entry
+ * repeated and lists = NULL.
+ *   The argument checks are those of the blocking call and run before anything is queued: a rejected call queues and writes nothing,
+ *     and the batches already queued still complete on the flush.
+ *   The params array and the list descriptor are copied by the call; the slot pairs, host-kind correspondence sets, `results` and
+ *     the list arrays must stay valid until the flush returns.
+ *   Entries with rot_noise_bound == 0 latch in enqueue order, as in the raw enqueue forms.
+ *   Records and lists are byte-identical to those of the blocking call. */
+int qb200_register_cached_enqueue_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                        qb200_result* results, const qb200_pair_lists* lists);
+int qb200_solve_batch_enqueue_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params,
+                                   qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
 /* qb200_cache_scans with one params entry per scan: scan i is voxelized and described with params[i] and slot_ids[i] records that
  * entry's front-end signature (qb200_cache_copy carries it).  Slot s's voxels, normals and descriptors (qb200_cache_read) are
  * byte-identical to qb200_cache_scans of that scan alone with its entry.  A bad entry fails the call with QB200_ERR_BAD_ARG before

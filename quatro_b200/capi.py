@@ -237,6 +237,8 @@ _SIGNATURES = {
     "qb200_register_batch_enqueue_mixed": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_register_cached_mixed": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
     "qb200_cache_scans_each": (i32, [vp, P(vp), P(i32), P(i32), i32, P(Params), i32]),
+    "qb200_register_cached_enqueue_mixed": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
+    "qb200_solve_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -715,6 +717,19 @@ class Handle:
         sp = _slot_array(slot_pairs)
         assert len(params) == len(sp)
         return self._batch_lists("qb200_register_cached_mixed", len(sp), (_ptr(sp), len(sp), self.params_array(params)), buffers)
+
+    def register_cached_enqueue_mixed_raw(self, slot_array, n: int, params_array, out: np.ndarray, buffers: Optional[ListBuffers] = None):
+        """qb200_register_cached_enqueue_mixed: params_array (params_array()) is copied by the call; slot_array (_slot_array()), `out`
+        and the buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_register_cached_enqueue_mixed(self.h, _ptr(slot_array), n, params_array, _ptr(out),
+                                                                        self._lists_arg(buffers)), "qb200_register_cached_enqueue_mixed")
+
+    def solve_batch_enqueue_each_raw(self, set_array, n: int, params_array, kind: int, out: np.ndarray,
+                                     buffers: Optional[ListBuffers] = None):
+        """qb200_solve_batch_enqueue_each: params_array (params_array()) is copied by the call; set_array (_set_array()), its points
+        (host kind), `out` and the buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_solve_batch_enqueue_each(self.h, set_array, n, params_array, kind, _ptr(out),
+                                                                   self._lists_arg(buffers)), "qb200_solve_batch_enqueue_each")
 
     def last_features(self, which: int, cap: Optional[int] = None):
         """(normals (n,4), descriptors (n,33)) of the source (0) / target (1) cloud of the last match_and_pack."""

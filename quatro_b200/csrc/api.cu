@@ -95,6 +95,8 @@ int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   QB_CUDA_TRY(L, L->h_cloud_n.alloc(C));
   QB_CUDA_TRY(L, L->h_raw_off.alloc(C + 1));
   QB_CUDA_TRY(L, L->raw_stage.alloc(C * R));
+  QB_CUDA_TRY(L, L->d_slot_of_cloud.alloc(C));
+  QB_CUDA_TRY(L, L->h_slot_of_cloud.alloc(C));
   // the sort workspace serves the voxel sort (C*R items, digit histograms in val_a, chunk counts C*kVsChunks <= n_sort in val_b),
   // the lattice / norm sorts (C*V items) and, afterwards, the duplicate-class tables of K6 (2S*V + 2S words in key_a): size it for
   // the largest user
@@ -336,11 +338,11 @@ namespace {
 // 111-118); a loop-closure sweep matches one scan against many.  The cache keeps voxel points, normals and FPFH-33 of a scan
 // resident on the device so that the front end (voxel + normals + FPFH, ~45 % of a wave) runs once per SCAN, not once per pair.
 
-// clouds [0, n_clouds) of lane L's wave to (to_cache = 1) or from their cache slots h->h_slot_of_cloud[]
+// clouds [0, n_clouds) of lane L's wave to (to_cache = 1) or from their cache slots L->h_slot_of_cloud[]
 int cache_copy(qb200_handle* h, Lane* L, int to_cache, int n_clouds) {
-  QB_CUDA_TRY(L, cudaMemcpyAsync(h->d_slot_of_cloud, h->h_slot_of_cloud, (size_t)n_clouds * sizeof(int), cudaMemcpyHostToDevice, L->stream));
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_slot_of_cloud, L->h_slot_of_cloud, (size_t)n_clouds * sizeof(int), cudaMemcpyHostToDevice, L->stream));
   const dim3 g((L->V + 255) / 256, 43, n_clouds);
-  cache_copy_kernel<<<g, 256, 0, L->stream>>>(to_cache, h->d_slot_of_cloud, L->V, L->vox_pts, L->normals, L->desc_t, L->ctr.n_vox, L->ctr.cloud_status,
+  cache_copy_kernel<<<g, 256, 0, L->stream>>>(to_cache, L->d_slot_of_cloud, L->V, L->vox_pts, L->normals, L->desc_t, L->ctr.n_vox, L->ctr.cloud_status,
                                               h->c_vox, h->c_nrm, h->c_desc, h->c_n, h->c_status);
   L->launches++;
   QB_CUDA_TRY(L, cudaGetLastError());
@@ -476,8 +478,8 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     cudaEventRecord(L->ev[3], L->stream);
   } else if (in.slots) {
     for (int s = 0; s < np; ++s) {
-      h->h_slot_of_cloud[2 * s] = in.slots[w0 + s].src_slot;
-      h->h_slot_of_cloud[2 * s + 1] = in.slots[w0 + s].tgt_slot;
+      L->h_slot_of_cloud[2 * s] = in.slots[w0 + s].src_slot;
+      L->h_slot_of_cloud[2 * s + 1] = in.slots[w0 + s].tgt_slot;
     }
     if ((rc = wave_reset(L, ncl))) return rc;
     cudaEventRecord(L->ev[2], L->stream);
@@ -654,15 +656,14 @@ int check_call(qb200_handle* h, const BatchCall& c) {
   return QB200_OK;
 }
 
-// Check a batch call and queue it: its waves rotate over lanes, and a lane is collected (its records copied out) only when it is
-// needed again, so the tail of one batch runs under the copies and front-end kernels of the next.  Raw scans rotate over up to
-// h->max_lanes lanes.  Cached pairs and sets run on lane 0 alone, after the raw batches still queued are flushed: the slot table
-// h_slot_of_cloud is the handle's, and one lane keeps their schedule.  The caller's scans (host kind) and `results` must stay valid
-// until batch_flush (in qb200_register_batch_flush or the next call that is not an enqueue) has returned them.
+// Check a batch call and queue it: its waves rotate over up to h->max_lanes lanes whatever its input, and a lane is collected (its
+// records copied out) only when it is needed again, so the tail of one batch runs under the copies and front-end kernels of the
+// next.  Each lane has its own slot table, and waves only read the scan cache; the calls that write the cache flush first (enter).
+// The caller's input arrays (host kind), `results` and lists must stay valid until batch_flush (in qb200_register_batch_flush or
+// the next call that is not an enqueue) has returned them.
 int enqueue_call(qb200_handle* h, BatchCall c) {
   if (!h) return QB200_ERR_BAD_ARG;
   int rc;
-  if (!c.pairs && (rc = enter(h))) return rc;
   if ((rc = check_call(h, c))) return rc;
   cudaSetDevice(h->cfg.device);
   const bool pipelined = h->lanes_active > 0;  // waves of an earlier enqueue are still in flight
@@ -673,16 +674,18 @@ int enqueue_call(qb200_handle* h, BatchCall c) {
   const std::unique_ptr<qb200_params[]> pr = resolve_call(h, c.caller, c.n, c.each);
   if (!pr) return QB200_ERR_CUDA;
   c.params = pr.get();
-  const int S = h->cfg.max_batch_slots, lanes = c.pairs ? h->max_lanes : 1;
+  const int S = h->cfg.max_batch_slots, lanes = h->max_lanes;
+  // raw host scans cross PCIe: the copy stream and the quarter-wave opening below are theirs alone
+  const bool host_scans = c.pairs && c.kind == QB200_MEM_HOST;
   // More than one wave: rotate over the lanes so that one wave's PCIe copies and single-warp solver tail run under the
   // other waves' dense kernels.  Results do not depend on the lane (no state is shared between waves).
-  // Wave plan.  Host inputs: nothing can run before the first wave's scans crossed PCIe, so the batch opens with a quarter
+  // Wave plan.  Host scans: nothing can run before the first wave's scans crossed PCIe, so the batch opens with a quarter
   // wave (its copy is the only one that is not hidden) followed by the remaining three quarters; all other waves are full.
   // (Closing with small waves as well does not pay: every wave carries the same single-warp solver tail.)
   int wave_n[64], n_waves = 0;
   {
     int left = c.n;
-    if (c.kind == QB200_MEM_HOST && c.n > S && S >= 8 && lanes > 1) {
+    if (host_scans && c.n > S && S >= 8 && lanes > 1) {
       wave_n[n_waves++] = S / 4;
       wave_n[n_waves++] = S - S / 4;
       left -= S;
@@ -715,7 +718,7 @@ int enqueue_call(qb200_handle* h, BatchCall c) {
     }
   }
   // host scans of a multi-wave batch: one copy stream, ordered after whatever the caller queued on lane 0's stream
-  if (c.kind == QB200_MEM_HOST && n_lanes > 1) {
+  if (host_scans && n_lanes > 1) {
     c.copy_stream = h->copy_stream;
     if (fresh) QB_CUDA_TRY(h, cudaStreamWaitEvent(c.copy_stream, h->ev_fork, 0));
   }
@@ -765,7 +768,7 @@ int cache_scans(qb200_handle* h, const float* const* scans4, const int32_t* n_po
       L->h_cloud_ptr[c] = reinterpret_cast<const float4*>(scans4[c0 + c]);
       L->h_cloud_n[c] = n_points[c0 + c];
       L->h_front[c] = front_entry(pc);
-      h->h_slot_of_cloud[c] = slot_ids[c0 + c];
+      L->h_slot_of_cloud[c] = slot_ids[c0 + c];
       float* sig = h->c_sig.get() + 4 * (size_t)slot_ids[c0 + c];
       sig[0] = pc.voxel_size; sig[1] = pc.normal_radius; sig[2] = pc.fpfh_radius; sig[3] = lattice_cell(pc);
     }
@@ -890,6 +893,11 @@ int qb200_solve_batch_each(qb200_handle* h, const qb200_corr_set* sets, int32_t 
   return run_call(h, {nullptr, nullptr, sets, n_sets, kind, params, true, results, lists});
 }
 
+int qb200_solve_batch_enqueue_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params,
+                                   qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_call(h, {nullptr, nullptr, sets, n_sets, kind, params, true, results, lists});
+}
+
 // ---- raw scans -> pose ------------------------------------------------------------------------------
 int qb200_register_batch_flush(qb200_handle* h) { return enter(h); }
 
@@ -956,8 +964,7 @@ int qb200_cache_reserve(qb200_handle* h, int32_t n_slots) {
   QB_CUDA_TRY(h, cudaStreamSynchronize(h->lane[0]->stream));
   // the old cache goes first, so the device never holds two
   h->c_slots = 0;
-  h->c_vox.reset(); h->c_nrm.reset(); h->c_desc.reset(); h->c_n.reset(); h->c_status.reset();
-  h->d_slot_of_cloud.reset(); h->h_slot_of_cloud.reset(); h->c_sig.reset();
+  h->c_vox.reset(); h->c_nrm.reset(); h->c_desc.reset(); h->c_n.reset(); h->c_status.reset(); h->c_sig.reset();
   if (n_slots == 0) return QB200_OK;
   const size_t V = h->cfg.max_voxel_points, N = (size_t)n_slots;
   QB_CUDA_TRY(h, h->c_vox.alloc(N * V));
@@ -965,8 +972,6 @@ int qb200_cache_reserve(qb200_handle* h, int32_t n_slots) {
   QB_CUDA_TRY(h, h->c_desc.alloc(N * kDescK * V));
   QB_CUDA_TRY(h, h->c_n.alloc(N));
   QB_CUDA_TRY(h, h->c_status.alloc(N));
-  QB_CUDA_TRY(h, h->d_slot_of_cloud.alloc(2 * (size_t)h->cfg.max_batch_slots));
-  QB_CUDA_TRY(h, h->h_slot_of_cloud.alloc(2 * (size_t)h->cfg.max_batch_slots));
   QB_CUDA_TRY(h, cudaMemset(h->c_n, 0, N * sizeof(int)));
   QB_CUDA_TRY(h, cudaMemset(h->c_status, 0, N * sizeof(int)));
   QB_CUDA_TRY(h, cudaMemset(h->c_desc, 0, N * kDescK * V * sizeof(float)));
@@ -1003,6 +1008,11 @@ int qb200_register_cached_each(qb200_handle* h, const qb200_slot_pair* pairs, in
 int qb200_register_cached_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                 qb200_result* results, const qb200_pair_lists* lists) {
   return run_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists, true});
+}
+
+int qb200_register_cached_enqueue_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                        qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists, true});
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

@@ -75,6 +75,7 @@ struct Lane {
   DeviceMem<int> d_raw_off;   // [2S+1] offsets into the concatenated sort arrays
   PinnedMem<const float4*> h_cloud_ptr; PinnedMem<int> h_cloud_n, h_raw_off;  // pinned mirrors
   DeviceMem<float4> raw_stage; // [2S*R] staging for host inputs
+  DeviceMem<int> d_slot_of_cloud; PinnedMem<int> h_slot_of_cloud;  // [2S] cache slot of every cloud of the wave, and its pinned mirror
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
   int pend_t0, pend_t1;       // ... the stage-time slots [t0, t1) it records
   qb200_result* pend_dst;     // ... and the caller's record array of its batch
@@ -173,13 +174,12 @@ struct qb200_handle {
   qb::Stream copy_stream;     // host scans of a multi-wave batch cross PCIe on ONE stream, wave after wave (api.cu: wave_submit)
   qb::Event ev_copied;        // a wave's scans have arrived (recorded on the copy stream)
 
-  // ---- scan cache (qb200_cache_*): front-end results of whole scans, resident on the device ----
+  // ---- scan cache (qb200_cache_*): front-end results of whole scans, resident on the device.  Waves of every lane read it (each
+  // through its lane's slot table); only calls that flush first write it ----
   int c_slots;
   qb::DeviceMem<float4> c_vox, c_nrm;  // [slots*V]
   qb::DeviceMem<float> c_desc;         // [slots*40*V] dimension-major like desc_t
   qb::DeviceMem<int> c_n, c_status;    // [slots]
-  qb::DeviceMem<int> d_slot_of_cloud;  // [2S] cache slot of every cloud of the current wave
-  qb::PinnedMem<int> h_slot_of_cloud;  // [2S] its pinned mirror
   std::unique_ptr<float[]> c_sig;      // host [slots*4]: (voxel, normal_r, fpfh_r, cell) a slot was computed with
 
   // ---- multi-GPU gather of the result records (comm.cu) ----
