@@ -365,10 +365,10 @@ int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_
  * earlier wave only when it needs that lane again), so the single-warp tail of one batch runs under the PCIe copies and front-end
  * kernels of the next; _flush waits for everything queued and completes the record arrays.  The scans (host kind) and `results` of
  * every queued batch must stay valid until a flush (or qb200_register_batch, = enqueue + flush) returns.  Other entry points flush
- * implicitly.  Raw, cached and correspondence-set batches (qb200_register_cached_enqueue_mixed, qb200_solve_batch_enqueue_each) may
- * be queued in one stream and completed by a single flush.  The calls that write the scan cache (qb200_cache_reserve,
- * qb200_cache_scans, _cache_scans_each, qb200_cache_copy) and qb200_cache_read flush first, so a queued cached batch registers the
- * slot contents it was enqueued against, and the calls after it see the new ones. */
+ * implicitly.  Raw, cached and correspondence-set batches (qb200_register_cached_enqueue_mixed, qb200_solve_batch_enqueue_each) and
+ * scan-cache writes (qb200_cache_scans_enqueue_each) may be queued in one stream and completed by a single flush; every access to a
+ * cache slot follows enqueue order, so a queued cached batch registers the slot contents it was enqueued against.  qb200_cache_reserve,
+ * qb200_cache_copy, qb200_cache_read and the pre-processing calls flush first, so they see every write queued before them. */
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                                  qb200_result* results);
 int qb200_register_batch_flush(qb200_handle* h);
@@ -406,7 +406,8 @@ int qb200_register_batch_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_
 typedef struct qb200_slot_pair { int32_t src_slot, tgt_slot; } qb200_slot_pair;
 int qb200_cache_reserve(qb200_handle* h, int32_t n_slots);   /* (re)allocates; 0 frees.  192 B per voxel point and slot: ~3.1 MB at
                                                                  max_voxel_points = 16384, ~50 MB at 262144 */
-/* voxelize + normals + FPFH of n_scans raw scans (scans4[i]: n_points[i] x {x,y,z,w}) into slots slot_ids[i] */
+/* voxelize + normals + FPFH of n_scans raw scans (scans4[i]: n_points[i] x {x,y,z,w}) into slots slot_ids[i] (a slot named twice
+ * ends with the last scan that names it); = qb200_cache_scans_enqueue_each with p repeated + qb200_register_batch_flush */
 int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
                       const qb200_params* p, qb200_mem_kind kind);
 /* match + graph + clique + pose for pairs of cached scans (= qb200_register_batch without its front end); p's front-end parameters
@@ -491,6 +492,21 @@ int qb200_solve_batch_enqueue_each(qb200_handle* h, const qb200_corr_set* sets, 
  * any slot is written, and qb200_last_error names it. */
 int qb200_cache_scans_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
                            const qb200_params* params, qb200_mem_kind kind);
+/* qb200_cache_scans_each, queued: completed by qb200_register_batch_flush like every enqueue (a SLAM back end caches each keyframe and
+ * queues its candidate batches without draining the stream).  A narrower form is this call with the entry repeated.
+ *   The argument checks are those of qb200_cache_scans_each and run before anything is queued: a rejected call queues nothing, writes
+ *     no slot and no slot signature, names the bad entry or scan in qb200_last_error, and the batches already queued still complete
+ *     on the flush.
+ *   Order: every access to a slot follows enqueue order.  A cached batch enqueued before the write registers the slot's old contents,
+ *     one enqueued after it the new ones; two queued writes to one slot land in enqueue order; a slot named twice in one call ends
+ *     with the last scan that names it, as in the blocking call.
+ *   Each written slot's front-end signature is recorded when the call is queued, so a cached batch enqueued after it is checked
+ *     against the new signature.
+ *   The scans4, n_points, slot_ids and params arrays are read by the call; host-kind scans must stay valid until the flush returns.
+ *   Slot contents (qb200_cache_read), and everything registered from them, are byte-identical to the blocking calls made in the
+ *     same order. */
+int qb200_cache_scans_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids,
+                                   int32_t n_scans, const qb200_params* params, qb200_mem_kind kind);
 /* read a cached scan back: voxel points (n x 4), normals (n x {nx,ny,nz,curvature}), descriptors (n x 33); any may be NULL */
 int qb200_cache_read(qb200_handle* h, int32_t slot, float* vox4, float* normals4, float* desc33, int32_t cap, int32_t* n);
 
@@ -537,12 +553,14 @@ int qb200_get_last_correspondences(qb200_handle* h, int32_t* corr, float* src_ma
 int qb200_get_last_features(qb200_handle* h, int32_t which, float* normals4, float* desc33, int32_t cap, int32_t* n);
 
 /* Per-stage device time of the last batch call in milliseconds (CUDA events); the single-pair registration and solve are batches
- * of one: [0]=h2d [1]=voxel [2]=fpfh [3]=match [4]=graph [5]=clique [6]=pose [7]=d2h; n<=8. */
+ * of one: [0]=h2d [1]=voxel [2]=fpfh [3]=match [4]=graph [5]=clique [6]=pose [7]=d2h; n<=8.  The times start from zero with every
+ * call that finds nothing queued, and qb200_cache_scans{,_each} count as batch calls that register nothing: right after one of them
+ * (or after a flush of queued cache writes alone) this and qb200_get_kernel_ms report zeros, not the previous batch's times. */
 int qb200_get_stage_ms(qb200_handle* h, float* ms, int32_t n);
 
 /* Device time (CUDA events on the handle's stream) and launch count of the two roofline kernels
  * during the last batch call: [0] = the tensor-core nearest-neighbour passes (tc_match_kernel x3),
- * [1] = tim_graph_kernel (TIM consistency graph); n <= 2. */
+ * [1] = tim_graph_kernel (TIM consistency graph); n <= 2.  Zeros after a cache write, as qb200_get_stage_ms. */
 int qb200_get_kernel_ms(qb200_handle* h, float* ms, int32_t* launches, int32_t n);
 
 /* Diagnostics: the tensor-core (wgmma, 3xTF32) approximate squared distances that pre-filter the 33-D

@@ -239,6 +239,7 @@ _SIGNATURES = {
     "qb200_cache_scans_each": (i32, [vp, P(vp), P(i32), P(i32), i32, P(Params), i32]),
     "qb200_register_cached_enqueue_mixed": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
     "qb200_solve_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_cache_scans_enqueue_each": (i32, [vp, P(vp), P(i32), P(i32), i32, P(Params), i32]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -730,6 +731,12 @@ class Handle:
         (host kind), `out` and the buffers must stay alive until register_batch_flush."""
         return self._check(self.lib.qb200_solve_batch_enqueue_each(self.h, set_array, n, params_array, kind, _ptr(out),
                                                                    self._lists_arg(buffers)), "qb200_solve_batch_enqueue_each")
+
+    def cache_scans_enqueue_each_raw(self, scan_ptrs, counts, slot_ids, n: int, params_array, kind: int):
+        """qb200_cache_scans_enqueue_each: scan_ptrs / counts (_scan_arrays()), slot_ids (c_int32 * n) and params_array
+        (params_array()) are read by the call; host-kind scans must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_cache_scans_enqueue_each(self.h, scan_ptrs, counts, slot_ids, n, params_array, kind),
+                           "qb200_cache_scans_enqueue_each")
 
     def last_features(self, which: int, cap: Optional[int] = None):
         """(normals (n,4), descriptors (n,33)) of the source (0) / target (1) cloud of the last match_and_pack."""

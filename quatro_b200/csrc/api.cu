@@ -5,9 +5,11 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <map>
 #include <mutex>
 #include <utility>
+#include <vector>
 
 #include "handle.cuh"
 
@@ -170,6 +172,8 @@ int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   carve_counters(L->hctr_block, S, &L->hctr);
   for (Event& e : L->ev) QB_CUDA_TRY(L, e.create());
   for (Event& e : L->kev) QB_CUDA_TRY(L, e.create());
+  QB_CUDA_TRY(L, L->ev_cache_in.create(cudaEventDisableTiming));
+  QB_CUDA_TRY(L, L->ev_cache_out.create(cudaEventDisableTiming));
   QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
   *out = std::move(L);
   return QB200_OK;
@@ -349,9 +353,41 @@ int cache_copy(qb200_handle* h, Lane* L, int to_cache, int n_clouds) {
   return QB200_OK;
 }
 
+bool share_a_slot(const std::vector<int>& a, const std::vector<int>& b) {
+  for (size_t i = 0, j = 0; i < a.size() && j < b.size();) {
+    if (a[i] == b[j]) return true;
+    if (a[i] < b[j]) ++i; else ++j;
+  }
+  return false;
+}
+
+// The slots of the wave about to copy clouds [0, ncl) of lane L to (write) or from its slot table L->h_slot_of_cloud go to
+// L->pend_slots, and L's stream waits for the conflicting cache copies of the waves in flight on the other lanes: a write for their
+// copy-ins and copy-outs of its slots (WAR, WAW), a read for their copy-outs (RAW).  Every wave that was enqueued earlier has been
+// collected or is the one wave in flight on its lane, and a lane's waves run in order, so these device-side waits put every access to
+// a slot in enqueue order.  A write names a slot more than once only when scans of one call do: the last one wins, as it would in a
+// later wave, and the others are not copied.
+int cache_waits(qb200_handle* h, Lane* L, int ncl, bool write) {
+  std::vector<std::pair<int, int>> by_slot(ncl);
+  for (int c = 0; c < ncl; ++c) by_slot[c] = std::make_pair(L->h_slot_of_cloud[c], c);
+  std::sort(by_slot.begin(), by_slot.end());
+  L->pend_slots.clear();
+  L->pend_writes = write;
+  for (int i = 0; i < ncl; ++i) {
+    if (i + 1 == ncl || by_slot[i + 1].first != by_slot[i].first) L->pend_slots.push_back(by_slot[i].first);
+    else if (write) L->h_slot_of_cloud[by_slot[i].second] = -1;
+  }
+  for (const std::unique_ptr<Lane>& Y : h->lane) {
+    if (!Y || Y.get() == L || Y->pend_np == 0 || !(write || Y->pend_writes) || !share_a_slot(L->pend_slots, Y->pend_slots)) continue;
+    QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, Y->pend_writes ? Y->ev_cache_out : Y->ev_cache_in, 0));
+  }
+  return QB200_OK;
+}
+
 // ---- batch calls ----------------------------------------------------------------------------------------------------------
-// One batch call as its entry point received it.  Its input is n pairs of raw scans (in `kind` memory), n pairs of cached scans, or
-// n correspondence sets (in `kind` memory): exactly one of the three is set.  The entry points fill the fields up to `lists` in order.
+// One batch call as its entry point received it.  Its input is n pairs of raw scans (in `kind` memory), n pairs of cached scans,
+// n correspondence sets (in `kind` memory), or n raw scans to cache (cache_write): exactly one of the four is set.  The registering
+// entry points fill the fields up to `lists` in order.
 struct BatchCall {
   const qb200_pair* pairs = nullptr;
   const qb200_slot_pair* slots = nullptr;
@@ -366,6 +402,10 @@ struct BatchCall {
   const qb200_pair_lists* lists = nullptr;
   // (each) the entries may differ in their front-end fields too (the _mixed forms); otherwise those are bit-identical in every entry
   bool mixed = false;
+  // a cache write: scan i (n_points[i] points in `kind` memory) is voxelized and described with its entry into slot slot_ids[i]
+  const float* const* scans = nullptr;
+  const int32_t* n_points = nullptr;
+  const int32_t* slot_ids = nullptr;
   // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved, laid out like `caller`.
   const qb200_params* params = nullptr;
   // raw host scans of a multi-wave batch: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies queued on
@@ -440,25 +480,39 @@ int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
 
 // Enqueue one wave (pairs [w0, w0 + np), np <= S) on lane L: the front of the wave its input needs (raw scans: H2D, K1..K6;
 // cached scans: the copy out of the cache, K6; correspondence sets: their H2D), then K8..K11 and the D2H of the result records.
+// A cache write's wave is scans [w0, w0 + np), np <= 2S: their H2D, K1..K5 and the copy into their slots, with no records.
 // No sync: wave_collect hands the records out to in.results[w0...].  The lane's previous wave must have been collected.
 int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
-  const int ncl = 2 * np;
+  const bool raw = in.pairs || in.scans;
+  const int ncl = in.scans ? np : 2 * np;
   int rc;
   L->kev_armed[0] = L->kev_armed[1] = 0;
+  L->pend_slots.clear();
+  L->pend_writes = 0;
   // the wave's tables (the lane's previous wave has been collected: their pinned mirrors are free), copied before anything else of the
   // wave: on a stream of host batches the copy engine carries the scans, and a copy queued ahead of this wave's scans only waits for
   // the earlier waves' scans, which the lane waits for anyway.  A pair's entry and both of its clouds' come from its own params.
   for (int s = 0; s < np; ++s) {
     const bool own = in.each || s == 0;
     const qb200_params& p = in.params[in.each ? w0 + s : 0];
+    if (in.scans) {
+      L->h_front[s] = own ? front_entry(p) : L->h_front[0];
+      continue;
+    }
     L->h_solve[s] = own ? solve_entry(p) : L->h_solve[0];
     if (in.pairs) L->h_front[2 * s] = L->h_front[2 * s + 1] = own ? front_entry(p) : L->h_front[0];
   }
-  if ((rc = upload_solve(L, np))) return rc;
-  if (in.pairs && (rc = upload_front(L, ncl))) return rc;
-  if (in.pairs) {
+  if (!in.scans && (rc = upload_solve(L, np))) return rc;
+  if (raw && (rc = upload_front(L, ncl))) return rc;
+  if (raw) {
     cudaEventRecord(L->ev[0], L->stream);
     for (int s = 0; s < np; ++s) {
+      if (in.scans) {
+        L->h_cloud_ptr[s] = reinterpret_cast<const float4*>(in.scans[w0 + s]);
+        L->h_cloud_n[s] = in.n_points[w0 + s];
+        L->h_slot_of_cloud[s] = in.slot_ids[w0 + s];
+        continue;
+      }
       const qb200_pair& pr = in.pairs[w0 + s];
       L->h_cloud_ptr[2 * s] = reinterpret_cast<const float4*>(pr.src);
       L->h_cloud_ptr[2 * s + 1] = reinterpret_cast<const float4*>(pr.tgt);
@@ -482,8 +536,10 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       L->h_slot_of_cloud[2 * s + 1] = in.slots[w0 + s].tgt_slot;
     }
     if ((rc = wave_reset(L, ncl))) return rc;
+    if ((rc = cache_waits(h, L, ncl, false))) return rc;
     cudaEventRecord(L->ev[2], L->stream);
     if ((rc = cache_copy(h, L, 0, ncl))) return rc;
+    QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_in, L->stream));
     cudaEventRecord(L->ev[3], L->stream);
   } else {
     if ((rc = wave_reset(L, ncl))) return rc;
@@ -498,22 +554,29 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     }
     QB_CUDA_TRY(L, cudaMemcpyAsync(L->ctr.n_corr, L->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, L->stream));
   }
-  if (!in.sets && (rc = launch_match(L, np))) return rc;
-  cudaEventRecord(L->ev[4], L->stream);
-  cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
-  if ((rc = run_solver(L, np, in.sets ? 0 : 1))) return rc;
-  cudaEventRecord(L->ev[7], L->stream);
-  if (in.lists && (rc = submit_lists(L, *in.lists, w0, np))) return rc;
-  QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
-  cudaEventRecord(L->ev[8], L->stream);
+  if (in.scans) {
+    if ((rc = cache_waits(h, L, ncl, true))) return rc;
+    if ((rc = cache_copy(h, L, 1, ncl))) return rc;
+    QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_out, L->stream));
+  } else {
+    if (!in.sets && (rc = launch_match(L, np))) return rc;
+    cudaEventRecord(L->ev[4], L->stream);
+    cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
+    if ((rc = run_solver(L, np, in.sets ? 0 : 1))) return rc;
+    cudaEventRecord(L->ev[7], L->stream);
+    if (in.lists && (rc = submit_lists(L, *in.lists, w0, np))) return rc;
+    QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
+    cudaEventRecord(L->ev[8], L->stream);
+  }
   L->pend_w0 = w0;
   L->pend_np = np;
-  L->pend_dst = in.results;
+  L->pend_dst = in.results;  // nullptr for a cache write: no records
   if (in.lists) L->pend_lists = *in.lists;
   else L->pend_lists.cap_per_pair = 0;
-  // stage-time slots of qb200_get_stage_ms this wave reports: raw scans all eight, the other inputs their first stage to pose
-  L->pend_t0 = in.pairs ? 0 : in.slots ? 2 : 4;
-  L->pend_t1 = in.pairs ? 8 : 7;
+  // stage-time slots of qb200_get_stage_ms this wave reports: raw scans all eight, the other inputs their first stage to pose, a cache
+  // write none (it registers nothing)
+  L->pend_t0 = in.pairs ? 0 : in.slots ? 2 : in.sets ? 4 : 8;
+  L->pend_t1 = in.pairs || in.scans ? 8 : 7;
   return QB200_OK;
 }
 
@@ -526,7 +589,7 @@ int wave_collect(qb200_handle* h, Lane* L) {
     h->fail(__FILE__, __LINE__, cudaGetErrorString(cudaGetLastError()));
     return QB200_ERR_CUDA;
   }
-  memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
+  if (L->pend_dst) memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
   if (L->pend_lists.cap_per_pair > 0 && L->pend_lists.kind == QB200_MEM_HOST) deliver_lists(L, L->pend_lists, L->pend_w0, np);
   if (h->timeline && L->pend_t0 == 0) {  // stage boundaries of a raw-scan wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
     fprintf(stderr, "[qb200 timeline] wave w0=%d np=%d:", L->pend_w0, np);
@@ -607,7 +670,7 @@ std::unique_ptr<qb200_params[]> resolve_call(qb200_handle* h, const qb200_params
 }
 
 // Every argument check of a batch call, in one order whatever its input, so that a call with several faults returns the same code:
-// counts and arrays, the params entries, the cross-check, the lists, then every pair or set.  A rejection names its fault in
+// counts and arrays, the params entries, the cross-check, the lists, then every pair, set or scan.  A rejection names its fault in
 // qb200_last_error.
 int check_call(qb200_handle* h, const BatchCall& c) {
   auto reject = [h](const char* why) {
@@ -615,13 +678,14 @@ int check_call(qb200_handle* h, const BatchCall& c) {
     return QB200_ERR_BAD_ARG;
   };
   if (c.n < 0) return reject("n < 0");
-  if (c.n > 0 && !c.pairs && !c.slots && !c.sets) return reject("the input array is null");
-  if (c.n > 0 && !c.results) return reject("the results array is null");
+  if (c.n > 0 && !c.pairs && !c.slots && !c.sets && !c.scans) return reject("the input array is null");
+  if (c.n > 0 && c.scans && (!c.n_points || !c.slot_ids)) return reject("the n_points or slot_ids array is null");
+  if (c.n > 0 && !c.scans && !c.results) return reject("the results array is null");
   if (c.kind != QB200_MEM_HOST && c.kind != QB200_MEM_DEVICE) return reject("unknown memory kind of the inputs");
   const qb200_params* p = c.caller;
   char why[128];
   if (int rc = check_params(h, p, c.n, c.each, !c.sets && !c.mixed)) return rc;
-  for (int i = 0; !c.sets && i < (c.each ? c.n : 1); ++i) {
+  for (int i = 0; !c.sets && !c.scans && i < (c.each ? c.n : 1); ++i) {
     if (!p[i].use_crosscheck) {
       if (c.each) {
         snprintf(why, sizeof(why), "params entry %d: use_crosscheck = 0 is not supported", i);
@@ -648,9 +712,15 @@ int check_call(qb200_handle* h, const BatchCall& c) {
           return reject(why);
         }
       }
-    } else {
+    } else if (c.sets) {
       const qb200_corr_set& s = c.sets[i];
       if (s.L < 0 || s.L > h->cfg.max_corr || (s.L > 0 && (!s.a || !s.b))) return reject("correspondence set is null or exceeds max_corr");
+    } else {
+      const int sl = c.slot_ids[i], np = c.n_points[i];
+      if (sl < 0 || sl >= h->c_slots || np < 0 || np > R || (np > 0 && !c.scans[i])) {
+        snprintf(why, sizeof(why), "scan %d is null, exceeds max_raw_points or names a slot outside qb200_cache_reserve()", i);
+        return reject(why);
+      }
     }
   }
   return QB200_OK;
@@ -658,9 +728,9 @@ int check_call(qb200_handle* h, const BatchCall& c) {
 
 // Check a batch call and queue it: its waves rotate over up to h->max_lanes lanes whatever its input, and a lane is collected (its
 // records copied out) only when it is needed again, so the tail of one batch runs under the copies and front-end kernels of the
-// next.  Each lane has its own slot table, and waves only read the scan cache; the calls that write the cache flush first (enter).
-// The caller's input arrays (host kind), `results` and lists must stay valid until batch_flush (in qb200_register_batch_flush or
-// the next call that is not an enqueue) has returned them.
+// next.  Each lane has its own slot table; cache writes and cached pairs order their copies to and from the scan cache by
+// cache_waits, and qb200_cache_reserve / _copy / _read flush first (enter).  The caller's input arrays (host kind), `results` and
+// lists must stay valid until batch_flush (in qb200_register_batch_flush or the next call that is not an enqueue) has returned them.
 int enqueue_call(qb200_handle* h, BatchCall c) {
   if (!h) return QB200_ERR_BAD_ARG;
   int rc;
@@ -671,12 +741,14 @@ int enqueue_call(qb200_handle* h, BatchCall c) {
   // An empty call resolves no params: the reference latches the rotation noise bound inside computeTransformation, which an empty
   // batch never calls.
   if (c.n == 0) return QB200_OK;
-  const std::unique_ptr<qb200_params[]> pr = resolve_call(h, c.caller, c.n, c.each);
-  if (!pr) return QB200_ERR_CUDA;
-  c.params = pr.get();
-  const int S = h->cfg.max_batch_slots, lanes = h->max_lanes;
+  // a cache write resolves nothing: only the solver reads the rotation noise bound
+  std::unique_ptr<qb200_params[]> pr;
+  if (!c.scans && !(pr = resolve_call(h, c.caller, c.n, c.each))) return QB200_ERR_CUDA;
+  c.params = c.scans ? c.caller : pr.get();
+  // S: inputs per wave, pairs or (a cache write) scans; the clouds of a wave fill the lane's 2 * max_batch_slots cloud buffers
+  const int S = h->cfg.max_batch_slots * (c.scans ? 2 : 1), lanes = h->max_lanes;
   // raw host scans cross PCIe: the copy stream and the quarter-wave opening below are theirs alone
-  const bool host_scans = c.pairs && c.kind == QB200_MEM_HOST;
+  const bool host_scans = (c.pairs || c.scans) && c.kind == QB200_MEM_HOST;
   // More than one wave: rotate over the lanes so that one wave's PCIe copies and single-warp solver tail run under the
   // other waves' dense kernels.  Results do not depend on the lane (no state is shared between waves).
   // Wave plan.  Host scans: nothing can run before the first wave's scans crossed PCIe, so the batch opens with a quarter
@@ -723,6 +795,13 @@ int enqueue_call(qb200_handle* h, BatchCall c) {
     if (fresh) QB_CUDA_TRY(h, cudaStreamWaitEvent(c.copy_stream, h->ev_fork, 0));
   }
   h->lanes_active = n_lanes;
+  // a cache write's signatures, in scan order (a slot named twice ends with its last scan's): the checks of the calls queued after it
+  // see them
+  for (int i = 0; c.scans && i < c.n; ++i) {
+    const qb200_params& pc = c.params[c.each ? i : 0];
+    float* sig = h->c_sig.get() + 4 * (size_t)c.slot_ids[i];
+    sig[0] = pc.voxel_size; sig[1] = pc.normal_radius; sig[2] = pc.fpfh_radius; sig[3] = lattice_cell(pc);
+  }
   for (int w0 = 0, wave = 0; w0 < c.n && rc == QB200_OK; ++wave) {
     Lane* L = h->lane[h->lane_cursor].get();
     int np = planned ? wave_n[wave] : S;
@@ -741,46 +820,17 @@ int run_call(qb200_handle* h, const BatchCall& c) {
   int rc = enqueue_call(h, c);
   const int rc2 = h ? batch_flush(h) : QB200_OK;
   if (rc == QB200_OK) rc = rc2;
-  if (rc == QB200_OK && c.n == 1) set_last(h, c.results[0]);
+  if (rc == QB200_OK && c.n == 1 && c.results) set_last(h, c.results[0]);
   return rc;
 }
 
-// qb200_cache_scans (each = false: p is one entry for every scan) and qb200_cache_scans_each (p[i] for scan i): waves of up to 2S
-// scans on lane 0, each scan voxelized and described with its entry, and its slot records that entry's front-end signature
-int cache_scans(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
-                const qb200_params* p, bool each, qb200_mem_kind kind) {
-  if (int rc = enter(h)) return rc;
-  if (n_scans < 0 || (n_scans > 0 && (!scans4 || !n_points || !slot_ids))) return QB200_ERR_BAD_ARG;
-  if (!each && !params_ok(p)) return QB200_ERR_BAD_ARG;
-  if (each && n_scans > 0 && check_params(h, p, n_scans, true, false)) return QB200_ERR_BAD_ARG;
-  Lane* L = h->lane[0].get();
-  for (int i = 0; i < n_scans; ++i)
-    if (slot_ids[i] < 0 || slot_ids[i] >= h->c_slots || n_points[i] < 0 || n_points[i] > L->R || (n_points[i] > 0 && !scans4[i])) {
-      h->fail(__FILE__, __LINE__, "scan is null, exceeds max_raw_points or names a slot outside qb200_cache_reserve()");
-      return QB200_ERR_BAD_ARG;
-    }
-  const int C = 2 * L->S;
-  for (int c0 = 0; c0 < n_scans; c0 += C) {
-    const int nc = n_scans - c0 < C ? n_scans - c0 : C;
-    int rc;
-    for (int c = 0; c < nc; ++c) {
-      const qb200_params& pc = p[each ? c0 + c : 0];
-      L->h_cloud_ptr[c] = reinterpret_cast<const float4*>(scans4[c0 + c]);
-      L->h_cloud_n[c] = n_points[c0 + c];
-      L->h_front[c] = front_entry(pc);
-      L->h_slot_of_cloud[c] = slot_ids[c0 + c];
-      float* sig = h->c_sig.get() + 4 * (size_t)slot_ids[c0 + c];
-      sig[0] = pc.voxel_size; sig[1] = pc.normal_radius; sig[2] = pc.fpfh_radius; sig[3] = lattice_cell(pc);
-    }
-    if ((rc = upload_front(L, nc))) return rc;
-    if ((rc = stage_raw(L, nc, kind, L->stream))) return rc;
-    if ((rc = wave_reset(L, nc))) return rc;
-    if ((rc = launch_voxel(L, nc))) return rc;
-    if ((rc = launch_fpfh(L, nc))) return rc;
-    if ((rc = cache_copy(h, L, 1, nc))) return rc;
-    QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));  // the pinned tables are reused by the next wave
-  }
-  return QB200_OK;
+// qb200_cache_scans (each = false: p is one entry for every scan) and qb200_cache_scans_each (p[i] for scan i) as a batch call
+BatchCall cache_write(const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans, const qb200_params* p,
+                      bool each, qb200_mem_kind kind) {
+  BatchCall c;
+  c.n = n_scans; c.kind = kind; c.caller = p; c.each = each; c.mixed = true;
+  c.scans = scans4; c.n_points = n_points; c.slot_ids = slot_ids;
+  return c;
 }
 
 }  // namespace
@@ -983,12 +1033,17 @@ int qb200_cache_reserve(qb200_handle* h, int32_t n_slots) {
 
 int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
                       const qb200_params* p, qb200_mem_kind kind) {
-  return cache_scans(h, scans4, n_points, slot_ids, n_scans, p, false, kind);
+  return run_call(h, cache_write(scans4, n_points, slot_ids, n_scans, p, false, kind));
 }
 
 int qb200_cache_scans_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
                            const qb200_params* params, qb200_mem_kind kind) {
-  return cache_scans(h, scans4, n_points, slot_ids, n_scans, params, true, kind);
+  return run_call(h, cache_write(scans4, n_points, slot_ids, n_scans, params, true, kind));
+}
+
+int qb200_cache_scans_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids,
+                                   int32_t n_scans, const qb200_params* params, qb200_mem_kind kind) {
+  return enqueue_call(h, cache_write(scans4, n_points, slot_ids, n_scans, params, true, kind));
 }
 
 int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_result* results) {

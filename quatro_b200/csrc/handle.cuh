@@ -5,6 +5,7 @@
 #include <string.h>
 
 #include <memory>
+#include <vector>
 
 #include "common.cuh"
 #include "owners.cuh"
@@ -80,6 +81,12 @@ struct Lane {
   int pend_t0, pend_t1;       // ... the stage-time slots [t0, t1) it records
   qb200_result* pend_dst;     // ... and the caller's record array of its batch
   qb200_pair_lists pend_lists; // ... and a copy of its batch's list descriptor (cap_per_pair == 0: no lists)
+  // ... and the cache slots it reads (cached pairs) or writes (scans to cache), ascending and unique; empty: it does not touch the
+  // cache.  A wave reads the cache only in its copy-in and writes it only in its copy-out, so other lanes order their conflicting
+  // copies after those events (api.cu: cache_waits)
+  std::vector<int> pend_slots;
+  int pend_writes;
+  Event ev_cache_in, ev_cache_out;
 
   // ---- sort workspace (voxel sort, then lattice sort) ----
   DeviceMem<uint64_t> key_a, key_b;  // [2S*max(R,V)]
@@ -175,12 +182,13 @@ struct qb200_handle {
   qb::Event ev_copied;        // a wave's scans have arrived (recorded on the copy stream)
 
   // ---- scan cache (qb200_cache_*): front-end results of whole scans, resident on the device.  Waves of every lane read it (each
-  // through its lane's slot table); only calls that flush first write it ----
+  // through its lane's slot table), and cache-write waves write it; qb200_cache_reserve / _copy flush first ----
   int c_slots;
   qb::DeviceMem<float4> c_vox, c_nrm;  // [slots*V]
   qb::DeviceMem<float> c_desc;         // [slots*40*V] dimension-major like desc_t
   qb::DeviceMem<int> c_n, c_status;    // [slots]
-  std::unique_ptr<float[]> c_sig;      // host [slots*4]: (voxel, normal_r, fpfh_r, cell) a slot was computed with
+  std::unique_ptr<float[]> c_sig;      // host [slots*4]: (voxel, normal_r, fpfh_r, cell) a slot was computed with (set when the
+                                       // write is queued, so the checks of the calls after it see the new signature)
 
   // ---- multi-GPU gather of the result records (comm.cu) ----
   void* comm;                 // ncclComm_t
