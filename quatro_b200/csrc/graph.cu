@@ -16,7 +16,8 @@
 // (derivation in DESIGN.md 5.2).  Each lane evaluates its columns with scalar IEEE-rn operations (explicit
 // __fmaf_rn / __fadd_rn: no contraction decides the rounding).  Only pairs with |t_c| <= q -- a band of ~1e-4 relative width around the threshold --
 // or with both distances ~0 (the literal expression is NaN -> false for coincident duplicates) evaluate the literal fp64
-// expression, so the adjacency is bit-identical to the fp64 reference.
+// expression, and so does every test whose M exceeds 2^62 (the bound needs D^2, 2 beta^2 s' and q finite), so the adjacency is
+// bit-identical to the fp64 reference for any input.
 //
 // Work decomposition.  A WARP work item is 64 rows x 128 columns of the upper triangle (any pair of the launch: one global item
 // list); the warp stages its 64 row points in shared memory as (-2a, |a|^2 - beta^2/4 | -2b, |b|^2 - beta^2/4) -- read back as
@@ -215,7 +216,8 @@ __global__ void __launch_bounds__(kGW * 32, 4) tim_graph_kernel(const float4* __
             if (r != lane) sm = fminf(sm, Ap + Bp);
           }
         }
-        if (sm <= fmaf(64.0f * 5.9604645e-8f, Mj[c], -gc.b2)) am = ~0u;
+        // M beyond 2^62 (or inf / NaN): D^2, 2 beta^2 s' or q may overflow, and the band no longer bounds the error (DESIGN 5.2)
+        if (sm <= fmaf(64.0f * 5.9604645e-8f, Mj[c], -gc.b2) || !(Mj[c] <= 0x1p62f)) am = ~0u;
         am &= live;
         if (am) {
           const int j = cbk * 32 + lane;
