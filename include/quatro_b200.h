@@ -23,6 +23,8 @@
  *   qb200_*_each                <- one Quatro object per pair: Quatro::reset(Params) + setPreEstaimatedRyRx for every pair of a batch
  *   qb200_*_mixed               <- the same, plus voxelize / FPFHManager / matcher flags and seed per pair
  *                                  (examples/run_global_registration.cpp:206-209)
+ *   qb200_register_features_*   <- Matcher::calculateCorrespondences + Quatro::computeTransformation for every pair of a batch
+ *                                  of caller keypoints and FPFH-33 descriptors (include/fpfh_manager.hpp:125-127)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -365,8 +367,8 @@ int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_
  * earlier wave only when it needs that lane again), so the single-warp tail of one batch runs under the PCIe copies and front-end
  * kernels of the next; _flush waits for everything queued and completes the record arrays.  The scans (host kind) and `results` of
  * every queued batch must stay valid until a flush (or qb200_register_batch, = enqueue + flush) returns.  Other entry points flush
- * implicitly.  Raw, cached and correspondence-set batches (qb200_register_cached_enqueue_mixed, qb200_solve_batch_enqueue_each) and
- * scan-cache writes (qb200_cache_scans_enqueue_each) may be queued in one stream and completed by a single flush; every access to a
+ * implicitly.  Raw, cached, caller-feature and correspondence-set batches (qb200_register_cached_enqueue_mixed,
+ * qb200_register_features_enqueue_each, qb200_solve_batch_enqueue_each) and scan-cache writes (qb200_cache_scans_enqueue_each) may be queued in one stream and completed by a single flush; every access to a
  * cache slot follows enqueue order, so a queued cached batch registers the slot contents it was enqueued against.  qb200_cache_reserve,
  * qb200_cache_copy, qb200_cache_read and the pre-processing calls flush first, so they see every write queued before them. */
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
@@ -509,6 +511,45 @@ int qb200_cache_scans_enqueue_each(qb200_handle* h, const float* const* scans4, 
                                    int32_t n_scans, const qb200_params* params, qb200_mem_kind kind);
 /* read a cached scan back: voxel points (n x 4), normals (n x {nx,ny,nz,curvature}), descriptors (n x 33); any may be NULL */
 int qb200_cache_read(qb200_handle* h, int32_t slot, float* vox4, float* normals4, float* desc33, int32_t cap, int32_t* n);
+
+/* --- caller keypoints and FPFH-33 descriptors: the matcher boundary in batches ---------------------------------------------------
+ * Matcher::calculateCorrespondences(source_points, target_points, source_features, target_features, ...)
+ * (include/teaser_utils/feature_matcher.h:42-74, called by FPFHManager::setFeaturePair, include/fpfh_manager.hpp:125-127) followed by
+ * Quatro::computeTransformation, for a batch of pairs whose keypoints and descriptors the caller already holds: PCL's
+ * FPFHEstimationOMP output, a map database, or qb200_cache_read of another handle.  Pair i is matched and solved with params[i], as
+ * qb200_match followed by qb200_solve_correspondences would; the waves rotate over the lanes like every batch call.
+ *   Matcher fields (use_tuple_test, tuple_scale, tuple_trials_per_corr, seed) and solver fields may differ from pair to pair.  The
+ *     voxel and lattice fields (voxel_size, normal_radius, fpfh_radius, grid_cell, skip_flagged) are ignored; no slot signature is
+ *     involved.
+ *   Pair i's record and lists are byte-identical to those of this call on pair i alone with params[i]; they never depend on the batch,
+ *     the wave, the lane, the memory kind or the other pairs of the wave.
+ *   n_src_vox / n_tgt_vox are n_src / n_tgt.  corr indexes the caller's keypoint arrays; src_matched4 / tgt_matched4 are the caller's
+ *     keypoint records, w included.
+ *   An empty side gives QB200_DEGENERATE_INPUT, as a raw pair with an empty cloud does; more than max_corr correspondences give
+ *     QB200_CAPACITY_EXCEEDED.
+ *   Checks run before anything starts or is queued.  n < 0, n > max_voxel_points, or a NULL array on a non-empty side give
+ *     QB200_ERR_BAD_ARG, and so does, in QB200_MEM_DEVICE kind, an array that is not memory of the handle's device or is misaligned
+ *     (keypoints 16-byte, descriptors 4-byte aligned).  A params entry that fails the checks of the _each forms gives QB200_ERR_BAD_ARG,
+ *     use_crosscheck = 0 QB200_ERR_UNSUPPORTED.  A rejected call writes no record or list and queues nothing, qb200_last_error names
+ *     the entry, and the batches already queued still complete on the flush.
+ *   Entries with rot_noise_bound == 0 latch in pair order (enqueue order for the queued form), as in the other _each forms.
+ *   qb200_get_stage_ms reports the features' copy and import under [0] (h2d); [1] and [2] (voxel, fpfh) stay zero; [3] .. [7] as usual.
+ * A narrower call is this one with the entry repeated and lists = NULL.  The params array and the list descriptor are copied by the
+ * call. */
+typedef struct qb200_feature_pair {
+  const float* src;       /* n_src x {x,y,z,w}: keypoints (e.g. voxel centroids) */
+  const float* src_desc;  /* n_src x 33: pcl::FPFHSignature33 rows, the layout qb200_match takes */
+  const float* tgt;
+  const float* tgt_desc;
+  int32_t n_src, n_tgt;
+} qb200_feature_pair;
+int qb200_register_features_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                 qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+/* qb200_register_features_each, queued: completed by qb200_register_batch_flush like every enqueue, in one stream with raw, cached and
+ * correspondence-set batches and cache writes.  Host-kind keypoints and descriptors, `results` and the list arrays must stay valid until
+ * the flush returns.  Records and lists are byte-identical to those of the blocking call. */
+int qb200_register_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                         qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
 
 /* --- multi-GPU: batches of independent pairs shard across the GPUs of one box; the only communication is ONE all-gather (NCCL over
  * NVLink) of the fixed-size result records per batch -- north_star / SURVEY.md 8(e).  The reference has no counterpart (it is a

@@ -84,6 +84,12 @@ class Pair(C.Structure):
     _fields_ = [("src", C.c_void_p), ("tgt", C.c_void_p), ("n_src", C.c_int32), ("n_tgt", C.c_int32)]
 
 
+class FeaturePair(C.Structure):
+    """qb200_feature_pair: one pair's keypoints ({x,y,z,w} records) and FPFH-33 descriptor rows."""
+    _fields_ = [("src", C.c_void_p), ("src_desc", C.c_void_p), ("tgt", C.c_void_p), ("tgt_desc", C.c_void_p), ("n_src", C.c_int32),
+                ("n_tgt", C.c_int32)]
+
+
 class CorrSet(C.Structure):
     _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("L", C.c_int32), ("reserved", C.c_int32)]
 
@@ -240,6 +246,8 @@ _SIGNATURES = {
     "qb200_register_cached_enqueue_mixed": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
     "qb200_solve_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_cache_scans_enqueue_each": (i32, [vp, P(vp), P(i32), P(i32), i32, P(Params), i32]),
+    "qb200_register_features_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_register_features_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -288,6 +296,23 @@ def _set_array(sets: Sequence, kind: int):
             arr[i].a, arr[i].b, arr[i].L = a.ctypes.data, b.ctypes.data, len(a)
         else:
             arr[i].a, arr[i].b, arr[i].L = st[0], st[1], st[2]
+    return arr, keep
+
+
+def _feature_array(pairs: Sequence, kind: int = MEM_HOST):
+    """(FeaturePair * n) array of `pairs`: (src4, src_desc, tgt4, tgt_desc) numpy arrays (MEM_HOST) or (src_ptr, src_desc_ptr, n_src,
+    tgt_ptr, tgt_desc_ptr, n_tgt) device tuples (MEM_DEVICE); and the contiguous arrays it points to."""
+    arr = (FeaturePair * max(len(pairs), 1))()
+    keep = []
+    for i, pr in enumerate(pairs):
+        if kind == MEM_HOST:
+            s, sd, t, td = _f32(pr[0], 4), _f32(pr[1], 33), _f32(pr[2], 4), _f32(pr[3], 33)
+            assert len(s) == len(sd) and len(t) == len(td)
+            keep.append((s, sd, t, td))
+            arr[i].src, arr[i].src_desc, arr[i].n_src = s.ctypes.data, sd.ctypes.data, len(s)
+            arr[i].tgt, arr[i].tgt_desc, arr[i].n_tgt = t.ctypes.data, td.ctypes.data, len(t)
+        else:
+            arr[i].src, arr[i].src_desc, arr[i].n_src, arr[i].tgt, arr[i].tgt_desc, arr[i].n_tgt = pr
     return arr, keep
 
 
@@ -605,6 +630,7 @@ class Handle:
 
     pair_array = staticmethod(_pair_array)
     _set_array = staticmethod(_set_array)
+    feature_array = staticmethod(_feature_array)
 
     def register_batch(self, pairs: Sequence, params: Params, kind: int = MEM_HOST) -> np.ndarray:
         """pairs: sequence of (src, tgt).  MEM_HOST: numpy (n,4) float32 arrays; MEM_DEVICE:
@@ -731,6 +757,21 @@ class Handle:
         (host kind), `out` and the buffers must stay alive until register_batch_flush."""
         return self._check(self.lib.qb200_solve_batch_enqueue_each(self.h, set_array, n, params_array, kind, _ptr(out),
                                                                    self._lists_arg(buffers)), "qb200_solve_batch_enqueue_each")
+
+    # ---- caller keypoints and FPFH-33 descriptors (the matcher boundary) ----
+    def register_features_each(self, pairs: Sequence, params: Sequence[Params], kind: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
+        """qb200_register_features_each: pair i's keypoints and descriptors (feature_array()) are matched and solved with params[i];
+        corr indexes the caller's keypoints."""
+        assert len(params) == len(pairs)
+        arr, keep = self.feature_array(pairs, kind)
+        return self._batch_lists("qb200_register_features_each", len(pairs), (arr, len(pairs), self.params_array(params), kind), buffers)
+
+    def register_features_enqueue_each_raw(self, feature_array, n: int, params_array, kind: int, out: np.ndarray,
+                                           buffers: Optional[ListBuffers] = None):
+        """qb200_register_features_enqueue_each: params_array (params_array()) is copied by the call; feature_array (feature_array()),
+        its host arrays, `out` and the buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_register_features_enqueue_each(self.h, feature_array, n, params_array, kind, _ptr(out),
+                                                                         self._lists_arg(buffers)), "qb200_register_features_enqueue_each")
 
     def cache_scans_enqueue_each_raw(self, scan_ptrs, counts, slot_ids, n: int, params_array, kind: int):
         """qb200_cache_scans_enqueue_each: scan_ptrs / counts (_scan_arrays()), slot_ids (c_int32 * n) and params_array

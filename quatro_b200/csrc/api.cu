@@ -99,6 +99,8 @@ int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   QB_CUDA_TRY(L, L->raw_stage.alloc(C * R));
   QB_CUDA_TRY(L, L->d_slot_of_cloud.alloc(C));
   QB_CUDA_TRY(L, L->h_slot_of_cloud.alloc(C));
+  QB_CUDA_TRY(L, L->d_feat.alloc(C));
+  QB_CUDA_TRY(L, L->h_feat.alloc(C));
   // the sort workspace serves the voxel sort (C*R items, digit histograms in val_a, chunk counts C*kVsChunks <= n_sort in val_b),
   // the lattice / norm sorts (C*V items) and, afterwards, the duplicate-class tables of K6 (2S*V + 2S words in key_a): size it for
   // the largest user
@@ -333,6 +335,50 @@ int stage_raw(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs) {
   return QB200_OK;
 }
 
+int stage_features(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs) {
+  if (kind == QB200_MEM_HOST) {
+    // Host clouds are packed into areas a feature wave leaves idle: keypoints into normals, descriptor rows into spfh.  A run of
+    // clouds that lie back to back in the caller's memory crosses PCIe as one copy per array, as raw scans do (stage_raw).
+    const char* run_src[2] = {nullptr, nullptr};
+    char* run_dst[2] = {nullptr, nullptr};
+    size_t run_bytes[2] = {0, 0};
+    auto flush_run = [&](int k) -> int {
+      if (run_bytes[k] > 0) QB_CUDA_TRY(L, cudaMemcpyAsync(run_dst[k], run_src[k], run_bytes[k], cudaMemcpyHostToDevice, cs));
+      run_bytes[k] = 0;
+      return QB200_OK;
+    };
+    auto add = [&](int k, const void* src, void* dst, size_t bytes) -> int {
+      const char* s = static_cast<const char*>(src);
+      char* d = static_cast<char*>(dst);
+      if (bytes == 0) return QB200_OK;
+      if (run_bytes[k] > 0 && s == run_src[k] + run_bytes[k] && d == run_dst[k] + run_bytes[k]) {
+        run_bytes[k] += bytes;
+        return QB200_OK;
+      }
+      if (int rc = flush_run(k)) return rc;
+      run_src[k] = s; run_dst[k] = d; run_bytes[k] = bytes;
+      return QB200_OK;
+    };
+    size_t off = 0;
+    for (int c = 0; c < ncl; ++c) {
+      FeatureSrc& f = L->h_feat[c];
+      float4* pts = L->normals.get() + off;
+      float* desc = L->spfh + off * kDescDim;
+      if (f.pts) {
+        if (int rc = add(0, f.pts, pts, (size_t)f.n * sizeof(float4))) return rc;
+        f.pts = pts;
+      }
+      if (int rc = add(1, f.desc, desc, (size_t)f.n * kDescDim * sizeof(float))) return rc;
+      f.desc = desc;
+      off += f.n;
+    }
+    for (int k = 0; k < 2; ++k)
+      if (int rc = flush_run(k)) return rc;
+  }
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_feat, L->h_feat, (size_t)ncl * sizeof(FeatureSrc), cudaMemcpyHostToDevice, cs));
+  return QB200_OK;
+}
+
 }  // namespace qb
 
 namespace {
@@ -386,7 +432,8 @@ int cache_waits(qb200_handle* h, Lane* L, int ncl, bool write) {
 
 // ---- batch calls ----------------------------------------------------------------------------------------------------------
 // One batch call as its entry point received it.  Its input is n pairs of raw scans (in `kind` memory), n pairs of cached scans,
-// n correspondence sets (in `kind` memory), or n raw scans to cache (cache_write): exactly one of the four is set.  The registering
+// n correspondence sets (in `kind` memory), n raw scans to cache (cache_write), or n pairs of caller keypoints and descriptors (in
+// `kind` memory, feature_call): exactly one of the five is set.  The registering
 // entry points fill the fields up to `lists` in order.
 struct BatchCall {
   const qb200_pair* pairs = nullptr;
@@ -406,6 +453,8 @@ struct BatchCall {
   const float* const* scans = nullptr;
   const int32_t* n_points = nullptr;
   const int32_t* slot_ids = nullptr;
+  // caller features: pair i's keypoints and FPFH-33 rows, matched and solved with its own entry (front-end fields ignored)
+  const qb200_feature_pair* feats = nullptr;
   // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved, laid out like `caller`.
   const qb200_params* params = nullptr;
   // raw host scans of a multi-wave batch: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies queued on
@@ -479,7 +528,8 @@ int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
 }
 
 // Enqueue one wave (pairs [w0, w0 + np), np <= S) on lane L: the front of the wave its input needs (raw scans: H2D, K1..K6;
-// cached scans: the copy out of the cache, K6; correspondence sets: their H2D), then K8..K11 and the D2H of the result records.
+// cached scans: the copy out of the cache, K6; caller features: their H2D and import, K6; correspondence sets: their H2D), then
+// K8..K11 and the D2H of the result records.
 // A cache write's wave is scans [w0, w0 + np), np <= 2S: their H2D, K1..K5 and the copy into their slots, with no records.
 // No sync: wave_collect hands the records out to in.results[w0...].  The lane's previous wave must have been collected.
 int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
@@ -530,6 +580,21 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     cudaEventRecord(L->ev[2], L->stream);
     if ((rc = launch_fpfh(L, ncl))) return rc;
     cudaEventRecord(L->ev[3], L->stream);
+  } else if (in.feats) {
+    cudaEventRecord(L->ev[0], L->stream);
+    for (int s = 0; s < np; ++s) {
+      const qb200_feature_pair& f = in.feats[w0 + s];
+      L->h_feat[2 * s] = {reinterpret_cast<const float4*>(f.src), f.src_desc, f.n_src, 0};
+      L->h_feat[2 * s + 1] = {reinterpret_cast<const float4*>(f.tgt), f.tgt_desc, f.n_tgt, 0};
+    }
+    if ((rc = stage_features(L, ncl, in.kind, in.copy_stream ? in.copy_stream : L->stream))) return rc;
+    if ((rc = wave_reset(L, ncl))) return rc;
+    if (in.copy_stream) {
+      QB_CUDA_TRY(L, cudaEventRecord(h->ev_copied, in.copy_stream));
+      QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, h->ev_copied, 0));
+    }
+    if ((rc = launch_feature_import(L, ncl))) return rc;
+    for (int i = 1; i <= 3; ++i) cudaEventRecord(L->ev[i], L->stream);  // no voxel or FPFH stage: slots 1 and 2 are not reported
   } else if (in.slots) {
     for (int s = 0; s < np; ++s) {
       L->h_slot_of_cloud[2 * s] = in.slots[w0 + s].src_slot;
@@ -559,7 +624,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     if ((rc = cache_copy(h, L, 1, ncl))) return rc;
     QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_out, L->stream));
   } else {
-    if (!in.sets && (rc = launch_match(L, np))) return rc;
+    if (!in.sets && (rc = launch_match(L, np, in.feats != nullptr))) return rc;
     cudaEventRecord(L->ev[4], L->stream);
     cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
     if ((rc = run_solver(L, np, in.sets ? 0 : 1))) return rc;
@@ -573,10 +638,9 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   L->pend_dst = in.results;  // nullptr for a cache write: no records
   if (in.lists) L->pend_lists = *in.lists;
   else L->pend_lists.cap_per_pair = 0;
-  // stage-time slots of qb200_get_stage_ms this wave reports: raw scans all eight, the other inputs their first stage to pose, a cache
-  // write none (it registers nothing)
-  L->pend_t0 = in.pairs ? 0 : in.slots ? 2 : in.sets ? 4 : 8;
-  L->pend_t1 = in.pairs || in.scans ? 8 : 7;
+  // stage-time slots of qb200_get_stage_ms this wave reports: raw scans all eight, caller features h2d and match to d2h, the other
+  // inputs their first stage to pose, a cache write none (it registers nothing)
+  L->pend_stages = in.pairs ? 0xFFu : in.feats ? 0xF9u : in.slots ? 0x7Cu : in.sets ? 0x70u : 0u;
   return QB200_OK;
 }
 
@@ -591,7 +655,7 @@ int wave_collect(qb200_handle* h, Lane* L) {
   }
   if (L->pend_dst) memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
   if (L->pend_lists.cap_per_pair > 0 && L->pend_lists.kind == QB200_MEM_HOST) deliver_lists(L, L->pend_lists, L->pend_w0, np);
-  if (h->timeline && L->pend_t0 == 0) {  // stage boundaries of a raw-scan wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
+  if (h->timeline && (L->pend_stages & 1u)) {  // stage boundaries of a raw-scan or feature wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
     fprintf(stderr, "[qb200 timeline] wave w0=%d np=%d:", L->pend_w0, np);
     for (int i = 0; i < 9; ++i) {
       float ms = -1.f;
@@ -600,7 +664,8 @@ int wave_collect(qb200_handle* h, Lane* L) {
     }
     fprintf(stderr, "\n");
   }
-  for (int i = L->pend_t0; i < L->pend_t1; ++i) {
+  for (int i = 0; i < 8; ++i) {
+    if (!(L->pend_stages >> i & 1u)) continue;
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, L->ev[i], L->ev[i + 1]) == cudaSuccess) h->stage_ms[i] += ms;
   }
@@ -678,12 +743,12 @@ int check_call(qb200_handle* h, const BatchCall& c) {
     return QB200_ERR_BAD_ARG;
   };
   if (c.n < 0) return reject("n < 0");
-  if (c.n > 0 && !c.pairs && !c.slots && !c.sets && !c.scans) return reject("the input array is null");
+  if (c.n > 0 && !c.pairs && !c.slots && !c.sets && !c.scans && !c.feats) return reject("the input array is null");
   if (c.n > 0 && c.scans && (!c.n_points || !c.slot_ids)) return reject("the n_points or slot_ids array is null");
   if (c.n > 0 && !c.scans && !c.results) return reject("the results array is null");
   if (c.kind != QB200_MEM_HOST && c.kind != QB200_MEM_DEVICE) return reject("unknown memory kind of the inputs");
   const qb200_params* p = c.caller;
-  char why[128];
+  char why[192];
   if (int rc = check_params(h, p, c.n, c.each, !c.sets && !c.mixed)) return rc;
   for (int i = 0; !c.sets && !c.scans && i < (c.each ? c.n : 1); ++i) {
     if (!p[i].use_crosscheck) {
@@ -709,6 +774,22 @@ int check_call(qb200_handle* h, const BatchCall& c) {
         if (sig[0] != pe.voxel_size || sig[1] != pe.normal_radius || sig[2] != pe.fpfh_radius || sig[3] != lattice_cell(pe)) {
           snprintf(why, sizeof(why), "pair %d: cached scan in slot %d was computed with other front-end parameters (or the slot is empty)",
                    i, sl);
+          return reject(why);
+        }
+      }
+    } else if (c.feats) {
+      const qb200_feature_pair& f = c.feats[i];
+      for (int side = 0; side < 2; ++side) {
+        const int n = side ? f.n_tgt : f.n_src;
+        const float* pts = side ? f.tgt : f.src;
+        const float* desc = side ? f.tgt_desc : f.src_desc;
+        const char* bad = nullptr;
+        if (n < 0 || n > h->cfg.max_voxel_points) bad = "count outside 0 .. max_voxel_points";
+        else if (n > 0 && (!pts || !desc)) bad = "null keypoints or descriptors";
+        else if (n > 0 && c.kind == QB200_MEM_DEVICE && !(device_array_of(h, pts, 16) && device_array_of(h, desc, 4)))
+          bad = "keypoints (16-byte) or descriptors (4-byte) misaligned or not memory of the handle's device";
+        if (bad) {
+          snprintf(why, sizeof(why), "feature pair %d, %s: %s", i, side ? "target" : "source", bad);
           return reject(why);
         }
       }
@@ -747,8 +828,8 @@ int enqueue_call(qb200_handle* h, BatchCall c) {
   c.params = c.scans ? c.caller : pr.get();
   // S: inputs per wave, pairs or (a cache write) scans; the clouds of a wave fill the lane's 2 * max_batch_slots cloud buffers
   const int S = h->cfg.max_batch_slots * (c.scans ? 2 : 1), lanes = h->max_lanes;
-  // raw host scans cross PCIe: the copy stream and the quarter-wave opening below are theirs alone
-  const bool host_scans = (c.pairs || c.scans) && c.kind == QB200_MEM_HOST;
+  // raw host scans and host features cross PCIe: the copy stream and the quarter-wave opening below are theirs alone
+  const bool host_scans = (c.pairs || c.scans || c.feats) && c.kind == QB200_MEM_HOST;
   // More than one wave: rotate over the lanes so that one wave's PCIe copies and single-warp solver tail run under the
   // other waves' dense kernels.  Results do not depend on the lane (no state is shared between waves).
   // Wave plan.  Host scans: nothing can run before the first wave's scans crossed PCIe, so the batch opens with a quarter
@@ -830,6 +911,15 @@ BatchCall cache_write(const float* const* scans4, const int32_t* n_points, const
   BatchCall c;
   c.n = n_scans; c.kind = kind; c.caller = p; c.each = each; c.mixed = true;
   c.scans = scans4; c.n_points = n_points; c.slot_ids = slot_ids;
+  return c;
+}
+
+// qb200_register_features_each (enqueue = false) and qb200_register_features_enqueue_each as a batch call
+BatchCall feature_call(const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind, qb200_result* results,
+                       const qb200_pair_lists* lists) {
+  BatchCall c;
+  c.n = n_pairs; c.kind = kind; c.caller = params; c.each = true; c.results = results; c.lists = lists; c.mixed = true;
+  c.feats = pairs;
   return c;
 }
 
@@ -1068,6 +1158,17 @@ int qb200_register_cached_mixed(qb200_handle* h, const qb200_slot_pair* pairs, i
 int qb200_register_cached_enqueue_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                         qb200_result* results, const qb200_pair_lists* lists) {
   return enqueue_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists, true});
+}
+
+// ---- caller keypoints and descriptors -> pose ------------------------------------------------------------------------------
+int qb200_register_features_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                 qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return run_call(h, feature_call(pairs, n_pairs, params, kind, results, lists));
+}
+
+int qb200_register_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                         qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_call(h, feature_call(pairs, n_pairs, params, kind, results, lists));
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

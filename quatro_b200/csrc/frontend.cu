@@ -661,18 +661,39 @@ __global__ void __launch_bounds__(kNbrThreads) fpfh_rare_kernel(const float4* __
   for (int b = 22; b < 33; ++b) out[(size_t)b * V] = o[b] * g2;
 }
 
-// descriptor layout converters for the stage API (pcl::FPFHSignature33 rows <-> dimension-major)
+// dimension-major descriptors -> pcl::FPFHSignature33 rows (qb200_compute_fpfh, qb200_get_last_features, qb200_cache_read)
 __global__ void desc_to_aos_kernel(const float* __restrict__ desc_t, int V, int n, float* __restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n * kDescDim) return;
   const int q = i / kDescDim, d = i % kDescDim;
   out[i] = desc_t[(size_t)d * V + q];
 }
-__global__ void desc_from_aos_kernel(const float* __restrict__ in, int V, int n, float* __restrict__ desc_t) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n * kDescDim) return;
-  const int q = i / kDescDim, d = i % kDescDim;
-  desc_t[(size_t)d * V + q] = in[i];
+
+constexpr int kImportTile = 128, kImportThreads = 256;
+
+// Caller features of a wave -> the matcher's inputs: cloud c's keypoints into vox_pts, its n x 33 descriptor rows
+// (pcl::FPFHSignature33) into the 33 dimension-major rows of desc_t, and n into n_vox.  One CTA per tile of kImportTile points of a
+// cloud: the tile's AoS rows are one contiguous run of kImportTile * 132 bytes, read coalesced into shared memory, and every
+// dimension-major row segment is written coalesced from there (row stride 33 floats: the column reads are free of bank conflicts).
+// A pure copy: every value, NaN payloads included, arrives bit for bit.
+__global__ void __launch_bounds__(kImportThreads) feature_import_kernel(const FeatureSrc* __restrict__ table, int V, float4* __restrict__ vox_pts,
+                                                                        float* __restrict__ desc_t, int* __restrict__ n_vox) {
+  __shared__ float tile[kImportTile * kDescDim];
+  const int cloud = blockIdx.y, q0 = blockIdx.x * kImportTile, tid = threadIdx.x;
+  const FeatureSrc f = table[cloud];
+  if (blockIdx.x == 0 && tid == 0) n_vox[cloud] = f.n;
+  if (q0 >= f.n) return;
+  const int m = min(kImportTile, f.n - q0);
+  if (f.pts)  // (qb200_debug_tc_distances imports descriptors only)
+    for (int i = tid; i < m; i += kImportThreads) vox_pts[(size_t)cloud * V + q0 + i] = __ldg(f.pts + q0 + i);
+  const float* __restrict__ src = f.desc + (size_t)q0 * kDescDim;
+  for (int i = tid; i < m * kDescDim; i += kImportThreads) tile[i] = __ldg(src + i);
+  __syncthreads();
+  float* __restrict__ out = desc_t + (size_t)cloud * kDescK * V + q0;
+  for (int i = tid; i < kDescDim * kImportTile; i += kImportThreads) {
+    const int d = i / kImportTile, q = i % kImportTile;
+    if (q < m) out[(size_t)d * V + q] = tile[q * kDescDim + d];
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -764,9 +785,12 @@ int desc_to_aos_rows(Lane* h, const float* desc_rows, int n, float* d_out33) {
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;
 }
-int launch_desc_from_aos(Lane* h, int cloud, int n, const float* d_in33) {
-  if (n <= 0) return QB200_OK;
-  desc_from_aos_kernel<<<(n * kDescDim + 255) / 256, 256, 0, h->stream>>>(d_in33, h->V, n, h->desc_t + (size_t)cloud * kDescK * h->V);
+int launch_feature_import(Lane* h, int n_clouds) {
+  if (n_clouds <= 0) return QB200_OK;
+  int n_max = 1;  // at least one tile per cloud: its first CTA writes n_vox, also for an empty cloud
+  for (int c = 0; c < n_clouds; ++c) n_max = h->h_feat[c].n > n_max ? h->h_feat[c].n : n_max;
+  const dim3 g((n_max + kImportTile - 1) / kImportTile, n_clouds);
+  feature_import_kernel<<<g, kImportThreads, 0, h->stream>>>(h->d_feat, h->V, h->vox_pts, h->desc_t, h->ctr.n_vox);
   h->launches++;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;

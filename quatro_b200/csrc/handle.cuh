@@ -54,6 +54,14 @@ struct CloudFront {
 
 struct PpScan;   // one scan's pre-processing entry (preprocess.cu)
 
+// Where feature_import_kernel reads one cloud of a feature wave (frontend.cu): n keypoints and n FPFH-33 rows, in the caller's
+// device memory or in the lane's staging areas
+struct FeatureSrc {
+  const float4* pts;
+  const float* desc;
+  int n, pad;
+};
+
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
 // kernels of the others.  The lane owns its stream, buffers and events: deleting it releases them.
@@ -77,8 +85,9 @@ struct Lane {
   PinnedMem<const float4*> h_cloud_ptr; PinnedMem<int> h_cloud_n, h_raw_off;  // pinned mirrors
   DeviceMem<float4> raw_stage; // [2S*R] staging for host inputs
   DeviceMem<int> d_slot_of_cloud; PinnedMem<int> h_slot_of_cloud;  // [2S] cache slot of every cloud of the wave, and its pinned mirror
+  DeviceMem<FeatureSrc> d_feat; PinnedMem<FeatureSrc> h_feat;  // [2S] where a feature wave's clouds are read, and its pinned mirror
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
-  int pend_t0, pend_t1;       // ... the stage-time slots [t0, t1) it records
+  unsigned pend_stages;      // ... the stage-time slots it reports (bit i: qb200_get_stage_ms slot i)
   qb200_result* pend_dst;     // ... and the caller's record array of its batch
   qb200_pair_lists pend_lists; // ... and a copy of its batch's list descriptor (cap_per_pair == 0: no lists)
   // ... and the cache slots it reads (cached pairs) or writes (scans to cache), ascending and unique; empty: it does not touch the
@@ -92,15 +101,15 @@ struct Lane {
   DeviceMem<uint64_t> key_a, key_b;  // [2S*max(R,V)]
   DeviceMem<uint32_t> val_a, val_b;  // [2S*max(R,V)]; val_a also holds the voxel sort's digit histograms
   DeviceMem<void> cub_temp; size_t cub_bytes;  // library radix sort of up to 2S*V items (lattice / norm sorts of clouds too large for sort.cu)
-  DeviceMem<float> aos_scratch;  // [2*V*33] AoS descriptors of the stage entry points (qb200_compute_fpfh / qb200_match)
+  DeviceMem<float> aos_scratch;  // [2*V*33] AoS descriptors handed out by qb200_compute_fpfh / _get_last_features / _cache_read
 
   // ---- front end ----
   DeviceMem<int> vox_start;   // [2S*(V+1)] position (in the sorted raw array) of each voxel's first point
   DeviceMem<float4> vox_pts;  // [2S*V] centroids, ascending (k,j,i)
   DeviceMem<uint64_t> cell_key; // [2S*V] occupied lattice cells, ascending
   DeviceMem<int> cell_start;  // [2S*(V+1)]
-  DeviceMem<float4> normals;  // [2S*V]
-  DeviceMem<float> spfh;      // [2S*V*36] rows padded to 36 floats
+  DeviceMem<float4> normals;  // [2S*V]; a feature wave stages host keypoints here (packed, [sum n])
+  DeviceMem<float> spfh;      // [2S*V*36] rows padded to 36 floats; a feature wave stages host descriptors here (packed, [sum n][33])
   DeviceMem<uint32_t> nbr_list; // [2S][kNbrGlobalCap][V] fpfh_radius neighbour indices found by K2c (lattice order), read by K3..K5
   DeviceMem<int> nbr_cnt;     // [2S*V] neighbour count (self included); > kNbrGlobalCap: K5 walks the lattice itself
   DeviceMem<float> desc_t;    // [2S*40*V] FPFH, dimension-major per cloud (row d = bin d over all points; rows 33..39 zero)
@@ -232,7 +241,8 @@ size_t pose_ws_bytes(int Lc);
 // launches the tuple test only when h_solve has a pair that runs it.
 int launch_voxel(Lane* h, int n_clouds);
 int launch_fpfh(Lane* h, int n_clouds);
-int launch_match(Lane* h, int n_pairs);
+// keep_w: the matched points keep their keypoints' w (caller keypoints of a feature wave); otherwise w = 1
+int launch_match(Lane* h, int n_pairs, int keep_w);
 // a cloud's front-end entry: its voxel fields (frontend.cu), its lattice fields for these radii and this lattice cell (frontend.cu),
 // or both from p (api.cu)
 void front_voxel(CloudFront* e, float leaf, int skip_flagged);
@@ -277,7 +287,11 @@ int launch_match_exact(Lane* h, int n_pairs, const int* only);
 int launch_tc_debug_tile(Lane* h, float* d_out);
 int tc_footprint(Lane* h, int* out5);
 int launch_desc_to_aos(Lane* h, int cloud, int n, float* d_out33);
-int launch_desc_from_aos(Lane* h, int cloud, int n, const float* d_in33);
+// Feature waves (api.cu: stage_features, frontend.cu): h_feat[0, n) holds every cloud's caller pointers and count.  stage_features
+// copies host-kind inputs into the staging areas (inputs back to back in the caller's memory as one copy) and uploads the table, on
+// stream cs; launch_feature_import then fills vox_pts, desc_t and n_vox on the lane's stream (after wave_reset).
+int stage_features(Lane* L, int n_clouds, qb200_mem_kind kind, cudaStream_t cs);
+int launch_feature_import(Lane* h, int n_clouds);
 int desc_to_aos_rows(Lane* h, const float* desc_rows, int n, float* d_out33);
 size_t sort_temp_bytes(int max_items);
 void comm_release(qb200_handle* h);

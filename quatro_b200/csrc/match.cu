@@ -388,7 +388,7 @@ __global__ void __launch_bounds__(256) scatter_partner_kernel(const int* __restr
 __global__ void __launch_bounds__(1024) pack_corr_kernel(const int* __restrict__ partner, const float4* __restrict__ vox_pts, const int* __restrict__ n_vox,
                                                          int V, int Lc, int* __restrict__ corr_src, int* __restrict__ corr_tgt,
                                                          float4* __restrict__ ma, float4* __restrict__ mb, int* __restrict__ n_corr,
-                                                         int* __restrict__ cloud_status) {
+                                                         int* __restrict__ cloud_status, int keep_w) {
   __shared__ int sm[33];
   const int pair = blockIdx.x;
   const int nA = n_vox[2 * pair];
@@ -406,8 +406,8 @@ __global__ void __launch_bounds__(1024) pack_corr_kernel(const int* __restrict__
       corr_src[(size_t)pair * Lc + o] = s;
       corr_tgt[(size_t)pair * Lc + o] = t;
       const float4 a = ps[s], b = pt[t];
-      ma[(size_t)pair * Lc + o] = make_float4(a.x, a.y, a.z, 1.0f);
-      mb[(size_t)pair * Lc + o] = make_float4(b.x, b.y, b.z, 1.0f);
+      ma[(size_t)pair * Lc + o] = make_float4(a.x, a.y, a.z, keep_w ? a.w : 1.0f);
+      mb[(size_t)pair * Lc + o] = make_float4(b.x, b.y, b.z, keep_w ? b.w : 1.0f);
     }
     carry += tot;
   }
@@ -468,7 +468,7 @@ void match_fields(PairSolve* e, const qb200_params& p) {
   e->seed = p.seed;
 }
 
-int launch_match(Lane* h, int n_pairs) {
+int launch_match(Lane* h, int n_pairs, int keep_w) {
   if (n_pairs <= 0) return QB200_OK;
   const int V = h->V;
   int rc = h->force_exact_match ? launch_match_exact(h, n_pairs, nullptr) : launch_match_nn(h, n_pairs);
@@ -500,7 +500,7 @@ int launch_match(Lane* h, int n_pairs) {
   const dim3 gsc((V + 255) / 256, n_pairs);
   scatter_partner_kernel<<<gsc, 256, 0, h->stream>>>(h->mut_i, h->mut_j, h->ctr.n_mutual, h->ctr.swapped, h->mark, h->d_solve, V, h->partner);
   pack_corr_kernel<<<n_pairs, 1024, 0, h->stream>>>(h->partner, h->vox_pts, h->ctr.n_vox, V, h->Lc, h->corr_src, h->corr_tgt, h->ma, h->mb,
-                                                    h->ctr.n_corr, h->ctr.cloud_status);
+                                                    h->ctr.n_corr, h->ctr.cloud_status, keep_w);
   h->launches += 2;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;

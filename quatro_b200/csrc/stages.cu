@@ -130,19 +130,15 @@ int qb200_match(qb200_handle* h, const float* src4, int32_t n_src, const float* 
   if (n_src == 0 || n_tgt == 0) return QB200_OK;
   int rc = wave_reset(L, 2);
   if (rc) return rc;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(L->vox_pts, src4, (size_t)n_src * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
-  QB_CUDA_TRY(h, cudaMemcpyAsync(L->vox_pts + L->V, tgt4, (size_t)n_tgt * sizeof(float4), cudaMemcpyHostToDevice, L->stream));
   h->last_match_n[0] = n_src; h->last_match_n[1] = n_tgt;
-  float* scratch = L->aos_scratch;
-  float* scratch2 = scratch + (size_t)L->V * kDescDim;
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch, src_desc33, (size_t)n_src * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch2, tgt_desc33, (size_t)n_tgt * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
   MirrorHold hold{L};
-  if ((rc = write_counter(L, L->hctr.n_vox, n_src)) || (rc = write_counter(L, L->hctr.n_vox + 1, n_tgt))) return rc;
-  if ((rc = launch_desc_from_aos(L, 0, n_src, scratch)) || (rc = launch_desc_from_aos(L, 1, n_tgt, scratch2))) return rc;
+  // the features as a feature wave of one pair imports them (the import writes the clouds' counts)
+  L->h_feat[0] = {reinterpret_cast<const float4*>(src4), src_desc33, n_src, 0};
+  L->h_feat[1] = {reinterpret_cast<const float4*>(tgt4), tgt_desc33, n_tgt, 0};
+  if ((rc = stage_features(L, 2, QB200_MEM_HOST, L->stream)) || (rc = launch_feature_import(L, 2))) return rc;
   memset(&L->h_solve[0], 0, sizeof(PairSolve));  // a one-entry pair table: p's tuple test
   match_fields(&L->h_solve[0], *p);
-  if ((rc = upload_solve(L, 1)) || (rc = launch_match(L, 1)) || (rc = read_counters(L))) return rc;
+  if ((rc = upload_solve(L, 1)) || (rc = launch_match(L, 1, 0)) || (rc = read_counters(L))) return rc;
   QB_CUDA_TRY(h, hold.sync());
   if (n_mutual) *n_mutual = L->hctr.n_mutual[0];
   h->last_n_corr = L->hctr.n_corr[0];
@@ -169,7 +165,7 @@ int qb200_match_and_pack(qb200_handle* h, const float* src4, int32_t n_src, cons
   memset(&L->h_solve[0], 0, sizeof(PairSolve));
   match_fields(&L->h_solve[0], *p);
   if ((rc = upload_front(L, 2)) || (rc = upload_solve(L, 1)) || (rc = launch_fpfh(L, 2))) return rc;
-  if ((rc = launch_match(L, 1)) || (rc = read_counters(L))) return rc;
+  if ((rc = launch_match(L, 1, 0)) || (rc = read_counters(L))) return rc;
   QB_CUDA_TRY(h, hold.sync());
   h->last_n_corr = L->hctr.n_corr[0];
   if ((rc = qb200_get_last_correspondences(h, corr, src_matched4, tgt_matched4, cap, n_corr))) return rc;
@@ -398,12 +394,12 @@ int qb200_debug_tc_distances(qb200_handle* h, const float* a33, int32_t na, cons
   Lane* L = h->lane[0].get();
   int rc = wave_reset(L, 2);
   if (rc) return rc;
-  float* scratch = L->aos_scratch;  // b's descriptors go 128 rows further
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch, a33, (size_t)na * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
-  QB_CUDA_TRY(h, cudaMemcpyAsync(scratch + (size_t)128 * kDescDim, b33, (size_t)nb * kDescDim * sizeof(float), cudaMemcpyHostToDevice, L->stream));
   MirrorHold hold{L};
-  if ((rc = write_counter(L, L->hctr.n_vox, na)) || (rc = write_counter(L, L->hctr.n_vox + 1, nb))) return rc;
-  if ((rc = launch_desc_from_aos(L, 0, na, scratch)) || (rc = launch_desc_from_aos(L, 1, nb, scratch + (size_t)128 * kDescDim))) return rc;
+  // the descriptors as a feature wave imports them, without keypoints: the import's staging is in spfh, which
+  // the stream has passed before the memset below reuses it
+  L->h_feat[0] = {nullptr, a33, na, 0};
+  L->h_feat[1] = {nullptr, b33, nb, 0};
+  if ((rc = stage_features(L, 2, QB200_MEM_HOST, L->stream)) || (rc = launch_feature_import(L, 2))) return rc;
   float* d_out = L->spfh;  // not the sort scratch: K6 sorts the descriptors by norm first
   QB_CUDA_TRY(h, cudaMemsetAsync(d_out, 0, 128 * 128 * sizeof(float), L->stream));
   if ((rc = launch_tc_debug_tile(L, d_out))) return rc;
