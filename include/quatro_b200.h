@@ -25,6 +25,8 @@
  *                                  (examples/run_global_registration.cpp:206-209)
  *   qb200_register_features_*   <- Matcher::calculateCorrespondences + Quatro::computeTransformation for every pair of a batch
  *                                  of caller keypoints and FPFH-33 descriptors (include/fpfh_manager.hpp:125-127)
+ *   qb200_describe_batch_*      <- voxelize<T>() + FPFHEstimation::computeFPFHFeatures + FPFHManager::getObjDescriptor /
+ *                                  getTgtNormals for every scan of a batch (include/fpfh_manager.hpp:161-177)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -368,7 +370,8 @@ int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_
  * kernels of the next; _flush waits for everything queued and completes the record arrays.  The scans (host kind) and `results` of
  * every queued batch must stay valid until a flush (or qb200_register_batch, = enqueue + flush) returns.  Other entry points flush
  * implicitly.  Raw, cached, caller-feature and correspondence-set batches (qb200_register_cached_enqueue_mixed,
- * qb200_register_features_enqueue_each, qb200_solve_batch_enqueue_each) and scan-cache writes (qb200_cache_scans_enqueue_each) may be queued in one stream and completed by a single flush; every access to a
+ * qb200_register_features_enqueue_each, qb200_solve_batch_enqueue_each), scan-cache writes (qb200_cache_scans_enqueue_each) and describe
+ * calls (qb200_describe_batch_enqueue_each) may be queued in one stream and completed by a single flush; every access to a
  * cache slot follows enqueue order, so a queued cached batch registers the slot contents it was enqueued against.  qb200_cache_reserve,
  * qb200_cache_copy, qb200_cache_read and the pre-processing calls flush first, so they see every write queued before them. */
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
@@ -550,6 +553,47 @@ int qb200_register_features_each(qb200_handle* h, const qb200_feature_pair* pair
  * the flush returns.  Records and lists are byte-identical to those of the blocking call. */
 int qb200_register_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                          qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+
+/* --- the front end in batches: voxel keypoints, normals and FPFH-33 of many scans into caller memory ----------------------------------
+ * voxelize<T> (include/quatro.hpp:49-57) + FPFHEstimation::computeFPFHFeatures (src/teaser_utils/fpfh.cc:44-75), handed out as
+ * FPFHManager::getObjDescriptor / getSceneDescriptor / getTgtNormals do (include/fpfh_manager.hpp:161-177), for a batch of raw scans:
+ * a descriptor database, a map of keyframe features, or FPFH for another solver.  The output goes straight into the caller's arrays,
+ * and qb200_register_features_each of any handle takes it back as keypoints and descriptors.
+ *   Scan i (scans4[i]: n_points[i] x {x,y,z,w} in `kind` memory) is voxelized and described with the front-end fields of params[i]
+ *     (voxel_size, normal_radius, fpfh_radius, grid_cell, skip_flagged); the other fields are ignored.
+ *   Scan i's entries start at i * cap_per_scan in every array; min(counts[i], cap_per_scan) of them are written and nothing past them,
+ *     so a count above cap_per_scan shows the clipping.  The arrays are byte-identical to qb200_cache_scans_each of that scan alone
+ *     with params[i] followed by qb200_cache_read; they never depend on the batch, the wave, the lane, the memory kinds or the other
+ *     scans.
+ *   A scan refused on its own gets its status in status[i]: QB200_CAPACITY_EXCEEDED (more occupied voxels than max_voxel_points) or
+ *     QB200_ERR_VOXEL_OVERFLOW (PCL's voxel index would overflow; qb200_voxelize hands such a scan back unfiltered, this call does
+ *     not).  Its count is 0, nothing is written for it, and the other scans are unaffected.  Every other scan gets QB200_OK, an
+ *     empty one (or one whose points are all skipped) with count 0.
+ *   Checks run before anything starts or is queued: those of qb200_cache_scans_each (without the slots), cap_per_scan >= 1, non-NULL
+ *     counts and status, a known output kind, and in QB200_MEM_DEVICE output kind arrays of the handle's device, vox4 / normals4
+ *     16-byte and desc33 4-byte aligned.  A rejected call gives QB200_ERR_BAD_ARG, writes no count, status or entry, queues nothing,
+ *     and qb200_last_error names the bad scan, entry or array; batches already queued still complete on the flush.
+ *   The scans run in waves of 2 * max_batch_slots over the lanes, as cache writes do.  Host-kind output is complete when the call
+ *     returns, device-kind output when the call's stream work is done (the call itself waits for it).
+ *   Like a cache write, this is a batch call that registers nothing: qb200_get_stage_ms and qb200_get_kernel_ms report zeros after it.
+ * The params array and the output descriptor are copied by the call. */
+typedef struct qb200_feature_out {
+  int32_t cap_per_scan;  /* >= 1: keypoints reserved per scan in every array below */
+  int32_t kind;          /* qb200_mem_kind of the three arrays (QB200_MEM_DEVICE: the handle's device; vox4 / normals4 16-byte,
+                            desc33 4-byte aligned) */
+  float* vox4;           /* [n][cap][4] voxel centroids in the order qb200_voxelize / qb200_cache_read return, or NULL */
+  float* normals4;       /* [n][cap][4] {nx,ny,nz,curvature}, or NULL */
+  float* desc33;         /* [n][cap][33] pcl::FPFHSignature33 rows, or NULL */
+  int32_t* counts;       /* host [n]: voxel points of scan i, never clipped */
+  int32_t* status;       /* host [n]: that scan's own front-end status */
+} qb200_feature_out;
+int qb200_describe_batch_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
+                              const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out);
+/* qb200_describe_batch_each, queued: completed by qb200_register_batch_flush like every enqueue, in one stream with raw, cached,
+ * caller-feature and correspondence-set batches and cache writes.  Host-kind scans and every output array (counts and status
+ * included) must stay valid until the flush returns, which completes them.  The outputs are byte-identical to the blocking call's. */
+int qb200_describe_batch_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
+                                      const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out);
 
 /* --- multi-GPU: batches of independent pairs shard across the GPUs of one box; the only communication is ONE all-gather (NCCL over
  * NVLink) of the fixed-size result records per batch -- north_star / SURVEY.md 8(e).  The reference has no counterpart (it is a

@@ -110,6 +110,15 @@ class PreprocessOut(C.Structure):
 PREPROCESS_ARRAYS = ("ground4", "nonground4", "valid4", "outlier4")   # in the order of the four counts
 
 
+class FeatureOut(C.Structure):
+    """qb200_feature_out: caller-owned outputs of qb200_describe_batch_each, cap_per_scan keypoints reserved per scan."""
+    _fields_ = [("cap_per_scan", C.c_int32), ("kind", C.c_int32), ("vox4", C.c_void_p), ("normals4", C.c_void_p), ("desc33", C.c_void_p),
+                ("counts", C.c_void_p), ("status", C.c_void_p)]
+
+
+FEATURE_ARRAYS = {"vox4": 4, "normals4": 4, "desc33": 33}   # output array -> floats per keypoint
+
+
 # list name -> (element dtype, trailing shape, count field of the record)
 LIST_LAYOUT = {
     "corr": (np.int32, (2,), "n_corr"),
@@ -248,6 +257,8 @@ _SIGNATURES = {
     "qb200_cache_scans_enqueue_each": (i32, [vp, P(vp), P(i32), P(i32), i32, P(Params), i32]),
     "qb200_register_features_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_register_features_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_describe_batch_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
+    "qb200_describe_batch_enqueue_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -778,6 +789,54 @@ class Handle:
         (params_array()) are read by the call; host-kind scans must stay alive until register_batch_flush."""
         return self._check(self.lib.qb200_cache_scans_enqueue_each(self.h, scan_ptrs, counts, slot_ids, n, params_array, kind),
                            "qb200_cache_scans_enqueue_each")
+
+    # ---- raw scans -> voxel keypoints, normals and FPFH-33 (the front end in batches) ----
+    def feature_buffers(self, n: int, cap: int, dest: int = MEM_HOST, arrays=tuple(FEATURE_ARRAYS)) -> dict:
+        """Zeroed output arrays of a describe call by name: numpy (dest MEM_HOST) or CUDA tensors of the handle's device (MEM_DEVICE),
+        each of shape (n, cap, floats per keypoint)."""
+        shape = lambda k: (max(n, 1), cap, FEATURE_ARRAYS[k])
+        if dest == MEM_HOST:
+            return {k: np.zeros(shape(k), np.float32) for k in arrays}
+        import torch
+        return {k: torch.zeros(shape(k), dtype=torch.float32, device=f"cuda:{self.cfg.device}") for k in arrays}
+
+    @staticmethod
+    def feature_out(cap: int, dest: int, arrays: dict, counts: np.ndarray, status: np.ndarray) -> FeatureOut:
+        """The qb200_feature_out of `arrays` (feature_buffers()) and the host int32 arrays counts / status; a name left out is NULL."""
+        out = FeatureOut(cap, dest)
+        for k, a in arrays.items():
+            setattr(out, k, a.ctypes.data if dest == MEM_HOST else a.data_ptr())
+        out.counts, out.status = counts.ctypes.data, status.ctypes.data
+        return out
+
+    def describe_batch_each(self, scans: Sequence, params: Sequence[Params], kind: int = MEM_HOST, dest: int = MEM_HOST,
+                            cap_per_scan: Optional[int] = None, arrays: Optional[dict] = None):
+        """qb200_describe_batch_each: scan i (an (n,4) float32 array for MEM_HOST, a (device_ptr, n) tuple for MEM_DEVICE) is voxelized
+        and described with the front-end fields of params[i].  cap_per_scan: keypoints reserved per scan (default max_voxel_points).
+        arrays: the caller's own outputs by name (FEATURE_ARRAYS), numpy for dest MEM_HOST or CUDA tensors for MEM_DEVICE, each of
+        shape (n, cap, 4 or 33); a name left out is NULL.  Returns (per scan a tuple (vox4, normals4, desc33) trimmed to
+        min(count, cap): numpy copies, tensor views on the device, None for a NULL array; counts (n,) int32; status (n,) int32)."""
+        n = len(scans)
+        assert len(params) == n
+        cap = cap_per_scan or self.cfg.max_voxel_points
+        arrays = self.feature_buffers(n, cap, dest) if arrays is None else arrays
+        counts, status = np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.int32)
+        ptrs, cnts, keep = _scan_arrays(scans, kind)
+        out = self.feature_out(cap, dest, arrays, counts, status)
+        self._check(self.lib.qb200_describe_batch_each(self.h, ptrs, cnts, n, self.params_array(params), kind, C.byref(out)),
+                    "qb200_describe_batch_each")
+        per_scan = []
+        for i in range(n):
+            m = min(int(counts[i]), cap)
+            per_scan.append(tuple(None if k not in arrays else (arrays[k][i, :m].copy() if dest == MEM_HOST else arrays[k][i, :m])
+                                  for k in FEATURE_ARRAYS))
+        return per_scan, counts[:n], status[:n]
+
+    def describe_batch_enqueue_each_raw(self, scan_ptrs, counts, n: int, params_array, kind: int, out: FeatureOut):
+        """qb200_describe_batch_enqueue_each: scan_ptrs / counts (_scan_arrays()), params_array (params_array()) and the descriptor `out`
+        (feature_out()) are read by the call; host-kind scans and every array `out` names must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_describe_batch_enqueue_each(self.h, scan_ptrs, counts, n, params_array, kind, C.byref(out)),
+                           "qb200_describe_batch_enqueue_each")
 
     def last_features(self, which: int, cap: Optional[int] = None):
         """(normals (n,4), descriptors (n,33)) of the source (0) / target (1) cloud of the last match_and_pack."""

@@ -449,10 +449,13 @@ struct BatchCall {
   const qb200_pair_lists* lists = nullptr;
   // (each) the entries may differ in their front-end fields too (the _mixed forms); otherwise those are bit-identical in every entry
   bool mixed = false;
-  // a cache write: scan i (n_points[i] points in `kind` memory) is voxelized and described with its entry into slot slot_ids[i]
+  // a cache write: scan i (n_points[i] points in `kind` memory) is voxelized and described with its entry into slot slot_ids[i];
+  // a describe call (describe, no slot_ids): the same front end, into the caller's arrays of *out
   const float* const* scans = nullptr;
   const int32_t* n_points = nullptr;
   const int32_t* slot_ids = nullptr;
+  bool describe = false;
+  const qb200_feature_out* out = nullptr;
   // caller features: pair i's keypoints and FPFH-33 rows, matched and solved with its own entry (front-end fields ignored)
   const qb200_feature_pair* feats = nullptr;
   // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved, laid out like `caller`.
@@ -509,6 +512,70 @@ void deliver_lists(Lane* L, const qb200_pair_lists& l, int w0, int np) {
   }
 }
 
+// The lane's staging block as a describe wave's destination (base == nullptr: only its size): counts and status of the 2S clouds, and
+// in host kind min(cap_per_scan, V) entries per cloud of every array the caller asked for
+size_t export_stage(const Lane* L, const qb200_feature_out& o, unsigned char* base, ExportDst* d) {
+  qb200_feature_out staged = o;
+  if (o.kind == QB200_MEM_DEVICE) staged.vox4 = staged.normals4 = staged.desc33 = nullptr;  // counts and status only
+  return ExportDst::carve(base, 2 * L->S, o.cap_per_scan < L->V ? o.cap_per_scan : L->V, staged, d);
+}
+
+// Enqueue the export of a describe wave (scans [w0, w0 + ncl) of lane L): its counts and status into the lane's staging block, its
+// entries straight into the caller's device arrays or into that block, from where wave_collect hands them on (deliver_export).  The
+// lane's previous wave has been collected, so a block that must grow is not in use.
+int submit_export(Lane* L, const qb200_feature_out& o, int w0, int ncl) {
+  ExportDst d;
+  const size_t bytes = export_stage(L, o, nullptr, &d);
+  if (L->exp_bytes < bytes) {
+    PinnedMem<unsigned char> m;
+    QB_CUDA_TRY(L, m.alloc(bytes));
+    L->exp_stage = std::move(m);
+    L->exp_bytes = bytes;
+  }
+  export_stage(L, o, L->exp_stage, &d);
+  if (o.kind == QB200_MEM_DEVICE) {
+    const ExportDst to = ExportDst::caller(o, w0);
+    d.vox = to.vox; d.nrm = to.nrm; d.desc = to.desc; d.stride = to.stride; d.cap = to.cap;
+  }
+  const ExportSrc s{L->vox_pts, L->normals, L->desc_t, L->ctr.n_vox, L->ctr.cloud_status};
+  return launch_feature_export(L, ncl, s, d, L->V);
+}
+
+// a collected describe wave's counts and status, and in host kind its entries, from the lane's staging block to the caller
+void deliver_export(Lane* L, const qb200_feature_out& o, int w0, int ncl) {
+  ExportDst st;
+  export_stage(L, o, L->exp_stage, &st);
+  memcpy(o.counts + w0, st.counts, (size_t)ncl * sizeof(int));
+  memcpy(o.status + w0, st.status, (size_t)ncl * sizeof(int));
+  if (o.kind == QB200_MEM_DEVICE) return;
+  const ExportDst to = ExportDst::caller(o, w0);
+  for (int c = 0; c < ncl; ++c) {
+    const int m = st.counts[c] < st.cap ? st.counts[c] : st.cap;
+    if (m <= 0) continue;
+    const size_t d0 = (size_t)c * to.stride, s0 = (size_t)c * st.stride;
+    if (to.vox) memcpy(to.vox + d0, st.vox + s0, (size_t)m * sizeof(float4));
+    if (to.nrm) memcpy(to.nrm + d0, st.nrm + s0, (size_t)m * sizeof(float4));
+    if (to.desc) memcpy(to.desc + d0 * kDescDim, st.desc + s0 * kDescDim, (size_t)m * kDescDim * sizeof(float));
+  }
+}
+
+// An output descriptor of a describe call: capacity and kinds in range, counts and status present, device arrays on the handle's
+// device and aligned for the export's stores
+int check_out(qb200_handle* h, const qb200_feature_out* o) {
+  const char* why = nullptr;
+  if (!o) why = "the output descriptor is null";
+  else if (o->cap_per_scan < 1) why = "cap_per_scan < 1";
+  else if (!o->counts || !o->status) why = "the counts or status array is null";
+  else if (o->kind != QB200_MEM_HOST && o->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the outputs";
+  else if (o->kind == QB200_MEM_DEVICE && !device_array_of(h, o->vox4, 16)) why = "device vox4 is misaligned or not memory of the handle's device";
+  else if (o->kind == QB200_MEM_DEVICE && !device_array_of(h, o->normals4, 16))
+    why = "device normals4 is misaligned or not memory of the handle's device";
+  else if (o->kind == QB200_MEM_DEVICE && !device_array_of(h, o->desc33, 4)) why = "device desc33 is misaligned or not memory of the handle's device";
+  if (!why) return QB200_OK;
+  h->fail(__FILE__, __LINE__, why);
+  return QB200_ERR_BAD_ARG;
+}
+
 // A list descriptor from the caller: capacity and kind in range, device arrays on the handle's device and aligned for the pack's
 // vector stores; for_sets: the caller supplied the correspondences, so there are none to hand back.
 int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
@@ -530,7 +597,8 @@ int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
 // Enqueue one wave (pairs [w0, w0 + np), np <= S) on lane L: the front of the wave its input needs (raw scans: H2D, K1..K6;
 // cached scans: the copy out of the cache, K6; caller features: their H2D and import, K6; correspondence sets: their H2D), then
 // K8..K11 and the D2H of the result records.
-// A cache write's wave is scans [w0, w0 + np), np <= 2S: their H2D, K1..K5 and the copy into their slots, with no records.
+// A cache write's wave is scans [w0, w0 + np), np <= 2S: their H2D, K1..K5 and the copy into their slots, with no records; a describe
+// wave is the same with the export to the caller's arrays in place of the copy.
 // No sync: wave_collect hands the records out to in.results[w0...].  The lane's previous wave must have been collected.
 int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   const bool raw = in.pairs || in.scans;
@@ -560,7 +628,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       if (in.scans) {
         L->h_cloud_ptr[s] = reinterpret_cast<const float4*>(in.scans[w0 + s]);
         L->h_cloud_n[s] = in.n_points[w0 + s];
-        L->h_slot_of_cloud[s] = in.slot_ids[w0 + s];
+        if (in.slot_ids) L->h_slot_of_cloud[s] = in.slot_ids[w0 + s];
         continue;
       }
       const qb200_pair& pr = in.pairs[w0 + s];
@@ -619,7 +687,9 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     }
     QB_CUDA_TRY(L, cudaMemcpyAsync(L->ctr.n_corr, L->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, L->stream));
   }
-  if (in.scans) {
+  if (in.out) {
+    if ((rc = submit_export(L, *in.out, w0, ncl))) return rc;
+  } else if (in.scans) {
     if ((rc = cache_waits(h, L, ncl, true))) return rc;
     if ((rc = cache_copy(h, L, 1, ncl))) return rc;
     QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_out, L->stream));
@@ -635,9 +705,11 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   }
   L->pend_w0 = w0;
   L->pend_np = np;
-  L->pend_dst = in.results;  // nullptr for a cache write: no records
+  L->pend_dst = in.results;  // nullptr for a cache write or a describe call: no records
   if (in.lists) L->pend_lists = *in.lists;
   else L->pend_lists.cap_per_pair = 0;
+  if (in.out) L->pend_out = *in.out;
+  else L->pend_out.cap_per_scan = 0;
   // stage-time slots of qb200_get_stage_ms this wave reports: raw scans all eight, caller features h2d and match to d2h, the other
   // inputs their first stage to pose, a cache write none (it registers nothing)
   L->pend_stages = in.pairs ? 0xFFu : in.feats ? 0xF9u : in.slots ? 0x7Cu : in.sets ? 0x70u : 0u;
@@ -655,6 +727,7 @@ int wave_collect(qb200_handle* h, Lane* L) {
   }
   if (L->pend_dst) memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
   if (L->pend_lists.cap_per_pair > 0 && L->pend_lists.kind == QB200_MEM_HOST) deliver_lists(L, L->pend_lists, L->pend_w0, np);
+  if (L->pend_out.cap_per_scan > 0) deliver_export(L, L->pend_out, L->pend_w0, np);
   if (h->timeline && (L->pend_stages & 1u)) {  // stage boundaries of a raw-scan or feature wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
     fprintf(stderr, "[qb200 timeline] wave w0=%d np=%d:", L->pend_w0, np);
     for (int i = 0; i < 9; ++i) {
@@ -744,7 +817,7 @@ int check_call(qb200_handle* h, const BatchCall& c) {
   };
   if (c.n < 0) return reject("n < 0");
   if (c.n > 0 && !c.pairs && !c.slots && !c.sets && !c.scans && !c.feats) return reject("the input array is null");
-  if (c.n > 0 && c.scans && (!c.n_points || !c.slot_ids)) return reject("the n_points or slot_ids array is null");
+  if (c.n > 0 && c.scans && (!c.n_points || (!c.describe && !c.slot_ids))) return reject("the n_points or slot_ids array is null");
   if (c.n > 0 && !c.scans && !c.results) return reject("the results array is null");
   if (c.kind != QB200_MEM_HOST && c.kind != QB200_MEM_DEVICE) return reject("unknown memory kind of the inputs");
   const qb200_params* p = c.caller;
@@ -760,6 +833,8 @@ int check_call(qb200_handle* h, const BatchCall& c) {
     }
   }
   if (int rc = check_lists(h, c.lists, c.sets != nullptr)) return rc;
+  if (c.describe)
+    if (int rc = check_out(h, c.out)) return rc;
   const int R = h->cfg.max_raw_points;
   for (int i = 0; i < c.n; ++i) {
     if (c.pairs) {
@@ -796,6 +871,15 @@ int check_call(qb200_handle* h, const BatchCall& c) {
     } else if (c.sets) {
       const qb200_corr_set& s = c.sets[i];
       if (s.L < 0 || s.L > h->cfg.max_corr || (s.L > 0 && (!s.a || !s.b))) return reject("correspondence set is null or exceeds max_corr");
+    } else if (c.describe) {
+      const int np = c.n_points[i];
+      const char* bad = nullptr;
+      if (np < 0 || np > R) bad = "its point count is outside 0 .. max_raw_points";
+      else if (np > 0 && !c.scans[i]) bad = "it is null";
+      if (bad) {
+        snprintf(why, sizeof(why), "scan %d: %s", i, bad);
+        return reject(why);
+      }
     } else {
       const int sl = c.slot_ids[i], np = c.n_points[i];
       if (sl < 0 || sl >= h->c_slots || np < 0 || np > R || (np > 0 && !c.scans[i])) {
@@ -878,7 +962,7 @@ int enqueue_call(qb200_handle* h, BatchCall c) {
   h->lanes_active = n_lanes;
   // a cache write's signatures, in scan order (a slot named twice ends with its last scan's): the checks of the calls queued after it
   // see them
-  for (int i = 0; c.scans && i < c.n; ++i) {
+  for (int i = 0; c.slot_ids && i < c.n; ++i) {
     const qb200_params& pc = c.params[c.each ? i : 0];
     float* sig = h->c_sig.get() + 4 * (size_t)c.slot_ids[i];
     sig[0] = pc.voxel_size; sig[1] = pc.normal_radius; sig[2] = pc.fpfh_radius; sig[3] = lattice_cell(pc);
@@ -911,6 +995,15 @@ BatchCall cache_write(const float* const* scans4, const int32_t* n_points, const
   BatchCall c;
   c.n = n_scans; c.kind = kind; c.caller = p; c.each = each; c.mixed = true;
   c.scans = scans4; c.n_points = n_points; c.slot_ids = slot_ids;
+  return c;
+}
+
+// qb200_describe_batch_each and qb200_describe_batch_enqueue_each as a batch call: a cache write whose scans go to *out, not to slots
+BatchCall describe_call(const float* const* scans4, const int32_t* n_points, int32_t n_scans, const qb200_params* params, qb200_mem_kind kind,
+                        const qb200_feature_out* out) {
+  BatchCall c = cache_write(scans4, n_points, nullptr, n_scans, params, true, kind);
+  c.describe = true;
+  c.out = out;
   return c;
 }
 
@@ -1171,6 +1264,17 @@ int qb200_register_features_enqueue_each(qb200_handle* h, const qb200_feature_pa
   return enqueue_call(h, feature_call(pairs, n_pairs, params, kind, results, lists));
 }
 
+// ---- raw scans -> voxel keypoints, normals and FPFH-33 in caller memory ---------------------------------------------------------
+int qb200_describe_batch_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans, const qb200_params* params,
+                              qb200_mem_kind kind, const qb200_feature_out* out) {
+  return run_call(h, describe_call(scans4, n_points, n_scans, params, kind, out));
+}
+
+int qb200_describe_batch_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
+                                      const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out) {
+  return enqueue_call(h, describe_call(scans4, n_points, n_scans, params, kind, out));
+}
+
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {
   if (int rc = enter(h)) return rc;
   if (from_slot < 0 || to_slot < 0 || from_slot >= h->c_slots || to_slot >= h->c_slots) return QB200_ERR_BAD_ARG;
@@ -1201,7 +1305,7 @@ int qb200_cache_read(qb200_handle* h, int32_t slot, float* vox4, float* normals4
     if (vox4) QB_CUDA_TRY(h, cudaMemcpyAsync(vox4, h->c_vox + slot * V, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
     if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, h->c_nrm + slot * V, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
     if (desc33) {
-      desc_to_aos_rows(L, h->c_desc + slot * kDescK * V, m, L->aos_scratch);
+      if (int rc = export_desc_rows(L, h->c_desc + slot * kDescK * V, h->c_n + slot, m)) return rc;
       QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, L->aos_scratch, (size_t)m * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
     }
     QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));

@@ -661,12 +661,40 @@ __global__ void __launch_bounds__(kNbrThreads) fpfh_rare_kernel(const float4* __
   for (int b = 22; b < 33; ++b) out[(size_t)b * V] = o[b] * g2;
 }
 
-// dimension-major descriptors -> pcl::FPFHSignature33 rows (qb200_compute_fpfh, qb200_get_last_features, qb200_cache_read)
-__global__ void desc_to_aos_kernel(const float* __restrict__ desc_t, int V, int n, float* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n * kDescDim) return;
-  const int q = i / kDescDim, d = i % kDescDim;
-  out[i] = desc_t[(size_t)d * V + q];
+constexpr int kExportTile = 128, kExportThreads = 256;
+
+// Front-end results -> their destinations: cloud c's first m = min(n, cap) voxel points and normals, and its descriptors turned from
+// the dimension-major rows of desc_t (or a cache slot) into m rows of 33 floats (pcl::FPFHSignature33).  One launch serves a whole
+// describe wave (qb200_describe_batch_each) or the one cloud of qb200_compute_fpfh, qb200_get_last_features and qb200_cache_read.
+// One CTA per tile of kExportTile points of a cloud: every dimension's row segment is read coalesced into shared memory (row stride 33
+// floats: the transposed stores are free of bank conflicts), and the tile's output rows, one contiguous run of m * 132 bytes, are
+// written coalesced from there.  A pure copy: every value arrives bit for bit.
+__global__ void __launch_bounds__(kExportThreads) feature_export_kernel(ExportSrc s, int V, ExportDst d) {
+  __shared__ float tile[kExportTile * kDescDim];
+  const int cloud = blockIdx.y, q0 = blockIdx.x * kExportTile, tid = threadIdx.x;
+  const int st = s.status ? s.status[cloud] : QB200_OK;
+  const int n = st == QB200_OK ? s.n[cloud] : 0;  // a refused cloud reports 0 and gets nothing
+  if (blockIdx.x == 0 && tid == 0) {
+    if (d.counts) d.counts[cloud] = n;
+    if (d.status) d.status[cloud] = st;
+  }
+  const int m_all = min(n, d.cap);
+  if (q0 >= m_all) return;
+  const int m = min(kExportTile, m_all - q0);
+  const size_t from = (size_t)cloud * V + q0, to = (size_t)cloud * d.stride + q0;
+  for (int i = tid; i < m; i += kExportThreads) {
+    if (d.vox) d.vox[to + i] = __ldg(s.vox + from + i);
+    if (d.nrm) d.nrm[to + i] = __ldg(s.nrm + from + i);
+  }
+  if (!d.desc) return;
+  const float* __restrict__ col = s.desc + (size_t)cloud * kDescK * V + q0;
+  for (int i = tid; i < kDescDim * kExportTile; i += kExportThreads) {
+    const int dim = i / kExportTile, q = i % kExportTile;
+    if (q < m) tile[q * kDescDim + dim] = __ldg(col + (size_t)dim * V + q);
+  }
+  __syncthreads();
+  float* __restrict__ out = d.desc + to * kDescDim;
+  for (int i = tid; i < m * kDescDim; i += kExportThreads) out[i] = tile[i];
 }
 
 constexpr int kImportTile = 128, kImportThreads = 256;
@@ -770,20 +798,51 @@ int launch_fpfh(Lane* h, int n_clouds) {
   return QB200_OK;
 }
 
-int launch_desc_to_aos(Lane* h, int cloud, int n, float* d_out33) {
-  if (n <= 0) return QB200_OK;
-  desc_to_aos_kernel<<<(n * kDescDim + 255) / 256, 256, 0, h->stream>>>(h->desc_t + (size_t)cloud * kDescK * h->V, h->V, n, d_out33);
+int launch_feature_export(Lane* h, int n_clouds, const ExportSrc& src, const ExportDst& dst, int max_n) {
+  if (n_clouds <= 0) return QB200_OK;
+  const int m = max_n < dst.cap ? max_n : dst.cap;
+  const dim3 g(((m > 1 ? m : 1) + kExportTile - 1) / kExportTile, n_clouds);  // at least one tile: its first CTA reports the cloud
+  feature_export_kernel<<<g, kExportThreads, 0, h->stream>>>(src, h->V, dst);
   h->launches++;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;
 }
-// any dimension-major descriptor block [40][V] (e.g. a cache slot) -> AoS n x 33
-int desc_to_aos_rows(Lane* h, const float* desc_rows, int n, float* d_out33) {
-  if (n <= 0) return QB200_OK;
-  desc_to_aos_kernel<<<(n * kDescDim + 255) / 256, 256, 0, h->stream>>>(desc_rows, h->V, n, d_out33);
-  h->launches++;
-  QB_CUDA_TRY(h, cudaGetLastError());
-  return QB200_OK;
+
+int export_desc_rows(Lane* h, const float* desc, const int* n, int m) {
+  ExportSrc s{nullptr, nullptr, desc, n, nullptr};
+  ExportDst d{nullptr, nullptr, h->aos_scratch, m, m, nullptr, nullptr};
+  return launch_feature_export(h, 1, s, d, m);
+}
+
+ExportDst ExportDst::caller(const qb200_feature_out& o, long long first) {
+  const long long c = o.cap_per_scan;
+  ExportDst d;
+  d.vox = o.vox4 ? reinterpret_cast<float4*>(o.vox4) + first * c : nullptr;
+  d.nrm = o.normals4 ? reinterpret_cast<float4*>(o.normals4) + first * c : nullptr;
+  d.desc = o.desc33 ? o.desc33 + first * c * kDescDim : nullptr;
+  d.stride = c;
+  d.cap = o.cap_per_scan;
+  d.counts = d.status = nullptr;
+  return d;
+}
+
+size_t ExportDst::carve(unsigned char* base, int n, int cap, const qb200_feature_out& o, ExportDst* d) {
+  const size_t k = (size_t)n * cap;
+  size_t off = 0;
+  auto take = [&](size_t bytes, bool want) -> unsigned char* {
+    if (!want) return nullptr;
+    unsigned char* p = base ? base + off : nullptr;
+    off += (bytes + 15) & ~(size_t)15;
+    return p;
+  };
+  d->counts = reinterpret_cast<int*>(take((size_t)n * sizeof(int), true));
+  d->status = reinterpret_cast<int*>(take((size_t)n * sizeof(int), true));
+  d->vox = reinterpret_cast<float4*>(take(k * sizeof(float4), o.vox4));
+  d->nrm = reinterpret_cast<float4*>(take(k * sizeof(float4), o.normals4));
+  d->desc = reinterpret_cast<float*>(take(k * kDescDim * sizeof(float), o.desc33));
+  d->stride = cap;
+  d->cap = cap;
+  return off;
 }
 int launch_feature_import(Lane* h, int n_clouds) {
   if (n_clouds <= 0) return QB200_OK;

@@ -62,6 +62,34 @@ struct FeatureSrc {
   int n, pad;
 };
 
+// What feature_export_kernel reads (frontend.cu): cloud c's voxel points, normals and dimension-major descriptors at c * V points
+// (c * kDescK * V floats) past these pointers, and its count; status == nullptr: every cloud is written, else only the clouds whose
+// front-end status is QB200_OK
+struct ExportSrc {
+  const float4* vox;
+  const float4* nrm;
+  const float* desc;
+  const int* n;
+  const int* status;
+};
+
+// Where feature_export_kernel writes cloud c: c * stride keypoints past each array (nullptr = not asked for), at most cap of them; and,
+// when counts / status are set, its reported count and status (a refused cloud: count 0, nothing written)
+struct ExportDst {
+  float4* vox;
+  float4* nrm;
+  float* desc;
+  long long stride;
+  int cap;
+  int* counts;
+  int* status;
+  // the caller's arrays of qb200_feature_out from scan `first` on
+  static ExportDst caller(const qb200_feature_out& o, long long first);
+  // the requested arrays of o, placed in a staging block of n clouds of `cap` keypoints each (base == nullptr: only the size), with
+  // counts and status behind them
+  static size_t carve(unsigned char* base, int n, int cap, const qb200_feature_out& o, ExportDst* out);
+};
+
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
 // kernels of the others.  The lane owns its stream, buffers and events: deleting it releases them.
@@ -95,6 +123,9 @@ struct Lane {
   // copies after those events (api.cu: cache_waits)
   std::vector<int> pend_slots;
   int pend_writes;
+  // ... and (a describe wave: pend_out.cap_per_scan > 0) a copy of its batch's output descriptor, whose counts and status (and, in
+  // host kind, entries) wave_collect hands on from exp_stage
+  qb200_feature_out pend_out;
   Event ev_cache_in, ev_cache_out;
 
   // ---- sort workspace (voxel sort, then lattice sort) ----
@@ -156,6 +187,9 @@ struct Lane {
   PinnedMem<qb200_result> h_results; // [S]
   PinnedMem<unsigned char> lst_stage; int lst_cap;  // host-kind pair lists, grown on first use: [S][lst_cap] entries of every list
                                                     // (ListDst::carve), written by pack_lists_kernel through the mapped address
+  PinnedMem<unsigned char> exp_stage; size_t exp_bytes;  // a describe wave's counts and status, and in host kind its entries
+                                                         // (ExportDst::carve over 2S clouds), written by feature_export_kernel through
+                                                         // the mapped address; grown on first use
   WaveCounters ctr, hctr;     // the counter block, and the same layout over its pinned mirror (stage calls read it back whole)
   DeviceMem<int> ctr_block; PinnedMem<int> hctr_block; size_t ctr_ints;
 
@@ -286,13 +320,16 @@ int launch_match_nn(Lane* h, int n_pairs);
 int launch_match_exact(Lane* h, int n_pairs, const int* only);
 int launch_tc_debug_tile(Lane* h, float* d_out);
 int tc_footprint(Lane* h, int* out5);
-int launch_desc_to_aos(Lane* h, int cloud, int n, float* d_out33);
+// Clouds [0, n_clouds) of src to dst in one launch: keypoints, normals and 33-float descriptor rows (pcl::FPFHSignature33) of each
+// cloud's first min(n, dst.cap) points.  max_n: a host bound of the entries any cloud writes (the launch's tile count).
+int launch_feature_export(Lane* h, int n_clouds, const ExportSrc& src, const ExportDst& dst, int max_n);
+// the first min(*n, m) descriptor rows of one cloud (its dimension-major block desc, its count at the device address n) into aos_scratch
+int export_desc_rows(Lane* h, const float* desc, const int* n, int m);
 // Feature waves (api.cu: stage_features, frontend.cu): h_feat[0, n) holds every cloud's caller pointers and count.  stage_features
 // copies host-kind inputs into the staging areas (inputs back to back in the caller's memory as one copy) and uploads the table, on
 // stream cs; launch_feature_import then fills vox_pts, desc_t and n_vox on the lane's stream (after wave_reset).
 int stage_features(Lane* L, int n_clouds, qb200_mem_kind kind, cudaStream_t cs);
 int launch_feature_import(Lane* h, int n_clouds);
-int desc_to_aos_rows(Lane* h, const float* desc_rows, int n, float* d_out33);
 size_t sort_temp_bytes(int max_items);
 void comm_release(qb200_handle* h);
 int collect_batch(qb200_handle* h, const qb200_result* dst);  // api.cu: wait for every wave in flight that writes into dst[...]

@@ -108,7 +108,7 @@ int qb200_compute_fpfh(qb200_handle* h, const float* pts4, int32_t n, float norm
   if ((rc = write_counter(L, L->hctr.n_vox, n)) || (rc = upload_front(L, 1)) || (rc = launch_fpfh(L, 1))) return rc;
   if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, L->normals, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
   if (desc33) {
-    if ((rc = launch_desc_to_aos(L, 0, n, L->aos_scratch))) return rc;
+    if ((rc = export_desc_rows(L, L->desc_t, L->ctr.n_vox, n))) return rc;
     QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, L->aos_scratch, (size_t)n * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
   }
   QB_CUDA_TRY(h, hold.sync());
@@ -348,7 +348,7 @@ int qb200_get_last_features(qb200_handle* h, int32_t which, float* normals4, flo
   if (m > 0) {
     if (normals4) QB_CUDA_TRY(h, cudaMemcpyAsync(normals4, L->normals + (size_t)which * L->V, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
     if (desc33) {
-      if (int rc = launch_desc_to_aos(L, which, m, L->aos_scratch)) return rc;
+      if (int rc = export_desc_rows(L, L->desc_t + (size_t)which * kDescK * L->V, L->ctr.n_vox + which, m)) return rc;
       QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, L->aos_scratch, (size_t)m * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
     }
     QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
