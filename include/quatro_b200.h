@@ -27,6 +27,8 @@
  *                                  of caller keypoints and FPFH-33 descriptors (include/fpfh_manager.hpp:125-127)
  *   qb200_describe_batch_*      <- voxelize<T>() + FPFHEstimation::computeFPFHFeatures + FPFHManager::getObjDescriptor /
  *                                  getTgtNormals for every scan of a batch (include/fpfh_manager.hpp:161-177)
+ *   qb200_describe_points_*     <- FPFHEstimation::computeFPFHFeatures for every caller keypoint cloud of a batch
+ *                                  (src/teaser_utils/fpfh.cc:44-75)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -371,7 +373,8 @@ int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_
  * every queued batch must stay valid until a flush (or qb200_register_batch, = enqueue + flush) returns.  Other entry points flush
  * implicitly.  Raw, cached, caller-feature and correspondence-set batches (qb200_register_cached_enqueue_mixed,
  * qb200_register_features_enqueue_each, qb200_solve_batch_enqueue_each), scan-cache writes (qb200_cache_scans_enqueue_each) and describe
- * calls (qb200_describe_batch_enqueue_each) may be queued in one stream and completed by a single flush; every access to a
+ * calls (qb200_describe_batch_enqueue_each, qb200_describe_points_enqueue_each) may be queued in one stream and completed by a single
+ * flush; every access to a
  * cache slot follows enqueue order, so a queued cached batch registers the slot contents it was enqueued against.  qb200_cache_reserve,
  * qb200_cache_copy, qb200_cache_read and the pre-processing calls flush first, so they see every write queued before them. */
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
@@ -594,6 +597,39 @@ int qb200_describe_batch_each(qb200_handle* h, const float* const* scans4, const
  * included) must stay valid until the flush returns, which completes them.  The outputs are byte-identical to the blocking call's. */
 int qb200_describe_batch_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
                                       const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out);
+
+/* --- FPFH of caller keypoint clouds in batches: normals and FPFH-33 of many clouds, without the voxel filter ------------------------
+ * FPFHEstimation::computeFPFHFeatures (src/teaser_utils/fpfh.cc:44-75) takes whatever cloud it is handed; this call does the same for a
+ * batch of clouds whose keypoints the caller chose: a PCL VoxelGrid run elsewhere, uniform or random sampling, a keypoint detector,
+ * a map database that stores keypoints but not descriptors, or the same keypoints described again at other radii.  The output goes
+ * straight into the caller's arrays, and qb200_register_features_each of any handle takes it back with the caller's keypoints.
+ *   Cloud i (pts4[i]: n_points[i] x {x,y,z,w} in `kind` memory) gets normals and FPFH-33 computed with the lattice fields of params[i]:
+ *     normal_radius, fpfh_radius and grid_cell (<= 0 resolves, as everywhere else, to (1 + 2^-9) fpfh_radius).  Every other field is
+ *     ignored.  The points are taken in the caller's order, as they are: no voxel filter, no dropping of w < 0, no merging of
+ *     duplicates.
+ *   normals4[i] and desc33[i] are byte-identical to qb200_compute_fpfh on that cloud alone with the resolved radii and cell, clouds
+ *     with points the lattice drops (non-finite, outside the lattice) and coincident duplicates included.  They never depend on the
+ *     batch, the wave, the lane, the memory kinds or the other clouds.
+ *   The output descriptor is qb200_feature_out, with vox4 NULL (the keypoints are the caller's own).  counts[i] = n_points[i] and
+ *     status[i] = QB200_OK, since every refusal is decided for the whole call.  cap_per_scan and the clipping behave as in
+ *     qb200_describe_batch_each: cloud i's entries start at i * cap_per_scan, min(n_points[i], cap_per_scan) of them are written.
+ *   Checks run before anything starts or is queued.  QB200_ERR_BAD_ARG for n_points[i] < 0 or > max_voxel_points (the rule of
+ *     qb200_compute_fpfh and qb200_register_features_each), a NULL cloud with n_points[i] > 0, in QB200_MEM_DEVICE kind a cloud that
+ *     is not memory of the handle's device or not 16-byte aligned, a params entry whose radii are not finite and positive, whose
+ *     normal_radius exceeds its fpfh_radius or whose grid_cell is not finite, a non-NULL vox4, and the output checks of
+ *     qb200_describe_batch_each (cap_per_scan >= 1, counts and status, output kind, device arrays and their alignment).  A rejected
+ *     call writes no count, status or entry, queues nothing, and qb200_last_error names the bad cloud, entry or array; batches already
+ *     queued still complete on the flush.
+ *   The clouds run in waves of 2 * max_batch_slots over the lanes, as describe calls do.  Like them it registers nothing:
+ *     qb200_get_stage_ms and qb200_get_kernel_ms report zeros after it.
+ * The params array and the output descriptor are copied by the call. */
+int qb200_describe_points_each(qb200_handle* h, const float* const* pts4, const int32_t* n_points, int32_t n_clouds,
+                               const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out);
+/* qb200_describe_points_each, queued: completed by qb200_register_batch_flush like every enqueue, in one stream with every other
+ * enqueue form.  Host-kind clouds and every output array (counts and status included) must stay valid until the flush returns,
+ * which completes them.  The outputs are byte-identical to the blocking call's. */
+int qb200_describe_points_enqueue_each(qb200_handle* h, const float* const* pts4, const int32_t* n_points, int32_t n_clouds,
+                                       const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out);
 
 /* --- multi-GPU: batches of independent pairs shard across the GPUs of one box; the only communication is ONE all-gather (NCCL over
  * NVLink) of the fixed-size result records per batch -- north_star / SURVEY.md 8(e).  The reference has no counterpart (it is a

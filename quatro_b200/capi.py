@@ -111,12 +111,14 @@ PREPROCESS_ARRAYS = ("ground4", "nonground4", "valid4", "outlier4")   # in the o
 
 
 class FeatureOut(C.Structure):
-    """qb200_feature_out: caller-owned outputs of qb200_describe_batch_each, cap_per_scan keypoints reserved per scan."""
+    """qb200_feature_out: caller-owned outputs of qb200_describe_batch_each and qb200_describe_points_each, cap_per_scan keypoints
+    reserved per scan or cloud."""
     _fields_ = [("cap_per_scan", C.c_int32), ("kind", C.c_int32), ("vox4", C.c_void_p), ("normals4", C.c_void_p), ("desc33", C.c_void_p),
                 ("counts", C.c_void_p), ("status", C.c_void_p)]
 
 
 FEATURE_ARRAYS = {"vox4": 4, "normals4": 4, "desc33": 33}   # output array -> floats per keypoint
+POINT_ARRAYS = ("normals4", "desc33")   # what qb200_describe_points_each can return (the keypoints are the caller's own)
 
 
 # list name -> (element dtype, trailing shape, count field of the record)
@@ -259,6 +261,8 @@ _SIGNATURES = {
     "qb200_register_features_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_describe_batch_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
     "qb200_describe_batch_enqueue_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
+    "qb200_describe_points_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
+    "qb200_describe_points_enqueue_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -837,6 +841,37 @@ class Handle:
         (feature_out()) are read by the call; host-kind scans and every array `out` names must stay alive until register_batch_flush."""
         return self._check(self.lib.qb200_describe_batch_enqueue_each(self.h, scan_ptrs, counts, n, params_array, kind, C.byref(out)),
                            "qb200_describe_batch_enqueue_each")
+
+    # ---- caller keypoint clouds -> normals and FPFH-33 (FPFH without the voxel filter, in batches) ----
+    def describe_points_each(self, clouds: Sequence, params: Sequence[Params], kind: int = MEM_HOST, dest: int = MEM_HOST,
+                             cap_per_scan: Optional[int] = None, arrays: Optional[dict] = None):
+        """qb200_describe_points_each: cloud i (an (n,4) float32 array for MEM_HOST, a (device_ptr, n) tuple for MEM_DEVICE) is described
+        as it is with the lattice fields of params[i].  cap_per_scan: keypoints reserved per cloud (default max_voxel_points).  arrays:
+        the caller's own normals4 / desc33 outputs by name, numpy for dest MEM_HOST or CUDA tensors for MEM_DEVICE, each of shape
+        (n, cap, 4 or 33); a name left out is NULL.  Returns (per cloud a tuple (normals4, desc33) trimmed to min(count, cap): numpy
+        copies, tensor views on the device, None for a NULL array; counts (n,) int32; status (n,) int32)."""
+        n = len(clouds)
+        assert len(params) == n
+        cap = cap_per_scan or self.cfg.max_voxel_points
+        arrays = self.feature_buffers(n, cap, dest, POINT_ARRAYS) if arrays is None else arrays
+        counts, status = np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.int32)
+        ptrs, cnts, keep = _scan_arrays(clouds, kind)
+        out = self.feature_out(cap, dest, arrays, counts, status)
+        self._check(self.lib.qb200_describe_points_each(self.h, ptrs, cnts, n, self.params_array(params), kind, C.byref(out)),
+                    "qb200_describe_points_each")
+        per_cloud = []
+        for i in range(n):
+            m = min(int(counts[i]), cap)
+            per_cloud.append(tuple(None if k not in arrays else (arrays[k][i, :m].copy() if dest == MEM_HOST else arrays[k][i, :m])
+                                   for k in POINT_ARRAYS))
+        return per_cloud, counts[:n], status[:n]
+
+    def describe_points_enqueue_each_raw(self, cloud_ptrs, counts, n: int, params_array, kind: int, out: FeatureOut):
+        """qb200_describe_points_enqueue_each: cloud_ptrs / counts (_scan_arrays()), params_array (params_array()) and the descriptor
+        `out` (feature_out(), without vox4) are read by the call; host-kind clouds and every array `out` names must stay alive until
+        register_batch_flush."""
+        return self._check(self.lib.qb200_describe_points_enqueue_each(self.h, cloud_ptrs, counts, n, params_array, kind, C.byref(out)),
+                           "qb200_describe_points_enqueue_each")
 
     def last_features(self, which: int, cap: Optional[int] = None):
         """(normals (n,4), descriptors (n,33)) of the source (0) / target (1) cloud of the last match_and_pack."""

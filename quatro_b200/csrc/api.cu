@@ -1,5 +1,6 @@
 // api.cu -- the C-ABI of include/quatro_b200.h: handle lifetime, lanes, waves, pair lists, the scan cache and the batch entry
 // points.  The single-pair stage entry points, the qb200_get_last_* getters and the debug hooks are in stages.cu.
+#include <cmath>
 #include <new>
 #include <stddef.h>
 #include <stdio.h>
@@ -227,10 +228,17 @@ bool params_ok(const qb200_params* p) {
 // neighbour within +-1 even after the float rounding of x / cell, so the walk covers 27 cells instead of 125
 float lattice_cell(const qb200_params& p) { return p.grid_cell > 0 ? p.grid_cell : p.fpfh_radius * 1.001953125f; }
 
-CloudFront front_entry(const qb200_params& p) {
+// The lattice fields of an entry of qb200_describe_points_each, the only ones it reads: finite positive radii, normal_radius <=
+// fpfh_radius (fpfh_manager.hpp:99-102), a finite grid_cell and a finite resolved cell
+bool lattice_ok(const qb200_params& p) {
+  return std::isfinite(p.normal_radius) && std::isfinite(p.fpfh_radius) && p.normal_radius > 0 && p.fpfh_radius > 0 &&
+         p.normal_radius <= p.fpfh_radius && std::isfinite(p.grid_cell) && std::isfinite(lattice_cell(p));
+}
+
+CloudFront front_entry(const qb200_params& p, bool lattice_only) {
   CloudFront e;
   memset(&e, 0, sizeof(e));
-  front_voxel(&e, p.voxel_size, p.skip_flagged);
+  if (!lattice_only) front_voxel(&e, p.voxel_size, p.skip_flagged);
   front_lattice(&e, p.normal_radius, p.fpfh_radius, lattice_cell(p));
   return e;
 }
@@ -368,8 +376,10 @@ int stage_features(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs) {
         if (int rc = add(0, f.pts, pts, (size_t)f.n * sizeof(float4))) return rc;
         f.pts = pts;
       }
-      if (int rc = add(1, f.desc, desc, (size_t)f.n * kDescDim * sizeof(float))) return rc;
-      f.desc = desc;
+      if (f.desc) {  // (a describe-points wave stages keypoints only)
+        if (int rc = add(1, f.desc, desc, (size_t)f.n * kDescDim * sizeof(float))) return rc;
+        f.desc = desc;
+      }
       off += f.n;
     }
     for (int k = 0; k < 2; ++k)
@@ -450,11 +460,12 @@ struct BatchCall {
   // (each) the entries may differ in their front-end fields too (the _mixed forms); otherwise those are bit-identical in every entry
   bool mixed = false;
   // a cache write: scan i (n_points[i] points in `kind` memory) is voxelized and described with its entry into slot slot_ids[i];
-  // a describe call (describe, no slot_ids): the same front end, into the caller's arrays of *out
+  // a describe call (describe, no slot_ids): the same front end, into the caller's arrays of *out; a describe-points call (points
+  // too): scan i is the caller's keypoint cloud, imported as it is and described with the lattice fields of its entry
   const float* const* scans = nullptr;
   const int32_t* n_points = nullptr;
   const int32_t* slot_ids = nullptr;
-  bool describe = false;
+  bool describe = false, points = false;
   const qb200_feature_out* out = nullptr;
   // caller features: pair i's keypoints and FPFH-33 rows, matched and solved with its own entry (front-end fields ignored)
   const qb200_feature_pair* feats = nullptr;
@@ -560,10 +571,11 @@ void deliver_export(Lane* L, const qb200_feature_out& o, int w0, int ncl) {
 }
 
 // An output descriptor of a describe call: capacity and kinds in range, counts and status present, device arrays on the handle's
-// device and aligned for the export's stores
-int check_out(qb200_handle* h, const qb200_feature_out* o) {
+// device and aligned for the export's stores; points: no vox4 (the keypoints are the caller's own)
+int check_out(qb200_handle* h, const qb200_feature_out* o, bool points) {
   const char* why = nullptr;
   if (!o) why = "the output descriptor is null";
+  else if (points && o->vox4) why = "vox4 must be null: the keypoints are the caller's own";
   else if (o->cap_per_scan < 1) why = "cap_per_scan < 1";
   else if (!o->counts || !o->status) why = "the counts or status array is null";
   else if (o->kind != QB200_MEM_HOST && o->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the outputs";
@@ -598,10 +610,11 @@ int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
 // cached scans: the copy out of the cache, K6; caller features: their H2D and import, K6; correspondence sets: their H2D), then
 // K8..K11 and the D2H of the result records.
 // A cache write's wave is scans [w0, w0 + np), np <= 2S: their H2D, K1..K5 and the copy into their slots, with no records; a describe
-// wave is the same with the export to the caller's arrays in place of the copy.
+// wave is the same with the export to the caller's arrays in place of the copy, and a describe-points wave imports its keypoint
+// clouds as a feature wave does (without descriptors) in place of the H2D and K1.
 // No sync: wave_collect hands the records out to in.results[w0...].  The lane's previous wave must have been collected.
 int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
-  const bool raw = in.pairs || in.scans;
+  const bool raw = in.pairs || (in.scans && !in.points);
   const int ncl = in.scans ? np : 2 * np;
   int rc;
   L->kev_armed[0] = L->kev_armed[1] = 0;
@@ -614,14 +627,14 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     const bool own = in.each || s == 0;
     const qb200_params& p = in.params[in.each ? w0 + s : 0];
     if (in.scans) {
-      L->h_front[s] = own ? front_entry(p) : L->h_front[0];
+      L->h_front[s] = own ? front_entry(p, in.points) : L->h_front[0];
       continue;
     }
     L->h_solve[s] = own ? solve_entry(p) : L->h_solve[0];
     if (in.pairs) L->h_front[2 * s] = L->h_front[2 * s + 1] = own ? front_entry(p) : L->h_front[0];
   }
   if (!in.scans && (rc = upload_solve(L, np))) return rc;
-  if (raw && (rc = upload_front(L, ncl))) return rc;
+  if ((raw || in.points) && (rc = upload_front(L, ncl))) return rc;
   if (raw) {
     cudaEventRecord(L->ev[0], L->stream);
     for (int s = 0; s < np; ++s) {
@@ -648,9 +661,13 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     cudaEventRecord(L->ev[2], L->stream);
     if ((rc = launch_fpfh(L, ncl))) return rc;
     cudaEventRecord(L->ev[3], L->stream);
-  } else if (in.feats) {
+  } else if (in.feats || in.points) {
     cudaEventRecord(L->ev[0], L->stream);
     for (int s = 0; s < np; ++s) {
+      if (in.points) {  // keypoints without descriptors: K2..K5 describe them below
+        L->h_feat[s] = {reinterpret_cast<const float4*>(in.scans[w0 + s]), nullptr, in.n_points[w0 + s], 0};
+        continue;
+      }
       const qb200_feature_pair& f = in.feats[w0 + s];
       L->h_feat[2 * s] = {reinterpret_cast<const float4*>(f.src), f.src_desc, f.n_src, 0};
       L->h_feat[2 * s + 1] = {reinterpret_cast<const float4*>(f.tgt), f.tgt_desc, f.n_tgt, 0};
@@ -662,7 +679,9 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, h->ev_copied, 0));
     }
     if ((rc = launch_feature_import(L, ncl))) return rc;
-    for (int i = 1; i <= 3; ++i) cudaEventRecord(L->ev[i], L->stream);  // no voxel or FPFH stage: slots 1 and 2 are not reported
+    for (int i = 1; i <= 2; ++i) cudaEventRecord(L->ev[i], L->stream);  // no voxel stage: slot 1 is not reported
+    if (in.points && (rc = launch_fpfh(L, ncl))) return rc;
+    cudaEventRecord(L->ev[3], L->stream);  // no FPFH stage in a feature wave: slot 2 is not reported either
   } else if (in.slots) {
     for (int s = 0; s < np; ++s) {
       L->h_slot_of_cloud[2 * s] = in.slots[w0 + s].src_slot;
@@ -822,7 +841,16 @@ int check_call(qb200_handle* h, const BatchCall& c) {
   if (c.kind != QB200_MEM_HOST && c.kind != QB200_MEM_DEVICE) return reject("unknown memory kind of the inputs");
   const qb200_params* p = c.caller;
   char why[192];
-  if (int rc = check_params(h, p, c.n, c.each, !c.sets && !c.mixed)) return rc;
+  if (c.points) {  // only the lattice fields are read
+    for (int i = 0; i < c.n; ++i) {
+      if (!p || !lattice_ok(p[i])) {
+        snprintf(why, sizeof(why), "params entry %d is null or its radii or lattice cell are out of range", i);
+        return reject(why);
+      }
+    }
+  } else if (int rc = check_params(h, p, c.n, c.each, !c.sets && !c.mixed)) {
+    return rc;
+  }
   for (int i = 0; !c.sets && !c.scans && i < (c.each ? c.n : 1); ++i) {
     if (!p[i].use_crosscheck) {
       if (c.each) {
@@ -834,7 +862,7 @@ int check_call(qb200_handle* h, const BatchCall& c) {
   }
   if (int rc = check_lists(h, c.lists, c.sets != nullptr)) return rc;
   if (c.describe)
-    if (int rc = check_out(h, c.out)) return rc;
+    if (int rc = check_out(h, c.out, c.points)) return rc;
   const int R = h->cfg.max_raw_points;
   for (int i = 0; i < c.n; ++i) {
     if (c.pairs) {
@@ -871,6 +899,17 @@ int check_call(qb200_handle* h, const BatchCall& c) {
     } else if (c.sets) {
       const qb200_corr_set& s = c.sets[i];
       if (s.L < 0 || s.L > h->cfg.max_corr || (s.L > 0 && (!s.a || !s.b))) return reject("correspondence set is null or exceeds max_corr");
+    } else if (c.points) {
+      const int np = c.n_points[i];
+      const char* bad = nullptr;
+      if (np < 0 || np > h->cfg.max_voxel_points) bad = "its point count is outside 0 .. max_voxel_points";
+      else if (np > 0 && !c.scans[i]) bad = "it is null";
+      else if (np > 0 && c.kind == QB200_MEM_DEVICE && !device_array_of(h, c.scans[i], 16))
+        bad = "it is misaligned (16 bytes) or not memory of the handle's device";
+      if (bad) {
+        snprintf(why, sizeof(why), "cloud %d: %s", i, bad);
+        return reject(why);
+      }
     } else if (c.describe) {
       const int np = c.n_points[i];
       const char* bad = nullptr;
@@ -1004,6 +1043,14 @@ BatchCall describe_call(const float* const* scans4, const int32_t* n_points, int
   BatchCall c = cache_write(scans4, n_points, nullptr, n_scans, params, true, kind);
   c.describe = true;
   c.out = out;
+  return c;
+}
+
+// qb200_describe_points_each and qb200_describe_points_enqueue_each as a batch call: a describe call whose clouds are keypoints
+BatchCall describe_points_call(const float* const* pts4, const int32_t* n_points, int32_t n_clouds, const qb200_params* params,
+                               qb200_mem_kind kind, const qb200_feature_out* out) {
+  BatchCall c = describe_call(pts4, n_points, n_clouds, params, kind, out);
+  c.points = true;
   return c;
 }
 
@@ -1273,6 +1320,17 @@ int qb200_describe_batch_each(qb200_handle* h, const float* const* scans4, const
 int qb200_describe_batch_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
                                       const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out) {
   return enqueue_call(h, describe_call(scans4, n_points, n_scans, params, kind, out));
+}
+
+// ---- caller keypoint clouds -> normals and FPFH-33 in caller memory -------------------------------------------------------------
+int qb200_describe_points_each(qb200_handle* h, const float* const* pts4, const int32_t* n_points, int32_t n_clouds, const qb200_params* params,
+                               qb200_mem_kind kind, const qb200_feature_out* out) {
+  return run_call(h, describe_points_call(pts4, n_points, n_clouds, params, kind, out));
+}
+
+int qb200_describe_points_enqueue_each(qb200_handle* h, const float* const* pts4, const int32_t* n_points, int32_t n_clouds,
+                                       const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out) {
+  return enqueue_call(h, describe_points_call(pts4, n_points, n_clouds, params, kind, out));
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

@@ -703,7 +703,8 @@ constexpr int kImportTile = 128, kImportThreads = 256;
 // (pcl::FPFHSignature33) into the 33 dimension-major rows of desc_t, and n into n_vox.  One CTA per tile of kImportTile points of a
 // cloud: the tile's AoS rows are one contiguous run of kImportTile * 132 bytes, read coalesced into shared memory, and every
 // dimension-major row segment is written coalesced from there (row stride 33 floats: the column reads are free of bank conflicts).
-// A pure copy: every value, NaN payloads included, arrives bit for bit.
+// A pure copy: every value, NaN payloads included, arrives bit for bit.  A cloud without descriptors (a keypoint wave of
+// qb200_describe_points_each, which K2..K5 describe next) imports its keypoints and count only.
 __global__ void __launch_bounds__(kImportThreads) feature_import_kernel(const FeatureSrc* __restrict__ table, int V, float4* __restrict__ vox_pts,
                                                                         float* __restrict__ desc_t, int* __restrict__ n_vox) {
   __shared__ float tile[kImportTile * kDescDim];
@@ -714,6 +715,7 @@ __global__ void __launch_bounds__(kImportThreads) feature_import_kernel(const Fe
   const int m = min(kImportTile, f.n - q0);
   if (f.pts)  // (qb200_debug_tc_distances imports descriptors only)
     for (int i = tid; i < m; i += kImportThreads) vox_pts[(size_t)cloud * V + q0 + i] = __ldg(f.pts + q0 + i);
+  if (!f.desc) return;  // the same for every thread of the CTA: no thread waits at the barrier below
   const float* __restrict__ src = f.desc + (size_t)q0 * kDescDim;
   for (int i = tid; i < m * kDescDim; i += kImportThreads) tile[i] = __ldg(src + i);
   __syncthreads();

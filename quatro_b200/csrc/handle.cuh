@@ -55,7 +55,7 @@ struct CloudFront {
 struct PpScan;   // one scan's pre-processing entry (preprocess.cu)
 
 // Where feature_import_kernel reads one cloud of a feature wave (frontend.cu): n keypoints and n FPFH-33 rows, in the caller's
-// device memory or in the lane's staging areas
+// device memory or in the lane's staging areas; desc == nullptr: keypoints only (a describe-points wave, described by K2..K5)
 struct FeatureSrc {
   const float4* pts;
   const float* desc;
@@ -139,7 +139,8 @@ struct Lane {
   DeviceMem<float4> vox_pts;  // [2S*V] centroids, ascending (k,j,i)
   DeviceMem<uint64_t> cell_key; // [2S*V] occupied lattice cells, ascending
   DeviceMem<int> cell_start;  // [2S*(V+1)]
-  DeviceMem<float4> normals;  // [2S*V]; a feature wave stages host keypoints here (packed, [sum n])
+  DeviceMem<float4> normals;  // [2S*V]; a feature or describe-points wave stages host keypoints here (packed, [sum n]), and the
+                              // import has read them before K3 writes the normals
   DeviceMem<float> spfh;      // [2S*V*36] rows padded to 36 floats; a feature wave stages host descriptors here (packed, [sum n][33])
   DeviceMem<uint32_t> nbr_list; // [2S][kNbrGlobalCap][V] fpfh_radius neighbour indices found by K2c (lattice order), read by K3..K5
   DeviceMem<int> nbr_cnt;     // [2S*V] neighbour count (self included); > kNbrGlobalCap: K5 walks the lattice itself
@@ -278,10 +279,10 @@ int launch_fpfh(Lane* h, int n_clouds);
 // keep_w: the matched points keep their keypoints' w (caller keypoints of a feature wave); otherwise w = 1
 int launch_match(Lane* h, int n_pairs, int keep_w);
 // a cloud's front-end entry: its voxel fields (frontend.cu), its lattice fields for these radii and this lattice cell (frontend.cu),
-// or both from p (api.cu)
+// or both (lattice_only: the lattice fields alone, the voxel fields zero) from p (api.cu)
 void front_voxel(CloudFront* e, float leaf, int skip_flagged);
 void front_lattice(CloudFront* e, float normal_radius, float fpfh_radius, float cell);
-CloudFront front_entry(const qb200_params& p);
+CloudFront front_entry(const qb200_params& p, bool lattice_only = false);
 // the entries [0, n) of h_front to d_front on the lane's stream: one copy (h_front must stay as it is until the stream passed it)
 int upload_front(Lane* h, int n);
 void match_fields(PairSolve* e, const qb200_params& p);  // K7's fields of a pair's entry (match.cu)
