@@ -29,6 +29,8 @@
  *                                  getTgtNormals for every scan of a batch (include/fpfh_manager.hpp:161-177)
  *   qb200_describe_points_*     <- FPFHEstimation::computeFPFHFeatures for every caller keypoint cloud of a batch
  *                                  (src/teaser_utils/fpfh.cc:44-75)
+ *   qb200_match_*               <- FPFHManager::setFeaturePair + getCorrespondences / getSrcMatched / getTgtMatched for every pair
+ *                                  of a batch, without the solve (include/fpfh_manager.hpp:98-153, 234-236)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -373,8 +375,8 @@ int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_
  * every queued batch must stay valid until a flush (or qb200_register_batch, = enqueue + flush) returns.  Other entry points flush
  * implicitly.  Raw, cached, caller-feature and correspondence-set batches (qb200_register_cached_enqueue_mixed,
  * qb200_register_features_enqueue_each, qb200_solve_batch_enqueue_each), scan-cache writes (qb200_cache_scans_enqueue_each) and describe
- * calls (qb200_describe_batch_enqueue_each, qb200_describe_points_enqueue_each) may be queued in one stream and completed by a single
- * flush; every access to a
+ * calls (qb200_describe_batch_enqueue_each, qb200_describe_points_enqueue_each) and match calls (qb200_match_*_enqueue_*) may be queued
+ * in one stream and completed by a single flush; every access to a
  * cache slot follows enqueue order, so a queued cached batch registers the slot contents it was enqueued against.  qb200_cache_reserve,
  * qb200_cache_copy, qb200_cache_read and the pre-processing calls flush first, so they see every write queued before them. */
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
@@ -556,6 +558,50 @@ int qb200_register_features_each(qb200_handle* h, const qb200_feature_pair* pair
  * the flush returns.  Records and lists are byte-identical to those of the blocking call. */
 int qb200_register_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                          qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+
+/* --- matching in batches: correspondences and matched points of many pairs, not solved -------------------------------------------
+ * FPFHManager::setFeaturePair followed by getCorrespondences / getSrcMatched / getTgtMatched (include/fpfh_manager.hpp:98-153,
+ * 234-236) for every pair of a batch: what a caller needs who picks the pairs worth solving from n_mutual / n_corr (a loop-closure
+ * pre-filter), hands the correspondences to another estimator, solves one match under several solver settings, or fills a cache of
+ * matched pairs.  Each call takes the arguments of its register counterpart and honours the same per-pair fields:
+ *   qb200_match_batch_mixed / _enqueue_mixed     raw pairs, as qb200_register_batch_mixed: front-end and matcher fields
+ *   qb200_match_cached_mixed / _enqueue_mixed    slot pairs, as qb200_register_cached_mixed: matcher fields, and the entry must match
+ *                                                the front-end signature of both slots
+ *   qb200_match_features_each / _enqueue_each    caller features, as qb200_register_features_each: matcher fields
+ * Contract:
+ *   Lists.  Only corr, src_matched4 and tgt_matched4 may be non-NULL; a clique, final-inlier or mask array gives QB200_ERR_BAD_ARG.
+ *     lists == NULL gives the records only.  Pair i's corr, src_matched4 and tgt_matched4 are byte-identical to the lists of the
+ *     register counterpart on the same inputs and params; they never depend on the batch, the wave, the lane, the memory kinds or the
+ *     other pairs.
+ *   Records.  status, n_src_vox, n_tgt_vox, n_mutual, n_corr and the matcher's flags (with QB200_FLAG_LISTS_TRUNCATED) equal the register
+ *     counterpart's.  Nothing is solved: valid = 0, T is the identity, and max_core, clique_size, gnc_iters, n_rot_inliers,
+ *     n_final_inliers, n_edges and cost are 0.
+ *   Status.  QB200_DEGENERATE_INPUT for an empty side, QB200_CAPACITY_EXCEEDED for more voxels or correspondences than the handle
+ *     holds, or the front-end status the register counterpart gives the pair.  Every other pair is QB200_OK, one with 0 or 1
+ *     correspondences included: the caller has its list and decides.
+ *   Params.  The solver fields (noise_bound .. RyRx) are ignored and not checked.  The front-end and matcher fields pass the checks of
+ *     the register counterpart, and use_crosscheck = 0 gives QB200_ERR_UNSUPPORTED.  Nothing is latched: entries with
+ *     rot_noise_bound == 0 stay unresolved, so a match followed by qb200_solve_batch_each latches as the register call would.
+ *   Rejections cover the whole call and are decided before anything is queued: no record or list entry is written, qb200_last_error
+ *     names the bad pair, entry or array, and the batches already queued still complete on the flush.
+ *   The queued forms share the stream and the single flush of every other enqueue form; a queued cached match sees the slot contents
+ *     it was enqueued against.  Host-kind inputs, `results` and the list arrays must stay valid until the flush returns.
+ *   qb200_get_stage_ms reports the stages that ran: h2d, voxel and fpfh as the input has them, match and d2h; graph, clique and pose
+ *     are 0.
+ * The params array and the list descriptor are copied by the call.  src_matched4 + i * cap_per_pair * 4 with L = n_corr is pair i's
+ * qb200_corr_set for qb200_solve_batch_each, device arrays included. */
+int qb200_match_batch_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
+                            qb200_result* results, const qb200_pair_lists* lists);
+int qb200_match_batch_enqueue_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
+                                    qb200_result* results, const qb200_pair_lists* lists);
+int qb200_match_cached_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_result* results,
+                             const qb200_pair_lists* lists);
+int qb200_match_cached_enqueue_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                     qb200_result* results, const qb200_pair_lists* lists);
+int qb200_match_features_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                              qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+int qb200_match_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                      qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
 
 /* --- the front end in batches: voxel keypoints, normals and FPFH-33 of many scans into caller memory ----------------------------------
  * voxelize<T> (include/quatro.hpp:49-57) + FPFHEstimation::computeFPFHFeatures (src/teaser_utils/fpfh.cc:44-75), handed out as

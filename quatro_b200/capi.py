@@ -132,6 +132,7 @@ LIST_LAYOUT = {
     "trans_inlier_mask": (np.uint8, (), "clique_size"),
 }
 SET_LISTS = ("clique", "final_inliers", "rot_inlier_mask", "trans_inlier_mask")   # what qb200_solve_batch_ex can return
+MATCH_LISTS = ("corr", "src_matched4", "tgt_matched4")   # what the qb200_match_* calls can return
 
 
 class ListBuffers:
@@ -263,6 +264,12 @@ _SIGNATURES = {
     "qb200_describe_batch_enqueue_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
     "qb200_describe_points_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
     "qb200_describe_points_enqueue_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
+    "qb200_match_batch_mixed": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_match_batch_enqueue_mixed": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_match_cached_mixed": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
+    "qb200_match_cached_enqueue_mixed": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
+    "qb200_match_features_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_match_features_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -787,6 +794,58 @@ class Handle:
         its host arrays, `out` and the buffers must stay alive until register_batch_flush."""
         return self._check(self.lib.qb200_register_features_enqueue_each(self.h, feature_array, n, params_array, kind, _ptr(out),
                                                                          self._lists_arg(buffers)), "qb200_register_features_enqueue_each")
+
+    # ---- raw, cached or caller-feature pairs -> correspondences and matched points, not solved (the qb200_match_* calls) ----
+    # buffers: a ListBuffers of MATCH_LISTS only, or None for records only.  Each returns (records, lists) like the register forms.
+    @staticmethod
+    def _match_lists(buffers: Optional[ListBuffers]) -> Optional[ListBuffers]:
+        assert buffers is None or set(buffers.arrays) <= set(MATCH_LISTS), "a match call returns corr and the matched points only"
+        return buffers
+
+    def match_batch_mixed(self, pairs: Sequence, params: Sequence[Params], kind: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
+        """qb200_match_batch_mixed: pair i is voxelized, described and matched with params[i] (solver fields ignored)."""
+        assert len(params) == len(pairs)
+        arr, keep = self.pair_array(pairs, kind)
+        return self._batch_lists("qb200_match_batch_mixed", len(pairs), (arr, len(pairs), self.params_array(params), kind),
+                                 self._match_lists(buffers))
+
+    def match_batch_enqueue_mixed_raw(self, pair_array, n: int, params_array, kind: int, out: np.ndarray,
+                                      buffers: Optional[ListBuffers] = None):
+        """qb200_match_batch_enqueue_mixed: params_array (params_array()) is copied by the call; pair_array, its scans, `out` and the
+        buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_match_batch_enqueue_mixed(self.h, pair_array, n, params_array, kind, _ptr(out),
+                                                                    self._lists_arg(self._match_lists(buffers))),
+                           "qb200_match_batch_enqueue_mixed")
+
+    def match_cached_mixed(self, slot_pairs, params: Sequence[Params], buffers: Optional[ListBuffers] = None):
+        """qb200_match_cached_mixed: slot pair i is matched with params[i], whose front-end fields must be the ones both of its slots
+        were cached with."""
+        sp = _slot_array(slot_pairs)
+        assert len(params) == len(sp)
+        return self._batch_lists("qb200_match_cached_mixed", len(sp), (_ptr(sp), len(sp), self.params_array(params)), self._match_lists(buffers))
+
+    def match_cached_enqueue_mixed_raw(self, slot_array, n: int, params_array, out: np.ndarray, buffers: Optional[ListBuffers] = None):
+        """qb200_match_cached_enqueue_mixed: params_array (params_array()) is copied by the call; slot_array (_slot_array()), `out` and
+        the buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_match_cached_enqueue_mixed(self.h, _ptr(slot_array), n, params_array, _ptr(out),
+                                                                     self._lists_arg(self._match_lists(buffers))),
+                           "qb200_match_cached_enqueue_mixed")
+
+    def match_features_each(self, pairs: Sequence, params: Sequence[Params], kind: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
+        """qb200_match_features_each: pair i's keypoints and descriptors (feature_array()) are matched with params[i]; corr indexes the
+        caller's keypoints."""
+        assert len(params) == len(pairs)
+        arr, keep = self.feature_array(pairs, kind)
+        return self._batch_lists("qb200_match_features_each", len(pairs), (arr, len(pairs), self.params_array(params), kind),
+                                 self._match_lists(buffers))
+
+    def match_features_enqueue_each_raw(self, feature_array, n: int, params_array, kind: int, out: np.ndarray,
+                                        buffers: Optional[ListBuffers] = None):
+        """qb200_match_features_enqueue_each: params_array (params_array()) is copied by the call; feature_array (feature_array()), its
+        host arrays, `out` and the buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_match_features_enqueue_each(self.h, feature_array, n, params_array, kind, _ptr(out),
+                                                                      self._lists_arg(self._match_lists(buffers))),
+                           "qb200_match_features_enqueue_each")
 
     def cache_scans_enqueue_each_raw(self, scan_ptrs, counts, slot_ids, n: int, params_array, kind: int):
         """qb200_cache_scans_enqueue_each: scan_ptrs / counts (_scan_arrays()), slot_ids (c_int32 * n) and params_array

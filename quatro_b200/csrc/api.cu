@@ -213,14 +213,16 @@ int wave_reset(Lane* L, int n_clouds) {
   return QB200_OK;
 }
 
-bool params_ok(const qb200_params* p) {
+bool params_ok(const qb200_params* p, bool solver) {
   if (!p) return false;
   if (!(p->voxel_size > 0) || !(p->normal_radius > 0) || !(p->fpfh_radius > 0)) return false;
   if (p->normal_radius > p->fpfh_radius) return false;  // FPFHManager::setFeaturePair throws here, fpfh_manager.hpp:99-102
+  if (p->tuple_trials_per_corr < 0) return false;
+  if (!solver) return true;
   if (!(p->noise_bound > 0) || !(p->cbar2 > 0) || !(p->cote_noise_bound > 0)) return false;
   if (p->cote_mode != QB200_COTE_MEDIAN && p->cote_mode != QB200_COTE_WEIGHTED_MEAN) return false;  // quatro.hpp:911
   if (p->inlier_selection_mode < 0 || p->inlier_selection_mode > 3 || p->max_clique_node_limit < 0) return false;
-  if (p->rotation_max_iterations < 0 || p->tuple_trials_per_corr < 0) return false;
+  if (p->rotation_max_iterations < 0) return false;
   return true;
 }
 
@@ -260,6 +262,14 @@ void set_last(qb200_handle* h, const qb200_result& r) {
   h->last_n_corr = r.n_corr;
   h->last_n_clique = r.clique_size;
   h->last_n_final = r.n_final_inliers;
+}
+
+// a match wave's entry: the matcher fields of p (K7's tuple test), nothing of the solver
+PairSolve match_entry(const qb200_params& p) {
+  PairSolve e;
+  memset(&e, 0, sizeof(e));
+  match_fields(&e, p);
+  return e;
 }
 
 PairSolve solve_entry(const qb200_params& p) {
@@ -469,6 +479,9 @@ struct BatchCall {
   const qb200_feature_out* out = nullptr;
   // caller features: pair i's keypoints and FPFH-33 rows, matched and solved with its own entry (front-end fields ignored)
   const qb200_feature_pair* feats = nullptr;
+  // a match call (pairs, slots or feats): every wave runs its front end and the matcher, then writes the matcher's records and the
+  // correspondence lists without solving; the solver fields of the entries are neither checked nor resolved
+  bool match = false;
   // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved, laid out like `caller`.
   const qb200_params* params = nullptr;
   // raw host scans of a multi-wave batch: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies queued on
@@ -589,13 +602,16 @@ int check_out(qb200_handle* h, const qb200_feature_out* o, bool points) {
 }
 
 // A list descriptor from the caller: capacity and kind in range, device arrays on the handle's device and aligned for the pack's
-// vector stores; for_sets: the caller supplied the correspondences, so there are none to hand back.
-int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
+// vector stores; for_sets: the caller supplied the correspondences, so there are none to hand back; for_match: nothing is solved, so
+// there are no clique, final inliers or masks to hand back.
+int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets, bool for_match) {
   if (!l) return QB200_OK;
   const char* why = nullptr;
   if (l->cap_per_pair < 1 || l->cap_per_pair > h->cfg.max_corr) why = "cap_per_pair outside 1 .. max_corr";
   else if (l->kind != QB200_MEM_HOST && l->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the lists";
   else if (for_sets && (l->corr || l->src_matched4 || l->tgt_matched4)) why = "a correspondence-set batch has no corr / matched points to return";
+  else if (for_match && (l->clique || l->final_inliers || l->rot_inlier_mask || l->trans_inlier_mask))
+    why = "a match call solves nothing: it has no clique, final inliers or inlier masks to return";
   else if (l->kind == QB200_MEM_DEVICE &&
            !(device_array_of(h, l->corr, 8) && device_array_of(h, l->src_matched4, 16) && device_array_of(h, l->tgt_matched4, 16) &&
              device_array_of(h, l->clique, 1) && device_array_of(h, l->final_inliers, 1) && device_array_of(h, l->rot_inlier_mask, 1) &&
@@ -608,7 +624,8 @@ int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets) {
 
 // Enqueue one wave (pairs [w0, w0 + np), np <= S) on lane L: the front of the wave its input needs (raw scans: H2D, K1..K6;
 // cached scans: the copy out of the cache, K6; caller features: their H2D and import, K6; correspondence sets: their H2D), then
-// K8..K11 and the D2H of the result records.
+// K8..K11 and the D2H of the result records.  A match wave (in.match) runs the same front and K6..K7, then match_records_kernel in
+// place of K8..K11, and hands out the records and the correspondence lists.
 // A cache write's wave is scans [w0, w0 + np), np <= 2S: their H2D, K1..K5 and the copy into their slots, with no records; a describe
 // wave is the same with the export to the caller's arrays in place of the copy, and a describe-points wave imports its keypoint
 // clouds as a feature wave does (without descriptors) in place of the H2D and K1.
@@ -630,7 +647,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       L->h_front[s] = own ? front_entry(p, in.points) : L->h_front[0];
       continue;
     }
-    L->h_solve[s] = own ? solve_entry(p) : L->h_solve[0];
+    L->h_solve[s] = own ? (in.match ? match_entry(p) : solve_entry(p)) : L->h_solve[0];
     if (in.pairs) L->h_front[2 * s] = L->h_front[2 * s + 1] = own ? front_entry(p) : L->h_front[0];
   }
   if (!in.scans && (rc = upload_solve(L, np))) return rc;
@@ -714,10 +731,15 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_out, L->stream));
   } else {
     if (!in.sets && (rc = launch_match(L, np, in.feats != nullptr))) return rc;
-    cudaEventRecord(L->ev[4], L->stream);
-    cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
-    if ((rc = run_solver(L, np, in.sets ? 0 : 1))) return rc;
-    cudaEventRecord(L->ev[7], L->stream);
+    if (in.match) {  // no solver tail: the records come from the matcher's counters, and graph, clique and pose take no time
+      if ((rc = launch_match_records(L, np))) return rc;
+      for (int i = 4; i <= 7; ++i) cudaEventRecord(L->ev[i], L->stream);
+    } else {
+      cudaEventRecord(L->ev[4], L->stream);
+      cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
+      if ((rc = run_solver(L, np, in.sets ? 0 : 1))) return rc;
+      cudaEventRecord(L->ev[7], L->stream);
+    }
     if (in.lists && (rc = submit_lists(L, *in.lists, w0, np))) return rc;
     QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
     cudaEventRecord(L->ev[8], L->stream);
@@ -730,8 +752,9 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   if (in.out) L->pend_out = *in.out;
   else L->pend_out.cap_per_scan = 0;
   // stage-time slots of qb200_get_stage_ms this wave reports: raw scans all eight, caller features h2d and match to d2h, the other
-  // inputs their first stage to pose, a cache write none (it registers nothing)
+  // inputs their first stage to pose, a cache write none (it registers nothing); a match wave the same without graph, clique and pose
   L->pend_stages = in.pairs ? 0xFFu : in.feats ? 0xF9u : in.slots ? 0x7Cu : in.sets ? 0x70u : 0u;
+  if (in.match) L->pend_stages = (L->pend_stages & 0x0Fu) | 0x80u;
   return QB200_OK;
 }
 
@@ -793,13 +816,14 @@ int batch_flush(qb200_handle* h) {
 }
 
 // The params of a call: one entry for the whole batch, or (each) one per pair (n entries; NULL is fine when n == 0).  Every entry passes
-// params_ok; same_frontend: the call runs a front end or matches cached scans with one front-end configuration (the _each forms), so
-// every entry carries the first entry's front-end fields (voxel_size .. seed, bit for bit).  A rejection names the entry.
-int check_params(qb200_handle* h, const qb200_params* p, int n, bool each, bool same_frontend) {
+// params_ok (solver: its solver fields too); same_frontend: the call runs a front end or matches cached scans with one front-end
+// configuration (the _each forms), so every entry carries the first entry's front-end fields (voxel_size .. seed, bit for bit).  A
+// rejection names the entry.
+int check_params(qb200_handle* h, const qb200_params* p, int n, bool each, bool same_frontend, bool solver) {
   const int m = each ? n : 1;
   char why[128];
   for (int i = 0; i < m; ++i) {
-    if (!params_ok(p ? p + i : nullptr)) {
+    if (!params_ok(p ? p + i : nullptr, solver)) {
       if (each) snprintf(why, sizeof(why), "params entry %d is null or out of range", i);
       h->fail(__FILE__, __LINE__, each ? why : "params are null or out of range");
       return QB200_ERR_BAD_ARG;
@@ -848,7 +872,7 @@ int check_call(qb200_handle* h, const BatchCall& c) {
         return reject(why);
       }
     }
-  } else if (int rc = check_params(h, p, c.n, c.each, !c.sets && !c.mixed)) {
+  } else if (int rc = check_params(h, p, c.n, c.each, !c.sets && !c.mixed, !c.match)) {
     return rc;
   }
   for (int i = 0; !c.sets && !c.scans && i < (c.each ? c.n : 1); ++i) {
@@ -860,7 +884,7 @@ int check_call(qb200_handle* h, const BatchCall& c) {
       return QB200_ERR_UNSUPPORTED;
     }
   }
-  if (int rc = check_lists(h, c.lists, c.sets != nullptr)) return rc;
+  if (int rc = check_lists(h, c.lists, c.sets != nullptr, c.match)) return rc;
   if (c.describe)
     if (int rc = check_out(h, c.out, c.points)) return rc;
   const int R = h->cfg.max_raw_points;
@@ -945,10 +969,11 @@ int enqueue_call(qb200_handle* h, BatchCall c) {
   // An empty call resolves no params: the reference latches the rotation noise bound inside computeTransformation, which an empty
   // batch never calls.
   if (c.n == 0) return QB200_OK;
-  // a cache write resolves nothing: only the solver reads the rotation noise bound
+  // a cache write or a match call resolves nothing: only the solver reads the rotation noise bound
   std::unique_ptr<qb200_params[]> pr;
-  if (!c.scans && !(pr = resolve_call(h, c.caller, c.n, c.each))) return QB200_ERR_CUDA;
-  c.params = c.scans ? c.caller : pr.get();
+  const bool solves = !c.scans && !c.match;
+  if (solves && !(pr = resolve_call(h, c.caller, c.n, c.each))) return QB200_ERR_CUDA;
+  c.params = solves ? pr.get() : c.caller;
   // S: inputs per wave, pairs or (a cache write) scans; the clouds of a wave fill the lane's 2 * max_batch_slots cloud buffers
   const int S = h->cfg.max_batch_slots * (c.scans ? 2 : 1), lanes = h->max_lanes;
   // raw host scans and host features cross PCIe: the copy stream and the quarter-wave opening below are theirs alone
@@ -1060,6 +1085,12 @@ BatchCall feature_call(const qb200_feature_pair* pairs, int32_t n_pairs, const q
   BatchCall c;
   c.n = n_pairs; c.kind = kind; c.caller = params; c.each = true; c.results = results; c.lists = lists; c.mixed = true;
   c.feats = pairs;
+  return c;
+}
+
+// the match form of a registering batch call: the same inputs, matched and not solved
+BatchCall match_call(BatchCall c) {
+  c.match = true;
   return c;
 }
 
@@ -1331,6 +1362,37 @@ int qb200_describe_points_each(qb200_handle* h, const float* const* pts4, const 
 int qb200_describe_points_enqueue_each(qb200_handle* h, const float* const* pts4, const int32_t* n_points, int32_t n_clouds,
                                        const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out) {
   return enqueue_call(h, describe_points_call(pts4, n_points, n_clouds, params, kind, out));
+}
+
+// ---- raw, cached or caller-feature pairs -> correspondences and matched points, not solved --------------------------------------
+int qb200_match_batch_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
+                            qb200_result* results, const qb200_pair_lists* lists) {
+  return run_call(h, match_call({pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists, true}));
+}
+
+int qb200_match_batch_enqueue_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
+                                    qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_call(h, match_call({pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists, true}));
+}
+
+int qb200_match_cached_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_result* results,
+                             const qb200_pair_lists* lists) {
+  return run_call(h, match_call({nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists, true}));
+}
+
+int qb200_match_cached_enqueue_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                     qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_call(h, match_call({nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists, true}));
+}
+
+int qb200_match_features_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                              qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return run_call(h, match_call(feature_call(pairs, n_pairs, params, kind, results, lists)));
+}
+
+int qb200_match_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                      qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_call(h, match_call(feature_call(pairs, n_pairs, params, kind, results, lists)));
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

@@ -278,6 +278,9 @@ int launch_voxel(Lane* h, int n_clouds);
 int launch_fpfh(Lane* h, int n_clouds);
 // keep_w: the matched points keep their keypoints' w (caller keypoints of a feature wave); otherwise w = 1
 int launch_match(Lane* h, int n_pairs, int keep_w);
+// A match wave's records (pairs [0, n), after launch_match), in place of the solver tail: the matcher's counters, status and flags
+// from the counter block, and the values of a pair that was not solved
+int launch_match_records(Lane* h, int n_pairs);
 // a cloud's front-end entry: its voxel fields (frontend.cu), its lattice fields for these radii and this lattice cell (frontend.cu),
 // or both (lattice_only: the lattice fields alone, the voxel fields zero) from p (api.cu)
 void front_voxel(CloudFront* e, float leaf, int skip_flagged);
@@ -341,7 +344,8 @@ bool device_array_of(const qb200_handle* h, const void* a, size_t align);
 int wave_reset(Lane* L, int n_clouds);
 int stage_raw(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs);
 int launch_degree(Lane* h, int n_pairs);
-bool params_ok(const qb200_params* p);
+// the checks every entry of a registering call passes; solver = false: the front-end and matcher fields only (a match call)
+bool params_ok(const qb200_params* p, bool solver = true);
 float lattice_cell(const qb200_params& p);
 qb200_params resolve_params(qb200_handle* h, const qb200_params& p);
 void set_last(qb200_handle* h, const qb200_result& r);

@@ -3,7 +3,8 @@
 //
 // The lists already lie in the lane's [S * Lc] buffers when the wave's pose is done; pack_lists_kernel copies each pair's live
 // prefix to its destination and marks the record when a list had to be clipped, so it runs after finalize_status_kernel and before
-// the D2H of the records (api.cu: wave_submit).  The destination is the caller's device arrays, or the lane's pinned staging block
+// the D2H of the records (api.cu: wave_submit).  In a match wave it runs after match_records_kernel instead: the clique and mask arrays
+// are absent from its ListDst and clique_size is 0, so it packs the correspondences and matched points only.  The destination is the caller's device arrays, or the lane's pinned staging block
 // written through its mapped address, so that only live entries cross PCIe; wave_collect copies them on to the caller's host arrays.
 #include "handle.cuh"
 

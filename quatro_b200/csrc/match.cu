@@ -461,6 +461,40 @@ __global__ void match_verify_kernel(const unsigned long long* __restrict__ rb_tc
   }
 }
 
+// One thread per pair of a match wave: the record a register call would hold after its matcher (fill_counters_kernel's counters,
+// finalize_status_kernel's front-end status), with the solver fields of a pair that was not solved.  An empty side is
+// QB200_DEGENERATE_INPUT; any other pair is QB200_OK, whatever its correspondence count.
+__global__ void match_records_kernel(qb200_result* __restrict__ results, int n_pairs, WaveCounters c) {
+  const int pair = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pair >= n_pairs) return;
+  qb200_result* r = results + pair;
+  const int ns = c.n_vox[2 * pair], nt = c.n_vox[2 * pair + 1];
+  const int s0 = c.cloud_status[2 * pair], s1 = c.cloud_status[2 * pair + 1];
+  r->valid = 0;
+  r->status = s0 != 0 ? s0 : s1 != 0 ? s1 : (ns <= 0 || nt <= 0) ? QB200_DEGENERATE_INPUT : QB200_OK;
+  r->n_src_vox = ns;
+  r->n_tgt_vox = nt;
+  r->n_mutual = c.n_mutual[pair];
+  r->n_corr = c.n_corr[pair];
+  r->max_core = 0;
+  r->clique_size = 0;
+  r->gnc_iters = 0;
+  r->n_rot_inliers = 0;
+  r->n_final_inliers = 0;
+  r->flags = c.flags[pair];
+  r->n_edges = 0;
+  r->cost = 0.0;
+  for (int i = 0; i < 16; ++i) r->T[i] = (i % 5 == 0) ? 1.0 : 0.0;
+}
+
+int launch_match_records(Lane* h, int n_pairs) {
+  if (n_pairs <= 0) return QB200_OK;
+  match_records_kernel<<<(n_pairs + 127) / 128, 128, 0, h->stream>>>(h->d_results, n_pairs, h->ctr);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+
 void match_fields(PairSolve* e, const qb200_params& p) {
   e->use_tuple = (p.use_tuple_test && p.tuple_scale != 0.0f) ? 1 : 0;
   e->tuple_scale = p.tuple_scale;
