@@ -498,6 +498,7 @@ __global__ void __launch_bounds__(128) normals_kernel(const float4* __restrict__
 // SPFH rows are stored as three padded thirds [11 bins, 0][11 bins, 0][11 bins, 0] (36 floats): a third is three 16-byte loads.
 constexpr int kSpfhThreads = kNbrThreads;
 static_assert(kNbrGlobalCap < 65536, "spfh_kernel<false> counts in 16 bits");
+constexpr int kSpfhRowStride = kDescPad + 1;  // floats per row staged in shared memory: odd, so a warp's row stores hit 32 banks
 __device__ __forceinline__ int spfh_slot(int b) { return b + b / 11; }
 template <bool kRare>
 __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __restrict__ pts, const float4* __restrict__ normals,
@@ -509,53 +510,72 @@ __global__ void __launch_bounds__(kSpfhThreads) spfh_kernel(const float4* __rest
   using Count = typename std::conditional<kRare, unsigned, unsigned short>::type;
   __shared__ Count cnts[kDescDim][kSpfhThreads];
   __shared__ uint32_t nbr[kRare ? kNbrCap : 1][kNbrThreads];
+  __shared__ float staged[kRare ? 1 : kSpfhThreads * kSpfhRowStride];  // kRare = false: the CTA's rows, stored together at the end
+  __shared__ bool listed[kRare ? 1 : kSpfhThreads];
   const int cloud = blockIdx.y;
-  const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= n_pts[cloud]) return;
-  int k = nbr_cnt[(size_t)cloud * V + q];
-  if ((k > kNbrGlobalCap) != kRare) return;
-  const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, front[cloud].inv_cell);
-  const float4* __restrict__ nrm = normals + (size_t)cloud * V;
-  const float4 pq = L.pts[q];
-  const float4 nq = nrm[q];
+  const int n_cloud = n_pts[cloud];
+  const int q0 = blockIdx.x * blockDim.x;
+  if (q0 >= n_cloud) return;  // the whole CTA
+  const int q = q0 + threadIdx.x;
+  int k = q < n_cloud ? nbr_cnt[(size_t)cloud * V + q] : 0;
+  const bool mine = q < n_cloud && (k > kNbrGlobalCap) == kRare;
+  if (!kRare) listed[threadIdx.x] = mine;
+  if (mine) {
+    const LatticeView L = make_view(cloud, V, pts, cell_key, cell_start, order, n_cells, front[cloud].inv_cell);
+    const float4* __restrict__ nrm = normals + (size_t)cloud * V;
+    const float4 pq = L.pts[q];
+    const float4 nq = nrm[q];
 #pragma unroll
-  for (int b = 0; b < kDescDim; ++b) cnts[b][threadIdx.x] = 0;
-  auto feature = [&](int p) {
-    if (p == q) return;
-    const float4 pp = L.pts[p];
-    const float4 np = nrm[p];
-    float f1, f2, f3;
-    if (!qb_pair_features(pq.x, pq.y, pq.z, nq.x, nq.y, nq.z, pp.x, pp.y, pp.z, np.x, np.y, np.z, &f1, &f2, &f3)) return;
-    int b1, b2, b3;
-    qb_feature_bins(f1, f2, f3, &b1, &b2, &b3);
-    cnts[b1][threadIdx.x]++;
-    cnts[11 + b2][threadIdx.x]++;
-    cnts[22 + b3][threadIdx.x]++;
-  };
-  if (!kRare) {
-    const uint32_t* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
-    for (int t = 0; t < k; ++t) feature((int)gl[(size_t)t * V]);
-  } else {
-    k = 0;
-    WalkPos pos;
-    const int m = front[cloud].mf;
-    const float r2 = front[cloud].rf2;
-    const int rows = (2 * m + 1) * (2 * m + 1);
-    while (pos.row < rows) {
-      const int n = walk_chunk(L, pq, m, r2, pos, nbr);
-      for (int t = 0; t < n; ++t) feature((int)nbr[t][threadIdx.x]);
-      k += n;
+    for (int b = 0; b < kDescDim; ++b) cnts[b][threadIdx.x] = 0;
+    auto feature = [&](int p) {
+      if (p == q) return;
+      const float4 pp = L.pts[p];
+      const float4 np = nrm[p];
+      float f1, f2, f3;
+      if (!qb_pair_features(pq.x, pq.y, pq.z, nq.x, nq.y, nq.z, pp.x, pp.y, pp.z, np.x, np.y, np.z, &f1, &f2, &f3)) return;
+      int b1, b2, b3;
+      qb_feature_bins(f1, f2, f3, &b1, &b2, &b3);
+      cnts[b1][threadIdx.x]++;
+      cnts[11 + b2][threadIdx.x]++;
+      cnts[22 + b3][threadIdx.x]++;
+    };
+    if (!kRare) {
+      const uint32_t* __restrict__ gl = nbr_list + (size_t)cloud * kNbrGlobalCap * V + q;
+      for (int t = 0; t < k; ++t) feature((int)gl[(size_t)t * V]);
+    } else {
+      k = 0;
+      WalkPos pos;
+      const int m = front[cloud].mf;
+      const float r2 = front[cloud].rf2;
+      const int rows = (2 * m + 1) * (2 * m + 1);
+      while (pos.row < rows) {
+        const int n = walk_chunk(L, pq, m, r2, pos, nbr);
+        for (int t = 0; t < n; ++t) feature((int)nbr[t][threadIdx.x]);
+        k += n;
+      }
     }
+    // three padded thirds: 16-byte gathers in K5
+    float* __restrict__ out = kRare ? spfh + ((size_t)cloud * V + q) * kDescPad : staged + threadIdx.x * kSpfhRowStride;
+    const float incr = k >= 2 ? 100.0f / (float)(k - 1) : 0.0f;
+    for (int b = 0; b < kDescDim; ++b) {
+      const int c = (int)cnts[b][threadIdx.x];  // at most the neighbour count, which fits an int
+      float v = 0.0f;
+      for (int t = 0; t < c; ++t) v += incr;
+      out[spfh_slot(b)] = v;
+    }
+    out[11] = 0.0f; out[23] = 0.0f; out[35] = 0.0f;
   }
-  float* __restrict__ out = spfh + ((size_t)cloud * V + q) * kDescPad;  // three padded thirds: 16-byte gathers in K5
-  const float incr = k >= 2 ? 100.0f / (float)(k - 1) : 0.0f;
-  for (int b = 0; b < kDescDim; ++b) {
-    const int c = (int)cnts[b][threadIdx.x];  // at most the neighbour count, which fits an int
-    float v = 0.0f;
-    for (int t = 0; t < c; ++t) v += incr;
-    out[spfh_slot(b)] = v;
+  if (kRare) return;
+  // The CTA's rows are one contiguous run of spfh.  Copied from shared memory by consecutive threads, every warp store writes 128
+  // contiguous bytes; stored by their own threads, each of a warp's 36 row stores would write 4 bytes into each of 32 rows.  Rows
+  // this launch does not own (points with more than kNbrGlobalCap neighbours, and beyond the cloud) are left alone.
+  __syncthreads();
+  const int m = min(kSpfhThreads, n_cloud - q0);
+  float* __restrict__ dst = spfh + ((size_t)cloud * V + q0) * kDescPad;
+  for (int i = threadIdx.x; i < m * kDescPad; i += kSpfhThreads) {
+    const int r = i / kDescPad;
+    if (listed[r]) dst[i] = staged[r * kSpfhRowStride + (i - r * kDescPad)];
   }
-  out[11] = 0.0f; out[23] = 0.0f; out[35] = 0.0f;
 }
 
 // K5: FPFH = per-third renormalised sum of neighbour SPFHs weighted by 1/d^2, neighbours in lattice
