@@ -879,21 +879,7 @@ class Handle:
         arrays: the caller's own outputs by name (FEATURE_ARRAYS), numpy for dest MEM_HOST or CUDA tensors for MEM_DEVICE, each of
         shape (n, cap, 4 or 33); a name left out is NULL.  Returns (per scan a tuple (vox4, normals4, desc33) trimmed to
         min(count, cap): numpy copies, tensor views on the device, None for a NULL array; counts (n,) int32; status (n,) int32)."""
-        n = len(scans)
-        assert len(params) == n
-        cap = cap_per_scan or self.cfg.max_voxel_points
-        arrays = self.feature_buffers(n, cap, dest) if arrays is None else arrays
-        counts, status = np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.int32)
-        ptrs, cnts, keep = _scan_arrays(scans, kind)
-        out = self.feature_out(cap, dest, arrays, counts, status)
-        self._check(self.lib.qb200_describe_batch_each(self.h, ptrs, cnts, n, self.params_array(params), kind, C.byref(out)),
-                    "qb200_describe_batch_each")
-        per_scan = []
-        for i in range(n):
-            m = min(int(counts[i]), cap)
-            per_scan.append(tuple(None if k not in arrays else (arrays[k][i, :m].copy() if dest == MEM_HOST else arrays[k][i, :m])
-                                  for k in FEATURE_ARRAYS))
-        return per_scan, counts[:n], status[:n]
+        return self._describe("qb200_describe_batch_each", tuple(FEATURE_ARRAYS), scans, params, kind, dest, cap_per_scan, arrays)
 
     def describe_batch_enqueue_each_raw(self, scan_ptrs, counts, n: int, params_array, kind: int, out: FeatureOut):
         """qb200_describe_batch_enqueue_each: scan_ptrs / counts (_scan_arrays()), params_array (params_array()) and the descriptor `out`
@@ -909,20 +895,23 @@ class Handle:
         the caller's own normals4 / desc33 outputs by name, numpy for dest MEM_HOST or CUDA tensors for MEM_DEVICE, each of shape
         (n, cap, 4 or 33); a name left out is NULL.  Returns (per cloud a tuple (normals4, desc33) trimmed to min(count, cap): numpy
         copies, tensor views on the device, None for a NULL array; counts (n,) int32; status (n,) int32)."""
+        return self._describe("qb200_describe_points_each", POINT_ARRAYS, clouds, params, kind, dest, cap_per_scan, arrays)
+
+    def _describe(self, fn: str, names, clouds, params, kind, dest, cap_per_scan, arrays):
+        """The two blocking describe calls: `names` = the output arrays the call can fill, in the order of the returned tuples."""
         n = len(clouds)
         assert len(params) == n
         cap = cap_per_scan or self.cfg.max_voxel_points
-        arrays = self.feature_buffers(n, cap, dest, POINT_ARRAYS) if arrays is None else arrays
+        arrays = self.feature_buffers(n, cap, dest, names) if arrays is None else arrays
         counts, status = np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.int32)
         ptrs, cnts, keep = _scan_arrays(clouds, kind)
         out = self.feature_out(cap, dest, arrays, counts, status)
-        self._check(self.lib.qb200_describe_points_each(self.h, ptrs, cnts, n, self.params_array(params), kind, C.byref(out)),
-                    "qb200_describe_points_each")
+        self._check(getattr(self.lib, fn)(self.h, ptrs, cnts, n, self.params_array(params), kind, C.byref(out)), fn)
         per_cloud = []
         for i in range(n):
             m = min(int(counts[i]), cap)
             per_cloud.append(tuple(None if k not in arrays else (arrays[k][i, :m].copy() if dest == MEM_HOST else arrays[k][i, :m])
-                                   for k in POINT_ARRAYS))
+                                   for k in names))
         return per_cloud, counts[:n], status[:n]
 
     def describe_points_enqueue_each_raw(self, cloud_ptrs, counts, n: int, params_array, kind: int, out: FeatureOut):

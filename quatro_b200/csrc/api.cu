@@ -451,44 +451,95 @@ int cache_waits(qb200_handle* h, Lane* L, int ncl, bool write) {
 }
 
 // ---- batch calls ----------------------------------------------------------------------------------------------------------
-// One batch call as its entry point received it.  Its input is n pairs of raw scans (in `kind` memory), n pairs of cached scans,
-// n correspondence sets (in `kind` memory), n raw scans to cache (cache_write), or n pairs of caller keypoints and descriptors (in
-// `kind` memory, feature_call): exactly one of the five is set.  The registering
-// entry points fill the fields up to `lists` in order.
+// The params entries of a call: one for the whole batch, one per input whose front-end fields (voxel_size .. seed) are bit-identical
+// in every entry, or one per input that may differ in any field (the _mixed forms and the calls that read no shared front end)
+enum class Entries { One, Each, Mixed };
+
+// One batch call as its entry point received it (handle.cuh lists the valid source and sink pairs): n inputs of its source, of
+// which only the array of that source is read, in `kind` memory (cached pairs: host), and the outputs of its sink.
 struct BatchCall {
-  const qb200_pair* pairs = nullptr;
-  const qb200_slot_pair* slots = nullptr;
-  const qb200_corr_set* sets = nullptr;
+  Source src = Source::RawPairs;
+  Sink sink = Sink::Solve;
   int n = 0;
   qb200_mem_kind kind = QB200_MEM_HOST;
-  // the caller's params: one entry for the whole batch, or (each) one per pair
   const qb200_params* caller = nullptr;
-  bool each = false;
-  qb200_result* results = nullptr;
-  // the batch's per-pair lists (qb200_pair_lists), nullptr = records only
-  const qb200_pair_lists* lists = nullptr;
-  // (each) the entries may differ in their front-end fields too (the _mixed forms); otherwise those are bit-identical in every entry
-  bool mixed = false;
-  // a cache write: scan i (n_points[i] points in `kind` memory) is voxelized and described with its entry into slot slot_ids[i];
-  // a describe call (describe, no slot_ids): the same front end, into the caller's arrays of *out; a describe-points call (points
-  // too): scan i is the caller's keypoint cloud, imported as it is and described with the lattice fields of its entry
-  const float* const* scans = nullptr;
-  const int32_t* n_points = nullptr;
-  const int32_t* slot_ids = nullptr;
-  bool describe = false, points = false;
-  const qb200_feature_out* out = nullptr;
-  // caller features: pair i's keypoints and FPFH-33 rows, matched and solved with its own entry (front-end fields ignored)
-  const qb200_feature_pair* feats = nullptr;
-  // a match call (pairs, slots or feats): every wave runs its front end and the matcher, then writes the matcher's records and the
-  // correspondence lists without solving; the solver fields of the entries are neither checked nor resolved
-  bool match = false;
-  // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved, laid out like `caller`.
+  Entries entries = Entries::One;
+  // the inputs, one array per source
+  const qb200_pair* pairs = nullptr;           // RawPairs
+  const qb200_slot_pair* slots = nullptr;      // CachedPairs
+  const qb200_feature_pair* feats = nullptr;   // FeaturePairs: keypoints and FPFH-33 rows, front-end fields of the entries ignored
+  const qb200_corr_set* sets = nullptr;        // CorrSets
+  const float* const* scans = nullptr;         // RawScans, KeypointClouds (described with the lattice fields of their entries alone):
+  const int32_t* n_points = nullptr;           // scan i has n_points[i] points
+  // the outputs, one set per sink
+  qb200_result* results = nullptr;             // Solve, Match: one record per input
+  const qb200_pair_lists* lists = nullptr;     // ... and the per-pair lists, nullptr = records only
+  const int32_t* slot_ids = nullptr;           // CacheSlots: scan i goes to slot slot_ids[i]
+  const qb200_feature_out* out = nullptr;      // Export: the caller's feature arrays
+  // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved (Solve), laid out like `caller`.
   const qb200_params* params = nullptr;
-  // raw host scans of a multi-wave batch: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies queued on
-  // several streams share the PCIe link, so every wave's scans would arrive late; on one stream they arrive wave after wave and
-  // the first waves compute while the later ones are still crossing.
+  // host inputs of a multi-wave batch crossing PCIe: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies
+  // queued on several streams share the PCIe link, so every wave's scans would arrive late; on one stream they arrive wave after
+  // wave and the first waves compute while the later ones are still crossing.
   cudaStream_t copy_stream = nullptr;
+  bool each() const { return entries != Entries::One; }
 };
+
+// The facts of each source that the checks and the waves read, written down once
+
+// clouds one input takes in the wave's 2S cloud buffers: two per pair, one per scan, none per set (its matched points go to ma / mb)
+int clouds_per_input(Source s) {
+  switch (s) {
+    case Source::RawPairs: case Source::CachedPairs: case Source::FeaturePairs: return 2;
+    case Source::RawScans: case Source::KeypointClouds: return 1;
+    case Source::CorrSets: return 0;
+  }
+  return 0;
+}
+
+// the wave matches pairs of clouds (K6..K7) before its records: the solver's counters come from a front end (have_frontend)
+bool is_pairs(Source s) { return clouds_per_input(s) == 2; }
+
+// Host-kind inputs of the source cross PCIe in a staged front (stage_raw, stage_features): a multi-wave batch sends them on the
+// shared copy stream and opens with a quarter wave.  Cached pairs and correspondence sets do neither.
+bool crosses_pcie(Source s) {
+  switch (s) {
+    case Source::RawPairs: case Source::FeaturePairs: case Source::RawScans: case Source::KeypointClouds: return true;
+    case Source::CachedPairs: case Source::CorrSets: return false;
+  }
+  return false;
+}
+
+// The wave uploads the front-end table d_front: K1..K5 (K2..K5 for keypoint clouds) read each cloud's entry.  The solver table
+// d_solve is uploaded by the waves with records (Solve, Match), i.e. of pairs and sets.
+bool runs_front_end(Source s) {
+  switch (s) {
+    case Source::RawPairs: case Source::RawScans: case Source::KeypointClouds: return true;
+    case Source::CachedPairs: case Source::FeaturePairs: case Source::CorrSets: return false;
+  }
+  return false;
+}
+
+bool has_records(Sink k) { return k == Sink::Solve || k == Sink::Match; }
+
+// The stage-time slots of qb200_get_stage_ms a wave reports (bit i = slot i, the time between events i and i + 1 of Lane::ev).
+// A wave reports the stages its source runs: cached pairs their copy-in in the fpfh slot, caller features their copy and import in
+// h2d.  Cached pairs and sets report no d2h slot; waves without records report none (they register nothing).  A match wave reports
+// the slots up to match as its source has them, and d2h.
+unsigned stage_slots(Source s, Sink k) {
+  enum : unsigned { kH2d = 1, kVoxel = 2, kFpfh = 4, kMatch = 8, kGraph = 16, kClique = 32, kPose = 64, kD2h = 128 };
+  constexpr unsigned kSolver = kGraph | kClique | kPose;
+  if (!has_records(k)) return 0u;
+  unsigned m = 0;
+  switch (s) {
+    case Source::RawPairs: m = kH2d | kVoxel | kFpfh | kMatch | kSolver | kD2h; break;
+    case Source::FeaturePairs: m = kH2d | kMatch | kSolver | kD2h; break;
+    case Source::CachedPairs: m = kFpfh | kMatch | kSolver; break;
+    case Source::CorrSets: m = kSolver; break;
+    case Source::RawScans: case Source::KeypointClouds: break;
+  }
+  return k == Sink::Match ? (m & (kH2d | kVoxel | kFpfh | kMatch)) | kD2h : m;
+}
 
 // Host-kind lists: the lane's pinned staging block holds cap entries of every list for each slot.  It only grows, and a failed
 // allocation leaves the lane as it was.  The lane's previous wave has been collected, so the old block is not in use.
@@ -622,143 +673,185 @@ int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets, bool 
   return QB200_ERR_BAD_ARG;
 }
 
-// Enqueue one wave (pairs [w0, w0 + np), np <= S) on lane L: the front of the wave its input needs (raw scans: H2D, K1..K6;
-// cached scans: the copy out of the cache, K6; caller features: their H2D and import, K6; correspondence sets: their H2D), then
-// K8..K11 and the D2H of the result records.  A match wave (in.match) runs the same front and K6..K7, then match_records_kernel in
-// place of K8..K11, and hands out the records and the correspondence lists.
-// A cache write's wave is scans [w0, w0 + np), np <= 2S: their H2D, K1..K5 and the copy into their slots, with no records; a describe
-// wave is the same with the export to the caller's arrays in place of the copy, and a describe-points wave imports its keypoint
-// clouds as a feature wave does (without descriptors) in place of the H2D and K1.
-// No sync: wave_collect hands the records out to in.results[w0...].  The lane's previous wave must have been collected.
+// The wave's tables (the lane's previous wave has been collected: their pinned mirrors are free), copied before anything else of the
+// wave: on a stream of host batches the copy engine carries the scans, and a copy queued ahead of this wave's scans only waits for
+// the earlier waves' scans, which the lane waits for anyway.  An input's entries (a pair's and both of its clouds') come from its own
+// params.
+int fill_tables(Lane* L, const BatchCall& in, int w0, int np) {
+  const bool one_cloud = clouds_per_input(in.src) == 1;
+  for (int s = 0; s < np; ++s) {
+    const bool own = in.each() || s == 0;
+    const qb200_params& p = in.params[in.each() ? w0 + s : 0];
+    if (one_cloud) {
+      L->h_front[s] = own ? front_entry(p, in.src == Source::KeypointClouds) : L->h_front[0];
+      continue;
+    }
+    L->h_solve[s] = own ? (in.sink == Sink::Match ? match_entry(p) : solve_entry(p)) : L->h_solve[0];
+    if (in.src == Source::RawPairs) L->h_front[2 * s] = L->h_front[2 * s + 1] = own ? front_entry(p) : L->h_front[0];
+  }
+  int rc;
+  if (has_records(in.sink) && (rc = upload_solve(L, np))) return rc;
+  if (runs_front_end(in.src) && (rc = upload_front(L, np * clouds_per_input(in.src)))) return rc;
+  return QB200_OK;
+}
+
+// The H2D of the staged fronts: the wave's inputs (raw scans, or caller keypoints and rows) on the batch's copy stream or the lane's
+// own, then the reset of the wave's counters, and the lane's stream waits for the copies
+int stage_inputs(qb200_handle* h, Lane* L, const BatchCall& in, int ncl) {
+  const cudaStream_t cs = in.copy_stream ? in.copy_stream : L->stream;
+  const bool raw = in.src == Source::RawPairs || in.src == Source::RawScans;
+  int rc = raw ? stage_raw(L, ncl, in.kind, cs) : stage_features(L, ncl, in.kind, cs);
+  if (rc || (rc = wave_reset(L, ncl))) return rc;
+  if (in.copy_stream) {
+    QB_CUDA_TRY(L, cudaEventRecord(h->ev_copied, in.copy_stream));
+    QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, h->ev_copied, 0));
+  }
+  return QB200_OK;
+}
+
+// Raw pairs and raw scans: the H2D of host scans, K1 (voxel) and K2..K5 (normals, FPFH)
+int front_raw(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np, int ncl) {
+  int rc;
+  cudaEventRecord(L->ev[0], L->stream);
+  for (int s = 0; s < np; ++s) {
+    if (in.src == Source::RawScans) {
+      L->h_cloud_ptr[s] = reinterpret_cast<const float4*>(in.scans[w0 + s]);
+      L->h_cloud_n[s] = in.n_points[w0 + s];
+      if (in.sink == Sink::CacheSlots) L->h_slot_of_cloud[s] = in.slot_ids[w0 + s];
+      continue;
+    }
+    const qb200_pair& pr = in.pairs[w0 + s];
+    L->h_cloud_ptr[2 * s] = reinterpret_cast<const float4*>(pr.src);
+    L->h_cloud_ptr[2 * s + 1] = reinterpret_cast<const float4*>(pr.tgt);
+    L->h_cloud_n[2 * s] = pr.n_src;
+    L->h_cloud_n[2 * s + 1] = pr.n_tgt;
+  }
+  if ((rc = stage_inputs(h, L, in, ncl))) return rc;
+  cudaEventRecord(L->ev[1], L->stream);
+  if ((rc = launch_voxel(L, ncl))) return rc;
+  cudaEventRecord(L->ev[2], L->stream);
+  if ((rc = launch_fpfh(L, ncl))) return rc;
+  cudaEventRecord(L->ev[3], L->stream);
+  return QB200_OK;
+}
+
+// Feature pairs and keypoint clouds: the caller's keypoints (and a feature pair's descriptor rows) imported as they are; keypoint
+// clouds, which come without descriptors, are then described by K2..K5
+int front_features(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np, int ncl) {
+  int rc;
+  cudaEventRecord(L->ev[0], L->stream);
+  for (int s = 0; s < np; ++s) {
+    if (in.src == Source::KeypointClouds) {
+      L->h_feat[s] = {reinterpret_cast<const float4*>(in.scans[w0 + s]), nullptr, in.n_points[w0 + s], 0};
+      continue;
+    }
+    const qb200_feature_pair& f = in.feats[w0 + s];
+    L->h_feat[2 * s] = {reinterpret_cast<const float4*>(f.src), f.src_desc, f.n_src, 0};
+    L->h_feat[2 * s + 1] = {reinterpret_cast<const float4*>(f.tgt), f.tgt_desc, f.n_tgt, 0};
+  }
+  if ((rc = stage_inputs(h, L, in, ncl))) return rc;
+  if ((rc = launch_feature_import(L, ncl))) return rc;
+  for (int i = 1; i <= 2; ++i) cudaEventRecord(L->ev[i], L->stream);  // no voxel stage: slot 1 is not reported
+  if (in.src == Source::KeypointClouds && (rc = launch_fpfh(L, ncl))) return rc;
+  cudaEventRecord(L->ev[3], L->stream);  // no FPFH stage in a feature wave: slot 2 is not reported either
+  return QB200_OK;
+}
+
+// Cached pairs: both clouds of every pair copied out of their cache slots
+int front_cached(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np, int ncl) {
+  int rc;
+  for (int s = 0; s < np; ++s) {
+    L->h_slot_of_cloud[2 * s] = in.slots[w0 + s].src_slot;
+    L->h_slot_of_cloud[2 * s + 1] = in.slots[w0 + s].tgt_slot;
+  }
+  if ((rc = wave_reset(L, ncl))) return rc;
+  if ((rc = cache_waits(h, L, ncl, false))) return rc;
+  cudaEventRecord(L->ev[2], L->stream);
+  if ((rc = cache_copy(h, L, 0, ncl))) return rc;
+  QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_in, L->stream));
+  cudaEventRecord(L->ev[3], L->stream);
+  return QB200_OK;
+}
+
+// Correspondence sets: the matched points of every set into ma / mb and its size into n_corr
+int front_sets(Lane* L, const BatchCall& in, int w0, int np) {
+  if (int rc = wave_reset(L, 0)) return rc;
+  const cudaMemcpyKind ck = in.kind == QB200_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+  for (int s = 0; s < np; ++s) {
+    const qb200_corr_set& cs = in.sets[w0 + s];
+    L->h_cloud_n[s] = cs.L;
+    if (cs.L > 0) {
+      QB_CUDA_TRY(L, cudaMemcpyAsync(L->ma + (size_t)s * L->Lc, cs.a, (size_t)cs.L * sizeof(float4), ck, L->stream));
+      QB_CUDA_TRY(L, cudaMemcpyAsync(L->mb + (size_t)s * L->Lc, cs.b, (size_t)cs.L * sizeof(float4), ck, L->stream));
+    }
+  }
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->ctr.n_corr, L->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, L->stream));
+  return QB200_OK;
+}
+
+// The end of every wave with records: the list pack, the D2H of the records
+int send_records(Lane* L, const BatchCall& in, int w0, int np) {
+  if (in.lists)
+    if (int rc = submit_lists(L, *in.lists, w0, np)) return rc;
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
+  cudaEventRecord(L->ev[8], L->stream);
+  return QB200_OK;
+}
+
+// Enqueue one wave (inputs [w0, w0 + np) of the call: np <= S pairs or sets, or np <= 2S scans) on lane L: its tables, the front of
+// its source, then the tail of its sink: Solve K6..K7 (pairs) and K8..K11, Match K6..K7 and match_records_kernel, both then the lists
+// and the D2H of the records; CacheSlots the copy into the cache slots; Export the export to the caller's arrays.  No sync:
+// wave_collect hands the outputs on.  The lane's previous wave must have been collected.
 int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
-  const bool raw = in.pairs || (in.scans && !in.points);
-  const int ncl = in.scans ? np : 2 * np;
+  const int ncl = np * clouds_per_input(in.src);
   int rc;
   L->kev_armed[0] = L->kev_armed[1] = 0;
   L->pend_slots.clear();
   L->pend_writes = 0;
-  // the wave's tables (the lane's previous wave has been collected: their pinned mirrors are free), copied before anything else of the
-  // wave: on a stream of host batches the copy engine carries the scans, and a copy queued ahead of this wave's scans only waits for
-  // the earlier waves' scans, which the lane waits for anyway.  A pair's entry and both of its clouds' come from its own params.
-  for (int s = 0; s < np; ++s) {
-    const bool own = in.each || s == 0;
-    const qb200_params& p = in.params[in.each ? w0 + s : 0];
-    if (in.scans) {
-      L->h_front[s] = own ? front_entry(p, in.points) : L->h_front[0];
-      continue;
-    }
-    L->h_solve[s] = own ? (in.match ? match_entry(p) : solve_entry(p)) : L->h_solve[0];
-    if (in.pairs) L->h_front[2 * s] = L->h_front[2 * s + 1] = own ? front_entry(p) : L->h_front[0];
+  if ((rc = fill_tables(L, in, w0, np))) return rc;
+  switch (in.src) {
+    case Source::RawPairs: case Source::RawScans: rc = front_raw(h, L, in, w0, np, ncl); break;
+    case Source::FeaturePairs: case Source::KeypointClouds: rc = front_features(h, L, in, w0, np, ncl); break;
+    case Source::CachedPairs: rc = front_cached(h, L, in, w0, np, ncl); break;
+    case Source::CorrSets: rc = front_sets(L, in, w0, np); break;
   }
-  if (!in.scans && (rc = upload_solve(L, np))) return rc;
-  if ((raw || in.points) && (rc = upload_front(L, ncl))) return rc;
-  if (raw) {
-    cudaEventRecord(L->ev[0], L->stream);
-    for (int s = 0; s < np; ++s) {
-      if (in.scans) {
-        L->h_cloud_ptr[s] = reinterpret_cast<const float4*>(in.scans[w0 + s]);
-        L->h_cloud_n[s] = in.n_points[w0 + s];
-        if (in.slot_ids) L->h_slot_of_cloud[s] = in.slot_ids[w0 + s];
-        continue;
-      }
-      const qb200_pair& pr = in.pairs[w0 + s];
-      L->h_cloud_ptr[2 * s] = reinterpret_cast<const float4*>(pr.src);
-      L->h_cloud_ptr[2 * s + 1] = reinterpret_cast<const float4*>(pr.tgt);
-      L->h_cloud_n[2 * s] = pr.n_src;
-      L->h_cloud_n[2 * s + 1] = pr.n_tgt;
-    }
-    if ((rc = stage_raw(L, ncl, in.kind, in.copy_stream ? in.copy_stream : L->stream))) return rc;
-    if ((rc = wave_reset(L, ncl))) return rc;
-    if (in.copy_stream) {
-      QB_CUDA_TRY(L, cudaEventRecord(h->ev_copied, in.copy_stream));
-      QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, h->ev_copied, 0));
-    }
-    cudaEventRecord(L->ev[1], L->stream);
-    if ((rc = launch_voxel(L, ncl))) return rc;
-    cudaEventRecord(L->ev[2], L->stream);
-    if ((rc = launch_fpfh(L, ncl))) return rc;
-    cudaEventRecord(L->ev[3], L->stream);
-  } else if (in.feats || in.points) {
-    cudaEventRecord(L->ev[0], L->stream);
-    for (int s = 0; s < np; ++s) {
-      if (in.points) {  // keypoints without descriptors: K2..K5 describe them below
-        L->h_feat[s] = {reinterpret_cast<const float4*>(in.scans[w0 + s]), nullptr, in.n_points[w0 + s], 0};
-        continue;
-      }
-      const qb200_feature_pair& f = in.feats[w0 + s];
-      L->h_feat[2 * s] = {reinterpret_cast<const float4*>(f.src), f.src_desc, f.n_src, 0};
-      L->h_feat[2 * s + 1] = {reinterpret_cast<const float4*>(f.tgt), f.tgt_desc, f.n_tgt, 0};
-    }
-    if ((rc = stage_features(L, ncl, in.kind, in.copy_stream ? in.copy_stream : L->stream))) return rc;
-    if ((rc = wave_reset(L, ncl))) return rc;
-    if (in.copy_stream) {
-      QB_CUDA_TRY(L, cudaEventRecord(h->ev_copied, in.copy_stream));
-      QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, h->ev_copied, 0));
-    }
-    if ((rc = launch_feature_import(L, ncl))) return rc;
-    for (int i = 1; i <= 2; ++i) cudaEventRecord(L->ev[i], L->stream);  // no voxel stage: slot 1 is not reported
-    if (in.points && (rc = launch_fpfh(L, ncl))) return rc;
-    cudaEventRecord(L->ev[3], L->stream);  // no FPFH stage in a feature wave: slot 2 is not reported either
-  } else if (in.slots) {
-    for (int s = 0; s < np; ++s) {
-      L->h_slot_of_cloud[2 * s] = in.slots[w0 + s].src_slot;
-      L->h_slot_of_cloud[2 * s + 1] = in.slots[w0 + s].tgt_slot;
-    }
-    if ((rc = wave_reset(L, ncl))) return rc;
-    if ((rc = cache_waits(h, L, ncl, false))) return rc;
-    cudaEventRecord(L->ev[2], L->stream);
-    if ((rc = cache_copy(h, L, 0, ncl))) return rc;
-    QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_in, L->stream));
-    cudaEventRecord(L->ev[3], L->stream);
-  } else {
-    if ((rc = wave_reset(L, ncl))) return rc;
-    const cudaMemcpyKind ck = in.kind == QB200_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
-    for (int s = 0; s < np; ++s) {
-      const qb200_corr_set& cs = in.sets[w0 + s];
-      L->h_cloud_n[s] = cs.L;
-      if (cs.L > 0) {
-        QB_CUDA_TRY(L, cudaMemcpyAsync(L->ma + (size_t)s * L->Lc, cs.a, (size_t)cs.L * sizeof(float4), ck, L->stream));
-        QB_CUDA_TRY(L, cudaMemcpyAsync(L->mb + (size_t)s * L->Lc, cs.b, (size_t)cs.L * sizeof(float4), ck, L->stream));
-      }
-    }
-    QB_CUDA_TRY(L, cudaMemcpyAsync(L->ctr.n_corr, L->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, L->stream));
-  }
-  if (in.out) {
-    if ((rc = submit_export(L, *in.out, w0, ncl))) return rc;
-  } else if (in.scans) {
-    if ((rc = cache_waits(h, L, ncl, true))) return rc;
-    if ((rc = cache_copy(h, L, 1, ncl))) return rc;
-    QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_out, L->stream));
-  } else {
-    if (!in.sets && (rc = launch_match(L, np, in.feats != nullptr))) return rc;
-    if (in.match) {  // no solver tail: the records come from the matcher's counters, and graph, clique and pose take no time
-      if ((rc = launch_match_records(L, np))) return rc;
-      for (int i = 4; i <= 7; ++i) cudaEventRecord(L->ev[i], L->stream);
-    } else {
+  if (rc) return rc;
+  const bool match_pairs = is_pairs(in.src);
+  switch (in.sink) {
+    case Sink::Solve:
+      if (match_pairs && (rc = launch_match(L, np, in.src == Source::FeaturePairs))) return rc;
       cudaEventRecord(L->ev[4], L->stream);
       cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
-      if ((rc = run_solver(L, np, in.sets ? 0 : 1))) return rc;
+      if ((rc = run_solver(L, np, match_pairs ? 1 : 0))) return rc;
       cudaEventRecord(L->ev[7], L->stream);
-    }
-    if (in.lists && (rc = submit_lists(L, *in.lists, w0, np))) return rc;
-    QB_CUDA_TRY(L, cudaMemcpyAsync(L->h_results, L->d_results, (size_t)np * sizeof(qb200_result), cudaMemcpyDeviceToHost, L->stream));
-    cudaEventRecord(L->ev[8], L->stream);
+      rc = send_records(L, in, w0, np);
+      break;
+    case Sink::Match:  // no solver tail: the records come from the matcher's counters, and graph, clique and pose take no time
+      if ((rc = launch_match(L, np, in.src == Source::FeaturePairs))) return rc;
+      if ((rc = launch_match_records(L, np))) return rc;
+      for (int i = 4; i <= 7; ++i) cudaEventRecord(L->ev[i], L->stream);
+      rc = send_records(L, in, w0, np);
+      break;
+    case Sink::CacheSlots:
+      if ((rc = cache_waits(h, L, ncl, true))) return rc;
+      if ((rc = cache_copy(h, L, 1, ncl))) return rc;
+      QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_out, L->stream));
+      break;
+    case Sink::Export: rc = submit_export(L, *in.out, w0, ncl); break;
   }
+  if (rc) return rc;
   L->pend_w0 = w0;
   L->pend_np = np;
-  L->pend_dst = in.results;  // nullptr for a cache write or a describe call: no records
+  L->pend_stages = stage_slots(in.src, in.sink);
+  L->pend_sink = in.sink;
+  L->pend_dst = in.results;
+  L->pend_host_lists = in.lists && in.lists->kind == QB200_MEM_HOST;
   if (in.lists) L->pend_lists = *in.lists;
-  else L->pend_lists.cap_per_pair = 0;
-  if (in.out) L->pend_out = *in.out;
-  else L->pend_out.cap_per_scan = 0;
-  // stage-time slots of qb200_get_stage_ms this wave reports: raw scans all eight, caller features h2d and match to d2h, the other
-  // inputs their first stage to pose, a cache write none (it registers nothing); a match wave the same without graph, clique and pose
-  L->pend_stages = in.pairs ? 0xFFu : in.feats ? 0xF9u : in.slots ? 0x7Cu : in.sets ? 0x70u : 0u;
-  if (in.match) L->pend_stages = (L->pend_stages & 0x0Fu) | 0x80u;
+  if (in.sink == Sink::Export) L->pend_out = *in.out;
   return QB200_OK;
 }
 
-// wait for the wave in flight on lane L, hand out its records and add its stage / kernel times to the handle
+// wait for the wave in flight on lane L, hand out what its sink produced and add its stage / kernel times to the handle
 int wave_collect(qb200_handle* h, Lane* L) {
   if (L->pend_np == 0) return QB200_OK;
   const int np = L->pend_np;
@@ -767,9 +860,14 @@ int wave_collect(qb200_handle* h, Lane* L) {
     h->fail(__FILE__, __LINE__, cudaGetErrorString(cudaGetLastError()));
     return QB200_ERR_CUDA;
   }
-  if (L->pend_dst) memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
-  if (L->pend_lists.cap_per_pair > 0 && L->pend_lists.kind == QB200_MEM_HOST) deliver_lists(L, L->pend_lists, L->pend_w0, np);
-  if (L->pend_out.cap_per_scan > 0) deliver_export(L, L->pend_out, L->pend_w0, np);
+  switch (L->pend_sink) {
+    case Sink::Solve: case Sink::Match:
+      memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
+      if (L->pend_host_lists) deliver_lists(L, L->pend_lists, L->pend_w0, np);
+      break;
+    case Sink::CacheSlots: break;
+    case Sink::Export: deliver_export(L, L->pend_out, L->pend_w0, np); break;
+  }
   if (h->timeline && (L->pend_stages & 1u)) {  // stage boundaries of a raw-scan or feature wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
     fprintf(stderr, "[qb200 timeline] wave w0=%d np=%d:", L->pend_w0, np);
     for (int i = 0; i < 9; ++i) {
@@ -850,104 +948,130 @@ std::unique_ptr<qb200_params[]> resolve_call(qb200_handle* h, const qb200_params
   return r;
 }
 
-// Every argument check of a batch call, in one order whatever its input, so that a call with several faults returns the same code:
-// counts and arrays, the params entries, the cross-check, the lists, then every pair, set or scan.  A rejection names its fault in
+// the call's input array: the one of its source
+const void* input_of(const BatchCall& c) {
+  switch (c.src) {
+    case Source::RawPairs: return c.pairs;
+    case Source::CachedPairs: return c.slots;
+    case Source::FeaturePairs: return c.feats;
+    case Source::CorrSets: return c.sets;
+    case Source::RawScans: case Source::KeypointClouds: return c.scans;
+  }
+  return nullptr;
+}
+
+// Every argument check of a batch call, in one order whatever its source, so that a call with several faults returns the same code:
+// counts and arrays, the params entries, the cross-check, the lists, the outputs, then every input.  A rejection names its fault in
 // qb200_last_error.
 int check_call(qb200_handle* h, const BatchCall& c) {
   auto reject = [h](const char* why) {
     h->fail(__FILE__, __LINE__, why);
     return QB200_ERR_BAD_ARG;
   };
+  const bool scans = clouds_per_input(c.src) == 1;
   if (c.n < 0) return reject("n < 0");
-  if (c.n > 0 && !c.pairs && !c.slots && !c.sets && !c.scans && !c.feats) return reject("the input array is null");
-  if (c.n > 0 && c.scans && (!c.n_points || (!c.describe && !c.slot_ids))) return reject("the n_points or slot_ids array is null");
-  if (c.n > 0 && !c.scans && !c.results) return reject("the results array is null");
+  if (c.n > 0 && !input_of(c)) return reject("the input array is null");
+  if (c.n > 0 && scans && (!c.n_points || (c.sink == Sink::CacheSlots && !c.slot_ids))) return reject("the n_points or slot_ids array is null");
+  if (c.n > 0 && has_records(c.sink) && !c.results) return reject("the results array is null");
   if (c.kind != QB200_MEM_HOST && c.kind != QB200_MEM_DEVICE) return reject("unknown memory kind of the inputs");
   const qb200_params* p = c.caller;
   char why[192];
-  if (c.points) {  // only the lattice fields are read
+  if (c.src == Source::KeypointClouds) {  // only the lattice fields are read
     for (int i = 0; i < c.n; ++i) {
       if (!p || !lattice_ok(p[i])) {
         snprintf(why, sizeof(why), "params entry %d is null or its radii or lattice cell are out of range", i);
         return reject(why);
       }
     }
-  } else if (int rc = check_params(h, p, c.n, c.each, !c.sets && !c.mixed, !c.match)) {
+  } else if (int rc = check_params(h, p, c.n, c.each(), c.src != Source::CorrSets && c.entries == Entries::Each, c.sink != Sink::Match)) {
     return rc;
   }
-  for (int i = 0; !c.sets && !c.scans && i < (c.each ? c.n : 1); ++i) {
+  for (int i = 0; is_pairs(c.src) && i < (c.each() ? c.n : 1); ++i) {
     if (!p[i].use_crosscheck) {
-      if (c.each) {
+      if (c.each()) {
         snprintf(why, sizeof(why), "params entry %d: use_crosscheck = 0 is not supported", i);
         h->fail(__FILE__, __LINE__, why);
       }
       return QB200_ERR_UNSUPPORTED;
     }
   }
-  if (int rc = check_lists(h, c.lists, c.sets != nullptr, c.match)) return rc;
-  if (c.describe)
-    if (int rc = check_out(h, c.out, c.points)) return rc;
+  if (int rc = check_lists(h, c.lists, c.src == Source::CorrSets, c.sink == Sink::Match)) return rc;
+  if (c.sink == Sink::Export)
+    if (int rc = check_out(h, c.out, c.src == Source::KeypointClouds)) return rc;
   const int R = h->cfg.max_raw_points;
   for (int i = 0; i < c.n; ++i) {
-    if (c.pairs) {
-      const qb200_pair& q = c.pairs[i];
-      if (q.n_src < 0 || q.n_tgt < 0 || q.n_src > R || q.n_tgt > R || (q.n_src > 0 && !q.src) || (q.n_tgt > 0 && !q.tgt))
-        return reject("pair has a null cloud or exceeds max_raw_points");
-    } else if (c.slots) {
-      const qb200_params& pe = p[c.each ? i : 0];  // the pair's own entry
-      for (const int sl : {c.slots[i].src_slot, c.slots[i].tgt_slot}) {
-        if (sl < 0 || sl >= h->c_slots) return reject("slot outside qb200_cache_reserve()");
-        const float* sig = h->c_sig.get() + 4 * (size_t)sl;
-        if (sig[0] != pe.voxel_size || sig[1] != pe.normal_radius || sig[2] != pe.fpfh_radius || sig[3] != lattice_cell(pe)) {
-          snprintf(why, sizeof(why), "pair %d: cached scan in slot %d was computed with other front-end parameters (or the slot is empty)",
-                   i, sl);
-          return reject(why);
-        }
+    const char* bad = nullptr;
+    switch (c.src) {
+      case Source::RawPairs: {
+        const qb200_pair& q = c.pairs[i];
+        if (q.n_src < 0 || q.n_tgt < 0 || q.n_src > R || q.n_tgt > R || (q.n_src > 0 && !q.src) || (q.n_tgt > 0 && !q.tgt))
+          return reject("pair has a null cloud or exceeds max_raw_points");
+        break;
       }
-    } else if (c.feats) {
-      const qb200_feature_pair& f = c.feats[i];
-      for (int side = 0; side < 2; ++side) {
-        const int n = side ? f.n_tgt : f.n_src;
-        const float* pts = side ? f.tgt : f.src;
-        const float* desc = side ? f.tgt_desc : f.src_desc;
-        const char* bad = nullptr;
-        if (n < 0 || n > h->cfg.max_voxel_points) bad = "count outside 0 .. max_voxel_points";
-        else if (n > 0 && (!pts || !desc)) bad = "null keypoints or descriptors";
-        else if (n > 0 && c.kind == QB200_MEM_DEVICE && !(device_array_of(h, pts, 16) && device_array_of(h, desc, 4)))
-          bad = "keypoints (16-byte) or descriptors (4-byte) misaligned or not memory of the handle's device";
+      case Source::CachedPairs: {
+        const qb200_params& pe = p[c.each() ? i : 0];  // the pair's own entry
+        for (const int sl : {c.slots[i].src_slot, c.slots[i].tgt_slot}) {
+          if (sl < 0 || sl >= h->c_slots) return reject("slot outside qb200_cache_reserve()");
+          const float* sig = h->c_sig.get() + 4 * (size_t)sl;
+          if (sig[0] != pe.voxel_size || sig[1] != pe.normal_radius || sig[2] != pe.fpfh_radius || sig[3] != lattice_cell(pe)) {
+            snprintf(why, sizeof(why), "pair %d: cached scan in slot %d was computed with other front-end parameters (or the slot is empty)",
+                     i, sl);
+            return reject(why);
+          }
+        }
+        break;
+      }
+      case Source::FeaturePairs: {
+        const qb200_feature_pair& f = c.feats[i];
+        for (int side = 0; side < 2; ++side) {
+          const int n = side ? f.n_tgt : f.n_src;
+          const float* pts = side ? f.tgt : f.src;
+          const float* desc = side ? f.tgt_desc : f.src_desc;
+          if (n < 0 || n > h->cfg.max_voxel_points) bad = "count outside 0 .. max_voxel_points";
+          else if (n > 0 && (!pts || !desc)) bad = "null keypoints or descriptors";
+          else if (n > 0 && c.kind == QB200_MEM_DEVICE && !(device_array_of(h, pts, 16) && device_array_of(h, desc, 4)))
+            bad = "keypoints (16-byte) or descriptors (4-byte) misaligned or not memory of the handle's device";
+          if (bad) {
+            snprintf(why, sizeof(why), "feature pair %d, %s: %s", i, side ? "target" : "source", bad);
+            return reject(why);
+          }
+        }
+        break;
+      }
+      case Source::CorrSets: {
+        const qb200_corr_set& s = c.sets[i];
+        if (s.L < 0 || s.L > h->cfg.max_corr || (s.L > 0 && (!s.a || !s.b))) return reject("correspondence set is null or exceeds max_corr");
+        break;
+      }
+      case Source::KeypointClouds: {
+        const int np = c.n_points[i];
+        if (np < 0 || np > h->cfg.max_voxel_points) bad = "its point count is outside 0 .. max_voxel_points";
+        else if (np > 0 && !c.scans[i]) bad = "it is null";
+        else if (np > 0 && c.kind == QB200_MEM_DEVICE && !device_array_of(h, c.scans[i], 16))
+          bad = "it is misaligned (16 bytes) or not memory of the handle's device";
         if (bad) {
-          snprintf(why, sizeof(why), "feature pair %d, %s: %s", i, side ? "target" : "source", bad);
+          snprintf(why, sizeof(why), "cloud %d: %s", i, bad);
           return reject(why);
         }
+        break;
       }
-    } else if (c.sets) {
-      const qb200_corr_set& s = c.sets[i];
-      if (s.L < 0 || s.L > h->cfg.max_corr || (s.L > 0 && (!s.a || !s.b))) return reject("correspondence set is null or exceeds max_corr");
-    } else if (c.points) {
-      const int np = c.n_points[i];
-      const char* bad = nullptr;
-      if (np < 0 || np > h->cfg.max_voxel_points) bad = "its point count is outside 0 .. max_voxel_points";
-      else if (np > 0 && !c.scans[i]) bad = "it is null";
-      else if (np > 0 && c.kind == QB200_MEM_DEVICE && !device_array_of(h, c.scans[i], 16))
-        bad = "it is misaligned (16 bytes) or not memory of the handle's device";
-      if (bad) {
-        snprintf(why, sizeof(why), "cloud %d: %s", i, bad);
-        return reject(why);
-      }
-    } else if (c.describe) {
-      const int np = c.n_points[i];
-      const char* bad = nullptr;
-      if (np < 0 || np > R) bad = "its point count is outside 0 .. max_raw_points";
-      else if (np > 0 && !c.scans[i]) bad = "it is null";
-      if (bad) {
-        snprintf(why, sizeof(why), "scan %d: %s", i, bad);
-        return reject(why);
-      }
-    } else {
-      const int sl = c.slot_ids[i], np = c.n_points[i];
-      if (sl < 0 || sl >= h->c_slots || np < 0 || np > R || (np > 0 && !c.scans[i])) {
-        snprintf(why, sizeof(why), "scan %d is null, exceeds max_raw_points or names a slot outside qb200_cache_reserve()", i);
-        return reject(why);
+      case Source::RawScans: {
+        const int np = c.n_points[i];
+        if (c.sink == Sink::CacheSlots) {
+          const int sl = c.slot_ids[i];
+          if (sl < 0 || sl >= h->c_slots || np < 0 || np > R || (np > 0 && !c.scans[i])) {
+            snprintf(why, sizeof(why), "scan %d is null, exceeds max_raw_points or names a slot outside qb200_cache_reserve()", i);
+            return reject(why);
+          }
+          break;
+        }
+        if (np < 0 || np > R) bad = "its point count is outside 0 .. max_raw_points";
+        else if (np > 0 && !c.scans[i]) bad = "it is null";
+        if (bad) {
+          snprintf(why, sizeof(why), "scan %d: %s", i, bad);
+          return reject(why);
+        }
+        break;
       }
     }
   }
@@ -969,15 +1093,15 @@ int enqueue_call(qb200_handle* h, BatchCall c) {
   // An empty call resolves no params: the reference latches the rotation noise bound inside computeTransformation, which an empty
   // batch never calls.
   if (c.n == 0) return QB200_OK;
-  // a cache write or a match call resolves nothing: only the solver reads the rotation noise bound
+  // only the solver reads the rotation noise bound: the other sinks resolve nothing
   std::unique_ptr<qb200_params[]> pr;
-  const bool solves = !c.scans && !c.match;
-  if (solves && !(pr = resolve_call(h, c.caller, c.n, c.each))) return QB200_ERR_CUDA;
+  const bool solves = c.sink == Sink::Solve;
+  if (solves && !(pr = resolve_call(h, c.caller, c.n, c.each()))) return QB200_ERR_CUDA;
   c.params = solves ? pr.get() : c.caller;
-  // S: inputs per wave, pairs or (a cache write) scans; the clouds of a wave fill the lane's 2 * max_batch_slots cloud buffers
-  const int S = h->cfg.max_batch_slots * (c.scans ? 2 : 1), lanes = h->max_lanes;
-  // raw host scans and host features cross PCIe: the copy stream and the quarter-wave opening below are theirs alone
-  const bool host_scans = (c.pairs || c.scans || c.feats) && c.kind == QB200_MEM_HOST;
+  // S: inputs per wave, pairs, sets or scans; the clouds of a wave fill the lane's 2 * max_batch_slots cloud buffers
+  const int S = h->cfg.max_batch_slots * (clouds_per_input(c.src) == 1 ? 2 : 1), lanes = h->max_lanes;
+  // host inputs crossing PCIe: the copy stream and the quarter-wave opening below are theirs alone
+  const bool host_scans = crosses_pcie(c.src) && c.kind == QB200_MEM_HOST;
   // More than one wave: rotate over the lanes so that one wave's PCIe copies and single-warp solver tail run under the
   // other waves' dense kernels.  Results do not depend on the lane (no state is shared between waves).
   // Wave plan.  Host scans: nothing can run before the first wave's scans crossed PCIe, so the batch opens with a quarter
@@ -1026,8 +1150,8 @@ int enqueue_call(qb200_handle* h, BatchCall c) {
   h->lanes_active = n_lanes;
   // a cache write's signatures, in scan order (a slot named twice ends with its last scan's): the checks of the calls queued after it
   // see them
-  for (int i = 0; c.slot_ids && i < c.n; ++i) {
-    const qb200_params& pc = c.params[c.each ? i : 0];
+  for (int i = 0; c.sink == Sink::CacheSlots && i < c.n; ++i) {
+    const qb200_params& pc = c.params[c.each() ? i : 0];
     float* sig = h->c_sig.get() + 4 * (size_t)c.slot_ids[i];
     sig[0] = pc.voxel_size; sig[1] = pc.normal_radius; sig[2] = pc.fpfh_radius; sig[3] = lattice_cell(pc);
   }
@@ -1049,48 +1173,53 @@ int run_call(qb200_handle* h, const BatchCall& c) {
   int rc = enqueue_call(h, c);
   const int rc2 = h ? batch_flush(h) : QB200_OK;
   if (rc == QB200_OK) rc = rc2;
-  if (rc == QB200_OK && c.n == 1 && c.results) set_last(h, c.results[0]);
+  if (rc == QB200_OK && c.n == 1 && has_records(c.sink)) set_last(h, c.results[0]);
   return rc;
 }
 
-// qb200_cache_scans (each = false: p is one entry for every scan) and qb200_cache_scans_each (p[i] for scan i) as a batch call
-BatchCall cache_write(const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans, const qb200_params* p,
-                      bool each, qb200_mem_kind kind) {
-  BatchCall c;
-  c.n = n_scans; c.kind = kind; c.caller = p; c.each = each; c.mixed = true;
-  c.scans = scans4; c.n_points = n_points; c.slot_ids = slot_ids;
+// One constructor per source: the call's inputs, its params entries and the outputs of its sink
+BatchCall raw_pairs(Sink k, Entries e, const qb200_pair* pairs, int32_t n, const qb200_params* p, qb200_mem_kind kind, qb200_result* results,
+                    const qb200_pair_lists* lists) {
+  BatchCall c{Source::RawPairs, k, n, kind, p, e};
+  c.pairs = pairs; c.results = results; c.lists = lists;
   return c;
 }
 
-// qb200_describe_batch_each and qb200_describe_batch_enqueue_each as a batch call: a cache write whose scans go to *out, not to slots
-BatchCall describe_call(const float* const* scans4, const int32_t* n_points, int32_t n_scans, const qb200_params* params, qb200_mem_kind kind,
-                        const qb200_feature_out* out) {
-  BatchCall c = cache_write(scans4, n_points, nullptr, n_scans, params, true, kind);
-  c.describe = true;
-  c.out = out;
-  return c;
-}
-
-// qb200_describe_points_each and qb200_describe_points_enqueue_each as a batch call: a describe call whose clouds are keypoints
-BatchCall describe_points_call(const float* const* pts4, const int32_t* n_points, int32_t n_clouds, const qb200_params* params,
-                               qb200_mem_kind kind, const qb200_feature_out* out) {
-  BatchCall c = describe_call(pts4, n_points, n_clouds, params, kind, out);
-  c.points = true;
-  return c;
-}
-
-// qb200_register_features_each (enqueue = false) and qb200_register_features_enqueue_each as a batch call
-BatchCall feature_call(const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind, qb200_result* results,
+// cached scans are on the device, and their slot pairs in host memory
+BatchCall cached_pairs(Sink k, Entries e, const qb200_slot_pair* slots, int32_t n, const qb200_params* p, qb200_result* results,
                        const qb200_pair_lists* lists) {
-  BatchCall c;
-  c.n = n_pairs; c.kind = kind; c.caller = params; c.each = true; c.results = results; c.lists = lists; c.mixed = true;
-  c.feats = pairs;
+  BatchCall c{Source::CachedPairs, k, n, QB200_MEM_HOST, p, e};
+  c.slots = slots; c.results = results; c.lists = lists;
   return c;
 }
 
-// the match form of a registering batch call: the same inputs, matched and not solved
-BatchCall match_call(BatchCall c) {
-  c.match = true;
+// the entries' front-end fields are ignored, so they may differ
+BatchCall feature_pairs(Sink k, const qb200_feature_pair* feats, int32_t n, const qb200_params* p, qb200_mem_kind kind, qb200_result* results,
+                        const qb200_pair_lists* lists) {
+  BatchCall c{Source::FeaturePairs, k, n, kind, p, Entries::Mixed};
+  c.feats = feats; c.results = results; c.lists = lists;
+  return c;
+}
+
+BatchCall corr_sets(Sink k, Entries e, const qb200_corr_set* sets, int32_t n, const qb200_params* p, qb200_mem_kind kind, qb200_result* results,
+                    const qb200_pair_lists* lists) {
+  BatchCall c{Source::CorrSets, k, n, kind, p, e};
+  c.sets = sets; c.results = results; c.lists = lists;
+  return c;
+}
+
+// slot_ids for the CacheSlots sink, out for Export; every scan runs its own front end, so the entries may differ
+BatchCall raw_scans(Sink k, Entries e, const float* const* scans4, const int32_t* n_points, int32_t n, const qb200_params* p, qb200_mem_kind kind,
+                    const int32_t* slot_ids, const qb200_feature_out* out) {
+  BatchCall c{Source::RawScans, k, n, kind, p, e};
+  c.scans = scans4; c.n_points = n_points; c.slot_ids = slot_ids; c.out = out;
+  return c;
+}
+
+BatchCall keypoint_clouds(Sink k, const float* const* pts4, const int32_t* n_points, int32_t n, const qb200_params* p, qb200_mem_kind kind,
+                          const qb200_feature_out* out) {
+  BatchCall c{Source::KeypointClouds, k, n, kind, p, Entries::Mixed};
+  c.scans = pts4; c.n_points = n_points; c.out = out;
   return c;
 }
 
@@ -1196,17 +1325,17 @@ int qb200_solve_batch(qb200_handle* h, const qb200_corr_set* sets, int32_t n_set
 
 int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* p, qb200_mem_kind kind,
                          qb200_result* results, const qb200_pair_lists* lists) {
-  return run_call(h, {nullptr, nullptr, sets, n_sets, kind, p, false, results, lists});
+  return run_call(h, corr_sets(Sink::Solve, Entries::One, sets, n_sets, p, kind, results, lists));
 }
 
 int qb200_solve_batch_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params, qb200_mem_kind kind,
                            qb200_result* results, const qb200_pair_lists* lists) {
-  return run_call(h, {nullptr, nullptr, sets, n_sets, kind, params, true, results, lists});
+  return run_call(h, corr_sets(Sink::Solve, Entries::Each, sets, n_sets, params, kind, results, lists));
 }
 
 int qb200_solve_batch_enqueue_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params,
                                    qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_call(h, {nullptr, nullptr, sets, n_sets, kind, params, true, results, lists});
+  return enqueue_call(h, corr_sets(Sink::Solve, Entries::Each, sets, n_sets, params, kind, results, lists));
 }
 
 // ---- raw scans -> pose ------------------------------------------------------------------------------
@@ -1219,37 +1348,37 @@ int qb200_register_batch(qb200_handle* h, const qb200_pair* pairs, int32_t n_pai
 
 int qb200_register_batch_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                             qb200_result* results, const qb200_pair_lists* lists) {
-  return run_call(h, {pairs, nullptr, nullptr, n_pairs, kind, p, false, results, lists});
+  return run_call(h, raw_pairs(Sink::Solve, Entries::One, pairs, n_pairs, p, kind, results, lists));
 }
 
 int qb200_register_batch_each(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
                               qb200_result* results, const qb200_pair_lists* lists) {
-  return run_call(h, {pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists});
+  return run_call(h, raw_pairs(Sink::Solve, Entries::Each, pairs, n_pairs, params, kind, results, lists));
 }
 
 int qb200_register_batch_enqueue(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                                  qb200_result* results) {
-  return enqueue_call(h, {pairs, nullptr, nullptr, n_pairs, kind, p, false, results, nullptr});
+  return enqueue_call(h, raw_pairs(Sink::Solve, Entries::One, pairs, n_pairs, p, kind, results, nullptr));
 }
 
 int qb200_register_batch_enqueue_ex(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_mem_kind kind,
                                     qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_call(h, {pairs, nullptr, nullptr, n_pairs, kind, p, false, results, lists});
+  return enqueue_call(h, raw_pairs(Sink::Solve, Entries::One, pairs, n_pairs, p, kind, results, lists));
 }
 
 int qb200_register_batch_enqueue_each(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                       qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_call(h, {pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists});
+  return enqueue_call(h, raw_pairs(Sink::Solve, Entries::Each, pairs, n_pairs, params, kind, results, lists));
 }
 
 int qb200_register_batch_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
                                qb200_result* results, const qb200_pair_lists* lists) {
-  return run_call(h, {pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists, true});
+  return run_call(h, raw_pairs(Sink::Solve, Entries::Mixed, pairs, n_pairs, params, kind, results, lists));
 }
 
 int qb200_register_batch_enqueue_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                        qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_call(h, {pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists, true});
+  return enqueue_call(h, raw_pairs(Sink::Solve, Entries::Mixed, pairs, n_pairs, params, kind, results, lists));
 }
 
 int qb200_register_pair(qb200_handle* h, const float* src4, int32_t n_src, const float* tgt4, int32_t n_tgt, const qb200_params* p,
@@ -1294,17 +1423,17 @@ int qb200_cache_reserve(qb200_handle* h, int32_t n_slots) {
 
 int qb200_cache_scans(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
                       const qb200_params* p, qb200_mem_kind kind) {
-  return run_call(h, cache_write(scans4, n_points, slot_ids, n_scans, p, false, kind));
+  return run_call(h, raw_scans(Sink::CacheSlots, Entries::One, scans4, n_points, n_scans, p, kind, slot_ids, nullptr));
 }
 
 int qb200_cache_scans_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids, int32_t n_scans,
                            const qb200_params* params, qb200_mem_kind kind) {
-  return run_call(h, cache_write(scans4, n_points, slot_ids, n_scans, params, true, kind));
+  return run_call(h, raw_scans(Sink::CacheSlots, Entries::Mixed, scans4, n_points, n_scans, params, kind, slot_ids, nullptr));
 }
 
 int qb200_cache_scans_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, const int32_t* slot_ids,
                                    int32_t n_scans, const qb200_params* params, qb200_mem_kind kind) {
-  return enqueue_call(h, cache_write(scans4, n_points, slot_ids, n_scans, params, true, kind));
+  return enqueue_call(h, raw_scans(Sink::CacheSlots, Entries::Mixed, scans4, n_points, n_scans, params, kind, slot_ids, nullptr));
 }
 
 int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_result* results) {
@@ -1313,86 +1442,86 @@ int qb200_register_cached(qb200_handle* h, const qb200_slot_pair* pairs, int32_t
 
 int qb200_register_cached_ex(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* p, qb200_result* results,
                              const qb200_pair_lists* lists) {
-  return run_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, p, false, results, lists});
+  return run_call(h, cached_pairs(Sink::Solve, Entries::One, pairs, n_pairs, p, results, lists));
 }
 
 int qb200_register_cached_each(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_result* results,
                                const qb200_pair_lists* lists) {
-  return run_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists});
+  return run_call(h, cached_pairs(Sink::Solve, Entries::Each, pairs, n_pairs, params, results, lists));
 }
 
 int qb200_register_cached_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                 qb200_result* results, const qb200_pair_lists* lists) {
-  return run_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists, true});
+  return run_call(h, cached_pairs(Sink::Solve, Entries::Mixed, pairs, n_pairs, params, results, lists));
 }
 
 int qb200_register_cached_enqueue_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                         qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_call(h, {nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists, true});
+  return enqueue_call(h, cached_pairs(Sink::Solve, Entries::Mixed, pairs, n_pairs, params, results, lists));
 }
 
 // ---- caller keypoints and descriptors -> pose ------------------------------------------------------------------------------
 int qb200_register_features_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                  qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
-  return run_call(h, feature_call(pairs, n_pairs, params, kind, results, lists));
+  return run_call(h, feature_pairs(Sink::Solve, pairs, n_pairs, params, kind, results, lists));
 }
 
 int qb200_register_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                          qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_call(h, feature_call(pairs, n_pairs, params, kind, results, lists));
+  return enqueue_call(h, feature_pairs(Sink::Solve, pairs, n_pairs, params, kind, results, lists));
 }
 
 // ---- raw scans -> voxel keypoints, normals and FPFH-33 in caller memory ---------------------------------------------------------
 int qb200_describe_batch_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans, const qb200_params* params,
                               qb200_mem_kind kind, const qb200_feature_out* out) {
-  return run_call(h, describe_call(scans4, n_points, n_scans, params, kind, out));
+  return run_call(h, raw_scans(Sink::Export, Entries::Mixed, scans4, n_points, n_scans, params, kind, nullptr, out));
 }
 
 int qb200_describe_batch_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
                                       const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out) {
-  return enqueue_call(h, describe_call(scans4, n_points, n_scans, params, kind, out));
+  return enqueue_call(h, raw_scans(Sink::Export, Entries::Mixed, scans4, n_points, n_scans, params, kind, nullptr, out));
 }
 
 // ---- caller keypoint clouds -> normals and FPFH-33 in caller memory -------------------------------------------------------------
 int qb200_describe_points_each(qb200_handle* h, const float* const* pts4, const int32_t* n_points, int32_t n_clouds, const qb200_params* params,
                                qb200_mem_kind kind, const qb200_feature_out* out) {
-  return run_call(h, describe_points_call(pts4, n_points, n_clouds, params, kind, out));
+  return run_call(h, keypoint_clouds(Sink::Export, pts4, n_points, n_clouds, params, kind, out));
 }
 
 int qb200_describe_points_enqueue_each(qb200_handle* h, const float* const* pts4, const int32_t* n_points, int32_t n_clouds,
                                        const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out) {
-  return enqueue_call(h, describe_points_call(pts4, n_points, n_clouds, params, kind, out));
+  return enqueue_call(h, keypoint_clouds(Sink::Export, pts4, n_points, n_clouds, params, kind, out));
 }
 
 // ---- raw, cached or caller-feature pairs -> correspondences and matched points, not solved --------------------------------------
 int qb200_match_batch_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
                             qb200_result* results, const qb200_pair_lists* lists) {
-  return run_call(h, match_call({pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists, true}));
+  return run_call(h, raw_pairs(Sink::Match, Entries::Mixed, pairs, n_pairs, params, kind, results, lists));
 }
 
 int qb200_match_batch_enqueue_mixed(qb200_handle* h, const qb200_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_mem_kind kind,
                                     qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_call(h, match_call({pairs, nullptr, nullptr, n_pairs, kind, params, true, results, lists, true}));
+  return enqueue_call(h, raw_pairs(Sink::Match, Entries::Mixed, pairs, n_pairs, params, kind, results, lists));
 }
 
 int qb200_match_cached_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params, qb200_result* results,
                              const qb200_pair_lists* lists) {
-  return run_call(h, match_call({nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists, true}));
+  return run_call(h, cached_pairs(Sink::Match, Entries::Mixed, pairs, n_pairs, params, results, lists));
 }
 
 int qb200_match_cached_enqueue_mixed(qb200_handle* h, const qb200_slot_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                      qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_call(h, match_call({nullptr, pairs, nullptr, n_pairs, QB200_MEM_HOST, params, true, results, lists, true}));
+  return enqueue_call(h, cached_pairs(Sink::Match, Entries::Mixed, pairs, n_pairs, params, results, lists));
 }
 
 int qb200_match_features_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
                               qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
-  return run_call(h, match_call(feature_call(pairs, n_pairs, params, kind, results, lists)));
+  return run_call(h, feature_pairs(Sink::Match, pairs, n_pairs, params, kind, results, lists));
 }
 
 int qb200_match_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                       qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
-  return enqueue_call(h, match_call(feature_call(pairs, n_pairs, params, kind, results, lists)));
+  return enqueue_call(h, feature_pairs(Sink::Match, pairs, n_pairs, params, kind, results, lists));
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

@@ -90,6 +90,17 @@ struct ExportDst {
   static size_t carve(unsigned char* base, int n, int cap, const qb200_feature_out& o, ExportDst* out);
 };
 
+// What a batch call reads (api.cu: BatchCall), per input: a pair of raw scans, a pair of cached scans (slots), a pair of caller
+// keypoint clouds with their FPFH-33 rows, a correspondence set, one raw scan, or one caller keypoint cloud
+enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, KeypointClouds };
+// What a batch call produces: solved records (and lists), the matcher's records (and lists), cache slots, or front-end features in
+// caller memory.  The valid (source, sink) pairs:
+//   RawPairs, CachedPairs, FeaturePairs  x  Solve, Match   qb200_register_batch*, _cached*, _features*; qb200_match_*
+//   CorrSets                             x  Solve          qb200_solve_batch*
+//   RawScans                             x  CacheSlots     qb200_cache_scans*
+//   RawScans, KeypointClouds             x  Export         qb200_describe_batch*, qb200_describe_points*
+enum class Sink { Solve, Match, CacheSlots, Export };
+
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
 // kernels of the others.  The lane owns its stream, buffers and events: deleting it releases them.
@@ -116,16 +127,17 @@ struct Lane {
   DeviceMem<FeatureSrc> d_feat; PinnedMem<FeatureSrc> h_feat;  // [2S] where a feature wave's clouds are read, and its pinned mirror
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
   unsigned pend_stages;      // ... the stage-time slots it reports (bit i: qb200_get_stage_ms slot i)
-  qb200_result* pend_dst;     // ... and the caller's record array of its batch
-  qb200_pair_lists pend_lists; // ... and a copy of its batch's list descriptor (cap_per_pair == 0: no lists)
-  // ... and the cache slots it reads (cached pairs) or writes (scans to cache), ascending and unique; empty: it does not touch the
+  Sink pend_sink;             // ... what wave_collect hands on for it: the fields below of its sink
+  qb200_result* pend_dst;     // ... (Solve, Match) the caller's record array of its batch, nullptr for the other sinks
+  bool pend_host_lists;       // ... (Solve, Match) its batch has host-kind lists, which wave_collect hands on from lst_stage
+  qb200_pair_lists pend_lists; // ... and then a copy of their descriptor
+  qb200_feature_out pend_out; // ... (Export) a copy of its batch's output descriptor, whose counts and status (and, in host kind,
+                              // entries) wave_collect hands on from exp_stage
+  // ... and the cache slots it reads (cached pairs) or writes (CacheSlots), ascending and unique; empty: it does not touch the
   // cache.  A wave reads the cache only in its copy-in and writes it only in its copy-out, so other lanes order their conflicting
   // copies after those events (api.cu: cache_waits)
   std::vector<int> pend_slots;
   int pend_writes;
-  // ... and (a describe wave: pend_out.cap_per_scan > 0) a copy of its batch's output descriptor, whose counts and status (and, in
-  // host kind, entries) wave_collect hands on from exp_stage
-  qb200_feature_out pend_out;
   Event ev_cache_in, ev_cache_out;
 
   // ---- sort workspace (voxel sort, then lattice sort) ----

@@ -13,7 +13,8 @@ from quatro_b200 import capi, synth
 from quatro_b200.capi import MEM_DEVICE, MEM_HOST, PMC_EXACT, INLIER_NONE, RESULT_DTYPE, Handle, default_params
 
 CSRC = Path(__file__).resolve().parent.parent / "quatro_b200" / "csrc"
-DELETED = ("run_waves", "solve_batch_impl", "enqueue_impl", "register_batch_impl", "register_cached_impl", "device_array_ok")
+DELETED = ("run_waves", "solve_batch_impl", "enqueue_impl", "register_batch_impl", "register_cached_impl", "device_array_ok",
+           "cache_write", "describe_call", "describe_points_call", "feature_call", "match_call")
 
 
 def _sources():
@@ -24,6 +25,14 @@ def _sources():
 def test_per_input_drivers_and_validators_are_gone():
     found = [f"{name}: {d}" for name, text in _sources().items() for d in DELETED if re.search(rf"\b{d}\b", text)]
     assert not found, "\n".join(found)
+
+
+def test_batch_call_names_its_source_and_sink():
+    """A call says what it reads and what it produces in two fields, not in flags beside its input pointers."""
+    body = re.search(r"struct BatchCall \{(.*?)\n\};", _sources()["api.cu"], re.S).group(1)
+    code = re.sub(r"//[^\n]*", "", body)
+    assert re.search(r"\bSource src\b", code) and re.search(r"\bSink sink\b", code), code
+    assert not re.findall(r"\b(describe|points|match)\s*[=;,]", code), code
 
 
 def test_one_wave_submit_call_site_and_one_pointer_query():
