@@ -31,6 +31,8 @@
  *                                  (src/teaser_utils/fpfh.cc:44-75)
  *   qb200_match_*               <- FPFHManager::setFeaturePair + getCorrespondences / getSrcMatched / getTgtMatched for every pair
  *                                  of a batch, without the solve (include/fpfh_manager.hpp:98-153, 234-236)
+ *   qb200_max_clique_batch_*    <- teaser::Graph + MaxCliqueSolver::findMaxClique for every caller graph of a batch
+ *                                  (include/teaser/graph.h:29-274, src/graph.cc:12-130)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -676,6 +678,50 @@ int qb200_describe_points_each(qb200_handle* h, const float* const* pts4, const 
  * which completes them.  The outputs are byte-identical to the blocking call's. */
 int qb200_describe_points_enqueue_each(qb200_handle* h, const float* const* pts4, const int32_t* n_points, int32_t n_clouds,
                                        const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out);
+
+/* --- maximum cliques of caller graphs in batches -------------------------------------------------------------------------------------
+ * teaser::Graph (include/teaser/graph.h:29-207) + teaser::MaxCliqueSolver::findMaxClique (graph.h:219-274, src/graph.cc:12-130) for a
+ * batch of graphs the library did not build: complete TIM graphs, consistency tests of the caller's own, pairwise-consistency outlier
+ * rejection across sessions.  Each graph runs the k-core peel and the clique search of qb200_max_clique_ex, in waves of max_batch_slots
+ * graphs over the lanes like every batch call.
+ *   Graph i is an edge list or an adjacency matrix in `kind` memory (below) and is solved with params[i].  Only inlier_selection_mode
+ *     (QB200_PMC_EXACT, QB200_PMC_HEU or QB200_KCORE_HEU), kcore_heuristic_threshold and max_clique_node_limit are read; every other
+ *     field is ignored.  QB200_INLIER_NONE, an unknown mode or a negative node limit gives QB200_ERR_BAD_ARG.
+ *   Edge lists have teaser::Graph::addEdge semantics: (u, v) and (v, u) are one edge, a repeated edge is ignored, and edge order never
+ *     matters.  In adjacency rows, bits at columns >= L are ignored.
+ *   Invalid graphs: a self-loop, a vertex outside [0, L), an adjacency matrix that is not symmetric or one with a diagonal bit gives
+ *     that graph the status QB200_ERR_BAD_ARG, in either memory kind.  This is decided on the device; the graph gets no clique and no
+ *     list entries, and the other graphs are unaffected.
+ *   Records.  status (QB200_OK for every valid graph), n_corr = L, n_edges (distinct undirected edges = Graph::numEdges()), max_core,
+ *     clique_size and flags (QB200_FLAG_CLIQUE_TRUNCATED, QB200_FLAG_LISTS_TRUNCATED).  Nothing is registered: valid = 0, T is the
+ *     identity, and n_src_vox, n_tgt_vox, n_mutual, gnc_iters, n_rot_inliers, n_final_inliers and cost are 0.
+ *   Lists.  Only clique may be non-NULL; any other list array gives QB200_ERR_BAD_ARG.  The clique is in ascending vertex ids, clipped
+ *     to cap_per_pair as in every _ex call.
+ *   Equality.  For every valid graph the record fields above and the clique are byte-identical to qb200_max_clique_ex on the same
+ *     adjacency with the same mode, threshold and node limit.  They never depend on the batch, the wave, the lane, the memory kinds,
+ *     edge list versus adjacency input, or the other graphs.
+ *   Checks run before anything starts or is queued: n < 0, L < 0 or L > max_corr, edges and adj both non-NULL, neither of them while
+ *     L > 0 and n_edges > 0, n_edges < 0, words_per_row < ceil(L / 32) with adj, a NULL results array, a bad params entry, a bad list
+ *     descriptor, and in QB200_MEM_DEVICE kind an array that is not memory of the handle's device or is misaligned (edges 8-byte, adj
+ *     4-byte).  A rejected call gives QB200_ERR_BAD_ARG, writes no record or list entry, queues nothing, and qb200_last_error names
+ *     the graph, entry or array; batches already queued still complete on the flush.
+ *   qb200_get_stage_ms reports [0] h2d (tables and host adjacency rows), [4] graph (the import and its checks, host edge lists
+ *     included: they cross PCIe in chunks under the import), [5] clique and [7] d2h; the other stages are 0.
+ * The params array and the list descriptor are copied by the call. */
+typedef struct qb200_graph {
+  const int32_t* edges;      /* n_edges x {u, v} (the teaser::Graph::addEdge calls), or NULL */
+  const uint32_t* adj;       /* L rows x words_per_row uint32, bit j of row i = edge (i, j) (qb200_max_clique's layout), or NULL */
+  int64_t n_edges;           /* edges only */
+  int32_t L;                 /* vertices 0 .. L-1 (Graph::populateVertices), <= max_corr */
+  int32_t words_per_row;     /* adj only: >= ceil(L / 32) */
+} qb200_graph;
+int qb200_max_clique_batch_each(qb200_handle* h, const qb200_graph* graphs, int32_t n_graphs, const qb200_params* params,
+                                qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+/* qb200_max_clique_batch_each, queued: completed by qb200_register_batch_flush like every enqueue, in one stream with every other
+ * enqueue form.  The graphs array is read by the call; host-kind edge lists and rows, `results` and the list arrays must stay valid
+ * until the flush returns.  Records and lists are byte-identical to the blocking call's. */
+int qb200_max_clique_batch_enqueue_each(qb200_handle* h, const qb200_graph* graphs, int32_t n_graphs, const qb200_params* params,
+                                        qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
 
 /* --- multi-GPU: batches of independent pairs shard across the GPUs of one box; the only communication is ONE all-gather (NCCL over
  * NVLink) of the fixed-size result records per batch -- north_star / SURVEY.md 8(e).  The reference has no counterpart (it is a

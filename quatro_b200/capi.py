@@ -94,6 +94,12 @@ class CorrSet(C.Structure):
     _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("L", C.c_int32), ("reserved", C.c_int32)]
 
 
+class Graph(C.Structure):
+    """qb200_graph: one caller graph of qb200_max_clique_batch_each, as an edge list or as adjacency rows (one of the two, or neither
+    for a graph without edges)."""
+    _fields_ = [("edges", C.c_void_p), ("adj", C.c_void_p), ("n_edges", C.c_int64), ("L", C.c_int32), ("words_per_row", C.c_int32)]
+
+
 class PairLists(C.Structure):
     """qb200_pair_lists: caller-owned per-pair lists of the batch entry points, cap_per_pair entries reserved per pair."""
     _fields_ = [("cap_per_pair", C.c_int32), ("kind", C.c_int32), ("corr", C.c_void_p), ("src_matched4", C.c_void_p),
@@ -133,6 +139,7 @@ LIST_LAYOUT = {
 }
 SET_LISTS = ("clique", "final_inliers", "rot_inlier_mask", "trans_inlier_mask")   # what qb200_solve_batch_ex can return
 MATCH_LISTS = ("corr", "src_matched4", "tgt_matched4")   # what the qb200_match_* calls can return
+GRAPH_LISTS = ("clique",)   # what qb200_max_clique_batch_each can return
 
 
 class ListBuffers:
@@ -270,6 +277,8 @@ _SIGNATURES = {
     "qb200_match_cached_enqueue_mixed": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
     "qb200_match_features_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_match_features_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_max_clique_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_max_clique_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -335,6 +344,26 @@ def _feature_array(pairs: Sequence, kind: int = MEM_HOST):
             arr[i].tgt, arr[i].tgt_desc, arr[i].n_tgt = t.ctypes.data, td.ctypes.data, len(t)
         else:
             arr[i].src, arr[i].src_desc, arr[i].n_src, arr[i].tgt, arr[i].tgt_desc, arr[i].n_tgt = pr
+    return arr, keep
+
+
+def _graph_array(graphs: Sequence):
+    """(Graph * n) array of `graphs`: each a Graph (pointers of any kind, used as they are), a (L, wpr) uint32 adjacency array, or an
+    (L, edges) tuple with an (m, 2) int32 edge array; and the contiguous host arrays it points to."""
+    arr = (Graph * max(len(graphs), 1))()
+    keep = []
+    for i, g in enumerate(graphs):
+        if isinstance(g, Graph):
+            arr[i] = g
+        elif isinstance(g, tuple):
+            L, e = g
+            e = np.ascontiguousarray(np.asarray(e, np.int32).reshape(-1, 2))
+            keep.append(e)
+            arr[i].edges, arr[i].n_edges, arr[i].L = (e.ctypes.data if len(e) else None), len(e), L
+        else:
+            a = np.ascontiguousarray(g, np.uint32)
+            keep.append(a)
+            arr[i].adj, arr[i].L, arr[i].words_per_row = (a.ctypes.data if a.size else None), a.shape[0], a.shape[1]
     return arr, keep
 
 
@@ -846,6 +875,30 @@ class Handle:
         return self._check(self.lib.qb200_match_features_enqueue_each(self.h, feature_array, n, params_array, kind, _ptr(out),
                                                                       self._lists_arg(self._match_lists(buffers))),
                            "qb200_match_features_enqueue_each")
+
+    # ---- caller graphs -> maximum cliques (qb200_max_clique_batch_each) ----
+    graph_array = staticmethod(_graph_array)
+
+    @staticmethod
+    def _graph_lists(buffers: Optional[ListBuffers]) -> Optional[ListBuffers]:
+        assert buffers is None or set(buffers.arrays) <= set(GRAPH_LISTS), "a graph batch returns the clique only"
+        return buffers
+
+    def max_clique_batch_each(self, graphs: Sequence, params: Sequence[Params], kind: int = MEM_HOST, buffers: Optional[ListBuffers] = None):
+        """qb200_max_clique_batch_each: graph i (see graph_array()) is solved with the inlier_selection_mode, kcore_heuristic_threshold
+        and max_clique_node_limit of params[i]; buffers: a ListBuffers of GRAPH_LISTS, or None for records only."""
+        assert len(params) == len(graphs)
+        arr, keep = self.graph_array(graphs)
+        return self._batch_lists("qb200_max_clique_batch_each", len(graphs), (arr, len(graphs), self.params_array(params), kind),
+                                 self._graph_lists(buffers))
+
+    def max_clique_batch_enqueue_each_raw(self, graph_array, n: int, params_array, kind: int, out: np.ndarray,
+                                          buffers: Optional[ListBuffers] = None):
+        """qb200_max_clique_batch_enqueue_each: graph_array (graph_array()) and params_array (params_array()) are read by the call; the
+        host arrays behind graph_array, `out` and the buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_max_clique_batch_enqueue_each(self.h, graph_array, n, params_array, kind, _ptr(out),
+                                                                        self._lists_arg(self._graph_lists(buffers))),
+                           "qb200_max_clique_batch_enqueue_each")
 
     def cache_scans_enqueue_each_raw(self, scan_ptrs, counts, slot_ids, n: int, params_array, kind: int):
         """qb200_cache_scans_enqueue_each: scan_ptrs / counts (_scan_arrays()), slot_ids (c_int32 * n) and params_array

@@ -102,6 +102,8 @@ int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   QB_CUDA_TRY(L, L->h_slot_of_cloud.alloc(C));
   QB_CUDA_TRY(L, L->d_feat.alloc(C));
   QB_CUDA_TRY(L, L->h_feat.alloc(C));
+  QB_CUDA_TRY(L, L->d_graph.alloc(S));
+  QB_CUDA_TRY(L, L->h_graph.alloc(S));
   // the sort workspace serves the voxel sort (C*R items, digit histograms in val_a, chunk counts C*kVsChunks <= n_sort in val_b),
   // the lattice / norm sorts (C*V items) and, afterwards, the duplicate-class tables of K6 (2S*V + 2S words in key_a): size it for
   // the largest user
@@ -269,6 +271,16 @@ PairSolve match_entry(const qb200_params& p) {
   PairSolve e;
   memset(&e, 0, sizeof(e));
   match_fields(&e, p);
+  return e;
+}
+
+// a graph wave's entry: the clique fields of p as qb200_max_clique_ex takes them, nothing of the graph or pose stages
+PairSolve clique_entry(const qb200_params& p) {
+  PairSolve e;
+  memset(&e, 0, sizeof(e));
+  e.kcore_thr = p.kcore_heuristic_threshold;
+  e.node_limit = p.max_clique_node_limit > 0 ? p.max_clique_node_limit : (long long)QB200_DEFAULT_CLIQUE_NODE_LIMIT;
+  e.mode = p.inlier_selection_mode;
   return e;
 }
 
@@ -469,10 +481,11 @@ struct BatchCall {
   const qb200_slot_pair* slots = nullptr;      // CachedPairs
   const qb200_feature_pair* feats = nullptr;   // FeaturePairs: keypoints and FPFH-33 rows, front-end fields of the entries ignored
   const qb200_corr_set* sets = nullptr;        // CorrSets
+  const qb200_graph* graphs = nullptr;         // Graphs
   const float* const* scans = nullptr;         // RawScans, KeypointClouds (described with the lattice fields of their entries alone):
   const int32_t* n_points = nullptr;           // scan i has n_points[i] points
   // the outputs, one set per sink
-  qb200_result* results = nullptr;             // Solve, Match: one record per input
+  qb200_result* results = nullptr;             // Solve, Match, Clique: one record per input
   const qb200_pair_lists* lists = nullptr;     // ... and the per-pair lists, nullptr = records only
   const int32_t* slot_ids = nullptr;           // CacheSlots: scan i goes to slot slot_ids[i]
   const qb200_feature_out* out = nullptr;      // Export: the caller's feature arrays
@@ -488,11 +501,12 @@ struct BatchCall {
 // The facts of each source that the checks and the waves read, written down once
 
 // clouds one input takes in the wave's 2S cloud buffers: two per pair, one per scan, none per set (its matched points go to ma / mb)
+// or graph (its adjacency goes to adj)
 int clouds_per_input(Source s) {
   switch (s) {
     case Source::RawPairs: case Source::CachedPairs: case Source::FeaturePairs: return 2;
     case Source::RawScans: case Source::KeypointClouds: return 1;
-    case Source::CorrSets: return 0;
+    case Source::CorrSets: case Source::Graphs: return 0;
   }
   return 0;
 }
@@ -501,42 +515,43 @@ int clouds_per_input(Source s) {
 bool is_pairs(Source s) { return clouds_per_input(s) == 2; }
 
 // Host-kind inputs of the source cross PCIe in a staged front (stage_raw, stage_features): a multi-wave batch sends them on the
-// shared copy stream and opens with a quarter wave.  Cached pairs and correspondence sets do neither.
+// shared copy stream and opens with a quarter wave.  Cached pairs, correspondence sets and graphs do neither.
 bool crosses_pcie(Source s) {
   switch (s) {
     case Source::RawPairs: case Source::FeaturePairs: case Source::RawScans: case Source::KeypointClouds: return true;
-    case Source::CachedPairs: case Source::CorrSets: return false;
+    case Source::CachedPairs: case Source::CorrSets: case Source::Graphs: return false;
   }
   return false;
 }
 
 // The wave uploads the front-end table d_front: K1..K5 (K2..K5 for keypoint clouds) read each cloud's entry.  The solver table
-// d_solve is uploaded by the waves with records (Solve, Match), i.e. of pairs and sets.
+// d_solve is uploaded by the waves with records (Solve, Match, Clique), i.e. of pairs, sets and graphs.
 bool runs_front_end(Source s) {
   switch (s) {
     case Source::RawPairs: case Source::RawScans: case Source::KeypointClouds: return true;
-    case Source::CachedPairs: case Source::FeaturePairs: case Source::CorrSets: return false;
+    case Source::CachedPairs: case Source::FeaturePairs: case Source::CorrSets: case Source::Graphs: return false;
   }
   return false;
 }
 
-bool has_records(Sink k) { return k == Sink::Solve || k == Sink::Match; }
+bool has_records(Sink k) { return k == Sink::Solve || k == Sink::Match || k == Sink::Clique; }
 
 // The stage-time slots of qb200_get_stage_ms a wave reports (bit i = slot i, the time between events i and i + 1 of Lane::ev).
 // A wave reports the stages its source runs: cached pairs their copy-in in the fpfh slot, caller features their copy and import in
 // h2d.  Cached pairs and sets report no d2h slot; waves without records report none (they register nothing).  A match wave reports
-// the slots up to match as its source has them, and d2h.
+// the slots up to match as its source has them, and d2h.  A graph wave reports h2d, its import in the graph slot, clique and d2h.
 unsigned stage_slots(Source s, Sink k) {
   enum : unsigned { kH2d = 1, kVoxel = 2, kFpfh = 4, kMatch = 8, kGraph = 16, kClique = 32, kPose = 64, kD2h = 128 };
   constexpr unsigned kSolver = kGraph | kClique | kPose;
   if (!has_records(k)) return 0u;
+  if (k == Sink::Clique) return kH2d | kGraph | kClique | kD2h;
   unsigned m = 0;
   switch (s) {
     case Source::RawPairs: m = kH2d | kVoxel | kFpfh | kMatch | kSolver | kD2h; break;
     case Source::FeaturePairs: m = kH2d | kMatch | kSolver | kD2h; break;
     case Source::CachedPairs: m = kFpfh | kMatch | kSolver; break;
     case Source::CorrSets: m = kSolver; break;
-    case Source::RawScans: case Source::KeypointClouds: break;
+    case Source::RawScans: case Source::KeypointClouds: case Source::Graphs: break;
   }
   return k == Sink::Match ? (m & (kH2d | kVoxel | kFpfh | kMatch)) | kD2h : m;
 }
@@ -654,12 +669,14 @@ int check_out(qb200_handle* h, const qb200_feature_out* o, bool points) {
 
 // A list descriptor from the caller: capacity and kind in range, device arrays on the handle's device and aligned for the pack's
 // vector stores; for_sets: the caller supplied the correspondences, so there are none to hand back; for_match: nothing is solved, so
-// there are no clique, final inliers or masks to hand back.
-int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets, bool for_match) {
+// there are no clique, final inliers or masks to hand back; for_graphs: a graph has a clique and nothing else.
+int check_lists(qb200_handle* h, const qb200_pair_lists* l, bool for_sets, bool for_match, bool for_graphs) {
   if (!l) return QB200_OK;
   const char* why = nullptr;
   if (l->cap_per_pair < 1 || l->cap_per_pair > h->cfg.max_corr) why = "cap_per_pair outside 1 .. max_corr";
   else if (l->kind != QB200_MEM_HOST && l->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the lists";
+  else if (for_graphs && (l->corr || l->src_matched4 || l->tgt_matched4 || l->final_inliers || l->rot_inlier_mask || l->trans_inlier_mask))
+    why = "a graph batch has only a clique to return";
   else if (for_sets && (l->corr || l->src_matched4 || l->tgt_matched4)) why = "a correspondence-set batch has no corr / matched points to return";
   else if (for_match && (l->clique || l->final_inliers || l->rot_inlier_mask || l->trans_inlier_mask))
     why = "a match call solves nothing: it has no clique, final inliers or inlier masks to return";
@@ -686,7 +703,7 @@ int fill_tables(Lane* L, const BatchCall& in, int w0, int np) {
       L->h_front[s] = own ? front_entry(p, in.src == Source::KeypointClouds) : L->h_front[0];
       continue;
     }
-    L->h_solve[s] = own ? (in.sink == Sink::Match ? match_entry(p) : solve_entry(p)) : L->h_solve[0];
+    L->h_solve[s] = !own ? L->h_solve[0] : in.sink == Sink::Match ? match_entry(p) : in.sink == Sink::Clique ? clique_entry(p) : solve_entry(p);
     if (in.src == Source::RawPairs) L->h_front[2 * s] = L->h_front[2 * s + 1] = own ? front_entry(p) : L->h_front[0];
   }
   int rc;
@@ -789,6 +806,73 @@ int front_sets(Lane* L, const BatchCall& in, int w0, int np) {
   return QB200_OK;
 }
 
+// Host edge lists cross PCIe through the larger of two lane buffers that a graph wave leaves idle: raw_stage (it reads no scans) and
+// adjp (K9 writes it only after the import).  Returns the capacity in edges.
+long long edge_stage(Lane* L, int2** out) {
+  const long long raw = 2LL * L->S * L->R * (long long)(sizeof(float4) / sizeof(int2));
+  const long long perm = (long long)L->S * L->Lc * L->W * (long long)sizeof(uint32_t) / (long long)sizeof(int2);
+  *out = raw >= perm ? reinterpret_cast<int2*>(L->raw_stage.get()) : reinterpret_cast<int2*>(L->adjp.get());
+  return raw >= perm ? raw : perm;
+}
+
+// Graphs: every graph's adjacency into its slot of adj.  Host rows arrive by one 2-D copy each; host edge lists are packed into the
+// edge staging as long as they fit, and a list that does not fit crosses in chunks after the wave's launch, each chunk imported before
+// the next one overwrites the staging (the stream orders them).  Device edges and rows are read in place.
+int front_graphs(Lane* L, const BatchCall& in, int w0, int np) {
+  cudaEventRecord(L->ev[0], L->stream);
+  if (int rc = wave_reset(L, 0)) return rc;
+  const bool host = in.kind == QB200_MEM_HOST;
+  int2* stage = nullptr;
+  const long long cap = edge_stage(L, &stage);
+  long long used = 0, max_edges = 0;
+  int max_L = 0;
+  std::vector<int> streamed;  // host edge lists that did not fit beside the others
+  for (int s = 0; s < np; ++s) {
+    const qb200_graph& g = in.graphs[w0 + s];
+    GraphSrc& e = L->h_graph[s];
+    e = GraphSrc{nullptr, nullptr, g.edges ? g.n_edges : 0, g.L, 0};
+    L->h_cloud_n[s] = g.L;
+    max_L = std::max(max_L, g.L);
+    if (g.adj && g.L > 0) {
+      uint32_t* slot = L->adj + (size_t)s * L->Lc * L->W;
+      const size_t nb = (size_t)(g.L + 31) / 32;
+      if (host)
+        QB_CUDA_TRY(L, cudaMemcpy2DAsync(slot, (size_t)L->W * 4, g.adj, (size_t)g.words_per_row * 4, nb * 4, g.L, cudaMemcpyHostToDevice,
+                                         L->stream));
+      e.rows = host ? slot : g.adj;
+      e.stride = host ? L->W : g.words_per_row;
+    }
+    if (!g.edges || g.n_edges <= 0) continue;
+    const int2* src = reinterpret_cast<const int2*>(g.edges);
+    if (!host) {
+      e.edges = src;
+    } else if (g.n_edges <= cap - used) {
+      QB_CUDA_TRY(L, cudaMemcpyAsync(stage + used, src, (size_t)g.n_edges * sizeof(int2), cudaMemcpyHostToDevice, L->stream));
+      e.edges = stage + used;
+      used += g.n_edges;
+    } else {
+      streamed.push_back(s);
+      continue;
+    }
+    max_edges = std::max(max_edges, (long long)g.n_edges);
+  }
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_graph, L->h_graph, (size_t)np * sizeof(GraphSrc), cudaMemcpyHostToDevice, L->stream));
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->ctr.n_corr, L->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, L->stream));
+  for (int i = 1; i <= 4; ++i) cudaEventRecord(L->ev[i], L->stream);  // no voxel, fpfh or match stage: slots 1 .. 3 are not reported
+  int rc;
+  if ((rc = launch_row_import(L, np, max_L)) || (rc = launch_edge_import(L, np, max_edges, -1, nullptr))) return rc;
+  for (const int s : streamed) {
+    const qb200_graph& g = in.graphs[w0 + s];
+    const int2* src = reinterpret_cast<const int2*>(g.edges);
+    for (long long off = 0; off < g.n_edges; off += cap) {
+      const long long m = std::min(cap, (long long)g.n_edges - off);
+      QB_CUDA_TRY(L, cudaMemcpyAsync(stage, src + off, (size_t)m * sizeof(int2), cudaMemcpyHostToDevice, L->stream));
+      if ((rc = launch_edge_import(L, 1, m, s, stage))) return rc;
+    }
+  }
+  return launch_symmetry_check(L, np, max_L);
+}
+
 // The end of every wave with records: the list pack, the D2H of the records
 int send_records(Lane* L, const BatchCall& in, int w0, int np) {
   if (in.lists)
@@ -814,6 +898,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     case Source::FeaturePairs: case Source::KeypointClouds: rc = front_features(h, L, in, w0, np, ncl); break;
     case Source::CachedPairs: rc = front_cached(h, L, in, w0, np, ncl); break;
     case Source::CorrSets: rc = front_sets(L, in, w0, np); break;
+    case Source::Graphs: rc = front_graphs(L, in, w0, np); break;
   }
   if (rc) return rc;
   const bool match_pairs = is_pairs(in.src);
@@ -838,6 +923,17 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_out, L->stream));
       break;
     case Sink::Export: rc = submit_export(L, *in.out, w0, ncl); break;
+    case Sink::Clique: {  // K9 on the imported graphs (a refused graph is in QB200_INLIER_NONE now, and every K9 kernel skips it)
+      bool exact = false;
+      for (int s = 0; s < np; ++s) exact |= L->h_solve[s].mode == QB200_PMC_EXACT;
+      cudaEventRecord(L->ev[5], L->stream);
+      if ((rc = launch_degree(L, np)) || (rc = launch_clique(L, np, exact))) return rc;
+      cudaEventRecord(L->ev[6], L->stream);
+      if ((rc = launch_clique_records(L, np))) return rc;
+      cudaEventRecord(L->ev[7], L->stream);
+      rc = send_records(L, in, w0, np);
+      break;
+    }
   }
   if (rc) return rc;
   L->pend_w0 = w0;
@@ -861,7 +957,7 @@ int wave_collect(qb200_handle* h, Lane* L) {
     return QB200_ERR_CUDA;
   }
   switch (L->pend_sink) {
-    case Sink::Solve: case Sink::Match:
+    case Sink::Solve: case Sink::Match: case Sink::Clique:
       memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
       if (L->pend_host_lists) deliver_lists(L, L->pend_lists, L->pend_w0, np);
       break;
@@ -956,6 +1052,7 @@ const void* input_of(const BatchCall& c) {
     case Source::FeaturePairs: return c.feats;
     case Source::CorrSets: return c.sets;
     case Source::RawScans: case Source::KeypointClouds: return c.scans;
+    case Source::Graphs: return c.graphs;
   }
   return nullptr;
 }
@@ -983,6 +1080,15 @@ int check_call(qb200_handle* h, const BatchCall& c) {
         return reject(why);
       }
     }
+  } else if (c.src == Source::Graphs) {  // only the clique fields are read
+    for (int i = 0; i < c.n; ++i) {
+      if (!p || (p[i].inlier_selection_mode != QB200_PMC_EXACT && p[i].inlier_selection_mode != QB200_PMC_HEU &&
+                 p[i].inlier_selection_mode != QB200_KCORE_HEU) || p[i].max_clique_node_limit < 0) {
+        snprintf(why, sizeof(why), "params entry %d is null, its inlier_selection_mode is not PMC_EXACT, PMC_HEU or KCORE_HEU, or its "
+                 "max_clique_node_limit is negative", i);
+        return reject(why);
+      }
+    }
   } else if (int rc = check_params(h, p, c.n, c.each(), c.src != Source::CorrSets && c.entries == Entries::Each, c.sink != Sink::Match)) {
     return rc;
   }
@@ -995,7 +1101,7 @@ int check_call(qb200_handle* h, const BatchCall& c) {
       return QB200_ERR_UNSUPPORTED;
     }
   }
-  if (int rc = check_lists(h, c.lists, c.src == Source::CorrSets, c.sink == Sink::Match)) return rc;
+  if (int rc = check_lists(h, c.lists, c.src == Source::CorrSets, c.sink == Sink::Match, c.src == Source::Graphs)) return rc;
   if (c.sink == Sink::Export)
     if (int rc = check_out(h, c.out, c.src == Source::KeypointClouds)) return rc;
   const int R = h->cfg.max_raw_points;
@@ -1051,6 +1157,21 @@ int check_call(qb200_handle* h, const BatchCall& c) {
           bad = "it is misaligned (16 bytes) or not memory of the handle's device";
         if (bad) {
           snprintf(why, sizeof(why), "cloud %d: %s", i, bad);
+          return reject(why);
+        }
+        break;
+      }
+      case Source::Graphs: {
+        const qb200_graph& g = c.graphs[i];
+        if (g.L < 0 || g.L > h->cfg.max_corr) bad = "L is outside 0 .. max_corr";
+        else if (g.edges && g.adj) bad = "edges and adj are both given";
+        else if (g.edges && g.n_edges < 0) bad = "n_edges < 0";
+        else if (!g.edges && !g.adj && g.L > 0 && g.n_edges > 0) bad = "it has edges but neither an edge list nor an adjacency matrix";
+        else if (g.adj && g.words_per_row < (g.L + 31) / 32) bad = "words_per_row < ceil(L / 32)";
+        else if (c.kind == QB200_MEM_DEVICE && !(device_array_of(h, g.edges, 8) && device_array_of(h, g.adj, 4)))
+          bad = "edges (8-byte) or adj (4-byte) misaligned or not memory of the handle's device";
+        if (bad) {
+          snprintf(why, sizeof(why), "graph %d: %s", i, bad);
           return reject(why);
         }
         break;
@@ -1173,7 +1294,7 @@ int run_call(qb200_handle* h, const BatchCall& c) {
   int rc = enqueue_call(h, c);
   const int rc2 = h ? batch_flush(h) : QB200_OK;
   if (rc == QB200_OK) rc = rc2;
-  if (rc == QB200_OK && c.n == 1 && has_records(c.sink)) set_last(h, c.results[0]);
+  if (rc == QB200_OK && c.n == 1 && (c.sink == Sink::Solve || c.sink == Sink::Match)) set_last(h, c.results[0]);
   return rc;
 }
 
@@ -1220,6 +1341,14 @@ BatchCall keypoint_clouds(Sink k, const float* const* pts4, const int32_t* n_poi
                           const qb200_feature_out* out) {
   BatchCall c{Source::KeypointClouds, k, n, kind, p, Entries::Mixed};
   c.scans = pts4; c.n_points = n_points; c.out = out;
+  return c;
+}
+
+// each graph is solved with its own entry
+BatchCall caller_graphs(const qb200_graph* graphs, int32_t n, const qb200_params* p, qb200_mem_kind kind, qb200_result* results,
+                        const qb200_pair_lists* lists) {
+  BatchCall c{Source::Graphs, Sink::Clique, n, kind, p, Entries::Mixed};
+  c.graphs = graphs; c.results = results; c.lists = lists;
   return c;
 }
 
@@ -1522,6 +1651,17 @@ int qb200_match_features_each(qb200_handle* h, const qb200_feature_pair* pairs, 
 int qb200_match_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                       qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
   return enqueue_call(h, feature_pairs(Sink::Match, pairs, n_pairs, params, kind, results, lists));
+}
+
+// ---- caller graphs -> maximum cliques ----------------------------------------------------------------------------------------------
+int qb200_max_clique_batch_each(qb200_handle* h, const qb200_graph* graphs, int32_t n_graphs, const qb200_params* params, qb200_mem_kind kind,
+                                qb200_result* results, const qb200_pair_lists* lists) {
+  return run_call(h, caller_graphs(graphs, n_graphs, params, kind, results, lists));
+}
+
+int qb200_max_clique_batch_enqueue_each(qb200_handle* h, const qb200_graph* graphs, int32_t n_graphs, const qb200_params* params,
+                                        qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_call(h, caller_graphs(graphs, n_graphs, params, kind, results, lists));
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

@@ -19,6 +19,9 @@
 // expression, and so does every test whose M exceeds 2^62 (the bound needs D^2, 2 beta^2 s' and q finite), so the adjacency is
 // bit-identical to the fp64 reference for any input.
 //
+// The same file imports caller graphs for qb200_max_clique_batch_each (edge lists or adjacency rows into the lane's adj, with the
+// validity checks of DESIGN.md 5.4) in place of K8.
+//
 // Work decomposition.  A WARP work item is 64 rows x 128 columns of the upper triangle (any pair of the launch: one global item
 // list); the warp stages its 64 row points in shared memory as (-2a, |a|^2 - beta^2/4 | -2b, |b|^2 - beta^2/4) -- read back as
 // broadcast operands of the FMAs -- and each lane keeps FOUR columns in registers.  No CTA barrier in
@@ -268,6 +271,155 @@ int launch_degree(Lane* h, int n_pairs) {
   if (n_pairs <= 0) return QB200_OK;
   const dim3 gd((h->Lc + 7) / 8, n_pairs);
   degree_kernel<<<gd, 256, 0, h->stream>>>(h->adj, h->ctr.n_corr, h->Lc, h->W, h->d_solve, h->deg, h->ctr.n_edges);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+
+// ---- caller graphs (qb200_max_clique_batch_each): the adjacency of a graph wave from the caller's edge lists or rows ----------------
+// Every kernel finds graph g's entry in the wave's table (GraphSrc) and writes only the L rows, ceil(L / 32) words each, that K9 reads.
+
+// a graph is invalid: its status, and a mode that every K9 kernel skips (degree_kernel leaves its n_edges 0)
+__device__ __forceinline__ void refuse_graph(int g, PairSolve* __restrict__ solve, int* __restrict__ status) {
+  status[g] = QB200_ERR_BAD_ARG;
+  solve[g].mode = QB200_INLIER_NONE;
+}
+
+constexpr int kImportThreads = 256;
+
+// blockIdx.y = graph: its rows into its slot, the bits at columns >= L cleared; an edge-list graph (rows == nullptr) gets zeros, which
+// edge_import_kernel then fills.  Host rows were copied into the slot beforehand and are masked in place.
+__global__ void __launch_bounds__(kImportThreads) row_import_kernel(const GraphSrc* __restrict__ table, int Lc, int W, uint32_t* __restrict__ adj) {
+  const int g = blockIdx.y;
+  const GraphSrc s = table[g];
+  const int nb = (s.L + 31) >> 5;
+  const long long words = (long long)s.L * nb;
+  const uint32_t last = (s.L & 31) ? (1u << (s.L & 31)) - 1u : ~0u;
+  uint32_t* __restrict__ G = adj + (size_t)g * Lc * W;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < words; i += (long long)gridDim.x * blockDim.x) {
+    const int r = (int)(i / nb), w = (int)(i % nb);
+    uint32_t x = 0u;
+    if (s.rows) {
+      x = s.rows[(size_t)r * s.stride + w];
+      if (w == nb - 1) x &= last;
+    }
+    G[(size_t)r * W + w] = x;
+  }
+}
+
+// Grid over (edge chunk, graph): both bits of every edge (u, v) with 0 <= u, v < L and u != v; any other edge refuses the graph.
+// only < 0: blockIdx.y = graph, its edges from its table entry (nullptr: none in this launch); only >= 0: graph `only`, n edges at e.
+// atomicOr makes repeated edges and both orientations of one edge set the same two bits, so neither order nor chunking matters.
+__global__ void __launch_bounds__(kImportThreads) edge_import_kernel(const GraphSrc* __restrict__ table, int only, const int2* __restrict__ e,
+                                                                     long long n, int Lc, int W, uint32_t* __restrict__ adj,
+                                                                     PairSolve* __restrict__ solve, int* __restrict__ status) {
+  const int g = only >= 0 ? only : blockIdx.y;
+  if (only < 0) {
+    e = table[g].edges;
+    n = table[g].n_edges;
+  }
+  if (!e) return;
+  const int L = table[g].L;
+  uint32_t* __restrict__ G = adj + (size_t)g * Lc * W;
+  bool bad = false;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int2 uv = e[i];
+    if ((unsigned)uv.x >= (unsigned)L || (unsigned)uv.y >= (unsigned)L || uv.x == uv.y) {
+      bad = true;
+      continue;
+    }
+    atomicOr(&G[(size_t)uv.x * W + (uv.y >> 5)], 1u << (uv.y & 31));
+    atomicOr(&G[(size_t)uv.y * W + (uv.x >> 5)], 1u << (uv.x & 31));
+  }
+  if (bad) refuse_graph(g, solve, status);
+}
+
+// One warp per 32 x 32 tile (bi, bj >= bi) of a row graph: lane l holds row bi*32 + l of tile (bi, bj) and row bj*32 + l of tile
+// (bj, bi); the transpose of the first (warp_transpose32) must equal the second, and a diagonal tile must have no bit (i, i).  Rows
+// at or past L count as empty (row_import_kernel cleared their columns in the rows below L).
+constexpr int kCheckWarps = 8;
+__global__ void __launch_bounds__(kCheckWarps * 32) symmetry_check_kernel(const GraphSrc* __restrict__ table, int Lc, int W,
+                                                                          const uint32_t* __restrict__ adj, PairSolve* __restrict__ solve,
+                                                                          int* __restrict__ status) {
+  const int g = blockIdx.y, lane = lane_id();
+  const GraphSrc s = table[g];
+  if (!s.rows) return;  // edge lists are symmetric and loop-free by construction
+  const int L = s.L, nb = (L + 31) >> 5;
+  const uint32_t* __restrict__ G = adj + (size_t)g * Lc * W;
+  bool fault = false;
+  for (long long t = (long long)blockIdx.x * kCheckWarps + (threadIdx.x >> 5); t < (long long)nb * nb; t += (long long)gridDim.x * kCheckWarps) {
+    const int bi = (int)(t / nb), bj = (int)(t % nb);
+    if (bj < bi) continue;  // warp-uniform: the lower tiles are the transposes of the upper ones
+    const int ri = bi * 32 + lane, rj = bj * 32 + lane;
+    const uint32_t a = ri < L ? G[(size_t)ri * W + bj] : 0u;
+    const uint32_t b = rj < L ? G[(size_t)rj * W + bi] : 0u;
+    fault |= warp_transpose32(a) != b;
+    if (bi == bj) fault |= ((a >> lane) & 1u) != 0u;
+  }
+  if (__any_sync(0xffffffffu, fault) && lane == 0) refuse_graph(g, solve, status);
+}
+
+// One thread per graph: the record of a graph wave.  A refused graph keeps its status and zero counters (K9 skipped it).
+__global__ void clique_records_kernel(qb200_result* __restrict__ results, int n_graphs, WaveCounters c) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n_graphs) return;
+  qb200_result* r = results + g;
+  r->valid = 0;
+  r->status = c.cloud_status[g];
+  r->n_src_vox = 0;
+  r->n_tgt_vox = 0;
+  r->n_mutual = 0;
+  r->n_corr = c.n_corr[g];
+  r->max_core = c.max_core[g];
+  r->clique_size = c.n_clique[g];
+  r->gnc_iters = 0;
+  r->n_rot_inliers = 0;
+  r->n_final_inliers = 0;
+  r->flags = c.flags[g];
+  r->n_edges = c.n_edges[g] / 2;
+  r->cost = 0.0;
+  for (int i = 0; i < 16; ++i) r->T[i] = (i % 5 == 0) ? 1.0 : 0.0;
+}
+
+// enough CTAs to cover `items` per graph at one item per thread, at most 4096 (the kernels stride)
+static unsigned import_ctas(long long items) {
+  const long long b = (items + kImportThreads - 1) / kImportThreads;
+  return (unsigned)(b < 1 ? 1 : b > 4096 ? 4096 : b);
+}
+
+int launch_row_import(Lane* h, int n_graphs, int max_L) {
+  if (n_graphs <= 0) return QB200_OK;
+  const long long nb = (max_L + 31) / 32;
+  row_import_kernel<<<dim3(import_ctas((long long)max_L * nb), n_graphs), kImportThreads, 0, h->stream>>>(h->d_graph, h->Lc, h->W, h->adj);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+
+int launch_edge_import(Lane* h, int n_graphs, long long max_edges, int only, const int2* edges) {
+  if (n_graphs <= 0 || max_edges <= 0) return QB200_OK;
+  const dim3 grid(import_ctas(max_edges), only >= 0 ? 1 : n_graphs);
+  edge_import_kernel<<<grid, kImportThreads, 0, h->stream>>>(h->d_graph, only, edges, max_edges, h->Lc, h->W, h->adj, h->d_solve,
+                                                             h->ctr.cloud_status);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+
+int launch_symmetry_check(Lane* h, int n_graphs, int max_L) {
+  if (n_graphs <= 0 || max_L <= 0) return QB200_OK;
+  const long long nb = (max_L + 31) / 32, warps_ctas = (nb * nb + kCheckWarps - 1) / kCheckWarps;
+  const unsigned ctas = (unsigned)(warps_ctas > 8192 ? 8192 : warps_ctas);
+  symmetry_check_kernel<<<dim3(ctas, n_graphs), kCheckWarps * 32, 0, h->stream>>>(h->d_graph, h->Lc, h->W, h->adj, h->d_solve,
+                                                                                   h->ctr.cloud_status);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+
+int launch_clique_records(Lane* h, int n_graphs) {
+  if (n_graphs <= 0) return QB200_OK;
+  clique_records_kernel<<<(n_graphs + 127) / 128, 128, 0, h->stream>>>(h->d_results, n_graphs, h->ctr);
   h->launches++;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;

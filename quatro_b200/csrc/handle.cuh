@@ -90,16 +90,27 @@ struct ExportDst {
   static size_t carve(unsigned char* base, int n, int cap, const qb200_feature_out& o, ExportDst* out);
 };
 
+// Where the import kernels of a graph wave read one caller graph (graph.cu): its edge list (n_edges {u, v} pairs, in the caller's
+// device memory or the lane's staging; nullptr = none, or streamed in chunks after the wave's launch) or its adjacency rows (stride
+// words apart, in the caller's device memory or already copied into the graph's slot of adj; nullptr = none), and its vertex count
+struct GraphSrc {
+  const int2* edges;
+  const uint32_t* rows;
+  long long n_edges;
+  int L, stride;
+};
+
 // What a batch call reads (api.cu: BatchCall), per input: a pair of raw scans, a pair of cached scans (slots), a pair of caller
-// keypoint clouds with their FPFH-33 rows, a correspondence set, one raw scan, or one caller keypoint cloud
-enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, KeypointClouds };
-// What a batch call produces: solved records (and lists), the matcher's records (and lists), cache slots, or front-end features in
-// caller memory.  The valid (source, sink) pairs:
+// keypoint clouds with their FPFH-33 rows, a correspondence set, one raw scan, one caller keypoint cloud, or one caller graph
+enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, KeypointClouds, Graphs };
+// What a batch call produces: solved records (and lists), the matcher's records (and lists), cache slots, front-end features in
+// caller memory, or max-clique records (and clique lists).  The valid (source, sink) pairs:
 //   RawPairs, CachedPairs, FeaturePairs  x  Solve, Match   qb200_register_batch*, _cached*, _features*; qb200_match_*
 //   CorrSets                             x  Solve          qb200_solve_batch*
 //   RawScans                             x  CacheSlots     qb200_cache_scans*
 //   RawScans, KeypointClouds             x  Export         qb200_describe_batch*, qb200_describe_points*
-enum class Sink { Solve, Match, CacheSlots, Export };
+//   Graphs                               x  Clique         qb200_max_clique_batch*
+enum class Sink { Solve, Match, CacheSlots, Export, Clique };
 
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
@@ -125,11 +136,12 @@ struct Lane {
   DeviceMem<float4> raw_stage; // [2S*R] staging for host inputs
   DeviceMem<int> d_slot_of_cloud; PinnedMem<int> h_slot_of_cloud;  // [2S] cache slot of every cloud of the wave, and its pinned mirror
   DeviceMem<FeatureSrc> d_feat; PinnedMem<FeatureSrc> h_feat;  // [2S] where a feature wave's clouds are read, and its pinned mirror
+  DeviceMem<GraphSrc> d_graph; PinnedMem<GraphSrc> h_graph;   // [S] where a graph wave's graphs are read, and its pinned mirror
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
   unsigned pend_stages;      // ... the stage-time slots it reports (bit i: qb200_get_stage_ms slot i)
   Sink pend_sink;             // ... what wave_collect hands on for it: the fields below of its sink
-  qb200_result* pend_dst;     // ... (Solve, Match) the caller's record array of its batch, nullptr for the other sinks
-  bool pend_host_lists;       // ... (Solve, Match) its batch has host-kind lists, which wave_collect hands on from lst_stage
+  qb200_result* pend_dst;     // ... (Solve, Match, Clique) the caller's record array of its batch, nullptr for the other sinks
+  bool pend_host_lists;       // ... (Solve, Match, Clique) its batch has host-kind lists, which wave_collect hands on from lst_stage
   qb200_pair_lists pend_lists; // ... and then a copy of their descriptor
   qb200_feature_out pend_out; // ... (Export) a copy of its batch's output descriptor, whose counts and status (and, in host kind,
                               // entries) wave_collect hands on from exp_stage
@@ -356,6 +368,17 @@ bool device_array_of(const qb200_handle* h, const void* a, size_t align);
 int wave_reset(Lane* L, int n_clouds);
 int stage_raw(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs);
 int launch_degree(Lane* h, int n_pairs);
+// Graph waves (graph.cu): the adjacency of graphs [0, n) from the table d_graph into their slots of adj.  launch_row_import writes the
+// L rows (ceil(L / 32) words each) of every graph: its caller rows with the bits at columns >= L cleared, or zeros for an edge list.
+// launch_edge_import then sets both bits of every edge: of every graph whose table entry has edges (only < 0), or of the n edges at
+// `edges` of graph `only` alone (a chunk of a host edge list).  launch_symmetry_check compares every 32 x 32 tile of a row graph
+// with its transpose.  An invalid edge, an asymmetric pair of tiles or a diagonal bit gives the graph status QB200_ERR_BAD_ARG in
+// ctr.cloud_status and the mode QB200_INLIER_NONE in d_solve, so that K9 skips it.  max_L: the largest L of the graphs (grid size).
+int launch_row_import(Lane* h, int n_graphs, int max_L);
+int launch_edge_import(Lane* h, int n_graphs, long long max_edges, int only, const int2* edges);
+int launch_symmetry_check(Lane* h, int n_graphs, int max_L);
+// a graph wave's records (graphs [0, n), after K9): status, L, edges, max core, clique size and flags; the rest as a match record
+int launch_clique_records(Lane* h, int n_graphs);
 // the checks every entry of a registering call passes; solver = false: the front-end and matcher fields only (a match call)
 bool params_ok(const qb200_params* p, bool solver = true);
 float lattice_cell(const qb200_params& p);
