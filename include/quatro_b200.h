@@ -33,6 +33,8 @@
  *                                  of a batch, without the solve (include/fpfh_manager.hpp:98-153, 234-236)
  *   qb200_max_clique_batch_*    <- teaser::Graph + MaxCliqueSolver::findMaxClique for every caller graph of a batch
  *                                  (include/teaser/graph.h:29-274, src/graph.cc:12-130)
+ *   qb200_build_graph_batch_*   <- Quatro::computeTIMs + solveForScale + inlier_graph_.addEdge loop for every correspondence set of
+ *                                  a batch, the graph handed out (include/quatro.hpp:307-386, 784-789)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -722,6 +724,55 @@ int qb200_max_clique_batch_each(qb200_handle* h, const qb200_graph* graphs, int3
  * until the flush returns.  Records and lists are byte-identical to the blocking call's. */
 int qb200_max_clique_batch_enqueue_each(qb200_handle* h, const qb200_graph* graphs, int32_t n_graphs, const qb200_params* params,
                                         qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+
+/* --- TIM consistency graphs of correspondence sets in batches -------------------------------------------------------------------------
+ * Quatro::computeTIMs + solveForScale + the inlier_graph_.addEdge loop (include/quatro.hpp:307-386, 784-789) for every set of a batch,
+ * handed out instead of solved: for a clique or outlier solver of the caller's own, graph statistics as a loop-closure pre-filter, or
+ * one graph solved in several modes by qb200_max_clique_batch_each without building it again.  Sets run in waves of max_batch_slots
+ * over the lanes like every batch call.
+ *   Params.  Set i is built with params[i].noise_bound and params[i].cbar2 (beta = 2 noise_bound sqrt(cbar2)), which must be > 0 as
+ *     qb200_build_graph requires.  Every other field is ignored, inlier_selection_mode included: a QB200_INLIER_NONE entry still gets
+ *     its graph.  Nothing is latched (rot_noise_bound is neither read nor resolved).
+ *   Adjacency.  Set i's L rows at adj + i * rows_per_set * words_per_row are byte-identical to qb200_build_graph on that set alone with
+ *     the same noise_bound, cbar2 and words_per_row: words ceil(L / 32) .. words_per_row - 1 are written as zero.  Rows L ..
+ *     rows_per_set - 1 are left untouched.
+ *   Degrees.  Set i's L entries at degree + i * rows_per_set are qb200_build_graph's degree; entries past L are left untouched.
+ *   Edges.  Set i's list at edges + 2 * i * cap_edges is every edge {u, v}, u < v, in ascending (u, v) order: the sequence of the
+ *     reference's inlier_graph_.addEdge calls.  min(n_edges, cap_edges) entries are written and nothing past them; a clipped list sets
+ *     QB200_FLAG_LISTS_TRUNCATED in the record.
+ *   Records.  status = QB200_OK for every set (L = 0 or 1 included: the graph is empty), n_corr = L, n_edges = qb200_build_graph's count,
+ *     flags as above.  Nothing is solved: valid = 0, T is the identity, and every other counter and cost are 0.
+ *   Equality.  No output depends on the batch, the wave, the lane, QB200_LANES, the input or output memory kinds, or the other sets.
+ *   Checks run before anything starts or is queued: the set checks of qb200_solve_batch_each (L outside 0 .. max_corr, null points), a
+ *     bad params entry, a NULL results or out, an unknown kind or out->kind, rows_per_set below some set's L while adj or degree is
+ *     given, words_per_row < ceil(rows_per_set / 32) with adj, cap_edges < 1 with edges, and in QB200_MEM_DEVICE output kind an array
+ *     that is not memory of the handle's device or is misaligned (adj and degree 4-byte, edges 8-byte).  A rejected call gives
+ *     QB200_ERR_BAD_ARG, writes no record or output entry, queues nothing, and qb200_last_error names the set, entry or array; batches
+ *     already queued still complete on the flush.
+ *   qb200_get_stage_ms reports [0] h2d, [4] graph (K8, the degrees and the device-kind outputs) and [7] d2h; the other stages are 0.
+ *   qb200_get_kernel_ms[1] counts tim_graph_kernel as a solve batch does.
+ * QB200_MEM_HOST outputs are complete when the call returns (enqueue: when the flush returns); QB200_MEM_DEVICE outputs are written by the
+ * call's stream work under the same rule.  The params array and the output descriptor are copied by the call.
+ * {edges + 2 * i * cap_edges, NULL, n_edges, L, 0} (when n_edges <= cap_edges) and {NULL, adj + i * rows_per_set * words_per_row, 0, L,
+ * words_per_row} are set i's qb200_graph for qb200_max_clique_batch_each in the same memory kind, device arrays included. */
+typedef struct qb200_graph_out {
+  int32_t kind;            /* qb200_mem_kind of the three arrays (QB200_MEM_DEVICE: memory of the handle's device) */
+  int32_t rows_per_set;    /* adj, degree: rows reserved per set (>= every set's L when either is given) */
+  int32_t words_per_row;   /* adj: >= ceil(rows_per_set / 32) */
+  int32_t reserved;
+  int64_t cap_edges;       /* edges: entries reserved per set (>= 1 when edges is given) */
+  uint32_t* adj;           /* [n][rows_per_set][words_per_row], bit j of row i = edge (i, j): qb200_build_graph's layout, or NULL */
+  int32_t* degree;         /* [n][rows_per_set], or NULL */
+  int32_t* edges;          /* [n][cap_edges][2] {u, v}, u < v, or NULL */
+} qb200_graph_out;
+int qb200_build_graph_batch_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params,
+                                 qb200_mem_kind kind, qb200_result* results, const qb200_graph_out* out);
+/* qb200_build_graph_batch_each, queued: completed by qb200_register_batch_flush like every enqueue, in one stream with every other
+ * enqueue form, and returns without waiting for its own waves.  Host-kind sets, `results` and host-kind output arrays must stay valid
+ * until the flush returns; host-kind outputs are written when their wave is collected.  Records and outputs are byte-identical to the
+ * blocking call's. */
+int qb200_build_graph_batch_enqueue_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params,
+                                         qb200_mem_kind kind, qb200_result* results, const qb200_graph_out* out);
 
 /* --- multi-GPU: batches of independent pairs shard across the GPUs of one box; the only communication is ONE all-gather (NCCL over
  * NVLink) of the fixed-size result records per batch -- north_star / SURVEY.md 8(e).  The reference has no counterpart (it is a

@@ -100,6 +100,12 @@ class Graph(C.Structure):
     _fields_ = [("edges", C.c_void_p), ("adj", C.c_void_p), ("n_edges", C.c_int64), ("L", C.c_int32), ("words_per_row", C.c_int32)]
 
 
+class GraphOut(C.Structure):
+    """qb200_graph_out: caller-owned outputs of qb200_build_graph_batch_each: adjacency rows, degrees and edge lists of every set."""
+    _fields_ = [("kind", C.c_int32), ("rows_per_set", C.c_int32), ("words_per_row", C.c_int32), ("reserved", C.c_int32),
+                ("cap_edges", C.c_int64), ("adj", C.c_void_p), ("degree", C.c_void_p), ("edges", C.c_void_p)]
+
+
 class PairLists(C.Structure):
     """qb200_pair_lists: caller-owned per-pair lists of the batch entry points, cap_per_pair entries reserved per pair."""
     _fields_ = [("cap_per_pair", C.c_int32), ("kind", C.c_int32), ("corr", C.c_void_p), ("src_matched4", C.c_void_p),
@@ -178,6 +184,53 @@ class ListBuffers:
                 m = 0 if r["status"] == 3 else min(int(r[LIST_LAYOUT[name][2]]), self.cap)
                 d[name] = a[i, :m].copy() if self.kind == MEM_HOST else a[i, :m]
             out.append(d)
+        return out
+
+
+class GraphBuffers:
+    """The arrays of one qb200_graph_out: numpy arrays (MEM_HOST) or CUDA tensors of `device` (MEM_DEVICE, adj held as int32), filled
+    with `fill`: adj (n, rows_per_set, words_per_row) uint32, degree (n, rows_per_set) int32, edges (n, cap_edges, 2) int32."""
+    SHAPES = {"adj": (np.uint32, lambda b: (b.rows_per_set, b.words_per_row)), "degree": (np.int32, lambda b: (b.rows_per_set,)),
+              "edges": (np.int32, lambda b: (b.cap_edges, 2))}
+
+    def __init__(self, n: int, rows_per_set: int, words_per_row: int, cap_edges: int, kind: int = MEM_HOST,
+                 arrays: Sequence[str] = ("adj", "degree", "edges"), device: int = 0, fill: int = 0):
+        self.n, self.rows_per_set, self.words_per_row, self.cap_edges, self.kind = n, rows_per_set, words_per_row, cap_edges, kind
+        self.arrays = {}
+        for name in arrays:
+            dt, shape = self.SHAPES[name]
+            a = np.full((max(n, 1), *shape(self)), fill, np.int64).astype(dt)
+            if kind == MEM_HOST:
+                self.arrays[name] = a
+            else:
+                import torch
+                self.arrays[name] = torch.from_numpy(a.view(np.int32)).to(f"cuda:{device}")
+
+    def descriptor(self) -> GraphOut:
+        d = GraphOut(self.kind, self.rows_per_set, self.words_per_row, 0, self.cap_edges)
+        for name, a in self.arrays.items():
+            setattr(d, name, a.ctypes.data if self.kind == MEM_HOST else a.data_ptr())
+        return d
+
+    def host(self, name: str) -> np.ndarray:
+        """the array as numpy (a copy of a device array), adj as uint32"""
+        a = self.arrays[name]
+        a = a if self.kind == MEM_HOST else a.cpu().numpy()
+        return a.view(self.SHAPES[name][0])
+
+    def graphs(self, records: np.ndarray, use: str = "edges") -> list:
+        """Per set the Graph that qb200_max_clique_batch_each takes, in this kind: its edge list (use="edges"; a clipped list is
+        refused) or its adjacency rows (use="adj")."""
+        a = self.arrays[use]
+        base = a.ctypes.data if self.kind == MEM_HOST else a.data_ptr()
+        out = []
+        for i, r in enumerate(records):
+            L = int(r["n_corr"])
+            if use == "edges":
+                assert not r["flags"] & FLAG_LISTS_TRUNCATED, f"set {i}: its edge list was clipped to cap_edges"
+                out.append(Graph(base + 8 * i * self.cap_edges, None, int(r["n_edges"]), L, 0))
+            else:
+                out.append(Graph(None, base + 4 * i * self.rows_per_set * self.words_per_row, 0, L, self.words_per_row))
         return out
 
 
@@ -279,6 +332,8 @@ _SIGNATURES = {
     "qb200_match_features_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_max_clique_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_max_clique_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_build_graph_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(GraphOut)]),
+    "qb200_build_graph_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(GraphOut)]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -899,6 +954,26 @@ class Handle:
         return self._check(self.lib.qb200_max_clique_batch_enqueue_each(self.h, graph_array, n, params_array, kind, _ptr(out),
                                                                         self._lists_arg(self._graph_lists(buffers))),
                            "qb200_max_clique_batch_enqueue_each")
+
+    # ---- correspondence sets -> TIM graphs (qb200_build_graph_batch_each) ----
+    def build_graph_batch_each(self, sets: Sequence, params: Sequence[Params], kind: int = MEM_HOST,
+                               buffers: Optional[GraphBuffers] = None) -> np.ndarray:
+        """qb200_build_graph_batch_each: set i (as solve_batch takes it) is built with the noise_bound and cbar2 of params[i]; its
+        adjacency rows, degrees and edge list go to `buffers` (None: records only).  Returns the records."""
+        assert len(params) == len(sets)
+        arr, keep = self._set_array(sets, kind)
+        out = np.zeros(len(sets), RESULT_DTYPE)
+        d = GraphOut() if buffers is None else buffers.descriptor()
+        self._check(self.lib.qb200_build_graph_batch_each(self.h, arr, len(sets), self.params_array(params), kind, _ptr(out), C.byref(d)),
+                    "qb200_build_graph_batch_each")
+        return out
+
+    def build_graph_batch_enqueue_each_raw(self, set_array, n: int, params_array, kind: int, out: np.ndarray, buffers: GraphBuffers):
+        """qb200_build_graph_batch_enqueue_each: params_array (params_array()) and the descriptor are copied by the call; set_array
+        (_set_array()), its points (host kind), `out` and the buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_build_graph_batch_enqueue_each(self.h, set_array, n, params_array, kind, _ptr(out),
+                                                                         C.byref(buffers.descriptor())),
+                           "qb200_build_graph_batch_enqueue_each")
 
     def cache_scans_enqueue_each_raw(self, scan_ptrs, counts, slot_ids, n: int, params_array, kind: int):
         """qb200_cache_scans_enqueue_each: scan_ptrs / counts (_scan_arrays()), slot_ids (c_int32 * n) and params_array

@@ -284,6 +284,16 @@ PairSolve clique_entry(const qb200_params& p) {
   return e;
 }
 
+// a TIM graph wave's entry: K8's beta from noise_bound and cbar2, and a mode that builds the graph (K8 and degree_kernel skip
+// QB200_INLIER_NONE), as qb200_build_graph sets them; nothing of the matcher, clique or pose stages
+PairSolve graph_entry(const qb200_params& p) {
+  PairSolve e;
+  memset(&e, 0, sizeof(e));
+  e.gc = graph_const(p.noise_bound, p.cbar2);
+  e.mode = QB200_PMC_HEU;
+  return e;
+}
+
 PairSolve solve_entry(const qb200_params& p) {
   PairSolve e;
   memset(&e, 0, sizeof(e));
@@ -485,10 +495,11 @@ struct BatchCall {
   const float* const* scans = nullptr;         // RawScans, KeypointClouds (described with the lattice fields of their entries alone):
   const int32_t* n_points = nullptr;           // scan i has n_points[i] points
   // the outputs, one set per sink
-  qb200_result* results = nullptr;             // Solve, Match, Clique: one record per input
+  qb200_result* results = nullptr;             // Solve, Match, Clique, Graph: one record per input
   const qb200_pair_lists* lists = nullptr;     // ... and the per-pair lists, nullptr = records only
   const int32_t* slot_ids = nullptr;           // CacheSlots: scan i goes to slot slot_ids[i]
   const qb200_feature_out* out = nullptr;      // Export: the caller's feature arrays
+  const qb200_graph_out* graph_out = nullptr;  // Graph: the caller's adjacency, degree and edge arrays
   // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved (Solve), laid out like `caller`.
   const qb200_params* params = nullptr;
   // host inputs of a multi-wave batch crossing PCIe: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies
@@ -534,17 +545,19 @@ bool runs_front_end(Source s) {
   return false;
 }
 
-bool has_records(Sink k) { return k == Sink::Solve || k == Sink::Match || k == Sink::Clique; }
+bool has_records(Sink k) { return k == Sink::Solve || k == Sink::Match || k == Sink::Clique || k == Sink::Graph; }
 
 // The stage-time slots of qb200_get_stage_ms a wave reports (bit i = slot i, the time between events i and i + 1 of Lane::ev).
 // A wave reports the stages its source runs: cached pairs their copy-in in the fpfh slot, caller features their copy and import in
 // h2d.  Cached pairs and sets report no d2h slot; waves without records report none (they register nothing).  A match wave reports
-// the slots up to match as its source has them, and d2h.  A graph wave reports h2d, its import in the graph slot, clique and d2h.
+// the slots up to match as its source has them, and d2h.  A graph wave reports h2d, its import in the graph slot, clique and d2h; a
+// TIM graph wave h2d, graph (K8 and its outputs) and d2h.
 unsigned stage_slots(Source s, Sink k) {
   enum : unsigned { kH2d = 1, kVoxel = 2, kFpfh = 4, kMatch = 8, kGraph = 16, kClique = 32, kPose = 64, kD2h = 128 };
   constexpr unsigned kSolver = kGraph | kClique | kPose;
   if (!has_records(k)) return 0u;
   if (k == Sink::Clique) return kH2d | kGraph | kClique | kD2h;
+  if (k == Sink::Graph) return kH2d | kGraph | kD2h;
   unsigned m = 0;
   switch (s) {
     case Source::RawPairs: m = kH2d | kVoxel | kFpfh | kMatch | kSolver | kD2h; break;
@@ -667,6 +680,25 @@ int check_out(qb200_handle* h, const qb200_feature_out* o, bool points) {
   return QB200_ERR_BAD_ARG;
 }
 
+// The output descriptor of a TIM graph call: a known kind, row and word counts that hold the rows asked for, a capacity for the edges
+// asked for, and device arrays on the handle's device and aligned for the kernels' stores.  Each set's L is checked against
+// rows_per_set with the set.
+int check_graph_out(qb200_handle* h, const qb200_graph_out* o) {
+  const char* why = nullptr;
+  const bool device = o && o->kind == QB200_MEM_DEVICE;
+  if (!o) why = "the output descriptor is null";
+  else if (o->kind != QB200_MEM_HOST && o->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the outputs";
+  else if ((o->adj || o->degree) && o->rows_per_set < 0) why = "rows_per_set < 0";
+  else if (o->adj && o->words_per_row < (o->rows_per_set + 31LL) / 32) why = "words_per_row < ceil(rows_per_set / 32)";
+  else if (o->edges && o->cap_edges < 1) why = "cap_edges < 1";
+  else if (device && !device_array_of(h, o->adj, 4)) why = "device adj is misaligned or not memory of the handle's device";
+  else if (device && !device_array_of(h, o->degree, 4)) why = "device degree is misaligned or not memory of the handle's device";
+  else if (device && !device_array_of(h, o->edges, 8)) why = "device edges is misaligned or not memory of the handle's device";
+  if (!why) return QB200_OK;
+  h->fail(__FILE__, __LINE__, why);
+  return QB200_ERR_BAD_ARG;
+}
+
 // A list descriptor from the caller: capacity and kind in range, device arrays on the handle's device and aligned for the pack's
 // vector stores; for_sets: the caller supplied the correspondences, so there are none to hand back; for_match: nothing is solved, so
 // there are no clique, final inliers or masks to hand back; for_graphs: a graph has a clique and nothing else.
@@ -703,7 +735,11 @@ int fill_tables(Lane* L, const BatchCall& in, int w0, int np) {
       L->h_front[s] = own ? front_entry(p, in.src == Source::KeypointClouds) : L->h_front[0];
       continue;
     }
-    L->h_solve[s] = !own ? L->h_solve[0] : in.sink == Sink::Match ? match_entry(p) : in.sink == Sink::Clique ? clique_entry(p) : solve_entry(p);
+    L->h_solve[s] = !own                      ? L->h_solve[0]
+                    : in.sink == Sink::Match  ? match_entry(p)
+                    : in.sink == Sink::Clique ? clique_entry(p)
+                    : in.sink == Sink::Graph  ? graph_entry(p)
+                                              : solve_entry(p);
     if (in.src == Source::RawPairs) L->h_front[2 * s] = L->h_front[2 * s + 1] = own ? front_entry(p) : L->h_front[0];
   }
   int rc;
@@ -792,6 +828,7 @@ int front_cached(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np, 
 
 // Correspondence sets: the matched points of every set into ma / mb and its size into n_corr
 int front_sets(Lane* L, const BatchCall& in, int w0, int np) {
+  cudaEventRecord(L->ev[0], L->stream);
   if (int rc = wave_reset(L, 0)) return rc;
   const cudaMemcpyKind ck = in.kind == QB200_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
   for (int s = 0; s < np; ++s) {
@@ -803,6 +840,7 @@ int front_sets(Lane* L, const BatchCall& in, int w0, int np) {
     }
   }
   QB_CUDA_TRY(L, cudaMemcpyAsync(L->ctr.n_corr, L->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, L->stream));
+  for (int i = 1; i <= 4; ++i) cudaEventRecord(L->ev[i], L->stream);  // no voxel, fpfh or match stage: slots 1 .. 3 are not reported
   return QB200_OK;
 }
 
@@ -873,6 +911,61 @@ int front_graphs(Lane* L, const BatchCall& in, int w0, int np) {
   return launch_symmetry_check(L, np, max_L);
 }
 
+// TIM graphs: K8 and the degrees, then the device-kind outputs written straight into the caller's arrays, the edge offsets of every
+// set when edges are asked for (host-kind edges are emitted from them at collect time) and the records
+int submit_graph(Lane* L, const qb200_graph_out& o, int w0, int np) {
+  int rc;
+  if ((rc = launch_graph(L, np))) return rc;
+  const bool device = o.kind == QB200_MEM_DEVICE;
+  const size_t rows0 = (size_t)w0 * o.rows_per_set;
+  if (device) {
+    const GraphDst d{o.adj ? o.adj + rows0 * o.words_per_row : nullptr, o.degree ? o.degree + rows0 : nullptr, o.rows_per_set,
+                     o.words_per_row};
+    if ((rc = launch_graph_export(L, np, d))) return rc;
+  }
+  if (o.edges && (rc = launch_edge_offsets(L, np))) return rc;
+  if (o.edges && device) {
+    int2* e = reinterpret_cast<int2*>(o.edges) + (size_t)w0 * o.cap_edges;
+    if ((rc = launch_edge_emit(L, np, -1, 0, o.cap_edges, e, o.cap_edges))) return rc;
+  }
+  return launch_graph_records(L, np, o.edges ? o.cap_edges : 0);
+}
+
+// A collected TIM graph wave's host-kind outputs (h_results holds its records), before the lane is reused: each set's rows by one
+// 2-D copy with the words past ceil(L / 32) zeroed here, its degrees by one copy, and its edge list emitted in windows through the
+// edge staging (K9 does not run in a graph wave, so it is idle), each window copied out before the next one overwrites it.
+int deliver_graph(Lane* L, const qb200_graph_out& o, int w0, int np) {
+  int2* stage = nullptr;
+  const long long cap = edge_stage(L, &stage);
+  int rc;
+  for (int s = 0; s < np; ++s) {
+    const qb200_result& r = L->h_results[s];
+    const int n = r.n_corr, nb = (n + 31) / 32;
+    const size_t row0 = (size_t)(w0 + s) * o.rows_per_set;
+    if (o.adj && n > 0)
+      QB_CUDA_TRY(L, cudaMemcpy2DAsync(o.adj + row0 * o.words_per_row, (size_t)o.words_per_row * 4, L->adj + (size_t)s * L->Lc * L->W,
+                                       (size_t)L->W * 4, (size_t)nb * 4, n, cudaMemcpyDeviceToHost, L->stream));
+    if (o.degree && n > 0)
+      QB_CUDA_TRY(L, cudaMemcpyAsync(o.degree + row0, L->deg + (size_t)s * L->Lc, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
+    if (!o.edges) continue;
+    int2* dst = reinterpret_cast<int2*>(o.edges) + (size_t)(w0 + s) * o.cap_edges;
+    const long long m = std::min((long long)r.n_edges, (long long)o.cap_edges);
+    for (long long e0 = 0; e0 < m; e0 += cap) {
+      const long long e1 = std::min(m, e0 + cap);
+      if ((rc = launch_edge_emit(L, 1, s, e0, e1, stage, 0))) return rc;
+      QB_CUDA_TRY(L, cudaMemcpyAsync(dst + e0, stage, (size_t)(e1 - e0) * sizeof(int2), cudaMemcpyDeviceToHost, L->stream));
+    }
+  }
+  QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
+  for (int s = 0; o.adj && s < np; ++s) {
+    const int n = L->h_results[s].n_corr, nb = (n + 31) / 32;
+    if (o.words_per_row == nb) continue;
+    uint32_t* rows = o.adj + (size_t)(w0 + s) * o.rows_per_set * o.words_per_row;
+    for (int i = 0; i < n; ++i) memset(rows + (size_t)i * o.words_per_row + nb, 0, (size_t)(o.words_per_row - nb) * sizeof(uint32_t));
+  }
+  return QB200_OK;
+}
+
 // The end of every wave with records: the list pack, the D2H of the records
 int send_records(Lane* L, const BatchCall& in, int w0, int np) {
   if (in.lists)
@@ -923,6 +1016,11 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_out, L->stream));
       break;
     case Sink::Export: rc = submit_export(L, *in.out, w0, ncl); break;
+    case Sink::Graph:  // no clique or pose stage: the graph slot holds K8 and the outputs
+      if ((rc = submit_graph(L, *in.graph_out, w0, np))) return rc;
+      for (int i = 5; i <= 7; ++i) cudaEventRecord(L->ev[i], L->stream);
+      rc = send_records(L, in, w0, np);
+      break;
     case Sink::Clique: {  // K9 on the imported graphs (a refused graph is in QB200_INLIER_NONE now, and every K9 kernel skips it)
       bool exact = false;
       for (int s = 0; s < np; ++s) exact |= L->h_solve[s].mode == QB200_PMC_EXACT;
@@ -944,6 +1042,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   L->pend_host_lists = in.lists && in.lists->kind == QB200_MEM_HOST;
   if (in.lists) L->pend_lists = *in.lists;
   if (in.sink == Sink::Export) L->pend_out = *in.out;
+  if (in.sink == Sink::Graph) L->pend_graph = *in.graph_out;
   return QB200_OK;
 }
 
@@ -956,10 +1055,15 @@ int wave_collect(qb200_handle* h, Lane* L) {
     h->fail(__FILE__, __LINE__, cudaGetErrorString(cudaGetLastError()));
     return QB200_ERR_CUDA;
   }
+  int rc = QB200_OK;
   switch (L->pend_sink) {
     case Sink::Solve: case Sink::Match: case Sink::Clique:
       memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
       if (L->pend_host_lists) deliver_lists(L, L->pend_lists, L->pend_w0, np);
+      break;
+    case Sink::Graph:
+      memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
+      if (L->pend_graph.kind == QB200_MEM_HOST) rc = deliver_graph(L, L->pend_graph, L->pend_w0, np);
       break;
     case Sink::CacheSlots: break;
     case Sink::Export: deliver_export(L, L->pend_out, L->pend_w0, np); break;
@@ -986,7 +1090,7 @@ int wave_collect(qb200_handle* h, Lane* L) {
     }
     L->kev_armed[k] = 0;
   }
-  return QB200_OK;
+  return rc;
 }
 
 // wait for the waves in flight (oldest first) whose records go to dst, or for all of them (dst == nullptr), and hand out their records
@@ -1089,6 +1193,13 @@ int check_call(qb200_handle* h, const BatchCall& c) {
         return reject(why);
       }
     }
+  } else if (c.sink == Sink::Graph) {  // only noise_bound and cbar2 are read, checked as qb200_build_graph checks them
+    for (int i = 0; i < c.n; ++i) {
+      if (!p || !(p[i].noise_bound > 0) || !(p[i].cbar2 > 0)) {
+        snprintf(why, sizeof(why), "params entry %d is null, or its noise_bound or cbar2 is not > 0", i);
+        return reject(why);
+      }
+    }
   } else if (int rc = check_params(h, p, c.n, c.each(), c.src != Source::CorrSets && c.entries == Entries::Each, c.sink != Sink::Match)) {
     return rc;
   }
@@ -1104,6 +1215,8 @@ int check_call(qb200_handle* h, const BatchCall& c) {
   if (int rc = check_lists(h, c.lists, c.src == Source::CorrSets, c.sink == Sink::Match, c.src == Source::Graphs)) return rc;
   if (c.sink == Sink::Export)
     if (int rc = check_out(h, c.out, c.src == Source::KeypointClouds)) return rc;
+  if (c.sink == Sink::Graph)
+    if (int rc = check_graph_out(h, c.graph_out)) return rc;
   const int R = h->cfg.max_raw_points;
   for (int i = 0; i < c.n; ++i) {
     const char* bad = nullptr;
@@ -1146,7 +1259,14 @@ int check_call(qb200_handle* h, const BatchCall& c) {
       }
       case Source::CorrSets: {
         const qb200_corr_set& s = c.sets[i];
-        if (s.L < 0 || s.L > h->cfg.max_corr || (s.L > 0 && (!s.a || !s.b))) return reject("correspondence set is null or exceeds max_corr");
+        const bool rows = c.sink == Sink::Graph && (c.graph_out->adj || c.graph_out->degree);
+        if (s.L < 0 || s.L > h->cfg.max_corr || (s.L > 0 && (!s.a || !s.b))) bad = "it is null or its L is outside 0 .. max_corr";
+        else if (rows && s.L > c.graph_out->rows_per_set) bad = "its L exceeds rows_per_set";
+        if (bad && c.sink != Sink::Graph) return reject("correspondence set is null or exceeds max_corr");
+        if (bad) {
+          snprintf(why, sizeof(why), "set %d: %s", i, bad);
+          return reject(why);
+        }
         break;
       }
       case Source::KeypointClouds: {
@@ -1326,6 +1446,14 @@ BatchCall corr_sets(Sink k, Entries e, const qb200_corr_set* sets, int32_t n, co
                     const qb200_pair_lists* lists) {
   BatchCall c{Source::CorrSets, k, n, kind, p, e};
   c.sets = sets; c.results = results; c.lists = lists;
+  return c;
+}
+
+// TIM graphs of the sets into the caller's arrays: each set is built with its own entry
+BatchCall corr_sets(const qb200_corr_set* sets, int32_t n, const qb200_params* p, qb200_mem_kind kind, qb200_result* results,
+                    const qb200_graph_out* out) {
+  BatchCall c{Source::CorrSets, Sink::Graph, n, kind, p, Entries::Mixed};
+  c.sets = sets; c.results = results; c.graph_out = out;
   return c;
 }
 
@@ -1662,6 +1790,17 @@ int qb200_max_clique_batch_each(qb200_handle* h, const qb200_graph* graphs, int3
 int qb200_max_clique_batch_enqueue_each(qb200_handle* h, const qb200_graph* graphs, int32_t n_graphs, const qb200_params* params,
                                         qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
   return enqueue_call(h, caller_graphs(graphs, n_graphs, params, kind, results, lists));
+}
+
+// ---- correspondence sets -> TIM graphs ---------------------------------------------------------------------------------------------
+int qb200_build_graph_batch_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params,
+                                 qb200_mem_kind kind, qb200_result* results, const qb200_graph_out* out) {
+  return run_call(h, corr_sets(sets, n_sets, params, kind, results, out));
+}
+
+int qb200_build_graph_batch_enqueue_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params,
+                                         qb200_mem_kind kind, qb200_result* results, const qb200_graph_out* out) {
+  return enqueue_call(h, corr_sets(sets, n_sets, params, kind, results, out));
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

@@ -425,6 +425,145 @@ int launch_clique_records(Lane* h, int n_graphs) {
   return QB200_OK;
 }
 
+// ---- TIM graphs handed out (qb200_build_graph_batch_each): K8's rows, degrees and edge lists into caller layouts ------------------
+// K8 writes words 0 .. ceil(L / 32) - 1 of a set's L rows and degree_kernel reads only those: the words past them hold whatever an
+// earlier wave left there, so every kernel below reads the first ceil(L / 32) words of a row and nothing else.
+
+constexpr int kExportThreads = 256;
+
+// Grid over (chunk, set): set g's L rows with words_per_row words each (the words from ceil(L / 32) on as zero) and its L degrees
+__global__ void __launch_bounds__(kExportThreads) graph_export_kernel(const int* __restrict__ n_corr, int Lc, int W,
+                                                                      const uint32_t* __restrict__ adj, const int* __restrict__ deg,
+                                                                      GraphDst d) {
+  const int g = blockIdx.y, L = n_corr[g], nb = (L + 31) >> 5, wpr = d.words_per_row;
+  const uint32_t* __restrict__ G = adj + (size_t)g * Lc * W;
+  const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, step = (long long)gridDim.x * blockDim.x;
+  if (d.adj) {
+    uint32_t* __restrict__ out = d.adj + (size_t)g * d.rows_per_set * wpr;
+    for (long long i = t0; i < (long long)L * wpr; i += step) {
+      const int r = (int)(i / wpr), w = (int)(i % wpr);
+      out[i] = w < nb ? G[(size_t)r * W + w] : 0u;
+    }
+  }
+  if (d.degree)
+    for (long long r = t0; r < L; r += step) d.degree[(size_t)g * d.rows_per_set + r] = deg[(size_t)g * Lc + r];
+}
+
+// the bits j > i of word w of row i
+__device__ __forceinline__ uint32_t upper_bits(int i, int w, uint32_t x) {
+  const int wi = i >> 5, b = i & 31;
+  return w > wi ? x : w < wi || b == 31 ? 0u : x & (~0u << (b + 1));
+}
+
+// One CTA per set (blockIdx.x): off[i] = the edges (u, v), u < v, of the rows before i, and off[L] = all of them, at g * off_stride.
+// A warp per row counts its upper bits; the CTA then scans the counts in place, kEdgeScanThreads rows at a time.
+constexpr int kEdgeScanThreads = 1024;
+__global__ void __launch_bounds__(kEdgeScanThreads) edge_offsets_kernel(const int* __restrict__ n_corr, int Lc, int W,
+                                                                        const uint32_t* __restrict__ adj, int* __restrict__ off,
+                                                                        int off_stride) {
+  __shared__ int s_scan[33];
+  const int g = blockIdx.x, L = n_corr[g], nb = (L + 31) >> 5, lane = lane_id(), warp = threadIdx.x >> 5;
+  const uint32_t* __restrict__ G = adj + (size_t)g * Lc * W;
+  int* __restrict__ o = off + (size_t)g * off_stride;
+  for (int i = warp; i < L; i += kEdgeScanThreads / 32) {
+    int c = 0;
+    for (int w = (i >> 5) + lane; w < nb; w += 32) c += __popc(upper_bits(i, w, G[(size_t)i * W + w]));
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) c += __shfl_xor_sync(0xffffffffu, c, s);
+    if (lane == 0) o[i] = c;
+  }
+  __syncthreads();
+  int carry = 0;
+  for (int base = 0; base < L; base += kEdgeScanThreads) {
+    const int i = base + threadIdx.x;
+    int tot;
+    const int ex = block_excl_scan(i < L ? o[i] : 0, s_scan, &tot);
+    if (i < L) o[i] = carry + ex;
+    carry += tot;
+  }
+  if (threadIdx.x == 0) o[L] = carry;
+}
+
+// Grid over (row chunk, set), a warp per row: row i's edges (i, j), j > i, in ascending j, at their indices off[i] .. off[i + 1] - 1 of
+// the set's list; only the indices in [e0, e1) are written, at out + index - e0.  only < 0: blockIdx.y = set g, whose window starts at
+// out + g * out_stride; only >= 0: set `only` alone.  A lane takes one word of 32 and finds where its edges start from a warp prefix
+// of the words' popcounts.
+constexpr int kEmitWarps = 8;
+__global__ void __launch_bounds__(kEmitWarps * 32) edge_emit_kernel(const int* __restrict__ n_corr, int Lc, int W,
+                                                                    const uint32_t* __restrict__ adj, const int* __restrict__ off,
+                                                                    int off_stride, int only, long long e0, long long e1,
+                                                                    int2* __restrict__ out, long long out_stride) {
+  const int g = only >= 0 ? only : blockIdx.y, L = n_corr[g], nb = (L + 31) >> 5, lane = lane_id();
+  const uint32_t* __restrict__ G = adj + (size_t)g * Lc * W;
+  const int* __restrict__ o = off + (size_t)g * off_stride;
+  if (only < 0) out += (size_t)g * out_stride;
+  for (int i = blockIdx.x * kEmitWarps + (threadIdx.x >> 5); i < L; i += gridDim.x * kEmitWarps) {
+    long long idx = o[i];
+    if (idx >= e1 || o[i + 1] <= e0 || o[i + 1] == idx) continue;  // warp-uniform: no edge of this row falls in the window
+    for (int w0 = i >> 5; w0 < nb && idx < e1; w0 += 32) {
+      const int w = w0 + lane;
+      uint32_t x = w < nb ? upper_bits(i, w, G[(size_t)i * W + w]) : 0u;
+      const int c = __popc(x);
+      int tot;
+      long long k = idx + warp_excl_scan(c, &tot);
+      for (; x; x &= x - 1, ++k)
+        if (k >= e0 && k < e1) out[k - e0] = make_int2(i, w * 32 + __ffs(x) - 1);
+      idx += tot;
+    }
+  }
+}
+
+// One thread per set: the record of a graph wave.  cap_edges > 0: the set's edge list holds cap_edges entries.
+__global__ void graph_records_kernel(qb200_result* __restrict__ results, int n_sets, WaveCounters c, long long cap_edges) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n_sets) return;
+  qb200_result* r = results + g;
+  const long long e = c.n_edges[g] / 2;
+  memset(r, 0, sizeof(*r));
+  r->status = QB200_OK;
+  r->n_corr = c.n_corr[g];
+  r->n_edges = e;
+  r->flags = cap_edges > 0 && e > cap_edges ? QB200_FLAG_LISTS_TRUNCATED : 0;
+  for (int i = 0; i < 16; ++i) r->T[i] = (i % 5 == 0) ? 1.0 : 0.0;
+}
+
+int launch_graph_export(Lane* h, int n_sets, const GraphDst& d) {
+  if (n_sets <= 0 || (!d.adj && !d.degree)) return QB200_OK;
+  const long long words = (long long)h->Lc * (d.adj ? d.words_per_row : 1);
+  const long long b = (words + kExportThreads - 1) / kExportThreads;
+  const unsigned ctas = (unsigned)(b < 1 ? 1 : b > 2048 ? 2048 : b);
+  graph_export_kernel<<<dim3(ctas, n_sets), kExportThreads, 0, h->stream>>>(h->ctr.n_corr, h->Lc, h->W, h->adj, h->deg, d);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+
+int launch_edge_offsets(Lane* h, int n_sets) {
+  if (n_sets <= 0) return QB200_OK;
+  edge_offsets_kernel<<<n_sets, kEdgeScanThreads, 0, h->stream>>>(h->ctr.n_corr, h->Lc, h->W, h->adj, h->korder, h->Lc + 2);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+
+int launch_edge_emit(Lane* h, int n_sets, int only, long long e0, long long e1, int2* out, long long out_stride) {
+  if (n_sets <= 0 || e1 <= e0) return QB200_OK;
+  const unsigned ctas = (unsigned)((h->Lc + kEmitWarps - 1) / kEmitWarps);
+  edge_emit_kernel<<<dim3(ctas, only >= 0 ? 1 : n_sets), kEmitWarps * 32, 0, h->stream>>>(h->ctr.n_corr, h->Lc, h->W, h->adj, h->korder,
+                                                                                          h->Lc + 2, only, e0, e1, out, out_stride);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+
+int launch_graph_records(Lane* h, int n_sets, long long cap_edges) {
+  if (n_sets <= 0) return QB200_OK;
+  graph_records_kernel<<<(n_sets + 127) / 128, 128, 0, h->stream>>>(h->d_results, n_sets, h->ctr, cap_edges);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+
 GraphConst graph_const(double noise_bound, double cbar2) {
   const double beta = 2 * noise_bound * sqrt(cbar2);  // quatro.hpp:367
   const double u = 5.9604644775390625e-8;             // 2^-24

@@ -100,17 +100,27 @@ struct GraphSrc {
   int L, stride;
 };
 
+// Where a graph wave's device-kind outputs go (graph.cu: graph_export_kernel): set g's rows at adj + g * rows_per_set * words_per_row
+// and its degrees at degree + g * rows_per_set, from the wave's first set on (nullptr = not asked for)
+struct GraphDst {
+  uint32_t* adj;
+  int* degree;
+  long long rows_per_set;
+  int words_per_row;
+};
+
 // What a batch call reads (api.cu: BatchCall), per input: a pair of raw scans, a pair of cached scans (slots), a pair of caller
 // keypoint clouds with their FPFH-33 rows, a correspondence set, one raw scan, one caller keypoint cloud, or one caller graph
 enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, KeypointClouds, Graphs };
 // What a batch call produces: solved records (and lists), the matcher's records (and lists), cache slots, front-end features in
-// caller memory, or max-clique records (and clique lists).  The valid (source, sink) pairs:
+// caller memory, max-clique records (and clique lists), or TIM graphs in caller memory (and records).  The valid (source, sink)
+// pairs:
 //   RawPairs, CachedPairs, FeaturePairs  x  Solve, Match   qb200_register_batch*, _cached*, _features*; qb200_match_*
-//   CorrSets                             x  Solve          qb200_solve_batch*
+//   CorrSets                             x  Solve, Graph   qb200_solve_batch*, qb200_build_graph_batch*
 //   RawScans                             x  CacheSlots     qb200_cache_scans*
 //   RawScans, KeypointClouds             x  Export         qb200_describe_batch*, qb200_describe_points*
 //   Graphs                               x  Clique         qb200_max_clique_batch*
-enum class Sink { Solve, Match, CacheSlots, Export, Clique };
+enum class Sink { Solve, Match, CacheSlots, Export, Clique, Graph };
 
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
@@ -140,11 +150,12 @@ struct Lane {
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
   unsigned pend_stages;      // ... the stage-time slots it reports (bit i: qb200_get_stage_ms slot i)
   Sink pend_sink;             // ... what wave_collect hands on for it: the fields below of its sink
-  qb200_result* pend_dst;     // ... (Solve, Match, Clique) the caller's record array of its batch, nullptr for the other sinks
+  qb200_result* pend_dst;     // ... (Solve, Match, Clique, Graph) the caller's record array of its batch, nullptr for the other sinks
   bool pend_host_lists;       // ... (Solve, Match, Clique) its batch has host-kind lists, which wave_collect hands on from lst_stage
   qb200_pair_lists pend_lists; // ... and then a copy of their descriptor
   qb200_feature_out pend_out; // ... (Export) a copy of its batch's output descriptor, whose counts and status (and, in host kind,
                               // entries) wave_collect hands on from exp_stage
+  qb200_graph_out pend_graph; // ... (Graph) a copy of its batch's output descriptor, whose host-kind arrays wave_collect writes
   // ... and the cache slots it reads (cached pairs) or writes (CacheSlots), ascending and unique; empty: it does not touch the
   // cache.  A wave reads the cache only in its copy-in and writes it only in its copy-out, so other lanes order their conflicting
   // copies after those events (api.cu: cache_waits)
@@ -379,6 +390,16 @@ int launch_edge_import(Lane* h, int n_graphs, long long max_edges, int only, con
 int launch_symmetry_check(Lane* h, int n_graphs, int max_L);
 // a graph wave's records (graphs [0, n), after K9): status, L, edges, max core, clique size and flags; the rest as a match record
 int launch_clique_records(Lane* h, int n_graphs);
+// TIM graph waves (graph.cu), after launch_graph on sets [0, n): launch_graph_export writes every set's L rows (words ceil(L / 32) ..
+// words_per_row - 1 as zero) and degrees to d.  launch_edge_offsets finds where each row's edges (i, j), j > i, start in its set's
+// list (korder, Lc + 2 ints per set, is the scratch: K9 does not run in these waves).  launch_edge_emit then writes the edges whose
+// list index lies in [e0, e1) at out + index - e0: of every set (only < 0; set g's window at out + g * out_stride) or of set `only`.
+// launch_graph_records writes the records: status QB200_OK, L, n_edges, QB200_FLAG_LISTS_TRUNCATED past cap_edges (> 0: an edge list
+// was asked for), the rest as a match record.
+int launch_graph_export(Lane* h, int n_sets, const GraphDst& d);
+int launch_edge_offsets(Lane* h, int n_sets);
+int launch_edge_emit(Lane* h, int n_sets, int only, long long e0, long long e1, int2* out, long long out_stride);
+int launch_graph_records(Lane* h, int n_sets, long long cap_edges);
 // the checks every entry of a registering call passes; solver = false: the front-end and matcher fields only (a match call)
 bool params_ok(const qb200_params* p, bool solver = true);
 float lattice_cell(const qb200_params& p);
