@@ -835,7 +835,7 @@ int qb200_debug_tc_distances(qb200_handle* h, const float* a33, int32_t na, cons
 
 /* Diagnostics: cumulative counters of the tensor-core matcher since creation / the last reset:
  * out4[0] = descriptor pairs that went through the exact fp32 chain, [1] = 128 x 64 tiles drained,
- * [2] = warm-up passes, [3] = stripes handed to the exact kernel.  Synchronises the handle's stream. */
+ * [2] = 0 (unused), [3] = stripes handed to the exact kernel.  Synchronises the handle's stream. */
 int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset);
 /* Diagnostics: both nearest-neighbour tables of the most recent qb200_match, in point order: rowbest[i] = packed
  * (distance bits << 32 | target index) of the best target of source point i, colbest[j] = the same for the best source of target

@@ -1155,7 +1155,7 @@ class Handle:
     def debug_match_stats(self, reset: bool = True) -> dict:
         out = np.zeros(4, np.uint64)
         self._check(self.lib.qb200_debug_match_stats(self.h, _ptr(out), int(reset)), "qb200_debug_match_stats")
-        return {"exact_evals": int(out[0]), "tiles": int(out[1]), "warmups": int(out[2]), "aborted_stripes": int(out[3])}
+        return {"exact_evals": int(out[0]), "tiles": int(out[1]), "aborted_stripes": int(out[3])}
 
     def debug_nn_tables(self, n_src: int, n_tgt: int):
         """(best target of every source point, best source of every target point) of the last match, packed uint64

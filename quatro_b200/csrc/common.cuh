@@ -45,6 +45,13 @@ constexpr int kDescDim = 33;   // pcl::FPFHSignature33
 constexpr int kDescPad = 36;   // floats per SPFH row (16-byte multiple: float4 gathers)
 constexpr int kDescK = 40;     // rows (K extent) of the dimension-major FPFH matrices: 33 bins + zero padding to a multiple of
                                // the TF32 tensor-core K step (8)
+// One step of the matcher's exact descriptor distance: acc + (a - b)^2, the product-sum rounded once.  Every exact distance
+// of the matcher (match_stripe_kernel, tc_nn_kernel's evaluation and its seeds) is the chain of these steps over bins
+// 0 .. 32 in ascending order, so all of them produce the same bits.
+__device__ __forceinline__ float desc_dist_step(float acc, float a, float b) {
+  const float diff = a - b;
+  return __fmaf_rn(diff, diff, acc);
+}
 constexpr int kMatchTile = 128;
 constexpr int kNbrGlobalCap = 80;  // neighbour indices per point handed from K4 (SPFH) to K5 (FPFH)
 

@@ -184,7 +184,7 @@ struct Lane {
                               // shared-memory operand layout (one bulk copy per column tile, one per 128-row stripe)
   DeviceMem<float> desc_norm; // [2S*V] squared norms (fp32 fma chain)
   DeviceMem<int> tc_fallback; // [S] 1 = too many exact ties for the filter to pay off: pair re-done by the exact fp32 kernel
-  DeviceMem<unsigned long long> tc_stats; // [32] diagnostics, cumulative: [0..3] exact evaluations, tiles drained, warm-up passes, aborted stripes; [4..5] QB200_TC_VERIFY; [8..31] QB200_TC_PROF
+  DeviceMem<unsigned long long> tc_stats; // [32] diagnostics, cumulative: [0..3] exact evaluations, tiles drained, 0 (unused), aborted stripes; [4..5] QB200_TC_VERIFY; [8..31] QB200_TC_PROF
   // ---- matching ----
   DeviceMem<unsigned long long> rowbest; // [S*V] packed (dist bits << 32 | tgt idx) per source point
   DeviceMem<unsigned long long> colpart; // [colpart_count()] tensor-core K6 scratch: class results [2][S][V] and the tile-max cache

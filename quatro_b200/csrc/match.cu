@@ -102,10 +102,7 @@ match_stripe_kernel(const float* __restrict__ desc_t, const int* __restrict__ n_
 #pragma unroll
       for (int r = 0; r < 8; ++r)
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const float diff = a[r] - b[c];
-          acc[r][c] = __fmaf_rn(diff, diff, acc[r][c]);
-        }
+        for (int c = 0; c < 8; ++c) acc[r][c] = desc_dist_step(acc[r][c], a[r], b[c]);
     }
     // epilogue: fold into row minima (registers) and this tile's column minima
     const int cbase = jt * kMT + tx * 8, rbase = r0 + ty * 8;

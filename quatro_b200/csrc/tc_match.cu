@@ -12,6 +12,8 @@
 //   dedup_kernel      : runs of bit-identical descriptors (adjacent after the sort) collapse to their first rank = lowest index
 //   split_desc_kernel : hi = TF32(x'), lo = TF32(x' - hi), exact x, per block of 64 unique descriptors as ready-made
 //                       shared-memory operand images (hi | lo | exact), so an image is ONE cp.async.bulk
+//   tc_seed_kernel    : every unique row and column starts with the exact distance to its nearest-norm candidates of the
+//                       other cloud, so the filter and the tile skip have finite thresholds from the first tile on
 //   tc_nn_kernel      : per 128-row stripe, 64-column tiles in nearest-norm-first order; a tile whose lower bound
 //                       (gap of the norm ranges)^2 exceeds every current best of the stripe's rows and of its columns is
 //                       skipped unloaded; otherwise
@@ -55,6 +57,7 @@ constexpr float kTcNormMax = 0x1p124f;
 // arithmetic of the bound itself.  The 0.9999 factor covers the exact chain's own rounding (d computed >= d (1 - 36 * 2^-24)).
 constexpr float kTcNormRel = 4.0e-6f;
 constexpr int kSpinLimit = 400000;
+constexpr int kSeedW = 16;                        // seed candidates on either side of a descriptor's norm (tools/tc_seed_study.py)
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -267,6 +270,71 @@ __device__ __forceinline__ unsigned long long tc_pack(float d, int idx) {
   return ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)idx;
 }
 
+// exact distance of two descriptors given as their 9 float4 chunks of the exact image (a(kc), b(kc) = bins 4 kc .. 4 kc + 3)
+template <class FA, class FB>
+__device__ __forceinline__ float tc_exact_dist(FA a, FB b) {
+  float acc = 0.0f;
+#pragma unroll
+  for (int kc = 0; kc < (kDescDim + 3) / 4; ++kc) {
+    const float4 x = a(kc), y = b(kc);
+    acc = desc_dist_step(acc, x.x, y.x);
+    if (4 * kc + 1 < kDescDim) acc = desc_dist_step(acc, x.y, y.y);
+    if (4 * kc + 2 < kDescDim) acc = desc_dist_step(acc, x.z, y.z);
+    if (4 * kc + 3 < kDescDim) acc = desc_dist_step(acc, x.w, y.w);
+  }
+  return acc;
+}
+
+// Seeds.  Every unique rank of both clouds of a pair gets the exact distance to the 2 kSeedW unique descriptors of the other
+// cloud nearest to it in norm (kSeedW on either side), as a packed (distance | point index) word: rows into rowbest, columns
+// into colbest, and the max of each 32-column group's seeds into tile_cmax.  Seeds are exact distances to real points, so they
+// are upper bounds of the exact minima: tc_nn_kernel's filter (<=), its tile skip (strict >) and the atomicMin on packed words
+// (lowest index at equal distance) leave its results unchanged, and every row and column has a finite threshold before its
+// first tile.  Pairs flagged for the exact kernel are left alone.  One thread per rank; a warp is one 32-column group.
+__global__ void __launch_bounds__(256) tc_seed_kernel(const float* __restrict__ tiles, const float* __restrict__ norm,
+                                                      const int* __restrict__ n_vox, int V, const uint32_t* __restrict__ perm,
+                                                      const int* __restrict__ fallback, unsigned long long* __restrict__ rowbest,
+                                                      unsigned long long* __restrict__ colbest, unsigned* __restrict__ tile_cmax) {
+  const int cloud = blockIdx.y, pair = cloud >> 1, other = cloud ^ 1;
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  const int n = n_vox[cloud], no = n_vox[other];
+  // warp-uniform: every warp of a 64-column tile with a valid column writes its group's maximum, a group of padding included
+  if (fallback[pair] || (r & ~(kTcN - 1)) >= n) return;
+  const int NB = V / kTcBlk;
+  auto image = [&](int c, int q) {  // exact image of rank q of cloud c, chunk kc at [kc * kTcBlk]
+    return reinterpret_cast<const float4*>(tiles + ((size_t)(c * NB + q / kTcBlk) * kTcImages + 2) * kTileFloats) + q % kTcBlk;
+  };
+  unsigned long long best = ~0ull;
+  if (r < n && no > 0) {
+    const float4* __restrict__ ia = image(cloud, r);
+    float4 own[(kDescDim + 3) / 4];
+#pragma unroll
+    for (int kc = 0; kc < (kDescDim + 3) / 4; ++kc) own[kc] = ia[kc * kTcBlk];
+    // first rank of the other cloud whose norm is not below this one's (norms ascend with the rank)
+    const float* __restrict__ nrm = norm + (size_t)other * V;
+    const float key = norm[(size_t)cloud * V + r];
+    int lo = 0, hi = no;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (nrm[mid] < key) lo = mid + 1; else hi = mid;
+    }
+    const int j1 = min(no, lo + kSeedW);
+    for (int j = max(0, lo - kSeedW); j < j1; ++j) {
+      const float4* __restrict__ ib = image(other, j);
+      const float d = tc_exact_dist([&](int kc) { return own[kc]; }, [&](int kc) { return ib[kc * kTcBlk]; });
+      if (d == d) best = min(best, tc_pack(d, (int)perm[(size_t)other * V + j]));  // NaN never wins
+    }
+  }
+  if (cloud & 1) {
+    if (r < n) colbest[(size_t)pair * V + r] = best;
+    // padding columns do not count (as in tc_nn_kernel's refresh); a column without a seed keeps its group above +inf
+    const unsigned m = __reduce_max_sync(0xffffffffu, r < n ? (unsigned)(best >> 32) : 0u);
+    if ((threadIdx.x & 31) == 0) tile_cmax[((size_t)pair * (V / kTcN) + r / kTcN) * 2 + ((r / 32) & 1)] = m;
+  } else if (r < n) {
+    rowbest[(size_t)pair * V + r] = best;
+  }
+}
+
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory");
 }
@@ -279,7 +347,8 @@ __device__ __forceinline__ float tc_fkey_inv(unsigned key) { return __uint_as_fl
 
 // rows = source cloud (2*pair), columns = target cloud (2*pair+1): their UNIQUE descriptors in ascending-norm (rank) order;
 // n_vox / perm are the per-cloud unique counts and the point index of every unique rank.  rowbest / colbest_r are indexed by
-// unique rank (broadcast_best_kernel maps them back).  kDbg: additionally
+// unique rank (broadcast_best_kernel maps them back) and hold tc_seed_kernel's seeds on entry, tile_cmax their column maxima.
+// kDbg: additionally
 // dump d~ of every tile of stripe 0 (validation hook, at most 128 x 128 descriptors).
 //
 // Warp roles (no CTA-wide barrier inside the tile loop, everything is handed over through mbarriers):
@@ -307,7 +376,7 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
   __shared__ unsigned short s_queue[kTcEpiWarps][32];          //           one batch of candidates (lane << 5 | fragment index)
   __shared__ int s_seq[8];                                     // column tile of sequence position n (ring), -1 = end of the stripe
   __shared__ float s_tlb[kTcSmemTiles];                        // lower bound of every distance between the stripe and column tile t
-  __shared__ int s_dead, s_abort, s_evals, s_warm, s_npos;
+  __shared__ int s_dead, s_abort, s_evals, s_npos;
   __shared__ int s_ndec;                                       // sequence positions 0 .. s_ndec-1 have been decided (s_seq ring)
 
   const int pair = blockIdx.y, stripe = blockIdx.x;
@@ -344,10 +413,10 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     mbar_init(bar_fullhl, 1);
     for (int i = 0; i < kTcDone; ++i) mbar_init(bar_mma0 + 8 * i, kTcEpiWarps);
     mbar_init(bar_a, 1);
-    s_dead = 0; s_abort = 0; s_evals = 0; s_warm = 0; s_npos = 0; s_ndec = 0;
+    s_dead = 0; s_abort = 0; s_evals = 0; s_npos = 0; s_ndec = 0;
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
-  if (threadIdx.x < kTcM) s_rbest[threadIdx.x] = ~0ull;
+  if (threadIdx.x < kTcM) s_rbest[threadIdx.x] = r0 + (int)threadIdx.x < nA ? rowbest[(size_t)pair * V + r0 + threadIdx.x] : ~0ull;  // seeds
   __syncthreads();
   const long long t_setup = tick();
   if (kProf && threadIdx.x == 0) { atomicAdd(stats + 8, 1ull); atomicAdd(stats + 10, (unsigned long long)(t_setup - t_begin)); }
@@ -436,12 +505,12 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
       __syncwarp();
     }
     auto tlb = [&](int t) -> float { return t < kTcSmemTiles ? s_tlb[t] : tile_lb(t); };
-    int lo = t0 - 1, hi = t0 + 1;
-    bool first = true, done = false;
+    int lo = t0, hi = t0 + 1;
+    bool done = false;
     auto next_tile = [&]() -> int {  // warp-uniform
-      if (first) { first = false; return t0; }
-      // Inputs of a choice: the current worst row best of the stripe (+inf while any row is unknown) and the prefetched per-tile
-      // column maxima.  A tile whose lower bound exceeds both is skipped for good (bests only shrink).
+      // Inputs of a choice: the current worst row best of the stripe and the prefetched per-tile column maxima, seeded before
+      // the first choice (+inf only in a pair flagged for the exact kernel).  A tile whose lower bound exceeds both is skipped
+      // for good (bests only shrink).
       unsigned rmax = 0;
 #pragma unroll
       for (int i = 0; i < kTcM / 32; ++i) {
@@ -514,10 +583,12 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
       mbar_expect_tx(bar, kXBytes);
       bulk_g2s(sX0 + (n % kTcStages) * kXBytes, tB + ((size_t)t * kTcImages + 2) * kTileFloats, kXBytes, bar);
     };
-    for (int n = 0; n < 3; ++n) {
-      decide(n);
-      if (n < kTcStages) issue_x(n);
-    }
+    // positions 0 .. 2 up to the end marker (the first choice is a skip test like every other one), then their exact images
+    int nd = 0;
+    bool end_decided = false;
+    while (nd < 3 && !end_decided) end_decided = decide(nd++) < 0;
+    int nx = 0;
+    while (nx < kTcStages && nx < nd) issue_x(nx++);
     prof(11, tick() - t_setup);
     long long p_wm = 0, p_dec = 0, p_sf = 0;
     auto mbar_test = [&](uint32_t bar, uint32_t parity) -> bool {
@@ -534,8 +605,7 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     // Two duties, neither blocks the other: the exact image of position nx goes out as soon as every warp evaluated position
     // nx - kTcStages (its stage), and positions are chosen ahead (at most 3 beyond nx: the s_seq ring, and not before the MMAs of
     // position nd-3 completed, so that a choice sees the bests of the tiles before it) while that stage is still busy.
-    int nd = 3, nx = kTcStages;
-    bool ok = true, end_decided = v_seq[0] < 0 || v_seq[1] < 0 || v_seq[2] < 0;
+    bool ok = true;
     int idle = 0;
     long long t_idle = 0;
     while (ok && !(end_decided && nx == nd)) {
@@ -575,17 +645,16 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
     // the accumulators hold LB_ij = d~_ij - e_ij = kLow (na' + nb') - 2 dot (split_desc_kernel); an entry is a candidate iff
     // LB_ij <= the best exact distance known for row i or for column j
     const float kLow = 1.0f - 0.5f * kTcC;
-    const float kW = kTcC / kLow;                            // d~ + e = LB + kW (kLow na' + kLow nb')
+    const float kW = kTcC / kLow;                            // d~ + e = LB + kW (kLow na' + kLow nb') (kDbg dump)
     bool row_ok[2];
-    float nam[2], Ri_ub[2];
+    float nam[2];
     unsigned oa[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int gi = r0 + rbase + (lane >> 2) + 8 * h;
       row_ok[h] = gi < nA;
-      nam[h] = row_ok[h] ? kLow * nrmA[gi] : INFINITY;      // +inf: a padded row yields no upper bounds
+      nam[h] = row_ok[h] ? kLow * nrmA[gi] : INFINITY;
       oa[h] = row_ok[h] ? permA[gi] : 0u;                    // point index of the row
-      Ri_ub[h] = row_ok[h] ? INFINITY : -INFINITY;           // row threshold from the tile-local upper bounds (padded rows: never)
     }
     const uint32_t row_bits = (row_ok[0] ? 0x33333333u : 0u) | (row_ok[1] ? 0xCCCCCCCCu : 0u);  // fragment entries of valid rows
     // the warpgroup's A block (hi | lo | exact): operand rows of the MMAs, exact image of rows 64 wg + p (index p)
@@ -699,52 +768,17 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
         const float4* __restrict__ bex = reinterpret_cast<const float4*>(smem + kABytes + kHLBytes + st * kXBytes);  // exact image
         // ---- per-column filter data of the lane's two snapshot columns
         float dbest[2];
-        bool col_warm = false;
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
           const float nbm = bex[9 * kTcBlk + 32 * s + lane].x;  // kLow |b'_j|^2, +inf for padded columns (split_desc_kernel)
           dbest[s] = cb_cur[s] == ~0ull ? INFINITY : __uint_as_float((unsigned)(cb_cur[s] >> 32));
-          wcj[32 * s + lane] = nbm == INFINITY ? -INFINITY : dbest[s];  // column threshold: +inf while the column has no exact distance yet
-          col_warm |= cb_cur[s] == ~0ull && nbm != INFINITY;
+          wcj[32 * s + lane] = nbm == INFINITY ? -INFINITY : dbest[s];  // column threshold: the seed or a better exact distance
         }
         float Ri[2];
-        bool row_warm = false;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const unsigned long long rb = v_rbest[rbase + (lane >> 2) + 8 * h];
-          Ri[h] = fminf(Ri_ub[h], rb == ~0ull ? INFINITY : __uint_as_float((unsigned)(rb >> 32)));
-          row_warm |= row_ok[h] && Ri[h] == INFINITY;
-        }
-        __syncwarp();
-        // ---- warm-up: a row / column without any exact distance would let every entry through.  Upper bounds of the
-        // exact minima come from the tile itself: UB_ij = d~_ij + e_ij = (1+c/2)(na'+nb') - 2 dot >= d_ij.
-        if (__any_sync(0xffffffffu, row_warm || col_warm)) {
-          if (lane == 0) atomicAdd(&s_warm, 1);
-          float rowub[2] = {INFINITY, INFINITY};
-#pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int c = 2 * i + cl + e;  // = 8 (i >> 2) + cl + e: this entry pair's column of the tile
-              const float nbc = bex[9 * kTcBlk + c].x;
-              const float ub0 = fmaf(kW, nam[0] + nbc, d[i + e]), ub1 = fmaf(kW, nam[1] + nbc, d[i + 2 + e]);
-              rowub[0] = fminf(rowub[0], ub0);
-              rowub[1] = fminf(rowub[1], ub1);
-              // min over the warp's 16 rows (lanes of equal lane & 3); an upper bound of a distance is >= 0 (bit patterns order
-              // them), anything else is dropped
-              unsigned mn = min(ub0 >= 0.0f ? __float_as_uint(ub0) : 0xFFFFFFFFu, ub1 >= 0.0f ? __float_as_uint(ub1) : 0xFFFFFFFFu);
-              mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, 4));
-              mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, 8));
-              mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, 16));
-              if (lane < 4 && mn != 0xFFFFFFFFu && nbc != INFINITY) wcj[c] = fminf(wcj[c], __uint_as_float(mn));
-            }
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {  // min over the row's 64 columns (the 4 lanes of a row)
-            rowub[h] = fminf(rowub[h], __shfl_xor_sync(0xffffffffu, rowub[h], 1));
-            rowub[h] = fminf(rowub[h], __shfl_xor_sync(0xffffffffu, rowub[h], 2));
-            if (row_ok[h]) { Ri_ub[h] = fminf(Ri_ub[h], rowub[h]); Ri[h] = fminf(Ri[h], Ri_ub[h]); }
-          }
+          Ri[h] = rb == ~0ull ? INFINITY : __uint_as_float((unsigned)(rb >> 32));  // +inf: no seed (a pair flagged for the exact kernel)
         }
         __syncwarp();
         const long long q5 = tick();
@@ -796,16 +830,8 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
           const int sl = q >> 5, i = q & 31, h = (i >> 1) & 1;
           const int rr = rbase + (sl >> 2) + 8 * h;            // row of the stripe
           const int c = 8 * (i >> 2) + 2 * (sl & 3) + (i & 1);  // column of the tile
-          float acc = 0.0f;
-#pragma unroll
-          for (int kc = 0; kc < (kDescDim + 3) / 4; ++kc) {
-            const float4 a = aex[kc * kTcBlk + (rr & (kTcBlk - 1))], b = bex[kc * kTcBlk + c];
-            float diff = a.x - b.x;
-            acc = __fmaf_rn(diff, diff, acc);
-            if (4 * kc + 1 < kDescDim) { diff = a.y - b.y; acc = __fmaf_rn(diff, diff, acc); }
-            if (4 * kc + 2 < kDescDim) { diff = a.z - b.z; acc = __fmaf_rn(diff, diff, acc); }
-            if (4 * kc + 3 < kDescDim) { diff = a.w - b.w; acc = __fmaf_rn(diff, diff, acc); }
-          }
+          const float acc = tc_exact_dist([&](int kc) { return aex[kc * kTcBlk + (rr & (kTcBlk - 1))]; },
+                                          [&](int kc) { return bex[kc * kTcBlk + c]; });
           // column data live in lane c & 31 (snapshot s = c >> 5), row point indices in lane sl & ~3 (h)
           const float db0 = __shfl_sync(0xffffffffu, dbest[0], c & 31), db1 = __shfl_sync(0xffffffffu, dbest[1], c & 31);
           const unsigned ob0 = __shfl_sync(0xffffffffu, ob[0], c & 31), ob1 = __shfl_sync(0xffffffffu, ob[1], c & 31);
@@ -855,7 +881,6 @@ tc_nn_kernel(const float* __restrict__ tiles, const float* __restrict__ norm, co
   if (threadIdx.x == 0) {
     atomicAdd(stats + 0, (unsigned long long)s_evals);
     atomicAdd(stats + 1, (unsigned long long)s_npos);
-    atomicAdd(stats + 2, (unsigned long long)s_warm);
     if (aborted) {
       atomicAdd(stats + 3, 1ull);
       fallback[pair] = 1;
@@ -922,13 +947,14 @@ int launch_match_nn(Lane* h, int n_pairs) {
   // class results, indexed by unique rank (colpart is this kernel's scratch; the exact fallback works in rowbest / colbest)
   unsigned long long* colbest_u = h->colpart_col();
   unsigned long long* rowbest_u = h->colpart_row();
-  unsigned* tile_cmax = h->colpart_tile_cmax();  // [S][V/64][2] float bits, start above "+inf"
+  unsigned* tile_cmax = h->colpart_tile_cmax();  // [S][V/64][2] float bits: the seeds' column maxima
   QB_CUDA_TRY(h, cudaMemsetAsync(h->rowbest, 0xFF, (size_t)n_pairs * V * 8, h->stream));
   QB_CUDA_TRY(h, cudaMemsetAsync(h->colbest, 0xFF, (size_t)n_pairs * V * 8, h->stream));
   QB_CUDA_TRY(h, cudaMemsetAsync(h->colpart, 0xFF, h->colpart_count() * 8, h->stream));  // 0xFFFFFFFF > +inf bits
   QB_CUDA_TRY(h, cudaMemsetAsync(h->tc_fallback, 0, (size_t)n_pairs * sizeof(int), h->stream));
   const dim3 gsplit((V + 255) / 256, 2 * n_pairs);
   split_desc_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_t, n_unique, V, uperm, h->desc_tiles, h->desc_norm, h->tc_fallback);
+  tc_seed_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, V, uperm, h->tc_fallback, rowbest_u, colbest_u, tile_cmax);
   const dim3 g(h->NS, n_pairs);
   cudaEventRecord(h->kev[0], h->stream);
   if (h->tc_prof) {
@@ -942,7 +968,7 @@ int launch_match_nn(Lane* h, int n_pairs) {
   cudaEventRecord(h->kev[1], h->stream);
   h->kev_armed[0] = 1;
   broadcast_best_kernel<<<gsplit, 256, 0, h->stream>>>(rowbest_u, colbest_u, h->ctr.n_vox, V, h->val_b, class_of, h->rowbest, h->colbest);
-  h->launches += 3;
+  h->launches += 4;
   QB_CUDA_TRY(h, cudaGetLastError());
   return launch_match_exact(h, n_pairs, h->tc_fallback);
 }
@@ -960,10 +986,12 @@ int launch_tc_debug_tile(Lane* h, float* d_out) {
   QB_CUDA_TRY(h, cudaMemsetAsync(h->tc_fallback, 0, sizeof(int), h->stream));
   const dim3 gsplit((h->V + 255) / 256, 2);
   split_desc_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_t, n_unique, h->V, uperm, h->desc_tiles, h->desc_norm, h->tc_fallback);
+  tc_seed_kernel<<<gsplit, 256, 0, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, h->V, uperm, h->tc_fallback, h->colpart_row(),
+                                                h->colpart_col(), h->colpart_tile_cmax());
   const dim3 g(1, 1);
   tc_nn_kernel<true><<<g, kTcThreads, smem, h->stream>>>(h->desc_tiles, h->desc_norm, n_unique, h->V, uperm, h->colpart_row(), h->colpart_col(),
                                                          h->colpart_tile_cmax(), h->tc_fallback, h->tc_stats, d_out);
-  h->launches += 2;
+  h->launches += 3;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;
 }

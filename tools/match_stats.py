@@ -15,8 +15,7 @@ def main():
     st = h.debug_match_stats(True)
     entries = float(np.sum(res["n_src_vox"].astype(np.float64) * res["n_tgt_vox"]))
     print("pairs", n, "entries %.3e" % entries, st)
-    print("exact fraction %.4f%%  evals/tile %.1f  warmups/tile %.3f" % (100.0 * st["exact_evals"] / entries,
-          st["exact_evals"] / max(1, st["tiles"]), st["warmups"] / max(1, st["tiles"])))
+    print("exact fraction %.4f%%  evals/tile %.1f" % (100.0 * st["exact_evals"] / entries, st["exact_evals"] / max(1, st["tiles"])))
     print("kernel ms", h.kernel_ms())
 
 if __name__ == "__main__":

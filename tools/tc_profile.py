@@ -3,6 +3,8 @@
   QB200_TC_PROF=1 QB200_LANES=1 python tools/tc_profile.py [--pairs 64] [--scene street|dense]
 Prints per-CTA averages in microseconds at the measured SM clock.  Roles: "sched" = the scheduler warp (chooses the tiles,
 issues the exact-image copies), "copy" = the operand-copy warp, "epi" = the MMA + filter / evaluation warps (averaged over them).
+"stats" holds the wave's exact evaluations, tiles visited and aborted stripes.  "kernel_ms" is the device time per wave of the
+seed kernel and of tc_nn_kernel, from torch.profiler on a second handle built without the clock64 accounting.
 """
 import argparse, json, os, sys
 os.environ.setdefault("QB200_TC_PROF", "1")
@@ -46,6 +48,24 @@ def main():
             out[name + "_per_cta"] = round(v / n, 2)
         else:
             out[name + "_us_per_cta"] = round(v / n * cyc_us, 2)
+    h.close()
+    # kernel times without the clock64 accounting (the switch is read when a handle is created)
+    os.environ["QB200_TC_PROF"] = "0"
+    h = capi.Handle(device=0, max_batch_slots=a.pairs, **bench.SCENES[a.scene]["cfg"])
+    for rep in range(2):
+        h.register_batch(pairs, p)
+    waves = 3
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as tp:
+        for rep in range(waves):
+            h.register_batch(pairs, p)
+        torch.cuda.synchronize()
+    ms = {}
+    for ev in tp.events():
+        for k in ("tc_seed_kernel", "tc_nn_kernel"):
+            if k in ev.name:
+                ms[k] = ms.get(k, 0.0) + (ev.time_range.end - ev.time_range.start) / 1000.0 / waves   # kernel span, us
+    out["kernel_ms"] = {k: round(v, 3) for k, v in sorted(ms.items())}
+    h.close()
     print(json.dumps(out, indent=1))
 
 if __name__ == "__main__":
