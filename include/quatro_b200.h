@@ -35,6 +35,8 @@
  *                                  (include/teaser/graph.h:29-274, src/graph.cc:12-130)
  *   qb200_build_graph_batch_*   <- Quatro::computeTIMs + solveForScale + inlier_graph_.addEdge loop for every correspondence set of
  *                                  a batch, the graph handed out (include/quatro.hpp:307-386, 784-789)
+ *   qb200_solve_pose_batch_*    <- the tail of Quatro::computeTransformation (chain TIMs + GNC-TLS yaw + COTE + final inliers) for
+ *                                  every caller inlier set of a batch (include/quatro.hpp:806-936)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -773,6 +775,58 @@ int qb200_build_graph_batch_each(qb200_handle* h, const qb200_corr_set* sets, in
  * blocking call's. */
 int qb200_build_graph_batch_enqueue_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params,
                                          qb200_mem_kind kind, qb200_result* results, const qb200_graph_out* out);
+
+/* --- poses of caller inlier sets in batches ------------------------------------------------------------------------------------------
+ * The tail of Quatro::computeTransformation (include/quatro.hpp:806-936: chain TIMs, GNC-TLS yaw, COTE translation, the final inlier
+ * list) for every set of a batch whose inliers the caller supplies: a clique of qb200_max_clique_batch_each as it lies in device
+ * memory, the inliers of a clique solver or consistency filter of the caller's own, or one clique solved under several solver settings
+ * (with and without the roll/pitch prior, both COTE modes, other noise bounds) without building the graph or searching the clique
+ * again.  qb200_solve_pose_batch_each is qb200_solve_pose for a batch; sets run in waves of max_batch_slots over the lanes like every
+ * batch call.
+ *   Equality.  For every set that is not refused, the record (T, cost, gnc_iters, n_rot_inliers, n_final_inliers, clique_size, n_corr,
+ *     status, valid and every other field) is byte-identical to qb200_solve_pose on that set alone with the same list and params,
+ *     except for QB200_FLAG_LISTS_TRUNCATED.  The rotation and translation masks are byte-identical to what qb200_solve_pose writes,
+ *     the final inliers to qb200_get_last_final_inliers after that call.  No output depends on the batch, the wave, the lane,
+ *     QB200_LANES, the input or list memory kinds, or the other sets.
+ *   Order.  The list is taken in the caller's order and is not sorted; duplicates are accepted, as qb200_solve_pose accepts them.  The
+ *     chain TIMs follow the order of the list.  The reference sorts its clique first, so a caller who wants the reference's result
+ *     passes ascending ids (qb200_max_clique_batch_each writes them ascending).
+ *   Params.  Every entry must pass the checks of qb200_solve_pose.  The pose reads rot_noise_bound (0 resolves through the handle's
+ *     latch in set order, enqueue order for the queued form, as in every _each form), noise_bound (for that latch), cbar2 and
+ *     cote_noise_bound, rotation_gnc_factor, rotation_cost_threshold, rotation_max_iterations, cote_mode,
+ *     using_rot_inliers_when_estimating_cote, use_pre_estimated_RyRx and RyRx.  The front-end, matcher and clique fields are
+ *     ignored, inlier_selection_mode included: the caller supplied the inliers.
+ *   Degenerate sets follow qb200_solve_pose: L < 2 gives QB200_DEGENERATE_INPUT, at most one inlier QB200_DEGENERATE_CLIQUE; the pose
+ *     is the identity and the mask entries are 0.
+ *   Invalid sets.  An inlier id outside [0, L) refuses that set with status QB200_ERR_BAD_ARG, in either memory kind.  This is decided
+ *     on the device before the pose runs, so no point is read through such an id.  The refused set's record has valid = 0, an identity
+ *     T, n_corr = L and every other field 0; it gets no list entries, and the other sets are unaffected.  (qb200_solve_pose refuses
+ *     such an id for the whole call.)
+ *   Lists.  As in qb200_solve_batch_ex: corr, src_matched4 and tgt_matched4 must be NULL; clique echoes the list the pose used,
+ *     final_inliers and the masks are as above; clipping to cap_per_pair sets QB200_FLAG_LISTS_TRUNCATED.
+ *   Checks run before anything starts or is queued: n < 0, L < 0 or L > max_corr, n_inliers < 0 or n_inliers > L, NULL points with
+ *     L > 0, a NULL list with n_inliers > 0, a NULL results array, an unknown kind, a bad params entry, a bad list descriptor, and in
+ *     QB200_MEM_DEVICE kind points that are not memory of the handle's device or not 16-byte aligned, or ids that are not 4-byte
+ *     aligned.  A rejected call gives QB200_ERR_BAD_ARG, writes no record or list entry, queues nothing, and qb200_last_error names
+ *     the set, entry or array; batches already queued still complete on the flush.
+ *   qb200_get_stage_ms reports [0] h2d (points, ids and their import), [6] pose and [7] d2h; the other stages are 0.
+ *     qb200_get_kernel_ms reports zeros.
+ * The params array and the list descriptor are copied by the call.  A clique list of qb200_max_clique_batch_each (clique + i *
+ * cap_per_pair, n_inliers = clique_size) is set i's inlier list in the same memory kind, device arrays included. */
+typedef struct qb200_inlier_set {
+  const float* a;          /* L x 4 floats, source side (as qb200_corr_set) */
+  const float* b;          /* L x 4 floats, target side */
+  const int32_t* inliers;  /* n_inliers correspondence ids, in the order the chain TIMs take them, or NULL when n_inliers == 0 */
+  int32_t L;               /* <= max_corr */
+  int32_t n_inliers;       /* 0 .. L */
+} qb200_inlier_set;
+int qb200_solve_pose_batch_each(qb200_handle* h, const qb200_inlier_set* sets, int32_t n_sets, const qb200_params* params,
+                                qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+/* qb200_solve_pose_batch_each, queued: completed by qb200_register_batch_flush like every enqueue, in one stream with every other
+ * enqueue form.  The sets array is read by the call; host-kind points and ids, `results` and the host list arrays must stay valid until
+ * the flush returns.  Records and lists are byte-identical to the blocking call's. */
+int qb200_solve_pose_batch_enqueue_each(qb200_handle* h, const qb200_inlier_set* sets, int32_t n_sets, const qb200_params* params,
+                                        qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
 
 /* --- multi-GPU: batches of independent pairs shard across the GPUs of one box; the only communication is ONE all-gather (NCCL over
  * NVLink) of the fixed-size result records per batch -- north_star / SURVEY.md 8(e).  The reference has no counterpart (it is a

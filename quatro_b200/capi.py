@@ -100,6 +100,11 @@ class Graph(C.Structure):
     _fields_ = [("edges", C.c_void_p), ("adj", C.c_void_p), ("n_edges", C.c_int64), ("L", C.c_int32), ("words_per_row", C.c_int32)]
 
 
+class InlierSet(C.Structure):
+    """qb200_inlier_set: one set of qb200_solve_pose_batch_each, its matched points and the caller's inlier ids (in chain order)."""
+    _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("inliers", C.c_void_p), ("L", C.c_int32), ("n_inliers", C.c_int32)]
+
+
 class GraphOut(C.Structure):
     """qb200_graph_out: caller-owned outputs of qb200_build_graph_batch_each: adjacency rows, degrees and edge lists of every set."""
     _fields_ = [("kind", C.c_int32), ("rows_per_set", C.c_int32), ("words_per_row", C.c_int32), ("reserved", C.c_int32),
@@ -334,6 +339,8 @@ _SIGNATURES = {
     "qb200_max_clique_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_build_graph_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(GraphOut)]),
     "qb200_build_graph_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(GraphOut)]),
+    "qb200_solve_pose_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_solve_pose_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -419,6 +426,23 @@ def _graph_array(graphs: Sequence):
             a = np.ascontiguousarray(g, np.uint32)
             keep.append(a)
             arr[i].adj, arr[i].L, arr[i].words_per_row = (a.ctypes.data if a.size else None), a.shape[0], a.shape[1]
+    return arr, keep
+
+
+def _inlier_array(sets: Sequence, inliers: Sequence, kind: int):
+    """(InlierSet * n) array of `sets` (as _set_array takes them) with inliers[i] as set i's ids: an int array (MEM_HOST) or a
+    (ids_ptr, n_inliers) device tuple (MEM_DEVICE); and the contiguous host arrays it points to."""
+    assert len(inliers) == len(sets)
+    arr = (InlierSet * max(len(sets), 1))()
+    pts, keep = _set_array(sets, kind)
+    for i, ids in enumerate(inliers):
+        arr[i].a, arr[i].b, arr[i].L = pts[i].a, pts[i].b, pts[i].L
+        if kind == MEM_HOST:
+            ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+            keep.append(ids)
+            arr[i].inliers, arr[i].n_inliers = (ids.ctypes.data if len(ids) else None), len(ids)
+        else:
+            arr[i].inliers, arr[i].n_inliers = ids[0], ids[1]
     return arr, keep
 
 
@@ -974,6 +998,24 @@ class Handle:
         return self._check(self.lib.qb200_build_graph_batch_enqueue_each(self.h, set_array, n, params_array, kind, _ptr(out),
                                                                          C.byref(buffers.descriptor())),
                            "qb200_build_graph_batch_enqueue_each")
+
+    # ---- caller inlier sets -> poses (qb200_solve_pose_batch_each) ----
+    inlier_array = staticmethod(_inlier_array)
+
+    def solve_pose_batch_each(self, sets: Sequence, inliers: Sequence, params: Sequence[Params], kind: int = MEM_HOST,
+                              buffers: Optional[ListBuffers] = None):
+        """qb200_solve_pose_batch_each: set i (as solve_batch takes it) is solved from the ids inliers[i] (see inlier_array(); chain
+        order, not sorted) with params[i]; buffers: a ListBuffers of SET_LISTS, or None for records only."""
+        assert len(params) == len(sets)
+        arr, keep = self.inlier_array(sets, inliers, kind)
+        return self._batch_lists("qb200_solve_pose_batch_each", len(sets), (arr, len(sets), self.params_array(params), kind), buffers)
+
+    def solve_pose_batch_enqueue_each_raw(self, inlier_array, n: int, params_array, kind: int, out: np.ndarray,
+                                          buffers: Optional[ListBuffers] = None):
+        """qb200_solve_pose_batch_enqueue_each: inlier_array (inlier_array()) and params_array (params_array()) are read by the call;
+        the host arrays behind inlier_array, `out` and the buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_solve_pose_batch_enqueue_each(self.h, inlier_array, n, params_array, kind, _ptr(out),
+                                                                        self._lists_arg(buffers)), "qb200_solve_pose_batch_enqueue_each")
 
     def cache_scans_enqueue_each_raw(self, scan_ptrs, counts, slot_ids, n: int, params_array, kind: int):
         """qb200_cache_scans_enqueue_each: scan_ptrs / counts (_scan_arrays()), slot_ids (c_int32 * n) and params_array

@@ -104,6 +104,8 @@ int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   QB_CUDA_TRY(L, L->h_feat.alloc(C));
   QB_CUDA_TRY(L, L->d_graph.alloc(S));
   QB_CUDA_TRY(L, L->h_graph.alloc(S));
+  QB_CUDA_TRY(L, L->d_inl.alloc(S));
+  QB_CUDA_TRY(L, L->h_inl.alloc(S));
   // the sort workspace serves the voxel sort (C*R items, digit histograms in val_a, chunk counts C*kVsChunks <= n_sort in val_b),
   // the lattice / norm sorts (C*V items) and, afterwards, the duplicate-class tables of K6 (2S*V + 2S words in key_a): size it for
   // the largest user
@@ -281,6 +283,15 @@ PairSolve clique_entry(const qb200_params& p) {
   e.kcore_thr = p.kcore_heuristic_threshold;
   e.node_limit = p.max_clique_node_limit > 0 ? p.max_clique_node_limit : (long long)QB200_DEFAULT_CLIQUE_NODE_LIMIT;
   e.mode = p.inlier_selection_mode;
+  return e;
+}
+
+// a pose wave's entry: the pose fields of p (rotation noise bound resolved) as qb200_solve_pose reads them; nothing of the matcher,
+// graph or clique stages
+PairSolve pose_entry(const qb200_params& p) {
+  PairSolve e;
+  memset(&e, 0, sizeof(e));
+  e.pp = pose_params(p);
   return e;
 }
 
@@ -492,15 +503,16 @@ struct BatchCall {
   const qb200_feature_pair* feats = nullptr;   // FeaturePairs: keypoints and FPFH-33 rows, front-end fields of the entries ignored
   const qb200_corr_set* sets = nullptr;        // CorrSets
   const qb200_graph* graphs = nullptr;         // Graphs
+  const qb200_inlier_set* inlier_sets = nullptr;  // InlierSets
   const float* const* scans = nullptr;         // RawScans, KeypointClouds (described with the lattice fields of their entries alone):
   const int32_t* n_points = nullptr;           // scan i has n_points[i] points
   // the outputs, one set per sink
-  qb200_result* results = nullptr;             // Solve, Match, Clique, Graph: one record per input
+  qb200_result* results = nullptr;             // Solve, Match, Clique, Graph, Pose: one record per input
   const qb200_pair_lists* lists = nullptr;     // ... and the per-pair lists, nullptr = records only
   const int32_t* slot_ids = nullptr;           // CacheSlots: scan i goes to slot slot_ids[i]
   const qb200_feature_out* out = nullptr;      // Export: the caller's feature arrays
   const qb200_graph_out* graph_out = nullptr;  // Graph: the caller's adjacency, degree and edge arrays
-  // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved (Solve), laid out like `caller`.
+  // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved (Solve, Pose), laid out like `caller`.
   const qb200_params* params = nullptr;
   // host inputs of a multi-wave batch crossing PCIe: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies
   // queued on several streams share the PCIe link, so every wave's scans would arrive late; on one stream they arrive wave after
@@ -511,13 +523,13 @@ struct BatchCall {
 
 // The facts of each source that the checks and the waves read, written down once
 
-// clouds one input takes in the wave's 2S cloud buffers: two per pair, one per scan, none per set (its matched points go to ma / mb)
-// or graph (its adjacency goes to adj)
+// clouds one input takes in the wave's 2S cloud buffers: two per pair, one per scan, none per set (its matched points go to ma / mb,
+// an inlier set's ids to clique) or graph (its adjacency goes to adj)
 int clouds_per_input(Source s) {
   switch (s) {
     case Source::RawPairs: case Source::CachedPairs: case Source::FeaturePairs: return 2;
     case Source::RawScans: case Source::KeypointClouds: return 1;
-    case Source::CorrSets: case Source::Graphs: return 0;
+    case Source::CorrSets: case Source::Graphs: case Source::InlierSets: return 0;
   }
   return 0;
 }
@@ -526,45 +538,46 @@ int clouds_per_input(Source s) {
 bool is_pairs(Source s) { return clouds_per_input(s) == 2; }
 
 // Host-kind inputs of the source cross PCIe in a staged front (stage_raw, stage_features): a multi-wave batch sends them on the
-// shared copy stream and opens with a quarter wave.  Cached pairs, correspondence sets and graphs do neither.
+// shared copy stream and opens with a quarter wave.  Cached pairs, correspondence sets, graphs and inlier sets do neither.
 bool crosses_pcie(Source s) {
   switch (s) {
     case Source::RawPairs: case Source::FeaturePairs: case Source::RawScans: case Source::KeypointClouds: return true;
-    case Source::CachedPairs: case Source::CorrSets: case Source::Graphs: return false;
+    case Source::CachedPairs: case Source::CorrSets: case Source::Graphs: case Source::InlierSets: return false;
   }
   return false;
 }
 
 // The wave uploads the front-end table d_front: K1..K5 (K2..K5 for keypoint clouds) read each cloud's entry.  The solver table
-// d_solve is uploaded by the waves with records (Solve, Match, Clique), i.e. of pairs, sets and graphs.
+// d_solve is uploaded by the waves with records (Solve, Match, Clique, Graph, Pose), i.e. of pairs, sets and graphs.
 bool runs_front_end(Source s) {
   switch (s) {
     case Source::RawPairs: case Source::RawScans: case Source::KeypointClouds: return true;
-    case Source::CachedPairs: case Source::FeaturePairs: case Source::CorrSets: case Source::Graphs: return false;
+    case Source::CachedPairs: case Source::FeaturePairs: case Source::CorrSets: case Source::Graphs: case Source::InlierSets: return false;
   }
   return false;
 }
 
-bool has_records(Sink k) { return k == Sink::Solve || k == Sink::Match || k == Sink::Clique || k == Sink::Graph; }
+bool has_records(Sink k) { return k == Sink::Solve || k == Sink::Match || k == Sink::Clique || k == Sink::Graph || k == Sink::Pose; }
 
 // The stage-time slots of qb200_get_stage_ms a wave reports (bit i = slot i, the time between events i and i + 1 of Lane::ev).
 // A wave reports the stages its source runs: cached pairs their copy-in in the fpfh slot, caller features their copy and import in
 // h2d.  Cached pairs and sets report no d2h slot; waves without records report none (they register nothing).  A match wave reports
 // the slots up to match as its source has them, and d2h.  A graph wave reports h2d, its import in the graph slot, clique and d2h; a
-// TIM graph wave h2d, graph (K8 and its outputs) and d2h.
+// TIM graph wave h2d, graph (K8 and its outputs) and d2h; a pose wave h2d (with the id import), pose and d2h.
 unsigned stage_slots(Source s, Sink k) {
   enum : unsigned { kH2d = 1, kVoxel = 2, kFpfh = 4, kMatch = 8, kGraph = 16, kClique = 32, kPose = 64, kD2h = 128 };
   constexpr unsigned kSolver = kGraph | kClique | kPose;
   if (!has_records(k)) return 0u;
   if (k == Sink::Clique) return kH2d | kGraph | kClique | kD2h;
   if (k == Sink::Graph) return kH2d | kGraph | kD2h;
+  if (k == Sink::Pose) return kH2d | kPose | kD2h;
   unsigned m = 0;
   switch (s) {
     case Source::RawPairs: m = kH2d | kVoxel | kFpfh | kMatch | kSolver | kD2h; break;
     case Source::FeaturePairs: m = kH2d | kMatch | kSolver | kD2h; break;
     case Source::CachedPairs: m = kFpfh | kMatch | kSolver; break;
     case Source::CorrSets: m = kSolver; break;
-    case Source::RawScans: case Source::KeypointClouds: case Source::Graphs: break;
+    case Source::RawScans: case Source::KeypointClouds: case Source::Graphs: case Source::InlierSets: break;
   }
   return k == Sink::Match ? (m & (kH2d | kVoxel | kFpfh | kMatch)) | kD2h : m;
 }
@@ -739,6 +752,7 @@ int fill_tables(Lane* L, const BatchCall& in, int w0, int np) {
                     : in.sink == Sink::Match  ? match_entry(p)
                     : in.sink == Sink::Clique ? clique_entry(p)
                     : in.sink == Sink::Graph  ? graph_entry(p)
+                    : in.sink == Sink::Pose   ? pose_entry(p)
                                               : solve_entry(p);
     if (in.src == Source::RawPairs) L->h_front[2 * s] = L->h_front[2 * s + 1] = own ? front_entry(p) : L->h_front[0];
   }
@@ -826,20 +840,48 @@ int front_cached(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np, 
   return QB200_OK;
 }
 
+// set s's n matched points a / b (caller memory of the call's kind) into its slots of ma / mb, and n into h_cloud_n[s]
+int copy_set_points(Lane* L, const BatchCall& in, int s, const float* a, const float* b, int n) {
+  const cudaMemcpyKind ck = in.kind == QB200_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+  L->h_cloud_n[s] = n;
+  if (n > 0) {
+    QB_CUDA_TRY(L, cudaMemcpyAsync(L->ma + (size_t)s * L->Lc, a, (size_t)n * sizeof(float4), ck, L->stream));
+    QB_CUDA_TRY(L, cudaMemcpyAsync(L->mb + (size_t)s * L->Lc, b, (size_t)n * sizeof(float4), ck, L->stream));
+  }
+  return QB200_OK;
+}
+
 // Correspondence sets: the matched points of every set into ma / mb and its size into n_corr
 int front_sets(Lane* L, const BatchCall& in, int w0, int np) {
   cudaEventRecord(L->ev[0], L->stream);
   if (int rc = wave_reset(L, 0)) return rc;
-  const cudaMemcpyKind ck = in.kind == QB200_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
   for (int s = 0; s < np; ++s) {
     const qb200_corr_set& cs = in.sets[w0 + s];
-    L->h_cloud_n[s] = cs.L;
-    if (cs.L > 0) {
-      QB_CUDA_TRY(L, cudaMemcpyAsync(L->ma + (size_t)s * L->Lc, cs.a, (size_t)cs.L * sizeof(float4), ck, L->stream));
-      QB_CUDA_TRY(L, cudaMemcpyAsync(L->mb + (size_t)s * L->Lc, cs.b, (size_t)cs.L * sizeof(float4), ck, L->stream));
-    }
+    if (int rc = copy_set_points(L, in, s, cs.a, cs.b, cs.L)) return rc;
   }
   QB_CUDA_TRY(L, cudaMemcpyAsync(L->ctr.n_corr, L->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, L->stream));
+  for (int i = 1; i <= 4; ++i) cudaEventRecord(L->ev[i], L->stream);  // no voxel, fpfh or match stage: slots 1 .. 3 are not reported
+  return QB200_OK;
+}
+
+// Inlier sets: the matched points as front_sets copies them, then every set's ids into its slot of clique (inlier_import_kernel).
+// Device ids are read in place through the table d_inl; host ids cross PCIe into the set's slot of corr_src, which a pose wave leaves
+// idle (it has no correspondences to pack), and are imported from there.  The import is part of the h2d stage.
+int front_inlier_sets(Lane* L, const BatchCall& in, int w0, int np) {
+  cudaEventRecord(L->ev[0], L->stream);
+  if (int rc = wave_reset(L, 0)) return rc;
+  const bool host = in.kind == QB200_MEM_HOST;
+  for (int s = 0; s < np; ++s) {
+    const qb200_inlier_set& is = in.inlier_sets[w0 + s];
+    if (int rc = copy_set_points(L, in, s, is.a, is.b, is.L)) return rc;
+    int* stage = L->corr_src + (size_t)s * L->Lc;
+    if (host && is.n_inliers > 0)
+      QB_CUDA_TRY(L, cudaMemcpyAsync(stage, is.inliers, (size_t)is.n_inliers * sizeof(int), cudaMemcpyHostToDevice, L->stream));
+    L->h_inl[s] = InlierSrc{host ? stage : is.inliers, is.n_inliers, 0};
+  }
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_inl, L->h_inl, (size_t)np * sizeof(InlierSrc), cudaMemcpyHostToDevice, L->stream));
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->ctr.n_corr, L->h_cloud_n, (size_t)np * sizeof(int), cudaMemcpyHostToDevice, L->stream));
+  if (int rc = launch_inlier_import(L, np)) return rc;
   for (int i = 1; i <= 4; ++i) cudaEventRecord(L->ev[i], L->stream);  // no voxel, fpfh or match stage: slots 1 .. 3 are not reported
   return QB200_OK;
 }
@@ -992,6 +1034,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     case Source::CachedPairs: rc = front_cached(h, L, in, w0, np, ncl); break;
     case Source::CorrSets: rc = front_sets(L, in, w0, np); break;
     case Source::Graphs: rc = front_graphs(L, in, w0, np); break;
+    case Source::InlierSets: rc = front_inlier_sets(L, in, w0, np); break;
   }
   if (rc) return rc;
   const bool match_pairs = is_pairs(in.src);
@@ -1032,6 +1075,12 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       rc = send_records(L, in, w0, np);
       break;
     }
+    case Sink::Pose:  // K10 / K11 on the imported ids, with the counters qb200_solve_pose gives (no front end), then the refusals
+      for (int i = 5; i <= 6; ++i) cudaEventRecord(L->ev[i], L->stream);
+      if ((rc = launch_fill_counters(L, np, 0)) || (rc = launch_pose(L, np)) || (rc = launch_pose_records(L, np))) return rc;
+      cudaEventRecord(L->ev[7], L->stream);
+      rc = send_records(L, in, w0, np);
+      break;
   }
   if (rc) return rc;
   L->pend_w0 = w0;
@@ -1057,7 +1106,7 @@ int wave_collect(qb200_handle* h, Lane* L) {
   }
   int rc = QB200_OK;
   switch (L->pend_sink) {
-    case Sink::Solve: case Sink::Match: case Sink::Clique:
+    case Sink::Solve: case Sink::Match: case Sink::Clique: case Sink::Pose:
       memcpy(L->pend_dst + L->pend_w0, L->h_results, (size_t)np * sizeof(qb200_result));
       if (L->pend_host_lists) deliver_lists(L, L->pend_lists, L->pend_w0, np);
       break;
@@ -1157,6 +1206,7 @@ const void* input_of(const BatchCall& c) {
     case Source::CorrSets: return c.sets;
     case Source::RawScans: case Source::KeypointClouds: return c.scans;
     case Source::Graphs: return c.graphs;
+    case Source::InlierSets: return c.inlier_sets;
   }
   return nullptr;
 }
@@ -1212,7 +1262,8 @@ int check_call(qb200_handle* h, const BatchCall& c) {
       return QB200_ERR_UNSUPPORTED;
     }
   }
-  if (int rc = check_lists(h, c.lists, c.src == Source::CorrSets, c.sink == Sink::Match, c.src == Source::Graphs)) return rc;
+  const bool sets = c.src == Source::CorrSets || c.src == Source::InlierSets;
+  if (int rc = check_lists(h, c.lists, sets, c.sink == Sink::Match, c.src == Source::Graphs)) return rc;
   if (c.sink == Sink::Export)
     if (int rc = check_out(h, c.out, c.src == Source::KeypointClouds)) return rc;
   if (c.sink == Sink::Graph)
@@ -1263,6 +1314,23 @@ int check_call(qb200_handle* h, const BatchCall& c) {
         if (s.L < 0 || s.L > h->cfg.max_corr || (s.L > 0 && (!s.a || !s.b))) bad = "it is null or its L is outside 0 .. max_corr";
         else if (rows && s.L > c.graph_out->rows_per_set) bad = "its L exceeds rows_per_set";
         if (bad && c.sink != Sink::Graph) return reject("correspondence set is null or exceeds max_corr");
+        if (bad) {
+          snprintf(why, sizeof(why), "set %d: %s", i, bad);
+          return reject(why);
+        }
+        break;
+      }
+      case Source::InlierSets: {
+        const qb200_inlier_set& s = c.inlier_sets[i];
+        const bool device = c.kind == QB200_MEM_DEVICE;
+        if (s.L < 0 || s.L > h->cfg.max_corr) bad = "its L is outside 0 .. max_corr";
+        else if (s.n_inliers < 0 || s.n_inliers > s.L) bad = "its n_inliers is outside 0 .. L";
+        else if (s.L > 0 && (!s.a || !s.b)) bad = "its points are null";
+        else if (s.n_inliers > 0 && !s.inliers) bad = "its inlier list is null";
+        else if (device && s.L > 0 && !(device_array_of(h, s.a, 16) && device_array_of(h, s.b, 16)))
+          bad = "its points are misaligned (16 bytes) or not memory of the handle's device";
+        else if (device && s.n_inliers > 0 && !device_array_of(h, s.inliers, 4))
+          bad = "its inlier list is misaligned (4 bytes) or not memory of the handle's device";
         if (bad) {
           snprintf(why, sizeof(why), "set %d: %s", i, bad);
           return reject(why);
@@ -1334,9 +1402,9 @@ int enqueue_call(qb200_handle* h, BatchCall c) {
   // An empty call resolves no params: the reference latches the rotation noise bound inside computeTransformation, which an empty
   // batch never calls.
   if (c.n == 0) return QB200_OK;
-  // only the solver reads the rotation noise bound: the other sinks resolve nothing
+  // only the solver and the pose read the rotation noise bound: the other sinks resolve nothing
   std::unique_ptr<qb200_params[]> pr;
-  const bool solves = c.sink == Sink::Solve;
+  const bool solves = c.sink == Sink::Solve || c.sink == Sink::Pose;
   if (solves && !(pr = resolve_call(h, c.caller, c.n, c.each()))) return QB200_ERR_CUDA;
   c.params = solves ? pr.get() : c.caller;
   // S: inputs per wave, pairs, sets or scans; the clouds of a wave fill the lane's 2 * max_batch_slots cloud buffers
@@ -1477,6 +1545,14 @@ BatchCall caller_graphs(const qb200_graph* graphs, int32_t n, const qb200_params
                         const qb200_pair_lists* lists) {
   BatchCall c{Source::Graphs, Sink::Clique, n, kind, p, Entries::Mixed};
   c.graphs = graphs; c.results = results; c.lists = lists;
+  return c;
+}
+
+// each inlier set is solved with its own entry
+BatchCall inlier_sets(const qb200_inlier_set* sets, int32_t n, const qb200_params* p, qb200_mem_kind kind, qb200_result* results,
+                      const qb200_pair_lists* lists) {
+  BatchCall c{Source::InlierSets, Sink::Pose, n, kind, p, Entries::Mixed};
+  c.inlier_sets = sets; c.results = results; c.lists = lists;
   return c;
 }
 
@@ -1801,6 +1877,17 @@ int qb200_build_graph_batch_each(qb200_handle* h, const qb200_corr_set* sets, in
 int qb200_build_graph_batch_enqueue_each(qb200_handle* h, const qb200_corr_set* sets, int32_t n_sets, const qb200_params* params,
                                          qb200_mem_kind kind, qb200_result* results, const qb200_graph_out* out) {
   return enqueue_call(h, corr_sets(sets, n_sets, params, kind, results, out));
+}
+
+// ---- caller inlier sets -> poses ------------------------------------------------------------------------------------------------
+int qb200_solve_pose_batch_each(qb200_handle* h, const qb200_inlier_set* sets, int32_t n_sets, const qb200_params* params,
+                                qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return run_call(h, inlier_sets(sets, n_sets, params, kind, results, lists));
+}
+
+int qb200_solve_pose_batch_enqueue_each(qb200_handle* h, const qb200_inlier_set* sets, int32_t n_sets, const qb200_params* params,
+                                        qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_call(h, inlier_sets(sets, n_sets, params, kind, results, lists));
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

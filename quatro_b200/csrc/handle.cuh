@@ -109,18 +109,27 @@ struct GraphDst {
   int words_per_row;
 };
 
+// Where inlier_import_kernel reads one caller inlier set's correspondence ids (pose.cu): n ids in the caller's device memory or in
+// the lane's staging (corr_src, the set's slot)
+struct InlierSrc {
+  const int* ids;
+  int n, pad;
+};
+
 // What a batch call reads (api.cu: BatchCall), per input: a pair of raw scans, a pair of cached scans (slots), a pair of caller
-// keypoint clouds with their FPFH-33 rows, a correspondence set, one raw scan, one caller keypoint cloud, or one caller graph
-enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, KeypointClouds, Graphs };
+// keypoint clouds with their FPFH-33 rows, a correspondence set, one raw scan, one caller keypoint cloud, one caller graph, or a
+// correspondence set with the caller's inlier ids
+enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, KeypointClouds, Graphs, InlierSets };
 // What a batch call produces: solved records (and lists), the matcher's records (and lists), cache slots, front-end features in
-// caller memory, max-clique records (and clique lists), or TIM graphs in caller memory (and records).  The valid (source, sink)
-// pairs:
+// caller memory, max-clique records (and clique lists), TIM graphs in caller memory (and records), or poses of given inlier sets
+// (records and lists).  The valid (source, sink) pairs:
 //   RawPairs, CachedPairs, FeaturePairs  x  Solve, Match   qb200_register_batch*, _cached*, _features*; qb200_match_*
 //   CorrSets                             x  Solve, Graph   qb200_solve_batch*, qb200_build_graph_batch*
 //   RawScans                             x  CacheSlots     qb200_cache_scans*
 //   RawScans, KeypointClouds             x  Export         qb200_describe_batch*, qb200_describe_points*
 //   Graphs                               x  Clique         qb200_max_clique_batch*
-enum class Sink { Solve, Match, CacheSlots, Export, Clique, Graph };
+//   InlierSets                           x  Pose           qb200_solve_pose_batch*
+enum class Sink { Solve, Match, CacheSlots, Export, Clique, Graph, Pose };
 
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
@@ -147,11 +156,12 @@ struct Lane {
   DeviceMem<int> d_slot_of_cloud; PinnedMem<int> h_slot_of_cloud;  // [2S] cache slot of every cloud of the wave, and its pinned mirror
   DeviceMem<FeatureSrc> d_feat; PinnedMem<FeatureSrc> h_feat;  // [2S] where a feature wave's clouds are read, and its pinned mirror
   DeviceMem<GraphSrc> d_graph; PinnedMem<GraphSrc> h_graph;   // [S] where a graph wave's graphs are read, and its pinned mirror
+  DeviceMem<InlierSrc> d_inl; PinnedMem<InlierSrc> h_inl;     // [S] where a pose wave's inlier ids are read, and its pinned mirror
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
   unsigned pend_stages;      // ... the stage-time slots it reports (bit i: qb200_get_stage_ms slot i)
   Sink pend_sink;             // ... what wave_collect hands on for it: the fields below of its sink
-  qb200_result* pend_dst;     // ... (Solve, Match, Clique, Graph) the caller's record array of its batch, nullptr for the other sinks
-  bool pend_host_lists;       // ... (Solve, Match, Clique) its batch has host-kind lists, which wave_collect hands on from lst_stage
+  qb200_result* pend_dst;     // ... (Solve, Match, Clique, Graph, Pose) the caller's record array of its batch, nullptr for the other sinks
+  bool pend_host_lists;       // ... (Solve, Match, Clique, Pose) its batch has host-kind lists, which wave_collect hands on from lst_stage
   qb200_pair_lists pend_lists; // ... and then a copy of their descriptor
   qb200_feature_out pend_out; // ... (Export) a copy of its batch's output descriptor, whose counts and status (and, in host kind,
                               // entries) wave_collect hands on from exp_stage
@@ -400,6 +410,12 @@ int launch_graph_export(Lane* h, int n_sets, const GraphDst& d);
 int launch_edge_offsets(Lane* h, int n_sets);
 int launch_edge_emit(Lane* h, int n_sets, int only, long long e0, long long e1, int2* out, long long out_stride);
 int launch_graph_records(Lane* h, int n_sets, long long cap_edges);
+// Pose waves (pose.cu): launch_inlier_import writes the ids of every set of the table d_inl into its slot of clique and their count
+// into ctr.n_clique, and refuses a set with an id outside [0, n_corr): status QB200_ERR_BAD_ARG in ctr.cloud_status[set] and n_clique
+// 0, so that pose_kernel reads no point through it.  After pose_kernel, launch_pose_records turns every refused set's record into a
+// QB200_ERR_BAD_ARG record: valid 0, identity T, n_corr = L, the rest 0.
+int launch_inlier_import(Lane* h, int n_sets);
+int launch_pose_records(Lane* h, int n_sets);
 // the checks every entry of a registering call passes; solver = false: the front-end and matcher fields only (a match call)
 bool params_ok(const qb200_params* p, bool solver = true);
 float lattice_cell(const qb200_params& p);

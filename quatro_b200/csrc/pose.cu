@@ -13,6 +13,10 @@
 //    global-memory workspace of the pair (same code, L2-resident) -- and the running
 //    sums of the sweep are then accumulated sequentially by one thread in exactly the reference's
 //    order, so the argmin and the "median" candidate set follow the CPU path.
+//
+// A pose wave (qb200_solve_pose_batch_*) runs the same kernel on cliques the caller supplies: inlier_import_kernel brings each set's
+// ids into its clique slot and refuses a set with an id outside [0, L) before pose_kernel runs; pose_records_kernel writes the
+// refused sets' records after it.
 #include "handle.cuh"
 
 namespace qb {
@@ -345,6 +349,39 @@ __global__ void finalize_status_kernel(qb200_result* __restrict__ results, int n
   }
 }
 
+// One CTA per set of a pose wave: the caller's ids (device memory in place, host ids from the staging) into the set's clique slot, in
+// the caller's order, duplicates kept.  A set with an id outside [0, L) gets n_clique = 0 and QB200_ERR_BAD_ARG in bad[set]; it is
+// decided before pose_kernel runs, so no point is read through such an id.
+__global__ void __launch_bounds__(kPoseThreads) inlier_import_kernel(const InlierSrc* __restrict__ src, const int* __restrict__ n_corr, int Lc,
+                                                                     int* __restrict__ clique, int* __restrict__ n_clique, int* __restrict__ bad) {
+  const int set = blockIdx.x;
+  const InlierSrc e = src[set];
+  const unsigned L = (unsigned)n_corr[set];
+  int* __restrict__ cl = clique + (size_t)set * Lc;
+  int out = 0;
+  for (int i = threadIdx.x; i < e.n; i += kPoseThreads) {
+    const int v = e.ids[i];
+    out |= (unsigned)v >= L;  // -1 and INT32_MAX alike
+    cl[i] = v;
+  }
+  out = __syncthreads_or(out);
+  if (threadIdx.x == 0) {
+    n_clique[set] = out ? 0 : e.n;
+    bad[set] = out ? QB200_ERR_BAD_ARG : QB200_OK;
+  }
+}
+
+// after pose_kernel: a refused set's record (pose_kernel solved it as an empty clique) becomes QB200_ERR_BAD_ARG with n_corr = L
+__global__ void pose_records_kernel(qb200_result* __restrict__ results, int n_sets, const int* __restrict__ bad, const int* __restrict__ n_corr) {
+  const int set = blockIdx.x * blockDim.x + threadIdx.x;
+  if (set >= n_sets || bad[set] == QB200_OK) return;
+  qb200_result r = {};
+  r.status = bad[set];
+  r.n_corr = n_corr[set];
+  for (int i = 0; i < 16; ++i) r.T[i] = (i % 5 == 0) ? 1.0 : 0.0;
+  results[set] = r;
+}
+
 __global__ void iota_clique_kernel(const int* __restrict__ n_corr, const PairSolve* __restrict__ solve, int Lc, int* __restrict__ clique,
                                    int* __restrict__ n_clique, int* __restrict__ max_core) {
   const int pair = blockIdx.y;
@@ -398,6 +435,20 @@ int launch_fill_counters(Lane* h, int n_pairs, int have_frontend) {
 int launch_finalize_status(Lane* h, int n_pairs) {
   finalize_status_kernel<<<(n_pairs + 127) / 128, 128, 0, h->stream>>>(h->d_results, n_pairs, h->ctr);
   h->launches++;
+  return QB200_OK;
+}
+int launch_inlier_import(Lane* h, int n_sets) {
+  if (n_sets <= 0) return QB200_OK;
+  inlier_import_kernel<<<n_sets, kPoseThreads, 0, h->stream>>>(h->d_inl, h->ctr.n_corr, h->Lc, h->clique, h->ctr.n_clique, h->ctr.cloud_status);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+int launch_pose_records(Lane* h, int n_sets) {
+  if (n_sets <= 0) return QB200_OK;
+  pose_records_kernel<<<(n_sets + 127) / 128, 128, 0, h->stream>>>(h->d_results, n_sets, h->ctr.cloud_status, h->ctr.n_corr);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;
 }
 int launch_iota_clique(Lane* h, int n_pairs) {
