@@ -25,6 +25,7 @@
  *                                  (examples/run_global_registration.cpp:206-209)
  *   qb200_register_features_*   <- Matcher::calculateCorrespondences + Quatro::computeTransformation for every pair of a batch
  *                                  of caller keypoints and FPFH-33 descriptors (include/fpfh_manager.hpp:125-127)
+ *   qb200_voxelize_batch_*      <- voxelize<T>() for every scan of a batch (include/quatro.hpp:49-57)
  *   qb200_describe_batch_*      <- voxelize<T>() + FPFHEstimation::computeFPFHFeatures + FPFHManager::getObjDescriptor /
  *                                  getTgtNormals for every scan of a batch (include/fpfh_manager.hpp:161-177)
  *   qb200_describe_points_*     <- FPFHEstimation::computeFPFHFeatures for every caller keypoint cloud of a batch
@@ -381,7 +382,8 @@ int qb200_solve_batch_ex(qb200_handle* h, const qb200_corr_set* sets, int32_t n_
  * every queued batch must stay valid until a flush (or qb200_register_batch, = enqueue + flush) returns.  Other entry points flush
  * implicitly.  Raw, cached, caller-feature and correspondence-set batches (qb200_register_cached_enqueue_mixed,
  * qb200_register_features_enqueue_each, qb200_solve_batch_enqueue_each), scan-cache writes (qb200_cache_scans_enqueue_each) and describe
- * calls (qb200_describe_batch_enqueue_each, qb200_describe_points_enqueue_each) and match calls (qb200_match_*_enqueue_*) may be queued
+ * calls (qb200_describe_batch_enqueue_each, qb200_describe_points_enqueue_each), voxelize calls (qb200_voxelize_batch_enqueue_each)
+ * and match calls (qb200_match_*_enqueue_*) may be queued
  * in one stream and completed by a single flush; every access to a
  * cache slot follows enqueue order, so a queued cached batch registers the slot contents it was enqueued against.  qb200_cache_reserve,
  * qb200_cache_copy, qb200_cache_read and the pre-processing calls flush first, so they see every write queued before them. */
@@ -648,6 +650,42 @@ int qb200_describe_batch_each(qb200_handle* h, const float* const* scans4, const
  * caller-feature and correspondence-set batches and cache writes.  Host-kind scans and every output array (counts and status
  * included) must stay valid until the flush returns, which completes them.  The outputs are byte-identical to the blocking call's. */
 int qb200_describe_batch_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
+                                      const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out);
+
+/* --- the voxel filter in batches: VoxelGrid centroids of many scans into caller memory -----------------------------------------------
+ * voxelize<T> (include/quatro.hpp:49-57, pcl::VoxelGrid) for a batch of raw scans, each with its own leaf, and nothing after it: keyframes
+ * stored at a voxel size, another descriptor or registration back end, qb200_describe_points_each at radii chosen later.
+ *   Scan i (scans4[i]: n_points[i] x {x,y,z,w} in `kind` memory, 0 <= n_points[i] <= max_raw_points) is filtered with
+ *     params[i].voxel_size as the leaf and params[i].skip_flagged.  Every other field is ignored and not checked.
+ *   The output descriptor is qb200_feature_out with normals4 and desc33 NULL; vox4 may be NULL (counts and status only).
+ *   Scan i's outputs are byte-identical to qb200_voxelize(scan i, voxel_size, skip_flagged) on the same handle:
+ *     counts[i] is that call's *n_out given unlimited room, never clipped to cap_per_scan;
+ *     scan i's entries start at i * cap_per_scan, and the first min(counts[i], cap_per_scan) of the entries qb200_voxelize writes are
+ *     written, nothing past them;
+ *     status[i] is the scan's own filter status:
+ *       QB200_OK (an empty scan, or one whose points are all skipped, with count 0);
+ *       QB200_CAPACITY_EXCEEDED: more occupied voxels than max_voxel_points; the count is max_voxel_points and the entries are the
+ *         first centroids, as qb200_voxelize gives them;
+ *       QB200_ERR_VOXEL_OVERFLOW: PCL's pass-through.  The count is the number of kept points (finite x, y, z, and w >= 0 when
+ *         skip_flagged is set) and the entries are those input records, verbatim and in input order.  This count may exceed
+ *         max_voxel_points, up to max_raw_points.
+ *     Clipping by cap_per_scan shows only as counts[i] > cap_per_scan, never as a status: the one place where the call differs from
+ *     qb200_voxelize's return code.  No output depends on the batch, the wave, the lane, the memory kinds or the other scans.
+ *   Checks run before anything starts or is queued: n, the arrays and the kind; every scan's count and pointer (in QB200_MEM_DEVICE
+ *     kind memory of the handle's device, 16-byte aligned); every entry's voxel_size (> 0, as qb200_voxelize accepts a leaf; NaN is
+ *     refused); the output checks of qb200_describe_batch_each (cap_per_scan >= 1, counts and status, output kind, device vox4 on the
+ *     handle's device and 16-byte aligned); and NULL normals4 and desc33.  A rejected call gives QB200_ERR_BAD_ARG, writes no count,
+ *     status or entry, queues nothing, and qb200_last_error names the bad scan, entry or array; batches already queued still complete
+ *     on the flush.
+ *   The scans run in waves of 2 * max_batch_slots over the lanes, as describe calls do, and no normals or FPFH are computed.  Like
+ *     them it registers nothing: qb200_get_stage_ms and qb200_get_kernel_ms report zeros after it.
+ * The params array and the output descriptor are copied by the call. */
+int qb200_voxelize_batch_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
+                              const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out);
+/* qb200_voxelize_batch_each, queued: completed by qb200_register_batch_flush like every enqueue, in one stream with every other
+ * enqueue form.  Host-kind scans and every output array (counts and status included) must stay valid until the flush returns, which
+ * completes them.  The outputs are byte-identical to the blocking call's. */
+int qb200_voxelize_batch_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
                                       const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out);
 
 /* --- FPFH of caller keypoint clouds in batches: normals and FPFH-33 of many clouds, without the voxel filter ------------------------

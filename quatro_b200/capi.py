@@ -128,14 +128,15 @@ PREPROCESS_ARRAYS = ("ground4", "nonground4", "valid4", "outlier4")   # in the o
 
 
 class FeatureOut(C.Structure):
-    """qb200_feature_out: caller-owned outputs of qb200_describe_batch_each and qb200_describe_points_each, cap_per_scan keypoints
-    reserved per scan or cloud."""
+    """qb200_feature_out: caller-owned outputs of qb200_describe_batch_each, qb200_describe_points_each and qb200_voxelize_batch_each,
+    cap_per_scan keypoints reserved per scan or cloud."""
     _fields_ = [("cap_per_scan", C.c_int32), ("kind", C.c_int32), ("vox4", C.c_void_p), ("normals4", C.c_void_p), ("desc33", C.c_void_p),
                 ("counts", C.c_void_p), ("status", C.c_void_p)]
 
 
 FEATURE_ARRAYS = {"vox4": 4, "normals4": 4, "desc33": 33}   # output array -> floats per keypoint
 POINT_ARRAYS = ("normals4", "desc33")   # what qb200_describe_points_each can return (the keypoints are the caller's own)
+VOXEL_ARRAYS = ("vox4",)   # what qb200_voxelize_batch_each can return
 
 
 # list name -> (element dtype, trailing shape, count field of the record)
@@ -327,6 +328,8 @@ _SIGNATURES = {
     "qb200_register_features_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_describe_batch_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
     "qb200_describe_batch_enqueue_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
+    "qb200_voxelize_batch_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
+    "qb200_voxelize_batch_enqueue_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
     "qb200_describe_points_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
     "qb200_describe_points_enqueue_each": (i32, [vp, P(vp), P(i32), i32, P(Params), i32, P(FeatureOut)]),
     "qb200_match_batch_mixed": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
@@ -1057,6 +1060,25 @@ class Handle:
         return self._check(self.lib.qb200_describe_batch_enqueue_each(self.h, scan_ptrs, counts, n, params_array, kind, C.byref(out)),
                            "qb200_describe_batch_enqueue_each")
 
+    # ---- raw scans -> voxel centroids (the voxel filter in batches) ----
+    def voxelize_batch_each(self, scans: Sequence, params: Sequence[Params], kind: int = MEM_HOST, dest: int = MEM_HOST,
+                            cap_per_scan: Optional[int] = None, arrays: Optional[dict] = None):
+        """qb200_voxelize_batch_each: scan i (an (n,4) float32 array for MEM_HOST, a (device_ptr, n) tuple for MEM_DEVICE) is filtered
+        with params[i].voxel_size and skip_flagged, as voxelize() filters it.  cap_per_scan: entries reserved per scan (default
+        max_voxel_points).  arrays: the caller's own vox4 output ({"vox4": ...}, numpy for dest MEM_HOST or a CUDA tensor for MEM_DEVICE,
+        shape (n, cap, 4)), or {} for counts and status only.  Returns (per scan its vox4 trimmed to min(count, cap): a numpy copy, a
+        tensor view on the device, None without vox4; counts (n,) int32; status (n,) int32)."""
+        per_scan, counts, status = self._describe("qb200_voxelize_batch_each", VOXEL_ARRAYS, scans, params, kind, dest, cap_per_scan,
+                                                  arrays)
+        return [v[0] for v in per_scan], counts, status
+
+    def voxelize_batch_enqueue_each_raw(self, scan_ptrs, counts, n: int, params_array, kind: int, out: FeatureOut):
+        """qb200_voxelize_batch_enqueue_each: scan_ptrs / counts (_scan_arrays()), params_array (params_array()) and the descriptor `out`
+        (feature_out(), vox4 only or nothing) are read by the call; host-kind scans and every array `out` names must stay alive until
+        register_batch_flush."""
+        return self._check(self.lib.qb200_voxelize_batch_enqueue_each(self.h, scan_ptrs, counts, n, params_array, kind, C.byref(out)),
+                           "qb200_voxelize_batch_enqueue_each")
+
     # ---- caller keypoint clouds -> normals and FPFH-33 (FPFH without the voxel filter, in batches) ----
     def describe_points_each(self, clouds: Sequence, params: Sequence[Params], kind: int = MEM_HOST, dest: int = MEM_HOST,
                              cap_per_scan: Optional[int] = None, arrays: Optional[dict] = None):
@@ -1068,7 +1090,8 @@ class Handle:
         return self._describe("qb200_describe_points_each", POINT_ARRAYS, clouds, params, kind, dest, cap_per_scan, arrays)
 
     def _describe(self, fn: str, names, clouds, params, kind, dest, cap_per_scan, arrays):
-        """The two blocking describe calls: `names` = the output arrays the call can fill, in the order of the returned tuples."""
+        """The blocking describe and voxelize calls: `names` = the output arrays the call can fill, in the order of the returned
+        tuples."""
         n = len(clouds)
         assert len(params) == n
         cap = cap_per_scan or self.cfg.max_voxel_points

@@ -638,8 +638,11 @@ size_t export_stage(const Lane* L, const qb200_feature_out& o, unsigned char* ba
 
 // Enqueue the export of a describe wave (scans [w0, w0 + ncl) of lane L): its counts and status into the lane's staging block, its
 // entries straight into the caller's device arrays or into that block, from where wave_collect hands them on (deliver_export).  The
-// lane's previous wave has been collected, so a block that must grow is not in use.
-int submit_export(Lane* L, const qb200_feature_out& o, int w0, int ncl) {
+// lane's previous wave has been collected, so a block that must grow is not in use.  voxels: a voxelize wave, whose export reports
+// every cloud as qb200_voxelize does (ExportSrc::n_kept) and whose pass-through clouds get their kept points from passthrough_kernel:
+// straight into the caller's device vox4, or into their raw_stage regions, which no copy overwrites before wave_collect (the lane's next
+// wave stages its scans only after it).
+int submit_export(Lane* L, const qb200_feature_out& o, int w0, int ncl, bool voxels) {
   ExportDst d;
   const size_t bytes = export_stage(L, o, nullptr, &d);
   if (L->exp_bytes < bytes) {
@@ -649,30 +652,44 @@ int submit_export(Lane* L, const qb200_feature_out& o, int w0, int ncl) {
     L->exp_bytes = bytes;
   }
   export_stage(L, o, L->exp_stage, &d);
+  const ExportDst to = ExportDst::caller(o, w0);
   if (o.kind == QB200_MEM_DEVICE) {
-    const ExportDst to = ExportDst::caller(o, w0);
     d.vox = to.vox; d.nrm = to.nrm; d.desc = to.desc; d.stride = to.stride; d.cap = to.cap;
   }
-  const ExportSrc s{L->vox_pts, L->normals, L->desc_t, L->ctr.n_vox, L->ctr.cloud_status};
-  return launch_feature_export(L, ncl, s, d, L->V);
+  const ExportSrc s{L->vox_pts, L->normals, L->desc_t, L->ctr.n_vox, L->ctr.cloud_status, voxels ? L->ctr.n_valid : nullptr};
+  if (int rc = launch_feature_export(L, ncl, s, d, L->V)) return rc;
+  if (!voxels || !o.vox4) return QB200_OK;
+  return o.kind == QB200_MEM_DEVICE ? launch_passthrough(L, ncl, to.vox, to.stride, to.cap) : launch_passthrough(L, ncl, nullptr, 0, 0);
 }
 
-// a collected describe wave's counts and status, and in host kind its entries, from the lane's staging block to the caller
-void deliver_export(Lane* L, const qb200_feature_out& o, int w0, int ncl) {
+// a collected describe wave's counts and status, and in host kind its entries, from the lane's staging block to the caller; a
+// voxelize wave's pass-through clouds (voxels) from their raw_stage regions
+int deliver_export(Lane* L, const qb200_feature_out& o, int w0, int ncl, bool voxels) {
   ExportDst st;
   export_stage(L, o, L->exp_stage, &st);
   memcpy(o.counts + w0, st.counts, (size_t)ncl * sizeof(int));
   memcpy(o.status + w0, st.status, (size_t)ncl * sizeof(int));
-  if (o.kind == QB200_MEM_DEVICE) return;
+  if (o.kind == QB200_MEM_DEVICE) return QB200_OK;
   const ExportDst to = ExportDst::caller(o, w0);
+  bool copied = false;
   for (int c = 0; c < ncl; ++c) {
+    const size_t d0 = (size_t)c * to.stride, s0 = (size_t)c * st.stride;
+    if (voxels && st.status[c] == QB200_ERR_VOXEL_OVERFLOW) {
+      const int m = st.counts[c] < to.cap ? st.counts[c] : to.cap;
+      if (to.vox && m > 0) {
+        QB_CUDA_TRY(L, cudaMemcpyAsync(to.vox + d0, L->raw_stage + L->h_raw_off[c], (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, L->stream));
+        copied = true;
+      }
+      continue;
+    }
     const int m = st.counts[c] < st.cap ? st.counts[c] : st.cap;
     if (m <= 0) continue;
-    const size_t d0 = (size_t)c * to.stride, s0 = (size_t)c * st.stride;
     if (to.vox) memcpy(to.vox + d0, st.vox + s0, (size_t)m * sizeof(float4));
     if (to.nrm) memcpy(to.nrm + d0, st.nrm + s0, (size_t)m * sizeof(float4));
     if (to.desc) memcpy(to.desc + d0 * kDescDim, st.desc + s0 * kDescDim, (size_t)m * kDescDim * sizeof(float));
   }
+  if (copied) QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
+  return QB200_OK;
 }
 
 // An output descriptor of a describe call: capacity and kinds in range, counts and status present, device arrays on the handle's
@@ -744,6 +761,11 @@ int fill_tables(Lane* L, const BatchCall& in, int w0, int np) {
   for (int s = 0; s < np; ++s) {
     const bool own = in.each() || s == 0;
     const qb200_params& p = in.params[in.each() ? w0 + s : 0];
+    if (one_cloud && in.sink == Sink::Voxels) {  // the voxel fields alone: a voxelize call reads nothing else of its entries
+      memset(&L->h_front[s], 0, sizeof(CloudFront));
+      front_voxel(&L->h_front[s], p.voxel_size, p.skip_flagged);
+      continue;
+    }
     if (one_cloud) {
       L->h_front[s] = own ? front_entry(p, in.src == Source::KeypointClouds) : L->h_front[0];
       continue;
@@ -776,7 +798,7 @@ int stage_inputs(qb200_handle* h, Lane* L, const BatchCall& in, int ncl) {
   return QB200_OK;
 }
 
-// Raw pairs and raw scans: the H2D of host scans, K1 (voxel) and K2..K5 (normals, FPFH)
+// Raw pairs and raw scans: the H2D of host scans, K1 (voxel) and K2..K5 (normals, FPFH); a voxelize wave stops after K1
 int front_raw(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np, int ncl) {
   int rc;
   cudaEventRecord(L->ev[0], L->stream);
@@ -797,7 +819,7 @@ int front_raw(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np, int
   cudaEventRecord(L->ev[1], L->stream);
   if ((rc = launch_voxel(L, ncl))) return rc;
   cudaEventRecord(L->ev[2], L->stream);
-  if ((rc = launch_fpfh(L, ncl))) return rc;
+  if (in.sink != Sink::Voxels && (rc = launch_fpfh(L, ncl))) return rc;
   cudaEventRecord(L->ev[3], L->stream);
   return QB200_OK;
 }
@@ -1019,7 +1041,7 @@ int send_records(Lane* L, const BatchCall& in, int w0, int np) {
 
 // Enqueue one wave (inputs [w0, w0 + np) of the call: np <= S pairs or sets, or np <= 2S scans) on lane L: its tables, the front of
 // its source, then the tail of its sink: Solve K6..K7 (pairs) and K8..K11, Match K6..K7 and match_records_kernel, both then the lists
-// and the D2H of the records; CacheSlots the copy into the cache slots; Export the export to the caller's arrays.  No sync:
+// and the D2H of the records; CacheSlots the copy into the cache slots; Export and Voxels the export to the caller's arrays.  No sync:
 // wave_collect hands the outputs on.  The lane's previous wave must have been collected.
 int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   const int ncl = np * clouds_per_input(in.src);
@@ -1058,7 +1080,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       if ((rc = cache_copy(h, L, 1, ncl))) return rc;
       QB_CUDA_TRY(L, cudaEventRecord(L->ev_cache_out, L->stream));
       break;
-    case Sink::Export: rc = submit_export(L, *in.out, w0, ncl); break;
+    case Sink::Export: case Sink::Voxels: rc = submit_export(L, *in.out, w0, ncl, in.sink == Sink::Voxels); break;
     case Sink::Graph:  // no clique or pose stage: the graph slot holds K8 and the outputs
       if ((rc = submit_graph(L, *in.graph_out, w0, np))) return rc;
       for (int i = 5; i <= 7; ++i) cudaEventRecord(L->ev[i], L->stream);
@@ -1090,7 +1112,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   L->pend_dst = in.results;
   L->pend_host_lists = in.lists && in.lists->kind == QB200_MEM_HOST;
   if (in.lists) L->pend_lists = *in.lists;
-  if (in.sink == Sink::Export) L->pend_out = *in.out;
+  if (in.sink == Sink::Export || in.sink == Sink::Voxels) L->pend_out = *in.out;
   if (in.sink == Sink::Graph) L->pend_graph = *in.graph_out;
   return QB200_OK;
 }
@@ -1115,7 +1137,7 @@ int wave_collect(qb200_handle* h, Lane* L) {
       if (L->pend_graph.kind == QB200_MEM_HOST) rc = deliver_graph(L, L->pend_graph, L->pend_w0, np);
       break;
     case Sink::CacheSlots: break;
-    case Sink::Export: deliver_export(L, L->pend_out, L->pend_w0, np); break;
+    case Sink::Export: case Sink::Voxels: rc = deliver_export(L, L->pend_out, L->pend_w0, np, L->pend_sink == Sink::Voxels); break;
   }
   if (h->timeline && (L->pend_stages & 1u)) {  // stage boundaries of a raw-scan or feature wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
     fprintf(stderr, "[qb200 timeline] wave w0=%d np=%d:", L->pend_w0, np);
@@ -1227,7 +1249,14 @@ int check_call(qb200_handle* h, const BatchCall& c) {
   if (c.kind != QB200_MEM_HOST && c.kind != QB200_MEM_DEVICE) return reject("unknown memory kind of the inputs");
   const qb200_params* p = c.caller;
   char why[192];
-  if (c.src == Source::KeypointClouds) {  // only the lattice fields are read
+  if (c.sink == Sink::Voxels) {  // only voxel_size and skip_flagged are read; the leaf is checked as qb200_voxelize checks it
+    for (int i = 0; i < c.n; ++i) {
+      if (!p || !(p[i].voxel_size > 0)) {
+        snprintf(why, sizeof(why), "params entry %d is null or its voxel_size is not > 0", i);
+        return reject(why);
+      }
+    }
+  } else if (c.src == Source::KeypointClouds) {  // only the lattice fields are read
     for (int i = 0; i < c.n; ++i) {
       if (!p || !lattice_ok(p[i])) {
         snprintf(why, sizeof(why), "params entry %d is null or its radii or lattice cell are out of range", i);
@@ -1264,8 +1293,10 @@ int check_call(qb200_handle* h, const BatchCall& c) {
   }
   const bool sets = c.src == Source::CorrSets || c.src == Source::InlierSets;
   if (int rc = check_lists(h, c.lists, sets, c.sink == Sink::Match, c.src == Source::Graphs)) return rc;
-  if (c.sink == Sink::Export)
+  if (c.sink == Sink::Export || c.sink == Sink::Voxels)
     if (int rc = check_out(h, c.out, c.src == Source::KeypointClouds)) return rc;
+  if (c.sink == Sink::Voxels && (c.out->normals4 || c.out->desc33))
+    return reject("normals4 and desc33 must be null: a voxelize call returns voxel centroids alone");
   if (c.sink == Sink::Graph)
     if (int rc = check_graph_out(h, c.graph_out)) return rc;
   const int R = h->cfg.max_raw_points;
@@ -1376,6 +1407,8 @@ int check_call(qb200_handle* h, const BatchCall& c) {
         }
         if (np < 0 || np > R) bad = "its point count is outside 0 .. max_raw_points";
         else if (np > 0 && !c.scans[i]) bad = "it is null";
+        else if (c.sink == Sink::Voxels && np > 0 && c.kind == QB200_MEM_DEVICE && !device_array_of(h, c.scans[i], 16))
+          bad = "it is misaligned (16 bytes) or not memory of the handle's device";
         if (bad) {
           snprintf(why, sizeof(why), "scan %d: %s", i, bad);
           return reject(why);
@@ -1525,7 +1558,7 @@ BatchCall corr_sets(const qb200_corr_set* sets, int32_t n, const qb200_params* p
   return c;
 }
 
-// slot_ids for the CacheSlots sink, out for Export; every scan runs its own front end, so the entries may differ
+// slot_ids for the CacheSlots sink, out for Export and Voxels; every scan runs its own front end, so the entries may differ
 BatchCall raw_scans(Sink k, Entries e, const float* const* scans4, const int32_t* n_points, int32_t n, const qb200_params* p, qb200_mem_kind kind,
                     const int32_t* slot_ids, const qb200_feature_out* out) {
   BatchCall c{Source::RawScans, k, n, kind, p, e};
@@ -1813,6 +1846,17 @@ int qb200_describe_batch_each(qb200_handle* h, const float* const* scans4, const
 int qb200_describe_batch_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
                                       const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out) {
   return enqueue_call(h, raw_scans(Sink::Export, Entries::Mixed, scans4, n_points, n_scans, params, kind, nullptr, out));
+}
+
+// ---- raw scans -> voxel centroids in caller memory ------------------------------------------------------------------------------
+int qb200_voxelize_batch_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans, const qb200_params* params,
+                              qb200_mem_kind kind, const qb200_feature_out* out) {
+  return run_call(h, raw_scans(Sink::Voxels, Entries::Mixed, scans4, n_points, n_scans, params, kind, nullptr, out));
+}
+
+int qb200_voxelize_batch_enqueue_each(qb200_handle* h, const float* const* scans4, const int32_t* n_points, int32_t n_scans,
+                                      const qb200_params* params, qb200_mem_kind kind, const qb200_feature_out* out) {
+  return enqueue_call(h, raw_scans(Sink::Voxels, Entries::Mixed, scans4, n_points, n_scans, params, kind, nullptr, out));
 }
 
 // ---- caller keypoint clouds -> normals and FPFH-33 in caller memory -------------------------------------------------------------

@@ -693,12 +693,14 @@ __global__ void __launch_bounds__(kExportThreads) feature_export_kernel(ExportSr
   __shared__ float tile[kExportTile * kDescDim];
   const int cloud = blockIdx.y, q0 = blockIdx.x * kExportTile, tid = threadIdx.x;
   const int st = s.status ? s.status[cloud] : QB200_OK;
-  const int n = st == QB200_OK ? s.n[cloud] : 0;  // a refused cloud reports 0 and gets nothing
+  // a refused cloud reports 0 and gets nothing; a voxelize wave (n_kept) refuses none: see ExportSrc
+  const bool pass = s.n_kept && st == QB200_ERR_VOXEL_OVERFLOW;
+  const int n = st == QB200_OK || (s.n_kept && st == QB200_CAPACITY_EXCEEDED) ? s.n[cloud] : pass ? s.n_kept[cloud] : 0;
   if (blockIdx.x == 0 && tid == 0) {
     if (d.counts) d.counts[cloud] = n;
     if (d.status) d.status[cloud] = st;
   }
-  const int m_all = min(n, d.cap);
+  const int m_all = pass ? 0 : min(n, d.cap);
   if (q0 >= m_all) return;
   const int m = min(kExportTile, m_all - q0);
   const size_t from = (size_t)cloud * V + q0, to = (size_t)cloud * d.stride + q0;
@@ -715,6 +717,42 @@ __global__ void __launch_bounds__(kExportThreads) feature_export_kernel(ExportSr
   __syncthreads();
   float* __restrict__ out = d.desc + to * kDescDim;
   for (int i = tid; i < m * kDescDim; i += kExportThreads) out[i] = tile[i];
+}
+
+constexpr int kPassThreads = 1024;
+
+// K1d (voxelize waves): [EXT] pcl::VoxelGrid returns the input unfiltered when its int voxel index would overflow ("leaf size is too
+// small"); qb200_voxelize hands back the kept points of such a cloud, in input order.  One CTA per cloud; a cloud that run_heads_kernel
+// did not refuse with QB200_ERR_VOXEL_OVERFLOW exits at once.  The CTA walks the cloud one point per thread and round with the keep
+// test voxel_bbox_kernel counts into n_valid, and places the kept points by a block scan carried across rounds, as run_heads_kernel
+// does.  In place (host scans into their own raw_stage region) every point of a round is read before the scan's barriers and
+// written at or before its own position, so no point is overwritten before it is read: the pointers are not __restrict__ and the
+// loads do not go through the read-only cache.
+__global__ void __launch_bounds__(kPassThreads) passthrough_kernel(const float4* const* __restrict__ cloud_ptr, const int* __restrict__ cloud_n,
+                                                                   const CloudFront* __restrict__ front, const int* __restrict__ cloud_status,
+                                                                   const int* __restrict__ raw_off, float4* stage, float4* dst,
+                                                                   long long stride, int cap) {
+  __shared__ int sm[33];
+  const int cloud = blockIdx.x;
+  if (cloud_status[cloud] != QB200_ERR_VOXEL_OVERFLOW) return;
+  const int n = cloud_n[cloud], skip_flagged = front[cloud].skip_flagged;
+  const float4* src = cloud_ptr[cloud];
+  float4* out = dst ? dst + cloud * stride : stage + raw_off[cloud];
+  const int lim = dst ? cap : n;
+  int carry = 0;  // the same in every thread: the loop condition is uniform
+  for (int base = 0; base < n && carry < lim; base += blockDim.x) {
+    const int i = base + threadIdx.x;
+    float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
+    bool keep = false;
+    if (i < n) {
+      p = src[i];
+      keep = raw_point_kept(p, skip_flagged);
+    }
+    int tot;
+    const int pos = carry + block_excl_scan(keep ? 1 : 0, sm, &tot);
+    if (keep && pos < lim) out[pos] = p;
+    carry += tot;
+  }
 }
 
 constexpr int kImportTile = 128, kImportThreads = 256;
@@ -830,8 +868,17 @@ int launch_feature_export(Lane* h, int n_clouds, const ExportSrc& src, const Exp
   return QB200_OK;
 }
 
+int launch_passthrough(Lane* h, int n_clouds, float4* dst, long long stride, int cap) {
+  if (n_clouds <= 0) return QB200_OK;
+  passthrough_kernel<<<n_clouds, kPassThreads, 0, h->stream>>>(h->d_cloud_ptr, h->d_cloud_n, h->d_front, h->ctr.cloud_status, h->d_raw_off,
+                                                               h->raw_stage, dst, stride, cap);
+  h->launches++;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
+}
+
 int export_desc_rows(Lane* h, const float* desc, const int* n, int m) {
-  ExportSrc s{nullptr, nullptr, desc, n, nullptr};
+  ExportSrc s{nullptr, nullptr, desc, n, nullptr, nullptr};
   ExportDst d{nullptr, nullptr, h->aos_scratch, m, m, nullptr, nullptr};
   return launch_feature_export(h, 1, s, d, m);
 }

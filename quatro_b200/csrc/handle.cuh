@@ -64,13 +64,15 @@ struct FeatureSrc {
 
 // What feature_export_kernel reads (frontend.cu): cloud c's voxel points, normals and dimension-major descriptors at c * V points
 // (c * kDescK * V floats) past these pointers, and its count; status == nullptr: every cloud is written, else only the clouds whose
-// front-end status is QB200_OK
+// front-end status is QB200_OK.  n_kept != nullptr (a voxelize wave): QB200_CAPACITY_EXCEEDED clouds are written too, and a
+// QB200_ERR_VOXEL_OVERFLOW cloud reports n_kept[c], its kept raw points, and gets no entries here (passthrough_kernel writes them)
 struct ExportSrc {
   const float4* vox;
   const float4* nrm;
   const float* desc;
   const int* n;
   const int* status;
+  const int* n_kept;
 };
 
 // Where feature_export_kernel writes cloud c: c * stride keypoints past each array (nullptr = not asked for), at most cap of them; and,
@@ -127,9 +129,11 @@ enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, Key
 //   CorrSets                             x  Solve, Graph   qb200_solve_batch*, qb200_build_graph_batch*
 //   RawScans                             x  CacheSlots     qb200_cache_scans*
 //   RawScans, KeypointClouds             x  Export         qb200_describe_batch*, qb200_describe_points*
+//   RawScans                             x  Voxels         qb200_voxelize_batch*
 //   Graphs                               x  Clique         qb200_max_clique_batch*
 //   InlierSets                           x  Pose           qb200_solve_pose_batch*
-enum class Sink { Solve, Match, CacheSlots, Export, Clique, Graph, Pose };
+// Voxels is Export without K2..K5: the voxel centroids alone, with qb200_voxelize's capacity and pass-through outputs
+enum class Sink { Solve, Match, CacheSlots, Export, Voxels, Clique, Graph, Pose };
 
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
@@ -163,8 +167,8 @@ struct Lane {
   qb200_result* pend_dst;     // ... (Solve, Match, Clique, Graph, Pose) the caller's record array of its batch, nullptr for the other sinks
   bool pend_host_lists;       // ... (Solve, Match, Clique, Pose) its batch has host-kind lists, which wave_collect hands on from lst_stage
   qb200_pair_lists pend_lists; // ... and then a copy of their descriptor
-  qb200_feature_out pend_out; // ... (Export) a copy of its batch's output descriptor, whose counts and status (and, in host kind,
-                              // entries) wave_collect hands on from exp_stage
+  qb200_feature_out pend_out; // ... (Export, Voxels) a copy of its batch's output descriptor, whose counts and status (and, in host
+                              // kind, entries) wave_collect hands on from exp_stage (and a Voxels wave's pass-through from raw_stage)
   qb200_graph_out pend_graph; // ... (Graph) a copy of its batch's output descriptor, whose host-kind arrays wave_collect writes
   // ... and the cache slots it reads (cached pairs) or writes (CacheSlots), ascending and unique; empty: it does not touch the
   // cache.  A wave reads the cache only in its copy-in and writes it only in its copy-out, so other lanes order their conflicting
@@ -372,6 +376,11 @@ int tc_footprint(Lane* h, int* out5);
 // Clouds [0, n_clouds) of src to dst in one launch: keypoints, normals and 33-float descriptor rows (pcl::FPFHSignature33) of each
 // cloud's first min(n, dst.cap) points.  max_n: a host bound of the entries any cloud writes (the launch's tile count).
 int launch_feature_export(Lane* h, int n_clouds, const ExportSrc& src, const ExportDst& dst, int max_n);
+// Voxelize waves, after launch_voxel: PCL's pass-through of every cloud [0, n_clouds) refused with QB200_ERR_VOXEL_OVERFLOW, its kept
+// raw points (raw_point_kept) in input order.  dst != nullptr: the first `cap` of them at dst + c * stride (the caller's device array);
+// dst == nullptr: all of them at raw_stage + raw_off[c], the cloud's own region (in place for host scans), from where wave_collect
+// copies them to the caller's host array.
+int launch_passthrough(Lane* h, int n_clouds, float4* dst, long long stride, int cap);
 // the first min(*n, m) descriptor rows of one cloud (its dimension-major block desc, its count at the device address n) into aos_scratch
 int export_desc_rows(Lane* h, const float* desc, const int* n, int m);
 // Feature waves (api.cu: stage_features, frontend.cu): h_feat[0, n) holds every cloud's caller pointers and count.  stage_features
