@@ -1,9 +1,13 @@
-"""Helpers several test modules share: point and descriptor builders, bit-exact float comparison, result-record comparison and the
-C++ build against libquatro_b200.  A plain module (test files import it as `from support import ...`); fixtures live in conftest.py."""
+"""Helpers several test modules share: point and descriptor builders, bit-exact float comparison, result-record comparison, the
+params, handles, device copies and 0xA5-filled outputs of the batch tests, and the C++ build against libquatro_b200.  A plain module
+(test files import it as `from support import ...`); fixtures live in conftest.py."""
 import subprocess
 from pathlib import Path
 
 import numpy as np
+import pytest
+
+from quatro_b200.capi import MEM_HOST, Handle, default_params
 
 ROOT = Path(__file__).resolve().parent.parent
 
@@ -60,9 +64,69 @@ def same_lists(got: dict, want: dict):
         assert g.shape == w.shape and g.tobytes() == w.tobytes(), (name, g.shape, w.shape)
 
 
+def _host(a):
+    """a numpy array as it is, a CUDA tensor copied to one."""
+    return a if isinstance(a, np.ndarray) else a.cpu().numpy()
+
+
 def host_lists(lists):
     """Per-pair lists with every CUDA tensor copied to a numpy array."""
-    return [{k: (v if isinstance(v, np.ndarray) else v.cpu().numpy()) for k, v in d.items()} for d in lists]
+    return [{k: _host(v) for k, v in d.items()} for d in lists]
+
+
+def make_params(**kw):
+    """capi.default_params() with the fields in kw set.  rot_noise_bound is 2 * noise_bound unless kw sets it: explicit, as the
+    oracle has no latch; a test of the latch asks for it with rot_noise_bound=0."""
+    p = default_params()
+    p.rot_noise_bound = 2 * kw.get("noise_bound", p.noise_bound)
+    for k, v in kw.items():
+        setattr(p, k, v)
+    return p
+
+
+def make_handle(lanes, **cfg):
+    """A Handle of config `cfg` with QB200_LANES=lanes, or unset (the default lane count) for lanes=None; the variable is read when
+    the handle is created and restored after."""
+    with pytest.MonkeyPatch.context() as mp:
+        if lanes is None:
+            mp.delenv("QB200_LANES", raising=False)
+        else:
+            mp.setenv("QB200_LANES", str(lanes))
+        return Handle(**cfg)
+
+
+def device_copy(a):
+    """A CUDA copy of the host array a, in its own dtype, the copy finished."""
+    import torch
+    t = torch.from_numpy(np.ascontiguousarray(a)).cuda()
+    torch.cuda.synchronize()
+    return t
+
+
+def device_copies(arrays):
+    """CUDA float32 copies of host point or descriptor arrays: their (pointer, count) tuples, and the tensors, which must outlive
+    the pointers."""
+    keep = [device_copy(np.asarray(a, np.float32)) for a in arrays]
+    return [(t.data_ptr(), len(t)) for t in keep], keep
+
+
+def sentinel(shape, dtype=np.float32, kind=MEM_HOST):
+    """An output array of `shape` filled with 0xA5 bytes, which entries a call does not write keep: numpy for MEM_HOST, a CUDA
+    tensor for MEM_DEVICE."""
+    a = np.zeros(shape, dtype)
+    a.view(np.uint8)[...] = 0xA5
+    return a if kind == MEM_HOST else device_copy(a)
+
+
+def sentinel_lists(lb):
+    """ListBuffers lb with every byte of every array, host or device, set to 0xA5; returns lb."""
+    for a in lb.arrays.values():
+        if isinstance(a, np.ndarray):
+            a.view(np.uint8)[...] = 0xA5
+        else:
+            import torch
+            a.view(torch.uint8).fill_(0xA5)
+    return lb
 
 
 def build_against_lib(tmp_path, source):

@@ -11,6 +11,7 @@ import pytest
 
 from quatro_b200 import capi, synth
 from quatro_b200.capi import MEM_DEVICE, MEM_HOST, PMC_EXACT, INLIER_NONE, RESULT_DTYPE, Handle, default_params
+from support import sentinel
 
 CSRC = Path(__file__).resolve().parent.parent / "quatro_b200" / "csrc"
 DELETED = ("run_waves", "solve_batch_impl", "enqueue_impl", "register_batch_impl", "register_cached_impl", "device_array_ok",
@@ -72,12 +73,6 @@ def test_empty_call_latches_nothing(family):
         assert h.solve_batch([s], narrow).tobytes() == want.tobytes()
 
 
-def _sentinel(n):
-    out = np.zeros(max(n, 1), RESULT_DTYPE)
-    out.view(np.uint8)[...] = 0xA5
-    return out
-
-
 @pytest.mark.gpu
 def test_unknown_memory_kind_is_rejected_before_any_work():
     import torch
@@ -98,7 +93,7 @@ def test_unknown_memory_kind_is_rejected_before_any_work():
         }
         for name, call in calls.items():
             for n in (0, 1):
-                out = _sentinel(n)
+                out = sentinel(max(n, 1), RESULT_DTYPE)
                 before = h.launch_count()
                 st = call(n, out)
                 h.register_batch_flush()

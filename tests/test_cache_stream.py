@@ -11,8 +11,8 @@ import numpy as np
 import pytest
 
 from quatro_b200 import capi, synth
-from quatro_b200.capi import MEM_DEVICE, MEM_HOST, RESULT_DTYPE, Handle, ListBuffers, default_params
-from support import ROOT, host_lists
+from quatro_b200.capi import MEM_DEVICE, MEM_HOST, RESULT_DTYPE, ListBuffers, default_params
+from support import ROOT, device_copies, host_lists, make_handle, make_params
 
 NEW, SIBLING = "qb200_cache_scans_enqueue_each", "qb200_cache_scans_each"
 
@@ -39,25 +39,11 @@ def test_cache_enqueue_refuses_a_null_handle():
 
 
 # ---- configurations ----------------------------------------------------------------------------------------------------------------
-def make_params(**kw):
-    p = default_params()
-    for k, v in kw.items():
-        setattr(p, k, v)
-    if "rot_noise_bound" not in kw:
-        p.rot_noise_bound = 2 * p.noise_bound
-    return p
-
-
 SLOTS, LANES, RAW_CAP = 2, 4, 32768          # a write wave holds 2 * SLOTS = 4 scans
 N = 2 * SLOTS * LANES + 3                    # pairs of a reader batch: more waves than lanes
 BASE = make_params(seed=11)
+CFG = dict(max_batch_slots=SLOTS, max_raw_points=RAW_CAP)
 FRONTS = [BASE, make_params(voxel_size=0.4, grid_cell=0.4, seed=14), make_params(voxel_size=0.25, grid_cell=0.4, seed=13, noise_bound=0.35)]
-
-
-def _handle(lanes):
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))   # read when the handle is created
-        return Handle(max_batch_slots=SLOTS, max_raw_points=RAW_CAP)
 
 
 def _read(h, slot):
@@ -73,13 +59,6 @@ def _enqueue(h, scans, slots, params, kind=MEM_HOST):
     return keep
 
 
-def _device_scans(scans):
-    import torch
-    keep = [torch.from_numpy(np.ascontiguousarray(s, np.float32)).cuda() for s in scans]
-    torch.cuda.synchronize()
-    return [(t.data_ptr(), len(t)) for t in keep], keep
-
-
 # ---- GPU fixtures ------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def scans():
@@ -91,21 +70,21 @@ def scans():
 
 @pytest.fixture(scope="module")
 def h1():
-    h = _handle(1)
+    h = make_handle(1, **CFG)
     yield h
     h.close()
 
 
 @pytest.fixture(scope="module")
 def h4():
-    h = _handle(LANES)
+    h = make_handle(LANES, **CFG)
     yield h
     h.close()
 
 
 @pytest.fixture(scope="module")
 def ref():
-    h = _handle(LANES)
+    h = make_handle(LANES, **CFG)
     yield h
     h.close()
 
@@ -121,7 +100,7 @@ def test_queued_writes_fill_every_slot_like_the_blocking_call_alone(h1, h4, ref,
         ref.cache_scans_each([scans[i]], [i], [entries[i]])
         want.append(_read(ref, i))
     assert len(set(want)) == n and len({len(w) for w in want}) > 1
-    dev, keep_dev = _device_scans(scans[:n])
+    dev, keep_dev = device_copies(scans[:n])
     for h in (h1, h4):
         for kind, ss in ((MEM_HOST, scans[:n]), (MEM_DEVICE, dev)):
             h.cache_reserve(n)
@@ -147,7 +126,7 @@ def test_every_cache_path_matches_the_golden_slots(h1, h4):
         for k, v in g["fronts"][i % 3].items():
             setattr(p, k, v)
         entries.append(p)
-    dev, keep_dev = _device_scans(ss)
+    dev, keep_dev = device_copies(ss)
     for h in (h1, h4):
         for kind, scan_in in ((MEM_HOST, ss), (MEM_DEVICE, dev)):
             for queued in (False, True):
@@ -196,7 +175,7 @@ def test_one_stream_orders_writes_and_readers_of_a_slot(h4, ref, scans):
     for h in (h4, ref):
         h.cache_reserve(2 * N)
         h.cache_scans(scans[:2 * N], list(range(2 * N)), BASE)
-    dev = [_device_scans(w[0]) for w in writes]
+    dev = [device_copies(w[0]) for w in writes]
 
     # blocking, in order
     want = {"raw": ref.register_batch_mixed(raw_pairs, [BASE] * N)[0], "A": ref.register_cached(read_0, BASE)}

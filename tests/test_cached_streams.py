@@ -10,8 +10,8 @@ import pytest
 
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (COTE_WEIGHTED_MEAN, INLIER_NONE, KCORE_HEU, LIST_LAYOUT, MEM_DEVICE, MEM_HOST, RESULT_DTYPE, SET_LISTS,
-                              Handle, ListBuffers, default_params)
-from support import ROOT, host_lists, same_lists
+                              ListBuffers)
+from support import ROOT, device_copies, host_lists, make_handle, make_params, same_lists, sentinel, sentinel_lists
 
 NEW = {"qb200_register_cached_enqueue_mixed": "qb200_register_cached_mixed", "qb200_solve_batch_enqueue_each": "qb200_solve_batch_each"}
 
@@ -41,15 +41,6 @@ def test_enqueue_calls_refuse_a_null_handle():
 
 
 # ---- configurations ----------------------------------------------------------------------------------------------------------------
-def make_params(**kw):
-    p = default_params()
-    for k, v in kw.items():
-        setattr(p, k, v)
-    if "rot_noise_bound" not in kw:
-        p.rot_noise_bound = 2 * p.noise_bound   # explicit unless a test asks for the latch
-    return p
-
-
 SLOTS, LANES = 4, 4
 N = 2 * SLOTS * LANES + 3   # more waves than lanes: every lane runs more than one wave of a batch
 BASE = make_params(seed=11)
@@ -67,27 +58,8 @@ def cycled(n, sets):
     return [sets[i % len(sets)] for i in range(n)]
 
 
-def _sentinel_out(n):
-    out = np.zeros(max(n, 1), RESULT_DTYPE)
-    out.view(np.uint8)[...] = 0xA5
-    return out
-
-
-def _sentinel_lists(n, cap=64, names=tuple(LIST_LAYOUT)):
-    lb = ListBuffers(n, cap, MEM_HOST, names)
-    for a in lb.arrays.values():
-        a.view(np.uint8)[...] = 0xA5
-    return lb
-
-
 def _untouched(out, lb):
     return (out.view(np.uint8) == 0xA5).all() and all((a.view(np.uint8) == 0xA5).all() for a in lb.arrays.values())
-
-
-def _handle(lanes):
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))   # read when the handle is created
-        return Handle(max_batch_slots=SLOTS)
 
 
 # ---- GPU fixtures ------------------------------------------------------------------------------------------------------------------
@@ -118,7 +90,7 @@ def _cache(h, street):
 
 @pytest.fixture(scope="module")
 def h4(street):
-    h = _handle(LANES)
+    h = make_handle(LANES, max_batch_slots=SLOTS)
     _cache(h, street)
     yield h
     h.close()
@@ -126,18 +98,15 @@ def h4(street):
 
 @pytest.fixture(scope="module")
 def h1(street):
-    h = _handle(1)
+    h = make_handle(1, max_batch_slots=SLOTS)
     _cache(h, street)
     yield h
     h.close()
 
 
 def _device_sets(sets):
-    import torch
-    keep = [(torch.from_numpy(np.ascontiguousarray(a, np.float32)).cuda(), torch.from_numpy(np.ascontiguousarray(b, np.float32)).cuda())
-            for a, b in sets]
-    torch.cuda.synchronize()
-    return [(a.data_ptr(), b.data_ptr(), len(s[0])) for (a, b), s in zip(keep, sets)], keep
+    ptrs, keep = device_copies([x for s in sets for x in s])
+    return [(a, b, n) for (a, n), (b, _) in zip(ptrs[0::2], ptrs[1::2])], keep
 
 
 def _flat(recs, lb):
@@ -210,7 +179,7 @@ def test_one_stream_of_cached_raw_and_set_batches(street, sets):
             q.rot_noise_bound = q.rot_noise_bound or latch
         return out
 
-    with _handle(LANES) as h, _handle(LANES) as ref:
+    with make_handle(LANES, max_batch_slots=SLOTS) as h, make_handle(LANES, max_batch_slots=SLOTS) as ref:
         for hh in (h, ref):
             _cache(hh, street)
         dev, keep_dev = _device_sets(sets)
@@ -275,7 +244,7 @@ def test_a_rejected_enqueue_writes_nothing_and_keeps_the_queue(h4, sets):
 
     def cached(slot_pairs, ps, n_=None, cap=64):
         sp = capi._slot_array(slot_pairs)
-        out, lb = _sentinel_out(len(sp)), _sentinel_lists(len(sp))
+        out, lb = sentinel(max(len(sp), 1), RESULT_DTYPE), sentinel_lists(ListBuffers(len(sp), 64))
         d = lb.descriptor()
         d.cap_per_pair = cap
         st = lib.qb200_register_cached_enqueue_mixed(h4.h, capi._ptr(sp), len(sp) if n_ is None else n_, h4.params_array(ps),
@@ -283,7 +252,7 @@ def test_a_rejected_enqueue_writes_nothing_and_keeps_the_queue(h4, sets):
         return st, out, lb
 
     def set_call(n_=None, cap=64, ps=None):
-        out, lb = _sentinel_out(3), _sentinel_lists(3, names=SET_LISTS)
+        out, lb = sentinel(3, RESULT_DTYPE), sentinel_lists(ListBuffers(3, 64, MEM_HOST, SET_LISTS))
         d = lb.descriptor()
         d.cap_per_pair = cap
         st = lib.qb200_solve_batch_enqueue_each(h4.h, set_arr, 3 if n_ is None else n_, h4.params_array(ps or [BASE] * 3), MEM_HOST,

@@ -9,9 +9,9 @@ import numpy as np
 import pytest
 
 from quatro_b200 import capi, synth
-from quatro_b200.capi import (GRAPH_LISTS, KCORE_HEU, MATCH_LISTS, MEM_DEVICE, MEM_HOST, PMC_EXACT, PMC_HEU, RESULT_DTYPE, Graph, Handle,
+from quatro_b200.capi import (GRAPH_LISTS, KCORE_HEU, MATCH_LISTS, MEM_DEVICE, MEM_HOST, PMC_EXACT, PMC_HEU, RESULT_DTYPE, Graph,
                               ListBuffers, default_params)
-from support import ROOT
+from support import ROOT, device_copy, make_handle
 
 NEW = ("qb200_max_clique_batch_each", "qb200_max_clique_batch_enqueue_each")
 MODES = (PMC_EXACT, PMC_HEU, KCORE_HEU)
@@ -135,12 +135,6 @@ def assert_record(r, want, label):
     assert np.array_equal(np.asarray(r["T"]), np.eye(4).reshape(-1)), label
 
 
-def _handle(lanes, **kw):
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))
-        return Handle(**kw)
-
-
 def clique_lists(n, cap, kind=MEM_HOST):
     return ListBuffers(n, cap, kind, GRAPH_LISTS)
 
@@ -148,7 +142,7 @@ def clique_lists(n, cap, kind=MEM_HOST):
 @pytest.fixture(scope="module")
 def wide():
     """32768-vertex handle: 2 slots per wave over 2 lanes, so a batch of more than 4 graphs rotates"""
-    h = _handle(2, max_batch_slots=2, max_corr=32768)
+    h = make_handle(2, max_batch_slots=2, max_corr=32768)
     yield h
     h.close()
 
@@ -268,13 +262,6 @@ def test_tim_graphs_give_the_cliques_of_solve_batch(handle):
 
 
 # ---- GPU 5: device kinds, padded rows -------------------------------------------------------------------------------------------------
-def _device(a):
-    import torch
-    t = torch.from_numpy(np.ascontiguousarray(a)).cuda()
-    torch.cuda.synchronize()
-    return t
-
-
 def padded(adj, extra, rng):
     """adj with `extra` more words per row and every bit at columns >= L set"""
     L, w = adj.shape
@@ -299,7 +286,7 @@ def test_device_inputs_device_lists_and_padded_rows(handle):
     assert host_pad.tobytes() == ref.tobytes()
     keep, dev_rows, dev_edges = [], [], []
     for L, e, pa in zip(sizes, edges, pads):
-        tr, te = _device(pa), _device(shuffled_edges(rng, e))
+        tr, te = device_copy(pa), device_copy(shuffled_edges(rng, e))
         keep += [tr, te]
         dev_rows.append(Graph(None, tr.data_ptr() if L else None, 0, L, pa.shape[1]))
         dev_edges.append(Graph(te.data_ptr() if len(e) else None, None, te.shape[0], L, 0))
@@ -336,10 +323,10 @@ def test_invalid_graphs_are_refused_alone(handle):
             gs = []
             for g in graphs:
                 if isinstance(g, tuple):
-                    t = _device(np.ascontiguousarray(g[1], np.int32))
+                    t = device_copy(np.ascontiguousarray(g[1], np.int32))
                     gs.append(Graph(t.data_ptr(), None, len(g[1]), g[0], 0))
                 else:
-                    t = _device(g)
+                    t = device_copy(g)
                     gs.append(Graph(None, t.data_ptr(), 0, g.shape[0], g.shape[1]))
                 keep.append(t)
         lb = clique_lists(len(gs), 512)
@@ -366,7 +353,7 @@ def test_host_edge_lists_cross_in_chunks():
     """A handle whose edge staging holds 2048 edges (2 slots, 1 raw point per cloud, max_corr 256: the larger idle buffer is adjp,
     2 x 256 x 8 words).  Waves of two: a packed list beside a streamed dense one; two streamed lists, the first with an out-of-range
     vertex in a late chunk; a packed list beside one that no longer fits beside it and crosses in a single chunk."""
-    h = _handle(2, max_batch_slots=2, max_raw_points=1, max_corr=256)
+    h = make_handle(2, max_batch_slots=2, max_raw_points=1, max_corr=256)
     try:
         rng = np.random.default_rng(21)
         distinct = [random_graph(rng, 40), dense_edges(rng, 256, 0.9), dense_edges(rng, 200, 0.5), dense_edges(rng, 256, 0.3),
@@ -386,7 +373,7 @@ def test_host_edge_lists_cross_in_chunks():
             want, clique = expected_record(h, adj, m)
             assert_record(ref[i], want, i)
             assert rl[i]["clique"].tobytes() == clique.astype(np.int32).tobytes(), i
-        keep = [_device(e) for e in lists]
+        keep = [device_copy(e) for e in lists]
         device = [Graph(t.data_ptr(), None, t.shape[0], L, 0) for t, L in zip(keep, Ls)]
         for kind, gs in ((MEM_HOST, list(zip(Ls, lists))), (MEM_DEVICE, device)):
             recs, gl = h.max_clique_batch_each(gs, params, kind, buffers=clique_lists(len(gs), 256))

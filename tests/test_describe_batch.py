@@ -10,9 +10,8 @@ import numpy as np
 import pytest
 
 from quatro_b200 import capi, synth
-from quatro_b200.capi import (FEATURE_ARRAYS, LIST_LAYOUT, MEM_DEVICE, MEM_HOST, RESULT_DTYPE, SET_LISTS, FeatureOut, Handle, ListBuffers,
-                              default_params)
-from support import P4, ROOT, host_lists
+from quatro_b200.capi import (FEATURE_ARRAYS, LIST_LAYOUT, MEM_DEVICE, MEM_HOST, RESULT_DTYPE, SET_LISTS, FeatureOut, ListBuffers)
+from support import P4, ROOT, _host, device_copies, host_lists, make_handle, make_params, sentinel
 
 NEW = ("qb200_describe_batch_each", "qb200_describe_batch_enqueue_each")
 OK, CAPACITY, OVERFLOW = 0, 3, -5
@@ -45,34 +44,13 @@ def test_library_exports_the_describe_calls():
 
 
 # ---- configurations ----------------------------------------------------------------------------------------------------------------
-def make_params(**kw):
-    p = default_params()
-    for k, v in kw.items():
-        setattr(p, k, v)
-    if "rot_noise_bound" not in kw:
-        p.rot_noise_bound = 2 * p.noise_bound   # explicit: no test here depends on the latch
-    return p
-
-
 SLOTS, RAW_CAP = 2, 65536        # a describe wave holds 2 * SLOTS = 4 scans
+CFG = dict(max_batch_slots=SLOTS, max_raw_points=RAW_CAP)
 STREET = make_params()
 DENSE = make_params(voxel_size=0.22, use_tuple_test=0)
 COARSE = make_params(voxel_size=0.4, grid_cell=0.4, skip_flagged=0, seed=14)
 WIDE = make_params(voxel_size=0.25, normal_radius=0.6, fpfh_radius=0.9, grid_cell=1.0)
 INDOOR = make_params(voxel_size=0.08, normal_radius=0.16, fpfh_radius=0.24, noise_bound=0.05, cote_noise_bound=0.05)
-
-
-def _handle(lanes, **kw):
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))   # read when the handle is created
-        return Handle(max_batch_slots=SLOTS, max_raw_points=RAW_CAP, **kw)
-
-
-def _device_scans(scans):
-    import torch
-    keep = [torch.from_numpy(np.ascontiguousarray(s, np.float32)).cuda() for s in scans]
-    torch.cuda.synchronize()
-    return [(t.data_ptr(), len(t)) for t in keep], keep
 
 
 def _bytes(per_scan):
@@ -116,21 +94,21 @@ def mixed():
 
 @pytest.fixture(scope="module")
 def h1():
-    h = _handle(1)
+    h = make_handle(1, **CFG)
     yield h
     h.close()
 
 
 @pytest.fixture(scope="module")
 def h4():
-    h = _handle(4)
+    h = make_handle(4, **CFG)
     yield h
     h.close()
 
 
 @pytest.fixture(scope="module")
 def ref(mixed):
-    with _handle(4) as h:
+    with make_handle(4, **CFG) as h:
         yield _cache_ref(h, *mixed)
 
 
@@ -144,7 +122,7 @@ def test_describe_equals_the_cache_and_the_stage_calls(h1, h4, mixed, ref, lanes
     assert min(counts_ref) > 1000 and len(set(counts_ref)) > 5
     for i in (0, 3, 8, 10):
         assert _stage_ref(h, scans[i], params[i]) == ref[i][0], i
-    dev, keep = _device_scans(scans)
+    dev, keep = device_copies(scans)
     for kind, ss in ((MEM_HOST, scans), (MEM_DEVICE, dev)):
         for dest in (MEM_HOST, MEM_DEVICE):
             per_scan, counts, status = h.describe_batch_each(ss, params, kind, dest)
@@ -186,23 +164,6 @@ def _edge_batch():
         [(f"street {5 + k}", street[5 + k % 3], (STREET, DENSE, WIDE)[k % 3], OK) for k in range(7)]
 
 
-def _sentinel_arrays(n, cap, dest, device=0):
-    """output arrays of n + 1 scans (the last one a tail nothing may touch), filled with 0xA5 bytes"""
-    out = {}
-    for k, w in FEATURE_ARRAYS.items():
-        a = np.zeros((n + 1, cap, w), np.float32)
-        a.view(np.uint8)[...] = 0xA5
-        if dest == MEM_DEVICE:
-            import torch
-            a = torch.from_numpy(a).to(f"cuda:{device}")
-        out[k] = a
-    return out
-
-
-def _host(a):
-    return a if isinstance(a, np.ndarray) else a.cpu().numpy()
-
-
 def _lists(buffers, records):
     return [{k: v.tobytes() for k, v in d.items()} for d in host_lists(buffers.trimmed(records))]
 
@@ -214,12 +175,12 @@ def test_edge_scans_write_exactly_their_entries(h4, cap):
     n = len(batch)
     assert n == 2 * SLOTS * 4 + 1                                  # one more scan than a full rotation of waves over the lanes
     scans, params = [b[1] for b in batch], [b[2] for b in batch]
-    with _handle(4) as r:
+    with make_handle(4, **CFG) as r:
         ref = _cache_ref(r, scans, params)
-    dev, keep = _device_scans(scans)
+    dev, keep = device_copies(scans)
     for kind, ss in ((MEM_HOST, scans), (MEM_DEVICE, dev)):
         for dest in (MEM_HOST, MEM_DEVICE):
-            arrays = _sentinel_arrays(n, cap, dest)
+            arrays = {k: sentinel((n + 1, cap, w), kind=dest) for k, w in FEATURE_ARRAYS.items()}
             counts, status = np.full(n, -7, np.int32), np.full(n, -7, np.int32)
             out = h4.feature_out(cap, dest, arrays, counts, status)
             ptrs, cnts, keep_h = capi._scan_arrays(ss, kind)
@@ -252,7 +213,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
     pa = h4.params_array(params)
 
     def call(dest=MEM_HOST, cap_=cap, arrays=None, counts=True, ps=None, shift=None, kind_as=None):
-        arrays = arrays if arrays is not None else _sentinel_arrays(n, max(cap_, 1), dest)
+        arrays = arrays if arrays is not None else {k: sentinel((n + 1, max(cap_, 1), w), kind=dest) for k, w in FEATURE_ARRAYS.items()}
         c, s = np.full(n, -7, np.int32), np.full(n, -7, np.int32)
         out = h4.feature_out(cap_, dest, arrays, c, s)
         if kind_as is not None:
@@ -264,7 +225,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
         st = lib.qb200_describe_batch_enqueue_each(h4.h, ptrs, cnts, n, ps if ps is not None else pa, MEM_HOST, C.byref(out))
         return st, arrays, c, s
 
-    dev = _sentinel_arrays(n, cap, MEM_DEVICE)
+    dev = {k: sentinel((n + 1, cap, w), kind=MEM_DEVICE) for k, w in FEATURE_ARRAYS.items()}
     bad_ps = [capi.Params.from_buffer_copy(p) for p in params]
     bad_ps[4].fpfh_radius = 0.2                                    # below its normal radius
     cases = {
@@ -278,7 +239,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
     }
     for name, (fn, culprit) in cases.items():
         # a batch queued before the refused call completes on the flush
-        arrays0 = _sentinel_arrays(n, cap, MEM_HOST)
+        arrays0 = {k: sentinel((n + 1, cap, w), kind=MEM_HOST) for k, w in FEATURE_ARRAYS.items()}
         c0, s0 = np.zeros(n, np.int32), np.zeros(n, np.int32)
         out0 = h4.feature_out(cap, MEM_HOST, arrays0, c0, s0)
         assert lib.qb200_describe_batch_enqueue_each(h4.h, ptrs, cnts, n, pa, MEM_HOST, C.byref(out0)) == 0
@@ -306,12 +267,12 @@ def test_one_stream_of_describe_and_every_other_batch(mixed, ref):
     slot_pairs = [(0, 1), (2, 3), (4, 5)]
     cache_scans = [c for pr in pairs[:3] for c in pr]
     cache_pp = [p for p in pp[:3] for _ in (0, 1)]
-    with _handle(4) as h:
+    with make_handle(4, **CFG) as h:
         h.cache_reserve(6)
         # the features of the first two street pairs, described beforehand
         d, _, _ = h.describe_batch_each([c for pr in pairs[:2] for c in pr], [p for p in pp[:2] for _ in (0, 1)])
         feats = [(d[0][0], d[0][2], d[1][0], d[1][2]), (d[2][0], d[2][2], d[3][0], d[3][2])]
-        dev, keep = _device_scans(scans)
+        dev, keep = device_copies(scans)
         cap = h.cfg.max_voxel_points
 
         def run(queued):

@@ -11,9 +11,9 @@ import numpy as np
 import pytest
 
 from quatro_b200 import capi, synth
-from quatro_b200.capi import (FEATURE_ARRAYS, LIST_LAYOUT, MEM_DEVICE, MEM_HOST, POINT_ARRAYS, RESULT_DTYPE, SET_LISTS, FeatureOut, Handle,
-                              ListBuffers, default_params)
-from support import P4, ROOT, host_lists, same_bits
+from quatro_b200.capi import (FEATURE_ARRAYS, LIST_LAYOUT, MEM_DEVICE, MEM_HOST, POINT_ARRAYS, RESULT_DTYPE, SET_LISTS, FeatureOut,
+                              ListBuffers)
+from support import P4, ROOT, _host, device_copies, host_lists, make_handle, make_params, same_bits, sentinel
 
 NEW = ("qb200_describe_points_each", "qb200_describe_points_enqueue_each")
 OK = 0
@@ -65,16 +65,8 @@ def test_a_null_handle_is_refused():
 
 
 # ---- configurations ----------------------------------------------------------------------------------------------------------------
-def make_params(**kw):
-    p = default_params()
-    for k, v in kw.items():
-        setattr(p, k, v)
-    if "rot_noise_bound" not in kw:
-        p.rot_noise_bound = 2 * p.noise_bound   # explicit: no test here depends on the latch
-    return p
-
-
 SLOTS, RAW_CAP, BIG_V = 2, 65536, 32768   # a wave holds 2 * SLOTS = 4 clouds; above 17920 voxel points the lattice sort is the library's
+CFG = dict(max_batch_slots=SLOTS, max_raw_points=RAW_CAP)
 STREET = make_params()                                                         # 0.5 / 0.75, cell resolved
 EQUAL = make_params(normal_radius=0.75, fpfh_radius=0.75)                     # normal_radius == fpfh_radius
 COARSE = make_params(grid_cell=0.4)                                           # cell below the radius: a reach of two cells
@@ -85,23 +77,6 @@ IGNORED = make_params(voxel_size=-1.0, noise_bound=0.0, cbar2=0.0, use_crosschec
 
 def resolved_cell(p):
     return float(p.grid_cell) if p.grid_cell > 0 else float(np.float32(p.fpfh_radius) * np.float32(1.001953125))
-
-
-def _handle(lanes, **kw):
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))   # read when the handle is created
-        return Handle(max_batch_slots=SLOTS, max_raw_points=RAW_CAP, **kw)
-
-
-def _device(clouds):
-    import torch
-    keep = [torch.from_numpy(np.ascontiguousarray(c, np.float32)).cuda() for c in clouds]
-    torch.cuda.synchronize()
-    return [(t.data_ptr(), len(t)) for t in keep], keep
-
-
-def _host(a):
-    return a if isinstance(a, np.ndarray) else a.cpu().numpy()
 
 
 def _bytes(per_cloud):
@@ -133,7 +108,7 @@ def mixed_clouds():
     rng = np.random.default_rng(11)
     street = [synth.outdoor_pair(s, rings=32, azimuths=900)[0] for s in (40, 41)]
     indoor = synth.indoor_pair(3, n_rays=60000)[0]
-    with _handle(1, max_voxel_points=BIG_V) as h:
+    with make_handle(1, max_voxel_points=BIG_V, **CFG) as h:
         sv = h.voxelize(street[0], 0.3, 1, cap=BIG_V)[0]
         dv = h.voxelize(street[1], 0.22, 1, cap=BIG_V)[0]
         iv = h.voxelize(indoor, 0.08, 1, cap=BIG_V)[0]
@@ -167,21 +142,21 @@ def mixed():
 
 @pytest.fixture(scope="module")
 def h1():
-    h = _handle(1, max_voxel_points=BIG_V)
+    h = make_handle(1, max_voxel_points=BIG_V, **CFG)
     yield h
     h.close()
 
 
 @pytest.fixture(scope="module")
 def h4():
-    h = _handle(4, max_voxel_points=BIG_V)
+    h = make_handle(4, max_voxel_points=BIG_V, **CFG)
     yield h
     h.close()
 
 
 @pytest.fixture(scope="module")
 def ref(mixed):
-    with _handle(1, max_voxel_points=BIG_V) as h:
+    with make_handle(1, max_voxel_points=BIG_V, **CFG) as h:
         return _stage_ref(h, [c for _, c, _ in mixed], [p for _, _, p in mixed])
 
 
@@ -193,7 +168,7 @@ def test_every_cloud_equals_compute_fpfh_alone(h1, h4, mixed, ref, lanes):
     labels, clouds, params = zip(*mixed)
     n = len(clouds)
     assert n > 2 * SLOTS * 2 and len(clouds[-1]) == BIG_V == h.cfg.max_voxel_points
-    dev, keep = _device(clouds)
+    dev, keep = device_copies(clouds)
     for kind, cs in ((MEM_HOST, clouds), (MEM_DEVICE, dev)):
         for dest in (MEM_HOST, MEM_DEVICE):
             per_cloud, counts, status = h.describe_points_each(cs, params, kind, dest)
@@ -248,7 +223,7 @@ def test_described_keypoints_register_like_per_cloud_features(h1, h4):
         if i % 2:
             sv, tv = (v[np.sort(rng.permutation(len(v))[:int(0.7 * len(v))])] for v in (sv, tv))
         kps += [sv, tv]
-    dev, keep = _device(kps)
+    dev, keep = device_copies(kps)
     per_cloud, _, status = h4.describe_points_each(dev, [p for p in pp for _ in (0, 1)], MEM_DEVICE, MEM_DEVICE)
     assert (status == OK).all()
     feats_dev = [(dev[2 * i][0], per_cloud[2 * i][1].data_ptr(), dev[2 * i][1], dev[2 * i + 1][0], per_cloud[2 * i + 1][1].data_ptr(),
@@ -281,18 +256,6 @@ def test_a_cloud_alone_equals_the_cloud_in_a_batch(h4, mixed):
 
 
 # ---- GPU 6: refusals -------------------------------------------------------------------------------------------------------------------
-def _sentinel(n, cap, dest, names=POINT_ARRAYS):
-    out = {}
-    for k in names:
-        a = np.zeros((n + 1, cap, FEATURE_ARRAYS[k]), np.float32)
-        a.view(np.uint8)[...] = 0xA5
-        if dest == MEM_DEVICE:
-            import torch
-            a = torch.from_numpy(a).cuda()
-        out[k] = a
-    return out
-
-
 @pytest.mark.gpu
 def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
     lib = h4.lib
@@ -300,7 +263,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
     clouds, params = [mixed[i][1] for i in sel], [mixed[i][2] for i in sel]
     n, cap = len(clouds), BIG_V
     ptrs, cnts, keep = capi._scan_arrays(clouds, MEM_HOST)
-    dev, keep_d = _device(clouds)
+    dev, keep_d = device_copies(clouds)
     dptrs, dcnts, _ = capi._scan_arrays(dev, MEM_DEVICE)
     pa = h4.params_array(params)
     # a feature batch queued before every refused call: its records must come out as a blocking call gives them
@@ -309,7 +272,8 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
     want_rec, _ = h4.register_features_each(feats, fp)
 
     def call(dest=MEM_HOST, cap_=cap, arrays=None, counts=True, ps=None, shift=None, kind_as=None, kind=MEM_HOST, edit=None, vox=False):
-        arrays = arrays if arrays is not None else _sentinel(n, max(cap_, 1), dest, tuple(FEATURE_ARRAYS) if vox else POINT_ARRAYS)
+        names = FEATURE_ARRAYS if vox else POINT_ARRAYS
+        arrays = arrays if arrays is not None else {k: sentinel((n + 1, max(cap_, 1), FEATURE_ARRAYS[k]), kind=dest) for k in names}
         c, s = np.full(n, -7, np.int32), np.full(n, -7, np.int32)
         out = h4.feature_out(cap_, dest, arrays, c, s)
         if kind_as is not None:
@@ -339,7 +303,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
                 c2[i] = count
         return f
 
-    ddev = _sentinel(n, cap, MEM_DEVICE)
+    ddev = {k: sentinel((n + 1, cap, FEATURE_ARRAYS[k]), kind=MEM_DEVICE) for k in POINT_ARRAYS}
     cases = {
         "negative count": (lambda: call(edit=set_(3, count=-1)), "cloud 3"),
         "count above max_voxel_points": (lambda: call(edit=set_(2, count=BIG_V + 1)), "cloud 2"),
@@ -358,7 +322,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
         "cap_per_scan 0": (lambda: call(cap_=0), "cap_per_scan"),
     }
     for name, (fn, culprit) in cases.items():
-        arrays0 = _sentinel(n, cap, MEM_HOST)
+        arrays0 = {k: sentinel((n + 1, cap, FEATURE_ARRAYS[k]), kind=MEM_HOST) for k in POINT_ARRAYS}
         c0, s0 = np.zeros(n, np.int32), np.zeros(n, np.int32)
         out0 = h4.feature_out(cap, MEM_HOST, arrays0, c0, s0)
         assert lib.qb200_describe_points_enqueue_each(h4.h, ptrs, cnts, n, pa, MEM_HOST, C.byref(out0)) == 0
@@ -390,10 +354,10 @@ def test_one_stream_of_describe_points_and_every_other_batch(mixed, ref):
     slot_pairs = [(0, 1), (2, 3)]
     cache_scans = [c for pr in pairs[:2] for c in pr]
     cache_pp = [p for p in pp[:2] for _ in (0, 1)]
-    with _handle(4, max_voxel_points=BIG_V) as h:
+    with make_handle(4, max_voxel_points=BIG_V, **CFG) as h:
         h.cache_reserve(4)
         feats = [(clouds[0], np.frombuffer(ref[0][1], np.float32).reshape(-1, 33), clouds[3], np.frombuffer(ref[3][1], np.float32).reshape(-1, 33))]
-        dev, keep = _device(clouds)
+        dev, keep = device_copies(clouds)
         cap = h.cfg.max_voxel_points
 
         def run(queued):

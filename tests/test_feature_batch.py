@@ -11,8 +11,8 @@ import pytest
 
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (INLIER_NONE, KCORE_HEU, LIST_LAYOUT, MEM_DEVICE, MEM_HOST, PMC_EXACT, RESULT_DTYPE, SET_LISTS, FeaturePair,
-                              Handle, ListBuffers, default_params)
-from support import P4, ROOT, fpfh_like, host_lists
+                              ListBuffers, default_params)
+from support import P4, ROOT, device_copies, fpfh_like, host_lists, make_handle, make_params, sentinel, sentinel_lists
 
 NEW = ("qb200_register_features_each", "qb200_register_features_enqueue_each")
 
@@ -43,15 +43,6 @@ def test_library_exports_the_feature_calls():
 
 
 # ---- configurations ----------------------------------------------------------------------------------------------------------------
-def make_params(**kw):
-    p = default_params()
-    for k, v in kw.items():
-        setattr(p, k, v)
-    if "rot_noise_bound" not in kw:
-        p.rot_noise_bound = 2 * p.noise_bound   # explicit unless a test asks for the latch
-    return p
-
-
 SLOTS, N = 8, 20   # 20 pairs: three waves of up to 8 pairs
 # matcher and solver fields vary; the front end is the default one, which the slots are cached with
 PER_PAIR = [make_params(seed=11 + i % 3, use_tuple_test=int(i % 4 != 2), tuple_scale=0.9 if i % 5 == 1 else 0.95,
@@ -59,40 +50,18 @@ PER_PAIR = [make_params(seed=11 + i % 3, use_tuple_test=int(i % 4 != 2), tuple_s
                         inlier_selection_mode=(KCORE_HEU, INLIER_NONE, 1)[i % 3] if i % 7 else PMC_EXACT) for i in range(N)]
 
 
-def _handle(lanes, **kw):
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))   # read when the handle is created
-        return Handle(**kw)
-
-
 def _flat(recs, lb):
     return recs.tobytes(), [{k: v.tobytes() for k, v in d.items()} for d in host_lists(lb.trimmed(recs))]
-
-
-def _device(arrays):
-    import torch
-    keep = [torch.from_numpy(np.ascontiguousarray(a, np.float32)).cuda() for a in arrays]
-    torch.cuda.synchronize()
-    return keep
 
 
 def _device_pairs(feats):
     """(src, sdesc, tgt, tdesc) numpy tuples -> the MEM_DEVICE tuples of register_features_each, and the tensors behind them"""
     keep, out = [], []
     for s, sd, t, td in feats:
-        ts = _device([s, sd, t, td])
+        _, ts = device_copies([s, sd, t, td])
         keep.append(ts)
         out.append((ts[0].data_ptr(), ts[1].data_ptr(), len(s), ts[2].data_ptr(), ts[3].data_ptr(), len(t)))
     return out, keep
-
-
-def _sentinel(n, cap=64, names=tuple(LIST_LAYOUT)):
-    out = np.zeros(max(n, 1), RESULT_DTYPE)
-    out.view(np.uint8)[...] = 0xA5
-    lb = ListBuffers(max(n, 1), cap, MEM_HOST, names)
-    for a in lb.arrays.values():
-        a.view(np.uint8)[...] = 0xA5
-    return out, lb
 
 
 def _untouched(out, lb):
@@ -106,7 +75,7 @@ def street():
 
 
 def _cached_handle(lanes, street):
-    h = _handle(lanes, max_batch_slots=SLOTS)
+    h = make_handle(lanes, max_batch_slots=SLOTS)
     h.cache_reserve(2 * N)
     h.cache_scans([s for pr in street for s in pr], list(range(2 * N)), default_params())
     return h
@@ -258,7 +227,7 @@ def test_a_mixed_wave_equals_its_single_pair_calls():
     pairs = [_feature_pair(rng, ns, nt) for ns, nt in sizes]
     params = [make_params(use_tuple_test=i % 2, seed=100 + i, tuple_scale=(0.95, 0.9, 0.8)[i % 3],
                           inlier_selection_mode=(PMC_EXACT, INLIER_NONE, 1, KCORE_HEU)[i % 4]) for i in range(len(sizes))]
-    with _handle(4, max_batch_slots=16, max_voxel_points=V) as h:
+    with make_handle(4, max_batch_slots=16, max_voxel_points=V) as h:
         dev, keep = _device_pairs(pairs)
         single = []
         for pr, p in zip(pairs, params):
@@ -284,7 +253,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, feats):
     good_params = h4.params_array(PER_PAIR[:n])
     want, _ = h4.register_features_each(feats[:n], PER_PAIR[:n])
     s, sd, t, td = feats[1]
-    dev = _device([s, sd, t, td])
+    _, dev = device_copies([s, sd, t, td])
     raw = torch.zeros(4 * len(s) + 8, dtype=torch.float32, device="cuda")
     V = h4.cfg.max_voxel_points
     big = (np.zeros((V + 1, 4), np.float32), np.zeros((V + 1, 33), np.float32))
@@ -294,7 +263,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, feats):
         arr = (FeaturePair * len(entries))()
         for i, e in enumerate(entries):
             arr[i].src, arr[i].src_desc, arr[i].n_src, arr[i].tgt, arr[i].tgt_desc, arr[i].n_tgt = e
-        out, lb = _sentinel(len(entries))
+        out, lb = sentinel(max(len(entries), 1), RESULT_DTYPE), sentinel_lists(ListBuffers(max(len(entries), 1), 64))
         st = lib.qb200_register_features_enqueue_each(h4.h, arr, len(entries) if n_ is None else n_, h4.params_array(ps or [PER_PAIR[0]] * 3),
                                                       kind, capi._ptr(out), C.byref(lb.descriptor()))
         return st, out, lb

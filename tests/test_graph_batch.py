@@ -11,7 +11,7 @@ import pytest
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (GRAPH_LISTS, INLIER_NONE, KCORE_HEU, MATCH_LISTS, MEM_DEVICE, MEM_HOST, PMC_EXACT, PMC_HEU, RESULT_DTYPE,
                               GraphBuffers, GraphOut, Handle, ListBuffers, default_params)
-from support import P4, ROOT
+from support import P4, ROOT, device_copy, make_handle
 
 NEW = ("qb200_build_graph_batch_each", "qb200_build_graph_batch_enqueue_each")
 MODES = (PMC_EXACT, PMC_HEU, KCORE_HEU)
@@ -130,19 +130,6 @@ def check_set(i, rec, buf, adj, deg, n_edges, label):
         assert rec["flags"] == 0, label
 
 
-def _handle(lanes, **kw):
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))
-        return Handle(**kw)
-
-
-def _device(a):
-    import torch
-    t = torch.from_numpy(np.ascontiguousarray(a)).cuda()
-    torch.cuda.synchronize()
-    return t
-
-
 def buffers(n, rows, wpr, cap, kind=MEM_HOST, arrays=("adj", "degree", "edges")):
     return GraphBuffers(n, rows, wpr, cap, kind, arrays, fill=SENT)
 
@@ -171,7 +158,7 @@ def mixed():
 @pytest.mark.parametrize("lanes", [1, 4])
 def test_mixed_batch_equals_single_calls_and_the_oracle(mixed, oracle, lanes):
     sets, params = mixed
-    h = _handle(lanes, max_batch_slots=8, max_corr=8192)
+    h = make_handle(lanes, max_batch_slots=8, max_corr=8192)
     try:
         assert len(sets) > 3 * 8
         rows = max(len(a) for a, _ in sets)
@@ -202,7 +189,7 @@ def test_memory_kinds_give_the_same_bytes(handle):
     ref = handle.build_graph_batch_each(sets, params, MEM_HOST, ref_buf)
     for i, (adj, deg, ne) in enumerate(single):
         check_set(i, ref[i], ref_buf, adj, deg, ne, i)
-    keep = [(_device(a), _device(b)) for a, b in sets]
+    keep = [(device_copy(a), device_copy(b)) for a, b in sets]
     dev_sets = [(ta.data_ptr(), tb.data_ptr(), len(a)) for (ta, tb), (a, _) in zip(keep, sets)]
     for kind, ss in ((MEM_HOST, sets), (MEM_DEVICE, dev_sets)):
         for dest in (MEM_HOST, MEM_DEVICE):
@@ -243,7 +230,7 @@ def test_clipped_edge_lists_carry_the_flag(handle):
 def test_host_edge_lists_cross_in_windows():
     """One slot per wave, one raw point per cloud, max_corr 4096: the edge staging (adjp, 4096 x 128 words) holds 262 144 edges, and a
     near-complete graph of 4096 vertices has about 8.4 M"""
-    h = _handle(2, max_batch_slots=1, max_raw_points=1, max_corr=4096)
+    h = make_handle(2, max_batch_slots=1, max_raw_points=1, max_corr=4096)
     try:
         rng = np.random.default_rng(34)
         a = rng.uniform(-20, 20, (4096, 3))

@@ -10,8 +10,8 @@ import pytest
 
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (INLIER_NONE, KCORE_HEU, LIST_LAYOUT, MATCH_LISTS, MEM_DEVICE, MEM_HOST, PMC_EXACT, RESULT_DTYPE, SET_LISTS,
-                              FeaturePair, Handle, ListBuffers, default_params)
-from support import P4, ROOT, host_lists
+                              FeaturePair, ListBuffers, default_params)
+from support import P4, ROOT, device_copies, host_lists, make_handle, make_params, sentinel, sentinel_lists
 
 # new call -> the register call whose arguments it takes
 NEW = {"qb200_match_batch_mixed": "qb200_register_batch_mixed", "qb200_match_batch_enqueue_mixed": "qb200_register_batch_enqueue_mixed",
@@ -55,15 +55,6 @@ def test_a_null_handle_is_refused():
 
 
 # ---- configurations ----------------------------------------------------------------------------------------------------------------
-def make_params(**kw):
-    p = default_params()
-    for k, v in kw.items():
-        setattr(p, k, v)
-    if "rot_noise_bound" not in kw:
-        p.rot_noise_bound = 2 * p.noise_bound   # explicit unless a test asks for the latch
-    return p
-
-
 SLOTS, N = 8, 20   # 20 pairs: three waves of up to 8 pairs
 # matcher and solver fields vary; the front end is the default one, which the slots are cached with
 PER_PAIR = [make_params(seed=11 + i % 3, use_tuple_test=int(i % 4 != 2), tuple_scale=0.9 if i % 5 == 1 else 0.95,
@@ -76,24 +67,11 @@ RAW = [make_params(voxel_size=(0.3, 0.35, 0.4)[i % 3], normal_radius=(0.5, 0.6)[
 SLOT_PAIRS = [(2 * i, 2 * i + 1) for i in range(N)]
 
 
-def _handle(lanes, **kw):
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))   # read when the handle is created
-        return Handle(**kw)
-
-
-def _device(arrays):
-    import torch
-    keep = [torch.from_numpy(np.ascontiguousarray(a, np.float32)).cuda() for a in arrays]
-    torch.cuda.synchronize()
-    return keep
-
-
 def _device_pairs(pairs):
     """(src, tgt) numpy pairs -> the MEM_DEVICE tuples of the raw calls, and the tensors behind them"""
     keep, out = [], []
     for s, t in pairs:
-        ts = _device([s, t])
+        _, ts = device_copies([s, t])
         keep.append(ts)
         out.append((ts[0].data_ptr(), len(s), ts[1].data_ptr(), len(t)))
     return out, keep
@@ -102,7 +80,7 @@ def _device_pairs(pairs):
 def _device_feats(feats):
     keep, out = [], []
     for s, sd, t, td in feats:
-        ts = _device([s, sd, t, td])
+        _, ts = device_copies([s, sd, t, td])
         keep.append(ts)
         out.append((ts[0].data_ptr(), ts[1].data_ptr(), len(s), ts[2].data_ptr(), ts[3].data_ptr(), len(t)))
     return out, keep
@@ -132,15 +110,6 @@ def assert_matches_register(got, reg, label=""):
         assert np.array_equal(np.asarray(g["T"]), np.eye(4).reshape(-1)), (label, i)
 
 
-def _sentinel(n, cap=64, names=MATCH_LISTS):
-    out = np.zeros(max(n, 1), RESULT_DTYPE)
-    out.view(np.uint8)[...] = 0xA5
-    lb = ListBuffers(max(n, 1), cap, MEM_HOST, names)
-    for a in lb.arrays.values():
-        a.view(np.uint8)[...] = 0xA5
-    return out, lb
-
-
 def _untouched(out, lb):
     return (out.view(np.uint8) == 0xA5).all() and all((a.view(np.uint8) == 0xA5).all() for a in lb.arrays.values())
 
@@ -152,7 +121,7 @@ def street():
 
 
 def _cached_handle(lanes, street):
-    h = _handle(lanes, max_batch_slots=SLOTS)
+    h = make_handle(lanes, max_batch_slots=SLOTS)
     h.cache_reserve(2 * N)
     h.cache_scans([s for pr in street for s in pr], list(range(2 * N)), default_params())
     return h
@@ -278,7 +247,7 @@ def test_match_then_solve_equals_register(street, feats, source):
                           inlier_selection_mode=(PMC_EXACT, PMC_EXACT, KCORE_HEU, INLIER_NONE, 1)[i % 5],
                           using_rot_inliers_when_estimating_cote=i % 2, cote_mode=i % 3 == 2) for i in range(N)]
     inputs = street if source == "raw" else feats
-    with _handle(4, max_batch_slots=SLOTS) as hm:
+    with make_handle(4, max_batch_slots=SLOTS) as hm:
         cap = hm.cfg.max_corr
         lb = ListBuffers(N, cap, MEM_DEVICE, MATCH_LISTS, device=hm.cfg.device)
         m = (hm.match_batch_mixed if source == "raw" else hm.match_features_each)(inputs, params, buffers=lb)[0]
@@ -287,7 +256,7 @@ def test_match_then_solve_equals_register(street, feats, source):
         sets = [(sm.data_ptr() + i * cap * 16, tm.data_ptr() + i * cap * 16, int(m["n_corr"][i])) for i in range(N)]
         slb = ListBuffers(N, cap, MEM_HOST, SET_LISTS)
         solved, solved_lists = hm.solve_batch_each(sets, params, MEM_DEVICE, buffers=slb)
-    with _handle(4, max_batch_slots=SLOTS) as hr:
+    with make_handle(4, max_batch_slots=SLOTS) as hr:
         rlb = ListBuffers(N, cap, MEM_HOST, tuple(LIST_LAYOUT))
         reg, reg_lists = (hr.register_batch_mixed if source == "raw" else hr.register_features_each)(inputs, params, buffers=rlb)
     assert (reg["valid"] == 1).sum() >= N - 3
@@ -310,7 +279,7 @@ def test_a_mixed_wave_equals_its_single_pair_calls(street):
                           fpfh_radius=(0.75, 1.0, 0.8)[i % 3], use_tuple_test=i % 2, tuple_scale=(0.95, 0.9, 0.8)[i % 3],
                           tuple_trials_per_corr=(100, 30)[i % 2], seed=100 + i, noise_bound=float("nan") if i == 5 else 0.3)
               for i in range(len(pairs))]
-    with _handle(4, max_batch_slots=5) as h:
+    with make_handle(4, max_batch_slots=5) as h:
         single = []
         for pr, p in zip(pairs, params):
             lb = ListBuffers(1, h.cfg.max_corr, MEM_HOST, MATCH_LISTS)
@@ -331,7 +300,7 @@ def test_edge_cases(h4, street, feats):
     s, sd, t, td = feats[0]
     empty = (np.zeros((0, 4), np.float32), np.zeros((0, 33), np.float32))
     fp = [(*empty, t, td), (s, sd, *empty), (s, sd, t, td), (s[:1], sd[:1], t[:1], td[:1])]
-    out, lb = _sentinel(len(fp), cap=h4.cfg.max_corr)
+    out, lb = sentinel(max(len(fp), 1), RESULT_DTYPE), sentinel_lists(ListBuffers(max(len(fp), 1), h4.cfg.max_corr, MEM_HOST, MATCH_LISTS))
     arr, keep = h4.feature_array(fp)
     assert h4.lib.qb200_match_features_each(h4.h, arr, len(fp), h4.params_array([PER_PAIR[0]] * len(fp)), MEM_HOST, capi._ptr(out),
                                             C.byref(lb.descriptor())) == 0
@@ -354,7 +323,7 @@ def test_edge_cases(h4, street, feats):
     bare = h4.match_features_each([feats[2]], [PER_PAIR[2]])[0]
     assert bare.tobytes() == full.tobytes()
     # more correspondences than max_corr
-    with _handle(1, max_batch_slots=2, max_corr=32) as hs:
+    with make_handle(1, max_batch_slots=2, max_corr=32) as hs:
         lb = ListBuffers(2, 32, MEM_HOST, MATCH_LISTS)
         out, lists = hs.match_features_each([feats[2], (s[:20], sd[:20], t[:20], td[:20])], [PER_PAIR[2]] * 2, buffers=lb)
         assert out["status"][0] == 3 and all(len(v) == 0 for v in lists[0].values())
@@ -372,7 +341,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, street, feats):
     pair_arr, keep_pairs = h4.pair_array(street[:3])
     feat_arr, keep_feats = h4.feature_array(feats[:3])
     s, sd, t, td = feats[1]
-    dev = _device([s, sd, t, td])
+    _, dev = device_copies([s, sd, t, td])
     raw = torch.zeros(64, dtype=torch.float32, device="cuda")
 
     host_buf = np.zeros(64 * 3 * 16, np.uint8)
@@ -384,7 +353,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, street, feats):
         return d
 
     def call(fn_name, arr, ps=None, kind=MEM_HOST, lists=None):
-        out, lb = _sentinel(3)
+        out, lb = sentinel(3, RESULT_DTYPE), sentinel_lists(ListBuffers(3, 64, MEM_HOST, MATCH_LISTS))
         d = lists if lists is not None else lb.descriptor()
         args = [h4.h, arr, 3, h4.params_array(ps or PER_PAIR[:3])] + ([kind] if fn_name != "qb200_match_cached_enqueue_mixed" else [])
         st = getattr(lib, fn_name)(*args, capi._ptr(out), C.byref(d))
@@ -438,7 +407,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, street, feats):
 def test_one_stream_of_match_and_register_batches(street, feats):
     sets = [tuple(a[:L] for a in synth.matched_pairs(800 + i, L, inlier_ratio=0.35, noise=0.03)[:2]) for i, L in enumerate([40, 300, 900] * 3)]
     new_scan = synth.outdoor_pair(1999, rings=32, azimuths=900)[0]
-    with _handle(4, max_batch_slots=SLOTS) as h:
+    with make_handle(4, max_batch_slots=SLOTS) as h:
         h.cache_reserve(2 * N)
         h.cache_scans([s for pr in street for s in pr], list(range(2 * N)), default_params())
         before = h.match_cached_mixed(SLOT_PAIRS, PER_PAIR)[0]

@@ -9,7 +9,7 @@ import pytest
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (Handle, ListBuffers, LIST_LAYOUT, SET_LISTS, FLAG_LISTS_TRUNCATED, MEM_HOST, MEM_DEVICE, PMC_EXACT,
                               INLIER_NONE, RESULT_DTYPE, default_params)
-from support import build_against_lib, host_lists, same_lists
+from support import build_against_lib, host_lists, same_lists, sentinel_lists
 
 FIXTURE = "tests/fixtures/pair_lists_shim.cpp"
 
@@ -181,16 +181,6 @@ def test_solve_batch_lists(oracle):
         assert e.value.code == -1
 
 
-def _sentinel(lb):
-    """every byte of every array 0xA5: entries a call does not write keep it"""
-    for a in lb.arrays.values():
-        if isinstance(a, np.ndarray):
-            a.view(np.uint8)[...] = 0xA5
-        else:
-            import torch
-            a.view(torch.uint8).fill_(0xA5)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("dest", [MEM_HOST, MEM_DEVICE])
 def test_truncated_lists_are_prefixes_and_flagged(street, dest):
@@ -201,7 +191,7 @@ def test_truncated_lists_are_prefixes_and_flagged(street, dest):
         cap = int(np.median(full_recs["clique_size"]))
         for names in (SET_LISTS, tuple(LIST_LAYOUT)):
             lb = ListBuffers(len(pairs), cap, dest, tuple(LIST_LAYOUT), h.cfg.device)
-            _sentinel(lb)
+            sentinel_lists(lb)
             d = lb.descriptor()
             for n in set(LIST_LAYOUT) - set(names):
                 setattr(d, n, None)                       # not asked for: must stay all sentinel
@@ -234,7 +224,7 @@ def test_capacity_exceeded_pair_gets_no_entries(street):
     pairs = [street[0], small, street[1]]
     with Handle(max_batch_slots=4, max_corr=64) as h:
         lb = ListBuffers(len(pairs), 64, MEM_HOST)
-        _sentinel(lb)
+        sentinel_lists(lb)
         recs, _ = h.register_batch_lists(pairs, p, buffers=lb)
         assert recs.tobytes() == h.register_batch(pairs, p).tobytes()
         over = recs["status"] == 3

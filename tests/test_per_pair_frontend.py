@@ -11,7 +11,7 @@ import pytest
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (COTE_WEIGHTED_MEAN, INLIER_NONE, KCORE_HEU, LIST_LAYOUT, MEM_DEVICE, MEM_HOST, RESULT_DTYPE, Handle,
                               ListBuffers, default_params)
-from support import ROOT, assert_same_record, build_against_lib, host_lists, same_lists
+from support import ROOT, assert_same_record, build_against_lib, host_lists, make_handle, make_params, same_lists, sentinel, sentinel_lists
 
 MIXED = {"qb200_register_batch_mixed": "qb200_register_batch_each", "qb200_register_batch_enqueue_mixed": "qb200_register_batch_enqueue_each",
          "qb200_register_cached_mixed": "qb200_register_cached_each", "qb200_cache_scans_each": "qb200_cache_scans"}
@@ -47,14 +47,6 @@ def test_mixed_calls_refuse_a_null_handle():
 
 
 # ---- configurations -----------------------------------------------------------------------------------------------------------------
-def make_params(**kw):
-    p = default_params()
-    for k, v in kw.items():
-        setattr(p, k, v)
-    p.rot_noise_bound = 2 * p.noise_bound   # explicit: the oracle has no latch
-    return p
-
-
 # Cycled over the pairs: bench.py's street and dense presets, three voxel sizes whose explicit lattice cell gives a lattice reach of 2
 # for both radii (ceil(0.75 / 0.4), ceil(0.5 / 0.4), ...), equal radii, flagged points kept, the tuple test switched off by its scale,
 # zero and 250 trials per correspondence; every entry its own seed, and solver fields varied alongside.
@@ -77,24 +69,6 @@ N_PAIRS = 2 * SLOTS * LANES + 3   # more waves than lanes: every lane runs more 
 
 def cycled(n, offset=0, sets=CONFIGS):
     return [sets[(i + offset) % len(sets)] for i in range(n)]
-
-
-def _handle(monkeypatch, **kw):
-    monkeypatch.delenv("QB200_LANES", raising=False)   # read when the handle is created
-    return Handle(max_batch_slots=SLOTS, **kw)
-
-
-def _sentinel_out(n):
-    out = np.zeros(max(n, 1), RESULT_DTYPE)
-    out.view(np.uint8)[...] = 0xA5
-    return out
-
-
-def _sentinel_lists(n):
-    lb = ListBuffers(n, 64, MEM_HOST)
-    for a in lb.arrays.values():
-        a.view(np.uint8)[...] = 0xA5
-    return lb
 
 
 def _untouched(out, lb):
@@ -181,13 +155,12 @@ def test_size_faults_stay_per_pair(h, street, broadcast):
 
 # ---- GPU 4: clouds above the shared-memory lattice sort in a mixed wave -------------------------------------------------------------
 @pytest.mark.gpu
-def test_indoor_and_street_pairs_in_one_large_v_wave(street, monkeypatch):
+def test_indoor_and_street_pairs_in_one_large_v_wave(street):
     indoor = make_params(voxel_size=0.05, normal_radius=0.10, fpfh_radius=0.15, noise_bound=0.05, cote_noise_bound=0.05, skip_flagged=0,
                          seed=41)   # bench.py's indoor preset
     pairs = [street[0], synth.indoor_pair(5)[:2], street[1]]
     params = [CONFIGS[0], indoor, CONFIGS[1]]
-    monkeypatch.delenv("QB200_LANES", raising=False)
-    with Handle(max_batch_slots=4, max_raw_points=524288, max_voxel_points=65536) as hb:
+    with make_handle(None, max_batch_slots=4, max_raw_points=524288, max_voxel_points=65536) as hb:
         recs, lists = hb.register_batch_mixed(pairs, params, buffers=ListBuffers(3, hb.cfg.max_corr))
         assert recs["n_src_vox"][1] > 17920
         for i, (pr, p) in enumerate(zip(pairs, params)):
@@ -248,7 +221,7 @@ def test_cache_scans_each_and_register_cached_mixed(h, street):
         # a pair whose entry does not match one of its slots (slot 2 holds configuration 1) rejects the whole call
         bad = [pairs[0], (0, 2), pairs[2]]
         sp = np.ascontiguousarray(np.asarray(bad, np.int32))
-        out, lb = _sentinel_out(3), _sentinel_lists(3)
+        out, lb = sentinel(3, RESULT_DTYPE), sentinel_lists(ListBuffers(3, 64))
         st = h.lib.qb200_register_cached_mixed(h.h, capi._ptr(sp), 3, h.params_array([sets[0], sets[0], sets[2]]), capi._ptr(out),
                                                C.byref(lb.descriptor()))
         assert st == -1 and _untouched(out, lb)
@@ -257,7 +230,7 @@ def test_cache_scans_each_and_register_cached_mixed(h, street):
         h.cache_copy(2, 0)
         got, _ = h.register_cached_mixed([(0, 3)], [sets[1]])
         assert got.tobytes() == h.register_cached_lists([(2, 3)], sets[1])[0].tobytes()
-        out = _sentinel_out(1)
+        out = sentinel(1, RESULT_DTYPE)
         sp = np.ascontiguousarray(np.asarray([(0, 3)], np.int32))
         assert h.lib.qb200_register_cached_mixed(h.h, capi._ptr(sp), 1, h.params_array([sets[0]]), capi._ptr(out), None) == -1
     finally:
@@ -284,7 +257,7 @@ def test_identical_entries_equal_the_broadcast_call(h, street, k):
 
 # ---- GPU 8: validation --------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_a_bad_entry_rejects_the_whole_call(street, monkeypatch):
+def test_a_bad_entry_rejects_the_whole_call(street):
     pairs = street[:SLOTS + 2]
     n = len(pairs)
 
@@ -300,7 +273,7 @@ def test_a_bad_entry_rejects_the_whole_call(street, monkeypatch):
 
     cases = [(bad(3, normal_radius=float("nan")), -1), (bad(0, fpfh_radius=float("nan")), -1), (bad(n - 1, normal_radius=1.0), -1),
              (bad(2, voxel_size=0.0), -1), (bad(1, noise_bound=-1.0), -1), (bad(4, use_crosscheck=0), -4)]
-    with _handle(monkeypatch) as h1, _handle(monkeypatch) as h2:
+    with make_handle(None, max_batch_slots=SLOTS) as h1, make_handle(None, max_batch_slots=SLOTS) as h2:
         scans = [s for pr in pairs for s in pr]
         h1.cache_reserve(2 * n)
         h1.cache_scans(scans, list(range(2 * n)), default_params())
@@ -313,7 +286,7 @@ def test_a_bad_entry_rejects_the_whole_call(street, monkeypatch):
         }
         for name, call in calls.items():
             for ps, code in cases:
-                out, lb = _sentinel_out(n), _sentinel_lists(n)
+                out, lb = sentinel(max(n, 1), RESULT_DTYPE), sentinel_lists(ListBuffers(n, 64))
                 st = call(h1.params_array(ps), out, C.byref(lb.descriptor()))
                 msg = h1.lib.qb200_last_error(h1.h).decode()
                 h1.register_batch_flush()

@@ -10,7 +10,7 @@ import pytest
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (COTE_WEIGHTED_MEAN, FLAG_CLIQUE_TRUNCATED, INLIER_NONE, KCORE_HEU, LIST_LAYOUT, MEM_DEVICE, MEM_HOST,
                               PMC_EXACT, PMC_HEU, RESULT_DTYPE, SET_LISTS, Handle, ListBuffers, default_params)
-from support import ROOT, assert_same_record, host_lists, same_lists
+from support import ROOT, assert_same_record, host_lists, make_handle, make_params, same_lists, sentinel
 
 EACH = {"qb200_register_batch_each": "qb200_register_batch_ex", "qb200_register_batch_enqueue_each": "qb200_register_batch_enqueue_ex",
         "qb200_register_cached_each": "qb200_register_cached_ex", "qb200_solve_batch_each": "qb200_solve_batch_ex"}
@@ -38,24 +38,11 @@ def test_ctypes_signatures_match_the_ex_siblings():
 
 # ---- parameter sets ------------------------------------------------------------------------------------------------------------
 def ryrx(roll_deg, pitch_deg):
-    """Ry(pitch) Rx(roll): the roll/pitch prior an IMU gives for a scan (setPreEstaimatedRyRx)."""
+    """Ry(pitch) Rx(roll), the Params.RyRx field: the roll/pitch prior an IMU gives for a scan (setPreEstaimatedRyRx)."""
     r, p = np.radians(roll_deg), np.radians(pitch_deg)
     rx = np.array([[1, 0, 0], [0, np.cos(r), -np.sin(r)], [0, np.sin(r), np.cos(r)]])
     ry = np.array([[np.cos(p), 0, np.sin(p)], [0, 1, 0], [-np.sin(p), 0, np.cos(p)]])
-    return ry @ rx
-
-
-def make_params(rot_noise_bound=None, RyRx=None, **kw):
-    p = default_params()
-    for k, v in kw.items():
-        setattr(p, k, v)
-    # explicit rotation noise bounds: the oracle has no latch (the latch has a test of its own)
-    p.rot_noise_bound = 2 * p.noise_bound if rot_noise_bound is None else rot_noise_bound
-    if RyRx is not None:
-        p.use_pre_estimated_RyRx = 1
-        for i, v in enumerate(np.asarray(RyRx, np.float64).ravel()):
-            p.RyRx[i] = v
-    return p
+    return (C.c_double * 9)(*(ry @ rx).ravel())
 
 
 # Six configurations cycled over the pairs: all four inlier modes (PMC_EXACT once with a one-node limit), both COTE modes with the
@@ -64,14 +51,14 @@ def make_params(rot_noise_bound=None, RyRx=None, **kw):
 SETS = [
     make_params(),
     make_params(inlier_selection_mode=PMC_EXACT, max_clique_node_limit=1, noise_bound=0.6, cbar2=1.2, cote_noise_bound=0.25,
-                cote_mode=COTE_WEIGHTED_MEAN, using_rot_inliers_when_estimating_cote=1, RyRx=ryrx(1.5, -0.8)),
+                cote_mode=COTE_WEIGHTED_MEAN, using_rot_inliers_when_estimating_cote=1, use_pre_estimated_RyRx=1, RyRx=ryrx(1.5, -0.8)),
     make_params(inlier_selection_mode=KCORE_HEU, kcore_heuristic_threshold=0.3, noise_bound=0.35, cbar2=0.8, cote_noise_bound=0.4,
-                rotation_gnc_factor=1.6, rotation_max_iterations=20, RyRx=ryrx(-2.0, 1.0)),
+                rotation_gnc_factor=1.6, rotation_max_iterations=20, use_pre_estimated_RyRx=1, RyRx=ryrx(-2.0, 1.0)),
     make_params(inlier_selection_mode=INLIER_NONE, cote_mode=COTE_WEIGHTED_MEAN, rotation_gnc_factor=1.2, rotation_max_iterations=8,
-                RyRx=ryrx(0.5, 2.5)),
+                use_pre_estimated_RyRx=1, RyRx=ryrx(0.5, 2.5)),
     make_params(inlier_selection_mode=PMC_EXACT, using_rot_inliers_when_estimating_cote=1),
     make_params(rotation_gnc_factor=1.8, rotation_max_iterations=30, rotation_cost_threshold=1e-3, cote_noise_bound=0.35,
-                using_rot_inliers_when_estimating_cote=1, RyRx=ryrx(-1.2, -1.7), rot_noise_bound=0.5),
+                using_rot_inliers_when_estimating_cote=1, use_pre_estimated_RyRx=1, RyRx=ryrx(-1.2, -1.7), rot_noise_bound=0.5),
 ]
 LANES = 4   # the default lane count (QB200_LANES unset)
 SLOTS = 4
@@ -80,11 +67,6 @@ N_PAIRS = 2 * SLOTS * LANES + 3   # more waves than lanes: every lane runs more 
 
 def cycled(n, offset=0):
     return [SETS[(i + offset) % len(SETS)] for i in range(n)]
-
-
-def _fresh_handle(monkeypatch, **kw):
-    monkeypatch.delenv("QB200_LANES", raising=False)   # read when the handle is created
-    return Handle(max_batch_slots=SLOTS, **kw)
 
 
 # ---- GPU fixtures ----------------------------------------------------------------------------------------------------------------
@@ -197,10 +179,10 @@ def solve_sets():
 
 
 @pytest.mark.gpu
-def test_solve_batch_each_mixed_waves_equal_broadcast_and_oracle(oracle, monkeypatch):
+def test_solve_batch_each_mixed_waves_equal_broadcast_and_oracle(oracle):
     sets = solve_sets()
     params = cycled(len(sets))
-    with _fresh_handle(monkeypatch, max_corr=16384) as hs:
+    with make_handle(None, max_batch_slots=SLOTS, max_corr=16384) as hs:
         ref = [hs.solve_batch_lists(sets, p) for p in SETS]
         recs, lists = hs.solve_batch_each(sets, params, buffers=ListBuffers(len(sets), hs.cfg.max_corr, MEM_HOST, SET_LISTS))
     _check_against_broadcast(recs, lists, ref, range(len(sets)), [i % len(SETS) for i in range(len(sets))])
@@ -233,12 +215,12 @@ def test_identical_entries_equal_the_broadcast_call(h, street, mode):
 
 # ---- GPU: the rotation noise latch ----------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_latch_resolves_in_pair_order(street, monkeypatch):
+def test_latch_resolves_in_pair_order(street):
     pairs = street[:SLOTS + 3]
     params = []
     for i, nb in enumerate((0.35, 0.25, 0.3, 0.4, 0.25, 0.3, 0.35)):
         params.append(make_params(noise_bound=nb, rot_noise_bound=0.0 if i != 2 else 0.45))
-    with _fresh_handle(monkeypatch) as h1, _fresh_handle(monkeypatch) as h2:
+    with make_handle(None, max_batch_slots=SLOTS) as h1, make_handle(None, max_batch_slots=SLOTS) as h2:
         recs, _ = h1.register_batch_each(pairs, params)
         single = b"".join(bytes(h2.register_pair(s, t, p)[0]) for (s, t), p in zip(pairs, params))
         assert recs.tobytes() == single
@@ -248,14 +230,8 @@ def test_latch_resolves_in_pair_order(street, monkeypatch):
 
 
 # ---- GPU: validation -----------------------------------------------------------------------------------------------------------
-def _sentinel_out(n):
-    out = np.zeros(n, RESULT_DTYPE)
-    out.view(np.uint8)[...] = 0xA5
-    return out
-
-
 @pytest.mark.gpu
-def test_bad_entries_reject_the_whole_call(street, monkeypatch):
+def test_bad_entries_reject_the_whole_call(street):
     pairs = street[:SLOTS + 2]
     n = len(pairs)
     good = [make_params(noise_bound=nb, rot_noise_bound=0.0) for nb in (0.3, 0.25, 0.35, 0.3, 0.25, 0.35)]
@@ -271,7 +247,7 @@ def test_bad_entries_reject_the_whole_call(street, monkeypatch):
         ps[k].voxel_size = 0.31
         return ps
 
-    with _fresh_handle(monkeypatch) as h1, _fresh_handle(monkeypatch) as h2:
+    with make_handle(None, max_batch_slots=SLOTS) as h1, make_handle(None, max_batch_slots=SLOTS) as h2:
         h1.cache_reserve(2 * n)
         h1.cache_scans([s for pr in pairs for s in pr], list(range(2 * n)), default_params())
         arr, keep = h1.pair_array(pairs)
@@ -288,7 +264,7 @@ def test_bad_entries_reject_the_whole_call(street, monkeypatch):
         for name, call in calls.items():
             cases = bad + ([frontend_mismatch(3), frontend_mismatch(n - 1)] if name != "solve" else [])
             for ps in cases:
-                out = _sentinel_out(n)
+                out = sentinel(n, RESULT_DTYPE)
                 lb = ListBuffers(n, 64, MEM_HOST, SET_LISTS)
                 for a in lb.arrays.values():
                     a.view(np.uint8)[...] = 0xA5

@@ -13,7 +13,7 @@ import pytest
 from quatro_b200 import capi, synth
 from quatro_b200.capi import (COTE_MEDIAN, COTE_WEIGHTED_MEAN, GRAPH_LISTS, MATCH_LISTS, MEM_DEVICE, MEM_HOST, RESULT_DTYPE, SET_LISTS,
                               GraphBuffers, Handle, InlierSet, ListBuffers, default_params)
-from support import P4, ROOT, host_lists
+from support import P4, ROOT, device_copy, host_lists, make_handle
 
 NEW = ("qb200_solve_pose_batch_each", "qb200_solve_pose_batch_enqueue_each")
 SIZES = (0, 1, 2, 31, 32, 33, 4095, 4096, 4097, 8192, 32768)
@@ -140,22 +140,9 @@ def untouched(lb, i):
     return all((lb.host(n)[i].view(np.uint8) == SENT).all() for n in lb.arrays)
 
 
-def _handle(lanes, **kw):
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))
-        return Handle(**kw)
-
-
-def _device(a):
-    import torch
-    t = torch.from_numpy(np.ascontiguousarray(a)).cuda()
-    torch.cuda.synchronize()
-    return t
-
-
 def device_sets(sets, inliers):
     """the same sets and ids in device memory: (sets, inliers as the call takes them, the tensors that hold them)"""
-    keep = [(_device(a), _device(b), _device(np.asarray(i, np.int32).reshape(-1) if len(i) else np.zeros(1, np.int32)))
+    keep = [(device_copy(a), device_copy(b), device_copy(np.asarray(i, np.int32).reshape(-1) if len(i) else np.zeros(1, np.int32)))
             for (a, b), i in zip(sets, inliers)]
     return ([(ta.data_ptr(), tb.data_ptr(), len(a)) for (ta, tb, _), (a, _) in zip(keep, sets)],
             [(ti.data_ptr() if len(i) else None, len(i)) for (_, _, ti), i in zip(keep, inliers)], keep)
@@ -194,7 +181,7 @@ def mixed():
 @pytest.mark.parametrize("lanes", [1, 4])
 def test_mixed_batch_equals_single_calls_and_the_oracle(mixed, oracle, lanes):
     sets, inliers, params, cmp = mixed
-    h = _handle(lanes, max_batch_slots=8, max_corr=8192)
+    h = make_handle(lanes, max_batch_slots=8, max_corr=8192)
     try:
         assert len(sets) > 3 * 8 and any(len(i) > 4096 for i in inliers)
         recs, lists = h.solve_pose_batch_each(sets, inliers, params, buffers=ListBuffers(len(sets), 8192, MEM_HOST, SET_LISTS))
@@ -251,7 +238,7 @@ def test_per_set_params_and_the_latch_follow_set_order():
     sets, inliers = [(a, b) for a, b, _ in base], [i for _, _, i in base]
     with Handle(max_batch_slots=4) as seq:
         want = [single(seq, a, b, i, p) for (a, b), i, p in zip(sets, inliers, params)]
-    with _handle(4, max_batch_slots=4) as h:
+    with make_handle(4, max_batch_slots=4) as h:
         recs, lists = h.solve_pose_batch_each(sets, inliers, params, buffers=ListBuffers(len(sets), 1024, MEM_HOST, SET_LISTS))
         for i, ids in enumerate(inliers):
             check_set(recs[i], lists[i], want[i], ids, 1024, i)
@@ -364,7 +351,7 @@ def test_out_of_range_ids_refuse_only_their_set(kind):
 def test_rejections_write_nothing_and_name_the_set(handle):
     import torch
     a4, b4, ids = scene(470, 40)
-    ta, tb, ti = _device(a4), _device(b4), _device(ids)
+    ta, tb, ti = device_copy(a4), device_copy(b4), device_copy(ids)
     p = pose_params()
     bad_p = pose_params(cote_noise_bound=0.0)
     lb = sentinel_lists(2, 64)
@@ -463,7 +450,7 @@ def test_memory_kinds_and_clipped_lists_give_the_same_bytes(wave_sets):
 def test_lanes_and_wave_sizes(wave_sets, lanes):
     sets, inliers, params, want = wave_sets
     S = 4
-    h = _handle(lanes, max_batch_slots=S)
+    h = make_handle(lanes, max_batch_slots=S)
     try:
         for n in (S - 1, S, S + 1, 3 * S + 5):
             recs, lists = h.solve_pose_batch_each(sets[:n], inliers[:n], params[:n], buffers=ListBuffers(n, 1024, MEM_HOST, SET_LISTS))

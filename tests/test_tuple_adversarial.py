@@ -34,7 +34,7 @@ import pytest
 
 from independent_ref import cloud_mean, philox4x32_10, philox4x32_10_words, tuple_decide, tuple_match
 from quatro_b200.capi import MATCH_LISTS, MEM_HOST, ListBuffers, default_params
-from support import fpfh_like
+from support import fpfh_like, make_handle
 
 F32 = np.float32
 FLT_MIN = float(np.finfo(np.float32).tiny)
@@ -359,16 +359,9 @@ def test_oracle_clips_at_its_capacity(oracle):
 
 
 # ---- GPU ---------------------------------------------------------------------------------------------------------------------------
-def _handle(lanes):
-    from quatro_b200.capi import Handle
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))                    # read when the handle is created
-        return Handle(max_batch_slots=4, max_voxel_points=V_MAX, max_corr=CORR_MAX)
-
-
 @pytest.fixture(scope="module")
 def h1():
-    h = _handle(1)
+    h = make_handle(1, max_batch_slots=4, max_voxel_points=V_MAX, max_corr=CORR_MAX)
     yield h
     h.close()
 
@@ -406,7 +399,7 @@ def test_device_matchers_equal_restatement(h1, singles, name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("lanes", [1, 4])
 def test_mixed_wave_equals_single_calls(h1, singles, lanes):
-    h = h1 if lanes == 1 else _handle(4)
+    h = h1 if lanes == 1 else make_handle(4, max_batch_slots=4, max_voxel_points=V_MAX, max_corr=CORR_MAX)
     try:
         order = NAMES[::-1] if lanes == 4 else NAMES
         recs, lists = _feature_call(h, order)

@@ -10,9 +10,10 @@ import numpy as np
 import pytest
 
 from quatro_b200 import capi, synth
-from quatro_b200.capi import (MEM_DEVICE, MEM_HOST, PREPROCESS_ARRAYS, RESULT_DTYPE, Handle, ListBuffers, default_params, default_patchwork_params,
+from quatro_b200.capi import (MEM_DEVICE, MEM_HOST, PREPROCESS_ARRAYS, RESULT_DTYPE, Handle, ListBuffers, default_patchwork_params,
                               default_segment_params)
-from support import P4
+import support
+from support import P4, _host, device_copies, make_handle, sentinel
 
 NEW = ("qb200_voxelize_batch_each", "qb200_voxelize_batch_enqueue_each")
 OK, CAPACITY, OVERFLOW = 0, 3, -5
@@ -32,35 +33,17 @@ def test_library_exports_the_voxelize_calls():
 
 # ---- configurations ----------------------------------------------------------------------------------------------------------------
 def make_params(**kw):
-    p = default_params()
-    for k, v in kw.items():
-        setattr(p, k, v)
-    return p
+    """support.make_params keeping default_params()'s rot_noise_bound of 0, the latch: the register calls here run with it"""
+    return support.make_params(rot_noise_bound=0.0, **kw)
 
 
 SLOTS, RAW_CAP = 2, 65536        # a voxelize wave holds 2 * SLOTS = 4 scans
+CFG = dict(max_batch_slots=SLOTS, max_raw_points=RAW_CAP)
 STREET = make_params()
 DENSE = make_params(voxel_size=0.22)
 COARSE = make_params(voxel_size=0.4, skip_flagged=0)
 INDOOR = make_params(voxel_size=0.08)
 FINE_KEEP = make_params(voxel_size=0.25, skip_flagged=0)
-
-
-def _handle(lanes, **kw):
-    with pytest.MonkeyPatch.context() as mp:
-        mp.setenv("QB200_LANES", str(lanes))   # read when the handle is created
-        return Handle(max_batch_slots=SLOTS, max_raw_points=RAW_CAP, **kw)
-
-
-def _device_scans(scans):
-    import torch
-    keep = [torch.from_numpy(np.ascontiguousarray(s, np.float32)).cuda() for s in scans]
-    torch.cuda.synchronize()
-    return [(t.data_ptr(), len(t)) for t in keep], keep
-
-
-def _host(a):
-    return a if isinstance(a, np.ndarray) else a.cpu().numpy()
 
 
 def _ref(h, scans, params):
@@ -70,16 +53,6 @@ def _ref(h, scans, params):
         v, st = h.voxelize(s, p.voxel_size, p.skip_flagged, cap=max(1, len(s)))
         out.append((v.tobytes(), len(v), st))
     return out
-
-
-def _sentinel(n, cap, dest):
-    """a vox4 array of n + 1 scans (the last one a tail nothing may touch), filled with 0xA5 bytes"""
-    a = np.zeros((n + 1, cap, 4), np.float32)
-    a.view(np.uint8)[...] = 0xA5
-    if dest == MEM_DEVICE:
-        import torch
-        a = torch.from_numpy(a).cuda()
-    return {"vox4": a}
 
 
 # ---- GPU fixtures ------------------------------------------------------------------------------------------------------------------
@@ -96,21 +69,21 @@ def mixed():
 
 @pytest.fixture(scope="module")
 def h1():
-    h = _handle(1)
+    h = make_handle(1, **CFG)
     yield h
     h.close()
 
 
 @pytest.fixture(scope="module")
 def h4():
-    h = _handle(4)
+    h = make_handle(4, **CFG)
     yield h
     h.close()
 
 
 @pytest.fixture(scope="module")
 def ref(mixed):
-    with _handle(1) as h:
+    with make_handle(1, **CFG) as h:
         yield _ref(h, *mixed)
 
 
@@ -128,7 +101,7 @@ def test_voxelize_equals_the_stage_call_and_the_oracle(h1, h4, mixed, ref, oracl
     described, dcounts, dstatus = h.describe_batch_each(scans, params)
     assert (dstatus == OK).all()
     assert [d[0].tobytes() for d in described] == [r[0] for r in ref]
-    dev, keep = _device_scans(scans)
+    dev, keep = device_copies(scans)
     for kind, dest in KINDS:
         per_scan, counts, status = h.voxelize_batch_each(dev if kind == MEM_DEVICE else scans, params, kind, dest)
         assert list(counts) == [n for _, n, _ in ref] and list(status) == [st for _, _, st in ref], (kind, dest)
@@ -176,7 +149,7 @@ def _edge_batch():
 def edge():
     batch = _edge_batch()
     scans, params = [b[1] for b in batch], [b[2] for b in batch]
-    with _handle(1) as r:
+    with make_handle(1, **CFG) as r:
         want = _ref(r, scans, params)
         V = r.cfg.max_voxel_points
     st = {b[0]: w[2] for b, w in zip(batch, want)}
@@ -197,9 +170,9 @@ def test_edge_scans_write_exactly_their_entries(h4, edge, cap):
     assert n == 2 * SLOTS * 4 + 1                                  # one more scan than a full rotation of waves over the lanes
     V = h4.cfg.max_voxel_points
     cap = {"max_voxel_points": V, "above": V + 8192}.get(cap, cap)
-    dev, keep = _device_scans(scans)
+    dev, keep = device_copies(scans)
     for kind, dest in KINDS:
-        arrays = _sentinel(n, cap, dest)
+        arrays = {"vox4": sentinel((n + 1, cap, 4), kind=dest)}
         counts, status = np.full(n, -7, np.int32), np.full(n, -7, np.int32)
         out = h4.feature_out(cap, dest, arrays, counts, status)
         ptrs, cnts, keep_h = capi._scan_arrays(dev if kind == MEM_DEVICE else scans, kind)
@@ -220,7 +193,7 @@ def test_edge_scans_write_exactly_their_entries(h4, edge, cap):
 @pytest.mark.gpu
 def test_counts_only_call(h4, edge):
     batch, scans, params, want = edge
-    dev, keep = _device_scans(scans)
+    dev, keep = device_copies(scans)
     for kind, dest in KINDS:
         per_scan, counts, status = h4.voxelize_batch_each(dev if kind == MEM_DEVICE else scans, params, kind, dest, arrays={})
         assert all(v is None for v in per_scan)
@@ -234,7 +207,7 @@ def test_voxelize_then_describe_points_equals_describe(h4, mixed):
     wide = [make_params(voxel_size=p.voxel_size, skip_flagged=p.skip_flagged, normal_radius=2.5 * p.voxel_size,
                         fpfh_radius=(4.0 if i % 2 else 3.0) * p.voxel_size, grid_cell=0.0 if i % 3 else 4.5 * p.voxel_size)
             for i, p in enumerate(params)]
-    dev, keep = _device_scans(scans)
+    dev, keep = device_copies(scans)
     vox, counts, status = h4.voxelize_batch_each(dev, wide, MEM_DEVICE, MEM_DEVICE)
     assert (status == OK).all()
     clouds = [(v.data_ptr(), int(c)) for v, c in zip(vox, counts)]
@@ -288,7 +261,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
     scans, params = mixed
     n, cap = len(scans), h4.cfg.max_voxel_points
     ptrs, cnts, keep = capi._scan_arrays(scans, MEM_HOST)
-    dev, keep_d = _device_scans(scans)
+    dev, keep_d = device_copies(scans)
     pa = h4.params_array(params)
 
     def bad_entry(k, v):
@@ -298,7 +271,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
 
     def call(dest=MEM_HOST, cap_=cap, arrays=None, drop=None, ps=None, kind_as=None, extra=None, scan_ptrs=None, scan_n=None,
              kind=MEM_HOST):
-        arrays = arrays if arrays is not None else _sentinel(n, max(cap_, 1), dest)
+        arrays = arrays if arrays is not None else {"vox4": sentinel((n + 1, max(cap_, 1), 4), kind=dest)}
         c, s = np.full(n, -7, np.int32), np.full(n, -7, np.int32)
         out = h4.feature_out(cap_, dest, arrays, c, s)
         if kind_as is not None:
@@ -311,7 +284,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
                                                    C.byref(out))
         return st, arrays, c, s
 
-    dev_out = _sentinel(n, cap, MEM_DEVICE)
+    dev_out = {"vox4": sentinel((n + 1, cap, 4), kind=MEM_DEVICE)}
     spare = np.zeros((n, cap, 33), np.float32)
     too_many = (C.c_int32 * n)(*[len(s) for s in scans])
     too_many[6] = RAW_CAP + 1
@@ -332,7 +305,7 @@ def test_a_rejected_call_writes_and_queues_nothing(h4, mixed, ref):
     }
     for name, (fn, culprit) in cases.items():
         # a batch queued before the refused call completes on the flush
-        arrays0 = _sentinel(n, cap, MEM_HOST)
+        arrays0 = {"vox4": sentinel((n + 1, cap, 4), kind=MEM_HOST)}
         c0, s0 = np.zeros(n, np.int32), np.zeros(n, np.int32)
         out0 = h4.feature_out(cap, MEM_HOST, arrays0, c0, s0)
         assert lib.qb200_voxelize_batch_enqueue_each(h4.h, ptrs, cnts, n, pa, MEM_HOST, C.byref(out0)) == 0
@@ -360,9 +333,9 @@ def test_one_stream_of_voxelize_and_every_other_batch(mixed, ref, edge):
         p.rot_noise_bound = 2 * p.noise_bound
     cache_scans = [c for pr in pairs[:2] for c in pr]
     cache_pp = [p for p in pp[:2] for _ in (0, 1)]
-    with _handle(4) as h:
+    with make_handle(4, **CFG) as h:
         h.cache_reserve(4)
-        dev, keep = _device_scans(escans)
+        dev, keep = device_copies(escans)
         cap = h.cfg.max_voxel_points
 
         def run(queued):

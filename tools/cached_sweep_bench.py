@@ -22,20 +22,15 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 from pathlib import Path
 
 import numpy as np
 
+from harness import card, timed
+
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
-    return q.strip().splitlines()[0] if q.strip() else "unknown"
 
 
 def handle(lanes, **cfg):
@@ -49,19 +44,6 @@ def handle(lanes, **cfg):
         os.environ.pop("QB200_LANES", None)
         if old is not None:
             os.environ["QB200_LANES"] = old
-
-
-def timed(ways, warmup, rounds):
-    for fn in ways.values():
-        for _ in range(warmup):
-            fn()
-    ms = {k: [] for k in ways}
-    for _ in range(rounds):
-        for name, fn in ways.items():
-            t0 = time.perf_counter()
-            fn()
-            ms[name].append(1e3 * (time.perf_counter() - t0))
-    return {k: {"median": float(np.median(v)), "min": float(min(v)), "max": float(max(v))} for k, v in ms.items()}
 
 
 def main():
@@ -116,8 +98,8 @@ def main():
             hd.register_cached_enqueue_mixed_raw(slot_arr[a:b], b - a, par, out["cached_stream"][a:b])
         hd.register_batch_flush()
 
-    sweep = timed({"cached_lanes1": cached(h1, "cached_lanes1"), "cached_lanes": cached(hd, "cached_lanes"), "cached_stream": cached_stream,
-                   "uncached": lambda: hd.register_batch_raw(raw, P, p, MEM_DEVICE, out["uncached"])}, args.warmup, args.rounds)
+    sweep, _ = timed({"cached_lanes1": cached(h1, "cached_lanes1"), "cached_lanes": cached(hd, "cached_lanes"), "cached_stream": cached_stream,
+                      "uncached": lambda: hd.register_batch_raw(raw, P, p, MEM_DEVICE, out["uncached"])}, args.warmup, args.rounds)
     same_sweep = {k: out[k].tobytes() == out["cached_lanes1"].tobytes() for k in out}
 
     # correspondence sets
@@ -140,8 +122,8 @@ def main():
             hd.solve_batch_enqueue_each_raw(C.addressof(sets) + a * C.sizeof(CorrSet), b - a, par, MEM_DEVICE, sout["solve_stream"][a:b])
         hd.register_batch_flush()
 
-    solve_ms = timed({"solve_lanes1": solve(h1, "solve_lanes1"), "solve_lanes": solve(hd, "solve_lanes"), "solve_stream": solve_stream},
-                     args.warmup, args.rounds)
+    solve_ms, _ = timed({"solve_lanes1": solve(h1, "solve_lanes1"), "solve_lanes": solve(hd, "solve_lanes"), "solve_stream": solve_stream},
+                        args.warmup, args.rounds)
     same_sets = {k: sout[k].tobytes() == sout["solve_lanes1"].tobytes() for k in sout}
 
     print(json.dumps({

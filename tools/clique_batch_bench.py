@@ -17,20 +17,15 @@ from __future__ import annotations
 
 import argparse
 import json
-import subprocess
 import sys
-import time
 from pathlib import Path
 
 import numpy as np
 
+from harness import card, timed
+
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
-    return q.strip().splitlines()[0] if q.strip() else "unknown"
 
 
 def random_adj(rng, L, deg, k=16):
@@ -60,23 +55,15 @@ def workload(h, graphs, p, warmup, rounds):
     def loop():
         state["loop"] = [h.max_clique_ex(a, mode, thr)[0] for a in graphs]
 
-    for _ in range(warmup):
-        batch()
-        loop()
-    ms = {"batch": [], "loop": []}
-    same = True
-    for _ in range(rounds):
-        for name, fn in (("batch", batch), ("loop", loop)):
-            t0 = time.perf_counter()
-            fn()
-            ms[name].append(1e3 * (time.perf_counter() - t0))
+    def same():
         _, lists = state["batch"]
-        same &= all(d["clique"].tobytes() == c.astype(np.int32).tobytes() for d, c in zip(lists, state["loop"]))
-    out = {k: {"median": float(np.median(v)), "min": float(min(v)), "max": float(max(v))} for k, v in ms.items()}
+        return all(d["clique"].tobytes() == c.astype(np.int32).tobytes() for d, c in zip(lists, state["loop"]))
+
+    out, ok = timed({"batch": batch, "loop": loop}, warmup, rounds, {"loop": same})
     out["speedup"] = out["loop"]["median"] / out["batch"]["median"]
     out["graphs"] = len(graphs)
     out["vertices_mean"] = float(np.mean([a.shape[0] for a in graphs]))
-    return out, same
+    return out, ok["loop"]
 
 
 def main():

@@ -20,33 +20,15 @@ from __future__ import annotations
 
 import argparse
 import json
-import subprocess
 import sys
-import time
 from pathlib import Path
 
 import numpy as np
 
+from harness import card, timed
+
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
-    return q.strip().splitlines()[0] if q.strip() else "unknown"
-
-
-def timed(ways, warmup, rounds):
-    for fn in ways.values():
-        for _ in range(warmup):
-            fn()
-    ms = {k: [] for k in ways}
-    for _ in range(rounds):
-        for name, fn in ways.items():
-            t0 = time.perf_counter()
-            fn()
-            ms[name].append(1e3 * (time.perf_counter() - t0))
-    return {k: {"median": float(np.median(v)), "min": float(min(v)), "max": float(max(v))} for k, v in ms.items()}
 
 
 def main():
@@ -94,7 +76,7 @@ def main():
         "cached": lambda: out.__setitem__("cached", h.register_cached_mixed(slot_pairs, params)[0]),
         "match_loop": lambda: out.__setitem__("match_loop", match_loop()),
     }
-    ms = timed(ways, a.warmup, a.rounds)
+    ms, _ = timed(ways, a.warmup, a.rounds)
 
     same = {k: out[k].tobytes() == out["cached"].tobytes() for k in ("features_device", "features_host")}
     skip = {"n_src_vox", "n_tgt_vox", "n_mutual"}

@@ -18,20 +18,15 @@ from __future__ import annotations
 
 import argparse
 import json
-import subprocess
 import sys
-import time
 from pathlib import Path
 
 import numpy as np
 
+from harness import card, timed
+
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
-    return q.strip().splitlines()[0] if q.strip() else "unknown"
 
 
 def edges_match(edges, n_edges, adj_dev, L):
@@ -72,34 +67,27 @@ def workload(h, sets, p, warmup, rounds):
             torch.cuda.synchronize()
         return run
 
-    fns = {"loop": loop, **{k: batch(k) for k in bufs}}
-    for _ in range(warmup):
-        for fn in fns.values():
-            fn()
-    ms = {k: [] for k in fns}
-    same = True
-    for _ in range(rounds):
-        for name, fn in fns.items():
-            t0 = time.perf_counter()
-            fn()
-            ms[name].append(1e3 * (time.perf_counter() - t0))
+    def same():
+        ok = True
         ref = state["loop"]
         host_adj, host_deg = bufs["host_adj"].host("adj"), bufs["host_adj"].host("degree")
         dev_adj, dev_deg = bufs["device_adj"].host("adj"), bufs["device_adj"].host("degree")
         for i, (adj, deg, ne) in enumerate(ref):
             L = Ls[i]
             for recs in (state["host_adj"], state["device_adj"], state["device_edges"]):
-                same &= int(recs[i]["n_edges"]) == ne and int(recs[i]["n_corr"]) == L and int(recs[i]["flags"]) == 0
-            same &= host_adj[i, :L].tobytes() == adj.tobytes() and host_deg[i, :L].tobytes() == deg.tobytes()
-            same &= dev_adj[i, :L].tobytes() == adj.tobytes() and dev_deg[i, :L].tobytes() == deg.tobytes()
-            same &= edges_match(bufs["device_edges"].arrays["edges"][i], ne, bufs["device_adj"].arrays["adj"][i], L)
-    out = {k: {"median": float(np.median(v)), "min": float(min(v)), "max": float(max(v))} for k, v in ms.items()}
+                ok &= int(recs[i]["n_edges"]) == ne and int(recs[i]["n_corr"]) == L and int(recs[i]["flags"]) == 0
+            ok &= host_adj[i, :L].tobytes() == adj.tobytes() and host_deg[i, :L].tobytes() == deg.tobytes()
+            ok &= dev_adj[i, :L].tobytes() == adj.tobytes() and dev_deg[i, :L].tobytes() == deg.tobytes()
+            ok &= edges_match(bufs["device_edges"].arrays["edges"][i], ne, bufs["device_adj"].arrays["adj"][i], L)
+        return ok
+
+    out, ok = timed({"loop": loop, **{k: batch(k) for k in bufs}}, warmup, rounds, {"device_edges": same})
     for k in bufs:
         out[k]["speedup"] = out["loop"]["median"] / out[k]["median"]
     out["sets"] = n
     out["L_mean"] = float(np.mean(Ls))
     out["edges_mean"] = float(np.mean([ne for _, _, ne in state["loop"]]))
-    return out, bool(same)
+    return out, ok["device_edges"]
 
 
 def main():

@@ -23,19 +23,14 @@ import argparse
 import hashlib
 import json
 import os
-import subprocess
 import sys
-import time
 from pathlib import Path
 
 import numpy as np
 
+from harness import card, timed
+
 ROOT = Path(__file__).resolve().parent.parent
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
-    return q.strip().splitlines()[0] if q.strip() else "unknown"
 
 
 def handle(lanes, **cfg):
@@ -49,19 +44,6 @@ def handle(lanes, **cfg):
         os.environ.pop("QB200_LANES", None)
         if old is not None:
             os.environ["QB200_LANES"] = old
-
-
-def timed(ways, warmup, rounds):
-    for fn in ways.values():
-        for _ in range(warmup):
-            fn()
-    ms = {k: [] for k in ways}
-    for _ in range(rounds):
-        for name, fn in ways.items():
-            t0 = time.perf_counter()
-            fn()
-            ms[name].append(1e3 * (time.perf_counter() - t0))
-    return {k: {"median": float(np.median(v)), "min": float(min(v)), "max": float(max(v))} for k, v in ms.items()}
 
 
 def cache_digest(h, n):
@@ -125,7 +107,7 @@ def main():
 
     for h in (h1, hd):
         h.cache_reserve(B)
-    bulk_ms = timed({"bulk_lanes1": bulk(h1, "bulk_lanes1"), "bulk_lanes": bulk(hd, "bulk_lanes")}, args.warmup, args.rounds)
+    bulk_ms, _ = timed({"bulk_lanes1": bulk(h1, "bulk_lanes1"), "bulk_lanes": bulk(hd, "bulk_lanes")}, args.warmup, args.rounds)
     digests = {"bulk_lanes1": cache_digest(h1, B), "bulk_lanes": cache_digest(hd, B)}
     out = {"card": card(), "tree": "this" if args.tree.resolve() == ROOT else str(args.tree), "slots": args.slots, "rounds": args.rounds,
            "bulk": {"scans": B, "ms": bulk_ms, "scans_per_s": {k: B / (v["median"] / 1e3) for k, v in bulk_ms.items()},
@@ -163,8 +145,8 @@ def main():
             return run
 
         hd.cache_reserve(R)
-        kf_ms = timed({"keyframe_blocking": keyframes("keyframe_blocking", False), "keyframe_stream": keyframes("keyframe_stream", True)},
-                      args.warmup, args.rounds)
+        kf_ms, _ = timed({"keyframe_blocking": keyframes("keyframe_blocking", False), "keyframe_stream": keyframes("keyframe_stream", True)},
+                         args.warmup, args.rounds)
         ring_digest = cache_digest(hd, R)
 
         def flat_out(name):

@@ -12,13 +12,13 @@ record, and whether it equals the CPU oracle's (every counter, pose within 1e-9)
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from harness import card  # noqa: E402
 from quatro_b200 import capi, synth  # noqa: E402
 
 STAGES = ["h2d", "voxel", "fpfh", "match", "graph", "clique", "pose", "d2h"]
@@ -29,13 +29,6 @@ def indoor_params():
     p = capi.default_params()
     p.voxel_size, p.normal_radius, p.fpfh_radius, p.noise_bound, p.cote_noise_bound, p.skip_flagged = 0.05, 0.10, 0.15, 0.05, 0.05, 0
     return p
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(torch.cuda.current_device())],
-                       capture_output=True, text=True)
-    name, _, limit = q.stdout.strip().partition(",")
-    return {"name": name.strip() or torch.cuda.get_device_name(), "power_limit": limit.strip() or "unknown"}
 
 
 def main():
@@ -77,8 +70,9 @@ def main():
         if match is None:
             match = h.debug_match_stats()
     rec = out[0]
+    name, _, limit = card().partition(",")   # card() is "unknown" without nvidia-smi: name the device as torch does
     res = {
-        "card": card(),
+        "card": {"name": name.strip() if limit else torch.cuda.get_device_name(), "power_limit": limit.strip() or "unknown"},
         "pair": {"seed": a.seed, "extent": 9.0, "raw": [len(src), len(tgt)]},
         "wall_ms_median": round(float(np.median(wall)), 3),
         "wall_ms": [round(float(x), 3) for x in wall],

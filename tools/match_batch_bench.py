@@ -20,38 +20,17 @@ from __future__ import annotations
 
 import argparse
 import json
-import subprocess
 import sys
-import time
 from pathlib import Path
 
 import numpy as np
+
+from harness import card, timed
 
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 
 MATCHER = ("n_src_vox", "n_tgt_vox", "n_mutual", "n_corr")
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
-    return q.strip().splitlines()[0] if q.strip() else "unknown"
-
-
-def timed(ways, checks, warmup, rounds):
-    """ways: name -> call; checks: name -> check of that call's output (untimed, after every timed run)."""
-    for fn in ways.values():
-        for _ in range(warmup):
-            fn()
-    ms = {k: [] for k in ways}
-    same = {k: True for k in ways}
-    for _ in range(rounds):
-        for name, fn in ways.items():
-            t0 = time.perf_counter()
-            fn()
-            ms[name].append(1e3 * (time.perf_counter() - t0))
-            same[name] &= checks[name]()
-    return {k: {"median": float(np.median(v)), "min": float(min(v)), "max": float(max(v))} for k, v in ms.items()}, same
 
 
 def main():
@@ -119,7 +98,7 @@ def main():
             checks[name] = lambda src=src, name=name: flat(out[name], lbs[name]) == want[src]
     ways["match_loop"] = match_loop
     checks["match_loop"] = lambda: [np.ascontiguousarray(c).tobytes() for c in out["match_loop"]] == want_corr
-    ms, same = timed(ways, checks, a.warmup, a.rounds)
+    ms, same = timed(ways, a.warmup, a.rounds, checks)
 
     rec = out["match_features"]
     rate = {k: 1e3 * n / v["median"] for k, v in ms.items()}

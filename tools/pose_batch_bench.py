@@ -19,20 +19,15 @@ from __future__ import annotations
 
 import argparse
 import json
-import subprocess
 import sys
-import time
 from pathlib import Path
 
 import numpy as np
 
+from harness import card, timed
+
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
-    return q.strip().splitlines()[0] if q.strip() else "unknown"
 
 
 def scene(rng, L, c):
@@ -70,32 +65,28 @@ def workload(h, sets, inliers, p, warmup, rounds):
     def loop():
         state["loop"] = [h.solve_pose(a, b, i, p)[:3] for (a, b), i in zip(sets, inliers)]
 
-    runs = (("batch_host", batch(MEM_HOST)), ("batch_device", batch(MEM_DEVICE)), ("loop", loop))
-    for _ in range(warmup):
-        for _, fn in runs:
-            fn()
-    ms = {name: [] for name, _ in runs}
-    same = True
-    for _ in range(rounds):
-        for name, fn in runs:
-            t0 = time.perf_counter()
-            fn()
-            ms[name].append(1e3 * (time.perf_counter() - t0))
-            if name.startswith("batch"):
-                recs, lists = state["batch"]
-                state["last"] = (recs.copy(), [{k: v.copy() for k, v in d.items()} for d in lists])
+    def keep_batch():
+        recs, lists = state["batch"]
+        state["last"] = (recs.copy(), [{k: v.copy() for k, v in d.items()} for d in lists])
+        return True
+
+    def same():
+        ok = True
         recs, lists = state["last"]
         for r, d, (res, rm, tm) in zip(recs, lists, state["loop"]):
-            same &= r.tobytes() == bytes(res) and d["rot_inlier_mask"].tobytes() == rm.tobytes()
-            same &= d["trans_inlier_mask"].tobytes() == tm.tobytes()
-    out = {k: {"median": float(np.median(v)), "min": float(min(v)), "max": float(max(v))} for k, v in ms.items()}
+            ok &= r.tobytes() == bytes(res) and d["rot_inlier_mask"].tobytes() == rm.tobytes()
+            ok &= d["trans_inlier_mask"].tobytes() == tm.tobytes()
+        return ok
+
+    out, ok = timed({"batch_host": batch(MEM_HOST), "batch_device": batch(MEM_DEVICE), "loop": loop}, warmup, rounds,
+                    {"batch_host": keep_batch, "batch_device": keep_batch, "loop": same})
     for k in ("batch_host", "batch_device"):
         out[k]["speedup"] = out["loop"]["median"] / out[k]["median"]
     out["sets"] = n
     out["inliers_mean"] = float(np.mean([len(i) for i in inliers]))
     out["points_mean"] = float(np.mean([len(a) for a, _ in sets]))
     del keep
-    return out, same
+    return out, ok["loop"]
 
 
 def main():

@@ -10,7 +10,6 @@ the whole chain, next to the single-call chain (loop, then qb200_register_batch 
 against the loop's.  The card's name and power limit are read in the same run."""
 import argparse
 import json
-import subprocess
 import sys
 import time
 from pathlib import Path
@@ -18,13 +17,9 @@ from pathlib import Path
 import numpy as np
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+from harness import card  # noqa: E402
 from quatro_b200 import capi, synth  # noqa: E402
 from quatro_b200.capi import MEM_DEVICE, MEM_HOST, default_patchwork_params, default_segment_params  # noqa: E402
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
 
 
 def loop(h, scans, pp, sp):
@@ -43,7 +38,7 @@ def main():
     pairs = [synth.outdoor_pair(9000 + i)[:2] for i in range(max(a.pairs, 256))]
     scans = [s for pr in pairs for s in pr]
     sizes = [int(x) for x in a.sizes.split(",")]
-    res = {"card": card(), "scan_points_mean": float(np.mean([len(s) for s in scans])), "throughput": {}}
+    res = {"card": card("clocks.max.sm"), "scan_points_mean": float(np.mean([len(s) for s in scans])), "throughput": {}}
     h = capi.Handle()
     cap = sp.n_scan * sp.horizon_scan
     # the batch's output arrays are allocated once and reused, as a caller processing scan after scan would (the loop's small per-call

@@ -13,7 +13,6 @@ import argparse
 import ctypes as C
 import hashlib
 import json
-import subprocess
 import sys
 import time
 from pathlib import Path
@@ -21,13 +20,9 @@ from pathlib import Path
 import numpy as np
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+from harness import card  # noqa: E402
 from quatro_b200 import capi, synth  # noqa: E402
 from quatro_b200.capi import LIDAR_MODELS, MEM_DEVICE, MEM_HOST, PREPROCESS_ARRAYS  # noqa: E402
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
 
 
 class Outputs:
@@ -75,7 +70,7 @@ def main():
     lib = capi.load_library()
     N = a.scans
     models = list(LIDAR_MODELS)
-    res = {"card": card(), "scans": N, "reps": a.reps}
+    res = {"card": card("clocks.max.sm"), "scans": N, "reps": a.reps}
     h = capi.Handle()
 
     def run(fn, scans, pp_arg, sp_arg, out):

@@ -21,33 +21,15 @@ from __future__ import annotations
 import argparse
 import ctypes as C
 import json
-import subprocess
 import sys
-import time
 from pathlib import Path
 
 import numpy as np
 
+from harness import card, timed
+
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
-    return q.strip().splitlines()[0] if q.strip() else "unknown"
-
-
-def timed(ways, warmup, rounds):
-    for fn in ways.values():
-        for _ in range(warmup):
-            fn()
-    ms = {k: [] for k in ways}
-    for _ in range(rounds):
-        for name, fn in ways.items():
-            t0 = time.perf_counter()
-            fn()
-            ms[name].append(1e3 * (time.perf_counter() - t0))
-    return {k: {"median": float(np.median(v)), "min": float(min(v)), "max": float(max(v))} for k, v in ms.items()}
 
 
 def main():
@@ -102,7 +84,7 @@ def main():
         "describe_dd": batch("describe_dd", "qb200_describe_batch_each", MEM_DEVICE, MEM_DEVICE),
         "stage_loop": stage_loop,
     }
-    ms = timed(ways, a.warmup, a.rounds)
+    ms, _ = timed(ways, a.warmup, a.rounds)
 
     # every schedule's bytes, scan by scan, against the per-scan loop
     want = [v.tobytes() for v, _ in out["stage_loop"]]

@@ -18,24 +18,17 @@ Nothing is written to disk.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from harness import card  # noqa: E402
 from quatro_b200 import capi, synth  # noqa: E402
 
 STAGES = ["h2d", "voxel", "fpfh", "match", "graph", "clique", "pose", "d2h"]
 KEYS = ["n_src_vox", "n_tgt_vox", "n_mutual", "n_corr", "n_edges", "max_core", "clique_size", "valid", "status"]
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(torch.cuda.current_device())],
-                       capture_output=True, text=True)
-    name, _, limit = q.stdout.strip().partition(",")
-    return {"name": name.strip() or torch.cuda.get_device_name(), "power_limit": limit.strip() or "unknown"}
 
 
 def time_set(h, a4, b4, p, reps):
@@ -65,7 +58,9 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("wide_corr_bench: no CUDA device (the measurement has no CPU fallback)")
     torch.cuda.init()
-    res = {"card": card(), "reps": a.reps}
+    name, _, limit = card().partition(",")   # card() is "unknown" without nvidia-smi: name the device as torch does
+    res = {"card": {"name": name.strip() if limit else torch.cuda.get_device_name(), "power_limit": limit.strip() or "unknown"},
+           "reps": a.reps}
     p = capi.default_params()
     sets = {(L, r): synth.matched_pairs(L + int(100 * r), L, inlier_ratio=r, noise=0.05)[:2] for L in (8192, 16384, 32768) for r in (0.05, 0.5)}
     with capi.Handle(max_batch_slots=1, max_corr=32768) as h:
