@@ -306,7 +306,9 @@ int qb200_build_graph(qb200_handle* h, const float* a4, const float* b4, int32_t
                       double noise_bound, double cbar2, uint32_t* adj, int32_t words_per_row,
                       int32_t* degree, int64_t* n_edges);
 
-/* clique: ascending vertex ids.  kcore (L, pmc's core number + 1) and kcore_order (L) may be NULL. */
+/* clique: ascending vertex ids.  kcore (L, pmc's core number + 1) and kcore_order (L) may be NULL.  Bits at columns >= L of adj
+ * (the last used word's high bits and any padding words) are ignored.  QB200_KCORE_HEU compares max_core with
+ * (int)(kcore_heuristic_threshold * L) as x86-64 computes that cast: INT_MIN for NaN and for products outside int range. */
 int qb200_max_clique(qb200_handle* h, const uint32_t* adj, int32_t L, int32_t words_per_row,
                      int32_t mode, double kcore_heuristic_threshold, int32_t* clique, int32_t* n_clique,
                      int32_t* kcore, int32_t* kcore_order, int32_t* max_core);

@@ -34,6 +34,8 @@
 //   D10 VoxelGrid refuses a cloud (QB200_ERR_VOXEL_OVERFLOW, input returned unfiltered) not only on PCL's own check
 //      (truncated spans dx*dy*dz > INT_MAX) but wherever PCL's int arithmetic would overflow (UB, wraps in practice): a kept
 //      point's floor(p * inv) outside int32, or a product of the floor-based div_b above INT_MAX
+//   D18 KCORE_HEU limit (int)(kcore_heuristic_threshold * n) (src/graph.cc:69-70): undefined for NaN and out-of-range products; both
+//      sides compute what x86-64's cvttsd2si gives, INT_MIN, through qb_kcore_heu_limit (quatro_b200/csrc/kcore_cutoff.cuh)
 // =====================================================================================
 #include <algorithm>
 #include <cfloat>
@@ -53,6 +55,7 @@
 
 #include "../include/quatro_b200.h"
 #include "qo_math.h"
+#include "../quatro_b200/csrc/kcore_cutoff.cuh"
 
 namespace {
 
@@ -853,7 +856,7 @@ int max_clique(const uint32_t* adj, int L, int wpr, int mode, double kcore_thr, 
   if (flags_out) *flags_out = 0;
   const Csr g = to_csr(adj, L, wpr);
   compute_cores(g, kcore, order, max_core);
-  if (mode == QB200_KCORE_HEU && kcore_thr != 1 && max_core > (int)(kcore_thr * (double)L)) {  // graph.cc:67-82
+  if (mode == QB200_KCORE_HEU && qb_kcore_heu_shortcut(kcore_thr, L, max_core)) {  // graph.cc:67-82 (D18: the int cast as x86-64)
     for (int v = 0; v < L; ++v)
       if (kcore[v] >= max_core) clique.push_back(v);   // literal: k_cores[i] (= core+1) >= max_core
     return QB200_OK;

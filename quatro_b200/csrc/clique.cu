@@ -28,6 +28,7 @@
 //     are renumbered by (kcore, id) rank (permute_adj_kernel), so "largest (kcore,id) candidate" is the highest set
 //     bit of P and a descent step is one multi-word AND.
 #include "handle.cuh"
+#include "kcore_cutoff.cuh"
 
 namespace qb {
 
@@ -469,7 +470,7 @@ __global__ void __launch_bounds__(kCliqueWarps * 32) clique_cta_kernel(const uin
   const int nwl = (nbw + 31) >> 5;
   for (int w = tid; w < W; w += NT) idbits[w] = 0;
 
-  if (mode == QB200_KCORE_HEU && kcore_thr != 1.0 && max_core > (int)(kcore_thr * (double)L)) {
+  if (mode == QB200_KCORE_HEU && qb_kcore_heu_shortcut(kcore_thr, L, max_core)) {
     // src/graph.cc:67-82: keep every vertex whose k_cores entry (core + 1) is >= max_core
     __syncthreads();
     for (int v = tid; v < L; v += NT)

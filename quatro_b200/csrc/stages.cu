@@ -226,7 +226,12 @@ int qb200_max_clique_ex(qb200_handle* h, const uint32_t* adj, int32_t L, int32_t
   ln->h_solve[0].mode = mode;
   ln->h_solve[0].kcore_thr = kcore_thr;
   ln->h_solve[0].node_limit = node_limit > 0 ? node_limit : (long long)QB200_DEFAULT_CLIQUE_NODE_LIMIT;
-  if ((rc = write_counter(ln, ln->hctr.n_corr, L)) || (rc = upload_solve(ln, 1)) || (rc = launch_degree(ln, 1))) return rc;
+  // the rows just copied, masked in place like a batch graph's host rows: bits at columns >= L are ignored
+  ln->h_graph[0] = GraphSrc{nullptr, ln->adj, 0, L, ln->W};
+  QB_CUDA_TRY(h, cudaMemcpyAsync(ln->d_graph, ln->h_graph, sizeof(GraphSrc), cudaMemcpyHostToDevice, ln->stream));
+  if ((rc = write_counter(ln, ln->hctr.n_corr, L)) || (rc = upload_solve(ln, 1)) || (rc = launch_row_import(ln, 1, L)) ||
+      (rc = launch_degree(ln, 1)))
+    return rc;
   if ((rc = launch_clique(ln, 1, mode == QB200_PMC_EXACT)) || (rc = read_counters(ln))) return rc;
   QB_CUDA_TRY(h, hold.sync());
   const int nc = ln->hctr.n_clique[0];

@@ -2,9 +2,10 @@
 computePairFeatures, FPFHEstimation; FLANN exact 1-NN as brute force; the fp64 TIM mask of quatro.hpp:363-385), written from the
 published algorithms, and a float32 restatement of the matcher's back half (feature_matcher.cc:18-76 and :187-264: the swap rule,
 normalizePoints' mean, the tuple test with the counter-based Philox4x32-10 of deviation D1 in place of rand(), swap back, sort and
-unique).  This module never imports oracle/ or the CUDA library: tools/gen_independent_pins.py uses it to write the
-independent_*.npz fixtures, tests/test_independent_pins.py uses it to check the oracle and tests/test_tuple_adversarial.py to check
-the oracle and the device matcher."""
+unique), and a list-and-set restatement of pmc's k-core peel and heuristic, findMaxClique and the canonical exact search (src/graph.cc:
+12-130).  This module never imports oracle/ or the CUDA library: tools/gen_independent_pins.py uses it to write the
+independent_*.npz fixtures, tests/test_independent_pins.py uses it to check the oracle, tests/test_tuple_adversarial.py to check
+the oracle and the device matcher, and tests/test_clique_adversarial.py the oracle and K9."""
 import numpy as np
 from scipy.spatial import cKDTree
 
@@ -272,3 +273,250 @@ def tuple_match(src, tgt, mutual, use_tuple_test=1, tuple_scale=0.95, trials_per
         corres = corres[:, ::-1]
     out["corr"] = np.unique(corres, axis=0).astype(np.int32).reshape(-1, 2)
     return out
+
+
+# ---- K9: pmc's k-core peel and heuristic, findMaxClique (src/graph.cc:12-130) and the canonical exact search -------------------------
+# Plain lists and sets, written from the reference text and pmc's published algorithms (Rossi, Gleich, Gebremedhin, "Parallel maximum
+# clique algorithms with applications to network analysis", SIAM J. Sci. Comput. 37(5), 2015; Batagelj and Zaversnik, "An O(m)
+# algorithm for cores decomposition of networks", 2003).  A graph is (L, nbrs): nbrs[v] = neighbours of v in ascending id, the order
+# in which graph.cc:24-29 hands pmc its CSR rows.
+KCORE_HEU_MODE, PMC_HEU_MODE, PMC_EXACT_MODE = 2, 1, 0
+CLIQUE_TRUNCATED = 1
+
+
+def pmc_cores(L, nbrs):
+    """pmc_graph::compute_cores (Batagelj-Zaversnik with pmc's bucket mechanic): vertices sit in `vert`, grouped by current degree,
+    ids ascending inside a bin; peeling v decrements every neighbour u with deg[u] > deg[v] by swapping u with the FIRST vertex of
+    u's bin and advancing that bin's start.  Returns (kcore = core + 1 per vertex (pmc's K), peel order, max core)."""
+    deg = [len(nbrs[v]) for v in range(L)]
+    if L == 0:
+        return [], [], 0
+    md = max(deg)
+    bin_start = [0] * (md + 1)
+    for d in deg:
+        bin_start[d] += 1
+    start = 0
+    for d in range(md + 1):                 # bin_start[d] = first position of degree d
+        bin_start[d], start = start, start + bin_start[d]
+    pos, vert = [0] * L, [0] * L
+    fill = list(bin_start)
+    for v in range(L):                      # ids ascending inside a bin
+        pos[v] = fill[deg[v]]
+        vert[pos[v]] = v
+        fill[deg[v]] += 1
+    for i in range(L):
+        v = vert[i]
+        for u in nbrs[v]:
+            if deg[u] > deg[v]:
+                du, pu = deg[u], pos[u]
+                pw = bin_start[du]
+                w = vert[pw]
+                if u != w:                  # u changes places with the first vertex of its bin
+                    pos[u], vert[pu], pos[w], vert[pw] = pw, w, pu, u
+                bin_start[du] += 1
+                deg[u] -= 1
+    return [d + 1 for d in deg], vert, deg[vert[L - 1]]
+
+
+def pmc_heu(L, nbrs, K, order, ub, trace=None):
+    """pmc_heu::search with heu_strat = "kcore" (graph.cc:89-91), start vertices sequential in reverse peel order (oracle D4):
+    skip v when K[v] <= mc; P = neighbours u with K[u] > mc, skipped when |P| <= mc; P sorted stably by K (D3), so popping its back
+    takes the largest (K, id); each step keeps the P members adjacent to the popped vertex with K > mc; a chain longer than mc
+    replaces the incumbent; stop once mc >= ub.  Returns (mc, clique in push order); a list `trace` receives (peel position, new mc)
+    of every improvement."""
+    mc, best = 0, []
+    for i in range(L - 1, -1, -1):
+        if mc >= ub:
+            break
+        v = order[i]
+        if K[v] <= mc:
+            continue
+        P = [u for u in nbrs[v] if K[u] > mc]
+        if len(P) <= mc:
+            continue
+        P.sort(key=lambda u: K[u])          # list.sort is stable: ids stay ascending inside one K
+        popped = []
+        while P:
+            u = P.pop()
+            popped.append(u)
+            nu = set(nbrs[u])
+            P = [w for w in P if w in nu and K[w] > mc]
+        if len(popped) + 1 > mc:
+            mc = len(popped) + 1
+            best = popped[::-1] + [v]
+            if trace is not None:
+                trace.append((i, mc))
+    return mc, best
+
+
+def kcore_heu_limit(thr, L):
+    """(int)(thr * L) as x86-64's cvttsd2si computes it (the reference's only platform): the product truncated toward zero when that
+    fits in int32, INT_MIN for NaN, infinities and every product outside int range."""
+    x = float(thr) * float(L)
+    if x != x or not (-2147483649.0 < x < 2147483648.0):
+        return -2 ** 31
+    return int(x)
+
+
+def rank_space(L, K):
+    """vertices renumbered by (core number, id) ascending: (rank_of, by_rank, first[c] = first rank whose core number >= c)"""
+    by_rank = sorted(range(L), key=lambda v: (K[v], v))
+    rank_of = [0] * L
+    for r, v in enumerate(by_rank):
+        rank_of[v] = r
+    return rank_of, by_rank
+
+
+def canonical_exact(L, nbrs, K, max_core, incumbent, node_limit, depth_limit=None, pool_limit=None):
+    """The canonical branch and bound of DESIGN.md 5.3 / quatro_b200.h (qb200_max_clique_ex), in (core, id) rank space: root
+    candidates = vertices with core number >= |incumbent|; greedy sequential colouring, each class taking the lowest-ranked candidate
+    with no neighbour in it, listing only entries with colour > |incumbent| - |C|, in (colour, rank) order; the branch takes the list's
+    last entry; a level dies when |C| + colour <= |incumbent|; a strictly larger maximal clique replaces the incumbent and the search
+    ends when it reaches max_core + 1; every expanded node counts (++nodes > node_limit stops with the truncation flag).
+    depth_limit / pool_limit add the device's scratch limits: expanding to depth depth_limit, or a colour list that would need more
+    pool entries than pool_limit minus the entries of the lists on the current path (the consumed entry's slot passes to the child
+    level), stops the search like the node limit.  Returns (clique sorted, flags, nodes, stop): stop is None for a search that ran
+    out, else a dict of what ended it ("nodes", "depth" or "pool"), the depth of the node being expanded and the pool entries the
+    lists on the path held (for "pool": before the list that did not fit)."""
+    best = len(incumbent)
+    ub = max_core + 1
+    if L <= 0 or best <= 0 or best >= ub:
+        return sorted(incumbent), 0, 0, None
+    rank_of, by_rank = rank_space(L, K)
+    adj = [set() for _ in range(L)]
+    for v in range(L):
+        adj[rank_of[v]] = {rank_of[u] for u in nbrs[v]}
+    pool_cap = pool_limit if pool_limit is not None else float("inf")
+
+    def colour_sort(P, kmin, cap):
+        """the (rank, colour) list of P, or None when it needs more than cap entries"""
+        left = set(P)
+        out, col = [], 0
+        while left:
+            col += 1
+            free = left - adj[min(left)]    # candidates with no neighbour in the class so far (its first member included)
+            while free:
+                v = min(free)
+                free -= adj[v]
+                free.discard(v)
+                left.discard(v)
+                if col > kmin:
+                    if len(out) >= cap:
+                        return None
+                    out.append((v, col))
+        return out
+
+    core = [K[by_rank[r]] - 1 for r in range(L)]
+    root = {r for r in range(L) if core[r] >= min(best, max_core + 1)}
+    flags, nodes, best_c, stop = 0, 0, None, None
+    lst = colour_sort(root, best, pool_cap)
+    if lst is None:
+        return sorted(incumbent), CLIQUE_TRUNCATED, 0, dict(reason="pool", depth=0, pool=0)
+    stack = [[root, lst, 0]]                # per level: candidates, colour list, first pool slot of the list
+    C = []
+    while stack:
+        depth = len(stack) - 1
+        P, lst, begin = stack[-1]
+        if not lst:
+            stack.pop()
+            continue
+        v, col = lst.pop()
+        if depth + col <= best:
+            lst.clear()
+            continue
+        del C[depth:]
+        C.append(v)
+        NP = P & adj[v]
+        P.discard(v)
+        if not NP:
+            if depth + 1 > best:
+                best, best_c = depth + 1, list(C)
+                if best >= ub:
+                    break
+            continue
+        if depth + 1 + len(NP) <= best:
+            continue
+        nodes += 1
+        nbegin = begin + len(lst)           # the consumed entry's slot and everything after it is free again
+        if nodes > node_limit or (depth_limit is not None and depth + 1 >= depth_limit):
+            flags, stop = CLIQUE_TRUNCATED, dict(reason="nodes" if nodes > node_limit else "depth", depth=depth, pool=nbegin)
+            break
+        child = colour_sort(NP, best - (depth + 1), pool_cap - nbegin)
+        if child is None:
+            flags, stop = CLIQUE_TRUNCATED, dict(reason="pool", depth=depth, pool=nbegin)
+            break
+        stack.append([set(NP), child, nbegin])
+    clique = sorted(by_rank[r] for r in best_c) if best_c is not None else sorted(incumbent)
+    return clique, flags, nodes, stop
+
+
+def find_max_clique(L, nbrs, mode, thr=0.5, node_limit=262144, depth_limit=None, pool_limit=None):
+    """teaser::MaxCliqueSolver::findMaxClique (src/graph.cc:12-130) with the exact search in its canonical form.  Returns a dict:
+    kcore, order, max_core, clique (ascending ids, quatro.hpp:806), flags, heu (the heuristic's size), nodes and stop (canonical_exact)."""
+    K, order, max_core = pmc_cores(L, nbrs)
+    out = dict(kcore=K, order=order, max_core=max_core, flags=0, nodes=0, heu=0, stop=None)
+    # graph.cc:67-82: the literal k_cores >= max_core (K = core + 1), != 1 short-circuits the comparison
+    if mode == KCORE_HEU_MODE and thr != 1 and max_core > kcore_heu_limit(thr, L):
+        out["clique"] = [v for v in range(L) if K[v] >= max_core]
+        return out
+    ub = max_core + 1                       # graph.cc:84-86
+    lb, C = pmc_heu(L, nbrs, K, order, ub)  # graph.cc:89-91
+    out["heu"] = lb
+    if lb == 0 or lb == ub or mode != PMC_EXACT_MODE:   # graph.cc:93-104
+        out["clique"] = sorted(C)
+        return out
+    out["clique"], out["flags"], out["nodes"], out["stop"] = canonical_exact(L, nbrs, K, max_core, C, node_limit, depth_limit, pool_limit)
+    return out
+
+
+# ---- one peel step's bucket moves: pmc's swap sequence and the closed form of kcore_apply_moves (clique.cu) ---------------------------
+def group_moves_sequential(vert, pos, bin_start, deg, nbl):
+    """One peel step as pmc runs it: for each neighbour u of the list in order, swap u with the vertex on the first slot of its bin,
+    advance that bin and decrement deg[u].  Returns new (vert, pos, bin_start, deg); bin_start is a dict degree -> first slot."""
+    vert, pos, bin_start, deg = list(vert), dict(pos), dict(bin_start), dict(deg)
+    for u in nbl:
+        du, pu = deg[u], pos[u]
+        pw = bin_start[du]
+        w = vert[pw]
+        pos[u], vert[pu], pos[w], vert[pw] = pw, w, pu, u
+        bin_start[du] += 1
+        deg[u] -= 1
+    return vert, pos, bin_start, deg
+
+
+def group_moves_closed_form(vert, pos, bin_start, deg, nbl, chunk=32):
+    """The same step as kcore_apply_moves computes it: the list in chunks of 32 lanes; inside a chunk the lanes of one current degree
+    form a group (__match_any_sync) and lane rank t of a group of m lands on slot bin + t; a member that sat outside the m target
+    slots walks the chain slot -> member that sat there -> its rank's slot ... backwards from its own rank until it reaches a
+    non-member, which takes the member's old slot; rank 0 advances the bin by m after the chunk.  Every lane reads the state the
+    chunk started from."""
+    vert, pos, bin_start, deg = list(vert), dict(pos), dict(bin_start), dict(deg)
+    for c0 in range(0, len(nbl), chunk):
+        lanes = nbl[c0:c0 + chunk]
+        du = [deg[u] for u in lanes]
+        rank = [sum(1 for j in range(i) if du[j] == du[i]) for i in range(len(lanes))]
+        m = [du.count(d) for d in du]
+        b0 = [bin_start[d] for d in du]
+        pu = [pos[u] for u in lanes]
+        mrk = {u: rank[i] + 1 for i, u in enumerate(lanes)}
+        ys = []
+        for i in range(len(lanes)):
+            y = None
+            if pu[i] >= b0[i] + m[i]:
+                k = rank[i]
+                while True:
+                    y = vert[b0[i] + k]
+                    if y not in mrk:
+                        break
+                    k = mrk[y] - 1
+            ys.append(y)
+        for i, u in enumerate(lanes):
+            vert[b0[i] + rank[i]] = u
+            pos[u] = b0[i] + rank[i]
+            if ys[i] is not None:
+                vert[pu[i]] = ys[i]
+                pos[ys[i]] = pu[i]
+            deg[u] = du[i] - 1
+            if rank[i] == 0:
+                bin_start[du[i]] = b0[i] + m[i]
+    return vert, pos, bin_start, deg
