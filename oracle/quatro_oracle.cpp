@@ -36,6 +36,9 @@
 //      point's floor(p * inv) outside int32, or a product of the floor-based div_b above INT_MAX
 //   D18 KCORE_HEU limit (int)(kcore_heuristic_threshold * n) (src/graph.cc:69-70): undefined for NaN and out-of-range products; both
 //      sides compute what x86-64's cvttsd2si gives, INT_MIN, through qb_kcore_heu_limit (quatro_b200/csrc/kcore_cutoff.cuh)
+//   D19 radii are float32 (qb200_params, qb200_compute_fpfh): the squared radius is float(double(r) * double(r)) of the float radius,
+//      which equals float(r * r); PCL receives the reference's radii as doubles, and for 0.1 or 1/3 the float of the double square is
+//      one ulp lower, so a neighbour at exactly that d2 is kept here and dropped by PCL (tests/test_fpfh_adversarial.py)
 // =====================================================================================
 #include <algorithm>
 #include <cfloat>

@@ -5,7 +5,8 @@ normalizePoints' mean, the tuple test with the counter-based Philox4x32-10 of de
 unique), and a list-and-set restatement of pmc's k-core peel and heuristic, findMaxClique and the canonical exact search (src/graph.cc:
 12-130).  This module never imports oracle/ or the CUDA library: tools/gen_independent_pins.py uses it to write the
 independent_*.npz fixtures, tests/test_independent_pins.py uses it to check the oracle, tests/test_tuple_adversarial.py to check
-the oracle and the device matcher, and tests/test_clique_adversarial.py the oracle and K9."""
+the oracle and the device matcher, tests/test_clique_adversarial.py the oracle and K9, and tests/test_fpfh_adversarial.py the
+oracle's and the device's normals, SPFH and FPFH against the float32 restatement of PCL's NormalEstimation / FPFHEstimation below."""
 import numpy as np
 from scipy.spatial import cKDTree
 
@@ -520,3 +521,442 @@ def group_moves_closed_form(vert, pos, bin_start, deg, nbl, chunk=32):
             if rank[i] == 0:
                 bin_start[du[i]] = b0[i] + m[i]
     return vert, pos, bin_start, deg
+
+
+# ---- float32 restatement of PCL 1.8.1 NormalEstimation / FPFHEstimation over FLANN's radius search (src/teaser_utils/fpfh.cc:44-75) ----
+# Written from the PCL and FLANN texts: KdTreeFLANN::radiusSearch -> flann::L2_Simple<float> with RadiusResultSet's strict '<';
+# computeMeanAndCovarianceMatrix (single pass), eigen33 / computeRoots / computeRoots2, solvePlaneParameters, flipNormalTowardsViewpoint;
+# computePairFeatures, computePointSPFHSignature, weightPointSPFHSignature.  Every float32 operation is one numpy float32 operation in
+# the source's left-to-right order.  The transcendentals are a parameter: F64_MATH (float64 functions rounded once to float32, the
+# plain reading of PCL) or D7_MATH (numpy float32 copies of the project's fixed-order polynomials, deviation D7).  The neighbour
+# accumulation order is deviation D8's ascending (lattice cell key, index) from DESIGN section 2 (iv).
+F32, F64 = np.float32, np.float64
+FLT_EPSILON = F32(np.finfo(np.float32).eps)
+FLT_MIN = F32(np.finfo(np.float32).tiny)
+U32 = 2.0 ** -24                      # float32 unit roundoff
+CELL_FACTOR = F32(1.001953125)        # default lattice cell = (1 + 2^-9) * fpfh_radius (D8)
+_OFF_IJ, _OFF_K = 1 << 17, 1 << 15
+
+
+class Math:
+    """atan2(y, x), acos(x), sincos(x) -> (sin, cos) on float32 arrays or scalars, returning float32."""
+
+    def __init__(self, name, atan2, acos, sincos):
+        self.name, self.atan2, self.acos, self.sincos = name, atan2, acos, sincos
+
+
+def _f64_atan2(y, x):
+    r = np.arctan2(np.asarray(y, F64), np.asarray(x, F64))
+    return F32(r) if np.ndim(r) == 0 else r.astype(F32)
+
+
+def _f64_acos(x):
+    with np.errstate(invalid="ignore"):
+        r = np.arccos(np.asarray(x, F64))
+    return F32(r) if np.ndim(x) == 0 else r.astype(F32)
+
+
+def _f64_sincos(x):
+    x = np.asarray(x, F64)
+    s, c = np.sin(x).astype(F32), np.cos(x).astype(F32)
+    return (F32(s), F32(c)) if np.ndim(x) == 0 else (s, c)
+
+
+F64_MATH = Math("float64", _f64_atan2, _f64_acos, _f64_sincos)
+
+# D7's kernels (quatro_b200/csrc/qb_math.cuh, coefficients from tools/fit_math.py), each line one float32 operation
+_ATAN_C = [F32(c) for c in ("-4.044491798e-02", "7.135856152e-02", "-9.029050916e-02", "1.110749617e-01", "-1.428561211e-01",
+                            "1.999999881e-01", "-3.333333433e-01")]
+_ASIN_C = [F32(c) for c in ("3.109041601e-02", "1.048902422e-02", "2.363533154e-02", "3.026617132e-02", "4.464783147e-02",
+                            "7.499992102e-02", "1.666666716e-01")]
+_SIN_C = [F32(c) for c in ("1.469172284e-10", "-2.501203333e-08", "2.755685500e-06", "-1.984126720e-04", "8.333333768e-03",
+                           "-1.666666716e-01")]
+_COS_C = [F32(c) for c in ("3.323700412e-06", "-1.105757929e-05", "1.310664993e-05", "1.771735151e-05", "-1.387358177e-03",
+                           "4.166657478e-02")]
+PI_F, PI_2_F, PI_4_F = F32("3.14159274"), F32("1.57079637"), F32("0.785398185")
+
+
+def _horner(c, z):
+    p = np.full(np.shape(z), c[0], F32)
+    for k in c[1:]:
+        p = p * z + k
+    return p
+
+
+def _d7_atan2(y, x):
+    scalar = np.ndim(y) == 0 and np.ndim(x) == 0
+    y, x = np.atleast_1d(np.asarray(y, F32)), np.atleast_1d(np.asarray(x, F32))
+    y, x = np.broadcast_arrays(y, x)
+    with np.errstate(all="ignore"):
+        ax, ay = np.abs(x), np.abs(y)
+        hi, lo = np.where(ax > ay, ax, ay), np.where(ax > ay, ay, ax)
+        a = np.where(hi == np.inf, np.where(lo == np.inf, F32(1), F32(0)), lo / hi).astype(F32)
+        big = a > F32(0.41421357)
+        t = np.where(big, (a - F32(1)) / (a + F32(1)), a).astype(F32)
+        z = t * t
+        core = t + t * (z * _horner(_ATAN_C, z))
+        r = np.where(big, PI_4_F, F32(0)).astype(F32) + core
+        r = np.where(ay > ax, PI_2_F - r, r)
+        r = np.where((ax == 0) & (ay == 0), F32(0), r)
+        r = np.where(np.signbit(x), PI_F - r, r)
+        r = np.where(np.signbit(y), -r, r)
+        r = np.where(np.isnan(x) | np.isnan(y), F32(np.nan), r).astype(F32)
+    return r[0] if scalar else r
+
+
+def _d7_acos(x):
+    scalar = np.ndim(x) == 0
+    x = np.atleast_1d(np.asarray(x, F32))
+    with np.errstate(all="ignore"):
+        ax = np.abs(x)
+        z1 = ax * ax
+        r1 = PI_2_F - (ax + ax * (z1 * _horner(_ASIN_C, z1)))
+        z2 = (F32(1) - ax) * F32(0.5)
+        s = np.sqrt(z2)
+        r2 = F32(2) * (s + s * (z2 * _horner(_ASIN_C, z2)))
+        r = np.where(ax <= F32(0.5), r1, r2)
+        r = np.where(x < 0, PI_F - r, r)
+        r = np.where(np.isnan(x) | (ax > F32(1)), F32(np.nan), r).astype(F32)
+    return r[0] if scalar else r
+
+
+def _d7_sincos(x):
+    scalar = np.ndim(x) == 0
+    x = np.atleast_1d(np.asarray(x, F32))
+    z = x * x
+    s = x + x * (z * _horner(_SIN_C, z))
+    c = (F32(1) - F32(0.5) * z) + (z * z) * _horner(_COS_C, z)
+    return (s[0], c[0]) if scalar else (s, c)
+
+
+D7_MATH = Math("D7", _d7_atan2, _d7_acos, _d7_sincos)
+
+
+def flann_radius(pts, q, r):
+    """FLANN's radius search as PCL's KdTreeFLANN runs it: diff = query - point in float32, d2 = ((0 + dx*dx) + dy*dy) + dz*dz in
+    float32 (L2_Simple<float>), kept when d2 < float(double(r) * double(r)) (RadiusResultSet, strict; radius_sq).  The query is its own
+    neighbour.  Returns (mask over pts, d2 of every point)."""
+    p = np.asarray(pts, F32)[:, :3]
+    with np.errstate(all="ignore"):
+        d = p[q] - p
+        d2 = ((F32(0) + d[:, 0] * d[:, 0]) + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2]
+        return d2 < radius_sq(r), d2
+
+
+def radius_sq(r):
+    """KdTreeFLANN's squared radius, float(double(r) * double(r)).  PCL takes r as a double; the C-ABI takes a float32 radius
+    (deviation D19), and callers that restate the library pass float32(r)."""
+    return F32(F64(r) * F64(r))
+
+
+def lattice_rank(pts, cell):
+    """D8's canonical order: every point's rank in ascending (cell key, index), and whether it is in the lattice (finite, cell
+    (floor(x / cell), ...) with |i|, |j| < 2^17 and |k| < 2^15, the top cell of each range reserved; DESIGN section 2 (iv)).  The cell
+    coordinates are floor(p * (1 / cell)) in float32; key = (k + 2^15) << 36 | (j + 2^17) << 18 | (i + 2^17)."""
+    p = np.asarray(pts, F32)[:, :3]
+    inv = F32(1) / F32(cell)
+    with np.errstate(all="ignore"):
+        c = np.floor(p * inv)
+    ok = np.isfinite(p).all(1) & (c[:, 0] >= -_OFF_IJ) & (c[:, 0] < _OFF_IJ - 1) & (c[:, 1] >= -_OFF_IJ) & (c[:, 1] < _OFF_IJ - 1) \
+        & (c[:, 2] >= -_OFF_K) & (c[:, 2] < _OFF_K - 1)
+    ci = np.where(ok[:, None], c, 0).astype(np.int64)
+    key = ((ci[:, 2] + _OFF_K) << 36) | ((ci[:, 1] + _OFF_IJ) << 18) | (ci[:, 0] + _OFF_IJ)
+    order = np.lexsort((np.arange(len(p)), key))
+    rank = np.empty(len(p), np.int64)
+    rank[order] = np.arange(len(p))
+    return rank, ok
+
+
+def canonical_neighbours(pts, q, r, rank, in_lattice):
+    """q's radius neighbours (flann_radius) in D8 order, and their d2; none for a query outside the lattice."""
+    if not in_lattice[q]:
+        return np.zeros(0, np.int64), np.zeros(0, F32)
+    m, d2 = flann_radius(pts, q, r)
+    idx = np.flatnonzero(m & in_lattice)
+    idx = idx[np.argsort(rank[idx])]
+    return idx, d2[idx]
+
+
+def _compute_roots2(b, c):
+    d = F32(F64(b * b) - 4.0 * F64(c))
+    if d < 0:
+        d = F32(0)
+    sd = np.sqrt(d)
+    return [F32(0), F32(0.5) * (b - sd), F32(0.5) * (b + sd)]
+
+
+def _cross(a, b):
+    return [a[1] * b[2] - a[2] * b[1], a[2] * b[0] - a[0] * b[2], a[0] * b[1] - a[1] * b[0]]
+
+
+def _dot(a, b):
+    return (a[0] * b[0] + a[1] * b[1]) + a[2] * b[2]
+
+
+def normal_pcl32(nb, query, math):
+    """computePointNormal of one query over its neighbour points nb ((k, 3) float32, accumulation order): fewer than 3 -> NaN;
+    computeMeanAndCovarianceMatrix (float32 sums from 0, accu /= k, cov = accu[i] - accu[a] * accu[b]); eigen33 (scale = the largest
+    |coefficient|, 1 when that is <= FLT_MIN; computeRoots, the row cross products, the largest squared norm with '>=' ties to the
+    first); curvature |l0 / trace| (0 for a zero trace); the flip (vp - p) . n < 0 with the viewpoint at the origin.
+    Returns ((nx, ny, nz, curvature) float32, record): the record holds the float32 covariance, every decision's operands, and each
+    transcendental-dependent decision's margin over the error a change of <= 3 ulp in atan2 / sin / cos can cause (ratio > 1 clears)."""
+    nan4 = np.full(4, np.nan, F32)
+    rec = dict(k=len(nb), branch="few", margins={})
+    if len(nb) < 3:
+        return nan4, rec
+    nb = np.asarray(nb, F32)
+    x, y, z = nb[:, 0], nb[:, 1], nb[:, 2]
+    terms = np.stack([x * x, x * y, x * z, y * y, y * z, z * z, x, y, z], 1)
+    accu = np.add.accumulate(np.concatenate([np.zeros((1, 9), F32), terms]), axis=0, dtype=F32)[-1]
+    accu = accu / F32(len(nb))
+    cov = np.zeros(9, F32)
+    cov[0] = accu[0] - accu[6] * accu[6]
+    cov[1] = accu[1] - accu[6] * accu[7]
+    cov[2] = accu[2] - accu[6] * accu[8]
+    cov[4] = accu[3] - accu[7] * accu[7]
+    cov[5] = accu[4] - accu[7] * accu[8]
+    cov[8] = accu[5] - accu[8] * accu[8]
+    cov[3], cov[6], cov[7] = cov[1], cov[2], cov[5]
+    rec["cov"] = cov.reshape(3, 3).copy()
+    # eigen33
+    scale = F32(0)
+    for a in np.abs(cov):
+        scale = a if scale < a else scale
+    rec["scale_reset"] = not (scale > FLT_MIN)
+    if rec["scale_reset"]:
+        scale = F32(1)
+    s = [cov[i] / scale for i in range(9)]
+    m00, m01, m02, m11, m12, m22 = s[0], s[1], s[2], s[4], s[5], s[8]
+    c0 = m00 * m11 * m22 + F32(2) * m01 * m02 * m12 - m00 * m12 * m12 - m11 * m02 * m02 - m22 * m01 * m01
+    c1 = m00 * m11 - m01 * m01 + m00 * m22 - m02 * m02 + m11 * m22 - m12 * m12
+    c2 = m00 + m11 + m22
+    rec.update(c0=c0, c1=c1, c2=c2)
+    err_r = 0.0                                         # bound on the roots' change under a 3-ulp change of atan2 / sin / cos
+    if np.abs(c0) < FLT_EPSILON:
+        rec["branch"] = "roots2"
+        roots = _compute_roots2(c2, c1)
+    else:
+        rec["branch"] = "cubic"
+        s_inv3, s_sqrt3 = F32(1.0 / 3.0), np.sqrt(F32(3))
+        c2_over_3 = c2 * s_inv3
+        a_over_3 = (c1 - c2 * c2_over_3) * s_inv3
+        rec["a_over_3"] = a_over_3
+        if a_over_3 > 0:
+            a_over_3 = F32(0)
+        half_b = F32(0.5) * (c0 + c2_over_3 * (F32(2) * c2_over_3 * c2_over_3 - c1))
+        q = half_b * half_b + a_over_3 * a_over_3 * a_over_3
+        rec["q"] = q
+        if q > 0:
+            q = F32(0)
+        rho = np.sqrt(-a_over_3)
+        theta = math.atan2(np.sqrt(-q), half_b) * s_inv3
+        sin_t, cos_t = math.sincos(theta)
+        roots = [c2_over_3 + F32(2) * rho * cos_t, c2_over_3 - rho * (cos_t + s_sqrt3 * sin_t),
+                 c2_over_3 - rho * (cos_t - s_sqrt3 * sin_t)]
+        rec["roots_cubic"] = list(roots)
+        err_r = 16 * U32 * (abs(float(c2_over_3)) + 4 * float(rho))
+        gaps = []
+        if roots[0] >= roots[1]:
+            roots[0], roots[1] = roots[1], roots[0]
+        gaps.append(abs(float(roots[0]) - float(roots[1])))
+        if roots[1] >= roots[2]:
+            roots[1], roots[2] = roots[2], roots[1]
+            gaps.append(abs(float(roots[1]) - float(roots[2])))
+            if roots[0] >= roots[1]:
+                roots[0], roots[1] = roots[1], roots[0]
+            gaps.append(abs(float(roots[0]) - float(roots[1])))
+        else:
+            gaps.append(abs(float(roots[1]) - float(roots[2])))
+        rec["margins"]["root_swaps"] = min(gaps) / (2 * err_r) if err_r > 0 else np.inf
+        rec["margins"]["root0_sign"] = abs(float(roots[0])) / err_r if err_r > 0 else np.inf
+        rec["roots0_nonpositive"] = bool(roots[0] <= 0)
+        if roots[0] <= 0:
+            roots = _compute_roots2(c2, c1)
+            err_r = 0.0
+    rec["roots"] = list(roots)
+    eigenvalue = roots[0] * scale
+    s[0], s[4], s[8] = s[0] - roots[0], s[4] - roots[0], s[8] - roots[0]
+    v1, v2, v3 = _cross(s[0:3], s[3:6]), _cross(s[0:3], s[6:9]), _cross(s[3:6], s[6:9])
+    l1, l2, l3 = _dot(v1, v1), _dot(v2, v2), _dot(v3, v3)
+    rec["l"] = (l1, l2, l3)
+    if l1 >= l2 and l1 >= l3:
+        v, ll, pick = v1, l1, 0
+    elif l2 >= l1 and l2 >= l3:
+        v, ll, pick = v2, l2, 1
+    else:
+        v, ll, pick = v3, l3, 2
+    rec["pick"] = pick
+    sl = np.sqrt(ll)
+    with np.errstate(all="ignore"):
+        e = [v[0] / sl, v[1] / sl, v[2] / sl]
+        trace = cov[0] + cov[4] + cov[8]
+        curv = np.abs(eigenvalue / trace) if trace != 0 else F32(0)
+        vp = [F32(0) - F32(query[0]), F32(0) - F32(query[1]), F32(0) - F32(query[2])]
+        cos_theta = (vp[0] * e[0] + vp[1] * e[1]) + vp[2] * e[2]
+    rec["cos_theta"] = cos_theta
+    if cos_theta < 0:
+        e = [e[0] * F32(-1), e[1] * F32(-1), e[2] * F32(-1)]
+    # margins of the decisions downstream of the roots: which cross product, and the flip
+    if err_r > 0:
+        rowmax = max(abs(float(t)) for t in s)
+        others = sorted((float(l1), float(l2), float(l3)), reverse=True)
+        err_l = 16 * err_r * rowmax * (np.sqrt(others[0]) + rowmax * err_r) + 8 * U32 * others[0]
+        rec["margins"]["l_choice"] = (others[0] - others[1]) / err_l if err_l > 0 else np.inf
+        gap = max(abs(float(roots[1]) - float(roots[0])), 1e-300)
+        err_e = 4 * err_r / gap + 8 * U32
+        vpn = float(np.sqrt(sum(float(t) ** 2 for t in vp)))
+        rec["err_normal"] = err_e
+        rec["margins"]["flip"] = abs(float(cos_theta)) / (vpn * err_e) if vpn > 0 else np.inf
+    else:
+        rec["err_normal"] = 0.0
+    return np.array([e[0], e[1], e[2], curv], F32), rec
+
+
+def eig_reference(cov):
+    """The exact smallest eigenpair of a float32 covariance (as formed), in float64: (eigenvalues ascending, unit eigenvector of the
+    smallest, bound factor u * ||C|| / (l1 - l0), inf on a zero gap)."""
+    w, V = np.linalg.eigh(np.asarray(cov, F64))
+    gap = w[1] - w[0]
+    norm = np.abs(w).max()
+    return w, V[:, 0], (U32 * norm / gap if gap > 0 else np.inf)
+
+
+def _vec_cross(a, b):
+    return np.stack([a[:, 1] * b[:, 2] - a[:, 2] * b[:, 1], a[:, 2] * b[:, 0] - a[:, 0] * b[:, 2], a[:, 0] * b[:, 1] - a[:, 1] * b[:, 0]], 1)
+
+
+def _vec_dot(a, b):
+    return (a[:, 0] * b[:, 0] + a[:, 1] * b[:, 1]) + a[:, 2] * b[:, 2]
+
+
+D_PI = F32(1) / (F32(2) * F32(np.pi))                 # PCL's d_pi_ = 1.0f / (2.0f * static_cast<float> (M_PI))
+
+
+def feature_scaled(f1, f2, f3):
+    """The double expressions PCL floors: 11 * ((f1 + M_PI) * d_pi_), 11 * ((f2 + 1.0) * 0.5), 11 * ((f3 + 1.0) * 0.5)."""
+    return (11 * ((np.asarray(f1, F64) + np.pi) * F64(D_PI)), 11 * ((np.asarray(f2, F64) + 1.0) * 0.5),
+            11 * ((np.asarray(f3, F64) + 1.0) * 0.5))
+
+
+def feature_bin(scaled):
+    """floor, clamped to [0, 10]; NaN -> 0 (deviation D6: PCL's cast of NaN is undefined, INT_MIN on x86, clamped to 0)."""
+    with np.errstate(invalid="ignore"):
+        b = np.clip(np.floor(np.nan_to_num(scaled, nan=0.0)), 0, 10).astype(np.int64)
+    return b
+
+
+def pair_features_pcl32(p1, n1, p2, n2, math, err_n1=None, err_n2=None):
+    """computePairFeatures on m pairs at once ((m, 3) float32 arrays).  A pair is skipped (ok False) when f4 == 0 or ||v|| == 0.
+    The swap is acos(|a1|) > acos(|a2|) (false on NaN).  Returns dict(ok, f1, f2, f3, swap, a1, a2, and the margins: 'swap' and
+    'skip' of the two decisions, 'bins' (m, 3) of each scaled feature's distance to the nearest inner bin edge, each over the error that a
+    3-ulp change of acos / atan2 plus normals off by err_n1 / err_n2 radians can cause; ratio > 1 clears)."""
+    p1, n1, p2, n2 = (np.atleast_2d(np.asarray(a, F32)) for a in (p1, n1, p2, n2))
+    m = len(p1)
+    e1 = np.zeros(m) if err_n1 is None else np.broadcast_to(np.asarray(err_n1, F64), (m,))
+    e2 = np.zeros(m) if err_n2 is None else np.broadcast_to(np.asarray(err_n2, F64), (m,))
+    with np.errstate(all="ignore"):
+        dp = p2 - p1
+        f4 = np.sqrt(_vec_dot(dp, dp))
+        a1 = _vec_dot(n1, dp) / f4
+        a2 = _vec_dot(n2, dp) / f4
+        c1, c2 = math.acos(np.abs(a1)), math.acos(np.abs(a2))
+        swap = c1 > c2
+        n1c = np.where(swap[:, None], n2, n1)
+        n2c = np.where(swap[:, None], n1, n2)
+        dp = np.where(swap[:, None], dp * F32(-1), dp)
+        f3 = np.where(swap, -a2, a1)
+        v = _vec_cross(dp, n1c)
+        vn = np.sqrt(_vec_dot(v, v))
+        ok = (f4 != 0) & (vn != 0)
+        v = v / vn[:, None]
+        w = _vec_cross(n1c, v)
+        f2 = _vec_dot(v, n2c)
+        y, x = _vec_dot(w, n2c), _vec_dot(n1c, n2c)
+        f1 = math.atan2(y, x)
+        # margins
+        da = e1 + e2 + 8 * U32                                   # change of |a1| - |a2| from the normals and the dot products
+        acos_ulp = 3 * np.spacing(np.maximum(c1, c2).astype(F32)).astype(F64)
+        slope = np.sqrt(np.maximum(1 - np.maximum(np.abs(a1), np.abs(a2)).astype(F64) ** 2, 0))
+        m_swap = np.abs(np.abs(a1.astype(F64)) - np.abs(a2.astype(F64))) / (da + 2 * acos_ulp * np.maximum(slope, 1e-30))
+        m_swap = np.where(np.isnan(a1) | np.isnan(a2), np.inf, m_swap)
+        en = np.where(swap, e2, e1)
+        m_skip = vn.astype(F64) / ((en + 8 * U32) * f4.astype(F64))
+        df = 2 * (e1 + e2) + 16 * U32
+        df1 = 3 * np.spacing(np.abs(f1).astype(F32)).astype(F64) + df / np.maximum(np.hypot(y.astype(F64), x.astype(F64)), 1e-300) + 8 * U32
+        sc = feature_scaled(f1, f2, f3)
+        dist = [np.abs(t - np.clip(np.round(t), 1, 10)) for t in sc]
+        m_bins = np.stack([dist[0] / (11 / (2 * np.pi) * df1 + 1e-15), dist[1] / (5.5 * df + 1e-15), dist[2] / (5.5 * df + 1e-15)], 1)
+        m_bins = np.where(np.isnan(m_bins), np.inf, m_bins)
+    return dict(ok=ok, f1=f1, f2=f2, f3=f3, swap=swap, a1=a1, a2=a2, scaled=np.stack(sc, 1), bins=np.stack([feature_bin(t) for t in sc], 1),
+                margins=dict(swap=m_swap, skip=np.where(f4 == 0, np.inf, m_skip), bins=m_bins))
+
+
+def fpfh_pcl32(pts4, normal_radius, fpfh_radius, grid_cell=None, math=D7_MATH):
+    """NormalEstimation (normal_radius) and FPFHEstimation (fpfh_radius) of every point of pts4, float32 as PCL 1.8.1 evaluates them,
+    neighbours from flann_radius in D8 order (cell = grid_cell, else (1 + 2^-9) * fpfh_radius in float32).
+    SPFH (computePointSPFHSignature): k = every radius neighbour (the query, coincident duplicates and skipped pairs included); k < 2 ->
+    a zero row; hist_incr = 100.0f / (float)(k - 1) added once per pair and feature to bin floor(scaled) (pairs skipped by index, the
+    query's own); FPFH (weightPointSPFHSignature): neighbours with d2 == 0 skipped, weight = 1.0f / d2, float val = spfh * weight summed
+    into float bins and a double sum per third, then bins *= (float)(100.0 / sum) when sum != 0.
+    Returns dict(normals (n, 4), spfh (n, 33), desc (n, 33), nbr_n / nbr_f (index lists), d2_f, nrec (normal records), pairs (per
+    point: pair_features_pcl32's dict of its neighbour pairs), stable (n,) bool: every transcendental-dependent decision behind the
+    point's normal, SPFH row and descriptor clears its margin)."""
+    p4 = np.asarray(pts4, F32)
+    p = p4[:, :3]
+    n = len(p)
+    cell = F32(grid_cell) if grid_cell else F32(fpfh_radius) * CELL_FACTOR
+    rank, inl = lattice_rank(p, cell)
+    nbr_n, nbr_f, d2_f = [], [], []
+    for q in range(n):
+        i, _ = canonical_neighbours(p, q, F32(normal_radius), rank, inl)     # float32 radii (D19)
+        j, d2 = canonical_neighbours(p, q, F32(fpfh_radius), rank, inl)
+        nbr_n.append(i)
+        nbr_f.append(j)
+        d2_f.append(d2)
+    normals = np.zeros((n, 4), F32)
+    nrec = []
+    for q in range(n):
+        normals[q], r = normal_pcl32(p[nbr_n[q]], p[q], math)
+        nrec.append(r)
+    err_n = np.array([r.get("err_normal", 0.0) for r in nrec])
+    n_ok = np.array([all(v > 1 for v in r["margins"].values()) for r in nrec])
+    spfh = np.zeros((n, 33), F32)
+    pairs, spfh_ok = [], np.ones(n, bool)
+    for q in range(n):
+        nb = nbr_f[q]
+        k = len(nb)
+        other = nb[nb != q]
+        pf = pair_features_pcl32(np.broadcast_to(p[q], (len(other), 3)), np.broadcast_to(normals[q, :3], (len(other), 3)), p[other],
+                                 normals[other, :3], math, err_n[q], err_n[other])
+        pf["other"] = other
+        pairs.append(pf)
+        mg = pf["margins"]
+        spfh_ok[q] = n_ok[q] and n_ok[other].all() and (mg["swap"] > 1).all() and (mg["skip"] > 1).all() and \
+            (mg["bins"][pf["ok"]] > 1).all()
+        if k < 2:
+            continue
+        incr = F32(100) / F32(k - 1)
+        counts = np.zeros(33, np.int64)
+        for t in range(3):
+            np.add.at(counts, 11 * t + pf["bins"][pf["ok"], t], 1)
+        for b in np.flatnonzero(counts):
+            spfh[q, b] = np.add.accumulate(np.concatenate([[F32(0)], np.full(counts[b], incr, F32)]), dtype=F32)[-1]
+    desc = np.zeros((n, 33), F32)
+    for q in range(n):
+        keep = d2_f[q] != 0
+        nb, d2 = nbr_f[q][keep], d2_f[q][keep]
+        if len(nb) == 0:
+            continue
+        with np.errstate(all="ignore"):
+            weight = F32(1) / d2
+            val = spfh[nb] * weight[:, None]
+        desc[q] = np.add.accumulate(np.concatenate([np.zeros((1, 33), F32), val]), axis=0, dtype=F32)[-1]
+        for t in range(3):
+            ssum = np.add.accumulate(np.concatenate([[0.0], val[:, 11 * t:11 * t + 11].astype(F64).ravel()]))[-1]
+            if ssum != 0:
+                ssum = 100.0 / ssum
+            with np.errstate(all="ignore"):
+                desc[q, 11 * t:11 * t + 11] = desc[q, 11 * t:11 * t + 11] * F32(ssum)
+    stable = np.array([spfh_ok[nbr_f[q]].all() and n_ok[q] for q in range(n)], bool)
+    return dict(normals=normals, spfh=spfh, desc=desc, nbr_n=nbr_n, nbr_f=nbr_f, d2_f=d2_f, nrec=nrec, pairs=pairs, stable=stable,
+                normal_stable=n_ok, spfh_stable=spfh_ok, cell=cell)
