@@ -74,7 +74,9 @@ typedef enum qb200_status {
   QB200_ERR_UNSUPPORTED = -4,    /* e.g. use_crosscheck = 0, libnccl absent */
   QB200_ERR_VOXEL_OVERFLOW = -5  /* PCL's voxel index would not fit an int: the truncated spans dx*dy*dz > INT_MAX (PCL warns and
                                     returns the input unfiltered), a kept point's floor(p / leaf) outside int32, or the floor-based
-                                    grid div_b[0]*div_b[1]*div_b[2] > INT_MAX; the input is returned unfiltered in every case */
+                                    grid div_b[0]*div_b[1]*div_b[2] > INT_MAX, or a largest linear index above INT_MAX (PCL's
+                                    float subtraction can round a cell coordinate up to div_b); the input is returned
+                                    unfiltered in every case */
 } qb200_status;
 
 /* qb200_result.flags */

@@ -33,7 +33,8 @@
 //   D9 2x2 rotation: own two-sided Jacobi SVD (Eigen::JacobiSVD unavailable); fp64 sums in index order
 //   D10 VoxelGrid refuses a cloud (QB200_ERR_VOXEL_OVERFLOW, input returned unfiltered) not only on PCL's own check
 //      (truncated spans dx*dy*dz > INT_MAX) but wherever PCL's int arithmetic would overflow (UB, wraps in practice): a kept
-//      point's floor(p * inv) outside int32, or a product of the floor-based div_b above INT_MAX
+//      point's floor(p * inv) outside int32, a product of the floor-based div_b above INT_MAX, or a largest linear index above
+//      INT_MAX (PCL subtracts floor(p * inv) - min_b in float, which can round ijk up to div_b, so the index can exceed the product)
 //   D18 KCORE_HEU limit (int)(kcore_heuristic_threshold * n) (src/graph.cc:69-70): undefined for NaN and out-of-range products; both
 //      sides compute what x86-64's cvttsd2si gives, INT_MIN, through qb_kcore_heu_limit (quatro_b200/csrc/kcore_cutoff.cuh)
 //   D19 radii are float32 (qb200_params, qb200_compute_fpfh): the squared radius is float(double(r) * double(r)) of the float radius,
@@ -115,14 +116,14 @@ int voxelize(const P4* pts, int n, float leaf, int skip_flagged, std::vector<P4>
   }
   if (kept.empty()) return QB200_OK;
   // overflow check: PCL warns and copies the input through.  D10: also refused wherever PCL's own int arithmetic would overflow
-  // (a floor(p * inv) outside int32 -- the bbox corners decide, floor(p * inv) is monotone in p -- or a product of the floor-based
-  // div_b above INT_MAX), and PCL's int64 span product is evaluated without overflowing.
-  const auto product_exceeds = [](int64_t a, int64_t b, int64_t c) {  // factors >= 1
-    const int64_t lim = std::numeric_limits<int32_t>::max();
+  // (a floor(p * inv) outside int32 -- the bbox corners decide, floor(p * inv) is monotone in p --, a product of the floor-based
+  // div_b above INT_MAX, or a largest linear index above INT_MAX), and PCL's int64 span product is evaluated without overflowing.
+  const int64_t lim = std::numeric_limits<int32_t>::max();
+  const auto product_exceeds = [lim](int64_t a, int64_t b, int64_t c) {  // factors >= 1
     return a > lim || b > lim || c > lim || a * b > lim || a * b * c > lim;
   };
   bool refuse = false;
-  int64_t span[3], min_b[3], div_b[3];
+  int64_t span[3], min_b[3], div_b[3], top[3];
   for (int a = 0; a < 3; ++a) {
     const float lo = std::floor(mn[a] * inv), hi = std::floor(mx[a] * inv);
     const float s = (mx[a] - mn[a]) * inv;
@@ -130,12 +131,15 @@ int voxelize(const P4* pts, int n, float leaf, int skip_flagged, std::vector<P4>
     span[a] = (int64_t)s + 1;
     min_b[a] = (int64_t)lo;
     div_b[a] = (int64_t)hi - min_b[a] + 1;
+    top[a] = (int64_t)(hi - lo);  // the largest ijk of the axis: PCL's float subtraction rounds monotonically, the max corner decides
   }
-  if (refuse || product_exceeds(span[0], span[1], span[2]) || product_exceeds(div_b[0], div_b[1], div_b[2])) {
+  // top[a] <= 2^31 (fl(hi - lo) can round up to 2^31) and the div_b product is within INT_MAX: every term below is <= 2^62
+  if (refuse || product_exceeds(span[0], span[1], span[2]) || product_exceeds(div_b[0], div_b[1], div_b[2]) ||
+      top[0] + top[1] * div_b[0] + top[2] * div_b[0] * div_b[1] > lim) {
     for (int i : kept) out.push_back(pts[i]);
     return QB200_ERR_VOXEL_OVERFLOW;
   }
-  const int mul[3] = {1, (int)div_b[0], (int)(div_b[0] * div_b[1])};
+  const int64_t mul[3] = {1, div_b[0], div_b[0] * div_b[1]};
   std::vector<std::pair<int, int>> iv;  // (voxel idx, point idx)
   iv.reserve(kept.size());
   for (int i : kept) {
@@ -143,7 +147,7 @@ int voxelize(const P4* pts, int n, float leaf, int skip_flagged, std::vector<P4>
     const int ijk0 = (int)(std::floor(p.x * inv) - (float)min_b[0]);
     const int ijk1 = (int)(std::floor(p.y * inv) - (float)min_b[1]);
     const int ijk2 = (int)(std::floor(p.z * inv) - (float)min_b[2]);
-    iv.emplace_back(ijk0 * mul[0] + ijk1 * mul[1] + ijk2 * mul[2], i);
+    iv.emplace_back((int)(ijk0 * mul[0] + ijk1 * mul[1] + ijk2 * mul[2]), i);  // <= the largest index, so it fits an int
   }
   const auto by_voxel = [](const std::pair<int, int>& a, const std::pair<int, int>& b) { return a.first < b.first; };
   if (g_literal) std::sort(iv.begin(), iv.end(), by_voxel);  // [EXT] PCL: std::sort with operator< on the voxel index only

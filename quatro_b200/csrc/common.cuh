@@ -30,9 +30,9 @@ __host__ __device__ __forceinline__ uint64_t cell_key(int i, int j, int k) {
 }
 
 // ---- voxel keys (frontend.cu, voxsort.cu) ----
-constexpr int kVoxShift = 31;
+constexpr int kVoxShift = 32;
 constexpr uint64_t kVoxMask = (1ull << kVoxShift) - 1;
-constexpr uint64_t kVoxInvalid = kVoxMask;  // dx dy dz <= INT_MAX: a valid index is at most 2^31 - 2
+constexpr uint64_t kVoxInvalid = kVoxMask;  // a valid index is at most INT_MAX (vox_grid())
 constexpr int kVsChunks = 64;               // contiguous chunks of a raw scan whose kept points the bbox pass counts
 constexpr int kVsTile = 2048;               // items per tile of the voxel sort (voxsort.cu): 8 warps x 8 rounds x 32 lanes
 
@@ -111,9 +111,13 @@ __host__ __device__ __forceinline__ bool vox_product_exceeds(long long a, long l
 //   - PCL's check: the truncated spans (int64)((max - min) * inv) + 1 multiply to more than INT_MAX;
 //   - a kept point's floor(p * inv) lies outside int32 (floor(p * inv) is monotone in p: the bbox corners decide);
 //   - the floor-based div_b = max_b - min_b + 1, which can be one larger per axis than the truncated span, multiply to more than
-//     INT_MAX (the linear index would not fit an int).
+//     INT_MAX (divb_mul would not fit an int);
+//   - the largest linear index PCL computes exceeds INT_MAX.  PCL subtracts ijk = floor(p * inv) - (float)min_b in float, which
+//     rounds once the difference passes 2^24 and can round up to div_b, so that index can exceed div_b0 div_b1 div_b2 - 1.  The
+//     rounding is monotone, so the max corner gives each axis's largest ijk.
 // The index is relative to min_b, so a cloud far from the origin is voxelised like the same cloud moved to the origin.
-__device__ __forceinline__ bool vox_axis(int omin, int omax, float inv_leaf, long long* span, long long* min_b, long long* div_b) {
+__device__ __forceinline__ bool vox_axis(int omin, int omax, float inv_leaf, long long* span, long long* min_b, long long* div_b,
+                                         long long* top) {
   const float mn = ordered_float(omin), mx = ordered_float(omax);
   const float lo = floorf(mn * inv_leaf), hi = floorf(mx * inv_leaf);
   if (!(lo >= -2147483648.0f && hi < 2147483648.0f)) return false;
@@ -122,26 +126,28 @@ __device__ __forceinline__ bool vox_axis(int omin, int omax, float inv_leaf, lon
   *span = (long long)s + 1;
   *min_b = (long long)lo;
   *div_b = (long long)hi - *min_b + 1;
+  *top = (long long)__fsub_rn(hi, lo);     // the largest ijk of the axis
   return true;
 }
-__device__ __forceinline__ bool vox_grid(const int* __restrict__ bbox, float inv_leaf, long long* min_b, long long* div_b) {
-  long long t0, t1, t2;
-  if (!vox_axis(bbox[0], bbox[3], inv_leaf, &t0, &min_b[0], &div_b[0]) || !vox_axis(bbox[1], bbox[4], inv_leaf, &t1, &min_b[1], &div_b[1]) ||
-      !vox_axis(bbox[2], bbox[5], inv_leaf, &t2, &min_b[2], &div_b[2]))
-    return false;
-  return !vox_product_exceeds(t0, t1, t2) && !vox_product_exceeds(div_b[0], div_b[1], div_b[2]);
+// *max_idx: the largest linear index of the cloud (valid when true is returned)
+__device__ __forceinline__ bool vox_grid(const int* __restrict__ bbox, float inv_leaf, long long* min_b, long long* div_b,
+                                         long long* max_idx) {
+  long long t[3], a[3];
+  for (int k = 0; k < 3; ++k)
+    if (!vox_axis(bbox[k], bbox[k + 3], inv_leaf, &t[k], &min_b[k], &div_b[k], &a[k])) return false;
+  if (vox_product_exceeds(t[0], t[1], t[2]) || vox_product_exceeds(div_b[0], div_b[1], div_b[2])) return false;
+  *max_idx = a[0] + a[1] * div_b[0] + a[2] * div_b[0] * div_b[1];  // a[k] <= 2^31 and div_b0 div_b1 <= INT_MAX: no overflow
+  return *max_idx <= 2147483647LL;
 }
 
-// number of 8-bit digits the voxel keys of a cloud occupy: the keys are below div_b[0] div_b[1] div_b[2] of pcl::VoxelGrid's own
-// linear index (voxel_pack uses the same min_b / div_b).  -1: the cloud is refused (vox_grid()), nothing is sorted and run_heads
-// drops it.
+// number of 8-bit digits the voxel keys of a cloud occupy: the keys are at most the largest linear index of pcl::VoxelGrid
+// (vox_grid(); voxel_pack uses the same min_b / div_b).  -1: the cloud is refused, nothing is sorted and run_heads drops it.
 __device__ __forceinline__ int vox_digits(const int* __restrict__ bbox, int n_valid, float inv_leaf) {
   if (n_valid <= 0) return 0;
-  long long m[3], d[3];
-  if (!vox_grid(bbox, inv_leaf, m, d)) return -1;
-  const unsigned long long span = (unsigned long long)(d[0] * d[1] * d[2]);  // <= INT_MAX
-  int bits = 0;
-  while (bits < 31 && (1ull << bits) < span) ++bits;
+  long long m[3], d[3], top;
+  if (!vox_grid(bbox, inv_leaf, m, d, &top)) return -1;
+  int bits = 0;  // keys lie in [0, top], top <= INT_MAX
+  while (bits < 31 && (1ll << bits) <= top) ++bits;
   return (bits + 7) >> 3;
 }
 

@@ -46,9 +46,9 @@ static int clog2(int n) {
 // ------------------------------------------------------------------------------------------------
 // K1a: bounding box and per-chunk counts of the kept raw points (one pass, 128-bit loads).  The voxel key that the pack pass
 // (voxsort.cu) then builds is PCL's own linear index  (i - min_i) + (j - min_j) dx + (k - min_k) dx dy  ([EXT] pcl::VoxelGrid,
-// called from include/quatro.hpp:49-57), which the library requires to fit an int: at most 31 key bits, and for a given cloud
-// only the bits of dx dy dz (vox_digits()).  The bbox alone decides whether a cloud is refused (vox_grid()), so this pass keeps
-// no per-point range test.
+// called from include/quatro.hpp:49-57, each difference taken in float as PCL does), which the library requires to fit an int: at
+// most 31 key bits, and for a given cloud only the bits of its largest index (vox_digits()).  The bbox alone decides whether a
+// cloud is refused (vox_grid()), so this pass keeps no per-point range test.
 // ------------------------------------------------------------------------------------------------
 
 __global__ void __launch_bounds__(256) voxel_bbox_kernel(const float4* const* __restrict__ cloud_ptr, const int* __restrict__ cloud_n,

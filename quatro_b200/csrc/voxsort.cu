@@ -38,8 +38,9 @@ __global__ void __launch_bounds__(kVsThreads) voxel_pack_kernel(const float4* co
   const float4* __restrict__ pts = cloud_ptr[cloud];
   const float inv_leaf = front[cloud].inv_leaf;
   const int skip_flagged = front[cloud].skip_flagged;
-  long long m[3] = {0, 0, 0}, d[3] = {1, 1, 1};  // min_b / div_b of pcl::VoxelGrid::applyFilter
-  const bool grid_ok = n_valid[cloud] > 0 && vox_grid(bbox + cloud * 6, inv_leaf, m, d);
+  long long m[3] = {0, 0, 0}, d[3] = {1, 1, 1}, top;  // min_b / div_b of pcl::VoxelGrid::applyFilter
+  const bool grid_ok = n_valid[cloud] > 0 && vox_grid(bbox + cloud * 6, inv_leaf, m, d, &top);
+  const float lo[3] = {(float)m[0], (float)m[1], (float)m[2]};  // exact: min_b is the float floor of the bbox corner
   int base = 0;  // kept points of the preceding chunks
   {
     int v = 0;
@@ -61,9 +62,11 @@ __global__ void __launch_bounds__(kVsThreads) voxel_pack_kernel(const float4* co
         const float4 p = __ldg(pts + i);
         if (raw_point_kept(p, skip_flagged)) {  // exactly the points the bbox pass counted
           uint64_t cell = kVoxInvalid;         // refused cloud: run_heads drops it, any key will do
-          if (grid_ok) {                       // every floor(p * inv) fits an int and the index is below INT_MAX
-            const int ci = (int)floorf(p.x * inv_leaf), cj = (int)floorf(p.y * inv_leaf), ck = (int)floorf(p.z * inv_leaf);
-            cell = (uint64_t)(((long long)ci - m[0]) + ((long long)cj - m[1]) * d[0] + ((long long)ck - m[2]) * d[0] * d[1]);
+          if (grid_ok) {                       // every ijk fits an int and the index is at most INT_MAX
+            // PCL: ijk = static_cast<int>(floor(p * inv) - static_cast<float>(min_b)), the subtraction in float
+            const long long ci = (int)__fsub_rn(floorf(p.x * inv_leaf), lo[0]), cj = (int)__fsub_rn(floorf(p.y * inv_leaf), lo[1]),
+                            ck = (int)__fsub_rn(floorf(p.z * inv_leaf), lo[2]);
+            cell = (uint64_t)(ci + cj * d[0] + ck * d[0] * d[1]);
           }
           it[j] = (cell << idx_bits) | (uint64_t)i;
           keep[j] = 1;

@@ -6,7 +6,8 @@ unique), and a list-and-set restatement of pmc's k-core peel and heuristic, find
 12-130).  This module never imports oracle/ or the CUDA library: tools/gen_independent_pins.py uses it to write the
 independent_*.npz fixtures, tests/test_independent_pins.py uses it to check the oracle, tests/test_tuple_adversarial.py to check
 the oracle and the device matcher, tests/test_clique_adversarial.py the oracle and K9, and tests/test_fpfh_adversarial.py the
-oracle's and the device's normals, SPFH and FPFH against the float32 restatement of PCL's NormalEstimation / FPFHEstimation below."""
+oracle's and the device's normals, SPFH and FPFH against the float32 restatement of PCL's NormalEstimation / FPFHEstimation below, and
+tests/test_voxel_adversarial.py the oracle's and the device's voxel filter against the float32 restatement of PCL's VoxelGrid at the end."""
 import numpy as np
 from scipy.spatial import cKDTree
 
@@ -960,3 +961,92 @@ def fpfh_pcl32(pts4, normal_radius, fpfh_radius, grid_cell=None, math=D7_MATH):
     stable = np.array([spfh_ok[nbr_f[q]].all() and n_ok[q] for q in range(n)], bool)
     return dict(normals=normals, spfh=spfh, desc=desc, nbr_n=nbr_n, nbr_f=nbr_f, d2_f=d2_f, nrec=nrec, pairs=pairs, stable=stable,
                 normal_stable=n_ok, spfh_stable=spfh_ok, cell=cell)
+
+
+# ---- float32 restatement of pcl::VoxelGrid<PointXYZ>::applyFilter (PCL 1.8.1), include/quatro.hpp:49-57 ------------------------------
+# Written from the PCL text: inverse_leaf_size_ = 1 / leaf in float; getMinMax3D over the points the filter keeps; the int64 check of the
+# truncated spans; min_b_ / max_b_ by float floor; div_b_ and divb_mul_; ijk = int(floor(p * inv) - float(min_b)) with the subtraction in
+# FLOAT; the int index ijk0 + ijk1 * divb_mul[1] + ijk2 * divb_mul[2]; the sort of (index, point) pairs; a CentroidPoint per voxel (float
+# accumulators from +0.0, points added in sorted order, divided by float(count), w = 1).  Every float operation is one numpy float32
+# operation; index arithmetic is Python int or int64.
+VOX_OK, VOX_OVERFLOW = 0, -5            # QB200_OK, QB200_ERR_VOXEL_OVERFLOW
+INT32_MAX = 2 ** 31 - 1
+
+
+def _sequential_sums(xyz, start, counts):
+    """Per voxel, the float32 sum of its rows of xyz [start, start + count) added one by one from +0.0 (no pairwise reduction)."""
+    acc = np.zeros((len(start), 3), np.float32)
+    small = counts <= 64
+    with np.errstate(over="ignore"):                              # a voxel's sum may overflow to +-inf, as in float
+        for k in range(int(counts[small].max(initial=0))):       # round k adds the k-th point of every voxel that has one
+            v = np.nonzero(small & (counts > k))[0]
+            acc[v] = acc[v] + xyz[start[v] + k]
+        for v in np.nonzero(~small)[0]:                           # np.add.accumulate is sequential; +0.0 first, as the accumulator
+            seg = np.concatenate([np.zeros((1, 3), np.float32), xyz[start[v]:start[v] + counts[v]]])
+            acc[v] = np.add.accumulate(seg, axis=0, dtype=np.float32)[-1]
+    return acc
+
+
+def voxel_grid_pcl32(pts4, leaf, skip_flagged=1):
+    """pcl::VoxelGrid<PointXYZ>::applyFilter in float32 on n x 4 records.  Returns (out, status, grid):
+    out     the centroids (x, y, z, 1) in ascending voxel index, or on a refusal the kept records as they are (DESIGN section 2 (ii));
+    status  VOX_OK or VOX_OVERFLOW;
+    grid    dict: inv, lo / hi (float floors of the bbox corners), span (PCL's truncated spans), min_b, div_b, top (per axis, the
+            largest ijk: the float subtraction at the bbox corners), top_index (the largest linear index), refused (None or the rule),
+            and for accepted clouds idx (index per kept point), order (the stable sort), uniq / start / counts of the voxels.
+    Kept points: finite x, y, z and, with skip_flagged, not w < 0 (the library's ground flag).  Deviations from the PCL text:
+      D3   the sort is stable (PCL's std::sort leaves tied indices in an unspecified order);
+      D10  refused, besides PCL's own check, wherever PCL's int arithmetic would overflow: a floor outside int32 ("floor"), a product of
+           div_b above INT_MAX ("div_b"), or a largest linear index above INT_MAX ("top_index": the float subtraction can round ijk up to
+           div_b, so the index can exceed div_b0 * div_b1 * div_b2 - 1)."""
+    pts4 = np.asarray(pts4, np.float32).reshape(-1, 4)
+    keep = np.isfinite(pts4[:, :3]).all(1)
+    if skip_flagged:
+        keep &= ~(pts4[:, 3] < 0)
+    kept = pts4[keep]
+    with np.errstate(over="ignore", divide="ignore"):
+        inv = F32(1) / F32(leaf)
+    grid = dict(inv=inv, refused=None)
+    if len(kept) == 0:
+        return np.zeros((0, 4), np.float32), VOX_OK, grid
+    xyz = kept[:, :3]
+    mn, mx = xyz.min(0), xyz.max(0)
+    with np.errstate(over="ignore", invalid="ignore"):
+        lo, hi = np.floor(mn * inv), np.floor(mx * inv)
+        s = (mx - mn) * inv
+    grid.update(lo=lo, hi=hi)
+
+    def refuse(rule):
+        grid["refused"] = rule
+        return kept.copy(), VOX_OVERFLOW, grid
+
+    # PCL: dx = static_cast<int64_t>((max_p[0] - min_p[0]) * inverse_leaf_size_[0]) + 1, ...; dx * dy * dz > INT_MAX -> input returned.
+    # A span of 2^31 or more (or inf / NaN, where the int64 cast is undefined) fails that check on its own.
+    if not (s < 2.0 ** 31).all():
+        return refuse("span")
+    span = [int(v) + 1 for v in s]
+    if span[0] * span[1] * span[2] > INT32_MAX:
+        return refuse("span")
+    if not ((lo >= -2.0 ** 31).all() and (hi < 2.0 ** 31).all()):       # D10: min_b_ = static_cast<int>(floor(...)) must fit
+        return refuse("floor")
+    min_b = [int(v) for v in lo]
+    div_b = [int(h) - int(l) + 1 for h, l in zip(hi, lo)]               # div_b_ = max_b_ - min_b_ + 1
+    grid.update(span=span, min_b=min_b, div_b=div_b)
+    if div_b[0] * div_b[1] * div_b[2] > INT32_MAX:                       # D10: divb_mul_ and the index must fit an int
+        return refuse("div_b")
+    mul = [1, div_b[0], div_b[0] * div_b[1]]                             # divb_mul_
+    top = [int(F32(h - l)) for h, l in zip(hi, lo)]                      # floor(max * inv) - float(min_b), monotone in the point
+    top_index = top[0] * mul[0] + top[1] * mul[1] + top[2] * mul[2]
+    grid.update(top=top, top_index=top_index)
+    if top_index > INT32_MAX:                                            # D10: the largest index PCL computes must fit an int
+        return refuse("top_index")
+    with np.errstate(over="ignore", invalid="ignore"):
+        ijk = (np.floor(xyz * inv) - lo.astype(np.float32)).astype(np.int64)   # float(min_b) == lo exactly: lo is a float integer
+    idx = ijk[:, 0] * mul[0] + ijk[:, 1] * mul[1] + ijk[:, 2] * mul[2]
+    order = np.argsort(idx, kind="stable")                               # D3
+    uniq, start, counts = np.unique(idx[order], return_index=True, return_counts=True)
+    sums = _sequential_sums(xyz[order], start, counts)
+    out = np.ones((len(uniq), 4), np.float32)
+    out[:, :3] = sums / counts.astype(np.float32)[:, None]
+    grid.update(idx=idx, order=order, uniq=uniq, start=start, counts=counts)
+    return out, VOX_OK, grid

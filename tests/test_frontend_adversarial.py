@@ -11,7 +11,7 @@ import pytest
 
 from quatro_b200 import synth
 from quatro_b200.capi import Handle, default_params
-from independent_ref import voxel_grid
+from independent_ref import voxel_grid, voxel_grid_pcl32
 from support import P4, same_bits
 
 DEFAULT_CELL = float(np.float32(0.75) * np.float32(1.001953125))
@@ -20,26 +20,13 @@ INT_MAX = 2**31 - 1
 
 
 def grid_of(pts4, leaf, skip):
-    """PCL's grid of the kept points, evaluated the way the library does (float32 products, int64 spans), and the refusal rule:
-    (status, digits of the voxel key)."""
-    p = pts4[np.isfinite(pts4[:, :3]).all(1) & ~((skip != 0) & (pts4[:, 3] < 0))][:, :3]
-    if len(p) == 0:
-        return OK, 0
-    inv = np.float32(1.0) / np.float32(leaf)
-    mn, mx = p.min(0), p.max(0)
-    with np.errstate(over="ignore", invalid="ignore"):
-        lo, hi, s = np.floor(mn * inv), np.floor(mx * inv), (mx - mn) * inv
-    if not ((lo >= -2.0**31).all() and (hi < 2.0**31).all() and (s < 2.0**31).all()):
-        return OVERFLOW, None
-    trunc = [int(v) + 1 for v in s]
-    div = [int(h) - int(l) + 1 for h, l in zip(hi, lo)]
-    if np.prod(trunc, dtype=object) > INT_MAX or np.prod(div, dtype=object) > INT_MAX:
-        return OVERFLOW, None
-    span = int(np.prod(div, dtype=object))
-    bits = 0
-    while bits < 31 and (1 << bits) < span:
-        bits += 1
-    return OK, (bits + 7) >> 3
+    """The library's refusal rule and digit count of the voxel key, taken from the float32 restatement of PCL's grid
+    (independent_ref.voxel_grid_pcl32, the D10 rules included): (status, 8-bit digits of the largest linear index), digits None
+    for a refused cloud."""
+    _, st, grid = voxel_grid_pcl32(pts4, leaf, skip)
+    if st != OK:
+        return st, None
+    return OK, (int(grid.get("top_index", 0)).bit_length() + 7) >> 3
 
 
 # ---- the cloud set --------------------------------------------------------------------------------------------------------------
