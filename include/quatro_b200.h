@@ -351,9 +351,9 @@ int qb200_solve_batch(qb200_handle* h, const qb200_corr_set* sets, int32_t n_set
                       qb200_mem_kind kind, qb200_result* results);
 
 /* --- per-pair lists of the batch entry points: correspondences, max clique, final inliers, inlier masks -------------------------
- * The single-pair getters (qb200_get_last_*) read slot 0 after a single-pair call; the _ex forms of the batch entry points hand out
- * the same lists for every pair of a batch.  The caller owns every array; pair i's entries start at i * cap_per_pair whatever wave or
- * lane ran it.  Pair i gets min(count, cap_per_pair) entries of each list, count taken from its record: n_corr for corr and the
+ * The single-pair getters (qb200_get_last_*) read slot 0 after a single-pair call, until a later call reuses it (see
+ * qb200_get_last_clique); the _ex forms of the batch entry points hand out the same lists for every pair of a batch.  The caller
+ * owns every array; pair i's entries start at i * cap_per_pair whatever wave or lane ran it.  Pair i gets min(count, cap_per_pair) entries of each list, count taken from its record: n_corr for corr and the
  * matched points, clique_size for the clique and both masks, n_final_inliers for the final inliers.  Entries past that count are
  * left untouched, and a pair whose status is QB200_CAPACITY_EXCEEDED gets no entries.  A pair whose clique has at most one member
  * is not solved: its mask entries are 0.  When a list that was asked for (a non-NULL array) held more than cap_per_pair entries,
@@ -901,7 +901,20 @@ int qb200_comm_wait(qb200_handle* h);
 int qb200_bind_numa(qb200_handle* h);
 
 /* Introspection of the most recent single-pair solve on this handle (getMaxCliques,
- * getFinalInliersIndices, getCorrespondences; quatro.hpp:949-972, fpfh_manager.hpp:234-236). */
+ * getFinalInliersIndices, getCorrespondences; quatro.hpp:949-972, fpfh_manager.hpp:234-236).  Each list is set by these calls:
+ *   correspondences: a one-pair registration or match of raw, cached or feature pairs (qb200_register_pair, the batch entry
+ *     points with n = 1), qb200_match, qb200_match_and_pack;
+ *   clique and final inliers: a one-pair registration, match (empty lists) or solve (qb200_solve_correspondences, qb200_solve_batch*
+ *     with n = 1), qb200_solve_pose; the clique also qb200_max_clique / _ex;
+ *   features (qb200_get_last_features): a one-pair registration or match of raw pairs, qb200_match_and_pack, qb200_compute_fpfh;
+ *   nearest-neighbour tables (qb200_debug_nn_tables): qb200_match.
+ * The lists live in the buffers of the handle's first lane, which every later call that runs a wave there reuses: every batch,
+ * enqueue, describe, voxelize, cache-write, graph, clique and pose entry point whose waves reach that lane, and the stage calls
+ * qb200_voxelize, qb200_compute_fpfh, qb200_match, qb200_match_and_pack, qb200_build_graph, qb200_max_clique / _ex,
+ * qb200_solve_pose and qb200_debug_tc_distances.  (Pre-processing, qb200_patchwork, qb200_segment_cloud and qb200_cache_read,
+ * _copy and _reserve run no such wave.)  A getter hands out its list only if no such call ran after the call that set it;
+ * otherwise it returns QB200_ERR_BAD_ARG with *n = 0, and qb200_last_error says a later call reused the buffers.  Fetch the lists
+ * right after the call they describe (the _ex batch forms hand them out with the call). */
 int qb200_get_last_clique(qb200_handle* h, int32_t* idx, int32_t cap, int32_t* n);
 int qb200_get_last_final_inliers(qb200_handle* h, int32_t* idx, int32_t cap, int32_t* n);
 int qb200_get_last_correspondences(qb200_handle* h, int32_t* corr, float* src_matched4,
@@ -909,7 +922,8 @@ int qb200_get_last_correspondences(qb200_handle* h, int32_t* corr, float* src_ma
 
 /* Normals (n x {nx,ny,nz,curvature}) and FPFH-33 descriptors (n x 33) the most recent qb200_match_and_pack (which = 0 source,
  * 1 target) or qb200_compute_fpfh (which = 0) left on the device: FPFHManager::getObjDescriptor / getSceneDescriptor /
- * getTgtNormals (include/fpfh_manager.hpp:161-177).  Either pointer may be NULL. */
+ * getTgtNormals (include/fpfh_manager.hpp:161-177).  Either pointer may be NULL.  Refused once a later call reused the buffers, as
+ * qb200_get_last_clique. */
 int qb200_get_last_features(qb200_handle* h, int32_t which, float* normals4, float* desc33, int32_t cap, int32_t* n);
 
 /* Per-stage device time of the last batch call in milliseconds (CUDA events); the single-pair registration and solve are batches
@@ -936,7 +950,8 @@ int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset);
 /* Diagnostics: both nearest-neighbour tables of the most recent qb200_match, in point order: rowbest[i] = packed
  * (distance bits << 32 | target index) of the best target of source point i, colbest[j] = the same for the best source of target
  * point j, ~0 = none.  min(cap_rows, n_src) and min(cap_cols, n_tgt) entries are written (either pointer may be NULL); the
- * tables are those the mutual check read, after any stripe was redone by the exact kernel.  Synchronises the handle's stream. */
+ * tables are those the mutual check read, after any stripe was redone by the exact kernel.  Synchronises the handle's stream.
+ * QB200_ERR_BAD_ARG once a later call reused the buffers, as qb200_get_last_clique. */
 int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, uint64_t* colbest, int32_t cap_cols);
 /* Handles created with QB200_TC_PROF=1 only: per-role clock64 accounting of tc_nn_kernel (24 counters, see tools/tc_profile.py) */
 int qb200_debug_tc_profile(qb200_handle* h, uint64_t* out24, int32_t reset);

@@ -213,6 +213,7 @@ int wave_reset(Lane* L, int n_clouds) {
   const int n = (int)L->ctr_ints;
   wave_init_kernel<<<(n + 255) / 256, 256, 0, L->stream>>>(L->ctr_block, n, L->ctr.bbox, n_clouds);
   L->launches++;
+  L->waves++;
   QB_CUDA_TRY(L, cudaGetLastError());
   return QB200_OK;
 }
@@ -266,6 +267,16 @@ void set_last(qb200_handle* h, const qb200_result& r) {
   h->last_n_corr = r.n_corr;
   h->last_n_clique = r.clique_size;
   h->last_n_final = r.n_final_inliers;
+}
+
+void stamp_last(qb200_handle* h, std::initializer_list<LastList> lists) {
+  for (const LastList l : lists) h->last_wave[l] = h->lane[0]->waves;
+}
+
+bool last_is_live(qb200_handle* h, LastList list) {
+  if (h->lane[0]->waves == h->last_wave[list]) return true;
+  h->fail(__FILE__, __LINE__, "a later call reused the buffers of the most recent single-pair call: fetch its lists right after it");
+  return false;
 }
 
 // a match wave's entry: the matcher fields of p (K7's tuple test), nothing of the solver
@@ -1515,7 +1526,14 @@ int run_call(qb200_handle* h, const BatchCall& c) {
   int rc = enqueue_call(h, c);
   const int rc2 = h ? batch_flush(h) : QB200_OK;
   if (rc == QB200_OK) rc = rc2;
-  if (rc == QB200_OK && c.n == 1 && (c.sink == Sink::Solve || c.sink == Sink::Match)) set_last(h, c.results[0]);
+  if (rc == QB200_OK && c.n == 1 && (c.sink == Sink::Solve || c.sink == Sink::Match)) {
+    // what the wave left in slot 0: the clique and final inliers (none in a match), the packed correspondences of a pair (a set's
+    // are the caller's points, with no index pairs), the features of a raw pair
+    set_last(h, c.results[0]);
+    stamp_last(h, {kLastClique, kLastFinal});
+    if (is_pairs(c.src)) stamp_last(h, {kLastCorr});
+    if (c.src == Source::RawPairs) stamp_last(h, {kLastFeatures});
+  }
   return rc;
 }
 

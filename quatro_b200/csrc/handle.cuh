@@ -4,6 +4,7 @@
 #pragma once
 #include <string.h>
 
+#include <initializer_list>
 #include <memory>
 #include <vector>
 
@@ -150,6 +151,7 @@ struct Lane {
   cudaStream_t stream;       // own_stream, or the caller's stream of qb200_set_stream (lane 0)
   char* err;                 // the handle's message buffer (qb200_last_error)
   int64_t launches;
+  uint64_t waves;            // waves started on this lane (wave_reset): lane 0's count tells the getters whether slot 0 was reused
 
   // ---- wave description (host-known inputs) ----
   DeviceMem<const float4*> d_cloud_ptr; // [2S]
@@ -261,6 +263,10 @@ struct Lane {
   int* n_unique() const { return reinterpret_cast<int*>(class_of() + (size_t)2 * S * V); }
 };
 
+// The lists of lane 0's slot 0 that the single-pair getters hand out: correspondences and matched points, clique, final inliers,
+// normals and descriptors (qb200_get_last_*), and the nearest-neighbour tables (qb200_debug_nn_tables)
+enum LastList { kLastCorr, kLastClique, kLastFinal, kLastFeatures, kLastNn, kLastLists };
+
 }  // namespace qb
 
 struct qb200_handle {
@@ -299,6 +305,9 @@ struct qb200_handle {
   double rot_noise_bound_latched;  // quatro.hpp:469-470 (0 = not latched yet)
   int last_n_corr, last_n_clique, last_n_final;  // slot 0 of the most recent single-pair call
   int last_match_n[2];        // source / target points of the most recent qb200_match (qb200_debug_nn_tables)
+  // per list (qb::LastList): lane 0's wave count right after the most recent single-pair call that produced it.  Every later wave on
+  // lane 0 rewrites slot 0's buffers but not the counts above, so a getter hands out its list only while the count is unchanged.
+  uint64_t last_wave[qb::kLastLists];
 
   float stage_ms[8];
   float kernel_ms[2];
@@ -430,6 +439,11 @@ bool params_ok(const qb200_params* p, bool solver = true);
 float lattice_cell(const qb200_params& p);
 qb200_params resolve_params(qb200_handle* h, const qb200_params& p);
 void set_last(qb200_handle* h, const qb200_result& r);
+// the lists `lists` of lane 0's slot 0 are those of the single-pair call that just ended: the getters hand them out until lane 0
+// starts another wave
+void stamp_last(qb200_handle* h, std::initializer_list<LastList> lists);
+// whether lane 0 has started no wave since `list` was stamped; if it has, the message for qb200_last_error
+bool last_is_live(qb200_handle* h, LastList list);
 // Raise a kernel's dynamic shared-memory opt-in to at least `bytes` on `device`.  The attribute is a property of the
 // (function, device), not of a handle: handles of different capacities share it, so it is only ever raised (process-wide maximum).
 cudaError_t ensure_dyn_smem(int device, const void* kernel, size_t bytes);

@@ -112,6 +112,7 @@ int qb200_compute_fpfh(qb200_handle* h, const float* pts4, int32_t n, float norm
     QB_CUDA_TRY(h, cudaMemcpyAsync(desc33, L->aos_scratch, (size_t)n * kDescDim * sizeof(float), cudaMemcpyDeviceToHost, L->stream));
   }
   QB_CUDA_TRY(h, hold.sync());
+  stamp_last(h, {kLastFeatures});
   return QB200_OK;
 }
 
@@ -127,10 +128,13 @@ int qb200_match(qb200_handle* h, const float* src4, int32_t n_src, const float* 
   Lane* L = h->lane[0].get();
   if (n_src > L->V || n_tgt > L->V) { h->fail(__FILE__, __LINE__, "cloud exceeds max_voxel_points"); return QB200_ERR_BAD_ARG; }
   h->last_match_n[0] = h->last_match_n[1] = 0;
+  h->last_n_corr = 0;
+  stamp_last(h, {kLastCorr, kLastNn});
   if (n_src == 0 || n_tgt == 0) return QB200_OK;
   int rc = wave_reset(L, 2);
   if (rc) return rc;
   h->last_match_n[0] = n_src; h->last_match_n[1] = n_tgt;
+  stamp_last(h, {kLastNn});
   MirrorHold hold{L};
   // the features as a feature wave of one pair imports them (the import writes the clouds' counts)
   L->h_feat[0] = {reinterpret_cast<const float4*>(src4), src_desc33, n_src, 0};
@@ -142,6 +146,7 @@ int qb200_match(qb200_handle* h, const float* src4, int32_t n_src, const float* 
   QB_CUDA_TRY(h, hold.sync());
   if (n_mutual) *n_mutual = L->hctr.n_mutual[0];
   h->last_n_corr = L->hctr.n_corr[0];
+  stamp_last(h, {kLastCorr});
   if ((rc = qb200_get_last_correspondences(h, corr, nullptr, nullptr, cap, n_corr))) return rc;
   return L->hctr.cloud_status[0] == QB200_CAPACITY_EXCEEDED ? QB200_CAPACITY_EXCEEDED : QB200_OK;
 }
@@ -168,6 +173,7 @@ int qb200_match_and_pack(qb200_handle* h, const float* src4, int32_t n_src, cons
   if ((rc = launch_match(L, 1, 0)) || (rc = read_counters(L))) return rc;
   QB_CUDA_TRY(h, hold.sync());
   h->last_n_corr = L->hctr.n_corr[0];
+  stamp_last(h, {kLastCorr, kLastFeatures});
   if ((rc = qb200_get_last_correspondences(h, corr, src_matched4, tgt_matched4, cap, n_corr))) return rc;
   return L->hctr.cloud_status[0] == QB200_CAPACITY_EXCEEDED ? QB200_CAPACITY_EXCEEDED : QB200_OK;
 }
@@ -243,6 +249,7 @@ int qb200_max_clique_ex(qb200_handle* h, const uint32_t* adj, int32_t L, int32_t
   if (kcore_order) QB_CUDA_TRY(h, cudaMemcpyAsync(kcore_order, ln->korder, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, ln->stream));
   QB_CUDA_TRY(h, cudaStreamSynchronize(ln->stream));
   h->last_n_clique = nc;
+  stamp_last(h, {kLastClique});
   return QB200_OK;
 }
 
@@ -275,6 +282,7 @@ int qb200_solve_pose(qb200_handle* h, const float* a4, const float* b4, int32_t 
   QB_CUDA_TRY(h, hold.sync());
   *res = ln->h_results[0];
   set_last(h, *res);
+  stamp_last(h, {kLastClique, kLastFinal});  // the points are the caller's: no correspondences were packed
   if (res->status < 0) return res->status;
   if (res->valid) {
     const int nc = res->clique_size;
@@ -295,10 +303,15 @@ int qb200_solve_correspondences(qb200_handle* h, const float* a4, const float* b
 }
 
 // ---- introspection ----------------------------------------------------------------------------------
+// Slot 0 of lane 0 holds a single-pair call's lists only until the next wave on lane 0 rewrites it.  Each getter hands out its list
+// only if the most recent single-pair call that produced it was also the last call to run a wave on lane 0 (stamp_last); otherwise
+// it refuses (QB200_ERR_BAD_ARG, n = 0) rather than pair that call's count with another wave's entries.
 int qb200_get_last_clique(qb200_handle* h, int32_t* idx, int32_t cap, int32_t* n) {
   if (int rc = enter(h)) return rc;
   if (!n || cap < 0) return QB200_ERR_BAD_ARG;
   Lane* L = h->lane[0].get();
+  *n = 0;
+  if (!last_is_live(h, kLastClique)) return QB200_ERR_BAD_ARG;
   *n = h->last_n_clique;
   const int m = *n < cap ? *n : cap;
   if (m > 0 && idx) {
@@ -312,6 +325,8 @@ int qb200_get_last_final_inliers(qb200_handle* h, int32_t* idx, int32_t cap, int
   if (int rc = enter(h)) return rc;
   if (!n || cap < 0) return QB200_ERR_BAD_ARG;
   Lane* L = h->lane[0].get();
+  *n = 0;
+  if (!last_is_live(h, kLastFinal)) return QB200_ERR_BAD_ARG;
   *n = h->last_n_final;
   const int m = *n < cap ? *n : cap;
   if (m > 0 && idx) {
@@ -326,6 +341,8 @@ int qb200_get_last_correspondences(qb200_handle* h, int32_t* corr, float* src_ma
   if (int rc = enter(h)) return rc;
   if (!n || cap < 0) return QB200_ERR_BAD_ARG;
   Lane* L = h->lane[0].get();
+  *n = 0;
+  if (!last_is_live(h, kLastCorr)) return QB200_ERR_BAD_ARG;
   *n = h->last_n_corr;
   const int m = *n < cap ? *n : cap;
   if (m > 0) {
@@ -345,6 +362,8 @@ int qb200_get_last_features(qb200_handle* h, int32_t which, float* normals4, flo
   if (int rc = enter(h)) return rc;
   if (!n_out || which < 0 || which > 1 || cap < 0) return QB200_ERR_BAD_ARG;
   Lane* L = h->lane[0].get();
+  *n_out = 0;
+  if (!last_is_live(h, kLastFeatures)) return QB200_ERR_BAD_ARG;
   if (int rc = read_counters(L)) return rc;
   QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   const int n = L->hctr.n_vox[which];
@@ -375,6 +394,7 @@ int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, 
   if (int rc = enter(h)) return rc;
   if (cap_rows < 0 || cap_cols < 0) return QB200_ERR_BAD_ARG;
   Lane* L = h->lane[0].get();
+  if (!last_is_live(h, kLastNn)) return QB200_ERR_BAD_ARG;
   QB_CUDA_TRY(h, cudaStreamSynchronize(L->stream));
   const int nr = cap_rows < h->last_match_n[0] ? cap_rows : h->last_match_n[0];
   const int nc = cap_cols < h->last_match_n[1] ? cap_cols : h->last_match_n[1];
