@@ -38,6 +38,8 @@
  *                                  a batch, the graph handed out (include/quatro.hpp:307-386, 784-789)
  *   qb200_solve_pose_batch_*    <- the tail of Quatro::computeTransformation (chain TIMs + GNC-TLS yaw + COTE + final inliers) for
  *                                  every caller inlier set of a batch (include/quatro.hpp:806-936)
+ *   qb200_align_batch_*         <- pcl::transformPointCloud of the source scan and of the matched keypoints + the good-match loop
+ *                                  for every registered pair of a batch (examples/run_global_registration.cpp:253-288)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes, no C++/torch types.  All pointers are HOST pointers
@@ -869,6 +871,73 @@ int qb200_solve_pose_batch_each(qb200_handle* h, const qb200_inlier_set* sets, i
  * the flush returns.  Records and lists are byte-identical to the blocking call's. */
 int qb200_solve_pose_batch_enqueue_each(qb200_handle* h, const qb200_inlier_set* sets, int32_t n_sets, const qb200_params* params,
                                         qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+
+/* --- aligned scans and good matches of registered pairs in batches --------------------------------------------------------------------
+ * The example's last step after computeTransformation (examples/run_global_registration.cpp:253-288) for every pair of a batch: the
+ * source scan transformed by the pose (`aligned`, :257-258), the matched source keypoints transformed (`transformed_srcMatched`,
+ * :261-262), and the correspondences whose transformed source keypoint lies closer than voxel_size * 3.0 to its target keypoint
+ * (`good_matched_pcl`, :264-288).  A loop-closure back end reads the good-match count as its accept / reject statistic and fuses the
+ * aligned scan into its map, without taking the poses and lists to the host.  Sets run in waves of max_batch_slots over the lanes
+ * like every batch call.
+ *   Set i transforms its cloud (cloud, n_points) and its correspondences (corr, n_corr, indexing src_kp and tgt_kp) by T.  Only
+ *     params[i].voxel_size is read, as the threshold 3.0 * (double)voxel_size; every other field is ignored and not checked.  A
+ *     registration record's T, a qb200_pair_lists corr row and the keypoints of qb200_describe_batch_each are a set as they are.
+ *   Transform.  Every point x, y, z (widened to double) becomes (float)(T(r,0)*x + T(r,1)*y + T(r,2)*z + T(r,3)) for r = 0, 1, 2,
+ *     evaluated left to right in double with every product and sum rounded (no fused multiply-add): pcl::transformPointCloud with a
+ *     Matrix4d.  w is copied.  A point whose x, y or z is not finite is copied through unchanged, as PCL does for a cloud that is not
+ *     dense.  The cast overflows to +-inf past the float range.
+ *   aligned4.  Entry j of set i is its cloud's point j transformed.
+ *   matched4.  Entry k is src_kp[corr[k][0]] transformed, in correspondence order (`transformed_srcMatched`).
+ *   Good matches.  Correspondence k is good when sqrt(dx*dx + dy*dy + dz*dz) < 3.0 * (double)voxel_size, with d = the float
+ *     matched4 entry k minus the float tgt_kp[corr[k][1]], each widened to double, the three squares summed in that order and the
+ *     square root rounded correctly.  The example writes pow(d, 2); it is taken as d*d here, since pow is not correctly rounded
+ *     everywhere.  A distance exactly at the threshold is not good; a non-finite one never is.  good_ids are the ids k of the good
+ *     correspondences, ascending; good4 entry j is matched4 entry good_ids[j] (`good_matched_pcl`).
+ *   Counts and status.  counts[i] = {n_points, n_corr, n_good}, never clipped.  Set i's entries start at i * cap_points in aligned4 and
+ *     at i * cap_corr in the other arrays; it gets min(count, cap) of each, and nothing past that is written, so a count above the cap
+ *     shows the clipping.  status[i] is QB200_OK, or QB200_ERR_BAD_ARG for a set refused alone: a correspondence index outside
+ *     [0, n_src) or [0, n_tgt).  This is decided on the device; the refused set gets no counts and no entries, and the other sets are
+ *     unaffected.  Duplicate correspondences are taken as they are.
+ *   Equality.  Every output of a set is byte-identical to what the same call on that set alone writes.  No output depends on the batch,
+ *     the wave, the lane, QB200_LANES, the input or output memory kinds, or the other sets.
+ *   Limits.  n_points <= max_raw_points, n_src and n_tgt <= max_voxel_points, n_corr <= max_corr.
+ *   Checks run before anything starts or is queued: n < 0; a NULL sets array; an unknown kind or out->kind; a NULL out; a negative
+ *     cap, or a cap < 1 with its array given; a NULL params entry or one whose voxel_size is not > 0; a negative count or one over its
+ *     limit; a NULL array with a count > 0; a T entry that is not finite; and in QB200_MEM_DEVICE kind (inputs or outputs) an array
+ *     that is not memory of the handle's device or is misaligned (points 16-byte, corr 8-byte, good_ids 4-byte).  A rejected call gives
+ *     QB200_ERR_BAD_ARG, writes no count, status or entry, queues nothing, and qb200_last_error names the set, entry or array; batches
+ *     already queued still complete on the flush.
+ *   Host-kind inputs cross PCIe on the handle's copy stream; device-kind inputs are read in place.  Like the describe calls it
+ *     registers nothing: qb200_get_stage_ms and qb200_get_kernel_ms report zeros after it.
+ * QB200_MEM_HOST outputs are complete when the call returns (enqueue: when the flush returns); QB200_MEM_DEVICE outputs are written by the
+ * call's stream work under the same rule.  The sets and params arrays and the output descriptor are copied by the call. */
+typedef struct qb200_align_set {
+  const float* cloud;     /* n_points x {x,y,z,w}: the cloud to align (the raw source scan, or any cloud), or NULL with n_points = 0 */
+  const float* src_kp;    /* n_src x 4 source voxel keypoints (srcFeat): the cloud corr's first column indexes */
+  const float* tgt_kp;    /* n_tgt x 4 target voxel keypoints (tgtFeat): the cloud corr's second column indexes */
+  const int32_t* corr;    /* n_corr x {src idx, tgt idx}, e.g. a qb200_pair_lists corr row, or NULL with n_corr = 0 */
+  int32_t n_points, n_src, n_tgt, n_corr;
+  double T[16];           /* column-major 4x4, as in qb200_result.T */
+} qb200_align_set;
+typedef struct qb200_align_out {
+  int32_t cap_points;     /* entries per set in aligned4 */
+  int32_t cap_corr;       /* entries per set in matched4 / good_ids / good4 */
+  int32_t kind;           /* qb200_mem_kind of the four arrays below */
+  int32_t reserved;
+  float* aligned4;        /* [n][cap_points][4]  the cloud transformed                                (:257-258) */
+  float* matched4;        /* [n][cap_corr][4]    src_kp[corr[k][0]] transformed, correspondence order (:261-262) */
+  int32_t* good_ids;      /* [n][cap_corr]       ids k of the good correspondences, ascending */
+  float* good4;           /* [n][cap_corr][4]    good_matched_pcl: matched4 entries of those ids      (:264-288) */
+  int32_t* counts;        /* host [n][3]: n_points, n_corr, n_good, never clipped */
+  int32_t* status;        /* host [n] */
+} qb200_align_out;        /* any array may be NULL: nothing is written to it */
+int qb200_align_batch_each(qb200_handle* h, const qb200_align_set* sets, int32_t n_sets, const qb200_params* params,
+                           qb200_mem_kind kind, const qb200_align_out* out);
+/* qb200_align_batch_each, queued: completed by qb200_register_batch_flush like every enqueue, in one stream with every other enqueue
+ * form.  Host-kind inputs and every output array (counts and status included) must stay valid until the flush returns, which
+ * completes them.  The outputs are byte-identical to the blocking call's. */
+int qb200_align_batch_enqueue_each(qb200_handle* h, const qb200_align_set* sets, int32_t n_sets, const qb200_params* params,
+                                   qb200_mem_kind kind, const qb200_align_out* out);
 
 /* --- multi-GPU: batches of independent pairs shard across the GPUs of one box; the only communication is ONE all-gather (NCCL over
  * NVLink) of the fixed-size result records per batch -- north_star / SURVEY.md 8(e).  The reference has no counterpart (it is a

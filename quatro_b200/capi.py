@@ -105,6 +105,24 @@ class InlierSet(C.Structure):
     _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("inliers", C.c_void_p), ("L", C.c_int32), ("n_inliers", C.c_int32)]
 
 
+class AlignSet(C.Structure):
+    """qb200_align_set: one registered pair of qb200_align_batch_each: the cloud to align, the voxel keypoints of both sides, the
+    correspondences between them and the pose (column-major, as Result.T)."""
+    _fields_ = [("cloud", C.c_void_p), ("src_kp", C.c_void_p), ("tgt_kp", C.c_void_p), ("corr", C.c_void_p), ("n_points", C.c_int32),
+                ("n_src", C.c_int32), ("n_tgt", C.c_int32), ("n_corr", C.c_int32), ("T", C.c_double * 16)]
+
+
+class AlignOut(C.Structure):
+    """qb200_align_out: caller-owned outputs of qb200_align_batch_each, cap_points aligned points and cap_corr entries of each
+    correspondence array reserved per set."""
+    _fields_ = [("cap_points", C.c_int32), ("cap_corr", C.c_int32), ("kind", C.c_int32), ("reserved", C.c_int32),
+                ("aligned4", C.c_void_p), ("matched4", C.c_void_p), ("good_ids", C.c_void_p), ("good4", C.c_void_p),
+                ("counts", C.c_void_p), ("status", C.c_void_p)]
+
+
+ALIGN_ARRAYS = {"aligned4": (np.float32, (4,)), "matched4": (np.float32, (4,)), "good_ids": (np.int32, ()), "good4": (np.float32, (4,))}
+
+
 class GraphOut(C.Structure):
     """qb200_graph_out: caller-owned outputs of qb200_build_graph_batch_each: adjacency rows, degrees and edge lists of every set."""
     _fields_ = [("kind", C.c_int32), ("rows_per_set", C.c_int32), ("words_per_row", C.c_int32), ("reserved", C.c_int32),
@@ -344,6 +362,8 @@ _SIGNATURES = {
     "qb200_build_graph_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(GraphOut)]),
     "qb200_solve_pose_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_solve_pose_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_align_batch_each": (i32, [vp, vp, i32, P(Params), i32, P(AlignOut)]),
+    "qb200_align_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, P(AlignOut)]),
 }
 del vp, i32, i64, f32, f64, P
 EXPORTED_SYMBOLS = list(_SIGNATURES)
@@ -446,6 +466,32 @@ def _inlier_array(sets: Sequence, inliers: Sequence, kind: int):
             arr[i].inliers, arr[i].n_inliers = (ids.ctypes.data if len(ids) else None), len(ids)
         else:
             arr[i].inliers, arr[i].n_inliers = ids[0], ids[1]
+    return arr, keep
+
+
+def _align_array(sets: Sequence, kind: int):
+    """(AlignSet * n) array of `sets`: each a dict with cloud, src_kp, tgt_kp ((n,4) float32), corr ((m,2) int32) and T (4x4, row-major
+    as Result.matrix() gives it) for MEM_HOST, or with (device_ptr, n) tuples in place of the arrays for MEM_DEVICE (cloud may be None);
+    and the contiguous host arrays it points to."""
+    arr = (AlignSet * max(len(sets), 1))()
+    keep = []
+    for i, st in enumerate(sets):
+        e = arr[i]
+        for name, count, cols, dt in (("cloud", "n_points", 4, np.float32), ("src_kp", "n_src", 4, np.float32),
+                                      ("tgt_kp", "n_tgt", 4, np.float32), ("corr", "n_corr", 2, np.int32)):
+            a = st.get(name)
+            if kind == MEM_HOST:
+                a = np.ascontiguousarray(np.zeros((0, cols)) if a is None else a, dt).reshape(-1, cols)
+                keep.append(a)
+                setattr(e, name, a.ctypes.data if len(a) else None)
+                setattr(e, count, len(a))
+            else:
+                ptr, n = (None, 0) if a is None else a
+                setattr(e, name, ptr)
+                setattr(e, count, int(n))
+        T = np.asarray(st["T"], np.float64).reshape(4, 4)
+        for k, v in enumerate(T.T.ravel()):
+            e.T[k] = float(v)
     return arr, keep
 
 
@@ -1001,6 +1047,61 @@ class Handle:
         return self._check(self.lib.qb200_build_graph_batch_enqueue_each(self.h, set_array, n, params_array, kind, _ptr(out),
                                                                          C.byref(buffers.descriptor())),
                            "qb200_build_graph_batch_enqueue_each")
+
+    # ---- registered pairs -> aligned clouds and good matches (qb200_align_batch_each) ----
+    align_array = staticmethod(_align_array)
+
+    def align_buffers(self, n: int, cap_points: int, cap_corr: int, dest: int = MEM_HOST, arrays=tuple(ALIGN_ARRAYS)) -> dict:
+        """Zeroed output arrays of an align call by name: numpy (dest MEM_HOST) or CUDA tensors of the handle's device (MEM_DEVICE), of
+        shape (n, cap_points, 4) for aligned4 and (n, cap_corr, ...) for the others."""
+        def shape(k):
+            return (max(n, 1), cap_points if k == "aligned4" else cap_corr, *ALIGN_ARRAYS[k][1])
+        if dest == MEM_HOST:
+            return {k: np.zeros(shape(k), ALIGN_ARRAYS[k][0]) for k in arrays}
+        import torch
+        dt = {np.float32: torch.float32, np.int32: torch.int32}
+        return {k: torch.zeros(shape(k), dtype=dt[ALIGN_ARRAYS[k][0]], device=f"cuda:{self.cfg.device}") for k in arrays}
+
+    @staticmethod
+    def align_out(cap_points: int, cap_corr: int, dest: int, arrays: dict, counts: Optional[np.ndarray],
+                  status: Optional[np.ndarray]) -> AlignOut:
+        """The qb200_align_out of `arrays` (align_buffers()) and the host int32 arrays counts ((n, 3)) / status; a name left out, or a
+        None, is NULL."""
+        out = AlignOut(cap_points, cap_corr, dest)
+        for k, a in arrays.items():
+            setattr(out, k, a.ctypes.data if dest == MEM_HOST else a.data_ptr())
+        out.counts = None if counts is None else counts.ctypes.data
+        out.status = None if status is None else status.ctypes.data
+        return out
+
+    def align_batch_each(self, sets: Sequence, params: Sequence[Params], kind: int = MEM_HOST, dest: int = MEM_HOST,
+                         cap_points: Optional[int] = None, cap_corr: Optional[int] = None, arrays: Optional[dict] = None):
+        """qb200_align_batch_each: set i (see align_array()) is aligned with the threshold 3 * params[i].voxel_size.  cap_points /
+        cap_corr: entries reserved per set (default max_raw_points / max_corr).  arrays: the caller's own outputs by name
+        (ALIGN_ARRAYS), numpy for dest MEM_HOST or CUDA tensors for MEM_DEVICE; a name left out is NULL.  Returns (per set a dict of
+        its arrays trimmed to min(count, cap): numpy copies, tensor views on the device; counts (n, 3) int32; status (n,) int32)."""
+        n = len(sets)
+        assert len(params) == n
+        cp = self.cfg.max_raw_points if cap_points is None else cap_points
+        cc = self.cfg.max_corr if cap_corr is None else cap_corr
+        arrays = self.align_buffers(n, cp, cc, dest) if arrays is None else arrays
+        counts, status = np.zeros((max(n, 1), 3), np.int32), np.zeros(max(n, 1), np.int32)
+        arr, keep = self.align_array(sets, kind)
+        out = self.align_out(cp, cc, dest, arrays, counts, status)
+        self._check(self.lib.qb200_align_batch_each(self.h, arr, n, self.params_array(params), kind, C.byref(out)),
+                    "qb200_align_batch_each")
+        per_set = []
+        for i in range(n):
+            m = {"aligned4": min(int(counts[i, 0]), cp), "matched4": min(int(counts[i, 1]), cc), "good_ids": min(int(counts[i, 2]), cc),
+                 "good4": min(int(counts[i, 2]), cc)}
+            per_set.append({k: (a[i, :m[k]].copy() if dest == MEM_HOST else a[i, :m[k]]) for k, a in arrays.items()})
+        return per_set, counts[:n], status[:n]
+
+    def align_batch_enqueue_each_raw(self, align_array, n: int, params_array, kind: int, out: AlignOut):
+        """qb200_align_batch_enqueue_each: align_array (align_array()), params_array (params_array()) and the descriptor `out`
+        (align_out()) are read by the call; host-kind inputs and every array `out` names must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_align_batch_enqueue_each(self.h, align_array, n, params_array, kind, C.byref(out)),
+                           "qb200_align_batch_enqueue_each")
 
     # ---- caller inlier sets -> poses (qb200_solve_pose_batch_each) ----
     inlier_array = staticmethod(_inlier_array)

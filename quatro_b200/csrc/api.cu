@@ -106,6 +106,8 @@ int lane_alloc(const Lane& like, std::unique_ptr<Lane>* out) {
   QB_CUDA_TRY(L, L->h_graph.alloc(S));
   QB_CUDA_TRY(L, L->d_inl.alloc(S));
   QB_CUDA_TRY(L, L->h_inl.alloc(S));
+  QB_CUDA_TRY(L, L->d_aln.alloc(S));
+  QB_CUDA_TRY(L, L->h_aln.alloc(S));
   // the sort workspace serves the voxel sort (C*R items, digit histograms in val_a, chunk counts C*kVsChunks <= n_sort in val_b),
   // the lattice / norm sorts (C*V items) and, afterwards, the duplicate-class tables of K6 (2S*V + 2S words in key_a): size it for
   // the largest user
@@ -515,6 +517,7 @@ struct BatchCall {
   const qb200_corr_set* sets = nullptr;        // CorrSets
   const qb200_graph* graphs = nullptr;         // Graphs
   const qb200_inlier_set* inlier_sets = nullptr;  // InlierSets
+  const qb200_align_set* align_sets = nullptr;    // AlignSets
   const float* const* scans = nullptr;         // RawScans, KeypointClouds (described with the lattice fields of their entries alone):
   const int32_t* n_points = nullptr;           // scan i has n_points[i] points
   // the outputs, one set per sink
@@ -523,6 +526,7 @@ struct BatchCall {
   const int32_t* slot_ids = nullptr;           // CacheSlots: scan i goes to slot slot_ids[i]
   const qb200_feature_out* out = nullptr;      // Export: the caller's feature arrays
   const qb200_graph_out* graph_out = nullptr;  // Graph: the caller's adjacency, degree and edge arrays
+  const qb200_align_out* align_out = nullptr;  // AlignOut: the caller's aligned clouds, matched points, good matches, counts and status
   // set by enqueue_call.  The params the pairs are solved with, rotation noise bounds resolved (Solve, Pose), laid out like `caller`.
   const qb200_params* params = nullptr;
   // host inputs of a multi-wave batch crossing PCIe: the batch's copy stream, or nullptr = copy on the lane's own stream.  Copies
@@ -535,12 +539,12 @@ struct BatchCall {
 // The facts of each source that the checks and the waves read, written down once
 
 // clouds one input takes in the wave's 2S cloud buffers: two per pair, one per scan, none per set (its matched points go to ma / mb,
-// an inlier set's ids to clique) or graph (its adjacency goes to adj)
+// an inlier set's ids to clique), graph (its adjacency goes to adj) or align set (read through its own table entry)
 int clouds_per_input(Source s) {
   switch (s) {
     case Source::RawPairs: case Source::CachedPairs: case Source::FeaturePairs: return 2;
     case Source::RawScans: case Source::KeypointClouds: return 1;
-    case Source::CorrSets: case Source::Graphs: case Source::InlierSets: return 0;
+    case Source::CorrSets: case Source::Graphs: case Source::InlierSets: case Source::AlignSets: return 0;
   }
   return 0;
 }
@@ -548,11 +552,12 @@ int clouds_per_input(Source s) {
 // the wave matches pairs of clouds (K6..K7) before its records: the solver's counters come from a front end (have_frontend)
 bool is_pairs(Source s) { return clouds_per_input(s) == 2; }
 
-// Host-kind inputs of the source cross PCIe in a staged front (stage_raw, stage_features): a multi-wave batch sends them on the
-// shared copy stream and opens with a quarter wave.  Cached pairs, correspondence sets, graphs and inlier sets do neither.
+// Host-kind inputs of the source cross PCIe in a staged front (stage_raw, stage_features, front_align): a multi-wave batch sends them
+// on the shared copy stream and opens with a quarter wave.  Cached pairs, correspondence sets, graphs and inlier sets do neither.
 bool crosses_pcie(Source s) {
   switch (s) {
-    case Source::RawPairs: case Source::FeaturePairs: case Source::RawScans: case Source::KeypointClouds: return true;
+    case Source::RawPairs: case Source::FeaturePairs: case Source::RawScans: case Source::KeypointClouds: case Source::AlignSets:
+      return true;
     case Source::CachedPairs: case Source::CorrSets: case Source::Graphs: case Source::InlierSets: return false;
   }
   return false;
@@ -563,7 +568,9 @@ bool crosses_pcie(Source s) {
 bool runs_front_end(Source s) {
   switch (s) {
     case Source::RawPairs: case Source::RawScans: case Source::KeypointClouds: return true;
-    case Source::CachedPairs: case Source::FeaturePairs: case Source::CorrSets: case Source::Graphs: case Source::InlierSets: return false;
+    case Source::CachedPairs: case Source::FeaturePairs: case Source::CorrSets: case Source::Graphs: case Source::InlierSets:
+    case Source::AlignSets:
+      return false;
   }
   return false;
 }
@@ -588,7 +595,7 @@ unsigned stage_slots(Source s, Sink k) {
     case Source::FeaturePairs: m = kH2d | kMatch | kSolver | kD2h; break;
     case Source::CachedPairs: m = kFpfh | kMatch | kSolver; break;
     case Source::CorrSets: m = kSolver; break;
-    case Source::RawScans: case Source::KeypointClouds: case Source::Graphs: case Source::InlierSets: break;
+    case Source::RawScans: case Source::KeypointClouds: case Source::Graphs: case Source::InlierSets: case Source::AlignSets: break;
   }
   return k == Sink::Match ? (m & (kH2d | kVoxel | kFpfh | kMatch)) | kD2h : m;
 }
@@ -735,6 +742,24 @@ int check_graph_out(qb200_handle* h, const qb200_graph_out* o) {
   else if (device && !device_array_of(h, o->adj, 4)) why = "device adj is misaligned or not memory of the handle's device";
   else if (device && !device_array_of(h, o->degree, 4)) why = "device degree is misaligned or not memory of the handle's device";
   else if (device && !device_array_of(h, o->edges, 8)) why = "device edges is misaligned or not memory of the handle's device";
+  if (!why) return QB200_OK;
+  h->fail(__FILE__, __LINE__, why);
+  return QB200_ERR_BAD_ARG;
+}
+
+// The output descriptor of an align call: a known kind, caps that are not negative and at least 1 for the arrays given, and device
+// arrays on the handle's device and aligned for the kernels' stores
+int check_align_out(qb200_handle* h, const qb200_align_out* o) {
+  const char* why = nullptr;
+  const bool device = o && o->kind == QB200_MEM_DEVICE;
+  if (!o) why = "the output descriptor is null";
+  else if (o->kind != QB200_MEM_HOST && o->kind != QB200_MEM_DEVICE) why = "unknown memory kind of the outputs";
+  else if (o->cap_points < 0 || o->cap_corr < 0) why = "cap_points or cap_corr < 0";
+  else if (o->aligned4 && o->cap_points < 1) why = "cap_points < 1 with aligned4";
+  else if ((o->matched4 || o->good_ids || o->good4) && o->cap_corr < 1) why = "cap_corr < 1 with matched4, good_ids or good4";
+  else if (device && !(device_array_of(h, o->aligned4, 16) && device_array_of(h, o->matched4, 16) && device_array_of(h, o->good4, 16)))
+    why = "device aligned4, matched4 or good4 is misaligned (16 bytes) or not memory of the handle's device";
+  else if (device && !device_array_of(h, o->good_ids, 4)) why = "device good_ids is misaligned (4 bytes) or not memory of the handle's device";
   if (!why) return QB200_OK;
   h->fail(__FILE__, __LINE__, why);
   return QB200_ERR_BAD_ARG;
@@ -1041,6 +1066,119 @@ int deliver_graph(Lane* L, const qb200_graph_out& o, int w0, int np) {
   return QB200_OK;
 }
 
+// Align sets: every set's table entry (its pose rows, threshold, counts, caps and where it is read and written), host-kind inputs
+// staged: clouds back to back in raw_stage (at h_raw_off), source and target keypoints in the set's two slots of vox_pts, correspondences
+// in aln_stage.  Host-kind outputs go to staging that wave_collect copies out: aligned clouds to the set's raw_stage region (in place
+// for a host cloud), the correspondence outputs to aln_stage.  Device arrays are read and written in place.  Host inputs of a
+// multi-wave batch cross on the batch's copy stream, and the lane waits for them.
+int front_align(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np, int* n_blocks) {
+  const qb200_align_out& o = *in.align_out;
+  const bool host = in.kind == QB200_MEM_HOST, host_out = o.kind == QB200_MEM_HOST;
+  const cudaStream_t cs = in.copy_stream ? in.copy_stream : L->stream;
+  if ((host || host_out) && !L->aln_stage) QB_CUDA_TRY(L, L->aln_stage.alloc(AlignStage::bytes(L->S, L->Lc)));
+  const AlignStage st = L->aln_stage ? AlignStage::carve(L->aln_stage, L->S, L->Lc) : AlignStage{};
+  if (int rc = wave_reset(L, 0)) return rc;
+  auto h2d = [&](void* dst, const void* src, size_t bytes) -> int {
+    if (bytes) QB_CUDA_TRY(L, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, cs));
+    return QB200_OK;
+  };
+  int raw = 0, blocks = 0;
+  for (int s = 0; s < np; ++s) {
+    const qb200_align_set& a = in.align_sets[w0 + s];
+    const long long i = w0 + s;
+    AlignSrc& e = L->h_aln[s];
+    memset(&e, 0, sizeof(e));
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 4; ++c) e.T[4 * r + c] = a.T[4 * c + r];  // column-major in, T(r, c) out
+    e.thr = 3.0 * (double)in.caller[i].voxel_size;
+    e.n_points = a.n_points; e.n_src = a.n_src; e.n_tgt = a.n_tgt; e.n_corr = a.n_corr;
+    e.cap_points = o.cap_points; e.cap_corr = o.cap_corr;
+    e.cloud = reinterpret_cast<const float4*>(a.cloud);
+    e.src_kp = reinterpret_cast<const float4*>(a.src_kp);
+    e.tgt_kp = reinterpret_cast<const float4*>(a.tgt_kp);
+    e.corr = reinterpret_cast<const int2*>(a.corr);
+    float4* region = L->raw_stage + raw;
+    L->h_raw_off[s] = raw;
+    raw += a.n_points;
+    if (host) {
+      float4* sk = L->vox_pts + (size_t)s * L->V;
+      float4* tk = L->vox_pts + (size_t)(L->S + s) * L->V;
+      int2* cr = st.corr + (size_t)s * L->Lc;
+      int rc;
+      if ((o.aligned4 && (rc = h2d(region, a.cloud, (size_t)a.n_points * sizeof(float4)))) ||
+          (rc = h2d(sk, a.src_kp, (size_t)a.n_src * sizeof(float4))) || (rc = h2d(tk, a.tgt_kp, (size_t)a.n_tgt * sizeof(float4))) ||
+          (rc = h2d(cr, a.corr, (size_t)a.n_corr * sizeof(int2))))
+        return rc;
+      e.cloud = region; e.src_kp = sk; e.tgt_kp = tk; e.corr = cr;
+    }
+    if (host_out) {
+      if (o.aligned4) e.aligned = region;
+      if (o.matched4) e.matched = st.matched + (size_t)s * L->Lc;
+      if (o.good4) e.good = st.good + (size_t)s * L->Lc;
+      if (o.good_ids) e.good_ids = st.ids + (size_t)s * L->Lc;
+    } else {
+      if (o.aligned4) e.aligned = reinterpret_cast<float4*>(o.aligned4) + i * o.cap_points;
+      if (o.matched4) e.matched = reinterpret_cast<float4*>(o.matched4) + i * o.cap_corr;
+      if (o.good4) e.good = reinterpret_cast<float4*>(o.good4) + i * o.cap_corr;
+      if (o.good_ids) e.good_ids = o.good_ids + i * o.cap_corr;
+    }
+    e.blk0 = blocks;
+    if (o.aligned4) blocks += (std::min(a.n_points, o.cap_points) + kAlignPts - 1) / kAlignPts;
+  }
+  *n_blocks = blocks;
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->d_aln, L->h_aln, (size_t)np * sizeof(AlignSrc), cudaMemcpyHostToDevice, L->stream));
+  if (in.copy_stream) {
+    QB_CUDA_TRY(L, cudaEventRecord(h->ev_copied, in.copy_stream));
+    QB_CUDA_TRY(L, cudaStreamWaitEvent(L->stream, h->ev_copied, 0));
+  }
+  return QB200_OK;
+}
+
+// Align sets: the good matches (and the refusals) first, then the clouds of the sets that were not refused, then every set's status
+// and good count to the pinned mirror of the counter block
+int submit_align(Lane* L, int np, int n_blocks) {
+  int rc;
+  if ((rc = launch_align_good(L, np)) || (rc = launch_align_points(L, n_blocks, np))) return rc;
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->hctr.cloud_status, L->ctr.cloud_status, (size_t)np * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
+  QB_CUDA_TRY(L, cudaMemcpyAsync(L->hctr.n_final, L->ctr.n_final, (size_t)np * sizeof(int), cudaMemcpyDeviceToHost, L->stream));
+  return QB200_OK;
+}
+
+// A collected align wave: status and counts of every set to the caller's host arrays (a refused set: its status alone), and in host
+// kind the entries of every set that was not refused, from the staging its table entry names
+int deliver_align(Lane* L, const qb200_align_out& o, int w0, int np) {
+  bool copied = false;
+  auto d2h = [&](void* dst, const void* src, int m, size_t size) -> int {
+    if (dst && m > 0) {
+      QB_CUDA_TRY(L, cudaMemcpyAsync(dst, src, (size_t)m * size, cudaMemcpyDeviceToHost, L->stream));
+      copied = true;
+    }
+    return QB200_OK;
+  };
+  for (int s = 0; s < np; ++s) {
+    const AlignSrc& e = L->h_aln[s];
+    const int status = L->hctr.cloud_status[s], n_good = L->hctr.n_final[s];
+    const long long i = w0 + s;
+    if (o.status) o.status[i] = status;
+    if (status != QB200_OK) continue;
+    if (o.counts) {
+      o.counts[3 * i] = e.n_points;
+      o.counts[3 * i + 1] = e.n_corr;
+      o.counts[3 * i + 2] = n_good;
+    }
+    if (o.kind != QB200_MEM_HOST) continue;
+    const int mp = std::min(e.n_points, o.cap_points), mc = std::min(e.n_corr, o.cap_corr), mg = std::min(n_good, o.cap_corr);
+    int rc;
+    if ((rc = d2h(o.aligned4 ? o.aligned4 + 4 * i * o.cap_points : nullptr, e.aligned, mp, sizeof(float4))) ||
+        (rc = d2h(o.matched4 ? o.matched4 + 4 * i * o.cap_corr : nullptr, e.matched, mc, sizeof(float4))) ||
+        (rc = d2h(o.good_ids ? o.good_ids + i * o.cap_corr : nullptr, e.good_ids, mg, sizeof(int))) ||
+        (rc = d2h(o.good4 ? o.good4 + 4 * i * o.cap_corr : nullptr, e.good, mg, sizeof(float4))))
+      return rc;
+  }
+  if (copied) QB_CUDA_TRY(L, cudaStreamSynchronize(L->stream));
+  return QB200_OK;
+}
+
 // The end of every wave with records: the list pack, the D2H of the records
 int send_records(Lane* L, const BatchCall& in, int w0, int np) {
   if (in.lists)
@@ -1056,7 +1194,7 @@ int send_records(Lane* L, const BatchCall& in, int w0, int np) {
 // wave_collect hands the outputs on.  The lane's previous wave must have been collected.
 int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   const int ncl = np * clouds_per_input(in.src);
-  int rc;
+  int rc, n_blocks = 0;
   L->kev_armed[0] = L->kev_armed[1] = 0;
   L->pend_slots.clear();
   L->pend_writes = 0;
@@ -1068,6 +1206,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
     case Source::CorrSets: rc = front_sets(L, in, w0, np); break;
     case Source::Graphs: rc = front_graphs(L, in, w0, np); break;
     case Source::InlierSets: rc = front_inlier_sets(L, in, w0, np); break;
+    case Source::AlignSets: rc = front_align(h, L, in, w0, np, &n_blocks); break;
   }
   if (rc) return rc;
   const bool match_pairs = is_pairs(in.src);
@@ -1114,6 +1253,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       cudaEventRecord(L->ev[7], L->stream);
       rc = send_records(L, in, w0, np);
       break;
+    case Sink::AlignOut: rc = submit_align(L, np, n_blocks); break;
   }
   if (rc) return rc;
   L->pend_w0 = w0;
@@ -1125,6 +1265,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   if (in.lists) L->pend_lists = *in.lists;
   if (in.sink == Sink::Export || in.sink == Sink::Voxels) L->pend_out = *in.out;
   if (in.sink == Sink::Graph) L->pend_graph = *in.graph_out;
+  if (in.sink == Sink::AlignOut) L->pend_align = *in.align_out;
   return QB200_OK;
 }
 
@@ -1149,6 +1290,7 @@ int wave_collect(qb200_handle* h, Lane* L) {
       break;
     case Sink::CacheSlots: break;
     case Sink::Export: case Sink::Voxels: rc = deliver_export(L, L->pend_out, L->pend_w0, np, L->pend_sink == Sink::Voxels); break;
+    case Sink::AlignOut: rc = deliver_align(L, L->pend_align, L->pend_w0, np); break;
   }
   if (h->timeline && (L->pend_stages & 1u)) {  // stage boundaries of a raw-scan or feature wave relative to the start of the batch (ms): start, h2d, voxel, fpfh, match, graph, clique, pose, d2h
     fprintf(stderr, "[qb200 timeline] wave w0=%d np=%d:", L->pend_w0, np);
@@ -1240,6 +1382,7 @@ const void* input_of(const BatchCall& c) {
     case Source::RawScans: case Source::KeypointClouds: return c.scans;
     case Source::Graphs: return c.graphs;
     case Source::InlierSets: return c.inlier_sets;
+    case Source::AlignSets: return c.align_sets;
   }
   return nullptr;
 }
@@ -1283,6 +1426,13 @@ int check_call(qb200_handle* h, const BatchCall& c) {
         return reject(why);
       }
     }
+  } else if (c.sink == Sink::AlignOut) {  // only voxel_size is read: the good-match threshold
+    for (int i = 0; i < c.n; ++i) {
+      if (!p || !(p[i].voxel_size > 0)) {
+        snprintf(why, sizeof(why), "params entry %d is null or its voxel_size is not > 0", i);
+        return reject(why);
+      }
+    }
   } else if (c.sink == Sink::Graph) {  // only noise_bound and cbar2 are read, checked as qb200_build_graph checks them
     for (int i = 0; i < c.n; ++i) {
       if (!p || !(p[i].noise_bound > 0) || !(p[i].cbar2 > 0)) {
@@ -1310,6 +1460,8 @@ int check_call(qb200_handle* h, const BatchCall& c) {
     return reject("normals4 and desc33 must be null: a voxelize call returns voxel centroids alone");
   if (c.sink == Sink::Graph)
     if (int rc = check_graph_out(h, c.graph_out)) return rc;
+  if (c.sink == Sink::AlignOut)
+    if (int rc = check_align_out(h, c.align_out)) return rc;
   const int R = h->cfg.max_raw_points;
   for (int i = 0; i < c.n; ++i) {
     const char* bad = nullptr;
@@ -1373,6 +1525,27 @@ int check_call(qb200_handle* h, const BatchCall& c) {
           bad = "its points are misaligned (16 bytes) or not memory of the handle's device";
         else if (device && s.n_inliers > 0 && !device_array_of(h, s.inliers, 4))
           bad = "its inlier list is misaligned (4 bytes) or not memory of the handle's device";
+        if (bad) {
+          snprintf(why, sizeof(why), "set %d: %s", i, bad);
+          return reject(why);
+        }
+        break;
+      }
+      case Source::AlignSets: {
+        const qb200_align_set& s = c.align_sets[i];
+        const bool device = c.kind == QB200_MEM_DEVICE;
+        bool finite = true;
+        for (const double t : s.T) finite &= std::isfinite(t);
+        if (s.n_points < 0 || s.n_points > R) bad = "its n_points is outside 0 .. max_raw_points";
+        else if (s.n_src < 0 || s.n_src > h->cfg.max_voxel_points || s.n_tgt < 0 || s.n_tgt > h->cfg.max_voxel_points)
+          bad = "its n_src or n_tgt is outside 0 .. max_voxel_points";
+        else if (s.n_corr < 0 || s.n_corr > h->cfg.max_corr) bad = "its n_corr is outside 0 .. max_corr";
+        else if ((s.n_points > 0 && !s.cloud) || (s.n_src > 0 && !s.src_kp) || (s.n_tgt > 0 && !s.tgt_kp) || (s.n_corr > 0 && !s.corr))
+          bad = "an array with a count > 0 is null";
+        else if (!finite) bad = "its T has an entry that is not finite";
+        else if (device && !(device_array_of(h, s.cloud, 16) && device_array_of(h, s.src_kp, 16) && device_array_of(h, s.tgt_kp, 16) &&
+                             device_array_of(h, s.corr, 8)))
+          bad = "points (16-byte) or corr (8-byte) misaligned or not memory of the handle's device";
         if (bad) {
           snprintf(why, sizeof(why), "set %d: %s", i, bad);
           return reject(why);
@@ -1604,6 +1777,13 @@ BatchCall inlier_sets(const qb200_inlier_set* sets, int32_t n, const qb200_param
                       const qb200_pair_lists* lists) {
   BatchCall c{Source::InlierSets, Sink::Pose, n, kind, p, Entries::Mixed};
   c.inlier_sets = sets; c.results = results; c.lists = lists;
+  return c;
+}
+
+// each set is aligned with its own entry's voxel size
+BatchCall align_sets(const qb200_align_set* sets, int32_t n, const qb200_params* p, qb200_mem_kind kind, const qb200_align_out* out) {
+  BatchCall c{Source::AlignSets, Sink::AlignOut, n, kind, p, Entries::Mixed};
+  c.align_sets = sets; c.align_out = out;
   return c;
 }
 
@@ -1950,6 +2130,17 @@ int qb200_solve_pose_batch_each(qb200_handle* h, const qb200_inlier_set* sets, i
 int qb200_solve_pose_batch_enqueue_each(qb200_handle* h, const qb200_inlier_set* sets, int32_t n_sets, const qb200_params* params,
                                         qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
   return enqueue_call(h, inlier_sets(sets, n_sets, params, kind, results, lists));
+}
+
+// ---- registered pairs -> aligned clouds, transformed matches and good matches in caller memory -------------------------------------
+int qb200_align_batch_each(qb200_handle* h, const qb200_align_set* sets, int32_t n_sets, const qb200_params* params, qb200_mem_kind kind,
+                           const qb200_align_out* out) {
+  return run_call(h, align_sets(sets, n_sets, params, kind, out));
+}
+
+int qb200_align_batch_enqueue_each(qb200_handle* h, const qb200_align_set* sets, int32_t n_sets, const qb200_params* params,
+                                   qb200_mem_kind kind, const qb200_align_out* out) {
+  return enqueue_call(h, align_sets(sets, n_sets, params, kind, out));
 }
 
 int qb200_cache_copy(qb200_handle* h, int32_t from_slot, int32_t to_slot) {

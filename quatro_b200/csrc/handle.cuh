@@ -119,13 +119,33 @@ struct InlierSrc {
   int n, pad;
 };
 
+// One set of an align wave (align.cu), as the host resolved it: where its cloud, keypoints and correspondences are read (the caller's
+// device memory or the lane's staging), where its outputs go (the caller's device arrays from the set's first entry on, or the lane's
+// staging; nullptr = not asked for) and how many entries each receives, rows 0..2 of its pose and its good-match threshold.  blk0:
+// the set's first block of align_points_kernel.
+struct AlignSrc {
+  const float4* cloud;
+  const float4* src_kp;
+  const float4* tgt_kp;
+  const int2* corr;
+  float4* aligned;
+  float4* matched;
+  int* good_ids;
+  float4* good;
+  double T[12];              // T(r, c) at T[4 r + c]
+  double thr;                // 3.0 * (double)voxel_size
+  int n_points, n_src, n_tgt, n_corr;
+  int cap_points, cap_corr;
+  int blk0, pad;
+};
+
 // What a batch call reads (api.cu: BatchCall), per input: a pair of raw scans, a pair of cached scans (slots), a pair of caller
-// keypoint clouds with their FPFH-33 rows, a correspondence set, one raw scan, one caller keypoint cloud, one caller graph, or a
-// correspondence set with the caller's inlier ids
-enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, KeypointClouds, Graphs, InlierSets };
+// keypoint clouds with their FPFH-33 rows, a correspondence set, one raw scan, one caller keypoint cloud, one caller graph, a
+// correspondence set with the caller's inlier ids, or a registered pair to align (a cloud, keypoints, correspondences and a pose)
+enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, KeypointClouds, Graphs, InlierSets, AlignSets };
 // What a batch call produces: solved records (and lists), the matcher's records (and lists), cache slots, front-end features in
 // caller memory, max-clique records (and clique lists), TIM graphs in caller memory (and records), or poses of given inlier sets
-// (records and lists).  The valid (source, sink) pairs:
+// (records and lists), or aligned clouds and good matches in caller memory.  The valid (source, sink) pairs:
 //   RawPairs, CachedPairs, FeaturePairs  x  Solve, Match   qb200_register_batch*, _cached*, _features*; qb200_match_*
 //   CorrSets                             x  Solve, Graph   qb200_solve_batch*, qb200_build_graph_batch*
 //   RawScans                             x  CacheSlots     qb200_cache_scans*
@@ -133,8 +153,9 @@ enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, Key
 //   RawScans                             x  Voxels         qb200_voxelize_batch*
 //   Graphs                               x  Clique         qb200_max_clique_batch*
 //   InlierSets                           x  Pose           qb200_solve_pose_batch*
+//   AlignSets                            x  AlignOut       qb200_align_batch*
 // Voxels is Export without K2..K5: the voxel centroids alone, with qb200_voxelize's capacity and pass-through outputs
-enum class Sink { Solve, Match, CacheSlots, Export, Voxels, Clique, Graph, Pose };
+enum class Sink { Solve, Match, CacheSlots, Export, Voxels, Clique, Graph, Pose, AlignOut };
 
 // One lane: a stream and every device buffer of DESIGN §4 for one wave of S pairs.  Lane 0 is created with the handle; batches
 // of several waves rotate over up to 8 lanes, so the H2D copies and the latency-bound solver tail of one wave overlap the dense
@@ -163,6 +184,9 @@ struct Lane {
   DeviceMem<FeatureSrc> d_feat; PinnedMem<FeatureSrc> h_feat;  // [2S] where a feature wave's clouds are read, and its pinned mirror
   DeviceMem<GraphSrc> d_graph; PinnedMem<GraphSrc> h_graph;   // [S] where a graph wave's graphs are read, and its pinned mirror
   DeviceMem<InlierSrc> d_inl; PinnedMem<InlierSrc> h_inl;     // [S] where a pose wave's inlier ids are read, and its pinned mirror
+  DeviceMem<AlignSrc> d_aln; PinnedMem<AlignSrc> h_aln;       // [S] an align wave's sets, and its pinned mirror
+  DeviceMem<unsigned char> aln_stage;  // an align wave's host-kind correspondences and correspondence outputs, [S][Lc] of each
+                                       // (AlignStage), allocated on first use
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
   unsigned pend_stages;      // ... the stage-time slots it reports (bit i: qb200_get_stage_ms slot i)
   Sink pend_sink;             // ... what wave_collect hands on for it: the fields below of its sink
@@ -172,6 +196,8 @@ struct Lane {
   qb200_feature_out pend_out; // ... (Export, Voxels) a copy of its batch's output descriptor, whose counts and status (and, in host
                               // kind, entries) wave_collect hands on from exp_stage (and a Voxels wave's pass-through from raw_stage)
   qb200_graph_out pend_graph; // ... (Graph) a copy of its batch's output descriptor, whose host-kind arrays wave_collect writes
+  qb200_align_out pend_align; // ... (AlignOut) a copy of its batch's output descriptor, whose counts, status and host-kind arrays
+                              // wave_collect writes
   // ... and the cache slots it reads (cached pairs) or writes (CacheSlots), ascending and unique; empty: it does not touch the
   // cache.  A wave reads the cache only in its copy-in and writes it only in its copy-out, so other lanes order their conflicting
   // copies after those events (api.cu: cache_waits)
@@ -434,6 +460,27 @@ int launch_graph_records(Lane* h, int n_sets, long long cap_edges);
 // QB200_ERR_BAD_ARG record: valid 0, identity T, n_corr = L, the rest 0.
 int launch_inlier_import(Lane* h, int n_sets);
 int launch_pose_records(Lane* h, int n_sets);
+// Align waves (align.cu), sets [0, n) of the table d_aln: launch_align_good checks every set's correspondence indices (a set with one
+// outside [0, n_src) x [0, n_tgt) gets QB200_ERR_BAD_ARG in ctr.cloud_status and no output), writes the transformed source keypoints
+// and the good matches, and their count into ctr.n_final.  launch_align_points then transforms the clouds of the sets it did not
+// refuse; n_blocks: the blocks of every set (AlignSrc::blk0).
+int launch_align_good(Lane* h, int n_sets);
+int launch_align_points(Lane* h, int n_blocks, int n_sets);
+constexpr int kAlignPts = 1024;  // points per block of align_points_kernel
+// The lane's align staging (aln_stage), per set Lc entries of each array
+struct AlignStage {
+  int2* corr; float4* matched; float4* good; int* ids;
+  static size_t bytes(int S, int Lc) { return (size_t)S * Lc * (sizeof(int2) + 2 * sizeof(float4) + sizeof(int)); }
+  static AlignStage carve(unsigned char* base, int S, int Lc) {
+    const size_t n = (size_t)S * Lc;
+    AlignStage a;
+    a.matched = reinterpret_cast<float4*>(base);
+    a.good = a.matched + n;
+    a.corr = reinterpret_cast<int2*>(a.good + n);
+    a.ids = reinterpret_cast<int*>(a.corr + n);
+    return a;
+  }
+};
 // the checks every entry of a registering call passes; solver = false: the front-end and matcher fields only (a match call)
 bool params_ok(const qb200_params* p, bool solver = true);
 float lattice_cell(const qb200_params& p);
