@@ -617,6 +617,47 @@ int qb200_match_features_each(qb200_handle* h, const qb200_feature_pair* pairs, 
 int qb200_match_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                       qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
 
+/* --- caller descriptors of any length: match and register batches of pairs --------------------------------------------------------
+ * Matcher::calculateCorrespondences (include/teaser_utils/feature_matcher.h:42-74) reads the descriptor length from the features
+ * themselves, so it matches PCL's SHOT352 or PFHSignature125 and learned descriptors (FCGF, D3Feat: 32 floats) as well as FPFH-33.
+ * These four calls do the same for batches of pairs:
+ *   qb200_match_descriptors_each / _enqueue_each       as qb200_match_features_each / _enqueue_each
+ *   qb200_register_descriptors_each / _enqueue_each    as qb200_register_features_each / _enqueue_each
+ * Each takes the arguments of its _features_ form and follows its contract clause for clause: per-pair params, host or device kind,
+ * lists, records, statuses, rejections before anything is queued, latching, and one stream and one flush with every other enqueue.
+ *   Pair i's descriptors are the first `dim` floats of each of its rows, and its rows are `stride` floats apart (both sides alike).
+ *     Pairs of one batch may have different dim and stride.
+ *   Distances are the reference's squared L2: for every (source, target) row the chain acc = fmaf(a_d - b_d, a_d - b_d, acc) over
+ *     d = 0 .. dim - 1 in ascending order, from acc = 0.  A tie goes to the lowest index, and a NaN distance never wins.  Then the
+ *     mutual check and the tuple test run as in every other matching call.
+ *   dim == 33 (any stride) runs the tensor-core matcher of the FPFH path: records and lists are byte-identical to
+ *     qb200_*_features_each on the same 33 floats of every row.  Every other length runs a CUDA-core kernel that streams the
+ *     descriptors 32 dimensions at a time.  Pair i's record and lists are byte-identical to this call on pair i alone.
+ *   The bad-argument checks of the _features_ forms apply, and three more give QB200_ERR_BAD_ARG: dim outside 1 .. QB200_MAX_DESC_DIM,
+ *     stride < dim, and in QB200_MEM_DEVICE kind descriptor arrays that are not 4-byte aligned.
+ *   Descriptors other than 33 floats are copied into a device scratch of each lane sized by the largest wave seen (dim x n floats per
+ *     cloud, rounded up to 4 points, plus as much again for host-kind rows); it is allocated on the first such call.
+ *   A one-pair blocking qb200_match_descriptors_each sets the nearest-neighbour tables of qb200_debug_nn_tables, as qb200_match does. */
+#define QB200_MAX_DESC_DIM 512
+typedef struct qb200_descriptor_pair {
+  const float* src;        /* n_src x {x,y,z,w} keypoints */
+  const float* src_desc;   /* n_src rows of `stride` floats; the first `dim` of each row are the descriptor */
+  const float* tgt;
+  const float* tgt_desc;
+  int32_t n_src, n_tgt;
+  int32_t dim;             /* 1 .. QB200_MAX_DESC_DIM, per pair */
+  int32_t stride;          /* >= dim: e.g. 361 for pcl::SHOT352 (descriptor[352] + rf[9]), 33 for FPFHSignature33 */
+} qb200_descriptor_pair;
+int qb200_match_descriptors_each(qb200_handle* h, const qb200_descriptor_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                 qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+int qb200_match_descriptors_enqueue_each(qb200_handle* h, const qb200_descriptor_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                         qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+int qb200_register_descriptors_each(qb200_handle* h, const qb200_descriptor_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                    qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists);
+int qb200_register_descriptors_enqueue_each(qb200_handle* h, const qb200_descriptor_pair* pairs, int32_t n_pairs,
+                                            const qb200_params* params, qb200_mem_kind kind, qb200_result* results,
+                                            const qb200_pair_lists* lists);
+
 /* --- the front end in batches: voxel keypoints, normals and FPFH-33 of many scans into caller memory ----------------------------------
  * voxelize<T> (include/quatro.hpp:49-57) + FPFHEstimation::computeFPFHFeatures (src/teaser_utils/fpfh.cc:44-75), handed out as
  * FPFHManager::getObjDescriptor / getSceneDescriptor / getTgtNormals do (include/fpfh_manager.hpp:161-177), for a batch of raw scans:
@@ -971,12 +1012,12 @@ int qb200_bind_numa(qb200_handle* h);
 
 /* Introspection of the most recent single-pair solve on this handle (getMaxCliques,
  * getFinalInliersIndices, getCorrespondences; quatro.hpp:949-972, fpfh_manager.hpp:234-236).  Each list is set by these calls:
- *   correspondences: a one-pair registration or match of raw, cached or feature pairs (qb200_register_pair, the batch entry
- *     points with n = 1), qb200_match, qb200_match_and_pack;
+ *   correspondences: a one-pair registration or match of raw, cached, feature or descriptor pairs (qb200_register_pair, the batch
+ *     entry points with n = 1), qb200_match, qb200_match_and_pack;
  *   clique and final inliers: a one-pair registration, match (empty lists) or solve (qb200_solve_correspondences, qb200_solve_batch*
  *     with n = 1), qb200_solve_pose; the clique also qb200_max_clique / _ex;
  *   features (qb200_get_last_features): a one-pair registration or match of raw pairs, qb200_match_and_pack, qb200_compute_fpfh;
- *   nearest-neighbour tables (qb200_debug_nn_tables): qb200_match.
+ *   nearest-neighbour tables (qb200_debug_nn_tables): qb200_match, a blocking qb200_match_descriptors_each with n = 1.
  * The lists live in the buffers of the handle's first lane, which every later call that runs a wave there reuses: every batch,
  * enqueue, describe, voxelize, cache-write, graph, clique and pose entry point whose waves reach that lane, and the stage calls
  * qb200_voxelize, qb200_compute_fpfh, qb200_match, qb200_match_and_pack, qb200_build_graph, qb200_max_clique / _ex,

@@ -8,9 +8,9 @@ and the synthetic-scan generator.  There is no CPU fallback anywhere in this pac
 from .capi import (  # noqa: F401
     Params, Config, Result, Pair, Handle, QuatroB200Error, default_params, default_config, load_library,
     PMC_EXACT, PMC_HEU, KCORE_HEU, INLIER_NONE, COTE_MEDIAN, COTE_WEIGHTED_MEAN, MEM_HOST, MEM_DEVICE,
-    PairLists, ListBuffers, FLAG_LISTS_TRUNCATED, FeaturePair, FeatureOut, POINT_ARRAYS, VOXEL_ARRAYS, MATCH_LISTS,
+    PairLists, ListBuffers, FLAG_LISTS_TRUNCATED, FeaturePair, DescriptorPair, FeatureOut, POINT_ARRAYS, VOXEL_ARRAYS, MATCH_LISTS,
 )
 
 __all__ = ["Params", "Config", "Result", "Pair", "Handle", "QuatroB200Error", "default_params",
-           "default_config", "load_library", "PairLists", "ListBuffers", "FeaturePair", "FeatureOut",
+           "default_config", "load_library", "PairLists", "ListBuffers", "FeaturePair", "DescriptorPair", "FeatureOut",
            "POINT_ARRAYS", "VOXEL_ARRAYS", "MATCH_LISTS"]

@@ -90,6 +90,16 @@ class FeaturePair(C.Structure):
                 ("n_tgt", C.c_int32)]
 
 
+class DescriptorPair(C.Structure):
+    """qb200_descriptor_pair: one pair's keypoints ({x,y,z,w} records) and descriptor rows of `stride` floats, the first `dim` of
+    which are the descriptor (1 <= dim <= DESC_DIM_MAX)."""
+    _fields_ = [("src", C.c_void_p), ("src_desc", C.c_void_p), ("tgt", C.c_void_p), ("tgt_desc", C.c_void_p), ("n_src", C.c_int32),
+                ("n_tgt", C.c_int32), ("dim", C.c_int32), ("stride", C.c_int32)]
+
+
+DESC_DIM_MAX = 512   # QB200_MAX_DESC_DIM
+
+
 class CorrSet(C.Structure):
     _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("L", C.c_int32), ("reserved", C.c_int32)]
 
@@ -356,6 +366,10 @@ _SIGNATURES = {
     "qb200_match_cached_enqueue_mixed": (i32, [vp, vp, i32, P(Params), vp, P(PairLists)]),
     "qb200_match_features_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_match_features_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_match_descriptors_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_match_descriptors_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_register_descriptors_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
+    "qb200_register_descriptors_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_max_clique_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_max_clique_batch_enqueue_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(PairLists)]),
     "qb200_build_graph_batch_each": (i32, [vp, vp, i32, P(Params), i32, vp, P(GraphOut)]),
@@ -429,6 +443,30 @@ def _feature_array(pairs: Sequence, kind: int = MEM_HOST):
             arr[i].tgt, arr[i].tgt_desc, arr[i].n_tgt = t.ctypes.data, td.ctypes.data, len(t)
         else:
             arr[i].src, arr[i].src_desc, arr[i].n_src, arr[i].tgt, arr[i].tgt_desc, arr[i].n_tgt = pr
+    return arr, keep
+
+
+def _descriptor_array(pairs: Sequence, kind: int = MEM_HOST):
+    """(DescriptorPair * n) array of `pairs`, each a DescriptorPair (pointers of any kind, used as they are), (src4, src_rows, tgt4,
+    tgt_rows[, dim]) numpy arrays with rows of `stride` = rows.shape[1] floats (dim defaults to the stride; MEM_HOST), or (src_ptr,
+    src_desc_ptr, n_src, tgt_ptr, tgt_desc_ptr, n_tgt, dim, stride) device tuples (MEM_DEVICE); and the contiguous arrays it points
+    to."""
+    arr = (DescriptorPair * max(len(pairs), 1))()
+    keep = []
+    for i, pr in enumerate(pairs):
+        if isinstance(pr, DescriptorPair):
+            arr[i] = pr
+        elif kind == MEM_HOST:
+            s, t = _f32(pr[0], 4), _f32(pr[2], 4)
+            sd, td = np.ascontiguousarray(pr[1], np.float32), np.ascontiguousarray(pr[3], np.float32)
+            assert sd.ndim == td.ndim == 2 and sd.shape[1] == td.shape[1] and len(s) == len(sd) and len(t) == len(td)
+            stride = sd.shape[1]
+            keep.append((s, sd, t, td))
+            arr[i].src, arr[i].src_desc, arr[i].n_src = s.ctypes.data, sd.ctypes.data, len(s)
+            arr[i].tgt, arr[i].tgt_desc, arr[i].n_tgt = t.ctypes.data, td.ctypes.data, len(t)
+            arr[i].dim, arr[i].stride = (pr[4] if len(pr) > 4 else stride), stride
+        else:
+            (arr[i].src, arr[i].src_desc, arr[i].n_src, arr[i].tgt, arr[i].tgt_desc, arr[i].n_tgt, arr[i].dim, arr[i].stride) = pr
     return arr, keep
 
 
@@ -1003,6 +1041,43 @@ class Handle:
         return self._check(self.lib.qb200_match_features_enqueue_each(self.h, feature_array, n, params_array, kind, _ptr(out),
                                                                       self._lists_arg(self._match_lists(buffers))),
                            "qb200_match_features_enqueue_each")
+
+    # ---- caller keypoints and descriptors of any length (qb200_match_descriptors_each, qb200_register_descriptors_each) ----
+    descriptor_array = staticmethod(_descriptor_array)
+
+    def match_descriptors_each(self, pairs: Sequence, params: Sequence[Params], kind: int = MEM_HOST,
+                               buffers: Optional[ListBuffers] = None):
+        """qb200_match_descriptors_each: pair i's keypoints and descriptors (descriptor_array()) are matched with params[i]; corr
+        indexes the caller's keypoints."""
+        assert len(params) == len(pairs)
+        arr, keep = self.descriptor_array(pairs, kind)
+        return self._batch_lists("qb200_match_descriptors_each", len(pairs), (arr, len(pairs), self.params_array(params), kind),
+                                 self._match_lists(buffers))
+
+    def match_descriptors_enqueue_each_raw(self, descriptor_array, n: int, params_array, kind: int, out: np.ndarray,
+                                           buffers: Optional[ListBuffers] = None):
+        """qb200_match_descriptors_enqueue_each: params_array (params_array()) is copied by the call; descriptor_array
+        (descriptor_array()), its host arrays, `out` and the buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_match_descriptors_enqueue_each(self.h, descriptor_array, n, params_array, kind, _ptr(out),
+                                                                         self._lists_arg(self._match_lists(buffers))),
+                           "qb200_match_descriptors_enqueue_each")
+
+    def register_descriptors_each(self, pairs: Sequence, params: Sequence[Params], kind: int = MEM_HOST,
+                                  buffers: Optional[ListBuffers] = None):
+        """qb200_register_descriptors_each: pair i's keypoints and descriptors (descriptor_array()) are matched and solved with
+        params[i]; corr indexes the caller's keypoints."""
+        assert len(params) == len(pairs)
+        arr, keep = self.descriptor_array(pairs, kind)
+        return self._batch_lists("qb200_register_descriptors_each", len(pairs), (arr, len(pairs), self.params_array(params), kind),
+                                 buffers)
+
+    def register_descriptors_enqueue_each_raw(self, descriptor_array, n: int, params_array, kind: int, out: np.ndarray,
+                                              buffers: Optional[ListBuffers] = None):
+        """qb200_register_descriptors_enqueue_each: params_array (params_array()) is copied by the call; descriptor_array
+        (descriptor_array()), its host arrays, `out` and the buffers must stay alive until register_batch_flush."""
+        return self._check(self.lib.qb200_register_descriptors_enqueue_each(self.h, descriptor_array, n, params_array, kind,
+                                                                            _ptr(out), self._lists_arg(buffers)),
+                           "qb200_register_descriptors_enqueue_each")
 
     # ---- caller graphs -> maximum cliques (qb200_max_clique_batch_each) ----
     graph_array = staticmethod(_graph_array)

@@ -65,6 +65,7 @@ size_t carve_counters(int* base, size_t S, WaveCounters* c) {
   c->n_edges = reinterpret_cast<long long*>(take(2 * S));
   c->n_valid = take(C);
   c->n_vox = take(C);
+  c->n_fpfh = take(C);
   c->n_lat = take(C);
   c->n_cells = take(C);
   c->cloud_status = take(C);
@@ -399,10 +400,44 @@ int stage_raw(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs) {
   return QB200_OK;
 }
 
+// A descriptor wave's clouds of other lengths than 33 (h_feat[0, ncl) entries whose dim is not kDescDim) in the lane's dd_buf: each
+// cloud's dimension-major rows at FeatureSrc::out, ld = n rounded up to 4 points (every row starts 16-byte aligned for nn_dim_kernel's
+// cp.async), then, with host rows, those rows packed behind them from *stage on.  The buffer is allocated on the first wave that has
+// such a cloud and grows to the largest wave so far; the lane's previous wave has been collected, so the old buffer is idle.
+int layout_other_dims(Lane* L, int ncl, bool host, float** stage) {
+  size_t major = 0, rows = 0;
+  for (int c = 0; c < ncl; ++c) {
+    FeatureSrc& f = L->h_feat[c];
+    if (!f.desc || f.dim == kDescDim) continue;
+    f.ld = (f.n + 3) & ~3;
+    major += (size_t)f.dim * f.ld;
+    rows += (size_t)f.dim * f.n;
+  }
+  const size_t need = major + (host ? rows : 0);
+  if (need > L->dd_cap) {
+    L->dd_cap = 0;
+    QB_CUDA_TRY(L, L->dd_buf.alloc(need));
+    L->dd_cap = need;
+  }
+  size_t off = 0;
+  for (int c = 0; c < ncl; ++c) {
+    FeatureSrc& f = L->h_feat[c];
+    if (!f.desc || f.dim == kDescDim) continue;
+    f.out = L->dd_buf + off;
+    off += (size_t)f.dim * f.ld;
+  }
+  *stage = need > 0 ? L->dd_buf + major : nullptr;
+  return QB200_OK;
+}
+
 int stage_features(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs) {
+  float* other = nullptr;
+  if (int rc = layout_other_dims(L, ncl, kind == QB200_MEM_HOST, &other)) return rc;
   if (kind == QB200_MEM_HOST) {
-    // Host clouds are packed into areas a feature wave leaves idle: keypoints into normals, descriptor rows into spfh.  A run of
-    // clouds that lie back to back in the caller's memory crosses PCIe as one copy per array, as raw scans do (stage_raw).
+    // Host clouds are packed into areas a feature wave leaves idle: keypoints into normals, FPFH-33 rows into spfh (33 floats each),
+    // rows of other lengths behind the dimension-major rows of dd_buf (dim floats each).  A run of clouds that lie back to back in
+    // the caller's memory crosses PCIe as one copy per array, as raw scans do (stage_raw); rows with a stride past their descriptor
+    // cross by one 2-D copy per cloud that leaves the rest of each row behind.
     const char* run_src[2] = {nullptr, nullptr};
     char* run_dst[2] = {nullptr, nullptr};
     size_t run_bytes[2] = {0, 0};
@@ -427,14 +462,21 @@ int stage_features(Lane* L, int ncl, qb200_mem_kind kind, cudaStream_t cs) {
     for (int c = 0; c < ncl; ++c) {
       FeatureSrc& f = L->h_feat[c];
       float4* pts = L->normals.get() + off;
-      float* desc = L->spfh + off * kDescDim;
+      float* desc = f.dim == kDescDim ? L->spfh + off * kDescDim : other;
       if (f.pts) {
         if (int rc = add(0, f.pts, pts, (size_t)f.n * sizeof(float4))) return rc;
         f.pts = pts;
       }
       if (f.desc) {  // (a describe-points wave stages keypoints only)
-        if (int rc = add(1, f.desc, desc, (size_t)f.n * kDescDim * sizeof(float))) return rc;
+        const size_t row = (size_t)f.dim * sizeof(float);
+        if (f.stride == f.dim) {
+          if (int rc = add(1, f.desc, desc, f.n * row)) return rc;
+        } else if (f.n > 0) {
+          QB_CUDA_TRY(L, cudaMemcpy2DAsync(desc, row, f.desc, (size_t)f.stride * sizeof(float), row, f.n, cudaMemcpyHostToDevice, cs));
+        }
         f.desc = desc;
+        f.stride = f.dim;
+        if (f.dim != kDescDim) other += (size_t)f.dim * f.n;
       }
       off += f.n;
     }
@@ -514,6 +556,7 @@ struct BatchCall {
   const qb200_pair* pairs = nullptr;           // RawPairs
   const qb200_slot_pair* slots = nullptr;      // CachedPairs
   const qb200_feature_pair* feats = nullptr;   // FeaturePairs: keypoints and FPFH-33 rows, front-end fields of the entries ignored
+  const qb200_descriptor_pair* descs = nullptr;  // DescriptorPairs: keypoints and descriptor rows of any length, the same
   const qb200_corr_set* sets = nullptr;        // CorrSets
   const qb200_graph* graphs = nullptr;         // Graphs
   const qb200_inlier_set* inlier_sets = nullptr;  // InlierSets
@@ -542,7 +585,7 @@ struct BatchCall {
 // an inlier set's ids to clique), graph (its adjacency goes to adj) or align set (read through its own table entry)
 int clouds_per_input(Source s) {
   switch (s) {
-    case Source::RawPairs: case Source::CachedPairs: case Source::FeaturePairs: return 2;
+    case Source::RawPairs: case Source::CachedPairs: case Source::FeaturePairs: case Source::DescriptorPairs: return 2;
     case Source::RawScans: case Source::KeypointClouds: return 1;
     case Source::CorrSets: case Source::Graphs: case Source::InlierSets: case Source::AlignSets: return 0;
   }
@@ -556,7 +599,8 @@ bool is_pairs(Source s) { return clouds_per_input(s) == 2; }
 // on the shared copy stream and opens with a quarter wave.  Cached pairs, correspondence sets, graphs and inlier sets do neither.
 bool crosses_pcie(Source s) {
   switch (s) {
-    case Source::RawPairs: case Source::FeaturePairs: case Source::RawScans: case Source::KeypointClouds: case Source::AlignSets:
+    case Source::RawPairs: case Source::FeaturePairs: case Source::DescriptorPairs: case Source::RawScans: case Source::KeypointClouds:
+    case Source::AlignSets:
       return true;
     case Source::CachedPairs: case Source::CorrSets: case Source::Graphs: case Source::InlierSets: return false;
   }
@@ -568,8 +612,8 @@ bool crosses_pcie(Source s) {
 bool runs_front_end(Source s) {
   switch (s) {
     case Source::RawPairs: case Source::RawScans: case Source::KeypointClouds: return true;
-    case Source::CachedPairs: case Source::FeaturePairs: case Source::CorrSets: case Source::Graphs: case Source::InlierSets:
-    case Source::AlignSets:
+    case Source::CachedPairs: case Source::FeaturePairs: case Source::DescriptorPairs: case Source::CorrSets: case Source::Graphs:
+    case Source::InlierSets: case Source::AlignSets:
       return false;
   }
   return false;
@@ -592,7 +636,7 @@ unsigned stage_slots(Source s, Sink k) {
   unsigned m = 0;
   switch (s) {
     case Source::RawPairs: m = kH2d | kVoxel | kFpfh | kMatch | kSolver | kD2h; break;
-    case Source::FeaturePairs: m = kH2d | kMatch | kSolver | kD2h; break;
+    case Source::FeaturePairs: case Source::DescriptorPairs: m = kH2d | kMatch | kSolver | kD2h; break;
     case Source::CachedPairs: m = kFpfh | kMatch | kSolver; break;
     case Source::CorrSets: m = kSolver; break;
     case Source::RawScans: case Source::KeypointClouds: case Source::Graphs: case Source::InlierSets: case Source::AlignSets: break;
@@ -860,19 +904,35 @@ int front_raw(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np, int
   return QB200_OK;
 }
 
-// Feature pairs and keypoint clouds: the caller's keypoints (and a feature pair's descriptor rows) imported as they are; keypoint
-// clouds, which come without descriptors, are then described by K2..K5
+// Feature pairs, descriptor pairs and keypoint clouds: the caller's keypoints (and a pair's descriptor rows) imported as they are;
+// keypoint clouds, which come without descriptors, are then described by K2..K5.  A descriptor pair of 33 floats is imported into
+// desc_t like a feature pair (whatever its stride); one of another length into dd_buf (stage_features places it).
 int front_features(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np, int ncl) {
   int rc;
   cudaEventRecord(L->ev[0], L->stream);
   for (int s = 0; s < np; ++s) {
     if (in.src == Source::KeypointClouds) {
-      L->h_feat[s] = {reinterpret_cast<const float4*>(in.scans[w0 + s]), nullptr, in.n_points[w0 + s], 0};
+      L->h_feat[s] = fpfh_src(L, s, in.scans[w0 + s], nullptr, in.n_points[w0 + s]);
+      continue;
+    }
+    if (in.src == Source::DescriptorPairs) {
+      const qb200_descriptor_pair& d = in.descs[w0 + s];
+      for (int side = 0; side < 2; ++side) {
+        const int c = 2 * s + side;
+        FeatureSrc& f = L->h_feat[c];
+        f = fpfh_src(L, c, side ? d.tgt : d.src, side ? d.tgt_desc : d.src_desc, side ? d.n_tgt : d.n_src);
+        f.stride = d.stride;
+        if (d.dim != kDescDim) {  // dd_buf's: stage_features places it
+          f.out = nullptr;
+          f.dim = d.dim;
+          f.ld = 0;
+        }
+      }
       continue;
     }
     const qb200_feature_pair& f = in.feats[w0 + s];
-    L->h_feat[2 * s] = {reinterpret_cast<const float4*>(f.src), f.src_desc, f.n_src, 0};
-    L->h_feat[2 * s + 1] = {reinterpret_cast<const float4*>(f.tgt), f.tgt_desc, f.n_tgt, 0};
+    L->h_feat[2 * s] = fpfh_src(L, 2 * s, f.src, f.src_desc, f.n_src);
+    L->h_feat[2 * s + 1] = fpfh_src(L, 2 * s + 1, f.tgt, f.tgt_desc, f.n_tgt);
   }
   if ((rc = stage_inputs(h, L, in, ncl))) return rc;
   if ((rc = launch_feature_import(L, ncl))) return rc;
@@ -1201,7 +1261,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   if ((rc = fill_tables(L, in, w0, np))) return rc;
   switch (in.src) {
     case Source::RawPairs: case Source::RawScans: rc = front_raw(h, L, in, w0, np, ncl); break;
-    case Source::FeaturePairs: case Source::KeypointClouds: rc = front_features(h, L, in, w0, np, ncl); break;
+    case Source::FeaturePairs: case Source::DescriptorPairs: case Source::KeypointClouds: rc = front_features(h, L, in, w0, np, ncl); break;
     case Source::CachedPairs: rc = front_cached(h, L, in, w0, np, ncl); break;
     case Source::CorrSets: rc = front_sets(L, in, w0, np); break;
     case Source::Graphs: rc = front_graphs(L, in, w0, np); break;
@@ -1210,9 +1270,12 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
   }
   if (rc) return rc;
   const bool match_pairs = is_pairs(in.src);
+  const bool caller_kp = in.src == Source::FeaturePairs || in.src == Source::DescriptorPairs;
+  int dims = 0;  // a descriptor wave: which K6 its pairs need
+  for (int s = 0; in.src == Source::DescriptorPairs && s < np; ++s) dims |= in.descs[w0 + s].dim == kDescDim ? kDimsFpfh : kDimsOther;
   switch (in.sink) {
     case Sink::Solve:
-      if (match_pairs && (rc = launch_match(L, np, in.src == Source::FeaturePairs))) return rc;
+      if (match_pairs && (rc = launch_match(L, np, caller_kp, dims))) return rc;
       cudaEventRecord(L->ev[4], L->stream);
       cudaEventRecord(L->ev[5], L->stream);  // re-recorded inside run_solver when the graph stage runs
       if ((rc = run_solver(L, np, match_pairs ? 1 : 0))) return rc;
@@ -1220,7 +1283,7 @@ int wave_submit(qb200_handle* h, Lane* L, const BatchCall& in, int w0, int np) {
       rc = send_records(L, in, w0, np);
       break;
     case Sink::Match:  // no solver tail: the records come from the matcher's counters, and graph, clique and pose take no time
-      if ((rc = launch_match(L, np, in.src == Source::FeaturePairs))) return rc;
+      if ((rc = launch_match(L, np, caller_kp, dims))) return rc;
       if ((rc = launch_match_records(L, np))) return rc;
       for (int i = 4; i <= 7; ++i) cudaEventRecord(L->ev[i], L->stream);
       rc = send_records(L, in, w0, np);
@@ -1378,6 +1441,7 @@ const void* input_of(const BatchCall& c) {
     case Source::RawPairs: return c.pairs;
     case Source::CachedPairs: return c.slots;
     case Source::FeaturePairs: return c.feats;
+    case Source::DescriptorPairs: return c.descs;
     case Source::CorrSets: return c.sets;
     case Source::RawScans: case Source::KeypointClouds: return c.scans;
     case Source::Graphs: return c.graphs;
@@ -1497,6 +1561,29 @@ int check_call(qb200_handle* h, const BatchCall& c) {
             bad = "keypoints (16-byte) or descriptors (4-byte) misaligned or not memory of the handle's device";
           if (bad) {
             snprintf(why, sizeof(why), "feature pair %d, %s: %s", i, side ? "target" : "source", bad);
+            return reject(why);
+          }
+        }
+        break;
+      }
+      case Source::DescriptorPairs: {
+        const qb200_descriptor_pair& d = c.descs[i];
+        if (d.dim < 1 || d.dim > QB200_MAX_DESC_DIM) bad = "dim outside 1 .. QB200_MAX_DESC_DIM";
+        else if (d.stride < d.dim) bad = "stride < dim";
+        if (bad) {
+          snprintf(why, sizeof(why), "descriptor pair %d: %s", i, bad);
+          return reject(why);
+        }
+        for (int side = 0; side < 2; ++side) {
+          const int n = side ? d.n_tgt : d.n_src;
+          const float* pts = side ? d.tgt : d.src;
+          const float* desc = side ? d.tgt_desc : d.src_desc;
+          if (n < 0 || n > h->cfg.max_voxel_points) bad = "count outside 0 .. max_voxel_points";
+          else if (n > 0 && (!pts || !desc)) bad = "null keypoints or descriptors";
+          else if (n > 0 && c.kind == QB200_MEM_DEVICE && !(device_array_of(h, pts, 16) && device_array_of(h, desc, 4)))
+            bad = "keypoints (16-byte) or descriptors (4-byte) misaligned or not memory of the handle's device";
+          if (bad) {
+            snprintf(why, sizeof(why), "descriptor pair %d, %s: %s", i, side ? "target" : "source", bad);
             return reject(why);
           }
         }
@@ -1706,6 +1793,13 @@ int run_call(qb200_handle* h, const BatchCall& c) {
     stamp_last(h, {kLastClique, kLastFinal});
     if (is_pairs(c.src)) stamp_last(h, {kLastCorr});
     if (c.src == Source::RawPairs) stamp_last(h, {kLastFeatures});
+    if (c.src == Source::DescriptorPairs && c.sink == Sink::Match) {  // what match_mutual_kernel read, as after qb200_match
+      const qb200_descriptor_pair& d = c.descs[0];
+      const bool both = d.n_src > 0 && d.n_tgt > 0;
+      h->last_match_n[0] = both ? d.n_src : 0;
+      h->last_match_n[1] = both ? d.n_tgt : 0;
+      stamp_last(h, {kLastNn});
+    }
   }
   return rc;
 }
@@ -1731,6 +1825,14 @@ BatchCall feature_pairs(Sink k, const qb200_feature_pair* feats, int32_t n, cons
                         const qb200_pair_lists* lists) {
   BatchCall c{Source::FeaturePairs, k, n, kind, p, Entries::Mixed};
   c.feats = feats; c.results = results; c.lists = lists;
+  return c;
+}
+
+// the entries' front-end fields are ignored, so they may differ
+BatchCall descriptor_pairs(Sink k, const qb200_descriptor_pair* descs, int32_t n, const qb200_params* p, qb200_mem_kind kind,
+                           qb200_result* results, const qb200_pair_lists* lists) {
+  BatchCall c{Source::DescriptorPairs, k, n, kind, p, Entries::Mixed};
+  c.descs = descs; c.results = results; c.lists = lists;
   return c;
 }
 
@@ -2033,6 +2135,28 @@ int qb200_register_features_each(qb200_handle* h, const qb200_feature_pair* pair
 int qb200_register_features_enqueue_each(qb200_handle* h, const qb200_feature_pair* pairs, int32_t n_pairs, const qb200_params* params,
                                          qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
   return enqueue_call(h, feature_pairs(Sink::Solve, pairs, n_pairs, params, kind, results, lists));
+}
+
+// ---- caller keypoints and descriptors of any length -> correspondences, or pose --------------------------------------------------
+int qb200_match_descriptors_each(qb200_handle* h, const qb200_descriptor_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                 qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return run_call(h, descriptor_pairs(Sink::Match, pairs, n_pairs, params, kind, results, lists));
+}
+
+int qb200_match_descriptors_enqueue_each(qb200_handle* h, const qb200_descriptor_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                         qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return enqueue_call(h, descriptor_pairs(Sink::Match, pairs, n_pairs, params, kind, results, lists));
+}
+
+int qb200_register_descriptors_each(qb200_handle* h, const qb200_descriptor_pair* pairs, int32_t n_pairs, const qb200_params* params,
+                                    qb200_mem_kind kind, qb200_result* results, const qb200_pair_lists* lists) {
+  return run_call(h, descriptor_pairs(Sink::Solve, pairs, n_pairs, params, kind, results, lists));
+}
+
+int qb200_register_descriptors_enqueue_each(qb200_handle* h, const qb200_descriptor_pair* pairs, int32_t n_pairs,
+                                            const qb200_params* params, qb200_mem_kind kind, qb200_result* results,
+                                            const qb200_pair_lists* lists) {
+  return enqueue_call(h, descriptor_pairs(Sink::Solve, pairs, n_pairs, params, kind, results, lists));
 }
 
 // ---- raw scans -> voxel keypoints, normals and FPFH-33 in caller memory ---------------------------------------------------------

@@ -46,8 +46,8 @@ constexpr int kDescPad = 36;   // floats per SPFH row (16-byte multiple: float4 
 constexpr int kDescK = 40;     // rows (K extent) of the dimension-major FPFH matrices: 33 bins + zero padding to a multiple of
                                // the TF32 tensor-core K step (8)
 // One step of the matcher's exact descriptor distance: acc + (a - b)^2, the product-sum rounded once.  Every exact distance
-// of the matcher (match_stripe_kernel, tc_nn_kernel's evaluation and its seeds) is the chain of these steps over bins
-// 0 .. 32 in ascending order, so all of them produce the same bits.
+// of the matcher (match_stripe_kernel, tc_nn_kernel's evaluation and its seeds, nn_dim_kernel) is the chain of these steps over
+// bins 0 .. dim - 1 in ascending order, so all of them produce the same bits.
 __device__ __forceinline__ float desc_dist_step(float acc, float a, float b) {
   const float diff = a - b;
   return __fmaf_rn(diff, diff, acc);
@@ -60,6 +60,7 @@ constexpr int kNbrGlobalCap = 80;  // neighbour indices per point handed from K4
 struct WaveCounters {
   int* n_valid;      // [clouds] points kept by the voxel key pass
   int* n_vox;        // [clouds]
+  int* n_fpfh;       // [clouds] a descriptor wave's count of each cloud the FPFH-33 matcher takes: n_vox, or 0 for another length
   int* n_lat;        // [clouds] points inside the neighbour lattice
   int* n_cells;      // [clouds]
   int* cloud_status; // [clouds] qb200_status (0 ok)

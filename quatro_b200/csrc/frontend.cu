@@ -757,30 +757,41 @@ __global__ void __launch_bounds__(kPassThreads) passthrough_kernel(const float4*
 
 constexpr int kImportTile = 128, kImportThreads = 256;
 
-// Caller features of a wave -> the matcher's inputs: cloud c's keypoints into vox_pts, its n x 33 descriptor rows
-// (pcl::FPFHSignature33) into the 33 dimension-major rows of desc_t, and n into n_vox.  One CTA per tile of kImportTile points of a
-// cloud: the tile's AoS rows are one contiguous run of kImportTile * 132 bytes, read coalesced into shared memory, and every
-// dimension-major row segment is written coalesced from there (row stride 33 floats: the column reads are free of bank conflicts).
-// A pure copy: every value, NaN payloads included, arrives bit for bit.  A cloud without descriptors (a keypoint wave of
-// qb200_describe_points_each, which K2..K5 describe next) imports its keypoints and count only.
+// Caller features of a wave -> the matcher's inputs: cloud c's keypoints into vox_pts, the first `dim` floats of its n descriptor
+// rows (`stride` floats apart: pcl::FPFHSignature33 is 33 of 33, pcl::SHOT352 352 of 361) into `dim` dimension-major rows at
+// f.out, ld apart (desc_t for FPFH-33, dd_buf for other lengths), and n into n_vox and, for FPFH-33, n_fpfh.  One CTA per tile of
+// kImportTile points of a cloud, 33 dimensions at a time: the tile's rows are read as runs of up to 33 floats into shared memory,
+// and every dimension-major row segment is written coalesced from there (row pitch 33 floats: the column reads are free of bank
+// conflicts).  A pure copy: every value, NaN payloads included, arrives bit for bit.  A cloud without descriptors (a keypoint wave
+// of qb200_describe_points_each, which K2..K5 describe next) imports its keypoints and count only.
 __global__ void __launch_bounds__(kImportThreads) feature_import_kernel(const FeatureSrc* __restrict__ table, int V, float4* __restrict__ vox_pts,
-                                                                        float* __restrict__ desc_t, int* __restrict__ n_vox) {
+                                                                        int* __restrict__ n_vox, int* __restrict__ n_fpfh) {
   __shared__ float tile[kImportTile * kDescDim];
   const int cloud = blockIdx.y, q0 = blockIdx.x * kImportTile, tid = threadIdx.x;
   const FeatureSrc f = table[cloud];
-  if (blockIdx.x == 0 && tid == 0) n_vox[cloud] = f.n;
+  if (blockIdx.x == 0 && tid == 0) {
+    n_vox[cloud] = f.n;
+    n_fpfh[cloud] = f.dim == kDescDim ? f.n : 0;
+  }
   if (q0 >= f.n) return;
   const int m = min(kImportTile, f.n - q0);
   if (f.pts)  // (qb200_debug_tc_distances imports descriptors only)
     for (int i = tid; i < m; i += kImportThreads) vox_pts[(size_t)cloud * V + q0 + i] = __ldg(f.pts + q0 + i);
-  if (!f.desc) return;  // the same for every thread of the CTA: no thread waits at the barrier below
-  const float* __restrict__ src = f.desc + (size_t)q0 * kDescDim;
-  for (int i = tid; i < m * kDescDim; i += kImportThreads) tile[i] = __ldg(src + i);
-  __syncthreads();
-  float* __restrict__ out = desc_t + (size_t)cloud * kDescK * V + q0;
-  for (int i = tid; i < kDescDim * kImportTile; i += kImportThreads) {
-    const int d = i / kImportTile, q = i % kImportTile;
-    if (q < m) out[(size_t)d * V + q] = tile[q * kDescDim + d];
+  if (!f.desc) return;  // the same for every thread of the CTA: no thread waits at the barriers below
+  const float* __restrict__ src = f.desc + (size_t)q0 * f.stride;
+  for (int k0 = 0; k0 < f.dim; k0 += kDescDim) {
+    const int kw = min(kDescDim, f.dim - k0);
+    if (k0 > 0) __syncthreads();  // the previous chunk's column reads are done
+    for (int i = tid; i < m * kDescDim; i += kImportThreads) {
+      const int q = i / kDescDim, d = i % kDescDim;
+      if (d < kw) tile[i] = __ldg(src + (size_t)q * f.stride + k0 + d);
+    }
+    __syncthreads();
+    float* __restrict__ out = f.out + (size_t)k0 * f.ld + q0;
+    for (int i = tid; i < kw * kImportTile; i += kImportThreads) {
+      const int d = i / kImportTile, q = i % kImportTile;
+      if (q < m) out[(size_t)d * f.ld + q] = tile[q * kDescDim + d];
+    }
   }
 }
 
@@ -918,7 +929,7 @@ int launch_feature_import(Lane* h, int n_clouds) {
   int n_max = 1;  // at least one tile per cloud: its first CTA writes n_vox, also for an empty cloud
   for (int c = 0; c < n_clouds; ++c) n_max = h->h_feat[c].n > n_max ? h->h_feat[c].n : n_max;
   const dim3 g((n_max + kImportTile - 1) / kImportTile, n_clouds);
-  feature_import_kernel<<<g, kImportThreads, 0, h->stream>>>(h->d_feat, h->V, h->vox_pts, h->desc_t, h->ctr.n_vox);
+  feature_import_kernel<<<g, kImportThreads, 0, h->stream>>>(h->d_feat, h->V, h->vox_pts, h->ctr.n_vox, h->ctr.n_fpfh);
   h->launches++;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;

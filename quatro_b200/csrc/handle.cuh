@@ -55,12 +55,16 @@ struct CloudFront {
 
 struct PpScan;   // one scan's pre-processing entry (preprocess.cu)
 
-// Where feature_import_kernel reads one cloud of a feature wave (frontend.cu): n keypoints and n FPFH-33 rows, in the caller's
-// device memory or in the lane's staging areas; desc == nullptr: keypoints only (a describe-points wave, described by K2..K5)
+// Where feature_import_kernel reads one cloud of a feature or descriptor wave (frontend.cu): n keypoints and n descriptor rows of
+// `stride` floats, of which the first `dim` are the descriptor, in the caller's device memory or in the lane's staging areas;
+// desc == nullptr: keypoints only (a describe-points wave, described by K2..K5).  The import writes the cloud's descriptors
+// dimension-major, row d at out + d * ld: an FPFH-33 cloud into its block of desc_t (ld = V, fpfh_src), a cloud of another length
+// into the lane's dd_buf, which nn_dim_kernel reads through this same table.
 struct FeatureSrc {
   const float4* pts;
   const float* desc;
-  int n, pad;
+  float* out;
+  int n, dim, stride, ld;
 };
 
 // What feature_export_kernel reads (frontend.cu): cloud c's voxel points, normals and dimension-major descriptors at c * V points
@@ -140,13 +144,14 @@ struct AlignSrc {
 };
 
 // What a batch call reads (api.cu: BatchCall), per input: a pair of raw scans, a pair of cached scans (slots), a pair of caller
-// keypoint clouds with their FPFH-33 rows, a correspondence set, one raw scan, one caller keypoint cloud, one caller graph, a
+// keypoint clouds with their FPFH-33 rows, a pair of caller keypoint clouds with descriptor rows of any length, a correspondence set, one raw scan, one caller keypoint cloud, one caller graph, a
 // correspondence set with the caller's inlier ids, or a registered pair to align (a cloud, keypoints, correspondences and a pose)
-enum class Source { RawPairs, CachedPairs, FeaturePairs, CorrSets, RawScans, KeypointClouds, Graphs, InlierSets, AlignSets };
+enum class Source { RawPairs, CachedPairs, FeaturePairs, DescriptorPairs, CorrSets, RawScans, KeypointClouds, Graphs, InlierSets, AlignSets };
 // What a batch call produces: solved records (and lists), the matcher's records (and lists), cache slots, front-end features in
 // caller memory, max-clique records (and clique lists), TIM graphs in caller memory (and records), or poses of given inlier sets
 // (records and lists), or aligned clouds and good matches in caller memory.  The valid (source, sink) pairs:
-//   RawPairs, CachedPairs, FeaturePairs  x  Solve, Match   qb200_register_batch*, _cached*, _features*; qb200_match_*
+//   RawPairs, CachedPairs, FeaturePairs,
+//   DescriptorPairs                      x  Solve, Match   qb200_register_batch*, _cached*, _features*, _descriptors*; qb200_match_*
 //   CorrSets                             x  Solve, Graph   qb200_solve_batch*, qb200_build_graph_batch*
 //   RawScans                             x  CacheSlots     qb200_cache_scans*
 //   RawScans, KeypointClouds             x  Export         qb200_describe_batch*, qb200_describe_points*
@@ -185,6 +190,8 @@ struct Lane {
   DeviceMem<GraphSrc> d_graph; PinnedMem<GraphSrc> h_graph;   // [S] where a graph wave's graphs are read, and its pinned mirror
   DeviceMem<InlierSrc> d_inl; PinnedMem<InlierSrc> h_inl;     // [S] where a pose wave's inlier ids are read, and its pinned mirror
   DeviceMem<AlignSrc> d_aln; PinnedMem<AlignSrc> h_aln;       // [S] an align wave's sets, and its pinned mirror
+  DeviceMem<float> dd_buf; size_t dd_cap;  // a descriptor wave's clouds of other lengths than 33: dimension-major rows (FeatureSrc::out),
+                                           // then host-kind rows staged packed; grown to the largest wave so far, allocated on first use
   DeviceMem<unsigned char> aln_stage;  // an align wave's host-kind correspondences and correspondence outputs, [S][Lc] of each
                                        // (AlignStage), allocated on first use
   int pend_w0, pend_np;       // wave in flight on this lane (pend_np == 0: none)
@@ -360,8 +367,11 @@ size_t pose_ws_bytes(int Lc);
 // launches the tuple test only when h_solve has a pair that runs it.
 int launch_voxel(Lane* h, int n_clouds);
 int launch_fpfh(Lane* h, int n_clouds);
-// keep_w: the matched points keep their keypoints' w (caller keypoints of a feature wave); otherwise w = 1
-int launch_match(Lane* h, int n_pairs, int keep_w);
+// keep_w: the matched points keep their keypoints' w (caller keypoints of a feature wave); otherwise w = 1.  dims (a descriptor
+// wave, kDimsFpfh | kDimsOther): which K6 the wave's pairs need, the FPFH-33 matcher (on the counts ctr.n_fpfh) and nn_dim_kernel
+// (on the pairs whose d_feat entries have another length); 0: every pair is FPFH-33 and K6 reads ctr.n_vox.
+constexpr int kDimsFpfh = 1, kDimsOther = 2;
+int launch_match(Lane* h, int n_pairs, int keep_w, int dims = 0);
 // A match wave's records (pairs [0, n), after launch_match), in place of the solver tail: the matcher's counters, status and flags
 // from the counter block, and the values of a pair that was not solved
 int launch_match_records(Lane* h, int n_pairs);
@@ -404,8 +414,12 @@ __host__ __device__ inline int list_entries(int count, int Lc, int cap) {
   const int n = count < 0 ? 0 : count > Lc ? Lc : count;
   return n < cap ? n : cap;
 }
-int launch_match_nn(Lane* h, int n_pairs);
-int launch_match_exact(Lane* h, int n_pairs, const int* only);
+// the FPFH-33 K6 of pairs [0, n), on the clouds' counts n_pts (ctr.n_vox, or ctr.n_fpfh in a descriptor wave: a pair with a count
+// of 0 is skipped and its rowbest / colbest entries are left to nn_dim_kernel)
+int launch_match_nn(Lane* h, int n_pairs, const int* n_pts);
+int launch_match_exact(Lane* h, int n_pairs, const int* only, const int* n_pts);
+// nn_dim_kernel's K6 of the pairs of a descriptor wave whose d_feat entries have another length than 33 (match.cu)
+int launch_match_dim(Lane* h, int n_pairs);
 int launch_tc_debug_tile(Lane* h, float* d_out);
 int tc_footprint(Lane* h, int* out5);
 // Clouds [0, n_clouds) of src to dst in one launch: keypoints, normals and 33-float descriptor rows (pcl::FPFHSignature33) of each
@@ -423,6 +437,10 @@ int export_desc_rows(Lane* h, const float* desc, const int* n, int m);
 // stream cs; launch_feature_import then fills vox_pts, desc_t and n_vox on the lane's stream (after wave_reset).
 int stage_features(Lane* L, int n_clouds, qb200_mem_kind kind, cudaStream_t cs);
 int launch_feature_import(Lane* h, int n_clouds);
+// the table entry of an FPFH-33 cloud: n rows of 33 floats (or none) into cloud c's block of desc_t
+inline FeatureSrc fpfh_src(const Lane* L, int c, const float* pts4, const float* desc, int n) {
+  return FeatureSrc{reinterpret_cast<const float4*>(pts4), desc, L->desc_t + (size_t)c * kDescK * L->V, n, kDescDim, kDescDim, L->V};
+}
 size_t sort_temp_bytes(int max_items);
 void comm_release(qb200_handle* h);
 int collect_batch(qb200_handle* h, const qb200_result* dst);  // api.cu: wait for every wave in flight that writes into dst[...]

@@ -1,4 +1,4 @@
-// match.cu -- K6 (33-D all-pairs nearest neighbour, both directions) + K7 (mutual check, tuple
+// match.cu -- K6 (33-D all-pairs nearest neighbour, both directions; nn_dim_kernel for other lengths) + K7 (mutual check, tuple
 // test, dedupe/sort, packing of the matched point pairs).   sm_90a
 //
 // Replaces Matcher::calculateCorrespondences / normalizePoints / advancedMatching
@@ -36,6 +36,11 @@ __device__ __forceinline__ unsigned long long shfl_xor_u64(unsigned long long v,
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
   const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem));
+}
+// src_bytes < 16: the rest of the 16 bytes is zero-filled (0: nothing is read)
+__device__ __forceinline__ void cp_async16_zfill(void* smem, const void* gmem, int src_bytes) {
+  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem), "r"(src_bytes));
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N>
@@ -150,6 +155,149 @@ match_stripe_kernel(const float* __restrict__ desc_t, const int* __restrict__ n_
     m = umin64(m, shfl_xor_u64(m, 8));
     if (tx == 0 && r0 + ty * 8 + r < nA) rowbest[(size_t)pair * V + r0 + ty * 8 + r] = m;
   }
+}
+
+// ---- K6 for descriptors of any other length than 33 (a descriptor wave's pairs whose d_feat entries say so) ----
+// The structure of match_stripe_kernel with the K extent streamed: a CTA owns a 128-row stripe of the source and walks 128-column
+// tiles of the target; for each tile, chunks of kDimChunk dimensions of the stripe and of the tile arrive through one cp.async double
+// buffer, and every thread keeps its 8 x 8 distances in registers across the chunks.  So each distance is still one chain of
+// desc_dist_step over d = 0 .. dim - 1 in ascending order.  The rows past dim of the last chunk are zero-filled on both sides and add
+// fmaf(0, 0, acc) = acc (acc is +0, positive, +inf or NaN: never -0), so the chain is the reference's bit for bit.  Row and column
+// minima are folded as in match_stripe_kernel: packed (distance bits, index) u64, ties to the lowest index, NaN never wins.
+constexpr int kDimChunk = 32;
+
+// rows k0 .. k0 + 31 of a 128-wide column window [c0, c0 + 128) of a cloud's dimension-major rows (row d at src + d * ld, ld a
+// multiple of 4); rows >= dim and columns >= ld are zero-filled without a read
+__device__ __forceinline__ void load_chunk_async(float (*dst)[kMT], const float* __restrict__ src, int ld, int dim, int k0, int c0) {
+  for (int ch = threadIdx.x; ch < kDimChunk * (kMT / 4); ch += kMatchThreads) {
+    const int d = ch / (kMT / 4), c4 = (ch % (kMT / 4)) * 4;
+    const bool ok = k0 + d < dim && c0 + c4 < ld;
+    cp_async16_zfill(&dst[d][c4], ok ? src + (size_t)(k0 + d) * ld + c0 + c4 : src, ok ? 16 : 0);
+  }
+}
+
+__global__ void __launch_bounds__(kMatchThreads, 2)
+nn_dim_kernel(const FeatureSrc* __restrict__ table, int V, unsigned long long* __restrict__ rowbest, unsigned long long* __restrict__ colbest) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  float(*As)[kDimChunk][kMT] = reinterpret_cast<float(*)[kDimChunk][kMT]>(smem_raw);                                        // [2][32][128]
+  float(*Bs)[kDimChunk][kMT] = reinterpret_cast<float(*)[kDimChunk][kMT]>(smem_raw + 2 * sizeof(float) * kDimChunk * kMT);  // [2][32][128]
+  unsigned long long(*colred)[kMT] =
+      reinterpret_cast<unsigned long long(*)[kMT]>(smem_raw + 4 * sizeof(float) * kDimChunk * kMT);                          // [8][128]
+
+  const int pair = blockIdx.y, stripe = blockIdx.x;
+  const FeatureSrc fa = table[2 * pair], fb = table[2 * pair + 1];
+  if (fa.dim == kDescDim) return;  // an FPFH-33 pair: the tensor-core matcher's
+  const int nA = fa.n, nB = fb.n, dim = fa.dim;
+  const int r0 = stripe * kMT;
+  if (r0 >= nA || nB <= 0) return;
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4, warp = threadIdx.x >> 5;
+  const int n_chunks = (dim + kDimChunk - 1) / kDimChunk, n_tiles = (nB + kMT - 1) / kMT, n_steps = n_chunks * n_tiles;
+
+  // step s: chunk s % n_chunks of column tile s / n_chunks
+  load_chunk_async(As[0], fa.out, fa.ld, dim, 0, r0);
+  load_chunk_async(Bs[0], fb.out, fb.ld, dim, 0, 0);
+  cp_async_commit();
+
+  unsigned long long rbest[8];
+#pragma unroll
+  for (int r = 0; r < 8; ++r) rbest[r] = ~0ull;
+  float acc[8][8];
+  for (int st = 0, jt = 0, kc = 0; st < n_steps; ++st) {
+    const int buf = st & 1;
+    __syncthreads();  // every thread is done with the buffer the next load overwrites (read in step st - 1)
+    if (st + 1 < n_steps) {
+      const int kn = kc + 1 == n_chunks ? 0 : kc + 1, jn = kc + 1 == n_chunks ? jt + 1 : jt;
+      load_chunk_async(As[buf ^ 1], fa.out, fa.ld, dim, kn * kDimChunk, r0);
+      load_chunk_async(Bs[buf ^ 1], fb.out, fb.ld, dim, kn * kDimChunk, jn * kMT);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    if (kc == 0) {
+#pragma unroll
+      for (int r = 0; r < 8; ++r)
+#pragma unroll
+        for (int c = 0; c < 8; ++c) acc[r][c] = 0.0f;
+    }
+#pragma unroll 4
+    for (int d = 0; d < kDimChunk; ++d) {
+      const float4 a0 = *reinterpret_cast<const float4*>(&As[buf][d][ty * 8]), a1 = *reinterpret_cast<const float4*>(&As[buf][d][ty * 8 + 4]);
+      const float4 b0 = *reinterpret_cast<const float4*>(&Bs[buf][d][tx * 8]), b1 = *reinterpret_cast<const float4*>(&Bs[buf][d][tx * 8 + 4]);
+      const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+      const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+      for (int r = 0; r < 8; ++r)
+#pragma unroll
+        for (int c = 0; c < 8; ++c) acc[r][c] = desc_dist_step(acc[r][c], a[r], b[c]);
+    }
+    if (++kc < n_chunks) continue;
+    // the tile's distances are complete: fold them into row minima (registers) and the tile's column minima
+    kc = 0;
+    const int cbase = jt * kMT + tx * 8, rbase = r0 + ty * 8;
+    unsigned long long cbest[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) cbest[c] = ~0ull;
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      const bool rv = rbase + r < nA;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const float dd = acc[r][c];
+        const bool ok = rv && (cbase + c < nB) && (dd == dd);  // NaN never wins
+        const unsigned long long pr = ok ? pack_dist(dd, cbase + c) : ~0ull;
+        const unsigned long long pc = ok ? pack_dist(dd, rbase + r) : ~0ull;
+        rbest[r] = umin64(rbest[r], pr);
+        cbest[c] = umin64(cbest[c], pc);
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < 8; ++c) cbest[c] = umin64(cbest[c], shfl_xor_u64(cbest[c], 16));
+    if ((threadIdx.x & 31) < 16) {
+#pragma unroll
+      for (int c = 0; c < 8; ++c) colred[warp][tx * 8 + c] = cbest[c];
+    }
+    __syncthreads();
+    if (threadIdx.x < kMT) {
+      unsigned long long m = colred[0][threadIdx.x];
+#pragma unroll
+      for (int w = 1; w < 8; ++w) m = umin64(m, colred[w][threadIdx.x]);
+      const int col = jt * kMT + threadIdx.x;
+      if (col < nB && m != ~0ull) atomicMin(colbest + (size_t)pair * V + col, m);
+    }
+    ++jt;
+    // colred is written again only after the next tile's steps, each of which opens with a __syncthreads
+  }
+#pragma unroll
+  for (int r = 0; r < 8; ++r) {
+    unsigned long long m = rbest[r];
+    m = umin64(m, shfl_xor_u64(m, 1));
+    m = umin64(m, shfl_xor_u64(m, 2));
+    m = umin64(m, shfl_xor_u64(m, 4));
+    m = umin64(m, shfl_xor_u64(m, 8));
+    if (tx == 0 && r0 + ty * 8 + r < nA) rowbest[(size_t)pair * V + r0 + ty * 8 + r] = m;
+  }
+}
+
+// column minima of nn_dim_kernel's pairs start at "none" (~0)
+__global__ void __launch_bounds__(256) nn_dim_colreset_kernel(const FeatureSrc* __restrict__ table, int V, unsigned long long* __restrict__ colbest) {
+  const int pair = blockIdx.y, col = blockIdx.x * blockDim.x + threadIdx.x;
+  const FeatureSrc fb = table[2 * pair + 1];
+  if (fb.dim == kDescDim || col >= fb.n) return;
+  colbest[(size_t)pair * V + col] = ~0ull;
+}
+
+constexpr size_t kDimSmem = 4 * sizeof(float) * kDimChunk * kMT + 8 * kMT * sizeof(unsigned long long);
+
+int launch_match_dim(Lane* h, int n_pairs) {
+  const int V = h->V;
+  QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)nn_dim_kernel, kDimSmem));
+  nn_dim_colreset_kernel<<<dim3((V + 255) / 256, n_pairs), 256, 0, h->stream>>>(h->d_feat, V, h->colbest);
+  nn_dim_kernel<<<dim3(h->NS, n_pairs), kMatchThreads, kDimSmem, h->stream>>>(h->d_feat, V, h->rowbest, h->colbest);
+  h->launches += 2;
+  QB_CUDA_TRY(h, cudaGetLastError());
+  return QB200_OK;
 }
 
 // column minima of the pairs being (re)done start at "none" (~0); match_stripe_kernel then atomicMins every stripe's minima into them
@@ -421,15 +569,15 @@ size_t match_smem_bytes() { return 3 * sizeof(float) * kDescDim * kMT + 8 * kMT 
 
 // exact fp32 CUDA-core nearest neighbours (both directions).  only == nullptr: every pair; otherwise just the
 // pairs flagged in only[] (the tensor-core filter's overflow fallback).
-int launch_match_exact(Lane* h, int n_pairs, const int* only) {
+int launch_match_exact(Lane* h, int n_pairs, const int* only, const int* n_pts) {
   const int V = h->V;
   const size_t smem = match_smem_bytes();
   QB_CUDA_TRY(h, ensure_dyn_smem(h->device, (const void*)match_stripe_kernel, smem));
   const dim3 gf((V + 255) / 256, n_pairs);
-  match_colreset_kernel<<<gf, 256, 0, h->stream>>>(h->ctr.n_vox, V, only, h->colbest);
+  match_colreset_kernel<<<gf, 256, 0, h->stream>>>(n_pts, V, only, h->colbest);
   const dim3 gs(h->NS, n_pairs);
   if (only == nullptr) cudaEventRecord(h->kev[0], h->stream);
-  match_stripe_kernel<<<gs, kMatchThreads, smem, h->stream>>>(h->desc_t, h->ctr.n_vox, V, only, h->rowbest, h->colbest);
+  match_stripe_kernel<<<gs, kMatchThreads, smem, h->stream>>>(h->desc_t, n_pts, V, only, h->rowbest, h->colbest);
   if (only == nullptr) {
     cudaEventRecord(h->kev[1], h->stream);
     h->kev_armed[0] = 1;
@@ -499,22 +647,26 @@ void match_fields(PairSolve* e, const qb200_params& p) {
   e->seed = p.seed;
 }
 
-int launch_match(Lane* h, int n_pairs, int keep_w) {
+int launch_match(Lane* h, int n_pairs, int keep_w, int dims) {
   if (n_pairs <= 0) return QB200_OK;
   const int V = h->V;
-  int rc = h->force_exact_match ? launch_match_exact(h, n_pairs, nullptr) : launch_match_nn(h, n_pairs);
+  const int* n_pts = dims ? h->ctr.n_fpfh : h->ctr.n_vox;
+  const bool fpfh = dims == 0 || (dims & kDimsFpfh);
+  int rc = !fpfh ? QB200_OK : h->force_exact_match ? launch_match_exact(h, n_pairs, nullptr, n_pts) : launch_match_nn(h, n_pairs, n_pts);
   if (rc) return rc;
-  if (h->tc_verify && !h->force_exact_match) {
+  if (fpfh && h->tc_verify && !h->force_exact_match) {
     // whole-batch self-check: keep the tensor-core results, redo every pair with the exact CUDA-core kernel, compare
     unsigned long long* rb_tc = reinterpret_cast<unsigned long long*>(h->key_b.get());                   // the sort workspace is idle here
     unsigned long long* cb_tc = rb_tc + (size_t)h->S * V;
     QB_CUDA_TRY(h, cudaMemcpyAsync(rb_tc, h->rowbest, (size_t)n_pairs * V * 8, cudaMemcpyDeviceToDevice, h->stream));
     QB_CUDA_TRY(h, cudaMemcpyAsync(cb_tc, h->colbest, (size_t)n_pairs * V * 8, cudaMemcpyDeviceToDevice, h->stream));
-    if ((rc = launch_match_exact(h, n_pairs, nullptr))) return rc;
+    if ((rc = launch_match_exact(h, n_pairs, nullptr, n_pts))) return rc;
     const dim3 gv((V + 255) / 256, n_pairs);
-    match_verify_kernel<<<gv, 256, 0, h->stream>>>(rb_tc, cb_tc, h->rowbest, h->colbest, h->ctr.n_vox, V, h->tc_stats);
+    match_verify_kernel<<<gv, 256, 0, h->stream>>>(rb_tc, cb_tc, h->rowbest, h->colbest, n_pts, V, h->tc_stats);
     h->launches += 1;
   }
+  // after the FPFH-33 K6, whose clearing of rowbest / colbest covers every pair of the wave
+  if ((dims & kDimsOther) && (rc = launch_match_dim(h, n_pairs))) return rc;
   match_mutual_kernel<<<n_pairs, 1024, 0, h->stream>>>(h->rowbest, h->colbest, h->ctr.n_vox, V, h->mut_i, h->mut_j, h->ctr.n_mutual,
                                                        h->ctr.swapped, h->mark, h->partner);
   h->launches += 1;

@@ -137,8 +137,8 @@ int qb200_match(qb200_handle* h, const float* src4, int32_t n_src, const float* 
   stamp_last(h, {kLastNn});
   MirrorHold hold{L};
   // the features as a feature wave of one pair imports them (the import writes the clouds' counts)
-  L->h_feat[0] = {reinterpret_cast<const float4*>(src4), src_desc33, n_src, 0};
-  L->h_feat[1] = {reinterpret_cast<const float4*>(tgt4), tgt_desc33, n_tgt, 0};
+  L->h_feat[0] = fpfh_src(L, 0, src4, src_desc33, n_src);
+  L->h_feat[1] = fpfh_src(L, 1, tgt4, tgt_desc33, n_tgt);
   if ((rc = stage_features(L, 2, QB200_MEM_HOST, L->stream)) || (rc = launch_feature_import(L, 2))) return rc;
   memset(&L->h_solve[0], 0, sizeof(PairSolve));  // a one-entry pair table: p's tuple test
   match_fields(&L->h_solve[0], *p);
@@ -389,7 +389,8 @@ int qb200_debug_tc_profile(qb200_handle* h, uint64_t* out24, int32_t reset) { re
 
 int qb200_debug_match_stats(qb200_handle* h, uint64_t* out4, int32_t reset) { return read_tc_stats(h, 0, 4, out4, reset); }
 
-// Nearest-neighbour tables of the most recent qb200_match (pair 0 of the handle, point order): what match_mutual_kernel read
+// Nearest-neighbour tables of the most recent qb200_match or one-pair qb200_match_descriptors_each (pair 0 of the handle, point
+// order): what match_mutual_kernel read
 int qb200_debug_nn_tables(qb200_handle* h, uint64_t* rowbest, int32_t cap_rows, uint64_t* colbest, int32_t cap_cols) {
   if (int rc = enter(h)) return rc;
   if (cap_rows < 0 || cap_cols < 0) return QB200_ERR_BAD_ARG;
@@ -422,8 +423,8 @@ int qb200_debug_tc_distances(qb200_handle* h, const float* a33, int32_t na, cons
   MirrorHold hold{L};
   // the descriptors as a feature wave imports them, without keypoints: the import's staging is in spfh, which
   // the stream has passed before the memset below reuses it
-  L->h_feat[0] = {nullptr, a33, na, 0};
-  L->h_feat[1] = {nullptr, b33, nb, 0};
+  L->h_feat[0] = fpfh_src(L, 0, nullptr, a33, na);
+  L->h_feat[1] = fpfh_src(L, 1, nullptr, b33, nb);
   if ((rc = stage_features(L, 2, QB200_MEM_HOST, L->stream)) || (rc = launch_feature_import(L, 2))) return rc;
   float* d_out = L->spfh;  // not the sort scratch: K6 sorts the descriptors by norm first
   QB_CUDA_TRY(h, cudaMemsetAsync(d_out, 0, 128 * 128 * sizeof(float), L->stream));

@@ -919,27 +919,27 @@ int tc_footprint(Lane* h, int* out5) {
 
 // norm keys -> one radix sort for all clouds (h->val_b = rank -> point) -> duplicate classes.
 // Scratch (free once the sort consumed its inputs): val_a = unique rank -> point, key_a = [class of rank | unique counts].
-static int sort_and_dedup(Lane* h, int n_clouds, int dedup) {
+static int sort_and_dedup(Lane* h, int n_clouds, int dedup, const int* n_pts) {
   const int V = h->V;
   const dim3 g((V + 255) / 256, n_clouds);
-  norm_key_kernel<<<g, 256, 0, h->stream>>>(h->desc_t, h->ctr.n_vox, V, h->key_a, h->val_a);
+  norm_key_kernel<<<g, 256, 0, h->stream>>>(h->desc_t, n_pts, V, h->key_a, h->val_a);
   h->launches += 1;
   int bits = 0;
   while ((1 << bits) < n_clouds) ++bits;
-  int rc = launch_cloud_sort(h, n_clouds, h->ctr.n_vox, 32, 32);  // per-cloud shared-memory sort; device-wide radix sort for very large clouds
+  int rc = launch_cloud_sort(h, n_clouds, n_pts, 32, 32);  // per-cloud shared-memory sort; device-wide radix sort for very large clouds
   if (rc == QB200_ERR_UNSUPPORTED) rc = sort_pairs(h, n_clouds * V, 32 + bits);
   if (rc) return rc;
-  dedup_kernel<<<n_clouds, 1024, 0, h->stream>>>(h->desc_t, h->ctr.n_vox, V, h->key_b, h->val_b, dedup, h->val_a, h->class_of(), h->n_unique());
+  dedup_kernel<<<n_clouds, 1024, 0, h->stream>>>(h->desc_t, n_pts, V, h->key_b, h->val_b, dedup, h->val_a, h->class_of(), h->n_unique());
   h->launches += 1;
   QB_CUDA_TRY(h, cudaGetLastError());
   return QB200_OK;
 }
 
-int launch_match_nn(Lane* h, int n_pairs) {
+int launch_match_nn(Lane* h, int n_pairs, const int* n_pts) {
   const int V = h->V;
   const size_t smem = tc_smem_bytes();
   if (int rc = tc_prepare(h, (const void*)tc_nn_kernel<false>)) return rc;
-  int rc = sort_and_dedup(h, 2 * n_pairs, 1);
+  int rc = sort_and_dedup(h, 2 * n_pairs, 1, n_pts);
   if (rc) return rc;
   const uint32_t* uperm = h->val_a;
   const uint32_t* class_of = h->class_of();
@@ -967,10 +967,10 @@ int launch_match_nn(Lane* h, int n_pairs) {
   }
   cudaEventRecord(h->kev[1], h->stream);
   h->kev_armed[0] = 1;
-  broadcast_best_kernel<<<gsplit, 256, 0, h->stream>>>(rowbest_u, colbest_u, h->ctr.n_vox, V, h->val_b, class_of, h->rowbest, h->colbest);
+  broadcast_best_kernel<<<gsplit, 256, 0, h->stream>>>(rowbest_u, colbest_u, n_pts, V, h->val_b, class_of, h->rowbest, h->colbest);
   h->launches += 4;
   QB_CUDA_TRY(h, cudaGetLastError());
-  return launch_match_exact(h, n_pairs, h->tc_fallback);
+  return launch_match_exact(h, n_pairs, h->tc_fallback, n_pts);
 }
 
 // debug/validation hook: approximate distances d~ of stripe 0 of pair 0, both 64-column tiles of up to 128 x 128 descriptors
@@ -978,7 +978,7 @@ int launch_match_nn(Lane* h, int n_pairs) {
 int launch_tc_debug_tile(Lane* h, float* d_out) {
   const size_t smem = tc_smem_bytes();
   if (int rc0 = tc_prepare(h, (const void*)tc_nn_kernel<true>)) return rc0;
-  int rc = sort_and_dedup(h, 2, 0);
+  int rc = sort_and_dedup(h, 2, 0, h->ctr.n_vox);
   if (rc) return rc;
   const uint32_t* uperm = h->val_a;
   const int* n_unique = h->n_unique();
